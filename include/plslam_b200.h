@@ -43,7 +43,10 @@ typedef struct plf_ctx plf_ctx; /* opaque; one per (device, stream); not thread-
 /* Front-end parameters: the stvo-pl Config keys that pl-slam inherits
  * (config/config/config_euroc.yaml:9-77, SlamConfig : Config at include/slamConfig.h:28). */
 typedef struct plf_params {
-  /* switches (config_euroc.yaml:9-18) */
+  /* switches (config_euroc.yaml:9-18).  has_points / has_lines = 0 disables that kind in the batched front-end as stvo-pl
+   * does in extraction and f2fTracking: its n_kp_* / n_lines_* are reported as 0 and it contributes no stereo rows, no
+   * matches and no pose rows.  Both 0 is rejected by plf_create (PLF_ERR_INVALID).  The standalone operators (plf_orb,
+   * plf_lsd, plf_detect_lines) ignore the switches. */
   int has_points, has_lines, best_lr_matches;
   /* point tracking (config_euroc.yaml:22-25) */
   float max_dist_epip, min_disp, min_ratio_12_p;
@@ -57,11 +60,16 @@ typedef struct plf_params {
   int min_features, max_iters, max_iters_ref;
   double min_error, min_error_change, inlier_k; /* inlier_k: IGNORED - the outlier gate is the in-tree twin's chi2 threshold
                                                    sqrt(7.815) (src/mapHandler.cpp:3460,3479), not stvo-pl's MAD-scaled inlier_k */
-  /* ORB (config_euroc.yaml:59-67) */
+  /* ORB (config_euroc.yaml:59-67).  Supported: 1..8 levels, orb_wta_k 2, orb_score 1 (FAST), orb_patch_size 31, and
+   * orb_edge_th >= 19 (the reference configs' value: the oriented 31-pixel patch reaches 18 pixels from a keypoint, which
+   * OpenCV covers with a border-reflected padding the device path does not build); every pyramid level must measure at
+   * least 2 orb_edge_th + 8 pixels.  Other values fail with PLF_ERR_INVALID. */
   int orb_nfeatures;
   float orb_scale_factor;
   int orb_nlevels, orb_edge_th, orb_wta_k, orb_score, orb_patch_size, orb_fast_th;
-  /* LSD (config_euroc.yaml:68-77) */
+  /* LSD (config_euroc.yaml:68-77).  Only lsd_refine = 0 is supported; as in OpenCV, lsd_log_eps and lsd_density_th then
+   * have no effect.  lsd_n_bins must be in [1, 1024] and the Gaussian kernel 1 + 2 ceil(3.717 sigma) at most 15 taps
+   * (sigma = lsd_sigma_scale, divided by lsd_scale below 1); other values fail with PLF_ERR_INVALID. */
   int lsd_nfeatures, lsd_refine;
   double lsd_scale, lsd_sigma_scale, lsd_quant, lsd_ang_th, lsd_log_eps, lsd_density_th; /* LSDOptions: double */
   int lsd_n_bins;

@@ -35,11 +35,16 @@ from dataclasses import dataclass, field
 
 from oracle import matching as om
 
-DEFAULTS = dict(  # config/config/config_euroc.yaml:9-77
+DEFAULTS = dict(  # config/config/config_euroc.yaml:9-77; every field of plf_default_params() (pl-slam_b200/csrc/plf_ctx.cu)
+    has_points=True, has_lines=True,
     best_lr_matches=True, max_dist_epip=1.0, min_disp=1.0, min_ratio_12_p=0.9, line_sim_th=0.75,
     stereo_overlap_th=0.75, f2f_overlap_th=0.75, min_line_length=0.025, line_horiz_th=0.1, min_ratio_12_l=0.9,
     ls_min_disp_ratio=0.7, homog_th=1e-7, min_features=10, max_iters=5, max_iters_ref=10, min_error=1e-7,
-    min_error_change=1e-7, orb_nfeatures=800, orb_nlevels=4, orb_fast_th=20, lsd_nfeatures=300,
+    min_error_change=1e-7, inlier_k=4.0,
+    orb_nfeatures=800, orb_scale_factor=1.2, orb_nlevels=4, orb_edge_th=19, orb_wta_k=2, orb_score=1, orb_patch_size=31,
+    orb_fast_th=20,
+    lsd_nfeatures=300, lsd_refine=0, lsd_scale=1.2, lsd_sigma_scale=0.6, lsd_quant=2.0, lsd_ang_th=22.5, lsd_log_eps=1.0,
+    lsd_density_th=0.6, lsd_n_bins=1024,
     # matching strategy (config_euroc.yaml:55-57; 0 = descriptor only, the default of this library; the reference
     # configs select 3 = windowed) and the fall-back thresholds of the in-tree analogue (src/slamConfig.cpp:85-86)
     matching_strategy=0, matching_s_ws=10, matching_f2f_ws=3, min_pt_matches=10, min_ls_matches=6)
@@ -204,7 +209,11 @@ def extract_stereo(cam, left, right, prm, orb_fn=None, lines_fn=None, match_fn=N
     if orb_fn is None:
         orb_fn = lambda im: _orb_c(im, prm)
     if lines_fn is None:
-        lines_fn = lambda im: detect_lines(im, prm["lsd_nfeatures"], prm["min_line_length"])
+        lines_fn = lambda im: detect_lines(im, prm["lsd_nfeatures"], prm["min_line_length"], lsd_kwargs(prm))
+    # has_points / has_lines = false: stvo-pl neither detects nor matches the disabled kind
+    has_p, has_l = prm.get("has_points", True), prm.get("has_lines", True)
+    none = lambda im: (None, None)
+    orb_fn, lines_fn = (orb_fn if has_p else none), (lines_fn if has_l else none)
     if pool is not None:   # lr_in_parallel / pl_in_parallel (config_euroc.yaml:14-15): 4 concurrent tasks
         fa, fb, fc, fd = (pool.submit(orb_fn, left), pool.submit(orb_fn, right), pool.submit(lines_fn, left),
                           pool.submit(lines_fn, right))
@@ -213,14 +222,30 @@ def extract_stereo(cam, left, right, prm, orb_fn=None, lines_fn=None, match_fn=N
         kp_l, d_l = orb_fn(left); kp_r, d_r = orb_fn(right)
         kl_l, ld_l = lines_fn(left); kl_r, ld_r = lines_fn(right)
     f = Frame()
-    f.pt_pl, f.pt_disp, f.pt_P, f.pt_octave, f.pdesc = stereo_points(cam, kp_l, d_l, kp_r, d_r, prm, match_fn)
-    (f.ls_spl, f.ls_epl, f.ls_sdisp, f.ls_edisp, f.ls_sP, f.ls_eP, f.ls_le, f.ls_angle, f.ldesc) = \
-        stereo_lines(cam, kl_l, ld_l, kl_r, ld_r, prm, match_fn)
+    if has_p:
+        f.pt_pl, f.pt_disp, f.pt_P, f.pt_octave, f.pdesc = stereo_points(cam, kp_l, d_l, kp_r, d_r, prm, match_fn)
+    if has_l:
+        (f.ls_spl, f.ls_epl, f.ls_sdisp, f.ls_edisp, f.ls_sP, f.ls_eP, f.ls_le, f.ls_angle, f.ldesc) = \
+            stereo_lines(cam, kl_l, ld_l, kl_r, ld_r, prm, match_fn)
     return f
 
 
 def _orb_c(img, prm):
-    return clib.orb(img, prm["orb_nfeatures"], 1.2, prm["orb_nlevels"], 19, 31, prm["orb_fast_th"])
+    """cv::ORB::create(orb_nfeatures, orb_scale_factor, orb_nlevels, orb_edge_th, 0, orb_wta_k, orb_score,
+    orb_patch_size, orb_fast_th) as restated by oracle/orb.c: WTA_K 2 and the FAST score only."""
+    if prm.get("orb_wta_k", 2) != 2 or prm.get("orb_score", 1) != 1:
+        raise ValueError("the ORB oracle restates WTA_K = 2 with the FAST score only")
+    return clib.orb(img, prm["orb_nfeatures"], prm.get("orb_scale_factor", 1.2), prm["orb_nlevels"],
+                    prm.get("orb_edge_th", 19), prm.get("orb_patch_size", 31), prm["orb_fast_th"])
+
+
+def lsd_kwargs(prm):
+    """The cv::createLineSegmentDetector options of prm for clib.lsd.  lsd_log_eps / lsd_density_th only act when
+    lines are refined, which the oracle (like the library) does not support."""
+    if prm.get("lsd_refine", 0) != 0:
+        raise ValueError("the LSD oracle restates lsd_refine = 0 only")
+    return dict(scale=prm.get("lsd_scale", 1.2), sigma_scale=prm.get("lsd_sigma_scale", 0.6), quant=prm.get("lsd_quant", 2.0),
+                ang_th=prm.get("lsd_ang_th", 22.5), n_bins=prm.get("lsd_n_bins", 1024))
 
 
 def projection(cam, P):

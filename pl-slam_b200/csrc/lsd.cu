@@ -55,6 +55,7 @@ struct LsdState {
   int ws = 0, hs = 0;       // scaled size
   int ksize = 0;
   int taps[16];
+  bool taps_u8 = false;     // every tap <= 255: the packed-byte fast blur applies (a 256 centre tap at small sigma does not)
   int n_bins = 1024;
   double scale = 1.2, prec = 0, p = 0, rho = 0;
   int min_reg_size = 0;
@@ -1045,7 +1046,7 @@ static void gaussian_taps_q8(int ksize, double sigma, int* taps) {
   taps[ksize / 2] = 256 - 2 * s;
 }
 
-plf_status plf_lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
+static plf_status lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
   LsdState* s = ctx->lsd;
   if (s && s->w == w && s->h == h && s->nimg >= nimg && (s->two_parities || !two_parities)) return PLF_OK;
   if (s && s->two_parities) two_parities = true;
@@ -1074,6 +1075,8 @@ plf_status plf_lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_pariti
     s->ksize = 1 + 2 * (int)hk;
     if (s->ksize > 15) return plf_fail(ctx, PLF_ERR_INVALID, "LSD: Gaussian kernel %d > 15 unsupported", s->ksize);
     gaussian_taps_q8(s->ksize, sigma, s->taps);
+    s->taps_u8 = true;
+    for (int k = 0; k < s->ksize; ++k) s->taps_u8 = s->taps_u8 && s->taps[k] <= 255;
     s->ws = (int)nearbyint(w * s->scale);
     s->hs = (int)nearbyint(h * s->scale);
   } else {
@@ -1148,6 +1151,16 @@ plf_status plf_lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_pariti
   return PLF_OK;
 }
 
+// A failed (re)build leaves no state behind (see plf_orb_prepare).
+plf_status plf_lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
+  const plf_status st = lsd_prepare(ctx, w, h, nimg, two_parities);
+  if (st && ctx->lsd) {
+    lsd_release(ctx->lsd);
+    *ctx->lsd = LsdState();
+  }
+  return st;
+}
+
 // LSD on images [img0, img0+n) of a batch resident on the device, in two phases so that callers can overlap them with
 // other work: `pre` = blur, resample, gradient and seed ordering (bandwidth-bound), `grow` = region growing, rectangle
 // fit and the KeyLine stage (latency-bound).  `par` selects the buffer set that carries data from pre to grow.
@@ -1178,7 +1191,7 @@ plf_status plf_lsd_pre_range(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_str
   size_t scaled_stride = img_stride;
   int scaled_pitch = pitch;
   if (s->scale != 1.0) {
-    if (s->ksize == 7 || s->ksize == 5) {
+    if ((s->ksize == 7 || s->ksize == 5) && s->taps_u8) {
       // tensor map of the source images (two cached slots: the pipeline alternates between its two upload buffers)
       if (s->tm_stride != img_stride || s->tm_pitch != pitch || s->tm_nimg < img0 + n) {
         s->tm_src[0] = s->tm_src[1] = nullptr;

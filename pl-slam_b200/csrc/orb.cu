@@ -28,6 +28,7 @@
 #include "plf_tma.cuh"
 
 #define ORB_MAX_LEVELS 8
+#define ORB_MIN_EDGE 19   // smallest orb_edge_th: keypoint to level border >= the 18-pixel reach of the 37 x 37 window
 #define ORB_TW 64
 #define ORB_TH 16
 #define ORB_SORT_CAP 4096
@@ -704,13 +705,14 @@ static int8_t* g_dev_pattern = nullptr;  // shared by all contexts on a device (
 static int g_dev_pattern_device = -1;
 
 // (Re)builds the ORB state for images of w x h and up to nimg images per launch.
-plf_status plf_orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
+static plf_status orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
   OrbState* s = ctx->orb;
   if (s && s->w == w && s->h == h && s->nimg >= nimg && (s->two_parities || !two_parities)) return PLF_OK;
   if (s && s->two_parities) two_parities = true;
   if (s) {
     PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     orb_release(s);
+    *s = OrbState();
   } else {
     s = ctx->orb = new OrbState();
   }
@@ -720,6 +722,12 @@ plf_status plf_orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_pariti
     return plf_fail(ctx, PLF_ERR_INVALID,
                     "ORB: supported configuration is 1..8 levels, WTA_K=2, FAST score, patch 31 (got levels=%d "
                     "wta_k=%d score=%d patch=%d)", P.orb_nlevels, P.orb_wta_k, P.orb_score, P.orb_patch_size);
+  // keypoints lie >= edge pixels inside their level and the orientation / rBRIEF window (37 x 37) is read without border
+  // handling (k_ic_angle, k_rbrief), where OpenCV reads a border-reflected level padded by max(edge, 22): below 19 the
+  // window would cross the level's border (and, on level 0, the image buffer)
+  if (P.orb_edge_th < ORB_MIN_EDGE)
+    return plf_fail(ctx, PLF_ERR_INVALID, "ORB: orb_edge_th %d < %d unsupported (the 31-pixel patch needs that border)",
+                    P.orb_edge_th, ORB_MIN_EDGE);
   if (w >= 4096 || h >= 4096) return plf_fail(ctx, PLF_ERR_INVALID, "ORB: image larger than 4095 px");
   s->w = w; s->h = h; s->nimg = nimg;
   s->two_parities = two_parities;
@@ -835,6 +843,17 @@ plf_status plf_orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_pariti
       return plf_fail(ctx, PLF_ERR_CUDA, "ORB: cuTensorMapEncodeTiled failed for pyramid level %d", l);
   }
   return PLF_OK;
+}
+
+// A failed (re)build leaves no state behind: the next call starts from scratch and fails the same way, instead of finding
+// a size that matches the request and buffers that were released.
+plf_status plf_orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
+  const plf_status st = orb_prepare(ctx, w, h, nimg, two_parities);
+  if (st && ctx->orb) {
+    orb_release(ctx->orb);
+    *ctx->orb = OrbState();
+  }
+  return st;
 }
 
 // Runs ORB on nimg images resident at d_imgs ([nimg][h][pitch], pitch a multiple of 16, stride img_stride bytes).

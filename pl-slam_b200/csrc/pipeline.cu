@@ -765,9 +765,13 @@ plf_status plf_batch_run(plf_ctx* ctx, int B) {
   // the rest of the match phase works on its own copy of the extraction outputs; evX releases this parity to batch i+2
   PLF_CUDA(ctx, cudaMemcpyAsync(s->kpsM, kps, sizeof(plf_keypoint) * 2 * (size_t)B * K, cudaMemcpyDeviceToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->descM, odesc, 32 * 2 * (size_t)B * K, cudaMemcpyDeviceToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->kcntM, kcnt, sizeof(int) * 2 * (size_t)B, cudaMemcpyDeviceToDevice, cs));
+  // has_points / has_lines = 0 (stvo-pl skips the disabled kind in extraction and f2fTracking): its counts are zero from
+  // here on, so it has no stereo rows, no matches, no pose rows and reports 0 detected features
+  if (P.has_points) PLF_CUDA(ctx, cudaMemcpyAsync(s->kcntM, kcnt, sizeof(int) * 2 * (size_t)B, cudaMemcpyDeviceToDevice, cs));
+  else PLF_CUDA(ctx, cudaMemsetAsync(s->kcntM, 0, sizeof(int) * 2 * (size_t)B, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->klsM, kls, sizeof(plf_keyline) * 2 * (size_t)B * Ln, cudaMemcpyDeviceToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->lcntM, lcnt, sizeof(int) * 2 * (size_t)B, cudaMemcpyDeviceToDevice, cs));
+  if (P.has_lines) PLF_CUDA(ctx, cudaMemcpyAsync(s->lcntM, lcnt, sizeof(int) * 2 * (size_t)B, cudaMemcpyDeviceToDevice, cs));
+  else PLF_CUDA(ctx, cudaMemsetAsync(s->lcntM, 0, sizeof(int) * 2 * (size_t)B, cs));
   PLF_CUDA(ctx, cudaEventRecord(s->evX[par], cs));
   kps = s->kpsM; odesc = s->descM; kcnt = s->kcntM; kls = s->klsM; lcnt = s->lcntM;
   plf_mark(ctx, "copy extraction outputs");
@@ -885,8 +889,9 @@ plf_status plf_batch_download(plf_ctx* ctx, int B, plf_frame_result* out) {
   s->pend_B[0] = s->pend_B[1]; s->pend_B[1] = s->pend_B[2];
   s->n_pending--;
   memcpy(out, s->h_results[par], sizeof(plf_frame_result) * B);
-  if (s->h_ovf[par][0] || s->h_ovf[par][1]) {
-    const int o0 = s->h_ovf[par][0], o1 = s->h_ovf[par][1];
+  // an overflow of a disabled kind's extraction buffers does not reach the results
+  const int o0 = ctx->params.has_points ? s->h_ovf[par][0] : 0, o1 = ctx->params.has_lines ? s->h_ovf[par][1] : 0;
+  if (o0 || o1) {
     return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_batch_download: a fixed-capacity buffer overflowed (%s%s); raise plf_limits",
                     o0 ? "ORB keypoints " : "", o1 ? "LSD segments/lines" : "");
   }

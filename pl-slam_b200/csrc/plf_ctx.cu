@@ -211,6 +211,10 @@ plf_status plf_create(const plf_params* params, const plf_camera* cam, const plf
     delete ctx;
     return plf_fail(nullptr, PLF_ERR_INVALID, "plf_create: bad camera size or max_batch");
   }
+  if (!ctx->params.has_points && !ctx->params.has_lines) {
+    delete ctx;
+    return plf_fail(nullptr, PLF_ERR_INVALID, "plf_create: has_points and has_lines are both 0; a front-end needs one of them");
+  }
   plf_configure_lsd();
   cudaGetLastError();
   e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);

@@ -103,6 +103,12 @@ class plf_frame_view(C.Structure):
                 ("ls_angle", C.c_void_p), ("ldesc", C.c_void_p)]
 
 
+class plf_match_view(C.Structure):
+    _fields_ = [("cap_pt", C.c_int), ("cap_ls", C.c_int), ("n_pt", C.c_int), ("n_ls", C.c_int),
+                ("P", C.c_void_p), ("pl_obs", C.c_void_p), ("inlier_pt", C.c_void_p), ("sP", C.c_void_p),
+                ("eP", C.c_void_p), ("le_obs", C.c_void_p), ("inlier_ls", C.c_void_p)]
+
+
 class plf_lc_params(C.Structure):
     _fields_ = [("lc_res", C.c_double), ("lc_unc", C.c_double), ("lc_inl", C.c_double), ("lc_trs", C.c_double),
                 ("lc_rot", C.c_double), ("lc_inlier_ratio", C.c_double)]
@@ -573,6 +579,22 @@ class Frontend:
         for name, arr in a.items():
             n = v.n_pt if name.startswith("pt_") or name == "pdesc" else v.n_ls
             out[name] = arr[:n].copy()
+        return out
+
+    def get_matches(self, k):
+        """Frame-to-frame correspondences of pair k of the last batch (matched_pt / matched_ls after optimizePose), in the
+        previous frame's row order: dict with P, pl_obs, inlier_pt (bool) and sP, eP, le_obs, inlier_ls (bool)."""
+        K, Ln = self.limits.max_keypoints, self.limits.max_lines
+        a = dict(P=np.zeros((K, 3)), pl_obs=np.zeros((K, 2)), inlier_pt=np.zeros(K, np.uint8), sP=np.zeros((Ln, 3)),
+                 eP=np.zeros((Ln, 3)), le_obs=np.zeros((Ln, 3)), inlier_ls=np.zeros(Ln, np.uint8))
+        v = plf_match_view(cap_pt=K, cap_ls=Ln)
+        for name, arr in a.items():
+            setattr(v, name, arr.ctypes.data)
+        self._check(self.lib.plf_get_matches(self._ctx, int(k), C.byref(v)), "plf_get_matches")
+        out = {}
+        for name, arr in a.items():
+            n = v.n_pt if name in ("P", "pl_obs", "inlier_pt") else v.n_ls
+            out[name] = arr[:n].astype(bool) if name.startswith("inlier") else arr[:n].copy()
         return out
 
     # -- profiling -------------------------------------------------------------------------------

@@ -5,7 +5,9 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+import param_cases as pc
 from oracle import clib, synth
+from oracle import frontend as ofe
 from oracle.cvref import lsd_cv2
 
 GOLD = Path(__file__).parent / "golden" / "lines_v1.npz"
@@ -40,3 +42,25 @@ def test_lsd_scale_variants_vs_cv2():
 
 def test_lsd_flat_image_has_no_segments():
     assert len(clib.lsd(np.full((100, 150), 90, np.uint8))) == 0
+
+
+@pytest.mark.parametrize("case", sorted(pc.LSD_CASES))
+def test_lsd_oracle_matches_cv2_param_cases(case):
+    """The LSD settings of tests/param_cases.py (Gaussian kernels of 3 to 15 taps, quantisation, angle tolerance, bins)."""
+    pytest.importorskip("cv2")
+    prm = dict(ofe.DEFAULTS, **pc.LSD_CASES[case])
+    L, _ = synth.scene_pair(w=640, h=360, seed=3)
+    ref = lsd_cv2(L, scale=prm["lsd_scale"], sigma_scale=prm["lsd_sigma_scale"], quant=prm["lsd_quant"],
+                  ang_th=prm["lsd_ang_th"], n_bins=prm["lsd_n_bins"])
+    mine = clib.lsd(L, **ofe.lsd_kwargs(prm))
+    assert len(ref) > 50 and mine.shape == ref.shape and np.array_equal(mine, ref)
+
+
+def test_lsd_log_eps_density_th_have_no_effect_in_cv2():
+    """Without refinement cv2 ignores log_eps and density_th, which is why the library may ignore them."""
+    pytest.importorskip("cv2")
+    L, _ = synth.scene_pair(w=640, h=360, seed=3)
+    ref = lsd_cv2(L)
+    for kw in (dict(log_eps=pc.INVARIANT["lsd_log_eps"]), dict(density_th=pc.INVARIANT["lsd_density_th"]),
+               dict(log_eps=-2.0, density_th=0.1)):
+        assert np.array_equal(lsd_cv2(L, **kw), ref), kw

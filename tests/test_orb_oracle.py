@@ -4,7 +4,9 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+import param_cases as pc
 from oracle import clib, synth
+from oracle import frontend as ofe
 from oracle.cvref import orb_cv2
 
 GOLD = Path(__file__).parent / "golden" / "orb_v1.npz"
@@ -49,3 +51,15 @@ def test_fast_atan2_vs_cv2():
         y, x = (float(v) for v in rng.integers(-200000, 200000, 2))
         assert np.float32(clib.fast_atan2(y, x)) == np.float32(cv2.fastAtan2(y, x))
     assert clib.fast_atan2(0.0, 0.0) == cv2.fastAtan2(0.0, 0.0)
+
+
+@pytest.mark.parametrize("case", sorted(pc.ORB_CASES))
+def test_oracle_matches_cv2_param_cases(case):
+    """The ORB settings of tests/param_cases.py: the C restatement, called as the oracle front-end calls it, equals cv2."""
+    pytest.importorskip("cv2")
+    prm = dict(ofe.DEFAULTS, **pc.ORB_CASES[case])
+    L, _ = synth.scene_pair(w=640, h=360, seed=3)
+    kp, desc = ofe._orb_c(L, prm)
+    rk, rd = orb_cv2(L, prm["orb_nfeatures"], prm["orb_scale_factor"], prm["orb_nlevels"], prm["orb_edge_th"],
+                     prm["orb_wta_k"], prm["orb_patch_size"], prm["orb_fast_th"])
+    assert len(rk) > 100 and same_kps(kp, rk) and np.array_equal(desc, rd)

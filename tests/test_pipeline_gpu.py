@@ -29,9 +29,7 @@ def run_both(cam, frames, B, **prm_over):
     prm = dict(ofe.DEFAULTS, **prm_over)
     ref = ofe.run_sequence(cam, [(a, b) for a, b, _ in frames], prm)
     lim = plf.default_limits(); lim.max_batch = B
-    kw = {k: v for k, v in prm_over.items() if k in ("orb_nfeatures", "lsd_nfeatures", "max_iters", "max_iters_ref", "min_features",
-                                                     "matching_strategy", "matching_s_ws", "matching_f2f_ws", "min_pt_matches",
-                                                     "min_ls_matches")}
+    kw = {k: prm[k] for k, _ in plf.plf_params._fields_}   # the oracle's parameters, every one of them, on the device too
     got, feats = [], []
     with plf.Frontend(camera=cam, limits=lim, **kw) as fe:
         for s0 in range(0, len(frames), B):

@@ -37,8 +37,9 @@ def oracle_sequence(cam, frames, prm):
 
 def gpu_sequential(cam, frames, B, max_batch, **kw):
     lim = plf.default_limits(); lim.max_batch = max_batch
+    prm = dict(ofe.DEFAULTS, **kw)   # what oracle_sequence runs, forwarded field by field
     got, feats = [], []
-    with plf.Frontend(camera=cam, limits=lim, **kw) as fe:
+    with plf.Frontend(camera=cam, limits=lim, **{k: prm[k] for k, _ in plf.plf_params._fields_}) as fe:
         for s0 in range(0, len(frames), B):
             chunk = frames[s0:s0 + B]
             got += fe.process_batch(np.stack([c[0] for c in chunk]), np.stack([c[1] for c in chunk]))
