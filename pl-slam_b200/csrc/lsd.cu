@@ -14,9 +14,9 @@
 //   k_blur_q8_fast   separable Q8.8 Gaussian (tile + halo staged by one TMA bulk-tensor copy, DP4A row pass), one rounding
 //                    (k_blur_q8: generic variant for tiny images)
 //   k_resize_exact4  (orb.cu) INTER_LINEAR_EXACT resample to scale
-//   k_lsd_grad       2x2 gradient; for the DEFINED pixels only (|grad| > rho, ~12 %): the 16-byte record {angle
-//                    (cv::fastAtan2, degrees, f32), table index, cosf, sinf} fetched from a table keyed by (gx,gy), and one
-//                    entry of the raster-ordered seed list of the pixel's row segment; per-image max of |grad|^2.
+//   k_lsd_grad       2x2 gradient; for the DEFINED pixels only (|grad| > rho, ~12 %): the 8-byte record {angle
+//                    (cv::fastAtan2, degrees, f32, from a table keyed by (gx,gy)), table index}, and one packed entry
+//                    (column, |grad|^2) of the raster-ordered seed list of the pixel's row segment; per-image max of |grad|^2.
 //                    Nothing dense leaves the kernel (the record map restores itself to "undefined", see k_lsd_fill_notdef)
 //   k_lsd_rowhist / k_lsd_binscan / k_lsd_scatter
 //                    stable counting sort of the seed lists by magnitude bin (descending), raster order inside a
@@ -27,6 +27,8 @@
 //                    records of the current region point (fetched two queue entries ahead, L1-resident through a
 //                    look-ahead prefetch), the alignment tests run lane-parallel in the reference order, and the
 //                    region angle is only evaluated when a decision depends on it (see the kernel's comment; bit-exact).
+//                    The (cosf, sinf) a member adds to the region's sums comes from a table keyed by the record's index,
+//                    loaded off the decision chain and added one queue entry later, in the reference's order.
 //                    `used` is folded into the angle (a used pixel gets the NOTDEF sentinel).
 //   k_lsd_rect_order / k_lsd_rects
 //                    one thread per region, regions permuted into size classes: weighted centroid, inertia-matrix
@@ -69,32 +71,34 @@ struct LsdState {
   size_t tm_stride = 0; int tm_pitch = 0, tm_nimg = 0;
   uint32_t* rect_perm = nullptr;  // [nimg][max_regions] regions in size-class order (k_lsd_rect_order)
   struct LsdPix* pix_raw[2] = {nullptr, nullptr};  // allocation (pix + look-ahead slack on both sides)
-  struct LsdPix* pix[2] = {nullptr, nullptr};  // [nimg][guard + hs*ws]  {angle (deg, f32) | NOTDEF = undefined/used, cosf, sinf, pad}
+  struct LsdPix* pix[2] = {nullptr, nullptr};  // [nimg][guard + hs*ws]  {angle (deg, f32) | NOTDEF = undefined/used, table index}
   size_t pix_stride = 0;      // entries per image = guard (ws+1, permanently NOTDEF) + hs*ws
   int m2_min = 0;             // smallest gx^2+gy^2 whose gradient norm exceeds rho (defined pixel)
-  // seed lists per row segment (LSD_SEG columns): segment (y, xb) owns the entries [y * ws + LSD_SEG * xb, ...) of the three arrays
-  uint32_t* seedlist = nullptr; // [nimg][hs*ws] pixel index
-  uint32_t* seedm2 = nullptr;   // [nimg][hs*ws] gx^2 + gy^2
-  uint16_t* binmap = nullptr;   // [nimg][hs*ws] bin of the pseudo-ordering (k_lsd_rowhist)
+  // seed lists per row segment (LSD_SEG columns): segment (y, xb) owns the entries [y * ws + LSD_SEG * xb, ...);
+  // an entry is column-in-segment | gx^2+gy^2 << LSD_COL_BITS (k_lsd_grad), then column | bin << LSD_COL_BITS (k_lsd_rowhist)
+  uint32_t* seedlist = nullptr; // [nimg][hs*ws]
   int* segcnt = nullptr;        // [nimg][hs][nxb] entries per segment
   int nxb = 0;                  // segments per row
   int* maxmag2 = nullptr;     // [nimg]
   uint32_t* rowcnt = nullptr; // [nimg][nchunks][n_bins]  per-chunk bin counts -> prefixes
   uint32_t* binstart = nullptr; // [nimg][n_bins]
+  // per batch parity: what crosses from the pre-grow chain to the growing (pix, order, nseeds) and what the match phase
+  // reads (kls, nlines).  One copy: what only the growing / rectangle / KeyLine kernels of one batch write and read.
   int* nseeds[2] = {nullptr, nullptr};      // [nimg]
   uint32_t* order[2] = {nullptr, nullptr};  // [nimg][hs*ws]
-  uint32_t* regpts[2] = {nullptr, nullptr}; // [nimg][hs*ws]
-  uint4* regions[2] = {nullptr, nullptr};   // [nimg][max_regions] {start, count, angle_lo, angle_hi}
-  int* nregions[2] = {nullptr, nullptr};    // [nimg]
-  float4* segs[2] = {nullptr, nullptr};     // [nimg][max_regions]
   plf_keyline* kls[2] = {nullptr, nullptr}; // [nimg][max_lines]  final KeyLines (after top-K)
-  plf_keyline* kls_all[2] = {nullptr, nullptr}; // [nimg][max_regions] before top-K
   int* nlines[2] = {nullptr, nullptr};      // [nimg]
+  uint32_t* regpts = nullptr;   // [nimg][hs*ws]
+  uint4* regions = nullptr;     // [nimg][max_regions] {start, count, angle_lo, angle_hi}
+  int* nregions = nullptr;      // [nimg]
+  float4* segs = nullptr;       // [nimg][max_regions]
+  plf_keyline* kls_all = nullptr; // [nimg][max_regions] before top-K
   int* overflow = nullptr;    // [1]
   int* rs_tab = nullptr;      // resize tables
   size_t rs_x_off = 0, rs_y_off = 0, rs_xp_off = 0;
-  struct LsdPix* grad_lut = nullptr; // [1021*1021] gradient (gx,gy) -> LsdPix
-  float2* seed_lut = nullptr;        // [1021*1021] gradient (gx,gy) -> unit vector of a region seed
+  float* angle_lut = nullptr;   // [1021*1021] gradient (gx,gy) -> level-line angle (degrees) of a defined pixel
+  float2* cs_lut = nullptr;     // [1021*1021] gradient (gx,gy) -> (cosf, sinf) of float(angle in radians): a member's term of the region sums
+  float2* seed_lut = nullptr;   // [1021*1021] gradient (gx,gy) -> unit vector of a region seed
 };
 
 __constant__ int c_lsd_taps[16];
@@ -238,70 +242,79 @@ __device__ __forceinline__ float lsd_fast_atan2(float y, float x) {  // cv::fast
   return a;
 }
 
-// Per-pixel record read by the region-growing kernel: one 16-byte load per neighbour.
-struct __align__(16) LsdPix {
+// Per-pixel record read by the region-growing kernel: one 8-byte load per neighbour.
+struct __align__(8) LsdPix {
   float a;    // level-line angle in DEGREES exactly as cv::fastAtan2(gx,-gy) returns it (OpenCV stores a * DEG_TO_RADS as
               // f64; that product is re-formed where the f64 value is needed) or LSD_NOTDEF_F = undefined / used
-  uint32_t li; // index of the pixel's gradient in the (gx,gy) tables: the seed's unit vector is fetched from lut_seed[li]
-  float c, s; // cosf / sinf of float(angle in radians)
+  uint32_t li; // index of the pixel's gradient in the (gx,gy) tables: a member's (cosf, sinf) is lut_cs[li], a seed's unit
+               // vector lut_seed[li], and the rectangle fit recovers (gx, gy) from it
 };
 #define LSD_NOTDEF_F (-1024.f)
 
-// Gradient lookup table.  The 2x2 gradient (gx, gy) takes 1021 x 1021 integer values; the level-line angle, the NOTDEF
+// Gradient lookup tables.  The 2x2 gradient (gx, gy) takes 1021 x 1021 integer values; the level-line angle, the NOTDEF
 // decision (|grad| <= rho) and cosf/sinf of float(angle) are functions of (gx, gy) only.  They are tabulated once per
-// context with exactly the device functions used elsewhere (16 MB, L2-resident), which turns ~200 dependent
-// instructions per defined pixel into one 16-byte load.
+// context with exactly the device functions used elsewhere (4 + 8 + 8 MB, L2-resident), which turns ~200 dependent
+// instructions per defined pixel into table loads.
 #define LSD_LUT_DIM 1021
+// lut_angle: the angle of a defined gradient (NOTDEF otherwise; k_lsd_grad only looks up defined ones);
+// lut_cs: (cos(float(angle)), sin(float(angle))) as region_grow adds them, host libm -> glibc port;
 // lut_seed: the unit vector region_grow starts its sums from, float(cos(angle)), float(sin(angle)) of the f64 angle.
-__global__ void __launch_bounds__(256) k_lsd_build_lut(double rho, LsdPix* __restrict__ lut, float2* __restrict__ lut_seed) {
+__global__ void __launch_bounds__(256) k_lsd_build_lut(double rho, float* __restrict__ lut_angle, float2* __restrict__ lut_cs,
+                                                       float2* __restrict__ lut_seed) {
   const int i = blockIdx.x * 256 + threadIdx.x;
   if (i >= LSD_LUT_DIM * LSD_LUT_DIM) return;
   const int gx = i / LSD_LUT_DIM - 510, gy = i % LSD_LUT_DIM - 510;
-  LsdPix e;
-  e.a = LSD_NOTDEF_F; e.c = 0.f; e.s = 0.f; e.li = (uint32_t)i;
-  float2 sv = make_float2(0.f, 0.f);
+  float a = LSD_NOTDEF_F;
+  float2 cs = make_float2(0.f, 0.f), sv = make_float2(0.f, 0.f);
   const double norm = sqrt((double)(gx * gx + gy * gy) / 4.0);
   if (!(norm <= rho)) {
     const float adeg = lsd_fast_atan2((float)gx, (float)(-gy));
-    e.a = adeg;
-    const float af = (float)((double)adeg * LSD_DEG2RAD);  // region_grow: cos(float(angle)), sin(float(angle)), host libm -> glibc port
-    e.c = glibc_cosf(af);
-    e.s = glibc_sinf(af);
+    a = adeg;
+    const float af = (float)((double)adeg * LSD_DEG2RAD);
+    cs = make_float2(glibc_cosf(af), glibc_sinf(af));
     const double ad = (double)adeg * LSD_DEG2RAD;
     sv = make_float2((float)cos(ad), (float)sin(ad));
   }
-  lut[i] = e;
+  lut_angle[i] = a;
+  lut_cs[i] = cs;
   lut_seed[i] = sv;
 }
 
 // Every record of the map (guards included) starts as "undefined".  From then on the map returns to that state by itself:
 // the growing kernel visits every defined pixel - as a seed or as a member of a region - and marks it used (= NOTDEF), so
 // when a batch's region growing has finished, all records of its images read NOTDEF again.  The gradient kernel therefore
-// writes records for the DEFINED pixels only (~12 % of them): 6.5 instead of 13.4 MB of DRAM writes per image.
+// writes records for the DEFINED pixels only (~12 % of them).
 __global__ void k_lsd_fill_notdef(LsdPix* __restrict__ pix, size_t n) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   LsdPix e;
-  e.a = LSD_NOTDEF_F; e.c = 0.f; e.s = 0.f; e.li = 0u;
+  e.a = LSD_NOTDEF_F; e.li = 0u;
   pix[i] = e;
 }
 
 // pix points at pixel (0,0) of image 0 (i.e. past the guard); image stride pix_stride.
-// Only the DEFINED pixels (gradient norm above rho, ~12 %) leave the kernel: their 16-byte record (the map's other records
-// already read "undefined", see k_lsd_fill_notdef) and one entry (pixel index, gx^2 + gy^2) of the raster-ordered SEED LIST of
-// their row segment - the LSD_SEG columns of this block; segment (y, xb) stores its entries at the segment's own pixel offset
-// y * W + LSD_SEG * xb of the list arrays, so it can never overflow, and its length in segcnt.  Nothing dense is written: the
-// seed ordering works on the lists, and the rectangle fit reads the gradient of a region point back from its record (li).
+// Only the DEFINED pixels (gradient norm above rho, ~12 %) leave the kernel: their 8-byte record (the map's other records
+// already read "undefined", see k_lsd_fill_notdef) and one entry (column in the segment, gx^2 + gy^2) of the raster-ordered
+// SEED LIST of their row segment - the LSD_SEG columns of this block; segment (y, xb) stores its entries at the segment's own
+// pixel offset y * W + LSD_SEG * xb of the list array, so it can never overflow, and its length in segcnt.  Nothing dense is
+// written: the seed ordering works on the lists, and the rectangle fit reads the gradient of a region point back from its
+// record (li).
 #define LSD_SEG 512
 #define LSD_GRAD_THREADS (LSD_SEG / 4)
+// list entry: the low LSD_COL_BITS hold the column inside the segment, the high bits gx^2 + gy^2 (<= 2 * 510^2 over the
+// table's gradient range) and, after k_lsd_rowhist, the bin (< LSD_BINS_MAX)
+#define LSD_COL_BITS 9
+static_assert(LSD_SEG <= (1 << LSD_COL_BITS), "seed list: a segment column must fit the column field");
+static_assert(2u * 510u * 510u < (1u << (32 - LSD_COL_BITS)), "seed list: gx^2 + gy^2 must fit above the column field");
+static_assert(LSD_BINS_MAX <= (1 << (32 - LSD_COL_BITS)), "seed list: the bin must fit above the column field");
 // A thread produces FOUR adjacent columns of two rows from three aligned 32-bit words of the (16-byte pitched) image - the
 // fifth column of each row comes from the neighbour lane's word (lane 31 loads it) - so a warp issues 3 (+3) load instructions
 // for 256 pixels instead of 6 for 64.
 __global__ void __launch_bounds__(LSD_GRAD_THREADS) k_lsd_grad(const uint8_t* __restrict__ img, size_t img_stride, int IP, int W, int H,
-                                                               const LsdPix* __restrict__ lut, int m2_min, size_t stride,
+                                                               const float* __restrict__ lut_angle, int m2_min, size_t stride,
                                                                LsdPix* __restrict__ pix, size_t pix_stride,
-                                                               uint32_t* __restrict__ list_idx, uint32_t* __restrict__ list_m2,
-                                                               int* __restrict__ segcnt, int nxb, int* __restrict__ maxmag2) {
+                                                               uint32_t* __restrict__ list, int* __restrict__ segcnt, int nxb,
+                                                               int* __restrict__ maxmag2) {
   const int x4 = blockIdx.x * LSD_SEG + threadIdx.x * 4, y0 = blockIdx.y * 2, im = blockIdx.z;
   const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
   // words of rows y0 .. y0+2 at columns x4 .. x4+3 (rows / words beyond the image read as 0: those pixels are never defined -
@@ -340,8 +353,8 @@ __global__ void __launch_bounds__(LSD_GRAD_THREADS) k_lsd_grad(const uint8_t* __
 #pragma unroll
     for (int c = 0; c < 4; ++c)
       if (li[r][c] >= 0)
-        *reinterpret_cast<float4*>(&pix[(size_t)im * pix_stride + (size_t)(y0 + r) * W + x4 + c]) =
-            __ldg(reinterpret_cast<const float4*>(&lut[li[r][c]]));
+        *reinterpret_cast<uint2*>(&pix[(size_t)im * pix_stride + (size_t)(y0 + r) * W + x4 + c]) =
+            make_uint2(__float_as_uint(__ldg(&lut_angle[li[r][c]])), (uint32_t)li[r][c]);
   // ordered compaction of the two row segments (x ascending) + the per-image maximum: one barrier
   __shared__ int s_max[4], s_c[2][4];
   int cnt[2], incl[2];
@@ -375,8 +388,7 @@ __global__ void __launch_bounds__(LSD_GRAD_THREADS) k_lsd_grad(const uint8_t* __
 #pragma unroll
     for (int c = 0; c < 4; ++c)
       if (li[r][c] >= 0) {
-        list_idx[o] = (uint32_t)((y0 + r) * W + x4 + c);
-        list_m2[o] = (uint32_t)m2v[r][c];
+        list[o] = (uint32_t)(threadIdx.x * 4 + c) | ((uint32_t)m2v[r][c] << LSD_COL_BITS);
         ++o;
       }
   }
@@ -398,12 +410,12 @@ __device__ __forceinline__ double lsd_bin_coef(int maxmag2, int n_bins) {
 
 // The image is cut into chunks of LSD_CHUNK rows.  One CTA bins a chunk: its warps walk the chunk's row-segment lists (written
 // by the gradient kernel: only the defined pixels, ~12 %), turn gx^2 + gy^2 into the bin of the 1024-bin pseudo-ordering
-// (the per-image maximum is known by now) and count the bins; one warp then scatters the chunk's lists in raster order.
+// (the per-image maximum is known by now), store the bin in its place and count the bins; one warp then scatters the
+// chunk's lists in raster order.
 #define LSD_CHUNK 16
 __global__ void __launch_bounds__(256) k_lsd_rowhist(size_t stride, int W, int H, int n_bins, int nchunks, int nxb,
-                                                     const int* __restrict__ maxmag2, const uint32_t* __restrict__ list_m2,
-                                                     const int* __restrict__ segcnt, uint16_t* __restrict__ list_bin,
-                                                     uint32_t* __restrict__ chunkcnt) {
+                                                     const int* __restrict__ maxmag2, uint32_t* __restrict__ list,
+                                                     const int* __restrict__ segcnt, uint32_t* __restrict__ chunkcnt) {
   __shared__ uint32_t hist[LSD_BINS_MAX];
   const int ch = blockIdx.x, im = blockIdx.y, tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
   for (int i = tid; i < n_bins; i += 256) hist[i] = 0;
@@ -417,9 +429,10 @@ __global__ void __launch_bounds__(256) k_lsd_rowhist(size_t stride, int W, int H
     const int n = sc[(size_t)y * nxb + xb];
     const size_t o = (size_t)im * stride + (size_t)y * W + (size_t)xb * LSD_SEG;
     for (int i = lane; i < n; i += 32) {
-      const double norm = sqrt((double)list_m2[o + i] / 4.0);
+      const uint32_t e = list[o + i];
+      const double norm = sqrt((double)(e >> LSD_COL_BITS) / 4.0);
       const int b = (int)(norm * coef);
-      list_bin[o + i] = (uint16_t)b;
+      list[o + i] = (e & ((1u << LSD_COL_BITS) - 1u)) | ((uint32_t)b << LSD_COL_BITS);
       atomicAdd(&hist[b], 1u);
     }
   }
@@ -480,7 +493,7 @@ __global__ void __launch_bounds__(1024) k_lsd_binscan(uint32_t* __restrict__ chu
 }
 
 // one warp per (chunk, image): walks the chunk's row-segment lists in raster order, stable ranks via match_any
-__global__ void __launch_bounds__(128) k_lsd_scatter(const uint32_t* __restrict__ list_idx, const uint16_t* __restrict__ list_bin,
+__global__ void __launch_bounds__(128) k_lsd_scatter(const uint32_t* __restrict__ list,
                                                      const int* __restrict__ segcnt, size_t stride, int W, int H, int n_bins,
                                                      int nchunks, int nxb, const uint32_t* __restrict__ chunkcnt,
                                                      const uint32_t* __restrict__ binstart, uint32_t* __restrict__ order) {
@@ -502,12 +515,14 @@ __global__ void __launch_bounds__(128) k_lsd_scatter(const uint32_t* __restrict_
     const int n = n_next;
     n_next = sg + 1 < nseg ? sc[sg + 1] : 0;
     const int y = ya + sg / nxb, xb = sg - (sg / nxb) * nxb;
-    const size_t o = (size_t)im * stride + (size_t)y * W + (size_t)xb * LSD_SEG;
+    const uint32_t seg0 = (uint32_t)(y * W + xb * LSD_SEG);   // pixel index of the segment's first column
+    const size_t o = (size_t)im * stride + seg0;
     for (int i0 = 0; i0 < n; i0 += 32) {
       const int i = i0 + lane;
       const bool valid = i < n;
-      const uint32_t idx = valid ? list_idx[o + i] : 0u;
-      const int b = valid ? (int)list_bin[o + i] : -1;
+      const uint32_t e = valid ? list[o + i] : 0u;
+      const uint32_t idx = seg0 + (e & ((1u << LSD_COL_BITS) - 1u));
+      const int b = valid ? (int)(e >> LSD_COL_BITS) : -1;
       const unsigned vm = __ballot_sync(0xFFFFFFFFu, valid);
       if (valid) {
         const unsigned peers = __match_any_sync(vm, b);
@@ -539,26 +554,32 @@ __device__ __forceinline__ bool lsd_aligned_rad(double a, double theta, double p
 
 // The warp that grows an image is the only reader and writer of that image's records while the kernel runs, and a CTA
 // never leaves its SM, so L1-cached loads (ld.ca) are coherent with the warp's own stores.
-// Two loads (4 + 8 bytes) rather than one 16-byte load: the 2nd word of the record is not used here, and ptxas recycled
-// the register it would land in (as a ballot result) while the load was still in flight - a write-after-write wait on
-// the load that cost a quarter of the kernel's time.
-struct LsdRec { float a, c, s; };
+struct LsdRec { float a; uint32_t li; };
 __device__ __forceinline__ LsdRec lsd_load_pix(const LsdPix* p) {
-  const float2 cs = __ldca(reinterpret_cast<const float2*>(&p->c));
+  const uint2 v = __ldca(reinterpret_cast<const uint2*>(p));
   LsdRec r;
-  r.a = __ldca(&p->a);
-  r.c = cs.x; r.s = cs.y;
+  r.a = __uint_as_float(v.x);
+  r.li = v.y;
   return r;
 }
 __device__ __forceinline__ void lsd_prefetch(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
+#define LSD_REC_BYTES 8   // sizeof(LsdPix), as the byte stride of the growing kernel's address arithmetic
+static_assert(sizeof(LsdPix) == LSD_REC_BYTES, "LSD record size");
 
 // One warp per image.  Pixels are addressed by their linear index i = y*W + x; the 8 neighbours are i + {-W-1 .. W+1}.
 // No bounds tests are needed: the last column and last row of the map are always NOTDEF (ll_angle), so x-1 / x+1 wrap
 // onto NOTDEF pixels, y+1 stays inside, and a guard of W+1 permanently-NOTDEF records precedes pixel 0 for y-1.
-// Per region point: lanes 0..8 hold the 16-byte records of the 3x3 neighbourhood, fetched two queue entries AHEAD; cells
+// Per region point: lanes 0..8 hold the 8-byte records of the 3x3 neighbourhood, fetched two queue entries AHEAD; cells
 // accepted meanwhile are patched to "used" in the prefetched registers.  The neighbours are decided lane-parallel and
 // re-decided after every acceptance, which reproduces the reference's sequential semantics (each test sees the region
 // angle left by the previous acceptance).
+//
+// Region sums off the decision chain.  A member adds (cosf, sinf) of its angle to the sums S; that pair is lut_cs[li].
+// No acceptance decision reads S (see below: only an evaluation of the region angle and the region's end do), so an
+// accepted cell's lane copies its table entry into a shared-memory ring (cp.async: no register waits on the load), and
+// the staged terms are added in acceptance order only when S is about to be read - one wait per evaluation, not one per
+// acceptance.  A plain load would not do: its register is read by the next addition, which waits for it.
+#define LSD_CSQ 256   // staged terms (ring of float2; a full ring is summed early)
 //
 // Deferred region angle.  The reference recomputes theta_i = fastAtan2(S_i) after every acceptance (S_i = running sum of
 // the members' unit vectors).  Most decisions do not need it: with th = the last angle that WAS evaluated (at sum S_0),
@@ -573,11 +594,13 @@ __device__ __forceinline__ void lsd_prefetch(const void* p) { asm volatile("pref
 #define LSD_MARGIN0 0.05f
 __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size_t pix_stride, size_t stride, int W,
                                                  const uint32_t* __restrict__ order_all, const float2* __restrict__ lut_seed,
+                                                 const float2* __restrict__ lut_cs,
                                                  const int* __restrict__ nseeds, double prec, float prec_deg,
                                                  int min_reg_size, uint32_t* __restrict__ regpts_all,
                                                  uint4* __restrict__ regions_all, int max_regions,
                                                  int* __restrict__ nregions, int* __restrict__ overflow) {
   __shared__ uint32_t q[LSD_QCAP];
+  __shared__ __align__(8) float2 s_cs[LSD_CSQ];   // lut_cs of accepted cells, by acceptance count (qpos)
   const int im = blockIdx.x, lane = threadIdx.x;
   LsdPix* pix = pix_all + (size_t)im * pix_stride;
   const uint32_t* order = order_all + (size_t)im * stride;
@@ -593,7 +616,7 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
   const int ns = nseeds[im];
   const int kk = lane < 9 ? lane : 4;                  // neighbour slot served by this lane (lanes >= 9 idle on the centre)
   const int noff = (kk / 3 - 1) * W + (kk % 3 - 1);   // linear offset of that neighbour (row-major 3x3: reference order)
-  // look-ahead window fetched into L1/L2 whenever a pixel joins the region: 7 rows x 4 sectors around it (the cells the
+  // look-ahead window fetched into L1/L2 whenever a pixel joins the region: 7 rows x 8 records around it (the cells the
   // next two breadth-first layers will examine), one address per lane
   const int poff = lane < 28 ? (lane / 4 - 3) * W + (lane % 4) * 2 - 3 : 0;
   const int pmin = -(W + 1);  // first record of this image (the guard); smaller values mean "nothing fetched"
@@ -604,6 +627,10 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
   const float dmax = prec_deg + LSD_MARGIN0;
   uint32_t cursor = 0;
   int nreg_out = 0;
+  const uint32_t csb = (uint32_t)__cvta_generic_to_shared(&s_cs[0]);
+  // terms staged so far by this warp (ring slot = qpos % LSD_CSQ), and qpos at the last wait for all of them: a slot is
+  // reused only after its copy has been waited for (two outstanding copies to one address would be unordered)
+  uint32_t qpos = 0, qwait = 0;
   uint32_t seed_next = lane < ns ? order[lane] : 0u;
   for (int s0 = 0; s0 < ns; s0 += 32) {
     const int si = s0 + lane;
@@ -632,14 +659,26 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
         regpts[cursor] = sidx;
         asm volatile("st.shared.u32 [%0], %1;" ::"r"(qs), "r"(sidx) : "memory");
       }
-      lsd_prefetch(pb + (long long)((int)sidx + poff) * 16);
+      lsd_prefetch(pb + (long long)((int)sidx + poff) * LSD_REC_BYTES);
       __syncwarp();
       uint32_t nreg = 1;
       // neighbourhood records of queue entries r+1 (pf1) and r+2 (pf2), fetched while earlier entries are processed;
       // a cell accepted meanwhile is patched to "used" in both prefetched copies (i < pmin: nothing fetched)
       LsdRec pf1, pf2;
-      pf1.a = pf2.a = LSD_NOTDEF_F; pf1.c = pf1.s = pf2.c = pf2.s = 0.f;
+      pf1.a = pf2.a = LSD_NOTDEF_F; pf1.li = pf2.li = 0u;
       int i1 = pmin - 1, i2 = pmin - 1;
+      // the region's members whose terms are staged but not yet in S: ring positions [qsum, qpos), in acceptance order
+      uint32_t qsum = qpos;
+      auto add_staged = [&]() {
+        asm volatile("cp.async.wait_all;" ::: "memory");
+        __syncwarp();
+        for (; qsum != qpos; ++qsum) {
+          const float2 e = s_cs[qsum & (LSD_CSQ - 1)];
+          sumdx = __fadd_rn(sumdx, e.x);
+          sumdy = __fadd_rn(sumdy, e.y);
+        }
+        qwait = qpos;
+      };
       for (uint32_t r = 0; r < nreg; ++r) {
         LsdRec cur;
         int ci;
@@ -652,7 +691,7 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
           else pt = __ldcg(&regpts[cursor + r]);
           ci = (int)pt + noff;
           asm volatile("" : "+r"(ci));  // keep the index 32-bit: one IMAD.WIDE forms the address
-          cur = lsd_load_pix(reinterpret_cast<const LsdPix*>(pb + (long long)ci * 16));
+          cur = lsd_load_pix(reinterpret_cast<const LsdPix*>(pb + (long long)ci * LSD_REC_BYTES));
         }
         pf1 = pf2; i1 = i2;
         i2 = pmin - 1;
@@ -662,7 +701,7 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
           else pt = __ldcg(&regpts[cursor + r + 1]);
           i1 = (int)pt + noff;
           asm volatile("" : "+r"(i1));
-          pf1 = lsd_load_pix(reinterpret_cast<const LsdPix*>(pb + (long long)i1 * 16));
+          pf1 = lsd_load_pix(reinterpret_cast<const LsdPix*>(pb + (long long)i1 * LSD_REC_BYTES));
         }
         if (r + 2 < nreg) {
           uint32_t pt;
@@ -670,7 +709,7 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
           else pt = __ldcg(&regpts[cursor + r + 2]);
           i2 = (int)pt + noff;
           asm volatile("" : "+r"(i2));
-          pf2 = lsd_load_pix(reinterpret_cast<const LsdPix*>(pb + (long long)i2 * 16));
+          pf2 = lsd_load_pix(reinterpret_cast<const LsdPix*>(pb + (long long)i2 * LSD_REC_BYTES));
         }
         unsigned rem = __ballot_sync(0xFFFFFFFFu, lane < 9 && cur.a != LSD_NOTDEF_F);
         while (rem) {
@@ -683,6 +722,7 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
           const unsigned mi = __ballot_sync(0xFFFFFFFFu, mine && d < lo);   // certainly aligned
           if (!((mi >> k) & 1u)) {  // the first candidate sits in the band
             if (!fresh) {
+              add_staged();
               th = lsd_fast_atan2(sumdy, sumdx);
               inv0 = __fmul_rn(rsqrtf(__fadd_rn(__fmul_rn(sumdx, sumdx), __fmul_rn(sumdy, sumdy))), 1.02f);
               margin = margin0;
@@ -700,21 +740,24 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
           }
           rem &= ~((2u << k) - 1u);  // k and everything before it have been decided
           const int ai = __shfl_sync(0xFFFFFFFFu, ci, k);
-          const float ck = __shfl_sync(0xFFFFFFFFu, cur.c, k), sk = __shfl_sync(0xFFFFFFFFu, cur.s, k);
           const float dk = __shfl_sync(0xFFFFFFFFu, d, k);
           // lane 0 marks the cell used and appends it to the region / the queue (predicated: no divergent branch)
           asm volatile(
               "{\n\t.reg .pred p;\n\tsetp.ne.s32 p, %0, 0;\n\t"
               "@p st.global.f32 [%1], %2;\n\t@p st.global.u32 [%3], %4;\n\t@p st.shared.u32 [%5], %4;\n\t}"
-              ::"r"(l0), "l"(pb + (long long)ai * 16), "f"(LSD_NOTDEF_F), "l"(regpts + (cursor + nreg)), "r"(ai),
+              ::"r"(l0), "l"(pb + (long long)ai * LSD_REC_BYTES), "f"(LSD_NOTDEF_F), "l"(regpts + (cursor + nreg)), "r"(ai),
                 "r"(qs + ((nreg & (LSD_QCAP - 1)) << 2))
               : "memory");
           ++nreg;
-          lsd_prefetch(pb + (long long)(ai + poff) * 16);
+          lsd_prefetch(pb + (long long)(ai + poff) * LSD_REC_BYTES);
           if (i1 == ai) pf1.a = LSD_NOTDEF_F;  // prefetched copies of this cell are stale
           if (i2 == ai) pf2.a = LSD_NOTDEF_F;
-          sumdx = __fadd_rn(sumdx, ck);
-          sumdy = __fadd_rn(sumdy, sk);
+          // stage the member's term: lane k holds its record (landed: its angle was just tested)
+          if (qpos - qwait == LSD_CSQ) add_staged();   // ring full: its oldest slot is about to be reused
+          if (lane == k)
+            asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(csb + ((qpos & (LSD_CSQ - 1)) << 3)),
+                         "l"(lut_cs + cur.li) : "memory");
+          ++qpos;
           margin = __fmaf_rn(fminf(__fadd_rn(dk, margin), dmax), inv0, margin);
           lo = prec_deg - margin; hi = prec_deg + margin;
           fresh = false;
@@ -723,6 +766,7 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
       }
       if ((int)nreg >= min_reg_size) {
         if (nreg_out < max_regions) {
+          if (!fresh) add_staged();   // the members accepted since S was last read (fresh: none)
           if (lane == 0) {
             // region angle handed to the rectangle fit: the seed's own angle for a 1-pixel region, else the angle of the sum
             const double reg_angle = nreg == 1 ? th_seed : (double)(fresh ? th : lsd_fast_atan2(sumdy, sumdx)) * LSD_DEG2RAD;
@@ -746,9 +790,10 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
 }
 
 #define LSD_GROW_ARGS LsdPix* __restrict__ pix_all, size_t pix_stride, size_t stride, int W, const uint32_t* __restrict__ order_all, \
-    const float2* __restrict__ lut_seed, const int* __restrict__ nseeds, double prec, float prec_deg, int min_reg_size, uint32_t* __restrict__ regpts_all,              \
-    uint4* __restrict__ regions_all, int max_regions, int* __restrict__ nregions, int* __restrict__ overflow
-#define LSD_GROW_PASS pix_all, pix_stride, stride, W, order_all, lut_seed, nseeds, prec, prec_deg, min_reg_size, regpts_all, regions_all, max_regions, nregions, overflow
+    const float2* __restrict__ lut_seed, const float2* __restrict__ lut_cs, const int* __restrict__ nseeds, double prec, float prec_deg, \
+    int min_reg_size, uint32_t* __restrict__ regpts_all, uint4* __restrict__ regions_all, int max_regions, int* __restrict__ nregions,   \
+    int* __restrict__ overflow
+#define LSD_GROW_PASS pix_all, pix_stride, stride, W, order_all, lut_seed, lut_cs, nseeds, prec, prec_deg, min_reg_size, regpts_all, regions_all, max_regions, nregions, overflow
 __global__ void __launch_bounds__(32) k_lsd_grow(LSD_GROW_ARGS) { lsd_grow_body(LSD_GROW_PASS); }
 
 // ---- rectangle fit -------------------------------------------------------------------------------------------
@@ -1007,13 +1052,12 @@ __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ se
 // ---- host side -------------------------------------------------------------------------------------------------
 static void lsd_release(LsdState* s) {
   for (int p = 0; p < 2; ++p) {
-    cudaFree(s->pix_raw[p]); cudaFree(s->order[p]); cudaFree(s->nseeds[p]);
-    cudaFree(s->regpts[p]); cudaFree(s->regions[p]); cudaFree(s->nregions[p]); cudaFree(s->segs[p]); cudaFree(s->kls[p]);
-    cudaFree(s->kls_all[p]); cudaFree(s->nlines[p]);
+    cudaFree(s->pix_raw[p]); cudaFree(s->order[p]); cudaFree(s->nseeds[p]); cudaFree(s->kls[p]); cudaFree(s->nlines[p]);
   }
-  cudaFree(s->blur); cudaFree(s->scaled); cudaFree(s->binmap); cudaFree(s->seedlist); cudaFree(s->seedm2); cudaFree(s->segcnt); cudaFree(s->rect_perm);
+  cudaFree(s->regpts); cudaFree(s->regions); cudaFree(s->nregions); cudaFree(s->segs); cudaFree(s->kls_all);
+  cudaFree(s->blur); cudaFree(s->scaled); cudaFree(s->seedlist); cudaFree(s->segcnt); cudaFree(s->rect_perm);
   cudaFree(s->maxmag2); cudaFree(s->rowcnt); cudaFree(s->binstart); cudaFree(s->overflow); cudaFree(s->rs_tab);
-  cudaFree(s->grad_lut); cudaFree(s->seed_lut);
+  cudaFree(s->angle_lut); cudaFree(s->cs_lut); cudaFree(s->seed_lut);
 }
 
 extern "C" void plf_lsd_free(plf_ctx* ctx) {
@@ -1044,6 +1088,38 @@ static void gaussian_taps_q8(int ksize, double sigma, int* taps) {
     s += v0;
   }
   taps[ksize / 2] = 256 - 2 * s;
+}
+
+// Sizes of the LSD state for nimg images of w x h (scaled ws x hs): the allocation in lsd_prepare and the footprint
+// plf_batch_run weighs the second parity copy by come from here.
+struct LsdSizes {
+  size_t blur, scaled, rowcnt;   // bytes
+  size_t pix_stride, pix_pad, pix_raw;   // records
+  int nxb;
+  size_t once, per_parity;   // bytes of the single-copy buffers / of one parity copy (lookup tables included in once)
+};
+static LsdSizes lsd_sizes(int w, int h, int ws, int hs, int nimg, int n_bins, int max_regions, int max_lines) {
+  LsdSizes z;
+  const size_t N = (size_t)nimg, As = (size_t)ws * hs, R = (size_t)max_regions, L = (size_t)max_lines;
+  z.blur = (size_t)plf_pitch16(w) * h * N + 64;      // + slack: plf_load4 may read the aligned word that holds the
+  z.scaled = (size_t)plf_pitch16(ws) * hs * N + 64;  // last byte of the last image
+  z.rowcnt = N * ((hs + LSD_CHUNK - 1) / LSD_CHUNK) * n_bins * sizeof(uint32_t);
+  z.nxb = (ws + LSD_SEG - 1) / LSD_SEG;
+  z.pix_stride = As + (size_t)ws + 1;
+  z.pix_pad = 3 * (size_t)ws + 8;   // 3 rows + 8 records of slack on both sides: the look-ahead prefetches need no clamping
+  z.pix_raw = z.pix_stride * N + 2 * z.pix_pad;
+  const size_t lut = (size_t)LSD_LUT_DIM * LSD_LUT_DIM * (sizeof(float) + 2 * sizeof(float2));
+  z.once = z.blur + z.scaled + As * N * 4 /* seedlist */ + N * hs * z.nxb * 4 + N * R * 4 /* rect_perm */ + N * 4 + z.rowcnt +
+           N * n_bins * 4 + As * N * 4 /* regpts */ + N * R * (sizeof(uint4) + sizeof(float4) + sizeof(plf_keyline)) + N * 4 + lut;
+  z.per_parity = z.pix_raw * sizeof(LsdPix) + N * 4 + As * N * 4 /* order */ + N * L * sizeof(plf_keyline) + N * 4;
+  return z;
+}
+
+size_t plf_lsd_footprint(const plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
+  const double sc = ctx->params.lsd_scale;
+  const int ws = sc != 1.0 ? (int)nearbyint(w * sc) : w, hs = sc != 1.0 ? (int)nearbyint(h * sc) : h;
+  const LsdSizes z = lsd_sizes(w, h, ws, hs, nimg, ctx->params.lsd_n_bins, ctx->limits.max_segments, ctx->limits.max_lines);
+  return z.once + z.per_parity * (two_parities ? 2 : 1);
 }
 
 static plf_status lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
@@ -1091,48 +1167,43 @@ static plf_status lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
   s->max_regions = ctx->limits.max_segments;
   s->max_lines = ctx->limits.max_lines;
   s->bp = plf_pitch16(w); s->sp = plf_pitch16(s->ws);
-  const size_t N = (size_t)nimg, A = (size_t)s->bp * h, As = (size_t)s->ws * s->hs, Asp = (size_t)s->sp * s->hs;
-  s->pix_stride = As + (size_t)s->ws + 1;
+  const LsdSizes z = lsd_sizes(w, h, s->ws, s->hs, nimg, s->n_bins, s->max_regions, s->max_lines);
+  const size_t N = (size_t)nimg, As = (size_t)s->ws * s->hs;
+  s->pix_stride = z.pix_stride;
   for (s->m2_min = 0; s->m2_min <= 2 * 510 * 510; ++s->m2_min)  // same double expression as the kernels
     if (!(sqrt((double)s->m2_min / 4.0) <= s->rho)) break;
-  PLF_CUDA(ctx, cudaMalloc(&s->blur, A * N + 64));      // + slack: plf_load4 may read the aligned word that holds the
-  PLF_CUDA(ctx, cudaMalloc(&s->scaled, Asp * N + 64));  // last byte of the last image
-  PLF_CUDA(ctx, cudaMalloc(&s->binmap, As * N * sizeof(uint16_t)));
+  PLF_CUDA(ctx, cudaMalloc(&s->blur, z.blur));
+  PLF_CUDA(ctx, cudaMalloc(&s->scaled, z.scaled));
   PLF_CUDA(ctx, cudaMalloc(&s->seedlist, As * N * sizeof(uint32_t)));
-  PLF_CUDA(ctx, cudaMalloc(&s->seedm2, As * N * sizeof(uint32_t)));
-  s->nxb = (s->ws + LSD_SEG - 1) / LSD_SEG;
+  s->nxb = z.nxb;
   PLF_CUDA(ctx, cudaMalloc(&s->segcnt, N * (size_t)s->hs * s->nxb * sizeof(int)));
   PLF_CUDA(ctx, cudaMalloc(&s->rect_perm, N * s->max_regions * sizeof(uint32_t)));
   PLF_CUDA(ctx, cudaMalloc(&s->maxmag2, N * sizeof(int)));
-  PLF_CUDA(ctx, cudaMalloc(&s->rowcnt, N * ((s->hs + LSD_CHUNK - 1) / LSD_CHUNK) * s->n_bins * sizeof(uint32_t)));
+  PLF_CUDA(ctx, cudaMalloc(&s->rowcnt, z.rowcnt));
   PLF_CUDA(ctx, cudaMalloc(&s->binstart, N * s->n_bins * sizeof(uint32_t)));
-  // buffers that cross from the pre-grow phase to the grow / match phases exist twice (parity of the batch), so that
-  // batch i+1 can be extracted while batch i is still growing regions; standalone operators use parity 0 only
+  PLF_CUDA(ctx, cudaMalloc(&s->regpts, As * N * sizeof(uint32_t)));
+  PLF_CUDA(ctx, cudaMalloc(&s->regions, N * s->max_regions * sizeof(uint4)));
+  PLF_CUDA(ctx, cudaMalloc(&s->nregions, N * sizeof(int)));
+  PLF_CUDA(ctx, cudaMalloc(&s->segs, N * s->max_regions * sizeof(float4)));
+  PLF_CUDA(ctx, cudaMalloc(&s->kls_all, N * s->max_regions * sizeof(plf_keyline)));
+  // buffers that cross from the pre-grow phase to the growing (or to the match phase) exist twice (parity of the batch),
+  // so that batch i+1 can be extracted while batch i is still growing regions; standalone operators use parity 0 only
   for (int p = 0; p < (s->two_parities ? 2 : 1); ++p) {
-    // 3 rows + 8 records of slack on both sides: the growing kernel's look-ahead prefetches need no clamping
-    const size_t pad = 3 * (size_t)s->ws + 8;
-    PLF_CUDA(ctx, cudaMalloc(&s->pix_raw[p], (s->pix_stride * N + 2 * pad) * sizeof(LsdPix)));
-    s->pix[p] = s->pix_raw[p] + pad;
-    {
-      const size_t nrec = s->pix_stride * N + 2 * pad;
-      k_lsd_fill_notdef<<<(unsigned)((nrec + 255) / 256), 256, 0, ctx->stream>>>(s->pix_raw[p], nrec);
-    }
+    PLF_CUDA(ctx, cudaMalloc(&s->pix_raw[p], z.pix_raw * sizeof(LsdPix)));
+    s->pix[p] = s->pix_raw[p] + z.pix_pad;
+    k_lsd_fill_notdef<<<(unsigned)((z.pix_raw + 255) / 256), 256, 0, ctx->stream>>>(s->pix_raw[p], z.pix_raw);
     PLF_LAUNCH_CHECK(ctx);
     PLF_CUDA(ctx, cudaMalloc(&s->nseeds[p], N * sizeof(int)));
     PLF_CUDA(ctx, cudaMalloc(&s->order[p], As * N * sizeof(uint32_t)));
-    PLF_CUDA(ctx, cudaMalloc(&s->regpts[p], As * N * sizeof(uint32_t)));
-    PLF_CUDA(ctx, cudaMalloc(&s->regions[p], N * s->max_regions * sizeof(uint4)));
-    PLF_CUDA(ctx, cudaMalloc(&s->nregions[p], N * sizeof(int)));
-    PLF_CUDA(ctx, cudaMalloc(&s->segs[p], N * s->max_regions * sizeof(float4)));
     PLF_CUDA(ctx, cudaMalloc(&s->kls[p], N * s->max_lines * sizeof(plf_keyline)));
-    PLF_CUDA(ctx, cudaMalloc(&s->kls_all[p], N * s->max_regions * sizeof(plf_keyline)));
     PLF_CUDA(ctx, cudaMalloc(&s->nlines[p], N * sizeof(int)));
   }
   PLF_CUDA(ctx, cudaMalloc(&s->overflow, sizeof(int)));
   PLF_CUDA(ctx, cudaMemsetAsync(s->overflow, 0, sizeof(int), ctx->stream));
-  PLF_CUDA(ctx, cudaMalloc(&s->grad_lut, (size_t)LSD_LUT_DIM * LSD_LUT_DIM * sizeof(LsdPix)));
+  PLF_CUDA(ctx, cudaMalloc(&s->angle_lut, (size_t)LSD_LUT_DIM * LSD_LUT_DIM * sizeof(float)));
+  PLF_CUDA(ctx, cudaMalloc(&s->cs_lut, (size_t)LSD_LUT_DIM * LSD_LUT_DIM * sizeof(float2)));
   PLF_CUDA(ctx, cudaMalloc(&s->seed_lut, (size_t)LSD_LUT_DIM * LSD_LUT_DIM * sizeof(float2)));
-  k_lsd_build_lut<<<(LSD_LUT_DIM * LSD_LUT_DIM + 255) / 256, 256, 0, ctx->stream>>>(s->rho, s->grad_lut, s->seed_lut);
+  k_lsd_build_lut<<<(LSD_LUT_DIM * LSD_LUT_DIM + 255) / 256, 256, 0, ctx->stream>>>(s->rho, s->angle_lut, s->cs_lut, s->seed_lut);
   PLF_LAUNCH_CHECK(ctx);
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (s->scale != 1.0) {
@@ -1176,9 +1247,7 @@ plf_status plf_lsd_pre_range(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_str
   uint8_t* blur = s->blur + o * A;
   uint8_t* scaled_buf = s->scaled + o * Asp;
   LsdPix* pix = s->pix[par] + o * s->pix_stride + (s->ws + 1);  // pixel (0,0) of the first image of the range
-  uint16_t* binmap = s->binmap + o * As;
   uint32_t* seedlist = s->seedlist + o * As;
-  uint32_t* seedm2 = s->seedm2 + o * As;
   int* segcnt = s->segcnt + o * (size_t)H * s->nxb;
   int* maxmag2 = s->maxmag2 + o;
   const int nchunks = (H - 1 + LSD_CHUNK - 1) / LSD_CHUNK;
@@ -1224,17 +1293,17 @@ plf_status plf_lsd_pre_range(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_str
     scaled_pitch = s->sp;
   }
   PLF_CUDA(ctx, cudaMemsetAsync(maxmag2, 0xFF, (size_t)n * sizeof(int), cs));  // -1
-  k_lsd_grad<<<dim3(s->nxb, (H + 1) / 2, n), LSD_GRAD_THREADS, 0, cs>>>(scaled, scaled_stride, scaled_pitch, W, H, s->grad_lut, s->m2_min, As, pix, s->pix_stride,
-                                                               seedlist, seedm2, segcnt, s->nxb, maxmag2);
+  k_lsd_grad<<<dim3(s->nxb, (H + 1) / 2, n), LSD_GRAD_THREADS, 0, cs>>>(scaled, scaled_stride, scaled_pitch, W, H, s->angle_lut, s->m2_min, As, pix, s->pix_stride,
+                                                               seedlist, segcnt, s->nxb, maxmag2);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_grad");
-  k_lsd_rowhist<<<dim3(nchunks, n), 256, 0, cs>>>(As, W, H, s->n_bins, nchunks, s->nxb, maxmag2, seedm2, segcnt, binmap, rowcnt);
+  k_lsd_rowhist<<<dim3(nchunks, n), 256, 0, cs>>>(As, W, H, s->n_bins, nchunks, s->nxb, maxmag2, seedlist, segcnt, rowcnt);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_rowhist");
   k_lsd_binscan<<<n, 1024, 0, cs>>>(rowcnt, nchunks, s->n_bins, binstart, nseeds);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_binscan");
-  k_lsd_scatter<<<dim3((nchunks + 3) / 4, n), 128, 0, cs>>>(seedlist, binmap, segcnt, As, W, H, s->n_bins, nchunks, s->nxb, rowcnt, binstart, order);
+  k_lsd_scatter<<<dim3((nchunks + 3) / 4, n), 128, 0, cs>>>(seedlist, segcnt, As, W, H, s->n_bins, nchunks, s->nxb, rowcnt, binstart, order);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_scatter");
   return PLF_OK;
@@ -1250,16 +1319,17 @@ plf_status plf_lsd_grow_range(plf_ctx* ctx, int w, int h, int par, int img0, int
   LsdPix* pix = s->pix[par] + o * s->pix_stride + (s->ws + 1);
   int* nseeds = s->nseeds[par] + o;
   uint32_t* order = s->order[par] + o * As;
-  uint32_t* regpts = s->regpts[par] + o * As;
-  uint4* regions = s->regions[par] + o * s->max_regions;
-  int* nregions = s->nregions[par] + o;
-  float4* segs = s->segs[par] + o * s->max_regions;
+  // one copy: the growing, rectangle and KeyLine kernels of a batch run in stream order before those of the next
+  uint32_t* regpts = s->regpts + o * As;
+  uint4* regions = s->regions + o * s->max_regions;
+  int* nregions = s->nregions + o;
+  float4* segs = s->segs + o * s->max_regions;
   plf_keyline* kls = s->kls[par] + o * s->max_lines;
-  plf_keyline* kls_all = s->kls_all[par] + o * s->max_regions;
+  plf_keyline* kls_all = s->kls_all + o * s->max_regions;
   int* nlines = s->nlines[par] + o;
   // (thread / lane per image, register-capped and unrolled variants and an angle-map layout were all bit-exact and were
   // not kept; DESIGN.md section 5 lists them)
-  k_lsd_grow<<<n, 32, 0, cs>>>(pix, s->pix_stride, As, W, order, s->seed_lut, nseeds, s->prec, (float)(s->p * 180.0), s->min_reg_size, regpts,
+  k_lsd_grow<<<n, 32, 0, cs>>>(pix, s->pix_stride, As, W, order, s->seed_lut, s->cs_lut, nseeds, s->prec, (float)(s->p * 180.0), s->min_reg_size, regpts,
                                regions, s->max_regions, nregions, s->overflow);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_grow");
@@ -1319,13 +1389,13 @@ extern "C" plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   if (st) return st;
   LsdState* s = ctx->lsd;
   int n = 0;
-  PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->nregions[0], sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->nregions, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   st = lsd_check_overflow(ctx, "plf_lsd");
   if (st) return st;
   *n_out = n;
   if (n > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_lsd: %d segments > caller capacity %d", n, cap);
   if (n > 0) {
-    PLF_CUDA(ctx, cudaMemcpyAsync(segs, s->segs[0], (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
+    PLF_CUDA(ctx, cudaMemcpyAsync(segs, s->segs,(size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
     PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   }
   return PLF_OK;

@@ -450,16 +450,22 @@ __global__ void __launch_bounds__(256) k_mg_select(const int32_t* __restrict__ m
   if (!fall_back) m12[((size_t)k * 4 + 2 + which) * K + i] = m12g[((size_t)k * 2 + which) * K + i];
 }
 
-// The LSD hand-off maps (gradient, record, seed order, region points: 28 bytes per scaled pixel) exist once or per batch
-// parity (PLF_LSD_PARITIES = 2).  Per parity the pre-grow chain of batch i+1 (blur, resample, gradient, seed ordering) runs
-// on its own stream while batch i is still growing regions, which takes the pre-grow kernels off the LSD chain.  The second
-// copy costs 28 bytes per scaled pixel of every image of a batch (about 38 MB per KITTI-shape pair, more than half of what
-// a pair takes with one copy), which on an 80 GB H100 cuts the batch that fits by a third; the default stays ONE copy and
-// the memory is left to the batch size.
+// The LSD hand-off maps (8-byte record and seed order: 12 bytes per scaled pixel) exist once or per batch parity.  Per
+// parity the pre-grow chain of batch i+1 (blur, resample, gradient, seed ordering) runs on its own stream while batch i is
+// still growing regions, which takes the pre-grow kernels off the LSD chain.  The second copy costs 12 bytes per scaled
+// pixel of every image of a batch (about 16 MB per KITTI-shape pair); it is made whenever it fits the free device memory
+// with LSD_PARITY_MARGIN to spare.  PLF_LSD_PARITIES = 1 or 2 forces either layout.
+#define LSD_PARITY_MARGIN (4ull << 30)   // room left for what is allocated after the pipeline is prepared (the standalone
+                                         // operators' scratch, the caller's own buffers) and for allocation granularity
 static bool lsd_want_two_parities(const plf_ctx* ctx, int w, int h, int nimg) {
-  (void)ctx; (void)w; (void)h; (void)nimg;
   const char* e = getenv("PLF_LSD_PARITIES");
-  return e && atoi(e) >= 2;
+  if (e && *e) return atoi(e) >= 2;
+  size_t free_b = 0, total_b = 0;
+  if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return plf_lsd_footprint(ctx, w, h, nimg, true) + LSD_PARITY_MARGIN <= free_b;
 }
 
 static plf_status pipe_prepare(plf_ctx* ctx, int w, int h) {
@@ -727,9 +733,10 @@ plf_status plf_batch_run(plf_ctx* ctx, int B) {
   PLF_CUDA(ctx, cudaEventRecord(s->ev_free[run_slot], sE));  // the image buffer may be overwritten by the next upload
 
   // ---- P / G phases: the LSD chain.  P = blur / resize / gradient / seed ordering (bandwidth-bound), G = region growing
-  // (latency bound, one warp per image), rectangle fit and KeyLines.  With the hand-off maps per batch parity (lsd2) P runs
-  // on its own stream: P(i+1) overlaps G(i), and the chain on the critical path is G alone; with one copy (the maps are
-  // 2/3 of the pipeline's memory) P and G share a stream and LSD(i+1) starts when LSD(i) ends. ----
+  // (latency bound, one warp per image), rectangle fit and KeyLines.  With the hand-off maps per batch parity (lsd2, the
+  // default where they fit) P runs on its own stream: P(i+1) overlaps G(i), and the chain on the critical path is G alone;
+  // with one copy P and G share a stream and LSD(i+1) starts when LSD(i) ends.  The buffers only G writes and reads
+  // (region points, regions, segments) exist once either way: G(i+1) follows G(i) on its stream. ----
   ctx->cur = sP;
   PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_up[run_slot], 0));
   if (lsd2) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->evG[par], 0));   // batch i-2 (same parity) has finished growing / fitting on these maps

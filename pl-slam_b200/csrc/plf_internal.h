@@ -170,6 +170,7 @@ void plf_resize_pack_x(const int* ofs, const int* c1, int dw, int* out);   // ou
 
 // ---- LSD (lsd.cu) --------------------------------------------------------------------------------
 plf_status plf_lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities);
+size_t plf_lsd_footprint(const plf_ctx* ctx, int w, int h, int nimg, bool two_parities);   // bytes plf_lsd_prepare allocates
 plf_status plf_lsd_run(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int nimg);
 plf_status plf_lsd_pre_range(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int par, int img0, int n);
 plf_status plf_lsd_grow_range(plf_ctx* ctx, int w, int h, int par, int img0, int n);
