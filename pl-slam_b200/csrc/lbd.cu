@@ -31,10 +31,7 @@
 plf_status plf_lbd_init(plf_ctx* ctx);
 
 struct LbdState {
-  // cached tensor maps of the source images of k_blur5_sobel_fast (the pipeline alternates between two upload buffers)
-  const void* tm_src[2] = {nullptr, nullptr};
-  CUtensorMap tm[2];
-  size_t tm_stride = 0; int tm_pitch = 0, tm_w = 0, tm_h = 0, tm_nimg = 0;
+  PlfTmaCache tm;   // source images of k_blur5_sobel_fast
 };
 
 __constant__ float c_gaussL[21];  // (float)gaussCoefL_[i]
@@ -45,15 +42,6 @@ static const int h_comb[32][2] = {
     {0, 1}, {0, 2}, {0, 3}, {0, 4}, {0, 5}, {0, 6}, {1, 2}, {1, 3}, {1, 4}, {1, 5}, {1, 6},
     {2, 3}, {2, 4}, {2, 5}, {2, 6}, {2, 7}, {2, 8}, {3, 4}, {3, 5}, {3, 6}, {3, 7}, {3, 8},
     {4, 5}, {4, 6}, {4, 7}, {4, 8}, {5, 6}, {5, 7}, {5, 8}, {6, 7}, {6, 8}, {7, 8}};
-
-__device__ __forceinline__ int reflect101(int i, int n) {
-  if (n == 1) return 0;
-  while (i < 0 || i >= n) {  // iterates more than once only for images narrower than the halo
-    if (i < 0) i = -i;
-    if (i >= n) i = 2 * (n - 1) - i;
-  }
-  return i;
-}
 
 // grid: (ceil(w/64), ceil(h/16), nimg); block 256
 __global__ void __launch_bounds__(256) k_blur5_sobel(const uint8_t* __restrict__ imgs, int pitch,
@@ -70,9 +58,9 @@ __global__ void __launch_bounds__(256) k_blur5_sobel(const uint8_t* __restrict__
   const int lane = tid & 31, wrp = tid >> 5;
   const bool interior = x0 >= 3 && x0 + LBD_TW + 3 <= w && y0 >= 3 && y0 + LBD_TH + 3 <= h;
   for (int ry = wrp; ry < LBD_TH + 6; ry += 8) {
-    const int gy = interior ? y0 - 3 + ry : reflect101(y0 - 3 + ry, h);
+    const int gy = interior ? y0 - 3 + ry : plf_reflect101(y0 - 3 + ry, h);
     const uint8_t* row = img + (size_t)gy * pitch;
-    for (int rx = lane; rx < LBD_TW + 6; rx += 32) raw[ry][rx] = row[interior ? x0 - 3 + rx : reflect101(x0 - 3 + rx, w)];
+    for (int rx = lane; rx < LBD_TW + 6; rx += 32) raw[ry][rx] = row[interior ? x0 - 3 + rx : plf_reflect101(x0 - 3 + rx, w)];
   }
   __syncthreads();
   // horizontal 5-tap pass for halo-1 columns, all halo-3 rows (66 columns: lanes 0..31 take cx, cx+32, and 64/65)
@@ -206,21 +194,10 @@ plf_status plf_launch_blur5_sobel(plf_ctx* ctx, const uint8_t* imgs, int pitch, 
   if (w >= 8 && h >= 8 && (pitch & 15) == 0 && (img_stride & 15) == 0 && ((uintptr_t)imgs & 15) == 0) {
     plf_status st0 = plf_lbd_init(ctx);
     if (st0) return st0;
-    LbdState* s = ctx->lbd;
-    if (s->tm_stride != img_stride || s->tm_pitch != pitch || s->tm_w != w || s->tm_h != h || s->tm_nimg < nimg) {
-      s->tm_src[0] = s->tm_src[1] = nullptr;
-      s->tm_stride = img_stride; s->tm_pitch = pitch; s->tm_w = w; s->tm_h = h; s->tm_nimg = nimg;
-    }
-    int slot = -1;
-    for (int k = 0; k < 2; ++k) if (s->tm_src[k] == imgs) slot = k;
-    if (slot < 0) {
-      slot = s->tm_src[0] ? (s->tm_src[1] ? 0 : 1) : 0;
-      if (!plf_tma_encode_u8(&s->tm[slot], imgs, w, h, s->tm_nimg, pitch, img_stride ? img_stride : (size_t)pitch * h, 80, LBF_TH + 6))
-        return plf_fail(ctx, PLF_ERR_CUDA, "LBD: cuTensorMapEncodeTiled failed (pitch %d, stride %zu)", pitch, img_stride);
-      s->tm_src[slot] = imgs;
-    }
+    const CUtensorMap* tm = ctx->lbd->tm.get(imgs, w, h, nimg, pitch, img_stride ? img_stride : (size_t)pitch * h, 80, LBF_TH + 6);
+    if (!tm) return plf_fail(ctx, PLF_ERR_CUDA, "LBD: cuTensorMapEncodeTiled failed (pitch %d, stride %zu)", pitch, img_stride);
     dim3 grid(plf_tma_tiles_x(w, 3), (h + LBF_TH - 1) / LBF_TH, nimg);
-    k_blur5_sobel_fast<<<grid, 256, 0, ctx->cur>>>(s->tm[slot], w, h, grad, grad_stride);
+    k_blur5_sobel_fast<<<grid, 256, 0, ctx->cur>>>(*tm, w, h, grad, grad_stride);
   } else {  // tiny images / unpadded rows: generic kernel
     dim3 grid((w + LBD_TW - 1) / LBD_TW, (h + LBD_TH - 1) / LBD_TH, nimg);
     k_blur5_sobel<<<grid, 256, 0, ctx->cur>>>(imgs, pitch, img_stride, w, h, grad, grad_stride);

@@ -11,8 +11,10 @@
 // inside a bin) -> greedy region growing -> rectangle fit.  No NFA validation runs at refine 0.
 //
 // Kernels
-//   k_blur_q8_fast   separable Q8.8 Gaussian (tile + halo staged by one TMA bulk-tensor copy, DP4A row pass), one rounding
-//                    (k_blur_q8: generic variant for tiny images)
+//   k_lsd_build_lut / k_lsd_fill_notdef
+//                    once per state: the gradient lookup tables, and every record of the record maps set to "undefined"
+//   k_blur_q8_fast   separable Q8.8 Gaussian of 5 or 7 taps <= 255 (tile + halo staged by one TMA bulk-tensor copy, DP4A
+//                    row pass), one rounding (k_blur_q8: generic variant for the other kernels, up to 15 taps)
 //   k_resize_exact4  (orb.cu) INTER_LINEAR_EXACT resample to scale
 //   k_lsd_grad       2x2 gradient; for the DEFINED pixels only (|grad| > rho, ~12 %): the 8-byte record {angle
 //                    (cv::fastAtan2, degrees, f32, from a table keyed by (gx,gy)), table index}, and one packed entry
@@ -28,7 +30,7 @@
 //                    look-ahead prefetch), the alignment tests run lane-parallel in the reference order, and the
 //                    region angle is only evaluated when a decision depends on it (see the kernel's comment; bit-exact).
 //                    The (cosf, sinf) a member adds to the region's sums comes from a table keyed by the record's index,
-//                    loaded off the decision chain and added one queue entry later, in the reference's order.
+//                    staged in a shared-memory ring by cp.async and added, in the reference's order, when the sums are read.
 //                    `used` is folded into the angle (a used pixel gets the NOTDEF sentinel).
 //   k_lsd_rect_order / k_lsd_rects
 //                    one thread per region, regions permuted into size classes: weighted centroid, inertia-matrix
@@ -66,9 +68,7 @@ struct LsdState {
   uint8_t* blur = nullptr;    // [nimg][h][bp]   bp = plf_pitch16(w)
   uint8_t* scaled = nullptr;  // [nimg][hs][sp]  sp = plf_pitch16(ws)
   int bp = 0, sp = 0;
-  const void* tm_src[2] = {nullptr, nullptr};   // source buffers the cached tensor maps were encoded for
-  CUtensorMap tm_blur[2];
-  size_t tm_stride = 0; int tm_pitch = 0, tm_nimg = 0;
+  PlfTmaCache tm_blur;        // source images of k_blur_q8_fast
   uint32_t* rect_perm = nullptr;  // [nimg][max_regions] regions in size-class order (k_lsd_rect_order)
   struct LsdPix* pix_raw[2] = {nullptr, nullptr};  // allocation (pix + look-ahead slack on both sides)
   struct LsdPix* pix[2] = {nullptr, nullptr};  // [nimg][guard + hs*ws]  {angle (deg, f32) | NOTDEF = undefined/used, table index}
@@ -99,18 +99,10 @@ struct LsdState {
   float* angle_lut = nullptr;   // [1021*1021] gradient (gx,gy) -> level-line angle (degrees) of a defined pixel
   float2* cs_lut = nullptr;     // [1021*1021] gradient (gx,gy) -> (cosf, sinf) of float(angle in radians): a member's term of the region sums
   float2* seed_lut = nullptr;   // [1021*1021] gradient (gx,gy) -> unit vector of a region seed
+  DevBufList bufs;
 };
 
 __constant__ int c_lsd_taps[16];
-
-__device__ __forceinline__ int lsd_reflect101(int i, int n) {
-  if (n == 1) return 0;
-  while (i < 0 || i >= n) {
-    if (i < 0) i = -i;
-    if (i >= n) i = 2 * (n - 1) - i;
-  }
-  return i;
-}
 
 // ---- fixed-point Gaussian (ksize <= 15) ------------------------------------------------------------------
 #define BQ_TW 64
@@ -127,9 +119,9 @@ __global__ void __launch_bounds__(256) k_blur_q8(const uint8_t* __restrict__ src
   const int lane = tid & 31, wrp = tid >> 5;
   const bool interior = x0 >= r && x0 + BQ_TW + r <= w && y0 >= r && y0 + BQ_TH + r <= h;
   for (int ry = wrp; ry < RH; ry += 8) {  // one warp per row, lanes along x
-    const int gy = interior ? y0 - r + ry : lsd_reflect101(y0 - r + ry, h);
+    const int gy = interior ? y0 - r + ry : plf_reflect101(y0 - r + ry, h);
     const uint8_t* row = s + (size_t)gy * pitch;
-    for (int rx = lane; rx < RW; rx += 32) raw[ry][rx] = row[interior ? x0 - r + rx : lsd_reflect101(x0 - r + rx, w)];
+    for (int rx = lane; rx < RW; rx += 32) raw[ry][rx] = row[interior ? x0 - r + rx : plf_reflect101(x0 - r + rx, w)];
   }
   __syncthreads();
   const int ks = 2 * r + 1;
@@ -1050,19 +1042,9 @@ __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ se
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------
-static void lsd_release(LsdState* s) {
-  for (int p = 0; p < 2; ++p) {
-    cudaFree(s->pix_raw[p]); cudaFree(s->order[p]); cudaFree(s->nseeds[p]); cudaFree(s->kls[p]); cudaFree(s->nlines[p]);
-  }
-  cudaFree(s->regpts); cudaFree(s->regions); cudaFree(s->nregions); cudaFree(s->segs); cudaFree(s->kls_all);
-  cudaFree(s->blur); cudaFree(s->scaled); cudaFree(s->seedlist); cudaFree(s->segcnt); cudaFree(s->rect_perm);
-  cudaFree(s->maxmag2); cudaFree(s->rowcnt); cudaFree(s->binstart); cudaFree(s->overflow); cudaFree(s->rs_tab);
-  cudaFree(s->angle_lut); cudaFree(s->cs_lut); cudaFree(s->seed_lut);
-}
-
 extern "C" void plf_lsd_free(plf_ctx* ctx) {
   if (ctx->lsd) {
-    lsd_release(ctx->lsd);
+    ctx->lsd->bufs.release();
     delete ctx->lsd;
     ctx->lsd = nullptr;
   }
@@ -1090,36 +1072,69 @@ static void gaussian_taps_q8(int ksize, double sigma, int* taps) {
   taps[ksize / 2] = 256 - 2 * s;
 }
 
-// Sizes of the LSD state for nimg images of w x h (scaled ws x hs): the allocation in lsd_prepare and the footprint
-// plf_batch_run weighs the second parity copy by come from here.
-struct LsdSizes {
-  size_t blur, scaled, rowcnt;   // bytes
-  size_t pix_stride, pix_pad, pix_raw;   // records
-  int nxb;
-  size_t once, per_parity;   // bytes of the single-copy buffers / of one parity copy (lookup tables included in once)
-};
-static LsdSizes lsd_sizes(int w, int h, int ws, int hs, int nimg, int n_bins, int max_regions, int max_lines) {
-  LsdSizes z;
-  const size_t N = (size_t)nimg, As = (size_t)ws * hs, R = (size_t)max_regions, L = (size_t)max_lines;
-  z.blur = (size_t)plf_pitch16(w) * h * N + 64;      // + slack: plf_load4 may read the aligned word that holds the
-  z.scaled = (size_t)plf_pitch16(ws) * hs * N + 64;  // last byte of the last image
-  z.rowcnt = N * ((hs + LSD_CHUNK - 1) / LSD_CHUNK) * n_bins * sizeof(uint32_t);
-  z.nxb = (ws + LSD_SEG - 1) / LSD_SEG;
-  z.pix_stride = As + (size_t)ws + 1;
-  z.pix_pad = 3 * (size_t)ws + 8;   // 3 rows + 8 records of slack on both sides: the look-ahead prefetches need no clamping
-  z.pix_raw = z.pix_stride * N + 2 * z.pix_pad;
-  const size_t lut = (size_t)LSD_LUT_DIM * LSD_LUT_DIM * (sizeof(float) + 2 * sizeof(float2));
-  z.once = z.blur + z.scaled + As * N * 4 /* seedlist */ + N * hs * z.nxb * 4 + N * R * 4 /* rect_perm */ + N * 4 + z.rowcnt +
-           N * n_bins * 4 + As * N * 4 /* regpts */ + N * R * (sizeof(uint4) + sizeof(float4) + sizeof(plf_keyline)) + N * 4 + lut;
-  z.per_parity = z.pix_raw * sizeof(LsdPix) + N * 4 + As * N * 4 /* order */ + N * L * sizeof(plf_keyline) + N * 4;
-  return z;
+// The sizes an LSD state for nimg images of w x h takes from the context's parameters and limits.
+static void lsd_set_sizes(const plf_ctx* ctx, LsdState* s, int w, int h, int nimg, bool two_parities) {
+  s->w = w; s->h = h; s->nimg = nimg;
+  s->two_parities = two_parities;
+  s->scale = ctx->params.lsd_scale;
+  s->n_bins = ctx->params.lsd_n_bins;
+  s->ws = s->scale != 1.0 ? (int)nearbyint(w * s->scale) : w;
+  s->hs = s->scale != 1.0 ? (int)nearbyint(h * s->scale) : h;
+  s->max_regions = ctx->limits.max_segments;
+  s->max_lines = ctx->limits.max_lines;
+}
+
+// Records of one record map: nimg images of pix_stride records, plus 3 rows + 8 records of slack on both sides (the
+// look-ahead prefetches need no clamping).
+static size_t lsd_pix_pad(const LsdState* s) { return 3 * (size_t)s->ws + 8; }
+static size_t lsd_pix_records(const LsdState* s) { return s->pix_stride * s->nimg + 2 * lsd_pix_pad(s); }
+
+// The device buffers of an LSD state whose sizes are set (lsd_set_sizes), and the layout derived from those sizes.
+static void lsd_buffers(LsdState* s, DevBufList& b) {
+  const size_t N = (size_t)s->nimg, As = (size_t)s->ws * s->hs, R = (size_t)s->max_regions, LUT = (size_t)LSD_LUT_DIM * LSD_LUT_DIM;
+  s->bp = plf_pitch16(s->w); s->sp = plf_pitch16(s->ws);
+  s->nxb = (s->ws + LSD_SEG - 1) / LSD_SEG;
+  s->pix_stride = As + (size_t)s->ws + 1;
+  b.add(s->blur, (size_t)s->bp * s->h * N);
+  b.add(s->scaled, (size_t)s->sp * s->hs * N);
+  b.add(s->seedlist, As * N);
+  b.add(s->segcnt, N * s->hs * s->nxb);
+  b.add(s->rect_perm, N * R);
+  b.add(s->maxmag2, N);
+  b.add(s->rowcnt, N * ((s->hs + LSD_CHUNK - 1) / LSD_CHUNK) * s->n_bins);
+  b.add(s->binstart, N * s->n_bins);
+  b.add(s->regpts, As * N);
+  b.add(s->regions, N * R);
+  b.add(s->nregions, N);
+  b.add(s->segs, N * R);
+  b.add(s->kls_all, N * R);
+  // buffers that cross from the pre-grow phase to the growing (or to the match phase) exist twice (parity of the batch),
+  // so that batch i+1 can be extracted while batch i is still growing regions; standalone operators use parity 0 only
+  for (int p = 0; p < (s->two_parities ? 2 : 1); ++p) {
+    b.add(s->pix_raw[p], lsd_pix_records(s));
+    b.add(s->nseeds[p], N);
+    b.add(s->order[p], As * N);
+    b.add(s->kls[p], N * s->max_lines);
+    b.add(s->nlines[p], N);
+  }
+  b.add(s->overflow, 1);
+  b.add(s->angle_lut, LUT);
+  b.add(s->cs_lut, LUT);
+  b.add(s->seed_lut, LUT);
+  if (s->scale != 1.0) {
+    s->rs_x_off = 0;
+    s->rs_y_off = 2 * (size_t)s->ws;
+    s->rs_xp_off = (s->rs_y_off + 2 * (size_t)s->hs + 3) & ~(size_t)3;   // 16-byte aligned: read with 128-bit loads
+    b.add(s->rs_tab, s->rs_xp_off + plf_resize_packed_len(s->ws));
+  }
 }
 
 size_t plf_lsd_footprint(const plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
-  const double sc = ctx->params.lsd_scale;
-  const int ws = sc != 1.0 ? (int)nearbyint(w * sc) : w, hs = sc != 1.0 ? (int)nearbyint(h * sc) : h;
-  const LsdSizes z = lsd_sizes(w, h, ws, hs, nimg, ctx->params.lsd_n_bins, ctx->limits.max_segments, ctx->limits.max_lines);
-  return z.once + z.per_parity * (two_parities ? 2 : 1);
+  LsdState z;
+  lsd_set_sizes(ctx, &z, w, h, nimg, two_parities);
+  DevBufList b;
+  lsd_buffers(&z, b);
+  return b.bytes();
 }
 
 static plf_status lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
@@ -1128,7 +1143,7 @@ static plf_status lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
   if (s && s->two_parities) two_parities = true;
   if (s) {
     PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    lsd_release(s);
+    s->bufs.release();
     *s = LsdState();
   } else {
     s = ctx->lsd = new LsdState();
@@ -1138,10 +1153,7 @@ static plf_status lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
     return plf_fail(ctx, PLF_ERR_INVALID, "LSD: only lsd_refine = 0 (LSD_REFINE_NONE, the reference configs) is supported");
   if (P.lsd_n_bins < 1 || P.lsd_n_bins > LSD_BINS_MAX)
     return plf_fail(ctx, PLF_ERR_INVALID, "LSD: lsd_n_bins must be in [1,%d]", LSD_BINS_MAX);
-  s->w = w; s->h = h; s->nimg = nimg;
-  s->two_parities = two_parities;
-  s->scale = P.lsd_scale;
-  s->n_bins = P.lsd_n_bins;
+  lsd_set_sizes(ctx, s, w, h, nimg, two_parities);
   s->prec = LSD_PI * P.lsd_ang_th / 180;
   s->p = P.lsd_ang_th / 180;
   s->rho = P.lsd_quant / sin(s->prec);
@@ -1153,69 +1165,33 @@ static plf_status lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
     gaussian_taps_q8(s->ksize, sigma, s->taps);
     s->taps_u8 = true;
     for (int k = 0; k < s->ksize; ++k) s->taps_u8 = s->taps_u8 && s->taps[k] <= 255;
-    s->ws = (int)nearbyint(w * s->scale);
-    s->hs = (int)nearbyint(h * s->scale);
   } else {
     s->ksize = 0;
-    s->ws = w;
-    s->hs = h;
   }
   if (s->ws >= 65536 || s->hs >= 65536 || s->ws < 3 || s->hs < 3)
     return plf_fail(ctx, PLF_ERR_INVALID, "LSD: scaled image %dx%d out of range", s->ws, s->hs);
   const double LOG_NT = 5 * (log10((double)s->ws) + log10((double)s->hs)) / 2 + log10(11.0);
   s->min_reg_size = (int)(size_t)(-LOG_NT / log10(s->p));
-  s->max_regions = ctx->limits.max_segments;
-  s->max_lines = ctx->limits.max_lines;
-  s->bp = plf_pitch16(w); s->sp = plf_pitch16(s->ws);
-  const LsdSizes z = lsd_sizes(w, h, s->ws, s->hs, nimg, s->n_bins, s->max_regions, s->max_lines);
-  const size_t N = (size_t)nimg, As = (size_t)s->ws * s->hs;
-  s->pix_stride = z.pix_stride;
   for (s->m2_min = 0; s->m2_min <= 2 * 510 * 510; ++s->m2_min)  // same double expression as the kernels
     if (!(sqrt((double)s->m2_min / 4.0) <= s->rho)) break;
-  PLF_CUDA(ctx, cudaMalloc(&s->blur, z.blur));
-  PLF_CUDA(ctx, cudaMalloc(&s->scaled, z.scaled));
-  PLF_CUDA(ctx, cudaMalloc(&s->seedlist, As * N * sizeof(uint32_t)));
-  s->nxb = z.nxb;
-  PLF_CUDA(ctx, cudaMalloc(&s->segcnt, N * (size_t)s->hs * s->nxb * sizeof(int)));
-  PLF_CUDA(ctx, cudaMalloc(&s->rect_perm, N * s->max_regions * sizeof(uint32_t)));
-  PLF_CUDA(ctx, cudaMalloc(&s->maxmag2, N * sizeof(int)));
-  PLF_CUDA(ctx, cudaMalloc(&s->rowcnt, z.rowcnt));
-  PLF_CUDA(ctx, cudaMalloc(&s->binstart, N * s->n_bins * sizeof(uint32_t)));
-  PLF_CUDA(ctx, cudaMalloc(&s->regpts, As * N * sizeof(uint32_t)));
-  PLF_CUDA(ctx, cudaMalloc(&s->regions, N * s->max_regions * sizeof(uint4)));
-  PLF_CUDA(ctx, cudaMalloc(&s->nregions, N * sizeof(int)));
-  PLF_CUDA(ctx, cudaMalloc(&s->segs, N * s->max_regions * sizeof(float4)));
-  PLF_CUDA(ctx, cudaMalloc(&s->kls_all, N * s->max_regions * sizeof(plf_keyline)));
-  // buffers that cross from the pre-grow phase to the growing (or to the match phase) exist twice (parity of the batch),
-  // so that batch i+1 can be extracted while batch i is still growing regions; standalone operators use parity 0 only
+  lsd_buffers(s, s->bufs);
+  plf_status st = s->bufs.alloc(ctx, "LSD");
+  if (st) return st;
   for (int p = 0; p < (s->two_parities ? 2 : 1); ++p) {
-    PLF_CUDA(ctx, cudaMalloc(&s->pix_raw[p], z.pix_raw * sizeof(LsdPix)));
-    s->pix[p] = s->pix_raw[p] + z.pix_pad;
-    k_lsd_fill_notdef<<<(unsigned)((z.pix_raw + 255) / 256), 256, 0, ctx->stream>>>(s->pix_raw[p], z.pix_raw);
+    s->pix[p] = s->pix_raw[p] + lsd_pix_pad(s);
+    k_lsd_fill_notdef<<<(unsigned)((lsd_pix_records(s) + 255) / 256), 256, 0, ctx->stream>>>(s->pix_raw[p], lsd_pix_records(s));
     PLF_LAUNCH_CHECK(ctx);
-    PLF_CUDA(ctx, cudaMalloc(&s->nseeds[p], N * sizeof(int)));
-    PLF_CUDA(ctx, cudaMalloc(&s->order[p], As * N * sizeof(uint32_t)));
-    PLF_CUDA(ctx, cudaMalloc(&s->kls[p], N * s->max_lines * sizeof(plf_keyline)));
-    PLF_CUDA(ctx, cudaMalloc(&s->nlines[p], N * sizeof(int)));
   }
-  PLF_CUDA(ctx, cudaMalloc(&s->overflow, sizeof(int)));
   PLF_CUDA(ctx, cudaMemsetAsync(s->overflow, 0, sizeof(int), ctx->stream));
-  PLF_CUDA(ctx, cudaMalloc(&s->angle_lut, (size_t)LSD_LUT_DIM * LSD_LUT_DIM * sizeof(float)));
-  PLF_CUDA(ctx, cudaMalloc(&s->cs_lut, (size_t)LSD_LUT_DIM * LSD_LUT_DIM * sizeof(float2)));
-  PLF_CUDA(ctx, cudaMalloc(&s->seed_lut, (size_t)LSD_LUT_DIM * LSD_LUT_DIM * sizeof(float2)));
   k_lsd_build_lut<<<(LSD_LUT_DIM * LSD_LUT_DIM + 255) / 256, 256, 0, ctx->stream>>>(s->rho, s->angle_lut, s->cs_lut, s->seed_lut);
   PLF_LAUNCH_CHECK(ctx);
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (s->scale != 1.0) {
     PLF_CUDA(ctx, cudaMemcpyToSymbolAsync(c_lsd_taps, s->taps, sizeof(int) * 16, 0, cudaMemcpyHostToDevice, ctx->stream));
-    s->rs_x_off = 0;
-    s->rs_y_off = 2 * (size_t)s->ws;
-    s->rs_xp_off = (s->rs_y_off + 2 * (size_t)s->hs + 3) & ~(size_t)3;   // 16-byte aligned: read with 128-bit loads
     std::vector<int> tab(s->rs_xp_off + plf_resize_packed_len(s->ws));
     plf_linear_coeffs_host(w, s->ws, 1.0 / s->scale, &tab[0], &tab[s->ws]);
     plf_linear_coeffs_host(h, s->hs, 1.0 / s->scale, &tab[s->rs_y_off], &tab[s->rs_y_off + s->hs]);
     plf_resize_pack_x(&tab[0], &tab[s->ws], s->ws, &tab[s->rs_xp_off]);
-    PLF_CUDA(ctx, cudaMalloc(&s->rs_tab, tab.size() * sizeof(int)));
     PLF_CUDA(ctx, cudaMemcpyAsync(s->rs_tab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   }
@@ -1226,124 +1202,96 @@ static plf_status lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
 plf_status plf_lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
   const plf_status st = lsd_prepare(ctx, w, h, nimg, two_parities);
   if (st && ctx->lsd) {
-    lsd_release(ctx->lsd);
+    ctx->lsd->bufs.release();
     *ctx->lsd = LsdState();
   }
   return st;
 }
 
-// LSD on images [img0, img0+n) of a batch resident on the device, in two phases so that callers can overlap them with
-// other work: `pre` = blur, resample, gradient and seed ordering (bandwidth-bound), `grow` = region growing, rectangle
-// fit and the KeyLine stage (latency-bound).  `par` selects the buffer set that carries data from pre to grow.
-// State must be prepared for >= img0+n images.  Enqueued on ctx->cur; results stay on the device.
-plf_status plf_lsd_pre_range(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int par, int img0, int n) {
+// LSD on images [0, n) of a batch resident on the device, in two phases so that callers can overlap them with other
+// work: `pre` = blur, resample, gradient and seed ordering (bandwidth-bound), `grow` = region growing, rectangle fit and
+// the KeyLine stage (latency-bound).  `par` selects the buffer set that carries data from pre to grow.  State must be
+// prepared for >= n images.  Enqueued on ctx->cur; results stay on the device.
+plf_status plf_lsd_pre(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int par, int n) {
   LsdState* s = ctx->lsd;
-  if (!s || s->w != w || s->h != h || s->nimg < img0 + n || (par && !s->two_parities))
-    return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_pre_range: state not prepared for this image range");
+  if (!s || s->w != w || s->h != h || s->nimg < n || (par && !s->two_parities))
+    return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_pre: state not prepared for these images");
   cudaStream_t cs = ctx->cur;
   const int W = s->ws, H = s->hs;
-  const size_t As = (size_t)W * H, A = (size_t)s->bp * h, Asp = (size_t)s->sp * H, o = (size_t)img0;
-  const uint8_t* imgs = d_imgs + o * img_stride;
-  uint8_t* blur = s->blur + o * A;
-  uint8_t* scaled_buf = s->scaled + o * Asp;
-  LsdPix* pix = s->pix[par] + o * s->pix_stride + (s->ws + 1);  // pixel (0,0) of the first image of the range
-  uint32_t* seedlist = s->seedlist + o * As;
-  int* segcnt = s->segcnt + o * (size_t)H * s->nxb;
-  int* maxmag2 = s->maxmag2 + o;
+  const size_t As = (size_t)W * H, A = (size_t)s->bp * h, Asp = (size_t)s->sp * H;
+  LsdPix* pix = s->pix[par] + (s->ws + 1);  // pixel (0,0) of the first image
   const int nchunks = (H - 1 + LSD_CHUNK - 1) / LSD_CHUNK;
-  uint32_t* rowcnt = s->rowcnt + o * nchunks * s->n_bins;
-  uint32_t* binstart = s->binstart + o * s->n_bins;
-  int* nseeds = s->nseeds[par] + o;
-  uint32_t* order = s->order[par] + o * As;
   plf_status st;
-  const uint8_t* scaled = imgs;
+  const uint8_t* scaled = d_imgs;
   size_t scaled_stride = img_stride;
   int scaled_pitch = pitch;
   if (s->scale != 1.0) {
     if ((s->ksize == 7 || s->ksize == 5) && s->taps_u8) {
-      // tensor map of the source images (two cached slots: the pipeline alternates between its two upload buffers)
-      if (s->tm_stride != img_stride || s->tm_pitch != pitch || s->tm_nimg < img0 + n) {
-        s->tm_src[0] = s->tm_src[1] = nullptr;
-        s->tm_stride = img_stride; s->tm_pitch = pitch; s->tm_nimg = std::max(s->nimg, img0 + n);
-      }
-      int slot = -1;
-      for (int k = 0; k < 2; ++k) if (s->tm_src[k] == d_imgs) slot = k;
-      if (slot < 0) {
-        slot = s->tm_src[0] ? (s->tm_src[1] ? 0 : 1) : 0;
-        if (!plf_tma_encode_u8(&s->tm_blur[slot], d_imgs, w, h, s->tm_nimg, pitch, img_stride, 80, BF_TH + s->ksize - 1))
-          return plf_fail(ctx, PLF_ERR_CUDA, "LSD: cuTensorMapEncodeTiled failed for the source images (pitch %d, stride %zu)", pitch, img_stride);
-        s->tm_src[slot] = d_imgs;
-      }
+      const CUtensorMap* tm = s->tm_blur.get(d_imgs, w, h, n, pitch, img_stride, 80, BF_TH + s->ksize - 1);
+      if (!tm)
+        return plf_fail(ctx, PLF_ERR_CUDA, "LSD: cuTensorMapEncodeTiled failed for the source images (pitch %d, stride %zu)", pitch, img_stride);
       uint32_t tA = 0, tB = 0;
       for (int k = 0; k < s->ksize; ++k) (k < 4 ? tA : tB) |= (uint32_t)s->taps[k] << (8 * (k & 3));
       dim3 gf(plf_tma_tiles_x(w, s->ksize / 2), (h + BF_TH - 1) / BF_TH, n);
-      if (s->ksize == 7) k_blur_q8_fast<7><<<gf, 256, 0, cs>>>(s->tm_blur[slot], img0, w, h, tA, tB, blur, A, s->bp);
-      else k_blur_q8_fast<5><<<gf, 256, 0, cs>>>(s->tm_blur[slot], img0, w, h, tA, tB, blur, A, s->bp);
+      if (s->ksize == 7) k_blur_q8_fast<7><<<gf, 256, 0, cs>>>(*tm, 0, w, h, tA, tB, s->blur, A, s->bp);
+      else k_blur_q8_fast<5><<<gf, 256, 0, cs>>>(*tm, 0, w, h, tA, tB, s->blur, A, s->bp);
     } else {
       dim3 gb((w + BQ_TW - 1) / BQ_TW, (h + BQ_TH - 1) / BQ_TH, n);
-      k_blur_q8<<<gb, 256, 0, cs>>>(imgs, img_stride, pitch, w, h, s->ksize / 2, blur, A, s->bp);
+      k_blur_q8<<<gb, 256, 0, cs>>>(d_imgs, img_stride, pitch, w, h, s->ksize / 2, s->blur, A, s->bp);
     }
     PLF_LAUNCH_CHECK(ctx);
     plf_mark(ctx, "lsd.k_blur_q8");
-    st = plf_launch_resize_exact(ctx, blur, A, s->bp, w, h, scaled_buf, Asp, s->sp, W, H, s->rs_tab + s->rs_x_off, s->rs_tab + s->rs_xp_off, s->rs_tab + s->rs_y_off, n);
+    st = plf_launch_resize_exact(ctx, s->blur, A, s->bp, w, h, s->scaled, Asp, s->sp, W, H, s->rs_tab + s->rs_x_off, s->rs_tab + s->rs_xp_off, s->rs_tab + s->rs_y_off, n);
     if (st) return st;
     plf_mark(ctx, "lsd.k_resize_exact");
-    scaled = scaled_buf;
+    scaled = s->scaled;
     scaled_stride = Asp;
     scaled_pitch = s->sp;
   }
-  PLF_CUDA(ctx, cudaMemsetAsync(maxmag2, 0xFF, (size_t)n * sizeof(int), cs));  // -1
+  PLF_CUDA(ctx, cudaMemsetAsync(s->maxmag2, 0xFF, (size_t)n * sizeof(int), cs));  // -1
   k_lsd_grad<<<dim3(s->nxb, (H + 1) / 2, n), LSD_GRAD_THREADS, 0, cs>>>(scaled, scaled_stride, scaled_pitch, W, H, s->angle_lut, s->m2_min, As, pix, s->pix_stride,
-                                                               seedlist, segcnt, s->nxb, maxmag2);
+                                                               s->seedlist, s->segcnt, s->nxb, s->maxmag2);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_grad");
-  k_lsd_rowhist<<<dim3(nchunks, n), 256, 0, cs>>>(As, W, H, s->n_bins, nchunks, s->nxb, maxmag2, seedlist, segcnt, rowcnt);
+  k_lsd_rowhist<<<dim3(nchunks, n), 256, 0, cs>>>(As, W, H, s->n_bins, nchunks, s->nxb, s->maxmag2, s->seedlist, s->segcnt, s->rowcnt);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_rowhist");
-  k_lsd_binscan<<<n, 1024, 0, cs>>>(rowcnt, nchunks, s->n_bins, binstart, nseeds);
+  k_lsd_binscan<<<n, 1024, 0, cs>>>(s->rowcnt, nchunks, s->n_bins, s->binstart, s->nseeds[par]);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_binscan");
-  k_lsd_scatter<<<dim3((nchunks + 3) / 4, n), 128, 0, cs>>>(seedlist, segcnt, As, W, H, s->n_bins, nchunks, s->nxb, rowcnt, binstart, order);
+  k_lsd_scatter<<<dim3((nchunks + 3) / 4, n), 128, 0, cs>>>(s->seedlist, s->segcnt, As, W, H, s->n_bins, nchunks, s->nxb, s->rowcnt, s->binstart,
+                                                            s->order[par]);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_scatter");
   return PLF_OK;
 }
 
-plf_status plf_lsd_grow_range(plf_ctx* ctx, int w, int h, int par, int img0, int n) {
+plf_status plf_lsd_grow(plf_ctx* ctx, int w, int h, int par, int n) {
   LsdState* s = ctx->lsd;
-  if (!s || s->w != w || s->h != h || s->nimg < img0 + n || (par && !s->two_parities))
-    return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_grow_range: state not prepared for this image range");
+  if (!s || s->w != w || s->h != h || s->nimg < n || (par && !s->two_parities))
+    return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_grow: state not prepared for these images");
   cudaStream_t cs = ctx->cur;
   const int W = s->ws, H = s->hs;
-  const size_t As = (size_t)W * H, o = (size_t)img0;
-  LsdPix* pix = s->pix[par] + o * s->pix_stride + (s->ws + 1);
-  int* nseeds = s->nseeds[par] + o;
-  uint32_t* order = s->order[par] + o * As;
-  // one copy: the growing, rectangle and KeyLine kernels of a batch run in stream order before those of the next
-  uint32_t* regpts = s->regpts + o * As;
-  uint4* regions = s->regions + o * s->max_regions;
-  int* nregions = s->nregions + o;
-  float4* segs = s->segs + o * s->max_regions;
-  plf_keyline* kls = s->kls[par] + o * s->max_lines;
-  plf_keyline* kls_all = s->kls_all + o * s->max_regions;
-  int* nlines = s->nlines[par] + o;
+  const size_t As = (size_t)W * H;
+  LsdPix* pix = s->pix[par] + (s->ws + 1);
+  // one copy of regpts, regions, segs, kls_all: the growing, rectangle and KeyLine kernels of a batch run in stream order
+  // before those of the next
   // (thread / lane per image, register-capped and unrolled variants and an angle-map layout were all bit-exact and were
   // not kept; DESIGN.md section 5 lists them)
-  k_lsd_grow<<<n, 32, 0, cs>>>(pix, s->pix_stride, As, W, order, s->seed_lut, s->cs_lut, nseeds, s->prec, (float)(s->p * 180.0), s->min_reg_size, regpts,
-                               regions, s->max_regions, nregions, s->overflow);
+  k_lsd_grow<<<n, 32, 0, cs>>>(pix, s->pix_stride, As, W, s->order[par], s->seed_lut, s->cs_lut, s->nseeds[par], s->prec, (float)(s->p * 180.0),
+                               s->min_reg_size, s->regpts, s->regions, s->max_regions, s->nregions, s->overflow);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_grow");
-  uint32_t* perm = s->rect_perm + o * s->max_regions;
-  k_lsd_rect_order<<<n, 256, 0, cs>>>(regions, s->max_regions, nregions, perm);
+  k_lsd_rect_order<<<n, 256, 0, cs>>>(s->regions, s->max_regions, s->nregions, s->rect_perm);
   PLF_LAUNCH_CHECK(ctx);
-  k_lsd_rects<<<dim3((s->max_regions + 127) / 128, n), 128, 0, cs>>>(pix, s->pix_stride, As, W, regpts, regions, s->max_regions, nregions,
-                                                                     perm, s->prec, s->scale, segs);
+  k_lsd_rects<<<dim3((s->max_regions + 127) / 128, n), 128, 0, cs>>>(pix, s->pix_stride, As, W, s->regpts, s->regions, s->max_regions, s->nregions,
+                                                                     s->rect_perm, s->prec, s->scale, s->segs);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_rects");
   const double min_length = (double)ctx->params.min_line_length * (double)std::min(w, h);
   if (ctx->lsd_keylines_wait) PLF_CUDA(ctx, cudaStreamWaitEvent(cs, ctx->lsd_keylines_wait, 0));
-  k_keylines<<<n, 1024, 0, cs>>>(segs, nregions, s->max_regions, w, h, min_length, ctx->params.lsd_nfeatures, kls_all, kls,
-                                 s->max_lines, nlines, s->overflow);
+  k_keylines<<<n, 1024, 0, cs>>>(s->segs, s->nregions, s->max_regions, w, h, min_length, ctx->params.lsd_nfeatures, s->kls_all, s->kls[par],
+                                 s->max_lines, s->nlines[par], s->overflow);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_keylines");
   return PLF_OK;
@@ -1352,8 +1300,8 @@ plf_status plf_lsd_grow_range(plf_ctx* ctx, int w, int h, int par, int img0, int
 plf_status plf_lsd_run(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int nimg) {
   plf_status st = plf_lsd_prepare(ctx, w, h, nimg, false);
   if (st) return st;
-  if ((st = plf_lsd_pre_range(ctx, d_imgs, img_stride, pitch, w, h, 0, 0, nimg))) return st;
-  return plf_lsd_grow_range(ctx, w, h, 0, 0, nimg);
+  if ((st = plf_lsd_pre(ctx, d_imgs, img_stride, pitch, w, h, 0, nimg))) return st;
+  return plf_lsd_grow(ctx, w, h, 0, nimg);
 }
 
 int* plf_lsd_overflow_flag(plf_ctx* ctx) { return ctx->lsd->overflow; }

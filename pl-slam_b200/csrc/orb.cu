@@ -11,7 +11,7 @@
 //                    four outputs per thread from two unaligned 32-bit reads per source row (k_resize_exact: scalar
 //                    variant for scale factors above 1.9)
 //   k_fast_nms       FAST-9/16 corner score + 3x3 non-max suppression + border filter on a 62x30 tile staged in
-//                    shared memory by 32-bit words (halo 4): 4-pair rejection, survivors compacted, full ring + score
+//                    shared memory by one TMA box (halo 4): 4-pair rejection, survivors compacted, full ring + score
 //                    on dense warps; corners are appended to a per-(image,level) candidate list and a 256-bin
 //                    response histogram
 //   k_select_sort    KeyPointsFilter::retainBest: per-level response threshold from the histogram (n-th largest,
@@ -19,7 +19,8 @@
 //   k_ic_angle       intensity-centroid orientation: integer moments over the 31-px circular patch, one warp per
 //                    keypoint, cv::fastAtan2 polynomial
 //   k_orb_blur7_fast 7x7 sigma-2 Gaussian in float with FMA (OpenCV takes its sepFilter2D path for the pyramid ROI), 64x32
-//                    outputs per CTA, 4 per thread (k_orb_blur7: generic variant for tiny images)
+//                    outputs per CTA, 4 per thread
+//   k_orb_trig       (float) cos / sin of each keypoint angle, one thread per keypoint
 //   k_rbrief         256 rotated pair tests from a 37x37 shared-memory patch, one warp per keypoint (lane = byte)
 // Per-image algorithmic bytes are A0 + 2*sum(A_k>=1) + 2*S + 56*N (SURVEY §8d); what bounds each kernel (issue rate,
 // latency - none is HBM-bound) is discussed in DESIGN.md §4.
@@ -75,24 +76,13 @@ struct OrbState {
   float2* trig = nullptr;       // [nimg][max_kp] (cos, sin) of the keypoint angle (k_orb_trig -> k_rbrief)
   float blur_k[7];
   // TMA descriptors (plf_tma.cuh): halo boxes of the FAST tile (96 x 38) and of the blur tile (80 x 38) per level; level 0
-  // is the caller's image buffer (re-encoded when its address changes - the pipeline alternates between two)
+  // is the caller's image buffer
   CUtensorMap tm_fast[ORB_MAX_LEVELS], tm_blur[ORB_MAX_LEVELS];
-  const void* tm_src0[2] = {nullptr, nullptr};   // image buffers the cached level-0 maps were encoded for
-  CUtensorMap tm_fast0[2], tm_blur0[2];
-  size_t tm_stride0 = 0; int tm_pitch0 = 0, tm_nimg0 = 0;
-  bool tma_ok = false;
+  PlfTmaCache tm_fast0, tm_blur0;
+  DevBufList bufs;
 };
 
 __constant__ float c_blur7[7];
-
-__device__ __forceinline__ int orb_reflect101(int i, int n) {
-  if (n == 1) return 0;
-  while (i < 0 || i >= n) {
-    if (i < 0) i = -i;
-    if (i >= n) i = 2 * (n - 1) - i;
-  }
-  return i;
-}
 
 // ---- pyramid ---------------------------------------------------------------------------------------
 // tab layout per level: [ox(dw) | cx(dw) | oy(dh) | cy(dh) | packed x (k_resize_exact4)]
@@ -685,17 +675,9 @@ void plf_linear_coeffs_host(int srcsize, int dstsize, double scale, int* ofs, in
   }
 }
 
-static void orb_release(OrbState* s) {
-  if (!s) return;
-  cudaFree(s->pyr); cudaFree(s->blur); cudaFree(s->cand); cudaFree(s->cand_count); cudaFree(s->hist);
-  cudaFree(s->rs_tab); cudaFree(s->overflow); cudaFree(s->trig);
-  for (int p = 0; p < 2; ++p) { cudaFree(s->kps[p]); cudaFree(s->kp_lxy[p]); cudaFree(s->desc[p]); cudaFree(s->kp_count[p]); }
-  s->pyr = s->blur = nullptr;
-}
-
 extern "C" void plf_orb_free(plf_ctx* ctx) {
   if (ctx->orb) {
-    orb_release(ctx->orb);
+    ctx->orb->bufs.release();
     delete ctx->orb;
     ctx->orb = nullptr;
   }
@@ -711,7 +693,7 @@ static plf_status orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
   if (s && s->two_parities) two_parities = true;
   if (s) {
     PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    orb_release(s);
+    s->bufs.release();
     *s = OrbState();
   } else {
     s = ctx->orb = new OrbState();
@@ -798,22 +780,25 @@ static plf_status orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
     tab.resize(tab.size() + plf_resize_packed_len(dw));
     plf_resize_pack_x(&tab[s->rs_x_off[l]], &tab[s->rs_x_off[l] + dw], dw, &tab[s->rs_xp_off[l]]);
   }
-  const size_t N = (size_t)nimg;
-  PLF_CUDA(ctx, cudaMalloc(&s->pyr, std::max<size_t>(pyr, 256) * N + 64));  // + slack for plf_load4 (see plf_image_span)
-  PLF_CUDA(ctx, cudaMalloc(&s->blur, blur * N + 64));
-  PLF_CUDA(ctx, cudaMalloc(&s->cand, cand * N * sizeof(uint32_t)));
-  PLF_CUDA(ctx, cudaMalloc(&s->cand_count, N * ORB_MAX_LEVELS * sizeof(int)));
-  PLF_CUDA(ctx, cudaMalloc(&s->hist, N * ORB_MAX_LEVELS * 256 * sizeof(int)));
-  PLF_CUDA(ctx, cudaMalloc(&s->rs_tab, std::max<size_t>(tab.size(), 1) * sizeof(int)));
+  const size_t N = (size_t)nimg, M = (size_t)g.max_kp;
+  DevBufList& b = s->bufs;
+  b.add(s->pyr, std::max<size_t>(pyr, 256) * N);
+  b.add(s->blur, blur * N);
+  b.add(s->cand, cand * N);
+  b.add(s->cand_count, N * ORB_MAX_LEVELS);
+  b.add(s->hist, N * ORB_MAX_LEVELS * 256);
+  b.add(s->rs_tab, std::max<size_t>(tab.size(), 1));
   for (int p = 0; p < (two_parities ? 2 : 1); ++p) {  // outputs exist per batch parity (read by the match phase of batch i
-    PLF_CUDA(ctx, cudaMalloc(&s->kps[p], N * g.max_kp * sizeof(plf_keypoint)));  // while batch i+1 is being extracted)
-    PLF_CUDA(ctx, cudaMalloc(&s->kp_lxy[p], N * g.max_kp * sizeof(short2)));
-    PLF_CUDA(ctx, cudaMalloc(&s->desc[p], N * g.max_kp * 32));
-    PLF_CUDA(ctx, cudaMalloc(&s->kp_count[p], N * sizeof(int)));
+    b.add(s->kps[p], N * M);                           // while batch i+1 is being extracted)
+    b.add(s->kp_lxy[p], N * M);
+    b.add(s->desc[p], N * M * 32);
+    b.add(s->kp_count[p], N);
   }
-  PLF_CUDA(ctx, cudaMalloc(&s->overflow, sizeof(int)));
+  b.add(s->overflow, 1);
+  b.add(s->trig, N * M);
+  plf_status st = b.alloc(ctx, "ORB");
+  if (st) return st;
   PLF_CUDA(ctx, cudaMemsetAsync(s->overflow, 0, sizeof(int), ctx->stream));
-  PLF_CUDA(ctx, cudaMalloc(&s->trig, N * g.max_kp * sizeof(float2)));
   if (!tab.empty())
     PLF_CUDA(ctx, cudaMemcpyAsync(s->rs_tab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
   {  // getGaussianKernel(7, 2, CV_32F): host doubles -> float (pinned equal to cv2 in tests)
@@ -835,8 +820,7 @@ static plf_status orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
     g_dev_pattern_device = ctx->device;
   }
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  // tensor maps of the pyramid levels (fixed addresses); level 0 = the caller's image buffer, encoded per run
-  s->tm_src0[0] = s->tm_src0[1] = nullptr;
+  // tensor maps of the pyramid levels (fixed addresses); level 0 = the caller's image buffer, cached per run
   for (int l = 1; l < g.nlevels; ++l) {
     if (!plf_tma_encode_u8(&s->tm_fast[l], s->pyr + g.pyr_off[l], g.w[l], g.h[l], nimg, g.pitch[l], g.pyr_stride, 96, 38) ||
         !plf_tma_encode_u8(&s->tm_blur[l], s->pyr + g.pyr_off[l], g.w[l], g.h[l], nimg, g.pitch[l], g.pyr_stride, 80, OBF_TH + 6))
@@ -850,7 +834,7 @@ static plf_status orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
 plf_status plf_orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
   const plf_status st = orb_prepare(ctx, w, h, nimg, two_parities);
   if (st && ctx->orb) {
-    orb_release(ctx->orb);
+    ctx->orb->bufs.release();
     *ctx->orb = OrbState();
   }
   return st;
@@ -865,20 +849,10 @@ plf_status plf_orb_run(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, i
   OrbGeom g = s->g;
   g.pitch[0] = pitch;
   cudaStream_t cs = ctx->cur;
-  // level-0 tensor maps: two cached slots (the pipeline alternates between its two upload buffers)
-  int slot = -1;
-  if (s->tm_stride0 != img_stride || s->tm_pitch0 != pitch || s->tm_nimg0 < nimg) {
-    s->tm_src0[0] = s->tm_src0[1] = nullptr;
-    s->tm_stride0 = img_stride; s->tm_pitch0 = pitch; s->tm_nimg0 = nimg;
-  }
-  for (int k = 0; k < 2; ++k) if (s->tm_src0[k] == d_imgs) slot = k;
-  if (slot < 0) {
-    slot = s->tm_src0[0] ? (s->tm_src0[1] ? 0 : 1) : 0;
-    if (!plf_tma_encode_u8(&s->tm_fast0[slot], d_imgs, w, h, s->tm_nimg0, pitch, img_stride, 96, 38) ||
-        !plf_tma_encode_u8(&s->tm_blur0[slot], d_imgs, w, h, s->tm_nimg0, pitch, img_stride, 80, OBF_TH + 6))
-      return plf_fail(ctx, PLF_ERR_CUDA, "ORB: cuTensorMapEncodeTiled failed for the source images (pitch %d, stride %zu)", pitch, img_stride);
-    s->tm_src0[slot] = d_imgs;
-  }
+  const CUtensorMap* tm_fast0 = s->tm_fast0.get(d_imgs, w, h, nimg, pitch, img_stride, 96, 38);
+  const CUtensorMap* tm_blur0 = s->tm_blur0.get(d_imgs, w, h, nimg, pitch, img_stride, 80, OBF_TH + 6);
+  if (!tm_fast0 || !tm_blur0)
+    return plf_fail(ctx, PLF_ERR_CUDA, "ORB: cuTensorMapEncodeTiled failed for the source images (pitch %d, stride %zu)", pitch, img_stride);
   PLF_CUDA(ctx, cudaMemsetAsync(s->cand_count, 0, (size_t)nimg * ORB_MAX_LEVELS * sizeof(int), cs));
   PLF_CUDA(ctx, cudaMemsetAsync(s->hist, 0, (size_t)nimg * ORB_MAX_LEVELS * 256 * sizeof(int), cs));
   for (int l = 1; l < g.nlevels; ++l) {
@@ -892,7 +866,7 @@ plf_status plf_orb_run(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, i
   plf_mark(ctx, "orb.k_resize_exact");
   for (int l = 0; l < g.nlevels; ++l) {
     const int tx_ = (g.w[l] + FN_OW - 1) / FN_OW, ty_ = (g.h[l] + FN_OH - 1) / FN_OH;
-    k_fast_nms<<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(l == 0 ? s->tm_fast0[slot] : s->tm_fast[l], g, l, tx_, s->cand, s->cand_count,
+    k_fast_nms<<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(l == 0 ? *tm_fast0 : s->tm_fast[l], g, l, tx_, s->cand, s->cand_count,
                                                       s->hist, s->overflow);
     PLF_LAUNCH_CHECK(ctx);
   }
@@ -905,7 +879,7 @@ plf_status plf_orb_run(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, i
   plf_mark(ctx, "orb.k_ic_angle");
   for (int l = 0; l < g.nlevels; ++l) {
     const int tx_ = plf_tma_tiles_x(g.w[l], 3), ty_ = (g.h[l] + OBF_TH - 1) / OBF_TH;
-    k_orb_blur7_fast<<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(l == 0 ? s->tm_blur0[slot] : s->tm_blur[l], g, s->blur, l, tx_);
+    k_orb_blur7_fast<<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(l == 0 ? *tm_blur0 : s->tm_blur[l], g, s->blur, l, tx_);
     PLF_LAUNCH_CHECK(ctx);
   }
   plf_mark(ctx, "orb.k_orb_blur7");

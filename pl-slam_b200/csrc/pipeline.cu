@@ -15,17 +15,26 @@
 #include "plf_internal.h"
 #include "plf_tma.cuh"
 
-struct FrameSlots {  // stereo-valid features per frame slot: [slots][cap]
-  double2* pt_pl; double* pt_disp; double* pt_P; int* pt_octave; uint8_t* pdesc; int* pt_count;
-  double2* ls_spl; double2* ls_epl; double* ls_sdisp; double* ls_edisp; double* ls_sP; double* ls_eP; double* ls_le;
-  float* ls_angle; uint8_t* ldesc; int* ls_count;
+// Stereo-valid features per frame slot, [slots][cap][per]: one row per array, (name = its plf_frame_view member, element
+// type, capacity per slot: K = max_keypoints or Ln = max_lines, elements per feature).  The counts (one int per slot)
+// follow the arrays of their kind.
+#define PLF_PT_FIELDS(X) \
+  X(pt_pl, double2, K, 1) X(pt_disp, double, K, 1) X(pt_P, double, K, 3) X(pt_octave, int, K, 1) X(pdesc, uint8_t, K, 32)
+#define PLF_LS_FIELDS(X)                                                                                              \
+  X(ls_spl, double2, Ln, 1) X(ls_epl, double2, Ln, 1) X(ls_sdisp, double, Ln, 1) X(ls_edisp, double, Ln, 1)         \
+  X(ls_sP, double, Ln, 3) X(ls_eP, double, Ln, 3) X(ls_le, double, Ln, 3) X(ls_angle, float, Ln, 1) X(ldesc, uint8_t, Ln, 32)
+
+struct FrameSlots {
+#define PLF_FS_MEMBER(name, T, cap, per) T* name = nullptr;
+  PLF_PT_FIELDS(PLF_FS_MEMBER) int* pt_count = nullptr;
+  PLF_LS_FIELDS(PLF_FS_MEMBER) int* ls_count = nullptr;
+#undef PLF_FS_MEMBER
 };
 
 struct PipeState {
   int w = 0, h = 0, B = 0, max_kp = 0, max_ln = 0;
   int pitch = 0;               // row pitch of the device images: plf_pitch16(w) (16-byte rows: every halo tile is a legal TMA box)
   bool has_prev = false;
-  uint8_t* imgs = nullptr;     // images of the batch being run: = imgs2[run_slot]
   uint8_t* imgs2[2] = {nullptr, nullptr};  // double-buffered [2B][h][pitch]: upload of batch i+1 overlaps the run of batch i
   uint8_t* stage = nullptr;    // dense [2B][h][w] landing buffer of the H2D copy (one contiguous DMA per side), repacked to the padded pitch on the device
   int up_slot = 0;             // slot written by the last plf_batch_upload
@@ -75,45 +84,69 @@ struct PipeState {
   cudaEvent_t tE0[2] = {nullptr, nullptr}, tG0[2] = {nullptr, nullptr}, tM0[3] = {nullptr, nullptr, nullptr};  // phase starts (timeline)
   long long seq = 0;            // batches issued
   int pend_slot[3] = {0, 0, 0}, pend_B[3] = {0, 0, 0}, n_pending = 0;
-  void* orb_kps_seen = nullptr;  // sub-system output pointers baked into the problem descriptors
-  void* lsd_kls_seen = nullptr;
-  std::vector<void*> allocs;
+  DevBufList bufs;
 };
 
-template <typename T>
-static plf_status pipe_alloc(plf_ctx* ctx, PipeState* s, T** p, size_t n) {
-  void* q = nullptr;
-  cudaError_t e = cudaMalloc(&q, std::max<size_t>(n * sizeof(T), 256) + 64);  // + slack for plf_load4 (see plf_image_span)
-  if (e != cudaSuccess) return plf_fail(ctx, PLF_ERR_CUDA, "pipeline cudaMalloc(%zu): %s", n * sizeof(T), cudaGetErrorString(e));
-  *p = (T*)q;
-  s->allocs.push_back(q);
-  return PLF_OK;
+// The device buffers of the pipeline for B pairs of K keypoints / Ln lines per image.
+static void pipe_buffers(PipeState* s, bool windowed, DevBufList& b) {
+  const size_t B = s->B, K = s->max_kp, Ln = s->max_ln, A = (size_t)s->w * s->h, AP = (size_t)s->pitch * s->h, S = B + 1;
+  b.add(s->imgs2[0], 2 * B * AP);
+  b.add(s->imgs2[1], 2 * B * AP);
+  if (s->pitch != s->w) b.add(s->stage, 2 * B * A);
+  b.add(s->lbd_grad[0], 2 * B * A);
+  b.add(s->lbd_grad[1], 2 * B * A);
+  b.add(s->ldesc_raw, 2 * B * Ln * 32);
+  FrameSlots& f = s->fs;
+#define PLF_FS_ALLOC(name, T, cap, per) b.add(f.name, S * cap * per);
+  PLF_PT_FIELDS(PLF_FS_ALLOC) b.add(f.pt_count, S);
+  PLF_LS_FIELDS(PLF_FS_ALLOC) b.add(f.ls_count, S);
+#undef PLF_FS_ALLOC
+  b.add(s->knn_keys, B * 8 * 2 * K);
+  b.add(s->m12, B * 4 * K);
+  b.add(s->mcount, B * 4);
+  b.add(s->knn_stereo, B * 4); b.add(s->knn_f2f, B * 4);
+  b.add(s->nnr_stereo, B * 2); b.add(s->nnr_f2f, B * 2);
+  b.add(s->rev_flags, 2 * B * K); b.add(s->rev_list, 2 * B * K); b.add(s->rev_count, 2 * B);
+  b.add(s->kpsM, 2 * B * K); b.add(s->descM, 2 * B * K * 32); b.add(s->kcntM, 2 * B);
+  b.add(s->klsM, 2 * B * Ln); b.add(s->lcntM, 2 * B);
+  b.add(s->gnP, B * K * 3); b.add(s->gnObs, B * K * 2); b.add(s->gnInlP, B * K); b.add(s->gnNp, B);
+  b.add(s->gn_sP, B * Ln * 3); b.add(s->gn_eP, B * Ln * 3); b.add(s->gn_le, B * Ln * 3); b.add(s->gnInlL, B * Ln); b.add(s->gnNl, B);
+  b.add(s->gn_probs, B); b.add(s->gn_out, B); b.add(s->results, 3 * B);
+  b.add(s->d_ovf, 6);
+  if (windowed) {
+    for (int kind = 0; kind < 4; ++kind) {   // points: 2 cells per feature, lines: 2 end points
+      b.add(s->mg_q[kind], B * (kind & 1 ? Ln * 4 : K * 2));
+      b.add(s->mg_t[kind], B * (kind & 1 ? Ln * 4 : K * 2));
+    }
+    b.add(s->mg_dir[0], B * Ln * 2); b.add(s->mg_dir[1], B * Ln * 2);
+    b.add(s->m12g, B * 2 * K);
+    b.add(s->mgcount, B * 2);
+  }
+}
+
+// Every event of the pipeline: (array, count, creation flags).  plf_debug_timeline reads the timed ones.  evM uses
+// blocking sync: a host thread waiting in plf_batch_download sleeps instead of spinning, which matters when several ranks
+// share a fraction of a machine's CPUs.
+struct PipeEvents { cudaEvent_t* ev; int n; unsigned flags; };
+static std::vector<PipeEvents> pipe_events(PipeState* s) {
+  return {{s->ev_up, 2, cudaEventDisableTiming}, {s->ev_free, 2, cudaEventDisableTiming}, {s->ev_free2, 2, cudaEventDisableTiming},
+          {s->evM, 3, cudaEventBlockingSync},    {s->tM0, 3, cudaEventDefault},           {s->evE, 2, cudaEventDefault},
+          {s->evG, 2, cudaEventDefault},         {s->evX, 2, cudaEventDisableTiming},     {s->evP, 2, cudaEventDisableTiming},
+          {s->tE0, 2, cudaEventDefault},         {s->tG0, 2, cudaEventDefault}};
 }
 
 extern "C" void plf_pipe_free(plf_ctx* ctx) {
   PipeState* s = ctx->pipe;
   if (!s) return;
-  for (void* p : s->allocs) cudaFree(p);
+  s->bufs.release();
   for (int i = 0; i < 3; ++i) {
     if (s->h_results[i]) cudaFreeHost(s->h_results[i]);
     if (s->h_ovf[i]) cudaFreeHost(s->h_ovf[i]);
-    if (s->evM[i]) cudaEventDestroy(s->evM[i]);
-    if (s->tM0[i]) cudaEventDestroy(s->tM0[i]);
   }
-  for (int i = 0; i < 2; ++i) {
-    if (s->evE[i]) cudaEventDestroy(s->evE[i]);
-    if (s->evG[i]) cudaEventDestroy(s->evG[i]);
-    if (s->evX[i]) cudaEventDestroy(s->evX[i]);
-    if (s->evP[i]) cudaEventDestroy(s->evP[i]);
-    if (s->tE0[i]) cudaEventDestroy(s->tE0[i]);
-    if (s->tG0[i]) cudaEventDestroy(s->tG0[i]);
-  }
+  for (const PipeEvents& a : pipe_events(s))
+    for (int i = 0; i < a.n; ++i)
+      if (a.ev[i]) cudaEventDestroy(a.ev[i]);
   if (s->copy) { cudaStreamSynchronize(s->copy); cudaStreamDestroy(s->copy); }
-  for (int i = 0; i < 2; ++i) {
-    if (s->ev_up[i]) cudaEventDestroy(s->ev_up[i]);
-    if (s->ev_free[i]) cudaEventDestroy(s->ev_free[i]);
-    if (s->ev_free2[i]) cudaEventDestroy(s->ev_free2[i]);
-  }
   delete s;
   ctx->pipe = nullptr;
 }
@@ -468,111 +501,45 @@ static bool lsd_want_two_parities(const plf_ctx* ctx, int w, int h, int nimg) {
   return plf_lsd_footprint(ctx, w, h, nimg, true) + LSD_PARITY_MARGIN <= free_b;
 }
 
-static plf_status pipe_prepare(plf_ctx* ctx, int w, int h) {
-  PipeState* s = ctx->pipe;
-  if (s && s->w == w && s->h == h) {
-    // a standalone operator call on another image size may have rebuilt the ORB / LSD state meanwhile
-    plf_status st0;
-    if ((st0 = plf_orb_prepare(ctx, w, h, 2 * s->B, true))) return st0;
-    if ((st0 = plf_lsd_prepare(ctx, w, h, 2 * s->B, s->lsd2))) return st0;
-    plf_keypoint* kps0; uint8_t* d0; int* c0; int m0;
-    plf_orb_outputs(ctx, 0, &kps0, &d0, &c0, &m0);
-    plf_keyline* kl0; int* lc0; int ml0;
-    plf_lsd_outputs(ctx, 0, &kl0, &lc0, &ml0);
-    if (kps0 == s->orb_kps_seen && kl0 == s->lsd_kls_seen) return PLF_OK;
-  }
-  if (s) plf_pipe_free(ctx);
-  s = ctx->pipe = new PipeState();
+static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
+  PipeState* s = ctx->pipe = new PipeState();
   const int B = ctx->limits.max_batch, K = ctx->limits.max_keypoints, Ln = ctx->limits.max_lines;
   if (Ln > K || K > 65535)
     return plf_fail(ctx, PLF_ERR_INVALID, "limits: need max_lines <= max_keypoints <= 65535 (got %d, %d)", Ln, K);
   s->w = w; s->h = h; s->B = B; s->max_kp = K; s->max_ln = Ln;
   s->pitch = plf_pitch16(w);
-  plf_status st;
-#define PA(ptr, n) if ((st = pipe_alloc(ctx, s, &(ptr), (n)))) return st
-  const size_t A = (size_t)w * h, AP = (size_t)s->pitch * h, S = (size_t)B + 1;
-  PA(s->imgs2[0], 2 * (size_t)B * AP);
-  PA(s->imgs2[1], 2 * (size_t)B * AP);
-  if (s->pitch != w) PA(s->stage, 2 * (size_t)B * A);
-  s->imgs = s->imgs2[0];
+  const plf_params& P = ctx->params;
+  pipe_buffers(s, P.matching_strategy != 0, s->bufs);
+  plf_status st = s->bufs.alloc(ctx, "pipeline");
+  if (st) return st;
   PLF_CUDA(ctx, cudaStreamCreateWithFlags(&s->copy, cudaStreamNonBlocking));
-  for (int i = 0; i < 2; ++i) {
-    PLF_CUDA(ctx, cudaEventCreateWithFlags(&s->ev_up[i], cudaEventDisableTiming));
-    PLF_CUDA(ctx, cudaEventCreateWithFlags(&s->ev_free[i], cudaEventDisableTiming));
-    PLF_CUDA(ctx, cudaEventCreateWithFlags(&s->ev_free2[i], cudaEventDisableTiming));
-  }
-  PA(s->lbd_grad[0], 2 * (size_t)B * A);
-  PA(s->lbd_grad[1], 2 * (size_t)B * A);
-  PA(s->ldesc_raw, 2 * (size_t)B * Ln * 32);
-  FrameSlots& f = s->fs;
-  PA(f.pt_pl, S * K); PA(f.pt_disp, S * K); PA(f.pt_P, S * K * 3); PA(f.pt_octave, S * K); PA(f.pdesc, S * K * 32); PA(f.pt_count, S);
-  PA(f.ls_spl, S * Ln); PA(f.ls_epl, S * Ln); PA(f.ls_sdisp, S * Ln); PA(f.ls_edisp, S * Ln); PA(f.ls_sP, S * Ln * 3);
-  PA(f.ls_eP, S * Ln * 3); PA(f.ls_le, S * Ln * 3); PA(f.ls_angle, S * Ln); PA(f.ldesc, S * Ln * 32); PA(f.ls_count, S);
-  PA(s->knn_keys, (size_t)B * 8 * 2 * K);
-  PA(s->m12, (size_t)B * 4 * K);
-  PA(s->mcount, (size_t)B * 4);
-  PA(s->knn_stereo, (size_t)B * 4); PA(s->knn_f2f, (size_t)B * 4);
-  PA(s->nnr_stereo, (size_t)B * 2); PA(s->nnr_f2f, (size_t)B * 2);
-  PA(s->rev_flags, 2 * (size_t)B * K); PA(s->rev_list, 2 * (size_t)B * K); PA(s->rev_count, 2 * (size_t)B);
-  PA(s->kpsM, 2 * (size_t)B * K); PA(s->descM, 2 * (size_t)B * K * 32); PA(s->kcntM, 2 * (size_t)B);
-  PA(s->klsM, 2 * (size_t)B * Ln); PA(s->lcntM, 2 * (size_t)B);
-  PA(s->gnP, (size_t)B * K * 3); PA(s->gnObs, (size_t)B * K * 2); PA(s->gnInlP, (size_t)B * K); PA(s->gnNp, B);
-  PA(s->gn_sP, (size_t)B * Ln * 3); PA(s->gn_eP, (size_t)B * Ln * 3); PA(s->gn_le, (size_t)B * Ln * 3); PA(s->gnInlL, (size_t)B * Ln); PA(s->gnNl, B);
-  PA(s->gn_probs, B); PA(s->gn_out, B); PA(s->results, 3 * (size_t)B);
-  PA(s->d_ovf, 6);
-  if (ctx->params.matching_strategy) {
-    PA(s->mg_q[0], (size_t)B * K * 2); PA(s->mg_t[0], (size_t)B * K * 2);
-    PA(s->mg_q[1], (size_t)B * Ln * 4); PA(s->mg_t[1], (size_t)B * Ln * 4);
-    PA(s->mg_q[2], (size_t)B * K * 2); PA(s->mg_t[2], (size_t)B * K * 2);
-    PA(s->mg_q[3], (size_t)B * Ln * 4); PA(s->mg_t[3], (size_t)B * Ln * 4);
-    PA(s->mg_dir[0], (size_t)B * Ln * 2); PA(s->mg_dir[1], (size_t)B * Ln * 2);
-    PA(s->m12g, (size_t)B * 2 * K);
-    PA(s->mgcount, (size_t)B * 2);
-  }
-#undef PA
+  for (const PipeEvents& a : pipe_events(s))
+    for (int i = 0; i < a.n; ++i) PLF_CUDA(ctx, cudaEventCreateWithFlags(&a.ev[i], a.flags));
   for (int i = 0; i < 3; ++i) {
     PLF_CUDA(ctx, cudaHostAlloc(&s->h_results[i], sizeof(plf_frame_result) * B, cudaHostAllocDefault));
     PLF_CUDA(ctx, cudaHostAlloc(&s->h_ovf[i], 2 * sizeof(int), cudaHostAllocDefault));
-    // timing enabled (plf_debug_timeline) + blocking sync: a host thread waiting in plf_batch_download sleeps instead of
-    // spinning (8 ranks spinning on a box that gives the job a fraction of its CPUs was the round-1 scaling suspect)
-    PLF_CUDA(ctx, cudaEventCreateWithFlags(&s->evM[i], cudaEventBlockingSync));
-    PLF_CUDA(ctx, cudaEventCreate(&s->tM0[i]));
   }
-  for (int i = 0; i < 2; ++i) {
-    PLF_CUDA(ctx, cudaEventCreate(&s->evE[i]));
-    PLF_CUDA(ctx, cudaEventCreate(&s->evG[i]));
-    PLF_CUDA(ctx, cudaEventCreateWithFlags(&s->evX[i], cudaEventDisableTiming));
-    PLF_CUDA(ctx, cudaEventCreateWithFlags(&s->evP[i], cudaEventDisableTiming));
-    PLF_CUDA(ctx, cudaEventCreate(&s->tE0[i]));
-    PLF_CUDA(ctx, cudaEventCreate(&s->tG0[i]));
-  }
-  PLF_CUDA(ctx, cudaMemsetAsync(f.pt_count, 0, S * sizeof(int), ctx->stream));
-  PLF_CUDA(ctx, cudaMemsetAsync(f.ls_count, 0, S * sizeof(int), ctx->stream));
+  FrameSlots& f = s->fs;
+  cudaStream_t cs = ctx->stream;
+  PLF_CUDA(ctx, cudaMemsetAsync(f.pt_count, 0, (B + 1) * sizeof(int), cs));
+  PLF_CUDA(ctx, cudaMemsetAsync(f.ls_count, 0, (B + 1) * sizeof(int), cs));
   // sub-systems sized for 2B images
   if ((st = plf_orb_prepare(ctx, w, h, 2 * B, true))) return st;
   s->lsd2 = lsd_want_two_parities(ctx, w, h, 2 * B);
   if ((st = plf_lsd_prepare(ctx, w, h, 2 * B, s->lsd2))) return st;
-  // static problem descriptors (pointers never change; counts are read on the device)
-  const plf_params& P = ctx->params;
-  cudaStream_t cs = ctx->stream;
-  std::vector<KnnProblem> kf(B * 4);
-  std::vector<NnrProblem> nf(B * 2);
-  {
-  plf_keypoint* kps0; uint8_t* odesc0; int* kcnt0; int mk;
-  plf_orb_outputs(ctx, 0, &kps0, &odesc0, &kcnt0, &mk);
-  plf_keyline* kls0; int* lcnt0; int ml;
-  plf_lsd_outputs(ctx, 0, &kls0, &lcnt0, &ml);
-  s->orb_kps_seen = kps0;
-  s->lsd_kls_seen = kls0;
-  uint8_t* odesc = s->descM;
-  int* kcnt = s->kcntM;
-  int* lcnt = s->lcntM;
-  std::vector<KnnProblem> ks(B * 4);
-  std::vector<NnrProblem> ns(B * 2);
+  // static problem descriptors over the pipeline's own buffers (pointers never change; counts are read on the device):
+  // the stereo problems read the match phase's copies of the extraction outputs
+  const int* kcnt = s->kcntM;
+  const int* lcnt = s->lcntM;
+  const int best_lr = P.best_lr_matches ? 1 : 0;
+  std::vector<KnnProblem> ks(B * 4), kf(B * 4);
+  std::vector<NnrProblem> ns(B * 2), nf(B * 2);
+  std::vector<GnProblem> gp(B);
   for (int k = 0; k < B; ++k) {
     auto key = [&](int prob, int which) { return s->knn_keys + (((size_t)k * 8 + prob) * 2 + which) * K; };
-    const uint32_t* dl = (const uint32_t*)(odesc + (size_t)(2 * k) * K * 32);
-    const uint32_t* dr = (const uint32_t*)(odesc + (size_t)(2 * k + 1) * K * 32);
+    auto m12 = [&](int kind) { return s->m12 + ((size_t)k * 4 + kind) * K; };
+    const uint32_t* dl = (const uint32_t*)(s->descM + (size_t)(2 * k) * K * 32);
+    const uint32_t* dr = (const uint32_t*)(s->descM + (size_t)(2 * k + 1) * K * 32);
     const uint32_t* ll = (const uint32_t*)(s->ldesc_raw + (size_t)(2 * k) * Ln * 32);
     const uint32_t* lr = (const uint32_t*)(s->ldesc_raw + (size_t)(2 * k + 1) * Ln * 32);
     // forward problems (all left rows), then reverse problems restricted to the right rows the mutual check will read
@@ -580,10 +547,8 @@ static plf_status pipe_prepare(plf_ctx* ctx, int w, int h) {
     ks[2 * k + 1] = {ll, lr, lcnt + 2 * k, lcnt + 2 * k + 1, 0, 0, key(2, 0), key(2, 1), nullptr};
     ks[2 * B + 2 * k + 0] = {dr, dl, s->rev_count + 2 * k, kcnt + 2 * k, 0, 0, key(1, 0), key(1, 1), s->rev_list + (size_t)(2 * k) * K};
     ks[2 * B + 2 * k + 1] = {lr, ll, s->rev_count + 2 * k + 1, lcnt + 2 * k, 0, 0, key(3, 0), key(3, 1), s->rev_list + (size_t)(2 * k + 1) * K};
-    ns[2 * k + 0] = {key(0, 0), key(0, 1), key(1, 0), key(1, 1), kcnt + 2 * k, kcnt + 2 * k + 1, 0, 0, P.min_ratio_12_p,
-                     P.best_lr_matches ? 1 : 0, s->m12 + ((size_t)k * 4 + 0) * K, s->mcount + 4 * k + 0};
-    ns[2 * k + 1] = {key(2, 0), key(2, 1), key(3, 0), key(3, 1), lcnt + 2 * k, lcnt + 2 * k + 1, 0, 0, P.min_ratio_12_l,
-                     P.best_lr_matches ? 1 : 0, s->m12 + ((size_t)k * 4 + 1) * K, s->mcount + 4 * k + 1};
+    ns[2 * k + 0] = {key(0, 0), key(0, 1), key(1, 0), key(1, 1), kcnt + 2 * k, kcnt + 2 * k + 1, 0, 0, P.min_ratio_12_p, best_lr, m12(0), s->mcount + 4 * k + 0};
+    ns[2 * k + 1] = {key(2, 0), key(2, 1), key(3, 0), key(3, 1), lcnt + 2 * k, lcnt + 2 * k + 1, 0, 0, P.min_ratio_12_l, best_lr, m12(1), s->mcount + 4 * k + 1};
     // f2f: prev slot k, curr slot k+1
     const uint32_t* pp = (const uint32_t*)(f.pdesc + (size_t)k * K * 32);
     const uint32_t* pc = (const uint32_t*)(f.pdesc + (size_t)(k + 1) * K * 32);
@@ -593,20 +558,14 @@ static plf_status pipe_prepare(plf_ctx* ctx, int w, int h) {
     kf[4 * k + 1] = {pc, pp, f.pt_count + k + 1, f.pt_count + k, 0, 0, key(5, 0), key(5, 1)};
     kf[4 * k + 2] = {lp, lc, f.ls_count + k, f.ls_count + k + 1, 0, 0, key(6, 0), key(6, 1)};
     kf[4 * k + 3] = {lc, lp, f.ls_count + k + 1, f.ls_count + k, 0, 0, key(7, 0), key(7, 1)};
-    nf[2 * k + 0] = {key(4, 0), key(4, 1), key(5, 0), key(5, 1), f.pt_count + k, f.pt_count + k + 1, 0, 0, P.min_ratio_12_p,
-                     P.best_lr_matches ? 1 : 0, s->m12 + ((size_t)k * 4 + 2) * K, s->mcount + 4 * k + 2};
-    nf[2 * k + 1] = {key(6, 0), key(6, 1), key(7, 0), key(7, 1), f.ls_count + k, f.ls_count + k + 1, 0, 0, P.min_ratio_12_l,
-                     P.best_lr_matches ? 1 : 0, s->m12 + ((size_t)k * 4 + 3) * K, s->mcount + 4 * k + 3};
-  }
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->knn_stereo, ks.data(), ks.size() * sizeof(KnnProblem), cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->nnr_stereo, ns.data(), ns.size() * sizeof(NnrProblem), cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaStreamSynchronize(cs));
-  }
-  std::vector<GnProblem> gp(B);
-  for (int k = 0; k < B; ++k)
+    nf[2 * k + 0] = {key(4, 0), key(4, 1), key(5, 0), key(5, 1), f.pt_count + k, f.pt_count + k + 1, 0, 0, P.min_ratio_12_p, best_lr, m12(2), s->mcount + 4 * k + 2};
+    nf[2 * k + 1] = {key(6, 0), key(6, 1), key(7, 0), key(7, 1), f.ls_count + k, f.ls_count + k + 1, 0, 0, P.min_ratio_12_l, best_lr, m12(3), s->mcount + 4 * k + 3};
     gp[k] = {s->gnP + (size_t)k * K * 3, s->gnObs + (size_t)k * K * 2, s->gnInlP + (size_t)k * K, s->gnNp + k, 0,
              s->gn_sP + (size_t)k * Ln * 3, s->gn_eP + (size_t)k * Ln * 3, s->gn_le + (size_t)k * Ln * 3,
              s->gnInlL + (size_t)k * Ln, s->gnNl + k, 0, nullptr, s->gn_out + k};
+  }
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->knn_stereo, ks.data(), ks.size() * sizeof(KnnProblem), cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->nnr_stereo, ns.data(), ns.size() * sizeof(NnrProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->knn_f2f, kf.data(), kf.size() * sizeof(KnnProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->nnr_f2f, nf.data(), nf.size() * sizeof(NnrProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->gn_probs, gp.data(), gp.size() * sizeof(GnProblem), cudaMemcpyHostToDevice, cs));
@@ -614,15 +573,224 @@ static plf_status pipe_prepare(plf_ctx* ctx, int w, int h) {
   return PLF_OK;
 }
 
+static plf_status pipe_prepare(plf_ctx* ctx, int w, int h) {
+  PipeState* s = ctx->pipe;
+  if (s && s->w == w && s->h == h) {
+    // a standalone operator call on another image size may have rebuilt the ORB / LSD state meanwhile: rebuild it again.
+    // No pipeline buffer or problem descriptor points into that state, so the sequence goes on where it was.
+    const plf_status st = plf_orb_prepare(ctx, w, h, 2 * s->B, true);
+    return st ? st : plf_lsd_prepare(ctx, w, h, 2 * s->B, s->lsd2);
+  }
+  plf_pipe_free(ctx);
+  const plf_status st = pipe_build(ctx, w, h);
+  if (st) plf_pipe_free(ctx);   // a failed setup leaves no state behind (see plf_orb_prepare)
+  return st;
+}
+
 static plf_status copy_slot(plf_ctx* ctx, PipeState* s, int from, int to) {
   FrameSlots& f = s->fs;
   const size_t K = s->max_kp, Ln = s->max_ln;
   cudaStream_t cs = ctx->stream;
-#define CP(ptr, per) PLF_CUDA(ctx, cudaMemcpyAsync((char*)(ptr) + (size_t)to * (per), (char*)(ptr) + (size_t)from * (per), (per), cudaMemcpyDeviceToDevice, cs))
-  CP(f.pt_pl, K * sizeof(double2)); CP(f.pt_disp, K * 8); CP(f.pt_P, K * 24); CP(f.pt_octave, K * 4); CP(f.pdesc, K * 32); CP(f.pt_count, 4);
-  CP(f.ls_spl, Ln * 16); CP(f.ls_epl, Ln * 16); CP(f.ls_sdisp, Ln * 8); CP(f.ls_edisp, Ln * 8); CP(f.ls_sP, Ln * 24);
-  CP(f.ls_eP, Ln * 24); CP(f.ls_le, Ln * 24); CP(f.ls_angle, Ln * 4); CP(f.ldesc, Ln * 32); CP(f.ls_count, 4);
+#define CP(ptr, per) PLF_CUDA(ctx, cudaMemcpyAsync((ptr) + (size_t)to * (per), (ptr) + (size_t)from * (per), (per) * sizeof(*(ptr)), cudaMemcpyDeviceToDevice, cs));
+#define PLF_FS_COPY(name, T, cap, per) CP(f.name, cap * per)
+  PLF_PT_FIELDS(PLF_FS_COPY) CP(f.pt_count, 1)
+  PLF_LS_FIELDS(PLF_FS_COPY) CP(f.ls_count, 1)
+#undef PLF_FS_COPY
 #undef CP
+  return PLF_OK;
+}
+
+// One plf_batch_run call: its pairs, buffer parities and slots, and the streams of its phases.
+struct BatchRun {
+  int B;
+  int par;       // parity of the E -> G -> M hand-off buffers
+  int lp;        // parity of the LSD hand-off buffers (0 when they exist once)
+  int rp;        // slot of the result ring
+  int run_slot;  // upload slot consumed: the most recently uploaded batch
+  bool piped, lsd2;
+  cudaStream_t sM, sE, sG, sP;
+};
+
+// ---- E phase: ORB + LBD gradient prelude (bandwidth / ALU bound); outputs per batch parity ----
+static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
+  const int w = s->w, h = s->h, B = r.B, par = r.par;
+  const size_t A = (size_t)w * h, AP = (size_t)s->pitch * h;   // dense maps / padded images
+  const uint8_t* imgs = s->imgs2[r.run_slot];
+  cudaStream_t sE = r.sE;
+  ctx->cur = sE;
+  PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_up[r.run_slot], 0));  // images uploaded
+  PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->evX[par], 0));           // batch i-2 (same parity) no longer reads these buffers
+  plf_mark(ctx, "start");
+  PLF_CUDA(ctx, cudaEventRecord(s->tE0[par], sE));
+  plf_status st = plf_orb_run(ctx, imgs, AP, s->pitch, w, h, 2 * B, par);
+  if (!st) st = plf_launch_blur5_sobel(ctx, imgs, s->pitch, AP, w, h, 2 * B, s->lbd_grad[par], A);
+  if (st) return st;
+  plf_mark(ctx, "lbd.k_blur5_sobel");
+  // this batch's ORB overflow flag: snapshot + clear on the E stream, so that a flag raised by batch i+1's extraction is
+  // not reported on batch i's download
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp, plf_orb_overflow_flag(ctx), sizeof(int), cudaMemcpyDeviceToDevice, sE));
+  PLF_CUDA(ctx, cudaMemsetAsync(plf_orb_overflow_flag(ctx), 0, sizeof(int), sE));
+  PLF_CUDA(ctx, cudaEventRecord(s->evE[par], sE));
+  PLF_CUDA(ctx, cudaEventRecord(s->ev_free[r.run_slot], sE));  // the image buffer may be overwritten by the next upload
+  return PLF_OK;
+}
+
+// ---- P / G phases: the LSD chain.  P = blur / resize / gradient / seed ordering (bandwidth-bound), G = region growing
+// (latency bound, one warp per image), rectangle fit and KeyLines.  With the hand-off maps per batch parity (lsd2, the
+// default where they fit) P runs on its own stream: P(i+1) overlaps G(i), and the chain on the critical path is G alone;
+// with one copy P and G share a stream and LSD(i+1) starts when LSD(i) ends.  The buffers only G writes and reads
+// (region points, regions, segments) exist once either way: G(i+1) follows G(i) on its stream. ----
+static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
+  const int w = s->w, h = s->h, par = r.par;
+  const size_t AP = (size_t)s->pitch * h;
+  cudaStream_t sP = r.sP, sG = r.sG;
+  ctx->cur = sP;
+  PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_up[r.run_slot], 0));
+  if (r.lsd2) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->evG[par], 0));   // batch i-2 (same parity) has finished growing / fitting on these maps
+  PLF_CUDA(ctx, cudaEventRecord(s->tG0[par], sP));
+  plf_status st = plf_lsd_pre(ctx, s->imgs2[r.run_slot], AP, s->pitch, w, h, r.lp, 2 * r.B);
+  if (st) return st;
+  PLF_CUDA(ctx, cudaEventRecord(s->ev_free2[r.run_slot], sP));
+  PLF_CUDA(ctx, cudaEventRecord(s->evP[par], sP));
+  ctx->cur = sG;
+  PLF_CUDA(ctx, cudaStreamWaitEvent(sG, s->evP[par], 0));
+  // the KeyLine outputs are overwritten: the match phase that read them last (batch i-2 with two parities, batch i-1 with one)
+  // has taken its copy
+  ctx->lsd_keylines_wait = r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr;
+  st = plf_lsd_grow(ctx, w, h, r.lp, 2 * r.B);
+  ctx->lsd_keylines_wait = nullptr;
+  if (st) return st;
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp + 1, plf_lsd_overflow_flag(ctx), sizeof(int), cudaMemcpyDeviceToDevice, sG));
+  PLF_CUDA(ctx, cudaMemsetAsync(plf_lsd_overflow_flag(ctx), 0, sizeof(int), sG));
+  PLF_CUDA(ctx, cudaEventRecord(s->evG[par], sG));
+  return PLF_OK;
+}
+
+// One windowed-matching launch over B problems of one kind (points: cap = K, lines: cap = Ln).  Problem p matches the
+// descriptor rows of image / slot p * step of `desc` (n1[p * step] of them) against those of the next image / slot.
+static MgbArgs mgb_args(const plf_params& P, MgGrid g, bool lines, int cap, int step, const int* q_geo, const int* t_geo,
+                        const double* t_dir, const uint8_t* desc, const int* cnt, int32_t* m12, size_t m12_stride, int* count,
+                        int count_stride) {
+  MgbArgs a = {};
+  a.g = g;
+  a.is_lines = lines ? 1 : 0; a.K = cap; a.best_lr = P.best_lr_matches ? 1 : 0;
+  a.nnr = lines ? P.min_ratio_12_l : P.min_ratio_12_p;
+  a.line_sim_th = (double)P.line_sim_th;
+  a.q_geo = q_geo; a.t_geo = t_geo; a.t_dir = t_dir;
+  a.d1 = desc; a.d2 = desc + (size_t)cap * 32; a.d1_stride = a.d2_stride = (size_t)step * cap * 32;
+  a.n1 = cnt; a.n2 = cnt + 1; a.n1_stride = a.n2_stride = step;
+  a.m12 = m12; a.m12_stride = m12_stride; a.count = count; a.count_stride = count_stride;
+  return a;
+}
+
+// ---- M phase: LBD, stereo association, frame-to-frame tracking, pose (needs the previous batch's M phase) ----
+static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
+  const int w = s->w, h = s->h, B = r.B, par = r.par, rp = r.rp;
+  const size_t A = (size_t)w * h;
+  const int K = s->max_kp, Ln = s->max_ln;
+  const plf_params& P = ctx->params;
+  plf_keypoint* kps; uint8_t* odesc; int* kcnt; int mk;
+  plf_keyline* kls; int* lcnt; int ml;
+  plf_orb_outputs(ctx, par, &kps, &odesc, &kcnt, &mk);
+  plf_lsd_outputs(ctx, r.lp, &kls, &lcnt, &ml);
+  cudaStream_t cs = r.sM;
+  ctx->cur = cs;
+  plf_status st;
+  PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->evG[par], 0));
+  PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->evE[par], 0));
+  PLF_CUDA(ctx, cudaEventRecord(s->tM0[rp], cs));
+  if (!s->has_prev) {  // initialize(): no previous frame to track against
+    PLF_CUDA(ctx, cudaMemsetAsync(s->fs.pt_count, 0, sizeof(int), cs));
+    PLF_CUDA(ctx, cudaMemsetAsync(s->fs.ls_count, 0, sizeof(int), cs));
+  }
+  if ((st = plf_launch_lbd(ctx, s->lbd_grad[par], A, w, h, 2 * B, kls, lcnt, Ln, s->ldesc_raw, nullptr))) return st;
+  plf_mark(ctx, "lbd.k_lbd");
+  // the rest of the match phase works on its own copy of the extraction outputs; evX releases this parity to batch i+2
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->kpsM, kps, sizeof(plf_keypoint) * 2 * (size_t)B * K, cudaMemcpyDeviceToDevice, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->descM, odesc, 32 * 2 * (size_t)B * K, cudaMemcpyDeviceToDevice, cs));
+  // has_points / has_lines = 0 (stvo-pl skips the disabled kind in extraction and f2fTracking): its counts are zero from
+  // here on, so it has no stereo rows, no matches, no pose rows and reports 0 detected features
+  if (P.has_points) PLF_CUDA(ctx, cudaMemcpyAsync(s->kcntM, kcnt, sizeof(int) * 2 * (size_t)B, cudaMemcpyDeviceToDevice, cs));
+  else PLF_CUDA(ctx, cudaMemsetAsync(s->kcntM, 0, sizeof(int) * 2 * (size_t)B, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->klsM, kls, sizeof(plf_keyline) * 2 * (size_t)B * Ln, cudaMemcpyDeviceToDevice, cs));
+  if (P.has_lines) PLF_CUDA(ctx, cudaMemcpyAsync(s->lcntM, lcnt, sizeof(int) * 2 * (size_t)B, cudaMemcpyDeviceToDevice, cs));
+  else PLF_CUDA(ctx, cudaMemsetAsync(s->lcntM, 0, sizeof(int) * 2 * (size_t)B, cs));
+  PLF_CUDA(ctx, cudaEventRecord(s->evX[par], cs));
+  kps = s->kpsM; odesc = s->descM; kcnt = s->kcntM; kls = s->klsM; lcnt = s->lcntM;
+  plf_mark(ctx, "copy extraction outputs");
+  PLF_CUDA(ctx, cudaMemsetAsync(s->mcount, 0, (size_t)B * 4 * sizeof(int), cs));
+  const double mg_iw = PLF_GRID_COLS / (double)w, mg_ih = PLF_GRID_ROWS / (double)h;   // StereoFrame::inv_width / inv_height
+  if (P.matching_strategy) {
+    // stereo association through matchGrid(): window (matching_s_ws, 0) x (0, 0) over the right image's grid
+    k_mg_geom_stereo<<<dim3((std::max(K, Ln) + 255) / 256, 2 * B), 256, 0, cs>>>(kps, kcnt, K, kls, lcnt, Ln, mg_iw, mg_ih, s->mg_q[0],
+                                                                                 s->mg_t[0], s->mg_q[1], s->mg_t[1], s->mg_dir[0]);
+    PLF_LAUNCH_CHECK(ctx);
+    const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, P.matching_s_ws, 0, 0, 0};
+    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 2, s->mg_q[0], s->mg_t[0], nullptr, odesc, kcnt, s->m12,
+                                                        4 * (size_t)K, s->mcount, 4), B, K))) return st;
+    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 2, s->mg_q[1], s->mg_t[1], s->mg_dir[0], s->ldesc_raw, lcnt,
+                                                        s->m12 + K, 4 * (size_t)K, s->mcount + 1, 4), B, Ln))) return st;
+    plf_mark(ctx, "stereo.k_mgb (matchGrid)");
+  } else {
+    // L->R 2-NN for every left feature; R->L only for the right features that are somebody's accepted best match
+    // (k_nnr_mutual reads nothing else of the reverse direction): the same matches for ~2/3 of the popcounts
+    if ((st = plf_launch_knn2(ctx, s->knn_stereo, 2 * B, std::max(K, Ln)))) return st;
+    if (P.best_lr_matches) {
+      PLF_CUDA(ctx, cudaMemsetAsync(s->rev_flags, 0, 2 * (size_t)B * K * sizeof(int), cs));
+      PLF_CUDA(ctx, cudaMemsetAsync(s->rev_count, 0, 2 * (size_t)B * sizeof(int), cs));
+      if ((st = plf_launch_nnr_mark(ctx, s->nnr_stereo, 2 * B, std::max(K, Ln), s->rev_flags, s->rev_list, s->rev_count, K))) return st;
+      // the reverse problems are laid out after the forward problems of ALL max_batch pairs (pipe_prepare), not of this
+      // call's B pairs: a partial batch (B < max_batch) must still start at 2 * max_batch
+      if ((st = plf_launch_knn2(ctx, s->knn_stereo + 2 * s->B, 2 * B, std::max(K, Ln)))) return st;
+    }
+    plf_mark(ctx, "stereo.k_hamming_knn2");
+    if ((st = plf_launch_nnr(ctx, s->nnr_stereo, 2 * B, std::max(K, Ln)))) return st;
+    plf_mark(ctx, "stereo.k_nnr_mutual");
+  }
+  StereoPrm sp = {P.max_dist_epip, P.min_disp, P.line_horiz_th, P.stereo_overlap_th, P.ls_min_disp_ratio,
+                  ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy, ctx->cam.b};
+  k_stereo_points<<<B, 1024, 0, cs>>>(kps, odesc, kcnt, K, s->m12, 4 * K, sp, s->fs, 1);
+  PLF_LAUNCH_CHECK(ctx);
+  k_stereo_lines<<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, sp, s->fs, 1);
+  PLF_LAUNCH_CHECK(ctx);
+  plf_mark(ctx, "stereo.k_stereo_points+lines");
+  if ((st = plf_launch_knn2(ctx, s->knn_f2f, 4 * B, std::max(K, Ln)))) return st;
+  plf_mark(ctx, "f2f.k_hamming_knn2");
+  if ((st = plf_launch_nnr(ctx, s->nnr_f2f, 2 * B, std::max(K, Ln)))) return st;
+  if (P.matching_strategy) {
+    // frame-to-frame: matchGrid() in a +-matching_f2f_ws window around the projected feature; the match() result above
+    // stands where the window search found fewer than min_pt_matches / min_ls_matches
+    PLF_CUDA(ctx, cudaMemsetAsync(s->mgcount, 0, (size_t)B * 2 * sizeof(int), cs));
+    k_mg_geom_f2f<<<dim3((std::max(K, Ln) + 255) / 256, B), 256, 0, cs>>>(s->fs, K, Ln, sp, mg_iw, mg_ih, s->mg_q[2], s->mg_t[2],
+                                                                          s->mg_q[3], s->mg_t[3], s->mg_dir[1]);
+    PLF_LAUNCH_CHECK(ctx);
+    const int ws = P.matching_f2f_ws;
+    const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, ws, ws, ws, ws};
+    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 1, s->mg_q[2], s->mg_t[2], nullptr, s->fs.pdesc, s->fs.pt_count,
+                                                        s->m12g, 2 * (size_t)K, s->mgcount, 2), B, K))) return st;
+    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 1, s->mg_q[3], s->mg_t[3], s->mg_dir[1], s->fs.ldesc, s->fs.ls_count,
+                                                        s->m12g + K, 2 * (size_t)K, s->mgcount + 1, 2), B, Ln))) return st;
+    k_mg_select<<<dim3((K + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.pt_count, K, K, 0, P.min_pt_matches, s->m12);
+    PLF_LAUNCH_CHECK(ctx);
+    k_mg_select<<<dim3((Ln + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.ls_count, Ln, K, 1, P.min_ls_matches, s->m12);
+    PLF_LAUNCH_CHECK(ctx);
+    plf_mark(ctx, "f2f.k_mgb (matchGrid)");
+  }
+  k_f2f_build<<<B, 1024, 0, cs>>>(s->fs, 0, K, Ln, s->m12 + 2 * K, s->m12 + 3 * K, 4 * K, s->gnP, s->gnObs, s->gnInlP, s->gnNp,
+                                  s->gn_sP, s->gn_eP, s->gn_le, s->gnInlL, s->gnNl);
+  PLF_LAUNCH_CHECK(ctx);
+  plf_mark(ctx, "f2f.k_nnr_mutual+k_f2f_build");
+  if ((st = plf_launch_gn(ctx, s->gn_probs, B, plf_gn_opts_from_params(P)))) return st;
+  plf_mark(ctx, "gn.k_gn_pose");
+  k_finalize<<<(B + 127) / 128, 128, 0, cs>>>(s->gn_out, s->gnNp, s->gnNl, kcnt, lcnt, s->fs, 1, P.min_features,
+                                               s->has_prev ? 0 : 1, B, s->results + (size_t)rp * s->B);
+  PLF_LAUNCH_CHECK(ctx);
+  if ((st = copy_slot(ctx, s, B, 0))) return st;  // carry the last frame to the next batch
+  plf_mark(ctx, "k_finalize+carry");
+  // results + overflow flags to pinned memory as part of this batch's stream work; evM marks them ready
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->h_results[rp], s->results + (size_t)rp * s->B, sizeof(plf_frame_result) * B, cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->h_ovf[rp], s->d_ovf + 2 * rp, 2 * sizeof(int), cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaEventRecord(s->evM[rp], cs));
   return PLF_OK;
 }
 
@@ -690,192 +858,31 @@ void* plf_batch_device_images(plf_ctx* ctx) {
 plf_status plf_batch_run(plf_ctx* ctx, int B) {
   if (!ctx || B < 1 || B > ctx->limits.max_batch) return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_run: bad B");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  const int w = ctx->cam.width, h = ctx->cam.height;
-  plf_status st = pipe_prepare(ctx, w, h);
+  plf_status st = pipe_prepare(ctx, ctx->cam.width, ctx->cam.height);
   if (st) return st;
   PipeState* s = ctx->pipe;
   if (s->n_pending >= 3)
     return plf_fail(ctx, PLF_ERR_STATE, "plf_batch_run: three batches already in flight; call plf_batch_download first");
-  const size_t A = (size_t)w * h, AP = (size_t)s->pitch * h;   // dense maps / padded images
-  const int K = s->max_kp, Ln = s->max_ln;
-  const plf_params& P = ctx->params;
-  const int par = (int)(s->seq & 1);   // parity of the E -> G -> M hand-off buffers
-  const int rp = (int)(s->seq % 3);    // slot of the result ring
-  const int run_slot = s->up_slot;  // consume the most recently uploaded batch
-  const uint8_t* imgs = s->imgs2[run_slot];
-  s->imgs = s->imgs2[run_slot];
+  BatchRun r;
+  r.B = B;
+  r.par = (int)(s->seq & 1);
+  r.rp = (int)(s->seq % 3);
+  r.run_slot = s->up_slot;
   // With profiling on everything is serialised on the main stream so that the per-kernel marks are meaningful.
-  const bool piped = !ctx->profile || ctx->profile_piped;
-  cudaStream_t sM = ctx->stream, sE = piped ? ctx->aux[0] : sM, sG = piped ? ctx->aux[1] : sM;
-  const bool lsd2 = s->lsd2;
-  cudaStream_t sP = (piped && lsd2) ? ctx->aux[2] : sG;   // LSD pre-grow chain: own stream when its outputs exist per parity
-  const int lp = lsd2 ? par : 0;                         // parity of the LSD hand-off buffers
-  plf_keypoint* kps; uint8_t* odesc; int* kcnt; int mk;
-  plf_keyline* kls; int* lcnt; int ml;
-  plf_orb_outputs(ctx, par, &kps, &odesc, &kcnt, &mk);
-  plf_lsd_outputs(ctx, lp, &kls, &lcnt, &ml);
-
-  // ---- E phase: ORB + LBD gradient prelude (bandwidth / ALU bound); outputs per batch parity ----
-  ctx->cur = sE;
-  PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_up[run_slot], 0));  // images uploaded
-  PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->evX[par], 0));         // batch i-2 (same parity) no longer reads these buffers
-  plf_mark(ctx, "start");
-  PLF_CUDA(ctx, cudaEventRecord(s->tE0[par], sE));
-  st = plf_orb_run(ctx, imgs, AP, s->pitch, w, h, 2 * B, par);
-  if (!st) st = plf_launch_blur5_sobel(ctx, imgs, s->pitch, AP, w, h, 2 * B, s->lbd_grad[par], A);
-  if (st) { ctx->cur = sM; return st; }
-  plf_mark(ctx, "lbd.k_blur5_sobel");
-  // this batch's ORB overflow flag: snapshot + clear on the E stream, so that a flag raised by batch i+1's extraction is
-  // not reported on batch i's download
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * rp, plf_orb_overflow_flag(ctx), sizeof(int), cudaMemcpyDeviceToDevice, sE));
-  PLF_CUDA(ctx, cudaMemsetAsync(plf_orb_overflow_flag(ctx), 0, sizeof(int), sE));
-  PLF_CUDA(ctx, cudaEventRecord(s->evE[par], sE));
-  PLF_CUDA(ctx, cudaEventRecord(s->ev_free[run_slot], sE));  // the image buffer may be overwritten by the next upload
-
-  // ---- P / G phases: the LSD chain.  P = blur / resize / gradient / seed ordering (bandwidth-bound), G = region growing
-  // (latency bound, one warp per image), rectangle fit and KeyLines.  With the hand-off maps per batch parity (lsd2, the
-  // default where they fit) P runs on its own stream: P(i+1) overlaps G(i), and the chain on the critical path is G alone;
-  // with one copy P and G share a stream and LSD(i+1) starts when LSD(i) ends.  The buffers only G writes and reads
-  // (region points, regions, segments) exist once either way: G(i+1) follows G(i) on its stream. ----
-  ctx->cur = sP;
-  PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_up[run_slot], 0));
-  if (lsd2) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->evG[par], 0));   // batch i-2 (same parity) has finished growing / fitting on these maps
-  PLF_CUDA(ctx, cudaEventRecord(s->tG0[par], sP));
-  st = plf_lsd_pre_range(ctx, imgs, AP, s->pitch, w, h, lp, 0, 2 * B);
-  if (st) { ctx->cur = sM; return st; }
-  PLF_CUDA(ctx, cudaEventRecord(s->ev_free2[run_slot], sP));
-  PLF_CUDA(ctx, cudaEventRecord(s->evP[par], sP));
-  ctx->cur = sG;
-  PLF_CUDA(ctx, cudaStreamWaitEvent(sG, s->evP[par], 0));
-  // the KeyLine outputs are overwritten: the match phase that read them last (batch i-2 with two parities, batch i-1 with one)
-  // has taken its copy
-  ctx->lsd_keylines_wait = piped ? s->evX[lsd2 ? par : par ^ 1] : nullptr;
-  st = plf_lsd_grow_range(ctx, w, h, lp, 0, 2 * B);
-  ctx->lsd_keylines_wait = nullptr;
-  if (st) { ctx->cur = sM; return st; }
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * rp + 1, plf_lsd_overflow_flag(ctx), sizeof(int), cudaMemcpyDeviceToDevice, sG));
-  PLF_CUDA(ctx, cudaMemsetAsync(plf_lsd_overflow_flag(ctx), 0, sizeof(int), sG));
-  PLF_CUDA(ctx, cudaEventRecord(s->evG[par], sG));
-
-  // ---- M phase: LBD, stereo association, frame-to-frame tracking, pose (needs the previous batch's M phase) ----
-  ctx->cur = sM;
-  cudaStream_t cs = sM;
-  PLF_CUDA(ctx, cudaStreamWaitEvent(sM, s->evG[par], 0));
-  PLF_CUDA(ctx, cudaStreamWaitEvent(sM, s->evE[par], 0));
-  PLF_CUDA(ctx, cudaEventRecord(s->tM0[rp], sM));
-  if (!s->has_prev) {  // initialize(): no previous frame to track against
-    PLF_CUDA(ctx, cudaMemsetAsync(s->fs.pt_count, 0, sizeof(int), cs));
-    PLF_CUDA(ctx, cudaMemsetAsync(s->fs.ls_count, 0, sizeof(int), cs));
-  }
-  if ((st = plf_launch_lbd(ctx, s->lbd_grad[par], A, w, h, 2 * B, kls, lcnt, Ln, s->ldesc_raw, nullptr))) return st;
-  plf_mark(ctx, "lbd.k_lbd");
-  // the rest of the match phase works on its own copy of the extraction outputs; evX releases this parity to batch i+2
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->kpsM, kps, sizeof(plf_keypoint) * 2 * (size_t)B * K, cudaMemcpyDeviceToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->descM, odesc, 32 * 2 * (size_t)B * K, cudaMemcpyDeviceToDevice, cs));
-  // has_points / has_lines = 0 (stvo-pl skips the disabled kind in extraction and f2fTracking): its counts are zero from
-  // here on, so it has no stereo rows, no matches, no pose rows and reports 0 detected features
-  if (P.has_points) PLF_CUDA(ctx, cudaMemcpyAsync(s->kcntM, kcnt, sizeof(int) * 2 * (size_t)B, cudaMemcpyDeviceToDevice, cs));
-  else PLF_CUDA(ctx, cudaMemsetAsync(s->kcntM, 0, sizeof(int) * 2 * (size_t)B, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->klsM, kls, sizeof(plf_keyline) * 2 * (size_t)B * Ln, cudaMemcpyDeviceToDevice, cs));
-  if (P.has_lines) PLF_CUDA(ctx, cudaMemcpyAsync(s->lcntM, lcnt, sizeof(int) * 2 * (size_t)B, cudaMemcpyDeviceToDevice, cs));
-  else PLF_CUDA(ctx, cudaMemsetAsync(s->lcntM, 0, sizeof(int) * 2 * (size_t)B, cs));
-  PLF_CUDA(ctx, cudaEventRecord(s->evX[par], cs));
-  kps = s->kpsM; odesc = s->descM; kcnt = s->kcntM; kls = s->klsM; lcnt = s->lcntM;
-  plf_mark(ctx, "copy extraction outputs");
-  PLF_CUDA(ctx, cudaMemsetAsync(s->mcount, 0, (size_t)B * 4 * sizeof(int), cs));
-  const double mg_iw = PLF_GRID_COLS / (double)w, mg_ih = PLF_GRID_ROWS / (double)h;   // StereoFrame::inv_width / inv_height
-  MgbArgs mga = {};
-  if (P.matching_strategy) {
-    // stereo association through matchGrid(): window (matching_s_ws, 0) x (0, 0) over the right image's grid
-    k_mg_geom_stereo<<<dim3((std::max(K, Ln) + 255) / 256, 2 * B), 256, 0, cs>>>(kps, kcnt, K, kls, lcnt, Ln, mg_iw, mg_ih, s->mg_q[0],
-                                                                                 s->mg_t[0], s->mg_q[1], s->mg_t[1], s->mg_dir[0]);
-    PLF_LAUNCH_CHECK(ctx);
-    mga.g = {PLF_GRID_COLS, PLF_GRID_ROWS, P.matching_s_ws, 0, 0, 0};
-    mga.best_lr = P.best_lr_matches ? 1 : 0;
-    mga.line_sim_th = (double)P.line_sim_th;
-    mga.is_lines = 0; mga.K = K; mga.nnr = P.min_ratio_12_p;
-    mga.q_geo = s->mg_q[0]; mga.t_geo = s->mg_t[0]; mga.t_dir = nullptr;
-    mga.d1 = odesc; mga.d1_stride = 2 * (size_t)K * 32; mga.d2 = odesc + (size_t)K * 32; mga.d2_stride = 2 * (size_t)K * 32;
-    mga.n1 = kcnt; mga.n1_stride = 2; mga.n2 = kcnt + 1; mga.n2_stride = 2;
-    mga.m12 = s->m12; mga.m12_stride = 4 * (size_t)K; mga.count = s->mcount; mga.count_stride = 4;
-    if ((st = plf_launch_match_grid_batch(ctx, mga, B, K))) return st;
-    mga.is_lines = 1; mga.K = Ln; mga.nnr = P.min_ratio_12_l;
-    mga.q_geo = s->mg_q[1]; mga.t_geo = s->mg_t[1]; mga.t_dir = s->mg_dir[0];
-    mga.d1 = s->ldesc_raw; mga.d1_stride = 2 * (size_t)Ln * 32; mga.d2 = s->ldesc_raw + (size_t)Ln * 32; mga.d2_stride = 2 * (size_t)Ln * 32;
-    mga.n1 = lcnt; mga.n2 = lcnt + 1;
-    mga.m12 = s->m12 + K; mga.count = s->mcount + 1;
-    if ((st = plf_launch_match_grid_batch(ctx, mga, B, Ln))) return st;
-    plf_mark(ctx, "stereo.k_mgb (matchGrid)");
-  } else {
-  // L->R 2-NN for every left feature; R->L only for the right features that are somebody's accepted best match
-  // (k_nnr_mutual reads nothing else of the reverse direction): the same matches for ~2/3 of the popcounts
-  if ((st = plf_launch_knn2(ctx, s->knn_stereo, 2 * B, std::max(K, Ln)))) return st;
-  if (P.best_lr_matches) {
-    PLF_CUDA(ctx, cudaMemsetAsync(s->rev_flags, 0, 2 * (size_t)B * K * sizeof(int), cs));
-    PLF_CUDA(ctx, cudaMemsetAsync(s->rev_count, 0, 2 * (size_t)B * sizeof(int), cs));
-    if ((st = plf_launch_nnr_mark(ctx, s->nnr_stereo, 2 * B, std::max(K, Ln), s->rev_flags, s->rev_list, s->rev_count, K))) return st;
-    // the reverse problems are laid out after the forward problems of ALL max_batch pairs (pipe_prepare), not of this
-    // call's B pairs: a partial batch (B < max_batch) must still start at 2 * max_batch
-    if ((st = plf_launch_knn2(ctx, s->knn_stereo + 2 * s->B, 2 * B, std::max(K, Ln)))) return st;
-  }
-  plf_mark(ctx, "stereo.k_hamming_knn2");
-  if ((st = plf_launch_nnr(ctx, s->nnr_stereo, 2 * B, std::max(K, Ln)))) return st;
-  plf_mark(ctx, "stereo.k_nnr_mutual");
-  }
-  StereoPrm sp = {P.max_dist_epip, P.min_disp, P.line_horiz_th, P.stereo_overlap_th, P.ls_min_disp_ratio,
-                  ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy, ctx->cam.b};
-  k_stereo_points<<<B, 1024, 0, cs>>>(kps, odesc, kcnt, K, s->m12, 4 * K, sp, s->fs, 1);
-  PLF_LAUNCH_CHECK(ctx);
-  k_stereo_lines<<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, sp, s->fs, 1);
-  PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "stereo.k_stereo_points+lines");
-  if ((st = plf_launch_knn2(ctx, s->knn_f2f, 4 * B, std::max(K, Ln)))) return st;
-  plf_mark(ctx, "f2f.k_hamming_knn2");
-  if ((st = plf_launch_nnr(ctx, s->nnr_f2f, 2 * B, std::max(K, Ln)))) return st;
-  if (P.matching_strategy) {
-    // frame-to-frame: matchGrid() in a +-matching_f2f_ws window around the projected feature; the match() result above
-    // stands where the window search found fewer than min_pt_matches / min_ls_matches
-    PLF_CUDA(ctx, cudaMemsetAsync(s->mgcount, 0, (size_t)B * 2 * sizeof(int), cs));
-    k_mg_geom_f2f<<<dim3((std::max(K, Ln) + 255) / 256, B), 256, 0, cs>>>(s->fs, K, Ln, sp, mg_iw, mg_ih, s->mg_q[2], s->mg_t[2],
-                                                                          s->mg_q[3], s->mg_t[3], s->mg_dir[1]);
-    PLF_LAUNCH_CHECK(ctx);
-    const int ws = P.matching_f2f_ws;
-    mga.g = {PLF_GRID_COLS, PLF_GRID_ROWS, ws, ws, ws, ws};
-    mga.is_lines = 0; mga.K = K; mga.nnr = P.min_ratio_12_p;
-    mga.q_geo = s->mg_q[2]; mga.t_geo = s->mg_t[2]; mga.t_dir = nullptr;
-    mga.d1 = s->fs.pdesc; mga.d1_stride = (size_t)K * 32; mga.d2 = s->fs.pdesc + (size_t)K * 32; mga.d2_stride = (size_t)K * 32;
-    mga.n1 = s->fs.pt_count; mga.n1_stride = 1; mga.n2 = s->fs.pt_count + 1; mga.n2_stride = 1;
-    mga.m12 = s->m12g; mga.m12_stride = 2 * (size_t)K; mga.count = s->mgcount; mga.count_stride = 2;
-    if ((st = plf_launch_match_grid_batch(ctx, mga, B, K))) return st;
-    mga.is_lines = 1; mga.K = Ln; mga.nnr = P.min_ratio_12_l;
-    mga.q_geo = s->mg_q[3]; mga.t_geo = s->mg_t[3]; mga.t_dir = s->mg_dir[1];
-    mga.d1 = s->fs.ldesc; mga.d1_stride = (size_t)Ln * 32; mga.d2 = s->fs.ldesc + (size_t)Ln * 32; mga.d2_stride = (size_t)Ln * 32;
-    mga.n1 = s->fs.ls_count; mga.n2 = s->fs.ls_count + 1;
-    mga.m12 = s->m12g + K; mga.count = s->mgcount + 1;
-    if ((st = plf_launch_match_grid_batch(ctx, mga, B, Ln))) return st;
-    k_mg_select<<<dim3((K + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.pt_count, K, K, 0, P.min_pt_matches, s->m12);
-    PLF_LAUNCH_CHECK(ctx);
-    k_mg_select<<<dim3((Ln + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.ls_count, Ln, K, 1, P.min_ls_matches, s->m12);
-    PLF_LAUNCH_CHECK(ctx);
-    plf_mark(ctx, "f2f.k_mgb (matchGrid)");
-  }
-  k_f2f_build<<<B, 1024, 0, cs>>>(s->fs, 0, K, Ln, s->m12 + 2 * K, s->m12 + 3 * K, 4 * K, s->gnP, s->gnObs, s->gnInlP, s->gnNp,
-                                  s->gn_sP, s->gn_eP, s->gn_le, s->gnInlL, s->gnNl);
-  PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "f2f.k_nnr_mutual+k_f2f_build");
-  if ((st = plf_launch_gn(ctx, s->gn_probs, B, plf_gn_opts_from_params(P)))) return st;
-  plf_mark(ctx, "gn.k_gn_pose");
-  k_finalize<<<(B + 127) / 128, 128, 0, cs>>>(s->gn_out, s->gnNp, s->gnNl, kcnt, lcnt, s->fs, 1, P.min_features,
-                                               s->has_prev ? 0 : 1, B, s->results + (size_t)rp * s->B);
-  PLF_LAUNCH_CHECK(ctx);
-  if ((st = copy_slot(ctx, s, B, 0))) return st;  // carry the last frame to the next batch
-  plf_mark(ctx, "k_finalize+carry");
-  // results + overflow flags to pinned memory as part of this batch's stream work; evM marks them ready
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->h_results[rp], s->results + (size_t)rp * s->B, sizeof(plf_frame_result) * B, cudaMemcpyDeviceToHost, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->h_ovf[rp], s->d_ovf + 2 * rp, 2 * sizeof(int), cudaMemcpyDeviceToHost, cs));
-  PLF_CUDA(ctx, cudaEventRecord(s->evM[rp], cs));
+  r.piped = !ctx->profile || ctx->profile_piped;
+  r.lsd2 = s->lsd2;
+  r.lp = r.lsd2 ? r.par : 0;
+  r.sM = ctx->stream;
+  r.sE = r.piped ? ctx->aux[0] : r.sM;
+  r.sG = r.piped ? ctx->aux[1] : r.sM;
+  r.sP = (r.piped && r.lsd2) ? ctx->aux[2] : r.sG;   // LSD pre-grow chain: own stream when its outputs exist per parity
+  st = run_extract(ctx, s, r);
+  if (!st) st = run_lsd(ctx, s, r);
+  if (!st) st = run_match(ctx, s, r);
+  ctx->cur = r.sM;
+  if (st) return st;
   s->has_prev = true;
-  s->pend_slot[s->n_pending] = rp;
+  s->pend_slot[s->n_pending] = r.rp;
   s->pend_B[s->n_pending] = B;
   s->n_pending++;
   s->seq++;
@@ -967,12 +974,16 @@ plf_status plf_get_frame(plf_ctx* ctx, int k, plf_frame_view* v) {
   v->n_pt = np; v->n_ls = nl;
   if (np > v->cap_pt || nl > v->cap_ls)
     return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_get_frame: %d points / %d lines exceed the view capacity", np, nl);
-#define GET(dst, src, per, n, base) if ((dst) && (n) > 0) PLF_CUDA(ctx, cudaMemcpyAsync((dst), (const char*)(src) + (size_t)slot * (base) * (per), (size_t)(n) * (per), cudaMemcpyDeviceToHost, cs))
-  GET(v->pt_pl, f.pt_pl, 16, np, K); GET(v->pt_disp, f.pt_disp, 8, np, K); GET(v->pt_P, f.pt_P, 24, np, K);
-  GET(v->pt_octave, f.pt_octave, 4, np, K); GET(v->pdesc, f.pdesc, 32, np, K);
-  GET(v->ls_spl, f.ls_spl, 16, nl, Ln); GET(v->ls_epl, f.ls_epl, 16, nl, Ln); GET(v->ls_sdisp, f.ls_sdisp, 8, nl, Ln);
-  GET(v->ls_edisp, f.ls_edisp, 8, nl, Ln); GET(v->ls_sP, f.ls_sP, 24, nl, Ln); GET(v->ls_eP, f.ls_eP, 24, nl, Ln);
-  GET(v->ls_le, f.ls_le, 24, nl, Ln); GET(v->ls_angle, f.ls_angle, 4, nl, Ln); GET(v->ldesc, f.ldesc, 32, nl, Ln);
+#define GET(name, n, cap, per)                                                                                       \
+  if (v->name && (n) > 0)                                                                                            \
+    PLF_CUDA(ctx, cudaMemcpyAsync(v->name, f.name + (size_t)slot * cap * per, (size_t)(n) * per * sizeof(*f.name),   \
+                                  cudaMemcpyDeviceToHost, cs));
+#define GET_PT(name, T, cap, per) GET(name, np, cap, per)
+#define GET_LS(name, T, cap, per) GET(name, nl, cap, per)
+  PLF_PT_FIELDS(GET_PT)
+  PLF_LS_FIELDS(GET_LS)
+#undef GET_LS
+#undef GET_PT
 #undef GET
   PLF_CUDA(ctx, cudaStreamSynchronize(cs));
   return PLF_OK;

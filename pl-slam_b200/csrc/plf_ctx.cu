@@ -21,6 +21,30 @@ plf_status plf_fail(plf_ctx* ctx, plf_status code, const char* fmt, ...) {
   return code;
 }
 
+size_t DevBufList::bytes() const {
+  size_t n = 0;
+  for (const Entry& e : entries) n += e.bytes;
+  return n;
+}
+
+plf_status DevBufList::alloc(plf_ctx* ctx, const char* owner) {
+  for (const Entry& e : entries) {
+    const cudaError_t err = cudaMalloc(e.slot, e.bytes + 64);
+    if (err != cudaSuccess) {
+      *e.slot = nullptr;
+      return plf_fail(ctx, PLF_ERR_CUDA, "%s: cudaMalloc(%zu): %s", owner, e.bytes, cudaGetErrorString(err));
+    }
+  }
+  return PLF_OK;
+}
+
+void DevBufList::release() {
+  for (const Entry& e : entries) {
+    cudaFree(*e.slot);
+    *e.slot = nullptr;
+  }
+}
+
 void* plf_scratch(plf_ctx* ctx, int slot, size_t bytes) {
   DevBuf& b = ctx->scratch[slot];
   if (b.bytes >= bytes && b.p) return b.p;

@@ -16,10 +16,16 @@ struct DevBuf {
   size_t bytes = 0;
 };
 
-// Scratch arena: grows on demand (cudaMalloc), never shrinks; all users are stream-ordered on
-// ctx->stream so reuse between calls is safe.
-struct Scratch {
-  std::vector<DevBuf> bufs;
+// The device buffers of one subsystem, declared once as (pointer slot, bytes): the same list gives the footprint, the
+// allocation (one cudaMalloc per buffer, each with 64 bytes of slack for plf_load4, see plf_image_span) and the release.
+struct DevBufList {
+  struct Entry { void** slot; size_t bytes; };
+  std::vector<Entry> entries;
+  template <typename T>
+  void add(T*& p, size_t n) { entries.push_back({reinterpret_cast<void**>(&p), n * sizeof(T)}); }
+  size_t bytes() const;
+  plf_status alloc(plf_ctx* ctx, const char* owner);   // on failure the buffers allocated so far stay listed
+  void release();                                      // frees every buffer and nulls its slot
 };
 
 struct plf_ctx {
@@ -27,7 +33,7 @@ struct plf_ctx {
   cudaStream_t stream = nullptr;  // main stream: copies, the serial part of the pipeline, standalone operators
   cudaStream_t cur = nullptr;     // stream the launch helpers enqueue on (== stream except inside forked sections)
   cudaStream_t aux[3] = {nullptr, nullptr, nullptr};  // streams of the extraction (E), LSD growing (G) and LSD pre-grow (P) phases of plf_batch_run
-  cudaEvent_t lsd_keylines_wait = nullptr;  // if set: plf_lsd_grow_range waits for it before it overwrites the KeyLine outputs
+  cudaEvent_t lsd_keylines_wait = nullptr;  // if set: plf_lsd_grow waits for it before it overwrites the KeyLine outputs
   plf_params params;
   plf_camera cam;
   plf_limits limits;
@@ -172,8 +178,8 @@ void plf_resize_pack_x(const int* ofs, const int* c1, int dw, int* out);   // ou
 plf_status plf_lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities);
 size_t plf_lsd_footprint(const plf_ctx* ctx, int w, int h, int nimg, bool two_parities);   // bytes plf_lsd_prepare allocates
 plf_status plf_lsd_run(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int nimg);
-plf_status plf_lsd_pre_range(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int par, int img0, int n);
-plf_status plf_lsd_grow_range(plf_ctx* ctx, int w, int h, int par, int img0, int n);
+plf_status plf_lsd_pre(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int par, int n);
+plf_status plf_lsd_grow(plf_ctx* ctx, int w, int h, int par, int n);
 void plf_lsd_outputs(plf_ctx* ctx, int par, plf_keyline** kls, int** nlines, int* max_lines);
 int* plf_orb_overflow_flag(plf_ctx* ctx);
 int* plf_lsd_overflow_flag(plf_ctx* ctx);

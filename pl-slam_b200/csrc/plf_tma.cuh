@@ -44,6 +44,36 @@ static inline bool plf_tma_encode_u8(CUtensorMap* map, const void* base, int w, 
             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// Host: the tensor maps of one kernel over caller-owned images, two entries keyed by source pointer and geometry (the
+// batched pipeline alternates between two upload buffers).  An entry is reused while its image count covers the
+// request; otherwise the least recently used entry is re-encoded.  The box is the owner's and fixed for its lifetime.
+struct PlfTmaCache {
+  struct Entry {
+    const void* src = nullptr;
+    int w = 0, h = 0, nimg = 0;
+    size_t pitch = 0, img_stride = 0;
+    CUtensorMap map;
+  };
+  Entry e[2];
+  int last = 1;   // entry used by the previous call
+  // The map over images [0, nimg) of src, or nullptr if encoding fails.
+  const CUtensorMap* get(const void* src, int w, int h, int nimg, size_t pitch, size_t img_stride, int box_w, int box_h) {
+    for (int k = 0; k < 2; ++k) {
+      const Entry& c = e[k];
+      if (c.src == src && c.w == w && c.h == h && c.pitch == pitch && c.img_stride == img_stride && c.nimg >= nimg) {
+        last = k;
+        return &c.map;
+      }
+    }
+    last ^= 1;
+    Entry& c = e[last];
+    c = Entry();
+    if (!plf_tma_encode_u8(&c.map, src, w, h, nimg, pitch, img_stride, box_w, box_h)) return nullptr;
+    c.src = src; c.w = w; c.h = h; c.nimg = nimg; c.pitch = pitch; c.img_stride = img_stride;
+    return &c.map;
+  }
+};
+
 #ifdef __CUDACC__
 __device__ __forceinline__ uint32_t plf_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 

@@ -173,6 +173,49 @@ def test_batches_in_flight_match_sequential(built):
             assert np.array_equal(a["DT"], b["DT"])          # same kernels, same inputs: bit-identical poses
 
 
+def test_standalone_operators_between_batches(built):
+    """fe.orb / fe.lsd / fe.detect_lines / fe.lbd on an image of another size, called between batches on the same
+    context, rebuild the ORB and LSD state and use their own tensor maps: the batches after them give exactly the results
+    and frames of an uninterrupted run, and the operators return what they return on a fresh context."""
+    cam = dict(plf.KITTI_CAMERA, width=640, height=360, cx=320.0, cy=180.0, fx=500.0, fy=500.0)
+    world = synth.World(seed=4, length=50.0, n_quads=160, n_segs=80, half_width=8.0, half_height=3.5)
+    frames = list(synth.stream(cam, 8, world=world, seed=21, step=0.12))
+    Ls, Rs = np.stack([f[0] for f in frames]), np.stack([f[1] for f in frames])
+    other = next(iter(synth.stream(dict(cam, width=480, height=300, cx=240.0, cy=150.0), 1, world=world, seed=5)))[0]
+    lim = plf.default_limits(); lim.max_batch = 2
+    prm = dict(orb_nfeatures=700, lsd_nfeatures=150)
+
+    def batch(fe, s0):
+        res = fe.process_batch(Ls[s0:s0 + 2], Rs[s0:s0 + 2])
+        return res, [fe.get_frame(k) for k in range(2)]
+
+    def operators(fe):
+        kps, desc = fe.orb(other)
+        segs = fe.lsd(other)
+        kls, ldesc = fe.detect_lines(other)
+        return kps, desc, segs, kls, ldesc, fe.lbd(other, kls)
+
+    with plf.Frontend(camera=cam, limits=lim, **prm) as fe:
+        base = [batch(fe, s0) for s0 in (0, 2, 4, 6)]
+    with plf.Frontend(camera=cam, limits=lim, **prm) as fe:
+        got = [batch(fe, 0), batch(fe, 2)]
+        ops = operators(fe)
+        got += [batch(fe, 4), batch(fe, 6)]
+    with plf.Frontend(camera=cam, limits=lim, **prm) as fe:
+        fresh = operators(fe)
+    assert len(ops[0]) > 0 and len(ops[3]) > 0
+    for a, b in zip(ops, fresh):
+        assert np.array_equal(a, b)
+    for (res_a, fr_a), (res_b, fr_b) in zip(base, got):
+        for a, b in zip(res_a, res_b):
+            for f in plf.RESULT_FIELDS:
+                assert a[f] == b[f], f
+            assert np.array_equal(a["DT"], b["DT"])
+        for a, b in zip(fr_a, fr_b):
+            for k in a:
+                assert np.array_equal(a[k], b[k]), k
+
+
 def test_trajectory_ate_vs_oracle_and_ground_truth(built):
     """north_star: trajectory ATE within 1 % of the reference (CPU oracle) on the same synthetic sequence."""
     cam = dict(plf.KITTI_CAMERA, width=800, height=300, cx=400.0, cy=150.0, fx=520.0, fy=520.0)
