@@ -461,6 +461,56 @@ typedef struct plf_match_view {
 } plf_match_view;
 plf_status plf_get_matches(plf_ctx* ctx, int k, plf_match_view* view);
 
+/* Keyframe matching (SURVEY 8(f) f1): the matching parts of MapHandler::matchKF2KFPoints / matchKF2KFLines and
+ * matchMap2KFPoints / matchMap2KFLines, called by lookForCommonMatches (src/mapHandler.cpp:754-821), on the device from one
+ * upload to one download: projection, visibility, compaction, GridStructure cells, matchGrid() in a +-matching_f2f_ws
+ * window, the match() fallback and the epipolar gate.  The landmark bookkeeping that follows each (new MapPoint / MapLine,
+ * observations, full_graph) stays with the caller.  has_points / has_lines, best_lr_matches, matching_f2f_ws,
+ * min_pt_matches / min_ls_matches, min_ratio_12_p / min_ratio_12_l, line_sim_th and the camera come from the ctx (SlamConfig
+ * inherits them).  Work is enqueued on plf_stream, so a call between batches in flight is safe.  A kind returns 0 (every
+ * entry -1) when it is disabled or the keyframe has no stereo features of it.  Semantics reproduced as written, quirks
+ * included (DESIGN.md 8): see oracle/kfmatching.py. */
+typedef struct plf_kf_match_opts {
+  int fast_matching;    /* SlamConfig::fastMatching  src/slamConfig.cpp:43: 0 = brute-force match() only, and only when
+                           the fallback condition holds (else no pairs) */
+  double max_kf_epip_p; /* SlamConfig::maxKFEpipP  :51 */
+  double max_kf_epip_l; /* SlamConfig::maxKFEpipL  :52 */
+} plf_kf_match_opts;
+
+/* matchKF2KFPoints + matchKF2KFLines (src/mapHandler.cpp:234-278, :365-426), matching part.
+ * prev / curr: the stereo-valid features of the two keyframes in the layout plf_get_frame fills; read: n_pt, n_ls, pt_P,
+ * pdesc, ls_sP, ls_eP, ldesc (prev) and n_pt, n_ls, pt_pl, pdesc, ls_spl, ls_epl, ldesc (curr).  DT: row-major 4x4
+ * (MapHandler::DT).  m_pt[prev->n_pt], m_ls[prev->n_ls]: matches_12 (curr index or -1).  *n_pt, *n_ls: the reference's
+ * return values (may be NULL).  The projected query lines stay in pixels as the reference leaves them (:392-393).
+ * n_pt, n_ls <= 8192 per keyframe; device scratch 2 x prev->n_* x curr->n_* bytes per kind, kept until plf_destroy. */
+plf_status plf_match_kf2kf(plf_ctx* ctx, const plf_kf_match_opts* opts, const plf_frame_view* prev,
+                           const plf_frame_view* curr, const double DT[16], int32_t* m_pt, int32_t* m_ls, int* n_pt,
+                           int* n_ls);
+
+/* The landmarks of MapHandler::map_points / map_lines, in index order (host arrays). */
+typedef struct plf_local_map {
+  int n_pt;
+  const double* pt_X;      /* [n_pt][3] MapPoint::point3D */
+  const uint8_t* pt_desc;  /* [n_pt][32] MapPoint::med_desc */
+  const uint8_t* pt_use;   /* [n_pt] 1 = non-null && local && kf_obs_list.back() != kf_idx (:547); NULL = all */
+  int n_ls;
+  const double* ls_X;      /* [n_ls][6] MapLine::line3D (start | end) */
+  const uint8_t* ls_desc;  /* [n_ls][32] */
+  const uint8_t* ls_use;   /* [n_ls] (:648); NULL = all */
+} plf_local_map;
+
+/* matchMap2KFPoints + matchMap2KFLines (src/mapHandler.cpp:532-632, :634-752): visibility, matching and the epipolar gate.
+ * Twf: row-major 4x4 (MapHandler::Twf).  kf: read n_pt, n_ls, pt_pl, pdesc, ls_spl, ls_epl, ls_le, ldesc.
+ * kf_pt_lm / kf_ls_lm: the keyframe features' landmark index, -1 = unmatched (:565, :670); NULL = all unmatched.
+ * lm_pt[map->n_pt], lm_ls[map->n_ls]: per landmark (original index) the keyframe feature (original index) it was matched
+ * to and that passed the gate, else -1.  *n_pt / *n_ls: the reference's return values (matches minus gate rejects).
+ * At most 65535 landmarks and 8192 keyframe features per kind.  Device scratch: the windowed matcher's distance matrix is
+ * sized from the uncompacted counts, 2 x (map->n_*) x (kf->n_*) bytes per kind (about 1 GB at both limits), and stays
+ * allocated in the ctx (scratch grows, never shrinks) until plf_destroy. */
+plf_status plf_match_map2kf(plf_ctx* ctx, const plf_kf_match_opts* opts, const plf_local_map* map, const double Twf[16],
+                            const plf_frame_view* kf, const int32_t* kf_pt_lm, const int32_t* kf_ls_lm, int32_t* lm_pt,
+                            int32_t* lm_ls, int* n_pt, int* n_ls);
+
 /* Debug: device-clock timeline (ms) of the two most recent batches of the software pipeline: for each, the start/end of
  * the E (extract), G (region growing) and M (match/track/pose) phases relative to the older batch's E start.
  * No reference counterpart (the reference times whole calls with its Timer, app/plslam_dataset.cpp:126-132). */

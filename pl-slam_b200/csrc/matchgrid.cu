@@ -258,24 +258,72 @@ __global__ void __launch_bounds__(128) k_mgb_qmask(MgbArgs a, int p0) {
   }
 }
 
+// The same mask, walking only the steps of the Bresenham line whose window can reach the grid: along the major axis a
+// cell further than the window from the grid contributes nothing, so the walk starts at the first step that can and
+// stops after the last one.  The state of the walk at step n is closed-form - err_n = (dx/2 - n dy) mod dx and the minor
+// coordinate advanced by (err_n - dx/2 + n dy) / dx - so the cells visited are exactly those of the full walk.  Used for
+// queries in pixel units (KF-to-KF lines), whose walk would otherwise cross thousands of cells outside the grid.
+__global__ void __launch_bounds__(128) k_mgb_qmask_clip(MgbArgs a, int p0) {
+  const int pl = blockIdx.y, p = p0 + pl;
+  const int i1 = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K);
+  if (i1 >= n1) return;
+  uint32_t* m = a.qmask + ((size_t)pl * a.K + i1) * MGB_MASK_WORDS;
+  for (int k = lane; k < MGB_MASK_WORDS; k += 32) m[k] = 0u;
+  __syncwarp();
+  const int* q = a.q_geo + ((size_t)p * a.K + i1) * 4;
+  const MgGrid& g = a.g;
+  long long x1 = q[0], y1 = q[1], x2 = q[2], y2 = q[3];
+  const bool steep = llabs(y2 - y1) > llabs(x2 - x1);
+  if (steep) { long long t = x1; x1 = y1; y1 = t; t = x2; x2 = y2; y2 = t; }
+  if (x1 > x2) { long long t = x1; x1 = x2; x2 = t; t = y1; y1 = y2; y2 = t; }
+  const long long dx = x2 - x1, dy = llabs(y2 - y1), e0 = dx / 2, ystep = y1 < y2 ? 1 : -1;
+  // major-axis range whose window reaches the grid
+  const long long lo = steep ? -(long long)g.h_hi : -(long long)g.w_hi;
+  const long long hi = steep ? (long long)g.rows - 1 + g.h_lo : (long long)g.cols - 1 + g.w_lo;
+  const long long n0 = max(0ll, lo - x1), n_end = min(x2, hi) - x1;
+  if (n0 > n_end) return;
+  long long err = e0, y = y1;
+  if (n0 > 0) {   // dx > 0 here (n0 <= n_end <= dx)
+    err = (e0 - n0 * dy) % dx;
+    if (err < 0) err += dx;
+    y = y1 + ystep * ((err - e0 + n0 * dy) / dx);
+  }
+  for (long long n = n0; n <= n_end; ++n) {   // warp-uniform walk; the window's cells are spread over the lanes
+    const long long xx = x1 + n;
+    const int cx = (int)(steep ? y : xx), cy = (int)(steep ? xx : y);   // y may be far outside: its window is then empty
+    err -= dy;
+    if (err < 0) { y += ystep; err += dx; }
+    const long long fx0 = (long long)cx - g.w_lo, fy0 = (long long)cy - g.h_lo;
+    const int x0 = (int)max(0ll, fx0), xe = (int)min((long long)g.cols, (long long)cx + g.w_hi + 1);
+    const int y0 = (int)max(0ll, fy0), ye = (int)min((long long)g.rows, (long long)cy + g.h_hi + 1);
+    const int nx = xe - x0, ny = ye - y0;
+    if (nx <= 0 || ny <= 0) continue;
+    for (int k = lane; k < nx * ny; k += 32) {
+      const int c = (x0 + k / ny) * g.rows + (y0 + k % ny);
+      atomicOr(&m[c >> 5], 1u << (c & 31));
+    }
+  }
+}
+
 template <int IS_LINES>
 __global__ void __launch_bounds__(128) k_mgb_columns(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
   const int i2 = blockIdx.x * 128 + threadIdx.x;
-  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K), n2 = min(a.n2[(size_t)p * a.n2_stride], a.K);
+  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K), n2 = min(a.n2[(size_t)p * a.n2_stride], a.Kt);
   if (i2 >= n2) return;
   const MgGrid& g = a.g;
   const uint4* b = reinterpret_cast<const uint4*>(a.d2 + (size_t)p * a.d2_stride) + 2 * (size_t)i2;
   const uint4* q1 = reinterpret_cast<const uint4*>(a.d1 + (size_t)p * a.d1_stride);
-  const int* tg = a.t_geo + ((size_t)p * a.K + i2) * (IS_LINES ? 4 : 2);
+  const int* tg = a.t_geo + ((size_t)p * a.Kt + i2) * (IS_LINES ? 4 : 2);
   const int* qg = a.q_geo + (size_t)p * a.K * (IS_LINES ? 4 : 2);
-  unsigned short* D = a.D + (size_t)pl * a.K * a.K;
+  unsigned short* D = a.D + (size_t)pl * a.K * a.Kt;
   int tx = 0, ty = 0, t4[4] = {0, 0, 0, 0};
   double tdx = 0, tdy = 0;
   bool t_in = false;
   if (IS_LINES) {
     t4[0] = tg[0]; t4[1] = tg[1]; t4[2] = tg[2]; t4[3] = tg[3];
-    tdx = a.t_dir[((size_t)p * a.K + i2) * 2]; tdy = a.t_dir[((size_t)p * a.K + i2) * 2 + 1];
+    tdx = a.t_dir[((size_t)p * a.Kt + i2) * 2]; tdy = a.t_dir[((size_t)p * a.Kt + i2) * 2 + 1];
   } else {
     tx = tg[0]; ty = tg[1];
     t_in = tx >= 0 && tx < g.cols && ty >= 0 && ty < g.rows;   // pushed outside the grid: never returned
@@ -312,18 +360,18 @@ __global__ void __launch_bounds__(128) k_mgb_columns(MgbArgs a, int p0) {
         out = (unsigned short)d;
       }
     }
-    D[(size_t)i1 * a.K + i2] = out;
+    D[(size_t)i1 * a.Kt + i2] = out;
   }
-  a.m21[(size_t)pl * a.K + i2] = who;
+  a.m21[(size_t)pl * a.Kt + i2] = who;
 }
 
 __global__ void __launch_bounds__(128) k_mgb_rows(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
   const int i1 = blockIdx.x * 128 + threadIdx.x;
-  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K), n2 = min(a.n2[(size_t)p * a.n2_stride], a.K);
+  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K), n2 = min(a.n2[(size_t)p * a.n2_stride], a.Kt);
   if (i1 >= n1) return;
   int best_d = 0x7FFFFFFF, best_d2 = 0x7FFFFFFF, best_idx = -1;
-  const unsigned short* row = a.D + (size_t)pl * a.K * a.K + (size_t)i1 * a.K;
+  const unsigned short* row = a.D + (size_t)pl * a.K * a.Kt + (size_t)i1 * a.Kt;
   for (int i2 = 0; i2 < n2; ++i2) {
     const int d = row[i2];
     if (d == MG_NONE) continue;
@@ -342,40 +390,42 @@ __global__ void __launch_bounds__(128) k_mgb_mutual(MgbArgs a, int p0) {
     int32_t* m12 = a.m12 + (size_t)p * a.m12_stride;
     const int i2 = m12[i1];
     ok = i2 >= 0;
-    if (ok && a.best_lr && a.m21[(size_t)pl * a.K + i2] != i1) { m12[i1] = -1; ok = false; }
+    if (ok && a.best_lr && a.m21[(size_t)pl * a.Kt + i2] != i1) { m12[i1] = -1; ok = false; }
   }
   const unsigned bal = __ballot_sync(0xFFFFFFFFu, ok);
   if ((threadIdx.x & 31) == 0 && bal) atomicAdd(&a.count[(size_t)p * a.count_stride], __popc(bal));
 }
 
-// Runs nprob windowed matching problems.  scratch: MGB scratch of the context (slot 9), sized here.
-plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n) {
+// Runs nprob windowed matching problems.  scratch: MGB scratch of the context (slot `slot`), sized here.
+plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n1, int max_n2, int slot) {
   if (nprob <= 0) return PLF_OK;
   if (a.g.cols * a.g.rows > 32 * MGB_MASK_WORDS) return plf_fail(ctx, PLF_ERR_INVALID, "match grid: %dx%d cells exceed the mask", a.g.cols, a.g.rows);
-  const int K = a.K;
-  const size_t perD = (size_t)K * K * 2, perM = a.is_lines ? (size_t)K * MGB_MASK_WORDS * 4 : 0, per21 = (size_t)K * 4;
+  const int K = a.K, Kt = a.Kt;
+  const size_t perD = (size_t)K * Kt * 2, perM = a.is_lines ? (size_t)K * MGB_MASK_WORDS * 4 : 0, per21 = (size_t)Kt * 4;
   const size_t per = mg_align(perD) + mg_align(perM) + mg_align(per21);
   int chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)nprob, (size_t(1) << 31) / per));   // <= 2 GB of scratch
-  uint8_t* base = (uint8_t*)plf_scratch(ctx, 9, per * chunk);
+  uint8_t* base = (uint8_t*)plf_scratch(ctx, slot, per * chunk);
   if (!base) return PLF_ERR_CUDA;
   a.D = (unsigned short*)base;
   a.qmask = (uint32_t*)(base + mg_align(perD) * chunk);
   a.m21 = (int*)(base + (mg_align(perD) + mg_align(perM)) * chunk);
   cudaStream_t cs = ctx->cur;
-  const int gx = (max_n + 127) / 128;
+  const int gx1 = (max_n1 + 127) / 128, gx2 = (max_n2 + 127) / 128;
+  if (gx1 == 0 || gx2 == 0) return PLF_OK;
   for (int p0 = 0; p0 < nprob; p0 += chunk) {
     const int np = std::min(chunk, nprob - p0);
     if (a.is_lines) {
-      k_mgb_qmask<<<dim3((max_n + 3) / 4, np), 128, 0, cs>>>(a, p0);
+      if (a.clip) k_mgb_qmask_clip<<<dim3((max_n1 + 3) / 4, np), 128, 0, cs>>>(a, p0);
+      else k_mgb_qmask<<<dim3((max_n1 + 3) / 4, np), 128, 0, cs>>>(a, p0);
       PLF_LAUNCH_CHECK(ctx);
-      k_mgb_columns<1><<<dim3(gx, np), 128, 0, cs>>>(a, p0);
+      k_mgb_columns<1><<<dim3(gx2, np), 128, 0, cs>>>(a, p0);
     } else {
-      k_mgb_columns<0><<<dim3(gx, np), 128, 0, cs>>>(a, p0);
+      k_mgb_columns<0><<<dim3(gx2, np), 128, 0, cs>>>(a, p0);
     }
     PLF_LAUNCH_CHECK(ctx);
-    k_mgb_rows<<<dim3(gx, np), 128, 0, cs>>>(a, p0);
+    k_mgb_rows<<<dim3(gx1, np), 128, 0, cs>>>(a, p0);
     PLF_LAUNCH_CHECK(ctx);
-    k_mgb_mutual<<<dim3(gx, np), 128, 0, cs>>>(a, p0);
+    k_mgb_mutual<<<dim3(gx1, np), 128, 0, cs>>>(a, p0);
     PLF_LAUNCH_CHECK(ctx);
   }
   return PLF_OK;

@@ -13,6 +13,7 @@
 // images [2B][H][W] (2k = left, 2k+1 = right) -> ORB / LSD / LBD over 2B images -> per-pair kernels.  The last
 // frame's stereo features are carried to the next call (slot 0).
 #include "plf_internal.h"
+#include "plf_geom.cuh"
 #include "plf_tma.cuh"
 
 // Stereo-valid features per frame slot, [slots][cap][per]: one row per array, (name = its plf_frame_view member, element
@@ -407,9 +408,7 @@ __global__ void k_finalize(const plf_pose_result* __restrict__ gn, const int* __
 }
 
 // ---- windowed matching: grid geometry on the device (oracle/frontend.py grid_match_points / grid_match_lines) ----
-#define PLF_GRID_ROWS 48   // stvo-pl gridStructure.h (SURVEY Appendix A.2)
-#define PLF_GRID_COLS 64
-__device__ __forceinline__ int mg_cell(double v) { return (int)v; }   // double -> int as in C++ (truncation)
+// (cells and projection: plf_geom.cuh)
 
 // stereo: queries = left key points / KeyLines of pair k (image 2k), train = the right ones (image 2k+1)
 __global__ void __launch_bounds__(256) k_mg_geom_stereo(const plf_keypoint* __restrict__ kps, const int* __restrict__ kcnt, int K,
@@ -445,9 +444,9 @@ __global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, int K, int L
   const int ps = k, cs = k + 1;
   if (i < min(fs.pt_count[ps], K)) {
     const double* P = fs.pt_P + 3 * ((size_t)ps * K + i);
-    const double u = c.cx + c.fx * P[0] / P[2], v = c.cy + c.fy * P[1] / P[2];   // PinholeStereoCamera::projection
-    qp[((size_t)k * K + i) * 2] = mg_cell(u * iw);
-    qp[((size_t)k * K + i) * 2 + 1] = mg_cell(v * ih);
+    const double2 u = plf_project(c.fx, c.fy, c.cx, c.cy, P[0], P[1], P[2]);
+    qp[((size_t)k * K + i) * 2] = mg_cell(u.x * iw);
+    qp[((size_t)k * K + i) * 2 + 1] = mg_cell(u.y * ih);
   }
   if (i < min(fs.pt_count[cs], K)) {
     const double2 p = fs.pt_pl[(size_t)cs * K + i];
@@ -458,17 +457,12 @@ __global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, int K, int L
     const double* S = fs.ls_sP + 3 * ((size_t)ps * Ln + i);
     const double* E = fs.ls_eP + 3 * ((size_t)ps * Ln + i);
     int* d = ql + ((size_t)k * Ln + i) * 4;
-    d[0] = mg_cell((c.cx + c.fx * S[0] / S[2]) * iw); d[1] = mg_cell((c.cy + c.fy * S[1] / S[2]) * ih);
-    d[2] = mg_cell((c.cx + c.fx * E[0] / E[2]) * iw); d[3] = mg_cell((c.cy + c.fy * E[1] / E[2]) * ih);
+    d[0] = mg_cell(plf_project_u(c.fx, c.cx, S[0], S[2]) * iw); d[1] = mg_cell(plf_project_v(c.fy, c.cy, S[1], S[2]) * ih);
+    d[2] = mg_cell(plf_project_u(c.fx, c.cx, E[0], E[2]) * iw); d[3] = mg_cell(plf_project_v(c.fy, c.cy, E[1], E[2]) * ih);
   }
-  if (i < min(fs.ls_count[cs], Ln)) {
-    const double2 sp = fs.ls_spl[(size_t)cs * Ln + i], ep = fs.ls_epl[(size_t)cs * Ln + i];
-    int* d = tl + ((size_t)k * Ln + i) * 4;
-    d[0] = mg_cell(sp.x * iw); d[1] = mg_cell(sp.y * ih); d[2] = mg_cell(ep.x * iw); d[3] = mg_cell(ep.y * ih);
-    const double vx = (ep.x - sp.x) * iw, vy = (ep.y - sp.y) * ih, nrm = sqrt(vx * vx + vy * vy);
-    tdir[((size_t)k * Ln + i) * 2] = vx / nrm;
-    tdir[((size_t)k * Ln + i) * 2 + 1] = vy / nrm;
-  }
+  if (i < min(fs.ls_count[cs], Ln))
+    plf_train_line(fs.ls_spl[(size_t)cs * Ln + i], fs.ls_epl[(size_t)cs * Ln + i], iw, ih, tl + ((size_t)k * Ln + i) * 4,
+                   tdir + ((size_t)k * Ln + i) * 2);
 }
 
 // src/mapHandler.cpp:274-278 / :421-425: keep the windowed result unless both frames hold more than `kmin` features and
@@ -673,7 +667,7 @@ static MgbArgs mgb_args(const plf_params& P, MgGrid g, bool lines, int cap, int 
                         int count_stride) {
   MgbArgs a = {};
   a.g = g;
-  a.is_lines = lines ? 1 : 0; a.K = cap; a.best_lr = P.best_lr_matches ? 1 : 0;
+  a.is_lines = lines ? 1 : 0; a.K = a.Kt = cap; a.best_lr = P.best_lr_matches ? 1 : 0;
   a.nnr = lines ? P.min_ratio_12_l : P.min_ratio_12_p;
   a.line_sim_th = (double)P.line_sim_th;
   a.q_geo = q_geo; a.t_geo = t_geo; a.t_dir = t_dir;
@@ -727,9 +721,9 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     PLF_LAUNCH_CHECK(ctx);
     const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, P.matching_s_ws, 0, 0, 0};
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 2, s->mg_q[0], s->mg_t[0], nullptr, odesc, kcnt, s->m12,
-                                                        4 * (size_t)K, s->mcount, 4), B, K))) return st;
+                                                        4 * (size_t)K, s->mcount, 4), B, K, K, 9))) return st;
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 2, s->mg_q[1], s->mg_t[1], s->mg_dir[0], s->ldesc_raw, lcnt,
-                                                        s->m12 + K, 4 * (size_t)K, s->mcount + 1, 4), B, Ln))) return st;
+                                                        s->m12 + K, 4 * (size_t)K, s->mcount + 1, 4), B, Ln, Ln, 9))) return st;
     plf_mark(ctx, "stereo.k_mgb (matchGrid)");
   } else {
     // L->R 2-NN for every left feature; R->L only for the right features that are somebody's accepted best match
@@ -767,9 +761,9 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     const int ws = P.matching_f2f_ws;
     const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, ws, ws, ws, ws};
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 1, s->mg_q[2], s->mg_t[2], nullptr, s->fs.pdesc, s->fs.pt_count,
-                                                        s->m12g, 2 * (size_t)K, s->mgcount, 2), B, K))) return st;
+                                                        s->m12g, 2 * (size_t)K, s->mgcount, 2), B, K, K, 9))) return st;
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 1, s->mg_q[3], s->mg_t[3], s->mg_dir[1], s->fs.ldesc, s->fs.ls_count,
-                                                        s->m12g + K, 2 * (size_t)K, s->mgcount + 1, 2), B, Ln))) return st;
+                                                        s->m12g + K, 2 * (size_t)K, s->mgcount + 1, 2), B, Ln, Ln, 9))) return st;
     k_mg_select<<<dim3((K + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.pt_count, K, K, 0, P.min_pt_matches, s->m12);
     PLF_LAUNCH_CHECK(ctx);
     k_mg_select<<<dim3((Ln + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.ls_count, Ln, K, 1, P.min_ls_matches, s->m12);

@@ -121,11 +121,14 @@ struct MgGrid { int cols, rows, w_lo, w_hi, h_lo, h_hi; };
 struct MgbArgs {
   MgGrid g;
   int is_lines, K, best_lr;
+  int Kt;                // train capacity per problem (K: query capacity); D is K x Kt per problem
+  int clip;              // lines: walk only the part of a query's Bresenham line whose window can reach the grid (for
+                         // queries far outside it, e.g. pixel-unit projections); 0 walks every cell
   float nnr;
   double line_sim_th;
   const int* q_geo;      // [P][K][2|4]  query cells (points) / integer end points in grid units (lines)
-  const int* t_geo;      // [P][K][2|4]
-  const double* t_dir;   // [P][K][2] (lines) unit directions of the train lines
+  const int* t_geo;      // [P][Kt][2|4]
+  const double* t_dir;   // [P][Kt][2] (lines) unit directions of the train lines
   const uint8_t* d1; size_t d1_stride;   // descriptor rows of problem p: d1 + p * d1_stride
   const uint8_t* d2; size_t d2_stride;
   const int* n1; int n1_stride;          // counts: n1[p * n1_stride]
@@ -136,7 +139,8 @@ struct MgbArgs {
   int32_t* m12; size_t m12_stride;       // output rows of problem p: m12 + p * m12_stride
   int* count; int count_stride;          // matches of problem p (accumulated; zeroed by the caller)
 };
-plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n);
+// max_n1 / max_n2: upper bounds of the query / train counts; slot: the scratch slot D, the query masks and m21 live in.
+plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n1, int max_n2, int slot);
 
 // ---- LBD (lbd.cu) ------------------------------------------------------------------------------
 plf_status plf_launch_blur5_sobel(plf_ctx* ctx, const uint8_t* imgs, int pitch, size_t img_stride,

@@ -126,6 +126,33 @@ class plf_lc_result(C.Structure):
                 ("r", C.c_double), ("x_inc", C.c_double * 6), ("pose_inc", C.c_double * 6)]
 
 
+class plf_kf_match_opts(C.Structure):
+    _fields_ = [("fast_matching", C.c_int), ("max_kf_epip_p", C.c_double), ("max_kf_epip_l", C.c_double)]
+
+
+class plf_local_map(C.Structure):
+    _fields_ = [("n_pt", C.c_int), ("pt_X", C.c_void_p), ("pt_desc", C.c_void_p), ("pt_use", C.c_void_p),
+                ("n_ls", C.c_int), ("ls_X", C.c_void_p), ("ls_desc", C.c_void_p), ("ls_use", C.c_void_p)]
+
+
+# the plf_frame_view fields the keyframe matchers read: (name, dtype, columns)
+_KF_VIEW_FIELDS = (("pt_pl", np.float64, 2), ("pt_P", np.float64, 3), ("pdesc", np.uint8, 32), ("ls_spl", np.float64, 2),
+                   ("ls_epl", np.float64, 2), ("ls_sP", np.float64, 3), ("ls_eP", np.float64, 3), ("ls_le", np.float64, 3),
+                   ("ldesc", np.uint8, 32))
+
+
+def _frame_view(frame, keep):
+    """A plf_frame_view over the arrays of a get_frame dict (missing arrays stay NULL; `keep` holds the copies alive)."""
+    v = plf_frame_view()
+    v.n_pt, v.n_ls = len(frame.get("pdesc", ())), len(frame.get("ldesc", ()))
+    for name, dt, cols in _KF_VIEW_FIELDS:
+        if name in frame:
+            a = np.ascontiguousarray(frame[name], dt).reshape(-1, cols)
+            keep.append(a)
+            setattr(v, name, a.ctypes.data if a.size else None)
+    return v
+
+
 RESULT_DTYPE = np.dtype([("DT", np.float64, (4, 4)), ("DT_cov", np.float64, (6, 6)), ("err", np.float64),
                          ("status", np.int32), ("n_kp_l", np.int32), ("n_kp_r", np.int32), ("n_lines_l", np.int32),
                          ("n_lines_r", np.int32), ("n_stereo_pt", np.int32), ("n_stereo_ls", np.int32),
@@ -431,6 +458,57 @@ class Frontend:
         self._check(self.lib.plf_local_ba(self._ctx, C.byref(o), C.byref(p), C.byref(res)), "plf_local_ba")
         return dict(kf_pose=kf, pt=pt, ls=ls, pt_moved=pm[:len(pt)].astype(bool), ls_moved=lm[:len(ls)].astype(bool),
                     iters=res.iters, err=res.err, lambda_=res.lambda_)
+
+    def match_kf2kf(self, prev, curr, DT, fast_matching=True, max_kf_epip_p=1.0, max_kf_epip_l=1.0):
+        """MapHandler::matchKF2KFPoints / matchKF2KFLines, matching part (plf_match_kf2kf).  prev / curr: get_frame dicts;
+        DT: 4x4.  Returns dict(m_pt, n_pt, m_ls, n_ls): per previous-keyframe feature the current one or -1."""
+        keep = []
+        p, c = _frame_view(prev, keep), _frame_view(curr, keep)
+        T = np.ascontiguousarray(DT, np.float64).reshape(16)
+        o = plf_kf_match_opts(int(bool(fast_matching)), float(max_kf_epip_p), float(max_kf_epip_l))
+        m_pt, m_ls = np.full(max(p.n_pt, 1), -1, np.int32), np.full(max(p.n_ls, 1), -1, np.int32)
+        n_pt, n_ls = C.c_int(0), C.c_int(0)
+        self._check(self.lib.plf_match_kf2kf(self._ctx, C.byref(o), C.byref(p), C.byref(c), T.ctypes.data_as(C.c_void_p),
+                                             m_pt.ctypes.data_as(C.c_void_p), m_ls.ctypes.data_as(C.c_void_p), C.byref(n_pt),
+                                             C.byref(n_ls)), "plf_match_kf2kf")
+        return dict(m_pt=m_pt[:p.n_pt].copy(), n_pt=n_pt.value, m_ls=m_ls[:p.n_ls].copy(), n_ls=n_ls.value)
+
+    def match_map2kf(self, local_map, Twf, kf, kf_pt_lm=None, kf_ls_lm=None, fast_matching=True, max_kf_epip_p=1.0,
+                     max_kf_epip_l=1.0):
+        """MapHandler::matchMap2KFPoints / matchMap2KFLines (plf_match_map2kf).  local_map: dict pt_X [n,3], pt_desc,
+        optional pt_use, ls_X [n,6], ls_desc, optional ls_use; kf: get_frame dict; kf_*_lm: landmark index per keyframe
+        feature (-1 = unmatched) or None.  Returns dict(lm_pt, n_pt, lm_ls, n_ls)."""
+        keep = []
+        kv = _frame_view(kf, keep)
+        m = plf_local_map()
+
+        def arr(a, dt, cols):
+            a = np.ascontiguousarray(a, dt).reshape(-1, cols) if cols else np.ascontiguousarray(a, dt).ravel()
+            keep.append(a)
+            return a
+        for key, cols in (("pt", 3), ("ls", 6)):
+            X = arr(local_map.get(key + "_X", np.zeros((0, cols))), np.float64, cols)
+            d = arr(local_map.get(key + "_desc", np.zeros((0, 32))), np.uint8, 32)
+            u = local_map.get(key + "_use")
+            setattr(m, "n_" + key, len(X))
+            setattr(m, key + "_X", X.ctypes.data if X.size else None)
+            setattr(m, key + "_desc", d.ctypes.data if d.size else None)
+            if u is not None:
+                u = arr(np.asarray(u).astype(np.uint8), np.uint8, 0)
+                setattr(m, key + "_use", u.ctypes.data if u.size else None)
+        lms = [None if v is None else arr(v, np.int32, 0) for v in (kf_pt_lm, kf_ls_lm)]
+        for a, n, name in ((lms[0], kv.n_pt, "kf_pt_lm"), (lms[1], kv.n_ls, "kf_ls_lm")):
+            if a is not None and len(a) != n:
+                raise PlfError(f"match_map2kf: {name} has {len(a)} entries for {n} keyframe features")
+        T = np.ascontiguousarray(Twf, np.float64).reshape(16)
+        o = plf_kf_match_opts(int(bool(fast_matching)), float(max_kf_epip_p), float(max_kf_epip_l))
+        lm_pt, lm_ls = np.full(max(m.n_pt, 1), -1, np.int32), np.full(max(m.n_ls, 1), -1, np.int32)
+        n_pt, n_ls = C.c_int(0), C.c_int(0)
+        self._check(self.lib.plf_match_map2kf(self._ctx, C.byref(o), C.byref(m), T.ctypes.data_as(C.c_void_p), C.byref(kv),
+                                              *[C.c_void_p(a.ctypes.data if a is not None and a.size else None) for a in lms],
+                                              lm_pt.ctypes.data_as(C.c_void_p), lm_ls.ctypes.data_as(C.c_void_p),
+                                              C.byref(n_pt), C.byref(n_ls)), "plf_match_map2kf")
+        return dict(lm_pt=lm_pt[:m.n_pt].copy(), n_pt=n_pt.value, lm_ls=lm_ls[:m.n_ls].copy(), n_ls=n_ls.value)
 
     def expmap_se3(self, x):
         x = np.ascontiguousarray(x, np.float64).reshape(6)
