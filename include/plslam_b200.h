@@ -511,6 +511,63 @@ plf_status plf_match_map2kf(plf_ctx* ctx, const plf_kf_match_opts* opts, const p
                             const plf_frame_view* kf, const int32_t* kf_pt_lm, const int32_t* kf_ls_lm, int32_t* lm_pt,
                             int32_t* lm_ls, int* n_pt, int* n_ls);
 
+/* ------------------------------------------------------------------------------------------------
+ * Place recognition: DBoW2 bag-of-words vectors and L1 scores (SURVEY 8(f) f5)
+ * ---------------------------------------------------------------------------------------------- */
+
+/* A DBoW2 TemplatedVocabulary<FORB> as its YAML file lists it (3rdparty/DBoW2/include/DBoW2/TemplatedVocabulary.h:1437-1486):
+ * the nodes in FILE order (the root, id 0, is not listed; a parent's children keep file order, which decides ties in the
+ * descent), then the words.  Node ids must be 1..n_nodes.  Only scoring 0 (L1_NORM) and weighting 0 (TF_IDF), the types of
+ * pl-slam's vocabularies, are supported. */
+typedef struct plf_vocab {
+  int k, L, scoring, weighting;
+  int n_nodes;
+  int32_t* node_id;   /* [n_nodes] */
+  int32_t* parent_id; /* [n_nodes] */
+  double* weight;     /* [n_nodes] idf weight; a word of weight <= 0 drops the features that reach it (:1073) */
+  uint8_t* desc;      /* [n_nodes][32] */
+  int n_words;
+  int32_t* word_id;   /* [n_words] */
+  int32_t* word_node; /* [n_words] */
+} plf_vocab;
+
+/* Reads a vocabulary YAML file in the form TemplatedVocabulary::save writes and load reads (:1317-1486), e.g. the files of
+ * the reference's vocabulary/voc.tar.gz.  Host only (no device, no ctx); errors: plf_last_error(NULL).  PLF_ERR_INVALID for
+ * a malformed file: scoring other than L1 or weighting other than TF-IDF, k outside 1..32, duplicate or out-of-range node
+ * ids, a missing parent or a cycle, more than k children, a leaf without a word or a word on an inner node, duplicate or
+ * out-of-range word ids, a descriptor that is not 32 integers in 0..255.  On success the arrays are malloc'ed; release
+ * them with plf_vocab_free.  A plf_vocab may also be filled by the caller from its own arrays. */
+plf_status plf_vocab_read_yml(const char* path, plf_vocab* out);   /* numbers are read in the C locale */
+void plf_vocab_free(plf_vocab* v);
+
+/* Uploads the vocabulary of kind 0 (points, ORB) or 1 (lines, LBD), validated by the rules of plf_vocab_read_yml, and
+ * empties that kind's database.  The tree is stored re-laid out by parent (each node's children contiguous, in file order):
+ * 48 bytes per node. */
+plf_status plf_bow_set_vocabulary(plf_ctx* ctx, int kind, const plf_vocab* voc);
+
+/* Replaces the transform and scoring part of MapHandler::insertKFBowVectorP / L / PL (src/mapHandler.cpp:3007-3128) and the
+ * transform of MapHandler::initialize (:82-98): the BoW vectors of the keyframe's stereo descriptors, kf->pdesc [n_pt][32]
+ * and kf->ldesc [n_ls][32] (the rows of pdesc_l / ldesc_l), are computed with TemplatedVocabulary::transform (:1046-1101,
+ * :1198-1239), stored under kf_idx, and scored with L1Scoring::score (ScoringObject.cpp:23-68) against every keyframe
+ * stored before: score_p / score_l [kf_idx + 1] (either may be NULL), entry i = score(v_kf_idx, v_i), entry kf_idx the
+ * self-score, NaN for an index never inserted or erased.  Bit-exact to DBoW2 (sums in its order).  A kind disabled by
+ * has_points / has_lines is not touched (its row is left as it is) and needs no vocabulary; an enabled kind without one
+ * returns PLF_ERR_STATE.  kf_idx must exceed every index inserted into the kind before (gaps are absent keyframes) and be
+ * below 2^24; n_pt, n_ls <= 8192.  Other values return PLF_ERR_INVALID and change nothing.  One upload, kernels on
+ * plf_stream, one download.  Database, per kind: 12 bytes per stored (word, value) entry plus 8 bytes per keyframe index;
+ * it grows by reallocation (doubling) and never shrinks until the vocabulary is set again or plf_destroy.  At most 2^31 - 1
+ * entries per kind (PLF_ERR_CAPACITY beyond, nothing changed). */
+plf_status plf_bow_insert(plf_ctx* ctx, int kf_idx, const plf_frame_view* kf, double* score_p, double* score_l);
+
+/* The counterpart of removeRedundantKFs deleting a keyframe (src/mapHandler.cpp:2931-2932): later rows report NaN for it.
+ * Erasing an absent index is a no-op; kf_idx < 0 returns PLF_ERR_INVALID. */
+plf_status plf_bow_erase(plf_ctx* ctx, int kf_idx);
+
+/* The stored BowVector (KeyFrame::descDBoW_P / descDBoW_L) of keyframe kf_idx, kind 0 / 1, in ascending word order: *n
+ * entries.  words / values may be NULL to query *n; PLF_ERR_CAPACITY if *n > cap.  An absent keyframe or a kind never
+ * inserted returns PLF_ERR_INVALID. */
+plf_status plf_bow_get(plf_ctx* ctx, int kf_idx, int kind, int cap, uint32_t* words, double* values, int* n);
+
 /* Debug: device-clock timeline (ms) of the two most recent batches of the software pipeline: for each, the start/end of
  * the E (extract), G (region growing) and M (match/track/pose) phases relative to the older batch's E start.
  * No reference counterpart (the reference times whole calls with its Timer, app/plslam_dataset.cpp:126-132). */

@@ -237,6 +237,8 @@ struct DescMat {
   int rows = 0;
   static constexpr int cols = PLF_DESC_BYTES;
   const uint8_t* row(int i) const { return data.data() + (size_t)i * cols; }
+  // cv::Mat::ptr<uchar>(i): the same expression then reads both the shim's block and a continuous CV_8U cv::Mat
+  template <typename T> const T* ptr(int i = 0) const { return reinterpret_cast<const T*>(row(i)); }
 };
 
 // stvo-pl StereoFrame: the fields KeyFrame deep-copies (src/keyFrame.cpp:39-53)

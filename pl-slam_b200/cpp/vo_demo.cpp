@@ -1,9 +1,12 @@
 // vo_demo — the VO part of the reference's frame loop (app/plslam_dataset.cpp:111-163) on top of the C++ shim.
-// Usage: vo_demo <frames.bin> [orb_nfeatures lsd_nfeatures] [--grid-selftest | --kf-match-selftest]
+// Usage: vo_demo <frames.bin> [orb_nfeatures lsd_nfeatures] [--grid-selftest | --kf-match-selftest |
+//                                                            --bow-selftest <voc_p.yml> <voc_l.yml>]
 // frames.bin: int32 n, w, h; double fx, fy, cx, cy, b; then n x (left h*w bytes, right h*w bytes).
 // Prints one line per frame: idx status n_stereo_pt n_stereo_ls n_inliers newKF Tfw(16 values, row-major).
 #include <cstdio>
 #include <cstdlib>
+#include <stdexcept>
+#include <string>
 #include <vector>
 
 #include "stvo_shim.h"
@@ -154,8 +157,111 @@ static int kf_match_selftest(plf_ctx* ctx, KfArrays& prev_kf, KfArrays& curr_kf)
   return 0;
 }
 
+// ---- INTEGRATION.md §4 f5: DBoW2 place recognition (the text between the two markers is the snippet shown there) ----
+// What MapHandler's BoW code reads: KeyFrame::kf_idx and KeyFrame::stereo_frame (include/keyFrame.h), the map_keyframes
+// list (NULL once removeRedundantKFs deleted a keyframe) and conf_matrix (include/mapHandler.h:147).
+struct KeyFrame {
+  int kf_idx;
+  StVO::StereoFrame* stereo_frame;
+};
+struct BowMap {
+  plf_ctx* ctx;
+  bool has_points, has_lines;   // SlamConfig::hasPoints() / hasLines()
+  std::vector<KeyFrame*> map_keyframes;
+  std::vector<std::vector<float>> conf_matrix;
+};
+// BEGIN f5
+static void plf_check(plf_ctx* ctx, plf_status st, const char* what) {
+  if (st != PLF_OK) throw std::runtime_error(std::string(what) + ": " + plf_last_error(ctx));
+}
+
+// MapHandler construction, where dbow_voc_p / dbow_voc_l are loaded (kind 0 = points, 1 = lines)
+static void bow_load_vocabulary(plf_ctx* ctx, int kind, const char* path) {
+  plf_vocab v;
+  plf_check(nullptr, plf_vocab_read_yml(path, &v), "plf_vocab_read_yml");
+  const plf_status st = plf_bow_set_vocabulary(ctx, kind, &v);
+  plf_vocab_free(&v);
+  plf_check(ctx, st, "plf_bow_set_vocabulary");
+}
+
+// initialize (:82-98, the transform) and insertKFBowVectorP / L / PL (:3007-3128, the transform and the score rows):
+// one call.  score_p / score_l come back with kf->kf_idx + 1 entries, NaN where map_keyframes[i] is absent or erased.
+static void bow_insert(BowMap& m, KeyFrame* kf, std::vector<double>& score_p, std::vector<double>& score_l) {
+  const StVO::StereoFrame* sf = kf->stereo_frame;
+  plf_frame_view v = {};                                   // the rows of pdesc_l / ldesc_l
+  v.n_pt = sf->pdesc_l.rows; v.pdesc = const_cast<uint8_t*>(sf->pdesc_l.ptr<uint8_t>());
+  v.n_ls = sf->ldesc_l.rows; v.ldesc = const_cast<uint8_t*>(sf->ldesc_l.ptr<uint8_t>());
+  score_p.assign(kf->kf_idx + 1, 0.0);
+  score_l.assign(kf->kf_idx + 1, 0.0);
+  plf_check(m.ctx, plf_bow_insert(m.ctx, kf->kf_idx, &v, m.has_points ? score_p.data() : nullptr,
+                                  m.has_lines ? score_l.data() : nullptr), "plf_bow_insert");
+}
+
+// insertKFBowVectorP (:3018-3029); insertKFBowVectorL is the same on score_l.  insertKFBowVectorPL keeps its loop
+// (:3070-3127, it reads stvo-pl's vector_stdv) with score_p[i] / score_l[i] in place of the two score() calls.
+static void bow_fill_conf_matrix_p(BowMap& m, const KeyFrame* kf, const std::vector<double>& score_p) {
+  const int idx = kf->kf_idx;
+  for (int i = 0; i < idx; i++) {
+    if (m.map_keyframes[i] != NULL) {
+      m.conf_matrix[idx][i] = score_p[i];
+      m.conf_matrix[i][idx] = score_p[i];
+    }
+  }
+  m.conf_matrix[idx][idx] = score_p[idx];
+}
+
+// removeRedundantKFs (:2931-2932), next to `delete map_keyframes[kf_idx]; map_keyframes[kf_idx] = nullptr;`
+static void bow_erase(BowMap& m, int kf_idx) { plf_check(m.ctx, plf_bow_erase(m.ctx, kf_idx), "plf_bow_erase"); }
+// END f5
+
+static void print_doubles(const char* name, int k, const std::vector<double>& v) {
+  std::printf("bow %s %d", name, k);
+  for (double x : v) std::printf(" %.17g", x);
+  std::printf("\n");
+}
+
+// `vo_demo frames.bin ... --bow-selftest voc_p.yml voc_l.yml`: every frame becomes keyframe kf_idx = frame index through
+// the f5 functions above; keyframe 1 is erased after keyframe 2 is inserted.  Prints each keyframe's two score rows, its
+// conf_matrix row, and its two stored BowVectors, which the Python binding must reproduce.
+static void bow_selftest_frame(BowMap& m, StVO::StereoFrame* cur, int frame_counter) {
+  KeyFrame* kf = new KeyFrame{frame_counter, cur};
+  m.map_keyframes.push_back(kf);
+  for (auto& row : m.conf_matrix) row.resize(m.map_keyframes.size(), 0.f);
+  m.conf_matrix.emplace_back(m.map_keyframes.size(), 0.f);
+  std::vector<double> sp, sl;
+  bow_insert(m, kf, sp, sl);
+  bow_fill_conf_matrix_p(m, kf, sp);
+  print_doubles("score_p", kf->kf_idx, sp);
+  print_doubles("score_l", kf->kf_idx, sl);
+  std::vector<double> conf(m.conf_matrix[kf->kf_idx].begin(), m.conf_matrix[kf->kf_idx].end());
+  print_doubles("conf", kf->kf_idx, conf);
+  for (int kind = 0; kind < 2; ++kind) {
+    int n = 0;
+    plf_check(m.ctx, plf_bow_get(m.ctx, kf->kf_idx, kind, 0, nullptr, nullptr, &n), "plf_bow_get");
+    std::vector<uint32_t> w(n);
+    std::vector<double> x(n);
+    plf_check(m.ctx, plf_bow_get(m.ctx, kf->kf_idx, kind, n, w.data(), x.data(), &n), "plf_bow_get");
+    std::printf("bow words%d %d", kind, kf->kf_idx);
+    for (uint32_t v : w) std::printf(" %u", v);
+    std::printf("\n");
+    print_doubles(kind ? "vals1" : "vals0", kf->kf_idx, x);
+  }
+  kf->stereo_frame = nullptr;   // the frame is the handler's; only the index stays
+  if (frame_counter == 2) {
+    bow_erase(m, 1);
+    delete m.map_keyframes[1];
+    m.map_keyframes[1] = nullptr;
+  }
+}
+
 int main(int argc, char** argv) {
   bool grid_test = false, kf_test = false;
+  const char* bow_voc[2] = {nullptr, nullptr};
+  if (argc >= 4 && std::string(argv[argc - 3]) == "--bow-selftest") {
+    bow_voc[0] = argv[argc - 2];
+    bow_voc[1] = argv[argc - 1];
+    argc -= 3;
+  }
   if (argc >= 2 && std::string(argv[argc - 1]) == "--grid-selftest") { grid_test = true; --argc; }
   if (argc >= 2 && std::string(argv[argc - 1]) == "--kf-match-selftest") { kf_test = true; --argc; }
   if (argc < 2) {
@@ -176,6 +282,11 @@ int main(int argc, char** argv) {
     if (argc >= 4) { prm.orb_nfeatures = std::atoi(argv[2]); prm.lsd_nfeatures = std::atoi(argv[3]); }
     StVO::StereoFrameHandler* StVO_ = new StVO::StereoFrameHandler(&cam_pin, &prm);   // app:109
     KfArrays* first_kf = nullptr;   // --kf-match-selftest: frame 0 against the last frame
+    BowMap bow = {StVO_->ctx(), prm.has_points != 0, prm.has_lines != 0, {}, {}};
+    if (bow_voc[0]) {
+      bow_load_vocabulary(bow.ctx, 0, bow_voc[0]);
+      bow_load_vocabulary(bow.ctx, 1, bow_voc[1]);
+    }
     int rc = 0;
     for (int frame_counter = 0; frame_counter < n; ++frame_counter) {                   // app:111
       if (std::fread(buf.data(), 1, buf.size(), f) != buf.size()) { std::fprintf(stderr, "short read\n"); return 1; }
@@ -200,6 +311,7 @@ int main(int argc, char** argv) {
                   StVO_->n_inliers, new_kf ? 1 : 0);
       for (int i = 0; i < 16; ++i) std::printf(" %.17g", cur->Tfw.v[i]);
       std::printf("\n");
+      if (bow_voc[0]) bow_selftest_frame(bow, cur, frame_counter);
       if (kf_test && frame_counter == 0) first_kf = new KfArrays(cur);
       if (kf_test && frame_counter == n - 1 && first_kf) {
         KfArrays last_kf(cur);
@@ -208,6 +320,7 @@ int main(int argc, char** argv) {
       if (frame_counter > 0) StVO_->updateFrame();                                      // app:159
     }
     delete first_kf;
+    for (KeyFrame* kf : bow.map_keyframes) delete kf;
     delete StVO_;
     if (rc) return rc;
   } catch (const std::exception& e) {

@@ -1,0 +1,814 @@
+// Place recognition (SURVEY 8(f) f5): DBoW2 bag-of-words vectors of keyframes and their L1 scores against every earlier
+// keyframe, bit-exact to 3rdparty/DBoW2 (TemplatedVocabulary<FORB>, TF-IDF weighting, L1 scoring).
+//
+// Host: plf_vocab_read_yml (the YAML form TemplatedVocabulary::save writes, TemplatedVocabulary.h:1340-1432, read in load's
+// order :1437-1486), the vocabulary checks, the re-layout of the tree by parent, the database bookkeeping.
+// Kernels, all on plf_stream, one upload and one download per plf_bow_insert:
+//   k_bow_transform  one warp per feature, one lane per child: the descent of transform() (:1198-1239);
+//   k_bow_assemble   one block per kind: the (word, feature) pairs sorted by word (stable in feature order), addWeight in
+//                    feature order (BowVector.cpp:34-46), the sequential L1 norm in ascending word order (:62-84), the
+//                    division, the append to the kind's database;
+//   k_bow_score      one warp per earlier keyframe: L1Scoring::score (ScoringObject.cpp:23-68), the common words' terms
+//                    summed sequentially in ascending word order.
+#include <errno.h>
+#include <locale.h>
+#include <math.h>
+
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+
+#include "plf_internal.h"
+
+#define BOW_MAX_FEATURES 8192   // per kind, as keyframe matching
+#define BOW_MAX_KF (1 << 24)    // keyframe indices (rows are kf_idx + 1 doubles)
+#define BOW_SORT_THREADS 1024
+
+// ------------------------------------------------------------------------------------------------------------------
+// Device state
+// ------------------------------------------------------------------------------------------------------------------
+
+struct BowKind {
+  // vocabulary (48 bytes per node)
+  bool has_voc = false;
+  int root_n = 0;
+  uint4* desc = nullptr;     // [n][2]
+  int2* meta = nullptr;      // [n]
+  double* weight = nullptr;  // [n]
+  // database: 12 bytes per stored entry + 8 per keyframe index
+  uint32_t* words = nullptr;
+  double* vals = nullptr;
+  size_t cap = 0, end = 0;
+  int2* ent = nullptr;       // [ent_cap] (offset, nnz); nnz < 0: absent or erased
+  int ent_cap = 0;
+  std::vector<int2> host_ent;
+  int last = -1;             // largest index inserted since the vocabulary was set
+};
+
+struct BowState {
+  BowKind kind[2];
+  uint8_t* io = nullptr;     // per-call upload / work / download region
+  size_t io_bytes = 0;
+  int n_sm = 0;
+  bool attr_set = false;
+};
+
+namespace {
+
+// ------------------------------------------------------------------------------------------------------------------
+// Vocabulary checks and layout (host)
+// ------------------------------------------------------------------------------------------------------------------
+
+// The tree re-laid out by parent: slot s holds a node; the root's children are slots [0, root_n), every inner node's
+// children are contiguous, in file order.  meta[s] = (first child slot, child count) for an inner node, (-1 - word, 0) for
+// a leaf.
+struct VocabLayout {
+  int root_n = 0;
+  std::vector<uint8_t> desc;   // [n][32]
+  std::vector<int2> meta;
+  std::vector<double> weight;
+};
+
+// Validates `v` (the rules documented at plf_vocab_read_yml) and, if `lay` is given, builds the layout.  Returns an empty
+// string when valid, else the reason.
+std::string vocab_check(const plf_vocab* v, VocabLayout* lay) {
+  char buf[256];
+  if (v->scoring != 0 || v->weighting != 0) {
+    snprintf(buf, sizeof buf, "scoring %d / weighting %d: only L1_NORM (0) / TF_IDF (0) are supported", v->scoring, v->weighting);
+    return buf;
+  }
+  if (v->k < 1 || v->k > 32) return "k = " + std::to_string(v->k) + " (must be in 1..32)";
+  const int n = v->n_nodes, nw = v->n_words;
+  if (n < 1 || nw < 1) return "the vocabulary has no nodes or no words";
+  if (!v->node_id || !v->parent_id || !v->weight || !v->desc || !v->word_id || !v->word_node) return "an array is NULL";
+  std::vector<int> pos(n + 1, -1);     // node id -> file index
+  std::vector<int> nchild(n + 1, 0);
+  for (int i = 0; i < n; ++i) {
+    const int id = v->node_id[i], p = v->parent_id[i];
+    if (id < 1 || id > n) return "node id " + std::to_string(id) + " out of range 1.." + std::to_string(n);
+    if (pos[id] >= 0) return "duplicate node id " + std::to_string(id);
+    pos[id] = i;
+    if (p < 0 || p > n) return "node " + std::to_string(id) + ": parent " + std::to_string(p) + " does not exist";
+    if (++nchild[p] > v->k) return "node " + std::to_string(p) + " has more than k = " + std::to_string(v->k) + " children";
+  }
+  if (nchild[0] == 0) return "the root has no children";
+  std::vector<int> word_of(n + 1, -1), seen(nw, 0);
+  for (int j = 0; j < nw; ++j) {
+    const int w = v->word_id[j], nd = v->word_node[j];
+    if (w < 0 || w >= nw) return "word id " + std::to_string(w) + " out of range 0.." + std::to_string(nw - 1);
+    if (seen[w]++) return "duplicate word id " + std::to_string(w);
+    if (nd < 1 || nd > n) return "word " + std::to_string(w) + ": node " + std::to_string(nd) + " does not exist";
+    if (nchild[nd] > 0) return "word " + std::to_string(w) + " lies on inner node " + std::to_string(nd);
+    if (word_of[nd] >= 0) return "node " + std::to_string(nd) + " carries two words";
+    word_of[nd] = w;
+  }
+  for (int id = 1; id <= n; ++id)
+    if (nchild[id] == 0 && word_of[id] < 0) return "leaf " + std::to_string(id) + " has no word";
+  // children lists in file order (load push_backs them in file order, :1468): counting sort by parent, stable
+  std::vector<int> cstart(n + 2, 0);
+  for (int p = 0; p <= n; ++p) cstart[p + 1] = cstart[p] + nchild[p];
+  std::vector<int> child(n), fill(cstart.begin(), cstart.end() - 1);
+  for (int i = 0; i < n; ++i) child[fill[v->parent_id[i]]++] = v->node_id[i];
+  // breadth-first from the root: every node is reached unless it lies on a cycle
+  std::vector<int> order;   // slot -> node id
+  order.reserve(n);
+  for (int c = cstart[0]; c < cstart[1]; ++c) order.push_back(child[c]);
+  for (size_t s = 0; s < order.size(); ++s) {
+    const int id = order[s];
+    for (int c = cstart[id]; c < cstart[id + 1]; ++c) order.push_back(child[c]);
+  }
+  if ((int)order.size() != n) return "a parent chain does not reach the root (cycle)";
+  if (!lay) return "";
+  lay->root_n = nchild[0];
+  lay->desc.resize((size_t)n * 32);
+  lay->meta.resize(n);
+  lay->weight.resize(n);
+  int next = nchild[0];
+  for (int s = 0; s < n; ++s) {
+    const int id = order[s], i = pos[id];
+    memcpy(&lay->desc[(size_t)s * 32], v->desc + (size_t)i * 32, 32);
+    lay->weight[s] = v->weight[i];
+    if (nchild[id] > 0) {
+      lay->meta[s] = make_int2(next, nchild[id]);
+      next += nchild[id];
+    } else {
+      lay->meta[s] = make_int2(-1 - word_of[id], 0);
+    }
+  }
+  return "";
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// YAML reader: the subset cv::FileStorage writes for TemplatedVocabulary::save (top-level map "vocabulary" with scalar
+// keys, then the block sequences "nodes" and "words" of flow maps).
+// ------------------------------------------------------------------------------------------------------------------
+
+struct Parser {
+  const char* p;
+  const char* e;
+  std::string err;
+  void ws() { while (p < e && (*p == ' ' || *p == '\t' || *p == '\r' || *p == '\n')) ++p; }
+};
+
+bool parse_int(const std::string& s, long* out) {
+  if (s.empty()) return false;
+  char* end = nullptr;
+  errno = 0;
+  const long x = strtol(s.c_str(), &end, 10);
+  if (errno || *end) return false;
+  *out = x;
+  return true;
+}
+
+// One flow map "{ key:value, key:"string", ... }" at p; keys and raw values (quotes removed) in order.
+bool parse_flow_map(Parser& ps, std::vector<std::pair<std::string, std::string>>& kv) {
+  kv.clear();
+  ps.ws();
+  if (ps.p >= ps.e || *ps.p != '{') return false;
+  ++ps.p;
+  for (;;) {
+    ps.ws();
+    if (ps.p < ps.e && *ps.p == '}') { ++ps.p; return true; }
+    const char* k0 = ps.p;
+    while (ps.p < ps.e && *ps.p != ':' && *ps.p != '}' && *ps.p != '\n') ++ps.p;
+    if (ps.p >= ps.e || *ps.p != ':') return false;
+    std::string key(k0, ps.p);
+    while (!key.empty() && key.back() == ' ') key.pop_back();
+    ++ps.p;
+    ps.ws();
+    std::string val;
+    if (ps.p < ps.e && *ps.p == '"') {
+      const char* v0 = ++ps.p;
+      while (ps.p < ps.e && *ps.p != '"') ++ps.p;
+      if (ps.p >= ps.e) return false;
+      val.assign(v0, ps.p++);
+    } else {
+      const char* v0 = ps.p;
+      while (ps.p < ps.e && *ps.p != ',' && *ps.p != '}' && *ps.p != ' ' && *ps.p != '\n' && *ps.p != '\r') ++ps.p;
+      val.assign(v0, ps.p);
+    }
+    kv.emplace_back(key, val);
+    ps.ws();
+    if (ps.p < ps.e && *ps.p == ',') ++ps.p;
+  }
+}
+
+const std::string* find_key(const std::vector<std::pair<std::string, std::string>>& kv, const char* key) {
+  for (const auto& x : kv)
+    if (x.first == key) return &x.second;
+  return nullptr;
+}
+
+// The entries of a block sequence "- { ... }" (or "[]") up to `end`.
+template <typename F>
+bool parse_seq(Parser& ps, const char* end, const char* what, F&& each) {
+  std::vector<std::pair<std::string, std::string>> kv;
+  ps.ws();
+  if (ps.p < end && *ps.p == '[') {   // an empty sequence is written "[]"
+    ++ps.p;
+    ps.ws();
+    if (ps.p < end && *ps.p == ']') { ++ps.p; return true; }
+    ps.err = std::string(what) + ": flow sequences are not supported";
+    return false;
+  }
+  size_t i = 0;
+  for (;; ++i) {
+    ps.ws();
+    if (ps.p >= end) return true;
+    if (*ps.p != '-') { ps.err = std::string(what) + ": expected '-' at entry " + std::to_string(i); return false; }
+    ++ps.p;
+    if (!parse_flow_map(ps, kv)) { ps.err = std::string(what) + ": malformed entry " + std::to_string(i); return false; }
+    std::string why = each(kv);
+    if (!why.empty()) { ps.err = std::string(what) + " entry " + std::to_string(i) + ": " + why; return false; }
+  }
+}
+
+std::string parse_vocab(Parser& ps, std::vector<int32_t>& nid, std::vector<int32_t>& pid, std::vector<double>& wt,
+                        std::vector<uint8_t>& desc, std::vector<int32_t>& wid, std::vector<int32_t>& wnode, int hdr[4]) {
+  const std::string text(ps.p, ps.e - ps.p);   // only for the section searches
+  const size_t nodes_at = text.find("nodes:");
+  const size_t words_at = text.find("words:", nodes_at == std::string::npos ? 0 : nodes_at);
+  if (text.compare(0, 5, "%YAML") != 0) return "not a YAML file (no %YAML header)";
+  if (nodes_at == std::string::npos || words_at == std::string::npos) return "no nodes / words sequence";
+  // header: the scalar keys of the "vocabulary" map, one per line
+  static const char* keys[4] = {"k", "L", "scoringType", "weightingType"};
+  bool have[4] = {false, false, false, false};
+  bool in_voc = false;
+  size_t line = 0;
+  while (line < nodes_at) {
+    size_t eol = text.find('\n', line);
+    if (eol == std::string::npos || eol > nodes_at) eol = nodes_at;
+    std::string l = text.substr(line, eol - line);
+    line = eol + 1;
+    const size_t a = l.find_first_not_of(" \t\r");
+    if (a == std::string::npos || l[a] == '%' || l.compare(a, 3, "---") == 0) continue;
+    const size_t c = l.find(':', a);
+    if (c == std::string::npos) return "header line without ':': " + l;
+    std::string key = l.substr(a, c - a), val = l.substr(c + 1);
+    while (!val.empty() && (val.back() == ' ' || val.back() == '\r')) val.pop_back();
+    val.erase(0, val.find_first_not_of(' ') == std::string::npos ? val.size() : val.find_first_not_of(' '));
+    if (key == "vocabulary" && val.empty()) { in_voc = true; continue; }
+    int ki = -1;
+    for (int q = 0; q < 4; ++q)
+      if (key == keys[q]) ki = q;
+    if (ki < 0 || !in_voc) return "unexpected header key " + key;
+    long x;
+    if (!parse_int(val, &x) || x < INT32_MIN || x > INT32_MAX) return "header key " + key + ": not an integer: " + val;
+    hdr[ki] = (int)x;
+    have[ki] = true;
+  }
+  for (int q = 0; q < 4; ++q)
+    if (!have[q]) return std::string("header key ") + keys[q] + " missing";
+  const char* base = ps.p;
+  ps.p = base + nodes_at + 6;
+  if (!parse_seq(ps, base + words_at, "nodes", [&](const std::vector<std::pair<std::string, std::string>>& kv) -> std::string {
+        const std::string *s_id = find_key(kv, "nodeId"), *s_p = find_key(kv, "parentId"), *s_w = find_key(kv, "weight"),
+                          *s_d = find_key(kv, "descriptor");
+        if (!s_id || !s_p || !s_w || !s_d || kv.size() != 4) return "needs exactly nodeId, parentId, weight, descriptor";
+        long a, b;
+        if (!parse_int(*s_id, &a) || !parse_int(*s_p, &b) || a < INT32_MIN || a > INT32_MAX || b < INT32_MIN || b > INT32_MAX)
+          return "nodeId / parentId is not an integer";
+        char* end = nullptr;
+        // in the C locale whatever LC_NUMERIC the host application set: the file's decimal separator is '.'
+        static const locale_t c_locale = newlocale(LC_ALL_MASK, "C", (locale_t)0);
+        const double w = strtod_l(s_w->c_str(), &end, c_locale);
+        if (s_w->empty() || *end) return "weight is not a number: " + *s_w;
+        const char* q = s_d->c_str();
+        uint8_t d[32];
+        int cnt = 0;
+        for (;;) {
+          while (*q == ' ') ++q;
+          if (!*q) break;
+          long x = strtol(q, &end, 10);
+          if (end == q || (*end && *end != ' ') || x < 0 || x > 255 || cnt == 32)
+            return "descriptor is not 32 integers in 0..255";
+          d[cnt++] = (uint8_t)x;
+          q = end;
+        }
+        if (cnt != 32) return "descriptor is not 32 integers in 0..255";
+        nid.push_back((int32_t)a);
+        pid.push_back((int32_t)b);
+        wt.push_back(w);
+        desc.insert(desc.end(), d, d + 32);
+        return "";
+      }))
+    return ps.err;
+  ps.p = base + words_at + 6;
+  if (!parse_seq(ps, ps.e, "words", [&](const std::vector<std::pair<std::string, std::string>>& kv) -> std::string {
+        const std::string *s_w = find_key(kv, "wordId"), *s_n = find_key(kv, "nodeId");
+        long a, b;
+        if (!s_w || !s_n || kv.size() != 2) return "needs exactly wordId, nodeId";
+        if (!parse_int(*s_w, &a) || !parse_int(*s_n, &b) || a < INT32_MIN || a > INT32_MAX || b < INT32_MIN || b > INT32_MAX)
+          return "wordId / nodeId is not an integer";
+        wid.push_back((int32_t)a);
+        wnode.push_back((int32_t)b);
+        return "";
+      }))
+    return ps.err;
+  return "";
+}
+
+template <typename T>
+T* dup_array(const std::vector<T>& v) {
+  T* p = (T*)malloc(v.size() * sizeof(T) + 1);
+  if (p && !v.empty()) memcpy(p, v.data(), v.size() * sizeof(T));
+  return p;
+}
+
+void free_db(BowKind& k) {
+  cudaFree(k.words);
+  cudaFree(k.vals);
+  cudaFree(k.ent);
+  k.words = nullptr;
+  k.vals = nullptr;
+  k.ent = nullptr;
+  k.cap = k.end = 0;
+  k.ent_cap = 0;
+  k.host_ent.clear();
+  k.last = -1;
+}
+
+void free_kind(BowKind& k) {
+  cudaFree(k.desc);
+  cudaFree(k.meta);
+  cudaFree(k.weight);
+  k.desc = nullptr;
+  k.meta = nullptr;
+  k.weight = nullptr;
+  k.has_voc = false;
+  free_db(k);
+}
+
+BowState* bow_state(plf_ctx* ctx) {
+  if (!ctx->bow) {
+    ctx->bow = new BowState();
+    cudaDeviceGetAttribute(&ctx->bow->n_sm, cudaDevAttrMultiProcessorCount, ctx->device);
+    if (ctx->bow->n_sm <= 0) ctx->bow->n_sm = 132;
+  }
+  return ctx->bow;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Kernels
+// ------------------------------------------------------------------------------------------------------------------
+
+struct TreeView {
+  const uint4* desc;
+  const int2* meta;
+  const double* weight;
+  int root_n;
+};
+
+// TemplatedVocabulary::transform(feature, word_id, weight) (:1198-1239).  Features [0, n0) are kind 0, [n0, n0 + n1) kind
+// 1.  The child distance is FORB::distance (an integer Hamming count, returned as double), so the strict `d < best_d` of
+// :1224 picks the first minimum in child order: the lane minimum of (d << 5 | lane).  word[f] = -1 where the weight is not
+// > 0 (:1073: the feature is dropped).
+__global__ void __launch_bounds__(256) k_bow_transform(TreeView t0, TreeView t1, const uint4* __restrict__ feat, int n0,
+                                                       int n1, int* __restrict__ word, double* __restrict__ wt) {
+  const int f = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (f >= n0 + n1) return;
+  const TreeView t = f < n0 ? t0 : t1;
+  const uint4 a = feat[2 * f], b = feat[2 * f + 1];
+  int base = 0, cnt = t.root_n;
+  for (;;) {
+    unsigned key = 0xFFFFFFFFu;
+    if (lane < cnt) {
+      const uint4 c = __ldg(&t.desc[2 * (base + lane)]), e = __ldg(&t.desc[2 * (base + lane) + 1]);
+      const int d = __popc(a.x ^ c.x) + __popc(a.y ^ c.y) + __popc(a.z ^ c.z) + __popc(a.w ^ c.w) + __popc(b.x ^ e.x) +
+                    __popc(b.y ^ e.y) + __popc(b.z ^ e.z) + __popc(b.w ^ e.w);
+      key = ((unsigned)d << 5) | (unsigned)lane;
+    }
+    key = __reduce_min_sync(0xFFFFFFFFu, key);
+    const int s = base + (int)(key & 31u);
+    const int2 m = __ldg(&t.meta[s]);
+    if (m.y == 0) {
+      if (lane == 0) {
+        const double w = __ldg(&t.weight[s]);
+        word[f] = w > 0 ? -1 - m.x : -1;
+        wt[f] = w;
+      }
+      return;
+    }
+    base = m.x;
+    cnt = m.y;
+  }
+}
+
+struct AssembleKind {
+  int active, n, feat0;      // features [feat0, feat0 + n) of word / wt
+  uint32_t* words;           // the kind's database, entries appended at `end`
+  double* vals;
+  int2* ent;
+  long long end;
+};
+
+// TemplatedVocabulary::transform(features, v) for TF-IDF with L1 mustNormalize (:1046-1101): one block per kind.
+__global__ void __launch_bounds__(BOW_SORT_THREADS) k_bow_assemble(AssembleKind k0, AssembleKind k1, const int* __restrict__ word,
+                                                                   const double* __restrict__ wt, int kf_idx, int* __restrict__ nnz_out) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem);           // [8192]
+  double* sv = reinterpret_cast<double*>(smem + BOW_MAX_FEATURES * 8);               // [8192]
+  __shared__ int s_scan[BOW_SORT_THREADS / 32];
+  __shared__ double s_norm;
+  const AssembleKind K = blockIdx.x ? k1 : k0;
+  if (!K.active) return;
+  const int tid = threadIdx.x, n = K.n;
+  int N = 1;
+  while (N < n) N <<= 1;
+  // (word, feature) keys; dropped features sort last
+  for (int i = tid; i < N; i += blockDim.x) {
+    unsigned long long key = ~0ull;
+    if (i < n) {
+      const int w = word[K.feat0 + i];
+      if (w >= 0) key = ((unsigned long long)w << 13) | (unsigned)i;
+    }
+    keys[i] = key;
+  }
+  __syncthreads();
+  // bitonic sort, ascending: (word, feature) is unique, so the order is the stable one
+  for (int k = 2; k <= N; k <<= 1)
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = tid; i < N; i += blockDim.x) {
+        const int ixj = i ^ j;
+        if (ixj > i) {
+          const unsigned long long a = keys[i], b = keys[ixj];
+          if ((a > b) == ((i & k) == 0)) { keys[i] = b; keys[ixj] = a; }
+        }
+      }
+      __syncthreads();
+    }
+  // m valid pairs; a run of equal words is one BowVector entry
+  int m = 0;
+  for (int c = 0; c < N; c += blockDim.x) m += __syncthreads_count(c + tid < N && keys[c + tid] != ~0ull);
+  const int per = (m + blockDim.x - 1) / blockDim.x, i0 = min(tid * per, m), i1 = min(i0 + per, m);
+  auto head = [&](int i) { return i == 0 || (keys[i] >> 13) != (keys[i - 1] >> 13); };
+  int cnt = 0;
+  for (int i = i0; i < i1; ++i) cnt += head(i);
+  // exclusive block scan of the head counts
+  const int lane = tid & 31, wid = tid >> 5;
+  int incl = cnt;
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+    if (lane >= o) incl += y;
+  }
+  if (lane == 31) s_scan[wid] = incl;
+  __syncthreads();
+  if (wid == 0) {
+    int x = lane < (int)(blockDim.x >> 5) ? s_scan[lane] : 0;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xFFFFFFFFu, x, o);
+      if (lane >= o) x += y;
+    }
+    if (lane < (int)(blockDim.x >> 5)) s_scan[lane] = x;
+  }
+  __syncthreads();
+  int j = incl - cnt + (wid ? s_scan[wid - 1] : 0);
+  const int nnz = s_scan[(blockDim.x >> 5) - 1];
+  // addWeight (BowVector.cpp:34-46): the first feature inserts its weight, each later one adds to it, in feature order
+  for (int i = i0; i < i1; ++i) {
+    if (!head(i)) continue;
+    const unsigned long long w = keys[i] >> 13;
+    double v = wt[K.feat0 + (int)(keys[i] & 8191u)];
+    for (int t = i + 1; t < m && (keys[t] >> 13) == w; ++t) v += wt[K.feat0 + (int)(keys[t] & 8191u)];
+    K.words[K.end + j] = (uint32_t)w;
+    sv[j++] = v;
+  }
+  __syncthreads();
+  // BowVector::normalize(L1) (:62-84): norm = sum |v| in ascending word order, sequentially; divide when > 0
+  if (tid == 0) {
+    double norm = 0.0;
+    for (int i = 0; i < nnz; ++i) norm += fabs(sv[i]);
+    s_norm = norm;
+    K.ent[kf_idx] = make_int2((int)K.end, nnz);
+    nnz_out[blockIdx.x] = nnz;
+  }
+  __syncthreads();
+  const double norm = s_norm;
+  for (int i = tid; i < nnz; i += blockDim.x) K.vals[K.end + i] = norm > 0.0 ? sv[i] / norm : sv[i];
+}
+
+struct ScoreKind {
+  int active;
+  const uint32_t* words;
+  const double* vals;
+  const int2* ent;
+  double* row;               // [kf_idx + 1]
+};
+
+// L1Scoring::score(v_new, v_i) (ScoringObject.cpp:23-68) for every i <= kf_idx: one warp per keyframe, grid-stride.  The new
+// vector's words are staged in shared memory once per block; keyframe i's word list is read once, 32 coalesced words at
+// a time, each looked up in the new vector.  The terms |v - w| - |v| - |w| of the common words are added by every lane in
+// ascending word order (the ballot's bits), as DBoW2's merge adds them; score = -sum / 2.  Absent keyframes: NaN.
+__global__ void __launch_bounds__(256) k_bow_score(ScoreKind k0, ScoreKind k1, int kf_idx) {
+  __shared__ uint32_t s_w[BOW_MAX_FEATURES];
+  const ScoreKind K = blockIdx.y ? k1 : k0;
+  if (!K.active) return;
+  const int2 me = K.ent[kf_idx];
+  const int nn = me.y;
+  for (int i = threadIdx.x; i < nn; i += blockDim.x) s_w[i] = K.words[me.x + i];
+  __syncthreads();
+  const double* nv = K.vals + me.x;
+  const int lane = threadIdx.x & 31;
+  const int nwarps = gridDim.x * 8;
+  for (int i = blockIdx.x * 8 + (threadIdx.x >> 5); i <= kf_idx; i += nwarps) {
+    const int2 e = K.ent[i];
+    if (e.y < 0) {
+      if (lane == 0) K.row[i] = __longlong_as_double(0x7FF8000000000000ll);
+      continue;
+    }
+    double score = 0;
+    for (int c = 0; c < e.y; c += 32) {
+      const int jj = c + lane;
+      bool hit = false;
+      double term = 0;
+      if (jj < e.y) {
+        const uint32_t w = K.words[e.x + jj];
+        int lo = 0, hi = nn;
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          if (s_w[mid] < w) lo = mid + 1; else hi = mid;
+        }
+        if (lo < nn && s_w[lo] == w) {
+          hit = true;
+          const double vi = nv[lo], wi = K.vals[e.x + jj];
+          term = fabs(vi - wi) - fabs(vi) - fabs(wi);
+        }
+      }
+      unsigned mask = __ballot_sync(0xFFFFFFFFu, hit);
+      while (mask) {
+        const int bl = __ffs(mask) - 1;
+        score += __shfl_sync(0xFFFFFFFFu, term, bl);
+        mask &= mask - 1;
+      }
+    }
+    if (lane == 0) K.row[i] = -score / 2.0;
+  }
+}
+
+// Grows the kind's database to hold `more` entries after `end` and keyframe indices up to kf_idx.
+plf_status grow_db(plf_ctx* ctx, BowKind& k, size_t more, int kf_idx) {
+  if (k.end + more > (size_t)INT32_MAX)   // entry offsets are int32 (int2 index entries)
+    return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_bow_insert: the %s database would exceed 2^31 - 1 entries", &k == &ctx->bow->kind[0] ? "point" : "line");
+  if (k.end + more > k.cap) {
+    size_t nc = std::max(std::max(2 * k.cap, k.end + more), (size_t)1 << 16);
+    uint32_t* w = nullptr;
+    double* v = nullptr;
+    if (cudaMalloc(&w, nc * 4) != cudaSuccess || cudaMalloc(&v, nc * 8) != cudaSuccess) {
+      cudaFree(w);
+      return plf_fail(ctx, PLF_ERR_CUDA, "plf_bow_insert: cudaMalloc of a %zu-entry database failed", nc);
+    }
+    if (k.end) {
+      PLF_CUDA(ctx, cudaMemcpyAsync(w, k.words, k.end * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+      PLF_CUDA(ctx, cudaMemcpyAsync(v, k.vals, k.end * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+    }
+    PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    cudaFree(k.words);
+    cudaFree(k.vals);
+    k.words = w;
+    k.vals = v;
+    k.cap = nc;
+  }
+  if (kf_idx >= k.ent_cap) {
+    const int nc = (int)std::min<long long>(std::max<long long>(std::max(2LL * k.ent_cap, (long long)kf_idx + 1), 1024), BOW_MAX_KF);
+    int2* e = nullptr;
+    if (cudaMalloc(&e, (size_t)nc * 8) != cudaSuccess)
+      return plf_fail(ctx, PLF_ERR_CUDA, "plf_bow_insert: cudaMalloc of %d keyframe entries failed", nc);
+    PLF_CUDA(ctx, cudaMemsetAsync(e, 0xFF, (size_t)nc * 8, ctx->stream));
+    if (k.ent_cap) PLF_CUDA(ctx, cudaMemcpyAsync(e, k.ent, (size_t)k.ent_cap * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+    PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    cudaFree(k.ent);
+    k.ent = e;
+    k.ent_cap = nc;
+  }
+  return PLF_OK;
+}
+
+size_t align_up(size_t x) { return (x + 255) & ~size_t(255); }
+
+}  // namespace
+
+extern "C" {
+
+void plf_bow_free(plf_ctx* ctx) {
+  if (!ctx->bow) return;
+  for (BowKind& k : ctx->bow->kind) free_kind(k);
+  cudaFree(ctx->bow->io);
+  delete ctx->bow;
+  ctx->bow = nullptr;
+}
+
+plf_status plf_vocab_read_yml(const char* path, plf_vocab* out) {
+  if (!path || !out) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_vocab_read_yml: path and out are required");
+  memset(out, 0, sizeof *out);
+  FILE* f = fopen(path, "rb");
+  if (!f) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_vocab_read_yml: cannot open %s", path);
+  std::string buf;
+  char chunk[1 << 16];
+  size_t got;
+  while ((got = fread(chunk, 1, sizeof chunk, f)) > 0) buf.append(chunk, got);
+  fclose(f);
+  Parser ps{buf.data(), buf.data() + buf.size(), ""};
+  std::vector<int32_t> nid, pid, wid, wnode;
+  std::vector<double> wt;
+  std::vector<uint8_t> desc;
+  int hdr[4] = {0, 0, 0, 0};
+  std::string why = parse_vocab(ps, nid, pid, wt, desc, wid, wnode, hdr);
+  if (!why.empty()) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_vocab_read_yml: %s: %s", path, why.c_str());
+  plf_vocab v;
+  v.k = hdr[0];
+  v.L = hdr[1];
+  v.scoring = hdr[2];
+  v.weighting = hdr[3];
+  v.n_nodes = (int)nid.size();
+  v.n_words = (int)wid.size();
+  v.node_id = nid.data();
+  v.parent_id = pid.data();
+  v.weight = wt.data();
+  v.desc = desc.data();
+  v.word_id = wid.data();
+  v.word_node = wnode.data();
+  why = vocab_check(&v, nullptr);
+  if (!why.empty()) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_vocab_read_yml: %s: %s", path, why.c_str());
+  v.node_id = dup_array(nid);
+  v.parent_id = dup_array(pid);
+  v.weight = dup_array(wt);
+  v.desc = dup_array(desc);
+  v.word_id = dup_array(wid);
+  v.word_node = dup_array(wnode);
+  *out = v;
+  if (!v.node_id || !v.parent_id || !v.weight || !v.desc || !v.word_id || !v.word_node) {
+    plf_vocab_free(out);
+    return plf_fail(nullptr, PLF_ERR_INVALID, "plf_vocab_read_yml: out of host memory");
+  }
+  return PLF_OK;
+}
+
+void plf_vocab_free(plf_vocab* v) {
+  if (!v) return;
+  free(v->node_id);
+  free(v->parent_id);
+  free(v->weight);
+  free(v->desc);
+  free(v->word_id);
+  free(v->word_node);
+  memset(v, 0, sizeof *v);
+}
+
+plf_status plf_bow_set_vocabulary(plf_ctx* ctx, int kind, const plf_vocab* voc) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if ((kind != 0 && kind != 1) || !voc) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_set_vocabulary: kind 0 or 1 and a vocabulary");
+  VocabLayout lay;
+  const std::string why = vocab_check(voc, &lay);
+  if (!why.empty()) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_set_vocabulary: %s", why.c_str());
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  BowState* S = bow_state(ctx);
+  BowKind& k = S->kind[kind];
+  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  free_kind(k);
+  const size_t n = lay.meta.size();
+  if (cudaMalloc(&k.desc, n * 32) != cudaSuccess || cudaMalloc(&k.meta, n * 8) != cudaSuccess ||
+      cudaMalloc(&k.weight, n * 8) != cudaSuccess) {
+    free_kind(k);
+    return plf_fail(ctx, PLF_ERR_CUDA, "plf_bow_set_vocabulary: cudaMalloc for %zu nodes failed", n);
+  }
+  PLF_CUDA(ctx, cudaMemcpy(k.desc, lay.desc.data(), n * 32, cudaMemcpyHostToDevice));
+  PLF_CUDA(ctx, cudaMemcpy(k.meta, lay.meta.data(), n * 8, cudaMemcpyHostToDevice));
+  PLF_CUDA(ctx, cudaMemcpy(k.weight, lay.weight.data(), n * 8, cudaMemcpyHostToDevice));
+  k.root_n = lay.root_n;
+  k.has_voc = true;
+  return PLF_OK;
+}
+
+plf_status plf_bow_insert(plf_ctx* ctx, int kf_idx, const plf_frame_view* kf, double* score_p, double* score_l) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (!kf) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_insert: kf is NULL");
+  if (kf_idx < 0 || kf_idx >= BOW_MAX_KF)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_insert: kf_idx %d out of range [0, %d)", kf_idx, BOW_MAX_KF);
+  const int n[2] = {kf->n_pt, kf->n_ls};
+  const uint8_t* d[2] = {kf->pdesc, kf->ldesc};
+  const bool on[2] = {ctx->params.has_points != 0, ctx->params.has_lines != 0};
+  double* rows[2] = {score_p, score_l};
+  BowState* S = bow_state(ctx);
+  for (int c = 0; c < 2; ++c) {
+    if (!on[c]) continue;
+    if (n[c] < 0 || n[c] > BOW_MAX_FEATURES)
+      return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_insert: %d %s features (at most %d)", n[c], c ? "line" : "point", BOW_MAX_FEATURES);
+    if (n[c] > 0 && !d[c]) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_insert: %s descriptors are NULL", c ? "line" : "point");
+    if (!S->kind[c].has_voc)
+      return plf_fail(ctx, PLF_ERR_STATE, "plf_bow_insert: no %s vocabulary (plf_bow_set_vocabulary)", c ? "line" : "point");
+    if (kf_idx <= S->kind[c].last)
+      return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_insert: kf_idx %d does not exceed %d, inserted before", kf_idx,
+                      S->kind[c].last);
+  }
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t cs = ctx->stream;
+  ctx->cur = cs;
+  for (int c = 0; c < 2; ++c)
+    if (on[c]) {
+      plf_status st = grow_db(ctx, S->kind[c], (size_t)n[c], kf_idx);
+      if (st) return st;
+    }
+  // io region: in = descriptors [n0 + n1][32]; work = word [.] int, weight [.] f64; out = nnz [2] int, rows [2][kf_idx + 1]
+  const int m0 = on[0] ? n[0] : 0, m1 = on[1] ? n[1] : 0, nf = m0 + m1;
+  const size_t in_b = align_up((size_t)nf * 32), w_off = in_b, wt_off = w_off + align_up((size_t)nf * 4),
+               out_off = wt_off + align_up((size_t)nf * 8), row_b = (size_t)(kf_idx + 1) * 8;
+  const size_t out_b = 16 + 2 * align_up(row_b), total = out_off + out_b;
+  if (S->io_bytes < total) {
+    PLF_CUDA(ctx, cudaStreamSynchronize(cs));
+    cudaFree(S->io);
+    S->io = nullptr;
+    S->io_bytes = 0;
+    const size_t want = std::max(total, (size_t)1 << 20);
+    if (cudaMalloc(&S->io, want) != cudaSuccess) return plf_fail(ctx, PLF_ERR_CUDA, "plf_bow_insert: cudaMalloc(%zu)", want);
+    S->io_bytes = want;
+  }
+  uint8_t* pin = (uint8_t*)plf_pinned(ctx, std::max(in_b, out_b));
+  if (!pin) return PLF_ERR_CUDA;
+  if (m0) memcpy(pin, d[0], (size_t)m0 * 32);
+  if (m1) memcpy(pin + (size_t)m0 * 32, d[1], (size_t)m1 * 32);
+  uint8_t* io = S->io;
+  int* d_word = (int*)(io + w_off);
+  double* d_wt = (double*)(io + wt_off);
+  int* d_nnz = (int*)(io + out_off);
+  double* d_row[2] = {(double*)(io + out_off + 16), (double*)(io + out_off + 16 + align_up(row_b))};
+  if (nf) PLF_CUDA(ctx, cudaMemcpyAsync(io, pin, (size_t)nf * 32, cudaMemcpyHostToDevice, cs));
+  if (nf) {
+    const BowKind &a = S->kind[0], &b = S->kind[1];
+    const TreeView t0 = {a.desc, a.meta, a.weight, a.root_n}, t1 = {b.desc, b.meta, b.weight, b.root_n};
+    k_bow_transform<<<(nf + 7) / 8, 256, 0, cs>>>(t0, t1, (const uint4*)io, m0, m1, d_word, d_wt);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  const size_t smem = (size_t)BOW_MAX_FEATURES * 16;
+  if (!S->attr_set) {
+    PLF_CUDA(ctx, cudaFuncSetAttribute(k_bow_assemble, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    S->attr_set = true;
+  }
+  AssembleKind ak[2];
+  for (int c = 0; c < 2; ++c) {
+    BowKind& k = S->kind[c];
+    ak[c] = {on[c] ? 1 : 0, c ? m1 : m0, c ? m0 : 0, k.words, k.vals, k.ent, (long long)k.end};
+  }
+  k_bow_assemble<<<2, BOW_SORT_THREADS, smem, cs>>>(ak[0], ak[1], d_word, d_wt, kf_idx, d_nnz);
+  PLF_LAUNCH_CHECK(ctx);
+  ScoreKind sk[2];
+  bool any_row = false;
+  for (int c = 0; c < 2; ++c) {
+    BowKind& k = S->kind[c];
+    sk[c] = {on[c] && rows[c] ? 1 : 0, k.words, k.vals, k.ent, d_row[c]};
+    any_row |= sk[c].active != 0;
+  }
+  if (any_row) {
+    const int blocks = std::min((kf_idx + 1 + 7) / 8, 4 * S->n_sm);
+    k_bow_score<<<dim3(blocks, 2), 256, 0, cs>>>(sk[0], sk[1], kf_idx);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  // one download: the counts and the rows
+  const size_t dl = any_row ? (size_t)(d_row[sk[1].active ? 1 : 0] - (double*)(io + out_off + 16)) * 8 + 16 + row_b : 16;
+  PLF_CUDA(ctx, cudaMemcpyAsync(pin, io + out_off, dl, cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaStreamSynchronize(cs));
+  const int* nnz = (const int*)pin;
+  for (int c = 0; c < 2; ++c) {
+    if (!on[c]) continue;
+    BowKind& k = S->kind[c];
+    if ((int)k.host_ent.size() < kf_idx + 1) k.host_ent.resize(kf_idx + 1, make_int2(-1, -1));
+    k.host_ent[kf_idx] = make_int2((int)k.end, nnz[c]);
+    k.end += (size_t)nnz[c];
+    k.last = kf_idx;
+    if (rows[c]) memcpy(rows[c], pin + 16 + (size_t)(d_row[c] - d_row[0]) * 8, row_b);
+  }
+  return PLF_OK;
+}
+
+plf_status plf_bow_erase(plf_ctx* ctx, int kf_idx) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (kf_idx < 0) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_erase: kf_idx %d < 0", kf_idx);
+  if (!ctx->bow) return PLF_OK;
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  for (BowKind& k : ctx->bow->kind) {
+    if (kf_idx >= (int)k.host_ent.size() || k.host_ent[kf_idx].y < 0) continue;
+    k.host_ent[kf_idx] = make_int2(-1, -1);
+    PLF_CUDA(ctx, cudaMemsetAsync(k.ent + kf_idx, 0xFF, 8, ctx->stream));
+  }
+  return PLF_OK;
+}
+
+plf_status plf_bow_get(plf_ctx* ctx, int kf_idx, int kind, int cap, uint32_t* words, double* values, int* n) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (!n || (kind != 0 && kind != 1)) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_get: kind 0 or 1 and n are required");
+  *n = 0;
+  const BowKind* k = ctx->bow ? &ctx->bow->kind[kind] : nullptr;
+  if (!k || kf_idx < 0 || kf_idx >= (int)k->host_ent.size() || k->host_ent[kf_idx].y < 0)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_get: keyframe %d has no stored %s vector", kf_idx, kind ? "line" : "point");
+  const int2 e = k->host_ent[kf_idx];
+  *n = e.y;
+  if (!words && !values) return PLF_OK;
+  if (e.y > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_bow_get: %d entries, capacity %d", e.y, cap);
+  if (e.y == 0) return PLF_OK;
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (words) PLF_CUDA(ctx, cudaMemcpy(words, k->words + e.x, (size_t)e.y * 4, cudaMemcpyDeviceToHost));
+  if (values) PLF_CUDA(ctx, cudaMemcpy(values, k->vals + e.x, (size_t)e.y * 8, cudaMemcpyDeviceToHost));
+  return PLF_OK;
+}
+
+}  // extern "C"

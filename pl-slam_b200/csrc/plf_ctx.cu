@@ -271,12 +271,14 @@ void plf_orb_free(plf_ctx* ctx);
 void plf_lsd_free(plf_ctx* ctx);
 void plf_lbd_free(plf_ctx* ctx);
 void plf_pipe_free(plf_ctx* ctx);
+void plf_bow_free(plf_ctx* ctx);
 
 void plf_destroy(plf_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   plf_pipe_free(ctx);
+  plf_bow_free(ctx);
   plf_orb_free(ctx);
   plf_lsd_free(ctx);
   plf_lbd_free(ctx);

@@ -49,6 +49,7 @@ struct plf_ctx {
   struct LsdState* lsd = nullptr;
   struct LbdState* lbd = nullptr;
   struct PipeState* pipe = nullptr;
+  struct BowState* bow = nullptr;   // DBoW2 vocabularies and keyframe database (dbow.cu)
   // optional per-stage timing (plf_profile_enable): events recorded after each kernel of plf_batch_run
   bool profile = false;
   bool profile_piped = false;  // marks recorded while the E/G/M software pipeline stays enabled (durations under overlap)

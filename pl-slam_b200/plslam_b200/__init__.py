@@ -135,6 +135,47 @@ class plf_local_map(C.Structure):
                 ("n_ls", C.c_int), ("ls_X", C.c_void_p), ("ls_desc", C.c_void_p), ("ls_use", C.c_void_p)]
 
 
+class plf_vocab(C.Structure):
+    _fields_ = [("k", C.c_int), ("L", C.c_int), ("scoring", C.c_int), ("weighting", C.c_int), ("n_nodes", C.c_int),
+                ("node_id", C.c_void_p), ("parent_id", C.c_void_p), ("weight", C.c_void_p), ("desc", C.c_void_p),
+                ("n_words", C.c_int), ("word_id", C.c_void_p), ("word_node", C.c_void_p)]
+
+
+# plf_vocab arrays: (name, dtype, columns, count field)
+_VOCAB_ARRAYS = (("node_id", np.int32, 0, "n_nodes"), ("parent_id", np.int32, 0, "n_nodes"),
+                 ("weight", np.float64, 0, "n_nodes"), ("desc", np.uint8, 32, "n_nodes"),
+                 ("word_id", np.int32, 0, "n_words"), ("word_node", np.int32, 0, "n_words"))
+
+
+def read_vocab_yml(path) -> dict:
+    """plf_vocab_read_yml: a DBoW2 vocabulary YAML file as a dict of k, L, scoring, weighting and the arrays in file order
+    (node_id, parent_id, weight, desc [n][32], word_id, word_node).  Host only; raises PlfError on a malformed file."""
+    lib = load_library()
+    v = plf_vocab()
+    st = lib.plf_vocab_read_yml(str(path).encode(), C.byref(v))
+    if st != 0:
+        raise PlfError(f"plf_vocab_read_yml failed ({st}): {lib.plf_last_error(None).decode()}")
+    try:
+        out = dict(k=v.k, L=v.L, scoring=v.scoring, weighting=v.weighting)
+        for name, dt, cols, count in _VOCAB_ARRAYS:
+            n = getattr(v, count) * max(cols, 1)
+            a = np.ctypeslib.as_array(C.cast(getattr(v, name), C.POINTER(np.ctypeslib.as_ctypes_type(dt))), (n,)).copy()
+            out[name] = a.reshape(-1, cols) if cols else a
+    finally:
+        lib.plf_vocab_free(C.byref(v))
+    return out
+
+
+def _vocab_struct(voc: dict, keep: list) -> plf_vocab:
+    v = plf_vocab(int(voc["k"]), int(voc.get("L", 0)), int(voc.get("scoring", 0)), int(voc.get("weighting", 0)))
+    for name, dt, cols, count in _VOCAB_ARRAYS:
+        a = np.ascontiguousarray(voc[name], dt)
+        keep.append(a)
+        setattr(v, name, a.ctypes.data if a.size else None)
+        setattr(v, count, len(a))
+    return v
+
+
 # the plf_frame_view fields the keyframe matchers read: (name, dtype, columns)
 _KF_VIEW_FIELDS = (("pt_pl", np.float64, 2), ("pt_P", np.float64, 3), ("pdesc", np.uint8, 32), ("ls_spl", np.float64, 2),
                    ("ls_epl", np.float64, 2), ("ls_sP", np.float64, 3), ("ls_eP", np.float64, 3), ("ls_le", np.float64, 3),
@@ -509,6 +550,44 @@ class Frontend:
                                               lm_pt.ctypes.data_as(C.c_void_p), lm_ls.ctypes.data_as(C.c_void_p),
                                               C.byref(n_pt), C.byref(n_ls)), "plf_match_map2kf")
         return dict(lm_pt=lm_pt[:m.n_pt].copy(), n_pt=n_pt.value, lm_ls=lm_ls[:m.n_ls].copy(), n_ls=n_ls.value)
+
+    # -- place recognition (DBoW2) -----------------------------------------------------------------
+    def bow_set_vocabulary(self, kind, voc):
+        """plf_bow_set_vocabulary: kind 0 (points) / 1 (lines); voc: a YAML path or a dict as read_vocab_yml returns.
+        Empties that kind's keyframe database."""
+        if not isinstance(voc, dict):
+            voc = read_vocab_yml(voc)
+        keep = []
+        v = _vocab_struct(voc, keep)
+        self._check(self.lib.plf_bow_set_vocabulary(self._ctx, int(kind), C.byref(v)), "plf_bow_set_vocabulary")
+
+    def bow_insert(self, kf_idx, pdesc=None, ldesc=None, rows=(True, True)):
+        """plf_bow_insert: stores the BoW vectors of the keyframe's descriptors under kf_idx and returns (score_p, score_l),
+        float64 [kf_idx + 1] each (NaN: absent keyframe), None for a row not requested (rows) or of a disabled kind."""
+        keep = []
+        fr = {}
+        if pdesc is not None:
+            fr["pdesc"] = pdesc
+        if ldesc is not None:
+            fr["ldesc"] = ldesc
+        v = _frame_view(fr, keep)
+        enabled = (self.params.has_points, self.params.has_lines)
+        out = [np.full(kf_idx + 1, np.nan) if (rows[c] and enabled[c] and kf_idx >= 0) else None for c in range(2)]
+        ptr = [C.c_void_p(o.ctypes.data) if o is not None else C.c_void_p() for o in out]
+        self._check(self.lib.plf_bow_insert(self._ctx, int(kf_idx), C.byref(v), ptr[0], ptr[1]), "plf_bow_insert")
+        return out[0], out[1]
+
+    def bow_erase(self, kf_idx):
+        self._check(self.lib.plf_bow_erase(self._ctx, int(kf_idx)), "plf_bow_erase")
+
+    def bow_vector(self, kf_idx, kind):
+        """plf_bow_get: the stored BowVector of keyframe kf_idx, kind 0 / 1, as (words uint32, values float64)."""
+        n = C.c_int(0)
+        self._check(self.lib.plf_bow_get(self._ctx, int(kf_idx), int(kind), 0, None, None, C.byref(n)), "plf_bow_get")
+        w, x = np.zeros(max(n.value, 1), np.uint32), np.zeros(max(n.value, 1), np.float64)
+        self._check(self.lib.plf_bow_get(self._ctx, int(kf_idx), int(kind), n.value, C.c_void_p(w.ctypes.data),
+                                         C.c_void_p(x.ctypes.data), C.byref(n)), "plf_bow_get")
+        return w[:n.value].copy(), x[:n.value].copy()
 
     def expmap_se3(self, x):
         x = np.ascontiguousarray(x, np.float64).reshape(6)
