@@ -332,6 +332,28 @@ typedef struct plf_lba_result {
 } plf_lba_result;
 plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* problem, plf_lba_result* out);
 
+/* Global bundle adjustment.  Replaces MapHandler::levMarquardtOptimizationGBA (src/mapHandler.cpp:2101-2699), the
+ * numerical core of MapHandler::globalBundleAdjustment (:1995-2099): the same Levenberg-Marquardt as plf_local_ba over
+ * every live keyframe except keyframe 0 and every landmark of the map.  The problem has plf_local_ba's layout, assembled
+ * as :1995-2090 does:
+ *   kf_pose  x_kf_w of every live keyframe except keyframe 0, in kf_idx order (:2001-2014), in / out
+ *   pt / ls  every point / line landmark, in map order, in / out
+ *   fixed_T  T_kf_w of keyframe 0 (and of any other keyframe the caller holds fixed)
+ *   observations grouped per landmark in ascending landmark order (:2017-2090).  Observations made by erased keyframes
+ *   are skipped by the reference (:2131, :2239), so the caller leaves them out, and leaves out a landmark whose
+ *   observations all came from erased keyframes: a landmark without observations is refused.
+ *   pt_moved / ls_moved may be NULL (the reference has no such write-back; they are filled as plf_local_ba fills them).
+ * opts: lambda / lambda_k / max_iters = SlamConfig::lambdaLbaLM / lambdaLbaK / maxItersLba, which GBA reuses (:2116, :2391);
+ * min_error = min_error_change = DBL_EPSILON, the literals of :2637, :2667.  ref_quirks = 1 reproduces six oddities of
+ * the reference as written (oracle/gba.py lists them as g1-g6 with their lines), 0 follows its evident intent.
+ * Limits: n_kf <= 4096 (else PLF_ERR_CAPACITY).  PLF_ERR_INVALID for an empty problem, a landmark without observations,
+ * ungrouped observations, out-of-range indices or NULL arrays; the context stays usable after any error.
+ * Work is enqueued on plf_stream and uses scratch slot 10 (shared with plf_local_ba), which stays allocated until
+ * plf_destroy: about 288 n_kf^2 bytes for the dense reduced system (1.2 GB at 2048 keyframes, 4.8 GB at 4096) plus
+ * 144 bytes per observation and about 650 bytes per landmark.  Up to n_kf = 64 the reduced system is factored by one CTA as in
+ * plf_local_ba; beyond, by a tiled LDL^T across the GPU that skips exactly-zero tiles. */
+plf_status plf_global_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* problem, plf_lba_result* out);
+
 /* Relative pose between two keyframes (SURVEY 8(f) f2).  Replaces MapHandler::isLoopClosure (src/mapHandler.cpp:3192-3300:
  * match() on the points :3223 and on the lines :3249 of kf0 / kf1, the inlier-ratio pre-condition :3277-3299) followed by
  * MapHandler::computeRelativePoseRobustGN (:3566-3957: two-stage robust GN from identity with the chi2 gate in between,

@@ -1,12 +1,15 @@
 // vo_demo — the VO part of the reference's frame loop (app/plslam_dataset.cpp:111-163) on top of the C++ shim.
 // Usage: vo_demo <frames.bin> [orb_nfeatures lsd_nfeatures] [--grid-selftest | --kf-match-selftest |
 //                                                            --bow-selftest <voc_p.yml> <voc_l.yml>]
+//        vo_demo --gba-selftest <problem.bin>
 // frames.bin: int32 n, w, h; double fx, fy, cx, cy, b; then n x (left h*w bytes, right h*w bytes).
 // Prints one line per frame: idx status n_stereo_pt n_stereo_ls n_inliers newKF Tfw(16 values, row-major).
+#include <cfloat>
 #include <cstdio>
 #include <cstdlib>
 #include <stdexcept>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "stvo_shim.h"
@@ -159,10 +162,13 @@ static int kf_match_selftest(plf_ctx* ctx, KfArrays& prev_kf, KfArrays& curr_kf)
 
 // ---- INTEGRATION.md §4 f5: DBoW2 place recognition (the text between the two markers is the snippet shown there) ----
 // What MapHandler's BoW code reads: KeyFrame::kf_idx and KeyFrame::stereo_frame (include/keyFrame.h), the map_keyframes
-// list (NULL once removeRedundantKFs deleted a keyframe) and conf_matrix (include/mapHandler.h:147).
+// list (NULL once removeRedundantKFs deleted a keyframe) and conf_matrix (include/mapHandler.h:147).  The global BA
+// (f6 below) reads x_kf_w and writes T_kf_w.
 struct KeyFrame {
   int kf_idx;
   StVO::StereoFrame* stereo_frame;
+  StVO::Vector6d x_kf_w;
+  StVO::Matrix4d T_kf_w;
 };
 struct BowMap {
   plf_ctx* ctx;
@@ -254,8 +260,202 @@ static void bow_selftest_frame(BowMap& m, StVO::StereoFrame* cur, int frame_coun
   }
 }
 
+// ---- INTEGRATION.md §4 f6: global bundle adjustment (the text between the two markers is the snippet shown there) ----
+// What MapHandler's GBA reads and writes: the map_keyframes / map_points / map_lines lists (NULL where deleted),
+// MapPoint::idx / point3D / obs_list / kf_obs_list and MapLine::idx / line3D / obs_list / kf_obs_list
+// (include/mapFeatures.h), and the SlamConfig values levMarquardtOptimizationGBA reuses.
+struct MapPoint {
+  int idx;
+  StVO::Vector3d point3D;
+  std::vector<StVO::Vector2d> obs_list;
+  std::vector<int> kf_obs_list;
+};
+struct MapLine {
+  int idx;
+  StVO::Vector6d line3D;
+  std::vector<StVO::Vector3d> obs_list;
+  std::vector<int> kf_obs_list;
+};
+struct GbaMap {
+  plf_ctx* ctx;
+  double lambda_lba_lm, lambda_lba_k, homog_th;   // SlamConfig::lambdaLbaLM / lambdaLbaK / homogTh
+  int max_iters_lba;                              // SlamConfig::maxItersLba
+  std::vector<KeyFrame*> map_keyframes;
+  std::vector<MapPoint*> map_points;
+  std::vector<MapLine*> map_lines;
+};
+// BEGIN f6
+// MapHandler::globalBundleAdjustment (:1995-2099): the lists, plf_global_ba, the write-back (:2673-2697)
+static plf_lba_result global_bundle_adjustment(GbaMap& m) {
+  std::vector<double> X;                                    // [x_kf_w of every live KF but 0 | point3D | line3D]
+  std::unordered_map<int, int> kf_loc;                      // kf_idx -> local index (:2001-2014)
+  std::vector<int> kf_list, pt_list, ls_list, pt_lm, pt_kf, ls_lm, ls_kf;
+  std::vector<double> pt_xy, ls_le, fixed_T;                // fixed_T: row-major T_kf_w of keyframe 0
+  for (KeyFrame* kf : m.map_keyframes)
+    if (kf && kf->kf_idx != 0) {
+      kf_loc[kf->kf_idx] = (int)kf_list.size();
+      kf_list.push_back(kf->kf_idx);
+      for (int i = 0; i < 6; ++i) X.push_back(kf->x_kf_w(i));
+    }
+  for (int r = 0; r < 4; ++r)
+    for (int c = 0; c < 4; ++c) fixed_T.push_back(m.map_keyframes[0]->T_kf_w(r, c));
+  auto kf_index = [&](int kf_idx) { auto it = kf_loc.find(kf_idx); return it == kf_loc.end() ? -1 : it->second; };
+  // :2017-2052 / :2054-2090.  The reference skips observations made by erased keyframes (:2131, :2239): they are left
+  // out, and so is a landmark left without observations (plf_global_ba refuses one: it would be a zero pivot).
+  for (MapPoint* pt : m.map_points) {
+    if (!pt) continue;
+    int n = 0;
+    for (size_t i = 0; i < pt->obs_list.size(); ++i) {
+      const int k = pt->kf_obs_list[i];
+      if (!m.map_keyframes[k]) continue;
+      pt_lm.push_back((int)pt_list.size());
+      pt_kf.push_back(kf_index(k));                         // -1: keyframe 0 = fixed_T[0]
+      for (int c = 0; c < 2; ++c) pt_xy.push_back(pt->obs_list[i](c));
+      ++n;
+    }
+    if (!n) continue;
+    pt_list.push_back(pt->idx);
+    for (int c = 0; c < 3; ++c) X.push_back(pt->point3D(c));
+  }
+  for (MapLine* ls : m.map_lines) {
+    if (!ls) continue;
+    int n = 0;
+    for (size_t i = 0; i < ls->obs_list.size(); ++i) {
+      const int k = ls->kf_obs_list[i];
+      if (!m.map_keyframes[k]) continue;
+      ls_lm.push_back((int)ls_list.size());
+      ls_kf.push_back(kf_index(k));
+      for (int c = 0; c < 3; ++c) ls_le.push_back(ls->obs_list[i](c));
+      ++n;
+    }
+    if (!n) continue;
+    ls_list.push_back(ls->idx);
+    for (int c = 0; c < 6; ++c) X.push_back(ls->line3D(c));
+  }
+  plf_lba_problem p = {};
+  p.n_kf = (int)kf_list.size(); p.n_pt = (int)pt_list.size(); p.n_ls = (int)ls_list.size(); p.n_fixed = 1;
+  p.kf_pose = X.data(); p.pt = X.data() + 6 * p.n_kf; p.ls = p.pt + 3 * p.n_pt; p.fixed_T = fixed_T.data();
+  p.n_pt_obs = (int)pt_lm.size(); p.pt_obs_lm = pt_lm.data(); p.pt_obs_kf = pt_kf.data(); p.pt_obs_xy = pt_xy.data();
+  p.n_ls_obs = (int)ls_lm.size(); p.ls_obs_lm = ls_lm.data(); p.ls_obs_kf = ls_kf.data(); p.ls_obs_le = ls_le.data();
+  plf_lba_opts o = {m.lambda_lba_lm, m.lambda_lba_k, m.max_iters_lba, m.homog_th,
+                    DBL_EPSILON, DBL_EPSILON, /*ref_quirks=*/1};  // :2116, :2391, :2637, :2667
+  plf_lba_result res;
+  plf_check(m.ctx, plf_global_ba(m.ctx, &o, &p, &res), "plf_global_ba");
+  for (size_t i = 0; i < kf_list.size(); ++i) {             // :2673-2697
+    StVO::Vector6d x;
+    for (int c = 0; c < 6; ++c) x(c) = p.kf_pose[6 * i + c];
+    m.map_keyframes[kf_list[i]]->T_kf_w = StVO::expmap_se3(x);
+  }
+  for (size_t i = 0; i < pt_list.size(); ++i)
+    for (int c = 0; c < 3; ++c) m.map_points[pt_list[i]]->point3D(c) = p.pt[3 * i + c];
+  for (size_t i = 0; i < ls_list.size(); ++i)
+    for (int c = 0; c < 6; ++c) m.map_lines[ls_list[i]]->line3D(c) = p.ls[6 * i + c];
+  return res;
+}
+// END f6
+
+// `vo_demo --gba-selftest problem.bin`: reads a map (little-endian: int32 width, height; f64 fx, fy, cx, cy, b, lambda,
+// lambda_k, homog_th; int32 max_iters; then keyframe, point and line slots, each an int32 `present` flag followed by
+// the object: keyframe x_kf_w[6], T_kf_w[16] row-major; point point3D[3], int32 n_obs, n_obs x (int32 kf_idx, f64[2]);
+// line line3D[6], int32 n_obs, n_obs x (int32 kf_idx, f64[3])), runs the f6 function above on it and prints the result,
+// every live keyframe's T_kf_w and every live landmark, which the Python binding must reproduce.
+static int gba_selftest(const char* path) {
+  FILE* f = std::fopen(path, "rb");
+  if (!f) { std::perror("open"); return 1; }
+  bool ok = true;
+  auto i32 = [&]() { int32_t v = 0; ok = ok && std::fread(&v, 4, 1, f) == 1; return (int)v; };
+  auto f64 = [&]() { double v = 0; ok = ok && std::fread(&v, 8, 1, f) == 1; return v; };
+  plf_camera cam;
+  cam.width = i32(); cam.height = i32();
+  cam.fx = f64(); cam.fy = f64(); cam.cx = f64(); cam.cy = f64(); cam.b = f64();
+  GbaMap m = {};
+  m.lambda_lba_lm = f64(); m.lambda_lba_k = f64(); m.homog_th = f64(); m.max_iters_lba = i32();
+  for (int i = 0, n = i32(); ok && i < n; ++i) {
+    KeyFrame* kf = nullptr;
+    if (i32()) {
+      kf = new KeyFrame{i, nullptr, {}, {}};
+      for (int c = 0; c < 6; ++c) kf->x_kf_w(c) = f64();
+      for (int c = 0; c < 16; ++c) kf->T_kf_w.v[c] = f64();
+    }
+    m.map_keyframes.push_back(kf);
+  }
+  for (int i = 0, n = i32(); ok && i < n; ++i) {
+    MapPoint* pt = nullptr;
+    if (i32()) {
+      pt = new MapPoint{i, {}, {}, {}};
+      for (int c = 0; c < 3; ++c) pt->point3D(c) = f64();
+      for (int k = 0, no = i32(); ok && k < no; ++k) {
+        pt->kf_obs_list.push_back(i32());
+        StVO::Vector2d z;
+        for (int c = 0; c < 2; ++c) z(c) = f64();
+        pt->obs_list.push_back(z);
+      }
+    }
+    m.map_points.push_back(pt);
+  }
+  for (int i = 0, n = i32(); ok && i < n; ++i) {
+    MapLine* ls = nullptr;
+    if (i32()) {
+      ls = new MapLine{i, {}, {}, {}};
+      for (int c = 0; c < 6; ++c) ls->line3D(c) = f64();
+      for (int k = 0, no = i32(); ok && k < no; ++k) {
+        ls->kf_obs_list.push_back(i32());
+        StVO::Vector3d z;
+        for (int c = 0; c < 3; ++c) z(c) = f64();
+        ls->obs_list.push_back(z);
+      }
+    }
+    m.map_lines.push_back(ls);
+  }
+  std::fclose(f);
+  int rc = 0;
+  if (!ok) { std::fprintf(stderr, "short read\n"); rc = 1; }
+  plf_params prm;
+  plf_default_params(&prm);
+  plf_limits lim;
+  plf_default_limits(&lim);
+  lim.max_batch = 1;
+  if (!rc && plf_create(&prm, &cam, &lim, 0, &m.ctx) != PLF_OK) {
+    std::fprintf(stderr, "plf_create: %s\n", plf_last_error(nullptr));
+    rc = 2;
+  }
+  if (!rc) {
+    try {
+      const plf_lba_result res = global_bundle_adjustment(m);
+      std::printf("gba result %d %.17g %.17g\n", res.iters, res.err, res.lambda);
+      for (KeyFrame* kf : m.map_keyframes) {
+        if (!kf || kf->kf_idx == 0) continue;
+        std::printf("gba kf %d", kf->kf_idx);
+        for (int c = 0; c < 16; ++c) std::printf(" %.17g", kf->T_kf_w.v[c]);
+        std::printf("\n");
+      }
+      for (MapPoint* pt : m.map_points) {
+        if (!pt) continue;
+        std::printf("gba pt %d", pt->idx);
+        for (int c = 0; c < 3; ++c) std::printf(" %.17g", pt->point3D(c));
+        std::printf("\n");
+      }
+      for (MapLine* ls : m.map_lines) {
+        if (!ls) continue;
+        std::printf("gba ls %d", ls->idx);
+        for (int c = 0; c < 6; ++c) std::printf(" %.17g", ls->line3D(c));
+        std::printf("\n");
+      }
+    } catch (const std::exception& e) {
+      std::fprintf(stderr, "error: %s\n", e.what());
+      rc = 2;
+    }
+    plf_destroy(m.ctx);
+  }
+  for (KeyFrame* kf : m.map_keyframes) delete kf;
+  for (MapPoint* pt : m.map_points) delete pt;
+  for (MapLine* ls : m.map_lines) delete ls;
+  return rc;
+}
+
 int main(int argc, char** argv) {
   bool grid_test = false, kf_test = false;
+  if (argc == 3 && std::string(argv[1]) == "--gba-selftest") return gba_selftest(argv[2]);
   const char* bow_voc[2] = {nullptr, nullptr};
   if (argc >= 4 && std::string(argv[argc - 3]) == "--bow-selftest") {
     bow_voc[0] = argv[argc - 2];

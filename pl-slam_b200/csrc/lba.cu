@@ -20,8 +20,28 @@
 // :1775,:1805).  opts.ref_quirks selects between the reference as written and its evident intent for the four oddities
 // documented in oracle/lba.c (division by the zero counters :1541, both line end points read from one block of X at
 // stride 3 :1678-1679, the map's pose for line rows :1681, the literal clamp); oracle = oracle/lba.c.
+//
+// Global bundle adjustment (SURVEY §8(f), after f1-f5): plf_global_ba replaces MapHandler::levMarquardtOptimizationGBA
+// (:2101-2699) with the same kernels and host loop over every keyframe but keyframe 0 and every landmark.  Its quirk set
+// (g1-g6, oracle/gba.py) selects the reference's GBA oddities instead of LBA's, and a reduced system larger than 384
+// (more than 64 keyframes) is factored by the tiled, multi-CTA LDL^T below (k_gba_*), whose trailing update runs on the
+// FP64 tensor cores (DMMA) and skips the tiles of the panel that are exactly zero.
 #include "plf_internal.h"
 #include "plf_se3.cuh"
+
+// Which of the reference's oddities the kernels and the host loop reproduce: plf_local_ba's ref_quirks selects q1-q4
+// (oracle/lba.c), plf_global_ba's g1-g6 (oracle/gba.py).  0 = the evident intent of both.
+enum : int {
+  BAQ_FIRST_ERR0 = 1,      // q1 / g1: the first pass divides the error by two counters never incremented
+  BAQ_LINE_STRIDE3 = 2,    // q2 / g4: LM line rows read both end points from one block of X at stride 3
+  BAQ_LINE_MAP_POSE = 4,   // q3 / g5: LM line rows take the map's pose
+  BAQ_LINE_LITERAL = 8,    // q4: LM line rows clamp with the literal 0.0000001
+  BAQ_ITER_ERR0 = 16,      // g3: the LM iterations divide the error by the zero counters too
+  BAQ_HMAX_INT = 32,       // g2: the first lambda multiplies by the diagonal maximum truncated to int
+  BAQ_SWAP_COUPLING = 64,  // g6: the first pass writes the line/keyframe coupling as w Jt Jx^T (landmark row x pose column)
+};
+constexpr int BAQ_LBA = BAQ_FIRST_ERR0 | BAQ_LINE_STRIDE3 | BAQ_LINE_MAP_POSE | BAQ_LINE_LITERAL;
+constexpr int BAQ_GBA = BAQ_FIRST_ERR0 | BAQ_LINE_STRIDE3 | BAQ_LINE_MAP_POSE | BAQ_ITER_ERR0 | BAQ_HMAX_INT | BAQ_SWAP_COUPLING;
 
 struct LbaDev {
   int nkf, npt, nls, N, npo, nlo, nobs, nlm;
@@ -35,7 +55,7 @@ struct LbaDev {
   double* A; double* gc;                       // nkf x 36, nkf x 6
   double* S; double* gred; double* dxc;        // n x n, n, n   (n = 6 nkf)
   double* DX;                                  // N
-  double* scal;                                // [0] err, [1] |dx|^2, [2] Hmax (as ordered bits)
+  double* scal;                                // [0] err, [1] |dx|^2, [2] Hmax (as ordered bits), [3] Hmax under g2
 };
 struct LbaCam { double fx, fy, cx, cy; };
 
@@ -54,7 +74,7 @@ __device__ __forceinline__ void lba_xform(const double* T, const double* P, doub
   for (int i = 0; i < 3; ++i) Q[i] = T[4 * i] * P[0] + T[4 * i + 1] * P[1] + T[4 * i + 2] * P[2] + T[4 * i + 3];
 }
 
-// mode 0: first pass on the map's values (X0 / T0inv); mode 1: LM iteration on X; quirks: see the header
+// mode 0: first pass on the map's values (X0 / T0inv); mode 1: LM iteration on X; quirks: BAQ_* set
 __global__ void __launch_bounds__(128) k_lba_rows(LbaDev d, LbaCam c, int mode, int quirks, double homog_th) {
   const int k = blockIdx.x * 128 + threadIdx.x;
   double e2w = 0.0;
@@ -63,7 +83,7 @@ __global__ void __launch_bounds__(128) k_lba_rows(LbaDev d, LbaCam c, int mode, 
     const int lm = d.obs_lm[k], kf = d.obs_kf[k];
     const double* X = mode == 0 ? d.X0 : d.X;
     double Ti[16];
-    const bool map_pose = mode == 0 || (is_line && quirks);   // (q3)
+    const bool map_pose = mode == 0 || (is_line && (quirks & BAQ_LINE_MAP_POSE));   // (q3, g5)
     if (kf >= 0) {
       if (map_pose) {
         for (int i = 0; i < 16; ++i) Ti[i] = d.T0inv[16 * kf + i];
@@ -93,10 +113,10 @@ __global__ void __launch_bounds__(128) k_lba_rows(LbaDev d, LbaCam c, int mode, 
       lba_rowvec_R(J3, Ti, JX);
       for (int i = 0; i < 3; ++i) JX[i] = JX[i] / den;
     } else {
-      const double hom = (mode == 1 && quirks) ? 0.0000001 : homog_th;   // (q4)
+      const double hom = (mode == 1 && (quirks & BAQ_LINE_LITERAL)) ? 0.0000001 : homog_th;   // (q4)
       const double *P, *Q;
-      if (mode == 1 && quirks) {
-        P = Q = X + 6 * d.nkf + 3 * d.npt + 3 * lm;                      // (q2)
+      if (mode == 1 && (quirks & BAQ_LINE_STRIDE3)) {
+        P = Q = X + 6 * d.nkf + 3 * d.npt + 3 * lm;                      // (q2, g4)
       } else {
         P = X + 6 * d.nkf + 3 * d.npt + 6 * lm;
         Q = P + 3;
@@ -191,10 +211,13 @@ __device__ void lba_inv_spd(double* M, int dim, double* Minv) {
   }
 }
 
-__global__ void __launch_bounds__(128) k_lba_lm_schur(LbaDev d, double lambda) {
+// swap (g6): for line landmarks the coupling block is w Jt Jx^T, so Jt is the landmark-side vector and Jx the pose side
+__global__ void __launch_bounds__(128) k_lba_lm_schur(LbaDev d, double lambda, int swap) {
   const int l = blockIdx.x * 128 + threadIdx.x;
   if (l >= d.nlm) return;
   const int dim = l < d.npt ? 3 : 6, n = 6 * d.nkf;
+  const double* U = swap && l >= d.npt ? d.Jt : d.Jx;   // landmark side of the coupling
+  const double* V = swap && l >= d.npt ? d.Jx : d.Jt;   // keyframe side
   double D[36], Di[36], g[6];
   for (int i = 0; i < 36; ++i) D[i] = d.D[36 * (size_t)l + i];
   for (int i = 0; i < 6; ++i) g[i] = d.gl[6 * (size_t)l + i];
@@ -205,8 +228,8 @@ __global__ void __launch_bounds__(128) k_lba_lm_schur(LbaDev d, double lambda) {
   for (int a = s; a < e; ++a) {
     const int ka = d.obs_kf[a];
     if (ka < 0) continue;
-    const double* jxa = d.Jx + 6 * (size_t)a;
-    const double* jta = d.Jt + 6 * (size_t)a;
+    const double* jxa = U + 6 * (size_t)a;
+    const double* jta = V + 6 * (size_t)a;
     const double wa = d.Wn[2 * (size_t)a];
     double y[6];
     for (int i = 0; i < dim; ++i) {
@@ -220,8 +243,8 @@ __global__ void __launch_bounds__(128) k_lba_lm_schur(LbaDev d, double lambda) {
     for (int b = s; b < e; ++b) {
       const int kb = d.obs_kf[b];
       if (kb < 0) continue;
-      const double* jxb = d.Jx + 6 * (size_t)b;
-      const double* jtb = d.Jt + 6 * (size_t)b;
+      const double* jxb = U + 6 * (size_t)b;
+      const double* jtb = V + 6 * (size_t)b;
       double cab = 0.0;
       for (int i = 0; i < dim; ++i) cab += y[i] * jxb[i];
       cab *= d.Wn[2 * (size_t)b];
@@ -274,17 +297,19 @@ __global__ void __launch_bounds__(256) k_lba_solve(LbaDev d, double lambda) {
   }
 }
 
-__global__ void __launch_bounds__(128) k_lba_backsub(LbaDev d) {
+__global__ void __launch_bounds__(128) k_lba_backsub(LbaDev d, int swap) {
   const int l = blockIdx.x * 128 + threadIdx.x;
   if (l >= d.nlm) return;
   const int dim = l < d.npt ? 3 : 6;
+  const double* U = swap && l >= d.npt ? d.Jt : d.Jx;   // as k_lba_lm_schur
+  const double* V = swap && l >= d.npt ? d.Jx : d.Jt;
   double r[6];
   for (int i = 0; i < 6; ++i) r[i] = d.gl[6 * (size_t)l + i];
   for (int a = d.lm_start[l]; a < d.lm_start[l + 1]; ++a) {
     const int ka = d.obs_kf[a];
     if (ka < 0) continue;
-    const double* jt = d.Jt + 6 * (size_t)a;
-    const double* jx = d.Jx + 6 * (size_t)a;
+    const double* jt = V + 6 * (size_t)a;
+    const double* jx = U + 6 * (size_t)a;
     double s = 0.0;
     for (int i = 0; i < 6; ++i) s += jt[i] * d.dxc[6 * ka + i];
     s *= d.Wn[2 * (size_t)a];
@@ -348,18 +373,253 @@ __global__ void k_lba_moved(LbaDev d, uint8_t* pt_moved, uint8_t* ls_moved) {
   if (l < d.npt) pt_moved[l] = m; else ls_moved[l - d.npt] = m;
 }
 
+// (g2) `int Hmax` scanned over the first pass's diagonal in index order (:2359-2364): `d > Hmax` compares with the int,
+// `Hmax = fabs(d)` truncates, and a value >= 2^31 converts to INT_MIN (x86-64 cvttsd2si), which the next diagonal entry
+// (>= 0) always replaces, unless it is NaN (both comparisons false).  So the result is INT_MIN when an entry is >= 2^31
+// and no non-NaN entry follows the last such one, else the truncated maximum of the non-NaN entries after the last one
+// >= 2^31 (or of all of them).  One CTA; leaves the value in scal[3].
+__global__ void __launch_bounds__(1024) k_gba_hmax_int(LbaDev d) {
+  __shared__ int last_big, any_after;
+  __shared__ unsigned long long mx;
+  const int tid = threadIdx.x, nk = 6 * d.nkf, np3 = 3 * d.npt;
+  if (tid == 0) { last_big = -1; any_after = 0; mx = 0ull; }
+  __syncthreads();
+  auto diag = [&](int i) -> double {
+    if (i < nk) return d.A[36 * (i / 6) + 7 * (i % 6)];
+    i -= nk;
+    if (i < np3) return d.D[36 * (size_t)(i / 3) + 7 * (i % 3)];
+    i -= np3;
+    return d.D[36 * (size_t)(d.npt + i / 6) + 7 * (i % 6)];
+  };
+  for (int i = tid; i < d.N; i += 1024)
+    if (fabs(diag(i)) >= 2147483648.0) atomicMax(&last_big, i);
+  __syncthreads();
+  for (int i = last_big + 1 + tid; i < d.N; i += 1024) {
+    const double v = fabs(diag(i));
+    if (v == v) {   // NaN: both comparisons false, skipped
+      atomicMax(&mx, (unsigned long long)__double_as_longlong(v));
+      any_after = 1;
+    }
+  }
+  __syncthreads();
+  if (tid == 0)
+    d.scal[3] = last_big >= 0 && !any_after ? -2147483648.0 : trunc(__longlong_as_double((long long)mx));
+}
+
+// ---- blocked LDL^T of the reduced system for n = 6 n_kf > 384 (plf_global_ba) -----------------------------------------
+// Right-looking over 64 x 64 tiles of S (row-major, leading dimension n; only the lower triangle is read), the same
+// factorisation as k_lba_solve: per tile column k, k_gba_diag factors the diagonal tile in shared memory, k_gba_panel
+// solves each tile below it (L_ik = S_ik L_kk^-T D_k^-1, keeping W_ik = L_ik D_k) and flags whether it is exactly zero,
+// and k_gba_update subtracts W_ik L_jk^T from every trailing lower tile (i, j) whose two panel tiles are non-zero, on
+// the FP64 tensor cores.  The substitutions run per tile (k_gba_fwd / k_gba_bwd) and skip the same zero tiles.  Tiles
+// past n are padded with the identity; n_t = ceil(n / 64).
+constexpr int GBA_T = 64, GBA_LD = 65;
+
+__device__ __forceinline__ double gba_S(const LbaDev& d, int r, int c) {   // S[r][c], 0 outside the matrix
+  const int n = 6 * d.nkf;
+  return r < n && c < n ? d.S[(size_t)r * n + c] : 0.0;
+}
+// the factored diagonal tile k: strictly lower L into L[64][GBA_LD] (diagonal = D, 1 in the padding)
+__device__ __forceinline__ void gba_load_lkk(const LbaDev& d, int k, double* L) {
+  const int n = 6 * d.nkf, r0 = GBA_T * k;
+  for (int e = threadIdx.x; e < GBA_T * GBA_T; e += blockDim.x) {
+    const int r = e >> 6, c = e & 63;
+    L[r * GBA_LD + c] = c > r ? 0.0 : (r0 + r < n ? gba_S(d, r0 + r, r0 + c) : (r == c ? 1.0 : 0.0));
+  }
+}
+
+__global__ void __launch_bounds__(256) k_gba_damp(LbaDev d, double lambda) {   // k_lba_solve's prologue
+  const int i = blockIdx.x * 256 + threadIdx.x, n = 6 * d.nkf;
+  if (i < 36 * d.nkf) {
+    const int kf = i / 36, r = (i % 36) / 6, cc = i % 6;
+    double v = d.A[i];
+    if (r == cc) v += lambda * v;
+    d.S[(size_t)(6 * kf + r) * n + 6 * kf + cc] += v;
+  } else if (i < 36 * d.nkf + n) {
+    d.gred[i - 36 * d.nkf] += d.gc[i - 36 * d.nkf];
+  }
+}
+
+__global__ void __launch_bounds__(256) k_gba_diag(LbaDev d, int k) {
+  __shared__ double T[GBA_T * GBA_LD];
+  const int n = 6 * d.nkf, r0 = GBA_T * k, tid = threadIdx.x;
+  for (int e = tid; e < GBA_T * GBA_T; e += 256) {
+    const int r = e >> 6, c = e & 63;
+    T[r * GBA_LD + c] = r0 + r < n && r0 + c < n ? d.S[(size_t)(r0 + r) * n + r0 + c] : (r == c ? 1.0 : 0.0);
+  }
+  __syncthreads();
+  for (int j = 0; j < GBA_T; ++j) {   // as k_lba_solve: after column j, T[i][j] = L_ij, T[j][j] = D_j
+    const double dj = T[j * GBA_LD + j];
+    for (int i = j + 1 + tid; i < GBA_T; i += 256) T[i * GBA_LD + j] /= dj;
+    __syncthreads();
+    const int m = GBA_T - j - 1;
+    for (int t = tid; t < m * m; t += 256) {
+      const int i = j + 1 + t / m, c = j + 1 + t % m;
+      if (c <= i) T[i * GBA_LD + c] -= T[i * GBA_LD + j] * dj * T[c * GBA_LD + j];
+    }
+    __syncthreads();
+  }
+  for (int e = tid; e < GBA_T * GBA_T; e += 256) {
+    const int r = e >> 6, c = e & 63;
+    if (c <= r && r0 + r < n) d.S[(size_t)(r0 + r) * n + r0 + c] = T[r * GBA_LD + c];
+  }
+}
+
+// one CTA per tile row i > k; dynamic shared memory 2 x 64 x GBA_LD doubles
+__global__ void __launch_bounds__(256) k_gba_panel(LbaDev d, double* Wp, uint8_t* nz, int k, int nt) {
+  extern __shared__ double gsm[];
+  double* L = gsm;
+  double* Z = gsm + GBA_T * GBA_LD;
+  const int n = 6 * d.nkf, i = k + 1 + blockIdx.x, r0 = GBA_T * i, c0 = GBA_T * k, tid = threadIdx.x;
+  int any = 0;
+  for (int e = tid; e < GBA_T * GBA_T; e += 256) {
+    const int r = e >> 6, c = e & 63;
+    const double v = gba_S(d, r0 + r, c0 + c);
+    Z[r * GBA_LD + c] = v;
+    any |= v != 0.0;
+  }
+  any = __syncthreads_or(any);
+  if (tid == 0) nz[(size_t)i * nt + k] = (uint8_t)any;
+  if (!any) return;   // L_ik = 0 exactly: nothing to write, nothing to update
+  gba_load_lkk(d, k, L);
+  __syncthreads();
+  // Z = S_ik L_kk^-T, column by column: once column c is final, Z[r][c2] -= Z[r][c] L[c2][c] for c2 > c
+  for (int c = 0; c < GBA_T - 1; ++c) {
+    const int m = GBA_T - 1 - c;
+    for (int t = tid; t < GBA_T * m; t += 256) {
+      const int r = t / m, c2 = c + 1 + t % m;
+      Z[r * GBA_LD + c2] -= Z[r * GBA_LD + c] * L[c2 * GBA_LD + c];
+    }
+    __syncthreads();
+  }
+  for (int e = tid; e < GBA_T * GBA_T; e += 256) {
+    const int r = e >> 6, c = e & 63;
+    const double z = Z[r * GBA_LD + c];
+    Wp[((size_t)i * GBA_T + r) * GBA_T + c] = z;
+    if (r0 + r < n && c0 + c < n) d.S[(size_t)(r0 + r) * n + c0 + c] = z / L[c * GBA_LD + c];
+  }
+}
+
+__device__ __forceinline__ void gba_dmma(double& c0, double& c1, double& c2, double& c3, double a0, double a1, double b0) {
+  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+               : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3) : "d"(a0), "d"(a1), "d"(b0));
+}
+
+// S_ij -= W_ik L_jk^T for the trailing lower tiles k < j <= i, one CTA per tile (blockIdx.x enumerates (i, j) row by
+// row).  8 warps; warp w owns rows 16 (w / 2) .. +16 and columns 32 (w % 2) .. +32 of the tile (4 m16n8 accumulators).
+constexpr int GBA_KC = 32, GBA_SLD = 36;   // k chunk; shared row stride (conflict-free fragment loads per half warp)
+__global__ void __launch_bounds__(256) k_gba_update(LbaDev d, const double* Wp, const uint8_t* nz, int k, int nt) {
+  const int t = blockIdx.x;
+  int a = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+  while ((a + 1) * (a + 2) / 2 <= t) ++a;
+  while (a * (a + 1) / 2 > t) --a;
+  const int i = k + 1 + a, j = k + 1 + (t - a * (a + 1) / 2);
+  if (!nz[(size_t)i * nt + k] || !nz[(size_t)j * nt + k]) return;
+  __shared__ double As[GBA_T * GBA_SLD], Bs[GBA_T * GBA_SLD];
+  const int n = 6 * d.nkf, tid = threadIdx.x, lane = tid & 31, w = tid >> 5, gid = lane >> 2, tig = lane & 3;
+  const int wr = 16 * (w >> 1), wc = 32 * (w & 1);
+  double acc[4][4];
+  for (int q = 0; q < 4; ++q)
+    for (int e = 0; e < 4; ++e) acc[q][e] = 0.0;
+  for (int kc = 0; kc < GBA_T; kc += GBA_KC) {
+    for (int e = tid; e < GBA_T * GBA_KC; e += 256) {
+      const int r = e / GBA_KC, c = e % GBA_KC;
+      As[r * GBA_SLD + c] = Wp[((size_t)i * GBA_T + r) * GBA_T + kc + c];
+      Bs[r * GBA_SLD + c] = gba_S(d, GBA_T * j + r, GBA_T * k + kc + c);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int ks = 0; ks < GBA_KC; ks += 4) {
+      const double a0 = As[(wr + gid) * GBA_SLD + ks + tig], a1 = As[(wr + gid + 8) * GBA_SLD + ks + tig];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const double b0 = Bs[(wc + 8 * q + gid) * GBA_SLD + ks + tig];
+        gba_dmma(acc[q][0], acc[q][1], acc[q][2], acc[q][3], a0, a1, b0);
+      }
+    }
+    __syncthreads();
+  }
+  for (int q = 0; q < 4; ++q)
+    for (int e = 0; e < 4; ++e) {
+      const int r = GBA_T * i + wr + gid + (e >> 1) * 8, c = GBA_T * j + wc + 8 * q + 2 * tig + (e & 1);
+      if (r < n && c < n) d.S[(size_t)r * n + c] -= acc[q][e];
+    }
+}
+
+// forward substitution step k: every CTA solves y_k = L_kk^-1 g_k (64 threads, in place of g's tile), CTA 0 stores it in
+// dxc, CTA b > 0 subtracts L_ik y_k from g_i (i = k + b) when that tile is non-zero
+__global__ void __launch_bounds__(256) k_gba_fwd(LbaDev d, const uint8_t* nz, int k, int nt) {
+  __shared__ double L[GBA_T * GBA_LD], y[GBA_T];
+  const int n = 6 * d.nkf, b = blockIdx.x, i = k + b, r0 = GBA_T * k, tid = threadIdx.x;
+  if (b > 0 && !nz[(size_t)i * nt + k]) return;
+  gba_load_lkk(d, k, L);
+  if (tid < GBA_T) y[tid] = r0 + tid < n ? d.gred[r0 + tid] : 0.0;
+  __syncthreads();
+  for (int c = 0; c < GBA_T - 1; ++c) {
+    if (tid > c && tid < GBA_T) y[tid] -= L[tid * GBA_LD + c] * y[c];
+    __syncthreads();
+  }
+  if (b == 0) {
+    if (tid < GBA_T && r0 + tid < n) d.dxc[r0 + tid] = y[tid];
+    return;
+  }
+  const int lane = tid & 31, w = tid >> 5;
+  for (int rr = 0; rr < 8; ++rr) {   // warp w: rows 8 w .. 8 w + 7 of tile i
+    const int r = GBA_T * i + 8 * w + rr;
+    double s = gba_S(d, r, r0 + lane) * y[lane] + gba_S(d, r, r0 + 32 + lane) * y[32 + lane];
+    for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, off);
+    if (lane == 0 && r < n) d.gred[r] -= s;
+  }
+}
+
+__global__ void k_gba_dscale(LbaDev d) {   // z = y / D
+  const int i = blockIdx.x * blockDim.x + threadIdx.x, n = 6 * d.nkf;
+  if (i < n) d.gred[i] = d.dxc[i] / d.S[(size_t)i * n + i];
+}
+
+// backward substitution step k (k = n_t - 1 .. 0): every CTA solves x_k = L_kk^-T z_k, CTA 0 stores it in dxc and DX,
+// CTA b > 0 subtracts L_kj^T x_k from z_j (j = b - 1) when that tile is non-zero
+__global__ void __launch_bounds__(256) k_gba_bwd(LbaDev d, const uint8_t* nz, int k, int nt) {
+  __shared__ double L[GBA_T * GBA_LD], x[GBA_T], part[4][GBA_T];
+  const int n = 6 * d.nkf, b = blockIdx.x, r0 = GBA_T * k, tid = threadIdx.x;
+  if (b > 0 && !nz[(size_t)k * nt + (b - 1)]) return;
+  gba_load_lkk(d, k, L);
+  if (tid < GBA_T) x[tid] = r0 + tid < n ? d.gred[r0 + tid] : 0.0;
+  __syncthreads();
+  for (int c = GBA_T - 1; c > 0; --c) {
+    if (tid < c) x[tid] -= L[c * GBA_LD + tid] * x[c];
+    __syncthreads();
+  }
+  if (b == 0) {
+    if (tid < GBA_T && r0 + tid < n) { d.dxc[r0 + tid] = x[tid]; d.DX[r0 + tid] = x[tid]; }
+    return;
+  }
+  const int j = b - 1, c = tid & 63, rq = tid >> 6;
+  double s = 0.0;
+  for (int r = 16 * rq; r < 16 * rq + 16; ++r) s += gba_S(d, r0 + r, GBA_T * j + c) * x[r];
+  part[rq][c] = s;
+  __syncthreads();
+  if (tid < GBA_T && GBA_T * j + tid < n) d.gred[GBA_T * j + tid] -= ((part[0][tid] + part[1][tid]) + part[2][tid]) + part[3][tid];
+}
+
 static size_t lba_al(size_t x) { return (x + 255) & ~size_t(255); }
 
-extern "C" plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out) {
+// The host loop of both routines: the reference's control flow, on the device kernels above.  `global` selects
+// levMarquardtOptimizationGBA (:2101-2699) over levMarquardtOptimizationLBA (:1332-1989): its quirk set, its error
+// normalisation in the LM iterations, up to 4096 keyframes (the blocked factorisation beyond n = 384) and a landmark
+// without observations refused.
+static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out, bool global) {
+  const char* fn = global ? "plf_global_ba" : "plf_local_ba";
   if (!ctx || !opts || !p || p->n_kf < 0 || p->n_pt < 0 || p->n_ls < 0 || p->n_pt_obs < 0 || p->n_ls_obs < 0 || p->n_fixed < 0)
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_local_ba: bad arguments");
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", fn);
   const int nkf = p->n_kf, npt = p->n_pt, nls = p->n_ls, npo = p->n_pt_obs, nlo = p->n_ls_obs, nobs = npo + nlo, nlm = npt + nls;
   const int N = 6 * nkf + 3 * npt + 6 * nls, n = 6 * nkf;
-  if (nobs == 0 || N == 0) return plf_fail(ctx, PLF_ERR_INVALID, "plf_local_ba: empty problem (the reference returns -1, :1324-1328)");
-  if (nkf > 64) return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_local_ba: %d local keyframes (limit 64)", nkf);
+  if (nobs == 0 || N == 0) return plf_fail(ctx, PLF_ERR_INVALID, "%s: empty problem (the reference returns -1, :1324-1328)", fn);
+  const int kf_cap = global ? 4096 : 64;
+  if (nkf > kf_cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: %d keyframes (limit %d)", fn, nkf, kf_cap);
   if ((nkf && !p->kf_pose) || (npt && !p->pt) || (nls && !p->ls) || (npo && (!p->pt_obs_lm || !p->pt_obs_kf || !p->pt_obs_xy)) ||
       (nlo && (!p->ls_obs_lm || !p->ls_obs_kf || !p->ls_obs_le)) || (p->n_fixed && !p->fixed_T))
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_local_ba: null array");
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: null array", fn);
   // observations are grouped per landmark in non-decreasing landmark order (how the reference builds its lists, :1249-1277)
   std::vector<int> lm_start(nlm + 1, 0), h_lm(nobs), h_kf(nobs);
   std::vector<double> h_z((size_t)nobs * 3, 0.0);
@@ -368,16 +628,22 @@ extern "C" plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const
     const int lm = is_line ? p->ls_obs_lm[k - npo] : p->pt_obs_lm[k], kf = is_line ? p->ls_obs_kf[k - npo] : p->pt_obs_kf[k];
     const int lim = is_line ? nls : npt;
     if (lm < 0 || lm >= lim || kf >= nkf || kf < -p->n_fixed)
-      return plf_fail(ctx, PLF_ERR_INVALID, "plf_local_ba: observation %d refers to landmark %d / keyframe %d out of range", k, lm, kf);
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: observation %d refers to landmark %d / keyframe %d out of range", fn, k, lm, kf);
     const int prev = k == 0 || k == npo ? -1 : (is_line ? p->ls_obs_lm[k - npo - 1] : p->pt_obs_lm[k - 1]);
-    if (lm < prev) return plf_fail(ctx, PLF_ERR_INVALID, "plf_local_ba: observations must be grouped by landmark in ascending order");
+    if (lm < prev) return plf_fail(ctx, PLF_ERR_INVALID, "%s: observations must be grouped by landmark in ascending order", fn);
     h_lm[k] = lm; h_kf[k] = kf;
     lm_start[(is_line ? npt : 0) + lm + 1]++;
     if (is_line) for (int c = 0; c < 3; ++c) h_z[3 * (size_t)k + c] = p->ls_obs_le[3 * (size_t)(k - npo) + c];
     else { h_z[3 * (size_t)k] = p->pt_obs_xy[2 * (size_t)k]; h_z[3 * (size_t)k + 1] = p->pt_obs_xy[2 * (size_t)k + 1]; }
   }
+  if (global)   // its landmark block would be zero: the reference would factor a zero pivot
+    for (int l = 0; l < nlm; ++l)
+      if (!lm_start[l + 1])
+        return plf_fail(ctx, PLF_ERR_INVALID, "%s: %s landmark %d has no observation", fn, l < npt ? "point" : "line", l < npt ? l : l - npt);
   for (int l = 0; l < nlm; ++l) lm_start[l + 1] += lm_start[l];
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  const bool blocked = n > 384;   // k_lba_solve (one CTA, one launch) up to 64 keyframes, the tiled LDL^T beyond
+  const int nt = (n + GBA_T - 1) / GBA_T;
   // one scratch block
   size_t off = 0;
   auto take = [&](size_t bytes) { const size_t o = off; off += lba_al(bytes); return o; };
@@ -387,8 +653,9 @@ extern "C" plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const
                oJt = take((size_t)nobs * 48), oJx = take((size_t)nobs * 48), oWn = take((size_t)nobs * 16),
                oD = take((size_t)std::max(nlm, 1) * 288), oGl = take((size_t)std::max(nlm, 1) * 48), oDi = take((size_t)std::max(nlm, 1) * 288),
                oA = take((size_t)std::max(nkf, 1) * 288), oGc = take((size_t)std::max(nkf, 1) * 48),
-               oS = take((size_t)std::max(n * n, 1) * 8), oGr = take((size_t)std::max(n, 1) * 8), oDc = take((size_t)std::max(n, 1) * 8),
-               oDX = take((size_t)N * 8), oSc = take(64), oPm = take((size_t)std::max(npt, 1)), oLmv = take((size_t)std::max(nls, 1));
+               oS = take(std::max((size_t)n * n, (size_t)1) * 8), oGr = take((size_t)std::max(n, 1) * 8), oDc = take((size_t)std::max(n, 1) * 8),
+               oDX = take((size_t)N * 8), oSc = take(64), oPm = take((size_t)std::max(npt, 1)), oLmv = take((size_t)std::max(nls, 1)),
+               oWp = take(blocked ? (size_t)nt * GBA_T * GBA_T * 8 : 8), oNz = take(blocked ? (size_t)nt * nt : 1);
   uint8_t* base = (uint8_t*)plf_scratch(ctx, 10, off);
   if (!base) return PLF_ERR_CUDA;
   LbaDev d;
@@ -404,6 +671,7 @@ extern "C" plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const
   d.S = (double*)(base + oS); d.gred = (double*)(base + oGr); d.dxc = (double*)(base + oDc);
   d.DX = (double*)(base + oDX); d.scal = (double*)(base + oSc);
   uint8_t* dPm = base + oPm; uint8_t* dLmv = base + oLmv;
+  double* dWp = (double*)(base + oWp); uint8_t* dNz = base + oNz;
   cudaStream_t cs = ctx->stream;
   ctx->cur = cs;
   std::vector<double> hX(N);
@@ -420,14 +688,14 @@ extern "C" plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const
   k_lba_prep<<<(std::max(nkf, p->n_fixed) + 63) / 64 + 1, 64, 0, cs>>>(d, dFT, dFTi, p->n_fixed);
   PLF_LAUNCH_CHECK(ctx);
   const LbaCam cam = {ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy};
-  const int q = opts->ref_quirks ? 1 : 0;
+  const int q = opts->ref_quirks ? (global ? BAQ_GBA : BAQ_LBA) : 0;
   double lambda = opts->lambda;
-  double h_scal[3];
+  double h_scal[4];
   // builds the normal equations of `mode` and leaves err / Hmax in scal
   auto build = [&](int mode) -> plf_status {
     PLF_CUDA(ctx, cudaMemsetAsync(d.A, 0, (size_t)std::max(nkf, 1) * 288, cs));
     PLF_CUDA(ctx, cudaMemsetAsync(d.gc, 0, (size_t)std::max(nkf, 1) * 48, cs));
-    PLF_CUDA(ctx, cudaMemsetAsync(d.S, 0, (size_t)std::max(n * n, 1) * 8, cs));
+    PLF_CUDA(ctx, cudaMemsetAsync(d.S, 0, std::max((size_t)n * n, (size_t)1) * 8, cs));
     PLF_CUDA(ctx, cudaMemsetAsync(d.gred, 0, (size_t)std::max(n, 1) * 8, cs));
     PLF_CUDA(ctx, cudaMemsetAsync(d.scal, 0, 64, cs));
     k_lba_rows<<<(nobs + 127) / 128, 128, 0, cs>>>(d, cam, mode, q, opts->homog_th);
@@ -438,49 +706,88 @@ extern "C" plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const
       k_lba_kf_diagmax<<<(6 * nkf + 63) / 64, 64, 0, cs>>>(d);
       PLF_LAUNCH_CHECK(ctx);
     }
-    PLF_CUDA(ctx, cudaMemcpyAsync(h_scal, d.scal, 24, cudaMemcpyDeviceToHost, cs));
+    if (mode == 0 && (q & BAQ_HMAX_INT)) {
+      k_gba_hmax_int<<<1, 1024, 0, cs>>>(d);
+      PLF_LAUNCH_CHECK(ctx);
+    }
+    PLF_CUDA(ctx, cudaMemcpyAsync(h_scal, d.scal, 32, cudaMemcpyDeviceToHost, cs));
     PLF_CUDA(ctx, cudaStreamSynchronize(cs));
     return PLF_OK;
   };
-  // solves the damped system and (optionally) applies the step; leaves |DX| in *dx_norm
-  auto solve = [&](int apply, double* dx_norm) -> plf_status {
-    k_lba_lm_schur<<<(nlm + 127) / 128, 128, 0, cs>>>(d, lambda);
+  // the blocked factorisation and the two substitutions of S dx_c = g_red (see k_gba_diag)
+  auto solve_blocked = [&]() -> plf_status {
+    k_gba_damp<<<(36 * nkf + n + 255) / 256, 256, 0, cs>>>(d, lambda);
     PLF_LAUNCH_CHECK(ctx);
-    if (nkf) {
+    const int smem = 2 * GBA_T * GBA_LD * 8;
+    PLF_CUDA(ctx, cudaFuncSetAttribute(k_gba_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    for (int k = 0; k < nt; ++k) {
+      k_gba_diag<<<1, 256, 0, cs>>>(d, k);
+      PLF_LAUNCH_CHECK(ctx);
+      const int m = nt - k - 1;
+      if (!m) break;
+      k_gba_panel<<<m, 256, smem, cs>>>(d, dWp, dNz, k, nt);
+      PLF_LAUNCH_CHECK(ctx);
+      k_gba_update<<<m * (m + 1) / 2, 256, 0, cs>>>(d, dWp, dNz, k, nt);
+      PLF_LAUNCH_CHECK(ctx);
+    }
+    for (int k = 0; k < nt; ++k) {
+      k_gba_fwd<<<nt - k, 256, 0, cs>>>(d, dNz, k, nt);
+      PLF_LAUNCH_CHECK(ctx);
+    }
+    k_gba_dscale<<<(n + 255) / 256, 256, 0, cs>>>(d);
+    PLF_LAUNCH_CHECK(ctx);
+    for (int k = nt - 1; k >= 0; --k) {
+      k_gba_bwd<<<k + 1, 256, 0, cs>>>(d, dNz, k, nt);
+      PLF_LAUNCH_CHECK(ctx);
+    }
+    return PLF_OK;
+  };
+  // solves the damped system and (optionally) applies the step; leaves |DX| in *dx_norm.  swap: (g6), first pass only
+  auto solve = [&](int apply, int swap, double* dx_norm) -> plf_status {
+    k_lba_lm_schur<<<(nlm + 127) / 128, 128, 0, cs>>>(d, lambda, swap);
+    PLF_LAUNCH_CHECK(ctx);
+    if (blocked) {
+      plf_status s = solve_blocked();
+      if (s) return s;
+    } else if (nkf) {
       k_lba_solve<<<1, 256, 0, cs>>>(d, lambda);
       PLF_LAUNCH_CHECK(ctx);
     }
-    k_lba_backsub<<<(nlm + 127) / 128, 128, 0, cs>>>(d);
+    k_lba_backsub<<<(nlm + 127) / 128, 128, 0, cs>>>(d, swap);
     PLF_LAUNCH_CHECK(ctx);
     k_lba_apply<<<(nkf + (N - 6 * nkf) + 127) / 128, 128, 0, cs>>>(d, apply);
     PLF_LAUNCH_CHECK(ctx);
-    PLF_CUDA(ctx, cudaMemcpyAsync(h_scal, d.scal, 24, cudaMemcpyDeviceToHost, cs));
+    PLF_CUDA(ctx, cudaMemcpyAsync(h_scal, d.scal, 32, cudaMemcpyDeviceToHost, cs));
     PLF_CUDA(ctx, cudaStreamSynchronize(cs));
     *dx_norm = sqrt(h_scal[1]);
     return PLF_OK;
   };
   plf_status st;
-  // ---- first pass on the map's values (:1352-1541), lambda *= Hmax (:1543-1550), first step applied unconditionally
+  // ---- first pass on the map's values (LBA :1352-1541, GBA :2117-2356), lambda *= Hmax (:1543-1550, :2358-2365), first
+  // step applied unconditionally
   if ((st = build(0))) return st;
   double err = h_scal[0];
   volatile int never_incremented = 0;   // Npt_obs + Nls_obs of the reference
-  if (q) err /= (double)never_incremented;   // (q1) :1541
+  if (q & BAQ_FIRST_ERR0) err /= (double)never_incremented;   // (q1) :1541, (g1) :2356
   else err /= (double)nobs;
   double Hmax;
-  { unsigned long long bits; memcpy(&bits, &h_scal[2], 8); memcpy(&Hmax, &bits, 8); }
+  if (q & BAQ_HMAX_INT) Hmax = h_scal[3];   // (g2)
+  else { unsigned long long bits; memcpy(&bits, &h_scal[2], 8); memcpy(&Hmax, &bits, 8); }
   lambda *= Hmax;
   double dxn = 0.0;
-  if ((st = solve(1, &dxn))) return st;
+  if ((st = solve(1, (q & BAQ_SWAP_COUPLING) ? 1 : 0, &dxn))) return st;
   double err_prev = err;
   int iters;
   for (iters = 1; iters < opts->max_iters; ++iters) {
     if ((st = build(1))) return st;
-    err = h_scal[0] / (double)(npt + nls);                                                       // :1773
-    if (fabs(err - err_prev) < opts->min_error_change || err < opts->min_error) break;           // :1775
+    if (q & BAQ_ITER_ERR0) err = h_scal[0] / (double)never_incremented;                           // (g3) :2635
+    else if (global) err = h_scal[0] / (double)nobs;
+    else err = h_scal[0] / (double)(npt + nls);                                                  // :1773
+    if (fabs(err - err_prev) < opts->min_error_change || err < opts->min_error) break;           // :1775, :2637
     const bool grew = err > err_prev;
-    if ((st = solve(grew ? 0 : 1, &dxn))) return st;                                             // :1777-1803
+    if ((st = solve(grew ? 0 : 1, 0, &dxn))) return st;                                          // :1777-1803, :2639-2665
     if (grew) lambda /= opts->lambda_k; else lambda *= opts->lambda_k;
-    if (dxn < opts->min_error_change) break;                                                     // :1805
+    if (dxn < opts->min_error_change) break;                                                     // :1805, :2667
     err_prev = err;
   }
   k_lba_moved<<<(nlm + 127) / 128, 128, 0, cs>>>(d, dPm, dLmv);
@@ -494,4 +801,12 @@ extern "C" plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const
   for (int i = 0; i < 6 * nls; ++i) p->ls[i] = hX[6 * nkf + 3 * npt + i];
   if (out) { out->iters = iters; out->err = err; out->lambda = lambda; }
   return PLF_OK;
+}
+
+extern "C" plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out) {
+  return ba_run(ctx, opts, p, out, false);
+}
+
+extern "C" plf_status plf_global_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out) {
+  return ba_run(ctx, opts, p, out, true);
 }

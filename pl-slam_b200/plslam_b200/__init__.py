@@ -265,6 +265,7 @@ KITTI_CAMERA = dict(width=1242, height=375, fx=718.856, fy=718.856, cx=607.1928,
                     b=0.537165719)  # config/dataset_params/kitti00-02.yaml:2-10
 EUROC_CAMERA = dict(width=752, height=480, fx=458.654, fy=457.296, cx=367.215, cy=248.375,
                     b=0.110077842)  # config/dataset_params/euroc_params.yaml:2,8 (pre-rectified)
+DBL_EPSILON = float(np.finfo(np.float64).eps)   # numeric_limits<double>::epsilon(), the GBA stop thresholds
 
 
 def _u8(a, shape_tail=None):
@@ -484,6 +485,18 @@ class Frontend:
                  min_error_change=1e-7, ref_quirks=1):
         """MapHandler::levMarquardtOptimizationLBA on the device (plf_local_ba; src/mapHandler.cpp:1332-1989).
         prob: dict as produced by synth.lba_problem (kf_pose, pt, ls, fixed_T, pt_obs_*, ls_obs_*)."""
+        return self._bundle_adjust("plf_local_ba", prob, lambda_, lambda_k, max_iters, homog_th, min_error,
+                                   min_error_change, ref_quirks)
+
+    def global_ba(self, prob, lambda_=1e-5, lambda_k=10.0, max_iters=15, homog_th=1e-7, min_error=DBL_EPSILON,
+                  min_error_change=DBL_EPSILON, ref_quirks=1):
+        """MapHandler::levMarquardtOptimizationGBA on the device (plf_global_ba; src/mapHandler.cpp:2101-2699): every
+        keyframe but keyframe 0 and every landmark.  prob: dict as produced by synth.gba_problem (plf_local_ba's layout;
+        fixed_T holds keyframe 0).  The stop thresholds default to the reference's DBL_EPSILON literals (:2637, :2667)."""
+        return self._bundle_adjust("plf_global_ba", prob, lambda_, lambda_k, max_iters, homog_th, min_error,
+                                   min_error_change, ref_quirks)
+
+    def _bundle_adjust(self, fn, prob, lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, ref_quirks):
         f64 = lambda a, c: np.ascontiguousarray(a, np.float64).reshape(-1, c).copy()
         i32 = lambda a: np.ascontiguousarray(a, np.int32).ravel().copy()
         kf, pt, ls = f64(prob["kf_pose"], 6), f64(prob["pt"], 3), f64(prob["ls"], 6)
@@ -496,7 +509,7 @@ class Frontend:
                             ad(po_xy), len(lo_lm), ad(lo_lm), ad(lo_kf), ad(lo_le), ad(pm), ad(lm))
         o = plf_lba_opts(lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, int(ref_quirks))
         res = plf_lba_result()
-        self._check(self.lib.plf_local_ba(self._ctx, C.byref(o), C.byref(p), C.byref(res)), "plf_local_ba")
+        self._check(getattr(self.lib, fn)(self._ctx, C.byref(o), C.byref(p), C.byref(res)), fn)
         return dict(kf_pose=kf, pt=pt, ls=ls, pt_moved=pm[:len(pt)].astype(bool), ls_moved=lm[:len(ls)].astype(bool),
                     iters=res.iters, err=res.err, lambda_=res.lambda_)
 

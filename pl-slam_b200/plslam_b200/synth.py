@@ -280,3 +280,88 @@ def lba_problem(cam, n_kf=4, n_fixed=2, n_pt=120, n_ls=40, seed=0, px_noise=0.3,
                 pt_obs_lm=np.array(po_lm, np.int32), pt_obs_kf=np.array(po_kf, np.int32), pt_obs_xy=np.array(po_xy).reshape(-1, 2),
                 ls_obs_lm=np.array(lo_lm, np.int32), ls_obs_kf=np.array(lo_kf, np.int32), ls_obs_le=np.array(lo_le).reshape(-1, 3),
                 truth=dict(kf_pose=kf_true, pt=pt, ls=ls))
+
+
+def gba_problem(cam, n_kf=64, pts_per_kf=100, ls_per_kf=15, loop=True, seed=0, n_fixed=1, n_views=3, px_noise=0.3,
+                pose_noise=0.01, lm_noise=0.02):
+    """A whole map as MapHandler::globalBundleAdjustment assembles it (src/mapHandler.cpp:1995-2090): n_fixed fixed
+    keyframes (keyframe 0 and any others held fixed) followed by n_kf optimised ones, in kf_idx order, on a circle of
+    0.8 m steps (a full turn when there are 40 keyframes or more) with the camera facing the same way throughout.  Each keyframe creates pts_per_kf points and
+    ls_per_kf lines in front of it; each landmark is observed by its creator and by the next n_views - 1 keyframes that
+    see it, so the reduced system is banded.  With `loop`, the last n_views keyframes also re-observe the landmarks of
+    the first ones where they see them (the loop closure).  Observations are grouped per landmark in ascending order;
+    every landmark is observed (by its creator).  Vectorised: 4096 keyframes generate in seconds."""
+    rng = np.random.default_rng(seed)
+    n_tot = n_kf + n_fixed
+    step = 0.8
+    dth = 2.0 * math.pi / max(n_tot, 40)
+    R = step / dth
+    th = dth * np.arange(n_tot)
+    # one heading throughout, 0.6 rad off the world axes: rotations near 0 or pi are where logmap_se3's acos loses digits
+    yaw = 0.6 + 0.002 * rng.standard_normal(n_tot)
+    c, s_ = np.cos(yaw), np.sin(yaw)
+    Tw = np.zeros((n_tot, 4, 4))
+    Tw[:, :3, 0] = np.stack([c, np.zeros_like(c), -s_], 1)       # right
+    Tw[:, :3, 1] = [0.0, 1.0, 0.0]                               # down
+    Tw[:, :3, 2] = np.stack([s_, np.zeros_like(c), c], 1)        # forward
+    Tw[:, :3, 3] = np.stack([R * (1 - np.cos(th)), 0.05 * rng.standard_normal(n_tot), R * np.sin(th)], 1)
+    Tw[:, 3, 3] = 1.0
+    Ti = np.linalg.inv(Tw)
+
+    def in_view(creators, n):
+        z = rng.uniform(4.0, 20.0, n)
+        u = rng.uniform(40, cam["width"] - 40, n); v = rng.uniform(30, cam["height"] - 30, n)
+        Pc = np.stack([(u - cam["cx"]) * z / cam["fx"], (v - cam["cy"]) * z / cam["fy"], z], 1)
+        return np.einsum("nij,nj->ni", Tw[creators, :3, :3], Pc) + Tw[creators, :3, 3]
+
+    def project(t, Pw):   # t: [m] observer indices, Pw: [m, 3]
+        Pc = np.einsum("nij,nj->ni", Ti[t, :3, :3], Pw) + Ti[t, :3, 3]
+        with np.errstate(divide="ignore", invalid="ignore"):
+            uv = np.stack([cam["cx"] + cam["fx"] * Pc[:, 0] / Pc[:, 2], cam["cy"] + cam["fy"] * Pc[:, 1] / Pc[:, 2]], 1)
+        ok = (Pc[:, 2] > 1.0) & (uv[:, 0] > 0) & (uv[:, 0] < cam["width"]) & (uv[:, 1] > 0) & (uv[:, 1] < cam["height"])
+        return uv, ok
+
+    def observers(creators):   # [n, 2 n_views] candidate observer per landmark, -1 where none, creator first
+        o = np.arange(n_views)
+        fwd = creators[:, None] + o[None, :]
+        fwd[fwd >= n_tot] = -1
+        back = np.full_like(fwd, -1)
+        if loop:
+            b = (n_tot - 1 - o)[None, :].repeat(len(creators), 0)
+            ok = (creators[:, None] < n_views) & (b > creators[:, None] + n_views - 1)
+            back[ok] = b[ok]
+        return np.concatenate([fwd, back], 1)
+
+    def observe(cand, ends):   # -> (landmark index, observer, projections of each end point) of the kept candidates
+        lm, col = np.nonzero(cand >= 0)
+        t = cand[lm, col]
+        uvs, ok = [], col == 0
+        keep = np.ones(len(t), bool)
+        for P in ends:
+            uv, vis = project(t, P[lm])
+            uvs.append(uv); keep &= vis
+        keep |= ok
+        return lm[keep], t[keep], [uv[keep] for uv in uvs]
+
+    kf_of = lambda t: np.where(t < n_fixed, -1 - t, t - n_fixed).astype(np.int32)
+    pc = np.repeat(np.arange(n_tot), pts_per_kf)
+    pt = in_view(pc, len(pc))
+    plm, pt_t, (puv,) = observe(observers(pc), [pt])
+    lc = np.repeat(np.arange(n_tot), ls_per_kf)
+    ls = np.concatenate([in_view(lc, len(lc)), in_view(lc, len(lc))], 1)
+    llm, ls_t, (suv, euv) = observe(observers(lc), [ls[:, :3], ls[:, 3:]])
+    sp = np.concatenate([suv + px_noise * rng.standard_normal(suv.shape), np.ones((len(suv), 1))], 1)
+    ep = np.concatenate([euv + px_noise * rng.standard_normal(euv.shape), np.ones((len(euv), 1))], 1)
+    le = np.cross(sp, ep)
+    le /= np.hypot(le[:, 0], le[:, 1])[:, None]
+    kf_true = np.stack([_logmap_se3(T) for T in Tw[n_fixed:]]) if n_kf else np.zeros((0, 6))
+    # the initial poses are perturbed in each keyframe's own frame: noise added to the se(3) vector of a keyframe far
+    # from the origin would move it by |t| times the rotation noise, metres on a long map
+    noise = pose_noise * rng.standard_normal(kf_true.shape)
+    kf_init = np.stack([_logmap_se3(T @ expmap_se3(e)) for T, e in zip(Tw[n_fixed:], noise)]) if n_kf else np.zeros((0, 6))
+    return dict(kf_pose=kf_init,
+                pt=pt + lm_noise * rng.standard_normal(pt.shape), ls=ls + lm_noise * rng.standard_normal(ls.shape),
+                fixed_T=Tw[:n_fixed].copy(),
+                pt_obs_lm=plm.astype(np.int32), pt_obs_kf=kf_of(pt_t), pt_obs_xy=puv + px_noise * rng.standard_normal(puv.shape),
+                ls_obs_lm=llm.astype(np.int32), ls_obs_kf=kf_of(ls_t), ls_obs_le=le,
+                truth=dict(kf_pose=kf_true, pt=pt, ls=ls))
