@@ -25,9 +25,9 @@
 //                    bin == OpenCV's ordered_points
 //   k_lsd_grow       region growing.  The algorithm is a sequential greedy partition (each accepted pixel updates the
 //                    region angle that the next test uses, and regions compete through the `used` map), so it is run by
-//                    ONE WARP PER IMAGE with thousands of images in flight: lanes 0..8 hold the 3x3 neighbourhood
-//                    records of the current region point (fetched two queue entries ahead, L1-resident through a
-//                    look-ahead prefetch), the alignment tests run lane-parallel in the reference order, and the
+//                    ONE WARP PER IMAGE with thousands of images in flight: lanes 9e..9e+8 hold the 3x3 neighbourhood
+//                    records of queue entry r+e, e < 3 (fetched one round ahead, L1-resident through a look-ahead
+//                    prefetch), the alignment tests run lane-parallel in the reference order, and the
 //                    region angle is only evaluated when a decision depends on it (see the kernel's comment; bit-exact).
 //                    The (cosf, sinf) a member adds to the region's sums comes from a table keyed by the record's index,
 //                    staged in a shared-memory ring by cp.async and added, in the reference's order, when the sums are read.
@@ -561,10 +561,14 @@ static_assert(sizeof(LsdPix) == LSD_REC_BYTES, "LSD record size");
 // One warp per image.  Pixels are addressed by their linear index i = y*W + x; the 8 neighbours are i + {-W-1 .. W+1}.
 // No bounds tests are needed: the last column and last row of the map are always NOTDEF (ll_angle), so x-1 / x+1 wrap
 // onto NOTDEF pixels, y+1 stays inside, and a guard of W+1 permanently-NOTDEF records precedes pixel 0 for y-1.
-// Per region point: lanes 0..8 hold the 8-byte records of the 3x3 neighbourhood, fetched two queue entries AHEAD; cells
-// accepted meanwhile are patched to "used" in the prefetched registers.  The neighbours are decided lane-parallel and
-// re-decided after every acceptance, which reproduces the reference's sequential semantics (each test sees the region
-// angle left by the previous acceptance).
+// Three queue entries per round: lane 9e + kk holds the 8-byte record of neighbour kk (row-major 3x3) of entry r + e, for
+// the E = min(3, nreg - r) entries that exist when the round starts; cells accepted in the round join the queue for a
+// later round.  Lane order is (entry, neighbour), the reference's order of tests, and the candidates are re-decided after
+// every acceptance, which reproduces the reference's sequential semantics (each test sees the region angle and the used
+// state left by the acceptances before it).  Two entries of a round share neighbours: accepting a cell also decides the
+// lanes that hold it for a later entry (match.any mask).  The next round's records are loaded one round ahead - at the
+// round's start for the entries that exist, at its acceptance for an entry added during the round - and a cell accepted
+// after its record was loaded is patched to "used" in the look-ahead registers.
 //
 // Region sums off the decision chain.  A member adds (cosf, sinf) of its angle to the sums S; that pair is lut_cs[li].
 // No acceptance decision reads S (see below: only an evaluation of the region angle and the region's end do), so an
@@ -606,7 +610,8 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
   asm volatile("" : "+l"(regions));
   asm volatile("" : "+r"(qs));
   const int ns = nseeds[im];
-  const int kk = lane < 9 ? lane : 4;                  // neighbour slot served by this lane (lanes >= 9 idle on the centre)
+  const int grp = lane < 27 ? lane / 9 : 3;           // entry of the round served by this lane (lanes 27..31 idle)
+  const int kk = lane < 27 ? lane - 9 * grp : 4;      // and the neighbour slot (row-major 3x3: the reference order)
   const int noff = (kk / 3 - 1) * W + (kk % 3 - 1);   // linear offset of that neighbour (row-major 3x3: reference order)
   // look-ahead window fetched into L1/L2 whenever a pixel joins the region: 7 rows x 8 records around it (the cells the
   // next two breadth-first layers will examine), one address per lane
@@ -654,11 +659,13 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
       lsd_prefetch(pb + (long long)((int)sidx + poff) * LSD_REC_BYTES);
       __syncwarp();
       uint32_t nreg = 1;
-      // neighbourhood records of queue entries r+1 (pf1) and r+2 (pf2), fetched while earlier entries are processed;
-      // a cell accepted meanwhile is patched to "used" in both prefetched copies (i < pmin: nothing fetched)
-      LsdRec pf1, pf2;
-      pf1.a = pf2.a = LSD_NOTDEF_F; pf1.li = pf2.li = 0u;
-      int i1 = pmin - 1, i2 = pmin - 1;
+      // records of the next round's entries on their lanes (nxt, cell ni; ni < pmin: nothing loaded): the seed's now,
+      // later ones one round ahead or when their cell is accepted.  A cell accepted meanwhile is patched to "used".
+      int ni = grp == 0 ? (int)sidx + noff : pmin - 1;
+      asm volatile("" : "+r"(ni));  // keep the index 32-bit: one IMAD.WIDE forms the address
+      LsdRec nxt;
+      nxt.a = LSD_NOTDEF_F; nxt.li = 0u;
+      if (grp == 0) nxt = lsd_load_pix(reinterpret_cast<const LsdPix*>(pb + (long long)ni * LSD_REC_BYTES));
       // the region's members whose terms are staged but not yet in S: ring positions [qsum, qpos), in acceptance order
       uint32_t qsum = qpos;
       auto add_staged = [&]() {
@@ -671,42 +678,36 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
         }
         qwait = qpos;
       };
-      for (uint32_t r = 0; r < nreg; ++r) {
-        LsdRec cur;
-        int ci;
-        if (i1 >= pmin) {
-          cur = pf1;
-          ci = i1;
-        } else {
+      for (uint32_t r = 0; r < nreg;) {
+        const uint32_t ne = min(3u, nreg - r);   // entries of this round: the ones that exist now
+        const uint32_t rn = r + ne;              // first entry of the next round
+        const LsdRec cur = nxt;
+        const int ci = ni;
+        // lanes that see the same cell (neighbours shared by two entries): accepting it decides all of them
+        const unsigned same = __match_any_sync(0xFFFFFFFFu, ci);
+        nxt.a = LSD_NOTDEF_F;
+        ni = pmin - 1;
+        const uint32_t nx = rn + (uint32_t)grp;  // the next round's entries that already exist: load them now
+        if (grp < 3 && nx < nreg) {
           uint32_t pt;
-          if (nreg - r <= LSD_QCAP) asm volatile("ld.shared.u32 %0, [%1];" : "=r"(pt) : "r"(qs + ((r & (LSD_QCAP - 1)) << 2)) : "memory");
-          else pt = __ldcg(&regpts[cursor + r]);
-          ci = (int)pt + noff;
-          asm volatile("" : "+r"(ci));  // keep the index 32-bit: one IMAD.WIDE forms the address
-          cur = lsd_load_pix(reinterpret_cast<const LsdPix*>(pb + (long long)ci * LSD_REC_BYTES));
+          if (nreg - nx <= LSD_QCAP) asm volatile("ld.shared.u32 %0, [%1];" : "=r"(pt) : "r"(qs + ((nx & (LSD_QCAP - 1)) << 2)) : "memory");
+          else pt = __ldcg(&regpts[cursor + nx]);
+          ni = (int)pt + noff;
+          asm volatile("" : "+r"(ni));
+          nxt = lsd_load_pix(reinterpret_cast<const LsdPix*>(pb + (long long)ni * LSD_REC_BYTES));
         }
-        pf1 = pf2; i1 = i2;
-        i2 = pmin - 1;
-        if (i1 < pmin && r + 1 < nreg) {
-          uint32_t pt;
-          if (nreg - (r + 1) <= LSD_QCAP) asm volatile("ld.shared.u32 %0, [%1];" : "=r"(pt) : "r"(qs + (((r + 1) & (LSD_QCAP - 1)) << 2)) : "memory");
-          else pt = __ldcg(&regpts[cursor + r + 1]);
-          i1 = (int)pt + noff;
-          asm volatile("" : "+r"(i1));
-          pf1 = lsd_load_pix(reinterpret_cast<const LsdPix*>(pb + (long long)i1 * LSD_REC_BYTES));
-        }
-        if (r + 2 < nreg) {
-          uint32_t pt;
-          if (nreg - (r + 2) <= LSD_QCAP) asm volatile("ld.shared.u32 %0, [%1];" : "=r"(pt) : "r"(qs + (((r + 2) & (LSD_QCAP - 1)) << 2)) : "memory");
-          else pt = __ldcg(&regpts[cursor + r + 2]);
-          i2 = (int)pt + noff;
-          asm volatile("" : "+r"(i2));
-          pf2 = lsd_load_pix(reinterpret_cast<const LsdPix*>(pb + (long long)i2 * LSD_REC_BYTES));
-        }
-        unsigned rem = __ballot_sync(0xFFFFFFFFu, lane < 9 && cur.a != LSD_NOTDEF_F);
+        // kk != 4: the centre is the entry itself (already used); with lane < 9 ne it also keeps the idle lanes out
+        unsigned rem = __ballot_sync(0xFFFFFFFFu, lane < 9 * (int)ne && kk != 4 && cur.a != LSD_NOTDEF_F);
+        // Off the decision chain: each lane's distance to th (changes only when th is evaluated) and the margin the
+        // region would have after accepting this lane's cell (the margin update of the reference order, done by every
+        // lane ahead of the decision; the accepted lane's value is taken by one shuffle)
+        auto lane_dist = [&]() {
+          float dd = fabsf(__fsub_rn(cur.a, th));
+          return dd > 180.f ? __fsub_rn(360.f, dd) : dd;
+        };
+        float d = lane_dist();
+        float mn = __fmaf_rn(fminf(__fadd_rn(d, margin), dmax), inv0, margin);
         while (rem) {
-          float d = fabsf(__fsub_rn(cur.a, th));
-          if (d > 180.f) d = __fsub_rn(360.f, d);
           const bool mine = (rem >> lane) & 1u;
           const unsigned mm = __ballot_sync(0xFFFFFFFFu, mine && d <= hi);  // aligned or undecided
           if (!mm) break;                                                    // everything left is clearly not aligned
@@ -720,6 +721,8 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
               margin = margin0;
               lo = prec_deg - margin; hi = prec_deg + margin;
               fresh = true;
+              d = lane_dist();
+              mn = __fmaf_rn(fminf(__fadd_rn(d, margin), dmax), inv0, margin);
               continue;
             }
             float av = cur.a;
@@ -730,9 +733,10 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
               continue;
             }
           }
-          rem &= ~((2u << k) - 1u);  // k and everything before it have been decided
           const int ai = __shfl_sync(0xFFFFFFFFu, ci, k);
-          const float dk = __shfl_sync(0xFFFFFFFFu, d, k);
+          margin = __shfl_sync(0xFFFFFFFFu, mn, k);
+          lo = prec_deg - margin; hi = prec_deg + margin;
+          rem &= ~(((2u << k) - 1u) | __shfl_sync(0xFFFFFFFFu, same, k));  // k, everything before it and k's cell: decided
           // lane 0 marks the cell used and appends it to the region / the queue (predicated: no divergent branch)
           asm volatile(
               "{\n\t.reg .pred p;\n\tsetp.ne.s32 p, %0, 0;\n\t"
@@ -740,21 +744,26 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
               ::"r"(l0), "l"(pb + (long long)ai * LSD_REC_BYTES), "f"(LSD_NOTDEF_F), "l"(regpts + (cursor + nreg)), "r"(ai),
                 "r"(qs + ((nreg & (LSD_QCAP - 1)) << 2))
               : "memory");
+          const uint32_t en = nreg - rn;   // the new entry's place in the next round
           ++nreg;
           lsd_prefetch(pb + (long long)(ai + poff) * LSD_REC_BYTES);
-          if (i1 == ai) pf1.a = LSD_NOTDEF_F;  // prefetched copies of this cell are stale
-          if (i2 == ai) pf2.a = LSD_NOTDEF_F;
+          if (ni == ai) nxt.a = LSD_NOTDEF_F;  // a look-ahead copy of this cell is stale
+          if (en < 3) {                      // the new entry is one of the next round's: load its neighbourhood now
+            if (grp == (int)en) ni = ai + noff;
+            __syncwarp();                    // after lane 0's store of this round's acceptances
+            if (grp == (int)en) nxt = lsd_load_pix(reinterpret_cast<const LsdPix*>(pb + (long long)ni * LSD_REC_BYTES));
+          }
           // stage the member's term: lane k holds its record (landed: its angle was just tested)
           if (qpos - qwait == LSD_CSQ) add_staged();   // ring full: its oldest slot is about to be reused
           if (lane == k)
             asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(csb + ((qpos & (LSD_CSQ - 1)) << 3)),
                          "l"(lut_cs + cur.li) : "memory");
           ++qpos;
-          margin = __fmaf_rn(fminf(__fadd_rn(dk, margin), dmax), inv0, margin);
-          lo = prec_deg - margin; hi = prec_deg + margin;
+          mn = __fmaf_rn(fminf(__fadd_rn(d, margin), dmax), inv0, margin);
           fresh = false;
         }
         __syncwarp();
+        r = rn;
       }
       if ((int)nreg >= min_reg_size) {
         if (nreg_out < max_regions) {
