@@ -47,8 +47,6 @@ struct BowKind {
 
 struct BowState {
   BowKind kind[2];
-  uint8_t* io = nullptr;     // per-call upload / work / download region
-  size_t io_bytes = 0;
   int n_sm = 0;
   bool attr_set = false;
 };
@@ -583,8 +581,6 @@ plf_status grow_db(plf_ctx* ctx, BowKind& k, size_t more, int kf_idx) {
   return PLF_OK;
 }
 
-size_t align_up(size_t x) { return (x + 255) & ~size_t(255); }
-
 }  // namespace
 
 extern "C" {
@@ -592,7 +588,6 @@ extern "C" {
 void plf_bow_free(plf_ctx* ctx) {
   if (!ctx->bow) return;
   for (BowKind& k : ctx->bow->kind) free_kind(k);
-  cudaFree(ctx->bow->io);
   delete ctx->bow;
   ctx->bow = nullptr;
 }
@@ -708,34 +703,29 @@ plf_status plf_bow_insert(plf_ctx* ctx, int kf_idx, const plf_frame_view* kf, do
       plf_status st = grow_db(ctx, S->kind[c], (size_t)n[c], kf_idx);
       if (st) return st;
     }
-  // io region: in = descriptors [n0 + n1][32]; work = word [.] int, weight [.] f64; out = nnz [2] int, rows [2][kf_idx + 1]
   const int m0 = on[0] ? n[0] : 0, m1 = on[1] ? n[1] : 0, nf = m0 + m1;
-  const size_t in_b = align_up((size_t)nf * 32), w_off = in_b, wt_off = w_off + align_up((size_t)nf * 4),
-               out_off = wt_off + align_up((size_t)nf * 8), row_b = (size_t)(kf_idx + 1) * 8;
-  const size_t out_b = 16 + 2 * align_up(row_b), total = out_off + out_b;
-  if (S->io_bytes < total) {
-    PLF_CUDA(ctx, cudaStreamSynchronize(cs));
-    cudaFree(S->io);
-    S->io = nullptr;
-    S->io_bytes = 0;
-    const size_t want = std::max(total, (size_t)1 << 20);
-    if (cudaMalloc(&S->io, want) != cudaSuccess) return plf_fail(ctx, PLF_ERR_CUDA, "plf_bow_insert: cudaMalloc(%zu)", want);
-    S->io_bytes = want;
-  }
-  uint8_t* pin = (uint8_t*)plf_pinned(ctx, std::max(in_b, out_b));
-  if (!pin) return PLF_ERR_CUDA;
+  const size_t row_b = (size_t)(kf_idx + 1) * 8;
+  StagedLayout L;
+  L.take_in((size_t)nf * 32);
+  const size_t w_off = L.take_work((size_t)nf * 4), wt_off = L.take_work((size_t)nf * 8);
+  const size_t nnz_off = L.take_out(2 * sizeof(int)), row_off[2] = {L.take_out(row_b), L.take_out(row_b)};
+  // the rows grow by 16 bytes per keyframe: 1 MB up front keeps the inserts of the first ~50 000 keyframes from
+  // reallocating the slot (a stream synchronisation) every 32 keyframes
+  if (!plf_scratch(ctx, PLF_SCR_BOW, (size_t)1 << 20)) return PLF_ERR_CUDA;
+  uint8_t *pin, *dev;
+  if (plf_status st = L.acquire(ctx, PLF_SCR_BOW, &pin, &dev)) return st;
   if (m0) memcpy(pin, d[0], (size_t)m0 * 32);
   if (m1) memcpy(pin + (size_t)m0 * 32, d[1], (size_t)m1 * 32);
-  uint8_t* io = S->io;
-  int* d_word = (int*)(io + w_off);
-  double* d_wt = (double*)(io + wt_off);
-  int* d_nnz = (int*)(io + out_off);
-  double* d_row[2] = {(double*)(io + out_off + 16), (double*)(io + out_off + 16 + align_up(row_b))};
-  if (nf) PLF_CUDA(ctx, cudaMemcpyAsync(io, pin, (size_t)nf * 32, cudaMemcpyHostToDevice, cs));
+  uint8_t *out = dev + L.in, *work = dev + L.in + L.out;
+  int* d_word = (int*)(work + w_off);
+  double* d_wt = (double*)(work + wt_off);
+  int* d_nnz = (int*)(out + nnz_off);
+  double* d_row[2] = {(double*)(out + row_off[0]), (double*)(out + row_off[1])};
+  if (nf) PLF_CUDA(ctx, cudaMemcpyAsync(dev, pin, (size_t)nf * 32, cudaMemcpyHostToDevice, cs));
   if (nf) {
     const BowKind &a = S->kind[0], &b = S->kind[1];
     const TreeView t0 = {a.desc, a.meta, a.weight, a.root_n}, t1 = {b.desc, b.meta, b.weight, b.root_n};
-    k_bow_transform<<<(nf + 7) / 8, 256, 0, cs>>>(t0, t1, (const uint4*)io, m0, m1, d_word, d_wt);
+    k_bow_transform<<<(nf + 7) / 8, 256, 0, cs>>>(t0, t1, (const uint4*)dev, m0, m1, d_word, d_wt);
     PLF_LAUNCH_CHECK(ctx);
   }
   const size_t smem = (size_t)BOW_MAX_FEATURES * 16;
@@ -763,10 +753,10 @@ plf_status plf_bow_insert(plf_ctx* ctx, int kf_idx, const plf_frame_view* kf, do
     PLF_LAUNCH_CHECK(ctx);
   }
   // one download: the counts and the rows
-  const size_t dl = any_row ? (size_t)(d_row[sk[1].active ? 1 : 0] - (double*)(io + out_off + 16)) * 8 + 16 + row_b : 16;
-  PLF_CUDA(ctx, cudaMemcpyAsync(pin, io + out_off, dl, cudaMemcpyDeviceToHost, cs));
+  const size_t dl = any_row ? row_off[sk[1].active ? 1 : 0] + row_b : nnz_off + 2 * sizeof(int);
+  PLF_CUDA(ctx, cudaMemcpyAsync(pin + L.in, out, dl, cudaMemcpyDeviceToHost, cs));
   PLF_CUDA(ctx, cudaStreamSynchronize(cs));
-  const int* nnz = (const int*)pin;
+  const int* nnz = (const int*)(pin + L.in + nnz_off);
   for (int c = 0; c < 2; ++c) {
     if (!on[c]) continue;
     BowKind& k = S->kind[c];
@@ -774,7 +764,7 @@ plf_status plf_bow_insert(plf_ctx* ctx, int kf_idx, const plf_frame_view* kf, do
     k.host_ent[kf_idx] = make_int2((int)k.end, nnz[c]);
     k.end += (size_t)nnz[c];
     k.last = kf_idx;
-    if (rows[c]) memcpy(rows[c], pin + 16 + (size_t)(d_row[c] - d_row[0]) * 8, row_b);
+    if (rows[c]) memcpy(rows[c], pin + L.in + row_off[c], row_b);
   }
   return PLF_OK;
 }

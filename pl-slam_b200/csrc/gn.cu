@@ -354,8 +354,6 @@ plf_status plf_launch_gn(plf_ctx* ctx, const GnProblem* d_probs, int nprob, cons
   return PLF_OK;
 }
 
-static size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
-
 extern "C" plf_status plf_gn_pose(plf_ctx* ctx, const plf_gn_opts* opts, const double* P, const double* pl_obs,
                                   uint8_t* inlier_pt, int np, const double* sP, const double* eP,
                                   const double* le_obs, uint8_t* inlier_ls, int nl, const double* T_init,
@@ -365,21 +363,15 @@ extern "C" plf_status plf_gn_pose(plf_ctx* ctx, const plf_gn_opts* opts, const d
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_gn_pose: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const plf_gn_opts o = opts ? *opts : plf_gn_opts_from_params(ctx->params);
-  const size_t bP = al256((size_t)np * 24 + 8), bO = al256((size_t)np * 16 + 8), bIp = al256((size_t)np + 8),
-               bL = al256((size_t)nl * 24 + 8), bIl = al256((size_t)nl + 8);
-  uint8_t* base = (uint8_t*)plf_scratch(ctx, 2, bP + bO + bIp + 3 * bL + bIl + 256 + 512 + 512);
-  if (!base) return PLF_ERR_CUDA;
-  uint8_t* p = base;
-  double* dP = (double*)p; p += bP;
-  double* dO = (double*)p; p += bO;
-  uint8_t* dIp = p; p += bIp;
-  double* dsP = (double*)p; p += bL;
-  double* deP = (double*)p; p += bL;
-  double* dle = (double*)p; p += bL;
-  uint8_t* dIl = p; p += bIl;
-  double* dT = (double*)p; p += 256;
-  plf_pose_result* dout = (plf_pose_result*)p; p += 512;
-  GnProblem* dprob = (GnProblem*)p;
+  double *dP, *dO, *dsP, *deP, *dle, *dT;
+  uint8_t *dIp, *dIl;
+  plf_pose_result* dout;
+  GnProblem* dprob;
+  DevBufList scr;
+  scr.add(dP, (size_t)np * 3); scr.add(dO, (size_t)np * 2); scr.add(dIp, np);
+  scr.add(dsP, (size_t)nl * 3); scr.add(deP, (size_t)nl * 3); scr.add(dle, (size_t)nl * 3); scr.add(dIl, nl);
+  scr.add(dT, 16); scr.add(dout, 1); scr.add(dprob, 1);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_GN)) return st;
   cudaStream_t s = ctx->stream;
   if (np) {
     PLF_CUDA(ctx, cudaMemcpyAsync(dP, P, (size_t)np * 24, cudaMemcpyHostToDevice, s));
@@ -422,13 +414,15 @@ __global__ void k_se3(int op, const double* in, double* out) {
 extern "C" plf_status plf_se3(plf_ctx* ctx, int op, const double* in, double* out) {
   if (!ctx || !in || !out || op < 0 || op > 1) return plf_fail(ctx, PLF_ERR_INVALID, "plf_se3: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  double* d = (double*)plf_scratch(ctx, 2, 512);
-  if (!d) return PLF_ERR_CUDA;
+  double *din, *dout;
+  DevBufList scr;
+  scr.add(din, 16); scr.add(dout, 16);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_GN)) return st;
   const int nin = op == 0 ? 6 : 16, nout = op == 0 ? 16 : 6;
-  PLF_CUDA(ctx, cudaMemcpyAsync(d, in, nin * 8, cudaMemcpyHostToDevice, ctx->stream));
-  k_se3<<<1, 1, 0, ctx->stream>>>(op, d, d + 32);
+  PLF_CUDA(ctx, cudaMemcpyAsync(din, in, nin * 8, cudaMemcpyHostToDevice, ctx->stream));
+  k_se3<<<1, 1, 0, ctx->stream>>>(op, din, dout);
   PLF_LAUNCH_CHECK(ctx);
-  PLF_CUDA(ctx, cudaMemcpyAsync(out, d + 32, nout * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  PLF_CUDA(ctx, cudaMemcpyAsync(out, dout, nout * 8, cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return PLF_OK;
 }

@@ -192,16 +192,6 @@ __global__ void __launch_bounds__(256) k_kf_select(KfKind k, int fast, int bf, i
 
 namespace {
 
-// Bump layout of one call: the host inputs [0, in), the outputs [in, in + out) and the device-only work after them.
-// The inputs are staged in pinned memory at the same offsets, so one copy uploads them and one copy downloads the outputs.
-struct Layout {
-  size_t in = 0, out = 0, work = 0;
-  static size_t al(size_t x) { return (x + 255) & ~size_t(255); }
-  size_t take_in(size_t b) { const size_t o = in; in += al(b); return o; }
-  size_t take_out(size_t b) { const size_t o = out; out += al(b); return o; }
-  size_t take_work(size_t b) { const size_t o = work; work += al(b); return o; }
-};
-
 struct KindPlan {
   bool active = false;
   int nq = 0, nt = 0;
@@ -217,7 +207,7 @@ struct HostKind {   // host arrays of one kind
   const double* ts; const double* te; const double* tle; const int32_t* tlm; const uint8_t* tdesc;
 };
 
-void plan_kind(KindPlan& p, Layout& L, bool lines, bool map_lines_le) {
+void plan_kind(KindPlan& p, StagedLayout& L, bool lines, bool map_lines_le) {
   const size_t q = p.nq, t = p.nt;
   p.x = L.take_in(q * (lines ? 6 : 3) * 8);
   p.xe = p.x;
@@ -297,7 +287,7 @@ struct KindRun {
   float nnr;
   int kmin;
   double gate;
-  int slot;
+  plf_scratch_slot slot;   // of the windowed matcher
   KnnProblem kp[2];
   NnrProblem np;
 };
@@ -353,15 +343,13 @@ plf_status run_kind(plf_ctx* ctx, KindRun& r, const KindPlan& p, uint8_t* dev, c
 plf_status kf_run(plf_ctx* ctx, bool map, const plf_kf_match_opts* o, const double* T, KindPlan plan[2], const HostKind host[2],
                   int32_t* outs[2], int* n_out[2]) {
   const plf_params& P = ctx->params;
-  Layout L;
+  StagedLayout L;
   for (int kd = 0; kd < 2; ++kd)
     if (plan[kd].active) plan_kind(plan[kd], L, kd == 1, map && kd == 1);
   const size_t t_off = L.take_in(16 * 8);
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  uint8_t* pin = (uint8_t*)plf_pinned(ctx, L.in + L.out);
-  if (!pin) return PLF_ERR_CUDA;
-  uint8_t* dev = (uint8_t*)plf_scratch(ctx, 11, L.in + L.out + L.work);
-  if (!dev) return PLF_ERR_CUDA;
+  uint8_t *pin, *dev;
+  if (plf_status st = L.acquire(ctx, PLF_SCR_KF, &pin, &dev)) return st;
   cudaStream_t cs = ctx->stream;
   ctx->cur = cs;
   const KfCam cam = {ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy, (double)ctx->cam.width, (double)ctx->cam.height,
@@ -377,7 +365,7 @@ plf_status kf_run(plf_ctx* ctx, bool map, const plf_kf_match_opts* o, const doub
     r.nnr = kd ? P.min_ratio_12_l : P.min_ratio_12_p;
     r.kmin = kd ? P.min_ls_matches : P.min_pt_matches;
     r.gate = kd ? o->max_kf_epip_l : o->max_kf_epip_p;
-    r.slot = 12 + kd;
+    r.slot = kd ? PLF_SCR_KF_MGB_LS : PLF_SCR_KF_MGB_PT;
     // the fallback needs more than kmin queries (and, KF-to-KF, more than kmin train features)
     r.bf = p.nq > r.kmin && (map || p.nt > r.kmin);
     prepare_bf(r, p, dev, P.best_lr_matches ? 1 : 0);

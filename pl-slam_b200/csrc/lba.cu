@@ -602,8 +602,6 @@ __global__ void __launch_bounds__(256) k_gba_bwd(LbaDev d, const uint8_t* nz, in
   if (tid < GBA_T && GBA_T * j + tid < n) d.gred[GBA_T * j + tid] -= ((part[0][tid] + part[1][tid]) + part[2][tid]) + part[3][tid];
 }
 
-static size_t lba_al(size_t x) { return (x + 255) & ~size_t(255); }
-
 // The host loop of both routines: the reference's control flow, on the device kernels above.  `global` selects
 // levMarquardtOptimizationGBA (:2101-2699) over levMarquardtOptimizationLBA (:1332-1989): its quirk set, its error
 // normalisation in the LM iterations, up to 4096 keyframes (the blocked factorisation beyond n = 384) and a landmark
@@ -644,34 +642,25 @@ static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_p
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const bool blocked = n > 384;   // k_lba_solve (one CTA, one launch) up to 64 keyframes, the tiled LDL^T beyond
   const int nt = (n + GBA_T - 1) / GBA_T;
-  // one scratch block
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += lba_al(bytes); return o; };
-  const size_t oX = take((size_t)N * 8), oX0 = take((size_t)N * 8), oT0 = take((size_t)std::max(nkf, 1) * 128),
-               oFT = take((size_t)std::max(p->n_fixed, 1) * 128), oFTi = take((size_t)std::max(p->n_fixed, 1) * 128),
-               oLm = take((size_t)nobs * 4), oKf = take((size_t)nobs * 4), oZ = take((size_t)nobs * 24), oLs = take((size_t)(nlm + 1) * 4),
-               oJt = take((size_t)nobs * 48), oJx = take((size_t)nobs * 48), oWn = take((size_t)nobs * 16),
-               oD = take((size_t)std::max(nlm, 1) * 288), oGl = take((size_t)std::max(nlm, 1) * 48), oDi = take((size_t)std::max(nlm, 1) * 288),
-               oA = take((size_t)std::max(nkf, 1) * 288), oGc = take((size_t)std::max(nkf, 1) * 48),
-               oS = take(std::max((size_t)n * n, (size_t)1) * 8), oGr = take((size_t)std::max(n, 1) * 8), oDc = take((size_t)std::max(n, 1) * 8),
-               oDX = take((size_t)N * 8), oSc = take(64), oPm = take((size_t)std::max(npt, 1)), oLmv = take((size_t)std::max(nls, 1)),
-               oWp = take(blocked ? (size_t)nt * GBA_T * GBA_T * 8 : 8), oNz = take(blocked ? (size_t)nt * nt : 1);
-  uint8_t* base = (uint8_t*)plf_scratch(ctx, 10, off);
-  if (!base) return PLF_ERR_CUDA;
   LbaDev d;
   d.nkf = nkf; d.npt = npt; d.nls = nls; d.N = N; d.npo = npo; d.nlo = nlo; d.nobs = nobs; d.nlm = nlm;
-  d.X = (double*)(base + oX); d.X0 = (double*)(base + oX0); d.T0inv = (double*)(base + oT0);
-  double* dFT = (double*)(base + oFT); double* dFTi = (double*)(base + oFTi);
+  double *dFT, *dFTi, *dZ, *dWp;
+  int *dLm, *dKf, *dLs;
+  uint8_t *dPm, *dLmv, *dNz;
+  DevBufList scr;
+  scr.add(d.X, N); scr.add(d.X0, N); scr.add(d.T0inv, (size_t)std::max(nkf, 1) * 16);
+  scr.add(dFT, (size_t)std::max(p->n_fixed, 1) * 16); scr.add(dFTi, (size_t)std::max(p->n_fixed, 1) * 16);
+  scr.add(dLm, nobs); scr.add(dKf, nobs); scr.add(dZ, (size_t)nobs * 3); scr.add(dLs, (size_t)nlm + 1);
+  scr.add(d.Jt, (size_t)nobs * 6); scr.add(d.Jx, (size_t)nobs * 6); scr.add(d.Wn, (size_t)nobs * 2);
+  scr.add(d.D, (size_t)std::max(nlm, 1) * 36); scr.add(d.gl, (size_t)std::max(nlm, 1) * 6); scr.add(d.Dinv, (size_t)std::max(nlm, 1) * 36);
+  scr.add(d.A, (size_t)std::max(nkf, 1) * 36); scr.add(d.gc, (size_t)std::max(nkf, 1) * 6);
+  scr.add(d.S, std::max((size_t)n * n, (size_t)1)); scr.add(d.gred, (size_t)std::max(n, 1)); scr.add(d.dxc, (size_t)std::max(n, 1));
+  scr.add(d.DX, N); scr.add(d.scal, 8);
+  scr.add(dPm, std::max(npt, 1)); scr.add(dLmv, std::max(nls, 1));
+  scr.add(dWp, blocked ? (size_t)nt * GBA_T * GBA_T : 1); scr.add(dNz, blocked ? (size_t)nt * nt : 1);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_BA)) return st;
   d.fixedTinv = dFTi;
-  int* dLm = (int*)(base + oLm); int* dKf = (int*)(base + oKf); double* dZ = (double*)(base + oZ); int* dLs = (int*)(base + oLs);
   d.obs_lm = dLm; d.obs_kf = dKf; d.obs_z = dZ; d.lm_start = dLs;
-  d.Jt = (double*)(base + oJt); d.Jx = (double*)(base + oJx); d.Wn = (double*)(base + oWn);
-  d.D = (double*)(base + oD); d.gl = (double*)(base + oGl); d.Dinv = (double*)(base + oDi);
-  d.A = (double*)(base + oA); d.gc = (double*)(base + oGc);
-  d.S = (double*)(base + oS); d.gred = (double*)(base + oGr); d.dxc = (double*)(base + oDc);
-  d.DX = (double*)(base + oDX); d.scal = (double*)(base + oSc);
-  uint8_t* dPm = base + oPm; uint8_t* dLmv = base + oLmv;
-  double* dWp = (double*)(base + oWp); uint8_t* dNz = base + oNz;
   cudaStream_t cs = ctx->stream;
   ctx->cur = cs;
   std::vector<double> hX(N);

@@ -375,21 +375,21 @@ extern "C" void plf_lbd_free(plf_ctx* ctx) {
   ctx->lbd = nullptr;
 }
 
-static size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
-
 extern "C" plf_status plf_lbd_gradients(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride,
                                         int16_t* dxdy) {
   if (!ctx || !img || !dxdy || w < 2 || h < 2 || stride < w)
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_lbd_gradients: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const int pitch = plf_pitch16(w);
-  const size_t ib = al256((size_t)pitch * h), gb = al256((size_t)w * h * 4);
-  uint8_t* base = (uint8_t*)plf_scratch(ctx, 1, ib + gb);
-  if (!base) return PLF_ERR_CUDA;
-  PLF_CUDA(ctx, cudaMemcpy2DAsync(base, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  plf_status st = plf_launch_blur5_sobel(ctx, base, pitch, (size_t)pitch * h, w, h, 1, (short2*)(base + ib), 0);
+  uint8_t* dimg;
+  short2* dgrad;
+  DevBufList scr;
+  scr.add(dimg, (size_t)pitch * h); scr.add(dgrad, (size_t)w * h);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_LBD)) return st;
+  PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
+  plf_status st = plf_launch_blur5_sobel(ctx, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
   if (st) return st;
-  PLF_CUDA(ctx, cudaMemcpyAsync(dxdy, base + ib, (size_t)w * h * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  PLF_CUDA(ctx, cudaMemcpyAsync(dxdy, dgrad, (size_t)w * h * 4, cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return PLF_OK;
 }
@@ -406,17 +406,15 @@ extern "C" plf_status plf_lbd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_lbd: %d lines (reference numOfFinalLine is a short, :1029)", n);
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const int pitch = plf_pitch16(w);
-  const size_t ib = al256((size_t)pitch * h), gb = al256((size_t)w * h * 4),
-               kb = al256((size_t)n * sizeof(plf_keyline)), db = al256((size_t)n * 32),
-               fb = al256((size_t)n * 72 * 4);
-  uint8_t* base = (uint8_t*)plf_scratch(ctx, 1, ib + gb + kb + db + fb + 256);
-  if (!base) return PLF_ERR_CUDA;
-  uint8_t* dimg = base;
-  short2* dgrad = (short2*)(base + ib);
-  plf_keyline* dkl = (plf_keyline*)(base + ib + gb);
-  uint8_t* ddesc = base + ib + gb + kb;
-  float* dfl = (float*)(base + ib + gb + kb + db);
-  int* dcount = (int*)(base + ib + gb + kb + db + fb);
+  uint8_t *dimg, *ddesc;
+  short2* dgrad;
+  plf_keyline* dkl;
+  float* dfl;
+  int* dcount;
+  DevBufList scr;
+  scr.add(dimg, (size_t)pitch * h); scr.add(dgrad, (size_t)w * h);
+  scr.add(dkl, n); scr.add(ddesc, (size_t)n * 32); scr.add(dfl, (size_t)n * 72); scr.add(dcount, 1);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_LBD)) return st;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyAsync(dkl, keylines, (size_t)n * sizeof(plf_keyline), cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyAsync(dcount, &n, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));

@@ -1339,7 +1339,7 @@ extern "C" plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_lsd: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const int pitch = plf_pitch16(w);
-  uint8_t* dimg = (uint8_t*)plf_scratch(ctx, 4, (size_t)pitch * h);
+  uint8_t* dimg = (uint8_t*)plf_scratch(ctx, PLF_SCR_LSD, (size_t)pitch * h);
   if (!dimg) return PLF_ERR_CUDA;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
   plf_status st = plf_lsd_run(ctx, dimg, (size_t)pitch * h, pitch, w, h, 1);
@@ -1364,12 +1364,11 @@ extern "C" plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, 
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_detect_lines: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const int pitch = plf_pitch16(w);
-  const size_t A = ((size_t)pitch * h + 255) & ~size_t(255);
-  uint8_t* base = (uint8_t*)plf_scratch(ctx, 4, A + A * 4 + (size_t)ctx->limits.max_lines * 32 + 256);
-  if (!base) return PLF_ERR_CUDA;
-  uint8_t* dimg = base;
-  short2* dgrad = (short2*)(base + A);
-  uint8_t* ddesc = base + A + A * 4;
+  uint8_t *dimg, *ddesc;
+  short2* dgrad;
+  DevBufList scr;
+  scr.add(dimg, (size_t)pitch * h); scr.add(dgrad, (size_t)w * h); scr.add(ddesc, (size_t)ctx->limits.max_lines * 32);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_LSD)) return st;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
   plf_status st = plf_lsd_run(ctx, dimg, (size_t)pitch * h, pitch, w, h, 1);
   if (st) return st;
@@ -1404,13 +1403,15 @@ __global__ void k_sincosf_probe(const float* in, float* s, float* c, int n) {
 extern "C" plf_status plf_debug_sincosf(plf_ctx* ctx, const float* in, float* s, float* c, int n) {
   if (!ctx || n <= 0) return PLF_ERR_INVALID;
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  float* d = (float*)plf_scratch(ctx, 4, (size_t)n * 12);
-  if (!d) return PLF_ERR_CUDA;
-  PLF_CUDA(ctx, cudaMemcpyAsync(d, in, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-  k_sincosf_probe<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d, d + n, d + 2 * (size_t)n, n);
+  float *din, *ds, *dc;
+  DevBufList scr;
+  scr.add(din, n); scr.add(ds, n); scr.add(dc, n);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_LSD)) return st;
+  PLF_CUDA(ctx, cudaMemcpyAsync(din, in, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+  k_sincosf_probe<<<(n + 255) / 256, 256, 0, ctx->stream>>>(din, ds, dc, n);
   PLF_LAUNCH_CHECK(ctx);
-  PLF_CUDA(ctx, cudaMemcpyAsync(s, d + n, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  PLF_CUDA(ctx, cudaMemcpyAsync(c, d + 2 * (size_t)n, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  PLF_CUDA(ctx, cudaMemcpyAsync(s, ds, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  PLF_CUDA(ctx, cudaMemcpyAsync(c, dc, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return PLF_OK;
 }

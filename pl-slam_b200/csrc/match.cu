@@ -220,8 +220,6 @@ plf_status plf_launch_nnr(plf_ctx* ctx, const NnrProblem* d_probs, int nprob, in
 
 // ---- host-pointer operator entry points ---------------------------------------------------------
 
-static size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
-
 extern "C" plf_status plf_hamming_knn2(plf_ctx* ctx, const uint8_t* d1, int n1, const uint8_t* d2,
                                        int n2, int32_t* idx1, int32_t* dist1, int32_t* idx2,
                                        int32_t* dist2) {
@@ -231,13 +229,13 @@ extern "C" plf_status plf_hamming_knn2(plf_ctx* ctx, const uint8_t* d1, int n1, 
                     n2);
   if (n1 == 0) return PLF_OK;
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  const size_t b1 = align256((size_t)n1 * 32), b2 = align256((size_t)(n2 > 0 ? n2 : 1) * 32),
-               bk = align256((size_t)n1 * 4);
-  uint8_t* base = (uint8_t*)plf_scratch(ctx, 0, b1 + b2 + 2 * bk + 256);
-  if (!base) return PLF_ERR_CUDA;
-  uint8_t *dq = base, *dt = base + b1;
-  uint32_t *dbest = (uint32_t*)(base + b1 + b2), *dsec = (uint32_t*)(base + b1 + b2 + bk);
-  KnnProblem* dprob = (KnnProblem*)(base + b1 + b2 + 2 * bk);
+  uint8_t *dq, *dt;
+  uint32_t *dbest, *dsec;
+  KnnProblem* dprob;
+  DevBufList scr;
+  scr.add(dq, (size_t)n1 * 32); scr.add(dt, (size_t)std::max(n2, 1) * 32);
+  scr.add(dbest, n1); scr.add(dsec, n1); scr.add(dprob, 1);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_MATCH)) return st;
   PLF_CUDA(ctx, cudaMemcpyAsync(dq, d1, (size_t)n1 * 32, cudaMemcpyHostToDevice, ctx->stream));
   if (n2 > 0)
     PLF_CUDA(ctx, cudaMemcpyAsync(dt, d2, (size_t)n2 * 32, cudaMemcpyHostToDevice, ctx->stream));
@@ -273,21 +271,18 @@ extern "C" plf_status plf_match(plf_ctx* ctx, const uint8_t* d1, int n1, const u
     return PLF_OK;
   }
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  const size_t b1 = align256((size_t)n1 * 32), b2 = align256((size_t)n2 * 32),
-               k1 = align256((size_t)n1 * 4), k2 = align256((size_t)n2 * 4);
-  uint8_t* base = (uint8_t*)plf_scratch(ctx, 0, b1 + b2 + 3 * k1 + 2 * k2 + 1024);
-  if (!base) return PLF_ERR_CUDA;
-  uint8_t* p = base;
-  uint8_t* dq = p; p += b1;
-  uint8_t* dt = p; p += b2;
-  uint32_t* b12 = (uint32_t*)p; p += k1;
-  uint32_t* s12 = (uint32_t*)p; p += k1;
-  int32_t* dm = (int32_t*)p; p += k1;
-  uint32_t* b21 = (uint32_t*)p; p += k2;
-  uint32_t* s21 = (uint32_t*)p; p += k2;
-  int* dcount = (int*)p; p += 256;
-  KnnProblem* dkp = (KnnProblem*)p; p += 256;
-  NnrProblem* dnp = (NnrProblem*)p;
+  uint8_t *dq, *dt;
+  uint32_t *b12, *s12, *b21, *s21;
+  int32_t* dm;
+  int* dcount;
+  KnnProblem* dkp;
+  NnrProblem* dnp;
+  DevBufList scr;
+  scr.add(dq, (size_t)n1 * 32); scr.add(dt, (size_t)n2 * 32);
+  scr.add(b12, n1); scr.add(s12, n1); scr.add(dm, n1);
+  scr.add(b21, n2); scr.add(s21, n2);
+  scr.add(dcount, 1); scr.add(dkp, 2); scr.add(dnp, 1);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_MATCH)) return st;
   PLF_CUDA(ctx, cudaMemcpyAsync(dq, d1, (size_t)n1 * 32, cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyAsync(dt, d2, (size_t)n2 * 32, cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaMemsetAsync(dcount, 0, sizeof(int), ctx->stream));
@@ -385,12 +380,13 @@ extern "C" plf_status plf_median_descriptors(plf_ctx* ctx, const uint8_t* desc, 
     if (n > MED_MAX_OBS) return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_median_descriptors: landmark %d has %d observations (max %d)", l, n, MED_MAX_OBS);
   }
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  const size_t bd = align256((size_t)total * 32), bo = align256((size_t)(n_landmarks + 1) * 4),
-               br = align256((size_t)total * 24), bi = align256((size_t)n_landmarks * 4), bm = align256((size_t)n_landmarks * 24);
-  uint8_t* base = (uint8_t*)plf_scratch(ctx, 0, bd + bo + br + bi + bm);
-  if (!base) return PLF_ERR_CUDA;
-  uint8_t* dd = base; int* dofs = (int*)(base + bd); double* ddir = (double*)(base + bd + bo);
-  int* didx = (int*)(base + bd + bo + br); double* dmed = (double*)(base + bd + bo + br + bi);
+  uint8_t* dd;
+  int *dofs, *didx;
+  double *ddir, *dmed;
+  DevBufList scr;
+  scr.add(dd, (size_t)total * 32); scr.add(dofs, (size_t)n_landmarks + 1); scr.add(ddir, (size_t)total * 3);
+  scr.add(didx, n_landmarks); scr.add(dmed, (size_t)n_landmarks * 3);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_MATCH)) return st;
   cudaStream_t cs = ctx->stream;
   if (total > 0) PLF_CUDA(ctx, cudaMemcpyAsync(dd, desc, (size_t)total * 32, cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(dofs, offsets, (size_t)(n_landmarks + 1) * 4, cudaMemcpyHostToDevice, cs));

@@ -134,8 +134,6 @@ __global__ void __launch_bounds__(128) k_mg_mutual(int32_t* __restrict__ m12, co
   if ((threadIdx.x & 31) == 0 && bal) atomicAdd(count, __popc(bal));
 }
 
-static size_t mg_align(size_t x) { return (x + 255) & ~size_t(255); }
-
 static plf_status mg_run(plf_ctx* ctx, const char* who, int is_lines, const int* q_geo, const uint8_t* d1, int n1,
                          const int* cell_start, const int* cell_items, const double* t_dir, const uint8_t* d2, int n2,
                          int cols, int rows, plf_grid_window w, float nnr, double line_sim_th, int best_lr,
@@ -166,22 +164,16 @@ static plf_status mg_run(plf_ctx* ctx, const char* who, int is_lines, const int*
       if (cell_items[k] >= 0 && cell_items[k] < n2) tcells[fill[cell_items[k]]++] = c;  // cell id = x * rows + y
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const int gq = is_lines ? 4 : 2;
-  const size_t bq = mg_align((size_t)n1 * gq * 4), bts = mg_align((size_t)(n2 + 1) * 4), btc = mg_align(tcells.size() * 4),
-               bdir = mg_align((size_t)n2 * 16), b1 = mg_align((size_t)n1 * 32), b2 = mg_align((size_t)n2 * 32),
-               bD = mg_align((size_t)n1 * n2 * 2), bm12 = mg_align((size_t)n1 * 4), bm21 = mg_align((size_t)n2 * 4);
-  uint8_t* base = (uint8_t*)plf_scratch(ctx, 0, bq + bts + btc + bdir + b1 + b2 + bD + bm12 + bm21 + 256);
-  if (!base) return PLF_ERR_CUDA;
-  uint8_t* p = base;
-  int* dq = (int*)p; p += bq;
-  int* dts = (int*)p; p += bts;
-  int* dtc = (int*)p; p += btc;
-  double* ddir = (double*)p; p += bdir;
-  uint8_t* dd1 = p; p += b1;
-  uint8_t* dd2 = p; p += b2;
-  unsigned short* D = (unsigned short*)p; p += bD;
-  int32_t* dm12 = (int32_t*)p; p += bm12;
-  int* dm21 = (int*)p; p += bm21;
-  int* dcount = (int*)p;
+  int *dq, *dts, *dtc, *dm21, *dcount;
+  double* ddir;
+  uint8_t *dd1, *dd2;
+  unsigned short* D;
+  int32_t* dm12;
+  DevBufList scr;
+  scr.add(dq, (size_t)n1 * gq); scr.add(dts, (size_t)n2 + 1); scr.add(dtc, tcells.size()); scr.add(ddir, (size_t)n2 * 2);
+  scr.add(dd1, (size_t)n1 * 32); scr.add(dd2, (size_t)n2 * 32);
+  scr.add(D, (size_t)n1 * n2); scr.add(dm12, n1); scr.add(dm21, n2); scr.add(dcount, 1);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_MATCH)) return st;
   cudaStream_t cs = ctx->stream;
   ctx->cur = cs;
   PLF_CUDA(ctx, cudaMemcpyAsync(dq, q_geo, (size_t)n1 * gq * 4, cudaMemcpyHostToDevice, cs));
@@ -397,18 +389,16 @@ __global__ void __launch_bounds__(128) k_mgb_mutual(MgbArgs a, int p0) {
 }
 
 // Runs nprob windowed matching problems.  scratch: MGB scratch of the context (slot `slot`), sized here.
-plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n1, int max_n2, int slot) {
+plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n1, int max_n2, plf_scratch_slot slot) {
   if (nprob <= 0) return PLF_OK;
   if (a.g.cols * a.g.rows > 32 * MGB_MASK_WORDS) return plf_fail(ctx, PLF_ERR_INVALID, "match grid: %dx%d cells exceed the mask", a.g.cols, a.g.rows);
   const int K = a.K, Kt = a.Kt;
-  const size_t perD = (size_t)K * Kt * 2, perM = a.is_lines ? (size_t)K * MGB_MASK_WORDS * 4 : 0, per21 = (size_t)Kt * 4;
-  const size_t per = mg_align(perD) + mg_align(perM) + mg_align(per21);
+  const size_t nD = (size_t)K * Kt, nM = a.is_lines ? (size_t)K * MGB_MASK_WORDS : 0;   // D and qmask elements per problem
+  const size_t per = plf_align256(nD * 2) + plf_align256(nM * 4) + plf_align256((size_t)Kt * 4);
   int chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)nprob, (size_t(1) << 31) / per));   // <= 2 GB of scratch
-  uint8_t* base = (uint8_t*)plf_scratch(ctx, slot, per * chunk);
-  if (!base) return PLF_ERR_CUDA;
-  a.D = (unsigned short*)base;
-  a.qmask = (uint32_t*)(base + mg_align(perD) * chunk);
-  a.m21 = (int*)(base + (mg_align(perD) + mg_align(perM)) * chunk);
+  DevBufList scr;
+  scr.add(a.D, nD * chunk); scr.add(a.qmask, nM * chunk); scr.add(a.m21, (size_t)Kt * chunk);
+  if (plf_status st = scr.carve(ctx, slot)) return st;
   cudaStream_t cs = ctx->cur;
   const int gx1 = (max_n1 + 127) / 128, gx2 = (max_n2 + 127) / 128;
   if (gx1 == 0 || gx2 == 0) return PLF_OK;

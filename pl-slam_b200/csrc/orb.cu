@@ -732,7 +732,7 @@ static plf_status orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
       return plf_fail(ctx, PLF_ERR_INVALID, "ORB: level %d (%dx%d) too small for edge threshold %d", l, g.w[l],
                       g.h[l], g.edge);
     g.pitch[l] = g.bpitch[l] = plf_pitch16(g.w[l]);   // level 0's source pitch is the caller's (set per run)
-    const size_t a = ((size_t)g.pitch[l] * g.h[l] + 255) & ~size_t(255);
+    const size_t a = plf_align256((size_t)g.pitch[l] * g.h[l]);
     if (l >= 1) { g.pyr_off[l] = pyr; pyr += a; }
     g.blur_off[l] = blur; blur += a;
     g.cand_cap[l] = (int)std::min<size_t>((size_t)g.w[l] * g.h[l] / 9 + 64, 32768);
@@ -905,7 +905,7 @@ extern "C" plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, in
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_orb: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const int pitch = plf_pitch16(w);
-  uint8_t* dimg = (uint8_t*)plf_scratch(ctx, 3, (size_t)pitch * h);
+  uint8_t* dimg = (uint8_t*)plf_scratch(ctx, PLF_SCR_ORB, (size_t)pitch * h);
   if (!dimg) return PLF_ERR_CUDA;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
   plf_status st = plf_orb_run(ctx, dimg, (size_t)pitch * h, pitch, w, h, 1, 0);

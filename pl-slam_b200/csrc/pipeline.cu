@@ -721,9 +721,9 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     PLF_LAUNCH_CHECK(ctx);
     const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, P.matching_s_ws, 0, 0, 0};
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 2, s->mg_q[0], s->mg_t[0], nullptr, odesc, kcnt, s->m12,
-                                                        4 * (size_t)K, s->mcount, 4), B, K, K, 9))) return st;
+                                                        4 * (size_t)K, s->mcount, 4), B, K, K, PLF_SCR_MGB_PIPE))) return st;
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 2, s->mg_q[1], s->mg_t[1], s->mg_dir[0], s->ldesc_raw, lcnt,
-                                                        s->m12 + K, 4 * (size_t)K, s->mcount + 1, 4), B, Ln, Ln, 9))) return st;
+                                                        s->m12 + K, 4 * (size_t)K, s->mcount + 1, 4), B, Ln, Ln, PLF_SCR_MGB_PIPE))) return st;
     plf_mark(ctx, "stereo.k_mgb (matchGrid)");
   } else {
     // L->R 2-NN for every left feature; R->L only for the right features that are somebody's accepted best match
@@ -761,9 +761,9 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     const int ws = P.matching_f2f_ws;
     const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, ws, ws, ws, ws};
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 1, s->mg_q[2], s->mg_t[2], nullptr, s->fs.pdesc, s->fs.pt_count,
-                                                        s->m12g, 2 * (size_t)K, s->mgcount, 2), B, K, K, 9))) return st;
+                                                        s->m12g, 2 * (size_t)K, s->mgcount, 2), B, K, K, PLF_SCR_MGB_PIPE))) return st;
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 1, s->mg_q[3], s->mg_t[3], s->mg_dir[1], s->fs.ldesc, s->fs.ls_count,
-                                                        s->m12g + K, 2 * (size_t)K, s->mgcount + 1, 2), B, Ln, Ln, 9))) return st;
+                                                        s->m12g + K, 2 * (size_t)K, s->mgcount + 1, 2), B, Ln, Ln, PLF_SCR_MGB_PIPE))) return st;
     k_mg_select<<<dim3((K + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.pt_count, K, K, 0, P.min_pt_matches, s->m12);
     PLF_LAUNCH_CHECK(ctx);
     k_mg_select<<<dim3((Ln + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.ls_count, Ln, K, 1, P.min_ls_matches, s->m12);

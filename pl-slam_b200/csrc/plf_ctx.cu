@@ -29,9 +29,9 @@ size_t DevBufList::bytes() const {
 
 plf_status DevBufList::alloc(plf_ctx* ctx, const char* owner) {
   for (const Entry& e : entries) {
-    const cudaError_t err = cudaMalloc(e.slot, e.bytes + 64);
+    const cudaError_t err = cudaMalloc(e.ptr, e.bytes + 64);
     if (err != cudaSuccess) {
-      *e.slot = nullptr;
+      *e.ptr = nullptr;
       return plf_fail(ctx, PLF_ERR_CUDA, "%s: cudaMalloc(%zu): %s", owner, e.bytes, cudaGetErrorString(err));
     }
   }
@@ -40,12 +40,28 @@ plf_status DevBufList::alloc(plf_ctx* ctx, const char* owner) {
 
 void DevBufList::release() {
   for (const Entry& e : entries) {
-    cudaFree(*e.slot);
-    *e.slot = nullptr;
+    cudaFree(*e.ptr);
+    *e.ptr = nullptr;
   }
 }
 
-void* plf_scratch(plf_ctx* ctx, int slot, size_t bytes) {
+plf_status DevBufList::carve(plf_ctx* ctx, plf_scratch_slot slot) const {
+  size_t total = 0;
+  for (const Entry& e : entries) total += plf_align256(e.bytes);
+  uint8_t* p = (uint8_t*)plf_scratch(ctx, slot, total);
+  if (!p) return PLF_ERR_CUDA;
+  for (const Entry& e : entries) { *e.ptr = p; p += plf_align256(e.bytes); }
+  return PLF_OK;
+}
+
+plf_status StagedLayout::acquire(plf_ctx* ctx, plf_scratch_slot slot, uint8_t** pin, uint8_t** dev) const {
+  *pin = (uint8_t*)plf_pinned(ctx, in + out);
+  if (!*pin) return PLF_ERR_CUDA;
+  *dev = (uint8_t*)plf_scratch(ctx, slot, in + out + work);
+  return *dev ? PLF_OK : PLF_ERR_CUDA;
+}
+
+void* plf_scratch(plf_ctx* ctx, plf_scratch_slot slot, size_t bytes) {
   DevBuf& b = ctx->scratch[slot];
   if (b.bytes >= bytes && b.p) return b.p;
   if (b.p) {
@@ -54,11 +70,10 @@ void* plf_scratch(plf_ctx* ctx, int slot, size_t bytes) {
     b.p = nullptr;
     b.bytes = 0;
   }
-  size_t want = bytes < 4096 ? 4096 : bytes;
-  want = (want + 255) & ~size_t(255);
+  const size_t want = plf_align256(bytes < 4096 ? 4096 : bytes);
   cudaError_t e = cudaMalloc(&b.p, want + 64);  // + slack for plf_load4 (see plf_image_span)
   if (e != cudaSuccess) {
-    plf_fail(ctx, PLF_ERR_CUDA, "cudaMalloc(%zu) scratch slot %d: %s", want, slot,
+    plf_fail(ctx, PLF_ERR_CUDA, "cudaMalloc(%zu) scratch slot %d: %s", want, (int)slot,
              cudaGetErrorString(e));
     b.p = nullptr;
     return nullptr;

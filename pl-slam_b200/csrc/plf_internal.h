@@ -16,16 +16,53 @@ struct DevBuf {
   size_t bytes = 0;
 };
 
-// The device buffers of one subsystem, declared once as (pointer slot, bytes): the same list gives the footprint, the
-// allocation (one cudaMalloc per buffer, each with 64 bytes of slack for plf_load4, see plf_image_span) and the release.
+// Every buffer carved out of a larger block starts on a 256-byte boundary.
+inline size_t plf_align256(size_t x) { return (x + 255) & ~size_t(255); }
+
+// The scratch slots of a context: device buffers that grow on demand (plf_scratch) and live until plf_destroy.  A slot
+// belongs to the operators named beside it and to nothing else.  An entry point must not call anything that uses its own
+// slot while pointers it carved from that slot are live: the call may reallocate the slot.
+enum plf_scratch_slot {
+  PLF_SCR_MATCH,       // plf_hamming_knn2, plf_match, plf_median_descriptors, plf_match_grid_points / _lines
+  PLF_SCR_LBD,         // plf_lbd_gradients, plf_lbd
+  PLF_SCR_GN,          // plf_gn_pose, plf_se3 (plf_loop_closure_pose calls them one after the other)
+  PLF_SCR_ORB,         // plf_orb
+  PLF_SCR_LSD,         // plf_lsd, plf_detect_lines, plf_debug_sincosf
+  PLF_SCR_MGB_PIPE,    // the windowed matcher of plf_batch_run (matching_strategy != 0)
+  PLF_SCR_BA,          // plf_local_ba, plf_global_ba
+  PLF_SCR_KF,          // plf_match_kf2kf, plf_match_map2kf: their staged layout
+  PLF_SCR_KF_MGB_PT,   // plf_match_kf2kf, plf_match_map2kf: the windowed matcher of points
+  PLF_SCR_KF_MGB_LS,   //   ... and of lines
+  PLF_SCR_BOW,         // plf_bow_insert
+  PLF_SCR_COUNT
+};
+
+// The device buffers of one subsystem or call, declared once as (pointer, bytes).  For persistent buffers the same list
+// gives the footprint, the allocation (one cudaMalloc per buffer, each with 64 bytes of slack for plf_load4, see
+// plf_image_span) and the release; for per-call scratch it gives the carve from a scratch slot.
 struct DevBufList {
-  struct Entry { void** slot; size_t bytes; };
+  struct Entry { void** ptr; size_t bytes; };
   std::vector<Entry> entries;
   template <typename T>
   void add(T*& p, size_t n) { entries.push_back({reinterpret_cast<void**>(&p), n * sizeof(T)}); }
   size_t bytes() const;
   plf_status alloc(plf_ctx* ctx, const char* owner);   // on failure the buffers allocated so far stay listed
-  void release();                                      // frees every buffer and nulls its slot
+  void release();                                      // frees every buffer and nulls its pointer
+  // Points every entry into one block of scratch slot `slot`, each at a 256-byte boundary.  On failure returns
+  // PLF_ERR_CUDA (error set) and leaves the pointers untouched.
+  plf_status carve(plf_ctx* ctx, plf_scratch_slot slot) const;
+};
+
+// The staged layout of one call: the host inputs [0, in), the outputs [in, in + out) and the device-only work after them,
+// with a pinned mirror of inputs and outputs at the same offsets, so one copy uploads and one copy downloads.
+// take_in / take_out / take_work return an offset from the start of their part.
+struct StagedLayout {
+  size_t in = 0, out = 0, work = 0;
+  size_t take_in(size_t b) { const size_t o = in; in += plf_align256(b); return o; }
+  size_t take_out(size_t b) { const size_t o = out; out += plf_align256(b); return o; }
+  size_t take_work(size_t b) { const size_t o = work; work += plf_align256(b); return o; }
+  // Fetches the pinned mirror (in + out bytes) and the device block (in + out + work bytes, scratch slot `slot`).
+  plf_status acquire(plf_ctx* ctx, plf_scratch_slot slot, uint8_t** pin, uint8_t** dev) const;
 };
 
 struct plf_ctx {
@@ -39,8 +76,8 @@ struct plf_ctx {
   plf_limits limits;
   std::string err;
   long long launches = 0;
-  // generic scratch slots (device) used by the host-pointer operator entry points
-  DevBuf scratch[16];
+  // scratch slots (device) of the host-pointer operator entry points
+  DevBuf scratch[PLF_SCR_COUNT];
   // pinned host staging
   void* pinned = nullptr;
   size_t pinned_bytes = 0;
@@ -62,7 +99,7 @@ void plf_mark(plf_ctx* ctx, const char* name);
 
 plf_status plf_fail(plf_ctx* ctx, plf_status code, const char* fmt, ...);
 // Ensures scratch slot `slot` holds at least `bytes`; returns device pointer or nullptr (error set).
-void* plf_scratch(plf_ctx* ctx, int slot, size_t bytes);
+void* plf_scratch(plf_ctx* ctx, plf_scratch_slot slot, size_t bytes);
 void* plf_pinned(plf_ctx* ctx, size_t bytes);
 
 #define PLF_CUDA(ctx, call)                                                                  \
@@ -141,7 +178,7 @@ struct MgbArgs {
   int* count; int count_stride;          // matches of problem p (accumulated; zeroed by the caller)
 };
 // max_n1 / max_n2: upper bounds of the query / train counts; slot: the scratch slot D, the query masks and m21 live in.
-plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n1, int max_n2, int slot);
+plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n1, int max_n2, plf_scratch_slot slot);
 
 // ---- LBD (lbd.cu) ------------------------------------------------------------------------------
 plf_status plf_launch_blur5_sobel(plf_ctx* ctx, const uint8_t* imgs, int pitch, size_t img_stride,
