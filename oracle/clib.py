@@ -115,7 +115,21 @@ def colpiv_qr_solve6(H, g):
     x = np.zeros(6); lib().orc_colpiv_qr_solve6(_p(H), _p(g), _p(x)); return x
 
 
-def gn_pose(cam, P, pl_obs, sP, eP, le_obs, inlier_pt=None, inlier_ls=None, T_init=None, opts=None):
+# stop-decision trace (orc_gn_pose_trace): exit reasons and one record per iteration
+GN_CONTINUE, GN_EXIT_ERROR, GN_EXIT_STEP, GN_EXIT_MAXIT = range(4)
+GN_TRACE_DTYPE = np.dtype([("stage", np.int32), ("exit", np.int32), ("e", np.float64), ("e_prev", np.float64),
+                           ("step", np.float64)])
+GN_ERR_PREV0 = 999999999.9   # the error the first change test compares with (gn.c gn_pose)
+
+
+class orc_gn_trace(C.Structure):
+    _fields_ = [("rec", C.c_void_p), ("cap", C.c_int), ("n", C.c_int), ("stage_exit", C.c_int * 2)]
+
+
+def gn_pose(cam, P, pl_obs, sP, eP, le_obs, inlier_pt=None, inlier_ls=None, T_init=None, opts=None, trace=False):
+    """orc_gn_pose.  trace=True adds res["trace"] = dict(rec=GN_TRACE_DTYPE records, one per accumulation of either
+    stage, exit=(stage-1 exit reason, stage-2 exit reason)).  An accumulation stopped by the error test takes no step
+    and does not count in iters; the others do."""
     f64 = lambda a, k: np.ascontiguousarray(a, np.float64).reshape(-1, k)
     P, pl_obs, sP, eP, le_obs = f64(P, 3), f64(pl_obs, 2), f64(sP, 3), f64(eP, 3), f64(le_obs, 3)
     ip = np.ones(len(P), np.uint8) if inlier_pt is None else np.ascontiguousarray(inlier_pt, np.uint8).copy()
@@ -124,11 +138,45 @@ def gn_pose(cam, P, pl_obs, sP, eP, le_obs, inlier_pt=None, inlier_ls=None, T_in
     c = orc_camera(**cam) if isinstance(cam, dict) else cam
     o = opts if opts is not None else gn_opts()
     out = orc_pose_result()
-    lib().orc_gn_pose(C.byref(c), C.byref(o), _p(P), _p(pl_obs), _p(ip), len(P), _p(sP), _p(eP), _p(le_obs),
-                      _p(il), len(sP), _p(T0), C.byref(out))
-    return dict(T=np.array(out.T).reshape(4, 4), cov=np.array(out.cov).reshape(6, 6), x=np.array(out.x),
-                err=out.err, iters=(out.iters1, out.iters2), inlier_pt=ip, inlier_ls=il,
-                n_inliers=(out.n_inliers_pt, out.n_inliers_ls))
+    args = (C.byref(c), C.byref(o), _p(P), _p(pl_obs), _p(ip), len(P), _p(sP), _p(eP), _p(le_obs), _p(il), len(sP),
+            _p(T0), C.byref(out))
+    if trace:
+        rec = np.zeros(max(o.max_iters, 0) + max(o.max_iters_ref, 0), GN_TRACE_DTYPE)
+        tr = orc_gn_trace(rec.ctypes.data, len(rec), 0)
+        lib().orc_gn_pose_trace(*args, C.byref(tr))
+        assert tr.n <= len(rec)
+    else:
+        lib().orc_gn_pose(*args)
+    res = dict(T=np.array(out.T).reshape(4, 4), cov=np.array(out.cov).reshape(6, 6), x=np.array(out.x),
+               err=out.err, iters=(out.iters1, out.iters2), inlier_pt=ip, inlier_ls=il,
+               n_inliers=(out.n_inliers_pt, out.n_inliers_ls))
+    if trace:
+        res["trace"] = dict(rec=rec[:tr.n].copy(), exit=(tr.stage_exit[0], tr.stage_exit[1]))
+    return res
+
+
+def gn_decidable(trace, opts, rel_band=1e-10):
+    """True when the iteration counts of a run are well defined under a change of summation order: every stop test the
+    oracle evaluated (trace of gn_pose(..., trace=True)) lies outside the band that order can move it by.
+
+    A solver that sums its rows in another order (a tree on the device) sees each error e with a relative difference of
+    about 1e-12, so a test within rel_band * max(e, e_prev) of its threshold (the change test | |e - e_prev| -
+    eps_change |, then the error test |e - eps_err|, which is only evaluated when the change test fails) may go either
+    way, and so may a step test with ||dx|| within [eps_step / 10, 10 eps_step].  The constant first e_prev
+    (GN_ERR_PREV0) carries no rounding and does not widen the band.  A NaN error (no row left) fails both tests on
+    every solver, and so does not count as near."""
+    for r in trace["rec"]:
+        e, ep = float(r["e"]), float(r["e_prev"])
+        if not np.isnan(e):
+            band = rel_band * (e if ep == GN_ERR_PREV0 else max(e, ep))
+            change = abs(e - ep)
+            if abs(change - opts.eps_change) <= band:
+                return False
+            if not change < opts.eps_change and abs(e - opts.eps_err) <= band:
+                return False
+        if r["step"] >= 0 and opts.eps_step / 10 <= r["step"] <= 10 * opts.eps_step:
+            return False
+    return True
 
 
 # ---- ORB (oracle/orb.c) ------------------------------------------------------------------------------

@@ -298,12 +298,14 @@ def track(prev: Frame, curr: Frame, prm, match_fn=None, cam=None):
 
 def optimize_pose(cam, tr, prm):
     """optimizePose: two-stage GN from identity; fewer than min_features rows -> identity.  Returns curr.DT
-    (= inverse of the optimised increment), the raw result and a status flag."""
+    (= inverse of the optimised increment), the raw result (with the solver's stop-decision trace, its options, camera
+    and rows, so that a result of another solver can be compared with it: clib.gn_decidable) and a status flag."""
     n = len(tr["P"]) + len(tr["sP"])
     if n < prm["min_features"]:
         return np.eye(4), None, 1
     o = clib.gn_opts(prm["homog_th"], prm["max_iters"], prm["max_iters_ref"], prm["min_error"], prm["min_error_change"])
-    r = clib.gn_pose(cam, tr["P"], tr["obs"], tr["sP"], tr["eP"], tr["le"], opts=o)
+    r = clib.gn_pose(cam, tr["P"], tr["obs"], tr["sP"], tr["eP"], tr["le"], opts=o, trace=True)
+    r.update(opts=o, cam=cam, rows={k: tr[k] for k in ("P", "obs", "sP", "eP", "le")})
     return clib.inverse_se3(r["T"]), r, 0
 
 

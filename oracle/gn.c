@@ -322,13 +322,25 @@ static int gn_accumulate(const orc_camera* cam, double homog_th, const double* T
   return N_l + N_p;
 }
 
+static void trace_put(orc_gn_trace* tr, const orc_gn_trace_rec* r) {
+  if (tr->n < tr->cap) tr->rec[tr->n] = *r;
+  tr->n++;
+}
+
+/* One stage.  tr (may be NULL) receives one record per accumulation and the stage's exit reason. */
 static int gn_stage(const orc_camera* cam, const orc_gn_opts* o, int max_iters, double* T, const double* P,
                     const double* obs, const uint8_t* inl_p, int np, const double* sP, const double* eP,
-                    const double* le, const uint8_t* inl_l, int nl, double* H, double* g, double* e, double* err_prev) {
-  int it = 0;
+                    const double* le, const uint8_t* inl_l, int nl, double* H, double* g, double* e, double* err_prev,
+                    int stage, orc_gn_trace* tr) {
+  int it = 0, why = ORC_GN_EXIT_MAXIT;
   for (; it < max_iters; it++) {
     gn_accumulate(cam, o->homog_th, T, P, obs, inl_p, np, sP, eP, le, inl_l, nl, H, g, e);
-    if (fabs(*e - *err_prev) < o->eps_change || *e < o->eps_err) break;
+    orc_gn_trace_rec rec = {stage, ORC_GN_CONTINUE, *e, *err_prev, -1.0};
+    if (fabs(*e - *err_prev) < o->eps_change || *e < o->eps_err) {
+      why = rec.exit = ORC_GN_EXIT_ERROR;
+      if (tr) trace_put(tr, &rec);
+      break;
+    }
     double dx[6], E[16], Ei[16];
     orc_colpiv_qr_solve6(H, g, dx);
     orc_expmap_se3(dx, E);
@@ -336,19 +348,28 @@ static int gn_stage(const orc_camera* cam, const orc_gn_opts* o, int max_iters, 
     mat4_mul(T, Ei, T);
     double nrm = 0;
     for (int k = 0; k < 6; k++) nrm += dx[k] * dx[k];
-    if (sqrt(nrm) < o->eps_step) { it++; break; }
+    rec.step = sqrt(nrm);
+    if (sqrt(nrm) < o->eps_step) {
+      why = rec.exit = ORC_GN_EXIT_STEP;
+      if (tr) trace_put(tr, &rec);
+      it++;
+      break;
+    }
+    if (it + 1 == max_iters) rec.exit = ORC_GN_EXIT_MAXIT;
+    if (tr) trace_put(tr, &rec);
     *err_prev = *e;
   }
+  if (tr) tr->stage_exit[stage] = why;
   return it;
 }
 
 /* Two-stage robust GN (:3566-3957).  T_init/T_out row-major 4x4.  inl_* are updated in place. */
-void orc_gn_pose(const orc_camera* cam, const orc_gn_opts* o, const double* P, const double* obs, uint8_t* inl_p,
-                 int np, const double* sP, const double* eP, const double* le, uint8_t* inl_l, int nl,
-                 const double* T_init, orc_pose_result* out) {
+static void gn_pose(const orc_camera* cam, const orc_gn_opts* o, const double* P, const double* obs, uint8_t* inl_p,
+                    int np, const double* sP, const double* eP, const double* le, uint8_t* inl_l, int nl,
+                    const double* T_init, orc_pose_result* out, orc_gn_trace* tr) {
   double T[16], H[36] = {0}, g[6] = {0}, e = 0, err_prev = 999999999.9;
   memcpy(T, T_init, sizeof T);
-  out->iters1 = gn_stage(cam, o, o->max_iters, T, P, obs, inl_p, np, sP, eP, le, inl_l, nl, H, g, &e, &err_prev);
+  out->iters1 = gn_stage(cam, o, o->max_iters, T, P, obs, inl_p, np, sP, eP, le, inl_l, nl, H, g, &e, &err_prev, 0, tr);
   const double gate = sqrt(7.815);
   for (int i = 0; i < np; i++) {
     if (!inl_p[i]) continue;
@@ -360,7 +381,7 @@ void orc_gn_pose(const orc_camera* cam, const orc_gn_opts* o, const double* P, c
     double e2[2], a[3], b[3];
     if (line_residual(cam, T, sP + 3 * i, eP + 3 * i, le + 3 * i, e2, a, b) > gate) inl_l[i] = 0;
   }
-  out->iters2 = gn_stage(cam, o, o->max_iters_ref, T, P, obs, inl_p, np, sP, eP, le, inl_l, nl, H, g, &e, &err_prev);
+  out->iters2 = gn_stage(cam, o, o->max_iters_ref, T, P, obs, inl_p, np, sP, eP, le, inl_l, nl, H, g, &e, &err_prev, 1, tr);
   memcpy(out->T, T, sizeof T);
   orc_logmap_se3(T, out->x);
   out->err = e;
@@ -370,4 +391,19 @@ void orc_gn_pose(const orc_camera* cam, const orc_gn_opts* o, const double* P, c
   for (int i = 0; i < nl; i++) b += inl_l[i] != 0;
   out->n_inliers_pt = a;
   out->n_inliers_ls = b;
+}
+
+void orc_gn_pose(const orc_camera* cam, const orc_gn_opts* o, const double* P, const double* obs, uint8_t* inl_p,
+                 int np, const double* sP, const double* eP, const double* le, uint8_t* inl_l, int nl,
+                 const double* T_init, orc_pose_result* out) {
+  gn_pose(cam, o, P, obs, inl_p, np, sP, eP, le, inl_l, nl, T_init, out, NULL);
+}
+
+/* orc_gn_pose plus the stop-decision trace: what each stop test saw, so that a caller comparing iteration counts
+ * with a solver that sums in another order can tell whether a test sat on its threshold. */
+void orc_gn_pose_trace(const orc_camera* cam, const orc_gn_opts* o, const double* P, const double* obs, uint8_t* inl_p,
+                       int np, const double* sP, const double* eP, const double* le, uint8_t* inl_l, int nl,
+                       const double* T_init, orc_pose_result* out, orc_gn_trace* tr) {
+  tr->n = 0;
+  gn_pose(cam, o, P, obs, inl_p, np, sP, eP, le, inl_l, nl, T_init, out, tr);
 }

@@ -74,6 +74,23 @@ int orc_inverse6(const double* A, double* Ainv);
 void orc_gn_pose(const orc_camera* cam, const orc_gn_opts* o, const double* P, const double* obs, uint8_t* inl_p,
                  int np, const double* sP, const double* eP, const double* le, uint8_t* inl_l, int nl,
                  const double* T_init, orc_pose_result* out);
+/* Stop-decision trace of orc_gn_pose_trace: one record per accumulation of either stage, in order. */
+enum { ORC_GN_CONTINUE = 0, ORC_GN_EXIT_ERROR = 1, ORC_GN_EXIT_STEP = 2, ORC_GN_EXIT_MAXIT = 3 };
+typedef struct orc_gn_trace_rec {
+  int stage;     /* 0 (robust) or 1 (refinement after the gate) */
+  int exit;      /* ORC_GN_CONTINUE, or why the stage ended on this iteration */
+  double e;      /* normalised error of this iteration's accumulation */
+  double e_prev; /* the error the change test compared it with */
+  double step;   /* ||dx|| of the step taken; -1 when the error test stopped the stage first */
+} orc_gn_trace_rec;
+typedef struct orc_gn_trace {
+  orc_gn_trace_rec* rec;
+  int cap, n;        /* records available / accumulations made (those past cap are counted, not stored) */
+  int stage_exit[2]; /* why each stage ended (ORC_GN_EXIT_MAXIT also for a stage of 0 iterations) */
+} orc_gn_trace;
+void orc_gn_pose_trace(const orc_camera* cam, const orc_gn_opts* o, const double* P, const double* obs, uint8_t* inl_p,
+                       int np, const double* sP, const double* eP, const double* le, uint8_t* inl_l, int nl,
+                       const double* T_init, orc_pose_result* out, orc_gn_trace* tr);
 
 /* ---- local bundle adjustment (oracle/lba.c; src/mapHandler.cpp:1332-1989) ---- */
 typedef struct orc_lba_opts {

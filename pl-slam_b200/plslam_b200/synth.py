@@ -66,15 +66,15 @@ def project(cam, P):
     return np.stack([cam["cx"] + cam["fx"] * P[:, 0] / P[:, 2], cam["cy"] + cam["fy"] * P[:, 1] / P[:, 2]], 1)
 
 
-def gn_problem(cam, n_pts=300, n_lines=80, seed=0, x_true=None, px_noise=0.3, outlier_frac=0.1):
-    """3-D points / segments in the previous camera frame + their observations in the current frame under a
-    planted increment T_true (current <- previous), with pixel noise and gross outliers."""
+def gn_problem(cam, n_pts=300, n_lines=80, seed=0, x_true=None, px_noise=0.3, outlier_frac=0.1, z_range=(4, 40)):
+    """3-D points / segments in the previous camera frame (depths uniform in z_range) + their observations in the
+    current frame under a planted increment T_true (current <- previous), with pixel noise and gross outliers."""
     rng = np.random.default_rng(seed)
     if x_true is None:
         x_true = np.array([0.05, -0.02, 0.9, 0.01, -0.03, 0.005])
     T = expmap_se3(x_true)
     def rand_pts(n):
-        z = rng.uniform(4, 40, n)
+        z = rng.uniform(z_range[0], z_range[1], n)
         u = rng.uniform(30, cam["width"] - 30, n); v = rng.uniform(20, cam["height"] - 20, n)
         return np.stack([(u - cam["cx"]) * z / cam["fx"], (v - cam["cy"]) * z / cam["fy"], z], 1)
     P = rand_pts(n_pts)

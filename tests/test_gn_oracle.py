@@ -52,3 +52,43 @@ def test_outliers_are_gated():
 def test_degenerate_inputs():
     r = clib.gn_pose(CAM, np.zeros((0, 3)), np.zeros((0, 2)), np.zeros((0, 3)), np.zeros((0, 3)), np.zeros((0, 3)))
     assert np.allclose(r["T"], np.eye(4)) and r["n_inliers"] == (0, 0)
+
+
+@pytest.mark.parametrize("cfg", [dict(max_iters=5, max_iters_ref=10), dict(max_iters=100, max_iters_ref=100),
+                                 dict(max_iters=100, max_iters_ref=100, eps_change=1e-2),
+                                 dict(max_iters=20, max_iters_ref=20, eps_step=1e-3),
+                                 dict(max_iters=0, max_iters_ref=1), dict(max_iters=1, max_iters_ref=0)])
+@pytest.mark.parametrize("exact", [False, True])
+def test_stop_trace_consistent_with_result(cfg, exact):
+    """orc_gn_pose_trace: one record per accumulation, in stage order; a stage's iteration count is its records
+    minus the one the error test stopped without a step; the stage's exit reason is its last record's (max_iters when
+    it ran none); the change test compares each error with the last one that took a step; the last error is err; and
+    the trace does not change the result."""
+    pr = synth.gn_problem(CAM, seed=9, **(dict(px_noise=0.0, outlier_frac=0.0) if exact else {}))
+    o = clib.gn_opts(**cfg)
+    r = clib.gn_pose(CAM, pr["P"], pr["obs"], pr["sP"], pr["eP"], pr["le"], opts=o, trace=True)
+    plain = clib.gn_pose(CAM, pr["P"], pr["obs"], pr["sP"], pr["eP"], pr["le"], opts=o)
+    for k in ("T", "cov", "x", "inlier_pt", "inlier_ls"):
+        assert np.array_equal(r[k], plain[k], equal_nan=True), k
+    assert r["iters"] == plain["iters"] and r["n_inliers"] == plain["n_inliers"]
+    rec, exits = r["trace"]["rec"], r["trace"]["exit"]
+    assert np.all(np.diff(rec["stage"]) >= 0)
+    e_prev = clib.GN_ERR_PREV0
+    for s in (0, 1):
+        st = rec[rec["stage"] == s]
+        assert len(st) <= (o.max_iters, o.max_iters_ref)[s]
+        assert r["iters"][s] == len(st) - (exits[s] == clib.GN_EXIT_ERROR)
+        assert exits[s] == (st["exit"][-1] if len(st) else clib.GN_EXIT_MAXIT)
+        assert np.all(st["exit"][:-1] == clib.GN_CONTINUE)
+        for t in st:
+            assert t["e_prev"] == e_prev
+            took_step = t["exit"] != clib.GN_EXIT_ERROR
+            assert (t["step"] >= 0) == took_step
+            if t["exit"] == clib.GN_EXIT_ERROR:
+                assert abs(t["e"] - t["e_prev"]) < o.eps_change or t["e"] < o.eps_err
+            if t["exit"] == clib.GN_EXIT_STEP:
+                assert t["step"] < o.eps_step
+            if t["exit"] in (clib.GN_CONTINUE, clib.GN_EXIT_MAXIT):
+                e_prev = t["e"]
+    if len(rec):
+        assert rec["e"][-1] == r["err"]
