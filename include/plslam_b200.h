@@ -201,7 +201,9 @@ typedef struct plf_keypoint {
  * Output order is canonical (octave, y, x): OpenCV's own order inside a level is the implementation-defined
  * result of std::nth_element (KeyPointsFilter::retainBest); the SET of keypoints, every field and every
  * descriptor are identical to OpenCV's.  kps/desc: host buffers with room for `cap` entries; *n receives
- * the count (PLF_ERR_CAPACITY if it exceeds cap or the ctx limit max_keypoints). */
+ * the count (PLF_ERR_CAPACITY if it exceeds cap or the ctx limit max_keypoints).  Work is enqueued on plf_stream in a
+ * working state of its own (one image, rebuilt when the image size changes) and never touches the batched pipeline's
+ * buffers, so a call between batches in flight is safe. */
 plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, plf_keypoint* kps,
                    uint8_t* desc, int cap, int* n);
 
@@ -227,14 +229,18 @@ typedef struct plf_keyline {
 /* Raw LSD segments.  Replaces cv::createLineSegmentDetector(lsd_refine (0), lsd_scale, lsd_sigma_scale, lsd_quant,
  * lsd_ang_th, lsd_log_eps, lsd_density_th, lsd_n_bins)->detect(img, lines) as called at
  * 3rdparty/line_descriptor/src/LSDDetector_custom.cpp:246-264.  segs: cap x 4 floats (x1,y1,x2,y2), OpenCV's
- * output order (seed order).  *n receives the count. */
+ * output order (seed order).  *n receives the count.  Work is enqueued on plf_stream in a working state of its own (one
+ * image, rebuilt when the image size changes, shared with plf_detect_lines) and never touches the batched pipeline's
+ * buffers, so a call between batches in flight is safe. */
 plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, float* segs, int cap, int* n);
 
 /* Line features of one image.  Replaces stvo-pl StereoFrame::detectLineFeatures (LSD branch):
  * LSDDetectorC::detect(img, lines, scale, 1, opts) (LSDDetector_custom.cpp:218-324, opts.min_length =
  * min_line_length * min(w,h)), then — when more than lsd_nfeatures lines are found and lsd_nfeatures != 0 — sort by
  * response (descending; ties keep detection order), keep lsd_nfeatures and set class_id = rank, then
- * BinaryDescriptor::compute (binary_descriptor_custom.cpp:524).  keylines/desc: host buffers of `cap` entries. */
+ * BinaryDescriptor::compute (binary_descriptor_custom.cpp:524).  keylines/desc: host buffers of `cap` entries.
+ * Enqueued on plf_stream in plf_lsd's working state; never touches the batched pipeline's buffers, so a call between
+ * batches in flight is safe. */
 plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride,
                             plf_keyline* keylines, uint8_t* desc, int cap, int* n);
 

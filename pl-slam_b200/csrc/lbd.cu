@@ -28,12 +28,6 @@
 #define LBD_WB 7
 #define LBD_ROWS 63
 
-plf_status plf_lbd_init(plf_ctx* ctx);
-
-struct LbdState {
-  PlfTmaCache tm;   // source images of k_blur5_sobel_fast
-};
-
 __constant__ float c_gaussL[21];  // (float)gaussCoefL_[i]
 __constant__ float c_gaussG[63];  // (float)gaussCoefG_[i]
 __constant__ int c_comb[32][2];
@@ -188,16 +182,14 @@ __global__ void __launch_bounds__(256) k_blur5_sobel_fast(const __grid_constant_
   }
 }
 
-plf_status plf_launch_blur5_sobel(plf_ctx* ctx, const uint8_t* imgs, int pitch, size_t img_stride,
+plf_status plf_launch_blur5_sobel(plf_ctx* ctx, PlfTmaCache* tm, const uint8_t* imgs, int pitch, size_t img_stride,
                                   int w, int h, int nimg, short2* grad, size_t grad_stride) {
   if (nimg <= 0) return PLF_OK;
   if (w >= 8 && h >= 8 && (pitch & 15) == 0 && (img_stride & 15) == 0 && ((uintptr_t)imgs & 15) == 0) {
-    plf_status st0 = plf_lbd_init(ctx);
-    if (st0) return st0;
-    const CUtensorMap* tm = ctx->lbd->tm.get(imgs, w, h, nimg, pitch, img_stride ? img_stride : (size_t)pitch * h, 80, LBF_TH + 6);
-    if (!tm) return plf_fail(ctx, PLF_ERR_CUDA, "LBD: cuTensorMapEncodeTiled failed (pitch %d, stride %zu)", pitch, img_stride);
+    const CUtensorMap* map = tm->get(imgs, w, h, nimg, pitch, img_stride ? img_stride : (size_t)pitch * h, 80, LBF_TH + 6);
+    if (!map) return plf_fail(ctx, PLF_ERR_CUDA, "LBD: cuTensorMapEncodeTiled failed (pitch %d, stride %zu)", pitch, img_stride);
     dim3 grid(plf_tma_tiles_x(w, 3), (h + LBF_TH - 1) / LBF_TH, nimg);
-    k_blur5_sobel_fast<<<grid, 256, 0, ctx->cur>>>(*tm, w, h, grad, grad_stride);
+    k_blur5_sobel_fast<<<grid, 256, 0, ctx->cur>>>(*map, w, h, grad, grad_stride);
   } else {  // tiny images / unpadded rows: generic kernel
     dim3 grid((w + LBD_TW - 1) / LBD_TW, (h + LBD_TH - 1) / LBD_TH, nimg);
     k_blur5_sobel<<<grid, 256, 0, ctx->cur>>>(imgs, pitch, img_stride, w, h, grad, grad_stride);
@@ -332,8 +324,8 @@ __global__ void __launch_bounds__(64, 12) k_lbd(const short2* __restrict__ grad,
   }
 }
 
-plf_status plf_lbd_init(plf_ctx* ctx) {
-  if (ctx->lbd) return PLF_OK;
+static plf_status plf_lbd_init(plf_ctx* ctx) {
+  if (ctx->lbd_tables) return PLF_OK;
   // BinaryDescriptor ctor, binary_descriptor_custom.cpp:217-259 (host doubles, narrowed at use sites)
   float gl[21], gg[63];
   {
@@ -354,7 +346,7 @@ plf_status plf_lbd_init(plf_ctx* ctx) {
   PLF_CUDA(ctx, cudaMemcpyToSymbolAsync(c_gaussG, gg, sizeof gg, 0, cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyToSymbolAsync(c_comb, h_comb, sizeof h_comb, 0, cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  ctx->lbd = new LbdState();
+  ctx->lbd_tables = true;
   return PLF_OK;
 }
 
@@ -370,16 +362,12 @@ plf_status plf_launch_lbd(plf_ctx* ctx, const short2* grad, size_t grad_stride, 
   return PLF_OK;
 }
 
-extern "C" void plf_lbd_free(plf_ctx* ctx) {
-  delete ctx->lbd;
-  ctx->lbd = nullptr;
-}
-
 extern "C" plf_status plf_lbd_gradients(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride,
                                         int16_t* dxdy) {
   if (!ctx || !img || !dxdy || w < 2 || h < 2 || stride < w)
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_lbd_gradients: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  ctx->cur = ctx->stream;
   const int pitch = plf_pitch16(w);
   uint8_t* dimg;
   short2* dgrad;
@@ -387,7 +375,8 @@ extern "C" plf_status plf_lbd_gradients(plf_ctx* ctx, const uint8_t* img, int w,
   scr.add(dimg, (size_t)pitch * h); scr.add(dgrad, (size_t)w * h);
   if (plf_status st = scr.carve(ctx, PLF_SCR_LBD)) return st;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  plf_status st = plf_launch_blur5_sobel(ctx, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
+  PlfTmaCache tm;
+  plf_status st = plf_launch_blur5_sobel(ctx, &tm, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
   if (st) return st;
   PLF_CUDA(ctx, cudaMemcpyAsync(dxdy, dgrad, (size_t)w * h * 4, cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -405,6 +394,7 @@ extern "C" plf_status plf_lbd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   if (n > 32767)
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_lbd: %d lines (reference numOfFinalLine is a short, :1029)", n);
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  ctx->cur = ctx->stream;
   const int pitch = plf_pitch16(w);
   uint8_t *dimg, *ddesc;
   short2* dgrad;
@@ -418,7 +408,8 @@ extern "C" plf_status plf_lbd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyAsync(dkl, keylines, (size_t)n * sizeof(plf_keyline), cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyAsync(dcount, &n, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-  plf_status st = plf_launch_blur5_sobel(ctx, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
+  PlfTmaCache tm;
+  plf_status st = plf_launch_blur5_sobel(ctx, &tm, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
   if (st) return st;
   st = plf_launch_lbd(ctx, dgrad, 0, w, h, 1, dkl, dcount, n, ddesc, desc_float ? dfl : nullptr);
   if (st) return st;

@@ -11,8 +11,9 @@
 // inside a bin) -> greedy region growing -> rectangle fit.  No NFA validation runs at refine 0.
 //
 // Kernels
-//   k_lsd_build_lut / k_lsd_fill_notdef
-//                    once per state: the gradient lookup tables, and every record of the record maps set to "undefined"
+//   k_lsd_build_lut  once per context: the gradient lookup tables (LsdTables)
+//   k_lsd_fill_notdef
+//                    once per state: every record of the record maps set to "undefined"
 //   k_blur_q8_fast   separable Q8.8 Gaussian of 5 or 7 taps <= 255 (tile + halo staged by one TMA bulk-tensor copy, DP4A
 //                    row pass), one rounding (k_blur_q8: generic variant for the other kernels, up to 15 taps)
 //   k_resize_exact4  (orb.cu) INTER_LINEAR_EXACT resample to scale
@@ -54,14 +55,24 @@
 #define LSD_BINS_MAX 1024
 #define LSD_QCAP 256   // shared-memory window of the region queue (entries)
 
+// What LSD derives from the context's parameters alone, built once per context and read by every LSD state.
+struct LsdTables {
+  int ksize = 0;            // Gaussian pre-blur (0: scale 1, no blur); its taps are also in c_lsd_taps
+  int taps[16];
+  bool taps_u8 = false;     // every tap <= 255: the packed-byte fast blur applies (a 256 centre tap at small sigma does not)
+  double prec = 0, p = 0, rho = 0;
+  int m2_min = 0;           // smallest gx^2+gy^2 whose gradient norm exceeds rho (defined pixel)
+  float* angle_lut = nullptr;   // [1021*1021] gradient (gx,gy) -> level-line angle (degrees) of a defined pixel
+  float2* cs_lut = nullptr;     // [1021*1021] gradient (gx,gy) -> (cosf, sinf) of float(angle in radians): a member's term of the region sums
+  float2* seed_lut = nullptr;   // [1021*1021] gradient (gx,gy) -> unit vector of a region seed
+  DevBufList bufs;
+};
+
 struct LsdState {
   int w = 0, h = 0, nimg = 0;
   int ws = 0, hs = 0;       // scaled size
-  int ksize = 0;
-  int taps[16];
-  bool taps_u8 = false;     // every tap <= 255: the packed-byte fast blur applies (a 256 centre tap at small sigma does not)
   int n_bins = 1024;
-  double scale = 1.2, prec = 0, p = 0, rho = 0;
+  double scale = 1.2;
   int min_reg_size = 0;
   int max_regions = 0, max_lines = 0;
   bool two_parities = false;
@@ -73,7 +84,6 @@ struct LsdState {
   struct LsdPix* pix_raw[2] = {nullptr, nullptr};  // allocation (pix + look-ahead slack on both sides)
   struct LsdPix* pix[2] = {nullptr, nullptr};  // [nimg][guard + hs*ws]  {angle (deg, f32) | NOTDEF = undefined/used, table index}
   size_t pix_stride = 0;      // entries per image = guard (ws+1, permanently NOTDEF) + hs*ws
-  int m2_min = 0;             // smallest gx^2+gy^2 whose gradient norm exceeds rho (defined pixel)
   // seed lists per row segment (LSD_SEG columns): segment (y, xb) owns the entries [y * ws + LSD_SEG * xb, ...);
   // an entry is column-in-segment | gx^2+gy^2 << LSD_COL_BITS (k_lsd_grad), then column | bin << LSD_COL_BITS (k_lsd_rowhist)
   uint32_t* seedlist = nullptr; // [nimg][hs*ws]
@@ -96,9 +106,6 @@ struct LsdState {
   int* overflow = nullptr;    // [1]
   int* rs_tab = nullptr;      // resize tables
   size_t rs_x_off = 0, rs_y_off = 0, rs_xp_off = 0;
-  float* angle_lut = nullptr;   // [1021*1021] gradient (gx,gy) -> level-line angle (degrees) of a defined pixel
-  float2* cs_lut = nullptr;     // [1021*1021] gradient (gx,gy) -> (cosf, sinf) of float(angle in radians): a member's term of the region sums
-  float2* seed_lut = nullptr;   // [1021*1021] gradient (gx,gy) -> unit vector of a region seed
   DevBufList bufs;
 };
 
@@ -1051,12 +1058,10 @@ __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ se
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------
-extern "C" void plf_lsd_free(plf_ctx* ctx) {
-  if (ctx->lsd) {
-    ctx->lsd->bufs.release();
-    delete ctx->lsd;
-    ctx->lsd = nullptr;
-  }
+void plf_lsd_free(LsdState* s) {
+  if (!s) return;
+  s->bufs.release();
+  delete s;
 }
 
 // getGaussianKernelBitExact + fixed-point error diffusion (see oracle/lbd.c orc_gaussian_kernel_q8)
@@ -1100,7 +1105,7 @@ static size_t lsd_pix_records(const LsdState* s) { return s->pix_stride * s->nim
 
 // The device buffers of an LSD state whose sizes are set (lsd_set_sizes), and the layout derived from those sizes.
 static void lsd_buffers(LsdState* s, DevBufList& b) {
-  const size_t N = (size_t)s->nimg, As = (size_t)s->ws * s->hs, R = (size_t)s->max_regions, LUT = (size_t)LSD_LUT_DIM * LSD_LUT_DIM;
+  const size_t N = (size_t)s->nimg, As = (size_t)s->ws * s->hs, R = (size_t)s->max_regions;
   s->bp = plf_pitch16(s->w); s->sp = plf_pitch16(s->ws);
   s->nxb = (s->ws + LSD_SEG - 1) / LSD_SEG;
   s->pix_stride = As + (size_t)s->ws + 1;
@@ -1118,7 +1123,7 @@ static void lsd_buffers(LsdState* s, DevBufList& b) {
   b.add(s->segs, N * R);
   b.add(s->kls_all, N * R);
   // buffers that cross from the pre-grow phase to the growing (or to the match phase) exist twice (parity of the batch),
-  // so that batch i+1 can be extracted while batch i is still growing regions; standalone operators use parity 0 only
+  // so that batch i+1 can be extracted while batch i is still growing regions
   for (int p = 0; p < (s->two_parities ? 2 : 1); ++p) {
     b.add(s->pix_raw[p], lsd_pix_records(s));
     b.add(s->nseeds[p], N);
@@ -1127,9 +1132,6 @@ static void lsd_buffers(LsdState* s, DevBufList& b) {
     b.add(s->nlines[p], N);
   }
   b.add(s->overflow, 1);
-  b.add(s->angle_lut, LUT);
-  b.add(s->cs_lut, LUT);
-  b.add(s->seed_lut, LUT);
   if (s->scale != 1.0) {
     s->rs_x_off = 0;
     s->rs_y_off = 2 * (size_t)s->ws;
@@ -1146,43 +1148,68 @@ size_t plf_lsd_footprint(const plf_ctx* ctx, int w, int h, int nimg, bool two_pa
   return b.bytes();
 }
 
-static plf_status lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
-  LsdState* s = ctx->lsd;
-  if (s && s->w == w && s->h == h && s->nimg >= nimg && (s->two_parities || !two_parities)) return PLF_OK;
-  if (s && s->two_parities) two_parities = true;
-  if (s) {
-    PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    s->bufs.release();
-    *s = LsdState();
-  } else {
-    s = ctx->lsd = new LsdState();
-  }
+static plf_status lsd_tables_build(plf_ctx* ctx, LsdTables* t) {
   const plf_params& P = ctx->params;
   if (P.lsd_refine != 0)
     return plf_fail(ctx, PLF_ERR_INVALID, "LSD: only lsd_refine = 0 (LSD_REFINE_NONE, the reference configs) is supported");
   if (P.lsd_n_bins < 1 || P.lsd_n_bins > LSD_BINS_MAX)
     return plf_fail(ctx, PLF_ERR_INVALID, "LSD: lsd_n_bins must be in [1,%d]", LSD_BINS_MAX);
-  lsd_set_sizes(ctx, s, w, h, nimg, two_parities);
-  s->prec = LSD_PI * P.lsd_ang_th / 180;
-  s->p = P.lsd_ang_th / 180;
-  s->rho = P.lsd_quant / sin(s->prec);
-  if (s->scale != 1.0) {
-    const double sigma = (s->scale < 1) ? (P.lsd_sigma_scale / s->scale) : P.lsd_sigma_scale;
+  t->prec = LSD_PI * P.lsd_ang_th / 180;
+  t->p = P.lsd_ang_th / 180;
+  t->rho = P.lsd_quant / sin(t->prec);
+  const double scale = P.lsd_scale;
+  if (scale != 1.0) {
+    const double sigma = (scale < 1) ? (P.lsd_sigma_scale / scale) : P.lsd_sigma_scale;
     const unsigned hk = (unsigned)(ceil(sigma * sqrt(2 * 3.0 * log(10.0))));
-    s->ksize = 1 + 2 * (int)hk;
-    if (s->ksize > 15) return plf_fail(ctx, PLF_ERR_INVALID, "LSD: Gaussian kernel %d > 15 unsupported", s->ksize);
-    gaussian_taps_q8(s->ksize, sigma, s->taps);
-    s->taps_u8 = true;
-    for (int k = 0; k < s->ksize; ++k) s->taps_u8 = s->taps_u8 && s->taps[k] <= 255;
-  } else {
-    s->ksize = 0;
+    t->ksize = 1 + 2 * (int)hk;
+    if (t->ksize > 15) return plf_fail(ctx, PLF_ERR_INVALID, "LSD: Gaussian kernel %d > 15 unsupported", t->ksize);
+    gaussian_taps_q8(t->ksize, sigma, t->taps);
+    t->taps_u8 = true;
+    for (int k = 0; k < t->ksize; ++k) t->taps_u8 = t->taps_u8 && t->taps[k] <= 255;
   }
+  for (t->m2_min = 0; t->m2_min <= 2 * 510 * 510; ++t->m2_min)  // same double expression as the kernels
+    if (!(sqrt((double)t->m2_min / 4.0) <= t->rho)) break;
+  const size_t LUT = (size_t)LSD_LUT_DIM * LSD_LUT_DIM;
+  t->bufs.add(t->angle_lut, LUT);
+  t->bufs.add(t->cs_lut, LUT);
+  t->bufs.add(t->seed_lut, LUT);
+  plf_status st = t->bufs.alloc(ctx, "LSD tables");
+  if (st) return st;
+  k_lsd_build_lut<<<(LSD_LUT_DIM * LSD_LUT_DIM + 255) / 256, 256, 0, ctx->stream>>>(t->rho, t->angle_lut, t->cs_lut, t->seed_lut);
+  PLF_LAUNCH_CHECK(ctx);
+  if (scale != 1.0)
+    PLF_CUDA(ctx, cudaMemcpyToSymbolAsync(c_lsd_taps, t->taps, sizeof(int) * 16, 0, cudaMemcpyHostToDevice, ctx->stream));
+  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return PLF_OK;
+}
+
+// Once per context, before any LSD state: c_lsd_taps is written here only, never while an LSD kernel may read it.
+plf_status plf_lsd_tables(plf_ctx* ctx) {
+  if (ctx->lsd_tables) return PLF_OK;
+  LsdTables* t = new LsdTables();
+  const plf_status st = lsd_tables_build(ctx, t);
+  if (st) {
+    t->bufs.release();
+    delete t;
+    return st;
+  }
+  ctx->lsd_tables = t;
+  return PLF_OK;
+}
+
+void plf_lsd_tables_free(plf_ctx* ctx) {
+  if (!ctx->lsd_tables) return;
+  ctx->lsd_tables->bufs.release();
+  delete ctx->lsd_tables;
+  ctx->lsd_tables = nullptr;
+}
+
+static plf_status lsd_build(plf_ctx* ctx, LsdState* s, int w, int h, int nimg, bool two_parities) {
+  lsd_set_sizes(ctx, s, w, h, nimg, two_parities);
   if (s->ws >= 65536 || s->hs >= 65536 || s->ws < 3 || s->hs < 3)
     return plf_fail(ctx, PLF_ERR_INVALID, "LSD: scaled image %dx%d out of range", s->ws, s->hs);
   const double LOG_NT = 5 * (log10((double)s->ws) + log10((double)s->hs)) / 2 + log10(11.0);
-  s->min_reg_size = (int)(size_t)(-LOG_NT / log10(s->p));
-  for (s->m2_min = 0; s->m2_min <= 2 * 510 * 510; ++s->m2_min)  // same double expression as the kernels
-    if (!(sqrt((double)s->m2_min / 4.0) <= s->rho)) break;
+  s->min_reg_size = (int)(size_t)(-LOG_NT / log10(ctx->lsd_tables->p));
   lsd_buffers(s, s->bufs);
   plf_status st = s->bufs.alloc(ctx, "LSD");
   if (st) return st;
@@ -1192,39 +1219,37 @@ static plf_status lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
     PLF_LAUNCH_CHECK(ctx);
   }
   PLF_CUDA(ctx, cudaMemsetAsync(s->overflow, 0, sizeof(int), ctx->stream));
-  k_lsd_build_lut<<<(LSD_LUT_DIM * LSD_LUT_DIM + 255) / 256, 256, 0, ctx->stream>>>(s->rho, s->angle_lut, s->cs_lut, s->seed_lut);
-  PLF_LAUNCH_CHECK(ctx);
-  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (s->scale != 1.0) {
-    PLF_CUDA(ctx, cudaMemcpyToSymbolAsync(c_lsd_taps, s->taps, sizeof(int) * 16, 0, cudaMemcpyHostToDevice, ctx->stream));
     std::vector<int> tab(s->rs_xp_off + plf_resize_packed_len(s->ws));
     plf_linear_coeffs_host(w, s->ws, 1.0 / s->scale, &tab[0], &tab[s->ws]);
     plf_linear_coeffs_host(h, s->hs, 1.0 / s->scale, &tab[s->rs_y_off], &tab[s->rs_y_off + s->hs]);
     plf_resize_pack_x(&tab[0], &tab[s->ws], s->ws, &tab[s->rs_xp_off]);
     PLF_CUDA(ctx, cudaMemcpyAsync(s->rs_tab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-    PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   }
+  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return PLF_OK;
 }
 
-// A failed (re)build leaves no state behind (see plf_orb_prepare).
-plf_status plf_lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
-  const plf_status st = lsd_prepare(ctx, w, h, nimg, two_parities);
-  if (st && ctx->lsd) {
-    ctx->lsd->bufs.release();
-    *ctx->lsd = LsdState();
+plf_status plf_lsd_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, LsdState** out) {
+  plf_status st = plf_lsd_tables(ctx);
+  if (st) return st;
+  LsdState* s = new LsdState();
+  if ((st = lsd_build(ctx, s, w, h, nimg, two_parities))) {
+    plf_lsd_free(s);
+    return st;
   }
-  return st;
+  *out = s;
+  return PLF_OK;
 }
 
 // LSD on images [0, n) of a batch resident on the device, in two phases so that callers can overlap them with other
 // work: `pre` = blur, resample, gradient and seed ordering (bandwidth-bound), `grow` = region growing, rectangle fit and
-// the KeyLine stage (latency-bound).  `par` selects the buffer set that carries data from pre to grow.  State must be
-// prepared for >= n images.  Enqueued on ctx->cur; results stay on the device.
-plf_status plf_lsd_pre(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int par, int n) {
-  LsdState* s = ctx->lsd;
-  if (!s || s->w != w || s->h != h || s->nimg < n || (par && !s->two_parities))
-    return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_pre: state not prepared for these images");
+// the KeyLine stage (latency-bound).  `par` selects the buffer set that carries data from pre to grow.  The state must
+// hold >= n images.  Enqueued on ctx->cur; results stay on the device.
+plf_status plf_lsd_pre(plf_ctx* ctx, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int par, int n) {
+  if (s->nimg < n) return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_pre: %d images > the state's %d", n, s->nimg);
+  const LsdTables& T = *ctx->lsd_tables;
+  const int w = s->w, h = s->h;
   cudaStream_t cs = ctx->cur;
   const int W = s->ws, H = s->hs;
   const size_t As = (size_t)W * H, A = (size_t)s->bp * h, Asp = (size_t)s->sp * H;
@@ -1235,18 +1260,18 @@ plf_status plf_lsd_pre(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, i
   size_t scaled_stride = img_stride;
   int scaled_pitch = pitch;
   if (s->scale != 1.0) {
-    if ((s->ksize == 7 || s->ksize == 5) && s->taps_u8) {
-      const CUtensorMap* tm = s->tm_blur.get(d_imgs, w, h, n, pitch, img_stride, 80, BF_TH + s->ksize - 1);
+    if ((T.ksize == 7 || T.ksize == 5) && T.taps_u8) {
+      const CUtensorMap* tm = s->tm_blur.get(d_imgs, w, h, n, pitch, img_stride, 80, BF_TH + T.ksize - 1);
       if (!tm)
         return plf_fail(ctx, PLF_ERR_CUDA, "LSD: cuTensorMapEncodeTiled failed for the source images (pitch %d, stride %zu)", pitch, img_stride);
       uint32_t tA = 0, tB = 0;
-      for (int k = 0; k < s->ksize; ++k) (k < 4 ? tA : tB) |= (uint32_t)s->taps[k] << (8 * (k & 3));
-      dim3 gf(plf_tma_tiles_x(w, s->ksize / 2), (h + BF_TH - 1) / BF_TH, n);
-      if (s->ksize == 7) k_blur_q8_fast<7><<<gf, 256, 0, cs>>>(*tm, 0, w, h, tA, tB, s->blur, A, s->bp);
+      for (int k = 0; k < T.ksize; ++k) (k < 4 ? tA : tB) |= (uint32_t)T.taps[k] << (8 * (k & 3));
+      dim3 gf(plf_tma_tiles_x(w, T.ksize / 2), (h + BF_TH - 1) / BF_TH, n);
+      if (T.ksize == 7) k_blur_q8_fast<7><<<gf, 256, 0, cs>>>(*tm, 0, w, h, tA, tB, s->blur, A, s->bp);
       else k_blur_q8_fast<5><<<gf, 256, 0, cs>>>(*tm, 0, w, h, tA, tB, s->blur, A, s->bp);
     } else {
       dim3 gb((w + BQ_TW - 1) / BQ_TW, (h + BQ_TH - 1) / BQ_TH, n);
-      k_blur_q8<<<gb, 256, 0, cs>>>(d_imgs, img_stride, pitch, w, h, s->ksize / 2, s->blur, A, s->bp);
+      k_blur_q8<<<gb, 256, 0, cs>>>(d_imgs, img_stride, pitch, w, h, T.ksize / 2, s->blur, A, s->bp);
     }
     PLF_LAUNCH_CHECK(ctx);
     plf_mark(ctx, "lsd.k_blur_q8");
@@ -1258,7 +1283,7 @@ plf_status plf_lsd_pre(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, i
     scaled_pitch = s->sp;
   }
   PLF_CUDA(ctx, cudaMemsetAsync(s->maxmag2, 0xFF, (size_t)n * sizeof(int), cs));  // -1
-  k_lsd_grad<<<dim3(s->nxb, (H + 1) / 2, n), LSD_GRAD_THREADS, 0, cs>>>(scaled, scaled_stride, scaled_pitch, W, H, s->angle_lut, s->m2_min, As, pix, s->pix_stride,
+  k_lsd_grad<<<dim3(s->nxb, (H + 1) / 2, n), LSD_GRAD_THREADS, 0, cs>>>(scaled, scaled_stride, scaled_pitch, W, H, T.angle_lut, T.m2_min, As, pix, s->pix_stride,
                                                                s->seedlist, s->segcnt, s->nxb, s->maxmag2);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_grad");
@@ -1275,10 +1300,10 @@ plf_status plf_lsd_pre(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, i
   return PLF_OK;
 }
 
-plf_status plf_lsd_grow(plf_ctx* ctx, int w, int h, int par, int n) {
-  LsdState* s = ctx->lsd;
-  if (!s || s->w != w || s->h != h || s->nimg < n || (par && !s->two_parities))
-    return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_grow: state not prepared for these images");
+plf_status plf_lsd_grow(plf_ctx* ctx, LsdState* s, int par, int n, cudaEvent_t keylines_wait) {
+  if (s->nimg < n) return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_grow: %d images > the state's %d", n, s->nimg);
+  const LsdTables& T = *ctx->lsd_tables;
+  const int w = s->w, h = s->h;
   cudaStream_t cs = ctx->cur;
   const int W = s->ws, H = s->hs;
   const size_t As = (size_t)W * H;
@@ -1287,18 +1312,18 @@ plf_status plf_lsd_grow(plf_ctx* ctx, int w, int h, int par, int n) {
   // before those of the next
   // (thread / lane per image, register-capped and unrolled variants and an angle-map layout were all bit-exact and were
   // not kept; DESIGN.md section 5 lists them)
-  k_lsd_grow<<<n, 32, 0, cs>>>(pix, s->pix_stride, As, W, s->order[par], s->seed_lut, s->cs_lut, s->nseeds[par], s->prec, (float)(s->p * 180.0),
+  k_lsd_grow<<<n, 32, 0, cs>>>(pix, s->pix_stride, As, W, s->order[par], T.seed_lut, T.cs_lut, s->nseeds[par], T.prec, (float)(T.p * 180.0),
                                s->min_reg_size, s->regpts, s->regions, s->max_regions, s->nregions, s->overflow);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_grow");
   k_lsd_rect_order<<<n, 256, 0, cs>>>(s->regions, s->max_regions, s->nregions, s->rect_perm);
   PLF_LAUNCH_CHECK(ctx);
   k_lsd_rects<<<dim3((s->max_regions + 127) / 128, n), 128, 0, cs>>>(pix, s->pix_stride, As, W, s->regpts, s->regions, s->max_regions, s->nregions,
-                                                                     s->rect_perm, s->prec, s->scale, s->segs);
+                                                                     s->rect_perm, T.prec, s->scale, s->segs);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, "lsd.k_lsd_rects");
   const double min_length = (double)ctx->params.min_line_length * (double)std::min(w, h);
-  if (ctx->lsd_keylines_wait) PLF_CUDA(ctx, cudaStreamWaitEvent(cs, ctx->lsd_keylines_wait, 0));
+  if (keylines_wait) PLF_CUDA(ctx, cudaStreamWaitEvent(cs, keylines_wait, 0));
   k_keylines<<<n, 1024, 0, cs>>>(s->segs, s->nregions, s->max_regions, w, h, min_length, ctx->params.lsd_nfeatures, s->kls_all, s->kls[par],
                                  s->max_lines, s->nlines[par], s->overflow);
   PLF_LAUNCH_CHECK(ctx);
@@ -1306,22 +1331,27 @@ plf_status plf_lsd_grow(plf_ctx* ctx, int w, int h, int par, int n) {
   return PLF_OK;
 }
 
-plf_status plf_lsd_run(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int nimg) {
-  plf_status st = plf_lsd_prepare(ctx, w, h, nimg, false);
-  if (st) return st;
-  if ((st = plf_lsd_pre(ctx, d_imgs, img_stride, pitch, w, h, 0, nimg))) return st;
-  return plf_lsd_grow(ctx, w, h, 0, nimg);
-}
+int* plf_lsd_overflow_flag(const LsdState* s) { return s->overflow; }
 
-int* plf_lsd_overflow_flag(plf_ctx* ctx) { return ctx->lsd->overflow; }
-
-void plf_lsd_outputs(plf_ctx* ctx, int par, plf_keyline** kls, int** nlines, int* max_lines) {
-  LsdState* s = ctx->lsd;
+void plf_lsd_outputs(const LsdState* s, int par, plf_keyline** kls, int** nlines, int* max_lines) {
   *kls = s->kls[par]; *nlines = s->nlines[par]; *max_lines = s->max_lines;
 }
 
-static plf_status lsd_check_overflow(plf_ctx* ctx, const char* what) {
-  LsdState* s = ctx->lsd;
+// LSD of the standalone operators on one w x h image at dimg, in ctx->lsd_standalone (rebuilt when the size changes).
+static plf_status lsd_standalone(plf_ctx* ctx, const uint8_t* dimg, int pitch, int w, int h) {
+  LsdState*& s = ctx->lsd_standalone;
+  plf_status st;
+  if (s && (s->w != w || s->h != h)) {
+    PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    plf_lsd_free(s);
+    s = nullptr;
+  }
+  if (!s && (st = plf_lsd_create(ctx, w, h, 1, false, &s))) return st;
+  if ((st = plf_lsd_pre(ctx, s, dimg, (size_t)pitch * h, pitch, 0, 1))) return st;
+  return plf_lsd_grow(ctx, s, 0, 1, nullptr);
+}
+
+static plf_status lsd_check_overflow(plf_ctx* ctx, const LsdState* s, const char* what) {
   int ovf = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&ovf, s->overflow, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -1338,16 +1368,17 @@ extern "C" plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   if (!ctx || !img || !n_out || w < 3 || h < 3 || stride < w || cap < 0 || (cap > 0 && !segs))
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_lsd: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  ctx->cur = ctx->stream;
   const int pitch = plf_pitch16(w);
   uint8_t* dimg = (uint8_t*)plf_scratch(ctx, PLF_SCR_LSD, (size_t)pitch * h);
   if (!dimg) return PLF_ERR_CUDA;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  plf_status st = plf_lsd_run(ctx, dimg, (size_t)pitch * h, pitch, w, h, 1);
+  plf_status st = lsd_standalone(ctx, dimg, pitch, w, h);
   if (st) return st;
-  LsdState* s = ctx->lsd;
+  const LsdState* s = ctx->lsd_standalone;
   int n = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->nregions, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  st = lsd_check_overflow(ctx, "plf_lsd");
+  st = lsd_check_overflow(ctx, s, "plf_lsd");
   if (st) return st;
   *n_out = n;
   if (n > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_lsd: %d segments > caller capacity %d", n, cap);
@@ -1363,6 +1394,7 @@ extern "C" plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, 
   if (!ctx || !img || !n_out || w < 3 || h < 3 || stride < w || cap < 0 || (cap > 0 && (!keylines || !desc)))
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_detect_lines: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  ctx->cur = ctx->stream;
   const int pitch = plf_pitch16(w);
   uint8_t *dimg, *ddesc;
   short2* dgrad;
@@ -1370,16 +1402,17 @@ extern "C" plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, 
   scr.add(dimg, (size_t)pitch * h); scr.add(dgrad, (size_t)w * h); scr.add(ddesc, (size_t)ctx->limits.max_lines * 32);
   if (plf_status st = scr.carve(ctx, PLF_SCR_LSD)) return st;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  plf_status st = plf_lsd_run(ctx, dimg, (size_t)pitch * h, pitch, w, h, 1);
+  plf_status st = lsd_standalone(ctx, dimg, pitch, w, h);
   if (st) return st;
-  LsdState* s = ctx->lsd;
-  st = plf_launch_blur5_sobel(ctx, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
+  const LsdState* s = ctx->lsd_standalone;
+  PlfTmaCache tm;
+  st = plf_launch_blur5_sobel(ctx, &tm, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
   if (st) return st;
   st = plf_launch_lbd(ctx, dgrad, 0, w, h, 1, s->kls[0], s->nlines[0], s->max_lines, ddesc, nullptr);
   if (st) return st;
   int n = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->nlines[0], sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  st = lsd_check_overflow(ctx, "plf_detect_lines");
+  st = lsd_check_overflow(ctx, s, "plf_detect_lines");
   if (st) return st;
   *n_out = n;
   if (n > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_detect_lines: %d lines > caller capacity %d", n, cap);

@@ -57,7 +57,6 @@ struct OrbGeom {
 
 struct OrbState {
   int w = 0, h = 0, nimg = 0;
-  bool two_parities = false;
   OrbGeom g;
   uint8_t* pyr = nullptr;    // levels 1..n-1, all images
   uint8_t* blur = nullptr;   // blurred levels 0..n-1
@@ -74,7 +73,6 @@ struct OrbState {
   int* kp_count[2] = {nullptr, nullptr};      // [nimg]
   int* overflow = nullptr;      // [1]
   float2* trig = nullptr;       // [nimg][max_kp] (cos, sin) of the keypoint angle (k_orb_trig -> k_rbrief)
-  float blur_k[7];
   // TMA descriptors (plf_tma.cuh): halo boxes of the FAST tile (96 x 38) and of the blur tile (80 x 38) per level; level 0
   // is the caller's image buffer
   CUtensorMap tm_fast[ORB_MAX_LEVELS], tm_blur[ORB_MAX_LEVELS];
@@ -675,29 +673,16 @@ void plf_linear_coeffs_host(int srcsize, int dstsize, double scale, int* ofs, in
   }
 }
 
-extern "C" void plf_orb_free(plf_ctx* ctx) {
-  if (ctx->orb) {
-    ctx->orb->bufs.release();
-    delete ctx->orb;
-    ctx->orb = nullptr;
-  }
+void plf_orb_free(OrbState* s) {
+  if (!s) return;
+  s->bufs.release();
+  delete s;
 }
 
-static int8_t* g_dev_pattern = nullptr;  // shared by all contexts on a device (read-only)
+static int8_t* g_dev_pattern = nullptr;  // shared by all contexts on a device (read-only), uploaded with c_blur7
 static int g_dev_pattern_device = -1;
 
-// (Re)builds the ORB state for images of w x h and up to nimg images per launch.
-static plf_status orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
-  OrbState* s = ctx->orb;
-  if (s && s->w == w && s->h == h && s->nimg >= nimg && (s->two_parities || !two_parities)) return PLF_OK;
-  if (s && s->two_parities) two_parities = true;
-  if (s) {
-    PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    s->bufs.release();
-    *s = OrbState();
-  } else {
-    s = ctx->orb = new OrbState();
-  }
+static plf_status orb_build(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, bool two_parities) {
   const plf_params& P = ctx->params;
   if (P.orb_nlevels < 1 || P.orb_nlevels > ORB_MAX_LEVELS || P.orb_wta_k != 2 || P.orb_score != 1 ||
       P.orb_patch_size != 31)
@@ -712,7 +697,6 @@ static plf_status orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
                     P.orb_edge_th, ORB_MIN_EDGE);
   if (w >= 4096 || h >= 4096) return plf_fail(ctx, PLF_ERR_INVALID, "ORB: image larger than 4095 px");
   s->w = w; s->h = h; s->nimg = nimg;
-  s->two_parities = two_parities;
   OrbGeom& g = s->g;
   memset(&g, 0, sizeof g);
   g.nlevels = P.orb_nlevels;
@@ -801,7 +785,14 @@ static plf_status orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
   PLF_CUDA(ctx, cudaMemsetAsync(s->overflow, 0, sizeof(int), ctx->stream));
   if (!tab.empty())
     PLF_CUDA(ctx, cudaMemcpyAsync(s->rs_tab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-  {  // getGaussianKernel(7, 2, CV_32F): host doubles -> float (pinned equal to cv2 in tests)
+  // The rBRIEF pattern and the blur kernel depend on nothing: uploaded once, not by every state (a state built while
+  // another one's kernels run must not write what they read)
+  if (!g_dev_pattern || g_dev_pattern_device != ctx->device) {
+    int8_t hp[1024];
+    for (int i = 0; i < 1024; ++i) hp[i] = (int8_t)h_orb_bit_pattern_31[i];
+    PLF_CUDA(ctx, cudaMalloc(&g_dev_pattern, 1024));
+    PLF_CUDA(ctx, cudaMemcpyAsync(g_dev_pattern, hp, 1024, cudaMemcpyHostToDevice, ctx->stream));
+    // getGaussianKernel(7, 2, CV_32F): host doubles -> float (pinned equal to cv2 in tests)
     double d[7], sum = 0;
     for (int i = 0; i < 7; ++i) {
       const double x = i - 3.0;
@@ -809,14 +800,9 @@ static plf_status orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
       sum += d[i];
     }
     sum = 1. / sum;
-    for (int i = 0; i < 7; ++i) s->blur_k[i] = (float)(d[i] * sum);
-    PLF_CUDA(ctx, cudaMemcpyToSymbolAsync(c_blur7, s->blur_k, sizeof s->blur_k, 0, cudaMemcpyHostToDevice, ctx->stream));
-  }
-  if (!g_dev_pattern || g_dev_pattern_device != ctx->device) {
-    int8_t hp[1024];
-    for (int i = 0; i < 1024; ++i) hp[i] = (int8_t)h_orb_bit_pattern_31[i];
-    PLF_CUDA(ctx, cudaMalloc(&g_dev_pattern, 1024));
-    PLF_CUDA(ctx, cudaMemcpyAsync(g_dev_pattern, hp, 1024, cudaMemcpyHostToDevice, ctx->stream));
+    float blur_k[7];
+    for (int i = 0; i < 7; ++i) blur_k[i] = (float)(d[i] * sum);
+    PLF_CUDA(ctx, cudaMemcpyToSymbolAsync(c_blur7, blur_k, sizeof blur_k, 0, cudaMemcpyHostToDevice, ctx->stream));
     g_dev_pattern_device = ctx->device;
   }
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -829,23 +815,22 @@ static plf_status orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_par
   return PLF_OK;
 }
 
-// A failed (re)build leaves no state behind: the next call starts from scratch and fails the same way, instead of finding
-// a size that matches the request and buffers that were released.
-plf_status plf_orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
-  const plf_status st = orb_prepare(ctx, w, h, nimg, two_parities);
-  if (st && ctx->orb) {
-    ctx->orb->bufs.release();
-    *ctx->orb = OrbState();
+plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, OrbState** out) {
+  OrbState* s = new OrbState();
+  const plf_status st = orb_build(ctx, s, w, h, nimg, two_parities);
+  if (st) {
+    plf_orb_free(s);
+    return st;
   }
-  return st;
+  *out = s;
+  return PLF_OK;
 }
 
-// Runs ORB on nimg images resident at d_imgs ([nimg][h][pitch], pitch a multiple of 16, stride img_stride bytes).
-// Results stay on the device.
-plf_status plf_orb_run(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int nimg, int par) {
-  plf_status st = plf_orb_prepare(ctx, w, h, nimg, par != 0);
-  if (st) return st;
-  OrbState* s = ctx->orb;
+// Runs ORB on nimg (<= s->nimg) images of s->w x s->h resident at d_imgs ([nimg][h][pitch], pitch a multiple of 16,
+// stride img_stride bytes).  Enqueued on ctx->cur; results stay on the device.
+plf_status plf_orb_run(plf_ctx* ctx, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par) {
+  const int w = s->w, h = s->h;
+  plf_status st;
   OrbGeom g = s->g;
   g.pitch[0] = pitch;
   cudaStream_t cs = ctx->cur;
@@ -891,11 +876,10 @@ plf_status plf_orb_run(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, i
   return PLF_OK;
 }
 
-int* plf_orb_overflow_flag(plf_ctx* ctx) { return ctx->orb->overflow; }
+int* plf_orb_overflow_flag(const OrbState* s) { return s->overflow; }
 
 // device-side accessors for the pipeline
-void plf_orb_outputs(plf_ctx* ctx, int par, plf_keypoint** kps, uint8_t** desc, int** counts, int* max_kp) {
-  OrbState* s = ctx->orb;
+void plf_orb_outputs(const OrbState* s, int par, plf_keypoint** kps, uint8_t** desc, int** counts, int* max_kp) {
   *kps = s->kps[par]; *desc = s->desc[par]; *counts = s->kp_count[par]; *max_kp = s->g.max_kp;
 }
 
@@ -904,13 +888,20 @@ extern "C" plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   if (!ctx || !img || !n_out || w < 8 || h < 8 || stride < w || cap < 0 || (cap > 0 && (!kps || !desc)))
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_orb: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  ctx->cur = ctx->stream;
+  OrbState*& s = ctx->orb_standalone;
+  plf_status st;
+  if (s && (s->w != w || s->h != h)) {
+    PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    plf_orb_free(s);
+    s = nullptr;
+  }
+  if (!s && (st = plf_orb_create(ctx, w, h, 1, false, &s))) return st;
   const int pitch = plf_pitch16(w);
   uint8_t* dimg = (uint8_t*)plf_scratch(ctx, PLF_SCR_ORB, (size_t)pitch * h);
   if (!dimg) return PLF_ERR_CUDA;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  plf_status st = plf_orb_run(ctx, dimg, (size_t)pitch * h, pitch, w, h, 1, 0);
-  if (st) return st;
-  OrbState* s = ctx->orb;
+  if ((st = plf_orb_run(ctx, s, dimg, (size_t)pitch * h, pitch, 1, 0))) return st;
   int n = 0, ovf = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->kp_count[0], sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyAsync(&ovf, s->overflow, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));

@@ -41,6 +41,9 @@ struct PipeState {
   int up_slot = 0;             // slot written by the last plf_batch_upload
   cudaStream_t copy = nullptr; // H2D stream
   cudaEvent_t ev_up[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr}, ev_free2[2] = {nullptr, nullptr};
+  OrbState* orb = nullptr;     // ORB of 2B images, outputs per batch parity
+  LsdState* lsd = nullptr;     // LSD of 2B images, hand-off buffers per batch parity if lsd2
+  PlfTmaCache lbd_tm;          // tensor maps of the LBD gradient prelude over imgs2
   short2* lbd_grad[2] = {nullptr, nullptr};  // [parity][2B][h*w]
   uint8_t* ldesc_raw = nullptr;  // [2B][max_ln][32]  LBD of every kept KeyLine
   FrameSlots fs;               // B+1 slots
@@ -139,6 +142,8 @@ static std::vector<PipeEvents> pipe_events(PipeState* s) {
 extern "C" void plf_pipe_free(plf_ctx* ctx) {
   PipeState* s = ctx->pipe;
   if (!s) return;
+  plf_orb_free(s->orb);
+  plf_lsd_free(s->lsd);
   s->bufs.release();
   for (int i = 0; i < 3; ++i) {
     if (s->h_results[i]) cudaFreeHost(s->h_results[i]);
@@ -517,10 +522,11 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
   cudaStream_t cs = ctx->stream;
   PLF_CUDA(ctx, cudaMemsetAsync(f.pt_count, 0, (B + 1) * sizeof(int), cs));
   PLF_CUDA(ctx, cudaMemsetAsync(f.ls_count, 0, (B + 1) * sizeof(int), cs));
-  // sub-systems sized for 2B images
-  if ((st = plf_orb_prepare(ctx, w, h, 2 * B, true))) return st;
+  // sub-systems sized for 2B images; the LSD tables come first, so that the parity decision sees the memory they take
+  if ((st = plf_orb_create(ctx, w, h, 2 * B, true, &s->orb))) return st;
+  if ((st = plf_lsd_tables(ctx))) return st;
   s->lsd2 = lsd_want_two_parities(ctx, w, h, 2 * B);
-  if ((st = plf_lsd_prepare(ctx, w, h, 2 * B, s->lsd2))) return st;
+  if ((st = plf_lsd_create(ctx, w, h, 2 * B, s->lsd2, &s->lsd))) return st;
   // static problem descriptors over the pipeline's own buffers (pointers never change; counts are read on the device):
   // the stereo problems read the match phase's copies of the extraction outputs
   const int* kcnt = s->kcntM;
@@ -567,17 +573,11 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
   return PLF_OK;
 }
 
-static plf_status pipe_prepare(plf_ctx* ctx, int w, int h) {
-  PipeState* s = ctx->pipe;
-  if (s && s->w == w && s->h == h) {
-    // a standalone operator call on another image size may have rebuilt the ORB / LSD state meanwhile: rebuild it again.
-    // No pipeline buffer or problem descriptor points into that state, so the sequence goes on where it was.
-    const plf_status st = plf_orb_prepare(ctx, w, h, 2 * s->B, true);
-    return st ? st : plf_lsd_prepare(ctx, w, h, 2 * s->B, s->lsd2);
-  }
-  plf_pipe_free(ctx);
-  const plf_status st = pipe_build(ctx, w, h);
-  if (st) plf_pipe_free(ctx);   // a failed setup leaves no state behind (see plf_orb_prepare)
+// Builds the pipeline for the camera's image size on first use; a failed setup leaves no state behind.
+static plf_status pipe_prepare(plf_ctx* ctx) {
+  if (ctx->pipe) return PLF_OK;
+  const plf_status st = pipe_build(ctx, ctx->cam.width, ctx->cam.height);
+  if (st) plf_pipe_free(ctx);
   return st;
 }
 
@@ -616,14 +616,14 @@ static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->evX[par], 0));           // batch i-2 (same parity) no longer reads these buffers
   plf_mark(ctx, "start");
   PLF_CUDA(ctx, cudaEventRecord(s->tE0[par], sE));
-  plf_status st = plf_orb_run(ctx, imgs, AP, s->pitch, w, h, 2 * B, par);
-  if (!st) st = plf_launch_blur5_sobel(ctx, imgs, s->pitch, AP, w, h, 2 * B, s->lbd_grad[par], A);
+  plf_status st = plf_orb_run(ctx, s->orb, imgs, AP, s->pitch, 2 * B, par);
+  if (!st) st = plf_launch_blur5_sobel(ctx, &s->lbd_tm, imgs, s->pitch, AP, w, h, 2 * B, s->lbd_grad[par], A);
   if (st) return st;
   plf_mark(ctx, "lbd.k_blur5_sobel");
   // this batch's ORB overflow flag: snapshot + clear on the E stream, so that a flag raised by batch i+1's extraction is
   // not reported on batch i's download
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp, plf_orb_overflow_flag(ctx), sizeof(int), cudaMemcpyDeviceToDevice, sE));
-  PLF_CUDA(ctx, cudaMemsetAsync(plf_orb_overflow_flag(ctx), 0, sizeof(int), sE));
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp, plf_orb_overflow_flag(s->orb), sizeof(int), cudaMemcpyDeviceToDevice, sE));
+  PLF_CUDA(ctx, cudaMemsetAsync(plf_orb_overflow_flag(s->orb), 0, sizeof(int), sE));
   PLF_CUDA(ctx, cudaEventRecord(s->evE[par], sE));
   PLF_CUDA(ctx, cudaEventRecord(s->ev_free[r.run_slot], sE));  // the image buffer may be overwritten by the next upload
   return PLF_OK;
@@ -635,14 +635,14 @@ static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
 // with one copy P and G share a stream and LSD(i+1) starts when LSD(i) ends.  The buffers only G writes and reads
 // (region points, regions, segments) exist once either way: G(i+1) follows G(i) on its stream. ----
 static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
-  const int w = s->w, h = s->h, par = r.par;
-  const size_t AP = (size_t)s->pitch * h;
+  const int par = r.par;
+  const size_t AP = (size_t)s->pitch * s->h;
   cudaStream_t sP = r.sP, sG = r.sG;
   ctx->cur = sP;
   PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_up[r.run_slot], 0));
   if (r.lsd2) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->evG[par], 0));   // batch i-2 (same parity) has finished growing / fitting on these maps
   PLF_CUDA(ctx, cudaEventRecord(s->tG0[par], sP));
-  plf_status st = plf_lsd_pre(ctx, s->imgs2[r.run_slot], AP, s->pitch, w, h, r.lp, 2 * r.B);
+  plf_status st = plf_lsd_pre(ctx, s->lsd, s->imgs2[r.run_slot], AP, s->pitch, r.lp, 2 * r.B);
   if (st) return st;
   PLF_CUDA(ctx, cudaEventRecord(s->ev_free2[r.run_slot], sP));
   PLF_CUDA(ctx, cudaEventRecord(s->evP[par], sP));
@@ -650,12 +650,10 @@ static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaStreamWaitEvent(sG, s->evP[par], 0));
   // the KeyLine outputs are overwritten: the match phase that read them last (batch i-2 with two parities, batch i-1 with one)
   // has taken its copy
-  ctx->lsd_keylines_wait = r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr;
-  st = plf_lsd_grow(ctx, w, h, r.lp, 2 * r.B);
-  ctx->lsd_keylines_wait = nullptr;
+  st = plf_lsd_grow(ctx, s->lsd, r.lp, 2 * r.B, r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr);
   if (st) return st;
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp + 1, plf_lsd_overflow_flag(ctx), sizeof(int), cudaMemcpyDeviceToDevice, sG));
-  PLF_CUDA(ctx, cudaMemsetAsync(plf_lsd_overflow_flag(ctx), 0, sizeof(int), sG));
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp + 1, plf_lsd_overflow_flag(s->lsd), sizeof(int), cudaMemcpyDeviceToDevice, sG));
+  PLF_CUDA(ctx, cudaMemsetAsync(plf_lsd_overflow_flag(s->lsd), 0, sizeof(int), sG));
   PLF_CUDA(ctx, cudaEventRecord(s->evG[par], sG));
   return PLF_OK;
 }
@@ -685,8 +683,8 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   const plf_params& P = ctx->params;
   plf_keypoint* kps; uint8_t* odesc; int* kcnt; int mk;
   plf_keyline* kls; int* lcnt; int ml;
-  plf_orb_outputs(ctx, par, &kps, &odesc, &kcnt, &mk);
-  plf_lsd_outputs(ctx, r.lp, &kls, &lcnt, &ml);
+  plf_orb_outputs(s->orb, par, &kps, &odesc, &kcnt, &mk);
+  plf_lsd_outputs(s->lsd, r.lp, &kls, &lcnt, &ml);
   cudaStream_t cs = r.sM;
   ctx->cur = cs;
   plf_status st;
@@ -805,7 +803,7 @@ plf_status plf_batch_upload(plf_ctx* ctx, int B, const uint8_t* left, const uint
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload: bad arguments (B=%d, max_batch=%d)", B, ctx ? ctx->limits.max_batch : 0);
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const int w = ctx->cam.width, h = ctx->cam.height;
-  plf_status st = pipe_prepare(ctx, w, h);
+  plf_status st = pipe_prepare(ctx);
   if (st) return st;
   PipeState* s = ctx->pipe;
   const size_t A = (size_t)s->pitch * h;
@@ -845,14 +843,14 @@ plf_status plf_batch_upload(plf_ctx* ctx, int B, const uint8_t* left, const uint
 
 void* plf_batch_device_images(plf_ctx* ctx) {
   if (!ctx) return nullptr;
-  if (pipe_prepare(ctx, ctx->cam.width, ctx->cam.height)) return nullptr;
+  if (pipe_prepare(ctx)) return nullptr;
   return ctx->pipe->imgs2[ctx->pipe->up_slot];
 }
 
 plf_status plf_batch_run(plf_ctx* ctx, int B) {
   if (!ctx || B < 1 || B > ctx->limits.max_batch) return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_run: bad B");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  plf_status st = pipe_prepare(ctx, ctx->cam.width, ctx->cam.height);
+  plf_status st = pipe_prepare(ctx);
   if (st) return st;
   PipeState* s = ctx->pipe;
   if (s->n_pending >= 3)

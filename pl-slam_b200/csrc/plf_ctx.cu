@@ -282,9 +282,6 @@ plf_status plf_create(const plf_params* params, const plf_camera* cam, const plf
 }
 
 // subsystem destructors (defined in their own translation units)
-void plf_orb_free(plf_ctx* ctx);
-void plf_lsd_free(plf_ctx* ctx);
-void plf_lbd_free(plf_ctx* ctx);
 void plf_pipe_free(plf_ctx* ctx);
 void plf_bow_free(plf_ctx* ctx);
 
@@ -294,9 +291,9 @@ void plf_destroy(plf_ctx* ctx) {
   cudaStreamSynchronize(ctx->stream);
   plf_pipe_free(ctx);
   plf_bow_free(ctx);
-  plf_orb_free(ctx);
-  plf_lsd_free(ctx);
-  plf_lbd_free(ctx);
+  plf_orb_free(ctx->orb_standalone);
+  plf_lsd_free(ctx->lsd_standalone);
+  plf_lsd_tables_free(ctx);
   for (auto& b : ctx->scratch)
     if (b.p) cudaFree(b.p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);

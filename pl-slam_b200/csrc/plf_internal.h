@@ -65,12 +65,15 @@ struct StagedLayout {
   plf_status acquire(plf_ctx* ctx, plf_scratch_slot slot, uint8_t** pin, uint8_t** dev) const;
 };
 
+struct OrbState;      // orb.cu
+struct LsdState;      // lsd.cu
+struct PlfTmaCache;   // plf_tma.cuh
+
 struct plf_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;  // main stream: copies, the serial part of the pipeline, standalone operators
   cudaStream_t cur = nullptr;     // stream the launch helpers enqueue on (== stream except inside forked sections)
   cudaStream_t aux[3] = {nullptr, nullptr, nullptr};  // streams of the extraction (E), LSD growing (G) and LSD pre-grow (P) phases of plf_batch_run
-  cudaEvent_t lsd_keylines_wait = nullptr;  // if set: plf_lsd_grow waits for it before it overwrites the KeyLine outputs
   plf_params params;
   plf_camera cam;
   plf_limits limits;
@@ -82,10 +85,11 @@ struct plf_ctx {
   void* pinned = nullptr;
   size_t pinned_bytes = 0;
   // subsystem state (owned by the respective .cu)
-  struct OrbState* orb = nullptr;
-  struct LsdState* lsd = nullptr;
-  struct LbdState* lbd = nullptr;
-  struct PipeState* pipe = nullptr;
+  struct OrbState* orb_standalone = nullptr;   // plf_orb's working state: one image, rebuilt when the image size changes
+  struct LsdState* lsd_standalone = nullptr;   // plf_lsd's and plf_detect_lines': likewise
+  struct LsdTables* lsd_tables = nullptr;      // the LSD lookup tables of the parameters, read by every LSD state
+  bool lbd_tables = false;                     // the LBD constant tables are uploaded
+  struct PipeState* pipe = nullptr;            // the batched pipeline, with its own ORB and LSD states
   struct BowState* bow = nullptr;   // DBoW2 vocabularies and keyframe database (dbow.cu)
   // optional per-stage timing (plf_profile_enable): events recorded after each kernel of plf_batch_run
   bool profile = false;
@@ -181,7 +185,8 @@ struct MgbArgs {
 plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n1, int max_n2, plf_scratch_slot slot);
 
 // ---- LBD (lbd.cu) ------------------------------------------------------------------------------
-plf_status plf_launch_blur5_sobel(plf_ctx* ctx, const uint8_t* imgs, int pitch, size_t img_stride,
+// tm: the caller's tensor-map cache over its source images (plf_tma.cuh)
+plf_status plf_launch_blur5_sobel(plf_ctx* ctx, PlfTmaCache* tm, const uint8_t* imgs, int pitch, size_t img_stride,
                                   int w, int h, int nimg, short2* grad, size_t grad_stride);
 plf_status plf_launch_lbd(plf_ctx* ctx, const short2* grad, size_t grad_stride, int w, int h, int nimg,
                           const plf_keyline* kls, const int* counts, int max_lines, uint8_t* desc,
@@ -207,9 +212,13 @@ plf_gn_opts plf_gn_opts_from_params(const plf_params& p);
 plf_status plf_launch_gn(plf_ctx* ctx, const GnProblem* d_probs, int nprob, const plf_gn_opts& o);
 
 // ---- ORB (orb.cu) --------------------------------------------------------------------------------
-plf_status plf_orb_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities);
-plf_status plf_orb_run(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int nimg, int par);
-void plf_orb_outputs(plf_ctx* ctx, int par, plf_keypoint** kps, uint8_t** desc, int** counts, int* max_kp);
+// A working state for up to nimg images of w x h, with outputs once or per batch parity (two_parities).  On failure
+// nothing is left allocated and *out is untouched.
+plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, OrbState** out);
+void plf_orb_free(OrbState* s);
+plf_status plf_orb_run(plf_ctx* ctx, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par);
+void plf_orb_outputs(const OrbState* s, int par, plf_keypoint** kps, uint8_t** desc, int** counts, int* max_kp);
+int* plf_orb_overflow_flag(const OrbState* s);
 void plf_linear_coeffs_host(int srcsize, int dstsize, double scale, int* ofs, int* c1);
 plf_status plf_launch_resize_exact(plf_ctx* ctx, const uint8_t* src, size_t src_stride, int sp, int sw, int sh, uint8_t* dst,
                                    size_t dst_stride, int dp, int dw, int dh, const int* tabx, const int* tabxp, const int* taby, int nimg);
@@ -217,14 +226,19 @@ size_t plf_resize_packed_len(int dw);                                 // ints of
 void plf_resize_pack_x(const int* ofs, const int* c1, int dw, int* out);   // out: 16-byte aligned
 
 // ---- LSD (lsd.cu) --------------------------------------------------------------------------------
-plf_status plf_lsd_prepare(plf_ctx* ctx, int w, int h, int nimg, bool two_parities);
-size_t plf_lsd_footprint(const plf_ctx* ctx, int w, int h, int nimg, bool two_parities);   // bytes plf_lsd_prepare allocates
-plf_status plf_lsd_run(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int nimg);
-plf_status plf_lsd_pre(plf_ctx* ctx, const uint8_t* d_imgs, size_t img_stride, int pitch, int w, int h, int par, int n);
-plf_status plf_lsd_grow(plf_ctx* ctx, int w, int h, int par, int n);
-void plf_lsd_outputs(plf_ctx* ctx, int par, plf_keyline** kls, int** nlines, int* max_lines);
-int* plf_orb_overflow_flag(plf_ctx* ctx);
-int* plf_lsd_overflow_flag(plf_ctx* ctx);
+// Builds ctx->lsd_tables, once per context (plf_lsd_create calls it too).
+plf_status plf_lsd_tables(plf_ctx* ctx);
+void plf_lsd_tables_free(plf_ctx* ctx);
+// A working state for up to nimg images of w x h, with the hand-off buffers once or per batch parity (two_parities).
+// On failure nothing is left allocated and *out is untouched.
+plf_status plf_lsd_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, LsdState** out);
+void plf_lsd_free(LsdState* s);
+size_t plf_lsd_footprint(const plf_ctx* ctx, int w, int h, int nimg, bool two_parities);   // bytes plf_lsd_create allocates
+plf_status plf_lsd_pre(plf_ctx* ctx, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int par, int n);
+// keylines_wait: if set, the KeyLine outputs are overwritten only after this event
+plf_status plf_lsd_grow(plf_ctx* ctx, LsdState* s, int par, int n, cudaEvent_t keylines_wait);
+void plf_lsd_outputs(const LsdState* s, int par, plf_keyline** kls, int** nlines, int* max_lines);
+int* plf_lsd_overflow_flag(const LsdState* s);
 
 void plf_configure_lsd();
 

@@ -207,47 +207,109 @@ def test_batches_in_flight_match_sequential(built):
             assert np.array_equal(a["DT"], b["DT"])          # same kernels, same inputs: bit-identical poses
 
 
+STANDALONE_CAM = dict(plf.KITTI_CAMERA, width=640, height=360, cx=320.0, cy=180.0, fx=500.0, fy=500.0)
+STANDALONE_WORLD = synth.World(seed=4, length=50.0, n_quads=160, n_segs=80, half_width=8.0, half_height=3.5)
+
+
+def drive_batches(fe, Ls, Rs, in_flight, between=lambda fe: None):
+    """Four batches of two pairs.  in_flight = 0: each batch is downloaded before the next, `between` runs after the second
+    with no batch in flight.  in_flight = 3: `between` runs with the first three batches in flight.  Returns the downloaded
+    results per batch, the frames (get_frame) of every batch that was alone in flight, and what `between` returned."""
+    res, frames, out = [], {}, None
+    for i, s0 in enumerate(range(0, 8, 2)):
+        fe.batch_upload(Ls[s0:s0 + 2], Rs[s0:s0 + 2]); fe.batch_run(2)
+        if in_flight == 3 and i < 2:
+            continue
+        if in_flight == 3 and i == 2:
+            out = between(fe)
+            res += [fe.batch_download_array(2) for _ in range(3)]
+            continue
+        res.append(fe.batch_download_array(2))
+        frames[i] = [fe.get_frame(k) for k in range(2)]
+        if in_flight == 0 and i == 1:
+            out = between(fe)
+    return res, frames, out
+
+
+def assert_same_batches(base, got):
+    res_a, fr_a, _ = base
+    res_b, fr_b, _ = got
+    assert len(res_a) == len(res_b) == 4 and fr_a.keys() == fr_b.keys()
+    for a, b in zip(res_a, res_b):
+        for f in a.dtype.names:   # field for field, bit for bit (DT included)
+            assert a[f].tobytes() == b[f].tobytes(), f
+    for i in fr_a:
+        for a, b in zip(fr_a[i], fr_b[i]):
+            for k in a:
+                assert np.array_equal(a[k], b[k]), (i, k)
+
+
 def test_standalone_operators_between_batches(built):
-    """fe.orb / fe.lsd / fe.detect_lines / fe.lbd on an image of another size, called between batches on the same
-    context, rebuild the ORB and LSD state and use their own tensor maps: the batches after them give exactly the results
-    and frames of an uninterrupted run, and the operators return what they return on a fresh context."""
-    cam = dict(plf.KITTI_CAMERA, width=640, height=360, cx=320.0, cy=180.0, fx=500.0, fy=500.0)
-    world = synth.World(seed=4, length=50.0, n_quads=160, n_segs=80, half_width=8.0, half_height=3.5)
+    """fe.orb / fe.lsd / fe.detect_lines / fe.lbd / fe.lbd_gradients, called between batches on the same context, at the
+    pipeline's own image size and at another one, with no batch and with three batches in flight.  The operators work
+    in their own state and never touch the pipeline's: every batch downloads exactly the results (and, where it was
+    alone in flight, the frames) of an uninterrupted run, and the operators return what they return on a fresh context."""
+    cam, world = STANDALONE_CAM, STANDALONE_WORLD
     frames = list(synth.stream(cam, 8, world=world, seed=21, step=0.12))
     Ls, Rs = np.stack([f[0] for f in frames]), np.stack([f[1] for f in frames])
-    other = next(iter(synth.stream(dict(cam, width=480, height=300, cx=240.0, cy=150.0), 1, world=world, seed=5)))[0]
+    images = {"pipeline size": next(iter(synth.stream(cam, 1, world=world, seed=5)))[0],
+              "other size": next(iter(synth.stream(dict(cam, width=480, height=300, cx=240.0, cy=150.0), 1, world=world, seed=5)))[0]}
     lim = plf.default_limits(); lim.max_batch = 2
     prm = dict(orb_nfeatures=700, lsd_nfeatures=150)
 
-    def batch(fe, s0):
-        res = fe.process_batch(Ls[s0:s0 + 2], Rs[s0:s0 + 2])
-        return res, [fe.get_frame(k) for k in range(2)]
+    def operators(img):
+        def call(fe):
+            kps, desc = fe.orb(img)
+            segs = fe.lsd(img)
+            kls, ldesc = fe.detect_lines(img)
+            return (kps, desc, segs, kls, ldesc, fe.lbd(img, kls)) + fe.lbd_gradients(img)
+        return call
 
-    def operators(fe):
-        kps, desc = fe.orb(other)
-        segs = fe.lsd(other)
-        kls, ldesc = fe.detect_lines(other)
-        return kps, desc, segs, kls, ldesc, fe.lbd(other, kls)
+    fresh = {}
+    for name, img in images.items():
+        with plf.Frontend(camera=cam, limits=lim, **prm) as fe:
+            fresh[name] = operators(img)(fe)
+        assert len(fresh[name][0]) > 0 and len(fresh[name][3]) > 0
+    for in_flight in (0, 3):
+        with plf.Frontend(camera=cam, limits=lim, **prm) as fe:
+            base = drive_batches(fe, Ls, Rs, in_flight)
+        assert len(base[1]) == (4 if in_flight == 0 else 1)
+        for name, img in images.items():
+            with plf.Frontend(camera=cam, limits=lim, **prm) as fe:
+                got = drive_batches(fe, Ls, Rs, in_flight, operators(img))
+            assert_same_batches(base, got)
+            for a, b in zip(got[2], fresh[name]):
+                assert a.tobytes() == b.tobytes(), (in_flight, name)
 
-    with plf.Frontend(camera=cam, limits=lim, **prm) as fe:
-        base = [batch(fe, s0) for s0 in (0, 2, 4, 6)]
-    with plf.Frontend(camera=cam, limits=lim, **prm) as fe:
-        got = [batch(fe, 0), batch(fe, 2)]
-        ops = operators(fe)
-        got += [batch(fe, 4), batch(fe, 6)]
-    with plf.Frontend(camera=cam, limits=lim, **prm) as fe:
-        fresh = operators(fe)
-    assert len(ops[0]) > 0 and len(ops[3]) > 0
-    for a, b in zip(ops, fresh):
-        assert np.array_equal(a, b)
-    for (res_a, fr_a), (res_b, fr_b) in zip(base, got):
-        for a, b in zip(res_a, res_b):
-            for f in plf.RESULT_FIELDS:
-                assert a[f] == b[f], f
-            assert np.array_equal(a["DT"], b["DT"])
-        for a, b in zip(fr_a, fr_b):
-            for k in a:
-                assert np.array_equal(a[k], b[k]), k
+
+def test_standalone_capacity_error_between_batches(built):
+    """A standalone call that exceeds max_keypoints (fe.orb on noise) or max_segments (fe.lsd on a few hundred boxes)
+    fails with a capacity error, while the batches in flight around it, whose frames stay within both limits, download
+    without error and with the results of an uninterrupted run."""
+    cam, world = STANDALONE_CAM, STANDALONE_WORLD
+    frames = list(synth.stream(cam, 8, world=world, seed=21, step=0.12))
+    Ls, Rs = np.stack([f[0] for f in frames]), np.stack([f[1] for f in frames])
+    noise = np.random.default_rng(0).integers(0, 256, (cam["height"], cam["width"]), dtype=np.uint8)
+    boxes = np.full((cam["height"], cam["width"]), 40, np.uint8)
+    rng = np.random.default_rng(1)
+    for _ in range(400):
+        x, y = rng.integers(0, cam["width"] - 20), rng.integers(0, cam["height"] - 20)
+        boxes[y:y + rng.integers(6, 20), x:x + rng.integers(6, 20)] = rng.integers(120, 255)
+    lim = plf.default_limits(); lim.max_batch = 2; lim.max_keypoints = 3000; lim.max_segments = 1000
+    prm = dict(orb_nfeatures=5000, lsd_nfeatures=150)   # the frames: < 1800 keypoints, < 500 segments per image
+
+    def overflow(fe):
+        with pytest.raises(plf.PlfError, match=r"plf_orb failed \(-4\).*capacity"):
+            fe.orb(noise)
+        with pytest.raises(plf.PlfError, match=r"plf_lsd failed \(-4\).*capacity"):
+            fe.lsd(boxes)
+
+    for in_flight in (0, 3):
+        with plf.Frontend(camera=cam, limits=lim, **prm) as fe:
+            base = drive_batches(fe, Ls, Rs, in_flight)
+        with plf.Frontend(camera=cam, limits=lim, **prm) as fe:
+            got = drive_batches(fe, Ls, Rs, in_flight, overflow)
+        assert_same_batches(base, got)
 
 
 def test_trajectory_ate_vs_oracle_and_ground_truth(built):
