@@ -697,7 +697,6 @@ plf_status plf_bow_insert(plf_ctx* ctx, int kf_idx, const plf_frame_view* kf, do
   }
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t cs = ctx->stream;
-  ctx->cur = cs;
   for (int c = 0; c < 2; ++c)
     if (on[c]) {
       plf_status st = grow_db(ctx, S->kind[c], (size_t)n[c], kf_idx);

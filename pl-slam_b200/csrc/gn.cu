@@ -346,10 +346,10 @@ plf_gn_opts plf_gn_opts_from_params(const plf_params& p) {
   return o;
 }
 
-plf_status plf_launch_gn(plf_ctx* ctx, const GnProblem* d_probs, int nprob, const plf_gn_opts& o) {
+plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs, int nprob, const plf_gn_opts& o) {
   if (nprob <= 0) return PLF_OK;
   GnCam c = {ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy};
-  k_gn_pose<<<nprob, GN_THREADS, 0, ctx->cur>>>(d_probs, c, o);
+  k_gn_pose<<<nprob, GN_THREADS, 0, cs>>>(d_probs, c, o);
   PLF_LAUNCH_CHECK(ctx);
   return PLF_OK;
 }
@@ -388,7 +388,7 @@ extern "C" plf_status plf_gn_pose(plf_ctx* ctx, const plf_gn_opts* opts, const d
   PLF_CUDA(ctx, cudaMemcpyAsync(dT, T_init ? T_init : Tid, sizeof Tid, cudaMemcpyHostToDevice, s));
   GnProblem hp = {dP, dO, dIp, nullptr, np, dsP, deP, dle, dIl, nullptr, nl, dT, dout};
   PLF_CUDA(ctx, cudaMemcpyAsync(dprob, &hp, sizeof hp, cudaMemcpyHostToDevice, s));
-  plf_status st = plf_launch_gn(ctx, dprob, 1, o);
+  plf_status st = plf_launch_gn(ctx, s, dprob, 1, o);
   if (st) return st;
   PLF_CUDA(ctx, cudaMemcpyAsync(out, dout, sizeof *out, cudaMemcpyDeviceToHost, s));
   if (np) PLF_CUDA(ctx, cudaMemcpyAsync(inlier_pt, dIp, (size_t)np, cudaMemcpyDeviceToHost, s));

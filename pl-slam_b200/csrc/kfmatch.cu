@@ -327,12 +327,12 @@ plf_status run_kind(plf_ctx* ctx, KindRun& r, const KindPlan& p, uint8_t* dev, c
     a.d1 = k.dq; a.d2 = k.dt; a.d1_stride = a.d2_stride = 0;
     a.n1 = k.nq; a.n2 = k.nt; a.n1_stride = a.n2_stride = 0;
     a.m12 = k.m_g; a.m12_stride = 0; a.count = k.stat + 2; a.count_stride = 0;
-    if ((st = plf_launch_match_grid_batch(ctx, a, 1, p.nq, p.nt, r.slot))) return st;
+    if ((st = plf_launch_match_grid_batch(ctx, a, 1, p.nq, p.nt, r.slot, cs))) return st;
   }
   if (r.bf) {
     const KnnProblem* dkp = (const KnnProblem*)(dev + p.kp);
-    if ((st = plf_launch_knn2(ctx, dkp, P.best_lr_matches ? 2 : 1, std::max(p.nq, p.nt)))) return st;
-    if ((st = plf_launch_nnr(ctx, (const NnrProblem*)(dev + p.np), 1, p.nq))) return st;
+    if ((st = plf_launch_knn2(ctx, cs, dkp, P.best_lr_matches ? 2 : 1, std::max(p.nq, p.nt)))) return st;
+    if ((st = plf_launch_nnr(ctx, cs, (const NnrProblem*)(dev + p.np), 1, p.nq))) return st;
   }
   k_kf_select<<<gq, 256, 0, cs>>>(k, fast, r.bf ? 1 : 0, r.kmin, r.gate);
   PLF_LAUNCH_CHECK(ctx);
@@ -351,7 +351,6 @@ plf_status kf_run(plf_ctx* ctx, bool map, const plf_kf_match_opts* o, const doub
   uint8_t *pin, *dev;
   if (plf_status st = L.acquire(ctx, PLF_SCR_KF, &pin, &dev)) return st;
   cudaStream_t cs = ctx->stream;
-  ctx->cur = cs;
   const KfCam cam = {ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy, (double)ctx->cam.width, (double)ctx->cam.height,
                      PLF_GRID_COLS / (double)ctx->cam.width, PLF_GRID_ROWS / (double)ctx->cam.height};
   memcpy(pin + t_off, T, 16 * 8);

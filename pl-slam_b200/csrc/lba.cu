@@ -662,7 +662,6 @@ static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_p
   d.fixedTinv = dFTi;
   d.obs_lm = dLm; d.obs_kf = dKf; d.obs_z = dZ; d.lm_start = dLs;
   cudaStream_t cs = ctx->stream;
-  ctx->cur = cs;
   std::vector<double> hX(N);
   for (int i = 0; i < 6 * nkf; ++i) hX[i] = p->kf_pose[i];
   for (int i = 0; i < 3 * npt; ++i) hX[6 * nkf + i] = p->pt[i];

@@ -28,11 +28,7 @@
 #define LBD_WB 7
 #define LBD_ROWS 63
 
-__constant__ float c_gaussL[21];  // (float)gaussCoefL_[i]
-__constant__ float c_gaussG[63];  // (float)gaussCoefG_[i]
-__constant__ int c_comb[32][2];
-
-static const int h_comb[32][2] = {
+__constant__ int c_comb[32][2] = {
     {0, 1}, {0, 2}, {0, 3}, {0, 4}, {0, 5}, {0, 6}, {1, 2}, {1, 3}, {1, 4}, {1, 5}, {1, 6},
     {2, 3}, {2, 4}, {2, 5}, {2, 6}, {2, 7}, {2, 8}, {3, 4}, {3, 5}, {3, 6}, {3, 7}, {3, 8},
     {4, 5}, {4, 6}, {4, 7}, {4, 8}, {5, 6}, {5, 7}, {5, 8}, {6, 7}, {6, 8}, {7, 8}};
@@ -182,27 +178,30 @@ __global__ void __launch_bounds__(256) k_blur5_sobel_fast(const __grid_constant_
   }
 }
 
-plf_status plf_launch_blur5_sobel(plf_ctx* ctx, PlfTmaCache* tm, const uint8_t* imgs, int pitch, size_t img_stride,
-                                  int w, int h, int nimg, short2* grad, size_t grad_stride) {
+plf_status plf_launch_blur5_sobel(plf_ctx* ctx, cudaStream_t cs, PlfTmaCache* tm, const uint8_t* imgs, int pitch,
+                                  size_t img_stride, int w, int h, int nimg, short2* grad, size_t grad_stride) {
   if (nimg <= 0) return PLF_OK;
   if (w >= 8 && h >= 8 && (pitch & 15) == 0 && (img_stride & 15) == 0 && ((uintptr_t)imgs & 15) == 0) {
     const CUtensorMap* map = tm->get(imgs, w, h, nimg, pitch, img_stride ? img_stride : (size_t)pitch * h, 80, LBF_TH + 6);
     if (!map) return plf_fail(ctx, PLF_ERR_CUDA, "LBD: cuTensorMapEncodeTiled failed (pitch %d, stride %zu)", pitch, img_stride);
     dim3 grid(plf_tma_tiles_x(w, 3), (h + LBF_TH - 1) / LBF_TH, nimg);
-    k_blur5_sobel_fast<<<grid, 256, 0, ctx->cur>>>(*map, w, h, grad, grad_stride);
+    k_blur5_sobel_fast<<<grid, 256, 0, cs>>>(*map, w, h, grad, grad_stride);
   } else {  // tiny images / unpadded rows: generic kernel
     dim3 grid((w + LBD_TW - 1) / LBD_TW, (h + LBD_TH - 1) / LBD_TH, nimg);
-    k_blur5_sobel<<<grid, 256, 0, ctx->cur>>>(imgs, pitch, img_stride, w, h, grad, grad_stride);
+    k_blur5_sobel<<<grid, 256, 0, cs>>>(imgs, pitch, img_stride, w, h, grad, grad_stride);
   }
   PLF_LAUNCH_CHECK(ctx);
   return PLF_OK;
 }
 
+// The band (L) and row (G) Gaussian weights: (float)gaussCoefL_[i], (float)gaussCoefG_[i].
+struct LbdGauss { float L[21], G[63]; };
+
 // One CTA per (image, line slot).  kls: [nimg][max_lines]; counts: [nimg]; desc: [nimg][max_lines][32].
 __global__ void __launch_bounds__(64, 12) k_lbd(const short2* __restrict__ grad, size_t grad_stride, int w,
                                             int h, const plf_keyline* __restrict__ kls,
                                             const int* __restrict__ counts, int max_lines,
-                                            uint8_t* __restrict__ desc, float* __restrict__ desc_f) {
+                                            uint8_t* __restrict__ desc, float* __restrict__ desc_f, const LbdGauss gs) {
   const int img = blockIdx.y, li = blockIdx.x;
   if (li >= counts[img]) return;
   const plf_keyline kl = kls[(size_t)img * max_lines + li];
@@ -242,7 +241,7 @@ __global__ void __launch_bounds__(64, 12) k_lbd(const short2* __restrict__ grad,
       sCorX = __fadd_rn(sCorX, dL0);
       sCorY = __fadd_rn(sCorY, dL1);
     }
-    const float cg = c_gaussG[hID];
+    const float cg = gs.G[hID];
     pL = __fmul_rn(cg, pL); nL = __fmul_rn(cg, nL); pO = __fmul_rn(cg, pO); nO = __fmul_rn(cg, nO);
     rowv[hID][0] = pL; rowv[hID][1] = nL;
     rowv[hID][2] = __fmul_rn(pL, pL); rowv[hID][3] = __fmul_rn(nL, nL);
@@ -260,7 +259,7 @@ __global__ void __launch_bounds__(64, 12) k_lbd(const short2* __restrict__ grad,
       const int rb = hh / LBD_WB;
       // own band: weights [7..13]; row of band b+1 feeds b as "band above": [14..20]; row of band b-1: [0..6]
       const int wi = (hh % LBD_WB) + (rb == b ? LBD_WB : (rb == b + 1 ? 2 * LBD_WB : 0));
-      const float c = c_gaussL[wi];
+      const float c = gs.L[wi];
       const float v = rowv[hh][q];
       acc = __fadd_rn(acc, sq ? __fmul_rn(__fmul_rn(c, c), v) : __fmul_rn(c, v));
     }
@@ -324,40 +323,30 @@ __global__ void __launch_bounds__(64, 12) k_lbd(const short2* __restrict__ grad,
   }
 }
 
-static plf_status plf_lbd_init(plf_ctx* ctx) {
-  if (ctx->lbd_tables) return PLF_OK;
-  // BinaryDescriptor ctor, binary_descriptor_custom.cpp:217-259 (host doubles, narrowed at use sites)
-  float gl[21], gg[63];
-  {
-    double u = (LBD_WB * 3 - 1) / 2, sigma = (LBD_WB * 2 + 1) / 2, inv = -1 / (2 * sigma * sigma);
-    for (int i = 0; i < 21; ++i) {
-      double dis = i - u;
-      gl[i] = (float)exp(dis * dis * inv);
-    }
-    u = (LBD_NB * LBD_WB - 1) / 2;
-    sigma = u;
-    inv = -1 / (2 * sigma * sigma);
-    for (int i = 0; i < 63; ++i) {
-      double dis = i - u;
-      gg[i] = (float)exp(dis * dis * inv);
-    }
+// BinaryDescriptor ctor, binary_descriptor_custom.cpp:217-259 (host doubles, narrowed at use sites)
+static LbdGauss lbd_gauss() {
+  LbdGauss gs;
+  double u = (LBD_WB * 3 - 1) / 2, sigma = (LBD_WB * 2 + 1) / 2, inv = -1 / (2 * sigma * sigma);
+  for (int i = 0; i < 21; ++i) {
+    double dis = i - u;
+    gs.L[i] = (float)exp(dis * dis * inv);
   }
-  PLF_CUDA(ctx, cudaMemcpyToSymbolAsync(c_gaussL, gl, sizeof gl, 0, cudaMemcpyHostToDevice, ctx->stream));
-  PLF_CUDA(ctx, cudaMemcpyToSymbolAsync(c_gaussG, gg, sizeof gg, 0, cudaMemcpyHostToDevice, ctx->stream));
-  PLF_CUDA(ctx, cudaMemcpyToSymbolAsync(c_comb, h_comb, sizeof h_comb, 0, cudaMemcpyHostToDevice, ctx->stream));
-  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  ctx->lbd_tables = true;
-  return PLF_OK;
+  u = (LBD_NB * LBD_WB - 1) / 2;
+  sigma = u;
+  inv = -1 / (2 * sigma * sigma);
+  for (int i = 0; i < 63; ++i) {
+    double dis = i - u;
+    gs.G[i] = (float)exp(dis * dis * inv);
+  }
+  return gs;
 }
 
-plf_status plf_launch_lbd(plf_ctx* ctx, const short2* grad, size_t grad_stride, int w, int h, int nimg,
+plf_status plf_launch_lbd(plf_ctx* ctx, cudaStream_t cs, const short2* grad, size_t grad_stride, int w, int h, int nimg,
                           const plf_keyline* kls, const int* counts, int max_lines, uint8_t* desc,
                           float* desc_f) {
   if (nimg <= 0 || max_lines <= 0) return PLF_OK;
-  plf_status st = plf_lbd_init(ctx);
-  if (st) return st;
   dim3 grid(max_lines, nimg);
-  k_lbd<<<grid, 64, 0, ctx->cur>>>(grad, grad_stride, w, h, kls, counts, max_lines, desc, desc_f);
+  k_lbd<<<grid, 64, 0, cs>>>(grad, grad_stride, w, h, kls, counts, max_lines, desc, desc_f, lbd_gauss());
   PLF_LAUNCH_CHECK(ctx);
   return PLF_OK;
 }
@@ -367,7 +356,6 @@ extern "C" plf_status plf_lbd_gradients(plf_ctx* ctx, const uint8_t* img, int w,
   if (!ctx || !img || !dxdy || w < 2 || h < 2 || stride < w)
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_lbd_gradients: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  ctx->cur = ctx->stream;
   const int pitch = plf_pitch16(w);
   uint8_t* dimg;
   short2* dgrad;
@@ -376,7 +364,7 @@ extern "C" plf_status plf_lbd_gradients(plf_ctx* ctx, const uint8_t* img, int w,
   if (plf_status st = scr.carve(ctx, PLF_SCR_LBD)) return st;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
   PlfTmaCache tm;
-  plf_status st = plf_launch_blur5_sobel(ctx, &tm, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
+  plf_status st = plf_launch_blur5_sobel(ctx, ctx->stream, &tm, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
   if (st) return st;
   PLF_CUDA(ctx, cudaMemcpyAsync(dxdy, dgrad, (size_t)w * h * 4, cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -394,7 +382,6 @@ extern "C" plf_status plf_lbd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   if (n > 32767)
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_lbd: %d lines (reference numOfFinalLine is a short, :1029)", n);
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  ctx->cur = ctx->stream;
   const int pitch = plf_pitch16(w);
   uint8_t *dimg, *ddesc;
   short2* dgrad;
@@ -409,9 +396,9 @@ extern "C" plf_status plf_lbd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   PLF_CUDA(ctx, cudaMemcpyAsync(dkl, keylines, (size_t)n * sizeof(plf_keyline), cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyAsync(dcount, &n, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
   PlfTmaCache tm;
-  plf_status st = plf_launch_blur5_sobel(ctx, &tm, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
+  plf_status st = plf_launch_blur5_sobel(ctx, ctx->stream, &tm, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
   if (st) return st;
-  st = plf_launch_lbd(ctx, dgrad, 0, w, h, 1, dkl, dcount, n, ddesc, desc_float ? dfl : nullptr);
+  st = plf_launch_lbd(ctx, ctx->stream, dgrad, 0, w, h, 1, dkl, dcount, n, ddesc, desc_float ? dfl : nullptr);
   if (st) return st;
   PLF_CUDA(ctx, cudaMemcpyAsync(desc, ddesc, (size_t)n * 32, cudaMemcpyDeviceToHost, ctx->stream));
   if (desc_float)

@@ -55,10 +55,13 @@
 #define LSD_BINS_MAX 1024
 #define LSD_QCAP 256   // shared-memory window of the region queue (entries)
 
+// The Q8 taps of the Gaussian pre-blur; k_blur_q8 takes them by value (8-byte aligned: read in pairs).
+struct __align__(8) LsdTaps { int k[16]; };
+
 // What LSD derives from the context's parameters alone, built once per context and read by every LSD state.
 struct LsdTables {
-  int ksize = 0;            // Gaussian pre-blur (0: scale 1, no blur); its taps are also in c_lsd_taps
-  int taps[16];
+  int ksize = 0;            // Gaussian pre-blur (0: scale 1, no blur)
+  LsdTaps taps;
   bool taps_u8 = false;     // every tap <= 255: the packed-byte fast blur applies (a 256 centre tap at small sigma does not)
   double prec = 0, p = 0, rho = 0;
   int m2_min = 0;           // smallest gx^2+gy^2 whose gradient norm exceeds rho (defined pixel)
@@ -109,14 +112,13 @@ struct LsdState {
   DevBufList bufs;
 };
 
-__constant__ int c_lsd_taps[16];
-
 // ---- fixed-point Gaussian (ksize <= 15) ------------------------------------------------------------------
 #define BQ_TW 64
 #define BQ_TH 16
 #define BQ_R 7
 __global__ void __launch_bounds__(256) k_blur_q8(const uint8_t* __restrict__ src, size_t src_stride, int pitch,
-                                                 int w, int h, int r, uint8_t* __restrict__ dst, size_t dst_stride, int dpitch) {
+                                                 int w, int h, int r, uint8_t* __restrict__ dst, size_t dst_stride, int dpitch,
+                                                 const __grid_constant__ LsdTaps taps) {
   __shared__ uint8_t raw[BQ_TH + 2 * BQ_R][BQ_TW + 2 * BQ_R + 2];
   __shared__ uint16_t hrow[BQ_TH + 2 * BQ_R][BQ_TW];
   const uint8_t* s = src + (size_t)blockIdx.z * src_stride;
@@ -135,7 +137,7 @@ __global__ void __launch_bounds__(256) k_blur_q8(const uint8_t* __restrict__ src
   const int tx = tid & (BQ_TW - 1), rg = tid >> 6;  // BQ_TW == 64
   for (int ry = rg; ry < RH; ry += 4) {
     uint32_t a = 0;
-    for (int k = 0; k < ks; ++k) a += (uint32_t)c_lsd_taps[k] * raw[ry][tx + k];
+    for (int k = 0; k < ks; ++k) a += (uint32_t)taps.k[k] * raw[ry][tx + k];
     hrow[ry][tx] = (uint16_t)a;
   }
   __syncthreads();
@@ -145,7 +147,7 @@ __global__ void __launch_bounds__(256) k_blur_q8(const uint8_t* __restrict__ src
       const int gy = y0 + ty;
       if (gy >= h) break;
       uint32_t a = 0;
-      for (int k = 0; k < ks; ++k) a += (uint32_t)c_lsd_taps[k] * hrow[ty + k][tx];
+      for (int k = 0; k < ks; ++k) a += (uint32_t)taps.k[k] * hrow[ty + k][tx];
       const uint32_t v = (a + (1u << 15)) >> 16;
       d[(size_t)gy * dpitch + gx] = (uint8_t)(v > 255 ? 255 : v);
     }
@@ -1163,9 +1165,9 @@ static plf_status lsd_tables_build(plf_ctx* ctx, LsdTables* t) {
     const unsigned hk = (unsigned)(ceil(sigma * sqrt(2 * 3.0 * log(10.0))));
     t->ksize = 1 + 2 * (int)hk;
     if (t->ksize > 15) return plf_fail(ctx, PLF_ERR_INVALID, "LSD: Gaussian kernel %d > 15 unsupported", t->ksize);
-    gaussian_taps_q8(t->ksize, sigma, t->taps);
+    gaussian_taps_q8(t->ksize, sigma, t->taps.k);
     t->taps_u8 = true;
-    for (int k = 0; k < t->ksize; ++k) t->taps_u8 = t->taps_u8 && t->taps[k] <= 255;
+    for (int k = 0; k < t->ksize; ++k) t->taps_u8 = t->taps_u8 && t->taps.k[k] <= 255;
   }
   for (t->m2_min = 0; t->m2_min <= 2 * 510 * 510; ++t->m2_min)  // same double expression as the kernels
     if (!(sqrt((double)t->m2_min / 4.0) <= t->rho)) break;
@@ -1177,13 +1179,11 @@ static plf_status lsd_tables_build(plf_ctx* ctx, LsdTables* t) {
   if (st) return st;
   k_lsd_build_lut<<<(LSD_LUT_DIM * LSD_LUT_DIM + 255) / 256, 256, 0, ctx->stream>>>(t->rho, t->angle_lut, t->cs_lut, t->seed_lut);
   PLF_LAUNCH_CHECK(ctx);
-  if (scale != 1.0)
-    PLF_CUDA(ctx, cudaMemcpyToSymbolAsync(c_lsd_taps, t->taps, sizeof(int) * 16, 0, cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return PLF_OK;
 }
 
-// Once per context, before any LSD state: c_lsd_taps is written here only, never while an LSD kernel may read it.
+// Once per context, before any LSD state.
 plf_status plf_lsd_tables(plf_ctx* ctx) {
   if (ctx->lsd_tables) return PLF_OK;
   LsdTables* t = new LsdTables();
@@ -1245,12 +1245,11 @@ plf_status plf_lsd_create(plf_ctx* ctx, int w, int h, int nimg, bool two_paritie
 // LSD on images [0, n) of a batch resident on the device, in two phases so that callers can overlap them with other
 // work: `pre` = blur, resample, gradient and seed ordering (bandwidth-bound), `grow` = region growing, rectangle fit and
 // the KeyLine stage (latency-bound).  `par` selects the buffer set that carries data from pre to grow.  The state must
-// hold >= n images.  Enqueued on ctx->cur; results stay on the device.
-plf_status plf_lsd_pre(plf_ctx* ctx, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int par, int n) {
+// hold >= n images.  Enqueued on cs; results stay on the device.
+plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int par, int n) {
   if (s->nimg < n) return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_pre: %d images > the state's %d", n, s->nimg);
   const LsdTables& T = *ctx->lsd_tables;
   const int w = s->w, h = s->h;
-  cudaStream_t cs = ctx->cur;
   const int W = s->ws, H = s->hs;
   const size_t As = (size_t)W * H, A = (size_t)s->bp * h, Asp = (size_t)s->sp * H;
   LsdPix* pix = s->pix[par] + (s->ws + 1);  // pixel (0,0) of the first image
@@ -1265,19 +1264,19 @@ plf_status plf_lsd_pre(plf_ctx* ctx, LsdState* s, const uint8_t* d_imgs, size_t 
       if (!tm)
         return plf_fail(ctx, PLF_ERR_CUDA, "LSD: cuTensorMapEncodeTiled failed for the source images (pitch %d, stride %zu)", pitch, img_stride);
       uint32_t tA = 0, tB = 0;
-      for (int k = 0; k < T.ksize; ++k) (k < 4 ? tA : tB) |= (uint32_t)T.taps[k] << (8 * (k & 3));
+      for (int k = 0; k < T.ksize; ++k) (k < 4 ? tA : tB) |= (uint32_t)T.taps.k[k] << (8 * (k & 3));
       dim3 gf(plf_tma_tiles_x(w, T.ksize / 2), (h + BF_TH - 1) / BF_TH, n);
       if (T.ksize == 7) k_blur_q8_fast<7><<<gf, 256, 0, cs>>>(*tm, 0, w, h, tA, tB, s->blur, A, s->bp);
       else k_blur_q8_fast<5><<<gf, 256, 0, cs>>>(*tm, 0, w, h, tA, tB, s->blur, A, s->bp);
     } else {
       dim3 gb((w + BQ_TW - 1) / BQ_TW, (h + BQ_TH - 1) / BQ_TH, n);
-      k_blur_q8<<<gb, 256, 0, cs>>>(d_imgs, img_stride, pitch, w, h, T.ksize / 2, s->blur, A, s->bp);
+      k_blur_q8<<<gb, 256, 0, cs>>>(d_imgs, img_stride, pitch, w, h, T.ksize / 2, s->blur, A, s->bp, T.taps);
     }
     PLF_LAUNCH_CHECK(ctx);
-    plf_mark(ctx, "lsd.k_blur_q8");
-    st = plf_launch_resize_exact(ctx, s->blur, A, s->bp, w, h, s->scaled, Asp, s->sp, W, H, s->rs_tab + s->rs_x_off, s->rs_tab + s->rs_xp_off, s->rs_tab + s->rs_y_off, n);
+    plf_mark(ctx, cs, "lsd.k_blur_q8");
+    st = plf_launch_resize_exact(ctx, cs, s->blur, A, s->bp, w, h, s->scaled, Asp, s->sp, W, H, s->rs_tab + s->rs_x_off, s->rs_tab + s->rs_xp_off, s->rs_tab + s->rs_y_off, n);
     if (st) return st;
-    plf_mark(ctx, "lsd.k_resize_exact");
+    plf_mark(ctx, cs, "lsd.k_resize_exact");
     scaled = s->scaled;
     scaled_stride = Asp;
     scaled_pitch = s->sp;
@@ -1286,25 +1285,24 @@ plf_status plf_lsd_pre(plf_ctx* ctx, LsdState* s, const uint8_t* d_imgs, size_t 
   k_lsd_grad<<<dim3(s->nxb, (H + 1) / 2, n), LSD_GRAD_THREADS, 0, cs>>>(scaled, scaled_stride, scaled_pitch, W, H, T.angle_lut, T.m2_min, As, pix, s->pix_stride,
                                                                s->seedlist, s->segcnt, s->nxb, s->maxmag2);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "lsd.k_lsd_grad");
+  plf_mark(ctx, cs, "lsd.k_lsd_grad");
   k_lsd_rowhist<<<dim3(nchunks, n), 256, 0, cs>>>(As, W, H, s->n_bins, nchunks, s->nxb, s->maxmag2, s->seedlist, s->segcnt, s->rowcnt);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "lsd.k_lsd_rowhist");
+  plf_mark(ctx, cs, "lsd.k_lsd_rowhist");
   k_lsd_binscan<<<n, 1024, 0, cs>>>(s->rowcnt, nchunks, s->n_bins, s->binstart, s->nseeds[par]);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "lsd.k_lsd_binscan");
+  plf_mark(ctx, cs, "lsd.k_lsd_binscan");
   k_lsd_scatter<<<dim3((nchunks + 3) / 4, n), 128, 0, cs>>>(s->seedlist, s->segcnt, As, W, H, s->n_bins, nchunks, s->nxb, s->rowcnt, s->binstart,
                                                             s->order[par]);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "lsd.k_lsd_scatter");
+  plf_mark(ctx, cs, "lsd.k_lsd_scatter");
   return PLF_OK;
 }
 
-plf_status plf_lsd_grow(plf_ctx* ctx, LsdState* s, int par, int n, cudaEvent_t keylines_wait) {
+plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int n, cudaEvent_t keylines_wait) {
   if (s->nimg < n) return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_grow: %d images > the state's %d", n, s->nimg);
   const LsdTables& T = *ctx->lsd_tables;
   const int w = s->w, h = s->h;
-  cudaStream_t cs = ctx->cur;
   const int W = s->ws, H = s->hs;
   const size_t As = (size_t)W * H;
   LsdPix* pix = s->pix[par] + (s->ws + 1);
@@ -1315,19 +1313,19 @@ plf_status plf_lsd_grow(plf_ctx* ctx, LsdState* s, int par, int n, cudaEvent_t k
   k_lsd_grow<<<n, 32, 0, cs>>>(pix, s->pix_stride, As, W, s->order[par], T.seed_lut, T.cs_lut, s->nseeds[par], T.prec, (float)(T.p * 180.0),
                                s->min_reg_size, s->regpts, s->regions, s->max_regions, s->nregions, s->overflow);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "lsd.k_lsd_grow");
+  plf_mark(ctx, cs, "lsd.k_lsd_grow");
   k_lsd_rect_order<<<n, 256, 0, cs>>>(s->regions, s->max_regions, s->nregions, s->rect_perm);
   PLF_LAUNCH_CHECK(ctx);
   k_lsd_rects<<<dim3((s->max_regions + 127) / 128, n), 128, 0, cs>>>(pix, s->pix_stride, As, W, s->regpts, s->regions, s->max_regions, s->nregions,
                                                                      s->rect_perm, T.prec, s->scale, s->segs);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "lsd.k_lsd_rects");
+  plf_mark(ctx, cs, "lsd.k_lsd_rects");
   const double min_length = (double)ctx->params.min_line_length * (double)std::min(w, h);
   if (keylines_wait) PLF_CUDA(ctx, cudaStreamWaitEvent(cs, keylines_wait, 0));
   k_keylines<<<n, 1024, 0, cs>>>(s->segs, s->nregions, s->max_regions, w, h, min_length, ctx->params.lsd_nfeatures, s->kls_all, s->kls[par],
                                  s->max_lines, s->nlines[par], s->overflow);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "lsd.k_keylines");
+  plf_mark(ctx, cs, "lsd.k_keylines");
   return PLF_OK;
 }
 
@@ -1347,8 +1345,8 @@ static plf_status lsd_standalone(plf_ctx* ctx, const uint8_t* dimg, int pitch, i
     s = nullptr;
   }
   if (!s && (st = plf_lsd_create(ctx, w, h, 1, false, &s))) return st;
-  if ((st = plf_lsd_pre(ctx, s, dimg, (size_t)pitch * h, pitch, 0, 1))) return st;
-  return plf_lsd_grow(ctx, s, 0, 1, nullptr);
+  if ((st = plf_lsd_pre(ctx, ctx->stream, s, dimg, (size_t)pitch * h, pitch, 0, 1))) return st;
+  return plf_lsd_grow(ctx, ctx->stream, s, 0, 1, nullptr);
 }
 
 static plf_status lsd_check_overflow(plf_ctx* ctx, const LsdState* s, const char* what) {
@@ -1368,7 +1366,6 @@ extern "C" plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   if (!ctx || !img || !n_out || w < 3 || h < 3 || stride < w || cap < 0 || (cap > 0 && !segs))
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_lsd: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  ctx->cur = ctx->stream;
   const int pitch = plf_pitch16(w);
   uint8_t* dimg = (uint8_t*)plf_scratch(ctx, PLF_SCR_LSD, (size_t)pitch * h);
   if (!dimg) return PLF_ERR_CUDA;
@@ -1394,7 +1391,6 @@ extern "C" plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, 
   if (!ctx || !img || !n_out || w < 3 || h < 3 || stride < w || cap < 0 || (cap > 0 && (!keylines || !desc)))
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_detect_lines: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  ctx->cur = ctx->stream;
   const int pitch = plf_pitch16(w);
   uint8_t *dimg, *ddesc;
   short2* dgrad;
@@ -1406,9 +1402,9 @@ extern "C" plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, 
   if (st) return st;
   const LsdState* s = ctx->lsd_standalone;
   PlfTmaCache tm;
-  st = plf_launch_blur5_sobel(ctx, &tm, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
+  st = plf_launch_blur5_sobel(ctx, ctx->stream, &tm, dimg, pitch, (size_t)pitch * h, w, h, 1, dgrad, 0);
   if (st) return st;
-  st = plf_launch_lbd(ctx, dgrad, 0, w, h, 1, s->kls[0], s->nlines[0], s->max_lines, ddesc, nullptr);
+  st = plf_launch_lbd(ctx, ctx->stream, dgrad, 0, w, h, 1, s->kls[0], s->nlines[0], s->max_lines, ddesc, nullptr);
   if (st) return st;
   int n = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->nlines[0], sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));

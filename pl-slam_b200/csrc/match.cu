@@ -148,10 +148,10 @@ __global__ void __launch_bounds__(KM_WARPS * 32) k_hamming_knn2_mma(const KnnPro
   }
 }
 
-plf_status plf_launch_knn2(plf_ctx* ctx, const KnnProblem* d_probs, int nprob, int max_nq) {
+plf_status plf_launch_knn2(plf_ctx* ctx, cudaStream_t cs, const KnnProblem* d_probs, int nprob, int max_nq) {
   if (nprob <= 0 || max_nq <= 0) return PLF_OK;
   dim3 grid((max_nq + KM_QPB - 1) / KM_QPB, nprob);
-  k_hamming_knn2_mma<<<grid, KM_WARPS * 32, 0, ctx->cur>>>(d_probs);
+  k_hamming_knn2_mma<<<grid, KM_WARPS * 32, 0, cs>>>(d_probs);
   PLF_LAUNCH_CHECK(ctx);
   return PLF_OK;
 }
@@ -201,19 +201,19 @@ __global__ void __launch_bounds__(256) k_nnr_mark(const NnrProblem* __restrict__
     qlist[(size_t)blockIdx.y * stride + atomicAdd(&qcount[blockIdx.y], 1)] = m;
 }
 
-plf_status plf_launch_nnr_mark(plf_ctx* ctx, const NnrProblem* d_probs, int nprob, int max_n1, int* flags, int* qlist,
+plf_status plf_launch_nnr_mark(plf_ctx* ctx, cudaStream_t cs, const NnrProblem* d_probs, int nprob, int max_n1, int* flags, int* qlist,
                                int* qcount, int stride) {
   if (nprob <= 0 || max_n1 <= 0) return PLF_OK;
   dim3 grid((max_n1 + 255) / 256, nprob);
-  k_nnr_mark<<<grid, 256, 0, ctx->cur>>>(d_probs, flags, qlist, qcount, stride);
+  k_nnr_mark<<<grid, 256, 0, cs>>>(d_probs, flags, qlist, qcount, stride);
   PLF_LAUNCH_CHECK(ctx);
   return PLF_OK;
 }
 
-plf_status plf_launch_nnr(plf_ctx* ctx, const NnrProblem* d_probs, int nprob, int max_n1) {
+plf_status plf_launch_nnr(plf_ctx* ctx, cudaStream_t cs, const NnrProblem* d_probs, int nprob, int max_n1) {
   if (nprob <= 0 || max_n1 <= 0) return PLF_OK;
   dim3 grid((max_n1 + 255) / 256, nprob);
-  k_nnr_mutual<<<grid, 256, 0, ctx->cur>>>(d_probs);
+  k_nnr_mutual<<<grid, 256, 0, cs>>>(d_probs);
   PLF_LAUNCH_CHECK(ctx);
   return PLF_OK;
 }
@@ -241,7 +241,7 @@ extern "C" plf_status plf_hamming_knn2(plf_ctx* ctx, const uint8_t* d1, int n1, 
     PLF_CUDA(ctx, cudaMemcpyAsync(dt, d2, (size_t)n2 * 32, cudaMemcpyHostToDevice, ctx->stream));
   KnnProblem hp = {(const uint32_t*)dq, (const uint32_t*)dt, nullptr, nullptr, n1, n2, dbest, dsec};
   PLF_CUDA(ctx, cudaMemcpyAsync(dprob, &hp, sizeof hp, cudaMemcpyHostToDevice, ctx->stream));
-  plf_status st = plf_launch_knn2(ctx, dprob, 1, n1);
+  plf_status st = plf_launch_knn2(ctx, ctx->stream, dprob, 1, n1);
   if (st) return st;
   std::vector<uint32_t> hb(n1), hs(n1);
   PLF_CUDA(ctx, cudaMemcpyAsync(hb.data(), dbest, (size_t)n1 * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -293,9 +293,9 @@ extern "C" plf_status plf_match(plf_ctx* ctx, const uint8_t* d1, int n1, const u
   const int nk = best_lr ? 2 : 1;
   PLF_CUDA(ctx, cudaMemcpyAsync(dkp, hk, sizeof(KnnProblem) * nk, cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyAsync(dnp, &hn, sizeof hn, cudaMemcpyHostToDevice, ctx->stream));
-  plf_status st = plf_launch_knn2(ctx, dkp, nk, n1 > n2 ? n1 : n2);
+  plf_status st = plf_launch_knn2(ctx, ctx->stream, dkp, nk, n1 > n2 ? n1 : n2);
   if (st) return st;
-  st = plf_launch_nnr(ctx, dnp, 1, n1);
+  st = plf_launch_nnr(ctx, ctx->stream, dnp, 1, n1);
   if (st) return st;
   int hcount = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(matches_12, dm, (size_t)n1 * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -392,7 +392,6 @@ extern "C" plf_status plf_median_descriptors(plf_ctx* ctx, const uint8_t* desc, 
   PLF_CUDA(ctx, cudaMemcpyAsync(dofs, offsets, (size_t)(n_landmarks + 1) * 4, cudaMemcpyHostToDevice, cs));
   const bool want_dir = dirs && med_dir;
   if (want_dir && total > 0) PLF_CUDA(ctx, cudaMemcpyAsync(ddir, dirs, (size_t)total * 24, cudaMemcpyHostToDevice, cs));
-  ctx->cur = cs;
   k_median_desc<<<(n_landmarks + 3) / 4, 128, 0, cs>>>((const uint32_t*)dd, dofs, want_dir ? ddir : nullptr, n_landmarks, didx,
                                                        want_dir ? dmed : nullptr);
   PLF_LAUNCH_CHECK(ctx);

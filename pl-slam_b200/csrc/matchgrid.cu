@@ -175,7 +175,6 @@ static plf_status mg_run(plf_ctx* ctx, const char* who, int is_lines, const int*
   scr.add(D, (size_t)n1 * n2); scr.add(dm12, n1); scr.add(dm21, n2); scr.add(dcount, 1);
   if (plf_status st = scr.carve(ctx, PLF_SCR_MATCH)) return st;
   cudaStream_t cs = ctx->stream;
-  ctx->cur = cs;
   PLF_CUDA(ctx, cudaMemcpyAsync(dq, q_geo, (size_t)n1 * gq * 4, cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(dts, tstart.data(), (size_t)(n2 + 1) * 4, cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(dtc, tcells.data(), tcells.size() * 4, cudaMemcpyHostToDevice, cs));
@@ -389,7 +388,8 @@ __global__ void __launch_bounds__(128) k_mgb_mutual(MgbArgs a, int p0) {
 }
 
 // Runs nprob windowed matching problems.  scratch: MGB scratch of the context (slot `slot`), sized here.
-plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n1, int max_n2, plf_scratch_slot slot) {
+plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n1, int max_n2, plf_scratch_slot slot,
+                                       cudaStream_t cs) {
   if (nprob <= 0) return PLF_OK;
   if (a.g.cols * a.g.rows > 32 * MGB_MASK_WORDS) return plf_fail(ctx, PLF_ERR_INVALID, "match grid: %dx%d cells exceed the mask", a.g.cols, a.g.rows);
   const int K = a.K, Kt = a.Kt;
@@ -399,7 +399,6 @@ plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int m
   DevBufList scr;
   scr.add(a.D, nD * chunk); scr.add(a.qmask, nM * chunk); scr.add(a.m21, (size_t)Kt * chunk);
   if (plf_status st = scr.carve(ctx, slot)) return st;
-  cudaStream_t cs = ctx->cur;
   const int gx1 = (max_n1 + 127) / 128, gx2 = (max_n2 + 127) / 128;
   if (gx1 == 0 || gx2 == 0) return PLF_OK;
   for (int p0 = 0; p0 < nprob; p0 += chunk) {

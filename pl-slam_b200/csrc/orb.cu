@@ -24,8 +24,8 @@
 //   k_rbrief         256 rotated pair tests from a 37x37 shared-memory patch, one warp per keypoint (lane = byte)
 // Per-image algorithmic bytes are A0 + 2*sum(A_k>=1) + 2*S + 56*N (SURVEY §8d); what bounds each kernel (issue rate,
 // latency - none is HBM-bound) is discussed in DESIGN.md §4.
-#include "orb_pattern.h"
 #include "plf_internal.h"
+#include "orb_pattern.h"
 #include "plf_tma.cuh"
 
 #define ORB_MAX_LEVELS 8
@@ -53,6 +53,7 @@ struct OrbGeom {
   int tiles_x[ORB_MAX_LEVELS];
   int edge, fast_th, patch, half_patch;
   int max_kp;
+  float blur7[7];                   // getGaussianKernel(7, 2, CV_32F), the taps of k_orb_blur7_fast
 };
 
 struct OrbState {
@@ -79,8 +80,6 @@ struct OrbState {
   PlfTmaCache tm_fast0, tm_blur0;
   DevBufList bufs;
 };
-
-__constant__ float c_blur7[7];
 
 // ---- pyramid ---------------------------------------------------------------------------------------
 // tab layout per level: [ox(dw) | cx(dw) | oy(dh) | cy(dh) | packed x (k_resize_exact4)]
@@ -157,15 +156,15 @@ void plf_resize_pack_x(const int* ofs, const int* c1, int dw, int* out) {
   }
 }
 
-plf_status plf_launch_resize_exact(plf_ctx* ctx, const uint8_t* src, size_t src_stride, int sp, int sw, int sh, uint8_t* dst,
+plf_status plf_launch_resize_exact(plf_ctx* ctx, cudaStream_t cs, const uint8_t* src, size_t src_stride, int sp, int sw, int sh, uint8_t* dst,
                                    size_t dst_stride, int dp, int dw, int dh, const int* tabx, const int* tabxp, const int* taby, int nimg) {
   if ((double)sw <= 1.9 * (double)dw) {  // four outputs span at most 3 * 1.9 + 2 < 8 source columns
     dim3 grid((dw + 255) / 256, (dh + 3) / 4, nimg);
-    k_resize_exact4<<<grid, dim3(64, 4), 0, ctx->cur>>>(src, src_stride, sp, sw, sh, dst, dst_stride, dp, dw, dh,
-                                                        reinterpret_cast<const int4*>(tabxp), taby);
+    k_resize_exact4<<<grid, dim3(64, 4), 0, cs>>>(src, src_stride, sp, sw, sh, dst, dst_stride, dp, dw, dh,
+                                                  reinterpret_cast<const int4*>(tabxp), taby);
   } else {
     dim3 grid((dw + 255) / 256, dh, nimg);
-    k_resize_exact<<<grid, 256, 0, ctx->cur>>>(src, src_stride, sp, sw, sh, dst, dst_stride, dp, dw, dh, tabx, taby);
+    k_resize_exact<<<grid, 256, 0, cs>>>(src, src_stride, sp, sw, sh, dst, dst_stride, dp, dw, dh, tabx, taby);
   }
   PLF_LAUNCH_CHECK(ctx);
   return PLF_OK;
@@ -529,7 +528,7 @@ __global__ void __launch_bounds__(256) k_orb_blur7_fast(const __grid_constant__ 
   if (!(x0 >= 3 && x0 - 3 + NEED <= W && y0 >= 3 && y0 + OBF_TH + 3 <= H))   // border tile: BORDER_REFLECT_101 in place
     plf_tma_reflect_fix<RH, RP>(raw, x0 - 3, y0 - 3, W, H, NEED);
   __syncthreads();
-  const float k0 = c_blur7[0], k1 = c_blur7[1], k2 = c_blur7[2], k3 = c_blur7[3], k4 = c_blur7[4], k5 = c_blur7[5], k6 = c_blur7[6];
+  const float k0 = g.blur7[0], k1 = g.blur7[1], k2 = g.blur7[2], k3 = g.blur7[3], k4 = g.blur7[4], k5 = g.blur7[5], k6 = g.blur7[6];
   for (int it = tid; it < RH * (OBF_TW / 4); it += 256) {
     const int ry = it >> 4, j = it & 15;
     const uint32_t* wp = reinterpret_cast<const uint32_t*>(&raw[ry][4 * j]);
@@ -591,13 +590,13 @@ __global__ void __launch_bounds__(256) k_orb_trig(OrbGeom g, const plf_keypoint*
 __global__ void __launch_bounds__(256) k_rbrief(const uint8_t* __restrict__ blur, OrbGeom g,
                                                 const plf_keypoint* __restrict__ kps,
                                                 const int* __restrict__ kp_count, const float2* __restrict__ trig,
-                                                const int8_t* __restrict__ pattern, uint8_t* __restrict__ desc) {
+                                                uint8_t* __restrict__ desc) {
   // the pattern as floats, transposed so that the 32 lanes of a warp read consecutive float4s for their j-th test:
   // test tt = lane * 8 + j lives at patf[j * 32 + lane]
   __shared__ __align__(16) float4 patf[256];
   __shared__ __align__(16) uint8_t patch[8][RB_D][RB_P];
   {
-    const uint32_t w = reinterpret_cast<const uint32_t*>(pattern)[threadIdx.x];  // 4 x int8 of test threadIdx.x
+    const uint32_t w = reinterpret_cast<const uint32_t*>(d_orb_bit_pattern_31)[threadIdx.x];  // 4 x int8 of test threadIdx.x
     patf[(threadIdx.x & 7) * 32 + (threadIdx.x >> 3)] =
         make_float4((float)(int8_t)(w & 0xFF), (float)(int8_t)((w >> 8) & 0xFF), (float)(int8_t)((w >> 16) & 0xFF), (float)(int8_t)(w >> 24));
   }
@@ -679,9 +678,6 @@ void plf_orb_free(OrbState* s) {
   delete s;
 }
 
-static int8_t* g_dev_pattern = nullptr;  // shared by all contexts on a device (read-only), uploaded with c_blur7
-static int g_dev_pattern_device = -1;
-
 static plf_status orb_build(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, bool two_parities) {
   const plf_params& P = ctx->params;
   if (P.orb_nlevels < 1 || P.orb_nlevels > ORB_MAX_LEVELS || P.orb_wta_k != 2 || P.orb_score != 1 ||
@@ -739,6 +735,16 @@ static plf_status orb_build(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, b
     }
     g.nfeat[g.nlevels - 1] = std::max(P.orb_nfeatures - sum, 0);
   }
+  {  // getGaussianKernel(7, 2, CV_32F): host doubles -> float (pinned equal to cv2 in tests)
+    double d[7], sum = 0;
+    for (int i = 0; i < 7; ++i) {
+      const double x = i - 3.0;
+      d[i] = exp(-0.5 / (2.0 * 2.0) * x * x);
+      sum += d[i];
+    }
+    sum = 1. / sum;
+    for (int i = 0; i < 7; ++i) g.blur7[i] = (float)(d[i] * sum);
+  }
   {  // umax
     const int hp = g.half_patch;
     int v, v0, vmax = (int)floor(hp * sqrt(2.f) / 2 + 1), vmin = (int)ceil(hp * sqrt(2.f) / 2);
@@ -785,26 +791,6 @@ static plf_status orb_build(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, b
   PLF_CUDA(ctx, cudaMemsetAsync(s->overflow, 0, sizeof(int), ctx->stream));
   if (!tab.empty())
     PLF_CUDA(ctx, cudaMemcpyAsync(s->rs_tab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-  // The rBRIEF pattern and the blur kernel depend on nothing: uploaded once, not by every state (a state built while
-  // another one's kernels run must not write what they read)
-  if (!g_dev_pattern || g_dev_pattern_device != ctx->device) {
-    int8_t hp[1024];
-    for (int i = 0; i < 1024; ++i) hp[i] = (int8_t)h_orb_bit_pattern_31[i];
-    PLF_CUDA(ctx, cudaMalloc(&g_dev_pattern, 1024));
-    PLF_CUDA(ctx, cudaMemcpyAsync(g_dev_pattern, hp, 1024, cudaMemcpyHostToDevice, ctx->stream));
-    // getGaussianKernel(7, 2, CV_32F): host doubles -> float (pinned equal to cv2 in tests)
-    double d[7], sum = 0;
-    for (int i = 0; i < 7; ++i) {
-      const double x = i - 3.0;
-      d[i] = exp(-0.5 / (2.0 * 2.0) * x * x);
-      sum += d[i];
-    }
-    sum = 1. / sum;
-    float blur_k[7];
-    for (int i = 0; i < 7; ++i) blur_k[i] = (float)(d[i] * sum);
-    PLF_CUDA(ctx, cudaMemcpyToSymbolAsync(c_blur7, blur_k, sizeof blur_k, 0, cudaMemcpyHostToDevice, ctx->stream));
-    g_dev_pattern_device = ctx->device;
-  }
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   // tensor maps of the pyramid levels (fixed addresses); level 0 = the caller's image buffer, cached per run
   for (int l = 1; l < g.nlevels; ++l) {
@@ -827,13 +813,12 @@ plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_paritie
 }
 
 // Runs ORB on nimg (<= s->nimg) images of s->w x s->h resident at d_imgs ([nimg][h][pitch], pitch a multiple of 16,
-// stride img_stride bytes).  Enqueued on ctx->cur; results stay on the device.
-plf_status plf_orb_run(plf_ctx* ctx, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par) {
+// stride img_stride bytes).  Enqueued on cs; results stay on the device.
+plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par) {
   const int w = s->w, h = s->h;
   plf_status st;
   OrbGeom g = s->g;
   g.pitch[0] = pitch;
-  cudaStream_t cs = ctx->cur;
   const CUtensorMap* tm_fast0 = s->tm_fast0.get(d_imgs, w, h, nimg, pitch, img_stride, 96, 38);
   const CUtensorMap* tm_blur0 = s->tm_blur0.get(d_imgs, w, h, nimg, pitch, img_stride, 80, OBF_TH + 6);
   if (!tm_fast0 || !tm_blur0)
@@ -843,36 +828,36 @@ plf_status plf_orb_run(plf_ctx* ctx, OrbState* s, const uint8_t* d_imgs, size_t 
   for (int l = 1; l < g.nlevels; ++l) {
     const uint8_t* src = (l == 1) ? d_imgs : s->pyr + g.pyr_off[l - 1];
     const size_t sstride = (l == 1) ? img_stride : g.pyr_stride;
-    st = plf_launch_resize_exact(ctx, src, sstride, g.pitch[l - 1], g.w[l - 1], g.h[l - 1], s->pyr + g.pyr_off[l], g.pyr_stride,
+    st = plf_launch_resize_exact(ctx, cs, src, sstride, g.pitch[l - 1], g.w[l - 1], g.h[l - 1], s->pyr + g.pyr_off[l], g.pyr_stride,
                                  g.pitch[l], g.w[l], g.h[l], s->rs_tab + s->rs_x_off[l], s->rs_tab + s->rs_xp_off[l],
                                  s->rs_tab + s->rs_y_off[l], nimg);
     if (st) return st;
   }
-  plf_mark(ctx, "orb.k_resize_exact");
+  plf_mark(ctx, cs, "orb.k_resize_exact");
   for (int l = 0; l < g.nlevels; ++l) {
     const int tx_ = (g.w[l] + FN_OW - 1) / FN_OW, ty_ = (g.h[l] + FN_OH - 1) / FN_OH;
     k_fast_nms<<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(l == 0 ? *tm_fast0 : s->tm_fast[l], g, l, tx_, s->cand, s->cand_count,
                                                       s->hist, s->overflow);
     PLF_LAUNCH_CHECK(ctx);
   }
-  plf_mark(ctx, "orb.k_fast_nms");
+  plf_mark(ctx, cs, "orb.k_fast_nms");
   k_select_sort<<<nimg, 1024, 0, cs>>>(g, s->cand, s->cand_count, s->hist, s->kps[par], s->kp_lxy[par], s->kp_count[par], s->overflow);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "orb.k_select_sort");
+  plf_mark(ctx, cs, "orb.k_select_sort");
   k_ic_angle<<<dim3((g.max_kp + 7) / 8, nimg), 256, 0, cs>>>(d_imgs, img_stride, s->pyr, g, s->kps[par], s->kp_lxy[par], s->kp_count[par]);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "orb.k_ic_angle");
+  plf_mark(ctx, cs, "orb.k_ic_angle");
   for (int l = 0; l < g.nlevels; ++l) {
     const int tx_ = plf_tma_tiles_x(g.w[l], 3), ty_ = (g.h[l] + OBF_TH - 1) / OBF_TH;
     k_orb_blur7_fast<<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(l == 0 ? *tm_blur0 : s->tm_blur[l], g, s->blur, l, tx_);
     PLF_LAUNCH_CHECK(ctx);
   }
-  plf_mark(ctx, "orb.k_orb_blur7");
+  plf_mark(ctx, cs, "orb.k_orb_blur7");
   k_orb_trig<<<dim3((g.max_kp + 255) / 256, nimg), 256, 0, cs>>>(g, s->kps[par], s->kp_count[par], s->trig);
   PLF_LAUNCH_CHECK(ctx);
-  k_rbrief<<<dim3((g.max_kp + 7) / 8, nimg), 256, 0, cs>>>(s->blur, g, s->kps[par], s->kp_count[par], s->trig, g_dev_pattern, s->desc[par]);
+  k_rbrief<<<dim3((g.max_kp + 7) / 8, nimg), 256, 0, cs>>>(s->blur, g, s->kps[par], s->kp_count[par], s->trig, s->desc[par]);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "orb.k_rbrief");
+  plf_mark(ctx, cs, "orb.k_rbrief");
   return PLF_OK;
 }
 
@@ -888,7 +873,6 @@ extern "C" plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   if (!ctx || !img || !n_out || w < 8 || h < 8 || stride < w || cap < 0 || (cap > 0 && (!kps || !desc)))
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_orb: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  ctx->cur = ctx->stream;
   OrbState*& s = ctx->orb_standalone;
   plf_status st;
   if (s && (s->w != w || s->h != h)) {
@@ -901,7 +885,7 @@ extern "C" plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   uint8_t* dimg = (uint8_t*)plf_scratch(ctx, PLF_SCR_ORB, (size_t)pitch * h);
   if (!dimg) return PLF_ERR_CUDA;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  if ((st = plf_orb_run(ctx, s, dimg, (size_t)pitch * h, pitch, 1, 0))) return st;
+  if ((st = plf_orb_run(ctx, ctx->stream, s, dimg, (size_t)pitch * h, pitch, 1, 0))) return st;
   int n = 0, ovf = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->kp_count[0], sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyAsync(&ovf, s->overflow, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));

@@ -611,15 +611,14 @@ static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   const size_t A = (size_t)w * h, AP = (size_t)s->pitch * h;   // dense maps / padded images
   const uint8_t* imgs = s->imgs2[r.run_slot];
   cudaStream_t sE = r.sE;
-  ctx->cur = sE;
   PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_up[r.run_slot], 0));  // images uploaded
   PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->evX[par], 0));           // batch i-2 (same parity) no longer reads these buffers
-  plf_mark(ctx, "start");
+  plf_mark(ctx, sE, "start");
   PLF_CUDA(ctx, cudaEventRecord(s->tE0[par], sE));
-  plf_status st = plf_orb_run(ctx, s->orb, imgs, AP, s->pitch, 2 * B, par);
-  if (!st) st = plf_launch_blur5_sobel(ctx, &s->lbd_tm, imgs, s->pitch, AP, w, h, 2 * B, s->lbd_grad[par], A);
+  plf_status st = plf_orb_run(ctx, sE, s->orb, imgs, AP, s->pitch, 2 * B, par);
+  if (!st) st = plf_launch_blur5_sobel(ctx, sE, &s->lbd_tm, imgs, s->pitch, AP, w, h, 2 * B, s->lbd_grad[par], A);
   if (st) return st;
-  plf_mark(ctx, "lbd.k_blur5_sobel");
+  plf_mark(ctx, sE, "lbd.k_blur5_sobel");
   // this batch's ORB overflow flag: snapshot + clear on the E stream, so that a flag raised by batch i+1's extraction is
   // not reported on batch i's download
   PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp, plf_orb_overflow_flag(s->orb), sizeof(int), cudaMemcpyDeviceToDevice, sE));
@@ -638,19 +637,17 @@ static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   const int par = r.par;
   const size_t AP = (size_t)s->pitch * s->h;
   cudaStream_t sP = r.sP, sG = r.sG;
-  ctx->cur = sP;
   PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_up[r.run_slot], 0));
   if (r.lsd2) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->evG[par], 0));   // batch i-2 (same parity) has finished growing / fitting on these maps
   PLF_CUDA(ctx, cudaEventRecord(s->tG0[par], sP));
-  plf_status st = plf_lsd_pre(ctx, s->lsd, s->imgs2[r.run_slot], AP, s->pitch, r.lp, 2 * r.B);
+  plf_status st = plf_lsd_pre(ctx, sP, s->lsd, s->imgs2[r.run_slot], AP, s->pitch, r.lp, 2 * r.B);
   if (st) return st;
   PLF_CUDA(ctx, cudaEventRecord(s->ev_free2[r.run_slot], sP));
   PLF_CUDA(ctx, cudaEventRecord(s->evP[par], sP));
-  ctx->cur = sG;
   PLF_CUDA(ctx, cudaStreamWaitEvent(sG, s->evP[par], 0));
   // the KeyLine outputs are overwritten: the match phase that read them last (batch i-2 with two parities, batch i-1 with one)
   // has taken its copy
-  st = plf_lsd_grow(ctx, s->lsd, r.lp, 2 * r.B, r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr);
+  st = plf_lsd_grow(ctx, sG, s->lsd, r.lp, 2 * r.B, r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr);
   if (st) return st;
   PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp + 1, plf_lsd_overflow_flag(s->lsd), sizeof(int), cudaMemcpyDeviceToDevice, sG));
   PLF_CUDA(ctx, cudaMemsetAsync(plf_lsd_overflow_flag(s->lsd), 0, sizeof(int), sG));
@@ -686,7 +683,6 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   plf_orb_outputs(s->orb, par, &kps, &odesc, &kcnt, &mk);
   plf_lsd_outputs(s->lsd, r.lp, &kls, &lcnt, &ml);
   cudaStream_t cs = r.sM;
-  ctx->cur = cs;
   plf_status st;
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->evG[par], 0));
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->evE[par], 0));
@@ -695,8 +691,8 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     PLF_CUDA(ctx, cudaMemsetAsync(s->fs.pt_count, 0, sizeof(int), cs));
     PLF_CUDA(ctx, cudaMemsetAsync(s->fs.ls_count, 0, sizeof(int), cs));
   }
-  if ((st = plf_launch_lbd(ctx, s->lbd_grad[par], A, w, h, 2 * B, kls, lcnt, Ln, s->ldesc_raw, nullptr))) return st;
-  plf_mark(ctx, "lbd.k_lbd");
+  if ((st = plf_launch_lbd(ctx, cs, s->lbd_grad[par], A, w, h, 2 * B, kls, lcnt, Ln, s->ldesc_raw, nullptr))) return st;
+  plf_mark(ctx, cs, "lbd.k_lbd");
   // the rest of the match phase works on its own copy of the extraction outputs; evX releases this parity to batch i+2
   PLF_CUDA(ctx, cudaMemcpyAsync(s->kpsM, kps, sizeof(plf_keypoint) * 2 * (size_t)B * K, cudaMemcpyDeviceToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->descM, odesc, 32 * 2 * (size_t)B * K, cudaMemcpyDeviceToDevice, cs));
@@ -709,7 +705,7 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   else PLF_CUDA(ctx, cudaMemsetAsync(s->lcntM, 0, sizeof(int) * 2 * (size_t)B, cs));
   PLF_CUDA(ctx, cudaEventRecord(s->evX[par], cs));
   kps = s->kpsM; odesc = s->descM; kcnt = s->kcntM; kls = s->klsM; lcnt = s->lcntM;
-  plf_mark(ctx, "copy extraction outputs");
+  plf_mark(ctx, cs, "copy extraction outputs");
   PLF_CUDA(ctx, cudaMemsetAsync(s->mcount, 0, (size_t)B * 4 * sizeof(int), cs));
   const double mg_iw = PLF_GRID_COLS / (double)w, mg_ih = PLF_GRID_ROWS / (double)h;   // StereoFrame::inv_width / inv_height
   if (P.matching_strategy) {
@@ -719,25 +715,25 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     PLF_LAUNCH_CHECK(ctx);
     const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, P.matching_s_ws, 0, 0, 0};
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 2, s->mg_q[0], s->mg_t[0], nullptr, odesc, kcnt, s->m12,
-                                                        4 * (size_t)K, s->mcount, 4), B, K, K, PLF_SCR_MGB_PIPE))) return st;
+                                                        4 * (size_t)K, s->mcount, 4), B, K, K, PLF_SCR_MGB_PIPE, cs))) return st;
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 2, s->mg_q[1], s->mg_t[1], s->mg_dir[0], s->ldesc_raw, lcnt,
-                                                        s->m12 + K, 4 * (size_t)K, s->mcount + 1, 4), B, Ln, Ln, PLF_SCR_MGB_PIPE))) return st;
-    plf_mark(ctx, "stereo.k_mgb (matchGrid)");
+                                                        s->m12 + K, 4 * (size_t)K, s->mcount + 1, 4), B, Ln, Ln, PLF_SCR_MGB_PIPE, cs))) return st;
+    plf_mark(ctx, cs, "stereo.k_mgb (matchGrid)");
   } else {
     // L->R 2-NN for every left feature; R->L only for the right features that are somebody's accepted best match
     // (k_nnr_mutual reads nothing else of the reverse direction): the same matches for ~2/3 of the popcounts
-    if ((st = plf_launch_knn2(ctx, s->knn_stereo, 2 * B, std::max(K, Ln)))) return st;
+    if ((st = plf_launch_knn2(ctx, cs, s->knn_stereo, 2 * B, std::max(K, Ln)))) return st;
     if (P.best_lr_matches) {
       PLF_CUDA(ctx, cudaMemsetAsync(s->rev_flags, 0, 2 * (size_t)B * K * sizeof(int), cs));
       PLF_CUDA(ctx, cudaMemsetAsync(s->rev_count, 0, 2 * (size_t)B * sizeof(int), cs));
-      if ((st = plf_launch_nnr_mark(ctx, s->nnr_stereo, 2 * B, std::max(K, Ln), s->rev_flags, s->rev_list, s->rev_count, K))) return st;
+      if ((st = plf_launch_nnr_mark(ctx, cs, s->nnr_stereo, 2 * B, std::max(K, Ln), s->rev_flags, s->rev_list, s->rev_count, K))) return st;
       // the reverse problems are laid out after the forward problems of ALL max_batch pairs (pipe_prepare), not of this
       // call's B pairs: a partial batch (B < max_batch) must still start at 2 * max_batch
-      if ((st = plf_launch_knn2(ctx, s->knn_stereo + 2 * s->B, 2 * B, std::max(K, Ln)))) return st;
+      if ((st = plf_launch_knn2(ctx, cs, s->knn_stereo + 2 * s->B, 2 * B, std::max(K, Ln)))) return st;
     }
-    plf_mark(ctx, "stereo.k_hamming_knn2");
-    if ((st = plf_launch_nnr(ctx, s->nnr_stereo, 2 * B, std::max(K, Ln)))) return st;
-    plf_mark(ctx, "stereo.k_nnr_mutual");
+    plf_mark(ctx, cs, "stereo.k_hamming_knn2");
+    if ((st = plf_launch_nnr(ctx, cs, s->nnr_stereo, 2 * B, std::max(K, Ln)))) return st;
+    plf_mark(ctx, cs, "stereo.k_nnr_mutual");
   }
   StereoPrm sp = {P.max_dist_epip, P.min_disp, P.line_horiz_th, P.stereo_overlap_th, P.ls_min_disp_ratio,
                   ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy, ctx->cam.b};
@@ -745,10 +741,10 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_LAUNCH_CHECK(ctx);
   k_stereo_lines<<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, sp, s->fs, 1);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "stereo.k_stereo_points+lines");
-  if ((st = plf_launch_knn2(ctx, s->knn_f2f, 4 * B, std::max(K, Ln)))) return st;
-  plf_mark(ctx, "f2f.k_hamming_knn2");
-  if ((st = plf_launch_nnr(ctx, s->nnr_f2f, 2 * B, std::max(K, Ln)))) return st;
+  plf_mark(ctx, cs, "stereo.k_stereo_points+lines");
+  if ((st = plf_launch_knn2(ctx, cs, s->knn_f2f, 4 * B, std::max(K, Ln)))) return st;
+  plf_mark(ctx, cs, "f2f.k_hamming_knn2");
+  if ((st = plf_launch_nnr(ctx, cs, s->nnr_f2f, 2 * B, std::max(K, Ln)))) return st;
   if (P.matching_strategy) {
     // frame-to-frame: matchGrid() in a +-matching_f2f_ws window around the projected feature; the match() result above
     // stands where the window search found fewer than min_pt_matches / min_ls_matches
@@ -759,26 +755,26 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     const int ws = P.matching_f2f_ws;
     const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, ws, ws, ws, ws};
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 1, s->mg_q[2], s->mg_t[2], nullptr, s->fs.pdesc, s->fs.pt_count,
-                                                        s->m12g, 2 * (size_t)K, s->mgcount, 2), B, K, K, PLF_SCR_MGB_PIPE))) return st;
+                                                        s->m12g, 2 * (size_t)K, s->mgcount, 2), B, K, K, PLF_SCR_MGB_PIPE, cs))) return st;
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 1, s->mg_q[3], s->mg_t[3], s->mg_dir[1], s->fs.ldesc, s->fs.ls_count,
-                                                        s->m12g + K, 2 * (size_t)K, s->mgcount + 1, 2), B, Ln, Ln, PLF_SCR_MGB_PIPE))) return st;
+                                                        s->m12g + K, 2 * (size_t)K, s->mgcount + 1, 2), B, Ln, Ln, PLF_SCR_MGB_PIPE, cs))) return st;
     k_mg_select<<<dim3((K + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.pt_count, K, K, 0, P.min_pt_matches, s->m12);
     PLF_LAUNCH_CHECK(ctx);
     k_mg_select<<<dim3((Ln + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.ls_count, Ln, K, 1, P.min_ls_matches, s->m12);
     PLF_LAUNCH_CHECK(ctx);
-    plf_mark(ctx, "f2f.k_mgb (matchGrid)");
+    plf_mark(ctx, cs, "f2f.k_mgb (matchGrid)");
   }
   k_f2f_build<<<B, 1024, 0, cs>>>(s->fs, 0, K, Ln, s->m12 + 2 * K, s->m12 + 3 * K, 4 * K, s->gnP, s->gnObs, s->gnInlP, s->gnNp,
                                   s->gn_sP, s->gn_eP, s->gn_le, s->gnInlL, s->gnNl);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, "f2f.k_nnr_mutual+k_f2f_build");
-  if ((st = plf_launch_gn(ctx, s->gn_probs, B, plf_gn_opts_from_params(P)))) return st;
-  plf_mark(ctx, "gn.k_gn_pose");
+  plf_mark(ctx, cs, "f2f.k_nnr_mutual+k_f2f_build");
+  if ((st = plf_launch_gn(ctx, cs, s->gn_probs, B, plf_gn_opts_from_params(P)))) return st;
+  plf_mark(ctx, cs, "gn.k_gn_pose");
   k_finalize<<<(B + 127) / 128, 128, 0, cs>>>(s->gn_out, s->gnNp, s->gnNl, kcnt, lcnt, s->fs, 1, P.min_features,
                                                s->has_prev ? 0 : 1, B, s->results + (size_t)rp * s->B);
   PLF_LAUNCH_CHECK(ctx);
   if ((st = copy_slot(ctx, s, B, 0))) return st;  // carry the last frame to the next batch
-  plf_mark(ctx, "k_finalize+carry");
+  plf_mark(ctx, cs, "k_finalize+carry");
   // results + overflow flags to pinned memory as part of this batch's stream work; evM marks them ready
   PLF_CUDA(ctx, cudaMemcpyAsync(s->h_results[rp], s->results + (size_t)rp * s->B, sizeof(plf_frame_result) * B, cudaMemcpyDeviceToHost, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->h_ovf[rp], s->d_ovf + 2 * rp, 2 * sizeof(int), cudaMemcpyDeviceToHost, cs));
@@ -871,7 +867,6 @@ plf_status plf_batch_run(plf_ctx* ctx, int B) {
   st = run_extract(ctx, s, r);
   if (!st) st = run_lsd(ctx, s, r);
   if (!st) st = run_match(ctx, s, r);
-  ctx->cur = r.sM;
   if (st) return st;
   s->has_prev = true;
   s->pend_slot[s->n_pending] = r.rp;

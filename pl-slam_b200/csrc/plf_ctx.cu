@@ -2,7 +2,6 @@
 #include <stdarg.h>
 
 #include "plf_internal.h"
-#include <cstdlib>
 #include <cstdio>
 #include <cstring>
 
@@ -101,7 +100,7 @@ void* plf_pinned(plf_ctx* ctx, size_t bytes) {
   return ctx->pinned;
 }
 
-void plf_mark(plf_ctx* ctx, const char* name) {
+void plf_mark(plf_ctx* ctx, cudaStream_t cs, const char* name) {
   if (!ctx->profile) return;
   if (ctx->prof_used == ctx->prof_ev.size()) {
     cudaEvent_t e;
@@ -110,7 +109,7 @@ void plf_mark(plf_ctx* ctx, const char* name) {
     ctx->prof_names.emplace_back();
   }
   ctx->prof_names[ctx->prof_used] = name;
-  cudaEventRecord(ctx->prof_ev[ctx->prof_used], ctx->cur);
+  cudaEventRecord(ctx->prof_ev[ctx->prof_used], cs);
   ctx->prof_used++;
 }
 
@@ -261,18 +260,8 @@ plf_status plf_create(const plf_params* params, const plf_camera* cam, const plf
     delete ctx;
     return plf_fail(nullptr, PLF_ERR_NO_DEVICE, "cudaStreamCreate: %s", cudaGetErrorString(e));
   }
-  ctx->cur = ctx->stream;
   bool ok = true;
-  // aux[1] carries the LSD chain of the batched pipeline, the longest dependent chain of a step.  PLF_G_PRIORITY=1 gives it the
-  // highest stream priority (its CTAs are dispatched ahead of the pending CTAs of the ORB / match streams).  Measured: no gain -
-  // the chain is slowed by sharing issue slots with the co-resident kernels, not by waiting for CTA slots (DESIGN.md 5) - so
-  // equal priorities stay the default.
-  int prio_lo = 0, prio_hi = 0;
-  cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-  const char* gp = getenv("PLF_G_PRIORITY");
-  const bool g_high = gp && gp[0] == '1';
-  for (int i = 0; i < 3 && ok; ++i)
-    ok = cudaStreamCreateWithPriority(&ctx->aux[i], cudaStreamNonBlocking, (i == 1 && g_high) ? prio_hi : prio_lo) == cudaSuccess;
+  for (int i = 0; i < 3 && ok; ++i) ok = cudaStreamCreateWithFlags(&ctx->aux[i], cudaStreamNonBlocking) == cudaSuccess;
   if (!ok) {
     plf_destroy(ctx);
     return plf_fail(nullptr, PLF_ERR_NO_DEVICE, "plf_create: could not create auxiliary streams/events");

@@ -72,7 +72,6 @@ struct PlfTmaCache;   // plf_tma.cuh
 struct plf_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;  // main stream: copies, the serial part of the pipeline, standalone operators
-  cudaStream_t cur = nullptr;     // stream the launch helpers enqueue on (== stream except inside forked sections)
   cudaStream_t aux[3] = {nullptr, nullptr, nullptr};  // streams of the extraction (E), LSD growing (G) and LSD pre-grow (P) phases of plf_batch_run
   plf_params params;
   plf_camera cam;
@@ -88,7 +87,6 @@ struct plf_ctx {
   struct OrbState* orb_standalone = nullptr;   // plf_orb's working state: one image, rebuilt when the image size changes
   struct LsdState* lsd_standalone = nullptr;   // plf_lsd's and plf_detect_lines': likewise
   struct LsdTables* lsd_tables = nullptr;      // the LSD lookup tables of the parameters, read by every LSD state
-  bool lbd_tables = false;                     // the LBD constant tables are uploaded
   struct PipeState* pipe = nullptr;            // the batched pipeline, with its own ORB and LSD states
   struct BowState* bow = nullptr;   // DBoW2 vocabularies and keyframe database (dbow.cu)
   // optional per-stage timing (plf_profile_enable): events recorded after each kernel of plf_batch_run
@@ -98,8 +96,8 @@ struct plf_ctx {
   std::vector<std::string> prof_names;
   size_t prof_used = 0;
 };
-// Records a timing mark on ctx->stream after the work named `name` (no-op unless profiling is enabled).
-void plf_mark(plf_ctx* ctx, const char* name);
+// Records a timing mark on cs, the stream of the work named `name`, after that work (no-op unless profiling is enabled).
+void plf_mark(plf_ctx* ctx, cudaStream_t cs, const char* name);
 
 plf_status plf_fail(plf_ctx* ctx, plf_status code, const char* fmt, ...);
 // Ensures scratch slot `slot` holds at least `bytes`; returns device pointer or nullptr (error set).
@@ -137,7 +135,7 @@ struct KnnProblem {
   const int* qlist;  // optional: the query rows to process (nq / *nq_ptr = its length); results stored at best[row]
 };
 // Launches the kNN kernel over `nprob` problems (device array), max_nq = upper bound of nq.
-plf_status plf_launch_knn2(plf_ctx* ctx, const KnnProblem* d_probs, int nprob, int max_nq);
+plf_status plf_launch_knn2(plf_ctx* ctx, cudaStream_t cs, const KnnProblem* d_probs, int nprob, int max_nq);
 
 struct NnrProblem {
   const uint32_t* best12;
@@ -152,11 +150,11 @@ struct NnrProblem {
   int32_t* matches12;  // [n1]
   int* count;          // device counter (accumulated with atomicAdd; caller zeroes)
 };
-plf_status plf_launch_nnr(plf_ctx* ctx, const NnrProblem* d_probs, int nprob, int max_n1);
+plf_status plf_launch_nnr(plf_ctx* ctx, cudaStream_t cs, const NnrProblem* d_probs, int nprob, int max_n1);
 // Marks, per problem, the train rows that are the NNR-accepted best match of some query: the only rows whose reverse
 // 2-NN the mutual-consistency check will read.  flags/qlist: [nprob][stride] (flags zeroed by the caller), qcount: [nprob].
-plf_status plf_launch_nnr_mark(plf_ctx* ctx, const NnrProblem* d_probs, int nprob, int max_n1, int* flags, int* qlist,
-                               int* qcount, int stride);
+plf_status plf_launch_nnr_mark(plf_ctx* ctx, cudaStream_t cs, const NnrProblem* d_probs, int nprob, int max_n1, int* flags,
+                               int* qlist, int* qcount, int stride);
 
 // ---- windowed greedy matcher, batched device-resident form (matchgrid.cu) ------------------------------------
 struct MgGrid { int cols, rows, w_lo, w_hi, h_lo, h_hi; };
@@ -181,14 +179,16 @@ struct MgbArgs {
   int32_t* m12; size_t m12_stride;       // output rows of problem p: m12 + p * m12_stride
   int* count; int count_stride;          // matches of problem p (accumulated; zeroed by the caller)
 };
-// max_n1 / max_n2: upper bounds of the query / train counts; slot: the scratch slot D, the query masks and m21 live in.
-plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n1, int max_n2, plf_scratch_slot slot);
+// max_n1 / max_n2: upper bounds of the query / train counts; slot: the scratch slot D, the query masks and m21 live in;
+// cs: the stream the launches are enqueued on.
+plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int max_n1, int max_n2, plf_scratch_slot slot,
+                                       cudaStream_t cs);
 
 // ---- LBD (lbd.cu) ------------------------------------------------------------------------------
 // tm: the caller's tensor-map cache over its source images (plf_tma.cuh)
-plf_status plf_launch_blur5_sobel(plf_ctx* ctx, PlfTmaCache* tm, const uint8_t* imgs, int pitch, size_t img_stride,
-                                  int w, int h, int nimg, short2* grad, size_t grad_stride);
-plf_status plf_launch_lbd(plf_ctx* ctx, const short2* grad, size_t grad_stride, int w, int h, int nimg,
+plf_status plf_launch_blur5_sobel(plf_ctx* ctx, cudaStream_t cs, PlfTmaCache* tm, const uint8_t* imgs, int pitch,
+                                  size_t img_stride, int w, int h, int nimg, short2* grad, size_t grad_stride);
+plf_status plf_launch_lbd(plf_ctx* ctx, cudaStream_t cs, const short2* grad, size_t grad_stride, int w, int h, int nimg,
                           const plf_keyline* kls, const int* counts, int max_lines, uint8_t* desc,
                           float* desc_f);
 
@@ -209,18 +209,18 @@ struct GnProblem {
   plf_pose_result* out;
 };
 plf_gn_opts plf_gn_opts_from_params(const plf_params& p);
-plf_status plf_launch_gn(plf_ctx* ctx, const GnProblem* d_probs, int nprob, const plf_gn_opts& o);
+plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs, int nprob, const plf_gn_opts& o);
 
 // ---- ORB (orb.cu) --------------------------------------------------------------------------------
 // A working state for up to nimg images of w x h, with outputs once or per batch parity (two_parities).  On failure
 // nothing is left allocated and *out is untouched.
 plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, OrbState** out);
 void plf_orb_free(OrbState* s);
-plf_status plf_orb_run(plf_ctx* ctx, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par);
+plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par);
 void plf_orb_outputs(const OrbState* s, int par, plf_keypoint** kps, uint8_t** desc, int** counts, int* max_kp);
 int* plf_orb_overflow_flag(const OrbState* s);
 void plf_linear_coeffs_host(int srcsize, int dstsize, double scale, int* ofs, int* c1);
-plf_status plf_launch_resize_exact(plf_ctx* ctx, const uint8_t* src, size_t src_stride, int sp, int sw, int sh, uint8_t* dst,
+plf_status plf_launch_resize_exact(plf_ctx* ctx, cudaStream_t cs, const uint8_t* src, size_t src_stride, int sp, int sw, int sh, uint8_t* dst,
                                    size_t dst_stride, int dp, int dw, int dh, const int* tabx, const int* tabxp, const int* taby, int nimg);
 size_t plf_resize_packed_len(int dw);                                 // ints of the packed x table of k_resize_exact4
 void plf_resize_pack_x(const int* ofs, const int* c1, int dw, int* out);   // out: 16-byte aligned
@@ -234,9 +234,9 @@ void plf_lsd_tables_free(plf_ctx* ctx);
 plf_status plf_lsd_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, LsdState** out);
 void plf_lsd_free(LsdState* s);
 size_t plf_lsd_footprint(const plf_ctx* ctx, int w, int h, int nimg, bool two_parities);   // bytes plf_lsd_create allocates
-plf_status plf_lsd_pre(plf_ctx* ctx, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int par, int n);
+plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int par, int n);
 // keylines_wait: if set, the KeyLine outputs are overwritten only after this event
-plf_status plf_lsd_grow(plf_ctx* ctx, LsdState* s, int par, int n, cudaEvent_t keylines_wait);
+plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int n, cudaEvent_t keylines_wait);
 void plf_lsd_outputs(const LsdState* s, int par, plf_keyline** kls, int** nlines, int* max_lines);
 int* plf_lsd_overflow_flag(const LsdState* s);
 

@@ -61,6 +61,26 @@ def test_lsd_param_cases(built, case, img):
         assert len(kl) == len(okl) and kl.tobytes() == okl.tobytes() and np.array_equal(desc, odesc)
 
 
+def test_lsd_contexts_with_different_blurs_coexist(built):
+    """Two contexts alive at once whose Gaussian pre-blurs differ (9 and 11 taps, both on the generic blur kernel): each
+    one's segments and KeyLines stay those of its own parameters, whichever context ran last."""
+    w, h, L = image("odd_641x359")
+    pa, pb = dict(ofe.DEFAULTS, **pc.LSD_CASES["sigma0.9_k9"]), dict(ofe.DEFAULTS, **pc.LSD_CASES["scale0.5_k11"])
+    assert (pc.lsd_ksize(pa), pc.lsd_ksize(pb)) == (9, 11)
+    ref_a, ref_b = clib.lsd(L, **ofe.lsd_kwargs(pa)), clib.lsd(L, **ofe.lsd_kwargs(pb))
+    lim = plf.default_limits(); lim.max_segments = 32768
+    with plf.Frontend(camera=cam(w, h), limits=lim, **pc.LSD_CASES["sigma0.9_k9"]) as fa, \
+            plf.Frontend(camera=cam(w, h), limits=lim, **pc.LSD_CASES["scale0.5_k11"]) as fb:
+        a1 = fa.lsd(L, cap=32768)
+        b1 = fb.lsd(L, cap=32768)
+        a2 = fa.lsd(L, cap=32768)
+        kl, desc = fa.detect_lines(L)
+    for got, ref in ((a1, ref_a), (b1, ref_b), (a2, ref_a)):
+        assert len(ref) > 50 and got.shape == ref.shape and np.array_equal(got, ref)
+    okl, odesc = ofe.detect_lines(L, pa["lsd_nfeatures"], pa["min_line_length"], ofe.lsd_kwargs(pa))
+    assert len(kl) == len(okl) and kl.tobytes() == okl.tobytes() and np.array_equal(desc, odesc)
+
+
 def test_ignored_lsd_parameters_leave_segments_unchanged(built):
     w, h, L = image("odd_641x359")
     with plf.Frontend(camera=cam(w, h)) as fe:
