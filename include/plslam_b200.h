@@ -360,6 +360,56 @@ plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_pr
  * plf_local_ba; beyond, by a tiled LDL^T across the GPU that skips exactly-zero tiles. */
 plf_status plf_global_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* problem, plf_lba_result* out);
 
+/* Loop-closure pose-graph optimisation.  Replaces the g2o call of MapHandler::loopClosureOptimizationCovGraphG2O
+ * (src/mapHandler.cpp:4185-4410): computeInitialGuess() then optimize(max_iters) of g2o's Levenberg-Marquardt over
+ * VertexSE3 / EdgeSE3 with identity information and g2o's 10 trials per iteration.  The caller builds the graph as
+ * :4198-4290 do and writes the poses back as :4298-4398 do (INTEGRATION.md §4 f7):
+ *   T     [n_v][16]  row-major isometries (T_kf_w of the live keyframes 0 .. kf_curr_idx, in id order), in / out
+ *   fixed [n_v]      1 for a vertex held fixed (keyframe 0)
+ *   from / to / Z [n_e]  edge k measures Z[k] (row-major) between vertex from[k] (g2o's vertex 0) and to[k]: the error
+ *                    is the MQT vector (t; q_x, q_y, q_z), w >= 0, of Z^-1 T_from^-1 T_to.  Edges in creation order:
+ *                    the kf2kf edges (i asc, j asc), then the loop edges, measuring expmap_se3(lc_pose).
+ * Initial guess: a breadth-first search from the fixed vertices (ascending id), visiting each vertex's edges in the
+ * order given, sets every reached free vertex to parent * Z (parent = from) or parent * Z^-1.  A vertex without edges is
+ * never touched; an edge between two fixed vertices adds to chi2 only.  Each trial solves (H + lambda I) x = b with the
+ * tiled LDL^T of plf_global_ba; H and b are summed in a fixed order, so two calls give bit-identical results.
+ * opts: max_iters = SlamConfig::maxItersPGO (100; 0 returns the initial guess), lambda_init = setUserLambdaInit (1e-10).
+ * out: iterations run, the stop reason (PLF_PGO_STOP_*), trials over the call, chi2 after the initial guess, final
+ *   chi2 and lambda; trace (may be NULL) receives the first trace_cap trials, n_trace of them (g2o's verbose output).
+ * Limits: at most 4096 free vertices with edges (PLF_ERR_CAPACITY, before any allocation).  PLF_ERR_INVALID for NULL
+ * arrays, out-of-range or self edges, non-finite T or Z, a lambda_init that is not positive and finite (g2o would derive
+ * one from H instead), and a connected component with edges but no fixed vertex.  The context stays usable after any
+ * error.  Work is enqueued on plf_stream and uses scratch slot 10 (shared with the bundle adjustments): 288 n_free^2
+ * bytes for the dense system (4.8 GB at 4096 free vertices) plus about 790 bytes per edge, 260 per vertex and 200 per
+ * free vertex; out->scratch_bytes reports what the call carved. */
+enum { PLF_PGO_STOP_MAX_ITERS = 0, PLF_PGO_STOP_TRIALS = 1, PLF_PGO_STOP_RHO_ZERO = 2, PLF_PGO_STOP_LAMBDA = 3 };
+typedef struct plf_pgo_opts {
+  int max_iters;
+  double lambda_init;
+} plf_pgo_opts;
+typedef struct plf_pgo_problem {
+  int n_v, n_e;
+  double* T;
+  const uint8_t* fixed;
+  const int* from;
+  const int* to;
+  const double* Z;
+} plf_pgo_problem;
+typedef struct plf_pgo_trial {
+  int iter, accepted;
+  double lambda;   /* the damping the trial solved with */
+  double chi, chi_t, rho;
+} plf_pgo_trial;
+typedef struct plf_pgo_result {
+  int iters, stop, trials;
+  double chi2_init, chi2, lambda;
+  plf_pgo_trial* trace;  /* in: caller's array (may be NULL) */
+  int trace_cap;         /* in */
+  int n_trace;           /* out: min(trials, trace_cap) */
+  size_t scratch_bytes;  /* out: device scratch the call carved */
+} plf_pgo_result;
+plf_status plf_pose_graph(plf_ctx* ctx, const plf_pgo_opts* opts, const plf_pgo_problem* problem, plf_pgo_result* out);
+
 /* Relative pose between two keyframes (SURVEY 8(f) f2).  Replaces MapHandler::isLoopClosure (src/mapHandler.cpp:3192-3300:
  * match() on the points :3223 and on the lines :3249 of kf0 / kf1, the inlier-ratio pre-condition :3277-3299) followed by
  * MapHandler::computeRelativePoseRobustGN (:3566-3957: two-stage robust GN from identity with the chi2 gate in between,

@@ -2,8 +2,11 @@
 // Usage: vo_demo <frames.bin> [orb_nfeatures lsd_nfeatures] [--grid-selftest | --kf-match-selftest |
 //                                                            --bow-selftest <voc_p.yml> <voc_l.yml>]
 //        vo_demo --gba-selftest <problem.bin>
+//        vo_demo --pgo-selftest <map.bin>
 // frames.bin: int32 n, w, h; double fx, fy, cx, cy, b; then n x (left h*w bytes, right h*w bytes).
 // Prints one line per frame: idx status n_stereo_pt n_stereo_ls n_inliers newKF Tfw(16 values, row-major).
+#include <algorithm>
+#include <array>
 #include <cfloat>
 #include <cstdio>
 #include <cstdlib>
@@ -263,18 +266,23 @@ static void bow_selftest_frame(BowMap& m, StVO::StereoFrame* cur, int frame_coun
 // ---- INTEGRATION.md §4 f6: global bundle adjustment (the text between the two markers is the snippet shown there) ----
 // What MapHandler's GBA reads and writes: the map_keyframes / map_points / map_lines lists (NULL where deleted),
 // MapPoint::idx / point3D / obs_list / kf_obs_list and MapLine::idx / line3D / obs_list / kf_obs_list
-// (include/mapFeatures.h), and the SlamConfig values levMarquardtOptimizationGBA reuses.
+// (include/mapFeatures.h), and the SlamConfig values levMarquardtOptimizationGBA reuses.  The pose graph (f7 below) also
+// moves med_obs_dir and dir_list.
 struct MapPoint {
   int idx;
   StVO::Vector3d point3D;
   std::vector<StVO::Vector2d> obs_list;
   std::vector<int> kf_obs_list;
+  StVO::Vector3d med_obs_dir;
+  std::vector<StVO::Vector3d> dir_list;
 };
 struct MapLine {
   int idx;
   StVO::Vector6d line3D;
   std::vector<StVO::Vector3d> obs_list;
   std::vector<int> kf_obs_list;
+  StVO::Vector3d med_obs_dir;
+  std::vector<StVO::Vector3d> dir_list;
 };
 struct GbaMap {
   plf_ctx* ctx;
@@ -453,9 +461,229 @@ static int gba_selftest(const char* path) {
   return rc;
 }
 
+// ---- INTEGRATION.md §4 f7: loop-closure pose graph (the text between the two markers is the snippet shown there) ----
+// What loopClosureOptimizationCovGraphG2O reads and writes (include/mapHandler.h): map_keyframes (T_kf_w, x_kf_w),
+// full_graph, lc_idx_list (Vector3i: the two keyframes and the "not yet optimised" flag), lc_pose_list, map_points /
+// map_lines with the landmarks anchored at each keyframe (map_points_kf_idx / map_lines_kf_idx), and
+// SlamConfig::minLMEssGraph / minLMCovGraph / maxItersPGO.
+struct PgoMap {
+  plf_ctx* ctx;
+  int min_lm_ess_graph, min_lm_cov_graph, max_iters_pgo;
+  std::vector<KeyFrame*> map_keyframes;
+  std::vector<std::vector<unsigned int>> full_graph;
+  std::vector<std::array<int, 3>> lc_idx_list;
+  std::vector<StVO::Vector6d> lc_pose_list;
+  std::vector<MapPoint*> map_points;
+  std::vector<MapLine*> map_lines;
+  std::vector<std::vector<int>> map_points_kf_idx, map_lines_kf_idx;
+};
+// BEGIN f7
+// Tkfw_corr.block(0,0,3,3) * v + Tkfw_corr.block(0,3,3,1): directions are moved like points, as the reference writes it
+static StVO::Vector3d pgo_xf(const StVO::Matrix4d& C, const StVO::Vector3d& v) {
+  StVO::Vector3d o;
+  for (int r = 0; r < 3; ++r) o(r) = C(r, 0) * v(0) + C(r, 1) * v(1) + C(r, 2) * v(2) + C(r, 3);
+  return o;
+}
+// MapHandler::loopClosureOptimizationCovGraphG2O (:4185-4410): the graph (:4198-4290), plf_pose_graph in place of g2o's
+// computeInitialGuess + optimize (:4290-4294), the write-back (:4298-4398).  loopClosureFuseLandmarks() follows.
+static plf_pgo_result loop_closure_optimization_cov_graph(PgoMap& m) {
+  int kf_curr_idx = -1;                                     // :4198-4208; kf_prev_idx is forced to 0
+  for (const auto& lc : m.lc_idx_list) kf_curr_idx = std::max(kf_curr_idx, lc[1]);
+  const int kf_prev_idx = 0;
+  std::vector<int> kf_list, pos(kf_curr_idx + 1, -1);      // vertex of each keyframe (the problem's vertices in id order)
+  std::vector<double> T, Z;                                 // row-major copies: never .data() of an Eigen::Matrix4d
+  std::vector<uint8_t> fixed;
+  std::vector<int> from, to;
+  auto push_rm = [](std::vector<double>& dst, const StVO::Matrix4d& M) {
+    double t[16];
+    row_major(M, t);
+    dst.insert(dst.end(), t, t + 16);
+  };
+  for (int i = kf_prev_idx; i <= kf_curr_idx; i++)          // :4211-4247
+    if (m.map_keyframes[i] != NULL) {
+      pos[i] = (int)kf_list.size();
+      kf_list.push_back(i);
+      push_rm(T, m.map_keyframes[i]->T_kf_w);
+      fixed.push_back(i == 0);
+    }
+  for (int i = kf_prev_idx; i <= kf_curr_idx; i++)          // :4250-4273, in (i asc, j asc) order
+    for (int j = i + 1; j <= kf_curr_idx; j++)
+      if (m.map_keyframes[i] != NULL && m.map_keyframes[j] != NULL &&
+          (m.full_graph[i][j] >= (unsigned)m.min_lm_ess_graph || m.full_graph[i][j] >= (unsigned)m.min_lm_cov_graph ||
+           std::abs(i - j) == 1)) {
+        from.push_back(pos[i]); to.push_back(pos[j]);
+        push_rm(Z, StVO::inverse_se3(m.map_keyframes[i]->T_kf_w) * m.map_keyframes[j]->T_kf_w);
+      }
+  for (size_t k = 0; k < m.lc_idx_list.size(); k++) {      // :4276-4288
+    from.push_back(pos[m.lc_idx_list[k][0]]); to.push_back(pos[m.lc_idx_list[k][1]]);
+    push_rm(Z, StVO::expmap_se3(m.lc_pose_list[k]));
+  }
+  plf_pgo_problem p = {};
+  p.n_v = (int)kf_list.size(); p.n_e = (int)from.size();
+  p.T = T.data(); p.fixed = fixed.data(); p.from = from.data(); p.to = to.data(); p.Z = Z.data();
+  plf_pgo_opts o = {m.max_iters_pgo, 1e-10};               // setUserLambdaInit(1e-10), optimize(maxItersPGO)
+  plf_pgo_result res = {};
+  plf_check(m.ctx, plf_pose_graph(m.ctx, &o, &p, &res), "plf_pose_graph");
+  auto move_landmarks = [&](int kf, const StVO::Matrix4d& C) {
+    for (int i : m.map_points_kf_idx.at(kf)) {
+      MapPoint* pt = m.map_points[i];
+      if (pt == NULL) continue;
+      pt->point3D = pgo_xf(C, pt->point3D);
+      pt->med_obs_dir = pgo_xf(C, pt->med_obs_dir);
+      for (auto& d : pt->dir_list) d = pgo_xf(C, d);
+    }
+    for (int i : m.map_lines_kf_idx.at(kf)) {
+      MapLine* ls = m.map_lines[i];
+      if (ls == NULL) continue;
+      StVO::Vector3d sP(ls->line3D(0), ls->line3D(1), ls->line3D(2)), eP(ls->line3D(3), ls->line3D(4), ls->line3D(5));
+      sP = pgo_xf(C, sP);
+      eP = pgo_xf(C, eP);
+      for (int c = 0; c < 3; ++c) { ls->line3D(c) = sP(c); ls->line3D(3 + c) = eP(c); }
+      ls->med_obs_dir = pgo_xf(C, ls->med_obs_dir);
+      for (auto& d : ls->dir_list) d = pgo_xf(C, d);
+    }
+  };
+  StVO::Matrix4d Tkfw_corr;                                 // :4298-4348
+  for (size_t n = 0; n < kf_list.size(); n++) {
+    KeyFrame* kf = m.map_keyframes[kf_list[n]];
+    StVO::Matrix4d Tkfw;
+    for (int r = 0; r < 4; ++r)
+      for (int c = 0; c < 4; ++c) Tkfw(r, c) = p.T[16 * n + 4 * r + c];
+    const StVO::Matrix4d Tkfw_prev = kf->T_kf_w;
+    kf->T_kf_w = Tkfw;
+    kf->x_kf_w = StVO::logmap_se3(Tkfw);
+    Tkfw_corr = Tkfw * StVO::inverse_se3(Tkfw_prev);
+    move_landmarks(kf_list[n], Tkfw_corr);
+  }
+  for (size_t i = kf_curr_idx + 1; i < m.map_keyframes.size(); i++) {   // :4351-4393, no NULL check (:4357)
+    m.map_keyframes[i]->T_kf_w = Tkfw_corr * m.map_keyframes[i]->T_kf_w;
+    m.map_keyframes[i]->x_kf_w = StVO::logmap_se3(m.map_keyframes[i]->T_kf_w);
+    move_landmarks((int)i, Tkfw_corr);
+  }
+  for (auto& lc : m.lc_idx_list) lc[2] = 0;                 // :4396-4397
+  return res;
+}
+// END f7
+
+// `vo_demo --pgo-selftest map.bin`: reads a map (little-endian: int32 minLMEssGraph, minLMCovGraph, maxItersPGO, n_kf;
+// n_kf keyframe slots, each an int32 `present` flag followed by T_kf_w[16] row-major; full_graph as n_kf x n_kf int32;
+// int32 n_lc, n_lc x (int32 kf0, kf1, f64 lc_pose[6]); int32 n_pt and the point slots: int32 present, point3D[3],
+// med_obs_dir[3], int32 n_dir, n_dir x f64[3]; the same for lines with line3D[6]; then per keyframe the anchored points
+// (int32 n, n x int32) and per keyframe the anchored lines), runs the f7 function above on it and prints the result,
+// every keyframe's T_kf_w and every landmark, which oracle/pgo.py's lists + the Python binding + its write-back must give.
+static int pgo_selftest(const char* path) {
+  FILE* f = std::fopen(path, "rb");
+  if (!f) { std::perror("open"); return 1; }
+  bool ok = true;
+  auto i32 = [&]() { int32_t v = 0; ok = ok && std::fread(&v, 4, 1, f) == 1; return (int)v; };
+  auto f64 = [&]() { double v = 0; ok = ok && std::fread(&v, 8, 1, f) == 1; return v; };
+  auto v3 = [&]() { StVO::Vector3d v; for (int c = 0; c < 3; ++c) v(c) = f64(); return v; };
+  PgoMap m = {};
+  m.min_lm_ess_graph = i32(); m.min_lm_cov_graph = i32(); m.max_iters_pgo = i32();
+  const int n_kf = i32();
+  for (int i = 0; ok && i < n_kf; ++i) {
+    KeyFrame* kf = nullptr;
+    if (i32()) {
+      kf = new KeyFrame{i, nullptr, {}, {}};
+      for (int c = 0; c < 16; ++c) kf->T_kf_w.v[c] = f64();
+      kf->x_kf_w = StVO::logmap_se3(kf->T_kf_w);
+    }
+    m.map_keyframes.push_back(kf);
+  }
+  m.full_graph.assign(std::max(n_kf, 0), std::vector<unsigned int>(std::max(n_kf, 0), 0));
+  for (int i = 0; ok && i < n_kf; ++i)
+    for (int j = 0; ok && j < n_kf; ++j) m.full_graph[i][j] = (unsigned)i32();
+  for (int k = 0, n = i32(); ok && k < n; ++k) {
+    const int a = i32(), b = i32();
+    m.lc_idx_list.push_back({a, b, 1});
+    StVO::Vector6d x;
+    for (int c = 0; c < 6; ++c) x(c) = f64();
+    m.lc_pose_list.push_back(x);
+  }
+  for (int i = 0, n = i32(); ok && i < n; ++i) {
+    MapPoint* pt = nullptr;
+    if (i32()) {
+      pt = new MapPoint{i, {}, {}, {}, {}, {}};
+      pt->point3D = v3();
+      pt->med_obs_dir = v3();
+      for (int k = 0, nd = i32(); ok && k < nd; ++k) pt->dir_list.push_back(v3());
+    }
+    m.map_points.push_back(pt);
+  }
+  for (int i = 0, n = i32(); ok && i < n; ++i) {
+    MapLine* ls = nullptr;
+    if (i32()) {
+      ls = new MapLine{i, {}, {}, {}, {}, {}};
+      for (int c = 0; c < 6; ++c) ls->line3D(c) = f64();
+      ls->med_obs_dir = v3();
+      for (int k = 0, nd = i32(); ok && k < nd; ++k) ls->dir_list.push_back(v3());
+    }
+    m.map_lines.push_back(ls);
+  }
+  for (auto* lists : {&m.map_points_kf_idx, &m.map_lines_kf_idx})
+    for (int i = 0; ok && i < n_kf; ++i) {
+      std::vector<int> l;
+      for (int k = 0, n = i32(); ok && k < n; ++k) l.push_back(i32());
+      lists->push_back(l);
+    }
+  std::fclose(f);
+  int rc = 0;
+  if (!ok) { std::fprintf(stderr, "short read\n"); rc = 1; }
+  plf_params prm;
+  plf_default_params(&prm);
+  plf_limits lim;
+  plf_default_limits(&lim);
+  lim.max_batch = 1;
+  plf_camera cam = {1242, 375, 718.856, 718.856, 607.1928, 185.2157, 0.537165719};
+  if (!rc && plf_create(&prm, &cam, &lim, 0, &m.ctx) != PLF_OK) {
+    std::fprintf(stderr, "plf_create: %s\n", plf_last_error(nullptr));
+    rc = 2;
+  }
+  auto print3 = [](const StVO::Vector3d& v) { for (int c = 0; c < 3; ++c) std::printf(" %.17g", v(c)); };
+  if (!rc) {
+    try {
+      const plf_pgo_result res = loop_closure_optimization_cov_graph(m);
+      std::printf("pgo result %d %d %d %.17g %.17g %.17g\n", res.iters, res.stop, res.trials, res.chi2_init, res.chi2,
+                  res.lambda);
+      for (KeyFrame* kf : m.map_keyframes) {
+        if (!kf) continue;
+        std::printf("pgo kf %d", kf->kf_idx);
+        for (int c = 0; c < 16; ++c) std::printf(" %.17g", kf->T_kf_w.v[c]);
+        std::printf("\n");
+      }
+      for (MapPoint* pt : m.map_points) {
+        if (!pt) continue;
+        std::printf("pgo pt %d", pt->idx);
+        print3(pt->point3D);
+        print3(pt->med_obs_dir);
+        for (const auto& d : pt->dir_list) print3(d);
+        std::printf("\n");
+      }
+      for (MapLine* ls : m.map_lines) {
+        if (!ls) continue;
+        std::printf("pgo ls %d", ls->idx);
+        for (int c = 0; c < 6; ++c) std::printf(" %.17g", ls->line3D(c));
+        print3(ls->med_obs_dir);
+        for (const auto& d : ls->dir_list) print3(d);
+        std::printf("\n");
+      }
+      for (const auto& lc : m.lc_idx_list) std::printf("pgo lc %d %d %d\n", lc[0], lc[1], lc[2]);
+    } catch (const std::exception& e) {
+      std::fprintf(stderr, "error: %s\n", e.what());
+      rc = 2;
+    }
+    plf_destroy(m.ctx);
+  }
+  for (KeyFrame* kf : m.map_keyframes) delete kf;
+  for (MapPoint* pt : m.map_points) delete pt;
+  for (MapLine* ls : m.map_lines) delete ls;
+  return rc;
+}
+
 int main(int argc, char** argv) {
   bool grid_test = false, kf_test = false;
   if (argc == 3 && std::string(argv[1]) == "--gba-selftest") return gba_selftest(argv[2]);
+  if (argc == 3 && std::string(argv[1]) == "--pgo-selftest") return pgo_selftest(argv[2]);
   const char* bow_voc[2] = {nullptr, nullptr};
   if (argc >= 4 && std::string(argv[argc - 3]) == "--bow-selftest") {
     bow_voc[0] = argv[argc - 2];

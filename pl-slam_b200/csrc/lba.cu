@@ -602,6 +602,39 @@ __global__ void __launch_bounds__(256) k_gba_bwd(LbaDev d, const uint8_t* nz, in
   if (tid < GBA_T && GBA_T * j + tid < n) d.gred[GBA_T * j + tid] -= ((part[0][tid] + part[1][tid]) + part[2][tid]) + part[3][tid];
 }
 
+// The tiled factorisation and the two substitutions (see k_gba_diag), shared by plf_global_ba and plf_pose_graph.  The
+// kernels read only the fields of LbaDev set here.
+plf_status plf_ldlt_tiled(plf_ctx* ctx, cudaStream_t cs, int n6, double* S, double* g, double* y, double* x, double* Wp,
+                          uint8_t* nz) {
+  static_assert(GBA_T == PLF_LDLT_TILE, "plf_internal.h states the tile size");
+  LbaDev d{};
+  d.nkf = n6; d.S = S; d.gred = g; d.dxc = y; d.DX = x;
+  const int n = 6 * n6, nt = (n + GBA_T - 1) / GBA_T;
+  const int smem = 2 * GBA_T * GBA_LD * 8;
+  PLF_CUDA(ctx, cudaFuncSetAttribute(k_gba_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  for (int k = 0; k < nt; ++k) {
+    k_gba_diag<<<1, 256, 0, cs>>>(d, k);
+    PLF_LAUNCH_CHECK(ctx);
+    const int m = nt - k - 1;
+    if (!m) break;
+    k_gba_panel<<<m, 256, smem, cs>>>(d, Wp, nz, k, nt);
+    PLF_LAUNCH_CHECK(ctx);
+    k_gba_update<<<m * (m + 1) / 2, 256, 0, cs>>>(d, Wp, nz, k, nt);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  for (int k = 0; k < nt; ++k) {
+    k_gba_fwd<<<nt - k, 256, 0, cs>>>(d, nz, k, nt);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  k_gba_dscale<<<(n + 255) / 256, 256, 0, cs>>>(d);
+  PLF_LAUNCH_CHECK(ctx);
+  for (int k = nt - 1; k >= 0; --k) {
+    k_gba_bwd<<<k + 1, 256, 0, cs>>>(d, nz, k, nt);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  return PLF_OK;
+}
+
 // The host loop of both routines: the reference's control flow, on the device kernels above.  `global` selects
 // levMarquardtOptimizationGBA (:2101-2699) over levMarquardtOptimizationLBA (:1332-1989): its quirk set, its error
 // normalisation in the LM iterations, up to 4096 keyframes (the blocked factorisation beyond n = 384) and a landmark
@@ -706,29 +739,7 @@ static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_p
   auto solve_blocked = [&]() -> plf_status {
     k_gba_damp<<<(36 * nkf + n + 255) / 256, 256, 0, cs>>>(d, lambda);
     PLF_LAUNCH_CHECK(ctx);
-    const int smem = 2 * GBA_T * GBA_LD * 8;
-    PLF_CUDA(ctx, cudaFuncSetAttribute(k_gba_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    for (int k = 0; k < nt; ++k) {
-      k_gba_diag<<<1, 256, 0, cs>>>(d, k);
-      PLF_LAUNCH_CHECK(ctx);
-      const int m = nt - k - 1;
-      if (!m) break;
-      k_gba_panel<<<m, 256, smem, cs>>>(d, dWp, dNz, k, nt);
-      PLF_LAUNCH_CHECK(ctx);
-      k_gba_update<<<m * (m + 1) / 2, 256, 0, cs>>>(d, dWp, dNz, k, nt);
-      PLF_LAUNCH_CHECK(ctx);
-    }
-    for (int k = 0; k < nt; ++k) {
-      k_gba_fwd<<<nt - k, 256, 0, cs>>>(d, dNz, k, nt);
-      PLF_LAUNCH_CHECK(ctx);
-    }
-    k_gba_dscale<<<(n + 255) / 256, 256, 0, cs>>>(d);
-    PLF_LAUNCH_CHECK(ctx);
-    for (int k = nt - 1; k >= 0; --k) {
-      k_gba_bwd<<<k + 1, 256, 0, cs>>>(d, dNz, k, nt);
-      PLF_LAUNCH_CHECK(ctx);
-    }
-    return PLF_OK;
+    return plf_ldlt_tiled(ctx, cs, nkf, d.S, d.gred, d.dxc, d.DX, dWp, dNz);
   };
   // solves the damped system and (optionally) applies the step; leaves |DX| in *dx_norm.  swap: (g6), first pass only
   auto solve = [&](int apply, int swap, double* dx_norm) -> plf_status {

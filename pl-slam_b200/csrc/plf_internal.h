@@ -29,7 +29,7 @@ enum plf_scratch_slot {
   PLF_SCR_ORB,         // plf_orb
   PLF_SCR_LSD,         // plf_lsd, plf_detect_lines, plf_debug_sincosf
   PLF_SCR_MGB_PIPE,    // the windowed matcher of plf_batch_run (matching_strategy != 0)
-  PLF_SCR_BA,          // plf_local_ba, plf_global_ba
+  PLF_SCR_BA,          // plf_local_ba, plf_global_ba, plf_pose_graph
   PLF_SCR_KF,          // plf_match_kf2kf, plf_match_map2kf: their staged layout
   PLF_SCR_KF_MGB_PT,   // plf_match_kf2kf, plf_match_map2kf: the windowed matcher of points
   PLF_SCR_KF_MGB_LS,   //   ... and of lines
@@ -210,6 +210,15 @@ struct GnProblem {
 };
 plf_gn_opts plf_gn_opts_from_params(const plf_params& p);
 plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs, int nprob, const plf_gn_opts& o);
+
+// ---- tiled LDL^T (lba.cu) ------------------------------------------------------------------------
+// Factors the symmetric n x n matrix S (n = 6 n6; row-major, leading dimension n; only its lower triangle is read) in
+// place as L D L^T without pivoting, over 64 x 64 tiles, skipping the tiles of L that are exactly zero, and solves
+// S x = g.  Afterwards S's diagonal holds D, y and x both hold the solution, and g has been overwritten.  Wp
+// (n_t x 64 x 64 doubles) and nz (n_t x n_t bytes) are work, n_t = ceil(n / 64).  Enqueued on cs.
+constexpr int PLF_LDLT_TILE = 64;
+plf_status plf_ldlt_tiled(plf_ctx* ctx, cudaStream_t cs, int n6, double* S, double* g, double* y, double* x, double* Wp,
+                          uint8_t* nz);
 
 // ---- ORB (orb.cu) --------------------------------------------------------------------------------
 // A working state for up to nimg images of w x h, with outputs once or per batch parity (two_parities).  On failure

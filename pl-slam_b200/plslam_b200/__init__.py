@@ -72,6 +72,32 @@ class plf_lba_result(C.Structure):
     _fields_ = [("iters", C.c_int), ("err", C.c_double), ("lambda_", C.c_double)]
 
 
+class plf_pgo_opts(C.Structure):
+    _fields_ = [("max_iters", C.c_int), ("lambda_init", C.c_double)]
+
+
+class plf_pgo_problem(C.Structure):
+    _fields_ = [("n_v", C.c_int), ("n_e", C.c_int), ("T", C.c_void_p), ("fixed", C.c_void_p), ("from_", C.c_void_p),
+                ("to", C.c_void_p), ("Z", C.c_void_p)]
+
+
+class plf_pgo_trial(C.Structure):
+    _fields_ = [("iter", C.c_int), ("accepted", C.c_int), ("lambda_", C.c_double), ("chi", C.c_double),
+                ("chi_t", C.c_double), ("rho", C.c_double)]
+
+
+class plf_pgo_result(C.Structure):
+    _fields_ = [("iters", C.c_int), ("stop", C.c_int), ("trials", C.c_int), ("chi2_init", C.c_double),
+                ("chi2", C.c_double), ("lambda_", C.c_double), ("trace", C.c_void_p), ("trace_cap", C.c_int),
+                ("n_trace", C.c_int), ("scratch_bytes", C.c_size_t)]
+
+
+PGO_STOP = {0: "max_iters", 1: "trials", 2: "rho_zero", 3: "lambda"}   # plf_pgo_result.stop
+PGO_TRACE_DTYPE = np.dtype([("iter", np.int32), ("accepted", np.int32), ("lambda_", np.float64), ("chi", np.float64),
+                            ("chi_t", np.float64), ("rho", np.float64)], align=True)
+assert PGO_TRACE_DTYPE.itemsize == C.sizeof(plf_pgo_trial)
+
+
 class plf_grid_window(C.Structure):
     _fields_ = [("width_lo", C.c_int), ("width_hi", C.c_int), ("height_lo", C.c_int), ("height_hi", C.c_int)]
 
@@ -512,6 +538,29 @@ class Frontend:
         self._check(getattr(self.lib, fn)(self._ctx, C.byref(o), C.byref(p), C.byref(res)), fn)
         return dict(kf_pose=kf, pt=pt, ls=ls, pt_moved=pm[:len(pt)].astype(bool), ls_moved=lm[:len(ls)].astype(bool),
                     iters=res.iters, err=res.err, lambda_=res.lambda_)
+
+    def pose_graph(self, prob, max_iters=100, lambda_init=1e-10, trace=True):
+        """The g2o optimisation of MapHandler::loopClosureOptimizationCovGraphG2O on the device (plf_pose_graph;
+        src/mapHandler.cpp:4185-4410).  prob: dict T [n_v, 4, 4], fixed [n_v], from / to [n_e], Z [n_e, 4, 4], as
+        synth.pose_graph_problem or oracle.pgo.cov_graph_lists give it.  Returns dict(T, iters, stop (PGO_STOP's names),
+        trials, chi2_init, chi2, lambda_, scratch_bytes, trace: a PGO_TRACE_DTYPE array with one row per trial when
+        `trace`)."""
+        T = np.ascontiguousarray(prob["T"], np.float64).reshape(-1, 16).copy()
+        fixed = np.ascontiguousarray(prob["fixed"], np.uint8).ravel()
+        frm = np.ascontiguousarray(prob["from"], np.int32).ravel()
+        to = np.ascontiguousarray(prob["to"], np.int32).ravel()
+        Z = np.ascontiguousarray(prob["Z"], np.float64).reshape(-1, 16)
+        ad = lambda a: a.ctypes.data if a.size else None
+        p = plf_pgo_problem(len(T), len(frm), ad(T), ad(fixed), ad(frm), ad(to), ad(Z))
+        o = plf_pgo_opts(int(max_iters), float(lambda_init))
+        tr = np.zeros(max(10 * int(max_iters), 1) if trace else 0, PGO_TRACE_DTYPE)
+        res = plf_pgo_result(trace=ad(tr), trace_cap=len(tr))
+        self._check(self.lib.plf_pose_graph(self._ctx, C.byref(o), C.byref(p), C.byref(res)), "plf_pose_graph")
+        out = dict(T=T.reshape(-1, 4, 4), iters=res.iters, stop=PGO_STOP[res.stop], trials=res.trials,
+                   chi2_init=res.chi2_init, chi2=res.chi2, lambda_=res.lambda_, scratch_bytes=res.scratch_bytes)
+        if trace:
+            out["trace"] = tr[:res.n_trace].copy()
+        return out
 
     def match_kf2kf(self, prev, curr, DT, fast_matching=True, max_kf_epip_p=1.0, max_kf_epip_l=1.0):
         """MapHandler::matchKF2KFPoints / matchKF2KFLines, matching part (plf_match_kf2kf).  prev / curr: get_frame dicts;

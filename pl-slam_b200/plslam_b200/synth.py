@@ -365,3 +365,69 @@ def gba_problem(cam, n_kf=64, pts_per_kf=100, ls_per_kf=15, loop=True, seed=0, n
                 pt_obs_lm=plm.astype(np.int32), pt_obs_kf=kf_of(pt_t), pt_obs_xy=puv + px_noise * rng.standard_normal(puv.shape),
                 ls_obs_lm=llm.astype(np.int32), ls_obs_kf=kf_of(ls_t), ls_obs_le=le,
                 truth=dict(kf_pose=kf_true, pt=pt, ls=ls))
+
+
+def _rodrigues(w):
+    """rotation matrices of the rotation vectors w [n, 3]"""
+    w = np.asarray(w, np.float64).reshape(-1, 3)
+    th = np.linalg.norm(w, axis=1)
+    k = w / np.where(th > 0, th, 1.0)[:, None]
+    K = np.zeros((len(w), 3, 3))
+    K[:, 0, 1], K[:, 0, 2], K[:, 1, 2] = -k[:, 2], k[:, 1], -k[:, 0]
+    K -= K.transpose(0, 2, 1)
+    s, c = np.sin(th)[:, None, None], np.cos(th)[:, None, None]
+    return np.eye(3) + s * K + (1.0 - c) * (K @ K)
+
+
+def _iso(R, t):
+    T = np.zeros((len(R), 4, 4))
+    T[:, :3, :3], T[:, :3, 3], T[:, 3, 3] = R, t, 1.0
+    return T
+
+
+def _iso_inv(T):
+    Rt = T[:, :3, :3].transpose(0, 2, 1)
+    return _iso(Rt, -np.einsum("nij,nj->ni", Rt, T[:, :3, 3]))
+
+
+def pose_graph_problem(n_kf=256, window=5, n_lc=2, drift=0.01, seed=0, step=0.5, lc_noise=1e-3):
+    """A loop-closure pose graph as MapHandler::loopClosureOptimizationCovGraphG2O builds it (plf_pose_graph's layout).
+    Ground truth: n_kf keyframes `step` apart on a closed loop (a circle with a vertical wave).  T (T_kf_w) integrates
+    the true relative motions perturbed by `drift` (radians and `drift * step` metres, normal, per step) from keyframe 0,
+    which is fixed.  kf2kf edges join every pair 1 <= j - i <= window in (i asc, j asc) order and measure T_i^-1 T_j of
+    the drifted poses, as the reference measures its current poses; then n_lc loop edges from a keyframe near the start
+    to one near the end measure the true relative pose perturbed by `lc_noise`.  Returns dict(T, T_true, fixed, from, to,
+    Z) with T [n_kf, 4, 4], fixed [n_kf] uint8, from / to [n_e] int32 and Z [n_e, 4, 4]."""
+    rng = np.random.default_rng(seed)
+    n = int(n_kf)
+    k = np.arange(n)
+    r = n * step / (2.0 * math.pi)
+    a = 2.0 * math.pi * k / n
+    yaw = a + math.pi / 2.0
+    p = np.stack([r * np.cos(a), r * np.sin(a), 0.5 * np.sin(3.0 * a)], 1)
+    Rt = _rodrigues(np.stack([0.02 * np.sin(5.0 * a), 0.02 * np.cos(7.0 * a), yaw], 1) * [[1.0, 1.0, 0.0]]) @ \
+        _rodrigues(np.stack([0 * a, 0 * a, yaw], 1))
+    T_true = _iso(Rt, p)
+    D = _iso_inv(T_true[:-1]) @ T_true[1:]                          # true relative motions
+    N = _iso(_rodrigues(drift * rng.standard_normal((n - 1, 3))), drift * step * rng.standard_normal((n - 1, 3)))
+    D = D @ N
+    T = np.empty_like(T_true)
+    T[0] = T_true[0]
+    for i in range(1, n):
+        T[i] = T[i - 1] @ D[i - 1]
+    ii, dd = np.meshgrid(k, np.arange(1, window + 1), indexing="ij")
+    jj = ii + dd
+    keep = jj < n
+    frm, to = ii[keep], jj[keep]
+    Z = _iso_inv(T[frm]) @ T[to]
+    if n_lc:
+        la = np.arange(n_lc) * max(1, window // 2 + 1)
+        lb = n - 1 - np.arange(n_lc) * max(1, window // 2 + 1)
+        ok = lb > la + window
+        la, lb = la[ok], lb[ok]
+        Zl = _iso_inv(T_true[la]) @ T_true[lb] @ _iso(_rodrigues(lc_noise * rng.standard_normal((len(la), 3))),
+                                                    lc_noise * rng.standard_normal((len(la), 3)))
+        frm, to, Z = np.concatenate([frm, la]), np.concatenate([to, lb]), np.concatenate([Z, Zl])
+    fixed = np.zeros(n, np.uint8)
+    fixed[0] = 1
+    return dict(T=T, T_true=T_true, fixed=fixed, **{"from": frm.astype(np.int32)}, to=to.astype(np.int32), Z=Z)
