@@ -21,9 +21,8 @@
 //                    (cv::fastAtan2, degrees, f32, from a table keyed by (gx,gy)), table index}, and one packed entry
 //                    (column, |grad|^2) of the raster-ordered seed list of the pixel's row segment; per-image max of |grad|^2.
 //                    Nothing dense leaves the kernel (the record map restores itself to "undefined", see k_lsd_fill_notdef)
-//   k_lsd_rowhist / k_lsd_binscan / k_lsd_scatter
-//                    stable counting sort of the seed lists by magnitude bin (descending), raster order inside a
-//                    bin == OpenCV's ordered_points
+//   k_lsd_seed_order stable counting sort of the seed lists by magnitude bin (descending), raster order inside a
+//                    bin == OpenCV's ordered_points; one CTA per image, bin counts in shared memory
 //   k_lsd_grow       region growing.  The algorithm is a sequential greedy partition (each accepted pixel updates the
 //                    region angle that the next test uses, and regions compete through the `used` map), so it is run by
 //                    ONE WARP PER IMAGE with thousands of images in flight: lanes 9e..9e+8 hold the 3x3 neighbourhood
@@ -88,13 +87,11 @@ struct LsdState {
   struct LsdPix* pix[2] = {nullptr, nullptr};  // [nimg][guard + hs*ws]  {angle (deg, f32) | NOTDEF = undefined/used, table index}
   size_t pix_stride = 0;      // entries per image = guard (ws+1, permanently NOTDEF) + hs*ws
   // seed lists per row segment (LSD_SEG columns): segment (y, xb) owns the entries [y * ws + LSD_SEG * xb, ...);
-  // an entry is column-in-segment | gx^2+gy^2 << LSD_COL_BITS (k_lsd_grad), then column | bin << LSD_COL_BITS (k_lsd_rowhist)
+  // an entry is column-in-segment | gx^2+gy^2 << LSD_COL_BITS (k_lsd_grad)
   uint32_t* seedlist = nullptr; // [nimg][hs*ws]
   int* segcnt = nullptr;        // [nimg][hs][nxb] entries per segment
   int nxb = 0;                  // segments per row
   int* maxmag2 = nullptr;     // [nimg]
-  uint32_t* rowcnt = nullptr; // [nimg][nchunks][n_bins]  per-chunk bin counts -> prefixes
-  uint32_t* binstart = nullptr; // [nimg][n_bins]
   // per batch parity: what crosses from the pre-grow chain to the growing (pix, order, nseeds) and what the match phase
   // reads (kls, nlines).  One copy: what only the growing / rectangle / KeyLine kernels of one batch write and read.
   int* nseeds[2] = {nullptr, nullptr};      // [nimg]
@@ -303,11 +300,10 @@ __global__ void k_lsd_fill_notdef(LsdPix* __restrict__ pix, size_t n) {
 #define LSD_SEG 512
 #define LSD_GRAD_THREADS (LSD_SEG / 4)
 // list entry: the low LSD_COL_BITS hold the column inside the segment, the high bits gx^2 + gy^2 (<= 2 * 510^2 over the
-// table's gradient range) and, after k_lsd_rowhist, the bin (< LSD_BINS_MAX)
+// table's gradient range)
 #define LSD_COL_BITS 9
 static_assert(LSD_SEG <= (1 << LSD_COL_BITS), "seed list: a segment column must fit the column field");
 static_assert(2u * 510u * 510u < (1u << (32 - LSD_COL_BITS)), "seed list: gx^2 + gy^2 must fit above the column field");
-static_assert(LSD_BINS_MAX <= (1 << (32 - LSD_COL_BITS)), "seed list: the bin must fit above the column field");
 // A thread produces FOUR adjacent columns of two rows from three aligned 32-bit words of the (16-byte pitched) image - the
 // fifth column of each row comes from the neighbour lane's word (lane 31 loads it) - so a warp issues 3 (+3) load instructions
 // for 256 pixels instead of 6 for 64.
@@ -409,137 +405,214 @@ __device__ __forceinline__ double lsd_bin_coef(int maxmag2, int n_bins) {
   return max_grad > 0 ? (double)(n_bins - 1) / max_grad : 0.0;
 }
 
-// The image is cut into chunks of LSD_CHUNK rows.  One CTA bins a chunk: its warps walk the chunk's row-segment lists (written
-// by the gradient kernel: only the defined pixels, ~12 %), turn gx^2 + gy^2 into the bin of the 1024-bin pseudo-ordering
-// (the per-image maximum is known by now), store the bin in its place and count the bins; one warp then scatters the
-// chunk's lists in raster order.
-#define LSD_CHUNK 16
-__global__ void __launch_bounds__(256) k_lsd_rowhist(size_t stride, int W, int H, int n_bins, int nchunks, int nxb,
-                                                     const int* __restrict__ maxmag2, uint32_t* __restrict__ list,
-                                                     const int* __restrict__ segcnt, uint32_t* __restrict__ chunkcnt) {
-  __shared__ uint32_t hist[LSD_BINS_MAX];
-  const int ch = blockIdx.x, im = blockIdx.y, tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
-  for (int i = tid; i < n_bins; i += 256) hist[i] = 0;
-  __syncthreads();
-  const double coef = lsd_bin_coef(maxmag2[im], n_bins);
-  const int ya = ch * LSD_CHUNK, y1 = min((ch + 1) * LSD_CHUNK, H - 1);
-  const int nseg = (y1 - ya) * nxb;
-  const int* sc = segcnt + (size_t)im * ((size_t)H * nxb);
-  for (int sg = wrp; sg < nseg; sg += 8) {
-    const int y = ya + sg / nxb, xb = sg - (sg / nxb) * nxb;
-    const int n = sc[(size_t)y * nxb + xb];
-    const size_t o = (size_t)im * stride + (size_t)y * W + (size_t)xb * LSD_SEG;
-    for (int i = lane; i < n; i += 32) {
-      const uint32_t e = list[o + i];
-      const double norm = sqrt((double)(e >> LSD_COL_BITS) / 4.0);
-      const int b = (int)(norm * coef);
-      list[o + i] = (e & ((1u << LSD_COL_BITS) - 1u)) | ((uint32_t)b << LSD_COL_BITS);
-      atomicAdd(&hist[b], 1u);
+// One CTA orders the seeds of one image.  The image's list entries, in raster order, are cut into LSD_SO_WARPS contiguous
+// ranges of equal length (by an entry-count prefix over segcnt, so a band of edge-dense rows is shared by all warps); each
+// warp counts the bins of its range into its own row of a shared [warp][bin] table, one scan turns the table into each
+// warp's first slot per bin (bins descending, then warps in range order), and each warp walks its range again in raster
+// order and stores every seed at its slot (match.any ranks inside 32 entries).  The bin is recomputed from gx^2 + gy^2 in
+// both walks: nothing is written back to the lists and no count leaves the CTA.
+#ifndef LSD_SO_WARPS
+#define LSD_SO_WARPS 16
+#endif
+#define LSD_SO_THREADS (32 * LSD_SO_WARPS)
+#define LSD_SO_AHEAD 4   // runs of 32 entries whose loads are in flight ahead of the one being processed
+#define LSD_SO_BPT ((LSD_BINS_MAX + LSD_SO_THREADS - 1) / LSD_SO_THREADS)   // bins per thread in the scan over the bins
+static size_t lsd_seed_order_smem(int n_bins) { return (size_t)LSD_SO_WARPS * n_bins * sizeof(uint32_t); }
+
+// Hands out one warp's range of list entries as runs of at most 32 entries of one row segment, in raster order.  Every
+// lane holds the same state; the lengths of 32 segments at a time sit one per lane, so runs of empty segments are
+// skipped with one ballot.
+struct LsdSegWalk {
+  const int* sc;        // segment lengths of the image
+  int nseg, nxb, W;
+  int seg, i, n;        // current segment, its next entry, its length
+  uint32_t p0;          // pixel offset of the current segment = where its list starts
+  uint32_t left;        // entries of the range not handed out yet
+  int cbase, c32;       // this lane's length: segment cbase + lane
+  unsigned nz;          // lanes whose segment is not empty
+
+  __device__ __forceinline__ void load_lengths(int base) {
+    const int lane = threadIdx.x & 31;
+    cbase = base;
+    c32 = base + lane < nseg ? __ldg(&sc[base + lane]) : 0;
+    nz = __ballot_sync(0xFFFFFFFFu, c32 > 0);
+  }
+  __device__ __forceinline__ void enter(int s) {
+    seg = s;
+    const int y = s / nxb;
+    p0 = (uint32_t)(y * W + (s - y * nxb) * LSD_SEG);
+  }
+  __device__ __forceinline__ void init(const int* sc_, int nseg_, int nxb_, int W_, int seg0, int off, uint32_t count) {
+    sc = sc_; nseg = nseg_; nxb = nxb_; W = W_;
+    left = count;
+    i = off;
+    if (count) {
+      enter(seg0);
+      load_lengths(seg0);
+      n = __shfl_sync(0xFFFFFFFFu, c32, 0);
     }
   }
-  __syncthreads();
-  uint32_t* out = chunkcnt + ((size_t)im * nchunks + ch) * n_bins;
-  for (int i = tid; i < n_bins; i += 256) out[i] = hist[i];
+  // the next run: its first list index (from the image's list start) and its length (0: the range is done); *q0 = the
+  // pixel offset of its segment
+  __device__ __forceinline__ int next(uint32_t* q0, uint32_t* l0) {
+    if (left == 0) return 0;
+    const int m = min(min(32, n - i), (int)left);
+    *q0 = p0;
+    *l0 = p0 + (uint32_t)i;
+    i += m;
+    left -= (uint32_t)m;
+    if (left && i == n) {   // on to the next segment with entries (one exists: entries are left)
+      for (;;) {
+        const int d = seg + 1 - cbase;
+        const unsigned ahead = d < 32 ? nz & (0xFFFFFFFFu << d) : 0u;
+        if (ahead) {
+          const int s = cbase + __ffs(ahead) - 1;
+          n = __shfl_sync(0xFFFFFFFFu, c32, s - cbase);
+          enter(s);
+          i = 0;
+          break;
+        }
+        load_lengths(cbase + 32);
+        seg = cbase - 1;
+      }
+    }
+    return m;
+  }
+};
+
+// Walks a warp's range with the entries of LSD_SO_AHEAD runs loaded ahead; f(entry, pixel offset of its segment, run
+// length) is called once per run, in raster order, by the whole warp (lanes >= run length hold no entry).
+template <class F>
+__device__ __forceinline__ void lsd_walk_range(LsdSegWalk wk, const uint32_t* __restrict__ lst, F f) {
+  const int lane = threadIdx.x & 31;
+  uint32_t e[LSD_SO_AHEAD], p0[LSD_SO_AHEAD];
+  int m[LSD_SO_AHEAD];
+  auto fetch = [&](int j) {
+    uint32_t l0 = 0;
+    m[j] = wk.next(&p0[j], &l0);
+    e[j] = lane < m[j] ? __ldg(&lst[l0 + lane]) : 0u;
+  };
+#pragma unroll
+  for (int j = 0; j < LSD_SO_AHEAD; ++j) fetch(j);
+  for (;;) {
+#pragma unroll
+    for (int j = 0; j < LSD_SO_AHEAD; ++j) {
+      if (m[j] == 0) return;
+      f(e[j], p0[j], m[j]);
+      fetch(j);
+    }
+  }
 }
 
-// one block (n_bins threads, <= 1024) per image: per-bin prefix over chunks, then start of each bin (bins descending).
-// The chunk counts of a bin are loaded 8 at a time before their prefixes are stored back (the loads of a plain
-// read-modify-write loop serialise behind the stores to the same array); the scan over the bins is two levels of warp shuffles.
-__global__ void __launch_bounds__(1024) k_lsd_binscan(uint32_t* __restrict__ chunkcnt, int nchunks, int n_bins,
-                                                      uint32_t* __restrict__ binstart, int* __restrict__ nseeds) {
-  __shared__ uint32_t tot[LSD_BINS_MAX];
-  __shared__ uint32_t wsum[32];
-  const int im = blockIdx.x, b = threadIdx.x, lane = b & 31, wrp = b >> 5;
-  uint32_t run = 0;
-  if (b < n_bins) {
-    uint32_t* c = chunkcnt + (size_t)im * nchunks * n_bins + b;
-    for (int k0 = 0; k0 < nchunks; k0 += 8) {
-      uint32_t v[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = k0 + j < nchunks ? __ldcg(&c[(size_t)(k0 + j) * n_bins]) : 0u;
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        if (k0 + j < nchunks) {
-          c[(size_t)(k0 + j) * n_bins] = run;
-          run += v[j];
-        }
-    }
-    tot[b] = run;
-  }
-  __syncthreads();
-  // exclusive scan over bins in DESCENDING bin order: thread b holds reversed element b = bin (n_bins - 1 - b)
-  const int rb = n_bins - 1 - b;
-  const uint32_t mine = b < n_bins ? tot[rb] : 0u;
-  uint32_t incl = mine;
+// Block-wide inclusive prefix of v over the CTA's threads; *total = the sum.  s_w: LSD_SO_WARPS words of shared memory.
+__device__ __forceinline__ uint32_t lsd_so_scan(uint32_t v, uint32_t* s_w, uint32_t* total) {
+  const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
 #pragma unroll
   for (int off = 1; off < 32; off <<= 1) {
-    const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, off);
-    if (lane >= off) incl += v;
+    const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, v, off);
+    if (lane >= off) v += u;
   }
-  if (lane == 31) wsum[wrp] = incl;
+  if (lane == 31) s_w[wrp] = v;
   __syncthreads();
-  if (wrp == 0) {
-    uint32_t w = wsum[lane], wi = w;
+  uint32_t base = 0, tot = 0;
 #pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, wi, off);
-      if (lane >= off) wi += v;
-    }
-    wsum[lane] = wi - w;   // exclusive prefix of the warp totals
+  for (int k = 0; k < LSD_SO_WARPS; ++k) {
+    const uint32_t x = s_w[k];
+    if (k < wrp) base += x;
+    tot += x;
   }
-  __syncthreads();
-  const uint32_t excl = wsum[wrp] + incl - mine;
-  if (b < n_bins) binstart[(size_t)im * n_bins + rb] = excl;
-  if (b == n_bins - 1) nseeds[im] = (int)(excl + mine);
+  __syncthreads();   // s_w is free again
+  *total = tot;
+  return base + v;
 }
 
-// one warp per (chunk, image): walks the chunk's row-segment lists in raster order, stable ranks via match_any
-__global__ void __launch_bounds__(128) k_lsd_scatter(const uint32_t* __restrict__ list,
-                                                     const int* __restrict__ segcnt, size_t stride, int W, int H, int n_bins,
-                                                     int nchunks, int nxb, const uint32_t* __restrict__ chunkcnt,
-                                                     const uint32_t* __restrict__ binstart, uint32_t* __restrict__ order) {
-  __shared__ uint32_t cnt[4][LSD_BINS_MAX];
-  const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ch = blockIdx.x * 4 + wid, im = blockIdx.y;
-  if (ch >= nchunks) return;
-  uint32_t* c = cnt[wid];
-  const uint32_t* rc = chunkcnt + ((size_t)im * nchunks + ch) * n_bins;
-  const uint32_t* bs = binstart + (size_t)im * n_bins;
-  for (int i = lane; i < n_bins; i += 32) c[i] = rc[i] + bs[i];
-  __syncwarp();
-  uint32_t* ord = order + (size_t)im * stride;
-  const int ya = ch * LSD_CHUNK, y1 = min((ch + 1) * LSD_CHUNK, H - 1);
-  const int nseg = (y1 - ya) * nxb;
-  const int* sc = segcnt + (size_t)im * ((size_t)H * nxb) + (size_t)ya * nxb;   // the chunk's segments are contiguous, row-major
-  int n_next = nseg > 0 ? sc[0] : 0;
-  for (int sg = 0; sg < nseg; ++sg) {
-    const int n = n_next;
-    n_next = sg + 1 < nseg ? sc[sg + 1] : 0;
-    const int y = ya + sg / nxb, xb = sg - (sg / nxb) * nxb;
-    const uint32_t seg0 = (uint32_t)(y * W + xb * LSD_SEG);   // pixel index of the segment's first column
-    const size_t o = (size_t)im * stride + seg0;
-    for (int i0 = 0; i0 < n; i0 += 32) {
-      const int i = i0 + lane;
-      const bool valid = i < n;
-      const uint32_t e = valid ? list[o + i] : 0u;
-      const uint32_t idx = seg0 + (e & ((1u << LSD_COL_BITS) - 1u));
-      const int b = valid ? (int)(e >> LSD_COL_BITS) : -1;
-      const unsigned vm = __ballot_sync(0xFFFFFFFFu, valid);
-      if (valid) {
-        const unsigned peers = __match_any_sync(vm, b);
-        const int rank = __popc(peers & ((1u << lane) - 1));
-        const int leader = __ffs(peers) - 1;
-        uint32_t base = 0;
-        if (lane == leader) {
-          base = c[b];
-          c[b] = base + __popc(peers);
-        }
-        base = __shfl_sync(peers, base, leader);
-        ord[base + rank] = idx;
-      }
-      __syncwarp();
+// list / order: image stride `stride` entries; segcnt: nseg = (H - 1) * nxb lengths per image (the last row holds no
+// seed).  Dynamic shared memory: LSD_SO_WARPS * n_bins words.
+__global__ void __launch_bounds__(LSD_SO_THREADS) k_lsd_seed_order(const uint32_t* __restrict__ list, const int* __restrict__ segcnt,
+                                                                   size_t stride, int W, int H, int nxb, int n_bins,
+                                                                   const int* __restrict__ maxmag2, uint32_t* __restrict__ order,
+                                                                   int* __restrict__ nseeds) {
+  extern __shared__ uint32_t s_cnt[];   // [warp][bin]: counts, then the warp's first slot per bin
+  __shared__ uint32_t s_w[LSD_SO_WARPS];
+  __shared__ int s_seg[LSD_SO_WARPS], s_off[LSD_SO_WARPS];
+  const int im = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
+  const int nseg = (H - 1) * nxb;
+  const int* sc = segcnt + (size_t)im * ((size_t)H * nxb);
+  const uint32_t* lst = list + (size_t)im * stride;
+  for (int k = tid; k < LSD_SO_WARPS * n_bins; k += LSD_SO_THREADS) s_cnt[k] = 0;
+  // the image's entry count, and the segment and offset at which each warp's range starts
+  uint32_t t = 0, total;
+  for (int s = tid; s < nseg; s += LSD_SO_THREADS) t += (uint32_t)__ldg(&sc[s]);
+  lsd_so_scan(t, s_w, &total);
+  uint32_t carry = 0;
+  for (int s0 = 0; s0 < nseg; s0 += LSD_SO_THREADS) {
+    const int s = s0 + tid;
+    const uint32_t n = s < nseg ? (uint32_t)__ldg(&sc[s]) : 0u;
+    uint32_t tile;
+    const uint32_t pre = carry + lsd_so_scan(n, s_w, &tile) - n;
+#pragma unroll
+    for (int k = 0; k < LSD_SO_WARPS; ++k) {
+      const uint32_t b = (uint32_t)((unsigned long long)k * total / LSD_SO_WARPS);
+      if (b - pre < n) { s_seg[k] = s; s_off[k] = (int)(b - pre); }
     }
+    carry += tile;
   }
+  __syncthreads();
+  const uint32_t r0 = (uint32_t)((unsigned long long)wrp * total / LSD_SO_WARPS);
+  const uint32_t r1 = (uint32_t)((unsigned long long)(wrp + 1) * total / LSD_SO_WARPS);
+  LsdSegWalk wk;
+  wk.init(sc, nseg, nxb, W, r1 > r0 ? s_seg[wrp] : 0, r1 > r0 ? s_off[wrp] : 0, r1 - r0);
+  const double coef = lsd_bin_coef(maxmag2[im], n_bins);
+  auto bin_of = [&](uint32_t e) { return (int)(sqrt((double)(e >> LSD_COL_BITS) / 4.0) * coef); };
+  uint32_t* cw = s_cnt + wrp * n_bins;
+  // count
+  lsd_walk_range(wk, lst, [&](uint32_t e, uint32_t, int m) {
+    if (lane < m) atomicAdd(&cw[bin_of(e)], 1u);
+  });
+  __syncthreads();
+  // slots: per bin, a prefix over the warps; over the bins, a prefix in descending bin order (thread tid holds the
+  // LSD_SO_BPT bins at descending positions LSD_SO_BPT * tid ...)
+  uint32_t bt[LSD_SO_BPT], sum = 0;
+#pragma unroll
+  for (int h = 0; h < LSD_SO_BPT; ++h) {
+    const int b = n_bins - 1 - (LSD_SO_BPT * tid + h);
+    bt[h] = 0;
+    if (b >= 0)
+      for (int w = 0; w < LSD_SO_WARPS; ++w) {
+        const uint32_t c = s_cnt[w * n_bins + b];
+        s_cnt[w * n_bins + b] = bt[h];
+        bt[h] += c;
+      }
+    sum += bt[h];
+  }
+  uint32_t all;
+  uint32_t base = lsd_so_scan(sum, s_w, &all) - sum;
+#pragma unroll
+  for (int h = 0; h < LSD_SO_BPT; ++h) {
+    const int b = n_bins - 1 - (LSD_SO_BPT * tid + h);
+    if (b >= 0)
+      for (int w = 0; w < LSD_SO_WARPS; ++w) s_cnt[w * n_bins + b] += base;
+    base += bt[h];
+  }
+  if (tid == 0) nseeds[im] = (int)all;
+  __syncthreads();
+  // scatter, in raster order: stable ranks among the run's lanes of one bin
+  uint32_t* ord = order + (size_t)im * stride;
+  lsd_walk_range(wk, lst, [&](uint32_t e, uint32_t p0, int m) {
+    if (lane < m) {
+      const int b = bin_of(e);
+      const unsigned peers = __match_any_sync(0xFFFFFFFFu >> (32 - m), b);
+      const int leader = __ffs(peers) - 1;
+      uint32_t slot = 0;
+      if (lane == leader) {
+        slot = cw[b];
+        cw[b] = slot + __popc(peers);
+      }
+      slot = __shfl_sync(peers, slot, leader) + __popc(peers & ((1u << lane) - 1u));
+      ord[slot] = p0 + (e & ((1u << LSD_COL_BITS) - 1u));
+    }
+    __syncwarp();
+  });
 }
 
 // ---- region growing ----------------------------------------------------------------------------------------
@@ -1117,8 +1190,6 @@ static void lsd_buffers(LsdState* s, DevBufList& b) {
   b.add(s->segcnt, N * s->hs * s->nxb);
   b.add(s->rect_perm, N * R);
   b.add(s->maxmag2, N);
-  b.add(s->rowcnt, N * ((s->hs + LSD_CHUNK - 1) / LSD_CHUNK) * s->n_bins);
-  b.add(s->binstart, N * s->n_bins);
   b.add(s->regpts, As * N);
   b.add(s->regions, N * R);
   b.add(s->nregions, N);
@@ -1253,7 +1324,6 @@ plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t
   const int W = s->ws, H = s->hs;
   const size_t As = (size_t)W * H, A = (size_t)s->bp * h, Asp = (size_t)s->sp * H;
   LsdPix* pix = s->pix[par] + (s->ws + 1);  // pixel (0,0) of the first image
-  const int nchunks = (H - 1 + LSD_CHUNK - 1) / LSD_CHUNK;
   plf_status st;
   const uint8_t* scaled = d_imgs;
   size_t scaled_stride = img_stride;
@@ -1286,16 +1356,10 @@ plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t
                                                                s->seedlist, s->segcnt, s->nxb, s->maxmag2);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "lsd.k_lsd_grad");
-  k_lsd_rowhist<<<dim3(nchunks, n), 256, 0, cs>>>(As, W, H, s->n_bins, nchunks, s->nxb, s->maxmag2, s->seedlist, s->segcnt, s->rowcnt);
+  k_lsd_seed_order<<<n, LSD_SO_THREADS, lsd_seed_order_smem(s->n_bins), cs>>>(s->seedlist, s->segcnt, As, W, H, s->nxb, s->n_bins,
+                                                                              s->maxmag2, s->order[par], s->nseeds[par]);
   PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, cs, "lsd.k_lsd_rowhist");
-  k_lsd_binscan<<<n, 1024, 0, cs>>>(s->rowcnt, nchunks, s->n_bins, s->binstart, s->nseeds[par]);
-  PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, cs, "lsd.k_lsd_binscan");
-  k_lsd_scatter<<<dim3((nchunks + 3) / 4, n), 128, 0, cs>>>(s->seedlist, s->segcnt, As, W, H, s->n_bins, nchunks, s->nxb, s->rowcnt, s->binstart,
-                                                            s->order[par]);
-  PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, cs, "lsd.k_lsd_scatter");
+  plf_mark(ctx, cs, "lsd.k_lsd_seed_order");
   return PLF_OK;
 }
 
@@ -1452,4 +1516,6 @@ extern "C" plf_status plf_debug_sincosf(plf_ctx* ctx, const float* in, float* s,
 // the overlapped batch 28 ms -> 7 ms, step 83.3 -> 81.9 ms.
 void plf_configure_lsd() {
   cudaFuncSetAttribute((const void*)k_lsd_grow, cudaFuncAttributePreferredSharedMemoryCarveout, 72);
+  cudaFuncSetAttribute((const void*)k_lsd_seed_order, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                       (int)lsd_seed_order_smem(LSD_BINS_MAX));
 }
