@@ -307,7 +307,12 @@ plf_status plf_gn_pose(plf_ctx* ctx, const plf_gn_opts* opts, const double* P, c
  *     inlier flag (:1826-1851).
  * opts: lambda / lambda_k / max_iters = SlamConfig::lambdaLbaLM / lambdaLbaK / maxItersLba (src/slamConfig.cpp:64-66);
  * ref_quirks = 1 reproduces four oddities of the reference as written (oracle/lba.c lists them with their lines),
- * 0 follows its evident intent.  Returns PLF_ERR_INVALID for an empty problem (the reference returns -1, :1324-1328). */
+ * 0 follows its evident intent.  Returns PLF_ERR_INVALID for an empty problem (the reference returns -1, :1324-1328), NULL
+ * arrays, ungrouped observations or out-of-range indices, and PLF_ERR_CAPACITY beyond 64 local keyframes.  A landmark
+ * without observations, or whose first-pass block (the sum of w Jx Jx^T over its rows) has an exactly zero diagonal
+ * entry - e.g. one seen once, at its exact projection - is refused with PLF_ERR_INVALID naming it, before any step and
+ * with the inputs unchanged: the reference would factor a zero pivot (its SimplicialLDLT's failure is not checked),
+ * and the landmark, then every keyframe that observes it, would turn NaN.  The context stays usable after any error. */
 typedef struct plf_lba_opts {
   double lambda, lambda_k;
   int max_iters;
@@ -352,8 +357,9 @@ plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_pr
  * opts: lambda / lambda_k / max_iters = SlamConfig::lambdaLbaLM / lambdaLbaK / maxItersLba, which GBA reuses (:2116, :2391);
  * min_error = min_error_change = DBL_EPSILON, the literals of :2637, :2667.  ref_quirks = 1 reproduces six oddities of
  * the reference as written (oracle/gba.py lists them as g1-g6 with their lines), 0 follows its evident intent.
- * Limits: n_kf <= 4096 (else PLF_ERR_CAPACITY).  PLF_ERR_INVALID for an empty problem, a landmark without observations,
- * ungrouped observations, out-of-range indices or NULL arrays; the context stays usable after any error.
+ * Limits: n_kf <= 4096 (else PLF_ERR_CAPACITY).  PLF_ERR_INVALID for an empty problem, a landmark without observations
+ * or with a zero diagonal entry in its first-pass block (as plf_local_ba), ungrouped observations, out-of-range indices
+ * or NULL arrays; the context stays usable after any error.
  * Work is enqueued on plf_stream and uses scratch slot 10 (shared with plf_local_ba), which stays allocated until
  * plf_destroy: about 288 n_kf^2 bytes for the dense reduced system (1.2 GB at 2048 keyframes, 4.8 GB at 4096) plus
  * 144 bytes per observation and about 650 bytes per landmark.  Up to n_kf = 64 the reduced system is factored by one CTA as in

@@ -239,7 +239,19 @@ class _LbaOpts(C.Structure):
 
 
 class _LbaResult(C.Structure):
-    _fields_ = [("iters", C.c_int), ("err", C.c_double), ("lambda_", C.c_double)]
+    _fields_ = [("iters", C.c_int), ("err", C.c_double), ("lambda_", C.c_double), ("zero_lm", C.c_int)]
+
+
+# orc_local_ba's return codes and its iteration trace (orc_local_ba_trace): record 0 is the first pass, record i the
+# i-th LM iteration; `stop` is LBA_CONTINUE or why the run ended after that pass
+LBA_EMPTY, LBA_ZERO_BLOCK = -1, -2
+LBA_CONTINUE, LBA_STOP_CHANGE, LBA_STOP_MIN_ERROR, LBA_STOP_STEP, LBA_STOP_MAXIT = range(5)
+LBA_TRACE_DTYPE = np.dtype([("err", np.float64), ("lambda_", np.float64), ("step", np.float64), ("applied", np.int32),
+                            ("stop", np.int32)])
+
+
+class _LbaTrace(C.Structure):
+    _fields_ = [("rec", C.c_void_p), ("cap", C.c_int), ("n", C.c_int)]
 
 
 def lba_opts(lambda_=1e-5, lambda_k=10.0, max_iters=15, homog_th=1e-7, min_error=1e-7, min_error_change=1e-7, ref_quirks=1):
@@ -250,7 +262,9 @@ def lba_opts(lambda_=1e-5, lambda_k=10.0, max_iters=15, homog_th=1e-7, min_error
 
 def local_ba(cam, prob, opts=None):
     """MapHandler::levMarquardtOptimizationLBA (oracle/lba.c).  prob: dict with kf_pose [nkf,6], pt [npt,3], ls [nls,6],
-    fixed_T [nf,4,4], pt_obs_lm / pt_obs_kf / pt_obs_xy, ls_obs_lm / ls_obs_kf / ls_obs_le (kf < 0: fixed keyframe -1-k)."""
+    fixed_T [nf,4,4], pt_obs_lm / pt_obs_kf / pt_obs_xy, ls_obs_lm / ls_obs_kf / ls_obs_le (kf < 0: fixed keyframe -1-k).
+    Returns rc (0, LBA_EMPTY or LBA_ZERO_BLOCK, with the refused landmark in zero_lm: points first, then lines), the
+    optimised values (the input's when refused), iters, err, lambda_ and trace: LBA_TRACE_DTYPE records, one per pass."""
     o = _LbaOpts(**(opts or lba_opts()))
     c = orc_camera(**{k: cam[k] for k in ("width", "height", "fx", "fy", "cx", "cy", "b")})
     kf = np.ascontiguousarray(prob["kf_pose"], np.float64).reshape(-1, 6)
@@ -264,11 +278,14 @@ def local_ba(cam, prob, opts=None):
     lo_lm, lo_kf, lo_le = i32("ls_obs_lm"), i32("ls_obs_kf"), f64("ls_obs_le")
     pm, lm = np.zeros(max(len(pt), 1), np.uint8), np.zeros(max(len(ls), 1), np.uint8)
     res = _LbaResult()
-    f = lib().orc_local_ba
+    rec = np.zeros(max(o.max_iters, 1), LBA_TRACE_DTYPE)
+    tr = _LbaTrace(rec.ctypes.data, len(rec), 0)
+    f = lib().orc_local_ba_trace
     f.restype = C.c_int
     rc = f(C.byref(c), C.byref(o), len(kf), len(pt), len(ls), _p(X), len(fT), _p(fT), len(po_lm), _p(po_lm), _p(po_kf), _p(po_xy),
-           len(lo_lm), _p(lo_lm), _p(lo_kf), _p(lo_le), _p(pm), _p(lm), C.byref(res))
+           len(lo_lm), _p(lo_lm), _p(lo_kf), _p(lo_le), _p(pm), _p(lm), C.byref(res), C.byref(tr))
+    assert tr.n <= len(rec)
     nk, npt = 6 * len(kf), 3 * len(pt)
     return dict(rc=rc, kf_pose=X[:nk].reshape(-1, 6), pt=X[nk:nk + npt].reshape(-1, 3), ls=X[nk + npt:].reshape(-1, 6),
                 pt_moved=pm[:len(pt)].astype(bool), ls_moved=lm[:len(ls)].astype(bool), iters=res.iters, err=res.err,
-                lambda_=res.lambda_)
+                lambda_=res.lambda_, zero_lm=res.zero_lm, trace=rec[:tr.n].copy())

@@ -193,6 +193,14 @@ def hmax_int(diag):
     return float(h)
 
 
+def zero_block_landmark(diag, nkf, npt):
+    """The first landmark (points, then lines) whose block on the diagonal `diag` of the first pass has an exactly zero
+    entry, else -1.  Such a problem is refused before any step, as oracle/lba.c and plf_global_ba refuse it."""
+    lm = np.asarray(diag)[6 * nkf:]
+    z = np.concatenate([(lm[:3 * npt].reshape(-1, 3) == 0).any(1), (lm[3 * npt:].reshape(-1, 6) == 0).any(1)])
+    return int(np.argmax(z)) if z.any() else -1
+
+
 def _apply(X, DX, nkf):
     Y = X.copy()
     for i in range(nkf):
@@ -209,7 +217,8 @@ def _div(a, b):
 
 def global_ba(cam, prob, o=None):
     """levMarquardtOptimizationGBA; prob as plf_global_ba takes it.  Returns clib.local_ba's dict (X split into
-    kf_pose / pt / ls, the moved flags plf_global_ba also fills, iters, err, lambda_)."""
+    kf_pose / pt / ls, the moved flags plf_global_ba also fills, iters, err, lambda_), or dict(rc=clib.LBA_ZERO_BLOCK,
+    zero_lm) for a landmark whose first-pass block has a zero diagonal entry."""
     o = o or opts()
     q = bool(o["ref_quirks"])
     kf = np.asarray(prob["kf_pose"], np.float64).reshape(-1, 6)
@@ -225,6 +234,9 @@ def global_ba(cam, prob, o=None):
     H, g, s = normal_equations(cam, prob, X0, T0inv, True, q, homog)
     err = _div(s, 0) if q else s / nobs                                          # (g1)
     dg = H.diagonal()
+    zl = zero_block_landmark(dg, nkf, npt)
+    if zl >= 0:
+        return dict(rc=clib.LBA_ZERO_BLOCK, zero_lm=zl)
     lam *= hmax_int(dg) if q else float(np.max(np.abs(dg)))                      # (g2)
     H = H + sp.diags(lam * dg)
     DX = solve_lower(H, g)

@@ -25,6 +25,9 @@
  * The lambda schedule (:1785-1790: divide by lambda_k when the error grew - without applying the step - multiply
  * otherwise) and the normalisation by the number of landmarks (:1773) are kept as written in both modes.
  * SimplicialLDLT (AMD-ordered sparse LDL^T) is restated as a dense LDL^T without pivoting.
+ * A landmark whose first-pass block has an exactly zero diagonal entry (no observation, or every row with a zero
+ * Jacobian: a single observation at its exact projection) would make the reference factor a zero pivot, whose failure
+ * it does not check; here, as on the device, the problem is refused (ORC_LBA_ZERO_BLOCK) before any step.
  */
 #include <math.h>
 #include <stdlib.h>
@@ -185,13 +188,32 @@ static void apply_step(double* X, const double* DX, int nkf, int N) {
   for (int i = 6 * nkf; i < N; i++) X[i] += DX[i];
 }
 
+static void trace_rec(orc_lba_trace* tr, double err, double lambda, double step, int applied, int stop) {
+  if (!tr) return;
+  if (tr->n < tr->cap) {
+    orc_lba_trace_rec* r = tr->rec + tr->n;
+    r->err = err; r->lambda = lambda; r->step = step; r->applied = applied; r->stop = stop;
+  }
+  tr->n++;
+}
+
 /* kf index of an observation: >= 0 local keyframe (pose = X block), < 0 fixed keyframe -1 - k (pose fixed_T[k]) */
 int orc_local_ba(const orc_camera* cam, const orc_lba_opts* o, int nkf, int npt, int nls, double* X, int n_fixed,
                  const double* fixed_T, int npo, const int* po_lm, const int* po_kf, const double* po_xy, int nlo,
                  const int* lo_lm, const int* lo_kf, const double* lo_le, uint8_t* pt_moved, uint8_t* ls_moved,
                  orc_lba_result* out) {
+  return orc_local_ba_trace(cam, o, nkf, npt, nls, X, n_fixed, fixed_T, npo, po_lm, po_kf, po_xy, nlo, lo_lm, lo_kf, lo_le,
+                            pt_moved, ls_moved, out, NULL);
+}
+
+int orc_local_ba_trace(const orc_camera* cam, const orc_lba_opts* o, int nkf, int npt, int nls, double* X, int n_fixed,
+                       const double* fixed_T, int npo, const int* po_lm, const int* po_kf, const double* po_xy, int nlo,
+                       const int* lo_lm, const int* lo_kf, const double* lo_le, uint8_t* pt_moved, uint8_t* ls_moved,
+                       orc_lba_result* out, orc_lba_trace* tr) {
   const int N = 6 * nkf + 3 * npt + 6 * nls;
   (void)n_fixed;
+  if (out) out->zero_lm = -1;
+  if (tr) tr->n = 0;
   if (N <= 0 || npo + nlo == 0) return -1;
   double* H = (double*)malloc((size_t)N * N * sizeof(double));
   double* g = (double*)malloc((size_t)N * sizeof(double));
@@ -223,6 +245,16 @@ int orc_local_ba(const orc_camera* cam, const orc_lba_opts* o, int nkf, int npt,
     const double* L = X0 + 6 * nkf + 3 * npt + 6 * lo_lm[k];
     add_line_row(&a, o->homog_th, Ti, L, L + 3, lo_le + 3 * k, lo_kf[k] >= 0 ? lo_kf[k] : -1, lo_lm[k]);
   }
+  /* a zero diagonal entry in a landmark's block: refused before any step (see the header) */
+  for (int l = 0; l < npt + nls; l++) {
+    const int off = l < npt ? 6 * nkf + 3 * l : 6 * nkf + 3 * npt + 6 * (l - npt), dim = l < npt ? 3 : 6;
+    for (int i = 0; i < dim; i++)
+      if (H[(size_t)(off + i) * N + off + i] == 0.0) {
+        if (out) out->zero_lm = l;
+        free(H); free(g); free(DX); free(X0); free(T0inv);
+        return ORC_LBA_ZERO_BLOCK;
+      }
+  }
   double err = a.err;
   if (o->ref_quirks) err /= (double)(0 + 0); /* (q1) */
   else err /= (double)(npo + nlo);
@@ -235,6 +267,12 @@ int orc_local_ba(const orc_camera* cam, const orc_lba_opts* o, int nkf, int npt,
   for (int i = 0; i < N; i++) H[(size_t)i * N + i] += lambda * H[(size_t)i * N + i];
   ldlt_solve(H, g, DX, N);
   apply_step(X, DX, nkf, N);
+  {
+    double n2 = 0;
+    for (int i = 0; i < N; i++) n2 += DX[i] * DX[i];
+    trace_rec(tr, err, lambda, sqrt(n2), 1, ORC_LBA_CONTINUE);
+  }
+  int stop = ORC_LBA_STOP_MAXIT;
   double err_prev = err;
   /* ---- LM iterations ---- */
   int iters;
@@ -264,10 +302,16 @@ int orc_local_ba(const orc_camera* cam, const orc_lba_opts* o, int nkf, int npt,
       add_line_row(&a, o->ref_quirks ? 0.0000001 : o->homog_th /* (q4) */, Ti, P, Q, lo_le + 3 * k, lo_kf[k] >= 0 ? lo_kf[k] : -1, lo_lm[k]);
     }
     err = a.err / (double)(npt + nls);
-    if (fabs(err - err_prev) < o->min_error_change || err < o->min_error) break;
+    if (fabs(err - err_prev) < o->min_error_change || err < o->min_error) {
+      stop = fabs(err - err_prev) < o->min_error_change ? ORC_LBA_STOP_CHANGE : ORC_LBA_STOP_MIN_ERROR;
+      trace_rec(tr, err, lambda, -1.0, 0, stop);
+      break;
+    }
     for (int i = 0; i < N; i++) H[(size_t)i * N + i] += lambda * H[(size_t)i * N + i];
     ldlt_solve(H, g, DX, N);
-    if (err > err_prev) {
+    const double lambda_used = lambda;
+    const int grew = err > err_prev;
+    if (grew) {
       lambda /= lambda_k;
     } else {
       lambda *= lambda_k;
@@ -275,9 +319,16 @@ int orc_local_ba(const orc_camera* cam, const orc_lba_opts* o, int nkf, int npt,
     }
     double n2 = 0;
     for (int i = 0; i < N; i++) n2 += DX[i] * DX[i];
-    if (sqrt(n2) < o->min_error_change) break;
+    const int small = sqrt(n2) < o->min_error_change;
+    trace_rec(tr, err, lambda_used, sqrt(n2), !grew, small ? ORC_LBA_STOP_STEP : ORC_LBA_CONTINUE);
+    if (small) {
+      stop = ORC_LBA_STOP_STEP;
+      break;
+    }
     err_prev = err;
   }
+  /* the loop counter ran out: the last pass made ends the run */
+  if (tr && stop == ORC_LBA_STOP_MAXIT && tr->n >= 1 && tr->n <= tr->cap) tr->rec[tr->n - 1].stop = ORC_LBA_STOP_MAXIT;
   /* landmarks that moved more than 1 cm lose their inlier flag (:1826-1851) */
   for (int i = 0; i < npt; i++) {
     double n2 = 0;

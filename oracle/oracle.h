@@ -102,9 +102,35 @@ typedef struct orc_lba_opts {
   double min_error_change; /* Config::minErrorChange */
   int ref_quirks;          /* 1: reproduce the reference as written (see lba.c), 0: the evident intent */
 } orc_lba_opts;
-typedef struct orc_lba_result { int iters; double err; double lambda; } orc_lba_result;
+typedef struct orc_lba_result {
+  int iters;
+  double err;
+  double lambda;
+  int zero_lm; /* rc ORC_LBA_ZERO_BLOCK: the landmark (points first, then lines) whose block has a zero diagonal entry */
+} orc_lba_result;
+/* return codes: 0, -1 (empty problem, as the reference), ORC_LBA_ZERO_BLOCK (a landmark's first-pass block D has an
+ * exactly zero diagonal entry, e.g. a landmark without observations or whose every row has a zero Jacobian: refused
+ * before any step, X unchanged) */
+enum { ORC_LBA_ZERO_BLOCK = -2 };
+/* Iteration trace of orc_local_ba_trace: record 0 is the first pass, record i the i-th LM iteration. */
+enum { ORC_LBA_CONTINUE = 0, ORC_LBA_STOP_CHANGE = 1, ORC_LBA_STOP_MIN_ERROR = 2, ORC_LBA_STOP_STEP = 3, ORC_LBA_STOP_MAXIT = 4 };
+typedef struct orc_lba_trace_rec {
+  double err;    /* normalised error of the pass */
+  double lambda; /* the damping of its solve (the current lambda when the error tests stopped the run first) */
+  double step;   /* |DX| of its solve; -1 when the error tests stopped the run first */
+  int applied;   /* 1 when its step was applied; 0 when the error grew (solved, not applied) or no step was solved */
+  int stop;      /* ORC_LBA_CONTINUE, or why the run ended after this pass (CHANGE / MIN_ERROR: the error tests, no solve) */
+} orc_lba_trace_rec;
+typedef struct orc_lba_trace {
+  orc_lba_trace_rec* rec;
+  int cap, n; /* records available / passes made (those past cap are counted, not stored) */
+} orc_lba_trace;
 int orc_local_ba(const orc_camera* cam, const orc_lba_opts* o, int nkf, int npt, int nls, double* X, int n_fixed,
                  const double* fixed_T, int npo, const int* po_lm, const int* po_kf, const double* po_xy, int nlo,
                  const int* lo_lm, const int* lo_kf, const double* lo_le, uint8_t* pt_moved, uint8_t* ls_moved,
                  orc_lba_result* out);
+int orc_local_ba_trace(const orc_camera* cam, const orc_lba_opts* o, int nkf, int npt, int nls, double* X, int n_fixed,
+                       const double* fixed_T, int npo, const int* po_lm, const int* po_kf, const double* po_xy, int nlo,
+                       const int* lo_lm, const int* lo_kf, const double* lo_le, uint8_t* pt_moved, uint8_t* ls_moved,
+                       orc_lba_result* out, orc_lba_trace* tr);
 #endif

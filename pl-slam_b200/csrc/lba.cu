@@ -55,7 +55,8 @@ struct LbaDev {
   double* A; double* gc;                       // nkf x 36, nkf x 6
   double* S; double* gred; double* dxc;        // n x n, n, n   (n = 6 nkf)
   double* DX;                                  // N
-  double* scal;                                // [0] err, [1] |dx|^2, [2] Hmax (as ordered bits), [3] Hmax under g2
+  double* scal;                                // [0] err, [1] |dx|^2, [2] Hmax (as ordered bits), [3] Hmax under g2,
+                                               // [4] first landmark with a zero diagonal entry in D (k_lba_lm_accum)
 };
 struct LbaCam { double fx, fy, cx, cy; };
 
@@ -185,10 +186,13 @@ __global__ void __launch_bounds__(128) k_lba_lm_accum(LbaDev d) {
     }
   }
   double mx = 0.0;
-  for (int i = 0; i < dim; ++i) mx = fmax(mx, fabs(D[7 * i]));
+  bool zero = false;
+  for (int i = 0; i < dim; ++i) { mx = fmax(mx, fabs(D[7 * i])); zero |= D[7 * i] == 0.0; }
   for (int i = 0; i < 36; ++i) d.D[36 * (size_t)l + i] = D[i];
   for (int i = 0; i < 6; ++i) d.gl[6 * (size_t)l + i] = g[i];
   lba_atomic_max_pos(&d.scal[2], mx);
+  // a zero diagonal entry: scal[4] (as an integer) keeps nlm - l of the first such landmark, 0 when there is none
+  if (zero) atomicMax(reinterpret_cast<unsigned long long*>(&d.scal[4]), (unsigned long long)(d.nlm - l));
 }
 
 __global__ void k_lba_kf_diagmax(LbaDev d) {
@@ -637,8 +641,10 @@ plf_status plf_ldlt_tiled(plf_ctx* ctx, cudaStream_t cs, int n6, double* S, doub
 
 // The host loop of both routines: the reference's control flow, on the device kernels above.  `global` selects
 // levMarquardtOptimizationGBA (:2101-2699) over levMarquardtOptimizationLBA (:1332-1989): its quirk set, its error
-// normalisation in the LM iterations, up to 4096 keyframes (the blocked factorisation beyond n = 384) and a landmark
-// without observations refused.
+// normalisation in the LM iterations and up to 4096 keyframes (the blocked factorisation beyond n = 384).  Both refuse a
+// landmark whose first-pass block D has an exactly zero diagonal entry, before any step: the reference would factor a
+// zero pivot (its SimplicialLDLT's failure is not checked) and the landmark, then every keyframe observing it, would
+// turn NaN.  A landmark without observations is refused by name first; the rest by one flag read with the first pass.
 static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out, bool global) {
   const char* fn = global ? "plf_global_ba" : "plf_local_ba";
   if (!ctx || !opts || !p || p->n_kf < 0 || p->n_pt < 0 || p->n_ls < 0 || p->n_pt_obs < 0 || p->n_ls_obs < 0 || p->n_fixed < 0)
@@ -667,10 +673,9 @@ static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_p
     if (is_line) for (int c = 0; c < 3; ++c) h_z[3 * (size_t)k + c] = p->ls_obs_le[3 * (size_t)(k - npo) + c];
     else { h_z[3 * (size_t)k] = p->pt_obs_xy[2 * (size_t)k]; h_z[3 * (size_t)k + 1] = p->pt_obs_xy[2 * (size_t)k + 1]; }
   }
-  if (global)   // its landmark block would be zero: the reference would factor a zero pivot
-    for (int l = 0; l < nlm; ++l)
-      if (!lm_start[l + 1])
-        return plf_fail(ctx, PLF_ERR_INVALID, "%s: %s landmark %d has no observation", fn, l < npt ? "point" : "line", l < npt ? l : l - npt);
+  for (int l = 0; l < nlm; ++l)   // its landmark block would be zero
+    if (!lm_start[l + 1])
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: %s landmark %d has no observation", fn, l < npt ? "point" : "line", l < npt ? l : l - npt);
   for (int l = 0; l < nlm; ++l) lm_start[l + 1] += lm_start[l];
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const bool blocked = n > 384;   // k_lba_solve (one CTA, one launch) up to 64 keyframes, the tiled LDL^T beyond
@@ -711,7 +716,7 @@ static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_p
   const LbaCam cam = {ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy};
   const int q = opts->ref_quirks ? (global ? BAQ_GBA : BAQ_LBA) : 0;
   double lambda = opts->lambda;
-  double h_scal[4];
+  double h_scal[5];
   // builds the normal equations of `mode` and leaves err / Hmax in scal
   auto build = [&](int mode) -> plf_status {
     PLF_CUDA(ctx, cudaMemsetAsync(d.A, 0, (size_t)std::max(nkf, 1) * 288, cs));
@@ -731,7 +736,7 @@ static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_p
       k_gba_hmax_int<<<1, 1024, 0, cs>>>(d);
       PLF_LAUNCH_CHECK(ctx);
     }
-    PLF_CUDA(ctx, cudaMemcpyAsync(h_scal, d.scal, 32, cudaMemcpyDeviceToHost, cs));
+    PLF_CUDA(ctx, cudaMemcpyAsync(h_scal, d.scal, 40, cudaMemcpyDeviceToHost, cs));
     PLF_CUDA(ctx, cudaStreamSynchronize(cs));
     return PLF_OK;
   };
@@ -765,6 +770,13 @@ static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_p
   // ---- first pass on the map's values (LBA :1352-1541, GBA :2117-2356), lambda *= Hmax (:1543-1550, :2358-2365), first
   // step applied unconditionally
   if ((st = build(0))) return st;
+  unsigned long long zero_flag;
+  memcpy(&zero_flag, &h_scal[4], 8);
+  if (zero_flag) {
+    const int l = nlm - (int)zero_flag;
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: %s landmark %d has a zero diagonal entry in its first-pass block (no row constrains it)",
+                    fn, l < npt ? "point" : "line", l < npt ? l : l - npt);
+  }
   double err = h_scal[0];
   volatile int never_incremented = 0;   // Npt_obs + Nls_obs of the reference
   if (q & BAQ_FIRST_ERR0) err /= (double)never_incremented;   // (q1) :1541, (g1) :2356

@@ -282,6 +282,84 @@ def lba_problem(cam, n_kf=4, n_fixed=2, n_pt=120, n_ls=40, seed=0, px_noise=0.3,
                 truth=dict(kf_pose=kf_true, pt=pt, ls=ls))
 
 
+def local_map_problem(cam, n_kf=8, n_fixed=2, pts_per_kf=6, ls_per_kf=2, seed=0, t0=0, single=0.3, max_track=3,
+                      px_noise=0.3, pose_noise=0.01, lm_noise=0.02):
+    """A local map shaped like the ones MapHandler::localBundleAdjustment assembles (src/mapHandler.cpp:1220-1330), from
+    a sliding window of n_fixed fixed keyframes followed by n_kf local ones, 0.8 m apart along the optical axis.  The
+    window starts at keyframe t0 of the trajectory, whose keyframe 0 is the world frame: with t0 = 0 the first fixed
+    keyframe (fixed_T[0]) is the identity, otherwise no keyframe is.
+    Every keyframe of the window creates pts_per_kf points and ls_per_kf lines that only it and the next k keyframes
+    observe.  A fraction `single` of the landmarks (rounded) has k = 0, one observation: all those the last keyframe
+    creates (it creates fewer when the window is too short for that to stay within `single`) and others drawn at
+    random.  The rest have k uniform in 1..max_track, cut at the window's end.  So some landmarks are seen by local
+    keyframes only, some by fixed ones only, and the fixed keyframes observe landmarks the local ones see too.
+    Observations are grouped per landmark in ascending order, creator first; kf_obs is the local index, or -1 - k for
+    fixed_T[k].  Observations are the true projections plus px_noise; the initial values are the truth plus pose_noise
+    / lm_noise.  truth holds the window's poses T_kf_w (fixed first) and the true landmarks."""
+    rng = np.random.default_rng(seed)
+    n_tot = n_kf + n_fixed
+    T = []
+    for i in range(n_tot):
+        t = t0 + i
+        x = np.zeros(6) if t == 0 else np.array([0.05 * rng.standard_normal(), 0.02 * rng.standard_normal(), 0.8 * t,
+                                                   0.01 * rng.standard_normal(), 0.03 * rng.standard_normal(),
+                                                   0.005 * rng.standard_normal()])
+        T.append(np.eye(4) if t == 0 else expmap_se3(x))
+    T = np.stack(T)
+    Ti = np.linalg.inv(T)
+    kf_id = lambda t: -1 - t if t < n_fixed else t - n_fixed
+
+    def counts(per):   # landmarks created by each keyframe: the last one's are all single
+        c = np.full(n_tot, per)
+        if n_tot > 1:
+            c[-1] = min(per, int(single * (n_tot - 1) * per / (1.0 - single)))
+        return c
+
+    def tracks(creator):   # k per landmark
+        n = len(creator)
+        k = np.minimum(rng.integers(1, max_track + 1, n), n_tot - 1 - creator)
+        forced = k == 0
+        extra = max(0, int(round(single * n)) - int(forced.sum()))
+        pick = rng.choice(np.flatnonzero(~forced), min(extra, int((~forced).sum())), replace=False)
+        k[pick] = 0
+        return k
+
+    def in_front(creator):   # a point 6-30 m ahead of its creator, within the middle of the image
+        z = rng.uniform(6.0, 30.0, len(creator))
+        u = rng.uniform(0.3, 0.7, len(creator)) * cam["width"]; v = rng.uniform(0.3, 0.7, len(creator)) * cam["height"]
+        Pc = np.stack([(u - cam["cx"]) * z / cam["fx"], (v - cam["cy"]) * z / cam["fy"], z, np.ones_like(z)], 1)
+        return np.einsum("nij,nj->ni", T[creator], Pc)[:, :3]
+
+    def project(t, P):
+        Pc = Ti[t, :3, :3] @ P + Ti[t, :3, 3]
+        return np.array([cam["cx"] + cam["fx"] * Pc[0] / Pc[2], cam["cy"] + cam["fy"] * Pc[1] / Pc[2]])
+
+    pc = np.repeat(np.arange(n_tot), counts(pts_per_kf))
+    lc = np.repeat(np.arange(n_tot), counts(ls_per_kf))
+    pt = in_front(pc)
+    ls = np.concatenate([in_front(lc), in_front(lc)], 1)
+    pk, lk = tracks(pc), tracks(lc)
+    po_lm, po_kf, po_xy, lo_lm, lo_kf, lo_le = [], [], [], [], [], []
+    for j in range(len(pt)):
+        for t in range(pc[j], pc[j] + pk[j] + 1):
+            po_lm.append(j); po_kf.append(kf_id(t)); po_xy.append(project(t, pt[j]) + px_noise * rng.standard_normal(2))
+    for j in range(len(ls)):
+        for t in range(lc[j], lc[j] + lk[j] + 1):
+            s = np.append(project(t, ls[j, :3]) + px_noise * rng.standard_normal(2), 1.0)
+            e = np.append(project(t, ls[j, 3:]) + px_noise * rng.standard_normal(2), 1.0)
+            le = np.cross(s, e)
+            lo_lm.append(j); lo_kf.append(kf_id(t)); lo_le.append(le / math.sqrt(le[0] * le[0] + le[1] * le[1]))
+    kf_true = np.stack([_logmap_se3(T[t]) for t in range(n_fixed, n_tot)]) if n_kf else np.zeros((0, 6))
+    return dict(kf_pose=kf_true + pose_noise * rng.standard_normal(kf_true.shape),
+                pt=pt + lm_noise * rng.standard_normal(pt.shape), ls=ls + lm_noise * rng.standard_normal(ls.shape),
+                fixed_T=T[:n_fixed].copy(),
+                pt_obs_lm=np.array(po_lm, np.int32), pt_obs_kf=np.array(po_kf, np.int32),
+                pt_obs_xy=np.array(po_xy, np.float64).reshape(-1, 2),
+                ls_obs_lm=np.array(lo_lm, np.int32), ls_obs_kf=np.array(lo_kf, np.int32),
+                ls_obs_le=np.array(lo_le, np.float64).reshape(-1, 3),
+                truth=dict(T=T, kf_pose=kf_true, pt=pt, ls=ls))
+
+
 def gba_problem(cam, n_kf=64, pts_per_kf=100, ls_per_kf=15, loop=True, seed=0, n_fixed=1, n_views=3, px_noise=0.3,
                 pose_noise=0.01, lm_noise=0.02):
     """A whole map as MapHandler::globalBundleAdjustment assembles it (src/mapHandler.cpp:1995-2090): n_fixed fixed
