@@ -372,8 +372,7 @@ __global__ void __launch_bounds__(256) k_bow_transform(TreeView t0, TreeView t1,
     unsigned key = 0xFFFFFFFFu;
     if (lane < cnt) {
       const uint4 c = __ldg(&t.desc[2 * (base + lane)]), e = __ldg(&t.desc[2 * (base + lane) + 1]);
-      const int d = __popc(a.x ^ c.x) + __popc(a.y ^ c.y) + __popc(a.z ^ c.z) + __popc(a.w ^ c.w) + __popc(b.x ^ e.x) +
-                    __popc(b.y ^ e.y) + __popc(b.z ^ e.z) + __popc(b.w ^ e.w);
+      const int d = plf_hamming256(a, b, c, e);
       key = ((unsigned)d << 5) | (unsigned)lane;
     }
     key = __reduce_min_sync(0xFFFFFFFFu, key);

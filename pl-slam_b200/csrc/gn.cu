@@ -25,11 +25,6 @@ struct GnCam {
   double fx, fy, cx, cy;
 };
 
-__device__ __forceinline__ void gn_transform(const double* T, const double* P, double* Q) {
-#pragma unroll
-  for (int i = 0; i < 3; ++i) Q[i] = T[4 * i] * P[0] + T[4 * i + 1] * P[1] + T[4 * i + 2] * P[2] + T[4 * i + 3];
-}
-
 __device__ __forceinline__ void gn_jac6(double fgz2, double gx, double gy, double gz, double ax, double ay,
                                         double* J) {
   J[0] = +fgz2 * ax * gz;
@@ -42,7 +37,7 @@ __device__ __forceinline__ void gn_jac6(double fgz2, double gx, double gy, doubl
 
 __device__ __forceinline__ double gn_point_res(const GnCam& c, const double* T, const double* P,
                                                const double* obs, double* e2, double* Pc) {
-  gn_transform(T, P, Pc);
+  d_transform(T, P, Pc);
   e2[0] = (c.cx + c.fx * Pc[0] / Pc[2]) - obs[0];
   e2[1] = (c.cy + c.fy * Pc[1] / Pc[2]) - obs[1];
   return sqrt(e2[0] * e2[0] + e2[1] * e2[1]);
@@ -51,8 +46,8 @@ __device__ __forceinline__ double gn_point_res(const GnCam& c, const double* T, 
 __device__ __forceinline__ double gn_line_res(const GnCam& c, const double* T, const double* sP,
                                               const double* eP, const double* l, double* e2, double* sPc,
                                               double* ePc) {
-  gn_transform(T, sP, sPc);
-  gn_transform(T, eP, ePc);
+  d_transform(T, sP, sPc);
+  d_transform(T, eP, ePc);
   const double sx = c.cx + c.fx * sPc[0] / sPc[2], sy = c.cy + c.fy * sPc[1] / sPc[2];
   const double ex = c.cx + c.fx * ePc[0] / ePc[2], ey = c.cy + c.fy * ePc[1] / ePc[2];
   e2[0] = l[0] * sx + l[1] * sy + l[2];

@@ -15,17 +15,13 @@
 //                       epipolar gate and the scatter back to original indices with an atomic count of the rejects
 #include "plf_internal.h"
 #include "plf_geom.cuh"
+#include "plf_se3.cuh"
 
 #define KF_MAX_LANDMARKS 65535   // 16-bit train index of the kNN keys (the reverse problem's train set is the queries)
 #define KF_MAX_FEATURES 8192     // the bound of plf_match_grid_*
 #define KF_CELL_LIM 268435456.0  // query cells are clamped to +-2^28 (the reference's double -> int is undefined beyond
                                  // int range; the clamp keeps Bresenham differences inside int), NaN -> 0
 
-// Rigid transform with the fixed evaluation order ((r0 x + r1 y) + r2 z) + t of each row (no contraction: --fmad=false).
-__device__ __forceinline__ double3 kf_rigid(const double* T, double x, double y, double z) {
-  return make_double3(((T[0] * x + T[1] * y) + T[2] * z) + T[3], ((T[4] * x + T[5] * y) + T[6] * z) + T[7],
-                      ((T[8] * x + T[9] * y) + T[10] * z) + T[11]);
-}
 __device__ __forceinline__ int kf_cell(double v) {
   if (v != v) return 0;
   return mg_cell(fmin(fmax(v, -KF_CELL_LIM), KF_CELL_LIM));
@@ -64,15 +60,15 @@ struct KfKind {
 __global__ void __launch_bounds__(256) k_kf_query_vis(KfKind k, const double* __restrict__ T, KfCam c) {
   const int i = blockIdx.x * 256 + threadIdx.x;
   if (i >= k.nq_in) return;
-  const double* S = k.X + (size_t)i * k.x_stride;
-  const double3 Ps = kf_rigid(T, S[0], S[1], S[2]);
-  const double2 ps = plf_project(c.fx, c.fy, c.cx, c.cy, Ps.x, Ps.y, Ps.z);
-  bool vis = ps.x > 0 && ps.x < c.w && ps.y > 0 && ps.y < c.h && Ps.z > 0.0;   // :551
+  double Ps[3];
+  d_transform(T, k.X + (size_t)i * k.x_stride, Ps);
+  const double2 ps = plf_project(c.fx, c.fy, c.cx, c.cy, Ps[0], Ps[1], Ps[2]);
+  bool vis = ps.x > 0 && ps.x < c.w && ps.y > 0 && ps.y < c.h && Ps[2] > 0.0;   // :551
   if (k.lines) {
-    const double* E = k.XE + (size_t)i * k.x_stride;
-    const double3 Pe = kf_rigid(T, E[0], E[1], E[2]);
-    const double2 pe = plf_project(c.fx, c.fy, c.cx, c.cy, Pe.x, Pe.y, Pe.z);
-    vis = vis && pe.x > 0 && pe.x < c.w && pe.y > 0 && pe.y < c.h && Pe.z > 0.0;   // :654-655
+    double Pe[3];
+    d_transform(T, k.XE + (size_t)i * k.x_stride, Pe);
+    const double2 pe = plf_project(c.fx, c.fy, c.cx, c.cy, Pe[0], Pe[1], Pe[2]);
+    vis = vis && pe.x > 0 && pe.x < c.w && pe.y > 0 && pe.y < c.h && Pe[2] > 0.0;   // :654-655
     k.proj[2 * (size_t)i] = ps;
     k.proj[2 * (size_t)i + 1] = pe;
   } else {

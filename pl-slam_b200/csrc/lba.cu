@@ -71,9 +71,6 @@ __device__ __forceinline__ void lba_jac_pose(double gz2, double fxdx, double fyd
 __device__ __forceinline__ void lba_rowvec_R(const double* v, const double* T, double* out) {
   for (int j = 0; j < 3; ++j) out[j] = v[0] * T[j] + v[1] * T[4 + j] + v[2] * T[8 + j];
 }
-__device__ __forceinline__ void lba_xform(const double* T, const double* P, double* Q) {
-  for (int i = 0; i < 3; ++i) Q[i] = T[4 * i] * P[0] + T[4 * i + 1] * P[1] + T[4 * i + 2] * P[2] + T[4 * i + 3];
-}
 
 // mode 0: first pass on the map's values (X0 / T0inv); mode 1: LM iteration on X; quirks: BAQ_* set
 __global__ void __launch_bounds__(128) k_lba_rows(LbaDev d, LbaCam c, int mode, int quirks, double homog_th) {
@@ -100,7 +97,7 @@ __global__ void __launch_bounds__(128) k_lba_rows(LbaDev d, LbaCam c, int mode, 
     const double* z = d.obs_z + 3 * k;
     if (!is_line) {
       double Xwi[3];
-      lba_xform(Ti, X + 6 * d.nkf + 3 * lm, Xwi);
+      d_transform(Ti, X + 6 * d.nkf + 3 * lm, Xwi);
       const double px = c.cx + c.fx * Xwi[0] / Xwi[2], py = c.cy + c.fy * Xwi[1] / Xwi[2];
       const double dx = z[0] - px, dy = z[1] - py;
       nrm = sqrt(dx * dx + dy * dy);
@@ -123,8 +120,8 @@ __global__ void __launch_bounds__(128) k_lba_rows(LbaDev d, LbaCam c, int mode, 
         Q = P + 3;
       }
       double Pwi[3], Qwi[3];
-      lba_xform(Ti, P, Pwi);
-      lba_xform(Ti, Q, Qwi);
+      d_transform(Ti, P, Pwi);
+      d_transform(Ti, Q, Qwi);
       const double ppx = c.cx + c.fx * Pwi[0] / Pwi[2], ppy = c.cy + c.fy * Pwi[1] / Pwi[2];
       const double qpx = c.cx + c.fx * Qwi[0] / Qwi[2], qpy = c.cy + c.fy * Qwi[1] / Qwi[2];
       const double e0 = z[0] * ppx + z[1] * ppy + z[2], e1 = z[0] * qpx + z[1] * qpy + z[2];

@@ -11,6 +11,7 @@
 #include <math.h>
 
 #include "plf_internal.h"
+#include "plf_se3.cuh"
 
 // largest eigenvalue of a symmetric 6x6 matrix (cyclic Jacobi; Eigen's SelfAdjointEigenSolver sorts ascending and the
 // reference reads element 5, :3883-3885)
@@ -135,11 +136,7 @@ extern "C" plf_status plf_loop_closure_pose(plf_ctx* ctx, const plf_lc_params* l
     return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_loop_closure_pose: %d point / %d line correspondences exceed the caller's capacity", kp, kl);
   double T[16], Ti[16];
   if ((st = plf_se3(ctx, 0, r.x, T))) return st;  // expmap_se3(x_inc)
-  for (int i = 0; i < 3; ++i) {                     // inverse_se3
-    for (int j = 0; j < 3; ++j) Ti[4 * i + j] = T[4 * j + i];
-    Ti[4 * i + 3] = -(T[i] * T[3] + T[4 + i] * T[7] + T[8 + i] * T[11]);
-  }
-  Ti[12] = Ti[13] = Ti[14] = 0; Ti[15] = 1;
+  d_inverse_se3(T, Ti);
   if ((st = plf_se3(ctx, 1, Ti, out->pose_inc))) return st;
   out->accepted = 1;
   return PLF_OK;

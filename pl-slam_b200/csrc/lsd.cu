@@ -18,7 +18,7 @@
 //                    row pass), one rounding (k_blur_q8: generic variant for the other kernels, up to 15 taps)
 //   k_resize_exact4  (orb.cu) INTER_LINEAR_EXACT resample to scale
 //   k_lsd_grad       2x2 gradient; for the DEFINED pixels only (|grad| > rho, ~12 %): the 8-byte record {angle
-//                    (cv::fastAtan2, degrees, f32, from a table keyed by (gx,gy)), table index}, and one packed entry
+//                    (cv::fastAtan2 = plf_fast_atan2, degrees, f32, from a table keyed by (gx,gy)), table index}, and one packed entry
 //                    (column, |grad|^2) of the raster-ordered seed list of the pixel's row segment; per-image max of |grad|^2.
 //                    Nothing dense leaves the kernel (the record map restores itself to "undefined", see k_lsd_fill_notdef)
 //   k_lsd_seed_order stable counting sort of the seed lists by magnitude bin (descending), raster order inside a
@@ -219,27 +219,6 @@ __global__ void __launch_bounds__(256) k_blur_q8_fast(const __grid_constant__ CU
 }
 
 // ---- gradient ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float lsd_fast_atan2(float y, float x) {  // cv::fastAtan2, see orb.cu
-  const float p1 = 0.9997878412794807f * (float)(180 / 3.14159265358979323846);
-  const float p3 = -0.3258083974640975f * (float)(180 / 3.14159265358979323846);
-  const float p5 = 0.1555786518463281f * (float)(180 / 3.14159265358979323846);
-  const float p7 = -0.04432655554792128f * (float)(180 / 3.14159265358979323846);
-  const float ax = fabsf(x), ay = fabsf(y);
-  float a, c, c2;
-  if (ax >= ay) {
-    c = __fdiv_rn(ay, __fadd_rn(ax, (float)2.2204460492503131e-16));
-    c2 = __fmul_rn(c, c);
-    a = __fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(p7, c2), p5), c2), p3), c2), p1), c);
-  } else {
-    c = __fdiv_rn(ax, __fadd_rn(ay, (float)2.2204460492503131e-16));
-    c2 = __fmul_rn(c, c);
-    a = __fsub_rn(90.f, __fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(p7, c2), p5), c2), p3), c2), p1), c));
-  }
-  if (x < 0) a = __fsub_rn(180.f, a);
-  if (y < 0) a = __fsub_rn(360.f, a);
-  return a;
-}
-
 // Per-pixel record read by the region-growing kernel: one 8-byte load per neighbour.
 struct __align__(8) LsdPix {
   float a;    // level-line angle in DEGREES exactly as cv::fastAtan2(gx,-gy) returns it (OpenCV stores a * DEG_TO_RADS as
@@ -266,7 +245,7 @@ __global__ void __launch_bounds__(256) k_lsd_build_lut(double rho, float* __rest
   float2 cs = make_float2(0.f, 0.f), sv = make_float2(0.f, 0.f);
   const double norm = sqrt((double)(gx * gx + gy * gy) / 4.0);
   if (!(norm <= rho)) {
-    const float adeg = lsd_fast_atan2((float)gx, (float)(-gy));
+    const float adeg = plf_fast_atan2((float)gx, (float)(-gy));
     a = adeg;
     const float af = (float)((double)adeg * LSD_DEG2RAD);
     cs = make_float2(glibc_cosf(af), glibc_sinf(af));
@@ -798,7 +777,7 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
           if (!((mi >> k) & 1u)) {  // the first candidate sits in the band
             if (!fresh) {
               add_staged();
-              th = lsd_fast_atan2(sumdy, sumdx);
+              th = plf_fast_atan2(sumdy, sumdx);
               inv0 = __fmul_rn(rsqrtf(__fadd_rn(__fmul_rn(sumdx, sumdx), __fmul_rn(sumdy, sumdy))), 1.02f);
               margin = margin0;
               lo = prec_deg - margin; hi = prec_deg + margin;
@@ -852,7 +831,7 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
           if (!fresh) add_staged();   // the members accepted since S was last read (fresh: none)
           if (lane == 0) {
             // region angle handed to the rectangle fit: the seed's own angle for a 1-pixel region, else the angle of the sum
-            const double reg_angle = nreg == 1 ? th_seed : (double)(fresh ? th : lsd_fast_atan2(sumdy, sumdx)) * LSD_DEG2RAD;
+            const double reg_angle = nreg == 1 ? th_seed : (double)(fresh ? th : plf_fast_atan2(sumdy, sumdx)) * LSD_DEG2RAD;
             const unsigned long long bits = (unsigned long long)__double_as_longlong(reg_angle);
             regions[nreg_out] = make_uint4(cursor, nreg, (uint32_t)bits, (uint32_t)(bits >> 32));
           }
@@ -983,8 +962,8 @@ __global__ void __launch_bounds__(128) k_lsd_rects(const LsdPix* __restrict__ pi
     }
   }
   const double lambda = 0.5 * (Ixx + Iyy - sqrt((Ixx - Iyy) * (Ixx - Iyy) + 4.0 * Ixy * Ixy));
-  double theta = (fabs(Ixx) > fabs(Iyy)) ? (double)lsd_fast_atan2((float)(lambda - Ixx), (float)Ixy)
-                                         : (double)lsd_fast_atan2((float)Ixy, (float)(lambda - Iyy));
+  double theta = (fabs(Ixx) > fabs(Iyy)) ? (double)plf_fast_atan2((float)(lambda - Ixx), (float)Ixy)
+                                         : (double)plf_fast_atan2((float)Ixy, (float)(lambda - Iyy));
   theta *= LSD_DEG2RAD;
   if (lsd_angle_diff(theta, reg_angle) > prec) theta += LSD_PI;
   const double dx = cos(theta), dy = sin(theta);

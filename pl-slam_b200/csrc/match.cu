@@ -13,12 +13,6 @@
 
 #define KNN_NONE 0xFFFFFFFFu
 
-__device__ __forceinline__ int hamming256(const uint4& qa, const uint4& qb, const uint4& a,
-                                          const uint4& b) {
-  return __popc(qa.x ^ a.x) + __popc(qa.y ^ a.y) + __popc(qa.z ^ a.z) + __popc(qa.w ^ a.w) +
-         __popc(qb.x ^ b.x) + __popc(qb.y ^ b.y) + __popc(qb.z ^ b.z) + __popc(qb.w ^ b.w);
-}
-
 // ---- the kNN kernel: tensor-core formulation ------------------------------------------------------------------------
 // (round 1 started with an XOR+POPC kernel - 64 queries x 4 lanes per CTA over a shared train tile - that ran at the
 //  POPC issue roofline, 13.1 ms per 3072 images; this formulation does the same work in 6.0 ms)
@@ -331,7 +325,7 @@ __global__ void __launch_bounds__(128) k_median_desc(const uint32_t* __restrict_
   for (int pr = lane; pr < n * n; pr += 32) {
     const int i = pr / n, j = pr - i * n;
     const uint4 a0 = dp[2 * i], a1 = dp[2 * i + 1], b0 = dp[2 * j], b1 = dp[2 * j + 1];
-    D[i][j] = (unsigned short)hamming256(a0, a1, b0, b1);
+    D[i][j] = (unsigned short)plf_hamming256(a0, a1, b0, b1);
   }
   __syncwarp();
   const int k = (int)(1 + 0.5 * (n - 1));  // position read by the reference; k <= n - 1 for n >= 2

@@ -13,21 +13,16 @@
 //                  cell - for lines: of one of the query's Bresenham cells - plus, for lines, the direction gate),
 //                  computes the Hamming distance of the candidates and writes d or "not considered" to a dense u16
 //                  matrix (the grid arrives as cell -> items lists, the host wrapper inverts it to item -> cells);
-//   k_mg_rows    : one thread per query scans its row in ascending train index with the reference's strict '<' updates,
+//   k_mgb_rows   : one thread per query scans its row in ascending train index with the reference's strict '<' updates,
 //                  applies the f32 ratio test and records matches_12; matches_21 comes from the column pass;
-//   k_mg_mutual  : drops i1 unless matches_21[matches_12[i1]] == i1, counts the matches.
+//   k_mgb_mutual : drops i1 unless matches_21[matches_12[i1]] == i1, counts the matches.
+// The row and mutual passes take the arguments of the batched form below (MgbArgs); plf_match_grid_* run them as one
+// problem.
 #include "plf_internal.h"
 #include <algorithm>
 #include <vector>
 
 #define MG_NONE 0xFFFFu
-
-
-__device__ __forceinline__ int mg_hamming(const uint4* a, const uint4* b) {
-  const uint4 a0 = a[0], a1 = a[1], b0 = b[0], b1 = b[1];
-  return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) +
-         __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
-}
 
 // 8-connected Bresenham walk over the cells of (x1,y1)-(x2,y2), end points included (used as a set).
 struct MgLine {
@@ -93,7 +88,8 @@ __global__ void __launch_bounds__(128) k_mg_columns(MgGrid g, int is_lines, cons
     }
     unsigned short out = MG_NONE;
     if (cand) {
-      const int d = mg_hamming(reinterpret_cast<const uint4*>(d1) + 2 * (size_t)i1, b);
+      const uint4* qd = reinterpret_cast<const uint4*>(d1) + 2 * (size_t)i1;
+      const int d = plf_hamming256(qd[0], qd[1], b[0], b[1]);
       if (best_lr) {
         if (d < run) { run = d; who = i1; out = (unsigned short)d; }
       } else {
@@ -105,12 +101,15 @@ __global__ void __launch_bounds__(128) k_mg_columns(MgGrid g, int is_lines, cons
   m21[i2] = who;
 }
 
-__global__ void __launch_bounds__(128) k_mg_rows(const unsigned short* __restrict__ D, int n1, int n2, float nnr,
-                                                 int32_t* __restrict__ m12) {
+// Row and mutual passes over problems p0 .. p0 + gridDim.y - 1 (MgbArgs, plf_internal.h); D and m21 hold the problems of
+// the current chunk (pl = p - p0).
+__global__ void __launch_bounds__(128) k_mgb_rows(MgbArgs a, int p0) {
+  const int pl = blockIdx.y, p = p0 + pl;
   const int i1 = blockIdx.x * 128 + threadIdx.x;
+  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K), n2 = min(a.n2[(size_t)p * a.n2_stride], a.Kt);
   if (i1 >= n1) return;
   int best_d = 0x7FFFFFFF, best_d2 = 0x7FFFFFFF, best_idx = -1;
-  const unsigned short* row = D + (size_t)i1 * n2;
+  const unsigned short* row = a.D + (size_t)pl * a.K * a.Kt + (size_t)i1 * a.Kt;
   for (int i2 = 0; i2 < n2; ++i2) {
     const int d = row[i2];
     if (d == MG_NONE) continue;
@@ -118,20 +117,31 @@ __global__ void __launch_bounds__(128) k_mg_rows(const unsigned short* __restric
     else if (d < best_d2) best_d2 = d;
   }
   // `best_d < best_d2 * nnr`: int * float -> f32 product, int -> f32 comparison (INT_MAX when there is one candidate)
-  m12[i1] = ((float)best_d < __fmul_rn((float)best_d2, nnr)) ? best_idx : -1;
+  a.m12[(size_t)p * a.m12_stride + i1] = ((float)best_d < __fmul_rn((float)best_d2, a.nnr)) ? best_idx : -1;
 }
 
-__global__ void __launch_bounds__(128) k_mg_mutual(int32_t* __restrict__ m12, const int* __restrict__ m21, int n1,
-                                                   int best_lr, int* __restrict__ count) {
+__global__ void __launch_bounds__(128) k_mgb_mutual(MgbArgs a, int p0) {
+  const int pl = blockIdx.y, p = p0 + pl;
   const int i1 = blockIdx.x * 128 + threadIdx.x;
+  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K);
   bool ok = false;
   if (i1 < n1) {
+    int32_t* m12 = a.m12 + (size_t)p * a.m12_stride;
     const int i2 = m12[i1];
     ok = i2 >= 0;
-    if (ok && best_lr && m21[i2] != i1) { m12[i1] = -1; ok = false; }
+    if (ok && a.best_lr && a.m21[(size_t)pl * a.Kt + i2] != i1) { m12[i1] = -1; ok = false; }
   }
   const unsigned bal = __ballot_sync(0xFFFFFFFFu, ok);
-  if ((threadIdx.x & 31) == 0 && bal) atomicAdd(count, __popc(bal));
+  if ((threadIdx.x & 31) == 0 && bal) atomicAdd(&a.count[(size_t)p * a.count_stride], __popc(bal));
+}
+
+static plf_status mgb_rows_mutual(plf_ctx* ctx, const MgbArgs& a, int p0, int np, int max_n1, cudaStream_t cs) {
+  const dim3 grid((max_n1 + 127) / 128, np);
+  k_mgb_rows<<<grid, 128, 0, cs>>>(a, p0);
+  PLF_LAUNCH_CHECK(ctx);
+  k_mgb_mutual<<<grid, 128, 0, cs>>>(a, p0);
+  PLF_LAUNCH_CHECK(ctx);
+  return PLF_OK;
 }
 
 static plf_status mg_run(plf_ctx* ctx, const char* who, int is_lines, const int* q_geo, const uint8_t* d1, int n1,
@@ -164,16 +174,19 @@ static plf_status mg_run(plf_ctx* ctx, const char* who, int is_lines, const int*
       if (cell_items[k] >= 0 && cell_items[k] < n2) tcells[fill[cell_items[k]]++] = c;  // cell id = x * rows + y
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const int gq = is_lines ? 4 : 2;
-  int *dq, *dts, *dtc, *dm21, *dcount;
+  int *dq, *dts, *dtc, *dn;
   double* ddir;
   uint8_t *dd1, *dd2;
-  unsigned short* D;
-  int32_t* dm12;
+  // the row and mutual passes run as one problem of the batched form: K = n1, Kt = n2, strides 0
+  MgbArgs a = {};
+  a.K = n1; a.Kt = n2; a.best_lr = best_lr ? 1 : 0; a.nnr = nnr;
   DevBufList scr;
   scr.add(dq, (size_t)n1 * gq); scr.add(dts, (size_t)n2 + 1); scr.add(dtc, tcells.size()); scr.add(ddir, (size_t)n2 * 2);
   scr.add(dd1, (size_t)n1 * 32); scr.add(dd2, (size_t)n2 * 32);
-  scr.add(D, (size_t)n1 * n2); scr.add(dm12, n1); scr.add(dm21, n2); scr.add(dcount, 1);
+  scr.add(a.D, (size_t)n1 * n2); scr.add(a.m12, n1); scr.add(a.m21, n2); scr.add(dn, 3);
   if (plf_status st = scr.carve(ctx, PLF_SCR_MATCH)) return st;
+  a.n1 = dn; a.n2 = dn + 1; a.count = dn + 2;
+  const int hn[3] = {n1, n2, 0};   // the counts, and the match count zeroed
   cudaStream_t cs = ctx->stream;
   PLF_CUDA(ctx, cudaMemcpyAsync(dq, q_geo, (size_t)n1 * gq * 4, cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(dts, tstart.data(), (size_t)(n2 + 1) * 4, cudaMemcpyHostToDevice, cs));
@@ -181,18 +194,15 @@ static plf_status mg_run(plf_ctx* ctx, const char* who, int is_lines, const int*
   if (is_lines) PLF_CUDA(ctx, cudaMemcpyAsync(ddir, t_dir, (size_t)n2 * 16, cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(dd1, d1, (size_t)n1 * 32, cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(dd2, d2, (size_t)n2 * 32, cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaMemsetAsync(dcount, 0, sizeof(int), cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(dn, hn, sizeof hn, cudaMemcpyHostToDevice, cs));
   const MgGrid g = {cols, rows, w.width_lo, w.width_hi, w.height_lo, w.height_hi};
   k_mg_columns<<<(n2 + 127) / 128, 128, 0, cs>>>(g, is_lines, dq, dts, dtc, ddir, line_sim_th, (const uint32_t*)dd1, n1,
-                                                 (const uint32_t*)dd2, n2, best_lr ? 1 : 0, D, dm21);
+                                                 (const uint32_t*)dd2, n2, a.best_lr, a.D, a.m21);
   PLF_LAUNCH_CHECK(ctx);
-  k_mg_rows<<<(n1 + 127) / 128, 128, 0, cs>>>(D, n1, n2, nnr, dm12);
-  PLF_LAUNCH_CHECK(ctx);
-  k_mg_mutual<<<(n1 + 127) / 128, 128, 0, cs>>>(dm12, dm21, n1, best_lr ? 1 : 0, dcount);
-  PLF_LAUNCH_CHECK(ctx);
+  if (plf_status st = mgb_rows_mutual(ctx, a, 0, 1, n1, cs)) return st;
   int cnt = 0;
-  PLF_CUDA(ctx, cudaMemcpyAsync(matches_12, dm12, (size_t)n1 * 4, cudaMemcpyDeviceToHost, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(&cnt, dcount, sizeof(int), cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(matches_12, a.m12, (size_t)n1 * 4, cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(&cnt, a.count, sizeof(int), cudaMemcpyDeviceToHost, cs));
   PLF_CUDA(ctx, cudaStreamSynchronize(cs));  // (the host vectors above are pageable: their copies completed at enqueue)
   if (n_matches) *n_matches = cnt;
   return PLF_OK;
@@ -222,7 +232,7 @@ extern "C" plf_status plf_match_grid_lines(plf_ctx* ctx, const int* q_line, cons
 //   k_mgb_columns one thread per train feature: candidate test (points: its cell inside the query's window; lines: one of
 //                 its own Bresenham cells set in the query's mask, then the direction gate), Hamming distance, exclusive
 //                 prefix-minimum down the column (best_lr_matches), dense u16 row-major matrix D
-//   k_mgb_rows / k_mgb_mutual: as k_mg_rows / k_mg_mutual
+//   k_mgb_rows / k_mgb_mutual (above)
 // D costs 2 * K * K bytes per problem, so the problems are processed in chunks that share one scratch buffer.
 #define MGB_MASK_WORDS 128   // >= cols * rows / 32 for the 64 x 48 grid (96 words)
 
@@ -253,7 +263,8 @@ __global__ void __launch_bounds__(128) k_mgb_qmask(MgbArgs a, int p0) {
 // cell further than the window from the grid contributes nothing, so the walk starts at the first step that can and
 // stops after the last one.  The state of the walk at step n is closed-form - err_n = (dx/2 - n dy) mod dx and the minor
 // coordinate advanced by (err_n - dx/2 + n dy) / dx - so the cells visited are exactly those of the full walk.  Used for
-// queries in pixel units (KF-to-KF lines), whose walk would otherwise cross thousands of cells outside the grid.
+// queries in pixel units (KF-to-KF lines), whose walk would otherwise cross thousands of cells outside the grid; on the
+// grid-unit queries of the batched front-end it takes longer than k_mgb_qmask (DESIGN.md §8).
 __global__ void __launch_bounds__(128) k_mgb_qmask_clip(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
   const int i1 = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -344,7 +355,8 @@ __global__ void __launch_bounds__(128) k_mgb_columns(MgbArgs a, int p0) {
     }
     unsigned short out = MG_NONE;
     if (cand) {
-      const int d = mg_hamming(q1 + 2 * (size_t)i1, b);
+      const uint4* qd = q1 + 2 * (size_t)i1;
+      const int d = plf_hamming256(qd[0], qd[1], b[0], b[1]);
       if (a.best_lr) {
         if (d < run) { run = d; who = i1; out = (unsigned short)d; }
       } else {
@@ -354,37 +366,6 @@ __global__ void __launch_bounds__(128) k_mgb_columns(MgbArgs a, int p0) {
     D[(size_t)i1 * a.Kt + i2] = out;
   }
   a.m21[(size_t)pl * a.Kt + i2] = who;
-}
-
-__global__ void __launch_bounds__(128) k_mgb_rows(MgbArgs a, int p0) {
-  const int pl = blockIdx.y, p = p0 + pl;
-  const int i1 = blockIdx.x * 128 + threadIdx.x;
-  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K), n2 = min(a.n2[(size_t)p * a.n2_stride], a.Kt);
-  if (i1 >= n1) return;
-  int best_d = 0x7FFFFFFF, best_d2 = 0x7FFFFFFF, best_idx = -1;
-  const unsigned short* row = a.D + (size_t)pl * a.K * a.Kt + (size_t)i1 * a.Kt;
-  for (int i2 = 0; i2 < n2; ++i2) {
-    const int d = row[i2];
-    if (d == MG_NONE) continue;
-    if (d < best_d) { best_d2 = best_d; best_d = d; best_idx = i2; }
-    else if (d < best_d2) best_d2 = d;
-  }
-  a.m12[(size_t)p * a.m12_stride + i1] = ((float)best_d < __fmul_rn((float)best_d2, a.nnr)) ? best_idx : -1;
-}
-
-__global__ void __launch_bounds__(128) k_mgb_mutual(MgbArgs a, int p0) {
-  const int pl = blockIdx.y, p = p0 + pl;
-  const int i1 = blockIdx.x * 128 + threadIdx.x;
-  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K);
-  bool ok = false;
-  if (i1 < n1) {
-    int32_t* m12 = a.m12 + (size_t)p * a.m12_stride;
-    const int i2 = m12[i1];
-    ok = i2 >= 0;
-    if (ok && a.best_lr && a.m21[(size_t)pl * a.Kt + i2] != i1) { m12[i1] = -1; ok = false; }
-  }
-  const unsigned bal = __ballot_sync(0xFFFFFFFFu, ok);
-  if ((threadIdx.x & 31) == 0 && bal) atomicAdd(&a.count[(size_t)p * a.count_stride], __popc(bal));
 }
 
 // Runs nprob windowed matching problems.  scratch: MGB scratch of the context (slot `slot`), sized here.
@@ -399,8 +380,8 @@ plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int m
   DevBufList scr;
   scr.add(a.D, nD * chunk); scr.add(a.qmask, nM * chunk); scr.add(a.m21, (size_t)Kt * chunk);
   if (plf_status st = scr.carve(ctx, slot)) return st;
-  const int gx1 = (max_n1 + 127) / 128, gx2 = (max_n2 + 127) / 128;
-  if (gx1 == 0 || gx2 == 0) return PLF_OK;
+  if (max_n1 <= 0 || max_n2 <= 0) return PLF_OK;
+  const int gx2 = (max_n2 + 127) / 128;
   for (int p0 = 0; p0 < nprob; p0 += chunk) {
     const int np = std::min(chunk, nprob - p0);
     if (a.is_lines) {
@@ -412,10 +393,7 @@ plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int m
       k_mgb_columns<0><<<dim3(gx2, np), 128, 0, cs>>>(a, p0);
     }
     PLF_LAUNCH_CHECK(ctx);
-    k_mgb_rows<<<dim3(gx1, np), 128, 0, cs>>>(a, p0);
-    PLF_LAUNCH_CHECK(ctx);
-    k_mgb_mutual<<<dim3(gx1, np), 128, 0, cs>>>(a, p0);
-    PLF_LAUNCH_CHECK(ctx);
+    if (plf_status st = mgb_rows_mutual(ctx, a, p0, np, max_n1, cs)) return st;
   }
   return PLF_OK;
 }

@@ -17,7 +17,7 @@
 //   k_select_sort    KeyPointsFilter::retainBest: per-level response threshold from the histogram (n-th largest,
 //                    ties kept), compaction, in-shared-memory bitonic sort to the canonical (octave, y, x) order
 //   k_ic_angle       intensity-centroid orientation: integer moments over the 31-px circular patch, one warp per
-//                    keypoint, cv::fastAtan2 polynomial
+//                    keypoint, cv::fastAtan2 polynomial (plf_fast_atan2, plf_internal.h)
 //   k_orb_blur7_fast 7x7 sigma-2 Gaussian in float with FMA (OpenCV takes its sepFilter2D path for the pyramid ROI), 64x32
 //                    outputs per CTA, 4 per thread
 //   k_orb_trig       (float) cos / sin of each keypoint angle, one thread per keypoint
@@ -443,28 +443,6 @@ __global__ void __launch_bounds__(1024) k_select_sort(OrbGeom g, const uint32_t*
 }
 
 // ---- orientation -------------------------------------------------------------------------------------
-// cv::fastAtan2 scalar path (degrees); unfused float ops in OpenCV's order.
-__device__ __forceinline__ float orb_fast_atan2(float y, float x) {
-  const float p1 = 0.9997878412794807f * (float)(180 / 3.14159265358979323846);
-  const float p3 = -0.3258083974640975f * (float)(180 / 3.14159265358979323846);
-  const float p5 = 0.1555786518463281f * (float)(180 / 3.14159265358979323846);
-  const float p7 = -0.04432655554792128f * (float)(180 / 3.14159265358979323846);
-  const float ax = fabsf(x), ay = fabsf(y);
-  float a, c, c2;
-  if (ax >= ay) {
-    c = __fdiv_rn(ay, __fadd_rn(ax, (float)2.2204460492503131e-16));
-    c2 = __fmul_rn(c, c);
-    a = __fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(p7, c2), p5), c2), p3), c2), p1), c);
-  } else {
-    c = __fdiv_rn(ax, __fadd_rn(ay, (float)2.2204460492503131e-16));
-    c2 = __fmul_rn(c, c);
-    a = __fsub_rn(90.f, __fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(p7, c2), p5), c2), p3), c2), p1), c));
-  }
-  if (x < 0) a = __fsub_rn(180.f, a);
-  if (y < 0) a = __fsub_rn(360.f, a);
-  return a;
-}
-
 __global__ void __launch_bounds__(256) k_ic_angle(const uint8_t* __restrict__ img0, size_t img0_stride,
                                                   const uint8_t* __restrict__ pyr, OrbGeom g,
                                                   plf_keypoint* __restrict__ kps, const short2* __restrict__ kp_lxy,
@@ -499,7 +477,7 @@ __global__ void __launch_bounds__(256) k_ic_angle(const uint8_t* __restrict__ im
     m01 += __shfl_xor_sync(0xFFFFFFFFu, m01, off);
     m10 += __shfl_xor_sync(0xFFFFFFFFu, m10, off);
   }
-  if (lane == 0) kp->angle = orb_fast_atan2((float)m01, (float)m10);
+  if (lane == 0) kp->angle = plf_fast_atan2((float)m01, (float)m10);
 }
 
 // ---- descriptor-stage blur -----------------------------------------------------------------------------

@@ -14,6 +14,7 @@
 // frame's stereo features are carried to the next call (slot 0).
 #include "plf_internal.h"
 #include "plf_geom.cuh"
+#include "plf_se3.cuh"
 #include "plf_tma.cuh"
 
 // Stereo-valid features per frame slot, [slots][cap][per]: one row per array, (name = its plf_frame_view member, element
@@ -398,11 +399,7 @@ __global__ void k_finalize(const plf_pose_result* __restrict__ gn, const int* __
       r.status = 1;
     } else {
       r.status = 0;
-      const double* T = g.T;
-      for (int i = 0; i < 3; ++i) {
-        for (int j = 0; j < 3; ++j) r.DT[4 * i + j] = T[4 * j + i];
-        r.DT[4 * i + 3] = -(T[i] * T[3] + T[4 + i] * T[7] + T[8 + i] * T[11]);
-      }
+      d_inverse_se3(g.T, r.DT);
       for (int i = 0; i < 36; ++i) r.DT_cov[i] = g.cov[i];
       r.err = g.err;
       r.n_inliers_pt = g.n_inliers_pt; r.n_inliers_ls = g.n_inliers_ls;

@@ -279,4 +279,32 @@ __device__ __forceinline__ uint32_t plf_load4_fast(const uint8_t* p) {
   const uint32_t* a = reinterpret_cast<const uint32_t*>((uintptr_t)p & ~(uintptr_t)3);
   return __funnelshift_r(__ldg(a), __ldg(a + 1), 8 * (int)((uintptr_t)p & 3));
 }
+
+// cv::fastAtan2 scalar path (degrees); unfused float ops in OpenCV's order.
+__device__ __forceinline__ float plf_fast_atan2(float y, float x) {
+  const float p1 = 0.9997878412794807f * (float)(180 / 3.14159265358979323846);
+  const float p3 = -0.3258083974640975f * (float)(180 / 3.14159265358979323846);
+  const float p5 = 0.1555786518463281f * (float)(180 / 3.14159265358979323846);
+  const float p7 = -0.04432655554792128f * (float)(180 / 3.14159265358979323846);
+  const float ax = fabsf(x), ay = fabsf(y);
+  float a, c, c2;
+  if (ax >= ay) {
+    c = __fdiv_rn(ay, __fadd_rn(ax, (float)2.2204460492503131e-16));
+    c2 = __fmul_rn(c, c);
+    a = __fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(p7, c2), p5), c2), p3), c2), p1), c);
+  } else {
+    c = __fdiv_rn(ax, __fadd_rn(ay, (float)2.2204460492503131e-16));
+    c2 = __fmul_rn(c, c);
+    a = __fsub_rn(90.f, __fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(p7, c2), p5), c2), p3), c2), p1), c));
+  }
+  if (x < 0) a = __fsub_rn(180.f, a);
+  if (y < 0) a = __fsub_rn(360.f, a);
+  return a;
+}
+
+// Hamming distance of two 256-bit descriptors, each as two uint4 halves (a0, a1) and (b0, b1).
+__device__ __forceinline__ int plf_hamming256(uint4 a0, uint4 a1, uint4 b0, uint4 b1) {
+  return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) +
+         __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
+}
 #endif

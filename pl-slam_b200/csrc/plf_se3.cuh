@@ -1,6 +1,7 @@
-// se(3) helpers shared by the pose solver (gn.cu) and the local bundle adjustment (lba.cu).  Conventions of stvo-pl's
-// auxiliar.h as used by pl-slam (SURVEY Appendix A.4; ordering x = [t; w] confirmed at src/mapHandler.cpp:3513-3514);
-// same operation order as oracle/gn.c.
+// se(3) helpers shared by the pose solver (gn.cu), the bundle adjustments (lba.cu), the keyframe matching (kfmatch.cu),
+// the batched front-end's epilogue (pipeline.cu) and the loop-closure decision (loopclosure.cu, on the host).
+// Conventions of stvo-pl's auxiliar.h as used by pl-slam (SURVEY Appendix A.4; ordering x = [t; w] confirmed at
+// src/mapHandler.cpp:3513-3514); same operation order as oracle/gn.c.
 #pragma once
 #include <math.h>
 
@@ -15,41 +16,10 @@ __device__ inline void d_mul3(const double* A, const double* B, double* C) {
       C[3 * i + j] = A[3 * i] * B[j] + A[3 * i + 1] * B[3 + j] + A[3 * i + 2] * B[6 + j];
 }
 
-// T <- T * inverse_se3(expmap_se3(x)),  x = [t; w]
-__device__ inline void d_update_pose(double* T, const double* x) {
-  double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, t[3] = {x[0], x[1], x[2]};
-  const double* w = x + 3;
-  const double theta = sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
-  if (!(theta < 0.000001)) {
-    double s[9], s2[9], V[9];
-    d_skew(w, s);
-    for (int i = 0; i < 9; ++i) s[i] /= theta;
-    d_mul3(s, s, s2);
-    const double sn = sin(theta), cs = cos(theta);
-    for (int i = 0; i < 9; ++i) {
-      const double I = (i % 4 == 0) ? 1.0 : 0.0;
-      R[i] = I + s[i] * sn + s2[i] * (1.0 - cs);
-      V[i] = I + s[i] * (1.0 - cs) / theta + s2[i] * (theta - sn) / theta;
-    }
-    const double t0 = t[0], t1 = t[1], t2 = t[2];
-    for (int i = 0; i < 3; ++i) t[i] = V[3 * i] * t0 + V[3 * i + 1] * t1 + V[3 * i + 2] * t2;
-  }
-  // E^-1 = [R^T, -R^T t]
-  double Ei[16];
-  for (int i = 0; i < 3; ++i) {
-    for (int j = 0; j < 3; ++j) Ei[4 * i + j] = R[3 * j + i];
-    Ei[4 * i + 3] = -(R[i] * t[0] + R[3 + i] * t[1] + R[6 + i] * t[2]);
-  }
-  Ei[12] = Ei[13] = Ei[14] = 0;
-  Ei[15] = 1;
-  double out[16];
-  for (int i = 0; i < 4; ++i)
-    for (int j = 0; j < 4; ++j) {
-      double a = 0;
-      for (int k = 0; k < 4; ++k) a += T[4 * i + k] * Ei[4 * k + j];
-      out[4 * i + j] = a;
-    }
-  for (int i = 0; i < 16; ++i) T[i] = out[i];
+// Q = R P + t of the row-major 4x4 T, each row summed ((r0 x + r1 y) + r2 z) + t (no contraction: --fmad=false)
+__device__ __forceinline__ void d_transform(const double* T, const double* P, double* Q) {
+#pragma unroll
+  for (int i = 0; i < 3; ++i) Q[i] = T[4 * i] * P[0] + T[4 * i + 1] * P[1] + T[4 * i + 2] * P[2] + T[4 * i + 3];
 }
 
 __device__ inline void d_logmap(const double* T, double* x) {
@@ -88,9 +58,6 @@ __device__ inline void d_logmap(const double* T, double* x) {
   x[5] = w[2];
 }
 
-// Column-pivoting Householder QR solve of the 6x6 system H x = g (Eigen ColPivHouseholderQR semantics:
-// rank-revealing, rank-deficient directions get 0).
-
 // T = expmap_se3(x) (row-major 4x4), computed directly (same operation order as oracle/gn.c orc_expmap_se3)
 __device__ inline void d_expmap(const double* x, double* T) {
   double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, t[3] = {x[0], x[1], x[2]};
@@ -117,8 +84,8 @@ __device__ inline void d_expmap(const double* x, double* T) {
   T[12] = T[13] = T[14] = 0;
   T[15] = 1;
 }
-// Ti = inverse_se3(T) = [R^T, -R^T t]
-__device__ inline void d_inverse_se3(const double* T, double* Ti) {
+// Ti = inverse_se3(T) = [R^T, -R^T t]  (Ti may be T)
+__host__ __device__ inline void d_inverse_se3(const double* T, double* Ti) {
   double out[16];
   for (int i = 0; i < 3; ++i) {
     for (int j = 0; j < 3; ++j) out[4 * i + j] = T[4 * j + i];
@@ -127,4 +94,19 @@ __device__ inline void d_inverse_se3(const double* T, double* Ti) {
   out[12] = out[13] = out[14] = 0;
   out[15] = 1;
   for (int i = 0; i < 16; ++i) Ti[i] = out[i];
+}
+
+// T <- T * inverse_se3(expmap_se3(x)),  x = [t; w]
+__device__ inline void d_update_pose(double* T, const double* x) {
+  double Ei[16];
+  d_expmap(x, Ei);
+  d_inverse_se3(Ei, Ei);
+  double out[16];
+  for (int i = 0; i < 4; ++i)
+    for (int j = 0; j < 4; ++j) {
+      double a = 0;
+      for (int k = 0; k < 4; ++k) a += T[4 * i + k] * Ei[4 * k + j];
+      out[4 * i + j] = a;
+    }
+  for (int i = 0; i < 16; ++i) T[i] = out[i];
 }
