@@ -497,7 +497,8 @@ typedef struct plf_frame_view {
   uint8_t* ldesc;      /* n_ls x 32  StereoFrame::ldesc_l */
 } plf_frame_view;
 
-/* Forget the previous frame (next batch starts with initialize(), app/plslam_dataset.cpp:115). */
+/* Forget the previous frame of every sequence (next batch starts with initialize(), app/plslam_dataset.cpp:115).  No batch
+ * may be in flight (PLF_ERR_STATE). */
 plf_status plf_reset_sequence(plf_ctx* ctx);
 
 /* Replaces B consecutive iterations of the VO part of the hot loop:
@@ -516,6 +517,22 @@ plf_status plf_process_batch(plf_ctx* ctx, int B, const uint8_t* left, const uin
 plf_status plf_batch_upload(plf_ctx* ctx, int B, const uint8_t* left, const uint8_t* right, int stride);
 plf_status plf_batch_run(plf_ctx* ctx, int B);
 plf_status plf_batch_download(plf_ctx* ctx, int B, plf_frame_result* out);
+
+/* Number of sequences a context can track at once (default 1), 1 <= n <= 2^20.  Call it before the first plf_batch_* call:
+ * PLF_ERR_STATE once the pipeline exists, PLF_ERR_INVALID for n out of range.  Each sequence keeps one carried frame slot
+ * on the device (84 * max_keypoints + 156 * max_lines + 8 bytes). */
+plf_status plf_set_max_sequences(plf_ctx* ctx, int n);
+/* plf_batch_run for pairs of several sequences.  seq[k] in [0, n) is the sequence of pair k (NULL = all 0).
+ * Pairs of one sequence appear in temporal order within the batch, and may be interleaved with other sequences in
+ * any way.  Pair k is tracked against the previous pair of seq[k] in this batch.  If there is none, it is tracked
+ * against that sequence's last pair in the most recent earlier run that contained it.
+ * restart (NULL = none): restart[k] != 0 makes pair k a first frame (status 2), like plf_reset_sequence.  So does
+ * the first pair a sequence ever has.  Restart flags are per pair, so they are valid with batches in flight; the
+ * sequence state is resolved when a batch is run.
+ * Invalid arguments return PLF_ERR_INVALID before anything is enqueued, and no sequence state changes.
+ * plf_batch_run(ctx, B) is plf_batch_run_sequences(ctx, B, NULL, NULL); plf_reset_sequence forgets every sequence's
+ * previous frame.  Results, plf_get_frame(k) and plf_get_matches(k) stay indexed by pair k of the batch. */
+plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, const uint8_t* restart);
 /* Poses of the OLDEST batch in flight, device to device: dst_device[B][16] f64 (DT, row-major) is filled on `stream`
  * (a cudaStream_t of the caller; NULL = an internal stream, synchronised before returning) behind that batch's match
  * phase - the buffer a multi-GPU caller passes to its NCCL pose all-gather on the same stream (SURVEY 8e; the reference

@@ -101,12 +101,15 @@ __global__ void __launch_bounds__(128) k_mg_columns(MgGrid g, int is_lines, cons
   m21[i2] = who;
 }
 
+// The slot of problem p's query rows and count (MgbArgs::q_slot).
+__device__ __forceinline__ size_t mgb_qslot(const MgbArgs& a, int p) { return a.q_slot ? (size_t)a.q_slot[p] : (size_t)p; }
+
 // Row and mutual passes over problems p0 .. p0 + gridDim.y - 1 (MgbArgs, plf_internal.h); D and m21 hold the problems of
 // the current chunk (pl = p - p0).
 __global__ void __launch_bounds__(128) k_mgb_rows(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
   const int i1 = blockIdx.x * 128 + threadIdx.x;
-  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K), n2 = min(a.n2[(size_t)p * a.n2_stride], a.Kt);
+  const int n1 = min(a.n1[mgb_qslot(a, p) * a.n1_stride], a.K), n2 = min(a.n2[(size_t)p * a.n2_stride], a.Kt);
   if (i1 >= n1) return;
   int best_d = 0x7FFFFFFF, best_d2 = 0x7FFFFFFF, best_idx = -1;
   const unsigned short* row = a.D + (size_t)pl * a.K * a.Kt + (size_t)i1 * a.Kt;
@@ -123,7 +126,7 @@ __global__ void __launch_bounds__(128) k_mgb_rows(MgbArgs a, int p0) {
 __global__ void __launch_bounds__(128) k_mgb_mutual(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
   const int i1 = blockIdx.x * 128 + threadIdx.x;
-  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K);
+  const int n1 = min(a.n1[mgb_qslot(a, p) * a.n1_stride], a.K);
   bool ok = false;
   if (i1 < n1) {
     int32_t* m12 = a.m12 + (size_t)p * a.m12_stride;
@@ -239,7 +242,7 @@ extern "C" plf_status plf_match_grid_lines(plf_ctx* ctx, const int* q_line, cons
 __global__ void __launch_bounds__(128) k_mgb_qmask(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
   const int i1 = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K);
+  const int n1 = min(a.n1[mgb_qslot(a, p) * a.n1_stride], a.K);
   if (i1 >= n1) return;
   uint32_t* m = a.qmask + ((size_t)pl * a.K + i1) * MGB_MASK_WORDS;
   for (int k = lane; k < MGB_MASK_WORDS; k += 32) m[k] = 0u;
@@ -268,7 +271,7 @@ __global__ void __launch_bounds__(128) k_mgb_qmask(MgbArgs a, int p0) {
 __global__ void __launch_bounds__(128) k_mgb_qmask_clip(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
   const int i1 = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K);
+  const int n1 = min(a.n1[mgb_qslot(a, p) * a.n1_stride], a.K);
   if (i1 >= n1) return;
   uint32_t* m = a.qmask + ((size_t)pl * a.K + i1) * MGB_MASK_WORDS;
   for (int k = lane; k < MGB_MASK_WORDS; k += 32) m[k] = 0u;
@@ -312,11 +315,12 @@ template <int IS_LINES>
 __global__ void __launch_bounds__(128) k_mgb_columns(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
   const int i2 = blockIdx.x * 128 + threadIdx.x;
-  const int n1 = min(a.n1[(size_t)p * a.n1_stride], a.K), n2 = min(a.n2[(size_t)p * a.n2_stride], a.Kt);
+  const size_t qs = mgb_qslot(a, p);
+  const int n1 = min(a.n1[qs * a.n1_stride], a.K), n2 = min(a.n2[(size_t)p * a.n2_stride], a.Kt);
   if (i2 >= n2) return;
   const MgGrid& g = a.g;
   const uint4* b = reinterpret_cast<const uint4*>(a.d2 + (size_t)p * a.d2_stride) + 2 * (size_t)i2;
-  const uint4* q1 = reinterpret_cast<const uint4*>(a.d1 + (size_t)p * a.d1_stride);
+  const uint4* q1 = reinterpret_cast<const uint4*>(a.d1 + qs * a.d1_stride);
   const int* tg = a.t_geo + ((size_t)p * a.Kt + i2) * (IS_LINES ? 4 : 2);
   const int* qg = a.q_geo + (size_t)p * a.K * (IS_LINES ? 4 : 2);
   unsigned short* D = a.D + (size_t)pl * a.K * a.Kt;

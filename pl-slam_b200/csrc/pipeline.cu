@@ -7,11 +7,12 @@
 // association rules restate SURVEY.md Appendix A.2/A.3 (see oracle/frontend.py, which this file must match
 // bit-for-bit on features / matches and to 1e-4 on the pose).
 //
-// One call processes B consecutive stereo pairs of ONE sequence.  Everything except the final SE(3) chaining is
-// independent per pair (extraction, stereo association) or per consecutive pair (tracking and the pose increment
-// start from identity: use_motion_model = false, config_euroc.yaml:18), so all B pairs run in the same launches:
-// images [2B][H][W] (2k = left, 2k+1 = right) -> ORB / LSD / LBD over 2B images -> per-pair kernels.  The last
-// frame's stereo features are carried to the next call (slot 0).
+// One call processes B stereo pairs of up to max_sequences sequences.  Everything except the final SE(3) chaining is
+// independent per pair (extraction, stereo association) or per pair and its previous frame of the same sequence
+// (tracking and the pose increment start from identity: use_motion_model = false, config_euroc.yaml:18), so all B
+// pairs run in the same launches: images [2B][H][W] (2k = left, 2k+1 = right) -> ORB / LSD / LBD over 2B images ->
+// per-pair kernels.  Pair k's previous frame is the slot prev[k] of the batch's sequence table; the last frame of each
+// sequence in the batch is carried to that sequence's carry slot for the next call.
 #include "plf_internal.h"
 #include "plf_geom.cuh"
 #include "plf_se3.cuh"
@@ -32,11 +33,25 @@ struct FrameSlots {
   PLF_LS_FIELDS(PLF_FS_MEMBER) int* ls_count = nullptr;
 #undef PLF_FS_MEMBER
 };
+#define PLF_FS_ONE(name, T, cap, per) +1
+constexpr int PLF_FS_NFIELDS = 0 PLF_PT_FIELDS(PLF_FS_ONE) PLF_LS_FIELDS(PLF_FS_ONE);
+#undef PLF_FS_ONE
 
 struct PipeState {
   int w = 0, h = 0, B = 0, max_kp = 0, max_ln = 0;
   int pitch = 0;               // row pitch of the device images: plf_pitch16(w) (16-byte rows: every halo tile is a legal TMA box)
-  bool has_prev = false;
+  // Sequences: frame slots 0 .. B-1 hold the pairs of the running batch, B + s carries sequence s's last frame and
+  // B + nseq is a slot whose counts stay 0, the "previous frame" of a first frame.
+  int nseq = 1;
+  std::vector<uint8_t> carried;  // [nseq] sequence s has a frame in its carry slot
+  std::vector<int> last_pair;    // [nseq] scratch of plf_batch_run_sequences: the batch's last pair of each sequence, or -1
+  // The sequence table of a batch: prev[max_batch] (slot of pair k's previous frame), then the carry list [max_batch][2]
+  // (frame slot, carry slot).  Rings indexed like h_results (up to three batches in flight): pinned h_tab, device seq_tab
+  // [3][3 max_batch].  The copy goes on the copy stream, in order behind the batch's own images and ahead of the next
+  // batch's upload; ev_tab marks it for the M phase.
+  int32_t* h_tab[3] = {nullptr, nullptr, nullptr};
+  int32_t* seq_tab = nullptr;
+  cudaEvent_t ev_tab[3] = {nullptr, nullptr, nullptr};
   uint8_t* imgs2[2] = {nullptr, nullptr};  // double-buffered [2B][h][pitch]: upload of batch i+1 overlaps the run of batch i
   uint8_t* stage = nullptr;    // dense [2B][h][w] landing buffer of the H2D copy (one contiguous DMA per side), repacked to the padded pitch on the device
   int up_slot = 0;             // slot written by the last plf_batch_upload
@@ -47,7 +62,7 @@ struct PipeState {
   PlfTmaCache lbd_tm;          // tensor maps of the LBD gradient prelude over imgs2
   short2* lbd_grad[2] = {nullptr, nullptr};  // [parity][2B][h*w]
   uint8_t* ldesc_raw = nullptr;  // [2B][max_ln][32]  LBD of every kept KeyLine
-  FrameSlots fs;               // B+1 slots
+  FrameSlots fs;               // B + nseq + 1 slots
   // matching scratch
   uint32_t* knn_keys = nullptr;   // [B][8][2][max_kp]
   int32_t* m12 = nullptr;         // [B][4][max_kp]  stereo pts, stereo lines, f2f pts, f2f lines
@@ -94,7 +109,8 @@ struct PipeState {
 
 // The device buffers of the pipeline for B pairs of K keypoints / Ln lines per image.
 static void pipe_buffers(PipeState* s, bool windowed, DevBufList& b) {
-  const size_t B = s->B, K = s->max_kp, Ln = s->max_ln, A = (size_t)s->w * s->h, AP = (size_t)s->pitch * s->h, S = B + 1;
+  const size_t B = s->B, K = s->max_kp, Ln = s->max_ln, A = (size_t)s->w * s->h, AP = (size_t)s->pitch * s->h;
+  const size_t S = B + s->nseq + 1;   // frame slots, carry slots, the empty slot
   b.add(s->imgs2[0], 2 * B * AP);
   b.add(s->imgs2[1], 2 * B * AP);
   if (s->pitch != s->w) b.add(s->stage, 2 * B * A);
@@ -118,6 +134,7 @@ static void pipe_buffers(PipeState* s, bool windowed, DevBufList& b) {
   b.add(s->gn_sP, B * Ln * 3); b.add(s->gn_eP, B * Ln * 3); b.add(s->gn_le, B * Ln * 3); b.add(s->gnInlL, B * Ln); b.add(s->gnNl, B);
   b.add(s->gn_probs, B); b.add(s->gn_out, B); b.add(s->results, 3 * B);
   b.add(s->d_ovf, 6);
+  b.add(s->seq_tab, 3 * 3 * B);
   if (windowed) {
     for (int kind = 0; kind < 4; ++kind) {   // points: 2 cells per feature, lines: 2 end points
       b.add(s->mg_q[kind], B * (kind & 1 ? Ln * 4 : K * 2));
@@ -137,7 +154,7 @@ static std::vector<PipeEvents> pipe_events(PipeState* s) {
   return {{s->ev_up, 2, cudaEventDisableTiming}, {s->ev_free, 2, cudaEventDisableTiming}, {s->ev_free2, 2, cudaEventDisableTiming},
           {s->evM, 3, cudaEventBlockingSync},    {s->tM0, 3, cudaEventDefault},           {s->evE, 2, cudaEventDefault},
           {s->evG, 2, cudaEventDefault},         {s->evX, 2, cudaEventDisableTiming},     {s->evP, 2, cudaEventDisableTiming},
-          {s->tE0, 2, cudaEventDefault},         {s->tG0, 2, cudaEventDefault}};
+          {s->tE0, 2, cudaEventDefault},         {s->tG0, 2, cudaEventDefault},           {s->ev_tab, 3, cudaEventDisableTiming}};
 }
 
 extern "C" void plf_pipe_free(plf_ctx* ctx) {
@@ -149,6 +166,7 @@ extern "C" void plf_pipe_free(plf_ctx* ctx) {
   for (int i = 0; i < 3; ++i) {
     if (s->h_results[i]) cudaFreeHost(s->h_results[i]);
     if (s->h_ovf[i]) cudaFreeHost(s->h_ovf[i]);
+    if (s->h_tab[i]) cudaFreeHost(s->h_tab[i]);
   }
   for (const PipeEvents& a : pipe_events(s))
     for (int i = 0; i < a.n; ++i)
@@ -191,11 +209,11 @@ __device__ __forceinline__ int block_scan_flags(bool flag, int* s_scan, int* s_t
 __global__ void __launch_bounds__(1024) k_stereo_points(const plf_keypoint* __restrict__ kps, const uint8_t* __restrict__ desc,
                                                          const int* __restrict__ kp_count, int max_kp,
                                                          const int32_t* __restrict__ m12_all, int m12_stride, StereoPrm prm,
-                                                         FrameSlots fs, int slot0) {
+                                                         FrameSlots fs) {
   __shared__ int s_scan[1024];
   __shared__ int s_total;
   const int k = blockIdx.x, tid = threadIdx.x;
-  const int il = 2 * k, ir = 2 * k + 1, slot = slot0 + k;
+  const int il = 2 * k, ir = 2 * k + 1, slot = k;
   const plf_keypoint* kl = kps + (size_t)il * max_kp;
   const plf_keypoint* kr = kps + (size_t)ir * max_kp;
   const int32_t* m12 = m12_all + (size_t)k * m12_stride;
@@ -256,11 +274,11 @@ __device__ __forceinline__ double line_overlap_stereo(double spl_obs, double epl
 __global__ void __launch_bounds__(1024) k_stereo_lines(const plf_keyline* __restrict__ kls, const uint8_t* __restrict__ ldesc,
                                                         const int* __restrict__ nlines, int max_ln,
                                                         const int32_t* __restrict__ m12_all, int m12_stride, StereoPrm prm,
-                                                        FrameSlots fs, int slot0) {
+                                                        FrameSlots fs) {
   __shared__ int s_scan[1024];
   __shared__ int s_total;
   const int k = blockIdx.x, tid = threadIdx.x;
-  const int il = 2 * k, ir = 2 * k + 1, slot = slot0 + k;
+  const int il = 2 * k, ir = 2 * k + 1, slot = k;
   const plf_keyline* L = kls + (size_t)il * max_ln;
   const plf_keyline* R = kls + (size_t)ir * max_ln;
   const int32_t* m12 = m12_all + (size_t)k * m12_stride;
@@ -316,8 +334,57 @@ __global__ void __launch_bounds__(1024) k_stereo_lines(const plf_keyline* __rest
   if (tid == 0) fs.ls_count[slot] = base;
 }
 
-// f2fTracking: gather the matched rows into the GN problem of pair k (prev slot = slot0+k-1 ... see host code)
-__global__ void __launch_bounds__(1024) k_f2f_build(FrameSlots fs, int prev_slot0, int max_kp, int max_ln,
+// f2fTracking problems of pair k: the previous frame (slot prev[k]) against the current one (slot k), 2-NN both ways
+// for points and lines, then the mutual NNR check; the forward best / second keys of problem kind c (4 = points,
+// 6 = lines) and the reverse ones (c + 1) live in the pair's knn_keys rows.
+__global__ void k_f2f_problems(FrameSlots fs, const int* __restrict__ prev, int B, int K, int Ln, uint32_t* __restrict__ knn_keys,
+                               int32_t* __restrict__ m12, int* __restrict__ mcount, float nnr_p, float nnr_l, int best_lr,
+                               KnnProblem* __restrict__ kf, NnrProblem* __restrict__ nf) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= B) return;
+  const int ps = prev[k], cs = k;
+  auto key = [&](int prob, int which) { return knn_keys + (((size_t)k * 8 + prob) * 2 + which) * K; };
+  const uint32_t* pp = (const uint32_t*)(fs.pdesc + (size_t)ps * K * 32);
+  const uint32_t* pc = (const uint32_t*)(fs.pdesc + (size_t)cs * K * 32);
+  const uint32_t* lp = (const uint32_t*)(fs.ldesc + (size_t)ps * Ln * 32);
+  const uint32_t* lc = (const uint32_t*)(fs.ldesc + (size_t)cs * Ln * 32);
+  const int *np = fs.pt_count + ps, *nc = fs.pt_count + cs, *lnp = fs.ls_count + ps, *lnc = fs.ls_count + cs;
+  kf[4 * k + 0] = KnnProblem{pp, pc, np, nc, 0, 0, key(4, 0), key(4, 1), nullptr};
+  kf[4 * k + 1] = KnnProblem{pc, pp, nc, np, 0, 0, key(5, 0), key(5, 1), nullptr};
+  kf[4 * k + 2] = KnnProblem{lp, lc, lnp, lnc, 0, 0, key(6, 0), key(6, 1), nullptr};
+  kf[4 * k + 3] = KnnProblem{lc, lp, lnc, lnp, 0, 0, key(7, 0), key(7, 1), nullptr};
+  nf[2 * k + 0] = NnrProblem{key(4, 0), key(4, 1), key(5, 0), key(5, 1), np, nc, 0, 0, nnr_p, best_lr, m12 + ((size_t)k * 4 + 2) * K,
+                             mcount + 4 * k + 2};
+  nf[2 * k + 1] = NnrProblem{key(6, 0), key(6, 1), key(7, 0), key(7, 1), lnp, lnc, 0, 0, nnr_l, best_lr, m12 + ((size_t)k * 4 + 3) * K,
+                             mcount + 4 * k + 3};
+}
+
+// Copies `rows` rows of row_bytes (a multiple of 4) from slot `from` to slot `to` of an array of `cap` rows per slot.
+__device__ __forceinline__ void carry_rows(void* base, size_t row_bytes, size_t cap, int from, int to, int rows) {
+  const uint32_t* src = reinterpret_cast<const uint32_t*>(static_cast<const uint8_t*>(base) + (size_t)from * cap * row_bytes);
+  uint32_t* dst = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(base) + (size_t)to * cap * row_bytes);
+  const size_t words = (size_t)rows * row_bytes / 4;
+  for (size_t i = threadIdx.x; i < words; i += blockDim.x) dst[i] = src[i];
+}
+
+// Carries the batch's last frame of each sequence to its carry slot: block (field, j) copies the stereo-valid rows of one
+// FrameSlots array for carry[j] = (frame slot, carry slot); the counts go with the first field.
+__global__ void __launch_bounds__(256) k_carry(FrameSlots fs, const int* __restrict__ carry, int K, int Ln) {
+  const int from = carry[2 * blockIdx.y], to = carry[2 * blockIdx.y + 1];
+  const int np = fs.pt_count[from], nl = fs.ls_count[from];
+  const int field = blockIdx.x;
+  if (field == 0 && threadIdx.x == 0) { fs.pt_count[to] = np; fs.ls_count[to] = nl; }
+  int f = 0;
+#define PLF_PT_CARRY(name, T, cap, per) if (field == f++) carry_rows(fs.name, sizeof(T) * (per), (size_t)(cap), from, to, min(np, cap));
+#define PLF_LS_CARRY(name, T, cap, per) if (field == f++) carry_rows(fs.name, sizeof(T) * (per), (size_t)(cap), from, to, min(nl, cap));
+  PLF_PT_FIELDS(PLF_PT_CARRY)
+  PLF_LS_FIELDS(PLF_LS_CARRY)
+#undef PLF_LS_CARRY
+#undef PLF_PT_CARRY
+}
+
+// f2fTracking: gather the matched rows into the GN problem of pair k (previous frame: slot prev[k], current: slot k)
+__global__ void __launch_bounds__(1024) k_f2f_build(FrameSlots fs, const int* __restrict__ prev, int max_kp, int max_ln,
                                                     const int32_t* __restrict__ m_pt_all, const int32_t* __restrict__ m_ls_all,
                                                     int m_stride, double* __restrict__ gnP, double* __restrict__ gnObs,
                                                     uint8_t* __restrict__ gnInlP, int* __restrict__ gnNp,
@@ -327,7 +394,7 @@ __global__ void __launch_bounds__(1024) k_f2f_build(FrameSlots fs, int prev_slot
   __shared__ int s_scan[1024];
   __shared__ int s_total;
   const int k = blockIdx.x, tid = threadIdx.x;
-  const int ps = prev_slot0 + k, cs = ps + 1;
+  const int ps = prev[k], cs = k;
   {  // points
     const int32_t* m = m_pt_all + (size_t)k * m_stride;
     const int n = min(fs.pt_count[ps], max_kp);
@@ -376,10 +443,12 @@ __global__ void __launch_bounds__(1024) k_f2f_build(FrameSlots fs, int prev_slot
   }
 }
 
-// optimizePose epilogue: curr.DT = inverse_se3(T_inc); identity when there were too few correspondences
+// optimizePose epilogue: curr.DT = inverse_se3(T_inc); identity when there were too few correspondences; a pair whose
+// previous frame is the empty slot is a first frame (initialize())
 __global__ void k_finalize(const plf_pose_result* __restrict__ gn, const int* __restrict__ gnNp, const int* __restrict__ gnNl,
-                           const int* __restrict__ kp_count, const int* __restrict__ nlines, FrameSlots fs, int slot0,
-                           int min_features, int first_is_init, int B, plf_frame_result* __restrict__ out) {
+                           const int* __restrict__ kp_count, const int* __restrict__ nlines, FrameSlots fs,
+                           const int* __restrict__ prev, int empty_slot, int min_features, int B,
+                           plf_frame_result* __restrict__ out) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= B) return;
   plf_frame_result r;
@@ -388,9 +457,9 @@ __global__ void k_finalize(const plf_pose_result* __restrict__ gn, const int* __
   r.err = -1.0;
   r.n_kp_l = kp_count[2 * k]; r.n_kp_r = kp_count[2 * k + 1];
   r.n_lines_l = nlines[2 * k]; r.n_lines_r = nlines[2 * k + 1];
-  r.n_stereo_pt = fs.pt_count[slot0 + k]; r.n_stereo_ls = fs.ls_count[slot0 + k];
+  r.n_stereo_pt = fs.pt_count[k]; r.n_stereo_ls = fs.ls_count[k];
   r.n_matched_pt = r.n_matched_ls = r.n_inliers_pt = r.n_inliers_ls = r.iters1 = r.iters2 = 0;
-  if (k == 0 && first_is_init) {
+  if (prev[k] == empty_slot) {
     r.status = 2;
   } else {
     const plf_pose_result& g = gn[k];
@@ -437,13 +506,13 @@ __global__ void __launch_bounds__(256) k_mg_geom_stereo(const plf_keypoint* __re
   }
 }
 
-// frame-to-frame: queries = the previous frame's 3-D features projected with DT = identity (slot k), train = the
-// current frame's image features (slot k+1)
-__global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, int K, int Ln, StereoPrm c, double iw, double ih,
-                                                     int* __restrict__ qp, int* __restrict__ tp, int* __restrict__ ql,
-                                                     int* __restrict__ tl, double* __restrict__ tdir) {
+// frame-to-frame: queries = the previous frame's 3-D features projected with DT = identity (slot prev[k]), train = the
+// current frame's image features (slot k)
+__global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, const int* __restrict__ prev, int K, int Ln, StereoPrm c,
+                                                     double iw, double ih, int* __restrict__ qp, int* __restrict__ tp,
+                                                     int* __restrict__ ql, int* __restrict__ tl, double* __restrict__ tdir) {
   const int k = blockIdx.y, i = blockIdx.x * 256 + threadIdx.x;
-  const int ps = k, cs = k + 1;
+  const int ps = prev[k], cs = k;
   if (i < min(fs.pt_count[ps], K)) {
     const double* P = fs.pt_P + 3 * ((size_t)ps * K + i);
     const double2 u = plf_project(c.fx, c.fy, c.cx, c.cy, P[0], P[1], P[2]);
@@ -470,10 +539,10 @@ __global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, int K, int L
 // src/mapHandler.cpp:274-278 / :421-425: keep the windowed result unless both frames hold more than `kmin` features and
 // fewer than `kmin` matches survived - then the brute-force match() result (already in m12) stands.
 __global__ void __launch_bounds__(256) k_mg_select(const int32_t* __restrict__ m12g, const int* __restrict__ mgcount,
-                                                   const int* __restrict__ cnt, int cap, int K, int which, int kmin,
-                                                   int32_t* __restrict__ m12) {
+                                                   const int* __restrict__ cnt, const int* __restrict__ prev, int cap, int K,
+                                                   int which, int kmin, int32_t* __restrict__ m12) {
   const int k = blockIdx.y, i = blockIdx.x * 256 + threadIdx.x;
-  const int n1 = min(cnt[k], cap), n2 = min(cnt[k + 1], cap);
+  const int n1 = min(cnt[prev[k]], cap), n2 = min(cnt[k], cap);
   if (i >= n1) return;
   const bool fall_back = n2 > kmin && n1 > kmin && mgcount[2 * k + which] < kmin;
   if (!fall_back) m12[((size_t)k * 4 + 2 + which) * K + i] = m12g[((size_t)k * 2 + which) * K + i];
@@ -504,6 +573,9 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
     return plf_fail(ctx, PLF_ERR_INVALID, "limits: need max_lines <= max_keypoints <= 65535 (got %d, %d)", Ln, K);
   s->w = w; s->h = h; s->B = B; s->max_kp = K; s->max_ln = Ln;
   s->pitch = plf_pitch16(w);
+  s->nseq = ctx->max_sequences;
+  s->carried.assign(s->nseq, 0);
+  s->last_pair.assign(s->nseq, -1);
   const plf_params& P = ctx->params;
   pipe_buffers(s, P.matching_strategy != 0, s->bufs);
   plf_status st = s->bufs.alloc(ctx, "pipeline");
@@ -514,23 +586,26 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
   for (int i = 0; i < 3; ++i) {
     PLF_CUDA(ctx, cudaHostAlloc(&s->h_results[i], sizeof(plf_frame_result) * B, cudaHostAllocDefault));
     PLF_CUDA(ctx, cudaHostAlloc(&s->h_ovf[i], 2 * sizeof(int), cudaHostAllocDefault));
+    PLF_CUDA(ctx, cudaHostAlloc(&s->h_tab[i], 3 * sizeof(int32_t) * B, cudaHostAllocDefault));
   }
   FrameSlots& f = s->fs;
   cudaStream_t cs = ctx->stream;
-  PLF_CUDA(ctx, cudaMemsetAsync(f.pt_count, 0, (B + 1) * sizeof(int), cs));
-  PLF_CUDA(ctx, cudaMemsetAsync(f.ls_count, 0, (B + 1) * sizeof(int), cs));
+  const size_t nslots = (size_t)B + s->nseq + 1;   // the empty slot's counts stay 0 from here on
+  PLF_CUDA(ctx, cudaMemsetAsync(f.pt_count, 0, nslots * sizeof(int), cs));
+  PLF_CUDA(ctx, cudaMemsetAsync(f.ls_count, 0, nslots * sizeof(int), cs));
   // sub-systems sized for 2B images; the LSD tables come first, so that the parity decision sees the memory they take
   if ((st = plf_orb_create(ctx, w, h, 2 * B, true, &s->orb))) return st;
   if ((st = plf_lsd_tables(ctx))) return st;
   s->lsd2 = lsd_want_two_parities(ctx, w, h, 2 * B);
   if ((st = plf_lsd_create(ctx, w, h, 2 * B, s->lsd2, &s->lsd))) return st;
   // static problem descriptors over the pipeline's own buffers (pointers never change; counts are read on the device):
-  // the stereo problems read the match phase's copies of the extraction outputs
+  // the stereo problems read the match phase's copies of the extraction outputs.  The frame-to-frame problems depend on
+  // the batch's sequence table and are built on the device per batch (k_f2f_problems).
   const int* kcnt = s->kcntM;
   const int* lcnt = s->lcntM;
   const int best_lr = P.best_lr_matches ? 1 : 0;
-  std::vector<KnnProblem> ks(B * 4), kf(B * 4);
-  std::vector<NnrProblem> ns(B * 2), nf(B * 2);
+  std::vector<KnnProblem> ks(B * 4);
+  std::vector<NnrProblem> ns(B * 2);
   std::vector<GnProblem> gp(B);
   for (int k = 0; k < B; ++k) {
     auto key = [&](int prob, int which) { return s->knn_keys + (((size_t)k * 8 + prob) * 2 + which) * K; };
@@ -546,25 +621,12 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
     ks[2 * B + 2 * k + 1] = {lr, ll, s->rev_count + 2 * k + 1, lcnt + 2 * k, 0, 0, key(3, 0), key(3, 1), s->rev_list + (size_t)(2 * k + 1) * K};
     ns[2 * k + 0] = {key(0, 0), key(0, 1), key(1, 0), key(1, 1), kcnt + 2 * k, kcnt + 2 * k + 1, 0, 0, P.min_ratio_12_p, best_lr, m12(0), s->mcount + 4 * k + 0};
     ns[2 * k + 1] = {key(2, 0), key(2, 1), key(3, 0), key(3, 1), lcnt + 2 * k, lcnt + 2 * k + 1, 0, 0, P.min_ratio_12_l, best_lr, m12(1), s->mcount + 4 * k + 1};
-    // f2f: prev slot k, curr slot k+1
-    const uint32_t* pp = (const uint32_t*)(f.pdesc + (size_t)k * K * 32);
-    const uint32_t* pc = (const uint32_t*)(f.pdesc + (size_t)(k + 1) * K * 32);
-    const uint32_t* lp = (const uint32_t*)(f.ldesc + (size_t)k * Ln * 32);
-    const uint32_t* lc = (const uint32_t*)(f.ldesc + (size_t)(k + 1) * Ln * 32);
-    kf[4 * k + 0] = {pp, pc, f.pt_count + k, f.pt_count + k + 1, 0, 0, key(4, 0), key(4, 1)};
-    kf[4 * k + 1] = {pc, pp, f.pt_count + k + 1, f.pt_count + k, 0, 0, key(5, 0), key(5, 1)};
-    kf[4 * k + 2] = {lp, lc, f.ls_count + k, f.ls_count + k + 1, 0, 0, key(6, 0), key(6, 1)};
-    kf[4 * k + 3] = {lc, lp, f.ls_count + k + 1, f.ls_count + k, 0, 0, key(7, 0), key(7, 1)};
-    nf[2 * k + 0] = {key(4, 0), key(4, 1), key(5, 0), key(5, 1), f.pt_count + k, f.pt_count + k + 1, 0, 0, P.min_ratio_12_p, best_lr, m12(2), s->mcount + 4 * k + 2};
-    nf[2 * k + 1] = {key(6, 0), key(6, 1), key(7, 0), key(7, 1), f.ls_count + k, f.ls_count + k + 1, 0, 0, P.min_ratio_12_l, best_lr, m12(3), s->mcount + 4 * k + 3};
-    gp[k] = {s->gnP + (size_t)k * K * 3, s->gnObs + (size_t)k * K * 2, s->gnInlP + (size_t)k * K, s->gnNp + k, 0,
+    gp[k] ={s->gnP + (size_t)k * K * 3, s->gnObs + (size_t)k * K * 2, s->gnInlP + (size_t)k * K, s->gnNp + k, 0,
              s->gn_sP + (size_t)k * Ln * 3, s->gn_eP + (size_t)k * Ln * 3, s->gn_le + (size_t)k * Ln * 3,
              s->gnInlL + (size_t)k * Ln, s->gnNl + k, 0, nullptr, s->gn_out + k};
   }
   PLF_CUDA(ctx, cudaMemcpyAsync(s->knn_stereo, ks.data(), ks.size() * sizeof(KnnProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->nnr_stereo, ns.data(), ns.size() * sizeof(NnrProblem), cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->knn_f2f, kf.data(), kf.size() * sizeof(KnnProblem), cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->nnr_f2f, nf.data(), nf.size() * sizeof(NnrProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->gn_probs, gp.data(), gp.size() * sizeof(GnProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaStreamSynchronize(cs));
   return PLF_OK;
@@ -578,22 +640,10 @@ static plf_status pipe_prepare(plf_ctx* ctx) {
   return st;
 }
 
-static plf_status copy_slot(plf_ctx* ctx, PipeState* s, int from, int to) {
-  FrameSlots& f = s->fs;
-  const size_t K = s->max_kp, Ln = s->max_ln;
-  cudaStream_t cs = ctx->stream;
-#define CP(ptr, per) PLF_CUDA(ctx, cudaMemcpyAsync((ptr) + (size_t)to * (per), (ptr) + (size_t)from * (per), (per) * sizeof(*(ptr)), cudaMemcpyDeviceToDevice, cs));
-#define PLF_FS_COPY(name, T, cap, per) CP(f.name, cap * per)
-  PLF_PT_FIELDS(PLF_FS_COPY) CP(f.pt_count, 1)
-  PLF_LS_FIELDS(PLF_FS_COPY) CP(f.ls_count, 1)
-#undef PLF_FS_COPY
-#undef CP
-  return PLF_OK;
-}
-
 // One plf_batch_run call: its pairs, buffer parities and slots, and the streams of its phases.
 struct BatchRun {
   int B;
+  int ncarry;    // entries of the carry list in h_tab[rp]: the sequences the batch holds
   int par;       // parity of the E -> G -> M hand-off buffers
   int lp;        // parity of the LSD hand-off buffers (0 when they exist once)
   int rp;        // slot of the result ring
@@ -653,18 +703,20 @@ static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
 }
 
 // One windowed-matching launch over B problems of one kind (points: cap = K, lines: cap = Ln).  Problem p matches the
-// descriptor rows of image / slot p * step of `desc` (n1[p * step] of them) against those of the next image / slot.
-static MgbArgs mgb_args(const plf_params& P, MgGrid g, bool lines, int cap, int step, const int* q_geo, const int* t_geo,
-                        const double* t_dir, const uint8_t* desc, const int* cnt, int32_t* m12, size_t m12_stride, int* count,
-                        int count_stride) {
+// descriptor rows of image / slot q_slot[p] * step of `desc` (p * step without q_slot; cnt[...] of them) against those of
+// image / slot p * step + t_off.
+static MgbArgs mgb_args(const plf_params& P, MgGrid g, bool lines, int cap, int step, const int* q_slot, int t_off,
+                        const int* q_geo, const int* t_geo, const double* t_dir, const uint8_t* desc, const int* cnt,
+                        int32_t* m12, size_t m12_stride, int* count, int count_stride) {
   MgbArgs a = {};
   a.g = g;
   a.is_lines = lines ? 1 : 0; a.K = a.Kt = cap; a.best_lr = P.best_lr_matches ? 1 : 0;
   a.nnr = lines ? P.min_ratio_12_l : P.min_ratio_12_p;
   a.line_sim_th = (double)P.line_sim_th;
   a.q_geo = q_geo; a.t_geo = t_geo; a.t_dir = t_dir;
-  a.d1 = desc; a.d2 = desc + (size_t)cap * 32; a.d1_stride = a.d2_stride = (size_t)step * cap * 32;
-  a.n1 = cnt; a.n2 = cnt + 1; a.n1_stride = a.n2_stride = step;
+  a.q_slot = q_slot;
+  a.d1 = desc; a.d2 = desc + (size_t)t_off * cap * 32; a.d1_stride = a.d2_stride = (size_t)step * cap * 32;
+  a.n1 = cnt; a.n2 = cnt + t_off; a.n1_stride = a.n2_stride = step;
   a.m12 = m12; a.m12_stride = m12_stride; a.count = count; a.count_stride = count_stride;
   return a;
 }
@@ -684,10 +736,16 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->evG[par], 0));
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->evE[par], 0));
   PLF_CUDA(ctx, cudaEventRecord(s->tM0[rp], cs));
-  if (!s->has_prev) {  // initialize(): no previous frame to track against
-    PLF_CUDA(ctx, cudaMemsetAsync(s->fs.pt_count, 0, sizeof(int), cs));
-    PLF_CUDA(ctx, cudaMemsetAsync(s->fs.ls_count, 0, sizeof(int), cs));
-  }
+  // the batch's sequence table: prev[B], then the carry list
+  int32_t* prev = s->seq_tab + (size_t)rp * 3 * s->B;
+  int32_t* carry = prev + s->B;
+  PLF_CUDA(ctx, cudaMemcpyAsync(prev, s->h_tab[rp], sizeof(int32_t) * B, cudaMemcpyHostToDevice, s->copy));
+  PLF_CUDA(ctx, cudaMemcpyAsync(carry, s->h_tab[rp] + s->B, sizeof(int32_t) * 2 * r.ncarry, cudaMemcpyHostToDevice, s->copy));
+  PLF_CUDA(ctx, cudaEventRecord(s->ev_tab[rp], s->copy));
+  PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_tab[rp], 0));
+  k_f2f_problems<<<(B + 127) / 128, 128, 0, cs>>>(s->fs, prev, B, K, Ln, s->knn_keys, s->m12, s->mcount, P.min_ratio_12_p,
+                                                  P.min_ratio_12_l, P.best_lr_matches ? 1 : 0, s->knn_f2f, s->nnr_f2f);
+  PLF_LAUNCH_CHECK(ctx);
   if ((st = plf_launch_lbd(ctx, cs, s->lbd_grad[par], A, w, h, 2 * B, kls, lcnt, Ln, s->ldesc_raw, nullptr))) return st;
   plf_mark(ctx, cs, "lbd.k_lbd");
   // the rest of the match phase works on its own copy of the extraction outputs; evX releases this parity to batch i+2
@@ -711,10 +769,10 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
                                                                                  s->mg_t[0], s->mg_q[1], s->mg_t[1], s->mg_dir[0]);
     PLF_LAUNCH_CHECK(ctx);
     const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, P.matching_s_ws, 0, 0, 0};
-    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 2, s->mg_q[0], s->mg_t[0], nullptr, odesc, kcnt, s->m12,
-                                                        4 * (size_t)K, s->mcount, 4), B, K, K, PLF_SCR_MGB_PIPE, cs))) return st;
-    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 2, s->mg_q[1], s->mg_t[1], s->mg_dir[0], s->ldesc_raw, lcnt,
-                                                        s->m12 + K, 4 * (size_t)K, s->mcount + 1, 4), B, Ln, Ln, PLF_SCR_MGB_PIPE, cs))) return st;
+    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 2, nullptr, 1, s->mg_q[0], s->mg_t[0], nullptr, odesc, kcnt,
+                                                        s->m12, 4 * (size_t)K, s->mcount, 4), B, K, K, PLF_SCR_MGB_PIPE, cs))) return st;
+    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 2, nullptr, 1, s->mg_q[1], s->mg_t[1], s->mg_dir[0], s->ldesc_raw,
+                                                        lcnt, s->m12 + K, 4 * (size_t)K, s->mcount + 1, 4), B, Ln, Ln, PLF_SCR_MGB_PIPE, cs))) return st;
     plf_mark(ctx, cs, "stereo.k_mgb (matchGrid)");
   } else {
     // L->R 2-NN for every left feature; R->L only for the right features that are somebody's accepted best match
@@ -734,9 +792,9 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   }
   StereoPrm sp = {P.max_dist_epip, P.min_disp, P.line_horiz_th, P.stereo_overlap_th, P.ls_min_disp_ratio,
                   ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy, ctx->cam.b};
-  k_stereo_points<<<B, 1024, 0, cs>>>(kps, odesc, kcnt, K, s->m12, 4 * K, sp, s->fs, 1);
+  k_stereo_points<<<B, 1024, 0, cs>>>(kps, odesc, kcnt, K, s->m12, 4 * K, sp, s->fs);
   PLF_LAUNCH_CHECK(ctx);
-  k_stereo_lines<<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, sp, s->fs, 1);
+  k_stereo_lines<<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, sp, s->fs);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "stereo.k_stereo_points+lines");
   if ((st = plf_launch_knn2(ctx, cs, s->knn_f2f, 4 * B, std::max(K, Ln)))) return st;
@@ -746,31 +804,32 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     // frame-to-frame: matchGrid() in a +-matching_f2f_ws window around the projected feature; the match() result above
     // stands where the window search found fewer than min_pt_matches / min_ls_matches
     PLF_CUDA(ctx, cudaMemsetAsync(s->mgcount, 0, (size_t)B * 2 * sizeof(int), cs));
-    k_mg_geom_f2f<<<dim3((std::max(K, Ln) + 255) / 256, B), 256, 0, cs>>>(s->fs, K, Ln, sp, mg_iw, mg_ih, s->mg_q[2], s->mg_t[2],
-                                                                          s->mg_q[3], s->mg_t[3], s->mg_dir[1]);
+    k_mg_geom_f2f<<<dim3((std::max(K, Ln) + 255) / 256, B), 256, 0, cs>>>(s->fs, prev, K, Ln, sp, mg_iw, mg_ih, s->mg_q[2],
+                                                                          s->mg_t[2], s->mg_q[3], s->mg_t[3], s->mg_dir[1]);
     PLF_LAUNCH_CHECK(ctx);
     const int ws = P.matching_f2f_ws;
     const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, ws, ws, ws, ws};
-    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 1, s->mg_q[2], s->mg_t[2], nullptr, s->fs.pdesc, s->fs.pt_count,
-                                                        s->m12g, 2 * (size_t)K, s->mgcount, 2), B, K, K, PLF_SCR_MGB_PIPE, cs))) return st;
-    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 1, s->mg_q[3], s->mg_t[3], s->mg_dir[1], s->fs.ldesc, s->fs.ls_count,
-                                                        s->m12g + K, 2 * (size_t)K, s->mgcount + 1, 2), B, Ln, Ln, PLF_SCR_MGB_PIPE, cs))) return st;
-    k_mg_select<<<dim3((K + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.pt_count, K, K, 0, P.min_pt_matches, s->m12);
+    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 1, prev, 0, s->mg_q[2], s->mg_t[2], nullptr, s->fs.pdesc,
+                                                        s->fs.pt_count, s->m12g, 2 * (size_t)K, s->mgcount, 2), B, K, K, PLF_SCR_MGB_PIPE, cs))) return st;
+    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 1, prev, 0, s->mg_q[3], s->mg_t[3], s->mg_dir[1], s->fs.ldesc,
+                                                        s->fs.ls_count, s->m12g + K, 2 * (size_t)K, s->mgcount + 1, 2), B, Ln, Ln, PLF_SCR_MGB_PIPE, cs))) return st;
+    k_mg_select<<<dim3((K + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.pt_count, prev, K, K, 0, P.min_pt_matches, s->m12);
     PLF_LAUNCH_CHECK(ctx);
-    k_mg_select<<<dim3((Ln + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.ls_count, Ln, K, 1, P.min_ls_matches, s->m12);
+    k_mg_select<<<dim3((Ln + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.ls_count, prev, Ln, K, 1, P.min_ls_matches, s->m12);
     PLF_LAUNCH_CHECK(ctx);
     plf_mark(ctx, cs, "f2f.k_mgb (matchGrid)");
   }
-  k_f2f_build<<<B, 1024, 0, cs>>>(s->fs, 0, K, Ln, s->m12 + 2 * K, s->m12 + 3 * K, 4 * K, s->gnP, s->gnObs, s->gnInlP, s->gnNp,
+  k_f2f_build<<<B, 1024, 0, cs>>>(s->fs, prev, K, Ln, s->m12 + 2 * K, s->m12 + 3 * K, 4 * K, s->gnP, s->gnObs, s->gnInlP, s->gnNp,
                                   s->gn_sP, s->gn_eP, s->gn_le, s->gnInlL, s->gnNl);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "f2f.k_nnr_mutual+k_f2f_build");
   if ((st = plf_launch_gn(ctx, cs, s->gn_probs, B, plf_gn_opts_from_params(P)))) return st;
   plf_mark(ctx, cs, "gn.k_gn_pose");
-  k_finalize<<<(B + 127) / 128, 128, 0, cs>>>(s->gn_out, s->gnNp, s->gnNl, kcnt, lcnt, s->fs, 1, P.min_features,
-                                               s->has_prev ? 0 : 1, B, s->results + (size_t)rp * s->B);
+  k_finalize<<<(B + 127) / 128, 128, 0, cs>>>(s->gn_out, s->gnNp, s->gnNl, kcnt, lcnt, s->fs, prev, s->B + s->nseq,
+                                               P.min_features, B, s->results + (size_t)rp * s->B);
   PLF_LAUNCH_CHECK(ctx);
-  if ((st = copy_slot(ctx, s, B, 0))) return st;  // carry the last frame to the next batch
+  k_carry<<<dim3(PLF_FS_NFIELDS, r.ncarry), 256, 0, cs>>>(s->fs, carry, K, Ln);   // the next batch tracks against these
+  PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "k_finalize+carry");
   // results + overflow flags to pinned memory as part of this batch's stream work; evM marks them ready
   PLF_CUDA(ctx, cudaMemcpyAsync(s->h_results[rp], s->results + (size_t)rp * s->B, sizeof(plf_frame_result) * B, cudaMemcpyDeviceToHost, cs));
@@ -786,8 +845,17 @@ plf_status plf_reset_sequence(plf_ctx* ctx) {
   if (ctx->pipe) {
     if (ctx->pipe->n_pending)
       return plf_fail(ctx, PLF_ERR_STATE, "plf_reset_sequence: %d batch(es) still in flight; download them first", ctx->pipe->n_pending);
-    ctx->pipe->has_prev = false;
+    std::fill(ctx->pipe->carried.begin(), ctx->pipe->carried.end(), 0);
   }
+  return PLF_OK;
+}
+
+plf_status plf_set_max_sequences(plf_ctx* ctx, int n) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (n < 1 || n > PLF_MAX_SEQUENCES)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_max_sequences: n = %d, need 1 <= n <= %d", n, PLF_MAX_SEQUENCES);
+  if (ctx->pipe) return plf_fail(ctx, PLF_ERR_STATE, "plf_set_max_sequences: the pipeline exists (a batch call was made)");
+  ctx->max_sequences = n;
   return PLF_OK;
 }
 
@@ -840,8 +908,14 @@ void* plf_batch_device_images(plf_ctx* ctx) {
   return ctx->pipe->imgs2[ctx->pipe->up_slot];
 }
 
-plf_status plf_batch_run(plf_ctx* ctx, int B) {
+plf_status plf_batch_run(plf_ctx* ctx, int B) { return plf_batch_run_sequences(ctx, B, nullptr, nullptr); }
+
+plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, const uint8_t* restart) {
   if (!ctx || B < 1 || B > ctx->limits.max_batch) return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_run: bad B");
+  if (seq)
+    for (int k = 0; k < B; ++k)
+      if (seq[k] < 0 || seq[k] >= ctx->max_sequences)
+        return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_run_sequences: seq[%d] = %d outside [0, %d)", k, seq[k], ctx->max_sequences);
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   plf_status st = pipe_prepare(ctx);
   if (st) return st;
@@ -852,6 +926,26 @@ plf_status plf_batch_run(plf_ctx* ctx, int B) {
   r.B = B;
   r.par = (int)(s->seq & 1);
   r.rp = (int)(s->seq % 3);
+  // The sequence table, into the ring entry of this batch (the batch that used it last has been downloaded): pair k tracks
+  // against the batch's previous pair of its sequence, else the sequence's carried frame, else (and on a restart) nothing
+  int32_t* prev = s->h_tab[r.rp];
+  int32_t* carry = prev + s->B;
+  const int empty = s->B + s->nseq;
+  for (int k = 0; k < B; ++k) {
+    const int q = seq ? seq[k] : 0;
+    if (restart && restart[k]) prev[k] = empty;
+    else if (s->last_pair[q] >= 0) prev[k] = s->last_pair[q];
+    else prev[k] = s->carried[q] ? s->B + q : empty;
+    s->last_pair[q] = k;
+  }
+  r.ncarry = 0;
+  for (int k = 0; k < B; ++k) {
+    const int q = seq ? seq[k] : 0;
+    if (s->last_pair[q] != k) continue;
+    carry[2 * r.ncarry] = k;
+    carry[2 * r.ncarry + 1] = s->B + q;
+    r.ncarry++;
+  }
   r.run_slot = s->up_slot;
   // With profiling on everything is serialised on the main stream so that the per-kernel marks are meaningful.
   r.piped = !ctx->profile || ctx->profile_piped;
@@ -864,8 +958,12 @@ plf_status plf_batch_run(plf_ctx* ctx, int B) {
   st = run_extract(ctx, s, r);
   if (!st) st = run_lsd(ctx, s, r);
   if (!st) st = run_match(ctx, s, r);
+  for (int k = 0; k < B; ++k) {
+    const int q = seq ? seq[k] : 0;
+    s->last_pair[q] = -1;
+    if (!st) s->carried[q] = 1;
+  }
   if (st) return st;
-  s->has_prev = true;
   s->pend_slot[s->n_pending] = r.rp;
   s->pend_B[s->n_pending] = B;
   s->n_pending++;
@@ -948,7 +1046,7 @@ plf_status plf_get_frame(plf_ctx* ctx, int k, plf_frame_view* v) {
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_get_frame: bad arguments");
   PipeState* s = ctx->pipe;
   FrameSlots& f = s->fs;
-  const int slot = k + 1;
+  const int slot = k;
   const size_t K = s->max_kp, Ln = s->max_ln;
   cudaStream_t cs = ctx->stream;
   int np = 0, nl = 0;

@@ -65,6 +65,9 @@ struct StagedLayout {
   plf_status acquire(plf_ctx* ctx, plf_scratch_slot slot, uint8_t** pin, uint8_t** dev) const;
 };
 
+// Upper bound of plf_set_max_sequences: keeps every slot index of the pipeline an int.
+#define PLF_MAX_SEQUENCES (1 << 20)
+
 struct OrbState;      // orb.cu
 struct LsdState;      // lsd.cu
 struct PlfTmaCache;   // plf_tma.cuh
@@ -76,6 +79,7 @@ struct plf_ctx {
   plf_params params;
   plf_camera cam;
   plf_limits limits;
+  int max_sequences = 1;          // plf_set_max_sequences: fixed once the pipeline exists
   std::string err;
   long long launches = 0;
   // scratch slots (device) of the host-pointer operator entry points
@@ -169,9 +173,10 @@ struct MgbArgs {
   const int* q_geo;      // [P][K][2|4]  query cells (points) / integer end points in grid units (lines)
   const int* t_geo;      // [P][Kt][2|4]
   const double* t_dir;   // [P][Kt][2] (lines) unit directions of the train lines
-  const uint8_t* d1; size_t d1_stride;   // descriptor rows of problem p: d1 + p * d1_stride
-  const uint8_t* d2; size_t d2_stride;
-  const int* n1; int n1_stride;          // counts: n1[p * n1_stride]
+  const int* q_slot;     // optional [P]: problem p reads the query rows and count of slot q_slot[p] instead of slot p
+  const uint8_t* d1; size_t d1_stride;   // query descriptor rows of problem p: d1 + slot * d1_stride (slot: see q_slot)
+  const uint8_t* d2; size_t d2_stride;   // train rows: d2 + p * d2_stride
+  const int* n1; int n1_stride;          // counts: n1[slot * n1_stride], n2[p * n2_stride]
   const int* n2; int n2_stride;
   unsigned short* D;     // scratch (set by the launcher)
   uint32_t* qmask;

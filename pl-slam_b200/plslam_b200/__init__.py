@@ -308,7 +308,8 @@ class Frontend:
     (app/plslam_dataset.cpp:109) plus the free operators the reference calls on the path."""
 
     def __init__(self, params: plf_params | None = None, camera: dict | plf_camera | None = None,
-                 limits: plf_limits | None = None, device: int = 0, **overrides):
+                 limits: plf_limits | None = None, device: int = 0, max_sequences: int = 1, **overrides):
+        """max_sequences: the number of sequences batch_run / process_batch can track at once (plf_set_max_sequences)."""
         self.lib = load_library()
         self.params = params if params is not None else default_params()
         for k, v in overrides.items():
@@ -325,6 +326,12 @@ class Frontend:
                                  int(device), C.byref(self._ctx))
         if st != 0:
             raise PlfError(f"plf_create failed ({st}): {self.lib.plf_last_error(None).decode()}")
+        try:
+            self._check(self.lib.plf_set_max_sequences(self._ctx, int(max_sequences)), "plf_set_max_sequences")
+        except PlfError:
+            self.close()
+            raise
+        self.max_sequences = int(max_sequences)
 
     # -- plumbing --------------------------------------------------------------------------------
     def close(self):
@@ -739,15 +746,21 @@ class Frontend:
         assert left.shape == right.shape and left.shape[1:] == (self.camera.height, self.camera.width)
         return left, right
 
-    def process_batch(self, left, right):
-        """B x (insertStereoPair + optimizePose): left/right uint8 [B,H,W] host arrays -> list of result dicts."""
+    def process_batch(self, left, right, seq=None, restart=None):
+        """B x (insertStereoPair + optimizePose): left/right uint8 [B,H,W] host arrays -> list of result dicts.  seq /
+        restart: as batch_run."""
         left, right = self._stack(left, right)
         B = left.shape[0]
-        res = (plf_frame_result * B)()
-        st = self.lib.plf_process_batch(self._ctx, B, _ptr(left, C.c_uint8), _ptr(right, C.c_uint8),
-                                        self.camera.width, res)
-        self._check(st, "plf_process_batch")
-        return self._result_dicts(res, B)
+        if seq is None and restart is None:
+            res = (plf_frame_result * B)()
+            st = self.lib.plf_process_batch(self._ctx, B, _ptr(left, C.c_uint8), _ptr(right, C.c_uint8),
+                                            self.camera.width, res)
+            self._check(st, "plf_process_batch")
+            return self._result_dicts(res, B)
+        seq_a, restart_a = self._sequence_table(B, seq, restart)   # checked before anything is uploaded
+        self.batch_upload(left, right)
+        self._run_sequences(B, seq_a, restart_a)
+        return self.batch_download(B)
 
     def batch_upload(self, left, right):
         left, right = self._stack(left, right)
@@ -760,8 +773,30 @@ class Frontend:
         self._check(self.lib.plf_batch_upload(self._ctx, int(B), C.c_void_p(left_ptr), C.c_void_p(right_ptr),
                                               self.camera.width), "plf_batch_upload")
 
-    def batch_run(self, B):
-        self._check(self.lib.plf_batch_run(self._ctx, int(B)), "plf_batch_run")
+    @staticmethod
+    def _sequence_table(B, seq, restart):
+        """seq: integer [B] (sequence of each pair, None = all 0); restart: bool / integer [B] (None = none)."""
+        def vec(a, name, kinds):
+            a = np.asarray(a)
+            if a.shape != (B,) or a.dtype.kind not in kinds:
+                raise PlfError(f"{name} must be a 1-D {'bool or ' if 'b' in kinds else ''}integer array of {B} entries "
+                               f"(got {a.dtype}{list(a.shape)})")
+            return a
+        s = None if seq is None else np.ascontiguousarray(vec(seq, "seq", "iu"), np.int32)
+        if s is not None and not np.array_equal(s, np.asarray(seq)):
+            raise PlfError("seq: values do not fit int32")
+        r = None if restart is None else np.ascontiguousarray(vec(restart, "restart", "biu") != 0, np.uint8)
+        return s, r
+
+    def _run_sequences(self, B, seq, restart):
+        self._check(self.lib.plf_batch_run_sequences(self._ctx, int(B), None if seq is None else _ptr(seq, C.c_int32),
+                                                     None if restart is None else _ptr(restart, C.c_uint8)),
+                    "plf_batch_run_sequences")
+
+    def batch_run(self, B, seq=None, restart=None):
+        """Runs the most recent upload.  seq: the sequence of each pair (integer [B] in [0, max_sequences), None = all 0);
+        restart: per pair, nonzero makes it a first frame (None = none).  plf_batch_run_sequences."""
+        self._run_sequences(B, *self._sequence_table(B, seq, restart))
 
     def batch_download(self, B):
         res = (plf_frame_result * B)()
