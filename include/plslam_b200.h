@@ -287,7 +287,8 @@ typedef struct plf_pose_result {
  * P: np x 3 (3-D points, previous camera frame), pl_obs: np x 2 (observed pixels, current frame),
  * sP,eP: nl x 3 (3-D endpoints), le_obs: nl x 3 (observed normalised line), all f64 host arrays;
  * inlier_pt / inlier_ls: u8 flags, in (rows to use) and out (after the chi2 gate).  T_init: row-major
- * 4x4 or NULL (identity).  opts NULL => thresholds from the ctx params (stvo-pl min_error/min_error_change). */
+ * 4x4 or NULL (identity).  opts NULL => thresholds from the ctx params (stvo-pl min_error/min_error_change).
+ * Projects with the context's camera (plf_create), not a sequence's (plf_set_sequence_camera). */
 plf_status plf_gn_pose(plf_ctx* ctx, const plf_gn_opts* opts, const double* P, const double* pl_obs,
                        uint8_t* inlier_pt, int np, const double* sP, const double* eP,
                        const double* le_obs, uint8_t* inlier_ls, int nl, const double* T_init,
@@ -341,6 +342,7 @@ typedef struct plf_lba_result {
   double err;    /* last normalised weighted error */
   double lambda; /* final damping */
 } plf_lba_result;
+/* Projects with the context's camera (plf_create), not a sequence's (plf_set_sequence_camera). */
 plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* problem, plf_lba_result* out);
 
 /* Global bundle adjustment.  Replaces MapHandler::levMarquardtOptimizationGBA (src/mapHandler.cpp:2101-2699), the
@@ -363,7 +365,8 @@ plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_pr
  * Work is enqueued on plf_stream and uses scratch slot 10 (shared with plf_local_ba), which stays allocated until
  * plf_destroy: about 288 n_kf^2 bytes for the dense reduced system (1.2 GB at 2048 keyframes, 4.8 GB at 4096) plus
  * 144 bytes per observation and about 650 bytes per landmark.  Up to n_kf = 64 the reduced system is factored by one CTA as in
- * plf_local_ba; beyond, by a tiled LDL^T across the GPU that skips exactly-zero tiles. */
+ * plf_local_ba; beyond, by a tiled LDL^T across the GPU that skips exactly-zero tiles.  Projects with the context's camera,
+ * as plf_local_ba. */
 plf_status plf_global_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* problem, plf_lba_result* out);
 
 /* Loop-closure pose-graph optimisation.  Replaces the g2o call of MapHandler::loopClosureOptimizationCovGraphG2O
@@ -450,7 +453,8 @@ typedef struct plf_lc_result {
   double x_inc[6];     /* logmap_se3(T_inc) */
   double pose_inc[6];  /* accepted only */
 } plf_lc_result;
-/* pt_pairs / ls_pairs: (i1 in kf0, i2 in kf1) per surviving correspondence, capacity cap_* pairs (may be NULL). */
+/* pt_pairs / ls_pairs: (i1 in kf0, i2 in kf1) per surviving correspondence, capacity cap_* pairs (may be NULL).
+ * Uses the context's camera (plf_create), not a sequence's (plf_set_sequence_camera). */
 plf_status plf_loop_closure_pose(plf_ctx* ctx, const plf_lc_params* lc, const plf_lc_keyframe* kf0,
                                  const plf_lc_keyframe* kf1, plf_lc_result* out, int32_t* pt_pairs, int cap_pt,
                                  int32_t* ls_pairs, int cap_ls);
@@ -533,6 +537,23 @@ plf_status plf_set_max_sequences(plf_ctx* ctx, int n);
  * plf_batch_run(ctx, B) is plf_batch_run_sequences(ctx, B, NULL, NULL); plf_reset_sequence forgets every sequence's
  * previous frame.  Results, plf_get_frame(k) and plf_get_matches(k) stay indexed by pair k of the batch. */
 plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, const uint8_t* restart);
+/* The calibration of sequence s, 0 <= s < n (plf_set_max_sequences).  The sequences of one context may differ in fx, fy,
+ * cx, cy and b; they share the image size, the parameters and the limits.  cam == NULL returns s to the context's camera
+ * (plf_create).  cam->width and cam->height must equal the context's; fx, fy and b must be finite and > 0; cx and cy must
+ * be finite.  Anything else returns PLF_ERR_INVALID, naming the field, and changes nothing.  The call may be made at any
+ * time: before or after the pipeline exists, and with batches in flight.
+ *   - The camera is resolved when a batch is run, like restart flags and sequence state.  Batches already run keep the
+ *     calibration they were run with; the next plf_batch_run_sequences that holds s uses the new one, for every pair of
+ *     s in that batch.
+ *   - A successful call restarts s, even with NULL or unchanged values: the first pair of s in the next run that holds
+ *     it is a first frame (status 2), since its carried frame was triangulated with another camera.
+ *   - plf_set_max_sequences drops every sequence's camera; plf_reset_sequence keeps them.
+ *   - plf_batch_run and plf_process_batch run sequence 0, so they use sequence 0's camera.
+ * The keyframe and back-end operators (plf_match_kf2kf, plf_match_map2kf, plf_loop_closure_pose, plf_gn_pose,
+ * plf_local_ba, plf_global_ba) keep using the context's camera. */
+plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam);
+/* The calibration the next batch will use for sequence s: its own, or the context's camera. */
+plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out);
 /* Poses of the OLDEST batch in flight, device to device: dst_device[B][16] f64 (DT, row-major) is filled on `stream`
  * (a cudaStream_t of the caller; NULL = an internal stream, synchronised before returning) behind that batch's match
  * phase - the buffer a multi-GPU caller passes to its NCCL pose all-gather on the same stream (SURVEY 8e; the reference
@@ -568,8 +589,9 @@ plf_status plf_get_matches(plf_ctx* ctx, int k, plf_match_view* view);
  * window, the match() fallback and the epipolar gate.  The landmark bookkeeping that follows each (new MapPoint / MapLine,
  * observations, full_graph) stays with the caller.  has_points / has_lines, best_lr_matches, matching_f2f_ws,
  * min_pt_matches / min_ls_matches, min_ratio_12_p / min_ratio_12_l, line_sim_th and the camera come from the ctx (SlamConfig
- * inherits them).  Work is enqueued on plf_stream, so a call between batches in flight is safe.  A kind returns 0 (every
- * entry -1) when it is disabled or the keyframe has no stereo features of it.  Semantics reproduced as written, quirks
+ * inherits them): the context's camera of plf_create, not a sequence's (plf_set_sequence_camera).  Work is enqueued on
+ * plf_stream, so a call between batches in flight is safe.  A kind returns 0 (every entry -1) when it is disabled or the
+ * keyframe has no stereo features of it.  Semantics reproduced as written, quirks
  * included (DESIGN.md 8): see oracle/kfmatching.py. */
 typedef struct plf_kf_match_opts {
   int fast_matching;    /* SlamConfig::fastMatching  src/slamConfig.cpp:43: 0 = brute-force match() only, and only when

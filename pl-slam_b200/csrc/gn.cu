@@ -179,9 +179,15 @@ __device__ void d_inverse6(const double* Ain, double* I) {
   }
 }
 
-__global__ void __launch_bounds__(GN_THREADS) k_gn_pose(const GnProblem* __restrict__ probs, GnCam cam,
-                                                         plf_gn_opts o) {
+// cams: optional per-problem cameras (a batch of several calibrations); null = launch_cam for every problem.
+__global__ void __launch_bounds__(GN_THREADS) k_gn_pose(const GnProblem* __restrict__ probs, GnCam launch_cam,
+                                                         const PlfPairCam* __restrict__ cams, plf_gn_opts o) {
   const GnProblem P = probs[blockIdx.x];
+  GnCam cam = launch_cam;
+  if (cams) {
+    const PlfPairCam q = cams[blockIdx.x];
+    cam = GnCam{q.fx, q.fy, q.cx, q.cy};
+  }
   const int np = P.np_ptr ? *P.np_ptr : P.np;
   const int nl = P.nl_ptr ? *P.nl_ptr : P.nl;
   __shared__ double sT[16];
@@ -341,10 +347,11 @@ plf_gn_opts plf_gn_opts_from_params(const plf_params& p) {
   return o;
 }
 
-plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs, int nprob, const plf_gn_opts& o) {
+plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs, int nprob, const plf_gn_opts& o,
+                         const PlfPairCam* d_cams) {
   if (nprob <= 0) return PLF_OK;
   GnCam c = {ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy};
-  k_gn_pose<<<nprob, GN_THREADS, 0, cs>>>(d_probs, c, o);
+  k_gn_pose<<<nprob, GN_THREADS, 0, cs>>>(d_probs, c, d_cams, o);
   PLF_LAUNCH_CHECK(ctx);
   return PLF_OK;
 }

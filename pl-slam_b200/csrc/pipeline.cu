@@ -13,6 +13,8 @@
 // pairs run in the same launches: images [2B][H][W] (2k = left, 2k+1 = right) -> ORB / LSD / LBD over 2B images ->
 // per-pair kernels.  Pair k's previous frame is the slot prev[k] of the batch's sequence table; the last frame of each
 // sequence in the batch is carried to that sequence's carry slot for the next call.
+#include <cmath>
+
 #include "plf_internal.h"
 #include "plf_geom.cuh"
 #include "plf_se3.cuh"
@@ -52,6 +54,11 @@ struct PipeState {
   int32_t* h_tab[3] = {nullptr, nullptr, nullptr};
   int32_t* seq_tab = nullptr;
   cudaEvent_t ev_tab[3] = {nullptr, nullptr, nullptr};
+  // The camera of each pair (plf_set_sequence_camera), beside prev[k]: rings h_cam / cam_tab [3][max_batch] like h_tab and
+  // seq_tab, copied with the table behind ev_tab.  Only a batch holding a sequence with its own camera fills them; the
+  // others pass no table and the kernels take the context's camera.
+  PlfPairCam* h_cam[3] = {nullptr, nullptr, nullptr};
+  PlfPairCam* cam_tab = nullptr;
   uint8_t* imgs2[2] = {nullptr, nullptr};  // double-buffered [2B][h][pitch]: upload of batch i+1 overlaps the run of batch i
   uint8_t* stage = nullptr;    // dense [2B][h][w] landing buffer of the H2D copy (one contiguous DMA per side), repacked to the padded pitch on the device
   int up_slot = 0;             // slot written by the last plf_batch_upload
@@ -135,6 +142,7 @@ static void pipe_buffers(PipeState* s, bool windowed, DevBufList& b) {
   b.add(s->gn_probs, B); b.add(s->gn_out, B); b.add(s->results, 3 * B);
   b.add(s->d_ovf, 6);
   b.add(s->seq_tab, 3 * 3 * B);
+  b.add(s->cam_tab, 3 * B);
   if (windowed) {
     for (int kind = 0; kind < 4; ++kind) {   // points: 2 cells per feature, lines: 2 end points
       b.add(s->mg_q[kind], B * (kind & 1 ? Ln * 4 : K * 2));
@@ -167,6 +175,7 @@ extern "C" void plf_pipe_free(plf_ctx* ctx) {
     if (s->h_results[i]) cudaFreeHost(s->h_results[i]);
     if (s->h_ovf[i]) cudaFreeHost(s->h_ovf[i]);
     if (s->h_tab[i]) cudaFreeHost(s->h_tab[i]);
+    if (s->h_cam[i]) cudaFreeHost(s->h_cam[i]);
   }
   for (const PipeEvents& a : pipe_events(s))
     for (int i = 0; i < a.n; ++i)
@@ -178,8 +187,17 @@ extern "C" void plf_pipe_free(plf_ctx* ctx) {
 
 struct StereoPrm {
   float max_dist_epip, min_disp, line_horiz_th, stereo_overlap_th, ls_min_disp_ratio;
-  double fx, fy, cx, cy, b;
+  double fx, fy, cx, cy, b;   // the context's camera
 };
+
+// The parameters of pair k: prm with the pair's camera from the batch's camera table, or prm itself without a table.
+__device__ __forceinline__ StereoPrm pair_prm(StereoPrm c, const PlfPairCam* __restrict__ cams, int k) {
+  if (cams) {
+    const PlfPairCam q = cams[k];
+    c.fx = q.fx; c.fy = q.fy; c.cx = q.cx; c.cy = q.cy; c.b = q.b;
+  }
+  return c;
+}
 
 __device__ __forceinline__ void back_projection(const StereoPrm& c, double u, double v, double disp, double* P) {
   const double Z = c.fx * c.b / disp;  // PinholeStereoCamera::backProjection (SURVEY A.4)
@@ -208,12 +226,13 @@ __device__ __forceinline__ int block_scan_flags(bool flag, int* s_scan, int* s_t
 // matchStereoPoints: epipolar + disparity gates, back-projection, compaction in left-index order.
 __global__ void __launch_bounds__(1024) k_stereo_points(const plf_keypoint* __restrict__ kps, const uint8_t* __restrict__ desc,
                                                          const int* __restrict__ kp_count, int max_kp,
-                                                         const int32_t* __restrict__ m12_all, int m12_stride, StereoPrm prm,
-                                                         FrameSlots fs) {
+                                                         const int32_t* __restrict__ m12_all, int m12_stride, StereoPrm prm0,
+                                                         const PlfPairCam* __restrict__ cams, FrameSlots fs) {
   __shared__ int s_scan[1024];
   __shared__ int s_total;
   const int k = blockIdx.x, tid = threadIdx.x;
   const int il = 2 * k, ir = 2 * k + 1, slot = k;
+  const StereoPrm prm = pair_prm(prm0, cams, k);
   const plf_keypoint* kl = kps + (size_t)il * max_kp;
   const plf_keypoint* kr = kps + (size_t)ir * max_kp;
   const int32_t* m12 = m12_all + (size_t)k * m12_stride;
@@ -273,12 +292,13 @@ __device__ __forceinline__ double line_overlap_stereo(double spl_obs, double epl
 // matchStereoLines
 __global__ void __launch_bounds__(1024) k_stereo_lines(const plf_keyline* __restrict__ kls, const uint8_t* __restrict__ ldesc,
                                                         const int* __restrict__ nlines, int max_ln,
-                                                        const int32_t* __restrict__ m12_all, int m12_stride, StereoPrm prm,
-                                                        FrameSlots fs) {
+                                                        const int32_t* __restrict__ m12_all, int m12_stride, StereoPrm prm0,
+                                                        const PlfPairCam* __restrict__ cams, FrameSlots fs) {
   __shared__ int s_scan[1024];
   __shared__ int s_total;
   const int k = blockIdx.x, tid = threadIdx.x;
   const int il = 2 * k, ir = 2 * k + 1, slot = k;
+  const StereoPrm prm = pair_prm(prm0, cams, k);
   const plf_keyline* L = kls + (size_t)il * max_ln;
   const plf_keyline* R = kls + (size_t)ir * max_ln;
   const int32_t* m12 = m12_all + (size_t)k * m12_stride;
@@ -507,12 +527,15 @@ __global__ void __launch_bounds__(256) k_mg_geom_stereo(const plf_keypoint* __re
 }
 
 // frame-to-frame: queries = the previous frame's 3-D features projected with DT = identity (slot prev[k]), train = the
-// current frame's image features (slot k)
-__global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, const int* __restrict__ prev, int K, int Ln, StereoPrm c,
-                                                     double iw, double ih, int* __restrict__ qp, int* __restrict__ tp,
-                                                     int* __restrict__ ql, int* __restrict__ tl, double* __restrict__ tdir) {
+// current frame's image features (slot k).  The projection uses pair k's camera: both frames belong to one sequence, and
+// a new camera restarts its sequence, so the previous frame was triangulated with the same one.
+__global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, const int* __restrict__ prev, int K, int Ln, StereoPrm c0,
+                                                     const PlfPairCam* __restrict__ cams, double iw, double ih,
+                                                     int* __restrict__ qp, int* __restrict__ tp, int* __restrict__ ql,
+                                                     int* __restrict__ tl, double* __restrict__ tdir) {
   const int k = blockIdx.y, i = blockIdx.x * 256 + threadIdx.x;
   const int ps = prev[k], cs = k;
+  const StereoPrm c = pair_prm(c0, cams, k);
   if (i < min(fs.pt_count[ps], K)) {
     const double* P = fs.pt_P + 3 * ((size_t)ps * K + i);
     const double2 u = plf_project(c.fx, c.fy, c.cx, c.cy, P[0], P[1], P[2]);
@@ -587,6 +610,7 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
     PLF_CUDA(ctx, cudaHostAlloc(&s->h_results[i], sizeof(plf_frame_result) * B, cudaHostAllocDefault));
     PLF_CUDA(ctx, cudaHostAlloc(&s->h_ovf[i], 2 * sizeof(int), cudaHostAllocDefault));
     PLF_CUDA(ctx, cudaHostAlloc(&s->h_tab[i], 3 * sizeof(int32_t) * B, cudaHostAllocDefault));
+    PLF_CUDA(ctx, cudaHostAlloc(&s->h_cam[i], sizeof(PlfPairCam) * B, cudaHostAllocDefault));
   }
   FrameSlots& f = s->fs;
   cudaStream_t cs = ctx->stream;
@@ -644,6 +668,7 @@ static plf_status pipe_prepare(plf_ctx* ctx) {
 struct BatchRun {
   int B;
   int ncarry;    // entries of the carry list in h_tab[rp]: the sequences the batch holds
+  bool cams;     // h_cam[rp] holds the pairs' cameras (a sequence of the batch has its own); else the context's camera
   int par;       // parity of the E -> G -> M hand-off buffers
   int lp;        // parity of the LSD hand-off buffers (0 when they exist once)
   int rp;        // slot of the result ring
@@ -741,6 +766,9 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   int32_t* carry = prev + s->B;
   PLF_CUDA(ctx, cudaMemcpyAsync(prev, s->h_tab[rp], sizeof(int32_t) * B, cudaMemcpyHostToDevice, s->copy));
   PLF_CUDA(ctx, cudaMemcpyAsync(carry, s->h_tab[rp] + s->B, sizeof(int32_t) * 2 * r.ncarry, cudaMemcpyHostToDevice, s->copy));
+  // the pairs' cameras, when the batch has them (null: every kernel takes the context's camera)
+  PlfPairCam* pcam = r.cams ? s->cam_tab + (size_t)rp * s->B : nullptr;
+  if (pcam) PLF_CUDA(ctx, cudaMemcpyAsync(pcam, s->h_cam[rp], sizeof(PlfPairCam) * B, cudaMemcpyHostToDevice, s->copy));
   PLF_CUDA(ctx, cudaEventRecord(s->ev_tab[rp], s->copy));
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_tab[rp], 0));
   k_f2f_problems<<<(B + 127) / 128, 128, 0, cs>>>(s->fs, prev, B, K, Ln, s->knn_keys, s->m12, s->mcount, P.min_ratio_12_p,
@@ -792,9 +820,9 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   }
   StereoPrm sp = {P.max_dist_epip, P.min_disp, P.line_horiz_th, P.stereo_overlap_th, P.ls_min_disp_ratio,
                   ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy, ctx->cam.b};
-  k_stereo_points<<<B, 1024, 0, cs>>>(kps, odesc, kcnt, K, s->m12, 4 * K, sp, s->fs);
+  k_stereo_points<<<B, 1024, 0, cs>>>(kps, odesc, kcnt, K, s->m12, 4 * K, sp, pcam, s->fs);
   PLF_LAUNCH_CHECK(ctx);
-  k_stereo_lines<<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, sp, s->fs);
+  k_stereo_lines<<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, sp, pcam, s->fs);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "stereo.k_stereo_points+lines");
   if ((st = plf_launch_knn2(ctx, cs, s->knn_f2f, 4 * B, std::max(K, Ln)))) return st;
@@ -804,8 +832,9 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     // frame-to-frame: matchGrid() in a +-matching_f2f_ws window around the projected feature; the match() result above
     // stands where the window search found fewer than min_pt_matches / min_ls_matches
     PLF_CUDA(ctx, cudaMemsetAsync(s->mgcount, 0, (size_t)B * 2 * sizeof(int), cs));
-    k_mg_geom_f2f<<<dim3((std::max(K, Ln) + 255) / 256, B), 256, 0, cs>>>(s->fs, prev, K, Ln, sp, mg_iw, mg_ih, s->mg_q[2],
-                                                                          s->mg_t[2], s->mg_q[3], s->mg_t[3], s->mg_dir[1]);
+    k_mg_geom_f2f<<<dim3((std::max(K, Ln) + 255) / 256, B), 256, 0, cs>>>(s->fs, prev, K, Ln, sp, pcam, mg_iw, mg_ih,
+                                                                          s->mg_q[2], s->mg_t[2], s->mg_q[3], s->mg_t[3],
+                                                                          s->mg_dir[1]);
     PLF_LAUNCH_CHECK(ctx);
     const int ws = P.matching_f2f_ws;
     const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, ws, ws, ws, ws};
@@ -823,7 +852,7 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
                                   s->gn_sP, s->gn_eP, s->gn_le, s->gnInlL, s->gnNl);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "f2f.k_nnr_mutual+k_f2f_build");
-  if ((st = plf_launch_gn(ctx, cs, s->gn_probs, B, plf_gn_opts_from_params(P)))) return st;
+  if ((st = plf_launch_gn(ctx, cs, s->gn_probs, B, plf_gn_opts_from_params(P), pcam))) return st;
   plf_mark(ctx, cs, "gn.k_gn_pose");
   k_finalize<<<(B + 127) / 128, 128, 0, cs>>>(s->gn_out, s->gnNp, s->gnNl, kcnt, lcnt, s->fs, prev, s->B + s->nseq,
                                                P.min_features, B, s->results + (size_t)rp * s->B);
@@ -856,6 +885,45 @@ plf_status plf_set_max_sequences(plf_ctx* ctx, int n) {
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_max_sequences: n = %d, need 1 <= n <= %d", n, PLF_MAX_SEQUENCES);
   if (ctx->pipe) return plf_fail(ctx, PLF_ERR_STATE, "plf_set_max_sequences: the pipeline exists (a batch call was made)");
   ctx->max_sequences = n;
+  ctx->seq_cam.clear();
+  ctx->seq_cam_own.clear();
+  return PLF_OK;
+}
+
+plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (s < 0 || s >= ctx->max_sequences)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: s = %d outside [0, %d)", s, ctx->max_sequences);
+  if (cam) {
+    if (cam->width != ctx->cam.width)
+      return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: width = %d, the context's is %d", cam->width, ctx->cam.width);
+    if (cam->height != ctx->cam.height)
+      return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: height = %d, the context's is %d", cam->height, ctx->cam.height);
+    const struct { const char* name; double v; bool positive; } f[] = {
+        {"fx", cam->fx, true}, {"fy", cam->fy, true}, {"cx", cam->cx, false}, {"cy", cam->cy, false}, {"b", cam->b, true}};
+    for (const auto& e : f)
+      if (!std::isfinite(e.v) || (e.positive && !(e.v > 0.0)))
+        return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: %s = %g, need a finite value%s", e.name, e.v,
+                        e.positive ? " > 0" : "");
+  }
+  if (ctx->seq_cam_own.empty()) {
+    ctx->seq_cam.assign(ctx->max_sequences, ctx->cam);
+    ctx->seq_cam_own.assign(ctx->max_sequences, 0);
+  }
+  ctx->seq_cam[s] = cam ? *cam : ctx->cam;
+  ctx->seq_cam_own[s] = cam ? 1 : 0;
+  // the sequence restarts: its next pair in a run is a first frame (the batches already run have their tables)
+  if (ctx->pipe) ctx->pipe->carried[s] = 0;
+  return PLF_OK;
+}
+
+plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out) {
+  if (!ctx) return PLF_ERR_INVALID;
+  plf_ctx* c = const_cast<plf_ctx*>(ctx);   // the error text is the only state a failed call writes
+  if (!out) return plf_fail(c, PLF_ERR_INVALID, "plf_get_sequence_camera: out is NULL");
+  if (s < 0 || s >= ctx->max_sequences)
+    return plf_fail(c, PLF_ERR_INVALID, "plf_get_sequence_camera: s = %d outside [0, %d)", s, ctx->max_sequences);
+  *out = !ctx->seq_cam_own.empty() && ctx->seq_cam_own[s] ? ctx->seq_cam[s] : ctx->cam;
   return PLF_OK;
 }
 
@@ -946,6 +1014,15 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
     carry[2 * r.ncarry + 1] = s->B + q;
     r.ncarry++;
   }
+  // the cameras of the pairs, resolved now: a later plf_set_sequence_camera does not reach this batch
+  r.cams = false;
+  if (!ctx->seq_cam_own.empty())
+    for (int k = 0; k < B && !r.cams; ++k) r.cams = ctx->seq_cam_own[seq ? seq[k] : 0] != 0;
+  if (r.cams)
+    for (int k = 0; k < B; ++k) {
+      const plf_camera& c = ctx->seq_cam[seq ? seq[k] : 0];
+      s->h_cam[r.rp][k] = PlfPairCam{c.fx, c.fy, c.cx, c.cy, c.b};
+    }
   r.run_slot = s->up_slot;
   // With profiling on everything is serialised on the main stream so that the per-kernel marks are meaningful.
   r.piped = !ctx->profile || ctx->profile_piped;

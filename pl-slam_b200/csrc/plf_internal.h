@@ -80,6 +80,10 @@ struct plf_ctx {
   plf_camera cam;
   plf_limits limits;
   int max_sequences = 1;          // plf_set_max_sequences: fixed once the pipeline exists
+  // plf_set_sequence_camera: [max_sequences] once a sequence has its own calibration, else empty; seq_cam[s] is used
+  // where seq_cam_own[s], else cam.  plf_set_max_sequences clears both.
+  std::vector<plf_camera> seq_cam;
+  std::vector<uint8_t> seq_cam_own;
   std::string err;
   long long launches = 0;
   // scratch slots (device) of the host-pointer operator entry points
@@ -213,8 +217,12 @@ struct GnProblem {
   const double* T_init;  // 16 or null
   plf_pose_result* out;
 };
+// The calibration of one pair of a batch: its sequence's camera when the batch was run (plf_set_sequence_camera).
+struct PlfPairCam { double fx, fy, cx, cy, b; };
 plf_gn_opts plf_gn_opts_from_params(const plf_params& p);
-plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs, int nprob, const plf_gn_opts& o);
+// d_cams: optional [nprob] device array, the camera of each problem (b unused); null = the context's camera.
+plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs, int nprob, const plf_gn_opts& o,
+                         const PlfPairCam* d_cams = nullptr);
 
 // ---- tiled LDL^T (lba.cu) ------------------------------------------------------------------------
 // Factors the symmetric n x n matrix S (n = 6 n6; row-major, leading dimension n; only its lower triangle is read) in

@@ -727,6 +727,20 @@ class Frontend:
     def reset_sequence(self):
         self._check(self.lib.plf_reset_sequence(self._ctx), "plf_reset_sequence")
 
+    def set_sequence_camera(self, s, camera=None):
+        """Gives sequence s its own calibration: a camera dict as Frontend(camera=...) takes, or a plf_camera, of the
+        context's width and height.  None returns s to the context's camera.  Either restarts s: its next pair in a run is
+        a first frame.  Batches already run keep their cameras.  plf_set_sequence_camera."""
+        cam = None if camera is None else (camera if isinstance(camera, plf_camera) else plf_camera(**camera))
+        self._check(self.lib.plf_set_sequence_camera(self._ctx, int(s), None if cam is None else C.byref(cam)),
+                    "plf_set_sequence_camera")
+
+    def sequence_camera(self, s):
+        """The calibration the next batch uses for sequence s, as a camera dict.  plf_get_sequence_camera."""
+        out = plf_camera()
+        self._check(self.lib.plf_get_sequence_camera(self._ctx, int(s), C.byref(out)), "plf_get_sequence_camera")
+        return {name: getattr(out, name) for name, _ in plf_camera._fields_}
+
     @staticmethod
     def _result_dicts(res, B):
         out = []
