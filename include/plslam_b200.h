@@ -342,8 +342,37 @@ typedef struct plf_lba_result {
   double err;    /* last normalised weighted error */
   double lambda; /* final damping */
 } plf_lba_result;
-/* Projects with the context's camera (plf_create), not a sequence's (plf_set_sequence_camera). */
+/* Projects with the context's camera (plf_create), not a sequence's (plf_set_sequence_camera); plf_local_ba_batch
+ * takes a sequence's. */
 plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* problem, plf_lba_result* out);
+
+/* Many local bundle adjustments in one call: the local maps of several sequences' new keyframes, each with its
+ * sequence's camera, solved in one launch chain with one host synchronisation (after the download).
+ *   problems [n_problems]  plf_local_ba's layout and rules, each in / out as in plf_local_ba
+ *   seq      [n_problems]  or NULL: the camera of problem p.  seq[p] = -1 (or seq NULL) uses the context's camera;
+ *                          0 <= seq[p] < n (plf_set_max_sequences) uses what plf_get_sequence_camera(ctx, seq[p]) returns
+ *                          at the time of the call.  Only fx, fy, cx and cy enter the LBA.
+ *   out      [n_problems]  or NULL;  status [n_problems], required.
+ * Problem p gets the result plf_local_ba(ctx, opts, &problems[p], &out[p]) gives with problem p's camera: the same
+ * iteration count and exit, moved flags, lambda and err to rounding, every block to rounding of the step (the sums are
+ * float atomics, as in plf_local_ba: no bit-reproducibility promise).  One opts applies to every problem.
+ * Refusals before any work: PLF_ERR_INVALID or PLF_ERR_CAPACITY, and nothing is written (no problem's arrays, out or
+ * status), when n_problems < 0, a seq entry is out of range, or any problem breaks one of plf_local_ba's host-side rules
+ * (empty problem, NULL arrays, ungrouped observations, out-of-range indices, a landmark without observations, more than
+ * 64 local keyframes); the message names the problem index and the rule.  n_problems = 0 returns PLF_OK.
+ * Refusal on the device: a landmark whose first-pass block has an exactly zero diagonal entry refuses its problem only:
+ * status[p] = PLF_ERR_INVALID, and its arrays and out[p] are left unchanged.  Every other problem is solved and written
+ * back with status PLF_OK.  The call then returns PLF_ERR_INVALID, and plf_last_error names the first refused problem and
+ * its landmark; else PLF_OK.  The context stays usable after any error.
+ * All opts.max_iters rounds are enqueued at once, and a round in which every problem has stopped still costs its eight
+ * launches (each returning at once), so the call's time grows with max_iters, not with the iterations run.
+ * Work is enqueued on plf_stream and uses its own scratch slot (not plf_local_ba's), which stays allocated until
+ * plf_destroy: 144 bytes per observation, 629 per landmark plus 24 per landmark coordinate (X, X0 and the step), 704 per
+ * local keyframe, 288 per local keyframe^2 of each problem, 256 per fixed keyframe and about 240 per problem, each part
+ * rounded up to 256 bytes; the context's pinned staging buffer holds the inputs and outputs.  The rules for batches in
+ * flight are plf_local_ba's. */
+plf_status plf_local_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems, const plf_lba_problem* problems,
+                              const int32_t* seq, plf_lba_result* out, plf_status* status);
 
 /* Global bundle adjustment.  Replaces MapHandler::levMarquardtOptimizationGBA (src/mapHandler.cpp:2101-2699), the
  * numerical core of MapHandler::globalBundleAdjustment (:1995-2099): the same Levenberg-Marquardt as plf_local_ba over

@@ -72,9 +72,12 @@ __device__ __forceinline__ void lba_rowvec_R(const double* v, const double* T, d
   for (int j = 0; j < 3; ++j) out[j] = v[0] * T[j] + v[1] * T[4 + j] + v[2] * T[8 + j];
 }
 
-// mode 0: first pass on the map's values (X0 / T0inv); mode 1: LM iteration on X; quirks: BAQ_* set
-__global__ void __launch_bounds__(128) k_lba_rows(LbaDev d, LbaCam c, int mode, int quirks, double homog_th) {
-  const int k = blockIdx.x * 128 + threadIdx.x;
+// Each kernel's work for one element (observation k, landmark l, ...) is a __device__ function of the problem's LbaDev,
+// so that plf_local_ba_batch's kernels (below plf_global_ba) run the same arithmetic on each problem of a batch.
+
+// mode 0: first pass on the map's values (X0 / T0inv); mode 1: LM iteration on X; quirks: BAQ_* set.  Every lane of the
+// warp calls it (the error is reduced over the warp).
+__device__ __forceinline__ void lba_rows(const LbaDev& d, const LbaCam& c, int k, int mode, int quirks, double homog_th) {
   double e2w = 0.0;
   if (k < d.nobs) {
     const bool is_line = k >= d.npo;
@@ -162,13 +165,15 @@ __global__ void __launch_bounds__(128) k_lba_rows(LbaDev d, LbaCam c, int mode, 
   for (int off = 16; off > 0; off >>= 1) e2w += __shfl_xor_sync(0xFFFFFFFFu, e2w, off);
   if ((threadIdx.x & 31) == 0 && e2w != 0.0) atomicAdd(&d.scal[0], e2w);
 }
+__global__ void __launch_bounds__(128) k_lba_rows(LbaDev d, LbaCam c, int mode, int quirks, double homog_th) {
+  lba_rows(d, c, blockIdx.x * 128 + threadIdx.x, mode, quirks, homog_th);
+}
 
 __device__ __forceinline__ void lba_atomic_max_pos(double* addr, double v) {   // v >= 0: the bit patterns are ordered
   atomicMax(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)__double_as_longlong(v));
 }
 
-__global__ void __launch_bounds__(128) k_lba_lm_accum(LbaDev d) {
-  const int l = blockIdx.x * 128 + threadIdx.x;
+__device__ __forceinline__ void lba_lm_accum(const LbaDev& d, int l) {
   if (l >= d.nlm) return;
   const int dim = l < d.npt ? 3 : 6;
   double D[36], g[6];
@@ -191,11 +196,12 @@ __global__ void __launch_bounds__(128) k_lba_lm_accum(LbaDev d) {
   // a zero diagonal entry: scal[4] (as an integer) keeps nlm - l of the first such landmark, 0 when there is none
   if (zero) atomicMax(reinterpret_cast<unsigned long long*>(&d.scal[4]), (unsigned long long)(d.nlm - l));
 }
+__global__ void __launch_bounds__(128) k_lba_lm_accum(LbaDev d) { lba_lm_accum(d, blockIdx.x * 128 + threadIdx.x); }
 
-__global__ void k_lba_kf_diagmax(LbaDev d) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void lba_kf_diagmax(const LbaDev& d, int i) {
   if (i < 6 * d.nkf) lba_atomic_max_pos(&d.scal[2], fabs(d.A[36 * (i / 6) + 7 * (i % 6)]));
 }
+__global__ void k_lba_kf_diagmax(LbaDev d) { lba_kf_diagmax(d, blockIdx.x * blockDim.x + threadIdx.x); }
 
 // in-place inverse of a symmetric positive definite dim x dim matrix (row stride 6) by Gauss-Jordan without pivoting
 __device__ void lba_inv_spd(double* M, int dim, double* Minv) {
@@ -213,8 +219,7 @@ __device__ void lba_inv_spd(double* M, int dim, double* Minv) {
 }
 
 // swap (g6): for line landmarks the coupling block is w Jt Jx^T, so Jt is the landmark-side vector and Jx the pose side
-__global__ void __launch_bounds__(128) k_lba_lm_schur(LbaDev d, double lambda, int swap) {
-  const int l = blockIdx.x * 128 + threadIdx.x;
+__device__ __forceinline__ void lba_lm_schur(const LbaDev& d, int l, double lambda, int swap) {
   if (l >= d.nlm) return;
   const int dim = l < d.npt ? 3 : 6, n = 6 * d.nkf;
   const double* U = swap && l >= d.npt ? d.Jt : d.Jx;   // landmark side of the coupling
@@ -254,9 +259,13 @@ __global__ void __launch_bounds__(128) k_lba_lm_schur(LbaDev d, double lambda, i
     }
   }
 }
+__global__ void __launch_bounds__(128) k_lba_lm_schur(LbaDev d, double lambda, int swap) {
+  lba_lm_schur(d, blockIdx.x * 128 + threadIdx.x, lambda, swap);
+}
 
-// One CTA: S += A' (block diagonal, damped), g_red += g_c, dense LDL^T without pivoting, solve S dx_c = g_red.
-__global__ void __launch_bounds__(256) k_lba_solve(LbaDev d, double lambda) {
+// One CTA of 256 threads: S += A' (block diagonal, damped), g_red += g_c, dense LDL^T without pivoting, solve
+// S dx_c = g_red.
+__device__ __forceinline__ void lba_solve(const LbaDev& d, double lambda) {
   const int n = 6 * d.nkf, tid = threadIdx.x;
   double* S = d.S;
   for (int i = tid; i < 36 * d.nkf; i += 256) {
@@ -297,9 +306,9 @@ __global__ void __launch_bounds__(256) k_lba_solve(LbaDev d, double lambda) {
     for (int i = 0; i < n; ++i) d.DX[i] = x[i];
   }
 }
+__global__ void __launch_bounds__(256) k_lba_solve(LbaDev d, double lambda) { lba_solve(d, lambda); }
 
-__global__ void __launch_bounds__(128) k_lba_backsub(LbaDev d, int swap) {
-  const int l = blockIdx.x * 128 + threadIdx.x;
+__device__ __forceinline__ void lba_backsub(const LbaDev& d, int l, int swap) {
   if (l >= d.nlm) return;
   const int dim = l < d.npt ? 3 : 6;
   const double* U = swap && l >= d.npt ? d.Jt : d.Jx;   // as k_lba_lm_schur
@@ -324,10 +333,11 @@ __global__ void __launch_bounds__(128) k_lba_backsub(LbaDev d, int swap) {
     d.DX[off + i] = v;
   }
 }
+__global__ void __launch_bounds__(128) k_lba_backsub(LbaDev d, int swap) { lba_backsub(d, blockIdx.x * 128 + threadIdx.x, swap); }
 
-// |DX|^2 always; the step itself only when `apply`
-__global__ void __launch_bounds__(128) k_lba_apply(LbaDev d, int apply) {
-  const int i = blockIdx.x * 128 + threadIdx.x;
+// |DX|^2 always; the step itself only when `apply`.  Element i: keyframe i (i < nkf), else one landmark coordinate.  Every
+// lane of the warp calls it.
+__device__ __forceinline__ void lba_apply(const LbaDev& d, int i, int apply) {
   double n2 = 0.0;
   if (i < d.nkf) {
     for (int c = 0; c < 6; ++c) n2 += d.DX[6 * i + c] * d.DX[6 * i + c];
@@ -347,9 +357,9 @@ __global__ void __launch_bounds__(128) k_lba_apply(LbaDev d, int apply) {
   for (int off = 16; off > 0; off >>= 1) n2 += __shfl_xor_sync(0xFFFFFFFFu, n2, off);
   if ((threadIdx.x & 31) == 0 && n2 != 0.0) atomicAdd(&d.scal[1], n2);
 }
+__global__ void __launch_bounds__(128) k_lba_apply(LbaDev d, int apply) { lba_apply(d, blockIdx.x * 128 + threadIdx.x, apply); }
 
-__global__ void k_lba_prep(LbaDev d, const double* fixedT, double* fixedTinv, int n_fixed) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void lba_prep(const LbaDev& d, int i, const double* fixedT, double* fixedTinv, int n_fixed) {
   if (i < d.nkf) {
     double T[16], Ti[16];
     d_expmap(d.X0 + 6 * i, T);
@@ -362,9 +372,11 @@ __global__ void k_lba_prep(LbaDev d, const double* fixedT, double* fixedTinv, in
     for (int k = 0; k < 16; ++k) fixedTinv[16 * i + k] = Ti[k];
   }
 }
+__global__ void k_lba_prep(LbaDev d, const double* fixedT, double* fixedTinv, int n_fixed) {
+  lba_prep(d, blockIdx.x * blockDim.x + threadIdx.x, fixedT, fixedTinv, n_fixed);
+}
 
-__global__ void k_lba_moved(LbaDev d, uint8_t* pt_moved, uint8_t* ls_moved) {
-  const int l = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void lba_moved(const LbaDev& d, int l, uint8_t* pt_moved, uint8_t* ls_moved) {
   if (l >= d.nlm) return;
   const int dim = l < d.npt ? 3 : 6;
   const int off = l < d.npt ? 6 * d.nkf + 3 * l : 6 * d.nkf + 3 * d.npt + 6 * (l - d.npt);
@@ -372,6 +384,9 @@ __global__ void k_lba_moved(LbaDev d, uint8_t* pt_moved, uint8_t* ls_moved) {
   for (int c = 0; c < dim; ++c) { const double v = d.X[off + c] - d.X0[off + c]; n2 += v * v; }
   const uint8_t m = sqrt(n2) > 0.01;   // :1829, :1843
   if (l < d.npt) pt_moved[l] = m; else ls_moved[l - d.npt] = m;
+}
+__global__ void k_lba_moved(LbaDev d, uint8_t* pt_moved, uint8_t* ls_moved) {
+  lba_moved(d, blockIdx.x * blockDim.x + threadIdx.x, pt_moved, ls_moved);
 }
 
 // (g2) `int Hmax` scanned over the first pass's diagonal in index order (:2359-2364): `d > Hmax` compares with the int,
@@ -642,21 +657,29 @@ plf_status plf_ldlt_tiled(plf_ctx* ctx, cudaStream_t cs, int n6, double* S, doub
 // landmark whose first-pass block D has an exactly zero diagonal entry, before any step: the reference would factor a
 // zero pivot (its SimplicialLDLT's failure is not checked) and the landmark, then every keyframe observing it, would
 // turn NaN.  A landmark without observations is refused by name first; the rest by one flag read with the first pass.
-static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out, bool global) {
-  const char* fn = global ? "plf_global_ba" : "plf_local_ba";
-  if (!ctx || !opts || !p || p->n_kf < 0 || p->n_pt < 0 || p->n_ls < 0 || p->n_pt_obs < 0 || p->n_ls_obs < 0 || p->n_fixed < 0)
+// The host-side rules of one problem, up to its observations: counts, emptiness, the keyframe limit and NULL arrays.
+// Messages start with `fn`.
+static plf_status lba_check_shape(plf_ctx* ctx, const char* fn, const plf_lba_problem* p, int kf_cap) {
+  if (p->n_kf < 0 || p->n_pt < 0 || p->n_ls < 0 || p->n_pt_obs < 0 || p->n_ls_obs < 0 || p->n_fixed < 0)
     return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", fn);
-  const int nkf = p->n_kf, npt = p->n_pt, nls = p->n_ls, npo = p->n_pt_obs, nlo = p->n_ls_obs, nobs = npo + nlo, nlm = npt + nls;
-  const int N = 6 * nkf + 3 * npt + 6 * nls, n = 6 * nkf;
-  if (nobs == 0 || N == 0) return plf_fail(ctx, PLF_ERR_INVALID, "%s: empty problem (the reference returns -1, :1324-1328)", fn);
-  const int kf_cap = global ? 4096 : 64;
+  const int nkf = p->n_kf, npt = p->n_pt, nls = p->n_ls, npo = p->n_pt_obs, nlo = p->n_ls_obs;
+  if (npo + nlo == 0 || 6 * nkf + 3 * npt + 6 * nls == 0)
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: empty problem (the reference returns -1, :1324-1328)", fn);
   if (nkf > kf_cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: %d keyframes (limit %d)", fn, nkf, kf_cap);
   if ((nkf && !p->kf_pose) || (npt && !p->pt) || (nls && !p->ls) || (npo && (!p->pt_obs_lm || !p->pt_obs_kf || !p->pt_obs_xy)) ||
       (nlo && (!p->ls_obs_lm || !p->ls_obs_kf || !p->ls_obs_le)) || (p->n_fixed && !p->fixed_T))
     return plf_fail(ctx, PLF_ERR_INVALID, "%s: null array", fn);
+  return PLF_OK;
+}
+
+// The rest of the host-side rules (indices in range, observations grouped, every landmark observed) while gathering the
+// observations into the device layout: obs_lm / obs_kf [nobs] (points first, then lines), obs_z [nobs][3] and
+// lm_start [nlm + 1] (each landmark's first observation).
+static plf_status lba_gather(plf_ctx* ctx, const char* fn, const plf_lba_problem* p, int* lm_start, int* h_lm, int* h_kf,
+                             double* h_z) {
+  const int nkf = p->n_kf, npt = p->n_pt, nls = p->n_ls, npo = p->n_pt_obs, nobs = npo + p->n_ls_obs, nlm = npt + nls;
+  for (int l = 0; l <= nlm; ++l) lm_start[l] = 0;
   // observations are grouped per landmark in non-decreasing landmark order (how the reference builds its lists, :1249-1277)
-  std::vector<int> lm_start(nlm + 1, 0), h_lm(nobs), h_kf(nobs);
-  std::vector<double> h_z((size_t)nobs * 3, 0.0);
   for (int k = 0; k < nobs; ++k) {
     const bool is_line = k >= npo;
     const int lm = is_line ? p->ls_obs_lm[k - npo] : p->pt_obs_lm[k], kf = is_line ? p->ls_obs_kf[k - npo] : p->pt_obs_kf[k];
@@ -668,12 +691,27 @@ static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_p
     h_lm[k] = lm; h_kf[k] = kf;
     lm_start[(is_line ? npt : 0) + lm + 1]++;
     if (is_line) for (int c = 0; c < 3; ++c) h_z[3 * (size_t)k + c] = p->ls_obs_le[3 * (size_t)(k - npo) + c];
-    else { h_z[3 * (size_t)k] = p->pt_obs_xy[2 * (size_t)k]; h_z[3 * (size_t)k + 1] = p->pt_obs_xy[2 * (size_t)k + 1]; }
+    else {
+      h_z[3 * (size_t)k] = p->pt_obs_xy[2 * (size_t)k]; h_z[3 * (size_t)k + 1] = p->pt_obs_xy[2 * (size_t)k + 1];
+      h_z[3 * (size_t)k + 2] = 0.0;
+    }
   }
   for (int l = 0; l < nlm; ++l)   // its landmark block would be zero
     if (!lm_start[l + 1])
       return plf_fail(ctx, PLF_ERR_INVALID, "%s: %s landmark %d has no observation", fn, l < npt ? "point" : "line", l < npt ? l : l - npt);
   for (int l = 0; l < nlm; ++l) lm_start[l + 1] += lm_start[l];
+  return PLF_OK;
+}
+
+static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out, bool global) {
+  const char* fn = global ? "plf_global_ba" : "plf_local_ba";
+  if (!ctx || !opts || !p) return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", fn);
+  if (plf_status st = lba_check_shape(ctx, fn, p, global ? 4096 : 64)) return st;
+  const int nkf = p->n_kf, npt = p->n_pt, nls = p->n_ls, npo = p->n_pt_obs, nlo = p->n_ls_obs, nobs = npo + nlo, nlm = npt + nls;
+  const int N = 6 * nkf + 3 * npt + 6 * nls, n = 6 * nkf;
+  std::vector<int> lm_start(nlm + 1), h_lm(nobs), h_kf(nobs);
+  std::vector<double> h_z((size_t)nobs * 3);
+  if (plf_status st = lba_gather(ctx, fn, p, lm_start.data(), h_lm.data(), h_kf.data(), h_z.data())) return st;
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const bool blocked = n > 384;   // k_lba_solve (one CTA, one launch) up to 64 keyframes, the tiled LDL^T beyond
   const int nt = (n + GBA_T - 1) / GBA_T;
@@ -817,4 +855,312 @@ extern "C" plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const
 
 extern "C" plf_status plf_global_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out) {
   return ba_run(ctx, opts, p, out, true);
+}
+
+// ---- plf_local_ba_batch: many local BAs in one launch chain -----------------------------------------------------------
+// The problems' arrays are concatenated into flat arrays; LbbProb holds problem p's counts, its offsets into each flat
+// array and its camera, and lbb_view() builds the LbaDev of its slice, so the kernels below run the single-problem
+// functions above on each problem.  They are gridded (problem, chunk): blockIdx.x is the problem and blockIdx.y strides
+// over its observations, landmarks or elements, so no warp mixes two problems.  ba_run's host loop runs on the device
+// in LbbCtrl, one thread per problem (k_lbb_first, k_lbb_test, k_lbb_step), with the same double expressions in the same
+// order.  A problem that has stopped, or was refused, is inactive, and every later kernel returns at once for it.  All
+// max_iters rounds are enqueued up front, so the call has one host synchronisation, after the download.
+struct LbbProb {
+  int nkf, npt, nls, npo, nobs, nlm, N, nfix;
+  long long xo, oo, lo, ko, fo, go, so;   // offsets into X (doubles), observations, landmarks, keyframes, fixed
+                                          // keyframes, rows of the reduced systems and S (doubles)
+  LbaCam cam;
+};
+struct LbbCtrl {
+  double lambda, err, err_prev;
+  int iters;     // the loop counter at exit: max(max_iters, 1) unless a stop test breaks the loop earlier
+  int active;    // 0 once the problem has stopped or was refused
+  int apply;     // this round's step is applied (the error did not grow)
+  int zero_lm;   // the first landmark whose first-pass block has a zero diagonal entry (the problem is refused), or -1
+};
+struct LbbDev {
+  const LbbProb* prob; LbbCtrl* ctrl; int P;
+  double* X; double* X0; double* T0inv; const double* fixedT; double* fixedTinv;
+  const int* obs_lm; const int* obs_kf; const double* obs_z; const int* lm_start;   // lm_start: nlm + 1 per problem
+  double* Jt; double* Jx; double* Wn; double* D; double* gl; double* Dinv; double* A; double* gc;
+  double* S; double* gred; double* dxc; double* DX; double* scal; uint8_t* moved;
+};
+
+__device__ __forceinline__ LbaDev lbb_view(const LbbDev& b, const LbbProb& q, int p) {
+  LbaDev d;
+  d.nkf = q.nkf; d.npt = q.npt; d.nls = q.nls; d.N = q.N; d.npo = q.npo; d.nlo = q.nobs - q.npo; d.nobs = q.nobs; d.nlm = q.nlm;
+  d.X = b.X + q.xo; d.X0 = b.X0 + q.xo; d.T0inv = b.T0inv + 16 * q.ko; d.fixedTinv = b.fixedTinv + 16 * q.fo;
+  d.obs_lm = b.obs_lm + q.oo; d.obs_kf = b.obs_kf + q.oo; d.obs_z = b.obs_z + 3 * q.oo; d.lm_start = b.lm_start + q.lo + p;
+  d.Jt = b.Jt + 6 * q.oo; d.Jx = b.Jx + 6 * q.oo; d.Wn = b.Wn + 2 * q.oo;
+  d.D = b.D + 36 * q.lo; d.gl = b.gl + 6 * q.lo; d.Dinv = b.Dinv + 36 * q.lo;
+  d.A = b.A + 36 * q.ko; d.gc = b.gc + 6 * q.ko;
+  d.S = b.S + q.so; d.gred = b.gred + q.go; d.dxc = b.dxc + q.go; d.DX = b.DX + q.xo;
+  d.scal = b.scal + 8 * p;
+  return d;
+}
+
+// T0inv / fixedTinv, X = X0 and the control state
+__global__ void __launch_bounds__(128) k_lbb_prep(LbbDev b, double lambda, int iters) {
+  const int p = blockIdx.x;
+  const LbbProb q = b.prob[p];
+  const LbaDev d = lbb_view(b, q, p);
+  for (int i = threadIdx.x; i < max(q.nkf, q.nfix); i += 128) lba_prep(d, i, b.fixedT + 16 * q.fo, b.fixedTinv + 16 * q.fo, q.nfix);
+  for (int i = threadIdx.x; i < q.N; i += 128) d.X[i] = d.X0[i];
+  if (threadIdx.x == 0) b.ctrl[p] = LbbCtrl{lambda, 0.0, 0.0, iters, 1, 1, -1};
+}
+
+__global__ void __launch_bounds__(128) k_lbb_rows(LbbDev b, int mode, int quirks, double homog_th) {
+  const int p = blockIdx.x;
+  if (!b.ctrl[p].active) return;
+  const LbbProb q = b.prob[p];
+  const LbaDev d = lbb_view(b, q, p);
+  for (int c = blockIdx.y; 128 * c < q.nobs; c += gridDim.y) lba_rows(d, q.cam, 128 * c + threadIdx.x, mode, quirks, homog_th);
+}
+
+__global__ void __launch_bounds__(128) k_lbb_lm_accum(LbbDev b) {
+  const int p = blockIdx.x;
+  if (!b.ctrl[p].active) return;
+  const LbbProb q = b.prob[p];
+  const LbaDev d = lbb_view(b, q, p);
+  for (int c = blockIdx.y; 128 * c < q.nlm; c += gridDim.y) lba_lm_accum(d, 128 * c + threadIdx.x);
+}
+
+__global__ void __launch_bounds__(128) k_lbb_kf_diagmax(LbbDev b) {
+  const int p = blockIdx.x;
+  const LbbProb q = b.prob[p];
+  const LbaDev d = lbb_view(b, q, p);
+  for (int i = threadIdx.x; i < 6 * q.nkf; i += 128) lba_kf_diagmax(d, i);
+}
+
+__global__ void __launch_bounds__(128) k_lbb_schur(LbbDev b) {
+  const int p = blockIdx.x;
+  if (!b.ctrl[p].active) return;
+  const LbbProb q = b.prob[p];
+  const LbaDev d = lbb_view(b, q, p);
+  const double lambda = b.ctrl[p].lambda;
+  for (int c = blockIdx.y; 128 * c < q.nlm; c += gridDim.y) lba_lm_schur(d, 128 * c + threadIdx.x, lambda, 0);
+}
+
+// One CTA per problem, as k_lba_solve; then zeroes A, g_c, S and g_red for the next round's accumulation.
+__global__ void __launch_bounds__(256) k_lbb_solve(LbbDev b) {
+  const int p = blockIdx.x;
+  if (!b.ctrl[p].active) return;
+  const LbbProb q = b.prob[p];
+  if (!q.nkf) return;
+  const LbaDev d = lbb_view(b, q, p);
+  lba_solve(d, b.ctrl[p].lambda);
+  __syncthreads();
+  const int n = 6 * q.nkf;
+  for (int i = threadIdx.x; i < n * n; i += 256) d.S[i] = 0.0;
+  for (int i = threadIdx.x; i < n; i += 256) d.gred[i] = 0.0;
+  for (int i = threadIdx.x; i < 6 * n; i += 256) d.A[i] = 0.0;
+  for (int i = threadIdx.x; i < n; i += 256) d.gc[i] = 0.0;
+}
+
+__global__ void __launch_bounds__(128) k_lbb_backsub(LbbDev b) {
+  const int p = blockIdx.x;
+  if (!b.ctrl[p].active) return;
+  const LbbProb q = b.prob[p];
+  const LbaDev d = lbb_view(b, q, p);
+  for (int c = blockIdx.y; 128 * c < q.nlm; c += gridDim.y) lba_backsub(d, 128 * c + threadIdx.x, 0);
+}
+
+__global__ void __launch_bounds__(128) k_lbb_apply(LbbDev b) {
+  const int p = blockIdx.x;
+  if (!b.ctrl[p].active) return;
+  const LbbProb q = b.prob[p];
+  const LbaDev d = lbb_view(b, q, p);
+  const int apply = b.ctrl[p].apply, ne = q.nkf + (q.N - 6 * q.nkf);
+  for (int c = blockIdx.y; 128 * c < ne; c += gridDim.y) lba_apply(d, 128 * c + threadIdx.x, apply);
+}
+
+// After the first pass: the refusal, the error normalisation (q1: the reference divides by two counters it never
+// increments, 0.0 here as there) and lambda *= Hmax.  The first step is applied unconditionally (apply = 1 from k_lbb_prep).
+__global__ void k_lbb_first(LbbDev b, int quirks) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= b.P) return;
+  LbbCtrl& c = b.ctrl[p];
+  const LbbProb& q = b.prob[p];
+  double* scal = b.scal + 8 * p;
+  const unsigned long long zero_flag = (unsigned long long)__double_as_longlong(scal[4]);
+  if (zero_flag) { c.zero_lm = q.nlm - (int)zero_flag; c.active = 0; return; }
+  double err = scal[0];
+  if (quirks & BAQ_FIRST_ERR0) err = __ddiv_rn(err, 0.0);   // (q1) :1541
+  else err /= (double)q.nobs;
+  c.lambda *= scal[2];   // Hmax, whose bit pattern k_lba_lm_accum / k_lba_kf_diagmax maximised
+  c.err = err;
+  c.err_prev = err;
+  scal[0] = 0.0;
+}
+
+// Round r >= 1 after its accumulation: the error, the change and min-error stops (:1773-1775) and whether it grew.
+__global__ void k_lbb_test(LbbDev b, int r, double min_error, double min_error_change) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= b.P || !b.ctrl[p].active) return;
+  LbbCtrl& c = b.ctrl[p];
+  const LbbProb& q = b.prob[p];
+  double* scal = b.scal + 8 * p;
+  const double err = scal[0] / (double)(q.npt + q.nls);
+  scal[0] = 0.0;
+  c.err = err;
+  if (fabs(err - c.err_prev) < min_error_change || err < min_error) { c.active = 0; c.iters = r; return; }
+  c.apply = !(err > c.err_prev);
+}
+
+// Round r after its step: the lambda schedule (:1785-1803) and the |DX| stop (:1805); round 0 only clears |DX|^2.
+__global__ void k_lbb_step(LbbDev b, int r, double lambda_k, double min_error_change) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= b.P || !b.ctrl[p].active) return;
+  LbbCtrl& c = b.ctrl[p];
+  double* scal = b.scal + 8 * p;
+  const double dxn = sqrt(scal[1]);
+  scal[1] = 0.0;
+  if (r == 0) return;
+  if (c.apply) c.lambda *= lambda_k; else c.lambda /= lambda_k;
+  if (dxn < min_error_change) { c.active = 0; c.iters = r; return; }
+  c.err_prev = c.err;
+}
+
+__global__ void __launch_bounds__(128) k_lbb_moved(LbbDev b) {
+  const int p = blockIdx.x;
+  if (b.ctrl[p].zero_lm >= 0) return;
+  const LbbProb q = b.prob[p];
+  const LbaDev d = lbb_view(b, q, p);
+  uint8_t* m = b.moved + q.lo;
+  for (int c = blockIdx.y; 128 * c < q.nlm; c += gridDim.y) lba_moved(d, 128 * c + threadIdx.x, m, m + q.npt);
+}
+
+extern "C" plf_status plf_local_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems, const plf_lba_problem* problems,
+                                         const int32_t* seq, plf_lba_result* out, plf_status* status) {
+  const char* fn = "plf_local_ba_batch";
+  if (!ctx || !opts || n_problems < 0 || (n_problems && (!problems || !status)))
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", fn);
+  const int P = n_problems;
+  if (!P) return PLF_OK;
+  // every refusal before any work: the cameras, then plf_local_ba's rules per problem
+  std::vector<LbbProb> hp(P);
+  long long tN = 0, tObs = 0, tLm = 0, tKf = 0, tFix = 0, tG = 0, tS = 0;
+  int mObs = 0, mLm = 0, mEl = 0;
+  char pfx[64];
+  for (int p = 0; p < P; ++p) {
+    const int s = seq ? seq[p] : -1;
+    if (s < -1 || s >= ctx->max_sequences)
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: seq[%d] = %d outside [-1, %d)", fn, p, s, ctx->max_sequences);
+    const plf_camera& c = s >= 0 && !ctx->seq_cam_own.empty() && ctx->seq_cam_own[s] ? ctx->seq_cam[s] : ctx->cam;
+    const plf_lba_problem& pr = problems[p];
+    snprintf(pfx, sizeof pfx, "%s: problem %d", fn, p);
+    if (plf_status st = lba_check_shape(ctx, pfx, &pr, 64)) return st;
+    LbbProb& q = hp[p];
+    q.nkf = pr.n_kf; q.npt = pr.n_pt; q.nls = pr.n_ls; q.npo = pr.n_pt_obs; q.nobs = pr.n_pt_obs + pr.n_ls_obs;
+    q.nlm = pr.n_pt + pr.n_ls; q.N = 6 * pr.n_kf + 3 * pr.n_pt + 6 * pr.n_ls; q.nfix = pr.n_fixed;
+    q.xo = tN; q.oo = tObs; q.lo = tLm; q.ko = tKf; q.fo = tFix; q.go = tG; q.so = tS;
+    q.cam = LbaCam{c.fx, c.fy, c.cx, c.cy};
+    tN += q.N; tObs += q.nobs; tLm += q.nlm; tKf += q.nkf; tFix += q.nfix; tG += 6 * q.nkf; tS += 36LL * q.nkf * q.nkf;
+    mObs = std::max(mObs, q.nobs); mLm = std::max(mLm, q.nlm); mEl = std::max(mEl, q.nkf + 3 * q.npt + 6 * q.nls);
+  }
+  // one staged upload (inputs), one download (X, moved flags, control); the device work after them, the part zeroed
+  // before the first pass (A, g_c, S, g_red, scal) last
+  StagedLayout L;
+  const size_t iProb = L.take_in(sizeof(LbbProb) * P), iX0 = L.take_in(8 * tN), iFT = L.take_in(128 * tFix);
+  const size_t iLm = L.take_in(4 * tObs), iKf = L.take_in(4 * tObs), iZ = L.take_in(24 * tObs), iLs = L.take_in(4 * (tLm + P));
+  const size_t oX = L.take_out(8 * tN), oMv = L.take_out(tLm), oCtl = L.take_out(sizeof(LbbCtrl) * P);
+  const size_t wT0 = L.take_work(128 * tKf), wFTi = L.take_work(128 * tFix), wJt = L.take_work(48 * tObs),
+               wJx = L.take_work(48 * tObs), wWn = L.take_work(16 * tObs), wD = L.take_work(288 * tLm),
+               wDi = L.take_work(288 * tLm), wGl = L.take_work(48 * tLm), wDxc = L.take_work(8 * tG), wDX = L.take_work(8 * tN);
+  const size_t wA = L.take_work(288 * tKf), wGc = L.take_work(48 * tKf), wS = L.take_work(8 * tS), wGr = L.take_work(8 * tG),
+               wSc = L.take_work(64 * (size_t)P);
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  uint8_t *pin, *dev;
+  if (plf_status st = L.acquire(ctx, PLF_SCR_BA_BATCH, &pin, &dev)) return st;
+  for (int p = 0; p < P; ++p) {
+    const plf_lba_problem& pr = problems[p];
+    const LbbProb& q = hp[p];
+    snprintf(pfx, sizeof pfx, "%s: problem %d", fn, p);
+    if (plf_status st = lba_gather(ctx, pfx, &pr, (int*)(pin + iLs) + q.lo + p, (int*)(pin + iLm) + q.oo, (int*)(pin + iKf) + q.oo,
+                                   (double*)(pin + iZ) + 3 * q.oo))
+      return st;
+    double* X0 = (double*)(pin + iX0) + q.xo;
+    if (q.nkf) memcpy(X0, pr.kf_pose, 48 * (size_t)q.nkf);
+    if (q.npt) memcpy(X0 + 6 * q.nkf, pr.pt, 24 * (size_t)q.npt);
+    if (q.nls) memcpy(X0 + 6 * q.nkf + 3 * q.npt, pr.ls, 48 * (size_t)q.nls);
+    if (q.nfix) memcpy((double*)(pin + iFT) + 16 * q.fo, pr.fixed_T, 128 * (size_t)q.nfix);
+  }
+  memcpy(pin + iProb, hp.data(), sizeof(LbbProb) * P);
+  cudaStream_t cs = ctx->stream;
+  PLF_CUDA(ctx, cudaMemcpyAsync(dev, pin, L.in, cudaMemcpyHostToDevice, cs));
+  uint8_t* const dout = dev + L.in;
+  uint8_t* const dwork = dout + L.out;
+  PLF_CUDA(ctx, cudaMemsetAsync(dwork + wA, 0, L.work - wA, cs));
+  LbbDev b;
+  b.prob = (const LbbProb*)(dev + iProb); b.ctrl = (LbbCtrl*)(dout + oCtl); b.P = P;
+  b.X = (double*)(dout + oX); b.X0 = (double*)(dev + iX0); b.T0inv = (double*)(dwork + wT0);
+  b.fixedT = (const double*)(dev + iFT); b.fixedTinv = (double*)(dwork + wFTi);
+  b.obs_lm = (const int*)(dev + iLm); b.obs_kf = (const int*)(dev + iKf); b.obs_z = (const double*)(dev + iZ);
+  b.lm_start = (const int*)(dev + iLs);
+  b.Jt = (double*)(dwork + wJt); b.Jx = (double*)(dwork + wJx); b.Wn = (double*)(dwork + wWn);
+  b.D = (double*)(dwork + wD); b.gl = (double*)(dwork + wGl); b.Dinv = (double*)(dwork + wDi);
+  b.A = (double*)(dwork + wA); b.gc = (double*)(dwork + wGc); b.S = (double*)(dwork + wS); b.gred = (double*)(dwork + wGr);
+  b.dxc = (double*)(dwork + wDxc); b.DX = (double*)(dwork + wDX); b.scal = (double*)(dwork + wSc); b.moved = dout + oMv;
+  // grids: (problem, chunks of 128 of the largest problem's count); the control kernels: one thread per problem
+  auto chunks = [](int n) { return std::max(1, std::min(65535, (n + 127) / 128)); };
+  const dim3 gObs(P, chunks(mObs)), gLm(P, chunks(mLm)), gEl(P, chunks(mEl));
+  const int gCtl = (P + 127) / 128;
+  const int q = opts->ref_quirks ? BAQ_LBA : 0;
+  k_lbb_prep<<<P, 128, 0, cs>>>(b, opts->lambda, std::max(opts->max_iters, 1));
+  PLF_LAUNCH_CHECK(ctx);
+  for (int r = 0; r < std::max(opts->max_iters, 1); ++r) {
+    k_lbb_rows<<<gObs, 128, 0, cs>>>(b, r ? 1 : 0, q, opts->homog_th);
+    PLF_LAUNCH_CHECK(ctx);
+    k_lbb_lm_accum<<<gLm, 128, 0, cs>>>(b);
+    PLF_LAUNCH_CHECK(ctx);
+    if (r == 0) {
+      k_lbb_kf_diagmax<<<P, 128, 0, cs>>>(b);
+      PLF_LAUNCH_CHECK(ctx);
+      k_lbb_first<<<gCtl, 128, 0, cs>>>(b, q);
+    } else {
+      k_lbb_test<<<gCtl, 128, 0, cs>>>(b, r, opts->min_error, opts->min_error_change);
+    }
+    PLF_LAUNCH_CHECK(ctx);
+    k_lbb_schur<<<gLm, 128, 0, cs>>>(b);
+    PLF_LAUNCH_CHECK(ctx);
+    k_lbb_solve<<<P, 256, 0, cs>>>(b);
+    PLF_LAUNCH_CHECK(ctx);
+    k_lbb_backsub<<<gLm, 128, 0, cs>>>(b);
+    PLF_LAUNCH_CHECK(ctx);
+    k_lbb_apply<<<gEl, 128, 0, cs>>>(b);
+    PLF_LAUNCH_CHECK(ctx);
+    k_lbb_step<<<gCtl, 128, 0, cs>>>(b, r, opts->lambda_k, opts->min_error_change);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  k_lbb_moved<<<gLm, 128, 0, cs>>>(b);
+  PLF_LAUNCH_CHECK(ctx);
+  PLF_CUDA(ctx, cudaMemcpyAsync(pin + L.in, dout, L.out, cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaStreamSynchronize(cs));
+  const LbbCtrl* ctl = (const LbbCtrl*)(pin + L.in + oCtl);
+  int refused = -1;
+  for (int p = 0; p < P; ++p) {
+    const plf_lba_problem& pr = problems[p];
+    const LbbProb& qp = hp[p];
+    const LbbCtrl& c = ctl[p];
+    if (c.zero_lm >= 0) {
+      status[p] = PLF_ERR_INVALID;
+      if (refused < 0) refused = p;
+      continue;
+    }
+    const double* X = (const double*)(pin + L.in + oX) + qp.xo;
+    if (qp.nkf) memcpy(pr.kf_pose, X, 48 * (size_t)qp.nkf);
+    if (qp.npt) memcpy(pr.pt, X + 6 * qp.nkf, 24 * (size_t)qp.npt);
+    if (qp.nls) memcpy(pr.ls, X + 6 * qp.nkf + 3 * qp.npt, 48 * (size_t)qp.nls);
+    const uint8_t* m = pin + L.in + oMv + qp.lo;
+    if (pr.pt_moved && qp.npt) memcpy(pr.pt_moved, m, qp.npt);
+    if (pr.ls_moved && qp.nls) memcpy(pr.ls_moved, m + qp.npt, qp.nls);
+    if (out) { out[p].iters = c.iters; out[p].err = c.err; out[p].lambda = c.lambda; }
+    status[p] = PLF_OK;
+  }
+  if (refused >= 0) {
+    const int l = ctl[refused].zero_lm, npt = hp[refused].npt;
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: %s landmark %d has a zero diagonal entry in its first-pass block (no row constrains it)",
+                    fn, refused, l < npt ? "point" : "line", l < npt ? l : l - npt);
+  }
+  return PLF_OK;
 }

@@ -34,6 +34,7 @@ enum plf_scratch_slot {
   PLF_SCR_KF_MGB_PT,   // plf_match_kf2kf, plf_match_map2kf: the windowed matcher of points
   PLF_SCR_KF_MGB_LS,   //   ... and of lines
   PLF_SCR_BOW,         // plf_bow_insert
+  PLF_SCR_BA_BATCH,    // plf_local_ba_batch: its staged layout
   PLF_SCR_COUNT
 };
 

@@ -529,7 +529,50 @@ class Frontend:
         return self._bundle_adjust("plf_global_ba", prob, lambda_, lambda_k, max_iters, homog_th, min_error,
                                    min_error_change, ref_quirks)
 
-    def _bundle_adjust(self, fn, prob, lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, ref_quirks):
+    def local_ba_batch(self, problems, seq=None, lambda_=1e-5, lambda_k=10.0, max_iters=15, homog_th=1e-7, min_error=1e-7,
+                       min_error_change=1e-7, ref_quirks=1):
+        """Many local BAs in one device call (plf_local_ba_batch), with local_ba's options for all of them.  problems:
+        dicts as local_ba takes; seq: per problem, -1 for the context's camera or a sequence whose camera
+        (sequence_camera) to project with (None = all -1).  Returns one dict per problem in local_ba's shape plus
+        `status` (0, or PLF_ERR_INVALID = -1 when the device refused that problem: a landmark whose first-pass block has a
+        zero diagonal entry; its dict then holds its unchanged inputs and iters / err / lambda_ None).  Raises PlfError
+        for the refusals before any work."""
+        problems = list(problems)
+        P = len(problems)
+        seq_a = self._problem_sequences(P, seq)
+        args = [self._lba_args(p) for p in problems]
+        arr = (plf_lba_problem * max(P, 1))(*[a[0] for a in args])
+        res = (plf_lba_result * max(P, 1))()
+        st = np.full(max(P, 1), 1, np.int32)   # 1 is no plf_status: marks entries the call did not write
+        o = plf_lba_opts(lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, int(ref_quirks))
+        rc = self.lib.plf_local_ba_batch(self._ctx, C.byref(o), P, arr, None if seq_a is None else _ptr(seq_a, C.c_int32),
+                                         res, _ptr(st, C.c_int32))
+        if rc != 0 and (P == 0 or np.any(st[:P] == 1)):
+            self._check(rc, "plf_local_ba_batch")
+        out = []
+        for k in range(P):
+            d = self._lba_result(args[k][1], res[k] if st[k] == 0 else None)
+            d["status"] = int(st[k])
+            out.append(d)
+        return out
+
+    @staticmethod
+    def _problem_sequences(P, seq):
+        """seq of local_ba_batch: None, or an integer array of P entries (checked before any library call)."""
+        if seq is None:
+            return None
+        a = np.asarray(seq)
+        if a.shape != (P,) or a.dtype.kind not in "iu":
+            raise PlfError(f"seq must be a 1-D integer array of {P} entries (got {a.dtype}{list(a.shape)})")
+        s = np.ascontiguousarray(a, np.int32)
+        if not np.array_equal(s, a):
+            raise PlfError("seq: values do not fit int32")
+        return s
+
+    @staticmethod
+    def _lba_args(prob):
+        """(plf_lba_problem, arrays): copies of a problem dict's arrays, which the call updates in place, and the struct
+        that points at them."""
         f64 = lambda a, c: np.ascontiguousarray(a, np.float64).reshape(-1, c).copy()
         i32 = lambda a: np.ascontiguousarray(a, np.int32).ravel().copy()
         kf, pt, ls = f64(prob["kf_pose"], 6), f64(prob["pt"], 3), f64(prob["ls"], 6)
@@ -540,11 +583,23 @@ class Frontend:
         ad = lambda a: a.ctypes.data if a.size else None
         p = plf_lba_problem(len(kf), len(pt), len(ls), len(fT), ad(kf), ad(pt), ad(ls), ad(fT), len(po_lm), ad(po_lm), ad(po_kf),
                             ad(po_xy), len(lo_lm), ad(lo_lm), ad(lo_kf), ad(lo_le), ad(pm), ad(lm))
+        arrays = dict(kf_pose=kf, pt=pt, ls=ls, fT=fT, po=(po_lm, po_kf, po_xy), lo=(lo_lm, lo_kf, lo_le), pm=pm, lm=lm)
+        return p, arrays
+
+    @staticmethod
+    def _lba_result(a, res):
+        """local_ba's result dict from _lba_args' arrays and a plf_lba_result (None: no result, the inputs unchanged)."""
+        n_pt, n_ls = len(a["pt"]), len(a["ls"])
+        return dict(kf_pose=a["kf_pose"], pt=a["pt"], ls=a["ls"], pt_moved=a["pm"][:n_pt].astype(bool),
+                    ls_moved=a["lm"][:n_ls].astype(bool), iters=None if res is None else res.iters,
+                    err=None if res is None else res.err, lambda_=None if res is None else res.lambda_)
+
+    def _bundle_adjust(self, fn, prob, lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, ref_quirks):
+        p, a = self._lba_args(prob)
         o = plf_lba_opts(lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, int(ref_quirks))
         res = plf_lba_result()
         self._check(getattr(self.lib, fn)(self._ctx, C.byref(o), C.byref(p), C.byref(res)), fn)
-        return dict(kf_pose=kf, pt=pt, ls=ls, pt_moved=pm[:len(pt)].astype(bool), ls_moved=lm[:len(ls)].astype(bool),
-                    iters=res.iters, err=res.err, lambda_=res.lambda_)
+        return self._lba_result(a, res)
 
     def pose_graph(self, prob, max_iters=100, lambda_init=1e-10, trace=True):
         """The g2o optimisation of MapHandler::loopClosureOptimizationCovGraphG2O on the device (plf_pose_graph;
