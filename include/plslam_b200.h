@@ -578,8 +578,9 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
  *     it is a first frame (status 2), since its carried frame was triangulated with another camera.
  *   - plf_set_max_sequences drops every sequence's camera; plf_reset_sequence keeps them.
  *   - plf_batch_run and plf_process_batch run sequence 0, so they use sequence 0's camera.
- * The keyframe and back-end operators (plf_match_kf2kf, plf_match_map2kf, plf_loop_closure_pose, plf_gn_pose,
- * plf_local_ba, plf_global_ba) keep using the context's camera. */
+ * The single keyframe and back-end operators (plf_match_kf2kf, plf_match_map2kf, plf_loop_closure_pose, plf_gn_pose,
+ * plf_local_ba, plf_global_ba) keep using the context's camera; plf_match_kf2kf_batch, plf_match_map2kf_batch and
+ * plf_local_ba_batch take a sequence's per problem. */
 plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam);
 /* The calibration the next batch will use for sequence s: its own, or the context's camera. */
 plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out);
@@ -618,10 +619,10 @@ plf_status plf_get_matches(plf_ctx* ctx, int k, plf_match_view* view);
  * window, the match() fallback and the epipolar gate.  The landmark bookkeeping that follows each (new MapPoint / MapLine,
  * observations, full_graph) stays with the caller.  has_points / has_lines, best_lr_matches, matching_f2f_ws,
  * min_pt_matches / min_ls_matches, min_ratio_12_p / min_ratio_12_l, line_sim_th and the camera come from the ctx (SlamConfig
- * inherits them): the context's camera of plf_create, not a sequence's (plf_set_sequence_camera).  Work is enqueued on
- * plf_stream, so a call between batches in flight is safe.  A kind returns 0 (every entry -1) when it is disabled or the
- * keyframe has no stereo features of it.  Semantics reproduced as written, quirks
- * included (DESIGN.md 8): see oracle/kfmatching.py. */
+ * inherits them): the single calls use the context's camera of plf_create, the batch calls (plf_match_kf2kf_batch,
+ * plf_match_map2kf_batch) a sequence's per problem (plf_set_sequence_camera).  Work is enqueued on plf_stream, so a call
+ * between batches in flight is safe.  A kind returns 0 (every entry -1) when it is disabled or the keyframe has no stereo
+ * features of it.  Semantics reproduced as written, quirks included (DESIGN.md 8): see oracle/kfmatching.py. */
 typedef struct plf_kf_match_opts {
   int fast_matching;    /* SlamConfig::fastMatching  src/slamConfig.cpp:43: 0 = brute-force match() only, and only when
                            the fallback condition holds (else no pairs) */
@@ -662,6 +663,51 @@ typedef struct plf_local_map {
 plf_status plf_match_map2kf(plf_ctx* ctx, const plf_kf_match_opts* opts, const plf_local_map* map, const double Twf[16],
                             const plf_frame_view* kf, const int32_t* kf_pt_lm, const int32_t* kf_ls_lm, int32_t* lm_pt,
                             int32_t* lm_ls, int* n_pt, int* n_ls);
+
+/* Many keyframe matchings in one call: the new keyframes of several sequences, each against its previous keyframe
+ * (plf_match_kf2kf_batch) or its local map (plf_match_map2kf_batch), each with its sequence's camera, in one upload, one
+ * launch chain and one download with one host synchronisation.
+ *   problems [n_problems]  the single call's inputs and outputs per problem (n_pt / n_ls: its return values)
+ *   seq      [n_problems]  or NULL: the camera of problem p, as in plf_local_ba_batch.  seq[p] = -1 (or seq NULL) uses
+ *                          the context's camera; 0 <= seq[p] < n (plf_set_max_sequences) uses what
+ *                          plf_get_sequence_camera(ctx, seq[p]) returns at the time of the call.  Only fx, fy, cx and cy
+ *                          enter; the image size and the grid scales stay the context's.
+ * Problem p's outputs are bit-identical to what the single call returns for its inputs on a context created with its
+ * camera and the same parameters.  One opts and the context's parameters apply to every problem.
+ * Refusals before any work: PLF_ERR_INVALID when n_problems < 0, a seq entry is out of range, or a problem breaks a
+ * host-side rule of the single call (NULL arrays with a count > 0, a NaN in DT / Twf, more than 8192 features or 65535
+ * landmarks per kind); PLF_ERR_CAPACITY when n_problems > 65535 (the grids' y dimension; no chunking).  The message names
+ * the problem index and the rule, and nothing is written: unlike the single call, no output is pre-filled.
+ * n_problems = 0 returns PLF_OK.  The context stays usable after any error.
+ * Launches: 5 per kind active in some problem, plus the windowed matcher's 3 (points) / 4 (lines) per chunk of problems
+ * when fast_matching, plus 2 or 3 (best_lr_matches) per kind when some problem can take the match() fallback; they do
+ * not depend on n_problems while the matcher's problems fit one chunk.  Device scratch: the single call's per problem, except
+ * that the windowed matcher's arrays are sized at the batch's largest counts K (queries) and Kt (train) per kind, so one
+ * large map pads every problem of the batch to its size.  Its distance matrix takes 2 K Kt bytes per problem and kind,
+ * in chunks of at most 2 GB (a batch beyond one chunk costs the matcher's launches once per chunk). */
+typedef struct plf_kf2kf_problem {
+  const plf_frame_view* prev;   /* read as plf_match_kf2kf reads it */
+  const plf_frame_view* curr;
+  double DT[16];                /* row-major MapHandler::DT */
+  int32_t* m_pt;                /* out [prev->n_pt] */
+  int32_t* m_ls;                /* out [prev->n_ls] */
+  int n_pt, n_ls;               /* out: the reference's return values */
+} plf_kf2kf_problem;
+plf_status plf_match_kf2kf_batch(plf_ctx* ctx, const plf_kf_match_opts* opts, int n_problems, plf_kf2kf_problem* problems,
+                                 const int32_t* seq);
+
+typedef struct plf_map2kf_problem {
+  const plf_local_map* map;
+  const plf_frame_view* kf;     /* read as plf_match_map2kf reads it */
+  double Twf[16];               /* row-major MapHandler::Twf */
+  const int32_t* kf_pt_lm;      /* [kf->n_pt] or NULL = all unmatched */
+  const int32_t* kf_ls_lm;      /* [kf->n_ls] or NULL */
+  int32_t* lm_pt;               /* out [map->n_pt] */
+  int32_t* lm_ls;               /* out [map->n_ls] */
+  int n_pt, n_ls;               /* out: the reference's return values */
+} plf_map2kf_problem;
+plf_status plf_match_map2kf_batch(plf_ctx* ctx, const plf_kf_match_opts* opts, int n_problems, plf_map2kf_problem* problems,
+                                  const int32_t* seq);
 
 /* ------------------------------------------------------------------------------------------------
  * Place recognition: DBoW2 bag-of-words vectors and L1 scores (SURVEY 8(f) f5)

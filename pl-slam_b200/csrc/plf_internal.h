@@ -30,8 +30,8 @@ enum plf_scratch_slot {
   PLF_SCR_LSD,         // plf_lsd, plf_detect_lines, plf_debug_sincosf
   PLF_SCR_MGB_PIPE,    // the windowed matcher of plf_batch_run (matching_strategy != 0)
   PLF_SCR_BA,          // plf_local_ba, plf_global_ba, plf_pose_graph
-  PLF_SCR_KF,          // plf_match_kf2kf, plf_match_map2kf: their staged layout
-  PLF_SCR_KF_MGB_PT,   // plf_match_kf2kf, plf_match_map2kf: the windowed matcher of points
+  PLF_SCR_KF,          // plf_match_kf2kf, plf_match_map2kf and their _batch forms: their staged layout
+  PLF_SCR_KF_MGB_PT,   // plf_match_kf2kf, plf_match_map2kf and their _batch forms: the windowed matcher of points
   PLF_SCR_KF_MGB_LS,   //   ... and of lines
   PLF_SCR_BOW,         // plf_bow_insert
   PLF_SCR_BA_BATCH,    // plf_local_ba_batch: its staged layout

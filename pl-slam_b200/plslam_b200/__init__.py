@@ -161,6 +161,17 @@ class plf_local_map(C.Structure):
                 ("n_ls", C.c_int), ("ls_X", C.c_void_p), ("ls_desc", C.c_void_p), ("ls_use", C.c_void_p)]
 
 
+class plf_kf2kf_problem(C.Structure):
+    _fields_ = [("prev", C.POINTER(plf_frame_view)), ("curr", C.POINTER(plf_frame_view)), ("DT", C.c_double * 16),
+                ("m_pt", C.c_void_p), ("m_ls", C.c_void_p), ("n_pt", C.c_int), ("n_ls", C.c_int)]
+
+
+class plf_map2kf_problem(C.Structure):
+    _fields_ = [("map", C.POINTER(plf_local_map)), ("kf", C.POINTER(plf_frame_view)), ("Twf", C.c_double * 16),
+                ("kf_pt_lm", C.c_void_p), ("kf_ls_lm", C.c_void_p), ("lm_pt", C.c_void_p), ("lm_ls", C.c_void_p),
+                ("n_pt", C.c_int), ("n_ls", C.c_int)]
+
+
 class plf_vocab(C.Structure):
     _fields_ = [("k", C.c_int), ("L", C.c_int), ("scoring", C.c_int), ("weighting", C.c_int), ("n_nodes", C.c_int),
                 ("node_id", C.c_void_p), ("parent_id", C.c_void_p), ("weight", C.c_void_p), ("desc", C.c_void_p),
@@ -220,7 +231,33 @@ def _frame_view(frame, keep):
     return v
 
 
-RESULT_DTYPE = np.dtype([("DT", np.float64, (4, 4)), ("DT_cov", np.float64, (6, 6)), ("err", np.float64),
+def _local_map(local_map, kf_view, kf_pt_lm, kf_ls_lm, keep, who):
+    """(plf_local_map, kf_pt_lm, kf_ls_lm) over a match_map2kf local-map dict and the keyframe's landmark indices (arrays
+    or None), checked against the keyframe's feature counts; `keep` holds the copies alive."""
+    m = plf_local_map()
+
+    def arr(a, dt, cols):
+        a = np.ascontiguousarray(a, dt).reshape(-1, cols) if cols else np.ascontiguousarray(a, dt).ravel()
+        keep.append(a)
+        return a
+    for key, cols in (("pt", 3), ("ls", 6)):
+        X = arr(local_map.get(key + "_X", np.zeros((0, cols))), np.float64, cols)
+        d = arr(local_map.get(key + "_desc", np.zeros((0, 32))), np.uint8, 32)
+        u = local_map.get(key + "_use")
+        setattr(m, "n_" + key, len(X))
+        setattr(m, key + "_X", X.ctypes.data if X.size else None)
+        setattr(m, key + "_desc", d.ctypes.data if d.size else None)
+        if u is not None:
+            u = arr(np.asarray(u).astype(np.uint8), np.uint8, 0)
+            setattr(m, key + "_use", u.ctypes.data if u.size else None)
+    lms = [None if v is None else arr(v, np.int32, 0) for v in (kf_pt_lm, kf_ls_lm)]
+    for a, n, name in ((lms[0], kf_view.n_pt, "kf_pt_lm"), (lms[1], kf_view.n_ls, "kf_ls_lm")):
+        if a is not None and len(a) != n:
+            raise PlfError(f"{who}: {name} has {len(a)} entries for {n} keyframe features")
+    return m, lms[0], lms[1]
+
+
+RESULT_DTYPE =np.dtype([("DT", np.float64, (4, 4)), ("DT_cov", np.float64, (6, 6)), ("err", np.float64),
                          ("status", np.int32), ("n_kp_l", np.int32), ("n_kp_r", np.int32), ("n_lines_l", np.int32),
                          ("n_lines_r", np.int32), ("n_stereo_pt", np.int32), ("n_stereo_ls", np.int32),
                          ("n_matched_pt", np.int32), ("n_matched_ls", np.int32), ("n_inliers_pt", np.int32),
@@ -558,7 +595,8 @@ class Frontend:
 
     @staticmethod
     def _problem_sequences(P, seq):
-        """seq of local_ba_batch: None, or an integer array of P entries (checked before any library call)."""
+        """seq of the batch calls (local_ba_batch, match_*_batch): None, or an integer array of P entries (checked before
+        any library call)."""
         if seq is None:
             return None
         a = np.asarray(seq)
@@ -645,26 +683,7 @@ class Frontend:
         feature (-1 = unmatched) or None.  Returns dict(lm_pt, n_pt, lm_ls, n_ls)."""
         keep = []
         kv = _frame_view(kf, keep)
-        m = plf_local_map()
-
-        def arr(a, dt, cols):
-            a = np.ascontiguousarray(a, dt).reshape(-1, cols) if cols else np.ascontiguousarray(a, dt).ravel()
-            keep.append(a)
-            return a
-        for key, cols in (("pt", 3), ("ls", 6)):
-            X = arr(local_map.get(key + "_X", np.zeros((0, cols))), np.float64, cols)
-            d = arr(local_map.get(key + "_desc", np.zeros((0, 32))), np.uint8, 32)
-            u = local_map.get(key + "_use")
-            setattr(m, "n_" + key, len(X))
-            setattr(m, key + "_X", X.ctypes.data if X.size else None)
-            setattr(m, key + "_desc", d.ctypes.data if d.size else None)
-            if u is not None:
-                u = arr(np.asarray(u).astype(np.uint8), np.uint8, 0)
-                setattr(m, key + "_use", u.ctypes.data if u.size else None)
-        lms = [None if v is None else arr(v, np.int32, 0) for v in (kf_pt_lm, kf_ls_lm)]
-        for a, n, name in ((lms[0], kv.n_pt, "kf_pt_lm"), (lms[1], kv.n_ls, "kf_ls_lm")):
-            if a is not None and len(a) != n:
-                raise PlfError(f"match_map2kf: {name} has {len(a)} entries for {n} keyframe features")
+        m, *lms = _local_map(local_map, kv, kf_pt_lm, kf_ls_lm, keep, "match_map2kf")
         T = np.ascontiguousarray(Twf, np.float64).reshape(16)
         o = plf_kf_match_opts(int(bool(fast_matching)), float(max_kf_epip_p), float(max_kf_epip_l))
         lm_pt, lm_ls = np.full(max(m.n_pt, 1), -1, np.int32), np.full(max(m.n_ls, 1), -1, np.int32)
@@ -674,6 +693,54 @@ class Frontend:
                                               lm_pt.ctypes.data_as(C.c_void_p), lm_ls.ctypes.data_as(C.c_void_p),
                                               C.byref(n_pt), C.byref(n_ls)), "plf_match_map2kf")
         return dict(lm_pt=lm_pt[:m.n_pt].copy(), n_pt=n_pt.value, lm_ls=lm_ls[:m.n_ls].copy(), n_ls=n_ls.value)
+
+    def match_kf2kf_batch(self, problems, seq=None, fast_matching=True, max_kf_epip_p=1.0, max_kf_epip_l=1.0):
+        """Many match_kf2kf in one device call (plf_match_kf2kf_batch), with one set of options.  problems: dicts
+        prev, curr (get_frame dicts) and DT (4x4); seq: per problem, -1 for the context's camera or a sequence whose
+        camera (sequence_camera) to project with (None = all -1).  Returns one match_kf2kf dict per problem."""
+        problems = list(problems)
+        P = len(problems)
+        seq_a = self._problem_sequences(P, seq)
+        keep, outs = [], []
+        arr = (plf_kf2kf_problem * max(P, 1))()
+        for k, pr in enumerate(problems):
+            p, c = _frame_view(pr["prev"], keep), _frame_view(pr["curr"], keep)
+            keep += [p, c]
+            m_pt, m_ls = np.full(max(p.n_pt, 1), -1, np.int32), np.full(max(p.n_ls, 1), -1, np.int32)
+            outs.append((m_pt[:p.n_pt], m_ls[:p.n_ls]))
+            arr[k] = plf_kf2kf_problem(C.pointer(p), C.pointer(c), (C.c_double * 16)(*np.asarray(pr["DT"], np.float64).ravel()),
+                                       m_pt.ctypes.data, m_ls.ctypes.data, 0, 0)
+            keep += [m_pt, m_ls]
+        o = plf_kf_match_opts(int(bool(fast_matching)), float(max_kf_epip_p), float(max_kf_epip_l))
+        self._check(self.lib.plf_match_kf2kf_batch(self._ctx, C.byref(o), P, arr,
+                                                   None if seq_a is None else _ptr(seq_a, C.c_int32)), "plf_match_kf2kf_batch")
+        return [dict(m_pt=m_pt.copy(), n_pt=arr[k].n_pt, m_ls=m_ls.copy(), n_ls=arr[k].n_ls) for k, (m_pt, m_ls) in enumerate(outs)]
+
+    def match_map2kf_batch(self, problems, seq=None, fast_matching=True, max_kf_epip_p=1.0, max_kf_epip_l=1.0):
+        """Many match_map2kf in one device call (plf_match_map2kf_batch), with one set of options.  problems: dicts
+        local_map, Twf, kf and optionally kf_pt_lm / kf_ls_lm, as match_map2kf takes them; seq: as match_kf2kf_batch.
+        Returns one match_map2kf dict per problem."""
+        problems = list(problems)
+        P = len(problems)
+        seq_a = self._problem_sequences(P, seq)
+        keep, outs = [], []
+        arr = (plf_map2kf_problem * max(P, 1))()
+        ad = lambda a: None if a is None or not a.size else a.ctypes.data
+        for k, pr in enumerate(problems):
+            kv = _frame_view(pr["kf"], keep)
+            m, pt_lm, ls_lm = _local_map(pr["local_map"], kv, pr.get("kf_pt_lm"), pr.get("kf_ls_lm"), keep,
+                                         f"match_map2kf_batch: problem {k}")
+            keep += [kv, m]
+            lm_pt, lm_ls = np.full(max(m.n_pt, 1), -1, np.int32), np.full(max(m.n_ls, 1), -1, np.int32)
+            outs.append((lm_pt[:m.n_pt], lm_ls[:m.n_ls]))
+            arr[k] = plf_map2kf_problem(C.pointer(m), C.pointer(kv), (C.c_double * 16)(*np.asarray(pr["Twf"], np.float64).ravel()),
+                                        ad(pt_lm), ad(ls_lm), lm_pt.ctypes.data, lm_ls.ctypes.data, 0, 0)
+            keep += [lm_pt, lm_ls]
+        o = plf_kf_match_opts(int(bool(fast_matching)), float(max_kf_epip_p), float(max_kf_epip_l))
+        self._check(self.lib.plf_match_map2kf_batch(self._ctx, C.byref(o), P, arr,
+                                                    None if seq_a is None else _ptr(seq_a, C.c_int32)), "plf_match_map2kf_batch")
+        return [dict(lm_pt=lm_pt.copy(), n_pt=arr[k].n_pt, lm_ls=lm_ls.copy(), n_ls=arr[k].n_ls)
+                for k, (lm_pt, lm_ls) in enumerate(outs)]
 
     # -- place recognition (DBoW2) -----------------------------------------------------------------
     def bow_set_vocabulary(self, kind, voc):
