@@ -34,7 +34,8 @@ enum {
   PLF_ERR_INVALID = -1,   /* bad argument */
   PLF_ERR_NO_DEVICE = -2, /* no CUDA device / CUDA runtime failure at create */
   PLF_ERR_CUDA = -3,      /* CUDA runtime error during a call */
-  PLF_ERR_CAPACITY = -4,  /* a fixed-capacity device buffer overflowed (see plf_limits) */
+  PLF_ERR_CAPACITY = -4,  /* a fixed-capacity device buffer overflowed: a plf_limits field or one of the internal
+                           * capacities listed below plf_limits; plf_last_error names the one that was hit */
   PLF_ERR_STATE = -5      /* call sequence error */
 };
 
@@ -97,6 +98,19 @@ typedef struct plf_limits {
   int max_segments;  /* raw LSD segments per image */
   int max_lines;     /* KeyLines kept per image after the top-K */
 } plf_limits;
+/* Internal capacities of the extraction kernels, not fields of plf_limits (DESIGN.md section 8).  Rendered and natural
+ * images stay far below them; an image built for it can reach each, the call then returns PLF_ERR_CAPACITY, never a
+ * truncated result, and plf_last_error names it - raising plf_limits does not move them:
+ *   ORB_SORT_CAP = 4096   keypoints kept on ONE pyramid level (csrc/orb.cu, k_select_sort).  retainBest keeps every
+ *                         corner that ties the level's threshold score, so a binary image of several thousand equal
+ *                         corners reaches it whatever orb_nfeatures is; so does an orb_nfeatures that gives one level a
+ *                         share above 4096 (about 12 700 at 4 levels) on an image with that many corners.  At the default
+ *                         max_keypoints (4096) the declared limit is always met first.
+ *   candidate capacity    FAST corners (after the 3 x 3 suppression) of ONE pyramid level: min(w h / 9 + 64, 32768) of
+ *                         the level's size (csrc/orb.cu, k_fast_nms).  Isolated bright pixels every 4 columns and rows
+ *                         give w h / 16 corners: above 32768 from about 760 x 760 or 1280 x 720 upwards.
+ *   KL_SORT_CAP = 4096    KeyLines of one image that can be ranked for the top lsd_nfeatures (csrc/lsd.cu, k_keylines);
+ *                         lsd_nfeatures = 0 ranks nothing and is bounded by max_segments / max_lines only. */
 
 /* Fills *p with the reference defaults (config/config/config_euroc.yaml). */
 void plf_default_params(plf_params* p);
@@ -201,7 +215,8 @@ typedef struct plf_keypoint {
  * Output order is canonical (octave, y, x): OpenCV's own order inside a level is the implementation-defined
  * result of std::nth_element (KeyPointsFilter::retainBest); the SET of keypoints, every field and every
  * descriptor are identical to OpenCV's.  kps/desc: host buffers with room for `cap` entries; *n receives
- * the count (PLF_ERR_CAPACITY if it exceeds cap or the ctx limit max_keypoints).  Work is enqueued on plf_stream in a
+ * the count (PLF_ERR_CAPACITY if it exceeds cap, the ctx limit max_keypoints or an internal capacity listed below
+ * plf_limits; nothing is written to kps / desc then, and the next call starts clean).  Work is enqueued on plf_stream in a
  * working state of its own (one image, rebuilt when the image size changes) and never touches the batched pipeline's
  * buffers, so a call between batches in flight is safe. */
 plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, plf_keypoint* kps,
@@ -229,7 +244,8 @@ typedef struct plf_keyline {
 /* Raw LSD segments.  Replaces cv::createLineSegmentDetector(lsd_refine (0), lsd_scale, lsd_sigma_scale, lsd_quant,
  * lsd_ang_th, lsd_log_eps, lsd_density_th, lsd_n_bins)->detect(img, lines) as called at
  * 3rdparty/line_descriptor/src/LSDDetector_custom.cpp:246-264.  segs: cap x 4 floats (x1,y1,x2,y2), OpenCV's
- * output order (seed order).  *n receives the count.  Work is enqueued on plf_stream in a working state of its own (one
+ * output order (seed order).  *n receives the count (PLF_ERR_CAPACITY beyond cap or max_segments: nothing is written to
+ * segs, and the next call starts clean).  Work is enqueued on plf_stream in a working state of its own (one
  * image, rebuilt when the image size changes, shared with plf_detect_lines) and never touches the batched pipeline's
  * buffers, so a call between batches in flight is safe. */
 plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, float* segs, int cap, int* n);
@@ -238,7 +254,8 @@ plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, f
  * LSDDetectorC::detect(img, lines, scale, 1, opts) (LSDDetector_custom.cpp:218-324, opts.min_length =
  * min_line_length * min(w,h)), then — when more than lsd_nfeatures lines are found and lsd_nfeatures != 0 — sort by
  * response (descending; ties keep detection order), keep lsd_nfeatures and set class_id = rank, then
- * BinaryDescriptor::compute (binary_descriptor_custom.cpp:524).  keylines/desc: host buffers of `cap` entries.
+ * BinaryDescriptor::compute (binary_descriptor_custom.cpp:524).  keylines/desc: host buffers of `cap` entries
+ * (PLF_ERR_CAPACITY beyond cap, max_segments, max_lines or - when lines are ranked - KL_SORT_CAP).
  * Enqueued on plf_stream in plf_lsd's working state; never touches the batched pipeline's buffers, so a call between
  * batches in flight is safe. */
 plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride,
@@ -546,7 +563,13 @@ plf_status plf_process_batch(plf_ctx* ctx, int B, const uint8_t* left, const uin
  * most recent upload) -> download (waits for the OLDEST batch in flight and returns its B results).
  * Batches are software-pipelined on the device: up to THREE may be in flight (run, run, run, download, run, ...);
  * a fourth plf_batch_run returns PLF_ERR_STATE.  Results are identical to run/download pairs.  plf_get_frame /
- * plf_get_matches refer to the batch most recently RUN, so call them with a single batch in flight. */
+ * plf_get_matches refer to the batch most recently RUN, so call them with a single batch in flight.
+ * plf_batch_download returns PLF_ERR_CAPACITY when an image of THAT batch overflowed a capacity (the batches in flight
+ * before and after it are not affected, and the message names the kind and the limit).  out[] is written all the same:
+ * the rows of pairs whose own images and whose sequence's previous frame stayed within the capacities are exact; the row
+ * of the overflowing pair is computed from its truncated feature lists (counts never exceed the limits) and is not the
+ * reference's result.  That pair's truncated frame is also what its sequence carries, so restart the sequence
+ * (plf_batch_run_sequences, restart[k] = 1) with its next pair; INTEGRATION.md section 4a. */
 plf_status plf_batch_upload(plf_ctx* ctx, int B, const uint8_t* left, const uint8_t* right, int stride);
 plf_status plf_batch_run(plf_ctx* ctx, int B);
 plf_status plf_batch_download(plf_ctx* ctx, int B, plf_frame_result* out);

@@ -838,7 +838,7 @@ __device__ __forceinline__ void lsd_grow_body(LsdPix* __restrict__ pix_all, size
           ++nreg_out;
           cursor += nreg;
         } else if (lane == 0) {
-          *overflow = 1;
+          atomicOr(overflow, PLF_LSD_OVF_SEGMENTS);
         }
       }
       pending &= ~((2u << src) - 1u);
@@ -1062,7 +1062,7 @@ __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ se
   if (nfeatures != 0 && m > nfeatures) {
     // stvo-pl: sort by response (descending), keep nfeatures, class_id = rank.  Ties: detection order.
     if (m > KL_SORT_CAP) {
-      if (tid == 0) *overflow = 1;
+      if (tid == 0) atomicOr(overflow, PLF_LSD_OVF_SORT);
     }
     const int mm = min(m, KL_SORT_CAP);
     int p2 = 1;
@@ -1093,7 +1093,7 @@ __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ se
       }
     keep = nfeatures;
     if (keep > max_lines) {
-      if (tid == 0) *overflow = 1;
+      if (tid == 0) atomicOr(overflow, PLF_LSD_OVF_LINES);
       keep = max_lines;
     }
     for (int i = tid; i < keep; i += 1024) {
@@ -1103,7 +1103,7 @@ __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ se
     }
   } else {
     if (keep > max_lines) {
-      if (tid == 0) *overflow = 1;
+      if (tid == 0) atomicOr(overflow, PLF_LSD_OVF_LINES);
       keep = max_lines;
     }
     for (int i = tid; i < keep; i += 1024) out[i] = all[i];
@@ -1374,6 +1374,22 @@ plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int
 
 int* plf_lsd_overflow_flag(const LsdState* s) { return s->overflow; }
 
+// Names every limit in `causes`.  max_segments and max_lines are plf_limits fields; KL_SORT_CAP is a fixed capacity of
+// k_keylines that raising plf_limits does not move (lsd_nfeatures = 0 does not rank and has no such bound).
+void plf_lsd_overflow_text(const LsdState* s, int causes, char* buf, size_t len) {
+  char seg[96] = "", lines[96] = "", sort[160] = "";
+  if (causes & PLF_LSD_OVF_SEGMENTS)
+    snprintf(seg, sizeof seg, "more segments in an image than plf_limits.max_segments=%d; ", s->max_regions);
+  if (causes & PLF_LSD_OVF_LINES)
+    snprintf(lines, sizeof lines, "more lines to return from an image than plf_limits.max_lines=%d; ", s->max_lines);
+  if (causes & PLF_LSD_OVF_SORT)
+    snprintf(sort, sizeof sort, "more than KL_SORT_CAP=%d lines to rank for the top lsd_nfeatures (internal, not a plf_limits "
+             "field); ", KL_SORT_CAP);
+  snprintf(buf, len, "%s%s%s", seg, lines, sort);
+  const size_t n = strlen(buf);
+  if (n >= 2) buf[n - 2] = 0;   // the last "; "
+}
+
 void plf_lsd_outputs(const LsdState* s, int par, plf_keyline** kls, int** nlines, int* max_lines) {
   *kls = s->kls[par]; *nlines = s->nlines[par]; *max_lines = s->max_lines;
 }
@@ -1392,14 +1408,18 @@ static plf_status lsd_standalone(plf_ctx* ctx, const uint8_t* dimg, int pitch, i
   return plf_lsd_grow(ctx, ctx->stream, s, 0, 1, nullptr);
 }
 
-static plf_status lsd_check_overflow(plf_ctx* ctx, const LsdState* s, const char* what) {
+// `causes`: the ones that spoil what the caller returns.  plf_lsd returns the raw segments, which the KeyLine stage's
+// capacities (it runs all the same) do not touch.
+static plf_status lsd_check_overflow(plf_ctx* ctx, const LsdState* s, const char* what, int causes) {
   int ovf = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&ovf, s->overflow, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (ovf) cudaMemsetAsync(s->overflow, 0, sizeof(int), ctx->stream);
+  ovf &= causes;
   if (ovf) {
-    cudaMemsetAsync(s->overflow, 0, sizeof(int), ctx->stream);
-    return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: segment/line capacity exceeded (max_segments=%d, max_lines=%d)", what,
-                    s->max_regions, s->max_lines);
+    char why[400];
+    plf_lsd_overflow_text(s, ovf, why, sizeof why);
+    return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: segment/line capacity exceeded: %s", what, why);
   }
   return PLF_OK;
 }
@@ -1418,7 +1438,7 @@ extern "C" plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   const LsdState* s = ctx->lsd_standalone;
   int n = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->nregions, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  st = lsd_check_overflow(ctx, s, "plf_lsd");
+  st = lsd_check_overflow(ctx, s, "plf_lsd", PLF_LSD_OVF_SEGMENTS);
   if (st) return st;
   *n_out = n;
   if (n > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_lsd: %d segments > caller capacity %d", n, cap);
@@ -1451,7 +1471,7 @@ extern "C" plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, 
   if (st) return st;
   int n = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->nlines[0], sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  st = lsd_check_overflow(ctx, s, "plf_detect_lines");
+  st = lsd_check_overflow(ctx, s, "plf_detect_lines", PLF_LSD_OVF_SEGMENTS | PLF_LSD_OVF_LINES | PLF_LSD_OVF_SORT);
   if (st) return st;
   *n_out = n;
   if (n > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_detect_lines: %d lines > caller capacity %d", n, cap);

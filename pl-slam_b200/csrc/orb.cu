@@ -344,7 +344,7 @@ __global__ void __launch_bounds__(256, 5) k_fast_nms(const __grid_constant__ CUt
     if (slot < g.cand_cap[l])
       cand[(size_t)img * g.cand_stride + g.cand_off[l] + slot] = ((uint32_t)gy << 20) | ((uint32_t)gx << 8) | (uint32_t)s;
     else
-      *overflow = 1;
+      atomicOr(overflow, PLF_ORB_OVF_CANDIDATES);
     atomicAdd(&hist[(img * ORB_MAX_LEVELS + l) * 256 + s], 1);
   }
 }
@@ -395,7 +395,7 @@ __global__ void __launch_bounds__(1024) k_select_sort(OrbGeom g, const uint32_t*
     __syncthreads();
     int m = s_cnt;
     if (m > ORB_SORT_CAP) {
-      if (tid == 0) *overflow = 1;
+      if (tid == 0) atomicOr(overflow, PLF_ORB_OVF_SORT);
       m = ORB_SORT_CAP;
     }
     int p2 = 1;
@@ -433,7 +433,7 @@ __global__ void __launch_bounds__(1024) k_select_sort(OrbGeom g, const uint32_t*
         kps[(size_t)img * g.max_kp + o] = kp;
         kp_lxy[(size_t)img * g.max_kp + o] = make_short2((short)x, (short)y);
       } else if (i == m - 1) {
-        *overflow = 1;
+        atomicOr(overflow, PLF_ORB_OVF_KEYPOINTS);
       }
     }
     base = min(base + m, g.max_kp);
@@ -841,6 +841,25 @@ plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t
 
 int* plf_orb_overflow_flag(const OrbState* s) { return s->overflow; }
 
+// Names every limit in `causes`.  Only max_keypoints is a plf_limits field; the other two are fixed capacities of the
+// kernels, per pyramid level, and raising plf_limits does not move them.
+void plf_orb_overflow_text(const OrbState* s, int causes, char* buf, size_t len) {
+  int largest = 0;
+  for (int l = 0; l < s->g.nlevels; ++l) largest = std::max(largest, s->g.cand_cap[l]);
+  char kp[96] = "", sort[128] = "", cand[160] = "";
+  if (causes & PLF_ORB_OVF_KEYPOINTS)
+    snprintf(kp, sizeof kp, "more keypoints in an image than plf_limits.max_keypoints=%d; ", s->g.max_kp);
+  if (causes & PLF_ORB_OVF_SORT)
+    snprintf(sort, sizeof sort, "more than ORB_SORT_CAP=%d keypoints kept on one pyramid level (internal, not a plf_limits field); ",
+             ORB_SORT_CAP);
+  if (causes & PLF_ORB_OVF_CANDIDATES)
+    snprintf(cand, sizeof cand, "more FAST corners on one pyramid level than its candidate capacity, at most %d here (internal, "
+             "not a plf_limits field); ", largest);
+  snprintf(buf, len, "%s%s%s", kp, sort, cand);
+  const size_t n = strlen(buf);
+  if (n >= 2) buf[n - 2] = 0;   // the last "; "
+}
+
 // device-side accessors for the pipeline
 void plf_orb_outputs(const OrbState* s, int par, plf_keypoint** kps, uint8_t** desc, int** counts, int* max_kp) {
   *kps = s->kps[par]; *desc = s->desc[par]; *counts = s->kp_count[par]; *max_kp = s->g.max_kp;
@@ -870,7 +889,9 @@ extern "C" plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (ovf) {
     cudaMemsetAsync(s->overflow, 0, sizeof(int), ctx->stream);
-    return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_orb: keypoint capacity exceeded (max_keypoints=%d)", s->g.max_kp);
+    char why[400];
+    plf_orb_overflow_text(s, ovf, why, sizeof why);
+    return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_orb: keypoint capacity exceeded: %s", why);
   }
   *n_out = n;
   if (n > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_orb: %d keypoints > caller capacity %d", n, cap);

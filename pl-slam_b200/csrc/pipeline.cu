@@ -1065,8 +1065,11 @@ plf_status plf_batch_download(plf_ctx* ctx, int B, plf_frame_result* out) {
   // an overflow of a disabled kind's extraction buffers does not reach the results
   const int o0 = ctx->params.has_points ? s->h_ovf[par][0] : 0, o1 = ctx->params.has_lines ? s->h_ovf[par][1] : 0;
   if (o0 || o1) {
-    return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_batch_download: a fixed-capacity buffer overflowed (%s%s); raise plf_limits",
-                    o0 ? "ORB keypoints " : "", o1 ? "LSD segments/lines" : "");
+    char why0[400] = "", why1[400] = "";
+    if (o0) plf_orb_overflow_text(s->orb, o0, why0, sizeof why0);
+    if (o1) plf_lsd_overflow_text(s->lsd, o1, why1, sizeof why1);
+    return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_batch_download: a fixed-capacity buffer overflowed in this batch (%s%s%s%s%s)",
+                    o0 ? "ORB keypoints: " : "", why0, o0 && o1 ? "; " : "", o1 ? "LSD segments/lines: " : "", why1);
   }
   return PLF_OK;
 }

@@ -241,7 +241,13 @@ plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_paritie
 void plf_orb_free(OrbState* s);
 plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par);
 void plf_orb_outputs(const OrbState* s, int par, plf_keypoint** kps, uint8_t** desc, int** counts, int* max_kp);
+// The overflow flag is a set of causes (one bit each, OR-ed in by the kernel that met it); plf_orb_overflow_text words them,
+// naming the limit that was actually hit: only max_keypoints is the caller's to raise.
+enum { PLF_ORB_OVF_KEYPOINTS = 1,    // an image has more keypoints than plf_limits.max_keypoints (k_select_sort)
+       PLF_ORB_OVF_SORT = 2,         // one pyramid level keeps more than ORB_SORT_CAP keypoints (k_select_sort)
+       PLF_ORB_OVF_CANDIDATES = 4 }; // one pyramid level has more FAST corners than its candidate list holds (k_fast_nms)
 int* plf_orb_overflow_flag(const OrbState* s);
+void plf_orb_overflow_text(const OrbState* s, int causes, char* buf, size_t len);
 void plf_linear_coeffs_host(int srcsize, int dstsize, double scale, int* ofs, int* c1);
 plf_status plf_launch_resize_exact(plf_ctx* ctx, cudaStream_t cs, const uint8_t* src, size_t src_stride, int sp, int sw, int sh, uint8_t* dst,
                                    size_t dst_stride, int dp, int dw, int dh, const int* tabx, const int* tabxp, const int* taby, int nimg);
@@ -261,7 +267,12 @@ plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t
 // keylines_wait: if set, the KeyLine outputs are overwritten only after this event
 plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int n, cudaEvent_t keylines_wait);
 void plf_lsd_outputs(const LsdState* s, int par, plf_keyline** kls, int** nlines, int* max_lines);
+// Causes of the LSD overflow flag, one bit each (as the ORB flag above)
+enum { PLF_LSD_OVF_SEGMENTS = 1,   // an image grows more regions than plf_limits.max_segments (k_lsd_grow)
+       PLF_LSD_OVF_LINES = 2,      // more KeyLines to return than plf_limits.max_lines (k_keylines)
+       PLF_LSD_OVF_SORT = 4 };     // more KeyLines to rank for the top lsd_nfeatures than KL_SORT_CAP (k_keylines)
 int* plf_lsd_overflow_flag(const LsdState* s);
+void plf_lsd_overflow_text(const LsdState* s, int causes, char* buf, size_t len);
 
 void plf_configure_lsd();
 

@@ -69,6 +69,9 @@ FULL = dict(
 REFERENCE_CONFIGS = {"kitti": KITTI, "config": CONFIG, "fast": FAST, "full": FULL}
 
 # cv::ORB::create settings away from the defaults (scale factor 1.2, 4 levels, edge 19, FAST threshold 20)
+# (orb_fast_th 127 and above - the other arm of the packed rejection test - is run by tests/test_adversarial_images*.py
+# on images built for it: the rendered scenes these cases run on keep 38 to 64 corners at 127 / 128 and none at 200, below
+# the 100 that test_orb_param_cases and test_oracle_matches_cv2_param_cases require of every case)
 ORB_CASES = {
     "sf1.1_l8": dict(orb_scale_factor=1.1, orb_nlevels=8),
     "sf1.5_l4": dict(orb_scale_factor=1.5, orb_nlevels=4),
