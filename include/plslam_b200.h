@@ -305,11 +305,35 @@ typedef struct plf_pose_result {
  * sP,eP: nl x 3 (3-D endpoints), le_obs: nl x 3 (observed normalised line), all f64 host arrays;
  * inlier_pt / inlier_ls: u8 flags, in (rows to use) and out (after the chi2 gate).  T_init: row-major
  * 4x4 or NULL (identity).  opts NULL => thresholds from the ctx params (stvo-pl min_error/min_error_change).
- * Projects with the context's camera (plf_create), not a sequence's (plf_set_sequence_camera). */
+ * Projects with the context's camera (plf_create); plf_gn_pose_batch takes a sequence's. */
 plf_status plf_gn_pose(plf_ctx* ctx, const plf_gn_opts* opts, const double* P, const double* pl_obs,
                        uint8_t* inlier_pt, int np, const double* sP, const double* eP,
                        const double* le_obs, uint8_t* inlier_ls, int nl, const double* T_init,
                        plf_pose_result* out);
+
+/* Many pose refinements in one call: the lookForCommonMatches refinements (src/mapHandler.cpp:768-808) of several
+ * sequences' new keyframes, each with its sequence's camera, in one upload, one launch and one download with one host
+ * synchronisation.
+ *   problems [n_problems]  plf_gn_pose's arguments per problem (inlier flags in / out, out: its result)
+ *   seq      [n_problems]  or NULL: the camera of problem p.  seq[p] = -1 (or seq NULL) uses the context's camera;
+ *                          0 <= seq[p] < n (plf_set_max_sequences) uses what plf_get_sequence_camera(ctx, seq[p]) returns
+ *                          at the time of the call.  Only fx, fy, cx and cy enter.
+ * One opts serves every problem (NULL = the ctx params, as plf_gn_pose).  Problem p's out and inlier flags are
+ * bit-identical to what plf_gn_pose returns for it on a context created with its camera: the solver sums in a fixed order,
+ * so the same rows in the same order give the same bits.  plf_gn_pose is this call with one problem.
+ * Refusals before any work, naming the problem and the rule, with nothing written: PLF_ERR_INVALID when n_problems < 0, a
+ * seq entry is out of range, or a count is negative or an array NULL while its count is > 0.  n_problems = 0 returns
+ * PLF_OK and launches nothing.  Launches: 1.  Work is enqueued on plf_stream; device scratch (plf_gn_pose's slot, kept
+ * until plf_destroy): 41 bytes per point row, 73 per line row and about 0.8 KB per problem, each part rounded up to 256
+ * bytes; the context's pinned staging buffer holds the inputs and outputs. */
+typedef struct plf_gn_problem {
+  const double* P; const double* pl_obs; uint8_t* inlier_pt; int np;   /* as plf_gn_pose; inlier flags in / out */
+  const double* sP; const double* eP; const double* le_obs; uint8_t* inlier_ls; int nl;
+  const double* T_init;          /* NULL = identity */
+  plf_pose_result out;           /* out */
+} plf_gn_problem;
+plf_status plf_gn_pose_batch(plf_ctx* ctx, const plf_gn_opts* opts, int n_problems, plf_gn_problem* problems,
+                             const int32_t* seq);
 
 /* Local bundle adjustment (SURVEY 8(f) f4).  Replaces MapHandler::levMarquardtOptimizationLBA (src/mapHandler.cpp:1332-1989),
  * the numerical core of MapHandler::localBundleAdjustment (:1220-1330): Levenberg-Marquardt over the local keyframes'
@@ -500,10 +524,45 @@ typedef struct plf_lc_result {
   double pose_inc[6];  /* accepted only */
 } plf_lc_result;
 /* pt_pairs / ls_pairs: (i1 in kf0, i2 in kf1) per surviving correspondence, capacity cap_* pairs (may be NULL).
- * Uses the context's camera (plf_create), not a sequence's (plf_set_sequence_camera). */
+ * At most 65535 features of a kind per keyframe (the matcher's 16-bit indices).  Uses the context's camera (plf_create);
+ * plf_loop_closure_pose_batch takes a sequence's.  This call is plf_loop_closure_pose_batch with one problem. */
 plf_status plf_loop_closure_pose(plf_ctx* ctx, const plf_lc_params* lc, const plf_lc_keyframe* kf0,
                                  const plf_lc_keyframe* kf1, plf_lc_result* out, int32_t* pt_pairs, int cap_pt,
                                  int32_t* ls_pairs, int cap_ls);
+
+/* Many loop-closure checks in one call: the candidates of several sequences' new keyframes (the loop-closure thread,
+ * src/mapHandler.cpp:1130-1214), each with its sequence's camera, in one upload, one launch chain and one download with
+ * one host synchronisation.
+ *   problems [n_problems]  kf0 = the candidate (map_keyframes[lc_kf_idx]), kf1 = the new keyframe, both read as
+ *                          plf_loop_closure_pose reads them; pt_pairs / cap_pt, ls_pairs / cap_ls as there (may be NULL);
+ *                          out: its result; status: PLF_OK, or PLF_ERR_CAPACITY when its pairs exceed its capacity
+ *   seq      [n_problems]  or NULL: the camera of problem p, as in plf_gn_pose_batch (only fx, fy, cx, cy enter)
+ * One lc and the context's parameters serve every problem.  Problem p's out, pairs and status are bit-identical to what
+ * plf_loop_closure_pose returns for it on a context created with its camera.
+ * Capacity: a problem whose surviving pairs exceed its capacity gets status PLF_ERR_CAPACITY and what the single call
+ * writes then (the first cap_* pairs, n_pt / n_ls, accepted = 0, no pose_inc); every other problem is solved and written.
+ * The call then returns PLF_ERR_CAPACITY, and plf_last_error names the first such problem.
+ * Refusals before any work, naming the problem and the rule, with nothing written (no out, pairs or status):
+ * PLF_ERR_INVALID when n_problems < 0, lc or problems is NULL, a seq entry is out of range, a keyframe is NULL or has a
+ * negative count, a matched kind's arrays are NULL (the single call's "arrays missing" rules) or it has more than 65535
+ * features in a keyframe; PLF_ERR_CAPACITY when n_problems > 65535 (the matcher's grid.y; no chunking).  n_problems = 0
+ * returns PLF_OK and launches nothing.  The context stays usable after any error.
+ * Launches: per kind that some problem matches (enabled, features of it in both keyframes), the forward 2-NN, the reverse
+ * one (best_lr_matches) and the ratio / mutual check over all its problems: 3 (2 without best_lr_matches); then 3 more:
+ * the inlier-ratio pre-condition with the compaction of the matches into solver rows, the pose solver and the acceptance
+ * tests.  9 at the defaults; they do not depend on n_problems.  Work is enqueued on plf_stream; device scratch (its own slot, kept until plf_destroy): about
+ * 125 bytes per kf0 point, 181 per kf0 line, 56 per kf1 point, 64 per kf1 line and 1.3 KB per problem, each part rounded
+ * up to 256 bytes; the context's pinned staging buffer holds the inputs and outputs. */
+typedef struct plf_lc_problem {
+  const plf_lc_keyframe* kf0;    /* the candidate, map_keyframes[lc_kf_idx] (read as plf_loop_closure_pose reads it) */
+  const plf_lc_keyframe* kf1;    /* the new keyframe */
+  int32_t* pt_pairs; int cap_pt; /* out, may be NULL: as plf_loop_closure_pose */
+  int32_t* ls_pairs; int cap_ls;
+  plf_lc_result out;             /* out */
+  int status;                    /* out: PLF_OK, or PLF_ERR_CAPACITY when this problem's pairs exceed its capacity */
+} plf_lc_problem;
+plf_status plf_loop_closure_pose_batch(plf_ctx* ctx, const plf_lc_params* lc, int n_problems, plf_lc_problem* problems,
+                                       const int32_t* seq);
 
 /* se(3) helpers of stvo-pl auxiliar.h used throughout src/mapHandler.cpp (e.g. :137-142,:3439,:3558):
  * op 0 = expmap_se3 (in: 6 = [t; w], out: 16 row-major), op 1 = logmap_se3 (in: 16, out: 6). */
@@ -601,9 +660,9 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
  *     it is a first frame (status 2), since its carried frame was triangulated with another camera.
  *   - plf_set_max_sequences drops every sequence's camera; plf_reset_sequence keeps them.
  *   - plf_batch_run and plf_process_batch run sequence 0, so they use sequence 0's camera.
- * The single keyframe and back-end operators (plf_match_kf2kf, plf_match_map2kf, plf_loop_closure_pose, plf_gn_pose,
- * plf_local_ba, plf_global_ba) keep using the context's camera; plf_match_kf2kf_batch, plf_match_map2kf_batch and
- * plf_local_ba_batch take a sequence's per problem. */
+ * Only plf_global_ba keeps the context's camera without a batch form.  The other keyframe and back-end operators use the
+ * context's camera in their single form and take a sequence's per problem in their batch form: plf_match_kf2kf_batch,
+ * plf_match_map2kf_batch, plf_local_ba_batch, plf_gn_pose_batch and plf_loop_closure_pose_batch. */
 plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam);
 /* The calibration the next batch will use for sequence s: its own, or the context's camera. */
 plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out);

@@ -5,7 +5,8 @@
 // rows :3331-3426, normalise :3432, stop :3434/:3441, solve :3437-3438, update :3439, gate :3451-3482).
 // se(3) helpers: stvo-pl auxiliar (SURVEY Appendix A.4), twist ordering [t; w] (src/mapHandler.cpp:3513-3514).
 //
-// One CTA (128 threads) per frame pair; many frame pairs per launch.  Each thread strides over the
+// One CTA (128 threads) per frame pair; many frame pairs per launch (the front-end's batch, plf_gn_pose_batch, the
+// loop-closure checks of plf_loop_closure_pose_batch; plf_gn_pose is a batch of one).  Each thread strides over the
 // feature rows, accumulates the 21 upper-triangular entries of J^T W J, the 6 of J^T W r, the error and the
 // row count in fp64 registers; a warp-shuffle butterfly + one shared-memory hop reduces them; thread 0
 // solves the 6x6 system with a column-pivoting Householder QR (same semantics as Eigen's
@@ -180,8 +181,11 @@ __device__ void d_inverse6(const double* Ain, double* I) {
 }
 
 // cams: optional per-problem cameras (a batch of several calibrations); null = launch_cam for every problem.
+// active: optional per-problem flags; a problem whose flag is 0 is skipped (nothing read or written); null = all run.
 __global__ void __launch_bounds__(GN_THREADS) k_gn_pose(const GnProblem* __restrict__ probs, GnCam launch_cam,
-                                                         const PlfPairCam* __restrict__ cams, plf_gn_opts o) {
+                                                         const PlfPairCam* __restrict__ cams,
+                                                         const int* __restrict__ active, plf_gn_opts o) {
+  if (active && !active[blockIdx.x]) return;
   const GnProblem P = probs[blockIdx.x];
   GnCam cam = launch_cam;
   if (cams) {
@@ -348,55 +352,108 @@ plf_gn_opts plf_gn_opts_from_params(const plf_params& p) {
 }
 
 plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs, int nprob, const plf_gn_opts& o,
-                         const PlfPairCam* d_cams) {
+                         const PlfPairCam* d_cams, const int* d_active) {
   if (nprob <= 0) return PLF_OK;
   GnCam c = {ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy};
-  k_gn_pose<<<nprob, GN_THREADS, 0, cs>>>(d_probs, c, d_cams, o);
+  k_gn_pose<<<nprob, GN_THREADS, 0, cs>>>(d_probs, c, d_cams, d_active, o);
   PLF_LAUNCH_CHECK(ctx);
   return PLF_OK;
 }
+
+namespace {
+
+// plf_gn_pose's host-side rules for one problem.
+bool gn_args_ok(const plf_gn_problem& q) {
+  return q.np >= 0 && q.nl >= 0 && !(q.np > 0 && (!q.P || !q.pl_obs || !q.inlier_pt)) &&
+         !(q.nl > 0 && (!q.sP || !q.eP || !q.le_obs || !q.inlier_ls));
+}
+
+// The whole call over problems whose host-side rules hold: every problem's rows staged in flat arrays behind a table of
+// GnProblem (offsets, counts, T_init) and a table of cameras, one upload, one k_gn_pose launch, one download.  The inlier
+// flags are inputs and outputs: they are staged in the output part and uploaded with the inputs.
+plf_status gn_run(plf_ctx* ctx, const plf_gn_opts& o, int n, plf_gn_problem* pr, const std::vector<const plf_camera*>& cams) {
+  if (n == 0) return PLF_OK;
+  std::vector<size_t> po(n), lo(n);
+  size_t NP = 0, NL = 0;
+  for (int p = 0; p < n; ++p) {
+    po[p] = NP; lo[p] = NL;
+    NP += (size_t)pr[p].np; NL += (size_t)pr[p].nl;
+  }
+  StagedLayout L;
+  const size_t oprob = L.take_in(n * sizeof(GnProblem)), ocam = L.take_in(n * sizeof(PlfPairCam)), oT = L.take_in(n * 128);
+  const size_t oP = L.take_in(NP * 24), oO = L.take_in(NP * 16);
+  const size_t osP = L.take_in(NL * 24), oeP = L.take_in(NL * 24), ole = L.take_in(NL * 24);
+  const size_t ores = L.take_out(n * sizeof(plf_pose_result)), oip = L.take_out(NP), oil = L.take_out(NL);
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  uint8_t *pin, *dev;
+  if (plf_status st = L.acquire(ctx, PLF_SCR_GN, &pin, &dev)) return st;
+  uint8_t *pout = pin + L.in, *dout = dev + L.in;
+  GnProblem* tab = (GnProblem*)(pin + oprob);
+  PlfPairCam* cam = (PlfPairCam*)(pin + ocam);
+  for (int p = 0; p < n; ++p) {
+    const plf_gn_problem& q = pr[p];
+    const size_t a = po[p], b = lo[p];
+    if (q.np) {
+      memcpy(pin + oP + 24 * a, q.P, (size_t)q.np * 24);
+      memcpy(pin + oO + 16 * a, q.pl_obs, (size_t)q.np * 16);
+      memcpy(pout + oip + a, q.inlier_pt, (size_t)q.np);
+    }
+    if (q.nl) {
+      memcpy(pin + osP + 24 * b, q.sP, (size_t)q.nl * 24);
+      memcpy(pin + oeP + 24 * b, q.eP, (size_t)q.nl * 24);
+      memcpy(pin + ole + 24 * b, q.le_obs, (size_t)q.nl * 24);
+      memcpy(pout + oil + b, q.inlier_ls, (size_t)q.nl);
+    }
+    if (q.T_init) memcpy(pin + oT + 128 * (size_t)p, q.T_init, 128);
+    tab[p] = {(const double*)(dev + oP) + 3 * a, (const double*)(dev + oO) + 2 * a, dout + oip + a, nullptr, q.np,
+              (const double*)(dev + osP) + 3 * b, (const double*)(dev + oeP) + 3 * b, (const double*)(dev + ole) + 3 * b,
+              dout + oil + b, nullptr, q.nl, q.T_init ? (const double*)(dev + oT) + 16 * p : nullptr,
+              (plf_pose_result*)(dout + ores) + p};
+    const plf_camera& c = *cams[p];
+    cam[p] = {c.fx, c.fy, c.cx, c.cy, c.b};
+  }
+  cudaStream_t s = ctx->stream;
+  PLF_CUDA(ctx, cudaMemcpyAsync(dev, pin, L.in + L.out, cudaMemcpyHostToDevice, s));
+  if (plf_status st = plf_launch_gn(ctx, s, (const GnProblem*)(dev + oprob), n, o, (const PlfPairCam*)(dev + ocam))) return st;
+  PLF_CUDA(ctx, cudaMemcpyAsync(pout, dout, L.out, cudaMemcpyDeviceToHost, s));
+  PLF_CUDA(ctx, cudaStreamSynchronize(s));
+  for (int p = 0; p < n; ++p) {
+    plf_gn_problem& q = pr[p];
+    memcpy(&q.out, pout + ores + p * sizeof(plf_pose_result), sizeof(plf_pose_result));
+    if (q.np) memcpy(q.inlier_pt, pout + oip + po[p], (size_t)q.np);
+    if (q.nl) memcpy(q.inlier_ls, pout + oil + lo[p], (size_t)q.nl);
+  }
+  return PLF_OK;
+}
+
+}  // namespace
 
 extern "C" plf_status plf_gn_pose(plf_ctx* ctx, const plf_gn_opts* opts, const double* P, const double* pl_obs,
                                   uint8_t* inlier_pt, int np, const double* sP, const double* eP,
                                   const double* le_obs, uint8_t* inlier_ls, int nl, const double* T_init,
                                   plf_pose_result* out) {
-  if (!ctx || !out || np < 0 || nl < 0 || (np > 0 && (!P || !pl_obs || !inlier_pt)) ||
-      (nl > 0 && (!sP || !eP || !le_obs || !inlier_ls)))
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_gn_pose: bad arguments");
-  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  const plf_gn_opts o = opts ? *opts : plf_gn_opts_from_params(ctx->params);
-  double *dP, *dO, *dsP, *deP, *dle, *dT;
-  uint8_t *dIp, *dIl;
-  plf_pose_result* dout;
-  GnProblem* dprob;
-  DevBufList scr;
-  scr.add(dP, (size_t)np * 3); scr.add(dO, (size_t)np * 2); scr.add(dIp, np);
-  scr.add(dsP, (size_t)nl * 3); scr.add(deP, (size_t)nl * 3); scr.add(dle, (size_t)nl * 3); scr.add(dIl, nl);
-  scr.add(dT, 16); scr.add(dout, 1); scr.add(dprob, 1);
-  if (plf_status st = scr.carve(ctx, PLF_SCR_GN)) return st;
-  cudaStream_t s = ctx->stream;
-  if (np) {
-    PLF_CUDA(ctx, cudaMemcpyAsync(dP, P, (size_t)np * 24, cudaMemcpyHostToDevice, s));
-    PLF_CUDA(ctx, cudaMemcpyAsync(dO, pl_obs, (size_t)np * 16, cudaMemcpyHostToDevice, s));
-    PLF_CUDA(ctx, cudaMemcpyAsync(dIp, inlier_pt, (size_t)np, cudaMemcpyHostToDevice, s));
+  plf_gn_problem q = {P, pl_obs, inlier_pt, np, sP, eP, le_obs, inlier_ls, nl, T_init, {}};
+  if (!ctx || !out || !gn_args_ok(q)) return plf_fail(ctx, PLF_ERR_INVALID, "plf_gn_pose: bad arguments");
+  const plf_status st = gn_run(ctx, opts ? *opts : plf_gn_opts_from_params(ctx->params), 1, &q, {&ctx->cam});
+  if (st == PLF_OK) *out = q.out;
+  return st;
+}
+
+extern "C" plf_status plf_gn_pose_batch(plf_ctx* ctx, const plf_gn_opts* opts, int n_problems, plf_gn_problem* problems,
+                                        const int32_t* seq) {
+  if (!ctx) return PLF_ERR_INVALID;
+  const char* fn = "plf_gn_pose_batch";
+  if (n_problems < 0 || (n_problems && !problems))
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments (n_problems = %d, problems)", fn, n_problems);
+  std::vector<const plf_camera*> cams;
+  if (plf_status st = plf_problem_cameras(ctx, fn, n_problems, seq, cams)) return st;
+  for (int p = 0; p < n_problems; ++p) {
+    const plf_gn_problem& q = problems[p];
+    if (!gn_args_ok(q))
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: np = %d, nl = %d: a count is negative or an array is NULL while "
+                      "its count is > 0", fn, p, q.np, q.nl);
   }
-  if (nl) {
-    PLF_CUDA(ctx, cudaMemcpyAsync(dsP, sP, (size_t)nl * 24, cudaMemcpyHostToDevice, s));
-    PLF_CUDA(ctx, cudaMemcpyAsync(deP, eP, (size_t)nl * 24, cudaMemcpyHostToDevice, s));
-    PLF_CUDA(ctx, cudaMemcpyAsync(dle, le_obs, (size_t)nl * 24, cudaMemcpyHostToDevice, s));
-    PLF_CUDA(ctx, cudaMemcpyAsync(dIl, inlier_ls, (size_t)nl, cudaMemcpyHostToDevice, s));
-  }
-  double Tid[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-  PLF_CUDA(ctx, cudaMemcpyAsync(dT, T_init ? T_init : Tid, sizeof Tid, cudaMemcpyHostToDevice, s));
-  GnProblem hp = {dP, dO, dIp, nullptr, np, dsP, deP, dle, dIl, nullptr, nl, dT, dout};
-  PLF_CUDA(ctx, cudaMemcpyAsync(dprob, &hp, sizeof hp, cudaMemcpyHostToDevice, s));
-  plf_status st = plf_launch_gn(ctx, s, dprob, 1, o);
-  if (st) return st;
-  PLF_CUDA(ctx, cudaMemcpyAsync(out, dout, sizeof *out, cudaMemcpyDeviceToHost, s));
-  if (np) PLF_CUDA(ctx, cudaMemcpyAsync(inlier_pt, dIp, (size_t)np, cudaMemcpyDeviceToHost, s));
-  if (nl) PLF_CUDA(ctx, cudaMemcpyAsync(inlier_ls, dIl, (size_t)nl, cudaMemcpyDeviceToHost, s));
-  PLF_CUDA(ctx, cudaStreamSynchronize(s));
-  return PLF_OK;
+  return gn_run(ctx, opts ? *opts : plf_gn_opts_from_params(ctx->params), n_problems, problems, cams);
 }
 
 // se(3) helpers exposed for the C++ shim / parity tests (stvo-pl auxiliar expmap_se3 / logmap_se3 /

@@ -20,6 +20,17 @@ plf_status plf_fail(plf_ctx* ctx, plf_status code, const char* fmt, ...) {
   return code;
 }
 
+plf_status plf_problem_cameras(plf_ctx* ctx, const char* fn, int n, const int32_t* seq, std::vector<const plf_camera*>& cams) {
+  cams.resize(n);
+  for (int p = 0; p < n; ++p) {
+    const int s = seq ? seq[p] : -1;
+    if (s < -1 || s >= ctx->max_sequences)
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: seq[%d] = %d outside [-1, %d)", fn, p, p, s, ctx->max_sequences);
+    cams[p] = s >= 0 && !ctx->seq_cam_own.empty() && ctx->seq_cam_own[s] ? &ctx->seq_cam[s] : &ctx->cam;
+  }
+  return PLF_OK;
+}
+
 size_t DevBufList::bytes() const {
   size_t n = 0;
   for (const Entry& e : entries) n += e.bytes;

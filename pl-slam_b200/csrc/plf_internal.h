@@ -25,7 +25,7 @@ inline size_t plf_align256(size_t x) { return (x + 255) & ~size_t(255); }
 enum plf_scratch_slot {
   PLF_SCR_MATCH,       // plf_hamming_knn2, plf_match, plf_median_descriptors, plf_match_grid_points / _lines
   PLF_SCR_LBD,         // plf_lbd_gradients, plf_lbd
-  PLF_SCR_GN,          // plf_gn_pose, plf_se3 (plf_loop_closure_pose calls them one after the other)
+  PLF_SCR_GN,          // plf_gn_pose, plf_gn_pose_batch, plf_se3
   PLF_SCR_ORB,         // plf_orb
   PLF_SCR_LSD,         // plf_lsd, plf_detect_lines, plf_debug_sincosf
   PLF_SCR_MGB_PIPE,    // the windowed matcher of plf_batch_run (matching_strategy != 0)
@@ -35,6 +35,7 @@ enum plf_scratch_slot {
   PLF_SCR_KF_MGB_LS,   //   ... and of lines
   PLF_SCR_BOW,         // plf_bow_insert
   PLF_SCR_BA_BATCH,    // plf_local_ba_batch: its staged layout
+  PLF_SCR_LC,          // plf_loop_closure_pose and plf_loop_closure_pose_batch: their staged layout
   PLF_SCR_COUNT
 };
 
@@ -109,6 +110,9 @@ struct plf_ctx {
 void plf_mark(plf_ctx* ctx, cudaStream_t cs, const char* name);
 
 plf_status plf_fail(plf_ctx* ctx, plf_status code, const char* fmt, ...);
+// The camera of each problem of a batch call: seq NULL or seq[p] = -1 the context's, 0 <= seq[p] < max_sequences what
+// plf_get_sequence_camera returns now.  Any other entry returns PLF_ERR_INVALID naming fn, the problem and the entry.
+plf_status plf_problem_cameras(plf_ctx* ctx, const char* fn, int n, const int32_t* seq, std::vector<const plf_camera*>& cams);
 // Ensures scratch slot `slot` holds at least `bytes`; returns device pointer or nullptr (error set).
 void* plf_scratch(plf_ctx* ctx, plf_scratch_slot slot, size_t bytes);
 void* plf_pinned(plf_ctx* ctx, size_t bytes);
@@ -222,8 +226,9 @@ struct GnProblem {
 struct PlfPairCam { double fx, fy, cx, cy, b; };
 plf_gn_opts plf_gn_opts_from_params(const plf_params& p);
 // d_cams: optional [nprob] device array, the camera of each problem (b unused); null = the context's camera.
+// d_active: optional [nprob] device flags; a problem whose flag is 0 is not solved (its out and flags are not written).
 plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs, int nprob, const plf_gn_opts& o,
-                         const PlfPairCam* d_cams = nullptr);
+                         const PlfPairCam* d_cams = nullptr, const int* d_active = nullptr);
 
 // ---- tiled LDL^T (lba.cu) ------------------------------------------------------------------------
 // Factors the symmetric n x n matrix S (n = 6 n6; row-major, leading dimension n; only its lower triangle is read) in

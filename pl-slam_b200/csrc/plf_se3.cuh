@@ -1,5 +1,5 @@
 // se(3) helpers shared by the pose solver (gn.cu), the bundle adjustments (lba.cu), the keyframe matching (kfmatch.cu),
-// the batched front-end's epilogue (pipeline.cu) and the loop-closure decision (loopclosure.cu, on the host).
+// the batched front-end's epilogue (pipeline.cu) and the loop-closure decision (loopclosure.cu).
 // Conventions of stvo-pl's auxiliar.h as used by pl-slam (SURVEY Appendix A.4; ordering x = [t; w] confirmed at
 // src/mapHandler.cpp:3513-3514); same operation order as oracle/gn.c.
 #pragma once
@@ -94,6 +94,42 @@ __host__ __device__ inline void d_inverse_se3(const double* T, double* Ti) {
   out[12] = out[13] = out[14] = 0;
   out[15] = 1;
   for (int i = 0; i < 16; ++i) Ti[i] = out[i];
+}
+
+// Largest eigenvalue of a symmetric 6x6 matrix (cyclic Jacobi; Eigen's SelfAdjointEigenSolver sorts ascending and
+// MapHandler::isLoopClosure reads element 5, src/mapHandler.cpp:3883-3885).  Host and device give the same bits: the
+// device is built --fmad=false, the host has no FMA contraction, and sqrt and the division are correctly rounded on both.
+__host__ __device__ inline double plf_sym6_max_eig(const double* A_in) {
+  double A[36];
+  for (int i = 0; i < 6; ++i)
+    for (int j = 0; j < 6; ++j) A[6 * i + j] = 0.5 * (A_in[6 * i + j] + A_in[6 * j + i]);
+  for (int sweep = 0; sweep < 64; ++sweep) {
+    double off = 0;
+    for (int i = 0; i < 6; ++i)
+      for (int j = i + 1; j < 6; ++j) off += A[6 * i + j] * A[6 * i + j];
+    if (off < 1e-300) break;
+    for (int p = 0; p < 6; ++p)
+      for (int q = p + 1; q < 6; ++q) {
+        const double apq = A[6 * p + q];
+        if (apq == 0.0) continue;
+        const double theta = (A[6 * q + q] - A[6 * p + p]) / (2.0 * apq);
+        const double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+        for (int k = 0; k < 6; ++k) {  // A <- J^T A J
+          const double akp = A[6 * k + p], akq = A[6 * k + q];
+          A[6 * k + p] = c * akp - s * akq;
+          A[6 * k + q] = s * akp + c * akq;
+        }
+        for (int k = 0; k < 6; ++k) {
+          const double apk = A[6 * p + k], aqk = A[6 * q + k];
+          A[6 * p + k] = c * apk - s * aqk;
+          A[6 * q + k] = s * apk + c * aqk;
+        }
+      }
+  }
+  double m = A[0];
+  for (int i = 1; i < 6; ++i) m = A[7 * i] > m ? A[7 * i] : m;
+  return m;
 }
 
 // T <- T * inverse_se3(expmap_se3(x)),  x = [t; w]

@@ -17,6 +17,7 @@ REPO_ROOT = _PKG_DIR.parent
 LIB_PATH = _PKG_DIR / "lib" / "libplslam_b200.so"
 
 DESC_BYTES = 32
+PLF_ERR_CAPACITY = -4   # plf_status of a call or batch problem that exceeded a capacity
 
 
 class PlfError(RuntimeError):
@@ -150,6 +151,18 @@ class plf_lc_result(C.Structure):
                 ("n_pt", C.c_int), ("n_ls", C.c_int), ("inl_ratio_pt", C.c_double), ("inl_ratio_ls", C.c_double),
                 ("err", C.c_double), ("max_cov_eig", C.c_double), ("ratio_inliers", C.c_double), ("t", C.c_double),
                 ("r", C.c_double), ("x_inc", C.c_double * 6), ("pose_inc", C.c_double * 6)]
+
+
+class plf_gn_problem(C.Structure):
+    _fields_ = [("P", C.c_void_p), ("pl_obs", C.c_void_p), ("inlier_pt", C.c_void_p), ("np", C.c_int),
+                ("sP", C.c_void_p), ("eP", C.c_void_p), ("le_obs", C.c_void_p), ("inlier_ls", C.c_void_p), ("nl", C.c_int),
+                ("T_init", C.c_void_p), ("out", plf_pose_result)]
+
+
+class plf_lc_problem(C.Structure):
+    _fields_ = [("kf0", C.POINTER(plf_lc_keyframe)), ("kf1", C.POINTER(plf_lc_keyframe)), ("pt_pairs", C.c_void_p),
+                ("cap_pt", C.c_int), ("ls_pairs", C.c_void_p), ("cap_ls", C.c_int), ("out", plf_lc_result),
+                ("status", C.c_int)]
 
 
 class plf_kf_match_opts(C.Structure):
@@ -519,6 +532,38 @@ class Frontend:
                     err=out.err, iters=(out.iters1, out.iters2), inlier_pt=ip, inlier_ls=il,
                     n_inliers=(out.n_inliers_pt, out.n_inliers_ls))
 
+    @staticmethod
+    def _gn_result(out, ip, il):
+        return dict(T=np.array(out.T).reshape(4, 4), cov=np.array(out.cov).reshape(6, 6), x=np.array(out.x),
+                    err=out.err, iters=(out.iters1, out.iters2), inlier_pt=ip, inlier_ls=il,
+                    n_inliers=(out.n_inliers_pt, out.n_inliers_ls))
+
+    def gn_pose_batch(self, problems, seq=None, opts=None):
+        """Many gn_pose in one device call (plf_gn_pose_batch), with one opts.  problems: dicts P, pl_obs, sP, eP, le_obs and
+        optionally inlier_pt, inlier_ls, T_init, as gn_pose takes them; seq: per problem, -1 for the context's camera or a
+        sequence whose camera (sequence_camera) to project with (None = all -1).  Returns one gn_pose dict per problem plus
+        `status` (0)."""
+        problems = list(problems)
+        P = len(problems)
+        seq_a = self._problem_sequences(P, seq)
+        f64 = lambda a, k: np.ascontiguousarray(a, np.float64).reshape(-1, k)
+        ad = lambda a: a.ctypes.data if a is not None and a.size else None
+        keep, flags = [], []
+        arr = (plf_gn_problem * max(P, 1))()
+        for k, pr in enumerate(problems):
+            Pp, O, sP, eP, le = f64(pr["P"], 3), f64(pr["pl_obs"], 2), f64(pr["sP"], 3), f64(pr["eP"], 3), f64(pr["le_obs"], 3)
+            ip = pr.get("inlier_pt"); il = pr.get("inlier_ls")
+            ip = np.ones(len(Pp), np.uint8) if ip is None else np.ascontiguousarray(ip, np.uint8).copy()
+            il = np.ones(len(sP), np.uint8) if il is None else np.ascontiguousarray(il, np.uint8).copy()
+            T0 = pr.get("T_init")
+            T0 = None if T0 is None else np.ascontiguousarray(T0, np.float64).reshape(16)
+            keep += [Pp, O, sP, eP, le, T0]
+            flags.append((ip, il))
+            arr[k] = plf_gn_problem(ad(Pp), ad(O), ad(ip), len(Pp), ad(sP), ad(eP), ad(le), ad(il), len(sP), ad(T0))
+        self._check(self.lib.plf_gn_pose_batch(self._ctx, C.byref(opts) if opts is not None else None, P, arr,
+                                               None if seq_a is None else _ptr(seq_a, C.c_int32)), "plf_gn_pose_batch")
+        return [dict(self._gn_result(arr[k].out, ip, il), status=0) for k, (ip, il) in enumerate(flags)]
+
     def loop_closure_pose(self, kf0, kf1, lc=None):
         """MapHandler::isLoopClosure + computeRelativePoseRobustGN (src/mapHandler.cpp:3192-3300, :3566-3957).
         kf0 / kf1: dicts with pdesc, P, pl, ldesc, sP, eP, le (numpy); lc: dict of the lc_* thresholds."""
@@ -550,6 +595,60 @@ class Frontend:
         r["x_inc"] = np.array(out.x_inc); r["pose_inc"] = np.array(out.pose_inc)
         r["pt_pairs"] = pp[:out.n_pt].copy(); r["ls_pairs"] = lp[:out.n_ls].copy()
         return r
+
+    @staticmethod
+    def _lc_keyframe(k, keep):
+        """plf_lc_keyframe over copies of a keyframe dict's arrays (kept alive in keep)."""
+        f = plf_lc_keyframe()
+        pd = _u8(k["pdesc"]).reshape(-1, 32); ld = _u8(k["ldesc"]).reshape(-1, 32)
+        arrs = dict(pdesc=pd, ldesc=ld)
+        for name, cols in (("P", 3), ("pl", 2), ("sP", 3), ("eP", 3), ("le", 3)):
+            arrs[name] = np.ascontiguousarray(k[name], np.float64).reshape(-1, cols)
+        f.n_pt, f.n_ls = len(pd), len(ld)
+        for name, a in arrs.items():
+            keep.append(a)
+            setattr(f, name, a.ctypes.data if a.size else None)
+        keep.append(f)
+        return f
+
+    def loop_closure_pose_batch(self, pairs, seq=None, lc=None):
+        """Many loop_closure_pose in one device call (plf_loop_closure_pose_batch), with one set of lc thresholds.  pairs:
+        (kf0, kf1) tuples of loop_closure_pose's keyframe dicts, or dicts kf0, kf1 and optionally cap_pt / cap_ls (pair
+        capacities; default: kf0's feature counts, which always suffice); seq: as gn_pose_batch.  Returns one
+        loop_closure_pose dict per pair plus `status` (0, or PLF_ERR_CAPACITY = -4 when that pair's correspondences
+        exceed its capacity: its dict then holds what the single call leaves, pairs cut at the capacity).  Raises
+        PlfError for the refusals before any work."""
+        pairs = list(pairs)
+        P = len(pairs)
+        seq_a = self._problem_sequences(P, seq)
+        d = dict(lc_res=1.0, lc_unc=0.01, lc_inl=0.3, lc_trs=1.5, lc_rot=35.0, lc_inlier_ratio=30.0)
+        d.update(lc or {})
+        lcp = plf_lc_params(**d)
+        keep, outs = [], []
+        arr = (plf_lc_problem * max(P, 1))()
+        for k, pr in enumerate(pairs):
+            if not isinstance(pr, dict):
+                pr = dict(kf0=pr[0], kf1=pr[1])
+            k0, k1 = self._lc_keyframe(pr["kf0"], keep), self._lc_keyframe(pr["kf1"], keep)
+            cap_p, cap_l = int(pr.get("cap_pt", k0.n_pt)), int(pr.get("cap_ls", k0.n_ls))
+            pp = np.full((max(cap_p, 1), 2), -1, np.int32); lp = np.full((max(cap_l, 1), 2), -1, np.int32)
+            outs.append((pp, lp))
+            arr[k] = plf_lc_problem(C.pointer(k0), C.pointer(k1), pp.ctypes.data, cap_p, lp.ctypes.data, cap_l,
+                                    plf_lc_result(), 1)   # 1 is no plf_status: marks entries the call did not write
+        rc = self.lib.plf_loop_closure_pose_batch(self._ctx, C.byref(lcp), P, arr,
+                                                  None if seq_a is None else _ptr(seq_a, C.c_int32))
+        if rc != 0 and (rc != PLF_ERR_CAPACITY or P == 0 or any(arr[k].status == 1 for k in range(P))):
+            self._check(rc, "plf_loop_closure_pose_batch")
+        res = []
+        for k, (pp, lp) in enumerate(outs):
+            out = arr[k].out
+            r = {f: getattr(out, f) for f, _ in plf_lc_result._fields_ if f not in ("x_inc", "pose_inc")}
+            r["accepted"] = bool(out.accepted); r["estimated"] = bool(out.estimated)
+            r["x_inc"] = np.array(out.x_inc); r["pose_inc"] = np.array(out.pose_inc)
+            r["pt_pairs"] = pp[:min(out.n_pt, arr[k].cap_pt)].copy(); r["ls_pairs"] = lp[:min(out.n_ls, arr[k].cap_ls)].copy()
+            r["status"] = int(arr[k].status)
+            res.append(r)
+        return res
 
     def local_ba(self, prob, lambda_=1e-5, lambda_k=10.0, max_iters=15, homog_th=1e-7, min_error=1e-7,
                  min_error_change=1e-7, ref_quirks=1):

@@ -121,6 +121,33 @@ class World:
         self.cells = cells
 
 
+def loop_closure_keyframes(cam, seed=0, x_true=None, n_pts=300, n_lines=80, flip_bits=6, shuffle=True, outlier_frac=0.1):
+    """A loop-closure candidate pair rendered with `cam` (the layout plf_loop_closure_pose reads): kf0 holds gn_problem's
+    3-D features with random 256-bit descriptors; kf1 observes them under the planted increment with noisy copies of the
+    descriptors (flip_bits random bit flips), in a shuffled order, plus n_pts / 5 and n_lines / 5 unrelated distractors.
+    Returns kf0, kf1, the gn_problem dict and kf1's position of every kf0 point / line."""
+    g = gn_problem(cam, n_pts=n_pts, n_lines=n_lines, seed=seed, x_true=x_true, outlier_frac=outlier_frac)
+    rng = np.random.default_rng(seed + 100)
+
+    def noisy(d):
+        out = d.copy()
+        for row in out:
+            for b in rng.integers(0, 256, flip_bits):
+                row[b >> 3] ^= np.uint8(1 << (b & 7))
+        return out
+    pd0 = rng.integers(0, 256, (n_pts, 32), dtype=np.uint8); ld0 = rng.integers(0, 256, (n_lines, 32), dtype=np.uint8)
+    n_dp, n_dl = n_pts // 5, n_lines // 5
+    pd1 = np.concatenate([noisy(pd0), rng.integers(0, 256, (n_dp, 32), dtype=np.uint8)])
+    ld1 = np.concatenate([noisy(ld0), rng.integers(0, 256, (n_dl, 32), dtype=np.uint8)])
+    pl1 = np.concatenate([g["obs"], rng.uniform(0, 400, (n_dp, 2))]); le1 = np.concatenate([g["le"], rng.normal(0, 1, (n_dl, 3))])
+    pp = rng.permutation(len(pd1)) if shuffle else np.arange(len(pd1))
+    lp = rng.permutation(len(ld1)) if shuffle else np.arange(len(ld1))
+    kf0 = dict(pdesc=pd0, P=g["P"], pl=np.zeros((n_pts, 2)), ldesc=ld0, sP=g["sP"], eP=g["eP"], le=np.zeros((n_lines, 3)))
+    kf1 = dict(pdesc=pd1[pp], P=np.zeros((len(pp), 3)), pl=pl1[pp], ldesc=ld1[lp], sP=np.zeros((len(lp), 3)),
+               eP=np.zeros((len(lp), 3)), le=le1[lp])
+    return kf0, kf1, g, np.argsort(pp), np.argsort(lp)
+
+
 def corridor_world(n_segs=450, seed=3):
     """Lines-dominant scene (BASELINE configs[4]): long low-contrast 3-D segments running along the corridor (few
     crossings, ends mostly outside the view), no textured quads."""
