@@ -264,6 +264,14 @@ plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, int h, int 
 /* Test hook: evaluates the device port of glibc sinf/cosf used by the LSD region-angle update. */
 plf_status plf_debug_sincosf(plf_ctx* ctx, const float* in, float* s, float* c, int n);
 
+/* Test hook: factors the symmetric n x n matrix S (n = 6 n6, row-major, only its lower triangle is read) as L D L^T
+ * without pivoting and solves S x = g, with the factorisation of plf_global_ba / plf_pose_graph (path 0: the tiled one,
+ * 1 <= n6 <= 4096) or that of plf_local_ba (path 1: one CTA, 1 <= n6 <= 64).  On return the lower triangle of S holds
+ * L strictly below the diagonal and D on it (entries above the diagonal are unspecified), x the solution, and nz
+ * (path 0 only, may be NULL; n_t x n_t bytes, n_t = ceil(n / 64)) the zero flag of each L tile (i > k) as the panel
+ * kernel set it, 0 elsewhere.  A bad path, an n6 out of range or a NULL S, g or x returns PLF_ERR_INVALID. */
+plf_status plf_debug_ldlt(plf_ctx* ctx, int path, int n6, double* S, const double* g, double* x, uint8_t* nz);
+
 /* LBD prelude: GaussianBlur 5x5 sigma 1 then Sobel k=3 to CV_16S.  Replaces
  * BinaryDescriptor::computeSobel (binary_descriptor_custom.cpp:373-398 -> :350-370).
  * img: h rows of `stride` bytes (host). dxdy: h*w interleaved int16 pairs (dx,dy) (host). */

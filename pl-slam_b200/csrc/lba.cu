@@ -651,6 +651,45 @@ plf_status plf_ldlt_tiled(plf_ctx* ctx, cudaStream_t cs, int n6, double* S, doub
   return PLF_OK;
 }
 
+// Test hook (plslam_b200.h): one of the two factorisations on a caller's matrix.  Path 0 is plf_ldlt_tiled as
+// plf_global_ba / plf_pose_graph call it; path 1 is k_lba_solve with zero keyframe blocks and gradient and lambda = 0, so
+// its prologue adds +0.0 to the diagonal 6 x 6 blocks and to g.  The zero flags are cleared first, so the ones the panel kernel never sets (i <= k) read 0.
+extern "C" plf_status plf_debug_ldlt(plf_ctx* ctx, int path, int n6, double* S, const double* g, double* x, uint8_t* nz) {
+  const char* fn = "plf_debug_ldlt";
+  if (!ctx || !S || !g || !x) return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", fn);
+  if (path != 0 && path != 1) return plf_fail(ctx, PLF_ERR_INVALID, "%s: path %d (0: tiled, 1: one CTA)", fn, path);
+  const int cap = path == 0 ? 4096 : 64;
+  if (n6 < 1 || n6 > cap) return plf_fail(ctx, PLF_ERR_INVALID, "%s: n6 = %d outside [1, %d] for path %d", fn, n6, cap, path);
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int n = 6 * n6, nt = (n + GBA_T - 1) / GBA_T;
+  LbaDev d{};
+  d.nkf = n6;
+  double* dWp = nullptr;
+  uint8_t* dNz = nullptr;
+  DevBufList scr;
+  scr.add(d.S, (size_t)n * n); scr.add(d.gred, n); scr.add(d.dxc, n); scr.add(d.DX, n);
+  if (path == 0) { scr.add(dWp, (size_t)nt * GBA_T * GBA_T); scr.add(dNz, (size_t)nt * nt); }
+  else { scr.add(d.A, (size_t)36 * n6); scr.add(d.gc, n); }
+  if (plf_status st = scr.carve(ctx, PLF_SCR_BA)) return st;
+  cudaStream_t cs = ctx->stream;
+  PLF_CUDA(ctx, cudaMemcpyAsync(d.S, S, (size_t)n * n * 8, cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(d.gred, g, (size_t)n * 8, cudaMemcpyHostToDevice, cs));
+  if (path == 0) {
+    PLF_CUDA(ctx, cudaMemsetAsync(dNz, 0, (size_t)nt * nt, cs));
+    if (plf_status st = plf_ldlt_tiled(ctx, cs, n6, d.S, d.gred, d.dxc, d.DX, dWp, dNz)) return st;
+  } else {
+    PLF_CUDA(ctx, cudaMemsetAsync(d.A, 0, (size_t)36 * n6 * 8, cs));
+    PLF_CUDA(ctx, cudaMemsetAsync(d.gc, 0, (size_t)n * 8, cs));
+    k_lba_solve<<<1, 256, 0, cs>>>(d, 0.0);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  PLF_CUDA(ctx, cudaMemcpyAsync(S, d.S, (size_t)n * n * 8, cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(x, d.DX, (size_t)n * 8, cudaMemcpyDeviceToHost, cs));
+  if (path == 0 && nz) PLF_CUDA(ctx, cudaMemcpyAsync(nz, dNz, (size_t)nt * nt, cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaStreamSynchronize(cs));
+  return PLF_OK;
+}
+
 // The host loop of both routines: the reference's control flow, on the device kernels above.  `global` selects
 // levMarquardtOptimizationGBA (:2101-2699) over levMarquardtOptimizationLBA (:1332-1989): its quirk set, its error
 // normalisation in the LM iterations and up to 4096 keyframes (the blocked factorisation beyond n = 384).  Both refuse a

@@ -938,6 +938,30 @@ class Frontend:
         self._check(st, "plf_debug_sincosf")
         return s, c
 
+    def debug_ldlt(self, S, g, path=0, overwrite_s=False):
+        """LDL^T without pivoting of the symmetric S (6 n6 x 6 n6, lower triangle read) and the solution of S x = g, by
+        the tiled factorisation of global_ba / pose_graph (path 0) or the one-CTA one of local_ba (path 1).  Returns
+        (LD, x, nz): LD holds L strictly below its diagonal and D on it (upper triangle unspecified); nz (path 0, else
+        None) is the n_t x n_t zero flag of each L tile (i > k), n_t = ceil(n / 64).  overwrite_s: factor S's own buffer
+        (a C-contiguous float64 array) instead of a copy.  plf_debug_ldlt."""
+        n = S.shape[0]
+        if S.shape != (n, n) or n % 6 or len(g) != n:
+            raise PlfError(f"debug_ldlt: S {S.shape} and g {len(g)} must be 6 n6 square and 6 n6 long")
+        if overwrite_s:
+            if S.dtype != np.float64 or not S.flags.c_contiguous or not S.flags.writeable:
+                raise PlfError("debug_ldlt: overwrite_s needs a writeable C-contiguous float64 S")
+            LD = S
+        else:
+            LD = np.array(S, np.float64, order="C")
+        g = np.ascontiguousarray(g, np.float64)
+        x = np.empty(n, np.float64)
+        nt = (n + 63) // 64
+        nz = np.zeros((nt, nt), np.uint8) if path == 0 else None
+        st = self.lib.plf_debug_ldlt(self._ctx, int(path), n // 6, _ptr(LD, C.c_double), _ptr(g, C.c_double),
+                                     _ptr(x, C.c_double), None if nz is None else _ptr(nz, C.c_uint8))
+        self._check(st, "plf_debug_ldlt")
+        return LD, x, nz
+
     def debug_timeline(self):
         """Device-clock start/end (ms) of the E, G, M phases of the two most recent batches: array [2, 3, 2]."""
         out = np.zeros(12, np.float32)
