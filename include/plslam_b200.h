@@ -670,7 +670,9 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
  *   - plf_batch_run and plf_process_batch run sequence 0, so they use sequence 0's camera.
  * Only plf_global_ba keeps the context's camera without a batch form.  The other keyframe and back-end operators use the
  * context's camera in their single form and take a sequence's per problem in their batch form: plf_match_kf2kf_batch,
- * plf_match_map2kf_batch, plf_local_ba_batch, plf_gn_pose_batch and plf_loop_closure_pose_batch. */
+ * plf_match_map2kf_batch, plf_local_ba_batch, plf_gn_pose_batch and plf_loop_closure_pose_batch.  Place recognition's
+ * batch form, plf_bow_insert_batch, takes a sequence's bag-of-words database instead: its vectors do not depend on the
+ * camera, so plf_set_sequence_camera leaves that database as it is. */
 plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam);
 /* The calibration the next batch will use for sequence s: its own, or the context's camera. */
 plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out);
@@ -829,7 +831,7 @@ plf_status plf_vocab_read_yml(const char* path, plf_vocab* out);   /* numbers ar
 void plf_vocab_free(plf_vocab* v);
 
 /* Uploads the vocabulary of kind 0 (points, ORB) or 1 (lines, LBD), validated by the rules of plf_vocab_read_yml, and
- * empties that kind's database.  The tree is stored re-laid out by parent (each node's children contiguous, in file order):
+ * empties that kind's database: the context's and every sequence's (plf_bow_insert_batch).  The tree is stored re-laid out by parent (each node's children contiguous, in file order):
  * 48 bytes per node. */
 plf_status plf_bow_set_vocabulary(plf_ctx* ctx, int kind, const plf_vocab* voc);
 
@@ -855,6 +857,57 @@ plf_status plf_bow_erase(plf_ctx* ctx, int kf_idx);
  * entries.  words / values may be NULL to query *n; PLF_ERR_CAPACITY if *n > cap.  An absent keyframe or a kind never
  * inserted returns PLF_ERR_INVALID. */
 plf_status plf_bow_get(plf_ctx* ctx, int kf_idx, int kind, int cap, uint32_t* words, double* values, int* n);
+
+/* Many keyframe inserts in one call: the new keyframes of several sequences, each transformed, stored and scored in its
+ * sequence's own database (the reference scores a keyframe against its own map's keyframes only, src/mapHandler.cpp:
+ * 3019-3028), in one upload, three launches and one download with one host synchronisation.
+ *   problems [n_problems]  kf_idx, kf (read: n_pt, n_ls, pdesc, ldesc), score_p / score_l: as plf_bow_insert's arguments
+ *   seq      [n_problems]  or NULL: the DATABASE of problem p.  seq[p] = -1 (or seq NULL) is the context's database, the
+ *                          one plf_bow_insert / plf_bow_erase / plf_bow_get use; 0 <= seq[p] < n (plf_set_max_sequences)
+ *                          is sequence seq[p]'s.
+ * Every database holds, per kind, the stored vectors under their indices and its own `last` index; all of them share the
+ * context's two vocabularies.  Each database numbers its keyframes from 0 by itself.
+ *   - Equality: problem p's rows, its stored vector (plf_bow_get_seq) and every later row scored against it are
+ *     bit-identical to plf_bow_insert on a context whose only database is p's, with the same vocabularies, the same
+ *     earlier inserts and erasures of that database, and this batch's problems of that database made one by one in
+ *     problem order.
+ *   - Several problems may target one database: their kf_idx must rise in problem order, and a later one's row includes
+ *     the earlier ones.
+ *   - Isolation: a row covers its own database only; an index stored by another sequence is NaN there, as any absent one.
+ *   - Kinds: has_points / has_lines apply as in plf_bow_insert: a disabled kind's row is left as it is and needs no
+ *     vocabulary.
+ *   - Lifecycle: plf_bow_set_vocabulary(kind) empties that kind in every database; plf_bow_clear_sequence(s) empties both
+ *     kinds of s and frees their device memory; plf_set_max_sequences drops every sequence's databases;
+ *     plf_reset_sequence and plf_set_sequence_camera leave them as they are.
+ *   - A sequence never inserted into holds no device memory (one host pointer).  A sequence database's first allocation
+ *     is 1024 entries and 64 indices per kind (the context's: 65536 and 1024); each grows by doubling, as plf_bow_insert's.
+ * Refusals before any work, naming the problem and the rule, with nothing changed: PLF_ERR_INVALID when n_problems < 0,
+ * a seq entry is outside [-1, n), kf is NULL, kf_idx is outside [0, 2^24) or, for an enabled kind, does not exceed its
+ * database's last index or an earlier problem's kf_idx on the same database, a count is outside [0, 8192], or
+ * descriptors are NULL with a count > 0; PLF_ERR_STATE when an enabled kind has no vocabulary; PLF_ERR_CAPACITY when a
+ * database would pass 2^31 - 1 entries or n_problems > 65535 (the assembly's grid.y; no chunking).  n_problems = 0
+ * returns PLF_OK.  The context stays usable after any error.
+ * Launches: the transform (when any feature is enabled), the assembly and the scoring (when any row is requested); they
+ * do not depend on n_problems.  Each problem reserves as many entries as it has features in its database; when two
+ * problems share a database, the unused part of the earlier one's reservation stays a hole (not returned by
+ * plf_bow_get_seq).  Work is enqueued on plf_stream; device scratch (PLF_SCR_BOW) and the pinned staging buffer hold 32
+ * bytes per feature and 124 per problem in, the rows and 8 bytes per problem out, 12 bytes per feature of work. */
+typedef struct plf_bow_problem {
+  int kf_idx;                  /* index in its database, as plf_bow_insert's kf_idx */
+  const plf_frame_view* kf;    /* read: n_pt, n_ls, pdesc, ldesc (as plf_bow_insert reads it) */
+  double* score_p;             /* out [kf_idx + 1] or NULL, as plf_bow_insert */
+  double* score_l;
+} plf_bow_problem;
+plf_status plf_bow_insert_batch(plf_ctx* ctx, int n_problems, plf_bow_problem* problems, const int32_t* seq);
+/* plf_bow_erase on sequence s's database (s = -1: the context's; exactly plf_bow_erase).  s outside [-1, n) returns
+ * PLF_ERR_INVALID; erasing from a sequence never inserted into is a no-op. */
+plf_status plf_bow_erase_seq(plf_ctx* ctx, int s, int kf_idx);
+/* plf_bow_get on sequence s's database (s = -1: the context's; exactly plf_bow_get).  s outside [-1, n) returns
+ * PLF_ERR_INVALID. */
+plf_status plf_bow_get_seq(plf_ctx* ctx, int s, int kf_idx, int kind, int cap, uint32_t* words, double* values, int* n);
+/* Empties both kinds of sequence s's database and frees its device memory, for a new recording that takes over slot s
+ * (INTEGRATION.md section 4a).  0 <= s < n, else PLF_ERR_INVALID; the next insert into s may start again at kf_idx 0. */
+plf_status plf_bow_clear_sequence(plf_ctx* ctx, int s);
 
 /* Debug: device-clock timeline (ms) of the two most recent batches of the software pipeline: for each, the start/end of
  * the E (extract), G (region growing) and M (match/track/pose) phases relative to the older batch's E start.

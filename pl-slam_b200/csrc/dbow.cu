@@ -3,13 +3,17 @@
 //
 // Host: plf_vocab_read_yml (the YAML form TemplatedVocabulary::save writes, TemplatedVocabulary.h:1340-1432, read in load's
 // order :1437-1486), the vocabulary checks, the re-layout of the tree by parent, the database bookkeeping.
-// Kernels, all on plf_stream, one upload and one download per plf_bow_insert:
-//   k_bow_transform  one warp per feature, one lane per child: the descent of transform() (:1198-1239);
-//   k_bow_assemble   one block per kind: the (word, feature) pairs sorted by word (stable in feature order), addWeight in
-//                    feature order (BowVector.cpp:34-46), the sequential L1 norm in ascending word order (:62-84), the
-//                    division, the append to the kind's database;
-//   k_bow_score      one warp per earlier keyframe: L1Scoring::score (ScoringObject.cpp:23-68), the common words' terms
-//                    summed sequentially in ascending word order.
+// Databases: the context's and one per sequence (created on its first insert), each per kind; all share the context's
+// two vocabularies.  plf_bow_insert is plf_bow_insert_batch with one problem on the context's database.
+// Kernels, all on plf_stream, one upload and one download per call, whatever the number of problems:
+//   k_bow_transform  one warp per feature, one lane per child: the descent of transform() (:1198-1239), over every
+//                    problem's point features and then every problem's line features;
+//   k_bow_assemble   one block per (problem, kind): the (word, feature) pairs sorted by word (stable in feature order),
+//                    addWeight in feature order (BowVector.cpp:34-46), the sequential L1 norm in ascending word order
+//                    (:62-84), the division, the store at the problem's reserved offset of its database;
+//   k_bow_score      one warp per earlier keyframe of a problem's database: L1Scoring::score (ScoringObject.cpp:23-68), the
+//                    common words' terms summed sequentially in ascending word order; a block-offset table spreads each
+//                    problem's row over blocks in proportion to its length.
 #include <errno.h>
 #include <locale.h>
 #include <math.h>
@@ -17,25 +21,30 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
+#include <unordered_map>
 
 #include "plf_internal.h"
 
 #define BOW_MAX_FEATURES 8192   // per kind, as keyframe matching
 #define BOW_MAX_KF (1 << 24)    // keyframe indices (rows are kf_idx + 1 doubles)
 #define BOW_SORT_THREADS 1024
+#define BOW_MAX_PROBLEMS 65535  // problems per plf_bow_insert_batch: grid.y of k_bow_assemble (no chunking)
 
 // ------------------------------------------------------------------------------------------------------------------
 // Device state
 // ------------------------------------------------------------------------------------------------------------------
 
-struct BowKind {
-  // vocabulary (48 bytes per node)
+struct BowVoc {   // 48 bytes per node
   bool has_voc = false;
   int root_n = 0;
   uint4* desc = nullptr;     // [n][2]
   int2* meta = nullptr;      // [n]
   double* weight = nullptr;  // [n]
-  // database: 12 bytes per stored entry + 8 per keyframe index
+};
+
+// One kind of one database: 12 bytes per stored entry + 8 per keyframe index.
+struct BowDb {
   uint32_t* words = nullptr;
   double* vals = nullptr;
   size_t cap = 0, end = 0;
@@ -45,8 +54,14 @@ struct BowKind {
   int last = -1;             // largest index inserted since the vocabulary was set
 };
 
+struct BowDbs {
+  BowDb kind[2];
+};
+
 struct BowState {
-  BowKind kind[2];
+  BowVoc voc[2];
+  BowDbs ctx_db;                                 // seq = -1: plf_bow_insert / plf_bow_erase / plf_bow_get
+  std::vector<std::unique_ptr<BowDbs>> seq_db;   // [max_sequences] once a sequence was inserted into, else empty
   int n_sm = 0;
   bool attr_set = false;
 };
@@ -313,7 +328,7 @@ T* dup_array(const std::vector<T>& v) {
   return p;
 }
 
-void free_db(BowKind& k) {
+void free_db(BowDb& k) {
   cudaFree(k.words);
   cudaFree(k.vals);
   cudaFree(k.ent);
@@ -326,7 +341,7 @@ void free_db(BowKind& k) {
   k.last = -1;
 }
 
-void free_kind(BowKind& k) {
+void free_voc(BowVoc& k) {
   cudaFree(k.desc);
   cudaFree(k.meta);
   cudaFree(k.weight);
@@ -334,7 +349,12 @@ void free_kind(BowKind& k) {
   k.meta = nullptr;
   k.weight = nullptr;
   k.has_voc = false;
-  free_db(k);
+}
+
+// The databases of seq (-1: the context's), or nullptr for a sequence never inserted into.
+BowDbs* dbs_of(BowState* S, int seq) {
+  if (seq < 0) return &S->ctx_db;
+  return seq < (int)S->seq_db.size() ? S->seq_db[seq].get() : nullptr;
 }
 
 BowState* bow_state(plf_ctx* ctx) {
@@ -391,24 +411,32 @@ __global__ void __launch_bounds__(256) k_bow_transform(TreeView t0, TreeView t1,
   }
 }
 
-struct AssembleKind {
-  int active, n, feat0;      // features [feat0, feat0 + n) of word / wt
-  uint32_t* words;           // the kind's database, entries appended at `end`
+// One kind of one problem of the problem table.
+struct BowProbKind {
+  uint32_t* words;           // its database
   double* vals;
   int2* ent;
-  long long end;
+  double* row;               // [kf_idx + 1] in the staged outputs, or nullptr: no row
+  long long off;             // the entries reserved for this problem start here (n of them)
+  int active, n, feat0;      // features [feat0, feat0 + n) of word / wt
+};
+struct BowProb {
+  BowProbKind k[2];
+  int kf_idx;
 };
 
-// TemplatedVocabulary::transform(features, v) for TF-IDF with L1 mustNormalize (:1046-1101): one block per kind.
-__global__ void __launch_bounds__(BOW_SORT_THREADS) k_bow_assemble(AssembleKind k0, AssembleKind k1, const int* __restrict__ word,
-                                                                   const double* __restrict__ wt, int kf_idx, int* __restrict__ nnz_out) {
+// TemplatedVocabulary::transform(features, v) for TF-IDF with L1 mustNormalize (:1046-1101): one block per (kind,
+// problem) = (blockIdx.x, blockIdx.y).  nnz_out[2 p + kind].
+__global__ void __launch_bounds__(BOW_SORT_THREADS) k_bow_assemble(const BowProb* __restrict__ probs, const int* __restrict__ word,
+                                                                   const double* __restrict__ wt, int* __restrict__ nnz_out) {
   extern __shared__ __align__(16) unsigned char smem[];
   unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem);           // [8192]
   double* sv = reinterpret_cast<double*>(smem + BOW_MAX_FEATURES * 8);               // [8192]
   __shared__ int s_scan[BOW_SORT_THREADS / 32];
   __shared__ double s_norm;
-  const AssembleKind K = blockIdx.x ? k1 : k0;
+  const BowProbKind K = probs[blockIdx.y].k[blockIdx.x];
   if (!K.active) return;
+  const int kf_idx = probs[blockIdx.y].kf_idx;
   const int tid = threadIdx.x, n = K.n;
   int N = 1;
   while (N < n) N <<= 1;
@@ -467,7 +495,7 @@ __global__ void __launch_bounds__(BOW_SORT_THREADS) k_bow_assemble(AssembleKind 
     const unsigned long long w = keys[i] >> 13;
     double v = wt[K.feat0 + (int)(keys[i] & 8191u)];
     for (int t = i + 1; t < m && (keys[t] >> 13) == w; ++t) v += wt[K.feat0 + (int)(keys[t] & 8191u)];
-    K.words[K.end + j] = (uint32_t)w;
+    K.words[K.off + j] = (uint32_t)w;
     sv[j++] = v;
   }
   __syncthreads();
@@ -476,38 +504,38 @@ __global__ void __launch_bounds__(BOW_SORT_THREADS) k_bow_assemble(AssembleKind 
     double norm = 0.0;
     for (int i = 0; i < nnz; ++i) norm += fabs(sv[i]);
     s_norm = norm;
-    K.ent[kf_idx] = make_int2((int)K.end, nnz);
-    nnz_out[blockIdx.x] = nnz;
+    K.ent[kf_idx] = make_int2((int)K.off, nnz);
+    nnz_out[2 * blockIdx.y + blockIdx.x] = nnz;
   }
   __syncthreads();
   const double norm = s_norm;
-  for (int i = tid; i < nnz; i += blockDim.x) K.vals[K.end + i] = norm > 0.0 ? sv[i] / norm : sv[i];
+  for (int i = tid; i < nnz; i += blockDim.x) K.vals[K.off + i] = norm > 0.0 ? sv[i] / norm : sv[i];
 }
 
-struct ScoreKind {
-  int active;
-  const uint32_t* words;
-  const double* vals;
-  const int2* ent;
-  double* row;               // [kf_idx + 1]
-};
-
-// L1Scoring::score(v_new, v_i) (ScoringObject.cpp:23-68) for every i <= kf_idx: one warp per keyframe, grid-stride.  The new
-// vector's words are staged in shared memory once per block; keyframe i's word list is read once, 32 coalesced words at
-// a time, each looked up in the new vector.  The terms |v - w| - |v| - |w| of the common words are added by every lane in
-// ascending word order (the ballot's bits), as DBoW2's merge adds them; score = -sum / 2.  Absent keyframes: NaN.
-__global__ void __launch_bounds__(256) k_bow_score(ScoreKind k0, ScoreKind k1, int kf_idx) {
+// L1Scoring::score(v_new, v_i) (ScoringObject.cpp:23-68) for every i <= kf_idx of each problem's database: one warp per
+// keyframe.  Blocks [boff[p], boff[p + 1]) of blockIdx.x serve problem p (kind blockIdx.y) and stride over its row.  The
+// new vector's words are staged in shared memory once per block; keyframe i's word list is read once, 32 coalesced words
+// at a time, each looked up in the new vector.  The terms |v - w| - |v| - |w| of the common words are added by every lane
+// in ascending word order (the ballot's bits), as DBoW2's merge adds them; score = -sum / 2.  Absent keyframes: NaN.
+__global__ void __launch_bounds__(256) k_bow_score(const BowProb* __restrict__ probs, const int* __restrict__ boff, int n_prob) {
   __shared__ uint32_t s_w[BOW_MAX_FEATURES];
-  const ScoreKind K = blockIdx.y ? k1 : k0;
-  if (!K.active) return;
+  // the problem of this block: the last p with boff[p] <= blockIdx.x (a problem without blocks is never the last)
+  int lo = 0, hi = n_prob - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(&boff[mid]) <= (int)blockIdx.x) lo = mid; else hi = mid - 1;
+  }
+  const BowProbKind K = probs[lo].k[blockIdx.y];
+  if (!K.row) return;
+  const int kf_idx = probs[lo].kf_idx, b0 = __ldg(&boff[lo]), nb = __ldg(&boff[lo + 1]) - b0;
   const int2 me = K.ent[kf_idx];
   const int nn = me.y;
   for (int i = threadIdx.x; i < nn; i += blockDim.x) s_w[i] = K.words[me.x + i];
   __syncthreads();
   const double* nv = K.vals + me.x;
   const int lane = threadIdx.x & 31;
-  const int nwarps = gridDim.x * 8;
-  for (int i = blockIdx.x * 8 + (threadIdx.x >> 5); i <= kf_idx; i += nwarps) {
+  const int nwarps = nb * 8;
+  for (int i = ((int)blockIdx.x - b0) * 8 + (threadIdx.x >> 5); i <= kf_idx; i += nwarps) {
     const int2 e = K.ent[i];
     if (e.y < 0) {
       if (lane == 0) K.row[i] = __longlong_as_double(0x7FF8000000000000ll);
@@ -542,17 +570,16 @@ __global__ void __launch_bounds__(256) k_bow_score(ScoreKind k0, ScoreKind k1, i
   }
 }
 
-// Grows the kind's database to hold `more` entries after `end` and keyframe indices up to kf_idx.
-plf_status grow_db(plf_ctx* ctx, BowKind& k, size_t more, int kf_idx) {
-  if (k.end + more > (size_t)INT32_MAX)   // entry offsets are int32 (int2 index entries)
-    return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_bow_insert: the %s database would exceed 2^31 - 1 entries", &k == &ctx->bow->kind[0] ? "point" : "line");
+// Grows one database kind to hold `more` entries after `end` and keyframe indices up to kf_idx; a first allocation takes
+// at least min_cap entries and min_ent indices.  The caller has checked end + more <= 2^31 - 1.
+plf_status grow_db(plf_ctx* ctx, const char* fn, BowDb& k, size_t more, int kf_idx, size_t min_cap, int min_ent) {
   if (k.end + more > k.cap) {
-    size_t nc = std::max(std::max(2 * k.cap, k.end + more), (size_t)1 << 16);
+    size_t nc = std::max(std::max(2 * k.cap, k.end + more), min_cap);
     uint32_t* w = nullptr;
     double* v = nullptr;
     if (cudaMalloc(&w, nc * 4) != cudaSuccess || cudaMalloc(&v, nc * 8) != cudaSuccess) {
       cudaFree(w);
-      return plf_fail(ctx, PLF_ERR_CUDA, "plf_bow_insert: cudaMalloc of a %zu-entry database failed", nc);
+      return plf_fail(ctx, PLF_ERR_CUDA, "%s: cudaMalloc of a %zu-entry database failed", fn, nc);
     }
     if (k.end) {
       PLF_CUDA(ctx, cudaMemcpyAsync(w, k.words, k.end * 4, cudaMemcpyDeviceToDevice, ctx->stream));
@@ -566,10 +593,10 @@ plf_status grow_db(plf_ctx* ctx, BowKind& k, size_t more, int kf_idx) {
     k.cap = nc;
   }
   if (kf_idx >= k.ent_cap) {
-    const int nc = (int)std::min<long long>(std::max<long long>(std::max(2LL * k.ent_cap, (long long)kf_idx + 1), 1024), BOW_MAX_KF);
+    const int nc = (int)std::min<long long>(std::max<long long>(std::max(2LL * k.ent_cap, (long long)kf_idx + 1), min_ent), BOW_MAX_KF);
     int2* e = nullptr;
     if (cudaMalloc(&e, (size_t)nc * 8) != cudaSuccess)
-      return plf_fail(ctx, PLF_ERR_CUDA, "plf_bow_insert: cudaMalloc of %d keyframe entries failed", nc);
+      return plf_fail(ctx, PLF_ERR_CUDA, "%s: cudaMalloc of %d keyframe entries failed", fn, nc);
     PLF_CUDA(ctx, cudaMemsetAsync(e, 0xFF, (size_t)nc * 8, ctx->stream));
     if (k.ent_cap) PLF_CUDA(ctx, cudaMemcpyAsync(e, k.ent, (size_t)k.ent_cap * 8, cudaMemcpyDeviceToDevice, ctx->stream));
     PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -580,13 +607,233 @@ plf_status grow_db(plf_ctx* ctx, BowKind& k, size_t more, int kf_idx) {
   return PLF_OK;
 }
 
+void free_dbs(BowDbs& d) {
+  for (BowDb& k : d.kind) free_db(k);
+}
+
+// Per database of a batch: the index and entry count its problems take per kind, and the next reserved offset.
+struct BatchDb {
+  BowDbs* dbs = nullptr;
+  int last[2] = {-1, -1};
+  size_t more[2] = {0, 0};
+  size_t next[2] = {0, 0};
+};
+
+// plf_bow_insert_batch; fn names the entry point in messages, and a call from plf_bow_insert (single) names no problem.
+plf_status bow_insert_problems(plf_ctx* ctx, const char* fn, bool single, int n_problems, plf_bow_problem* problems,
+                               const int32_t* seq) {
+  char who[96];
+  auto name = [&](int p) -> const char* {
+    if (single) snprintf(who, sizeof who, "%s", fn);
+    else snprintf(who, sizeof who, "%s: problem %d", fn, p);
+    return who;
+  };
+  if (n_problems < 0) return plf_fail(ctx, PLF_ERR_INVALID, "%s: n_problems = %d < 0", fn, n_problems);
+  if (n_problems > BOW_MAX_PROBLEMS)
+    return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: n_problems = %d exceeds %d (grid.y of the assembly; no chunking)", fn,
+                    n_problems, BOW_MAX_PROBLEMS);
+  if (n_problems == 0) return PLF_OK;
+  if (!problems) return plf_fail(ctx, PLF_ERR_INVALID, "%s: problems is NULL", fn);
+  const bool on[2] = {ctx->params.has_points != 0, ctx->params.has_lines != 0};
+  BowState* S = bow_state(ctx);
+  // refusals, before any work; one BatchDb per database the batch touches, in order of first use
+  std::unordered_map<int, int> db_at;
+  std::vector<BatchDb> bdb;
+  std::vector<int> prob_db(n_problems);
+  for (int p = 0; p < n_problems; ++p) {
+    const int s = seq ? seq[p] : -1;
+    if (s < -1 || s >= ctx->max_sequences)
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: seq[%d] = %d outside [-1, %d)", fn, p, p, s, ctx->max_sequences);
+    const plf_bow_problem& pr = problems[p];
+    if (!pr.kf) return plf_fail(ctx, PLF_ERR_INVALID, "%s: kf is NULL", name(p));
+    if (pr.kf_idx < 0 || pr.kf_idx >= BOW_MAX_KF)
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: kf_idx %d out of range [0, %d)", name(p), pr.kf_idx, BOW_MAX_KF);
+    auto it = db_at.find(s);
+    if (it == db_at.end()) {
+      it = db_at.emplace(s, (int)bdb.size()).first;
+      BatchDb b;
+      b.dbs = dbs_of(S, s);
+      for (int c = 0; c < 2; ++c) b.last[c] = b.dbs ? b.dbs->kind[c].last : -1;
+      bdb.push_back(b);
+    }
+    prob_db[p] = it->second;
+    BatchDb& b = bdb[it->second];
+    const int n[2] = {pr.kf->n_pt, pr.kf->n_ls};
+    const uint8_t* d[2] = {pr.kf->pdesc, pr.kf->ldesc};
+    for (int c = 0; c < 2; ++c) {
+      if (!on[c]) continue;
+      const char* kn = c ? "line" : "point";
+      if (n[c] < 0 || n[c] > BOW_MAX_FEATURES)
+        return plf_fail(ctx, PLF_ERR_INVALID, "%s: %d %s features (at most %d)", name(p), n[c], kn, BOW_MAX_FEATURES);
+      if (n[c] > 0 && !d[c]) return plf_fail(ctx, PLF_ERR_INVALID, "%s: %s descriptors are NULL", name(p), kn);
+      if (!S->voc[c].has_voc)
+        return plf_fail(ctx, PLF_ERR_STATE, "%s: no %s vocabulary (plf_bow_set_vocabulary)", name(p), kn);
+      if (pr.kf_idx <= b.last[c])
+        return plf_fail(ctx, PLF_ERR_INVALID, "%s: kf_idx %d does not exceed %d, inserted before into the %s database of "
+                        "seq %d", name(p), pr.kf_idx, b.last[c], kn, s);
+      b.last[c] = pr.kf_idx;
+      b.more[c] += (size_t)n[c];
+    }
+  }
+  for (const auto& e : db_at)
+    for (int c = 0; c < 2; ++c) {
+      const BatchDb& b = bdb[e.second];
+      const size_t end = b.dbs ? b.dbs->kind[c].end : 0;
+      if (on[c] && end + b.more[c] > (size_t)INT32_MAX)   // entry offsets are int32 (int2 index entries)
+        return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: the %s database of seq %d would exceed 2^31 - 1 entries", fn,
+                        c ? "line" : "point", e.first);
+    }
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t cs = ctx->stream;
+  // every database grows once, to its problems' upper bound; a sequence's first allocation is one keyframe's size
+  for (const auto& e : db_at) {
+    BatchDb& b = bdb[e.second];
+    if (!b.dbs) {
+      if (S->seq_db.empty()) S->seq_db.resize(ctx->max_sequences);
+      S->seq_db[e.first].reset(new BowDbs());
+      b.dbs = S->seq_db[e.first].get();
+    }
+    for (int c = 0; c < 2; ++c) {
+      if (!on[c]) continue;
+      BowDb& k = b.dbs->kind[c];
+      const bool own = e.first < 0;
+      if (plf_status st = grow_db(ctx, fn, k, b.more[c], b.last[c], own ? (size_t)1 << 16 : 1024, own ? 1024 : 64)) return st;
+      b.next[c] = k.end;
+    }
+  }
+  // the staged layout: descriptors (all points, then all lines), the problem table, the block offsets | the counts and
+  // the rows | the words and weights of the features
+  std::vector<BowProb> tab(n_problems);
+  std::vector<int> boff(n_problems + 1, 0);
+  int m[2] = {0, 0};
+  for (int p = 0; p < n_problems; ++p)
+    for (int c = 0; c < 2; ++c) m[c] += on[c] ? (c ? problems[p].kf->n_ls : problems[p].kf->n_pt) : 0;
+  const int nf = m[0] + m[1];
+  size_t row_b = 0;       // every requested row, packed
+  long long row_len = 0;  // the keyframes scored over all problems (one kind)
+  for (int p = 0; p < n_problems; ++p) {
+    const plf_bow_problem& pr = problems[p];
+    double* rows[2] = {pr.score_p, pr.score_l};
+    bool any = false;
+    for (int c = 0; c < 2; ++c) {
+      const bool r = on[c] && rows[c];
+      row_b += r ? (size_t)(pr.kf_idx + 1) * 8 : 0;
+      any |= r;
+    }
+    row_len += any ? pr.kf_idx + 1 : 0;
+  }
+  StagedLayout L;
+  const size_t desc_off = L.take_in((size_t)nf * 32), tab_off = L.take_in(sizeof(BowProb) * n_problems),
+               boff_off = L.take_in(sizeof(int) * (n_problems + 1));
+  const size_t nnz_off = L.take_out(2 * sizeof(int) * n_problems), rows_off = L.take_out(row_b);
+  const size_t w_off = L.take_work((size_t)nf * 4), wt_off = L.take_work((size_t)nf * 8);
+  // the rows grow by 16 bytes per keyframe: 1 MB up front keeps the inserts of the first ~50 000 keyframes from
+  // reallocating the slot (a stream synchronisation) every 32 keyframes
+  if (!plf_scratch(ctx, PLF_SCR_BOW, (size_t)1 << 20)) return PLF_ERR_CUDA;
+  uint8_t *pin, *dev;
+  if (plf_status st = L.acquire(ctx, PLF_SCR_BOW, &pin, &dev)) return st;
+  uint8_t *out = dev + L.in, *work = dev + L.in + L.out;
+  // the problem table; a problem's blocks of k_bow_score in proportion to its row, as one call's grid over one row
+  const long long budget = 4LL * S->n_sm;
+  size_t feat[2] = {0, (size_t)m[0]}, row_at = 0;
+  for (int p = 0; p < n_problems; ++p) {
+    const plf_bow_problem& pr = problems[p];
+    BatchDb& b = bdb[prob_db[p]];
+    const int n[2] = {pr.kf->n_pt, pr.kf->n_ls};
+    const uint8_t* d[2] = {pr.kf->pdesc, pr.kf->ldesc};
+    double* rows[2] = {pr.score_p, pr.score_l};
+    bool any = false;
+    for (int c = 0; c < 2; ++c) {
+      BowProbKind& K = tab[p].k[c];
+      memset(&K, 0, sizeof K);
+      if (!on[c]) continue;
+      const BowDb& k = b.dbs->kind[c];
+      K = {k.words, k.vals, k.ent, nullptr, (long long)b.next[c], 1, n[c], (int)feat[c]};
+      if (n[c]) memcpy(pin + desc_off + feat[c] * 32, d[c], (size_t)n[c] * 32);
+      feat[c] += n[c];
+      b.next[c] += n[c];
+      if (rows[c]) {
+        K.row = (double*)(out + rows_off + row_at);
+        row_at += (size_t)(pr.kf_idx + 1) * 8;
+        any = true;
+      }
+    }
+    tab[p].kf_idx = pr.kf_idx;
+    const long long len = any ? pr.kf_idx + 1 : 0;
+    boff[p + 1] = boff[p] + (int)std::min((len + 7) / 8, std::max(1LL, (budget * len + row_len - 1) / std::max(row_len, 1LL)));
+  }
+  memcpy(pin + tab_off, tab.data(), sizeof(BowProb) * n_problems);
+  memcpy(pin + boff_off, boff.data(), sizeof(int) * (n_problems + 1));
+  int* d_word = (int*)(work + w_off);
+  double* d_wt = (double*)(work + wt_off);
+  const BowProb* d_tab = (const BowProb*)(dev + tab_off);
+  PLF_CUDA(ctx, cudaMemcpyAsync(dev, pin, L.in, cudaMemcpyHostToDevice, cs));
+  if (nf) {
+    const BowVoc &a = S->voc[0], &b = S->voc[1];
+    const TreeView t0 = {a.desc, a.meta, a.weight, a.root_n}, t1 = {b.desc, b.meta, b.weight, b.root_n};
+    k_bow_transform<<<(nf + 7) / 8, 256, 0, cs>>>(t0, t1, (const uint4*)(dev + desc_off), m[0], m[1], d_word, d_wt);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  const size_t smem = (size_t)BOW_MAX_FEATURES * 16;
+  if (!S->attr_set) {
+    PLF_CUDA(ctx, cudaFuncSetAttribute(k_bow_assemble, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    S->attr_set = true;
+  }
+  k_bow_assemble<<<dim3(2, n_problems), BOW_SORT_THREADS, smem, cs>>>(d_tab, d_word, d_wt, (int*)(out + nnz_off));
+  PLF_LAUNCH_CHECK(ctx);
+  if (boff[n_problems]) {
+    k_bow_score<<<dim3(boff[n_problems], 2), 256, 0, cs>>>(d_tab, (const int*)(dev + boff_off), n_problems);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  // one download: the counts and the rows
+  PLF_CUDA(ctx, cudaMemcpyAsync(pin + L.in, out, row_b ? rows_off + row_b : nnz_off + 2 * sizeof(int) * n_problems,
+                                cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaStreamSynchronize(cs));
+  const int* nnz = (const int*)(pin + L.in + nnz_off);
+  for (int p = 0; p < n_problems; ++p) {
+    const plf_bow_problem& pr = problems[p];
+    BowDbs* dbs = bdb[prob_db[p]].dbs;
+    double* rows[2] = {pr.score_p, pr.score_l};
+    for (int c = 0; c < 2; ++c) {
+      if (!on[c]) continue;
+      BowDb& k = dbs->kind[c];
+      const BowProbKind& K = tab[p].k[c];
+      if ((int)k.host_ent.size() < pr.kf_idx + 1) k.host_ent.resize(pr.kf_idx + 1, make_int2(-1, -1));
+      k.host_ent[pr.kf_idx] = make_int2((int)K.off, nnz[2 * p + c]);
+      k.end = (size_t)K.off + (size_t)nnz[2 * p + c];
+      k.last = pr.kf_idx;
+      if (rows[c]) memcpy(rows[c], pin + L.in + ((uint8_t*)K.row - out), (size_t)(pr.kf_idx + 1) * 8);
+    }
+  }
+  return PLF_OK;
+}
+
+// The databases of seq for plf_bow_erase_seq / plf_bow_get_seq: PLF_OK with *d = nullptr when it has none.
+plf_status seq_dbs(plf_ctx* ctx, const char* fn, int s, BowDbs** d) {
+  *d = nullptr;
+  if (s < -1 || s >= ctx->max_sequences)
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: seq %d outside [-1, %d)", fn, s, ctx->max_sequences);
+  if (ctx->bow) *d = dbs_of(ctx->bow, s);
+  return PLF_OK;
+}
+
 }  // namespace
+
+void plf_bow_drop_sequences(plf_ctx* ctx) {
+  if (!ctx->bow) return;
+  for (auto& d : ctx->bow->seq_db)
+    if (d) free_dbs(*d);
+  ctx->bow->seq_db.clear();
+  ctx->bow->seq_db.shrink_to_fit();
+}
 
 extern "C" {
 
 void plf_bow_free(plf_ctx* ctx) {
   if (!ctx->bow) return;
-  for (BowKind& k : ctx->bow->kind) free_kind(k);
+  plf_bow_drop_sequences(ctx);
+  for (BowVoc& v : ctx->bow->voc) free_voc(v);
+  free_dbs(ctx->bow->ctx_db);
   delete ctx->bow;
   ctx->bow = nullptr;
 }
@@ -656,13 +903,17 @@ plf_status plf_bow_set_vocabulary(plf_ctx* ctx, int kind, const plf_vocab* voc) 
   if (!why.empty()) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_set_vocabulary: %s", why.c_str());
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   BowState* S = bow_state(ctx);
-  BowKind& k = S->kind[kind];
+  BowVoc& k = S->voc[kind];
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  free_kind(k);
+  free_voc(k);
+  // the kind is emptied in every database
+  free_db(S->ctx_db.kind[kind]);
+  for (auto& d : S->seq_db)
+    if (d) free_db(d->kind[kind]);
   const size_t n = lay.meta.size();
   if (cudaMalloc(&k.desc, n * 32) != cudaSuccess || cudaMalloc(&k.meta, n * 8) != cudaSuccess ||
       cudaMalloc(&k.weight, n * 8) != cudaSuccess) {
-    free_kind(k);
+    free_voc(k);
     return plf_fail(ctx, PLF_ERR_CUDA, "plf_bow_set_vocabulary: cudaMalloc for %zu nodes failed", n);
   }
   PLF_CUDA(ctx, cudaMemcpy(k.desc, lay.desc.data(), n * 32, cudaMemcpyHostToDevice));
@@ -675,104 +926,24 @@ plf_status plf_bow_set_vocabulary(plf_ctx* ctx, int kind, const plf_vocab* voc) 
 
 plf_status plf_bow_insert(plf_ctx* ctx, int kf_idx, const plf_frame_view* kf, double* score_p, double* score_l) {
   if (!ctx) return PLF_ERR_INVALID;
-  if (!kf) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_insert: kf is NULL");
-  if (kf_idx < 0 || kf_idx >= BOW_MAX_KF)
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_insert: kf_idx %d out of range [0, %d)", kf_idx, BOW_MAX_KF);
-  const int n[2] = {kf->n_pt, kf->n_ls};
-  const uint8_t* d[2] = {kf->pdesc, kf->ldesc};
-  const bool on[2] = {ctx->params.has_points != 0, ctx->params.has_lines != 0};
-  double* rows[2] = {score_p, score_l};
-  BowState* S = bow_state(ctx);
-  for (int c = 0; c < 2; ++c) {
-    if (!on[c]) continue;
-    if (n[c] < 0 || n[c] > BOW_MAX_FEATURES)
-      return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_insert: %d %s features (at most %d)", n[c], c ? "line" : "point", BOW_MAX_FEATURES);
-    if (n[c] > 0 && !d[c]) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_insert: %s descriptors are NULL", c ? "line" : "point");
-    if (!S->kind[c].has_voc)
-      return plf_fail(ctx, PLF_ERR_STATE, "plf_bow_insert: no %s vocabulary (plf_bow_set_vocabulary)", c ? "line" : "point");
-    if (kf_idx <= S->kind[c].last)
-      return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_insert: kf_idx %d does not exceed %d, inserted before", kf_idx,
-                      S->kind[c].last);
-  }
-  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t cs = ctx->stream;
-  for (int c = 0; c < 2; ++c)
-    if (on[c]) {
-      plf_status st = grow_db(ctx, S->kind[c], (size_t)n[c], kf_idx);
-      if (st) return st;
-    }
-  const int m0 = on[0] ? n[0] : 0, m1 = on[1] ? n[1] : 0, nf = m0 + m1;
-  const size_t row_b = (size_t)(kf_idx + 1) * 8;
-  StagedLayout L;
-  L.take_in((size_t)nf * 32);
-  const size_t w_off = L.take_work((size_t)nf * 4), wt_off = L.take_work((size_t)nf * 8);
-  const size_t nnz_off = L.take_out(2 * sizeof(int)), row_off[2] = {L.take_out(row_b), L.take_out(row_b)};
-  // the rows grow by 16 bytes per keyframe: 1 MB up front keeps the inserts of the first ~50 000 keyframes from
-  // reallocating the slot (a stream synchronisation) every 32 keyframes
-  if (!plf_scratch(ctx, PLF_SCR_BOW, (size_t)1 << 20)) return PLF_ERR_CUDA;
-  uint8_t *pin, *dev;
-  if (plf_status st = L.acquire(ctx, PLF_SCR_BOW, &pin, &dev)) return st;
-  if (m0) memcpy(pin, d[0], (size_t)m0 * 32);
-  if (m1) memcpy(pin + (size_t)m0 * 32, d[1], (size_t)m1 * 32);
-  uint8_t *out = dev + L.in, *work = dev + L.in + L.out;
-  int* d_word = (int*)(work + w_off);
-  double* d_wt = (double*)(work + wt_off);
-  int* d_nnz = (int*)(out + nnz_off);
-  double* d_row[2] = {(double*)(out + row_off[0]), (double*)(out + row_off[1])};
-  if (nf) PLF_CUDA(ctx, cudaMemcpyAsync(dev, pin, (size_t)nf * 32, cudaMemcpyHostToDevice, cs));
-  if (nf) {
-    const BowKind &a = S->kind[0], &b = S->kind[1];
-    const TreeView t0 = {a.desc, a.meta, a.weight, a.root_n}, t1 = {b.desc, b.meta, b.weight, b.root_n};
-    k_bow_transform<<<(nf + 7) / 8, 256, 0, cs>>>(t0, t1, (const uint4*)dev, m0, m1, d_word, d_wt);
-    PLF_LAUNCH_CHECK(ctx);
-  }
-  const size_t smem = (size_t)BOW_MAX_FEATURES * 16;
-  if (!S->attr_set) {
-    PLF_CUDA(ctx, cudaFuncSetAttribute(k_bow_assemble, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    S->attr_set = true;
-  }
-  AssembleKind ak[2];
-  for (int c = 0; c < 2; ++c) {
-    BowKind& k = S->kind[c];
-    ak[c] = {on[c] ? 1 : 0, c ? m1 : m0, c ? m0 : 0, k.words, k.vals, k.ent, (long long)k.end};
-  }
-  k_bow_assemble<<<2, BOW_SORT_THREADS, smem, cs>>>(ak[0], ak[1], d_word, d_wt, kf_idx, d_nnz);
-  PLF_LAUNCH_CHECK(ctx);
-  ScoreKind sk[2];
-  bool any_row = false;
-  for (int c = 0; c < 2; ++c) {
-    BowKind& k = S->kind[c];
-    sk[c] = {on[c] && rows[c] ? 1 : 0, k.words, k.vals, k.ent, d_row[c]};
-    any_row |= sk[c].active != 0;
-  }
-  if (any_row) {
-    const int blocks = std::min((kf_idx + 1 + 7) / 8, 4 * S->n_sm);
-    k_bow_score<<<dim3(blocks, 2), 256, 0, cs>>>(sk[0], sk[1], kf_idx);
-    PLF_LAUNCH_CHECK(ctx);
-  }
-  // one download: the counts and the rows
-  const size_t dl = any_row ? row_off[sk[1].active ? 1 : 0] + row_b : nnz_off + 2 * sizeof(int);
-  PLF_CUDA(ctx, cudaMemcpyAsync(pin + L.in, out, dl, cudaMemcpyDeviceToHost, cs));
-  PLF_CUDA(ctx, cudaStreamSynchronize(cs));
-  const int* nnz = (const int*)(pin + L.in + nnz_off);
-  for (int c = 0; c < 2; ++c) {
-    if (!on[c]) continue;
-    BowKind& k = S->kind[c];
-    if ((int)k.host_ent.size() < kf_idx + 1) k.host_ent.resize(kf_idx + 1, make_int2(-1, -1));
-    k.host_ent[kf_idx] = make_int2((int)k.end, nnz[c]);
-    k.end += (size_t)nnz[c];
-    k.last = kf_idx;
-    if (rows[c]) memcpy(rows[c], pin + L.in + row_off[c], row_b);
-  }
-  return PLF_OK;
+  plf_bow_problem pr = {kf_idx, kf, score_p, score_l};
+  return bow_insert_problems(ctx, "plf_bow_insert", true, 1, &pr, nullptr);
 }
 
-plf_status plf_bow_erase(plf_ctx* ctx, int kf_idx) {
+plf_status plf_bow_insert_batch(plf_ctx* ctx, int n_problems, plf_bow_problem* problems, const int32_t* seq) {
   if (!ctx) return PLF_ERR_INVALID;
-  if (kf_idx < 0) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_erase: kf_idx %d < 0", kf_idx);
-  if (!ctx->bow) return PLF_OK;
+  return bow_insert_problems(ctx, "plf_bow_insert_batch", false, n_problems, problems, seq);
+}
+
+plf_status plf_bow_erase_seq(plf_ctx* ctx, int s, int kf_idx) {
+  if (!ctx) return PLF_ERR_INVALID;
+  const char* fn = s < 0 ? "plf_bow_erase" : "plf_bow_erase_seq";
+  BowDbs* d;
+  if (plf_status st = seq_dbs(ctx, fn, s, &d)) return st;
+  if (kf_idx < 0) return plf_fail(ctx, PLF_ERR_INVALID, "%s: kf_idx %d < 0", fn, kf_idx);
+  if (!d) return PLF_OK;
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  for (BowKind& k : ctx->bow->kind) {
+  for (BowDb& k : d->kind) {
     if (kf_idx >= (int)k.host_ent.size() || k.host_ent[kf_idx].y < 0) continue;
     k.host_ent[kf_idx] = make_int2(-1, -1);
     PLF_CUDA(ctx, cudaMemsetAsync(k.ent + kf_idx, 0xFF, 8, ctx->stream));
@@ -780,22 +951,44 @@ plf_status plf_bow_erase(plf_ctx* ctx, int kf_idx) {
   return PLF_OK;
 }
 
-plf_status plf_bow_get(plf_ctx* ctx, int kf_idx, int kind, int cap, uint32_t* words, double* values, int* n) {
+plf_status plf_bow_erase(plf_ctx* ctx, int kf_idx) { return plf_bow_erase_seq(ctx, -1, kf_idx); }
+
+plf_status plf_bow_get_seq(plf_ctx* ctx, int s, int kf_idx, int kind, int cap, uint32_t* words, double* values, int* n) {
   if (!ctx) return PLF_ERR_INVALID;
-  if (!n || (kind != 0 && kind != 1)) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_get: kind 0 or 1 and n are required");
+  const char* fn = s < 0 ? "plf_bow_get" : "plf_bow_get_seq";
+  BowDbs* d;
+  if (plf_status st = seq_dbs(ctx, fn, s, &d)) return st;
+  if (!n || (kind != 0 && kind != 1)) return plf_fail(ctx, PLF_ERR_INVALID, "%s: kind 0 or 1 and n are required", fn);
   *n = 0;
-  const BowKind* k = ctx->bow ? &ctx->bow->kind[kind] : nullptr;
+  const BowDb* k = d ? &d->kind[kind] : nullptr;
   if (!k || kf_idx < 0 || kf_idx >= (int)k->host_ent.size() || k->host_ent[kf_idx].y < 0)
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_get: keyframe %d has no stored %s vector", kf_idx, kind ? "line" : "point");
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: keyframe %d has no stored %s vector", fn, kf_idx, kind ? "line" : "point");
   const int2 e = k->host_ent[kf_idx];
   *n = e.y;
   if (!words && !values) return PLF_OK;
-  if (e.y > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_bow_get: %d entries, capacity %d", e.y, cap);
+  if (e.y > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: %d entries, capacity %d", fn, e.y, cap);
   if (e.y == 0) return PLF_OK;
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (words) PLF_CUDA(ctx, cudaMemcpy(words, k->words + e.x, (size_t)e.y * 4, cudaMemcpyDeviceToHost));
   if (values) PLF_CUDA(ctx, cudaMemcpy(values, k->vals + e.x, (size_t)e.y * 8, cudaMemcpyDeviceToHost));
+  return PLF_OK;
+}
+
+plf_status plf_bow_get(plf_ctx* ctx, int kf_idx, int kind, int cap, uint32_t* words, double* values, int* n) {
+  return plf_bow_get_seq(ctx, -1, kf_idx, kind, cap, words, values, n);
+}
+
+plf_status plf_bow_clear_sequence(plf_ctx* ctx, int s) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (s < 0 || s >= ctx->max_sequences)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_clear_sequence: s = %d outside [0, %d)", s, ctx->max_sequences);
+  BowDbs* d = ctx->bow ? dbs_of(ctx->bow, s) : nullptr;
+  if (!d) return PLF_OK;
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  free_dbs(*d);
+  ctx->bow->seq_db[s].reset();
   return PLF_OK;
 }
 

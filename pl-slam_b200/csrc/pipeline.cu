@@ -887,6 +887,7 @@ plf_status plf_set_max_sequences(plf_ctx* ctx, int n) {
   ctx->max_sequences = n;
   ctx->seq_cam.clear();
   ctx->seq_cam_own.clear();
+  plf_bow_drop_sequences(ctx);
   return PLF_OK;
 }
 

@@ -33,7 +33,7 @@ enum plf_scratch_slot {
   PLF_SCR_KF,          // plf_match_kf2kf, plf_match_map2kf and their _batch forms: their staged layout
   PLF_SCR_KF_MGB_PT,   // plf_match_kf2kf, plf_match_map2kf and their _batch forms: the windowed matcher of points
   PLF_SCR_KF_MGB_LS,   //   ... and of lines
-  PLF_SCR_BOW,         // plf_bow_insert
+  PLF_SCR_BOW,         // plf_bow_insert, plf_bow_insert_batch
   PLF_SCR_BA_BATCH,    // plf_local_ba_batch: its staged layout
   PLF_SCR_LC,          // plf_loop_closure_pose and plf_loop_closure_pose_batch: their staged layout
   PLF_SCR_COUNT
@@ -116,6 +116,8 @@ plf_status plf_problem_cameras(plf_ctx* ctx, const char* fn, int n, const int32_
 // Ensures scratch slot `slot` holds at least `bytes`; returns device pointer or nullptr (error set).
 void* plf_scratch(plf_ctx* ctx, plf_scratch_slot slot, size_t bytes);
 void* plf_pinned(plf_ctx* ctx, size_t bytes);
+// Frees every sequence's bag-of-words databases (dbow.cu); plf_set_max_sequences drops them.
+void plf_bow_drop_sequences(plf_ctx* ctx);
 
 #define PLF_CUDA(ctx, call)                                                                  \
   do {                                                                                       \

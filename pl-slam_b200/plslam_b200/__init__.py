@@ -185,6 +185,10 @@ class plf_map2kf_problem(C.Structure):
                 ("n_pt", C.c_int), ("n_ls", C.c_int)]
 
 
+class plf_bow_problem(C.Structure):
+    _fields_ = [("kf_idx", C.c_int), ("kf", C.POINTER(plf_frame_view)), ("score_p", C.c_void_p), ("score_l", C.c_void_p)]
+
+
 class plf_vocab(C.Structure):
     _fields_ = [("k", C.c_int), ("L", C.c_int), ("scoring", C.c_int), ("weighting", C.c_int), ("n_nodes", C.c_int),
                 ("node_id", C.c_void_p), ("parent_id", C.c_void_p), ("weight", C.c_void_p), ("desc", C.c_void_p),
@@ -867,17 +871,52 @@ class Frontend:
         self._check(self.lib.plf_bow_insert(self._ctx, int(kf_idx), C.byref(v), ptr[0], ptr[1]), "plf_bow_insert")
         return out[0], out[1]
 
-    def bow_erase(self, kf_idx):
-        self._check(self.lib.plf_bow_erase(self._ctx, int(kf_idx)), "plf_bow_erase")
+    def bow_insert_batch(self, problems, seq=None, rows=(True, True)):
+        """Many bow_insert in one device call (plf_bow_insert_batch).  problems: dicts kf_idx, pdesc, ldesc (either
+        descriptor array may be missing: no features of that kind); seq: per problem the database, -1 for the context's
+        (the one bow_insert uses) or a sequence in [0, max_sequences) (None = all -1).  Returns one (score_p, score_l) per
+        problem, as bow_insert does.  Raises PlfError for the refusals before any work."""
+        problems = list(problems)
+        P = len(problems)
+        seq_a = self._problem_sequences(P, seq)
+        enabled = (self.params.has_points, self.params.has_lines)
+        keep, outs = [], []
+        arr = (plf_bow_problem * max(P, 1))()
+        for k, pr in enumerate(problems):
+            v = _frame_view({key: pr[key] for key in ("pdesc", "ldesc") if pr.get(key) is not None}, keep)
+            keep.append(v)
+            kf = int(pr["kf_idx"])
+            out = [np.full(kf + 1, np.nan) if (rows[c] and enabled[c] and kf >= 0) else None for c in range(2)]
+            outs.append(tuple(out))
+            arr[k] = plf_bow_problem(kf, C.pointer(v), *[o.ctypes.data if o is not None else None for o in out])
+        self._check(self.lib.plf_bow_insert_batch(self._ctx, P, arr, None if seq_a is None else _ptr(seq_a, C.c_int32)),
+                    "plf_bow_insert_batch")
+        return outs
 
-    def bow_vector(self, kf_idx, kind):
-        """plf_bow_get: the stored BowVector of keyframe kf_idx, kind 0 / 1, as (words uint32, values float64)."""
+    def bow_erase(self, kf_idx, seq=None):
+        """plf_bow_erase, or plf_bow_erase_seq on sequence seq's database (-1: the context's)."""
+        if seq is None:
+            self._check(self.lib.plf_bow_erase(self._ctx, int(kf_idx)), "plf_bow_erase")
+        else:
+            self._check(self.lib.plf_bow_erase_seq(self._ctx, int(seq), int(kf_idx)), "plf_bow_erase_seq")
+
+    def bow_vector(self, kf_idx, kind, seq=None):
+        """plf_bow_get: the stored BowVector of keyframe kf_idx, kind 0 / 1, as (words uint32, values float64); with seq,
+        plf_bow_get_seq on that sequence's database (-1: the context's)."""
+        if seq is None:
+            fn, get = "plf_bow_get", lambda *a: self.lib.plf_bow_get(self._ctx, *a)
+        else:
+            fn, get = "plf_bow_get_seq", lambda *a: self.lib.plf_bow_get_seq(self._ctx, int(seq), *a)
         n = C.c_int(0)
-        self._check(self.lib.plf_bow_get(self._ctx, int(kf_idx), int(kind), 0, None, None, C.byref(n)), "plf_bow_get")
+        self._check(get(int(kf_idx), int(kind), 0, None, None, C.byref(n)), fn)
         w, x = np.zeros(max(n.value, 1), np.uint32), np.zeros(max(n.value, 1), np.float64)
-        self._check(self.lib.plf_bow_get(self._ctx, int(kf_idx), int(kind), n.value, C.c_void_p(w.ctypes.data),
-                                         C.c_void_p(x.ctypes.data), C.byref(n)), "plf_bow_get")
+        self._check(get(int(kf_idx), int(kind), n.value, C.c_void_p(w.ctypes.data), C.c_void_p(x.ctypes.data),
+                        C.byref(n)), fn)
         return w[:n.value].copy(), x[:n.value].copy()
+
+    def bow_clear_sequence(self, s):
+        """plf_bow_clear_sequence: empties sequence s's bag-of-words database and frees its device memory."""
+        self._check(self.lib.plf_bow_clear_sequence(self._ctx, int(s)), "plf_bow_clear_sequence")
 
     def expmap_se3(self, x):
         x = np.ascontiguousarray(x, np.float64).reshape(6)
