@@ -57,28 +57,35 @@ def f32(x):
 
 
 def back_projection(cam, u, v, disp):
-    """PinholeStereoCamera::backProjection (SURVEY A.4): Z = fx b / d, X = Z (u - cx) / fx, Y = Z (v - cy) / fy."""
-    Z = cam["fx"] * cam["b"] / disp
-    return np.array([Z * (u - cam["cx"]) / cam["fx"], Z * (v - cam["cy"]) / cam["fy"], Z])
+    """PinholeStereoCamera::backProjection (SURVEY A.4): Z = fx b / d, X = Z (u - cx) / fx, Y = Z (v - cy) / fy, in IEEE
+    double arithmetic: a zero disparity (accepted where min_disp <= 0) gives Z = inf, and X or Y = NaN on the centre row
+    or column."""
+    with np.errstate(divide="ignore", invalid="ignore"):
+        Z = np.float64(cam["fx"] * cam["b"]) / np.float64(disp)
+        return np.array([Z * (u - cam["cx"]) / cam["fx"], Z * (v - cam["cy"]) / cam["fy"], Z])
 
 
-def line_overlap_stereo(spl_obs, epl_obs, spl_proj, epl_proj, line_horiz_th):
-    """stvo-pl StereoFrame::lineSegmentOverlapStereo on the endpoints' rows."""
-    overlap = 1.0
+def line_overlap_stereo(spl_obs, epl_obs, spl_proj, epl_proj, line_horiz_th, trace=False):
+    """stvo-pl StereoFrame::lineSegmentOverlapStereo on the endpoints' rows.  trace=True also returns the branch that
+    produced the overlap ("horizontal": the left line is within line_horiz_th of horizontal, overlap 1; "disjoint";
+    "containing": the right line's rows contain the left line's; "partial") and whether the clamp to 1 and the
+    length <= 0.01f rule acted."""
+    overlap, branch, clamped, short = 1.0, "horizontal", False, False
     if abs(epl_obs - spl_obs) > line_horiz_th:
         sln, eln = min(spl_obs, epl_obs), max(spl_obs, epl_obs)
         spn, epn = min(spl_proj, epl_proj), max(spl_proj, epl_proj)
         length = eln - spn
         if epn < sln or spn > eln:
-            overlap = 0.0
+            overlap, branch = 0.0, "disjoint"
         elif epn > eln and spn < sln:
-            overlap = eln - sln
+            overlap, branch = eln - sln, "containing"
         else:
-            overlap = min(eln, epn) - max(sln, spn)
-        overlap = overlap / length if length > f32(0.01) else 0.0
+            overlap, branch = min(eln, epn) - max(sln, spn), "partial"
+        short = not length > f32(0.01)
+        overlap = 0.0 if short else overlap / length
         if overlap > 1.0:
-            overlap = 1.0
-    return overlap
+            overlap, clamped = 1.0, True
+    return (overlap, branch, clamped, short) if trace else overlap
 
 
 @dataclass
@@ -105,9 +112,15 @@ def grid_scales(cam):
     return GRID_COLS / float(cam["width"]), GRID_ROWS / float(cam["height"])
 
 
+CELL_LIM = float(1 << 28)
+
+
 def _cell(v):
-    """double -> int conversion of a scaled coordinate (C++ truncation toward zero)."""
-    return np.trunc(np.asarray(v, np.float64)).astype(np.int64)
+    """double -> int conversion of a scaled coordinate: C++ truncation toward zero where the reference's conversion is
+    defined.  The library's one rule for the rest (plf_geom.cuh plf_qcell): NaN -> 0 (a projection at infinity), values
+    clamped to +-2^28 (beyond int range the conversion is undefined; the clamp keeps Bresenham differences inside int)."""
+    v = np.asarray(v, np.float64)
+    return np.where(np.isnan(v), 0, np.trunc(np.clip(v, -CELL_LIM, CELL_LIM))).astype(np.int64)
 
 
 def grid_match_points(cam, q_xy, d1, t_xy, d2, w, nnr, best_lr):
@@ -138,7 +151,10 @@ def grid_match_lines(cam, q_se, d1, t_se, d2, w, nnr, line_sim_th, best_lr):
                                float(np.float32(line_sim_th)), best_lr)
 
 
-def stereo_points(cam, kp_l, desc_l, kp_r, desc_r, prm, match_fn=None):
+def stereo_points(cam, kp_l, desc_l, kp_r, desc_r, prm, match_fn=None, trace=False):
+    """matchStereoPoints.  trace=True also returns, per matched left key point (in left-index order), the values the
+    gates compare and their decisions: i, j (left / right index), epip = f32 |yl - yr| (epip_f64: the same difference
+    in double), d = f32 xl - xr (nan where the epipolar gate rejects), epip_ok, disp_ok, ok."""
     if prm.get("matching_strategy", 0) and match_fn is None:
         # stvo-pl matchStereoPoints: window (matching_s_ws, 0) x (0, 0) left of / on the query's cell (A.2)
         q = np.stack([kp_l["x"].astype(np.float64), kp_l["y"].astype(np.float64)], 1)
@@ -148,31 +164,50 @@ def stereo_points(cam, kp_l, desc_l, kp_r, desc_r, prm, match_fn=None):
     else:
         m12, _ = (match_fn or om.match)(desc_l, desc_r, prm["min_ratio_12_p"], prm["best_lr_matches"])
     pl, disp, P, octv, rows = [], [], [], [], []
+    tr = []
     for i, j in enumerate(m12):
         if j < 0:
             continue
         xl, yl, xr, yr = kp_l["x"][i], kp_l["y"][i], kp_r["x"][j], kp_r["y"][j]   # float32 pixels
-        if abs(np.float32(yl - yr)) <= f32(prm["max_dist_epip"]):
+        epip = abs(np.float32(yl - yr))
+        epip_ok, disp_ok, d = bool(epip <= f32(prm["max_dist_epip"])), False, np.nan
+        if epip_ok:
             d = float(np.float32(xl - xr))
-            if d >= f32(prm["min_disp"]):
+            disp_ok = d >= f32(prm["min_disp"])
+            if disp_ok:
                 pl.append((float(xl), float(yl))); disp.append(d)
                 P.append(back_projection(cam, float(xl), float(yl), d)); octv.append(int(kp_l["octave"][i])); rows.append(i)
+        if trace:
+            tr.append((i, j, float(epip), abs(float(yl) - float(yr)), d, epip_ok, disp_ok, epip_ok and disp_ok))
     n = len(rows)
-    return (np.array(pl, np.float64).reshape(n, 2), np.array(disp, np.float64), np.array(P, np.float64).reshape(n, 3),
-            np.array(octv, np.int32), desc_l[rows].reshape(n, 32))
+    out = (np.array(pl, np.float64).reshape(n, 2), np.array(disp, np.float64), np.array(P, np.float64).reshape(n, 3),
+           np.array(octv, np.int32), desc_l[rows].reshape(n, 32))
+    if not trace:
+        return out
+    return out, _trace(tr, ("i", "j", "epip", "epip_f64", "d", "epip_ok", "disp_ok", "ok"))
+
+
+def _trace(rows, names):
+    cols = list(zip(*rows)) if rows else [()] * len(names)
+    return {k: np.array(c) for k, c in zip(names, cols)}
 
 
 def _kl_se(kl):
     return np.stack([kl["startPointX"], kl["startPointY"], kl["endPointX"], kl["endPointY"]], 1).astype(np.float64)
 
 
-def stereo_lines(cam, kl_l, desc_l, kl_r, desc_r, prm, match_fn=None):
+def stereo_lines(cam, kl_l, desc_l, kl_r, desc_r, prm, match_fn=None, trace=False):
+    """matchStereoLines.  trace=True also returns, per matched left line (in left-index order): i, j, r0 = the right
+    line's syr - eyr (f64) and horiz = f32 |r0|, overlap and its branch / clamped / short (line_overlap_stereo),
+    disp_s, disp_e and ratio = min / max (before the ratio gate resets the disparities), and the decisions ratio_ok,
+    disp_ok (both disparities >= min_disp after the ratio gate), horiz_ok, overlap_ok, ok."""
     if prm.get("matching_strategy", 0) and match_fn is None:
         m12, _ = grid_match_lines(cam, _kl_se(kl_l), desc_l, _kl_se(kl_r), desc_r, (int(prm["matching_s_ws"]), 0, 0, 0),
                                   prm["min_ratio_12_l"], prm["line_sim_th"], prm["best_lr_matches"])
     else:
         m12, _ = (match_fn or om.match)(desc_l, desc_r, prm["min_ratio_12_l"], prm["best_lr_matches"])
     out = dict(spl=[], epl=[], sdisp=[], edisp=[], sP=[], eP=[], le=[], angle=[], rows=[])
+    tr = []
     for i, j in enumerate(m12):
         if j < 0:
             continue
@@ -183,25 +218,38 @@ def stereo_lines(cam, kl_l, desc_l, kl_r, desc_r, prm, match_fn=None):
         sp_r = np.array([float(kl_r["startPointX"][j]), float(kl_r["startPointY"][j]), 1.0])
         ep_r = np.array([float(kl_r["endPointX"][j]), float(kl_r["endPointY"][j]), 1.0])
         le_r = np.cross(sp_r, ep_r)
-        overlap = line_overlap_stereo(sp_l[1], ep_l[1], sp_r[1], ep_r[1], f32(prm["line_horiz_th"]))
+        overlap, branch, clamped, short = line_overlap_stereo(sp_l[1], ep_l[1], sp_r[1], ep_r[1], f32(prm["line_horiz_th"]),
+                                                              trace=True)
         with np.errstate(divide="ignore", invalid="ignore"):
             sxr = -(le_r[2] + le_r[1] * sp_l[1]) / le_r[0]
             exr = -(le_r[2] + le_r[1] * ep_l[1]) / le_r[0]
         disp_s, disp_e = sp_l[0] - sxr, ep_l[0] - exr
+        ds0, de0 = disp_s, disp_e
         # filterLineSegmentDisparity
         with np.errstate(divide="ignore", invalid="ignore"):
-            if not (min(disp_s, disp_e) / max(disp_s, disp_e) >= f32(prm["ls_min_disp_ratio"])):
+            ratio = min(disp_s, disp_e) / max(disp_s, disp_e)
+            ratio_ok = bool(ratio >= f32(prm["ls_min_disp_ratio"]))
+            if not ratio_ok:
                 disp_s = disp_e = -1.0
-        if (disp_s >= f32(prm["min_disp"]) and disp_e >= f32(prm["min_disp"]) and
-                abs(np.float32(le_r[0])) > f32(prm["line_horiz_th"]) and overlap > f32(prm["stereo_overlap_th"])):
+        disp_ok = bool(disp_s >= f32(prm["min_disp"]) and disp_e >= f32(prm["min_disp"]))
+        horiz = abs(np.float32(le_r[0]))
+        horiz_ok, overlap_ok = bool(horiz > f32(prm["line_horiz_th"])), bool(overlap > f32(prm["stereo_overlap_th"]))
+        if trace:
+            tr.append((i, j, le_r[0], float(horiz), overlap, branch, clamped, short, ds0, de0, ratio, ratio_ok, disp_ok,
+                       horiz_ok, overlap_ok, disp_ok and horiz_ok and overlap_ok))
+        if disp_ok and horiz_ok and overlap_ok:
             out["spl"].append(sp_l[:2]); out["epl"].append(ep_l[:2]); out["sdisp"].append(disp_s); out["edisp"].append(disp_e)
             out["sP"].append(back_projection(cam, sp_l[0], sp_l[1], disp_s))
             out["eP"].append(back_projection(cam, ep_l[0], ep_l[1], disp_e))
             out["le"].append(le_l); out["angle"].append(kl_l["angle"][i]); out["rows"].append(i)
     n = len(out["rows"])
     a = lambda k, c: np.array(out[k], np.float64).reshape(n, c) if c > 1 else np.array(out[k], np.float64)
-    return (a("spl", 2), a("epl", 2), a("sdisp", 1), a("edisp", 1), a("sP", 3), a("eP", 3), a("le", 3),
-            np.array(out["angle"], np.float32), desc_l[out["rows"]].reshape(n, 32))
+    res = (a("spl", 2), a("epl", 2), a("sdisp", 1), a("edisp", 1), a("sP", 3), a("eP", 3), a("le", 3),
+           np.array(out["angle"], np.float32), desc_l[out["rows"]].reshape(n, 32))
+    if not trace:
+        return res
+    return res, _trace(tr, ("i", "j", "r0", "horiz", "overlap", "branch", "clamped", "short", "disp_s", "disp_e", "ratio",
+                            "ratio_ok", "disp_ok", "horiz_ok", "overlap_ok", "ok"))
 
 
 def extract_stereo(cam, left, right, prm, orb_fn=None, lines_fn=None, match_fn=None, pool=None):
@@ -251,7 +299,8 @@ def lsd_kwargs(prm):
 def projection(cam, P):
     """PinholeStereoCamera::projection (A.4)."""
     P = np.asarray(P, np.float64).reshape(-1, 3)
-    return np.stack([cam["cx"] + cam["fx"] * P[:, 0] / P[:, 2], cam["cy"] + cam["fy"] * P[:, 1] / P[:, 2]], 1)
+    with np.errstate(divide="ignore", invalid="ignore"):   # points at infinity project to NaN (DESIGN.md §8)
+        return np.stack([cam["cx"] + cam["fx"] * P[:, 0] / P[:, 2], cam["cy"] + cam["fy"] * P[:, 1] / P[:, 2]], 1)
 
 
 def track_matches(cam, prev: Frame, curr: Frame, prm, match_fn=None):

@@ -23,9 +23,7 @@ import numpy as np
 
 from oracle import matching as om
 from oracle import matchgrid as mg
-from oracle.frontend import GRID_COLS, GRID_ROWS
-
-CELL_LIM = float(1 << 28)
+from oracle.frontend import CELL_LIM, GRID_COLS, GRID_ROWS, _cell
 
 
 def rigid(T, X):
@@ -41,10 +39,7 @@ def project(cam, P):
         return np.stack([cam["cx"] + cam["fx"] * P[:, 0] / P[:, 2], cam["cy"] + cam["fy"] * P[:, 1] / P[:, 2]], 1)
 
 
-def qcell(v):
-    v = np.asarray(v, np.float64)
-    out = np.trunc(np.clip(v, -CELL_LIM, CELL_LIM))
-    return np.where(np.isnan(v), 0, out).astype(np.int64)
+qcell = _cell   # query cells: NaN -> 0, clamped to +-CELL_LIM (oracle/frontend.py _cell)
 
 
 def tcell(v):

@@ -25,13 +25,6 @@
 #define KF_MAX_LANDMARKS 65535   // 16-bit train index of the kNN keys (the reverse problem's train set is the queries)
 #define KF_MAX_FEATURES 8192     // the bound of plf_match_grid_*
 #define KF_MAX_PROBLEMS 65535    // problems per batch call: grid.y of the (chunk, problem) grids
-#define KF_CELL_LIM 268435456.0  // query cells are clamped to +-2^28 (the reference's double -> int is undefined beyond
-                                 // int range; the clamp keeps Bresenham differences inside int), NaN -> 0
-
-__device__ __forceinline__ int kf_cell(double v) {
-  if (v != v) return 0;
-  return mg_cell(fmin(fmax(v, -KF_CELL_LIM), KF_CELL_LIM));
-}
 
 struct KfCam { double fx, fy, cx, cy, w, h, iw, ih; };
 
@@ -154,11 +147,11 @@ __global__ void __launch_bounds__(256) k_kf_query_gather(KfKind k) {
   if (k.lines) {
     const double2 ps = k.proj[2 * i], pe = k.proj[2 * i + 1];
     int* d = k.q_geo + r * 4;
-    d[0] = kf_cell(ps.x * sx); d[1] = kf_cell(ps.y * sy); d[2] = kf_cell(pe.x * sx); d[3] = kf_cell(pe.y * sy);
+    d[0] = plf_qcell(ps.x * sx); d[1] = plf_qcell(ps.y * sy); d[2] = plf_qcell(pe.x * sx); d[3] = plf_qcell(pe.y * sy);
   } else {
     const double2 pp = k.proj[i];
-    k.q_geo[2 * r] = kf_cell(pp.x * sx);
-    k.q_geo[2 * r + 1] = kf_cell(pp.y * sy);
+    k.q_geo[2 * r] = plf_qcell(pp.x * sx);
+    k.q_geo[2 * r + 1] = plf_qcell(pp.y * sy);
   }
   const uint4* s = reinterpret_cast<const uint4*>(k.qdesc_in) + 2 * i;
   uint4* d = reinterpret_cast<uint4*>(k.dq) + 2 * r;

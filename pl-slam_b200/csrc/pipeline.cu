@@ -539,8 +539,8 @@ __global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, const int* _
   if (i < min(fs.pt_count[ps], K)) {
     const double* P = fs.pt_P + 3 * ((size_t)ps * K + i);
     const double2 u = plf_project(c.fx, c.fy, c.cx, c.cy, P[0], P[1], P[2]);
-    qp[((size_t)k * K + i) * 2] = mg_cell(u.x * iw);
-    qp[((size_t)k * K + i) * 2 + 1] = mg_cell(u.y * ih);
+    qp[((size_t)k * K + i) * 2] = plf_qcell(u.x * iw);
+    qp[((size_t)k * K + i) * 2 + 1] = plf_qcell(u.y * ih);
   }
   if (i < min(fs.pt_count[cs], K)) {
     const double2 p = fs.pt_pl[(size_t)cs * K + i];
@@ -551,8 +551,8 @@ __global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, const int* _
     const double* S = fs.ls_sP + 3 * ((size_t)ps * Ln + i);
     const double* E = fs.ls_eP + 3 * ((size_t)ps * Ln + i);
     int* d = ql + ((size_t)k * Ln + i) * 4;
-    d[0] = mg_cell(plf_project_u(c.fx, c.cx, S[0], S[2]) * iw); d[1] = mg_cell(plf_project_v(c.fy, c.cy, S[1], S[2]) * ih);
-    d[2] = mg_cell(plf_project_u(c.fx, c.cx, E[0], E[2]) * iw); d[3] = mg_cell(plf_project_v(c.fy, c.cy, E[1], E[2]) * ih);
+    d[0] = plf_qcell(plf_project_u(c.fx, c.cx, S[0], S[2]) * iw); d[1] = plf_qcell(plf_project_v(c.fy, c.cy, S[1], S[2]) * ih);
+    d[2] = plf_qcell(plf_project_u(c.fx, c.cx, E[0], E[2]) * iw); d[3] = plf_qcell(plf_project_v(c.fy, c.cy, E[1], E[2]) * ih);
   }
   if (i < min(fs.ls_count[cs], Ln))
     plf_train_line(fs.ls_spl[(size_t)cs * Ln + i], fs.ls_epl[(size_t)cs * Ln + i], iw, ih, tl + ((size_t)k * Ln + i) * 4,

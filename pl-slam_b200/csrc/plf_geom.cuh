@@ -7,6 +7,15 @@
 
 __device__ __forceinline__ int mg_cell(double v) { return (int)v; }   // double -> int as in C++ (truncation)
 
+// The cell of a projected query coordinate.  The reference converts with a plain double -> int, undefined for NaN and
+// beyond int range; the library defines both: NaN (a point at infinity projects to inf / inf) -> 0, and values clamped
+// to +-2^28, which keeps Bresenham differences inside int (oracle/frontend.py _cell).
+#define PLF_CELL_LIM 268435456.0
+__device__ __forceinline__ int plf_qcell(double v) {
+  if (v != v) return 0;
+  return mg_cell(fmin(fmax(v, -PLF_CELL_LIM), PLF_CELL_LIM));
+}
+
 // PinholeStereoCamera::projection: (cx + fx X / Z, cy + fy Y / Z), per coordinate and for both
 __device__ __forceinline__ double plf_project_u(double fx, double cx, double X, double Z) { return cx + fx * X / Z; }
 __device__ __forceinline__ double plf_project_v(double fy, double cy, double Y, double Z) { return cy + fy * Y / Z; }

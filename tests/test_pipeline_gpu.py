@@ -26,10 +26,13 @@ def check_frame(fg, fo: ofe.Frame):
         assert np.array_equal(fg[k], v), k
 
 
-def run_both(cam, frames, B, **prm_over):
+def run_both(cam, frames, B, limits=None, **prm_over):
+    """limits: plf_limits fields to set besides max_batch."""
     prm = dict(ofe.DEFAULTS, **prm_over)
     ref = ofe.run_sequence(cam, [(a, b) for a, b, _ in frames], prm)
     lim = plf.default_limits(); lim.max_batch = B
+    for k, v in (limits or {}).items():
+        setattr(lim, k, v)
     kw = {k: prm[k] for k, _ in plf.plf_params._fields_}   # the oracle's parameters, every one of them, on the device too
     got, feats = [], []
     with plf.Frontend(camera=cam, limits=lim, **kw) as fe:
