@@ -272,6 +272,13 @@ plf_status plf_debug_sincosf(plf_ctx* ctx, const float* in, float* s, float* c, 
  * kernel set it, 0 elsewhere.  A bad path, an n6 out of range or a NULL S, g or x returns PLF_ERR_INVALID. */
 plf_status plf_debug_ldlt(plf_ctx* ctx, int path, int n6, double* S, const double* g, double* x, uint8_t* nz);
 
+/* Test hook: plf_debug_ldlt's path 0 on n matrices of mixed sizes in one launch chain, the batched tiled LDL^T of
+ * plf_global_ba_batch: matrix i is n6[i] (1 <= n6[i] <= 4096) with S[i], g[i], x[i] and nz[i] (nz or nz[i] may be NULL)
+ * as plf_debug_ldlt takes them, and comes out as plf_debug_ldlt(ctx, 0, ...) leaves it.  n < 0, n > 65535, an n6 out of
+ * range or a NULL S, g or x returns PLF_ERR_INVALID; n = 0 returns PLF_OK. */
+plf_status plf_debug_ldlt_batch(plf_ctx* ctx, int n, const int* n6, double* const* S, const double* const* g,
+                                double* const* x, uint8_t* const* nz);
+
 /* LBD prelude: GaussianBlur 5x5 sigma 1 then Sobel k=3 to CV_16S.  Replaces
  * BinaryDescriptor::computeSobel (binary_descriptor_custom.cpp:373-398 -> :350-370).
  * img: h rows of `stride` bytes (host). dxdy: h*w interleaved int16 pairs (dx,dy) (host). */
@@ -444,8 +451,38 @@ plf_status plf_local_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts, int n_prob
  * plf_destroy: about 288 n_kf^2 bytes for the dense reduced system (1.2 GB at 2048 keyframes, 4.8 GB at 4096) plus
  * 144 bytes per observation and about 650 bytes per landmark.  Up to n_kf = 64 the reduced system is factored by one CTA as in
  * plf_local_ba; beyond, by a tiled LDL^T across the GPU that skips exactly-zero tiles.  Projects with the context's camera,
- * as plf_local_ba. */
+ * as plf_local_ba; plf_global_ba_batch takes a sequence's. */
 plf_status plf_global_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* problem, plf_lba_result* out);
+
+/* Many global bundle adjustments in one call: the maps of several sequences that end together, each with its sequence's
+ * camera, solved in one launch chain with one host synchronisation (after the download).  The contract is
+ * plf_local_ba_batch's, with plf_global_ba's rules per problem:
+ *   problems [n_problems]  plf_global_ba's layout and rules, each in / out as in plf_global_ba
+ *   seq      [n_problems]  or NULL: the camera of problem p, as in plf_local_ba_batch (-1: the context's camera;
+ *                          0 <= seq[p] < n: plf_get_sequence_camera(ctx, seq[p]) at the time of the call; fx, fy, cx, cy)
+ *   out      [n_problems]  or NULL;  status [n_problems], required.
+ * Problem p gets what plf_global_ba gives it on a context created with p's camera: the same iteration count, the same
+ * moved flags, lambda and err to rounding, every block to rounding of the step (both sum with float atomics).  One opts
+ * applies to every problem; ref_quirks selects plf_global_ba's quirk set (g1-g6).
+ * Refusals before any work, with nothing written (no problem's arrays, out or status) and a message naming the problem
+ * and the rule: PLF_ERR_INVALID when n_problems < 0, a seq entry is out of range, or a problem breaks one of
+ * plf_global_ba's host-side rules (empty problem, NULL arrays, ungrouped observations, out-of-range indices, a landmark
+ * without observations); PLF_ERR_CAPACITY beyond 4096 keyframes in a problem or 65535 problems.  n_problems = 0 returns
+ * PLF_OK.  Refusal on the device: as plf_local_ba_batch, a landmark whose first-pass block has an exactly zero diagonal
+ * entry refuses its own problem only (status[p] = PLF_ERR_INVALID, its arrays and out[p] unchanged), the others are
+ * solved and written back, and the call returns PLF_ERR_INVALID naming the first refused problem and its landmark.
+ * Problems up to 64 keyframes are factored by one CTA each, as in plf_local_ba_batch; larger ones by the tiled LDL^T of
+ * plf_global_ba, one launch per stage and tile column over all of them, at the largest problem's tile count n_t =
+ * ceil(6 n_kf / 64).  All opts.max_iters rounds are enqueued at once: 2 launches per call, 8 per round (9 in round 0,
+ * 10 under ref_quirks) and, when a problem has more than 64 keyframes, 5 n_t + 1 more per round, whatever the number of
+ * problems and the iterations they run.
+ * Work is enqueued on plf_stream and uses plf_local_ba_batch's scratch slot, which stays allocated until plf_destroy:
+ * its parts as listed there (288 bytes per keyframe^2 of each problem is the dense reduced system, 1.2 GB at 2048
+ * keyframes), plus 32768 n_t + n_t^2 bytes of tile work and 48 bytes of table per problem over 64 keyframes.  When the
+ * summed systems do not fit on the device the call fails with PLF_ERR_CUDA, as plf_global_ba does when its scratch cannot
+ * be allocated, and the context stays usable.  The rules for batches in flight are plf_global_ba's. */
+plf_status plf_global_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems, const plf_lba_problem* problems,
+                               const int32_t* seq, plf_lba_result* out, plf_status* status);
 
 /* Loop-closure pose-graph optimisation.  Replaces the g2o call of MapHandler::loopClosureOptimizationCovGraphG2O
  * (src/mapHandler.cpp:4185-4410): computeInitialGuess() then optimize(max_iters) of g2o's Levenberg-Marquardt over
@@ -668,9 +705,9 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
  *     it is a first frame (status 2), since its carried frame was triangulated with another camera.
  *   - plf_set_max_sequences drops every sequence's camera; plf_reset_sequence keeps them.
  *   - plf_batch_run and plf_process_batch run sequence 0, so they use sequence 0's camera.
- * Only plf_global_ba keeps the context's camera without a batch form.  The other keyframe and back-end operators use the
- * context's camera in their single form and take a sequence's per problem in their batch form: plf_match_kf2kf_batch,
- * plf_match_map2kf_batch, plf_local_ba_batch, plf_gn_pose_batch and plf_loop_closure_pose_batch.  Place recognition's
+ * The keyframe and back-end operators use the context's camera in their single form and take a sequence's per problem in
+ * their batch form: plf_match_kf2kf_batch, plf_match_map2kf_batch, plf_local_ba_batch, plf_global_ba_batch,
+ * plf_gn_pose_batch and plf_loop_closure_pose_batch.  Place recognition's
  * batch form, plf_bow_insert_batch, takes a sequence's bag-of-words database instead: its vectors do not depend on the
  * camera, so plf_set_sequence_camera leaves that database as it is. */
 plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam);

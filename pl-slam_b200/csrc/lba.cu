@@ -393,8 +393,8 @@ __global__ void k_lba_moved(LbaDev d, uint8_t* pt_moved, uint8_t* ls_moved) {
 // `Hmax = fabs(d)` truncates, and a value >= 2^31 converts to INT_MIN (x86-64 cvttsd2si), which the next diagonal entry
 // (>= 0) always replaces, unless it is NaN (both comparisons false).  So the result is INT_MIN when an entry is >= 2^31
 // and no non-NaN entry follows the last such one, else the truncated maximum of the non-NaN entries after the last one
-// >= 2^31 (or of all of them).  One CTA; leaves the value in scal[3].
-__global__ void __launch_bounds__(1024) k_gba_hmax_int(LbaDev d) {
+// >= 2^31 (or of all of them).  One CTA of 1024 threads; leaves the value in scal[3].
+__device__ __forceinline__ void gba_hmax_int(const LbaDev& d) {
   __shared__ int last_big, any_after;
   __shared__ unsigned long long mx;
   const int tid = threadIdx.x, nk = 6 * d.nkf, np3 = 3 * d.npt;
@@ -421,6 +421,7 @@ __global__ void __launch_bounds__(1024) k_gba_hmax_int(LbaDev d) {
   if (tid == 0)
     d.scal[3] = last_big >= 0 && !any_after ? -2147483648.0 : trunc(__longlong_as_double((long long)mx));
 }
+__global__ void __launch_bounds__(1024) k_gba_hmax_int(LbaDev d) { gba_hmax_int(d); }
 
 // ---- blocked LDL^T of the reduced system for n = 6 n_kf > 384 (plf_global_ba) -----------------------------------------
 // Right-looking over 64 x 64 tiles of S (row-major, leading dimension n; only the lower triangle is read), the same
@@ -444,8 +445,10 @@ __device__ __forceinline__ void gba_load_lkk(const LbaDev& d, int k, double* L) 
   }
 }
 
-__global__ void __launch_bounds__(256) k_gba_damp(LbaDev d, double lambda) {   // k_lba_solve's prologue
-  const int i = blockIdx.x * 256 + threadIdx.x, n = 6 * d.nkf;
+// Each stage's work for one CTA (or element) of one problem is a __device__ function of the problem's LbaDev, so that
+// plf_global_ba_batch's kernels (k_gbb_*) run the same arithmetic on every large problem of a batch.
+__device__ __forceinline__ void gba_damp(const LbaDev& d, double lambda, int i) {   // k_lba_solve's prologue
+  const int n = 6 * d.nkf;
   if (i < 36 * d.nkf) {
     const int kf = i / 36, r = (i % 36) / 6, cc = i % 6;
     double v = d.A[i];
@@ -455,8 +458,9 @@ __global__ void __launch_bounds__(256) k_gba_damp(LbaDev d, double lambda) {   /
     d.gred[i - 36 * d.nkf] += d.gc[i - 36 * d.nkf];
   }
 }
+__global__ void __launch_bounds__(256) k_gba_damp(LbaDev d, double lambda) { gba_damp(d, lambda, blockIdx.x * 256 + threadIdx.x); }
 
-__global__ void __launch_bounds__(256) k_gba_diag(LbaDev d, int k) {
+__device__ __forceinline__ void gba_diag(const LbaDev& d, int k) {
   __shared__ double T[GBA_T * GBA_LD];
   const int n = 6 * d.nkf, r0 = GBA_T * k, tid = threadIdx.x;
   for (int e = tid; e < GBA_T * GBA_T; e += 256) {
@@ -480,13 +484,13 @@ __global__ void __launch_bounds__(256) k_gba_diag(LbaDev d, int k) {
     if (c <= r && r0 + r < n) d.S[(size_t)(r0 + r) * n + r0 + c] = T[r * GBA_LD + c];
   }
 }
+__global__ void __launch_bounds__(256) k_gba_diag(LbaDev d, int k) { gba_diag(d, k); }
 
-// one CTA per tile row i > k; dynamic shared memory 2 x 64 x GBA_LD doubles
-__global__ void __launch_bounds__(256) k_gba_panel(LbaDev d, double* Wp, uint8_t* nz, int k, int nt) {
-  extern __shared__ double gsm[];
+// one CTA per tile row i > k; gsm: dynamic shared memory of 2 x 64 x GBA_LD doubles
+__device__ __forceinline__ void gba_panel(const LbaDev& d, double* Wp, uint8_t* nz, int k, int nt, int i, double* gsm) {
   double* L = gsm;
   double* Z = gsm + GBA_T * GBA_LD;
-  const int n = 6 * d.nkf, i = k + 1 + blockIdx.x, r0 = GBA_T * i, c0 = GBA_T * k, tid = threadIdx.x;
+  const int n = 6 * d.nkf, r0 = GBA_T * i, c0 = GBA_T * k, tid = threadIdx.x;
   int any = 0;
   for (int e = tid; e < GBA_T * GBA_T; e += 256) {
     const int r = e >> 6, c = e & 63;
@@ -515,17 +519,19 @@ __global__ void __launch_bounds__(256) k_gba_panel(LbaDev d, double* Wp, uint8_t
     if (r0 + r < n && c0 + c < n) d.S[(size_t)(r0 + r) * n + c0 + c] = z / L[c * GBA_LD + c];
   }
 }
+__global__ void __launch_bounds__(256) k_gba_panel(LbaDev d, double* Wp, uint8_t* nz, int k, int nt) {
+  extern __shared__ double gsm[];
+  gba_panel(d, Wp, nz, k, nt, k + 1 + blockIdx.x, gsm);
+}
 
 __device__ __forceinline__ void gba_dmma(double& c0, double& c1, double& c2, double& c3, double a0, double a1, double b0) {
   asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
                : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3) : "d"(a0), "d"(a1), "d"(b0));
 }
 
-// S_ij -= W_ik L_jk^T for the trailing lower tiles k < j <= i, one CTA per tile (blockIdx.x enumerates (i, j) row by
-// row).  8 warps; warp w owns rows 16 (w / 2) .. +16 and columns 32 (w % 2) .. +32 of the tile (4 m16n8 accumulators).
+// S_ij -= W_ik L_jk^T for the trailing lower tiles k < j <= i, one CTA per tile (t enumerates (i, j) row by row).  8 warps; warp w owns rows 16 (w / 2) .. +16 and columns 32 (w % 2) .. +32 of the tile (4 m16n8 accumulators).
 constexpr int GBA_KC = 32, GBA_SLD = 36;   // k chunk; shared row stride (conflict-free fragment loads per half warp)
-__global__ void __launch_bounds__(256) k_gba_update(LbaDev d, const double* Wp, const uint8_t* nz, int k, int nt) {
-  const int t = blockIdx.x;
+__device__ __forceinline__ void gba_update(const LbaDev& d, const double* Wp, const uint8_t* nz, int k, int nt, int t) {
   int a = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
   while ((a + 1) * (a + 2) / 2 <= t) ++a;
   while (a * (a + 1) / 2 > t) --a;
@@ -561,12 +567,15 @@ __global__ void __launch_bounds__(256) k_gba_update(LbaDev d, const double* Wp, 
       if (r < n && c < n) d.S[(size_t)r * n + c] -= acc[q][e];
     }
 }
+__global__ void __launch_bounds__(256) k_gba_update(LbaDev d, const double* Wp, const uint8_t* nz, int k, int nt) {
+  gba_update(d, Wp, nz, k, nt, blockIdx.x);
+}
 
 // forward substitution step k: every CTA solves y_k = L_kk^-1 g_k (64 threads, in place of g's tile), CTA 0 stores it in
 // dxc, CTA b > 0 subtracts L_ik y_k from g_i (i = k + b) when that tile is non-zero
-__global__ void __launch_bounds__(256) k_gba_fwd(LbaDev d, const uint8_t* nz, int k, int nt) {
+__device__ __forceinline__ void gba_fwd(const LbaDev& d, const uint8_t* nz, int k, int nt, int b) {
   __shared__ double L[GBA_T * GBA_LD], y[GBA_T];
-  const int n = 6 * d.nkf, b = blockIdx.x, i = k + b, r0 = GBA_T * k, tid = threadIdx.x;
+  const int n = 6 * d.nkf, i = k + b, r0 = GBA_T * k, tid = threadIdx.x;
   if (b > 0 && !nz[(size_t)i * nt + k]) return;
   gba_load_lkk(d, k, L);
   if (tid < GBA_T) y[tid] = r0 + tid < n ? d.gred[r0 + tid] : 0.0;
@@ -587,17 +596,19 @@ __global__ void __launch_bounds__(256) k_gba_fwd(LbaDev d, const uint8_t* nz, in
     if (lane == 0 && r < n) d.gred[r] -= s;
   }
 }
+__global__ void __launch_bounds__(256) k_gba_fwd(LbaDev d, const uint8_t* nz, int k, int nt) { gba_fwd(d, nz, k, nt, blockIdx.x); }
 
-__global__ void k_gba_dscale(LbaDev d) {   // z = y / D
-  const int i = blockIdx.x * blockDim.x + threadIdx.x, n = 6 * d.nkf;
+__device__ __forceinline__ void gba_dscale(const LbaDev& d, int i) {   // z = y / D
+  const int n = 6 * d.nkf;
   if (i < n) d.gred[i] = d.dxc[i] / d.S[(size_t)i * n + i];
 }
+__global__ void k_gba_dscale(LbaDev d) { gba_dscale(d, blockIdx.x * blockDim.x + threadIdx.x); }
 
 // backward substitution step k (k = n_t - 1 .. 0): every CTA solves x_k = L_kk^-T z_k, CTA 0 stores it in dxc and DX,
 // CTA b > 0 subtracts L_kj^T x_k from z_j (j = b - 1) when that tile is non-zero
-__global__ void __launch_bounds__(256) k_gba_bwd(LbaDev d, const uint8_t* nz, int k, int nt) {
+__device__ __forceinline__ void gba_bwd(const LbaDev& d, const uint8_t* nz, int k, int nt, int b) {
   __shared__ double L[GBA_T * GBA_LD], x[GBA_T], part[4][GBA_T];
-  const int n = 6 * d.nkf, b = blockIdx.x, r0 = GBA_T * k, tid = threadIdx.x;
+  const int n = 6 * d.nkf, r0 = GBA_T * k, tid = threadIdx.x;
   if (b > 0 && !nz[(size_t)k * nt + (b - 1)]) return;
   gba_load_lkk(d, k, L);
   if (tid < GBA_T) x[tid] = r0 + tid < n ? d.gred[r0 + tid] : 0.0;
@@ -617,6 +628,7 @@ __global__ void __launch_bounds__(256) k_gba_bwd(LbaDev d, const uint8_t* nz, in
   __syncthreads();
   if (tid < GBA_T && GBA_T * j + tid < n) d.gred[GBA_T * j + tid] -= ((part[0][tid] + part[1][tid]) + part[2][tid]) + part[3][tid];
 }
+__global__ void __launch_bounds__(256) k_gba_bwd(LbaDev d, const uint8_t* nz, int k, int nt) { gba_bwd(d, nz, k, nt, blockIdx.x); }
 
 // The tiled factorisation and the two substitutions (see k_gba_diag), shared by plf_global_ba and plf_pose_graph.  The
 // kernels read only the fields of LbaDev set here.
@@ -971,21 +983,23 @@ __global__ void __launch_bounds__(128) k_lbb_kf_diagmax(LbbDev b) {
   for (int i = threadIdx.x; i < 6 * q.nkf; i += 128) lba_kf_diagmax(d, i);
 }
 
-__global__ void __launch_bounds__(128) k_lbb_schur(LbbDev b) {
+// swap: (g6), round 0 of plf_global_ba_batch under its quirks
+__global__ void __launch_bounds__(128) k_lbb_schur(LbbDev b, int swap) {
   const int p = blockIdx.x;
   if (!b.ctrl[p].active) return;
   const LbbProb q = b.prob[p];
   const LbaDev d = lbb_view(b, q, p);
   const double lambda = b.ctrl[p].lambda;
-  for (int c = blockIdx.y; 128 * c < q.nlm; c += gridDim.y) lba_lm_schur(d, 128 * c + threadIdx.x, lambda, 0);
+  for (int c = blockIdx.y; 128 * c < q.nlm; c += gridDim.y) lba_lm_schur(d, 128 * c + threadIdx.x, lambda, swap);
 }
 
-// One CTA per problem, as k_lba_solve; then zeroes A, g_c, S and g_red for the next round's accumulation.
+// One CTA per problem with n = 6 n_kf <= 384, as k_lba_solve; then zeroes A, g_c, S and g_red for the next round's
+// accumulation.  Larger problems (plf_global_ba_batch) are solved by the k_gbb_* kernels.
 __global__ void __launch_bounds__(256) k_lbb_solve(LbbDev b) {
   const int p = blockIdx.x;
   if (!b.ctrl[p].active) return;
   const LbbProb q = b.prob[p];
-  if (!q.nkf) return;
+  if (!q.nkf || q.nkf > 64) return;
   const LbaDev d = lbb_view(b, q, p);
   lba_solve(d, b.ctrl[p].lambda);
   __syncthreads();
@@ -996,12 +1010,12 @@ __global__ void __launch_bounds__(256) k_lbb_solve(LbbDev b) {
   for (int i = threadIdx.x; i < n; i += 256) d.gc[i] = 0.0;
 }
 
-__global__ void __launch_bounds__(128) k_lbb_backsub(LbbDev b) {
+__global__ void __launch_bounds__(128) k_lbb_backsub(LbbDev b, int swap) {
   const int p = blockIdx.x;
   if (!b.ctrl[p].active) return;
   const LbbProb q = b.prob[p];
   const LbaDev d = lbb_view(b, q, p);
-  for (int c = blockIdx.y; 128 * c < q.nlm; c += gridDim.y) lba_backsub(d, 128 * c + threadIdx.x, 0);
+  for (int c = blockIdx.y; 128 * c < q.nlm; c += gridDim.y) lba_backsub(d, 128 * c + threadIdx.x, swap);
 }
 
 __global__ void __launch_bounds__(128) k_lbb_apply(LbbDev b) {
@@ -1013,9 +1027,12 @@ __global__ void __launch_bounds__(128) k_lbb_apply(LbbDev b) {
   for (int c = blockIdx.y; 128 * c < ne; c += gridDim.y) lba_apply(d, 128 * c + threadIdx.x, apply);
 }
 
-// After the first pass: the refusal, the error normalisation (q1: the reference divides by two counters it never
-// increments, 0.0 here as there) and lambda *= Hmax.  The first step is applied unconditionally (apply = 1 from k_lbb_prep).
-__global__ void k_lbb_first(LbbDev b, int quirks) {
+// The control of both routines: G selects plf_global_ba's (ba_run's `global` branch) over plf_local_ba's.
+// After the first pass: the refusal, the error normalisation (q1 / g1: the reference divides by two counters it never
+// increments, 0.0 here as there) and lambda *= Hmax (g2: the int-truncated maximum of k_gbb_hmax_int).  The first step
+// is applied unconditionally (apply = 1 from k_lbb_prep).
+template <bool G>
+__device__ __forceinline__ void lbb_first(const LbbDev& b, int quirks) {
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= b.P) return;
   LbbCtrl& c = b.ctrl[p];
@@ -1026,24 +1043,37 @@ __global__ void k_lbb_first(LbbDev b, int quirks) {
   double err = scal[0];
   if (quirks & BAQ_FIRST_ERR0) err = __ddiv_rn(err, 0.0);   // (q1) :1541
   else err /= (double)q.nobs;
-  c.lambda *= scal[2];   // Hmax, whose bit pattern k_lba_lm_accum / k_lba_kf_diagmax maximised
+  // Hmax: under (g2) scal[3], else the double whose bit pattern k_lba_lm_accum / k_lba_kf_diagmax maximised
+  c.lambda *= G && (quirks & BAQ_HMAX_INT) ? scal[3] : scal[2];
   c.err = err;
   c.err_prev = err;
   scal[0] = 0.0;
 }
+__global__ void k_lbb_first(LbbDev b, int quirks) { lbb_first<false>(b, quirks); }
+__global__ void k_gbb_first(LbbDev b, int quirks) { lbb_first<true>(b, quirks); }
 
-// Round r >= 1 after its accumulation: the error, the change and min-error stops (:1773-1775) and whether it grew.
-__global__ void k_lbb_test(LbbDev b, int r, double min_error, double min_error_change) {
+// Round r >= 1 after its accumulation: the error, the change and min-error stops (:1773-1775, :2637) and whether it
+// grew.  LBA divides the error by the landmark count (:1773), GBA by the observation count, or under (g3) by the zero
+// counters (:2635), so that only max_iters or the |DX| test ends its run.
+template <bool G>
+__device__ __forceinline__ void lbb_test(const LbbDev& b, int r, int quirks, double min_error, double min_error_change) {
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= b.P || !b.ctrl[p].active) return;
   LbbCtrl& c = b.ctrl[p];
   const LbbProb& q = b.prob[p];
   double* scal = b.scal + 8 * p;
-  const double err = scal[0] / (double)(q.npt + q.nls);
+  const double err = !G ? scal[0] / (double)(q.npt + q.nls)
+                        : (quirks & BAQ_ITER_ERR0) ? __ddiv_rn(scal[0], 0.0) : scal[0] / (double)q.nobs;
   scal[0] = 0.0;
   c.err = err;
   if (fabs(err - c.err_prev) < min_error_change || err < min_error) { c.active = 0; c.iters = r; return; }
   c.apply = !(err > c.err_prev);
+}
+__global__ void k_lbb_test(LbbDev b, int r, double min_error, double min_error_change) {
+  lbb_test<false>(b, r, 0, min_error, min_error_change);
+}
+__global__ void k_gbb_test(LbbDev b, int r, int quirks, double min_error, double min_error_change) {
+  lbb_test<true>(b, r, quirks, min_error, min_error_change);
 }
 
 // Round r after its step: the lambda schedule (:1785-1803) and the |DX| stop (:1805); round 0 only clears |DX|^2.
@@ -1069,17 +1099,136 @@ __global__ void __launch_bounds__(128) k_lbb_moved(LbbDev b) {
   for (int c = blockIdx.y; 128 * c < q.nlm; c += gridDim.y) lba_moved(d, 128 * c + threadIdx.x, m, m + q.npt);
 }
 
-extern "C" plf_status plf_local_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems, const plf_lba_problem* problems,
-                                         const int32_t* seq, plf_lba_result* out, plf_status* status) {
-  const char* fn = "plf_local_ba_batch";
+// ---- plf_global_ba_batch: the large problems' tiled LDL^T ---------------------------------------------------------------
+// A problem with n = 6 n_kf > 384 is factored by the tiled LDL^T above, with its own Wp and zero flags.  Per tile column
+// there is one launch of each stage over every large problem, gridded (tile, problem) at the largest problem's extent:
+// blockIdx.y picks the problem from the GbbBig table, and a CTA whose problem has fewer tiles, has stopped or was refused
+// returns at once.  Each CTA runs the single-problem function of the stage, so a problem's factorisation is plf_ldlt_tiled's
+// bit for bit.
+struct GbbBig {
+  int p, nkf;                     // the problem's index in the batch and its keyframe count
+  long long so, go, xo, wo, zo;   // offsets into S, g / y, x (doubles), Wp (doubles) and the zero flags (bytes)
+};
+struct GbbLdlt {
+  const GbbBig* big;
+  const LbbCtrl* ctrl;   // the problems' control state, NULL when every problem is active (plf_debug_ldlt_batch)
+  double* S; double* g; double* y; double* x; double* Wp; uint8_t* nz;
+};
+// The LbaDev fields the tiled kernels read, for problem blockIdx.y, and its tile count; false when it is not active.
+__device__ __forceinline__ bool gbb_view(const GbbLdlt& L, LbaDev& d, GbbBig& t, int& nt) {
+  t = L.big[blockIdx.y];
+  if (L.ctrl && !L.ctrl[t.p].active) return false;
+  d.nkf = t.nkf; d.S = L.S + t.so; d.gred = L.g + t.go; d.dxc = L.y + t.go; d.DX = L.x + t.xo;
+  nt = (6 * t.nkf + GBA_T - 1) / GBA_T;
+  return true;
+}
+
+__global__ void __launch_bounds__(256) k_gbb_diag(GbbLdlt L, int k) {
+  LbaDev d{}; GbbBig t; int nt;
+  if (!gbb_view(L, d, t, nt) || k >= nt) return;
+  gba_diag(d, k);
+}
+__global__ void __launch_bounds__(256) k_gbb_panel(GbbLdlt L, int k) {
+  extern __shared__ double gsm[];
+  LbaDev d{}; GbbBig t; int nt;
+  if (!gbb_view(L, d, t, nt) || k + 1 + (int)blockIdx.x >= nt) return;
+  gba_panel(d, L.Wp + t.wo, L.nz + t.zo, k, nt, k + 1 + blockIdx.x, gsm);
+}
+__global__ void __launch_bounds__(256) k_gbb_update(GbbLdlt L, int k) {
+  LbaDev d{}; GbbBig t; int nt;
+  if (!gbb_view(L, d, t, nt)) return;
+  const int m = nt - k - 1;
+  if (m <= 0 || (int)blockIdx.x >= m * (m + 1) / 2) return;
+  gba_update(d, L.Wp + t.wo, L.nz + t.zo, k, nt, blockIdx.x);
+}
+__global__ void __launch_bounds__(256) k_gbb_fwd(GbbLdlt L, int k) {
+  LbaDev d{}; GbbBig t; int nt;
+  if (!gbb_view(L, d, t, nt) || k + (int)blockIdx.x >= nt) return;
+  gba_fwd(d, L.nz + t.zo, k, nt, blockIdx.x);
+}
+__global__ void __launch_bounds__(256) k_gbb_dscale(GbbLdlt L) {
+  LbaDev d{}; GbbBig t; int nt;
+  if (!gbb_view(L, d, t, nt)) return;
+  gba_dscale(d, blockIdx.x * 256 + threadIdx.x);
+}
+__global__ void __launch_bounds__(256) k_gbb_bwd(GbbLdlt L, int k) {
+  LbaDev d{}; GbbBig t; int nt;
+  if (!gbb_view(L, d, t, nt) || k >= nt) return;
+  gba_bwd(d, L.nz + t.zo, k, nt, blockIdx.x);
+}
+
+// The tiled factorisation and the two substitutions of the nb problems in L.big, the largest with n_max rows: the
+// launches of plf_ldlt_tiled at n_max, each over every problem.
+static plf_status gbb_ldlt(plf_ctx* ctx, cudaStream_t cs, const GbbLdlt& L, int nb, int n_max) {
+  const int nt = (n_max + GBA_T - 1) / GBA_T, smem = 2 * GBA_T * GBA_LD * 8;
+  PLF_CUDA(ctx, cudaFuncSetAttribute(k_gbb_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  for (int k = 0; k < nt; ++k) {
+    k_gbb_diag<<<dim3(1, nb), 256, 0, cs>>>(L, k);
+    PLF_LAUNCH_CHECK(ctx);
+    const int m = nt - k - 1;
+    if (!m) break;
+    k_gbb_panel<<<dim3(m, nb), 256, smem, cs>>>(L, k);
+    PLF_LAUNCH_CHECK(ctx);
+    k_gbb_update<<<dim3(m * (m + 1) / 2, nb), 256, 0, cs>>>(L, k);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  for (int k = 0; k < nt; ++k) {
+    k_gbb_fwd<<<dim3(nt - k, nb), 256, 0, cs>>>(L, k);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  k_gbb_dscale<<<dim3((n_max + 255) / 256, nb), 256, 0, cs>>>(L);
+  PLF_LAUNCH_CHECK(ctx);
+  for (int k = nt - 1; k >= 0; --k) {
+    k_gbb_bwd<<<dim3(k + 1, nb), 256, 0, cs>>>(L, k);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  return PLF_OK;
+}
+
+// S += A' and g_red += g_c of every active large problem (k_gba_damp), gridded (chunk, problem)
+__global__ void __launch_bounds__(256) k_gbb_damp(LbbDev b, const GbbBig* big) {
+  const GbbBig t = big[blockIdx.y];
+  if (!b.ctrl[t.p].active) return;
+  const LbaDev d = lbb_view(b, b.prob[t.p], t.p);
+  const double lambda = b.ctrl[t.p].lambda;
+  for (int i = blockIdx.x * 256 + threadIdx.x; i < 42 * t.nkf; i += gridDim.x * 256) gba_damp(d, lambda, i);
+}
+
+// Zeroes S, g_red, A and g_c of every active large problem for the next round's accumulation (k_lbb_solve does it for
+// the small ones), across the GPU: S is 288 n_kf^2 bytes, 4.8 GB at 4096 keyframes.
+__global__ void __launch_bounds__(256) k_gbb_zero(LbbDev b, const GbbBig* big) {
+  const GbbBig t = big[blockIdx.y];
+  if (!b.ctrl[t.p].active) return;
+  const LbaDev d = lbb_view(b, b.prob[t.p], t.p);
+  const size_t n = 6 * (size_t)t.nkf, stride = (size_t)gridDim.x * 256;
+  for (size_t i = blockIdx.x * 256 + threadIdx.x; i < n * n; i += stride) d.S[i] = 0.0;
+  for (size_t i = blockIdx.x * 256 + threadIdx.x; i < n; i += stride) { d.gred[i] = 0.0; d.gc[i] = 0.0; }
+  for (size_t i = blockIdx.x * 256 + threadIdx.x; i < 6 * n; i += stride) d.A[i] = 0.0;
+}
+
+// (g2) on the first pass, one CTA of 1024 threads per problem
+__global__ void __launch_bounds__(1024) k_gbb_hmax_int(LbbDev b) {
+  const int p = blockIdx.x;
+  gba_hmax_int(lbb_view(b, b.prob[p], p));
+}
+
+// plf_local_ba_batch and plf_global_ba_batch: ba_run's rules per problem and its control on the device (k_lbb_first /
+// k_lbb_test, or k_gbb_first / k_gbb_test with global), one upload, every round enqueued, one download.
+static plf_status lbb_run(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems, const plf_lba_problem* problems,
+                          const int32_t* seq, plf_lba_result* out, plf_status* status, bool global) {
+  const char* fn = global ? "plf_global_ba_batch" : "plf_local_ba_batch";
   if (!ctx || !opts || n_problems < 0 || (n_problems && (!problems || !status)))
     return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", fn);
   const int P = n_problems;
   if (!P) return PLF_OK;
-  // every refusal before any work: the cameras, then plf_local_ba's rules per problem
+  // the large problems are gridded in y, at most 65535 of them; the limit is on the batch so that it does not depend on
+  // the problems' sizes
+  if (global && P > 65535) return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: %d problems (limit 65535)", fn, P);
+  // every refusal before any work: the cameras, then ba_run's rules per problem
   std::vector<LbbProb> hp(P);
-  long long tN = 0, tObs = 0, tLm = 0, tKf = 0, tFix = 0, tG = 0, tS = 0;
-  int mObs = 0, mLm = 0, mEl = 0;
+  std::vector<GbbBig> hb;
+  long long tN = 0, tObs = 0, tLm = 0, tKf = 0, tFix = 0, tG = 0, tS = 0, tWp = 0, tNz = 0;
+  int mObs = 0, mLm = 0, mEl = 0, mBig = 0;
   char pfx[64];
   for (int p = 0; p < P; ++p) {
     const int s = seq ? seq[p] : -1;
@@ -1088,24 +1237,33 @@ extern "C" plf_status plf_local_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts,
     const plf_camera& c = s >= 0 && !ctx->seq_cam_own.empty() && ctx->seq_cam_own[s] ? ctx->seq_cam[s] : ctx->cam;
     const plf_lba_problem& pr = problems[p];
     snprintf(pfx, sizeof pfx, "%s: problem %d", fn, p);
-    if (plf_status st = lba_check_shape(ctx, pfx, &pr, 64)) return st;
+    if (plf_status st = lba_check_shape(ctx, pfx, &pr, global ? 4096 : 64)) return st;
     LbbProb& q = hp[p];
     q.nkf = pr.n_kf; q.npt = pr.n_pt; q.nls = pr.n_ls; q.npo = pr.n_pt_obs; q.nobs = pr.n_pt_obs + pr.n_ls_obs;
     q.nlm = pr.n_pt + pr.n_ls; q.N = 6 * pr.n_kf + 3 * pr.n_pt + 6 * pr.n_ls; q.nfix = pr.n_fixed;
     q.xo = tN; q.oo = tObs; q.lo = tLm; q.ko = tKf; q.fo = tFix; q.go = tG; q.so = tS;
     q.cam = LbaCam{c.fx, c.fy, c.cx, c.cy};
+    if (q.nkf > 64) {   // n > 384: the tiled LDL^T (k_gbb_*), as ba_run's `blocked`
+      const long long nt = (6 * q.nkf + GBA_T - 1) / GBA_T;
+      hb.push_back(GbbBig{p, q.nkf, q.so, q.go, q.xo, tWp, tNz});
+      tWp += nt * GBA_T * GBA_T; tNz += nt * nt;
+      mBig = std::max(mBig, 6 * q.nkf);
+    }
     tN += q.N; tObs += q.nobs; tLm += q.nlm; tKf += q.nkf; tFix += q.nfix; tG += 6 * q.nkf; tS += 36LL * q.nkf * q.nkf;
     mObs = std::max(mObs, q.nobs); mLm = std::max(mLm, q.nlm); mEl = std::max(mEl, q.nkf + 3 * q.npt + 6 * q.nls);
   }
+  const int nb = (int)hb.size();
   // one staged upload (inputs), one download (X, moved flags, control); the device work after them, the part zeroed
   // before the first pass (A, g_c, S, g_red, scal) last
   StagedLayout L;
   const size_t iProb = L.take_in(sizeof(LbbProb) * P), iX0 = L.take_in(8 * tN), iFT = L.take_in(128 * tFix);
   const size_t iLm = L.take_in(4 * tObs), iKf = L.take_in(4 * tObs), iZ = L.take_in(24 * tObs), iLs = L.take_in(4 * (tLm + P));
+  const size_t iBig = L.take_in(sizeof(GbbBig) * nb);
   const size_t oX = L.take_out(8 * tN), oMv = L.take_out(tLm), oCtl = L.take_out(sizeof(LbbCtrl) * P);
   const size_t wT0 = L.take_work(128 * tKf), wFTi = L.take_work(128 * tFix), wJt = L.take_work(48 * tObs),
                wJx = L.take_work(48 * tObs), wWn = L.take_work(16 * tObs), wD = L.take_work(288 * tLm),
                wDi = L.take_work(288 * tLm), wGl = L.take_work(48 * tLm), wDxc = L.take_work(8 * tG), wDX = L.take_work(8 * tN);
+  const size_t wWp = L.take_work(8 * tWp), wNz = L.take_work(tNz);
   const size_t wA = L.take_work(288 * tKf), wGc = L.take_work(48 * tKf), wS = L.take_work(8 * tS), wGr = L.take_work(8 * tG),
                wSc = L.take_work(64 * (size_t)P);
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -1125,6 +1283,7 @@ extern "C" plf_status plf_local_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts,
     if (q.nfix) memcpy((double*)(pin + iFT) + 16 * q.fo, pr.fixed_T, 128 * (size_t)q.nfix);
   }
   memcpy(pin + iProb, hp.data(), sizeof(LbbProb) * P);
+  if (nb) memcpy(pin + iBig, hb.data(), sizeof(GbbBig) * nb);
   cudaStream_t cs = ctx->stream;
   PLF_CUDA(ctx, cudaMemcpyAsync(dev, pin, L.in, cudaMemcpyHostToDevice, cs));
   uint8_t* const dout = dev + L.in;
@@ -1140,11 +1299,16 @@ extern "C" plf_status plf_local_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts,
   b.D = (double*)(dwork + wD); b.gl = (double*)(dwork + wGl); b.Dinv = (double*)(dwork + wDi);
   b.A = (double*)(dwork + wA); b.gc = (double*)(dwork + wGc); b.S = (double*)(dwork + wS); b.gred = (double*)(dwork + wGr);
   b.dxc = (double*)(dwork + wDxc); b.DX = (double*)(dwork + wDX); b.scal = (double*)(dwork + wSc); b.moved = dout + oMv;
+  const GbbBig* dBig = (const GbbBig*)(dev + iBig);
+  const GbbLdlt gl{dBig, b.ctrl, b.S, b.gred, b.dxc, b.DX, (double*)(dwork + wWp), dwork + wNz};
   // grids: (problem, chunks of 128 of the largest problem's count); the control kernels: one thread per problem
   auto chunks = [](int n) { return std::max(1, std::min(65535, (n + 127) / 128)); };
   const dim3 gObs(P, chunks(mObs)), gLm(P, chunks(mLm)), gEl(P, chunks(mEl));
   const int gCtl = (P + 127) / 128;
-  const int q = opts->ref_quirks ? BAQ_LBA : 0;
+  const int q = opts->ref_quirks ? (global ? BAQ_GBA : BAQ_LBA) : 0;
+  // the large problems' damping (42 n_kf elements) and zeroing (36 n_kf^2 + 48 n_kf doubles), gridded (chunk, problem)
+  const dim3 gDamp((7 * mBig + 255) / 256, std::max(nb, 1));
+  const dim3 gZero((unsigned)std::min<long long>(2048, ((long long)mBig * mBig + 255) / 256), std::max(nb, 1));
   k_lbb_prep<<<P, 128, 0, cs>>>(b, opts->lambda, std::max(opts->max_iters, 1));
   PLF_LAUNCH_CHECK(ctx);
   for (int r = 0; r < std::max(opts->max_iters, 1); ++r) {
@@ -1155,16 +1319,31 @@ extern "C" plf_status plf_local_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts,
     if (r == 0) {
       k_lbb_kf_diagmax<<<P, 128, 0, cs>>>(b);
       PLF_LAUNCH_CHECK(ctx);
-      k_lbb_first<<<gCtl, 128, 0, cs>>>(b, q);
+      if (q & BAQ_HMAX_INT) {
+        k_gbb_hmax_int<<<P, 1024, 0, cs>>>(b);
+        PLF_LAUNCH_CHECK(ctx);
+      }
+      if (global) k_gbb_first<<<gCtl, 128, 0, cs>>>(b, q);
+      else k_lbb_first<<<gCtl, 128, 0, cs>>>(b, q);
+    } else if (global) {
+      k_gbb_test<<<gCtl, 128, 0, cs>>>(b, r, q, opts->min_error, opts->min_error_change);
     } else {
       k_lbb_test<<<gCtl, 128, 0, cs>>>(b, r, opts->min_error, opts->min_error_change);
     }
     PLF_LAUNCH_CHECK(ctx);
-    k_lbb_schur<<<gLm, 128, 0, cs>>>(b);
+    const int swap = r == 0 && (q & BAQ_SWAP_COUPLING) ? 1 : 0;   // (g6)
+    k_lbb_schur<<<gLm, 128, 0, cs>>>(b, swap);
     PLF_LAUNCH_CHECK(ctx);
     k_lbb_solve<<<P, 256, 0, cs>>>(b);
     PLF_LAUNCH_CHECK(ctx);
-    k_lbb_backsub<<<gLm, 128, 0, cs>>>(b);
+    if (nb) {
+      k_gbb_damp<<<gDamp, 256, 0, cs>>>(b, dBig);
+      PLF_LAUNCH_CHECK(ctx);
+      if (plf_status st = gbb_ldlt(ctx, cs, gl, nb, mBig)) return st;
+      k_gbb_zero<<<gZero, 256, 0, cs>>>(b, dBig);
+      PLF_LAUNCH_CHECK(ctx);
+    }
+    k_lbb_backsub<<<gLm, 128, 0, cs>>>(b, swap);
     PLF_LAUNCH_CHECK(ctx);
     k_lbb_apply<<<gEl, 128, 0, cs>>>(b);
     PLF_LAUNCH_CHECK(ctx);
@@ -1201,5 +1380,60 @@ extern "C" plf_status plf_local_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts,
     return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: %s landmark %d has a zero diagonal entry in its first-pass block (no row constrains it)",
                     fn, refused, l < npt ? "point" : "line", l < npt ? l : l - npt);
   }
+  return PLF_OK;
+}
+
+extern "C" plf_status plf_local_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems, const plf_lba_problem* problems,
+                                         const int32_t* seq, plf_lba_result* out, plf_status* status) {
+  return lbb_run(ctx, opts, n_problems, problems, seq, out, status, false);
+}
+
+extern "C" plf_status plf_global_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems, const plf_lba_problem* problems,
+                                          const int32_t* seq, plf_lba_result* out, plf_status* status) {
+  return lbb_run(ctx, opts, n_problems, problems, seq, out, status, true);
+}
+
+// Test hook (plslam_b200.h): the k_gbb_* chain on n caller matrices of mixed sizes, each as plf_debug_ldlt's path 0
+extern "C" plf_status plf_debug_ldlt_batch(plf_ctx* ctx, int n, const int* n6, double* const* S, const double* const* g,
+                                           double* const* x, uint8_t* const* nz) {
+  const char* fn = "plf_debug_ldlt_batch";
+  if (!ctx || n < 0 || (n && (!n6 || !S || !g || !x)) || n > 65535) return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", fn);
+  if (!n) return PLF_OK;
+  std::vector<GbbBig> hb(n);
+  long long tS = 0, tG = 0, tWp = 0, tNz = 0;
+  int mx = 0;
+  for (int i = 0; i < n; ++i) {
+    if (n6[i] < 1 || n6[i] > 4096 || !S[i] || !g[i] || !x[i])
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: matrix %d: n6 = %d outside [1, 4096] or a NULL array", fn, i, n6[i]);
+    const long long m = 6LL * n6[i], nt = (m + GBA_T - 1) / GBA_T;
+    hb[i] = GbbBig{i, n6[i], tS, tG, tG, tWp, tNz};
+    tS += m * m; tG += m; tWp += nt * GBA_T * GBA_T; tNz += nt * nt;
+    mx = std::max(mx, (int)m);
+  }
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  GbbBig* dBig = nullptr;
+  GbbLdlt L{};
+  double* dx = nullptr;
+  uint8_t* dNz = nullptr;
+  DevBufList scr;
+  scr.add(dBig, n); scr.add(L.S, tS); scr.add(L.g, tG); scr.add(L.y, tG); scr.add(dx, tG); scr.add(L.Wp, tWp); scr.add(dNz, tNz);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_BA)) return st;
+  L.big = dBig; L.x = dx; L.nz = dNz;
+  cudaStream_t cs = ctx->stream;
+  PLF_CUDA(ctx, cudaMemcpyAsync(dBig, hb.data(), sizeof(GbbBig) * n, cudaMemcpyHostToDevice, cs));
+  for (int i = 0; i < n; ++i) {
+    const size_t m = 6 * (size_t)n6[i];
+    PLF_CUDA(ctx, cudaMemcpyAsync(L.S + hb[i].so, S[i], m * m * 8, cudaMemcpyHostToDevice, cs));
+    PLF_CUDA(ctx, cudaMemcpyAsync(L.g + hb[i].go, g[i], m * 8, cudaMemcpyHostToDevice, cs));
+  }
+  PLF_CUDA(ctx, cudaMemsetAsync(dNz, 0, tNz, cs));
+  if (plf_status st = gbb_ldlt(ctx, cs, L, n, mx)) return st;
+  for (int i = 0; i < n; ++i) {
+    const size_t m = 6 * (size_t)n6[i], nt = (m + GBA_T - 1) / GBA_T;
+    PLF_CUDA(ctx, cudaMemcpyAsync(S[i], L.S + hb[i].so, m * m * 8, cudaMemcpyDeviceToHost, cs));
+    PLF_CUDA(ctx, cudaMemcpyAsync(x[i], dx + hb[i].xo, m * 8, cudaMemcpyDeviceToHost, cs));
+    if (nz && nz[i]) PLF_CUDA(ctx, cudaMemcpyAsync(nz[i], dNz + hb[i].zo, nt * nt, cudaMemcpyDeviceToHost, cs));
+  }
+  PLF_CUDA(ctx, cudaStreamSynchronize(cs));
   return PLF_OK;
 }

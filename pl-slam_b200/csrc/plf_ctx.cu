@@ -85,6 +85,7 @@ void* plf_scratch(plf_ctx* ctx, plf_scratch_slot slot, size_t bytes) {
   if (e != cudaSuccess) {
     plf_fail(ctx, PLF_ERR_CUDA, "cudaMalloc(%zu) scratch slot %d: %s", want, (int)slot,
              cudaGetErrorString(e));
+    cudaGetLastError();   // an allocation failure is not sticky: the next launch check must not report it again
     b.p = nullptr;
     return nullptr;
   }

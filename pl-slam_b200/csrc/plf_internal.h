@@ -34,7 +34,7 @@ enum plf_scratch_slot {
   PLF_SCR_KF_MGB_PT,   // plf_match_kf2kf, plf_match_map2kf and their _batch forms: the windowed matcher of points
   PLF_SCR_KF_MGB_LS,   //   ... and of lines
   PLF_SCR_BOW,         // plf_bow_insert, plf_bow_insert_batch
-  PLF_SCR_BA_BATCH,    // plf_local_ba_batch: its staged layout
+  PLF_SCR_BA_BATCH,    // plf_local_ba_batch and plf_global_ba_batch: their staged layout
   PLF_SCR_LC,          // plf_loop_closure_pose and plf_loop_closure_pose_batch: their staged layout
   PLF_SCR_COUNT
 };

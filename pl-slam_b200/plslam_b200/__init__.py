@@ -677,6 +677,21 @@ class Frontend:
         `status` (0, or PLF_ERR_INVALID = -1 when the device refused that problem: a landmark whose first-pass block has a
         zero diagonal entry; its dict then holds its unchanged inputs and iters / err / lambda_ None).  Raises PlfError
         for the refusals before any work."""
+        return self._bundle_adjust_batch("plf_local_ba_batch", problems, seq, lambda_, lambda_k, max_iters, homog_th,
+                                         min_error, min_error_change, ref_quirks)
+
+    def global_ba_batch(self, problems, seq=None, lambda_=1e-5, lambda_k=10.0, max_iters=15, homog_th=1e-7,
+                        min_error=DBL_EPSILON, min_error_change=DBL_EPSILON, ref_quirks=1):
+        """Many global BAs in one device call (plf_global_ba_batch), with global_ba's options (and its DBL_EPSILON stop
+        thresholds) for all of them.  problems: dicts as global_ba takes; seq and the result as local_ba_batch: one dict
+        per problem in global_ba's shape plus `status` (0, or PLF_ERR_INVALID = -1 when the device refused that problem;
+        its dict then holds its unchanged inputs and iters / err / lambda_ None).  Raises PlfError for the refusals before
+        any work."""
+        return self._bundle_adjust_batch("plf_global_ba_batch", problems, seq, lambda_, lambda_k, max_iters, homog_th,
+                                         min_error, min_error_change, ref_quirks)
+
+    def _bundle_adjust_batch(self, fn, problems, seq, lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change,
+                             ref_quirks):
         problems = list(problems)
         P = len(problems)
         seq_a = self._problem_sequences(P, seq)
@@ -685,10 +700,10 @@ class Frontend:
         res = (plf_lba_result * max(P, 1))()
         st = np.full(max(P, 1), 1, np.int32)   # 1 is no plf_status: marks entries the call did not write
         o = plf_lba_opts(lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, int(ref_quirks))
-        rc = self.lib.plf_local_ba_batch(self._ctx, C.byref(o), P, arr, None if seq_a is None else _ptr(seq_a, C.c_int32),
-                                         res, _ptr(st, C.c_int32))
+        rc = getattr(self.lib, fn)(self._ctx, C.byref(o), P, arr, None if seq_a is None else _ptr(seq_a, C.c_int32),
+                                   res, _ptr(st, C.c_int32))
         if rc != 0 and (P == 0 or np.any(st[:P] == 1)):
-            self._check(rc, "plf_local_ba_batch")
+            self._check(rc, fn)
         out = []
         for k in range(P):
             d = self._lba_result(args[k][1], res[k] if st[k] == 0 else None)
@@ -1000,6 +1015,29 @@ class Frontend:
                                      _ptr(x, C.c_double), None if nz is None else _ptr(nz, C.c_uint8))
         self._check(st, "plf_debug_ldlt")
         return LD, x, nz
+
+    def debug_ldlt_batch(self, mats):
+        """debug_ldlt(S, g, path=0) on every (S, g) of `mats`, factored in one launch chain by the batched tiled LDL^T
+        of global_ba_batch.  Returns one (LD, x, nz) per matrix, as debug_ldlt.  plf_debug_ldlt_batch."""
+        mats = list(mats)
+        n6, LDs, gs, xs, nzs = [], [], [], [], []
+        for S, g in mats:
+            n = S.shape[0]
+            if S.shape != (n, n) or n % 6 or len(g) != n:
+                raise PlfError(f"debug_ldlt_batch: S {S.shape} and g {len(g)} must be 6 n6 square and 6 n6 long")
+            n6.append(n // 6)
+            LDs.append(np.array(S, np.float64, order="C"))
+            gs.append(np.ascontiguousarray(g, np.float64))
+            xs.append(np.empty(n, np.float64))
+            nt = (n + 63) // 64
+            nzs.append(np.zeros((nt, nt), np.uint8))
+        k = max(len(mats), 1)
+        ptrs = lambda arrs: (C.c_void_p * k)(*[a.ctypes.data for a in arrs])
+        n6a = np.array(n6 or [0], np.int32)
+        st = self.lib.plf_debug_ldlt_batch(self._ctx, len(mats), _ptr(n6a, C.c_int32), ptrs(LDs), ptrs(gs), ptrs(xs),
+                                           ptrs(nzs))
+        self._check(st, "plf_debug_ldlt_batch")
+        return list(zip(LDs, xs, nzs))
 
     def debug_timeline(self):
         """Device-clock start/end (ms) of the E, G, M phases of the two most recent batches: array [2, 3, 2]."""
