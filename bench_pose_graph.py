@@ -7,8 +7,9 @@ Per size it reports:
   - device ms per call (CUDA events on plf_stream around the call, median of --timed calls after one warm-up call);
   - iterations and trials of the call;
   - the per-trial split from torch.profiler (a separate call): linearisation (k_pgo_linearize, once per iteration),
-    assembly (k_pgo_assemble and the memset of the dense system), factorisation (k_gba_diag / panel / update),
-    substitution (k_gba_fwd / dscale / bwd), step and chi2 (k_pgo_step, k_pgo_edge_chi2, k_pgo_reduce), each summed
+    assembly (k_pgo_assemble and the zeroing of the dense system: k_pgo_zero, a memset before it), factorisation
+    (k_gbb_diag / panel / update, k_gba_* before the batched driver), substitution (k_gbb_fwd / dscale / bwd, k_gba_*
+    likewise), step and chi2 (k_pgo_step, k_pgo_edge_chi2, k_pgo_reduce), each summed
     over the call and divided by the number of trials;
   - factorisation FLOPs: n^3 / 3 for a dense LDL^T (n = 6 n_free) and the count the tiled path executes after skipping
     exactly-zero tiles, from the tile-level symbolic factorisation of H's block pattern (64^3 / 3 per diagonal tile,
@@ -38,9 +39,9 @@ from plslam_b200 import synth  # noqa: E402
 T = 64
 GROUPS = {
     "linearize": ("k_pgo_linearize",),
-    "assembly": ("k_pgo_assemble", "Memset"),
-    "factorisation": ("k_gba_diag", "k_gba_panel", "k_gba_update"),
-    "substitution": ("k_gba_fwd", "k_gba_dscale", "k_gba_bwd"),
+    "assembly": ("k_pgo_assemble", "k_pgo_zero", "Memset"),
+    "factorisation": ("k_gba_diag", "k_gba_panel", "k_gba_update", "k_gbb_diag", "k_gbb_panel", "k_gbb_update"),
+    "substitution": ("k_gba_fwd", "k_gba_dscale", "k_gba_bwd", "k_gbb_fwd", "k_gbb_dscale", "k_gbb_bwd"),
     "step_chi2": ("k_pgo_step", "k_pgo_edge_chi2", "k_pgo_reduce"),
 }
 

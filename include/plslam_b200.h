@@ -534,6 +534,32 @@ typedef struct plf_pgo_result {
 } plf_pgo_result;
 plf_status plf_pose_graph(plf_ctx* ctx, const plf_pgo_opts* opts, const plf_pgo_problem* problem, plf_pgo_result* out);
 
+/* Many loop-closure pose graphs in one call: the sequences whose loop closures became ready together
+ * (INTEGRATION.md §4a), optimised in lockstep rounds with one launch chain and one host synchronisation per round.
+ *   problems [n_problems]  plf_pose_graph's layout and rules, T updated in place
+ *   out      [n_problems]  plf_pose_graph's result of each problem, with its own trace / trace_cap (trace may be NULL)
+ * One opts serves every problem.  Problem p's T, iters, stop, trials, chi2_init, chi2, lambda and trace rows are
+ * bit-identical to what plf_pose_graph returns for it alone, whatever the other problems are and in whatever order they
+ * come.  plf_pose_graph is this call with one problem.
+ * Refusals before any work, with nothing written (no T, no out field): PLF_ERR_INVALID when n_problems < 0, opts is NULL,
+ * problems or out is NULL with problems, or a problem breaks one of plf_pose_graph's rules (the message starts
+ * "plf_pose_graph_batch: problem k: " and goes on as plf_pose_graph's); PLF_ERR_CAPACITY beyond 65535 problems or 4096
+ * free vertices with edges in a problem.  n_problems = 0 returns PLF_OK and launches nothing.  When the problems' dense
+ * systems do not fit on the device together the call fails with PLF_ERR_CUDA naming the scratch, and nothing is written.
+ * The context stays usable after any error.
+ * Rounds: round 0 evaluates every problem's initial chi2; each later round is one trial (one solve of (H + lambda I) x = b)
+ * of every problem still running.  g2o's decisions (rho, acceptance, the lambda schedule, the 10-trial loop and the stop
+ * tests) stay on the host, in double, per problem.  The call synchronises 2 + max_p trials_p times.
+ * Launches: round 0: 2 (1 when no problem has an edge); a later round: 5 n_t + 4, plus 1 (the linearisation) when a
+ * running problem starts an iteration in it, with n_t = ceil(6 n_free / 64) of the largest problem still running.  They
+ * do not depend on n_problems: plf_pose_graph launches the same for its one problem.
+ * Work is enqueued on plf_stream and uses plf_pose_graph's scratch slot: the sum of what each problem takes there (288
+ * n_free^2 bytes of dense system, about 790 bytes per edge, 260 per vertex and 200 per free vertex, 32768 n_t + n_t^2
+ * bytes of tile work) plus about 300 bytes per problem; out[p].scratch_bytes reports the call's total.  The context's
+ * pinned staging buffer holds the inputs, the poses and the per-round control. */
+plf_status plf_pose_graph_batch(plf_ctx* ctx, const plf_pgo_opts* opts, int n_problems, const plf_pgo_problem* problems,
+                                plf_pgo_result* out);
+
 /* Relative pose between two keyframes (SURVEY 8(f) f2).  Replaces MapHandler::isLoopClosure (src/mapHandler.cpp:3192-3300:
  * match() on the points :3223 and on the lines :3249 of kf0 / kf1, the inlier-ratio pre-condition :3277-3299) followed by
  * MapHandler::computeRelativePoseRobustGN (:3566-3957: two-stage robust GN from identity with the chi2 gate in between,

@@ -1104,20 +1104,11 @@ __global__ void __launch_bounds__(128) k_lbb_moved(LbbDev b) {
 // there is one launch of each stage over every large problem, gridded (tile, problem) at the largest problem's extent:
 // blockIdx.y picks the problem from the GbbBig table, and a CTA whose problem has fewer tiles, has stopped or was refused
 // returns at once.  Each CTA runs the single-problem function of the stage, so a problem's factorisation is plf_ldlt_tiled's
-// bit for bit.
-struct GbbBig {
-  int p, nkf;                     // the problem's index in the batch and its keyframe count
-  long long so, go, xo, wo, zo;   // offsets into S, g / y, x (doubles), Wp (doubles) and the zero flags (bytes)
-};
-struct GbbLdlt {
-  const GbbBig* big;
-  const LbbCtrl* ctrl;   // the problems' control state, NULL when every problem is active (plf_debug_ldlt_batch)
-  double* S; double* g; double* y; double* x; double* Wp; uint8_t* nz;
-};
+// bit for bit.  GbbBig and GbbLdlt are declared in plf_internal.h: plf_pose_graph_batch factors through gbb_ldlt too.
 // The LbaDev fields the tiled kernels read, for problem blockIdx.y, and its tile count; false when it is not active.
 __device__ __forceinline__ bool gbb_view(const GbbLdlt& L, LbaDev& d, GbbBig& t, int& nt) {
-  t = L.big[blockIdx.y];
-  if (L.ctrl && !L.ctrl[t.p].active) return false;
+  t = L.big ? L.big[blockIdx.y] : L.one;
+  if (L.active && !L.active[(size_t)t.p * L.active_stride]) return false;
   d.nkf = t.nkf; d.S = L.S + t.so; d.gred = L.g + t.go; d.dxc = L.y + t.go; d.DX = L.x + t.xo;
   nt = (6 * t.nkf + GBA_T - 1) / GBA_T;
   return true;
@@ -1159,7 +1150,7 @@ __global__ void __launch_bounds__(256) k_gbb_bwd(GbbLdlt L, int k) {
 
 // The tiled factorisation and the two substitutions of the nb problems in L.big, the largest with n_max rows: the
 // launches of plf_ldlt_tiled at n_max, each over every problem.
-static plf_status gbb_ldlt(plf_ctx* ctx, cudaStream_t cs, const GbbLdlt& L, int nb, int n_max) {
+plf_status gbb_ldlt(plf_ctx* ctx, cudaStream_t cs, const GbbLdlt& L, int nb, int n_max) {
   const int nt = (n_max + GBA_T - 1) / GBA_T, smem = 2 * GBA_T * GBA_LD * 8;
   PLF_CUDA(ctx, cudaFuncSetAttribute(k_gbb_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   for (int k = 0; k < nt; ++k) {
@@ -1300,7 +1291,9 @@ static plf_status lbb_run(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems
   b.A = (double*)(dwork + wA); b.gc = (double*)(dwork + wGc); b.S = (double*)(dwork + wS); b.gred = (double*)(dwork + wGr);
   b.dxc = (double*)(dwork + wDxc); b.DX = (double*)(dwork + wDX); b.scal = (double*)(dwork + wSc); b.moved = dout + oMv;
   const GbbBig* dBig = (const GbbBig*)(dev + iBig);
-  const GbbLdlt gl{dBig, b.ctrl, b.S, b.gred, b.dxc, b.DX, (double*)(dwork + wWp), dwork + wNz};
+  static_assert(sizeof(LbbCtrl) % sizeof(int) == 0, "gbb_view reads LbbCtrl::active as a strided int");
+  const int* act = (const int*)((const uint8_t*)b.ctrl + offsetof(LbbCtrl, active));
+  const GbbLdlt gl{dBig, act, (int)(sizeof(LbbCtrl) / sizeof(int)), b.S, b.gred, b.dxc, b.DX, (double*)(dwork + wWp), dwork + wNz};
   // grids: (problem, chunks of 128 of the largest problem's count); the control kernels: one thread per problem
   auto chunks = [](int n) { return std::max(1, std::min(65535, (n + 127) / 128)); };
   const dim3 gObs(P, chunks(mObs)), gLm(P, chunks(mLm)), gEl(P, chunks(mEl));

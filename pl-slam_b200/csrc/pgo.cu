@@ -1,20 +1,24 @@
-// Loop-closure pose-graph optimisation on the GPU (DESIGN.md §1 row f7).
+// Loop-closure pose-graph optimisation on the GPU (DESIGN.md §1 row f7), one problem (plf_pose_graph) or many at once
+// (plf_pose_graph_batch, the same driver).
 //
 // Replaces the g2o part of MapHandler::loopClosureOptimizationCovGraphG2O (src/mapHandler.cpp:4185-4410):
 // computeInitialGuess() and optimize(maxItersPGO) of g2o's OptimizationAlgorithmLevenberg over VertexSE3 / EdgeSE3 with
-// identity information.  The host keeps g2o's control flow (oracle/pgo.py restates it); the numerical work runs here:
+// identity information.  The host keeps g2o's control flow (oracle/pgo.py restates it), one step function per problem;
+// the numerical work runs here, each kernel gridded (item, problem) over the problems still running:
 //   k_pgo_linearize   one thread per edge, once per iteration: E = Z^-1 X_i^-1 X_j, e = MQT(E) and the Jacobians J_i, J_j
 //                     at the iteration's estimate, reused by every trial of the iteration
+//   k_pgo_zero        the dense system S = 0, across the GPU
 //   k_pgo_assemble    one CTA per non-zero 6 x 6 block of the lower triangle of H: the block's contributions summed in
 //                     ascending edge order (a per-block edge list built once per call), written with + lambda I into
 //                     the dense system S; the diagonal blocks also write b = -sum J^T e.  No float atomics: two calls
 //                     are bit-identical.
-//   plf_ldlt_tiled    the tiled LDL^T and the two substitutions of plf_global_ba (lba.cu), unchanged
+//   gbb_ldlt          the tiled LDL^T and the two substitutions of plf_global_ba (lba.cu), batched (k_gbb_*)
 //   k_pgo_step        one thread per vertex: X_t = X (+) x, the pivot check on D and x (lambda x + b) per free vertex
 //   k_pgo_edge_chi2   one thread per edge: e^T e at a given estimate
-//   k_pgo_reduce      one CTA: chi2, sum x (lambda x + b) and the pivot flag, each summed in a fixed order
-// One 4-double copy per trial goes to the host for the trial's decision.
+//   k_pgo_reduce      one CTA per problem: chi2, sum x (lambda x + b) and the pivot flag, each summed in a fixed order
+// One 4-double copy per problem and trial goes to the host for the trial's decision.
 #include <math.h>
+#include <stddef.h>
 
 #include <unordered_map>
 
@@ -107,9 +111,8 @@ struct PgoDev {
   double* red;                            // 4: chi2, sum x (lambda x + b), pivot failure
 };
 
-__global__ void __launch_bounds__(128) k_pgo_linearize(PgoDev d) {
-  const int k = blockIdx.x * 128 + threadIdx.x;
-  if (k >= d.ne) return;
+// ---- one problem's work: each function is one edge, block, vertex or CTA of the problem d ----------------------------
+__device__ __forceinline__ void pgo_linearize(const PgoDev& d, int k) {
   const double* Z = d.Z + 16 * (size_t)k;
   double E[16], q[4], e[6];
   pgo_error(d.X + 16 * (size_t)d.efrom[k], d.X + 16 * (size_t)d.eto[k], Z, E, q, e);
@@ -140,9 +143,10 @@ __global__ void __launch_bounds__(128) k_pgo_linearize(PgoDev d) {
   for (int i = 0; i < 36; ++i) { d.Ji[36 * (size_t)k + i] = Ji[i]; d.Jj[36 * (size_t)k + i] = Jj[i]; }
 }
 
-// kind 0: J_i^T J_i, 1: J_j^T J_j, 2: J_i^T J_j (the block row is the edge's `from`), 3: J_j^T J_i
-__global__ void __launch_bounds__(64) k_pgo_assemble(PgoDev d, double lambda) {
-  const int blk = blockIdx.x, t = threadIdx.x, n = 6 * d.nf;
+// block blk, one CTA of 64 threads; kind 0: J_i^T J_i, 1: J_j^T J_j, 2: J_i^T J_j (the block row is the edge's `from`),
+// 3: J_j^T J_i
+__device__ __forceinline__ void pgo_assemble(const PgoDev& d, int blk, double lambda) {
+  const int t = threadIdx.x, n = 6 * d.nf;
   const int br = d.blk_rc[2 * blk], bc = d.blk_rc[2 * blk + 1], s = d.blk_start[blk], end = d.blk_start[blk + 1];
   if (t < 36) {
     const int r = t / 6, c = t % 6;
@@ -174,9 +178,7 @@ __global__ void __launch_bounds__(64) k_pgo_assemble(PgoDev d, double lambda) {
 }
 
 // X_t = X Inc(x_v): Inc = (R(q), x_t) with q = (sqrt(1 - |x_q|^2), x_q), the identity rotation when 1 - |x_q|^2 < 0
-__global__ void __launch_bounds__(128) k_pgo_step(PgoDev d, double lambda) {
-  const int v = blockIdx.x * 128 + threadIdx.x;
-  if (v >= d.nv) return;
+__device__ __forceinline__ void pgo_step(const PgoDev& d, int v, double lambda) {
   const double* X = d.X + 16 * (size_t)v;
   double* Xt = d.Xt + 16 * (size_t)v;
   const int f = d.fidx[v];
@@ -218,9 +220,7 @@ __global__ void __launch_bounds__(128) k_pgo_step(PgoDev d, double lambda) {
   d.bad[f] = bad;
 }
 
-__global__ void __launch_bounds__(128) k_pgo_edge_chi2(PgoDev d, const double* X) {
-  const int k = blockIdx.x * 128 + threadIdx.x;
-  if (k >= d.ne) return;
+__device__ __forceinline__ void pgo_edge_chi2(const PgoDev& d, const double* X, int k) {
   double E[16], q[4], e[6];
   pgo_error(X + 16 * (size_t)d.efrom[k], X + 16 * (size_t)d.eto[k], d.Z + 16 * (size_t)k, E, q, e);
   double s = 0.0;
@@ -242,8 +242,8 @@ __device__ inline double pgo_block_sum(double v, double* sh) {
   __syncthreads();
   return r;
 }
-__global__ void __launch_bounds__(PGO_RED) k_pgo_reduce(PgoDev d, int nf) {
-  __shared__ double sh[PGO_RED];
+// one CTA of PGO_RED threads: chi2 and the step's two other sums over nf free vertices (0 for the initial chi2)
+__device__ __forceinline__ void pgo_reduce(const PgoDev& d, int nf, double* sh) {
   const int t = threadIdx.x;
   double c = 0.0, s = 0.0, b = 0.0;
   for (int i = t; i < d.ne; i += PGO_RED) c += d.ce[i];
@@ -254,55 +254,154 @@ __global__ void __launch_bounds__(PGO_RED) k_pgo_reduce(PgoDev d, int nf) {
   if (t == 0) { d.red[0] = c; d.red[1] = s; d.red[2] = b; d.red[3] = 0.0; }
 }
 
-}  // namespace
+// ---- the batch: problem p's arrays are slices of flat arrays, at the offsets of its PgoProb -------------------------------
+struct PgoProb {
+  int nv, ne, nf, nb;
+  long long vo, eo, fo, bo, io, so;   // offsets: vertices, edges, free vertices, blocks, block items (blk_start: bo + p),
+                                      // S (doubles)
+};
+// A problem's part of the round, written by the host before each round
+struct PgoCtl {
+  double lambda;
+  int active;   // 0 once the problem has stopped: every kernel returns at once for it
+  int start;    // this round's trial starts an iteration: linearise at the estimate
+  int cur;      // the pose buffer (0 / 1) that holds the estimate X; the other receives the trial estimate X_t
+  int pad;
+};
+struct PgoBatch {
+  const PgoProb* prob; const PgoCtl* ctl;
+  const int* efrom; const int* eto; const double* Z; const int* fidx;
+  double* X; long long xpar;   // the two pose buffers, xpar doubles apart
+  double* e; double* Ji; double* Jj; double* ce;
+  const int* blk_rc; const int* blk_start; const int* blk_item;
+  double* S; double* b; double* g; double* y; double* x; double* dotp; uint8_t* bad; double* red;
+};
 
-extern "C" plf_status plf_pose_graph(plf_ctx* ctx, const plf_pgo_opts* opts, const plf_pgo_problem* p, plf_pgo_result* out) {
-  const char* fn = "plf_pose_graph";
-  if (!ctx || !opts || !p || !out || p->n_v < 0 || p->n_e < 0 || opts->max_iters < 0 || out->trace_cap < 0 ||
-      (out->trace_cap && !out->trace))
-    return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", fn);
-  // g2o takes a non-positive user lambda as "derive one from H"; both call sites pass 1e-10, so anything else is refused
-  if (!(opts->lambda_init > 0.0 && opts->lambda_init <= 1.7976931348623157e308))
-    return plf_fail(ctx, PLF_ERR_INVALID, "%s: lambda_init %g is not a positive finite number", fn, opts->lambda_init);
+__device__ __forceinline__ PgoDev pgo_view(const PgoBatch& B, int p) {
+  const PgoProb q = B.prob[p];
+  const int cur = B.ctl[p].cur;
+  PgoDev d;
+  d.nv = q.nv; d.ne = q.ne; d.nf = q.nf; d.nb = q.nb;
+  d.efrom = B.efrom + q.eo; d.eto = B.eto + q.eo; d.Z = B.Z + 16 * q.eo; d.fidx = B.fidx + q.vo;
+  d.X = B.X + cur * B.xpar + 16 * q.vo; d.Xt = B.X + (cur ^ 1) * B.xpar + 16 * q.vo;
+  d.e = B.e + 6 * q.eo; d.Ji = B.Ji + 36 * q.eo; d.Jj = B.Jj + 36 * q.eo; d.ce = B.ce + q.eo;
+  d.blk_rc = B.blk_rc + 2 * q.bo; d.blk_start = B.blk_start + q.bo + p; d.blk_item = B.blk_item + q.io;
+  d.S = B.S + q.so;
+  d.b = B.b + 6 * q.fo; d.g = B.g + 6 * q.fo; d.y = B.y + 6 * q.fo; d.x = B.x + 6 * q.fo;
+  d.dotp = B.dotp + q.fo; d.bad = B.bad + q.fo; d.red = B.red + 4 * p;
+  return d;
+}
+
+// The kernels are gridded (item, problem): blockIdx.y is the problem, blockIdx.x strides over its items at the extent of
+// the round's largest active problem.
+__global__ void __launch_bounds__(128) k_pgo_linearize(PgoBatch B) {
+  const int p = blockIdx.y;
+  if (!B.ctl[p].active || !B.ctl[p].start) return;
+  const PgoDev d = pgo_view(B, p);
+  const int k = blockIdx.x * 128 + threadIdx.x;
+  if (k < d.ne) pgo_linearize(d, k);
+}
+
+// S = 0 across the GPU, for the assembly (which writes only the non-zero blocks)
+__global__ void __launch_bounds__(256) k_pgo_zero(PgoBatch B) {
+  const int p = blockIdx.y;
+  if (!B.ctl[p].active) return;
+  const PgoProb q = B.prob[p];
+  const size_t n = 6 * (size_t)q.nf, stride = (size_t)gridDim.x * 256;
+  double* S = B.S + q.so;
+  for (size_t i = blockIdx.x * 256 + threadIdx.x; i < n * n; i += stride) S[i] = 0.0;
+}
+
+// one CTA per non-zero block
+__global__ void __launch_bounds__(64) k_pgo_assemble(PgoBatch B) {
+  const int p = blockIdx.y;
+  if (!B.ctl[p].active) return;
+  const PgoDev d = pgo_view(B, p);
+  if ((int)blockIdx.x < d.nb) pgo_assemble(d, blockIdx.x, B.ctl[p].lambda);
+}
+
+__global__ void __launch_bounds__(128) k_pgo_step(PgoBatch B) {
+  const int p = blockIdx.y;
+  if (!B.ctl[p].active) return;
+  const PgoDev d = pgo_view(B, p);
+  const int v = blockIdx.x * 128 + threadIdx.x;
+  if (v < d.nv) pgo_step(d, v, B.ctl[p].lambda);
+}
+
+// e^T e per edge at the estimate (trial 0: the initial chi2) or at the trial estimate
+__global__ void __launch_bounds__(128) k_pgo_edge_chi2(PgoBatch B, int trial) {
+  const int p = blockIdx.y;
+  if (!B.ctl[p].active) return;
+  const PgoDev d = pgo_view(B, p);
+  const int k = blockIdx.x * 128 + threadIdx.x;
+  if (k < d.ne) pgo_edge_chi2(d, trial ? d.Xt : d.X, k);
+}
+
+__global__ void __launch_bounds__(PGO_RED) k_pgo_reduce(PgoBatch B, int trial) {
+  __shared__ double sh[PGO_RED];
+  const int p = blockIdx.y;
+  if (!B.ctl[p].active) return;
+  const PgoDev d = pgo_view(B, p);
+  pgo_reduce(d, trial ? d.nf : 0, sh);
+}
+
+// ---- host side ---------------------------------------------------------------------------------------------------------
+// One problem after its checks: its system's blocks (the free vertices with edges, in id order), the initial guess and
+// the blocks of H's lower triangle with their contributions in ascending edge order.
+struct PgoHost {
+  int nf = 0;
+  std::vector<int> fidx, blk_rc, blk_start, blk_item;
+  std::vector<double> X;
+};
+
+// plf_pose_graph's rules for one problem after its argument checks, in order; pfx starts every message
+static plf_status pgo_check(plf_ctx* ctx, const char* pfx, const plf_pgo_problem* p, PgoHost& h) {
   const int nv = p->n_v, ne = p->n_e;
   if ((nv && (!p->T || !p->fixed)) || (ne && (!p->from || !p->to || !p->Z)))
-    return plf_fail(ctx, PLF_ERR_INVALID, "%s: null array", fn);
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: null array", pfx);
   std::vector<int> deg(nv, 0);
   for (int k = 0; k < ne; ++k) {
     const int a = p->from[k], b = p->to[k];
     if (a < 0 || a >= nv || b < 0 || b >= nv || a == b)
-      return plf_fail(ctx, PLF_ERR_INVALID, "%s: edge %d joins vertices %d and %d (%d vertices)", fn, k, a, b, nv);
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: edge %d joins vertices %d and %d (%d vertices)", pfx, k, a, b, nv);
     deg[a]++; deg[b]++;
   }
-  // the system's blocks: the free vertices with edges, in id order
-  std::vector<int> fidx(nv, -1);
+  h.fidx.assign(nv, -1);
   int nf = 0;
   for (int v = 0; v < nv; ++v)
-    if (!p->fixed[v] && deg[v]) fidx[v] = nf++;
-  if (nf > 4096) return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: %d free vertices with edges (limit 4096)", fn, nf);
+    if (!p->fixed[v] && deg[v]) h.fidx[v] = nf++;
+  h.nf = nf;
+  if (nf > 4096) return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: %d free vertices with edges (limit 4096)", pfx, nf);
   for (size_t i = 0; i < (size_t)nv * 16; ++i)
-    if (!isfinite(p->T[i])) return plf_fail(ctx, PLF_ERR_INVALID, "%s: non-finite pose of vertex %d", fn, (int)(i / 16));
+    if (!isfinite(p->T[i])) return plf_fail(ctx, PLF_ERR_INVALID, "%s: non-finite pose of vertex %d", pfx, (int)(i / 16));
   for (size_t i = 0; i < (size_t)ne * 16; ++i)
-    if (!isfinite(p->Z[i])) return plf_fail(ctx, PLF_ERR_INVALID, "%s: non-finite measurement of edge %d", fn, (int)(i / 16));
+    if (!isfinite(p->Z[i])) return plf_fail(ctx, PLF_ERR_INVALID, "%s: non-finite measurement of edge %d", pfx, (int)(i / 16));
   // every connected component with edges holds a fixed vertex (else its system is singular up to the damping)
-  {
-    std::vector<int> root(nv);
-    for (int v = 0; v < nv; ++v) root[v] = v;
-    auto find = [&](int v) { while (root[v] != v) v = root[v] = root[root[v]]; return v; };
-    for (int k = 0; k < ne; ++k) root[find(p->from[k])] = find(p->to[k]);
-    std::vector<uint8_t> anchored(nv, 0);
-    for (int v = 0; v < nv; ++v)
-      if (p->fixed[v]) anchored[find(v)] = 1;
-    for (int k = 0; k < ne; ++k)
-      if (!anchored[find(p->from[k])])
-        return plf_fail(ctx, PLF_ERR_INVALID, "%s: the component of edge %d has no fixed vertex", fn, k);
-  }
+  std::vector<int> root(nv);
+  for (int v = 0; v < nv; ++v) root[v] = v;
+  auto find = [&](int v) { while (root[v] != v) v = root[v] = root[root[v]]; return v; };
+  for (int k = 0; k < ne; ++k) root[find(p->from[k])] = find(p->to[k]);
+  std::vector<uint8_t> anchored(nv, 0);
+  for (int v = 0; v < nv; ++v)
+    if (p->fixed[v]) anchored[find(v)] = 1;
+  for (int k = 0; k < ne; ++k)
+    if (!anchored[find(p->from[k])])
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: the component of edge %d has no fixed vertex", pfx, k);
+  return PLF_OK;
+}
+
+// the initial guess and the block lists of a checked problem
+static void pgo_prepare(const plf_pgo_problem* p, PgoHost& h) {
+  const int nv = p->n_v, ne = p->n_e, nf = h.nf;
+  const std::vector<int>& fidx = h.fidx;
   // ---- initial guess (g2o computeInitialGuess): breadth-first from the fixed vertices in ascending id, each vertex's
   // edges in the order given; a reached free vertex takes parent * Z (parent = from) or parent * Z^-1
-  std::vector<double> X(p->T, p->T + (size_t)nv * 16);
+  std::vector<double>& X = h.X;
+  X.assign(p->T, p->T + (size_t)nv * 16);
   {
     std::vector<int> adj_start(nv + 1, 0), adj((size_t)2 * ne);
-    for (int v = 0; v < nv; ++v) adj_start[v + 1] = adj_start[v] + deg[v];
+    for (int k = 0; k < ne; ++k) { adj_start[p->from[k] + 1]++; adj_start[p->to[k] + 1]++; }
+    for (int v = 0; v < nv; ++v) adj_start[v + 1] += adj_start[v];
     std::vector<int> fill(adj_start.begin(), adj_start.end() - 1);
     for (int k = 0; k < ne; ++k) { adj[fill[p->from[k]]++] = k; adj[fill[p->to[k]]++] = k; }
     std::vector<uint8_t> seen(nv);
@@ -312,8 +411,8 @@ extern "C" plf_status plf_pose_graph(plf_ctx* ctx, const plf_pgo_opts* opts, con
       seen[v] = p->fixed[v] ? 1 : 0;
       if (p->fixed[v]) queue.push_back(v);
     }
-    for (size_t h = 0; h < queue.size(); ++h) {
-      const int v = queue[h];
+    for (size_t hd = 0; hd < queue.size(); ++hd) {
+      const int v = queue[hd];
       for (int a = adj_start[v]; a < adj_start[v + 1]; ++a) {
         const int k = adj[a], u = p->from[k] == v ? p->to[k] : p->from[k];
         if (seen[u]) continue;
@@ -330,7 +429,8 @@ extern "C" plf_status plf_pose_graph(plf_ctx* ctx, const plf_pgo_opts* opts, con
     }
   }
   // ---- the blocks of H's lower triangle and their contributions, in ascending edge order
-  std::vector<int> blk_rc;
+  std::vector<int>& blk_rc = h.blk_rc;
+  blk_rc.clear();
   blk_rc.reserve((size_t)2 * nf);
   for (int f = 0; f < nf; ++f) { blk_rc.push_back(f); blk_rc.push_back(f); }
   std::unordered_map<long long, int> off;
@@ -348,114 +448,244 @@ extern "C" plf_status plf_pose_graph(plf_ctx* ctx, const plf_pgo_opts* opts, con
     }
   }
   const int nb = (int)(blk_rc.size() / 2), nit = (int)it_blk.size();
-  std::vector<int> blk_start(nb + 1, 0), blk_item(nit);
-  for (int i = 0; i < nit; ++i) blk_start[it_blk[i] + 1]++;
-  for (int b = 0; b < nb; ++b) blk_start[b + 1] += blk_start[b];
-  {
-    std::vector<int> fill(blk_start.begin(), blk_start.end() - 1);
-    for (int i = 0; i < nit; ++i) blk_item[fill[it_blk[i]]++] = it_val[i];
+  h.blk_start.assign(nb + 1, 0);
+  h.blk_item.resize(nit);
+  for (int i = 0; i < nit; ++i) h.blk_start[it_blk[i] + 1]++;
+  for (int b = 0; b < nb; ++b) h.blk_start[b + 1] += h.blk_start[b];
+  std::vector<int> fill(h.blk_start.begin(), h.blk_start.end() - 1);
+  for (int i = 0; i < nit; ++i) h.blk_item[fill[it_blk[i]]++] = it_val[i];
+}
+
+// g2o's OptimizationAlgorithmLevenberg::solve for one problem, between two trials
+struct PgoLm {
+  int iter = 0, trials = 0;   // the iteration, and the trials it has run so far
+  double chi = 0.0, lambda = 0.0;
+  double ni = 2.0;            // g2o's _ni is a double: it doubles on every rejected trial and must reach lambda's overflow
+  bool running = false;
+  int cur = 0;                // the pose buffer holding the estimate
+};
+
+// The decision after one trial, from its sums red (chi2 at X_t, sum x (lambda x + b), pivot failure): the trace row,
+// g2o's acceptance and lambda / ni schedule, its do ... while (rho < 0 && trials < 10) and the three stop tests that end
+// the iteration loop.  The arithmetic stays on the host, in double: the device's pow is not glibc's.
+static void pgo_decide(PgoLm& s, const double* red, int max_iters, plf_pgo_result& out) {
+  const double chi_t = red[2] != 0.0 ? 1.7976931348623157e308 : red[0];   // failed solve: DBL_MAX
+  const double rho = (s.chi - chi_t) / (red[1] + 1e-3);
+  const bool accept = rho > 0.0 && isfinite(chi_t);
+  if (out.n_trace < out.trace_cap) {
+    plf_pgo_trial& tr = out.trace[out.n_trace++];
+    tr.iter = s.iter; tr.accepted = accept; tr.lambda = s.lambda; tr.chi = s.chi; tr.chi_t = chi_t; tr.rho = rho;
   }
-  // ---- device buffers (scratch slot PLF_SCR_BA)
+  if (accept) {
+    const double alpha = std::min(1.0 - pow(2.0 * rho - 1.0, 3), 2.0 / 3.0);
+    s.lambda *= std::max(1.0 / 3.0, alpha);
+    s.ni = 2;
+    s.cur ^= 1;
+    s.chi = chi_t;
+  } else {
+    s.lambda *= s.ni;
+    s.ni *= 2;
+  }
+  ++s.trials;
+  if (rho < 0.0 && s.trials < 10) return;   // the iteration's next trial
+  out.iters = s.iter + 1;
+  out.trials += s.trials;
+  if (s.trials == 10 || rho == 0.0 || !isfinite(s.lambda)) {
+    out.stop = s.trials == 10 ? PLF_PGO_STOP_TRIALS : (rho == 0.0 ? PLF_PGO_STOP_RHO_ZERO : PLF_PGO_STOP_LAMBDA);
+    s.running = false;
+  } else if (++s.iter == max_iters) {
+    s.running = false;
+  }
+  s.trials = 0;
+}
+
+// plf_pose_graph (one problem, batch = false) and plf_pose_graph_batch.  Every refusal comes before any work.  One
+// staged upload, then rounds in lockstep: round 0 evaluates every problem's initial chi2, each later round runs one trial
+// of every running problem in one launch chain, uploads the problems' lambdas and flags before it and downloads their
+// sums after it, with one host synchronisation.  One download of the poses ends the call.
+static plf_status pgo_run(plf_ctx* ctx, const plf_pgo_opts* opts, int P, const plf_pgo_problem* problems,
+                          plf_pgo_result* out, bool batch) {
+  const char* fn = batch ? "plf_pose_graph_batch" : "plf_pose_graph";
+  if (!ctx || !opts || P < 0 || (P && (!problems || !out)) || opts->max_iters < 0)
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", fn);
+  // g2o takes a non-positive user lambda as "derive one from H"; both call sites pass 1e-10, so anything else is refused
+  if (!(opts->lambda_init > 0.0 && opts->lambda_init <= 1.7976931348623157e308))
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: lambda_init %g is not a positive finite number", fn, opts->lambda_init);
+  if (!P) return PLF_OK;
+  // the problems are gridded in y
+  if (P > 65535) return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: %d problems (limit 65535)", fn, P);
+  std::vector<std::string> pfx(P);
+  for (int k = 0; k < P; ++k) {
+    char buf[64];
+    if (batch) snprintf(buf, sizeof buf, "%s: problem %d", fn, k);
+    pfx[k] = batch ? buf : fn;
+  }
+  // each problem's rules in the single call's order, the problems in turn: the first bad problem is the one named
+  std::vector<PgoHost> h(P);
+  for (int k = 0; k < P; ++k) {
+    const plf_pgo_problem& p = problems[k];
+    if (p.n_v < 0 || p.n_e < 0 || out[k].trace_cap < 0 || (out[k].trace_cap && !out[k].trace))
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", pfx[k].c_str());
+    if (plf_status st = pgo_check(ctx, pfx[k].c_str(), &p, h[k])) return st;
+  }
+  // ---- the flat layout
+  std::vector<PgoProb> hp(P);
+  std::vector<GbbBig> hb(P);
+  long long tV = 0, tE = 0, tF = 0, tB = 0, tI = 0, tS = 0, tWp = 0, tNz = 0;
+  int mE = 0;
+  for (int k = 0; k < P; ++k) {
+    pgo_prepare(&problems[k], h[k]);
+    PgoProb& q = hp[k];
+    q.nv = problems[k].n_v; q.ne = problems[k].n_e; q.nf = h[k].nf; q.nb = (int)(h[k].blk_rc.size() / 2);
+    q.vo = tV; q.eo = tE; q.fo = tF; q.bo = tB; q.io = tI; q.so = tS;
+    const long long n = 6LL * q.nf, nt = (n + PLF_LDLT_TILE - 1) / PLF_LDLT_TILE;
+    hb[k] = GbbBig{k, q.nf, tS, 6 * tF, 6 * tF, tWp, tNz};
+    tV += q.nv; tE += q.ne; tF += q.nf; tB += q.nb; tI += (long long)h[k].blk_item.size(); tS += n * n;
+    tWp += nt * PLF_LDLT_TILE * PLF_LDLT_TILE; tNz += nt * nt;
+    mE = std::max(mE, q.ne);
+  }
+  // inputs; outputs: the two pose buffers first, so that the initial guess in the first one goes up with the inputs
+  StagedLayout L;
+  const size_t iProb = L.take_in(sizeof(PgoProb) * P), iBig = L.take_in(sizeof(GbbBig) * P),
+               iCtl = L.take_in(sizeof(PgoCtl) * P), iFrom = L.take_in(4 * tE), iTo = L.take_in(4 * tE),
+               iZ = L.take_in(128 * tE), iFidx = L.take_in(4 * tV), iRc = L.take_in(8 * tB),
+               iStart = L.take_in(4 * (tB + P)), iItem = L.take_in(4 * tI);
+  const size_t oX = L.take_out(256 * tV), oRed = L.take_out(32 * (size_t)P);
+  const size_t wE = L.take_work(48 * tE), wJi = L.take_work(288 * tE), wJj = L.take_work(288 * tE),
+               wCe = L.take_work(8 * tE), wS = L.take_work(8 * tS), wB = L.take_work(48 * tF), wG = L.take_work(48 * tF),
+               wY = L.take_work(48 * tF), wX = L.take_work(48 * tF), wDot = L.take_work(8 * tF), wBad = L.take_work(tF),
+               wWp = L.take_work(8 * tWp), wNz = L.take_work(tNz);
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  const int n = 6 * nf, nt = (n + PLF_LDLT_TILE - 1) / PLF_LDLT_TILE;
-  PgoDev d;
-  d.nv = nv; d.ne = ne; d.nf = nf; d.nb = nb;
-  int *dFrom, *dTo, *dFidx, *dRc, *dStart, *dItem;
-  double *dZ, *dWp;
-  uint8_t* dNz;
-  const size_t one = 1;
-  DevBufList scr;
-  scr.add(dFrom, std::max((size_t)ne, one)); scr.add(dTo, std::max((size_t)ne, one));
-  scr.add(dZ, std::max((size_t)ne, one) * 16); scr.add(dFidx, std::max((size_t)nv, one));
-  scr.add(d.X, std::max((size_t)nv, one) * 16); scr.add(d.Xt, std::max((size_t)nv, one) * 16);
-  scr.add(d.e, std::max((size_t)ne, one) * 6); scr.add(d.Ji, std::max((size_t)ne, one) * 36);
-  scr.add(d.Jj, std::max((size_t)ne, one) * 36); scr.add(d.ce, std::max((size_t)ne, one));
-  scr.add(dRc, std::max((size_t)nb, one) * 2); scr.add(dStart, (size_t)nb + 1); scr.add(dItem, std::max((size_t)nit, one));
-  scr.add(d.S, std::max((size_t)n * n, one));
-  scr.add(d.b, std::max((size_t)n, one)); scr.add(d.g, std::max((size_t)n, one));
-  scr.add(d.y, std::max((size_t)n, one)); scr.add(d.x, std::max((size_t)n, one));
-  scr.add(d.dotp, std::max((size_t)nf, one)); scr.add(d.bad, std::max((size_t)nf, one)); scr.add(d.red, 4);
-  scr.add(dWp, std::max((size_t)nt, one) * PLF_LDLT_TILE * PLF_LDLT_TILE); scr.add(dNz, std::max((size_t)nt * nt, one));
-  if (plf_status st = scr.carve(ctx, PLF_SCR_BA)) return st;
-  out->scratch_bytes = scr.bytes();
-  d.efrom = dFrom; d.eto = dTo; d.Z = dZ; d.fidx = dFidx; d.blk_rc = dRc; d.blk_start = dStart; d.blk_item = dItem;
-  cudaStream_t cs = ctx->stream;
-  if (ne) {
-    PLF_CUDA(ctx, cudaMemcpyAsync(dFrom, p->from, (size_t)ne * 4, cudaMemcpyHostToDevice, cs));
-    PLF_CUDA(ctx, cudaMemcpyAsync(dTo, p->to, (size_t)ne * 4, cudaMemcpyHostToDevice, cs));
-    PLF_CUDA(ctx, cudaMemcpyAsync(dZ, p->Z, (size_t)ne * 128, cudaMemcpyHostToDevice, cs));
-  }
-  if (nv) {
-    PLF_CUDA(ctx, cudaMemcpyAsync(dFidx, fidx.data(), (size_t)nv * 4, cudaMemcpyHostToDevice, cs));
-    PLF_CUDA(ctx, cudaMemcpyAsync(d.X, X.data(), (size_t)nv * 128, cudaMemcpyHostToDevice, cs));
-  }
-  PLF_CUDA(ctx, cudaMemcpyAsync(dRc, blk_rc.data(), (size_t)std::max(nb, 1) * 8, cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(dStart, blk_start.data(), (size_t)(nb + 1) * 4, cudaMemcpyHostToDevice, cs));
-  if (nit) PLF_CUDA(ctx, cudaMemcpyAsync(dItem, blk_item.data(), (size_t)nit * 4, cudaMemcpyHostToDevice, cs));
-  double h_red[4];
-  // chi2 at `Xp` (and, for a trial, the step's two other sums of nf free vertices) into h_red
-  auto evaluate = [&](const double* Xp, int nf_sums) -> plf_status {
-    if (ne) {
-      k_pgo_edge_chi2<<<(ne + 127) / 128, 128, 0, cs>>>(d, Xp);
-      PLF_LAUNCH_CHECK(ctx);
+  uint8_t *pin, *dev;
+  if (plf_status st = L.acquire(ctx, PLF_SCR_BA, &pin, &dev)) return st;
+  PgoCtl* ctl = (PgoCtl*)(pin + iCtl);
+  double* Xpin = (double*)(pin + L.in + oX);
+  const double* red = (const double*)(pin + L.in + oRed);
+  for (int k = 0; k < P; ++k) {
+    const plf_pgo_problem& p = problems[k];
+    const PgoProb& q = hp[k];
+    if (q.ne) {
+      memcpy((int*)(pin + iFrom) + q.eo, p.from, 4 * (size_t)q.ne);
+      memcpy((int*)(pin + iTo) + q.eo, p.to, 4 * (size_t)q.ne);
+      memcpy((double*)(pin + iZ) + 16 * q.eo, p.Z, 128 * (size_t)q.ne);
     }
-    k_pgo_reduce<<<1, PGO_RED, 0, cs>>>(d, nf_sums);
-    PLF_LAUNCH_CHECK(ctx);
-    PLF_CUDA(ctx, cudaMemcpyAsync(h_red, d.red, 32, cudaMemcpyDeviceToHost, cs));
+    if (q.nv) {
+      memcpy((int*)(pin + iFidx) + q.vo, h[k].fidx.data(), 4 * (size_t)q.nv);
+      memcpy(Xpin + 16 * q.vo, h[k].X.data(), 128 * (size_t)q.nv);
+    }
+    if (q.nb) memcpy((int*)(pin + iRc) + 2 * q.bo, h[k].blk_rc.data(), 8 * (size_t)q.nb);
+    memcpy((int*)(pin + iStart) + q.bo + k, h[k].blk_start.data(), 4 * ((size_t)q.nb + 1));
+    if (!h[k].blk_item.empty()) memcpy((int*)(pin + iItem) + q.io, h[k].blk_item.data(), 4 * h[k].blk_item.size());
+    ctl[k] = PgoCtl{opts->lambda_init, 1, 0, 0, 0};
+  }
+  memcpy(pin + iProb, hp.data(), sizeof(PgoProb) * P);
+  memcpy(pin + iBig, hb.data(), sizeof(GbbBig) * P);
+  h.clear();
+  cudaStream_t cs = ctx->stream;
+  static_assert(sizeof(PgoCtl) % sizeof(int) == 0, "gbb_view reads PgoCtl::active as a strided int");
+  PLF_CUDA(ctx, cudaMemcpyAsync(dev, pin, L.in + 128 * tV, cudaMemcpyHostToDevice, cs));   // oX == 0
+  uint8_t* const dout = dev + L.in;
+  uint8_t* const dwork = dout + L.out;
+  PgoBatch B;
+  B.prob = (const PgoProb*)(dev + iProb); B.ctl = (const PgoCtl*)(dev + iCtl);
+  B.efrom = (const int*)(dev + iFrom); B.eto = (const int*)(dev + iTo); B.Z = (const double*)(dev + iZ);
+  B.fidx = (const int*)(dev + iFidx);
+  B.X = (double*)(dout + oX); B.xpar = 16 * tV;
+  B.e = (double*)(dwork + wE); B.Ji = (double*)(dwork + wJi); B.Jj = (double*)(dwork + wJj); B.ce = (double*)(dwork + wCe);
+  B.blk_rc = (const int*)(dev + iRc); B.blk_start = (const int*)(dev + iStart); B.blk_item = (const int*)(dev + iItem);
+  B.S = (double*)(dwork + wS); B.b = (double*)(dwork + wB); B.g = (double*)(dwork + wG); B.y = (double*)(dwork + wY);
+  B.x = (double*)(dwork + wX); B.dotp = (double*)(dwork + wDot); B.bad = dwork + wBad; B.red = (double*)(dout + oRed);
+  const GbbLdlt gl{(const GbbBig*)(dev + iBig), (const int*)(dev + iCtl + offsetof(PgoCtl, active)),
+                   (int)(sizeof(PgoCtl) / sizeof(int)), B.S, B.g, B.y, B.x, (double*)(dwork + wWp), dwork + wNz, {}};
+  const size_t bytes = L.in + L.out + L.work;
+  for (int k = 0; k < P; ++k) out[k].scratch_bytes = bytes;
+  auto blocks = [](long long n, int per) { return (unsigned)((n + per - 1) / per); };
+  // the round's sums of every problem to the host
+  auto sums = [&]() -> plf_status {
+    PLF_CUDA(ctx, cudaMemcpyAsync(pin + L.in + oRed, B.red, 32 * (size_t)P, cudaMemcpyDeviceToHost, cs));
     PLF_CUDA(ctx, cudaStreamSynchronize(cs));
     return PLF_OK;
   };
-  plf_status st;
-  if ((st = evaluate(d.X, 0))) return st;
-  double chi = h_red[0], lambda = opts->lambda_init;
-  out->chi2_init = chi;
-  out->iters = 0; out->stop = PLF_PGO_STOP_MAX_ITERS; out->trials = 0; out->n_trace = 0;
-  // ---- g2o's OptimizationAlgorithmLevenberg::solve, once per iteration (nothing to optimise without free vertices)
-  double ni = 2.0;   // g2o's _ni is a double: it doubles on every rejected trial and must reach lambda's overflow
-  for (int iter = 0; nf && iter < opts->max_iters; ++iter) {
-    k_pgo_linearize<<<(ne + 127) / 128, 128, 0, cs>>>(d);
+  // ---- round 0: the initial chi2 of every problem
+  if (mE) {
+    k_pgo_edge_chi2<<<dim3(blocks(mE, 128), P), 128, 0, cs>>>(B, 0);
     PLF_LAUNCH_CHECK(ctx);
-    int trials = 0;
-    double rho = 0.0;
-    do {
-      PLF_CUDA(ctx, cudaMemsetAsync(d.S, 0, (size_t)n * n * 8, cs));
-      k_pgo_assemble<<<nb, 64, 0, cs>>>(d, lambda);
-      PLF_LAUNCH_CHECK(ctx);
-      if ((st = plf_ldlt_tiled(ctx, cs, nf, d.S, d.g, d.y, d.x, dWp, dNz))) return st;
-      k_pgo_step<<<(nv + 127) / 128, 128, 0, cs>>>(d, lambda);
-      PLF_LAUNCH_CHECK(ctx);
-      if ((st = evaluate(d.Xt, nf))) return st;
-      const double chi_t = h_red[2] != 0.0 ? 1.7976931348623157e308 : h_red[0];   // failed solve: DBL_MAX
-      rho = (chi - chi_t) / (h_red[1] + 1e-3);
-      const bool accept = rho > 0.0 && isfinite(chi_t);
-      if (out->n_trace < out->trace_cap) {
-        plf_pgo_trial& tr = out->trace[out->n_trace++];
-        tr.iter = iter; tr.accepted = accept; tr.lambda = lambda; tr.chi = chi; tr.chi_t = chi_t; tr.rho = rho;
-      }
-      if (accept) {
-        const double alpha = std::min(1.0 - pow(2.0 * rho - 1.0, 3), 2.0 / 3.0);
-        lambda *= std::max(1.0 / 3.0, alpha);
-        ni = 2;
-        std::swap(d.X, d.Xt);
-        chi = chi_t;
-      } else {
-        lambda *= ni;
-        ni *= 2;
-      }
-      ++trials;
-    } while (rho < 0.0 && trials < 10);
-    out->iters = iter + 1;
-    out->trials += trials;
-    if (trials == 10 || rho == 0.0 || !isfinite(lambda)) {
-      out->stop = trials == 10 ? PLF_PGO_STOP_TRIALS : (rho == 0.0 ? PLF_PGO_STOP_RHO_ZERO : PLF_PGO_STOP_LAMBDA);
-      break;
-    }
   }
-  if (nv) {
-    PLF_CUDA(ctx, cudaMemcpyAsync(p->T, d.X, (size_t)nv * 128, cudaMemcpyDeviceToHost, cs));
+  k_pgo_reduce<<<dim3(1, P), PGO_RED, 0, cs>>>(B, 0);
+  PLF_LAUNCH_CHECK(ctx);
+  if (plf_status st = sums()) return st;
+  std::vector<PgoLm> s(P);
+  for (int k = 0; k < P; ++k) {
+    s[k].chi = red[4 * k];
+    s[k].lambda = opts->lambda_init;
+    s[k].running = hp[k].nf && opts->max_iters > 0;   // nothing to optimise without free vertices
+    plf_pgo_result& o = out[k];
+    o.chi2_init = s[k].chi;
+    o.iters = 0; o.stop = PLF_PGO_STOP_MAX_ITERS; o.trials = 0; o.n_trace = 0;
+  }
+  // ---- one trial of every running problem per round
+  for (;;) {
+    int rE = 0, rV = 0, rB = 0, rN = 0, running = 0, last = 0;
+    bool lin = false;
+    for (int k = 0; k < P; ++k) {
+      const PgoLm& sk = s[k];
+      ctl[k] = PgoCtl{sk.lambda, sk.running, sk.running && sk.trials == 0, sk.cur, 0};
+      if (!sk.running) continue;
+      ++running;
+      last = k;
+      lin |= sk.trials == 0;
+      rE = std::max(rE, hp[k].ne); rV = std::max(rV, hp[k].nv); rB = std::max(rB, hp[k].nb);
+      rN = std::max(rN, 6 * hp[k].nf);
+    }
+    if (!running) break;
+    PLF_CUDA(ctx, cudaMemcpyAsync(dev + iCtl, ctl, sizeof(PgoCtl) * P, cudaMemcpyHostToDevice, cs));
+    if (lin) {
+      k_pgo_linearize<<<dim3(blocks(rE, 128), P), 128, 0, cs>>>(B);
+      PLF_LAUNCH_CHECK(ctx);
+    }
+    k_pgo_zero<<<dim3((unsigned)std::min<long long>(2048, blocks((long long)rN * rN, 256)), P), 256, 0, cs>>>(B);
+    PLF_LAUNCH_CHECK(ctx);
+    k_pgo_assemble<<<dim3(rB, P), 64, 0, cs>>>(B);
+    PLF_LAUNCH_CHECK(ctx);
+    // the factorisation reads a table entry and a flag per CTA only where it must: one running problem passes its entry
+    // by value (every round of plf_pose_graph), and a round in which every problem runs needs no flags
+    GbbLdlt gr = gl;
+    if (running == 1) { gr.big = nullptr; gr.one = hb[last]; gr.active = nullptr; }
+    else if (running == P) gr.active = nullptr;
+    if (plf_status st = gbb_ldlt(ctx, cs, gr, running == 1 ? 1 : P, rN)) return st;
+    k_pgo_step<<<dim3(blocks(rV, 128), P), 128, 0, cs>>>(B);
+    PLF_LAUNCH_CHECK(ctx);
+    k_pgo_edge_chi2<<<dim3(blocks(rE, 128), P), 128, 0, cs>>>(B, 1);
+    PLF_LAUNCH_CHECK(ctx);
+    k_pgo_reduce<<<dim3(1, P), PGO_RED, 0, cs>>>(B, 1);
+    PLF_LAUNCH_CHECK(ctx);
+    if (plf_status st = sums()) return st;
+    for (int k = 0; k < P; ++k)
+      if (s[k].running) pgo_decide(s[k], red + 4 * k, opts->max_iters, out[k]);
+  }
+  // ---- the estimates back: both pose buffers in one copy, each problem's from the one holding its estimate
+  if (tV) {
+    PLF_CUDA(ctx, cudaMemcpyAsync(Xpin, B.X, 256 * (size_t)tV, cudaMemcpyDeviceToHost, cs));
     PLF_CUDA(ctx, cudaStreamSynchronize(cs));
   }
-  out->chi2 = chi;
-  out->lambda = lambda;
+  for (int k = 0; k < P; ++k) {
+    if (hp[k].nv) memcpy(problems[k].T, Xpin + s[k].cur * 16 * tV + 16 * hp[k].vo, 128 * (size_t)hp[k].nv);
+    out[k].chi2 = s[k].chi;
+    out[k].lambda = s[k].lambda;
+  }
   return PLF_OK;
+}
+
+}  // namespace
+
+extern "C" plf_status plf_pose_graph(plf_ctx* ctx, const plf_pgo_opts* opts, const plf_pgo_problem* p, plf_pgo_result* out) {
+  if (!ctx || !opts || !p || !out || p->n_v < 0 || p->n_e < 0 || opts->max_iters < 0 || out->trace_cap < 0 ||
+      (out->trace_cap && !out->trace))
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_pose_graph: bad arguments");
+  return pgo_run(ctx, opts, 1, p, out, false);
+}
+
+extern "C" plf_status plf_pose_graph_batch(plf_ctx* ctx, const plf_pgo_opts* opts, int n_problems,
+                                           const plf_pgo_problem* problems, plf_pgo_result* out) {
+  return pgo_run(ctx, opts, n_problems, problems, out, true);
 }

@@ -29,7 +29,7 @@ enum plf_scratch_slot {
   PLF_SCR_ORB,         // plf_orb
   PLF_SCR_LSD,         // plf_lsd, plf_detect_lines, plf_debug_sincosf
   PLF_SCR_MGB_PIPE,    // the windowed matcher of plf_batch_run (matching_strategy != 0)
-  PLF_SCR_BA,          // plf_local_ba, plf_global_ba, plf_pose_graph
+  PLF_SCR_BA,          // plf_local_ba, plf_global_ba, plf_pose_graph, plf_pose_graph_batch
   PLF_SCR_KF,          // plf_match_kf2kf, plf_match_map2kf and their _batch forms: their staged layout
   PLF_SCR_KF_MGB_PT,   // plf_match_kf2kf, plf_match_map2kf and their _batch forms: the windowed matcher of points
   PLF_SCR_KF_MGB_LS,   //   ... and of lines
@@ -240,6 +240,23 @@ plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs
 constexpr int PLF_LDLT_TILE = 64;
 plf_status plf_ldlt_tiled(plf_ctx* ctx, cudaStream_t cs, int n6, double* S, double* g, double* y, double* x, double* Wp,
                           uint8_t* nz);
+// The same factorisation and solve of many systems at once (plf_global_ba_batch, plf_pose_graph_batch,
+// plf_debug_ldlt_batch): one launch per stage and tile column over the nb systems of `big`, gridded (tile, system) at the
+// largest one's n_max rows.  Each system is factored and solved bit for bit as plf_ldlt_tiled would, with its own Wp and
+// zero flags.  System i is skipped when active[big[i].p * active_stride] is 0 (active NULL: none is).  With big NULL
+// the one system is `one` (nb = 1), read from the kernels' parameters: nothing is loaded before the factorisation's own
+// data, as in plf_ldlt_tiled.
+struct GbbBig {
+  int p, nkf;                     // the system's problem index in its batch and its block count (n = 6 nkf rows)
+  long long so, go, xo, wo, zo;   // offsets into S, g / y, x (doubles), Wp (doubles) and the zero flags (bytes)
+};
+struct GbbLdlt {
+  const GbbBig* big;
+  const int* active; int active_stride;   // the problems' activity flags, every active_stride ints, or NULL
+  double* S; double* g; double* y; double* x; double* Wp; uint8_t* nz;
+  GbbBig one;   // the system when big is NULL
+};
+plf_status gbb_ldlt(plf_ctx* ctx, cudaStream_t cs, const GbbLdlt& L, int nb, int n_max);
 
 // ---- ORB (orb.cu) --------------------------------------------------------------------------------
 // A working state for up to nimg images of w x h, with outputs once or per batch parity (two_parities).  On failure

@@ -763,6 +763,32 @@ class Frontend:
         synth.pose_graph_problem or oracle.pgo.cov_graph_lists give it.  Returns dict(T, iters, stop (PGO_STOP's names),
         trials, chi2_init, chi2, lambda_, scratch_bytes, trace: a PGO_TRACE_DTYPE array with one row per trial when
         `trace`)."""
+        p, a = self._pgo_args(prob, max_iters, trace)
+        o = plf_pgo_opts(int(max_iters), float(lambda_init))
+        res = plf_pgo_result(trace=a["trace"].ctypes.data if len(a["trace"]) else None, trace_cap=len(a["trace"]))
+        self._check(self.lib.plf_pose_graph(self._ctx, C.byref(o), C.byref(p), C.byref(res)), "plf_pose_graph")
+        return self._pgo_result(a, res, trace)
+
+    def pose_graph_batch(self, problems, max_iters=100, lambda_init=1e-10, trace=True):
+        """Many pose graphs in one device call (plf_pose_graph_batch), with one max_iters / lambda_init for all of them.
+        problems: dicts as pose_graph takes.  Returns one dict per problem in pose_graph's shape, each bit-identical to
+        what pose_graph returns for that problem alone.  Raises PlfError for the refusals (nothing is computed then)."""
+        problems = list(problems)
+        P = len(problems)
+        args = [self._pgo_args(p, max_iters, trace) for p in problems]
+        arr = (plf_pgo_problem * max(P, 1))(*[p for p, _ in args])
+        res = (plf_pgo_result * max(P, 1))()
+        for k, (_, a) in enumerate(args):
+            res[k].trace = a["trace"].ctypes.data if len(a["trace"]) else None
+            res[k].trace_cap = len(a["trace"])
+        o = plf_pgo_opts(int(max_iters), float(lambda_init))
+        self._check(self.lib.plf_pose_graph_batch(self._ctx, C.byref(o), P, arr, res), "plf_pose_graph_batch")
+        return [self._pgo_result(a, res[k], trace) for k, (_, a) in enumerate(args)]
+
+    @staticmethod
+    def _pgo_args(prob, max_iters, trace):
+        """(plf_pgo_problem, arrays): a copy of the problem's poses, which the call updates in place, its other arrays and
+        a trace of 10 max_iters rows (none without `trace`), and the struct that points at them."""
         T = np.ascontiguousarray(prob["T"], np.float64).reshape(-1, 16).copy()
         fixed = np.ascontiguousarray(prob["fixed"], np.uint8).ravel()
         frm = np.ascontiguousarray(prob["from"], np.int32).ravel()
@@ -770,14 +796,15 @@ class Frontend:
         Z = np.ascontiguousarray(prob["Z"], np.float64).reshape(-1, 16)
         ad = lambda a: a.ctypes.data if a.size else None
         p = plf_pgo_problem(len(T), len(frm), ad(T), ad(fixed), ad(frm), ad(to), ad(Z))
-        o = plf_pgo_opts(int(max_iters), float(lambda_init))
         tr = np.zeros(max(10 * int(max_iters), 1) if trace else 0, PGO_TRACE_DTYPE)
-        res = plf_pgo_result(trace=ad(tr), trace_cap=len(tr))
-        self._check(self.lib.plf_pose_graph(self._ctx, C.byref(o), C.byref(p), C.byref(res)), "plf_pose_graph")
-        out = dict(T=T.reshape(-1, 4, 4), iters=res.iters, stop=PGO_STOP[res.stop], trials=res.trials,
+        return p, dict(T=T, fixed=fixed, frm=frm, to=to, Z=Z, trace=tr)
+
+    @staticmethod
+    def _pgo_result(a, res, trace):
+        out = dict(T=a["T"].reshape(-1, 4, 4), iters=res.iters, stop=PGO_STOP[res.stop], trials=res.trials,
                    chi2_init=res.chi2_init, chi2=res.chi2, lambda_=res.lambda_, scratch_bytes=res.scratch_bytes)
         if trace:
-            out["trace"] = tr[:res.n_trace].copy()
+            out["trace"] = a["trace"][:res.n_trace].copy()
         return out
 
     def match_kf2kf(self, prev, curr, DT, fast_matching=True, max_kf_epip_p=1.0, max_kf_epip_l=1.0):
