@@ -972,6 +972,68 @@ plf_status plf_bow_get_seq(plf_ctx* ctx, int s, int kf_idx, int kind, int cap, u
  * (INTEGRATION.md section 4a).  0 <= s < n, else PLF_ERR_INVALID; the next insert into s may start again at kf_idx 0. */
 plf_status plf_bow_clear_sequence(plf_ctx* ctx, int s);
 
+/* Loop-closure candidate detection (SURVEY 8(f) f5): the score combination of MapHandler::insertKFBowVectorP / L / PL
+ * (src/mapHandler.cpp:3007-3128) and lookForLoopCandidates (:3130-3190), fused behind the insert and scoring of
+ * plf_bow_insert_batch.  The options are the SlamConfig values lookForLoopCandidates reads. */
+typedef struct plf_lc_detect_opts {
+  int lc_kf_dist;        /* SlamConfig::lcKFDist     src/slamConfig.cpp:80 (50) */
+  int lc_kf_max_dist;    /* lcKFMaxDist              :81 (50) */
+  int lc_nkf_closest;    /* lcNKFClosest             :82 (4)  */
+  int min_lm_cov_graph;  /* minLMCovGraph            :61 (75) */
+  int min_kf_local_map;  /* minKFLocalMap            :62 (3)  */
+} plf_lc_detect_opts;
+
+typedef struct plf_lc_detect_result {
+  int candidate;     /* kf_prev_idx, or -1 when lookForLoopCandidates returns false */
+  int best;          /* idx_max (first of the sorted list), -1 when the list is not sorted */
+  int n_listed;      /* max_confmat.size() */
+  int n_closest;     /* Nkf_closest (0 when not evaluated) */
+  double min_score;  /* lc_min_score; NaN when the list is not sorted (the reference never computes it then) */
+} plf_lc_detect_result;
+
+typedef struct plf_lc_detect_problem {
+  int kf_idx;                   /* as plf_bow_problem */
+  const plf_frame_view* kf;     /* read: n_pt, n_ls, pdesc, ldesc, pt_pl, ls_spl, ls_epl */
+  const uint32_t* covis;        /* [kf_idx]: full_graph[kf_idx][i] (symmetric), or NULL = all zero */
+  float* conf;                  /* out [kf_idx+1] or NULL: conf_matrix[kf_idx][i]; NaN where absent */
+  double* score_p, *score_l;    /* out or NULL, exactly as plf_bow_problem */
+  plf_lc_detect_result result;  /* out */
+} plf_lc_detect_problem;
+
+/* plf_bow_insert_batch, then per problem the conf_matrix column of its keyframe and lookForLoopCandidates on it, in one
+ * upload, five launches whatever the batch size, one download and one host synchronisation.
+ *   - Insert and score: exactly plf_bow_insert_batch (its refusals, its database state afterwards, bit-identical rows
+ *     and stored vectors).  The rows stay on the device; only those requested (score_p / score_l not NULL) come back.
+ *   - conf[i] for every live i <= kf_idx, as insertKFBowVector* writes conf_matrix[kf_idx][i], by has_points /
+ *     has_lines: P only (float)score_p; L only (float)score_l; both: score = 0.0; score += (sp n_pt + sl n_ls) / n_pl;
+ *     score += (sp std_pt + sl std_ls) / std_pl, in double in that order, rounded to float.  std_pt = stdv(pt_pl x) +
+ *     stdv(pt_pl y) over the n_pt points, std_ls the same over the line midpoints (spl + epl) * 0.5; stdv is stvo-pl's
+ *     vector_stdv (sequential mean, sqrt(sum (x - mean)^2 / (n - 1)), 0 for no element; DESIGN.md 8).  One point or line
+ *     alone, no feature at all or std_pl = 0 make the whole column NaN, and a NaN column yields no candidate.
+ *   - Detection: live i < kf_idx - lc_kf_dist are listed; with more than lc_kf_max_dist of them (a size_t comparison:
+ *     a negative lc_kf_max_dist never passes) lc_min_score is the minimum over i < kf_idx with covis[i] >=
+ *     (unsigned)min_lm_cov_graph or kf_idx - i <= min_kf_local_map + 3 of the scores in (0.001, 1.0) (absent i count as
+ *     0); best is the listed maximum, and Nkf_closest counts the other listed i with |i - best| <= lc_kf_max_dist and
+ *     score >= lc_min_score * 0.8.  Scores go through float and then double, as the reference reads conf_matrix.
+ *   - One deviation: among equal maxima, best is the lowest index.  The reference's std::sort (sort_confmat_by_score)
+ *     orders equal scores stably only below 17 listed keyframes under libstdc++; above that their order is
+ *     implementation-defined.  NaN scores rank below every number (a column is NaN whole, so this only decides
+ *     plf_debug_loop_candidates' inputs).
+ * Refusals: those of plf_bow_insert_batch, and opts NULL (PLF_ERR_INVALID), before any work, naming the problem and the
+ * rule.  A problem with covis NULL has no covisibility; its pt_pl / ls_spl / ls_epl are read only when both kinds are
+ * enabled, and must then be non-NULL where their count is > 0.  A keyframe is live when every enabled kind stores it.  Device scratch (PLF_SCR_BOW) adds 24 bytes per point and 40 per
+ * line, 4 per keyframe index (covis) in, and 13 + 8 per enabled kind per keyframe index of the rows and columns. */
+plf_status plf_bow_detect(plf_ctx* ctx, const plf_lc_detect_opts* opts, plf_lc_detect_problem* problem);  /* context's database */
+plf_status plf_bow_detect_batch(plf_ctx* ctx, const plf_lc_detect_opts* opts, int n_problems,
+                                plf_lc_detect_problem* problems, const int32_t* seq);  /* seq as plf_bow_insert_batch */
+/* The detection kernel of plf_bow_detect_batch on caller-supplied columns, for tests that put a decision exactly on a
+ * threshold: problem p is kf_idx[p] with conf[p] [kf_idx[p] + 1] (conf_matrix[i][kf_idx]), live[p] [kf_idx[p] + 1]
+ * (map_keyframes[i] != NULL) and covis[p] [kf_idx[p]] or NULL.  One upload, one launch, one download.  PLF_ERR_INVALID
+ * for opts or out NULL, n < 0, a kf_idx outside [0, 2^24) or a conf / live NULL; PLF_ERR_CAPACITY for n > 65535. */
+plf_status plf_debug_loop_candidates(plf_ctx* ctx, const plf_lc_detect_opts* opts, int n, const int* kf_idx,
+                                     const float* const* conf, const uint8_t* const* live,
+                                     const uint32_t* const* covis, plf_lc_detect_result* out);
+
 /* Debug: device-clock timeline (ms) of the two most recent batches of the software pipeline: for each, the start/end of
  * the E (extract), G (region growing) and M (match/track/pose) phases relative to the older batch's E start.
  * No reference counterpart (the reference times whole calls with its Timer, app/plslam_dataset.cpp:126-132). */

@@ -1,6 +1,7 @@
 // vo_demo — the VO part of the reference's frame loop (app/plslam_dataset.cpp:111-163) on top of the C++ shim.
 // Usage: vo_demo <frames.bin> [orb_nfeatures lsd_nfeatures] [--grid-selftest | --kf-match-selftest |
-//                                                            --bow-selftest <voc_p.yml> <voc_l.yml>]
+//                                                            --bow-selftest <voc_p.yml> <voc_l.yml> |
+//                                                            --lc-detect-selftest <voc_p.yml> <voc_l.yml>]
 //        vo_demo --gba-selftest <problem.bin>
 //        vo_demo --pgo-selftest <map.bin>
 // frames.bin: int32 n, w, h; double fx, fy, cx, cy, b; then n x (left h*w bytes, right h*w bytes).
@@ -260,6 +261,76 @@ static void bow_selftest_frame(BowMap& m, StVO::StereoFrame* cur, int frame_coun
     bow_erase(m, 1);
     delete m.map_keyframes[1];
     m.map_keyframes[1] = nullptr;
+  }
+}
+
+// ---- INTEGRATION.md §4 f8: loop-candidate detection (the text between the two markers is the snippet shown there) ----
+// What it reads beyond f5's BowMap: full_graph (include/mapHandler.h:145) and the SlamConfig values lookForLoopCandidates
+// reads; the keyframe's stereo_pt[i]->pl and stereo_ls[i]->spl / epl (the rows of pdesc_l / ldesc_l).
+struct LcMap {
+  BowMap bow;
+  std::vector<std::vector<unsigned int>> full_graph;
+  int lc_kf_dist, lc_kf_max_dist, lc_nkf_closest, min_lm_cov_graph, min_kf_local_map;   // SlamConfig::lcKFDist() ...
+};
+// BEGIN f8
+// insertKFBowVectorP / L / PL (:3007-3128) and lookForLoopCandidates (:3130-3190) in one call.  Call it where the
+// reference calls lookForLoopCandidates, once full_graph holds the keyframe's covisibility: loopClosureThread() right
+// after the insert (:1144-1154), loopClosure() at :2950 with the insert of addKeyFrame (:196-202) removed (nothing in
+// between reads conf_matrix or descDBoW_*, while the local BA may still lower full_graph).  Returns kf_prev_idx or -1.
+static int lc_detect(LcMap& m, KeyFrame* kf) {
+  const StVO::StereoFrame* sf = kf->stereo_frame;
+  const int idx = kf->kf_idx;
+  std::vector<double> pt_pl, ls_spl, ls_epl;                 // row i of pdesc_l <-> stereo_pt[i], of ldesc_l <-> stereo_ls[i]
+  for (const StVO::PointFeature* pt : sf->stereo_pt) { pt_pl.push_back(pt->pl(0)); pt_pl.push_back(pt->pl(1)); }
+  for (const StVO::LineFeature* ls : sf->stereo_ls) {
+    ls_spl.push_back(ls->spl(0)); ls_spl.push_back(ls->spl(1));
+    ls_epl.push_back(ls->epl(0)); ls_epl.push_back(ls->epl(1));
+  }
+  plf_frame_view v = {};
+  v.n_pt = sf->pdesc_l.rows; v.pdesc = const_cast<uint8_t*>(sf->pdesc_l.ptr<uint8_t>()); v.pt_pl = pt_pl.data();
+  v.n_ls = sf->ldesc_l.rows; v.ldesc = const_cast<uint8_t*>(sf->ldesc_l.ptr<uint8_t>());
+  v.ls_spl = ls_spl.data(); v.ls_epl = ls_epl.data();
+  std::vector<uint32_t> covis(m.full_graph[idx].begin(), m.full_graph[idx].begin() + idx);   // full_graph[idx][i], i < idx
+  std::vector<float> conf(idx + 1);
+  plf_lc_detect_opts o = {m.lc_kf_dist, m.lc_kf_max_dist, m.lc_nkf_closest, m.min_lm_cov_graph, m.min_kf_local_map};
+  plf_lc_detect_problem pr = {};
+  pr.kf_idx = idx; pr.kf = &v; pr.covis = covis.data(); pr.conf = conf.data();
+  plf_check(m.bow.ctx, plf_bow_detect(m.bow.ctx, &o, &pr), "plf_bow_detect");
+  // conf_matrix as insertKFBowVector* leaves it (only lookForLoopCandidates reads it; keep it for other readers)
+  for (int i = 0; i < idx; i++) {
+    if (m.bow.map_keyframes[i] != NULL) {
+      m.bow.conf_matrix[idx][i] = conf[i];
+      m.bow.conf_matrix[i][idx] = conf[i];
+    }
+  }
+  m.bow.conf_matrix[idx][idx] = conf[idx];
+  return pr.result.candidate;
+}
+// END f8
+
+// `vo_demo frames.bin ... --lc-detect-selftest voc_p.yml voc_l.yml`: every frame becomes keyframe kf_idx = frame index
+// through lc_detect, with full_graph[i][j] = (i j + i + j) mod 40 and options 1, 2, 1, 20, 0 (lcKFDist, lcKFMaxDist,
+// lcNKFClosest, minLMCovGraph, minKFLocalMap) so that short streams reach every step; keyframe 1 is erased after
+// keyframe 2.  Prints each keyframe's conf_matrix row and result, which the Python binding must reproduce.
+static void lc_selftest_frame(LcMap& m, StVO::StereoFrame* cur, int frame_counter) {
+  KeyFrame* kf = new KeyFrame{frame_counter, cur};
+  m.bow.map_keyframes.push_back(kf);
+  const size_t n = m.bow.map_keyframes.size();
+  for (auto& row : m.bow.conf_matrix) row.resize(n, 0.f);        // expandGraphs (:823-835)
+  m.bow.conf_matrix.emplace_back(n, 0.f);
+  for (auto& row : m.full_graph) row.resize(n, 0u);
+  m.full_graph.emplace_back(n, 0u);
+  for (size_t i = 0; i < n; ++i)
+    m.full_graph[n - 1][i] = m.full_graph[i][n - 1] = (unsigned)((i * (n - 1) + i + (n - 1)) % 40);
+  const int cand = lc_detect(m, kf);
+  std::printf("lc conf %d", kf->kf_idx);
+  for (float x : m.bow.conf_matrix[kf->kf_idx]) std::printf(" %.9g", x);
+  std::printf("\nlc cand %d %d\n", kf->kf_idx, cand);
+  kf->stereo_frame = nullptr;
+  if (frame_counter == 2) {
+    bow_erase(m.bow, 1);
+    delete m.bow.map_keyframes[1];
+    m.bow.map_keyframes[1] = nullptr;
   }
 }
 
@@ -685,7 +756,9 @@ int main(int argc, char** argv) {
   if (argc == 3 && std::string(argv[1]) == "--gba-selftest") return gba_selftest(argv[2]);
   if (argc == 3 && std::string(argv[1]) == "--pgo-selftest") return pgo_selftest(argv[2]);
   const char* bow_voc[2] = {nullptr, nullptr};
-  if (argc >= 4 && std::string(argv[argc - 3]) == "--bow-selftest") {
+  bool lc_test = false;
+  if (argc >= 4 && (std::string(argv[argc - 3]) == "--bow-selftest" || std::string(argv[argc - 3]) == "--lc-detect-selftest")) {
+    lc_test = std::string(argv[argc - 3]) == "--lc-detect-selftest";
     bow_voc[0] = argv[argc - 2];
     bow_voc[1] = argv[argc - 1];
     argc -= 3;
@@ -711,6 +784,7 @@ int main(int argc, char** argv) {
     StVO::StereoFrameHandler* StVO_ = new StVO::StereoFrameHandler(&cam_pin, &prm);   // app:109
     KfArrays* first_kf = nullptr;   // --kf-match-selftest: frame 0 against the last frame
     BowMap bow = {StVO_->ctx(), prm.has_points != 0, prm.has_lines != 0, {}, {}};
+    LcMap lc = {bow, {}, 1, 2, 1, 20, 0};
     if (bow_voc[0]) {
       bow_load_vocabulary(bow.ctx, 0, bow_voc[0]);
       bow_load_vocabulary(bow.ctx, 1, bow_voc[1]);
@@ -739,7 +813,8 @@ int main(int argc, char** argv) {
                   StVO_->n_inliers, new_kf ? 1 : 0);
       for (int i = 0; i < 16; ++i) std::printf(" %.17g", cur->Tfw.v[i]);
       std::printf("\n");
-      if (bow_voc[0]) bow_selftest_frame(bow, cur, frame_counter);
+      if (bow_voc[0] && !lc_test) bow_selftest_frame(bow, cur, frame_counter);
+      if (lc_test) lc_selftest_frame(lc, cur, frame_counter);
       if (kf_test && frame_counter == 0) first_kf = new KfArrays(cur);
       if (kf_test && frame_counter == n - 1 && first_kf) {
         KfArrays last_kf(cur);
@@ -749,6 +824,7 @@ int main(int argc, char** argv) {
     }
     delete first_kf;
     for (KeyFrame* kf : bow.map_keyframes) delete kf;
+    for (KeyFrame* kf : lc.bow.map_keyframes) delete kf;
     delete StVO_;
     if (rc) return rc;
   } catch (const std::exception& e) {

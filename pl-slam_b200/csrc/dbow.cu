@@ -14,6 +14,9 @@
 //   k_bow_score      one warp per earlier keyframe of a problem's database: L1Scoring::score (ScoringObject.cpp:23-68), the
 //                    common words' terms summed sequentially in ascending word order; a block-offset table spreads each
 //                    problem's row over blocks in proportion to its length.
+// plf_bow_detect_batch adds two kernels behind these (lookForLoopCandidates and the score combination that feeds it):
+//   k_lc_combine     one block per problem: the four dispersion chains of insertKFBowVectorPL, then the conf column;
+//   k_lc_detect      one block per problem: lookForLoopCandidates as block reductions (plf_debug_loop_candidates too).
 #include <errno.h>
 #include <locale.h>
 #include <math.h>
@@ -570,6 +573,148 @@ __global__ void __launch_bounds__(256) k_bow_score(const BowProb* __restrict__ p
   }
 }
 
+// One problem of loop-candidate detection: k_lc_combine reads the first block and writes conf / live, k_lc_detect reads
+// conf / live / covis and writes res.  plf_debug_loop_candidates fills the second block only.
+struct LcProb {
+  const double* row[2];     // the problem's score rows, device (nullptr: kind disabled)
+  const int2* ent[2];       // its database's index entries per kind: live where nnz >= 0
+  const double2* pt;        // [n_pt] pt_pl
+  const double2* ls;        // [n_ls][2] (spl, epl)
+  int n_pt, n_ls;
+  float* conf;              // [kf_idx + 1]
+  uint8_t* live;            // [kf_idx + 1]
+  const uint32_t* covis;    // [kf_idx] or nullptr (all zero)
+  plf_lc_detect_result* res;
+  int kf_idx;
+};
+
+// stvo-pl's vector_stdv over chain c of a problem (0 / 1: point x / y, 2 / 3: line midpoint x / y): the mean a sequential
+// sum in index order over n, then sqrt(sum of (x - mean) * (x - mean), sequentially, / (n - 1)); 0 for no element.  The
+// file is compiled with --fmad=false, so no product is contracted into the sums.
+__device__ double lc_stdv(const LcProb& P, int c) {
+  const int n = c < 2 ? P.n_pt : P.n_ls;
+  if (n == 0) return 0.0;
+  auto x = [&](int j) -> double {
+    if (c < 2) return c ? P.pt[j].y : P.pt[j].x;
+    const double2 s = P.ls[2 * j], e = P.ls[2 * j + 1];
+    return c == 3 ? (s.y + e.y) * 0.5 : (s.x + e.x) * 0.5;
+  };
+  double sum = 0.0;
+  for (int j = 0; j < n; ++j) sum += x(j);
+  const double mean = sum / n;
+  double acc = 0.0;
+  for (int j = 0; j < n; ++j) {
+    const double d = x(j) - mean;
+    acc += d * d;
+  }
+  return sqrt(acc / (n - 1));
+}
+
+// conf_matrix[kf_idx][i] of insertKFBowVectorP / L / PL (src/mapHandler.cpp:3018-3029, :3043-3054, :3070-3127): one block
+// per problem.  Threads 0..3 run the four dispersion chains (PL only); every thread then combines entries of the row.
+// live[i]: stored in every enabled kind; conf[i] NaN where not.
+__global__ void __launch_bounds__(256) k_lc_combine(const LcProb* __restrict__ probs, int on_p, int on_l) {
+  __shared__ double s_std[4];
+  const LcProb P = probs[blockIdx.x];
+  const bool pl = on_p && on_l;
+  if (pl && threadIdx.x < 4) s_std[threadIdx.x] = lc_stdv(P, threadIdx.x);
+  __syncthreads();
+  const double std_pt = pl ? s_std[0] + s_std[1] : 0.0, std_ls = pl ? s_std[2] + s_std[3] : 0.0;
+  const double std_pl = std_ls + std_pt;
+  const int n_pl = P.n_pt + P.n_ls;
+  for (int i = threadIdx.x; i <= P.kf_idx; i += blockDim.x) {
+    const bool live = (!on_p || P.ent[0][i].y >= 0) && (!on_l || P.ent[1][i].y >= 0);
+    float c = __int_as_float(0x7FC00000);
+    if (live) {
+      if (!pl) {
+        c = (float)(on_p ? P.row[0][i] : P.row[1][i]);
+      } else {
+        const double sp = P.row[0][i], sl = P.row[1][i];
+        double score = 0.0;
+        score += (sp * P.n_pt + sl * P.n_ls) / n_pl;
+        score += (sp * std_pt + sl * std_ls) / std_pl;
+        c = (float)score;
+      }
+    }
+    P.conf[i] = c;
+    P.live[i] = live;
+  }
+}
+
+__device__ __forceinline__ int lc_block_sum(int v, int* s) {
+  v = __reduce_add_sync(0xFFFFFFFFu, v);
+  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = v;
+  __syncthreads();
+  int t = 0;
+  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += s[w];
+  __syncthreads();
+  return t;
+}
+
+// lookForLoopCandidates (src/mapHandler.cpp:3130-3190) on one column per block.  The listed count, the minimum score,
+// the maximum and the count of close keyframes do not depend on the order of the reference's scans, so they are block
+// reductions.  The maximum is the largest (order-preserving float key, -index): equal maxima go to the lowest index (the
+// one deviation, DESIGN.md 8), -0 counts as +0 and NaN below every number.
+__global__ void __launch_bounds__(256) k_lc_detect(const LcProb* __restrict__ probs, plf_lc_detect_opts o) {
+  __shared__ int s_i[8];
+  __shared__ double s_d[8];
+  __shared__ unsigned long long s_k[8];
+  const LcProb P = probs[blockIdx.x];
+  const int kf = P.kf_idx, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const long long lim = min((long long)kf - o.lc_kf_dist, (long long)kf + 1);   // listed: live i < kf_idx - lcKFDist
+  const long long near = (long long)o.min_kf_local_map + 3;
+  int n_listed = 0;
+  double mn = 1.0;
+  unsigned long long key = 0;
+  for (int i = threadIdx.x; i <= kf; i += blockDim.x) {
+    const bool live = P.live[i];
+    const float f = P.conf[i];
+    const double s = live ? (double)f : 0.0;   // absent: conf_matrix's zero fill
+    if (live && i < lim) {
+      ++n_listed;
+      unsigned u = f == 0.0f ? 0u : __float_as_uint(f);
+      u = isnan(f) ? 0u : (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+      const unsigned long long k = ((unsigned long long)u << 32) | (0xFFFFFFFFu - (unsigned)i);
+      key = k > key ? k : key;
+    }
+    if (i < kf) {
+      const unsigned cov = P.covis ? P.covis[i] : 0u;
+      if ((cov >= (unsigned)o.min_lm_cov_graph || (long long)(kf - i) <= near) && s < mn && s > 0.001) mn = s;
+    }
+  }
+  for (int off = 16; off; off >>= 1) {
+    mn = fmin(mn, __shfl_xor_sync(0xFFFFFFFFu, mn, off));
+    const unsigned long long k = __shfl_xor_sync(0xFFFFFFFFu, key, off);
+    key = k > key ? k : key;
+  }
+  if (lane == 0) { s_d[wid] = mn; s_k[wid] = key; }
+  n_listed = lc_block_sum(n_listed, s_i);   // its barriers publish s_d / s_k
+  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) {
+    mn = fmin(mn, s_d[w]);
+    key = s_k[w] > key ? s_k[w] : key;
+  }
+  // max_confmat.size() > lcKFMaxDist(): a size_t comparison
+  const bool sorted = (unsigned long long)n_listed > (unsigned long long)(long long)o.lc_kf_max_dist;
+  const int best = sorted ? (int)(0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFull)) : -1;
+  const bool eval = sorted && (double)P.conf[best] >= mn;
+  int n_closest = 0;
+  if (eval) {
+    const double th = mn * 0.8;
+    for (int i = threadIdx.x; i < lim; i += blockDim.x)
+      n_closest += i != best && P.live[i] && abs(i - best) <= o.lc_kf_max_dist && (double)P.conf[i] >= th;
+    n_closest = lc_block_sum(n_closest, s_i);
+  }
+  if (threadIdx.x == 0) {
+    plf_lc_detect_result r;
+    r.candidate = eval && n_closest >= o.lc_nkf_closest ? best : -1;
+    r.best = best;
+    r.n_listed = n_listed;
+    r.n_closest = n_closest;
+    r.min_score = sorted ? mn : __longlong_as_double(0x7FF8000000000000ll);
+    *P.res = r;
+  }
+}
+
 // Grows one database kind to hold `more` entries after `end` and keyframe indices up to kf_idx; a first allocation takes
 // at least min_cap entries and min_ent indices.  The caller has checked end + more <= 2^31 - 1.
 plf_status grow_db(plf_ctx* ctx, const char* fn, BowDb& k, size_t more, int kf_idx, size_t min_cap, int min_ent) {
@@ -619,9 +764,17 @@ struct BatchDb {
   size_t next[2] = {0, 0};
 };
 
+// The detection that plf_bow_detect_batch adds to an insert: its options and its problems (parallel to the insert's).
+struct LcDetect {
+  plf_lc_detect_opts opts;
+  plf_lc_detect_problem* probs;
+};
+
 // plf_bow_insert_batch; fn names the entry point in messages, and a call from plf_bow_insert (single) names no problem.
+// det (plf_bow_detect_batch): every enabled kind's row is scored, into device work space where not requested, and two
+// more kernels combine the rows into conf columns and detect the candidates; without det the call is the plain insert.
 plf_status bow_insert_problems(plf_ctx* ctx, const char* fn, bool single, int n_problems, plf_bow_problem* problems,
-                               const int32_t* seq) {
+                               const int32_t* seq, const LcDetect* det = nullptr) {
   char who[96];
   auto name = [&](int p) -> const char* {
     if (single) snprintf(who, sizeof who, "%s", fn);
@@ -674,6 +827,11 @@ plf_status bow_insert_problems(plf_ctx* ctx, const char* fn, bool single, int n_
       b.last[c] = pr.kf_idx;
       b.more[c] += (size_t)n[c];
     }
+    if (det && on[0] && on[1]) {   // the dispersions read the stereo coordinates
+      if (n[0] > 0 && !pr.kf->pt_pl) return plf_fail(ctx, PLF_ERR_INVALID, "%s: pt_pl is NULL with %d points", name(p), n[0]);
+      if (n[1] > 0 && (!pr.kf->ls_spl || !pr.kf->ls_epl))
+        return plf_fail(ctx, PLF_ERR_INVALID, "%s: ls_spl / ls_epl is NULL with %d lines", name(p), n[1]);
+    }
   }
   for (const auto& e : db_at)
     for (int c = 0; c < 2; ++c) {
@@ -711,22 +869,44 @@ plf_status bow_insert_problems(plf_ctx* ctx, const char* fn, bool single, int n_
   const int nf = m[0] + m[1];
   size_t row_b = 0;       // every requested row, packed
   long long row_len = 0;  // the keyframes scored over all problems (one kind)
+  size_t urow_b = 0, col_n = 0, conf_n = 0, ucol_n = 0, covis_b = 0;   // detection: rows kept on the device, columns
   for (int p = 0; p < n_problems; ++p) {
     const plf_bow_problem& pr = problems[p];
     double* rows[2] = {pr.score_p, pr.score_l};
     bool any = false;
     for (int c = 0; c < 2; ++c) {
-      const bool r = on[c] && rows[c];
-      row_b += r ? (size_t)(pr.kf_idx + 1) * 8 : 0;
+      const bool r = on[c] && (rows[c] || det);
+      row_b += r && rows[c] ? (size_t)(pr.kf_idx + 1) * 8 : 0;
+      urow_b += r && !rows[c] ? (size_t)(pr.kf_idx + 1) * 8 : 0;
       any |= r;
     }
     row_len += any ? pr.kf_idx + 1 : 0;
+    if (det) {
+      const plf_lc_detect_problem& dp = det->probs[p];
+      col_n += (size_t)pr.kf_idx + 1;
+      (dp.conf ? conf_n : ucol_n) += (size_t)pr.kf_idx + 1;
+      covis_b += dp.covis ? (size_t)pr.kf_idx * 4 : 0;
+    }
   }
   StagedLayout L;
   const size_t desc_off = L.take_in((size_t)nf * 32), tab_off = L.take_in(sizeof(BowProb) * n_problems),
                boff_off = L.take_in(sizeof(int) * (n_problems + 1));
   const size_t nnz_off = L.take_out(2 * sizeof(int) * n_problems), rows_off = L.take_out(row_b);
   const size_t w_off = L.take_work((size_t)nf * 4), wt_off = L.take_work((size_t)nf * 8);
+  // detection: the coordinates (PL only), the covisibility columns and its table in; the results and the requested
+  // conf columns out; the other rows and columns and the live flags as work
+  const bool disp = det && on[0] && on[1];
+  size_t lc_off = 0, xy_off = 0, covis_off = 0, res_off = 0, conf_off = 0, urow_off = 0, ucol_off = 0, live_off = 0;
+  if (det) {
+    lc_off = L.take_in(sizeof(LcProb) * n_problems);
+    xy_off = L.take_in(disp ? (size_t)(m[0] + 2 * (size_t)m[1]) * 16 : 0);
+    covis_off = L.take_in(covis_b);
+    res_off = L.take_out(sizeof(plf_lc_detect_result) * n_problems);
+    conf_off = L.take_out(conf_n * 4);
+    urow_off = L.take_work(urow_b);
+    ucol_off = L.take_work(ucol_n * 4);
+    live_off = L.take_work(col_n);
+  }
   // the rows grow by 16 bytes per keyframe: 1 MB up front keeps the inserts of the first ~50 000 keyframes from
   // reallocating the slot (a stream synchronisation) every 32 keyframes
   if (!plf_scratch(ctx, PLF_SCR_BOW, (size_t)1 << 20)) return PLF_ERR_CUDA;
@@ -736,6 +916,8 @@ plf_status bow_insert_problems(plf_ctx* ctx, const char* fn, bool single, int n_
   // the problem table; a problem's blocks of k_bow_score in proportion to its row, as one call's grid over one row
   const long long budget = 4LL * S->n_sm;
   size_t feat[2] = {0, (size_t)m[0]}, row_at = 0;
+  size_t urow_at = 0, conf_at = 0, ucol_at = 0, live_at = 0, covis_at = 0, xy_at = 0;
+  std::vector<LcProb> lc(det ? n_problems : 0);
   for (int p = 0; p < n_problems; ++p) {
     const plf_bow_problem& pr = problems[p];
     BatchDb& b = bdb[prob_db[p]];
@@ -756,7 +938,50 @@ plf_status bow_insert_problems(plf_ctx* ctx, const char* fn, bool single, int n_
         K.row = (double*)(out + rows_off + row_at);
         row_at += (size_t)(pr.kf_idx + 1) * 8;
         any = true;
+      } else if (det) {
+        K.row = (double*)(work + urow_off + urow_at);
+        urow_at += (size_t)(pr.kf_idx + 1) * 8;
+        any = true;
       }
+    }
+    if (det) {
+      const plf_lc_detect_problem& dp = det->probs[p];
+      LcProb& q = lc[p];
+      memset(&q, 0, sizeof q);
+      const size_t len = (size_t)pr.kf_idx + 1;
+      for (int c = 0; c < 2; ++c) {
+        q.row[c] = tab[p].k[c].row;
+        q.ent[c] = tab[p].k[c].ent;
+      }
+      if (disp) {
+        double* xy = (double*)(pin + xy_off) + 2 * xy_at;
+        if (n[0]) memcpy(xy, pr.kf->pt_pl, (size_t)n[0] * 16);
+        for (int j = 0; j < n[1]; ++j) {
+          memcpy(xy + 2 * n[0] + 4 * j, pr.kf->ls_spl + 2 * j, 16);
+          memcpy(xy + 2 * n[0] + 4 * j + 2, pr.kf->ls_epl + 2 * j, 16);
+        }
+        q.pt = (const double2*)(dev + xy_off) + xy_at;
+        q.ls = q.pt + n[0];
+        q.n_pt = n[0];
+        q.n_ls = n[1];
+        xy_at += (size_t)n[0] + 2 * (size_t)n[1];
+      }
+      if (dp.conf) {
+        q.conf = (float*)(out + conf_off) + conf_at;
+        conf_at += len;
+      } else {
+        q.conf = (float*)(work + ucol_off) + ucol_at;
+        ucol_at += len;
+      }
+      q.live = work + live_off + live_at;
+      live_at += len;
+      if (dp.covis) {
+        if (pr.kf_idx) memcpy(pin + covis_off + covis_at * 4, dp.covis, (size_t)pr.kf_idx * 4);
+        q.covis = (const uint32_t*)(dev + covis_off) + covis_at;
+        covis_at += (size_t)pr.kf_idx;
+      }
+      q.res = (plf_lc_detect_result*)(out + res_off) + p;
+      q.kf_idx = pr.kf_idx;
     }
     tab[p].kf_idx = pr.kf_idx;
     const long long len = any ? pr.kf_idx + 1 : 0;
@@ -764,6 +989,7 @@ plf_status bow_insert_problems(plf_ctx* ctx, const char* fn, bool single, int n_
   }
   memcpy(pin + tab_off, tab.data(), sizeof(BowProb) * n_problems);
   memcpy(pin + boff_off, boff.data(), sizeof(int) * (n_problems + 1));
+  if (det) memcpy(pin + lc_off, lc.data(), sizeof(LcProb) * n_problems);
   int* d_word = (int*)(work + w_off);
   double* d_wt = (double*)(work + wt_off);
   const BowProb* d_tab = (const BowProb*)(dev + tab_off);
@@ -785,8 +1011,15 @@ plf_status bow_insert_problems(plf_ctx* ctx, const char* fn, bool single, int n_
     k_bow_score<<<dim3(boff[n_problems], 2), 256, 0, cs>>>(d_tab, (const int*)(dev + boff_off), n_problems);
     PLF_LAUNCH_CHECK(ctx);
   }
-  // one download: the counts and the rows
-  PLF_CUDA(ctx, cudaMemcpyAsync(pin + L.in, out, row_b ? rows_off + row_b : nnz_off + 2 * sizeof(int) * n_problems,
+  if (det) {
+    const LcProb* d_lc = (const LcProb*)(dev + lc_off);
+    k_lc_combine<<<n_problems, 256, 0, cs>>>(d_lc, on[0], on[1]);
+    PLF_LAUNCH_CHECK(ctx);
+    k_lc_detect<<<n_problems, 256, 0, cs>>>(d_lc, det->opts);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  // one download: the counts and the rows (and with detection the results and the requested columns after them)
+  PLF_CUDA(ctx, cudaMemcpyAsync(pin + L.in, out, det ? L.out : row_b ? rows_off + row_b : nnz_off + 2 * sizeof(int) * n_problems,
                                 cudaMemcpyDeviceToHost, cs));
   PLF_CUDA(ctx, cudaStreamSynchronize(cs));
   const int* nnz = (const int*)(pin + L.in + nnz_off);
@@ -804,7 +1037,66 @@ plf_status bow_insert_problems(plf_ctx* ctx, const char* fn, bool single, int n_
       k.last = pr.kf_idx;
       if (rows[c]) memcpy(rows[c], pin + L.in + ((uint8_t*)K.row - out), (size_t)(pr.kf_idx + 1) * 8);
     }
+    if (det) {
+      plf_lc_detect_problem& dp = det->probs[p];
+      memcpy(&dp.result, pin + L.in + ((uint8_t*)lc[p].res - out), sizeof(plf_lc_detect_result));
+      if (dp.conf) memcpy(dp.conf, pin + L.in + ((uint8_t*)lc[p].conf - out), (size_t)(pr.kf_idx + 1) * 4);
+    }
   }
+  return PLF_OK;
+}
+
+// plf_debug_loop_candidates: k_lc_detect on the caller's columns.
+plf_status lc_debug(plf_ctx* ctx, const plf_lc_detect_opts* opts, int n, const int* kf_idx, const float* const* conf,
+                    const uint8_t* const* live, const uint32_t* const* covis, plf_lc_detect_result* out) {
+  const char* fn = "plf_debug_loop_candidates";
+  if (!opts || !out) return plf_fail(ctx, PLF_ERR_INVALID, "%s: opts and out are required", fn);
+  if (n < 0) return plf_fail(ctx, PLF_ERR_INVALID, "%s: n = %d < 0", fn, n);
+  if (n > BOW_MAX_PROBLEMS) return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: n = %d exceeds %d", fn, n, BOW_MAX_PROBLEMS);
+  if (n == 0) return PLF_OK;
+  if (!kf_idx || !conf || !live) return plf_fail(ctx, PLF_ERR_INVALID, "%s: kf_idx, conf and live are required", fn);
+  size_t col_n = 0, covis_n = 0;
+  for (int p = 0; p < n; ++p) {
+    if (kf_idx[p] < 0 || kf_idx[p] >= BOW_MAX_KF)
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: kf_idx %d out of range [0, %d)", fn, p, kf_idx[p], BOW_MAX_KF);
+    if (!conf[p] || !live[p]) return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: conf or live is NULL", fn, p);
+    col_n += (size_t)kf_idx[p] + 1;
+    covis_n += covis && covis[p] ? (size_t)kf_idx[p] : 0;
+  }
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  StagedLayout L;
+  const size_t tab_off = L.take_in(sizeof(LcProb) * n), conf_off = L.take_in(col_n * 4), live_off = L.take_in(col_n),
+               covis_off = L.take_in(covis_n * 4);
+  const size_t res_off = L.take_out(sizeof(plf_lc_detect_result) * n);
+  uint8_t *pin, *dev;
+  if (plf_status st = L.acquire(ctx, PLF_SCR_BOW, &pin, &dev)) return st;
+  std::vector<LcProb> tab(n);
+  size_t at = 0, cat = 0;
+  for (int p = 0; p < n; ++p) {
+    LcProb& q = tab[p];
+    memset(&q, 0, sizeof q);
+    const size_t len = (size_t)kf_idx[p] + 1;
+    memcpy(pin + conf_off + at * 4, conf[p], len * 4);
+    memcpy(pin + live_off + at, live[p], len);
+    q.conf = (float*)(dev + conf_off) + at;
+    q.live = dev + live_off + at;
+    at += len;
+    if (covis && covis[p]) {
+      memcpy(pin + covis_off + cat * 4, covis[p], (size_t)kf_idx[p] * 4);
+      q.covis = (const uint32_t*)(dev + covis_off) + cat;
+      cat += (size_t)kf_idx[p];
+    }
+    q.res = (plf_lc_detect_result*)(dev + L.in + res_off) + p;
+    q.kf_idx = kf_idx[p];
+  }
+  memcpy(pin + tab_off, tab.data(), sizeof(LcProb) * n);
+  cudaStream_t cs = ctx->stream;
+  PLF_CUDA(ctx, cudaMemcpyAsync(dev, pin, L.in, cudaMemcpyHostToDevice, cs));
+  k_lc_detect<<<n, 256, 0, cs>>>((const LcProb*)(dev + tab_off), *opts);
+  PLF_LAUNCH_CHECK(ctx);
+  PLF_CUDA(ctx, cudaMemcpyAsync(pin + L.in, dev + L.in, L.out, cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaStreamSynchronize(cs));
+  memcpy(out, pin + L.in + res_off, sizeof(plf_lc_detect_result) * n);
   return PLF_OK;
 }
 
@@ -933,6 +1225,37 @@ plf_status plf_bow_insert(plf_ctx* ctx, int kf_idx, const plf_frame_view* kf, do
 plf_status plf_bow_insert_batch(plf_ctx* ctx, int n_problems, plf_bow_problem* problems, const int32_t* seq) {
   if (!ctx) return PLF_ERR_INVALID;
   return bow_insert_problems(ctx, "plf_bow_insert_batch", false, n_problems, problems, seq);
+}
+
+plf_status plf_bow_detect_batch(plf_ctx* ctx, const plf_lc_detect_opts* opts, int n_problems,
+                                plf_lc_detect_problem* problems, const int32_t* seq) {
+  if (!ctx) return PLF_ERR_INVALID;
+  const char* fn = "plf_bow_detect_batch";
+  if (!opts) return plf_fail(ctx, PLF_ERR_INVALID, "%s: opts is NULL", fn);
+  if (n_problems > 0 && n_problems <= BOW_MAX_PROBLEMS && problems) {
+    std::vector<plf_bow_problem> bp(n_problems);
+    for (int p = 0; p < n_problems; ++p)
+      bp[p] = {problems[p].kf_idx, problems[p].kf, problems[p].score_p, problems[p].score_l};
+    const LcDetect det = {*opts, problems};
+    return bow_insert_problems(ctx, fn, false, n_problems, bp.data(), seq, &det);
+  }
+  return bow_insert_problems(ctx, fn, false, n_problems, nullptr, seq);   // its refusals of n_problems and problems
+}
+
+plf_status plf_bow_detect(plf_ctx* ctx, const plf_lc_detect_opts* opts, plf_lc_detect_problem* problem) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (!opts) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_detect: opts is NULL");
+  if (!problem) return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_detect: problem is NULL");
+  plf_bow_problem bp = {problem->kf_idx, problem->kf, problem->score_p, problem->score_l};
+  const LcDetect det = {*opts, problem};
+  return bow_insert_problems(ctx, "plf_bow_detect", true, 1, &bp, nullptr, &det);
+}
+
+plf_status plf_debug_loop_candidates(plf_ctx* ctx, const plf_lc_detect_opts* opts, int n, const int* kf_idx,
+                                     const float* const* conf, const uint8_t* const* live,
+                                     const uint32_t* const* covis, plf_lc_detect_result* out) {
+  if (!ctx) return PLF_ERR_INVALID;
+  return lc_debug(ctx, opts, n, kf_idx, conf, live, covis, out);
 }
 
 plf_status plf_bow_erase_seq(plf_ctx* ctx, int s, int kf_idx) {

@@ -189,6 +189,31 @@ class plf_bow_problem(C.Structure):
     _fields_ = [("kf_idx", C.c_int), ("kf", C.POINTER(plf_frame_view)), ("score_p", C.c_void_p), ("score_l", C.c_void_p)]
 
 
+class plf_lc_detect_opts(C.Structure):
+    _fields_ = [("lc_kf_dist", C.c_int), ("lc_kf_max_dist", C.c_int), ("lc_nkf_closest", C.c_int),
+                ("min_lm_cov_graph", C.c_int), ("min_kf_local_map", C.c_int)]
+
+
+class plf_lc_detect_result(C.Structure):
+    _fields_ = [("candidate", C.c_int), ("best", C.c_int), ("n_listed", C.c_int), ("n_closest", C.c_int),
+                ("min_score", C.c_double)]
+
+
+class plf_lc_detect_problem(C.Structure):
+    _fields_ = [("kf_idx", C.c_int), ("kf", C.POINTER(plf_frame_view)), ("covis", C.c_void_p), ("conf", C.c_void_p),
+                ("score_p", C.c_void_p), ("score_l", C.c_void_p), ("result", plf_lc_detect_result)]
+
+
+# SlamConfig's loop-closure detection defaults (src/slamConfig.cpp:61-62, :80-82)
+LC_DETECT_DEFAULTS = dict(lc_kf_dist=50, lc_kf_max_dist=50, lc_nkf_closest=4, min_lm_cov_graph=75, min_kf_local_map=3)
+LC_RESULT_FIELDS = ("candidate", "best", "n_listed", "n_closest", "min_score")
+
+
+def _lc_opts(opts):
+    o = dict(LC_DETECT_DEFAULTS, **(opts or {}))
+    return plf_lc_detect_opts(*[int(o[f]) for f, _ in plf_lc_detect_opts._fields_])
+
+
 class plf_vocab(C.Structure):
     _fields_ = [("k", C.c_int), ("L", C.c_int), ("scoring", C.c_int), ("weighting", C.c_int), ("n_nodes", C.c_int),
                 ("node_id", C.c_void_p), ("parent_id", C.c_void_p), ("weight", C.c_void_p), ("desc", C.c_void_p),
@@ -934,6 +959,93 @@ class Frontend:
         self._check(self.lib.plf_bow_insert_batch(self._ctx, P, arr, None if seq_a is None else _ptr(seq_a, C.c_int32)),
                     "plf_bow_insert_batch")
         return outs
+
+    def _lc_problem(self, pr, rows, conf, keep, who):
+        """(plf_lc_detect_problem, (score_p, score_l), conf) over one bow_detect_batch problem dict."""
+        n = {d: 0 if pr.get(d) is None else len(pr[d]) for d in ("pdesc", "ldesc")}
+        for key, desc in (("pt_pl", "pdesc"), ("ls_spl", "ldesc"), ("ls_epl", "ldesc")):
+            if pr.get(key) is not None and np.asarray(pr[key]).size != 2 * n[desc]:
+                raise PlfError(f"{who}: {key} has {np.asarray(pr[key]).size} values for {n[desc]} rows of {desc} "
+                               f"(2 per row)")
+        v = _frame_view({key: pr[key] for key in ("pdesc", "ldesc", "pt_pl", "ls_spl", "ls_epl")
+                         if pr.get(key) is not None}, keep)
+        keep.append(v)
+        kf = int(pr["kf_idx"])
+        enabled = (self.params.has_points, self.params.has_lines)
+        out = [np.full(kf + 1, np.nan) if (rows[c] and enabled[c] and kf >= 0) else None for c in range(2)]
+        cf = np.full(max(kf + 1, 1), np.nan, np.float32) if conf else None
+        cov = pr.get("covis")
+        if cov is not None:
+            cov = np.ascontiguousarray(cov, np.uint32)
+            if len(cov) != max(kf, 0):
+                raise PlfError(f"{who}: covis has {len(cov)} entries for kf_idx {kf}")
+        keep += [out, cf, cov]
+        ad = lambda a: None if a is None or not a.size else a.ctypes.data
+        return (plf_lc_detect_problem(kf, C.pointer(v), ad(cov), ad(cf), ad(out[0]), ad(out[1])), out,
+                None if cf is None else cf[:kf + 1])
+
+    @staticmethod
+    def _lc_result(st, out, cf):
+        r = {f: getattr(st.result, f) for f in LC_RESULT_FIELDS}
+        r.update(conf=cf, score_p=out[0], score_l=out[1])
+        return r
+
+    def bow_detect_batch(self, problems, opts=None, seq=None, rows=(False, False), conf=True):
+        """Many keyframe inserts with loop-candidate detection in one device call (plf_bow_detect_batch).  problems: dicts
+        kf_idx, pdesc, ldesc, pt_pl [n_pt][2], ls_spl / ls_epl [n_ls][2] (the coordinates are read when both kinds are
+        enabled) and optionally covis [kf_idx] (full_graph[kf_idx][i]; missing = all zero); opts: a dict over
+        LC_DETECT_DEFAULTS; seq: as bow_insert_batch.  Returns one dict per problem: the result fields (candidate, best,
+        n_listed, n_closest, min_score), conf float32 [kf_idx + 1] (None unless conf) and score_p / score_l as
+        bow_insert_batch returns them for `rows`."""
+        problems = list(problems)
+        P = len(problems)
+        seq_a = self._problem_sequences(P, seq)
+        keep, outs = [], []
+        arr = (plf_lc_detect_problem * max(P, 1))()
+        for k, pr in enumerate(problems):
+            arr[k], out, cf = self._lc_problem(pr, rows, conf, keep, f"bow_detect_batch: problem {k}")
+            outs.append((out, cf))
+        o = _lc_opts(opts)
+        self._check(self.lib.plf_bow_detect_batch(self._ctx, C.byref(o), P, arr,
+                                                  None if seq_a is None else _ptr(seq_a, C.c_int32)), "plf_bow_detect_batch")
+        return [self._lc_result(arr[k], out, cf) for k, (out, cf) in enumerate(outs)]
+
+    def bow_detect(self, problem, opts=None, rows=(False, False), conf=True):
+        """plf_bow_detect: one bow_detect_batch problem on the context's database (the one bow_insert uses)."""
+        keep = []
+        pr, out, cf = self._lc_problem(problem, rows, conf, keep, "bow_detect")
+        o = _lc_opts(opts)
+        self._check(self.lib.plf_bow_detect(self._ctx, C.byref(o), C.byref(pr)), "plf_bow_detect")
+        return self._lc_result(pr, out, cf)
+
+    def debug_loop_candidates(self, columns, opts=None):
+        """plf_debug_loop_candidates: lookForLoopCandidates on the device over caller columns.  columns: dicts kf_idx,
+        conf float32 [kf_idx + 1], live bool [kf_idx + 1] and optionally covis uint32 [kf_idx].  Returns one result dict
+        per column."""
+        columns = list(columns)
+        n = len(columns)
+        keep = []
+        kf = np.array([int(c["kf_idx"]) for c in columns] or [0], np.int32)
+        pc, pl, pv = (C.c_void_p * max(n, 1))(), (C.c_void_p * max(n, 1))(), (C.c_void_p * max(n, 1))()
+        for k, c in enumerate(columns):
+            m = int(c["kf_idx"]) + 1
+            cf = np.ascontiguousarray(c["conf"], np.float32)
+            lv = np.ascontiguousarray(c["live"], np.uint8)
+            if len(cf) != m or len(lv) != m:
+                raise PlfError(f"debug_loop_candidates: column {k}: conf / live need kf_idx + 1 = {m} entries")
+            keep += [cf, lv]
+            pc[k], pl[k] = cf.ctypes.data, lv.ctypes.data
+            if c.get("covis") is not None:
+                cv = np.ascontiguousarray(c["covis"], np.uint32)
+                if len(cv) != m - 1:
+                    raise PlfError(f"debug_loop_candidates: column {k}: covis needs kf_idx = {m - 1} entries")
+                keep.append(cv)
+                pv[k] = cv.ctypes.data if cv.size else None
+        out = (plf_lc_detect_result * max(n, 1))()
+        o = _lc_opts(opts)
+        self._check(self.lib.plf_debug_loop_candidates(self._ctx, C.byref(o), n, _ptr(kf, C.c_int), pc, pl, pv, out),
+                    "plf_debug_loop_candidates")
+        return [{f: getattr(out[k], f) for f in LC_RESULT_FIELDS} for k in range(n)]
 
     def bow_erase(self, kf_idx, seq=None):
         """plf_bow_erase, or plf_bow_erase_seq on sequence seq's database (-1: the context's)."""
