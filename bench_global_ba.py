@@ -5,10 +5,12 @@ max_iters = 15, DBL_EPSILON stop thresholds).
 
 Per size it reports:
   - device ms per call (CUDA events on plf_stream around the call, median of --timed calls after one warm-up call);
-  - the per-iteration split from torch.profiler (a separate call): rows / landmark blocks (k_lba_rows, k_lba_lm_accum,
-    the diagonal maxima), Schur assembly (k_lba_lm_schur), factorisation (k_lba_solve up to 64 keyframes, which also
-    does the substitutions; k_gba_damp / diag / panel / update beyond), substitution (k_gba_fwd / dscale / bwd), step
-    (k_lba_backsub, k_lba_apply), each summed over the call and divided by the number of solves;
+  - the per-iteration split from torch.profiler (a separate call): rows / landmark blocks (k_lbb_rows, k_lbb_lm_accum,
+    the diagonal maxima), Schur assembly (k_lbb_schur), factorisation (k_lbb_solve up to 64 keyframes, which also does
+    the substitutions; k_gbb_damp / diag / panel / update beyond), substitution (k_gbb_fwd / dscale / bwd), step
+    (k_lbb_backsub, k_lbb_apply), zeroing of the next round's system (k_gbb_zero, memsets), each summed over the call
+    and divided by the number of solves (Schur launches).  Each group also lists the kernels of the earlier driver
+    (k_lba_*, k_gba_*), so that the script times builds from before and after it alike;
   - factorisation FLOPs: n^3 / 3 for a dense LDL^T (n = 6 n_kf), and the count the tiled path executes after skipping
     exactly-zero tiles, from the tile-level symbolic factorisation of the reduced system's pattern (64^3 / 3 per
     diagonal tile, 64^3 per panel tile, 2 * 64^3 per trailing tile update); achieved TFLOP/s = executed FLOPs over the
@@ -37,12 +39,16 @@ from plslam_b200 import synth  # noqa: E402
 
 T = 64
 GROUPS = {
-    "rows_landmark_blocks": ("k_lba_rows", "k_lba_lm_accum", "k_lba_kf_diagmax", "k_gba_hmax_int"),
-    "schur": ("k_lba_lm_schur",),
-    "factorisation": ("k_lba_solve", "k_gba_damp", "k_gba_diag", "k_gba_panel", "k_gba_update"),
-    "substitution": ("k_gba_fwd", "k_gba_dscale", "k_gba_bwd"),
-    "step": ("k_lba_backsub", "k_lba_apply"),
+    "rows_landmark_blocks": ("k_lba_rows", "k_lba_lm_accum", "k_lba_kf_diagmax", "k_gba_hmax_int",
+                             "k_lbb_rows", "k_lbb_lm_accum", "k_lbb_kf_diagmax", "k_gbb_hmax_int"),
+    "schur": ("k_lba_lm_schur", "k_lbb_schur"),
+    "factorisation": ("k_lba_solve", "k_gba_damp", "k_gba_diag", "k_gba_panel", "k_gba_update",
+                      "k_lbb_solve", "k_gbb_damp", "k_gbb_diag", "k_gbb_panel", "k_gbb_update"),
+    "substitution": ("k_gba_fwd", "k_gba_dscale", "k_gba_bwd", "k_gbb_fwd", "k_gbb_dscale", "k_gbb_bwd"),
+    "step": ("k_lba_backsub", "k_lba_apply", "k_lbb_backsub", "k_lbb_apply"),
+    "zero": ("k_gbb_zero", "Memset"),
 }
+SCHUR = GROUPS["schur"]   # one launch per solve
 
 
 def card():
@@ -114,13 +120,13 @@ def main():
                 torch.cuda.synchronize()
             ev = prof.key_averages()
             tot = {g: sum(e.device_time_total for e in ev if any(k in e.key for k in ks)) / 1e3 for g, ks in GROUPS.items()}
-            solves = sum(e.count for e in ev if "k_lba_lm_schur" in e.key)
+            solves = sum(e.count for e in ev if any(k in e.key for k in SCHUR))
             per_iter = {g: v / max(solves, 1) for g, v in tot.items()}
             dense, executed = tile_flops(p)
             fact_s = per_iter["factorisation"] * 1e-3
             entry = dict(n_kf=nkf, n=6 * nkf, n_pt=len(p["pt"]), n_ls=len(p["ls"]),
                          n_obs=int(len(p["pt_obs_lm"]) + len(p["ls_obs_lm"])), N=N, iters=r["iters"], solves=solves,
-                         solver="one CTA (k_lba_solve)" if 6 * nkf <= 384 else "tiled LDL^T (k_gba_*)",
+                         solver="one CTA" if 6 * nkf <= 384 else "tiled LDL^T",
                          device_ms=float(np.median(dev_ms)), wall_ms=float(np.median(wall_ms)),
                          per_iter_ms=per_iter, fact_flop_dense=dense,
                          fact_flop_executed=executed if 6 * nkf > 384 else None,

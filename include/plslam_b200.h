@@ -265,8 +265,9 @@ plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, int h, int 
 plf_status plf_debug_sincosf(plf_ctx* ctx, const float* in, float* s, float* c, int n);
 
 /* Test hook: factors the symmetric n x n matrix S (n = 6 n6, row-major, only its lower triangle is read) as L D L^T
- * without pivoting and solves S x = g, with the factorisation of plf_global_ba / plf_pose_graph (path 0: the tiled one,
- * 1 <= n6 <= 4096) or that of plf_local_ba (path 1: one CTA, 1 <= n6 <= 64).  On return the lower triangle of S holds
+ * without pivoting and solves S x = g, with the factorisation of plf_global_ba / plf_pose_graph beyond 64 keyframes
+ * (path 0: the tiled one, 1 <= n6 <= 4096, as one system on its own) or that of plf_local_ba (path 1: one CTA,
+ * 1 <= n6 <= 64).  On return the lower triangle of S holds
  * L strictly below the diagonal and D on it (entries above the diagonal are unspecified), x the solution, and nz
  * (path 0 only, may be NULL; n_t x n_t bytes, n_t = ceil(n / 64)) the zero flag of each L tile (i > k) as the panel
  * kernel set it, 0 elsewhere.  A bad path, an n6 out of range or a NULL S, g or x returns PLF_ERR_INVALID. */
@@ -399,7 +400,11 @@ typedef struct plf_lba_result {
   double lambda; /* final damping */
 } plf_lba_result;
 /* Projects with the context's camera (plf_create), not a sequence's (plf_set_sequence_camera); plf_local_ba_batch
- * takes a sequence's. */
+ * takes a sequence's.  The call is plf_local_ba_batch's launch chain with one problem: all opts.max_iters rounds are
+ * enqueued at once and a round after the problem has stopped still costs its eight launches (each returning at once),
+ * so the call's time grows with max_iters, not with the iterations run; one host synchronisation, after the download.
+ * Work is enqueued on plf_stream and uses the scratch slot plf_global_ba and plf_pose_graph use (not
+ * plf_local_ba_batch's), which stays allocated until plf_destroy: the sizes plf_local_ba_batch lists for one problem. */
 plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* problem, plf_lba_result* out);
 
 /* Many local bundle adjustments in one call: the local maps of several sequences' new keyframes, each with its
@@ -447,11 +452,16 @@ plf_status plf_local_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts, int n_prob
  * Limits: n_kf <= 4096 (else PLF_ERR_CAPACITY).  PLF_ERR_INVALID for an empty problem, a landmark without observations
  * or with a zero diagonal entry in its first-pass block (as plf_local_ba), ungrouped observations, out-of-range indices
  * or NULL arrays; the context stays usable after any error.
- * Work is enqueued on plf_stream and uses scratch slot 10 (shared with plf_local_ba), which stays allocated until
- * plf_destroy: about 288 n_kf^2 bytes for the dense reduced system (1.2 GB at 2048 keyframes, 4.8 GB at 4096) plus
- * 144 bytes per observation and about 650 bytes per landmark.  Up to n_kf = 64 the reduced system is factored by one CTA as in
- * plf_local_ba; beyond, by a tiled LDL^T across the GPU that skips exactly-zero tiles.  Projects with the context's camera,
- * as plf_local_ba; plf_global_ba_batch takes a sequence's. */
+ * The call is plf_global_ba_batch's launch chain with one problem: all opts.max_iters rounds are enqueued at once, and
+ * a round after the problem has stopped still costs its launches (8, plus 5 n_t + 1 beyond 64 keyframes, each returning
+ * at once), so the call's time grows with max_iters, not with the iterations run; one host synchronisation, after the
+ * download.
+ * Work is enqueued on plf_stream and uses the scratch slot plf_local_ba and plf_pose_graph use (not
+ * plf_global_ba_batch's), which stays allocated until plf_destroy: about 288 n_kf^2 bytes for the dense reduced system
+ * (1.2 GB at 2048 keyframes, 4.8 GB at 4096) plus 144 bytes per observation and about 650 bytes per landmark.  Up to
+ * n_kf = 64 the reduced system is factored by one CTA as in plf_local_ba; beyond, by a tiled LDL^T across the GPU that
+ * skips exactly-zero tiles (n_t = ceil(6 n_kf / 64) tile columns).  Projects with the context's camera, as
+ * plf_local_ba; plf_global_ba_batch takes a sequence's. */
 plf_status plf_global_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* problem, plf_lba_result* out);
 
 /* Many global bundle adjustments in one call: the maps of several sequences that end together, each with its sequence's
@@ -503,7 +513,7 @@ plf_status plf_global_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts, int n_pro
  * Limits: at most 4096 free vertices with edges (PLF_ERR_CAPACITY, before any allocation).  PLF_ERR_INVALID for NULL
  * arrays, out-of-range or self edges, non-finite T or Z, a lambda_init that is not positive and finite (g2o would derive
  * one from H instead), and a connected component with edges but no fixed vertex.  The context stays usable after any
- * error.  Work is enqueued on plf_stream and uses scratch slot 10 (shared with the bundle adjustments): 288 n_free^2
+ * error.  Work is enqueued on plf_stream and uses the scratch slot of plf_local_ba and plf_global_ba: 288 n_free^2
  * bytes for the dense system (4.8 GB at 4096 free vertices) plus about 790 bytes per edge, 260 per vertex and 200 per
  * free vertex; out->scratch_bytes reports what the call carved. */
 enum { PLF_PGO_STOP_MAX_ITERS = 0, PLF_PGO_STOP_TRIALS = 1, PLF_PGO_STOP_RHO_ZERO = 2, PLF_PGO_STOP_LAMBDA = 3 };

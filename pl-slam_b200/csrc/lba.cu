@@ -6,26 +6,29 @@
 // (the norm of the point reprojection error / of the two end-point distances to the observed line).  The reference
 // rebuilds a DENSE N x N Hessian every iteration and factors its sparse view with SimplicialLDLT; here the same normal
 // equations are solved through the Schur complement on the landmarks - every observation couples ONE keyframe with ONE
-// landmark, so the landmark block is block-diagonal (3x3 / 6x6) and each coupling block is rank one:
-//   k_lba_rows      one thread per observation: residual, weight, the two Jacobian rows (:1384-1400 points, :1441-1503
+// landmark, so the landmark block is block-diagonal (3x3 / 6x6) and each coupling block is rank one.  Each step is a
+// __device__ function of one problem's element, run on every problem of a call by the k_lbb_* kernels below:
+//   lba_rows        one thread per observation: residual, weight, the two Jacobian rows (:1384-1400 points, :1441-1503
 //                   lines); accumulates the keyframe blocks A (6x6) / g_c and the error
-//   k_lba_lm_accum  one thread per landmark: D = sum w Jx Jx^T, g_l (its observations are contiguous, in the reference's
+//   lba_lm_accum    one thread per landmark: D = sum w Jx Jx^T, g_l (its observations are contiguous, in the reference's
 //                   order), max |diagonal| for the initial lambda (:1543-1550)
-//   k_lba_lm_schur  one thread per landmark: D' = D + lambda diag(D), D'^-1, and the reduced-system contributions
+//   lba_lm_schur    one thread per landmark: D' = D + lambda diag(D), D'^-1, and the reduced-system contributions
 //                   S[a][b] -= w_b (y_a . Jx_b) Jt_a Jt_b^T, g_red[a] -= (y_a . g_l) Jt_a with y_a = w_a D'^-1 Jx_a
-//   k_lba_solve     one CTA: S += A', dense LDL^T (no pivoting, as SimplicialLDLT) and the two triangular solves
-//   k_lba_backsub   one thread per landmark: dx_l = D'^-1 (g_l - sum_a w_a Jx_a (Jt_a . dx_c[a]))
-//   k_lba_apply     T <- T * inverse_se3(expmap_se3(dx)) / X += dx (:1558-1570), |dx|^2
-// The host keeps the reference's control flow (first pass on the map's values, lambda schedule :1785-1803, stop tests
-// :1775,:1805).  opts.ref_quirks selects between the reference as written and its evident intent for the four oddities
-// documented in oracle/lba.c (division by the zero counters :1541, both line end points read from one block of X at
-// stride 3 :1678-1679, the map's pose for line rows :1681, the literal clamp); oracle = oracle/lba.c.
+//   lba_solve       one CTA: S += A', dense LDL^T (no pivoting, as SimplicialLDLT) and the two triangular solves
+//   lba_backsub     one thread per landmark: dx_l = D'^-1 (g_l - sum_a w_a Jx_a (Jt_a . dx_c[a]))
+//   lba_apply       T <- T * inverse_se3(expmap_se3(dx)) / X += dx (:1558-1570), |dx|^2
+// The reference's control flow (first pass on the map's values, lambda schedule :1785-1803, stop tests :1775,:1805)
+// runs on the device too, one thread per problem (k_lbb_first / k_lbb_test / k_lbb_step), so plf_local_ba is
+// plf_local_ba_batch's driver with one problem.  opts.ref_quirks selects between the reference as written and its
+// evident intent for the four oddities documented in oracle/lba.c (division by the zero counters :1541, both line end
+// points read from one block of X at stride 3 :1678-1679, the map's pose for line rows :1681, the literal clamp);
+// oracle = oracle/lba.c.
 //
 // Global bundle adjustment (SURVEY §8(f), after f1-f5): plf_global_ba replaces MapHandler::levMarquardtOptimizationGBA
-// (:2101-2699) with the same kernels and host loop over every keyframe but keyframe 0 and every landmark.  Its quirk set
-// (g1-g6, oracle/gba.py) selects the reference's GBA oddities instead of LBA's, and a reduced system larger than 384
-// (more than 64 keyframes) is factored by the tiled, multi-CTA LDL^T below (k_gba_*), whose trailing update runs on the
-// FP64 tensor cores (DMMA) and skips the tiles of the panel that are exactly zero.
+// (:2101-2699) with the same device functions and driver over every keyframe but keyframe 0 and every landmark.  Its
+// quirk set (g1-g6, oracle/gba.py) selects the reference's GBA oddities instead of LBA's, and a reduced system larger
+// than 384 (more than 64 keyframes) is factored by the tiled, multi-CTA LDL^T below (gba_*, run by k_gbb_*), whose
+// trailing update runs on the FP64 tensor cores (DMMA) and skips the tiles of the panel that are exactly zero.
 #include "plf_internal.h"
 #include "plf_se3.cuh"
 
@@ -56,7 +59,7 @@ struct LbaDev {
   double* S; double* gred; double* dxc;        // n x n, n, n   (n = 6 nkf)
   double* DX;                                  // N
   double* scal;                                // [0] err, [1] |dx|^2, [2] Hmax (as ordered bits), [3] Hmax under g2,
-                                               // [4] first landmark with a zero diagonal entry in D (k_lba_lm_accum)
+                                               // [4] first landmark with a zero diagonal entry in D (lba_lm_accum)
 };
 struct LbaCam { double fx, fy, cx, cy; };
 
@@ -72,8 +75,8 @@ __device__ __forceinline__ void lba_rowvec_R(const double* v, const double* T, d
   for (int j = 0; j < 3; ++j) out[j] = v[0] * T[j] + v[1] * T[4 + j] + v[2] * T[8 + j];
 }
 
-// Each kernel's work for one element (observation k, landmark l, ...) is a __device__ function of the problem's LbaDev,
-// so that plf_local_ba_batch's kernels (below plf_global_ba) run the same arithmetic on each problem of a batch.
+// Each step's work for one element (observation k, landmark l, ...) is a __device__ function of the problem's LbaDev,
+// which the k_lbb_* kernels below run on each problem of a call.
 
 // mode 0: first pass on the map's values (X0 / T0inv); mode 1: LM iteration on X; quirks: BAQ_* set.  Every lane of the
 // warp calls it (the error is reduced over the warp).
@@ -165,9 +168,6 @@ __device__ __forceinline__ void lba_rows(const LbaDev& d, const LbaCam& c, int k
   for (int off = 16; off > 0; off >>= 1) e2w += __shfl_xor_sync(0xFFFFFFFFu, e2w, off);
   if ((threadIdx.x & 31) == 0 && e2w != 0.0) atomicAdd(&d.scal[0], e2w);
 }
-__global__ void __launch_bounds__(128) k_lba_rows(LbaDev d, LbaCam c, int mode, int quirks, double homog_th) {
-  lba_rows(d, c, blockIdx.x * 128 + threadIdx.x, mode, quirks, homog_th);
-}
 
 __device__ __forceinline__ void lba_atomic_max_pos(double* addr, double v) {   // v >= 0: the bit patterns are ordered
   atomicMax(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)__double_as_longlong(v));
@@ -196,12 +196,10 @@ __device__ __forceinline__ void lba_lm_accum(const LbaDev& d, int l) {
   // a zero diagonal entry: scal[4] (as an integer) keeps nlm - l of the first such landmark, 0 when there is none
   if (zero) atomicMax(reinterpret_cast<unsigned long long*>(&d.scal[4]), (unsigned long long)(d.nlm - l));
 }
-__global__ void __launch_bounds__(128) k_lba_lm_accum(LbaDev d) { lba_lm_accum(d, blockIdx.x * 128 + threadIdx.x); }
 
 __device__ __forceinline__ void lba_kf_diagmax(const LbaDev& d, int i) {
   if (i < 6 * d.nkf) lba_atomic_max_pos(&d.scal[2], fabs(d.A[36 * (i / 6) + 7 * (i % 6)]));
 }
-__global__ void k_lba_kf_diagmax(LbaDev d) { lba_kf_diagmax(d, blockIdx.x * blockDim.x + threadIdx.x); }
 
 // in-place inverse of a symmetric positive definite dim x dim matrix (row stride 6) by Gauss-Jordan without pivoting
 __device__ void lba_inv_spd(double* M, int dim, double* Minv) {
@@ -259,9 +257,6 @@ __device__ __forceinline__ void lba_lm_schur(const LbaDev& d, int l, double lamb
     }
   }
 }
-__global__ void __launch_bounds__(128) k_lba_lm_schur(LbaDev d, double lambda, int swap) {
-  lba_lm_schur(d, blockIdx.x * 128 + threadIdx.x, lambda, swap);
-}
 
 // One CTA of 256 threads: S += A' (block diagonal, damped), g_red += g_c, dense LDL^T without pivoting, solve
 // S dx_c = g_red.
@@ -311,7 +306,7 @@ __global__ void __launch_bounds__(256) k_lba_solve(LbaDev d, double lambda) { lb
 __device__ __forceinline__ void lba_backsub(const LbaDev& d, int l, int swap) {
   if (l >= d.nlm) return;
   const int dim = l < d.npt ? 3 : 6;
-  const double* U = swap && l >= d.npt ? d.Jt : d.Jx;   // as k_lba_lm_schur
+  const double* U = swap && l >= d.npt ? d.Jt : d.Jx;   // as lba_lm_schur
   const double* V = swap && l >= d.npt ? d.Jx : d.Jt;
   double r[6];
   for (int i = 0; i < 6; ++i) r[i] = d.gl[6 * (size_t)l + i];
@@ -333,7 +328,6 @@ __device__ __forceinline__ void lba_backsub(const LbaDev& d, int l, int swap) {
     d.DX[off + i] = v;
   }
 }
-__global__ void __launch_bounds__(128) k_lba_backsub(LbaDev d, int swap) { lba_backsub(d, blockIdx.x * 128 + threadIdx.x, swap); }
 
 // |DX|^2 always; the step itself only when `apply`.  Element i: keyframe i (i < nkf), else one landmark coordinate.  Every
 // lane of the warp calls it.
@@ -357,7 +351,6 @@ __device__ __forceinline__ void lba_apply(const LbaDev& d, int i, int apply) {
   for (int off = 16; off > 0; off >>= 1) n2 += __shfl_xor_sync(0xFFFFFFFFu, n2, off);
   if ((threadIdx.x & 31) == 0 && n2 != 0.0) atomicAdd(&d.scal[1], n2);
 }
-__global__ void __launch_bounds__(128) k_lba_apply(LbaDev d, int apply) { lba_apply(d, blockIdx.x * 128 + threadIdx.x, apply); }
 
 __device__ __forceinline__ void lba_prep(const LbaDev& d, int i, const double* fixedT, double* fixedTinv, int n_fixed) {
   if (i < d.nkf) {
@@ -372,9 +365,6 @@ __device__ __forceinline__ void lba_prep(const LbaDev& d, int i, const double* f
     for (int k = 0; k < 16; ++k) fixedTinv[16 * i + k] = Ti[k];
   }
 }
-__global__ void k_lba_prep(LbaDev d, const double* fixedT, double* fixedTinv, int n_fixed) {
-  lba_prep(d, blockIdx.x * blockDim.x + threadIdx.x, fixedT, fixedTinv, n_fixed);
-}
 
 __device__ __forceinline__ void lba_moved(const LbaDev& d, int l, uint8_t* pt_moved, uint8_t* ls_moved) {
   if (l >= d.nlm) return;
@@ -384,9 +374,6 @@ __device__ __forceinline__ void lba_moved(const LbaDev& d, int l, uint8_t* pt_mo
   for (int c = 0; c < dim; ++c) { const double v = d.X[off + c] - d.X0[off + c]; n2 += v * v; }
   const uint8_t m = sqrt(n2) > 0.01;   // :1829, :1843
   if (l < d.npt) pt_moved[l] = m; else ls_moved[l - d.npt] = m;
-}
-__global__ void k_lba_moved(LbaDev d, uint8_t* pt_moved, uint8_t* ls_moved) {
-  lba_moved(d, blockIdx.x * blockDim.x + threadIdx.x, pt_moved, ls_moved);
 }
 
 // (g2) `int Hmax` scanned over the first pass's diagonal in index order (:2359-2364): `d > Hmax` compares with the int,
@@ -421,15 +408,14 @@ __device__ __forceinline__ void gba_hmax_int(const LbaDev& d) {
   if (tid == 0)
     d.scal[3] = last_big >= 0 && !any_after ? -2147483648.0 : trunc(__longlong_as_double((long long)mx));
 }
-__global__ void __launch_bounds__(1024) k_gba_hmax_int(LbaDev d) { gba_hmax_int(d); }
 
 // ---- blocked LDL^T of the reduced system for n = 6 n_kf > 384 (plf_global_ba) -----------------------------------------
 // Right-looking over 64 x 64 tiles of S (row-major, leading dimension n; only the lower triangle is read), the same
-// factorisation as k_lba_solve: per tile column k, k_gba_diag factors the diagonal tile in shared memory, k_gba_panel
-// solves each tile below it (L_ik = S_ik L_kk^-T D_k^-1, keeping W_ik = L_ik D_k) and flags whether it is exactly zero,
-// and k_gba_update subtracts W_ik L_jk^T from every trailing lower tile (i, j) whose two panel tiles are non-zero, on
-// the FP64 tensor cores.  The substitutions run per tile (k_gba_fwd / k_gba_bwd) and skip the same zero tiles.  Tiles
-// past n are padded with the identity; n_t = ceil(n / 64).
+// factorisation as lba_solve: per tile column k, gba_diag factors the diagonal tile in shared memory, gba_panel solves
+// each tile below it (L_ik = S_ik L_kk^-T D_k^-1, keeping W_ik = L_ik D_k) and flags whether it is exactly zero, and
+// gba_update subtracts W_ik L_jk^T from every trailing lower tile (i, j) whose two panel tiles are non-zero, on the FP64
+// tensor cores.  The substitutions run per tile (gba_fwd / gba_bwd) and skip the same zero tiles.  Tiles past n are
+// padded with the identity; n_t = ceil(n / 64).
 constexpr int GBA_T = 64, GBA_LD = 65;
 
 __device__ __forceinline__ double gba_S(const LbaDev& d, int r, int c) {   // S[r][c], 0 outside the matrix
@@ -445,9 +431,9 @@ __device__ __forceinline__ void gba_load_lkk(const LbaDev& d, int k, double* L) 
   }
 }
 
-// Each stage's work for one CTA (or element) of one problem is a __device__ function of the problem's LbaDev, so that
-// plf_global_ba_batch's kernels (k_gbb_*) run the same arithmetic on every large problem of a batch.
-__device__ __forceinline__ void gba_damp(const LbaDev& d, double lambda, int i) {   // k_lba_solve's prologue
+// Each stage's work for one CTA (or element) of one problem is a __device__ function of the problem's LbaDev, which the
+// k_gbb_* kernels run on every large problem of a call.
+__device__ __forceinline__ void gba_damp(const LbaDev& d, double lambda, int i) {   // lba_solve's prologue
   const int n = 6 * d.nkf;
   if (i < 36 * d.nkf) {
     const int kf = i / 36, r = (i % 36) / 6, cc = i % 6;
@@ -458,7 +444,6 @@ __device__ __forceinline__ void gba_damp(const LbaDev& d, double lambda, int i) 
     d.gred[i - 36 * d.nkf] += d.gc[i - 36 * d.nkf];
   }
 }
-__global__ void __launch_bounds__(256) k_gba_damp(LbaDev d, double lambda) { gba_damp(d, lambda, blockIdx.x * 256 + threadIdx.x); }
 
 __device__ __forceinline__ void gba_diag(const LbaDev& d, int k) {
   __shared__ double T[GBA_T * GBA_LD];
@@ -468,7 +453,7 @@ __device__ __forceinline__ void gba_diag(const LbaDev& d, int k) {
     T[r * GBA_LD + c] = r0 + r < n && r0 + c < n ? d.S[(size_t)(r0 + r) * n + r0 + c] : (r == c ? 1.0 : 0.0);
   }
   __syncthreads();
-  for (int j = 0; j < GBA_T; ++j) {   // as k_lba_solve: after column j, T[i][j] = L_ij, T[j][j] = D_j
+  for (int j = 0; j < GBA_T; ++j) {   // as lba_solve: after column j, T[i][j] = L_ij, T[j][j] = D_j
     const double dj = T[j * GBA_LD + j];
     for (int i = j + 1 + tid; i < GBA_T; i += 256) T[i * GBA_LD + j] /= dj;
     __syncthreads();
@@ -484,7 +469,6 @@ __device__ __forceinline__ void gba_diag(const LbaDev& d, int k) {
     if (c <= r && r0 + r < n) d.S[(size_t)(r0 + r) * n + r0 + c] = T[r * GBA_LD + c];
   }
 }
-__global__ void __launch_bounds__(256) k_gba_diag(LbaDev d, int k) { gba_diag(d, k); }
 
 // one CTA per tile row i > k; gsm: dynamic shared memory of 2 x 64 x GBA_LD doubles
 __device__ __forceinline__ void gba_panel(const LbaDev& d, double* Wp, uint8_t* nz, int k, int nt, int i, double* gsm) {
@@ -518,10 +502,6 @@ __device__ __forceinline__ void gba_panel(const LbaDev& d, double* Wp, uint8_t* 
     Wp[((size_t)i * GBA_T + r) * GBA_T + c] = z;
     if (r0 + r < n && c0 + c < n) d.S[(size_t)(r0 + r) * n + c0 + c] = z / L[c * GBA_LD + c];
   }
-}
-__global__ void __launch_bounds__(256) k_gba_panel(LbaDev d, double* Wp, uint8_t* nz, int k, int nt) {
-  extern __shared__ double gsm[];
-  gba_panel(d, Wp, nz, k, nt, k + 1 + blockIdx.x, gsm);
 }
 
 __device__ __forceinline__ void gba_dmma(double& c0, double& c1, double& c2, double& c3, double a0, double a1, double b0) {
@@ -567,9 +547,6 @@ __device__ __forceinline__ void gba_update(const LbaDev& d, const double* Wp, co
       if (r < n && c < n) d.S[(size_t)r * n + c] -= acc[q][e];
     }
 }
-__global__ void __launch_bounds__(256) k_gba_update(LbaDev d, const double* Wp, const uint8_t* nz, int k, int nt) {
-  gba_update(d, Wp, nz, k, nt, blockIdx.x);
-}
 
 // forward substitution step k: every CTA solves y_k = L_kk^-1 g_k (64 threads, in place of g's tile), CTA 0 stores it in
 // dxc, CTA b > 0 subtracts L_ik y_k from g_i (i = k + b) when that tile is non-zero
@@ -596,13 +573,11 @@ __device__ __forceinline__ void gba_fwd(const LbaDev& d, const uint8_t* nz, int 
     if (lane == 0 && r < n) d.gred[r] -= s;
   }
 }
-__global__ void __launch_bounds__(256) k_gba_fwd(LbaDev d, const uint8_t* nz, int k, int nt) { gba_fwd(d, nz, k, nt, blockIdx.x); }
 
 __device__ __forceinline__ void gba_dscale(const LbaDev& d, int i) {   // z = y / D
   const int n = 6 * d.nkf;
   if (i < n) d.gred[i] = d.dxc[i] / d.S[(size_t)i * n + i];
 }
-__global__ void k_gba_dscale(LbaDev d) { gba_dscale(d, blockIdx.x * blockDim.x + threadIdx.x); }
 
 // backward substitution step k (k = n_t - 1 .. 0): every CTA solves x_k = L_kk^-T z_k, CTA 0 stores it in dxc and DX,
 // CTA b > 0 subtracts L_kj^T x_k from z_j (j = b - 1) when that tile is non-zero
@@ -628,44 +603,12 @@ __device__ __forceinline__ void gba_bwd(const LbaDev& d, const uint8_t* nz, int 
   __syncthreads();
   if (tid < GBA_T && GBA_T * j + tid < n) d.gred[GBA_T * j + tid] -= ((part[0][tid] + part[1][tid]) + part[2][tid]) + part[3][tid];
 }
-__global__ void __launch_bounds__(256) k_gba_bwd(LbaDev d, const uint8_t* nz, int k, int nt) { gba_bwd(d, nz, k, nt, blockIdx.x); }
 
-// The tiled factorisation and the two substitutions (see k_gba_diag), shared by plf_global_ba and plf_pose_graph.  The
-// kernels read only the fields of LbaDev set here.
-plf_status plf_ldlt_tiled(plf_ctx* ctx, cudaStream_t cs, int n6, double* S, double* g, double* y, double* x, double* Wp,
-                          uint8_t* nz) {
-  static_assert(GBA_T == PLF_LDLT_TILE, "plf_internal.h states the tile size");
-  LbaDev d{};
-  d.nkf = n6; d.S = S; d.gred = g; d.dxc = y; d.DX = x;
-  const int n = 6 * n6, nt = (n + GBA_T - 1) / GBA_T;
-  const int smem = 2 * GBA_T * GBA_LD * 8;
-  PLF_CUDA(ctx, cudaFuncSetAttribute(k_gba_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  for (int k = 0; k < nt; ++k) {
-    k_gba_diag<<<1, 256, 0, cs>>>(d, k);
-    PLF_LAUNCH_CHECK(ctx);
-    const int m = nt - k - 1;
-    if (!m) break;
-    k_gba_panel<<<m, 256, smem, cs>>>(d, Wp, nz, k, nt);
-    PLF_LAUNCH_CHECK(ctx);
-    k_gba_update<<<m * (m + 1) / 2, 256, 0, cs>>>(d, Wp, nz, k, nt);
-    PLF_LAUNCH_CHECK(ctx);
-  }
-  for (int k = 0; k < nt; ++k) {
-    k_gba_fwd<<<nt - k, 256, 0, cs>>>(d, nz, k, nt);
-    PLF_LAUNCH_CHECK(ctx);
-  }
-  k_gba_dscale<<<(n + 255) / 256, 256, 0, cs>>>(d);
-  PLF_LAUNCH_CHECK(ctx);
-  for (int k = nt - 1; k >= 0; --k) {
-    k_gba_bwd<<<k + 1, 256, 0, cs>>>(d, nz, k, nt);
-    PLF_LAUNCH_CHECK(ctx);
-  }
-  return PLF_OK;
-}
-
-// Test hook (plslam_b200.h): one of the two factorisations on a caller's matrix.  Path 0 is plf_ldlt_tiled as
-// plf_global_ba / plf_pose_graph call it; path 1 is k_lba_solve with zero keyframe blocks and gradient and lambda = 0, so
-// its prologue adds +0.0 to the diagonal 6 x 6 blocks and to g.  The zero flags are cleared first, so the ones the panel kernel never sets (i <= k) read 0.
+// Test hook (plslam_b200.h): one of the two factorisations on a caller's matrix.  Path 0 is gbb_ldlt with the one system
+// by value and no activity flags, as plf_global_ba and plf_pose_graph run it; path 1 is k_lba_solve (lba_solve without
+// k_lbb_solve's zeroing, so S comes back factored) with zero keyframe blocks and gradient and lambda = 0, so its prologue
+// adds +0.0 to the diagonal 6 x 6 blocks and to g.  The zero flags are cleared first, so the ones the panel kernel never
+// sets (i <= k) read 0.
 extern "C" plf_status plf_debug_ldlt(plf_ctx* ctx, int path, int n6, double* S, const double* g, double* x, uint8_t* nz) {
   const char* fn = "plf_debug_ldlt";
   if (!ctx || !S || !g || !x) return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", fn);
@@ -688,7 +631,9 @@ extern "C" plf_status plf_debug_ldlt(plf_ctx* ctx, int path, int n6, double* S, 
   PLF_CUDA(ctx, cudaMemcpyAsync(d.gred, g, (size_t)n * 8, cudaMemcpyHostToDevice, cs));
   if (path == 0) {
     PLF_CUDA(ctx, cudaMemsetAsync(dNz, 0, (size_t)nt * nt, cs));
-    if (plf_status st = plf_ldlt_tiled(ctx, cs, n6, d.S, d.gred, d.dxc, d.DX, dWp, dNz)) return st;
+    GbbLdlt L{};
+    L.S = d.S; L.g = d.gred; L.y = d.dxc; L.x = d.DX; L.Wp = dWp; L.nz = dNz; L.one = GbbBig{0, n6, 0, 0, 0, 0, 0};
+    if (plf_status st = gbb_ldlt(ctx, cs, L, 1, n)) return st;
   } else {
     PLF_CUDA(ctx, cudaMemsetAsync(d.A, 0, (size_t)36 * n6 * 8, cs));
     PLF_CUDA(ctx, cudaMemsetAsync(d.gc, 0, (size_t)n * 8, cs));
@@ -702,12 +647,6 @@ extern "C" plf_status plf_debug_ldlt(plf_ctx* ctx, int path, int n6, double* S, 
   return PLF_OK;
 }
 
-// The host loop of both routines: the reference's control flow, on the device kernels above.  `global` selects
-// levMarquardtOptimizationGBA (:2101-2699) over levMarquardtOptimizationLBA (:1332-1989): its quirk set, its error
-// normalisation in the LM iterations and up to 4096 keyframes (the blocked factorisation beyond n = 384).  Both refuse a
-// landmark whose first-pass block D has an exactly zero diagonal entry, before any step: the reference would factor a
-// zero pivot (its SimplicialLDLT's failure is not checked) and the landmark, then every keyframe observing it, would
-// turn NaN.  A landmark without observations is refused by name first; the rest by one flag read with the first pass.
 // The host-side rules of one problem, up to its observations: counts, emptiness, the keyframe limit and NULL arrays.
 // Messages start with `fn`.
 static plf_status lba_check_shape(plf_ctx* ctx, const char* fn, const plf_lba_problem* p, int kf_cap) {
@@ -754,168 +693,14 @@ static plf_status lba_gather(plf_ctx* ctx, const char* fn, const plf_lba_problem
   return PLF_OK;
 }
 
-static plf_status ba_run(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out, bool global) {
-  const char* fn = global ? "plf_global_ba" : "plf_local_ba";
-  if (!ctx || !opts || !p) return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", fn);
-  if (plf_status st = lba_check_shape(ctx, fn, p, global ? 4096 : 64)) return st;
-  const int nkf = p->n_kf, npt = p->n_pt, nls = p->n_ls, npo = p->n_pt_obs, nlo = p->n_ls_obs, nobs = npo + nlo, nlm = npt + nls;
-  const int N = 6 * nkf + 3 * npt + 6 * nls, n = 6 * nkf;
-  std::vector<int> lm_start(nlm + 1), h_lm(nobs), h_kf(nobs);
-  std::vector<double> h_z((size_t)nobs * 3);
-  if (plf_status st = lba_gather(ctx, fn, p, lm_start.data(), h_lm.data(), h_kf.data(), h_z.data())) return st;
-  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  const bool blocked = n > 384;   // k_lba_solve (one CTA, one launch) up to 64 keyframes, the tiled LDL^T beyond
-  const int nt = (n + GBA_T - 1) / GBA_T;
-  LbaDev d;
-  d.nkf = nkf; d.npt = npt; d.nls = nls; d.N = N; d.npo = npo; d.nlo = nlo; d.nobs = nobs; d.nlm = nlm;
-  double *dFT, *dFTi, *dZ, *dWp;
-  int *dLm, *dKf, *dLs;
-  uint8_t *dPm, *dLmv, *dNz;
-  DevBufList scr;
-  scr.add(d.X, N); scr.add(d.X0, N); scr.add(d.T0inv, (size_t)std::max(nkf, 1) * 16);
-  scr.add(dFT, (size_t)std::max(p->n_fixed, 1) * 16); scr.add(dFTi, (size_t)std::max(p->n_fixed, 1) * 16);
-  scr.add(dLm, nobs); scr.add(dKf, nobs); scr.add(dZ, (size_t)nobs * 3); scr.add(dLs, (size_t)nlm + 1);
-  scr.add(d.Jt, (size_t)nobs * 6); scr.add(d.Jx, (size_t)nobs * 6); scr.add(d.Wn, (size_t)nobs * 2);
-  scr.add(d.D, (size_t)std::max(nlm, 1) * 36); scr.add(d.gl, (size_t)std::max(nlm, 1) * 6); scr.add(d.Dinv, (size_t)std::max(nlm, 1) * 36);
-  scr.add(d.A, (size_t)std::max(nkf, 1) * 36); scr.add(d.gc, (size_t)std::max(nkf, 1) * 6);
-  scr.add(d.S, std::max((size_t)n * n, (size_t)1)); scr.add(d.gred, (size_t)std::max(n, 1)); scr.add(d.dxc, (size_t)std::max(n, 1));
-  scr.add(d.DX, N); scr.add(d.scal, 8);
-  scr.add(dPm, std::max(npt, 1)); scr.add(dLmv, std::max(nls, 1));
-  scr.add(dWp, blocked ? (size_t)nt * GBA_T * GBA_T : 1); scr.add(dNz, blocked ? (size_t)nt * nt : 1);
-  if (plf_status st = scr.carve(ctx, PLF_SCR_BA)) return st;
-  d.fixedTinv = dFTi;
-  d.obs_lm = dLm; d.obs_kf = dKf; d.obs_z = dZ; d.lm_start = dLs;
-  cudaStream_t cs = ctx->stream;
-  std::vector<double> hX(N);
-  for (int i = 0; i < 6 * nkf; ++i) hX[i] = p->kf_pose[i];
-  for (int i = 0; i < 3 * npt; ++i) hX[6 * nkf + i] = p->pt[i];
-  for (int i = 0; i < 6 * nls; ++i) hX[6 * nkf + 3 * npt + i] = p->ls[i];
-  PLF_CUDA(ctx, cudaMemcpyAsync(d.X, hX.data(), (size_t)N * 8, cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(d.X0, hX.data(), (size_t)N * 8, cudaMemcpyHostToDevice, cs));
-  if (p->n_fixed) PLF_CUDA(ctx, cudaMemcpyAsync(dFT, p->fixed_T, (size_t)p->n_fixed * 128, cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(dLm, h_lm.data(), (size_t)nobs * 4, cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(dKf, h_kf.data(), (size_t)nobs * 4, cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(dZ, h_z.data(), (size_t)nobs * 24, cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(dLs, lm_start.data(), (size_t)(nlm + 1) * 4, cudaMemcpyHostToDevice, cs));
-  k_lba_prep<<<(std::max(nkf, p->n_fixed) + 63) / 64 + 1, 64, 0, cs>>>(d, dFT, dFTi, p->n_fixed);
-  PLF_LAUNCH_CHECK(ctx);
-  const LbaCam cam = {ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy};
-  const int q = opts->ref_quirks ? (global ? BAQ_GBA : BAQ_LBA) : 0;
-  double lambda = opts->lambda;
-  double h_scal[5];
-  // builds the normal equations of `mode` and leaves err / Hmax in scal
-  auto build = [&](int mode) -> plf_status {
-    PLF_CUDA(ctx, cudaMemsetAsync(d.A, 0, (size_t)std::max(nkf, 1) * 288, cs));
-    PLF_CUDA(ctx, cudaMemsetAsync(d.gc, 0, (size_t)std::max(nkf, 1) * 48, cs));
-    PLF_CUDA(ctx, cudaMemsetAsync(d.S, 0, std::max((size_t)n * n, (size_t)1) * 8, cs));
-    PLF_CUDA(ctx, cudaMemsetAsync(d.gred, 0, (size_t)std::max(n, 1) * 8, cs));
-    PLF_CUDA(ctx, cudaMemsetAsync(d.scal, 0, 64, cs));
-    k_lba_rows<<<(nobs + 127) / 128, 128, 0, cs>>>(d, cam, mode, q, opts->homog_th);
-    PLF_LAUNCH_CHECK(ctx);
-    k_lba_lm_accum<<<(nlm + 127) / 128, 128, 0, cs>>>(d);
-    PLF_LAUNCH_CHECK(ctx);
-    if (mode == 0 && nkf) {
-      k_lba_kf_diagmax<<<(6 * nkf + 63) / 64, 64, 0, cs>>>(d);
-      PLF_LAUNCH_CHECK(ctx);
-    }
-    if (mode == 0 && (q & BAQ_HMAX_INT)) {
-      k_gba_hmax_int<<<1, 1024, 0, cs>>>(d);
-      PLF_LAUNCH_CHECK(ctx);
-    }
-    PLF_CUDA(ctx, cudaMemcpyAsync(h_scal, d.scal, 40, cudaMemcpyDeviceToHost, cs));
-    PLF_CUDA(ctx, cudaStreamSynchronize(cs));
-    return PLF_OK;
-  };
-  // the blocked factorisation and the two substitutions of S dx_c = g_red (see k_gba_diag)
-  auto solve_blocked = [&]() -> plf_status {
-    k_gba_damp<<<(36 * nkf + n + 255) / 256, 256, 0, cs>>>(d, lambda);
-    PLF_LAUNCH_CHECK(ctx);
-    return plf_ldlt_tiled(ctx, cs, nkf, d.S, d.gred, d.dxc, d.DX, dWp, dNz);
-  };
-  // solves the damped system and (optionally) applies the step; leaves |DX| in *dx_norm.  swap: (g6), first pass only
-  auto solve = [&](int apply, int swap, double* dx_norm) -> plf_status {
-    k_lba_lm_schur<<<(nlm + 127) / 128, 128, 0, cs>>>(d, lambda, swap);
-    PLF_LAUNCH_CHECK(ctx);
-    if (blocked) {
-      plf_status s = solve_blocked();
-      if (s) return s;
-    } else if (nkf) {
-      k_lba_solve<<<1, 256, 0, cs>>>(d, lambda);
-      PLF_LAUNCH_CHECK(ctx);
-    }
-    k_lba_backsub<<<(nlm + 127) / 128, 128, 0, cs>>>(d, swap);
-    PLF_LAUNCH_CHECK(ctx);
-    k_lba_apply<<<(nkf + (N - 6 * nkf) + 127) / 128, 128, 0, cs>>>(d, apply);
-    PLF_LAUNCH_CHECK(ctx);
-    PLF_CUDA(ctx, cudaMemcpyAsync(h_scal, d.scal, 32, cudaMemcpyDeviceToHost, cs));
-    PLF_CUDA(ctx, cudaStreamSynchronize(cs));
-    *dx_norm = sqrt(h_scal[1]);
-    return PLF_OK;
-  };
-  plf_status st;
-  // ---- first pass on the map's values (LBA :1352-1541, GBA :2117-2356), lambda *= Hmax (:1543-1550, :2358-2365), first
-  // step applied unconditionally
-  if ((st = build(0))) return st;
-  unsigned long long zero_flag;
-  memcpy(&zero_flag, &h_scal[4], 8);
-  if (zero_flag) {
-    const int l = nlm - (int)zero_flag;
-    return plf_fail(ctx, PLF_ERR_INVALID, "%s: %s landmark %d has a zero diagonal entry in its first-pass block (no row constrains it)",
-                    fn, l < npt ? "point" : "line", l < npt ? l : l - npt);
-  }
-  double err = h_scal[0];
-  volatile int never_incremented = 0;   // Npt_obs + Nls_obs of the reference
-  if (q & BAQ_FIRST_ERR0) err /= (double)never_incremented;   // (q1) :1541, (g1) :2356
-  else err /= (double)nobs;
-  double Hmax;
-  if (q & BAQ_HMAX_INT) Hmax = h_scal[3];   // (g2)
-  else { unsigned long long bits; memcpy(&bits, &h_scal[2], 8); memcpy(&Hmax, &bits, 8); }
-  lambda *= Hmax;
-  double dxn = 0.0;
-  if ((st = solve(1, (q & BAQ_SWAP_COUPLING) ? 1 : 0, &dxn))) return st;
-  double err_prev = err;
-  int iters;
-  for (iters = 1; iters < opts->max_iters; ++iters) {
-    if ((st = build(1))) return st;
-    if (q & BAQ_ITER_ERR0) err = h_scal[0] / (double)never_incremented;                           // (g3) :2635
-    else if (global) err = h_scal[0] / (double)nobs;
-    else err = h_scal[0] / (double)(npt + nls);                                                  // :1773
-    if (fabs(err - err_prev) < opts->min_error_change || err < opts->min_error) break;           // :1775, :2637
-    const bool grew = err > err_prev;
-    if ((st = solve(grew ? 0 : 1, 0, &dxn))) return st;                                          // :1777-1803, :2639-2665
-    if (grew) lambda /= opts->lambda_k; else lambda *= opts->lambda_k;
-    if (dxn < opts->min_error_change) break;                                                     // :1805, :2667
-    err_prev = err;
-  }
-  k_lba_moved<<<(nlm + 127) / 128, 128, 0, cs>>>(d, dPm, dLmv);
-  PLF_LAUNCH_CHECK(ctx);
-  PLF_CUDA(ctx, cudaMemcpyAsync(hX.data(), d.X, (size_t)N * 8, cudaMemcpyDeviceToHost, cs));
-  if (p->pt_moved && npt) PLF_CUDA(ctx, cudaMemcpyAsync(p->pt_moved, dPm, (size_t)npt, cudaMemcpyDeviceToHost, cs));
-  if (p->ls_moved && nls) PLF_CUDA(ctx, cudaMemcpyAsync(p->ls_moved, dLmv, (size_t)nls, cudaMemcpyDeviceToHost, cs));
-  PLF_CUDA(ctx, cudaStreamSynchronize(cs));
-  for (int i = 0; i < 6 * nkf; ++i) p->kf_pose[i] = hX[i];
-  for (int i = 0; i < 3 * npt; ++i) p->pt[i] = hX[6 * nkf + i];
-  for (int i = 0; i < 6 * nls; ++i) p->ls[i] = hX[6 * nkf + 3 * npt + i];
-  if (out) { out->iters = iters; out->err = err; out->lambda = lambda; }
-  return PLF_OK;
-}
-
-extern "C" plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out) {
-  return ba_run(ctx, opts, p, out, false);
-}
-
-extern "C" plf_status plf_global_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out) {
-  return ba_run(ctx, opts, p, out, true);
-}
-
-// ---- plf_local_ba_batch: many local BAs in one launch chain -----------------------------------------------------------
+// ---- the driver: one problem or many in one launch chain ---------------------------------------------------------------
 // The problems' arrays are concatenated into flat arrays; LbbProb holds problem p's counts, its offsets into each flat
 // array and its camera, and lbb_view() builds the LbaDev of its slice, so the kernels below run the single-problem
 // functions above on each problem.  They are gridded (problem, chunk): blockIdx.x is the problem and blockIdx.y strides
-// over its observations, landmarks or elements, so no warp mixes two problems.  ba_run's host loop runs on the device
-// in LbbCtrl, one thread per problem (k_lbb_first, k_lbb_test, k_lbb_step), with the same double expressions in the same
-// order.  A problem that has stopped, or was refused, is inactive, and every later kernel returns at once for it.  All
-// max_iters rounds are enqueued up front, so the call has one host synchronisation, after the download.
+// over its observations, landmarks or elements, so no warp mixes two problems.  The reference's control flow runs on the
+// device in LbbCtrl, one thread per problem (k_lbb_first, k_lbb_test, k_lbb_step).  A problem that has stopped, or was
+// refused, is inactive, and every later kernel returns at once for it.  All max_iters rounds are enqueued up front, so
+// the call has one host synchronisation, after the download.
 struct LbbProb {
   int nkf, npt, nls, npo, nobs, nlm, N, nfix;
   long long xo, oo, lo, ko, fo, go, so;   // offsets into X (doubles), observations, landmarks, keyframes, fixed
@@ -993,8 +778,8 @@ __global__ void __launch_bounds__(128) k_lbb_schur(LbbDev b, int swap) {
   for (int c = blockIdx.y; 128 * c < q.nlm; c += gridDim.y) lba_lm_schur(d, 128 * c + threadIdx.x, lambda, swap);
 }
 
-// One CTA per problem with n = 6 n_kf <= 384, as k_lba_solve; then zeroes A, g_c, S and g_red for the next round's
-// accumulation.  Larger problems (plf_global_ba_batch) are solved by the k_gbb_* kernels.
+// One CTA per problem with n = 6 n_kf <= 384 (lba_solve); then zeroes A, g_c, S and g_red for the next round's
+// accumulation.  Larger problems (plf_global_ba) are solved by the k_gbb_* kernels.
 __global__ void __launch_bounds__(256) k_lbb_solve(LbbDev b) {
   const int p = blockIdx.x;
   if (!b.ctrl[p].active) return;
@@ -1027,7 +812,7 @@ __global__ void __launch_bounds__(128) k_lbb_apply(LbbDev b) {
   for (int c = blockIdx.y; 128 * c < ne; c += gridDim.y) lba_apply(d, 128 * c + threadIdx.x, apply);
 }
 
-// The control of both routines: G selects plf_global_ba's (ba_run's `global` branch) over plf_local_ba's.
+// The control of both routines: G selects plf_global_ba's over plf_local_ba's.
 // After the first pass: the refusal, the error normalisation (q1 / g1: the reference divides by two counters it never
 // increments, 0.0 here as there) and lambda *= Hmax (g2: the int-truncated maximum of k_gbb_hmax_int).  The first step
 // is applied unconditionally (apply = 1 from k_lbb_prep).
@@ -1043,7 +828,7 @@ __device__ __forceinline__ void lbb_first(const LbbDev& b, int quirks) {
   double err = scal[0];
   if (quirks & BAQ_FIRST_ERR0) err = __ddiv_rn(err, 0.0);   // (q1) :1541
   else err /= (double)q.nobs;
-  // Hmax: under (g2) scal[3], else the double whose bit pattern k_lba_lm_accum / k_lba_kf_diagmax maximised
+  // Hmax: under (g2) scal[3], else the double whose bit pattern lba_lm_accum / lba_kf_diagmax maximised
   c.lambda *= G && (quirks & BAQ_HMAX_INT) ? scal[3] : scal[2];
   c.err = err;
   c.err_prev = err;
@@ -1099,12 +884,13 @@ __global__ void __launch_bounds__(128) k_lbb_moved(LbbDev b) {
   for (int c = blockIdx.y; 128 * c < q.nlm; c += gridDim.y) lba_moved(d, 128 * c + threadIdx.x, m, m + q.npt);
 }
 
-// ---- plf_global_ba_batch: the large problems' tiled LDL^T ---------------------------------------------------------------
+// ---- plf_global_ba: the large problems' tiled LDL^T ----------------------------------------------------------------------
 // A problem with n = 6 n_kf > 384 is factored by the tiled LDL^T above, with its own Wp and zero flags.  Per tile column
 // there is one launch of each stage over every large problem, gridded (tile, problem) at the largest problem's extent:
-// blockIdx.y picks the problem from the GbbBig table, and a CTA whose problem has fewer tiles, has stopped or was refused
-// returns at once.  Each CTA runs the single-problem function of the stage, so a problem's factorisation is plf_ldlt_tiled's
-// bit for bit.  GbbBig and GbbLdlt are declared in plf_internal.h: plf_pose_graph_batch factors through gbb_ldlt too.
+// blockIdx.y picks the problem from the GbbBig table (or the one problem passed by value), and a CTA whose problem has
+// fewer tiles, has stopped or was refused returns at once.  Each CTA runs the single-problem function of the stage, so a
+// problem's factorisation does not depend on the others.  GbbBig and GbbLdlt are declared in plf_internal.h:
+// plf_pose_graph factors through gbb_ldlt too.
 // The LbaDev fields the tiled kernels read, for problem blockIdx.y, and its tile count; false when it is not active.
 __device__ __forceinline__ bool gbb_view(const GbbLdlt& L, LbaDev& d, GbbBig& t, int& nt) {
   t = L.big ? L.big[blockIdx.y] : L.one;
@@ -1148,9 +934,10 @@ __global__ void __launch_bounds__(256) k_gbb_bwd(GbbLdlt L, int k) {
   gba_bwd(d, L.nz + t.zo, k, nt, blockIdx.x);
 }
 
-// The tiled factorisation and the two substitutions of the nb problems in L.big, the largest with n_max rows: the
-// launches of plf_ldlt_tiled at n_max, each over every problem.
+// The tiled factorisation and the two substitutions of the nb problems in L.big (or of L.one), the largest with n_max
+// rows: per tile column k, gba_diag, gba_panel and gba_update; then gba_fwd per tile, gba_dscale and gba_bwd per tile.
 plf_status gbb_ldlt(plf_ctx* ctx, cudaStream_t cs, const GbbLdlt& L, int nb, int n_max) {
+  static_assert(GBA_T == PLF_LDLT_TILE, "plf_internal.h states the tile size");
   const int nt = (n_max + GBA_T - 1) / GBA_T, smem = 2 * GBA_T * GBA_LD * 8;
   PLF_CUDA(ctx, cudaFuncSetAttribute(k_gbb_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   for (int k = 0; k < nt; ++k) {
@@ -1176,7 +963,7 @@ plf_status gbb_ldlt(plf_ctx* ctx, cudaStream_t cs, const GbbLdlt& L, int nb, int
   return PLF_OK;
 }
 
-// S += A' and g_red += g_c of every active large problem (k_gba_damp), gridded (chunk, problem)
+// S += A' and g_red += g_c of every active large problem (gba_damp), gridded (chunk, problem)
 __global__ void __launch_bounds__(256) k_gbb_damp(LbbDev b, const GbbBig* big) {
   const GbbBig t = big[blockIdx.y];
   if (!b.ctrl[t.p].active) return;
@@ -1203,38 +990,49 @@ __global__ void __launch_bounds__(1024) k_gbb_hmax_int(LbbDev b) {
   gba_hmax_int(lbb_view(b, b.prob[p], p));
 }
 
-// plf_local_ba_batch and plf_global_ba_batch: ba_run's rules per problem and its control on the device (k_lbb_first /
-// k_lbb_test, or k_gbb_first / k_gbb_test with global), one upload, every round enqueued, one download.
+// plf_local_ba / plf_global_ba (one problem, batch = false) and their _batch forms: the host-side rules per problem and
+// the reference's control on the device (k_lbb_first / k_lbb_test, or k_gbb_first / k_gbb_test with global), one upload,
+// every round enqueued, one download.  `global` selects levMarquardtOptimizationGBA (:2101-2699) over
+// levMarquardtOptimizationLBA (:1332-1989): its quirk set, its error normalisation in the LM iterations and up to 4096
+// keyframes (the tiled factorisation beyond n = 384).  Both refuse a landmark whose first-pass block D has an exactly
+// zero diagonal entry, before any step: the reference would factor a zero pivot (its SimplicialLDLT's failure is not
+// checked) and the landmark, then every keyframe observing it, would turn NaN.  A landmark without observations is
+// refused by name on the host; the rest by one flag per problem set with the first pass.
 static plf_status lbb_run(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems, const plf_lba_problem* problems,
-                          const int32_t* seq, plf_lba_result* out, plf_status* status, bool global) {
-  const char* fn = global ? "plf_global_ba_batch" : "plf_local_ba_batch";
+                          const int32_t* seq, plf_lba_result* out, plf_status* status, bool global, bool batch) {
+  const char* fn = global ? (batch ? "plf_global_ba_batch" : "plf_global_ba") : (batch ? "plf_local_ba_batch" : "plf_local_ba");
   if (!ctx || !opts || n_problems < 0 || (n_problems && (!problems || !status)))
     return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments", fn);
   const int P = n_problems;
   if (!P) return PLF_OK;
   // the large problems are gridded in y, at most 65535 of them; the limit is on the batch so that it does not depend on
   // the problems' sizes
-  if (global && P > 65535) return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: %d problems (limit 65535)", fn, P);
-  // every refusal before any work: the cameras, then ba_run's rules per problem
+  if (batch && global && P > 65535) return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: %d problems (limit 65535)", fn, P);
+  // problem p's messages start with "fn: problem p", or with fn alone in the one-problem calls
+  char pfx[64];
+  auto prefix = [&](int p) -> const char* {
+    if (!batch) return fn;
+    snprintf(pfx, sizeof pfx, "%s: problem %d", fn, p);
+    return pfx;
+  };
+  // every refusal before any work: the cameras, then the host-side rules per problem
   std::vector<LbbProb> hp(P);
   std::vector<GbbBig> hb;
   long long tN = 0, tObs = 0, tLm = 0, tKf = 0, tFix = 0, tG = 0, tS = 0, tWp = 0, tNz = 0;
   int mObs = 0, mLm = 0, mEl = 0, mBig = 0;
-  char pfx[64];
   for (int p = 0; p < P; ++p) {
     const int s = seq ? seq[p] : -1;
     if (s < -1 || s >= ctx->max_sequences)
       return plf_fail(ctx, PLF_ERR_INVALID, "%s: seq[%d] = %d outside [-1, %d)", fn, p, s, ctx->max_sequences);
     const plf_camera& c = s >= 0 && !ctx->seq_cam_own.empty() && ctx->seq_cam_own[s] ? ctx->seq_cam[s] : ctx->cam;
     const plf_lba_problem& pr = problems[p];
-    snprintf(pfx, sizeof pfx, "%s: problem %d", fn, p);
-    if (plf_status st = lba_check_shape(ctx, pfx, &pr, global ? 4096 : 64)) return st;
+    if (plf_status st = lba_check_shape(ctx, prefix(p), &pr, global ? 4096 : 64)) return st;
     LbbProb& q = hp[p];
     q.nkf = pr.n_kf; q.npt = pr.n_pt; q.nls = pr.n_ls; q.npo = pr.n_pt_obs; q.nobs = pr.n_pt_obs + pr.n_ls_obs;
     q.nlm = pr.n_pt + pr.n_ls; q.N = 6 * pr.n_kf + 3 * pr.n_pt + 6 * pr.n_ls; q.nfix = pr.n_fixed;
     q.xo = tN; q.oo = tObs; q.lo = tLm; q.ko = tKf; q.fo = tFix; q.go = tG; q.so = tS;
     q.cam = LbaCam{c.fx, c.fy, c.cx, c.cy};
-    if (q.nkf > 64) {   // n > 384: the tiled LDL^T (k_gbb_*), as ba_run's `blocked`
+    if (q.nkf > 64) {   // n > 384: the tiled LDL^T (k_gbb_*)
       const long long nt = (6 * q.nkf + GBA_T - 1) / GBA_T;
       hb.push_back(GbbBig{p, q.nkf, q.so, q.go, q.xo, tWp, tNz});
       tWp += nt * GBA_T * GBA_T; tNz += nt * nt;
@@ -1259,12 +1057,13 @@ static plf_status lbb_run(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems
                wSc = L.take_work(64 * (size_t)P);
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   uint8_t *pin, *dev;
-  if (plf_status st = L.acquire(ctx, PLF_SCR_BA_BATCH, &pin, &dev)) return st;
+  // the one-problem calls share their slot with plf_pose_graph, so that a context running plf_global_ba and
+  // plf_pose_graph holds one allocation for the two dense systems, not two
+  if (plf_status st = L.acquire(ctx, batch ? PLF_SCR_BA_BATCH : PLF_SCR_BA, &pin, &dev)) return st;
   for (int p = 0; p < P; ++p) {
     const plf_lba_problem& pr = problems[p];
     const LbbProb& q = hp[p];
-    snprintf(pfx, sizeof pfx, "%s: problem %d", fn, p);
-    if (plf_status st = lba_gather(ctx, pfx, &pr, (int*)(pin + iLs) + q.lo + p, (int*)(pin + iLm) + q.oo, (int*)(pin + iKf) + q.oo,
+    if (plf_status st = lba_gather(ctx, prefix(p), &pr, (int*)(pin + iLs) + q.lo + p, (int*)(pin + iLm) + q.oo, (int*)(pin + iKf) + q.oo,
                                    (double*)(pin + iZ) + 3 * q.oo))
       return st;
     double* X0 = (double*)(pin + iX0) + q.xo;
@@ -1293,7 +1092,9 @@ static plf_status lbb_run(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems
   const GbbBig* dBig = (const GbbBig*)(dev + iBig);
   static_assert(sizeof(LbbCtrl) % sizeof(int) == 0, "gbb_view reads LbbCtrl::active as a strided int");
   const int* act = (const int*)((const uint8_t*)b.ctrl + offsetof(LbbCtrl, active));
-  const GbbLdlt gl{dBig, act, (int)(sizeof(LbbCtrl) / sizeof(int)), b.S, b.gred, b.dxc, b.DX, (double*)(dwork + wWp), dwork + wNz};
+  GbbLdlt gl{dBig, act, (int)(sizeof(LbbCtrl) / sizeof(int)), b.S, b.gred, b.dxc, b.DX, (double*)(dwork + wWp), dwork + wNz, {}};
+  // one large problem (every plf_global_ba over 64 keyframes) passes its entry by value: no table load per CTA
+  if (nb == 1) { gl.big = nullptr; gl.one = hb[0]; }
   // grids: (problem, chunks of 128 of the largest problem's count); the control kernels: one thread per problem
   auto chunks = [](int n) { return std::max(1, std::min(65535, (n + 127) / 128)); };
   const dim3 gObs(P, chunks(mObs)), gLm(P, chunks(mLm)), gEl(P, chunks(mEl));
@@ -1370,20 +1171,32 @@ static plf_status lbb_run(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems
   }
   if (refused >= 0) {
     const int l = ctl[refused].zero_lm, npt = hp[refused].npt;
-    return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: %s landmark %d has a zero diagonal entry in its first-pass block (no row constrains it)",
-                    fn, refused, l < npt ? "point" : "line", l < npt ? l : l - npt);
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: %s landmark %d has a zero diagonal entry in its first-pass block (no row constrains it)",
+                    prefix(refused), l < npt ? "point" : "line", l < npt ? l : l - npt);
   }
   return PLF_OK;
 }
 
+extern "C" plf_status plf_local_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out) {
+  if (!ctx || !opts || !p) return plf_fail(ctx, PLF_ERR_INVALID, "plf_local_ba: bad arguments");
+  plf_status st;
+  return lbb_run(ctx, opts, 1, p, nullptr, out, &st, false, false);
+}
+
+extern "C" plf_status plf_global_ba(plf_ctx* ctx, const plf_lba_opts* opts, const plf_lba_problem* p, plf_lba_result* out) {
+  if (!ctx || !opts || !p) return plf_fail(ctx, PLF_ERR_INVALID, "plf_global_ba: bad arguments");
+  plf_status st;
+  return lbb_run(ctx, opts, 1, p, nullptr, out, &st, true, false);
+}
+
 extern "C" plf_status plf_local_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems, const plf_lba_problem* problems,
                                          const int32_t* seq, plf_lba_result* out, plf_status* status) {
-  return lbb_run(ctx, opts, n_problems, problems, seq, out, status, false);
+  return lbb_run(ctx, opts, n_problems, problems, seq, out, status, false, true);
 }
 
 extern "C" plf_status plf_global_ba_batch(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems, const plf_lba_problem* problems,
                                           const int32_t* seq, plf_lba_result* out, plf_status* status) {
-  return lbb_run(ctx, opts, n_problems, problems, seq, out, status, true);
+  return lbb_run(ctx, opts, n_problems, problems, seq, out, status, true, true);
 }
 
 // Test hook (plslam_b200.h): the k_gbb_* chain on n caller matrices of mixed sizes, each as plf_debug_ldlt's path 0

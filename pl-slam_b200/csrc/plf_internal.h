@@ -29,7 +29,8 @@ enum plf_scratch_slot {
   PLF_SCR_ORB,         // plf_orb
   PLF_SCR_LSD,         // plf_lsd, plf_detect_lines, plf_debug_sincosf
   PLF_SCR_MGB_PIPE,    // the windowed matcher of plf_batch_run (matching_strategy != 0)
-  PLF_SCR_BA,          // plf_local_ba, plf_global_ba, plf_pose_graph, plf_pose_graph_batch
+  PLF_SCR_BA,          // plf_local_ba, plf_global_ba, plf_pose_graph, plf_pose_graph_batch: their staged layout;
+                       // plf_debug_ldlt, plf_debug_ldlt_batch
   PLF_SCR_KF,          // plf_match_kf2kf, plf_match_map2kf and their _batch forms: their staged layout
   PLF_SCR_KF_MGB_PT,   // plf_match_kf2kf, plf_match_map2kf and their _batch forms: the windowed matcher of points
   PLF_SCR_KF_MGB_LS,   //   ... and of lines
@@ -233,19 +234,16 @@ plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs
                          const PlfPairCam* d_cams = nullptr, const int* d_active = nullptr);
 
 // ---- tiled LDL^T (lba.cu) ------------------------------------------------------------------------
-// Factors the symmetric n x n matrix S (n = 6 n6; row-major, leading dimension n; only its lower triangle is read) in
+// Factors each symmetric n x n matrix S (n = 6 nkf; row-major, leading dimension n; only its lower triangle is read) in
 // place as L D L^T without pivoting, over 64 x 64 tiles, skipping the tiles of L that are exactly zero, and solves
 // S x = g.  Afterwards S's diagonal holds D, y and x both hold the solution, and g has been overwritten.  Wp
 // (n_t x 64 x 64 doubles) and nz (n_t x n_t bytes) are work, n_t = ceil(n / 64).  Enqueued on cs.
+// Used by plf_global_ba, plf_pose_graph, their _batch forms and the plf_debug_ldlt hooks: one launch per stage and tile
+// column over the nb systems of `big`, gridded (tile, system) at the largest one's n_max rows.  Each system is factored
+// and solved with its own Wp and zero flags, bit for bit as it would be alone.  System i is skipped when
+// active[big[i].p * active_stride] is 0 (active NULL: none is).  With big NULL the one system is `one` (nb = 1), read
+// from the kernels' parameters: nothing is loaded before the factorisation's own data.
 constexpr int PLF_LDLT_TILE = 64;
-plf_status plf_ldlt_tiled(plf_ctx* ctx, cudaStream_t cs, int n6, double* S, double* g, double* y, double* x, double* Wp,
-                          uint8_t* nz);
-// The same factorisation and solve of many systems at once (plf_global_ba_batch, plf_pose_graph_batch,
-// plf_debug_ldlt_batch): one launch per stage and tile column over the nb systems of `big`, gridded (tile, system) at the
-// largest one's n_max rows.  Each system is factored and solved bit for bit as plf_ldlt_tiled would, with its own Wp and
-// zero flags.  System i is skipped when active[big[i].p * active_stride] is 0 (active NULL: none is).  With big NULL
-// the one system is `one` (nb = 1), read from the kernels' parameters: nothing is loaded before the factorisation's own
-// data, as in plf_ldlt_tiled.
 struct GbbBig {
   int p, nkf;                     // the system's problem index in its batch and its block count (n = 6 nkf rows)
   long long so, go, xo, wo, zo;   // offsets into S, g / y, x (doubles), Wp (doubles) and the zero flags (bytes)

@@ -1133,7 +1133,8 @@ class Frontend:
 
     def debug_ldlt(self, S, g, path=0, overwrite_s=False):
         """LDL^T without pivoting of the symmetric S (6 n6 x 6 n6, lower triangle read) and the solution of S x = g, by
-        the tiled factorisation of global_ba / pose_graph (path 0) or the one-CTA one of local_ba (path 1).  Returns
+        the tiled factorisation of global_ba / pose_graph beyond 64 keyframes, on one system (path 0), or the one-CTA
+        one of local_ba, without the zeroing that follows it there (path 1).  Returns
         (LD, x, nz): LD holds L strictly below its diagonal and D on it (upper triangle unspecified); nz (path 0, else
         None) is the n_t x n_t zero flag of each L tile (i > k), n_t = ceil(n / 64).  overwrite_s: factor S's own buffer
         (a C-contiguous float64 array) instead of a copy.  plf_debug_ldlt."""

@@ -1,5 +1,5 @@
 """Symmetric matrices built to reach what the BA / PGO systems leave to chance in the two dense LDL^T factorisations
-(plf_ldlt_tiled and k_lba_solve, csrc/lba.cu): every pattern of zero 64 x 64 tiles the tiled one skips or fills, partial
+(gbb_ldlt's gba_* stages and lba_solve, csrc/lba.cu): every pattern of zero 64 x 64 tiles the tiled one skips or fills, partial
 last tiles, badly scaled and indefinite values, zero pivots and planted NaN / Inf; and the reference they are checked
 against.  Pure numpy (mpmath for the smallest sizes), seeded; every generator returns (S, g, record) where the record
 names the case and the tile pattern of S it is built to have.  tests/test_ldlt.py measures, without a GPU, that the
@@ -45,7 +45,7 @@ def tile_any(M):
 
 def lower_tiles(M):
     """The strictly lower tiles (I > K) of M that hold an entry other than +-0 in its lower triangle: the zero flags
-    k_gba_panel sets, as an n_t x n_t bool array (False on and above the tile diagonal)."""
+    gba_panel sets, as an n_t x n_t bool array (False on and above the tile diagonal)."""
     return np.tril(tile_any(np.tril(M)), -1)
 
 
@@ -333,10 +333,10 @@ def well_conditioned(case):
     return case.values in ("dominant", "quasi")
 
 
-# ---- k_gba_update's block index ---------------------------------------------------------------------------------------
+# ---- gba_update's block index -------------------------------------------------------------------------------------------
 
 def update_pair(t):
-    """k_gba_update's decode of its block index t (numpy int array) into the tile pair (a, b), 0 <= b <= a, restated:
+    """gba_update's decode of its block index t (numpy int array) into the tile pair (a, b), 0 <= b <= a, restated:
     a = (int)((sqrt(8 t + 1) - 1) * 0.5) in double, each operation rounded (the library is built with --fmad=false), then
     the two correction loops in int."""
     t = np.asarray(t, np.int64)

@@ -32,7 +32,7 @@ def _copy(p):
 
 def edge_map(homog_th, seed=11):
     """A local map (n_fixed = 3 from keyframe 0, the identity; 6 local keyframes) with five landmarks whose first pass
-    has a row on an edge of k_lba_rows, each also observed by well-posed rows of fixed keyframes:
+    has a row on an edge of lba_rows, each also observed by well-posed rows of fixed keyframes:
       point n   on keyframe 0's optical axis, observed there at (cx, cy): residual exactly 0 (nrm < homog_th)
       point n+1 on local keyframe 0's optical axis at depth sqrt(homog_th) / 2 (the depth clamp), observed there 316 px off
       point n+2 1 m behind local keyframe 0, observed by it at its (mirrored) projection: negative depth

@@ -1,8 +1,8 @@
 """GPU parity of the local bundle adjustment (plf_local_ba, csrc/lba.cu) with oracle/lba.c on maps shaped like the
 reference's local maps (synth.local_map_problem: a sliding window, 20-40 % of the landmarks seen once, fixed keyframes
-that are earlier keyframes), at the keyframe counts where k_lba_solve's strided loops change (one pass up to 42, a
-second from 43) up to its limit of 64, at every exit and branch of the host loop, with rows on the clamps and signs of
-k_lba_rows, and the refusals, after each of which the context stays usable.  Maps come from tests/test_lba_edges.py,
+that are earlier keyframes), at the keyframe counts where lba_solve's strided loops change (one pass up to 42, a
+second from 43) up to its limit of 64, at every exit and branch of the LM control, with rows on the clamps and signs of
+lba_rows, and the refusals, after each of which the context stays usable.  Maps come from tests/test_lba_edges.py,
 which checks them on the CPU."""
 import ctypes as C
 

@@ -1,6 +1,6 @@
 """CPU tests of tests/ldlt_cases.py: the long-double LDL^T reference against 50-digit mpmath and scipy's Cholesky, the
 tile pattern each generator claims and the fill the elimination produces from it, the sizes the sweep covers, and
-k_gba_update's decode of its block index into tile pairs.  No GPU."""
+gba_update's decode of its block index into tile pairs.  No GPU."""
 import functools
 
 import numpy as np
@@ -168,8 +168,9 @@ def test_band_plus_loops_fill_matches_the_reference_and_stays_clear_of_underflow
 
 
 def test_update_decode_enumerates_every_tile_pair_once():
-    """k_gba_update launches m (m + 1) / 2 CTAs at tile column k (m = n_t - k - 1 trailing tiles, up to 383) and decodes
-    blockIdx.x into (a, b), 0 <= b <= a < m: for every m each pair is produced exactly once, in row order"""
+    """k_gbb_update launches m (m + 1) / 2 CTAs per system at tile column k (m = n_t - k - 1 trailing tiles, up to 383)
+    and gba_update decodes blockIdx.x into (a, b), 0 <= b <= a < m: for every m each pair is produced exactly once, in
+    row order"""
     tmax = 383 * 384 // 2
     a, b = lc.update_pair(np.arange(tmax))
     assert np.all((0 <= b) & (b <= a))
