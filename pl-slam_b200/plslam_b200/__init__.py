@@ -207,11 +207,17 @@ class plf_lc_detect_problem(C.Structure):
 # SlamConfig's loop-closure detection defaults (src/slamConfig.cpp:61-62, :80-82)
 LC_DETECT_DEFAULTS = dict(lc_kf_dist=50, lc_kf_max_dist=50, lc_nkf_closest=4, min_lm_cov_graph=75, min_kf_local_map=3)
 LC_RESULT_FIELDS = ("candidate", "best", "n_listed", "n_closest", "min_score")
+# SlamConfig's loop-closure pose check defaults (src/slamConfig.cpp:73-77, :83)
+LC_POSE_DEFAULTS = dict(lc_res=1.0, lc_unc=0.01, lc_inl=0.3, lc_trs=1.5, lc_rot=35.0, lc_inlier_ratio=30.0)
 
 
 def _lc_opts(opts):
     o = dict(LC_DETECT_DEFAULTS, **(opts or {}))
     return plf_lc_detect_opts(*[int(o[f]) for f, _ in plf_lc_detect_opts._fields_])
+
+
+def _lc_params(lc):
+    return plf_lc_params(**dict(LC_POSE_DEFAULTS, **(lc or {})))
 
 
 class plf_vocab(C.Structure):
@@ -299,6 +305,35 @@ def _local_map(local_map, kf_view, kf_pt_lm, kf_ls_lm, keep, who):
     return m, lms[0], lms[1]
 
 
+def _kf_match_opts(fast_matching, max_kf_epip_p, max_kf_epip_l):
+    return plf_kf_match_opts(int(bool(fast_matching)), float(max_kf_epip_p), float(max_kf_epip_l))
+
+
+def _kf2kf_problem(prev, curr, DT, keep):
+    """(plf_kf2kf_problem, m_pt, m_ls) over match_kf2kf's arguments: the struct and its output arrays, cut to the previous
+    keyframe's feature counts; `keep` holds the copies alive."""
+    p, c = _frame_view(prev, keep), _frame_view(curr, keep)
+    m_pt, m_ls = np.full(max(p.n_pt, 1), -1, np.int32), np.full(max(p.n_ls, 1), -1, np.int32)
+    keep += [p, c]
+    T = (C.c_double * 16)(*np.ascontiguousarray(DT, np.float64).reshape(16))
+    prob = plf_kf2kf_problem(C.pointer(p), C.pointer(c), T, m_pt.ctypes.data, m_ls.ctypes.data, 0, 0)
+    return prob, m_pt[:p.n_pt], m_ls[:p.n_ls]
+
+
+def _map2kf_problem(local_map, Twf, kf, kf_pt_lm, kf_ls_lm, keep, who):
+    """(plf_map2kf_problem, lm_pt, lm_ls) over match_map2kf's arguments: the struct and its output arrays, cut to the
+    local map's landmark counts; `keep` holds the copies alive."""
+    kv = _frame_view(kf, keep)
+    m, pt_lm, ls_lm = _local_map(local_map, kv, kf_pt_lm, kf_ls_lm, keep, who)
+    lm_pt, lm_ls = np.full(max(m.n_pt, 1), -1, np.int32), np.full(max(m.n_ls, 1), -1, np.int32)
+    keep += [kv, m]
+    ad = lambda a: None if a is None or not a.size else a.ctypes.data
+    T = (C.c_double * 16)(*np.ascontiguousarray(Twf, np.float64).reshape(16))
+    prob = plf_map2kf_problem(C.pointer(m), C.pointer(kv), T, ad(pt_lm), ad(ls_lm), lm_pt.ctypes.data, lm_ls.ctypes.data,
+                              0, 0)
+    return prob, lm_pt[:m.n_pt], lm_ls[:m.n_ls]
+
+
 RESULT_DTYPE =np.dtype([("DT", np.float64, (4, 4)), ("DT_cov", np.float64, (6, 6)), ("err", np.float64),
                          ("status", np.int32), ("n_kp_l", np.int32), ("n_kp_r", np.int32), ("n_lines_l", np.int32),
                          ("n_lines_r", np.int32), ("n_stereo_pt", np.int32), ("n_stereo_ls", np.int32),
@@ -373,13 +408,21 @@ EUROC_CAMERA = dict(width=752, height=480, fx=458.654, fy=457.296, cx=367.215, c
 DBL_EPSILON = float(np.finfo(np.float64).eps)   # numeric_limits<double>::epsilon(), the GBA stop thresholds
 
 
-def _u8(a, shape_tail=None):
-    a = np.ascontiguousarray(a, dtype=np.uint8)
-    return a
+def _u8(a):
+    return np.ascontiguousarray(a, dtype=np.uint8)
 
 
 def _ptr(a, ctype):
     return a.ctypes.data_as(C.POINTER(ctype))
+
+
+def _i32_or_null(a):
+    """int32* over a, or NULL for None (the seq arrays of the batch calls)."""
+    return None if a is None else _ptr(a, C.c_int32)
+
+
+def _lba_opts(lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, ref_quirks):
+    return plf_lba_opts(lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, int(ref_quirks))
 
 
 class Frontend:
@@ -544,22 +587,30 @@ class Frontend:
     # -- pose refinement -------------------------------------------------------------------------
     def gn_pose(self, P, pl_obs, sP, eP, le_obs, inlier_pt=None, inlier_ls=None, T_init=None, opts=None):
         """StereoFrameHandler::optimizePose.  Returns dict(T, cov, x, err, iters, inlier_pt, inlier_ls)."""
-        f64 = lambda a, k: np.ascontiguousarray(a, np.float64).reshape(-1, k)
-        P, pl_obs, sP, eP, le_obs = f64(P, 3), f64(pl_obs, 2), f64(sP, 3), f64(eP, 3), f64(le_obs, 3)
-        n_p, n_l = len(P), len(sP)
-        ip = np.ones(n_p, np.uint8) if inlier_pt is None else np.ascontiguousarray(inlier_pt, np.uint8).copy()
-        il = np.ones(n_l, np.uint8) if inlier_ls is None else np.ascontiguousarray(inlier_ls, np.uint8).copy()
-        T0 = None if T_init is None else np.ascontiguousarray(T_init, np.float64).reshape(16)
-        out = plf_pose_result()
-        dp = lambda a: a.ctypes.data_as(C.POINTER(C.c_double)) if a is not None and a.size else None
-        up = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint8)) if a.size else None
-        st = self.lib.plf_gn_pose(self._ctx, C.byref(opts) if opts is not None else None, dp(P), dp(pl_obs),
-                                  up(ip), n_p, dp(sP), dp(eP), dp(le_obs), up(il), n_l,
-                                  dp(T0) if T0 is not None else None, C.byref(out))
+        keep = []
+        p, ip, il = self._gn_problem(dict(P=P, pl_obs=pl_obs, sP=sP, eP=eP, le_obs=le_obs, inlier_pt=inlier_pt,
+                                          inlier_ls=inlier_ls, T_init=T_init), keep)
+        vp = C.c_void_p
+        st = self.lib.plf_gn_pose(self._ctx, C.byref(opts) if opts is not None else None, vp(p.P), vp(p.pl_obs),
+                                  vp(p.inlier_pt), p.np, vp(p.sP), vp(p.eP), vp(p.le_obs), vp(p.inlier_ls), p.nl,
+                                  vp(p.T_init), C.byref(p.out))
         self._check(st, "plf_gn_pose")
-        return dict(T=np.array(out.T).reshape(4, 4), cov=np.array(out.cov).reshape(6, 6), x=np.array(out.x),
-                    err=out.err, iters=(out.iters1, out.iters2), inlier_pt=ip, inlier_ls=il,
-                    n_inliers=(out.n_inliers_pt, out.n_inliers_ls))
+        return self._gn_result(p.out, ip, il)
+
+    @staticmethod
+    def _gn_problem(pr, keep):
+        """(plf_gn_problem, inlier_pt, inlier_ls) over a gn_pose_batch problem dict's arrays, converted where needed and
+        kept alive in keep; the inlier flags are copies, which the call updates."""
+        f64 = lambda a, k: np.ascontiguousarray(a, np.float64).reshape(-1, k)
+        P, O, sP, eP, le = f64(pr["P"], 3), f64(pr["pl_obs"], 2), f64(pr["sP"], 3), f64(pr["eP"], 3), f64(pr["le_obs"], 3)
+        ip = pr.get("inlier_pt"); il = pr.get("inlier_ls")
+        ip = np.ones(len(P), np.uint8) if ip is None else np.ascontiguousarray(ip, np.uint8).copy()
+        il = np.ones(len(sP), np.uint8) if il is None else np.ascontiguousarray(il, np.uint8).copy()
+        T0 = pr.get("T_init")
+        T0 = None if T0 is None else np.ascontiguousarray(T0, np.float64).reshape(16)
+        keep += [P, O, sP, eP, le, T0]
+        ad = lambda a: a.ctypes.data if a is not None and a.size else None
+        return plf_gn_problem(ad(P), ad(O), ad(ip), len(P), ad(sP), ad(eP), ad(le), ad(il), len(sP), ad(T0)), ip, il
 
     @staticmethod
     def _gn_result(out, ip, il):
@@ -575,54 +626,35 @@ class Frontend:
         problems = list(problems)
         P = len(problems)
         seq_a = self._problem_sequences(P, seq)
-        f64 = lambda a, k: np.ascontiguousarray(a, np.float64).reshape(-1, k)
-        ad = lambda a: a.ctypes.data if a is not None and a.size else None
         keep, flags = [], []
         arr = (plf_gn_problem * max(P, 1))()
         for k, pr in enumerate(problems):
-            Pp, O, sP, eP, le = f64(pr["P"], 3), f64(pr["pl_obs"], 2), f64(pr["sP"], 3), f64(pr["eP"], 3), f64(pr["le_obs"], 3)
-            ip = pr.get("inlier_pt"); il = pr.get("inlier_ls")
-            ip = np.ones(len(Pp), np.uint8) if ip is None else np.ascontiguousarray(ip, np.uint8).copy()
-            il = np.ones(len(sP), np.uint8) if il is None else np.ascontiguousarray(il, np.uint8).copy()
-            T0 = pr.get("T_init")
-            T0 = None if T0 is None else np.ascontiguousarray(T0, np.float64).reshape(16)
-            keep += [Pp, O, sP, eP, le, T0]
+            arr[k], ip, il = self._gn_problem(pr, keep)
             flags.append((ip, il))
-            arr[k] = plf_gn_problem(ad(Pp), ad(O), ad(ip), len(Pp), ad(sP), ad(eP), ad(le), ad(il), len(sP), ad(T0))
         self._check(self.lib.plf_gn_pose_batch(self._ctx, C.byref(opts) if opts is not None else None, P, arr,
-                                               None if seq_a is None else _ptr(seq_a, C.c_int32)), "plf_gn_pose_batch")
+                                               _i32_or_null(seq_a)), "plf_gn_pose_batch")
         return [dict(self._gn_result(arr[k].out, ip, il), status=0) for k, (ip, il) in enumerate(flags)]
 
     def loop_closure_pose(self, kf0, kf1, lc=None):
         """MapHandler::isLoopClosure + computeRelativePoseRobustGN (src/mapHandler.cpp:3192-3300, :3566-3957).
         kf0 / kf1: dicts with pdesc, P, pl, ldesc, sP, eP, le (numpy); lc: dict of the lc_* thresholds."""
-        d = dict(lc_res=1.0, lc_unc=0.01, lc_inl=0.3, lc_trs=1.5, lc_rot=35.0, lc_inlier_ratio=30.0)
-        d.update(lc or {})
-        lcp = plf_lc_params(**d)
+        lcp = _lc_params(lc)
         keep = []
-
-        def kf(k):
-            f = plf_lc_keyframe()
-            pd = _u8(k["pdesc"]).reshape(-1, 32); ld = _u8(k["ldesc"]).reshape(-1, 32)
-            arrs = dict(pdesc=pd, ldesc=ld)
-            for name, cols in (("P", 3), ("pl", 2), ("sP", 3), ("eP", 3), ("le", 3)):
-                arrs[name] = np.ascontiguousarray(k[name], np.float64).reshape(-1, cols)
-            f.n_pt, f.n_ls = len(pd), len(ld)
-            for name, a in arrs.items():
-                keep.append(a)
-                setattr(f, name, a.ctypes.data if a.size else None)
-            return f
-        k0, k1 = kf(kf0), kf(kf1)
+        k0, k1 = self._lc_keyframe(kf0, keep), self._lc_keyframe(kf1, keep)
         cap_p, cap_l = max(k0.n_pt, 1), max(k0.n_ls, 1)
         pp = np.full((cap_p, 2), -1, np.int32); lp = np.full((cap_l, 2), -1, np.int32)
         out = plf_lc_result()
         st = self.lib.plf_loop_closure_pose(self._ctx, C.byref(lcp), C.byref(k0), C.byref(k1), C.byref(out),
                                             _ptr(pp, C.c_int32), cap_p, _ptr(lp, C.c_int32), cap_l)
         self._check(st, "plf_loop_closure_pose")
+        return self._lc_pose_result(out, pp, lp)
+
+    @staticmethod
+    def _lc_pose_result(out, pp, lp):
+        """loop_closure_pose's dict from a plf_lc_result and its pair arrays (cut to the capacities the call had)."""
         r = {f: getattr(out, f) for f, _ in plf_lc_result._fields_ if f not in ("x_inc", "pose_inc")}
-        r["accepted"] = bool(out.accepted); r["estimated"] = bool(out.estimated)
-        r["x_inc"] = np.array(out.x_inc); r["pose_inc"] = np.array(out.pose_inc)
-        r["pt_pairs"] = pp[:out.n_pt].copy(); r["ls_pairs"] = lp[:out.n_ls].copy()
+        r.update(accepted=bool(out.accepted), estimated=bool(out.estimated), x_inc=np.array(out.x_inc),
+                 pose_inc=np.array(out.pose_inc), pt_pairs=pp[:out.n_pt].copy(), ls_pairs=lp[:out.n_ls].copy())
         return r
 
     @staticmethod
@@ -650,9 +682,7 @@ class Frontend:
         pairs = list(pairs)
         P = len(pairs)
         seq_a = self._problem_sequences(P, seq)
-        d = dict(lc_res=1.0, lc_unc=0.01, lc_inl=0.3, lc_trs=1.5, lc_rot=35.0, lc_inlier_ratio=30.0)
-        d.update(lc or {})
-        lcp = plf_lc_params(**d)
+        lcp = _lc_params(lc)
         keep, outs = [], []
         arr = (plf_lc_problem * max(P, 1))()
         for k, pr in enumerate(pairs):
@@ -661,23 +691,14 @@ class Frontend:
             k0, k1 = self._lc_keyframe(pr["kf0"], keep), self._lc_keyframe(pr["kf1"], keep)
             cap_p, cap_l = int(pr.get("cap_pt", k0.n_pt)), int(pr.get("cap_ls", k0.n_ls))
             pp = np.full((max(cap_p, 1), 2), -1, np.int32); lp = np.full((max(cap_l, 1), 2), -1, np.int32)
-            outs.append((pp, lp))
+            outs.append((pp[:cap_p], lp[:cap_l]))
             arr[k] = plf_lc_problem(C.pointer(k0), C.pointer(k1), pp.ctypes.data, cap_p, lp.ctypes.data, cap_l,
                                     plf_lc_result(), 1)   # 1 is no plf_status: marks entries the call did not write
-        rc = self.lib.plf_loop_closure_pose_batch(self._ctx, C.byref(lcp), P, arr,
-                                                  None if seq_a is None else _ptr(seq_a, C.c_int32))
+        rc = self.lib.plf_loop_closure_pose_batch(self._ctx, C.byref(lcp), P, arr, _i32_or_null(seq_a))
         if rc != 0 and (rc != PLF_ERR_CAPACITY or P == 0 or any(arr[k].status == 1 for k in range(P))):
             self._check(rc, "plf_loop_closure_pose_batch")
-        res = []
-        for k, (pp, lp) in enumerate(outs):
-            out = arr[k].out
-            r = {f: getattr(out, f) for f, _ in plf_lc_result._fields_ if f not in ("x_inc", "pose_inc")}
-            r["accepted"] = bool(out.accepted); r["estimated"] = bool(out.estimated)
-            r["x_inc"] = np.array(out.x_inc); r["pose_inc"] = np.array(out.pose_inc)
-            r["pt_pairs"] = pp[:min(out.n_pt, arr[k].cap_pt)].copy(); r["ls_pairs"] = lp[:min(out.n_ls, arr[k].cap_ls)].copy()
-            r["status"] = int(arr[k].status)
-            res.append(r)
-        return res
+        return [dict(self._lc_pose_result(arr[k].out, pp, lp), status=int(arr[k].status))
+                for k, (pp, lp) in enumerate(outs)]
 
     def local_ba(self, prob, lambda_=1e-5, lambda_k=10.0, max_iters=15, homog_th=1e-7, min_error=1e-7,
                  min_error_change=1e-7, ref_quirks=1):
@@ -715,8 +736,7 @@ class Frontend:
         return self._bundle_adjust_batch("plf_global_ba_batch", problems, seq, lambda_, lambda_k, max_iters, homog_th,
                                          min_error, min_error_change, ref_quirks)
 
-    def _bundle_adjust_batch(self, fn, problems, seq, lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change,
-                             ref_quirks):
+    def _bundle_adjust_batch(self, fn, problems, seq, *opts):
         problems = list(problems)
         P = len(problems)
         seq_a = self._problem_sequences(P, seq)
@@ -724,9 +744,8 @@ class Frontend:
         arr = (plf_lba_problem * max(P, 1))(*[a[0] for a in args])
         res = (plf_lba_result * max(P, 1))()
         st = np.full(max(P, 1), 1, np.int32)   # 1 is no plf_status: marks entries the call did not write
-        o = plf_lba_opts(lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, int(ref_quirks))
-        rc = getattr(self.lib, fn)(self._ctx, C.byref(o), P, arr, None if seq_a is None else _ptr(seq_a, C.c_int32),
-                                   res, _ptr(st, C.c_int32))
+        rc = getattr(self.lib, fn)(self._ctx, C.byref(_lba_opts(*opts)), P, arr, _i32_or_null(seq_a), res,
+                                   _ptr(st, C.c_int32))
         if rc != 0 and (P == 0 or np.any(st[:P] == 1)):
             self._check(rc, fn)
         out = []
@@ -738,8 +757,8 @@ class Frontend:
 
     @staticmethod
     def _problem_sequences(P, seq):
-        """seq of the batch calls (local_ba_batch, match_*_batch): None, or an integer array of P entries (checked before
-        any library call)."""
+        """seq of the batch calls (local_ba_batch, match_*_batch, batch_run): None, or an integer array of P entries
+        (checked before any library call)."""
         if seq is None:
             return None
         a = np.asarray(seq)
@@ -775,11 +794,10 @@ class Frontend:
                     ls_moved=a["lm"][:n_ls].astype(bool), iters=None if res is None else res.iters,
                     err=None if res is None else res.err, lambda_=None if res is None else res.lambda_)
 
-    def _bundle_adjust(self, fn, prob, lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, ref_quirks):
+    def _bundle_adjust(self, fn, prob, *opts):
         p, a = self._lba_args(prob)
-        o = plf_lba_opts(lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, int(ref_quirks))
         res = plf_lba_result()
-        self._check(getattr(self.lib, fn)(self._ctx, C.byref(o), C.byref(p), C.byref(res)), fn)
+        self._check(getattr(self.lib, fn)(self._ctx, C.byref(_lba_opts(*opts)), C.byref(p), C.byref(res)), fn)
         return self._lba_result(a, res)
 
     def pose_graph(self, prob, max_iters=100, lambda_init=1e-10, trace=True):
@@ -788,9 +806,8 @@ class Frontend:
         synth.pose_graph_problem or oracle.pgo.cov_graph_lists give it.  Returns dict(T, iters, stop (PGO_STOP's names),
         trials, chi2_init, chi2, lambda_, scratch_bytes, trace: a PGO_TRACE_DTYPE array with one row per trial when
         `trace`)."""
-        p, a = self._pgo_args(prob, max_iters, trace)
+        p, res, a = self._pgo_args(prob, max_iters, trace)
         o = plf_pgo_opts(int(max_iters), float(lambda_init))
-        res = plf_pgo_result(trace=a["trace"].ctypes.data if len(a["trace"]) else None, trace_cap=len(a["trace"]))
         self._check(self.lib.plf_pose_graph(self._ctx, C.byref(o), C.byref(p), C.byref(res)), "plf_pose_graph")
         return self._pgo_result(a, res, trace)
 
@@ -801,19 +818,17 @@ class Frontend:
         problems = list(problems)
         P = len(problems)
         args = [self._pgo_args(p, max_iters, trace) for p in problems]
-        arr = (plf_pgo_problem * max(P, 1))(*[p for p, _ in args])
-        res = (plf_pgo_result * max(P, 1))()
-        for k, (_, a) in enumerate(args):
-            res[k].trace = a["trace"].ctypes.data if len(a["trace"]) else None
-            res[k].trace_cap = len(a["trace"])
+        arr = (plf_pgo_problem * max(P, 1))(*[p for p, _, _ in args])
+        res = (plf_pgo_result * max(P, 1))(*[r for _, r, _ in args])
         o = plf_pgo_opts(int(max_iters), float(lambda_init))
         self._check(self.lib.plf_pose_graph_batch(self._ctx, C.byref(o), P, arr, res), "plf_pose_graph_batch")
-        return [self._pgo_result(a, res[k], trace) for k, (_, a) in enumerate(args)]
+        return [self._pgo_result(a, res[k], trace) for k, (_, _, a) in enumerate(args)]
 
     @staticmethod
     def _pgo_args(prob, max_iters, trace):
-        """(plf_pgo_problem, arrays): a copy of the problem's poses, which the call updates in place, its other arrays and
-        a trace of 10 max_iters rows (none without `trace`), and the struct that points at them."""
+        """(plf_pgo_problem, plf_pgo_result, arrays): a copy of the problem's poses, which the call updates in place, its
+        other arrays and a trace of 10 max_iters rows (none without `trace`), the problem struct that points at them and
+        a result struct that points at the trace."""
         T = np.ascontiguousarray(prob["T"], np.float64).reshape(-1, 16).copy()
         fixed = np.ascontiguousarray(prob["fixed"], np.uint8).ravel()
         frm = np.ascontiguousarray(prob["from"], np.int32).ravel()
@@ -822,7 +837,8 @@ class Frontend:
         ad = lambda a: a.ctypes.data if a.size else None
         p = plf_pgo_problem(len(T), len(frm), ad(T), ad(fixed), ad(frm), ad(to), ad(Z))
         tr = np.zeros(max(10 * int(max_iters), 1) if trace else 0, PGO_TRACE_DTYPE)
-        return p, dict(T=T, fixed=fixed, frm=frm, to=to, Z=Z, trace=tr)
+        res = plf_pgo_result(trace=ad(tr), trace_cap=len(tr))
+        return p, res, dict(T=T, fixed=fixed, frm=frm, to=to, Z=Z, trace=tr)
 
     @staticmethod
     def _pgo_result(a, res, trace):
@@ -836,15 +852,12 @@ class Frontend:
         """MapHandler::matchKF2KFPoints / matchKF2KFLines, matching part (plf_match_kf2kf).  prev / curr: get_frame dicts;
         DT: 4x4.  Returns dict(m_pt, n_pt, m_ls, n_ls): per previous-keyframe feature the current one or -1."""
         keep = []
-        p, c = _frame_view(prev, keep), _frame_view(curr, keep)
-        T = np.ascontiguousarray(DT, np.float64).reshape(16)
-        o = plf_kf_match_opts(int(bool(fast_matching)), float(max_kf_epip_p), float(max_kf_epip_l))
-        m_pt, m_ls = np.full(max(p.n_pt, 1), -1, np.int32), np.full(max(p.n_ls, 1), -1, np.int32)
+        p, m_pt, m_ls = _kf2kf_problem(prev, curr, DT, keep)
+        o = _kf_match_opts(fast_matching, max_kf_epip_p, max_kf_epip_l)
         n_pt, n_ls = C.c_int(0), C.c_int(0)
-        self._check(self.lib.plf_match_kf2kf(self._ctx, C.byref(o), C.byref(p), C.byref(c), T.ctypes.data_as(C.c_void_p),
-                                             m_pt.ctypes.data_as(C.c_void_p), m_ls.ctypes.data_as(C.c_void_p), C.byref(n_pt),
-                                             C.byref(n_ls)), "plf_match_kf2kf")
-        return dict(m_pt=m_pt[:p.n_pt].copy(), n_pt=n_pt.value, m_ls=m_ls[:p.n_ls].copy(), n_ls=n_ls.value)
+        self._check(self.lib.plf_match_kf2kf(self._ctx, C.byref(o), p.prev, p.curr, p.DT, C.c_void_p(p.m_pt),
+                                             C.c_void_p(p.m_ls), C.byref(n_pt), C.byref(n_ls)), "plf_match_kf2kf")
+        return dict(m_pt=m_pt.copy(), n_pt=n_pt.value, m_ls=m_ls.copy(), n_ls=n_ls.value)
 
     def match_map2kf(self, local_map, Twf, kf, kf_pt_lm=None, kf_ls_lm=None, fast_matching=True, max_kf_epip_p=1.0,
                      max_kf_epip_l=1.0):
@@ -852,17 +865,13 @@ class Frontend:
         optional pt_use, ls_X [n,6], ls_desc, optional ls_use; kf: get_frame dict; kf_*_lm: landmark index per keyframe
         feature (-1 = unmatched) or None.  Returns dict(lm_pt, n_pt, lm_ls, n_ls)."""
         keep = []
-        kv = _frame_view(kf, keep)
-        m, *lms = _local_map(local_map, kv, kf_pt_lm, kf_ls_lm, keep, "match_map2kf")
-        T = np.ascontiguousarray(Twf, np.float64).reshape(16)
-        o = plf_kf_match_opts(int(bool(fast_matching)), float(max_kf_epip_p), float(max_kf_epip_l))
-        lm_pt, lm_ls = np.full(max(m.n_pt, 1), -1, np.int32), np.full(max(m.n_ls, 1), -1, np.int32)
+        p, lm_pt, lm_ls = _map2kf_problem(local_map, Twf, kf, kf_pt_lm, kf_ls_lm, keep, "match_map2kf")
+        o = _kf_match_opts(fast_matching, max_kf_epip_p, max_kf_epip_l)
         n_pt, n_ls = C.c_int(0), C.c_int(0)
-        self._check(self.lib.plf_match_map2kf(self._ctx, C.byref(o), C.byref(m), T.ctypes.data_as(C.c_void_p), C.byref(kv),
-                                              *[C.c_void_p(a.ctypes.data if a is not None and a.size else None) for a in lms],
-                                              lm_pt.ctypes.data_as(C.c_void_p), lm_ls.ctypes.data_as(C.c_void_p),
+        self._check(self.lib.plf_match_map2kf(self._ctx, C.byref(o), p.map, p.Twf, p.kf, C.c_void_p(p.kf_pt_lm),
+                                              C.c_void_p(p.kf_ls_lm), C.c_void_p(p.lm_pt), C.c_void_p(p.lm_ls),
                                               C.byref(n_pt), C.byref(n_ls)), "plf_match_map2kf")
-        return dict(lm_pt=lm_pt[:m.n_pt].copy(), n_pt=n_pt.value, lm_ls=lm_ls[:m.n_ls].copy(), n_ls=n_ls.value)
+        return dict(lm_pt=lm_pt.copy(), n_pt=n_pt.value, lm_ls=lm_ls.copy(), n_ls=n_ls.value)
 
     def match_kf2kf_batch(self, problems, seq=None, fast_matching=True, max_kf_epip_p=1.0, max_kf_epip_l=1.0):
         """Many match_kf2kf in one device call (plf_match_kf2kf_batch), with one set of options.  problems: dicts
@@ -874,16 +883,11 @@ class Frontend:
         keep, outs = [], []
         arr = (plf_kf2kf_problem * max(P, 1))()
         for k, pr in enumerate(problems):
-            p, c = _frame_view(pr["prev"], keep), _frame_view(pr["curr"], keep)
-            keep += [p, c]
-            m_pt, m_ls = np.full(max(p.n_pt, 1), -1, np.int32), np.full(max(p.n_ls, 1), -1, np.int32)
-            outs.append((m_pt[:p.n_pt], m_ls[:p.n_ls]))
-            arr[k] = plf_kf2kf_problem(C.pointer(p), C.pointer(c), (C.c_double * 16)(*np.asarray(pr["DT"], np.float64).ravel()),
-                                       m_pt.ctypes.data, m_ls.ctypes.data, 0, 0)
-            keep += [m_pt, m_ls]
-        o = plf_kf_match_opts(int(bool(fast_matching)), float(max_kf_epip_p), float(max_kf_epip_l))
-        self._check(self.lib.plf_match_kf2kf_batch(self._ctx, C.byref(o), P, arr,
-                                                   None if seq_a is None else _ptr(seq_a, C.c_int32)), "plf_match_kf2kf_batch")
+            arr[k], m_pt, m_ls = _kf2kf_problem(pr["prev"], pr["curr"], pr["DT"], keep)
+            outs.append((m_pt, m_ls))
+        o = _kf_match_opts(fast_matching, max_kf_epip_p, max_kf_epip_l)
+        self._check(self.lib.plf_match_kf2kf_batch(self._ctx, C.byref(o), P, arr, _i32_or_null(seq_a)),
+                    "plf_match_kf2kf_batch")
         return [dict(m_pt=m_pt.copy(), n_pt=arr[k].n_pt, m_ls=m_ls.copy(), n_ls=arr[k].n_ls) for k, (m_pt, m_ls) in enumerate(outs)]
 
     def match_map2kf_batch(self, problems, seq=None, fast_matching=True, max_kf_epip_p=1.0, max_kf_epip_l=1.0):
@@ -895,20 +899,13 @@ class Frontend:
         seq_a = self._problem_sequences(P, seq)
         keep, outs = [], []
         arr = (plf_map2kf_problem * max(P, 1))()
-        ad = lambda a: None if a is None or not a.size else a.ctypes.data
         for k, pr in enumerate(problems):
-            kv = _frame_view(pr["kf"], keep)
-            m, pt_lm, ls_lm = _local_map(pr["local_map"], kv, pr.get("kf_pt_lm"), pr.get("kf_ls_lm"), keep,
-                                         f"match_map2kf_batch: problem {k}")
-            keep += [kv, m]
-            lm_pt, lm_ls = np.full(max(m.n_pt, 1), -1, np.int32), np.full(max(m.n_ls, 1), -1, np.int32)
-            outs.append((lm_pt[:m.n_pt], lm_ls[:m.n_ls]))
-            arr[k] = plf_map2kf_problem(C.pointer(m), C.pointer(kv), (C.c_double * 16)(*np.asarray(pr["Twf"], np.float64).ravel()),
-                                        ad(pt_lm), ad(ls_lm), lm_pt.ctypes.data, lm_ls.ctypes.data, 0, 0)
-            keep += [lm_pt, lm_ls]
-        o = plf_kf_match_opts(int(bool(fast_matching)), float(max_kf_epip_p), float(max_kf_epip_l))
-        self._check(self.lib.plf_match_map2kf_batch(self._ctx, C.byref(o), P, arr,
-                                                    None if seq_a is None else _ptr(seq_a, C.c_int32)), "plf_match_map2kf_batch")
+            arr[k], lm_pt, lm_ls = _map2kf_problem(pr["local_map"], pr["Twf"], pr["kf"], pr.get("kf_pt_lm"),
+                                                   pr.get("kf_ls_lm"), keep, f"match_map2kf_batch: problem {k}")
+            outs.append((lm_pt, lm_ls))
+        o = _kf_match_opts(fast_matching, max_kf_epip_p, max_kf_epip_l)
+        self._check(self.lib.plf_match_map2kf_batch(self._ctx, C.byref(o), P, arr, _i32_or_null(seq_a)),
+                    "plf_match_map2kf_batch")
         return [dict(lm_pt=lm_pt.copy(), n_pt=arr[k].n_pt, lm_ls=lm_ls.copy(), n_ls=arr[k].n_ls)
                 for k, (lm_pt, lm_ls) in enumerate(outs)]
 
@@ -926,17 +923,17 @@ class Frontend:
         """plf_bow_insert: stores the BoW vectors of the keyframe's descriptors under kf_idx and returns (score_p, score_l),
         float64 [kf_idx + 1] each (NaN: absent keyframe), None for a row not requested (rows) or of a disabled kind."""
         keep = []
-        fr = {}
-        if pdesc is not None:
-            fr["pdesc"] = pdesc
-        if ldesc is not None:
-            fr["ldesc"] = ldesc
-        v = _frame_view(fr, keep)
-        enabled = (self.params.has_points, self.params.has_lines)
-        out = [np.full(kf_idx + 1, np.nan) if (rows[c] and enabled[c] and kf_idx >= 0) else None for c in range(2)]
+        v = _frame_view({key: d for key, d in (("pdesc", pdesc), ("ldesc", ldesc)) if d is not None}, keep)
+        out = self._score_rows(kf_idx, rows)
         ptr = [C.c_void_p(o.ctypes.data) if o is not None else C.c_void_p() for o in out]
         self._check(self.lib.plf_bow_insert(self._ctx, int(kf_idx), C.byref(v), ptr[0], ptr[1]), "plf_bow_insert")
         return out[0], out[1]
+
+    def _score_rows(self, kf_idx, rows):
+        """The (score_p, score_l) rows a keyframe insert fills: NaN float64 [kf_idx + 1] for each kind requested in
+        `rows` and enabled in the context's parameters, else None."""
+        enabled = (self.params.has_points, self.params.has_lines)
+        return [np.full(kf_idx + 1, np.nan) if (rows[c] and enabled[c] and kf_idx >= 0) else None for c in range(2)]
 
     def bow_insert_batch(self, problems, seq=None, rows=(True, True)):
         """Many bow_insert in one device call (plf_bow_insert_batch).  problems: dicts kf_idx, pdesc, ldesc (either
@@ -946,18 +943,16 @@ class Frontend:
         problems = list(problems)
         P = len(problems)
         seq_a = self._problem_sequences(P, seq)
-        enabled = (self.params.has_points, self.params.has_lines)
         keep, outs = [], []
         arr = (plf_bow_problem * max(P, 1))()
         for k, pr in enumerate(problems):
             v = _frame_view({key: pr[key] for key in ("pdesc", "ldesc") if pr.get(key) is not None}, keep)
             keep.append(v)
             kf = int(pr["kf_idx"])
-            out = [np.full(kf + 1, np.nan) if (rows[c] and enabled[c] and kf >= 0) else None for c in range(2)]
+            out = self._score_rows(kf, rows)
             outs.append(tuple(out))
             arr[k] = plf_bow_problem(kf, C.pointer(v), *[o.ctypes.data if o is not None else None for o in out])
-        self._check(self.lib.plf_bow_insert_batch(self._ctx, P, arr, None if seq_a is None else _ptr(seq_a, C.c_int32)),
-                    "plf_bow_insert_batch")
+        self._check(self.lib.plf_bow_insert_batch(self._ctx, P, arr, _i32_or_null(seq_a)), "plf_bow_insert_batch")
         return outs
 
     def _lc_problem(self, pr, rows, conf, keep, who):
@@ -971,8 +966,7 @@ class Frontend:
                          if pr.get(key) is not None}, keep)
         keep.append(v)
         kf = int(pr["kf_idx"])
-        enabled = (self.params.has_points, self.params.has_lines)
-        out = [np.full(kf + 1, np.nan) if (rows[c] and enabled[c] and kf >= 0) else None for c in range(2)]
+        out = self._score_rows(kf, rows)
         cf = np.full(max(kf + 1, 1), np.nan, np.float32) if conf else None
         cov = pr.get("covis")
         if cov is not None:
@@ -1006,8 +1000,8 @@ class Frontend:
             arr[k], out, cf = self._lc_problem(pr, rows, conf, keep, f"bow_detect_batch: problem {k}")
             outs.append((out, cf))
         o = _lc_opts(opts)
-        self._check(self.lib.plf_bow_detect_batch(self._ctx, C.byref(o), P, arr,
-                                                  None if seq_a is None else _ptr(seq_a, C.c_int32)), "plf_bow_detect_batch")
+        self._check(self.lib.plf_bow_detect_batch(self._ctx, C.byref(o), P, arr, _i32_or_null(seq_a)),
+                    "plf_bow_detect_batch")
         return [self._lc_result(arr[k], out, cf) for k, (out, cf) in enumerate(outs)]
 
     def bow_detect(self, problem, opts=None, rows=(False, False), conf=True):
@@ -1138,23 +1132,28 @@ class Frontend:
         (LD, x, nz): LD holds L strictly below its diagonal and D on it (upper triangle unspecified); nz (path 0, else
         None) is the n_t x n_t zero flag of each L tile (i > k), n_t = ceil(n / 64).  overwrite_s: factor S's own buffer
         (a C-contiguous float64 array) instead of a copy.  plf_debug_ldlt."""
-        n = S.shape[0]
-        if S.shape != (n, n) or n % 6 or len(g) != n:
-            raise PlfError(f"debug_ldlt: S {S.shape} and g {len(g)} must be 6 n6 square and 6 n6 long")
+        g, x, nz = self._ldlt_buffers(S, g, "debug_ldlt")
         if overwrite_s:
             if S.dtype != np.float64 or not S.flags.c_contiguous or not S.flags.writeable:
                 raise PlfError("debug_ldlt: overwrite_s needs a writeable C-contiguous float64 S")
             LD = S
         else:
             LD = np.array(S, np.float64, order="C")
-        g = np.ascontiguousarray(g, np.float64)
-        x = np.empty(n, np.float64)
-        nt = (n + 63) // 64
-        nz = np.zeros((nt, nt), np.uint8) if path == 0 else None
-        st = self.lib.plf_debug_ldlt(self._ctx, int(path), n // 6, _ptr(LD, C.c_double), _ptr(g, C.c_double),
+        nz = nz if path == 0 else None
+        st = self.lib.plf_debug_ldlt(self._ctx, int(path), len(x) // 6, _ptr(LD, C.c_double), _ptr(g, C.c_double),
                                      _ptr(x, C.c_double), None if nz is None else _ptr(nz, C.c_uint8))
         self._check(st, "plf_debug_ldlt")
         return LD, x, nz
+
+    @staticmethod
+    def _ldlt_buffers(S, g, who):
+        """(g, x, nz) of one debug_ldlt system, once S is checked 6 n6 square and g 6 n6 long: g as float64, the
+        solution and the tile zero flags to fill."""
+        n = S.shape[0]
+        if S.shape != (n, n) or n % 6 or len(g) != n:
+            raise PlfError(f"{who}: S {S.shape} and g {len(g)} must be 6 n6 square and 6 n6 long")
+        nt = (n + 63) // 64
+        return np.ascontiguousarray(g, np.float64), np.empty(n, np.float64), np.zeros((nt, nt), np.uint8)
 
     def debug_ldlt_batch(self, mats):
         """debug_ldlt(S, g, path=0) on every (S, g) of `mats`, factored in one launch chain by the batched tiled LDL^T
@@ -1162,15 +1161,10 @@ class Frontend:
         mats = list(mats)
         n6, LDs, gs, xs, nzs = [], [], [], [], []
         for S, g in mats:
-            n = S.shape[0]
-            if S.shape != (n, n) or n % 6 or len(g) != n:
-                raise PlfError(f"debug_ldlt_batch: S {S.shape} and g {len(g)} must be 6 n6 square and 6 n6 long")
-            n6.append(n // 6)
+            g, x, nz = self._ldlt_buffers(S, g, "debug_ldlt_batch")
+            n6.append(len(x) // 6)
             LDs.append(np.array(S, np.float64, order="C"))
-            gs.append(np.ascontiguousarray(g, np.float64))
-            xs.append(np.empty(n, np.float64))
-            nt = (n + 63) // 64
-            nzs.append(np.zeros((nt, nt), np.uint8))
+            gs.append(g); xs.append(x); nzs.append(nz)
         k = max(len(mats), 1)
         ptrs = lambda arrs: (C.c_void_p * k)(*[a.ctypes.data for a in arrs])
         n6a = np.array(n6 or [0], np.int32)
@@ -1252,20 +1246,16 @@ class Frontend:
     @staticmethod
     def _sequence_table(B, seq, restart):
         """seq: integer [B] (sequence of each pair, None = all 0); restart: bool / integer [B] (None = none)."""
-        def vec(a, name, kinds):
-            a = np.asarray(a)
-            if a.shape != (B,) or a.dtype.kind not in kinds:
-                raise PlfError(f"{name} must be a 1-D {'bool or ' if 'b' in kinds else ''}integer array of {B} entries "
-                               f"(got {a.dtype}{list(a.shape)})")
-            return a
-        s = None if seq is None else np.ascontiguousarray(vec(seq, "seq", "iu"), np.int32)
-        if s is not None and not np.array_equal(s, np.asarray(seq)):
-            raise PlfError("seq: values do not fit int32")
-        r = None if restart is None else np.ascontiguousarray(vec(restart, "restart", "biu") != 0, np.uint8)
-        return s, r
+        s = Frontend._problem_sequences(B, seq)
+        if restart is None:
+            return s, None
+        r = np.asarray(restart)
+        if r.shape != (B,) or r.dtype.kind not in "biu":
+            raise PlfError(f"restart must be a 1-D bool or integer array of {B} entries (got {r.dtype}{list(r.shape)})")
+        return s, np.ascontiguousarray(r != 0, np.uint8)
 
     def _run_sequences(self, B, seq, restart):
-        self._check(self.lib.plf_batch_run_sequences(self._ctx, int(B), None if seq is None else _ptr(seq, C.c_int32),
+        self._check(self.lib.plf_batch_run_sequences(self._ctx, int(B), _i32_or_null(seq),
                                                      None if restart is None else _ptr(restart, C.c_uint8)),
                     "plf_batch_run_sequences")
 
