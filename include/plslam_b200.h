@@ -749,6 +749,33 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
 plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam);
 /* The calibration the next batch will use for sequence s: its own, or the context's camera. */
 plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out);
+
+/* stvo-pl's adaptative_fast (config_euroc.yaml:17, :36-41): each sequence's FAST threshold follows its last tracked frame.
+ * The fields are the config keys fast_min_th, fast_max_th, fast_inc_th, fast_feat_th and fast_err_th. */
+typedef struct plf_adaptive_fast {
+  int min_th, max_th, inc_th, feat_th;
+  double err_th;
+} plf_adaptive_fast;
+/* Turns the adaptation on (cfg != NULL) or off (NULL, the default) for the batched pipeline; plf_orb and the other
+ * standalone detectors keep plf_params.orb_fast_th.  With it on, pair k of a batch is detected (both images) at its
+ * sequence's threshold, and after the pose that threshold moves by the rule of DESIGN.md section 8:
+ *   first frame (status 2)                      unchanged
+ *   DT == identity exactly, or err > err_th     th = max(min_th, th - 2 inc_th)   (status 1 has DT = identity)
+ *   else n_inliers_pt <  feat_th                th = max(min_th, th - 2 inc_th)
+ *   else n_inliers_pt <  2 feat_th              th = max(min_th, th - inc_th)
+ *   else n_inliers_pt >  3 feat_th              th = min(max_th, th + inc_th)
+ * Every first frame of a sequence (its first pair, restart[k], plf_reset_sequence, plf_set_sequence_camera) is detected
+ * at orb_fast_th (clamped to [0, 255]).  Frame k of a sequence needs the threshold frame k-1's pose gives, so with the
+ * adaptation on a batch may hold at most one pair of each sequence: plf_batch_run_sequences refuses a batch with two pairs
+ * of one sequence (PLF_ERR_INVALID, before anything is enqueued, no sequence state changed).  A single sequence therefore
+ * runs B = 1; many sequences run round-robin, one pair of each per batch (INTEGRATION.md section 4a).
+ * Valid only with no batch in flight (PLF_ERR_STATE).  PLF_ERR_INVALID, naming the field, unless
+ * 0 <= min_th <= max_th <= 255, inc_th >= 0, feat_th >= 0 and err_th is finite; nothing changes on a refusal.  A successful
+ * call sets every sequence's threshold back to orb_fast_th. */
+plf_status plf_set_adaptive_fast(plf_ctx* ctx, const plf_adaptive_fast* cfg);
+/* *th = the FAST threshold the next pair of sequence s will be detected with (orb_fast_th with the adaptation off or when
+ * that pair is a first frame).  May be called at any time; with batches in flight it waits for their match phases. */
+plf_status plf_get_sequence_fast_th(plf_ctx* ctx, int s, int* th);
 /* Poses of the OLDEST batch in flight, device to device: dst_device[B][16] f64 (DT, row-major) is filled on `stream`
  * (a cudaStream_t of the caller; NULL = an internal stream, synchronised before returning) behind that batch's match
  * phase - the buffer a multi-GPU caller passes to its NCCL pose all-gather on the same stream (SURVEY 8e; the reference

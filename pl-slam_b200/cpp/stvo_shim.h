@@ -273,13 +273,21 @@ class StereoFrame {
 // stvo-pl StereoFrameHandler (driven at app/plslam_dataset.cpp:109-159; reused at src/mapHandler.cpp:769-807)
 class StereoFrameHandler {
  public:
-  explicit StereoFrameHandler(PinholeStereoCamera* cam_, const plf_params* params = nullptr, int device = 0) : cam(cam_) {
+  // adaptive_fast: stvo-pl's adaptative_fast with its fast_*_th values, or NULL for a fixed orb_fast_th.  One frame per
+  // call (B = 1) is what makes the adaptation exact: frame k is detected at the threshold frame k-1's pose gave.
+  explicit StereoFrameHandler(PinholeStereoCamera* cam_, const plf_params* params = nullptr, int device = 0,
+                              const plf_adaptive_fast* adaptive_fast = nullptr) : cam(cam_) {
     plf_limits lim;
     plf_default_limits(&lim);
     lim.max_batch = 1;  // the class API is one frame per call; batched callers use plf_process_batch directly
     if (params) prm_ = *params; else plf_default_params(&prm_);
     if (plf_create(&prm_, &cam->raw(), &lim, device, &ctx_) != PLF_OK)
       throw std::runtime_error(std::string("[StereoFrameHandler] ") + plf_last_error(nullptr));
+    if (adaptive_fast && plf_set_adaptive_fast(ctx_, adaptive_fast) != PLF_OK) {
+      const std::string e = plf_last_error(ctx_);
+      plf_destroy(ctx_);
+      throw std::runtime_error("[StereoFrameHandler] " + e);
+    }
     lim_ = lim;
   }
   ~StereoFrameHandler() {
@@ -369,6 +377,14 @@ class StereoFrameHandler {
     T_prevKF = curr_frame->Tfw;
     cov_prevKF_currF = Matrix6d::Zero();
     N_prevKF_currF = 0;
+  }
+
+  // stvo-pl's orb_fast_th member: the FAST threshold the next frame is detected with (initialize() uses orb_fast_th).
+  // With adaptive_fast the device moves it after every tracked frame, so updateFrame has nothing left to do for it.
+  int orbFastTh() {
+    int th = 0;
+    check(plf_get_sequence_fast_th(ctx_, 0, &th));
+    return th;
   }
 
   // app/plslam_dataset.cpp:159

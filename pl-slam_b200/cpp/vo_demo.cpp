@@ -763,6 +763,16 @@ int main(int argc, char** argv) {
     bow_voc[1] = argv[argc - 1];
     argc -= 3;
   }
+  // --adaptive-fast min max inc feat err: stvo-pl's adaptative_fast (fast_min_th .. fast_err_th); prints "fast_th k th",
+  // the threshold frame k was detected with, after each frame's line
+  plf_adaptive_fast afast;
+  bool afast_on = false;
+  if (argc >= 7 && std::string(argv[argc - 6]) == "--adaptive-fast") {
+    afast = {std::atoi(argv[argc - 5]), std::atoi(argv[argc - 4]), std::atoi(argv[argc - 3]), std::atoi(argv[argc - 2]),
+             std::atof(argv[argc - 1])};
+    afast_on = true;
+    argc -= 6;
+  }
   if (argc >= 2 && std::string(argv[argc - 1]) == "--grid-selftest") { grid_test = true; --argc; }
   if (argc >= 2 && std::string(argv[argc - 1]) == "--kf-match-selftest") { kf_test = true; --argc; }
   if (argc < 2) {
@@ -781,7 +791,7 @@ int main(int argc, char** argv) {
     plf_params prm;
     plf_default_params(&prm);
     if (argc >= 4) { prm.orb_nfeatures = std::atoi(argv[2]); prm.lsd_nfeatures = std::atoi(argv[3]); }
-    StVO::StereoFrameHandler* StVO_ = new StVO::StereoFrameHandler(&cam_pin, &prm);   // app:109
+    StVO::StereoFrameHandler* StVO_ = new StVO::StereoFrameHandler(&cam_pin, &prm, 0, afast_on ? &afast : nullptr);   // app:109
     KfArrays* first_kf = nullptr;   // --kf-match-selftest: frame 0 against the last frame
     BowMap bow = {StVO_->ctx(), prm.has_points != 0, prm.has_lines != 0, {}, {}};
     LcMap lc = {bow, {}, 1, 2, 1, 20, 0};
@@ -795,6 +805,7 @@ int main(int argc, char** argv) {
       plf::Image img_l{buf.data(), w, h, w}, img_r{buf.data() + (size_t)w * h, w, h, w};
       bool new_kf = false;
       StVO::StereoFrame* cur;
+      const int fast_th = StVO_->orbFastTh();
       if (frame_counter == 0) {
         StVO_->initialize(img_l, img_r, 0);                                             // app:115
         cur = StVO_->prev_frame;
@@ -813,6 +824,7 @@ int main(int argc, char** argv) {
                   StVO_->n_inliers, new_kf ? 1 : 0);
       for (int i = 0; i < 16; ++i) std::printf(" %.17g", cur->Tfw.v[i]);
       std::printf("\n");
+      if (afast_on) std::printf("fast_th %d %d\n", frame_counter, fast_th);
       if (bow_voc[0] && !lc_test) bow_selftest_frame(bow, cur, frame_counter);
       if (lc_test) lc_selftest_frame(lc, cur, frame_counter);
       if (kf_test && frame_counter == 0) first_kf = new KfArrays(cur);

@@ -223,7 +223,7 @@ __device__ __forceinline__ uint32_t fast_gt4(uint32_t d, uint32_t k7, bool th_sm
   return (th_small ? (low | d) : (low & d)) & 0x80808080u;
 }
 __global__ void __launch_bounds__(256, 5) k_fast_nms(const __grid_constant__ CUtensorMap tmap, OrbGeom g, int l, int tiles_x,
-                                                  uint32_t* __restrict__ cand, int* __restrict__ cand_count,
+                                                  const int* __restrict__ img_th, uint32_t* __restrict__ cand, int* __restrict__ cand_count,
                                                   int* __restrict__ hist, int* __restrict__ overflow) {
   const int W = g.w[l], H = g.h[l];
   const int x0 = (blockIdx.x % tiles_x) * FN_OW, y0 = (blockIdx.x / tiles_x) * FN_OH;
@@ -247,7 +247,7 @@ __global__ void __launch_bounds__(256, 5) k_fast_nms(const __grid_constant__ CUt
   const int boxoff = (x0 - 4) - xs;   // box column of pixel x0 - 4
   // px[ry][rx] = pixel (x0 - 4 + rx, y0 - 4 + ry)
   const uint8_t (*px)[96] = reinterpret_cast<const uint8_t (*)[96]>(&pxb[0][boxoff]);
-  const int th = g.fast_th;
+  const int th = img_th ? img_th[img] : g.fast_th;   // per image with the adaptive FAST threshold, in [0, 255] either way
   const uint32_t k7 = (uint32_t)(0x7f - (th & 0x7f)) * 0x01010101u;
   const bool th_small = th < 128;
   plf_mbar_wait(&bar, 0);
@@ -792,7 +792,8 @@ plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_paritie
 
 // Runs ORB on nimg (<= s->nimg) images of s->w x s->h resident at d_imgs ([nimg][h][pitch], pitch a multiple of 16,
 // stride img_stride bytes).  Enqueued on cs; results stay on the device.
-plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par) {
+plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par,
+                       const int* img_th) {
   const int w = s->w, h = s->h;
   plf_status st;
   OrbGeom g = s->g;
@@ -814,7 +815,7 @@ plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t
   plf_mark(ctx, cs, "orb.k_resize_exact");
   for (int l = 0; l < g.nlevels; ++l) {
     const int tx_ = (g.w[l] + FN_OW - 1) / FN_OW, ty_ = (g.h[l] + FN_OH - 1) / FN_OH;
-    k_fast_nms<<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(l == 0 ? *tm_fast0 : s->tm_fast[l], g, l, tx_, s->cand, s->cand_count,
+    k_fast_nms<<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(l == 0 ? *tm_fast0 : s->tm_fast[l], g, l, tx_, img_th, s->cand, s->cand_count,
                                                       s->hist, s->overflow);
     PLF_LAUNCH_CHECK(ctx);
   }
@@ -882,7 +883,7 @@ extern "C" plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   uint8_t* dimg = (uint8_t*)plf_scratch(ctx, PLF_SCR_ORB, (size_t)pitch * h);
   if (!dimg) return PLF_ERR_CUDA;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  if ((st = plf_orb_run(ctx, ctx->stream, s, dimg, (size_t)pitch * h, pitch, 1, 0))) return st;
+  if ((st = plf_orb_run(ctx, ctx->stream, s, dimg, (size_t)pitch * h, pitch, 1, 0, nullptr))) return st;
   int n = 0, ovf = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->kp_count[0], sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyAsync(&ovf, s->overflow, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));

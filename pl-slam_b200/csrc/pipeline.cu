@@ -70,6 +70,11 @@ struct PipeState {
   short2* lbd_grad[2] = {nullptr, nullptr};  // [parity][2B][h*w]
   uint8_t* ldesc_raw = nullptr;  // [2B][max_ln][32]  LBD of every kept KeyLine
   FrameSlots fs;               // B + nseq + 1 slots
+  // plf_set_adaptive_fast: seq_th[s] = the FAST threshold of sequence s's next pair unless that pair is a first frame
+  // (written by k_fast_th_update, behind ev_th on the M stream); img_th = the threshold of each image of the running batch
+  int* seq_th = nullptr;       // [nseq]
+  int* img_th = nullptr;       // [2B]
+  cudaEvent_t ev_th = nullptr;
   // matching scratch
   uint32_t* knn_keys = nullptr;   // [B][8][2][max_kp]
   int32_t* m12 = nullptr;         // [B][4][max_kp]  stereo pts, stereo lines, f2f pts, f2f lines
@@ -129,6 +134,8 @@ static void pipe_buffers(PipeState* s, bool windowed, DevBufList& b) {
   PLF_PT_FIELDS(PLF_FS_ALLOC) b.add(f.pt_count, S);
   PLF_LS_FIELDS(PLF_FS_ALLOC) b.add(f.ls_count, S);
 #undef PLF_FS_ALLOC
+  b.add(s->seq_th, s->nseq);
+  b.add(s->img_th, 2 * B);
   b.add(s->knn_keys, B * 8 * 2 * K);
   b.add(s->m12, B * 4 * K);
   b.add(s->mcount, B * 4);
@@ -162,7 +169,8 @@ static std::vector<PipeEvents> pipe_events(PipeState* s) {
   return {{s->ev_up, 2, cudaEventDisableTiming}, {s->ev_free, 2, cudaEventDisableTiming}, {s->ev_free2, 2, cudaEventDisableTiming},
           {s->evM, 3, cudaEventBlockingSync},    {s->tM0, 3, cudaEventDefault},           {s->evE, 2, cudaEventDefault},
           {s->evG, 2, cudaEventDefault},         {s->evX, 2, cudaEventDisableTiming},     {s->evP, 2, cudaEventDisableTiming},
-          {s->tE0, 2, cudaEventDefault},         {s->tG0, 2, cudaEventDefault},           {s->ev_tab, 3, cudaEventDisableTiming}};
+          {s->tE0, 2, cudaEventDefault},         {s->tG0, 2, cudaEventDefault},           {s->ev_tab, 3, cudaEventDisableTiming},
+          {&s->ev_th, 1, cudaEventDisableTiming}};
 }
 
 extern "C" void plf_pipe_free(plf_ctx* ctx) {
@@ -498,6 +506,54 @@ __global__ void k_finalize(const plf_pose_result* __restrict__ gn, const int* __
   out[k] = r;
 }
 
+// ---- adaptative_fast (plf_set_adaptive_fast, DESIGN.md §8).  A batch holds at most one pair of each sequence, so prev[k]
+// is the empty slot (a first frame) or pair k's carry slot carry0 + s, and every pair is in the carry list. ----
+
+// The FAST threshold of both images of pair k: its sequence's, or th0 = orb_fast_th for a first frame.
+__global__ void k_fast_th_images(const int* __restrict__ prev, int B, int carry0, int empty, int th0,
+                                 const int* __restrict__ seq_th, int* __restrict__ img_th) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= B) return;
+  const int p = prev[k];
+  const int th = p == empty ? th0 : seq_th[p - carry0];
+  img_th[2 * k] = th;
+  img_th[2 * k + 1] = th;
+}
+
+// StereoFrameHandler::updateFrame's threshold step after pair k, detected at th with result r.  stvo-pl goes on with
+// "else if n_inliers_pt > 4 feat_th: th + 2 inc_th", which the "> 3 feat_th" test before it leaves unreachable.
+__device__ __forceinline__ int fast_th_next(int th, const plf_frame_result& r, const plf_adaptive_fast& a) {
+  if (r.status == 2) return th;   // initialize() runs no updateFrame
+  bool ident = true;
+  for (int i = 0; i < 16; ++i) ident &= r.DT[i] == ((i % 5 == 0) ? 1.0 : 0.0);
+  const long long n = r.n_inliers_pt, f = a.feat_th, t = th;
+  if (ident || r.err > a.err_th || n < f) return (int)max((long long)a.min_th, t - 2ll * a.inc_th);
+  if (n < 2 * f) return (int)max((long long)a.min_th, t - a.inc_th);
+  if (n > 3 * f) return (int)min((long long)a.max_th, t + a.inc_th);
+  return th;
+}
+
+// Carry entry j = (pair k, carry slot carry0 + s): sequence s's next threshold from pair k's result.
+__global__ void k_fast_th_update(const plf_frame_result* __restrict__ res, const int* __restrict__ carry, int ncarry, int carry0,
+                                 const int* __restrict__ img_th, plf_adaptive_fast a, int* __restrict__ seq_th) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= ncarry) return;
+  const int k = carry[2 * j];
+  seq_th[carry[2 * j + 1] - carry0] = fast_th_next(img_th[2 * k], res[k], a);
+}
+
+// orb_fast_th as k_fast_nms applies it without a per-image threshold
+static int fast_th0(const plf_ctx* ctx) { return std::min(std::max(ctx->params.orb_fast_th, 0), 255); }
+
+// Every sequence's threshold back to orb_fast_th (no batch in flight).
+static plf_status pipe_fast_th_reset(plf_ctx* ctx) {
+  PipeState* s = ctx->pipe;
+  const std::vector<int> v(s->nseq, fast_th0(ctx));
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->seq_th, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return PLF_OK;
+}
+
 // ---- windowed matching: grid geometry on the device (oracle/frontend.py grid_match_points / grid_match_lines) ----
 // (cells and projection: plf_geom.cuh)
 
@@ -653,7 +709,7 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
   PLF_CUDA(ctx, cudaMemcpyAsync(s->nnr_stereo, ns.data(), ns.size() * sizeof(NnrProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->gn_probs, gp.data(), gp.size() * sizeof(GnProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaStreamSynchronize(cs));
-  return PLF_OK;
+  return ctx->afast_on ? pipe_fast_th_reset(ctx) : PLF_OK;
 }
 
 // Builds the pipeline for the camera's image size on first use; a failed setup leaves no state behind.
@@ -669,6 +725,7 @@ struct BatchRun {
   int B;
   int ncarry;    // entries of the carry list in h_tab[rp]: the sequences the batch holds
   bool cams;     // h_cam[rp] holds the pairs' cameras (a sequence of the batch has its own); else the context's camera
+  bool afast;    // adaptive FAST thresholds (plf_set_adaptive_fast): the sequence table goes up before the E phase, which reads it
   int par;       // parity of the E -> G -> M hand-off buffers
   int lp;        // parity of the LSD hand-off buffers (0 when they exist once)
   int rp;        // slot of the result ring
@@ -676,6 +733,19 @@ struct BatchRun {
   bool piped, lsd2;
   cudaStream_t sM, sE, sG, sP;
 };
+
+// The batch's sequence table (prev[B], then the carry list) and its pairs' cameras, to ring entry rp of the device on the
+// copy stream, in order behind the batch's own images and ahead of the next batch's upload; ev_tab[rp] marks them.
+static plf_status send_tab(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
+  const int rp = r.rp;
+  int32_t* prev = s->seq_tab + (size_t)rp * 3 * s->B;
+  PLF_CUDA(ctx, cudaMemcpyAsync(prev, s->h_tab[rp], sizeof(int32_t) * r.B, cudaMemcpyHostToDevice, s->copy));
+  PLF_CUDA(ctx, cudaMemcpyAsync(prev + s->B, s->h_tab[rp] + s->B, sizeof(int32_t) * 2 * r.ncarry, cudaMemcpyHostToDevice, s->copy));
+  if (r.cams)
+    PLF_CUDA(ctx, cudaMemcpyAsync(s->cam_tab + (size_t)rp * s->B, s->h_cam[rp], sizeof(PlfPairCam) * r.B, cudaMemcpyHostToDevice, s->copy));
+  PLF_CUDA(ctx, cudaEventRecord(s->ev_tab[rp], s->copy));
+  return PLF_OK;
+}
 
 // ---- E phase: ORB + LBD gradient prelude (bandwidth / ALU bound); outputs per batch parity ----
 static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
@@ -687,7 +757,18 @@ static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->evX[par], 0));           // batch i-2 (same parity) no longer reads these buffers
   plf_mark(ctx, sE, "start");
   PLF_CUDA(ctx, cudaEventRecord(s->tE0[par], sE));
-  plf_status st = plf_orb_run(ctx, sE, s->orb, imgs, AP, s->pitch, 2 * B, par);
+  const int* img_th = nullptr;
+  if (r.afast) {
+    // the thresholds of the batch's images: the sequence table, and the previous batch's threshold update (which has
+    // also read img_th for the last time)
+    PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_tab[r.rp], 0));
+    PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_th, 0));
+    k_fast_th_images<<<(B + 127) / 128, 128, 0, sE>>>(s->seq_tab + (size_t)r.rp * 3 * s->B, B, s->B, s->B + s->nseq, fast_th0(ctx),
+                                                      s->seq_th, s->img_th);
+    PLF_LAUNCH_CHECK(ctx);
+    img_th = s->img_th;
+  }
+  plf_status st = plf_orb_run(ctx, sE, s->orb, imgs, AP, s->pitch, 2 * B, par, img_th);
   if (!st) st = plf_launch_blur5_sobel(ctx, sE, &s->lbd_tm, imgs, s->pitch, AP, w, h, 2 * B, s->lbd_grad[par], A);
   if (st) return st;
   plf_mark(ctx, sE, "lbd.k_blur5_sobel");
@@ -764,12 +845,9 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   // the batch's sequence table: prev[B], then the carry list
   int32_t* prev = s->seq_tab + (size_t)rp * 3 * s->B;
   int32_t* carry = prev + s->B;
-  PLF_CUDA(ctx, cudaMemcpyAsync(prev, s->h_tab[rp], sizeof(int32_t) * B, cudaMemcpyHostToDevice, s->copy));
-  PLF_CUDA(ctx, cudaMemcpyAsync(carry, s->h_tab[rp] + s->B, sizeof(int32_t) * 2 * r.ncarry, cudaMemcpyHostToDevice, s->copy));
   // the pairs' cameras, when the batch has them (null: every kernel takes the context's camera)
   PlfPairCam* pcam = r.cams ? s->cam_tab + (size_t)rp * s->B : nullptr;
-  if (pcam) PLF_CUDA(ctx, cudaMemcpyAsync(pcam, s->h_cam[rp], sizeof(PlfPairCam) * B, cudaMemcpyHostToDevice, s->copy));
-  PLF_CUDA(ctx, cudaEventRecord(s->ev_tab[rp], s->copy));
+  if (!r.afast && (st = send_tab(ctx, s, r))) return st;   // with adaptive FAST thresholds the E phase sent it
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_tab[rp], 0));
   k_f2f_problems<<<(B + 127) / 128, 128, 0, cs>>>(s->fs, prev, B, K, Ln, s->knn_keys, s->m12, s->mcount, P.min_ratio_12_p,
                                                   P.min_ratio_12_l, P.best_lr_matches ? 1 : 0, s->knn_f2f, s->nnr_f2f);
@@ -859,6 +937,12 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_LAUNCH_CHECK(ctx);
   k_carry<<<dim3(PLF_FS_NFIELDS, r.ncarry), 256, 0, cs>>>(s->fs, carry, K, Ln);   // the next batch tracks against these
   PLF_LAUNCH_CHECK(ctx);
+  if (r.afast) {   // the next batch's E phase waits for its sequences' thresholds
+    k_fast_th_update<<<(r.ncarry + 127) / 128, 128, 0, cs>>>(s->results + (size_t)rp * s->B, carry, r.ncarry, s->B, s->img_th,
+                                                             ctx->afast, s->seq_th);
+    PLF_LAUNCH_CHECK(ctx);
+    PLF_CUDA(ctx, cudaEventRecord(s->ev_th, cs));
+  }
   plf_mark(ctx, cs, "k_finalize+carry");
   // results + overflow flags to pinned memory as part of this batch's stream work; evM marks them ready
   PLF_CUDA(ctx, cudaMemcpyAsync(s->h_results[rp], s->results + (size_t)rp * s->B, sizeof(plf_frame_result) * B, cudaMemcpyDeviceToHost, cs));
@@ -928,6 +1012,45 @@ plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out) {
   return PLF_OK;
 }
 
+plf_status plf_set_adaptive_fast(plf_ctx* ctx, const plf_adaptive_fast* cfg) {
+  if (cfg) {   // checked first, so that a NULL context reports the field too (plf_last_error(NULL))
+    const plf_adaptive_fast& a = *cfg;
+    if (a.min_th < 0) return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_adaptive_fast: min_th = %d, need 0 <= min_th", a.min_th);
+    if (a.max_th > 255) return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_adaptive_fast: max_th = %d, need max_th <= 255", a.max_th);
+    if (a.min_th > a.max_th)
+      return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_adaptive_fast: min_th = %d > max_th = %d, need min_th <= max_th", a.min_th, a.max_th);
+    if (a.inc_th < 0) return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_adaptive_fast: inc_th = %d, need inc_th >= 0", a.inc_th);
+    if (a.feat_th < 0) return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_adaptive_fast: feat_th = %d, need feat_th >= 0", a.feat_th);
+    if (!std::isfinite(a.err_th)) return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_adaptive_fast: err_th = %g, need a finite value", a.err_th);
+  }
+  if (!ctx) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_set_adaptive_fast: ctx is NULL");
+  if (ctx->pipe && ctx->pipe->n_pending)
+    return plf_fail(ctx, PLF_ERR_STATE, "plf_set_adaptive_fast: %d batch(es) still in flight; download them first", ctx->pipe->n_pending);
+  if (cfg && ctx->pipe) {
+    PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+    const plf_status st = pipe_fast_th_reset(ctx);
+    if (st) return st;
+  }
+  ctx->afast_on = cfg != nullptr;
+  ctx->afast = cfg ? *cfg : plf_adaptive_fast{};
+  return PLF_OK;
+}
+
+plf_status plf_get_sequence_fast_th(plf_ctx* ctx, int s, int* th) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (!th) return plf_fail(ctx, PLF_ERR_INVALID, "plf_get_sequence_fast_th: th is NULL");
+  if (s < 0 || s >= ctx->max_sequences)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_get_sequence_fast_th: s = %d outside [0, %d)", s, ctx->max_sequences);
+  *th = fast_th0(ctx);
+  if (!ctx->afast_on || !ctx->pipe || !ctx->pipe->carried[s]) return PLF_OK;   // the next pair is detected at orb_fast_th
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  int v = 0;   // behind the threshold updates of every batch in flight (M stream)
+  PLF_CUDA(ctx, cudaMemcpyAsync(&v, ctx->pipe->seq_th + s, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  *th = v;
+  return PLF_OK;
+}
+
 plf_status plf_batch_upload(plf_ctx* ctx, int B, const uint8_t* left, const uint8_t* right, int stride) {
   if (!ctx || !left || !right || B < 1 || B > ctx->limits.max_batch || stride < ctx->cam.width)
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload: bad arguments (B=%d, max_batch=%d)", B, ctx ? ctx->limits.max_batch : 0);
@@ -991,6 +1114,19 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   PipeState* s = ctx->pipe;
   if (s->n_pending >= 3)
     return plf_fail(ctx, PLF_ERR_STATE, "plf_batch_run: three batches already in flight; call plf_batch_download first");
+  if (ctx->afast_on) {   // pair k of a sequence is detected at the threshold pair k-1's pose gives: one pair per sequence
+    int first = -1, dup = -1;
+    for (int k = 0; k < B && dup < 0; ++k) {
+      int& last = s->last_pair[seq ? seq[k] : 0];
+      if (last >= 0) { first = last; dup = k; }
+      else last = k;
+    }
+    for (int k = 0; k < B; ++k) s->last_pair[seq ? seq[k] : 0] = -1;
+    if (dup >= 0)
+      return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_run_sequences: pairs %d and %d are both of sequence %d; with adaptive FAST "
+                      "thresholds (plf_set_adaptive_fast) a batch holds at most one pair of each sequence",
+                      first, dup, seq ? seq[dup] : 0);
+  }
   BatchRun r;
   r.B = B;
   r.par = (int)(s->seq & 1);
@@ -1033,7 +1169,9 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   r.sE = r.piped ? ctx->aux[0] : r.sM;
   r.sG = r.piped ? ctx->aux[1] : r.sM;
   r.sP = (r.piped && r.lsd2) ? ctx->aux[2] : r.sG;   // LSD pre-grow chain: own stream when its outputs exist per parity
-  st = run_extract(ctx, s, r);
+  r.afast = ctx->afast_on;
+  st = r.afast ? send_tab(ctx, s, r) : PLF_OK;
+  if (!st) st = run_extract(ctx, s, r);
   if (!st) st = run_lsd(ctx, s, r);
   if (!st) st = run_match(ctx, s, r);
   for (int k = 0; k < B; ++k) {

@@ -87,6 +87,8 @@ struct plf_ctx {
   // where seq_cam_own[s], else cam.  plf_set_max_sequences clears both.
   std::vector<plf_camera> seq_cam;
   std::vector<uint8_t> seq_cam_own;
+  bool afast_on = false;          // plf_set_adaptive_fast: per-sequence FAST thresholds in the batched pipeline
+  plf_adaptive_fast afast = {};
   std::string err;
   long long launches = 0;
   // scratch slots (device) of the host-pointer operator entry points
@@ -261,7 +263,9 @@ plf_status gbb_ldlt(plf_ctx* ctx, cudaStream_t cs, const GbbLdlt& L, int nb, int
 // nothing is left allocated and *out is untouched.
 plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, OrbState** out);
 void plf_orb_free(OrbState* s);
-plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par);
+// img_th: the FAST threshold of each image, on the device (plf_set_adaptive_fast), or NULL for plf_params.orb_fast_th.
+plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par,
+                       const int* img_th);
 void plf_orb_outputs(const OrbState* s, int par, plf_keypoint** kps, uint8_t** desc, int** counts, int* max_kp);
 // The overflow flag is a set of causes (one bit each, OR-ed in by the kernel that met it); plf_orb_overflow_text words them,
 // naming the limit that was actually hit: only max_keypoints is the caller's to raise.

@@ -56,6 +56,14 @@ class plf_limits(C.Structure):
                 ("max_lines", C.c_int)]
 
 
+class plf_adaptive_fast(C.Structure):
+    _fields_ = [("min_th", C.c_int), ("max_th", C.c_int), ("inc_th", C.c_int), ("feat_th", C.c_int), ("err_th", C.c_double)]
+
+
+# stvo-pl's fast_*_th block as every reference config sets it (config_euroc.yaml:36-41; fast_min_th 0 in config_kitti.yaml)
+ADAPTIVE_FAST_DEFAULTS = dict(min_th=5, max_th=50, inc_th=5, feat_th=50, err_th=0.5)
+
+
 class plf_lba_opts(C.Structure):
     _fields_ = [("lambda_", C.c_double), ("lambda_k", C.c_double), ("max_iters", C.c_int), ("homog_th", C.c_double),
                 ("min_error", C.c_double), ("min_error_change", C.c_double), ("ref_quirks", C.c_int)]
@@ -430,8 +438,10 @@ class Frontend:
     (app/plslam_dataset.cpp:109) plus the free operators the reference calls on the path."""
 
     def __init__(self, params: plf_params | None = None, camera: dict | plf_camera | None = None,
-                 limits: plf_limits | None = None, device: int = 0, max_sequences: int = 1, **overrides):
-        """max_sequences: the number of sequences batch_run / process_batch can track at once (plf_set_max_sequences)."""
+                 limits: plf_limits | None = None, device: int = 0, max_sequences: int = 1,
+                 adaptive_fast: dict | None = None, **overrides):
+        """max_sequences: the number of sequences batch_run / process_batch can track at once (plf_set_max_sequences).
+        adaptive_fast: None, or the per-sequence FAST threshold adaptation as set_adaptive_fast takes it."""
         self.lib = load_library()
         self.params = params if params is not None else default_params()
         for k, v in overrides.items():
@@ -450,6 +460,8 @@ class Frontend:
             raise PlfError(f"plf_create failed ({st}): {self.lib.plf_last_error(None).decode()}")
         try:
             self._check(self.lib.plf_set_max_sequences(self._ctx, int(max_sequences)), "plf_set_max_sequences")
+            if adaptive_fast is not None:
+                self.set_adaptive_fast(adaptive_fast)
         except PlfError:
             self.close()
             raise
@@ -1196,6 +1208,25 @@ class Frontend:
         out = plf_camera()
         self._check(self.lib.plf_get_sequence_camera(self._ctx, int(s), C.byref(out)), "plf_get_sequence_camera")
         return {name: getattr(out, name) for name, _ in plf_camera._fields_}
+
+    def set_adaptive_fast(self, cfg=None):
+        """stvo-pl's adaptative_fast for the batched pipeline: a dict of min_th, max_th, inc_th, feat_th and err_th (the
+        config keys fast_*_th; missing keys take ADAPTIVE_FAST_DEFAULTS), or None to turn it off.  With it on, a batch
+        holds at most one pair of each sequence.  Every sequence's threshold starts again at orb_fast_th.
+        plf_set_adaptive_fast."""
+        a = None
+        if cfg is not None:
+            unknown = set(cfg) - set(ADAPTIVE_FAST_DEFAULTS)
+            if unknown:
+                raise PlfError(f"unknown adaptive_fast keys {sorted(unknown)}")
+            a = plf_adaptive_fast(**dict(ADAPTIVE_FAST_DEFAULTS, **cfg))
+        self._check(self.lib.plf_set_adaptive_fast(self._ctx, None if a is None else C.byref(a)), "plf_set_adaptive_fast")
+
+    def sequence_fast_th(self, s):
+        """The FAST threshold the next pair of sequence s will be detected with.  plf_get_sequence_fast_th."""
+        th = C.c_int(0)
+        self._check(self.lib.plf_get_sequence_fast_th(self._ctx, int(s), C.byref(th)), "plf_get_sequence_fast_th")
+        return th.value
 
     @staticmethod
     def _result_dicts(res, B):
