@@ -750,6 +750,31 @@ plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam);
 /* The calibration the next batch will use for sequence s: its own, or the context's camera. */
 plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out);
 
+/* Rectification of sequence s's raw pairs before extraction: stvo-pl's dataset reader
+ * cv::remap(img, out, map1, map2, INTER_LINEAR) with the default BORDER_CONSTANT 0, per image.  map1_*: w x h x 2 int16
+ * (x, y) and map2_*: w x h uint16, as cv::initUndistortRectifyMap(..., CV_16SC2) or cv::convertMaps give them, for the
+ * context's w x h (host arrays, copied).  All four NULL clears it.  The camera of the rectified images (P1's fx, fy, cx, cy
+ * and the baseline) is the caller's to set with plf_set_sequence_camera.
+ *   - map2 is read as OpenCV reads it, map2 & 1023; map1 may point anywhere: taps outside the image read 0.  The result is
+ *     byte for byte cv::remap's (DESIGN.md section 8).
+ *   - The call may be made at any time, like plf_set_sequence_camera: the maps are resolved when a batch is run, so
+ *     batches already run keep the maps they were run with.  With batches in flight the call waits until their
+ *     rectifications (the first work of each run) have finished.
+ *   - A successful call restarts s, even when it clears maps or sets the same ones: its next pair is a first frame
+ *     (status 2).
+ *   - plf_set_max_sequences drops every sequence's maps; plf_reset_sequence keeps them.
+ *   - plf_batch_run_sequences rectifies the pairs of rectified sequences in the image slot it consumes, in place, before
+ *     extraction reads it (plf_batch_device_images then holds the rectified images).  Run each upload once: a second run
+ *     of the same slot would rectify it again.  A batch without a pair of a rectified sequence does no rectification work.
+ *   - The standalone operators (plf_orb, plf_lsd, plf_detect_lines, plf_lbd) do not rectify.
+ * Device memory: 12 w h bytes per rectified sequence (4.3 MB at 752 x 480, 5.6 MB at 1242 x 375), allocated when its maps
+ * are first set and freed when they are cleared, by plf_set_max_sequences or by plf_destroy.  The first run with a
+ * rectified pair also allocates a scratch of 2 max_batch h pitch bytes (plus its pair table) kept until plf_destroy.
+ * PLF_ERR_INVALID for s out of range or some but not all of the four pointers NULL, with nothing changed; PLF_ERR_CUDA
+ * when the maps cannot be allocated or copied. */
+plf_status plf_set_sequence_rectification(plf_ctx* ctx, int s, const int16_t* map1_l, const uint16_t* map2_l,
+                                          const int16_t* map1_r, const uint16_t* map2_r);
+
 /* stvo-pl's adaptative_fast (config_euroc.yaml:17, :36-41): each sequence's FAST threshold follows its last tracked frame.
  * The fields are the config keys fast_min_th, fast_max_th, fast_inc_th, fast_feat_th and fast_err_th. */
 typedef struct plf_adaptive_fast {
@@ -783,7 +808,9 @@ plf_status plf_get_sequence_fast_th(plf_ctx* ctx, int s, int* th);
  * until plf_batch_download. */
 plf_status plf_batch_device_poses(plf_ctx* ctx, int B, double* dst_device, void* stream);
 /* Device buffer [2*max_batch][h][pitch] read by plf_batch_run (image 2k = left k, 2k+1 = right k), pitch = width rounded up
- * to a multiple of 16 bytes (every halo tile of every image is then a legal TMA box). */
+ * to a multiple of 16 bytes (every halo tile of every image is then a legal TMA box).  It is the slot of the most recent
+ * upload; once that upload has been run, the pairs of rectified sequences (plf_set_sequence_rectification) in it are the
+ * rectified images. */
 void* plf_batch_device_images(plf_ctx* ctx);
 
 /* Stereo-valid features of frame k of the last batch (what `new KeyFrame(StVO->curr_frame)` deep-copies,

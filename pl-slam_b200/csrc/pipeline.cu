@@ -39,6 +39,14 @@ struct FrameSlots {
 constexpr int PLF_FS_NFIELDS = 0 PLF_PT_FIELDS(PLF_FS_ONE) PLF_LS_FIELDS(PLF_FS_ONE);
 #undef PLF_FS_ONE
 
+// ---- rectification (plf_set_sequence_rectification, DESIGN.md section 8) ----
+// A sequence's maps, one device block of 12 w h bytes: map1 (x, y) of the left then the right image (short2 [2][h][w]),
+// then map2 of the left then the right image (uint16 [2][h][w]).
+#define PLF_RECT_MAP1(base, A, side) (reinterpret_cast<const short2*>(base) + (size_t)(side) * (A))
+#define PLF_RECT_MAP2(base, A, side) (reinterpret_cast<const uint16_t*>((base) + 8 * (A)) + (size_t)(side) * (A))
+// One rectified pair of a batch: its index and its sequence's maps.
+struct PlfRectPair { const uint8_t* maps; int pair; int pad; };
+
 struct PipeState {
   int w = 0, h = 0, B = 0, max_kp = 0, max_ln = 0;
   int pitch = 0;               // row pitch of the device images: plf_pitch16(w) (16-byte rows: every halo tile is a legal TMA box)
@@ -59,6 +67,9 @@ struct PipeState {
   // others pass no table and the kernels take the context's camera.
   PlfPairCam* h_cam[3] = {nullptr, nullptr, nullptr};
   PlfPairCam* cam_tab = nullptr;
+  // The pairs to rectify (plf_set_sequence_rectification): pinned ring h_rect [3][max_batch] like h_tab; the device copy
+  // lives in scratch slot PLF_SCR_RECT_PIPE, written and read on the copy stream only.
+  PlfRectPair* h_rect[3] = {nullptr, nullptr, nullptr};
   uint8_t* imgs2[2] = {nullptr, nullptr};  // double-buffered [2B][h][pitch]: upload of batch i+1 overlaps the run of batch i
   uint8_t* stage = nullptr;    // dense [2B][h][w] landing buffer of the H2D copy (one contiguous DMA per side), repacked to the padded pitch on the device
   int up_slot = 0;             // slot written by the last plf_batch_upload
@@ -184,6 +195,7 @@ extern "C" void plf_pipe_free(plf_ctx* ctx) {
     if (s->h_ovf[i]) cudaFreeHost(s->h_ovf[i]);
     if (s->h_tab[i]) cudaFreeHost(s->h_tab[i]);
     if (s->h_cam[i]) cudaFreeHost(s->h_cam[i]);
+    if (s->h_rect[i]) cudaFreeHost(s->h_rect[i]);
   }
   for (const PipeEvents& a : pipe_events(s))
     for (int i = 0; i < a.n; ++i)
@@ -667,6 +679,7 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
     PLF_CUDA(ctx, cudaHostAlloc(&s->h_ovf[i], 2 * sizeof(int), cudaHostAllocDefault));
     PLF_CUDA(ctx, cudaHostAlloc(&s->h_tab[i], 3 * sizeof(int32_t) * B, cudaHostAllocDefault));
     PLF_CUDA(ctx, cudaHostAlloc(&s->h_cam[i], sizeof(PlfPairCam) * B, cudaHostAllocDefault));
+    PLF_CUDA(ctx, cudaHostAlloc(&s->h_rect[i], sizeof(PlfRectPair) * B, cudaHostAllocDefault));
   }
   FrameSlots& f = s->fs;
   cudaStream_t cs = ctx->stream;
@@ -744,6 +757,65 @@ static plf_status send_tab(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   if (r.cams)
     PLF_CUDA(ctx, cudaMemcpyAsync(s->cam_tab + (size_t)rp * s->B, s->h_cam[rp], sizeof(PlfPairCam) * r.B, cudaMemcpyHostToDevice, s->copy));
   PLF_CUDA(ctx, cudaEventRecord(s->ev_tab[rp], s->copy));
+  return PLF_OK;
+}
+
+// cv::remap(src, dst, map1, map2, INTER_LINEAR, BORDER_CONSTANT, 0) of one image of a rectified pair: grid.z = 2 j + side
+// for entry j of tab.  map2 & 1023 = 32 fy + fx selects OpenCV's weights 32 (32 - fx) (32 - fy), 32 fx (32 - fy),
+// 32 (32 - fx) fy and 32 fx fy of the taps (x, y), (x+1, y), (x, y+1), (x+1, y+1) (exact: no rounding excess to move),
+// so (sum w p + 2^14) >> 15 is (sum (w / 32) p + 2^9) >> 10.  Taps outside the image read 0.
+__global__ void __launch_bounds__(256) k_rectify(const PlfRectPair* __restrict__ tab, const uint8_t* __restrict__ imgs, size_t AP,
+                                                 int pitch, int w, int h, uint8_t* __restrict__ out) {
+  const int x = blockIdx.x * 32 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y;
+  if (x >= w || y >= h) return;
+  const int j = blockIdx.z >> 1, side = blockIdx.z & 1;
+  const PlfRectPair e = tab[j];
+  const size_t A = (size_t)w * h, i = (size_t)y * w + x;
+  const short2 m = PLF_RECT_MAP1(e.maps, A, side)[i];
+  const int f = PLF_RECT_MAP2(e.maps, A, side)[i] & 1023, fx = f & 31, fy = f >> 5;
+  const uint8_t* src = imgs + (size_t)(2 * e.pair + side) * AP;
+  auto tap = [&](int u, int v) -> int {
+    return (unsigned)u < (unsigned)w && (unsigned)v < (unsigned)h ? __ldg(src + (size_t)v * pitch + u) : 0;
+  };
+  const int sx = m.x, sy = m.y;
+  const int acc = (32 - fx) * (32 - fy) * tap(sx, sy) + fx * (32 - fy) * tap(sx + 1, sy) + (32 - fx) * fy * tap(sx, sy + 1) +
+                  fx * fy * tap(sx + 1, sy + 1);
+  out[(size_t)blockIdx.z * AP + (size_t)y * pitch + x] = (uint8_t)((acc + 512) >> 10);
+}
+
+// Rectifies the pairs of the batch whose sequence has maps in the slot the run consumes, before any stream of the run
+// reads it: on the copy stream, behind the upload, each such pair is remapped into scratch and copied back in place, and
+// ev_up[run_slot] is recorded again, so the E and P phases (which wait for it) read the rectified images.  The copy stream
+// orders one batch's scratch use before the next's.  A batch without such a pair enqueues nothing.
+static plf_status run_rectify(plf_ctx* ctx, PipeState* s, const BatchRun& r, const int32_t* seq) {
+  if (ctx->seq_rect.empty()) return PLF_OK;
+  PlfRectPair* ht = s->h_rect[r.rp];
+  int nr = 0;
+  for (int k = 0; k < r.B; ++k)
+    if (const uint8_t* maps = ctx->seq_rect[seq ? seq[k] : 0]) ht[nr++] = PlfRectPair{maps, k, 0};
+  if (nr == 0) return PLF_OK;
+  const size_t AP = (size_t)s->pitch * s->h;
+  PlfRectPair* tab;
+  uint8_t* pairs;
+  DevBufList b;
+  b.add(tab, s->B);
+  b.add(pairs, 2 * (size_t)s->B * AP);
+  if (b.carve(ctx, PLF_SCR_RECT_PIPE)) return PLF_ERR_CUDA;
+  uint8_t* imgs = s->imgs2[r.run_slot];
+  cudaStream_t cs = s->copy;
+  // a run that read this slot before (a slot run twice) has finished with it
+  PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_free[r.run_slot], 0));
+  PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_free2[r.run_slot], 0));
+  PLF_CUDA(ctx, cudaMemcpyAsync(tab, ht, sizeof(PlfRectPair) * nr, cudaMemcpyHostToDevice, cs));
+  k_rectify<<<dim3((s->w + 31) / 32, (s->h + 7) / 8, 2 * nr), dim3(32, 8), 0, cs>>>(tab, imgs, AP, s->pitch, s->w, s->h, pairs);
+  PLF_LAUNCH_CHECK(ctx);
+  // back in runs of consecutive pairs, w bytes of each row (the slot's row padding stays as the upload left it)
+  for (int j0 = 0, j1; j0 < nr; j0 = j1) {
+    for (j1 = j0 + 1; j1 < nr && ht[j1].pair == ht[j1 - 1].pair + 1;) ++j1;
+    PLF_CUDA(ctx, cudaMemcpy2DAsync(imgs + 2 * (size_t)ht[j0].pair * AP, (size_t)s->pitch, pairs + 2 * (size_t)j0 * AP, (size_t)s->pitch,
+                                    (size_t)s->w, 2 * (size_t)(j1 - j0) * s->h, cudaMemcpyDeviceToDevice, cs));
+  }
+  PLF_CUDA(ctx, cudaEventRecord(s->ev_up[r.run_slot], cs));
   return PLF_OK;
 }
 
@@ -953,6 +1025,15 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
 
 extern "C" {
 
+}  // extern "C"
+
+void plf_rect_drop_sequences(plf_ctx* ctx) {
+  for (uint8_t* d : ctx->seq_rect) cudaFree(d);
+  ctx->seq_rect.clear();
+}
+
+extern "C" {
+
 plf_status plf_reset_sequence(plf_ctx* ctx) {
   if (!ctx) return PLF_ERR_INVALID;
   if (ctx->pipe) {
@@ -971,6 +1052,7 @@ plf_status plf_set_max_sequences(plf_ctx* ctx, int n) {
   ctx->max_sequences = n;
   ctx->seq_cam.clear();
   ctx->seq_cam_own.clear();
+  plf_rect_drop_sequences(ctx);
   plf_bow_drop_sequences(ctx);
   return PLF_OK;
 }
@@ -998,6 +1080,50 @@ plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam) {
   ctx->seq_cam[s] = cam ? *cam : ctx->cam;
   ctx->seq_cam_own[s] = cam ? 1 : 0;
   // the sequence restarts: its next pair in a run is a first frame (the batches already run have their tables)
+  if (ctx->pipe) ctx->pipe->carried[s] = 0;
+  return PLF_OK;
+}
+
+plf_status plf_set_sequence_rectification(plf_ctx* ctx, int s, const int16_t* map1_l, const uint16_t* map2_l,
+                                          const int16_t* map1_r, const uint16_t* map2_r) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (s < 0 || s >= ctx->max_sequences)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_rectification: s = %d outside [0, %d)", s, ctx->max_sequences);
+  const int given = !!map1_l + !!map2_l + !!map1_r + !!map2_r;
+  if (given != 0 && given != 4)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_rectification: %d of the four maps given, need all four or none (NULL clears)",
+                    given);
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  // the copy stream runs every rectification: once it is idle, no batch run so far reads sequence s's old maps
+  cudaStream_t cs = ctx->pipe ? ctx->pipe->copy : ctx->stream;
+  uint8_t* old = ctx->seq_rect.empty() ? nullptr : ctx->seq_rect[s];
+  const size_t A = (size_t)ctx->cam.width * ctx->cam.height;
+  if (given) {
+    uint8_t* d = old;
+    if (!d) {
+      const cudaError_t e = cudaMalloc(&d, 12 * A);
+      if (e != cudaSuccess) {
+        cudaGetLastError();
+        return plf_fail(ctx, PLF_ERR_CUDA, "plf_set_sequence_rectification: cudaMalloc(%zu): %s", 12 * A, cudaGetErrorString(e));
+      }
+    }
+    const void* src[4] = {map1_l, map1_r, map2_l, map2_r};
+    const size_t off[4] = {0, 4 * A, 8 * A, 10 * A}, len[4] = {4 * A, 4 * A, 2 * A, 2 * A};
+    cudaError_t e = cudaSuccess;
+    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = cudaMemcpyAsync(d + off[i], src[i], len[i], cudaMemcpyHostToDevice, cs);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
+    if (e != cudaSuccess) {
+      if (!old) cudaFree(d);
+      return plf_fail(ctx, PLF_ERR_CUDA, "plf_set_sequence_rectification: copying the maps: %s", cudaGetErrorString(e));
+    }
+    if (ctx->seq_rect.empty()) ctx->seq_rect.assign(ctx->max_sequences, nullptr);
+    ctx->seq_rect[s] = d;
+  } else if (old) {
+    PLF_CUDA(ctx, cudaStreamSynchronize(cs));
+    cudaFree(old);
+    ctx->seq_rect[s] = nullptr;
+  }
+  // the sequence restarts: its carried frame was extracted from other images (the batches already run have their tables)
   if (ctx->pipe) ctx->pipe->carried[s] = 0;
   return PLF_OK;
 }
@@ -1170,7 +1296,8 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   r.sG = r.piped ? ctx->aux[1] : r.sM;
   r.sP = (r.piped && r.lsd2) ? ctx->aux[2] : r.sG;   // LSD pre-grow chain: own stream when its outputs exist per parity
   r.afast = ctx->afast_on;
-  st = r.afast ? send_tab(ctx, s, r) : PLF_OK;
+  st = run_rectify(ctx, s, r, seq);
+  if (!st && r.afast) st = send_tab(ctx, s, r);
   if (!st) st = run_extract(ctx, s, r);
   if (!st) st = run_lsd(ctx, s, r);
   if (!st) st = run_match(ctx, s, r);

@@ -291,6 +291,7 @@ void plf_destroy(plf_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   plf_pipe_free(ctx);
+  plf_rect_drop_sequences(ctx);
   plf_bow_free(ctx);
   plf_orb_free(ctx->orb_standalone);
   plf_lsd_free(ctx->lsd_standalone);

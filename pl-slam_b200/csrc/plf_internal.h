@@ -37,6 +37,8 @@ enum plf_scratch_slot {
   PLF_SCR_BOW,         // plf_bow_insert, plf_bow_insert_batch
   PLF_SCR_BA_BATCH,    // plf_local_ba_batch and plf_global_ba_batch: their staged layout
   PLF_SCR_LC,          // plf_loop_closure_pose and plf_loop_closure_pose_batch: their staged layout
+  PLF_SCR_RECT_PIPE,   // the rectification of plf_batch_run_sequences (plf_set_sequence_rectification): its pair table
+                       // and remapped pairs, sized for max_batch pairs once, so that it never grows under batches in flight
   PLF_SCR_COUNT
 };
 
@@ -87,6 +89,9 @@ struct plf_ctx {
   // where seq_cam_own[s], else cam.  plf_set_max_sequences clears both.
   std::vector<plf_camera> seq_cam;
   std::vector<uint8_t> seq_cam_own;
+  // plf_set_sequence_rectification: [max_sequences] once a sequence has maps, else empty; seq_rect[s] is sequence s's
+  // device block of 12 w h bytes (PLF_RECT_* layout, pipeline.cu) or null.  plf_set_max_sequences and plf_destroy free them.
+  std::vector<uint8_t*> seq_rect;
   bool afast_on = false;          // plf_set_adaptive_fast: per-sequence FAST thresholds in the batched pipeline
   plf_adaptive_fast afast = {};
   std::string err;
@@ -121,6 +126,8 @@ void* plf_scratch(plf_ctx* ctx, plf_scratch_slot slot, size_t bytes);
 void* plf_pinned(plf_ctx* ctx, size_t bytes);
 // Frees every sequence's bag-of-words databases (dbow.cu); plf_set_max_sequences drops them.
 void plf_bow_drop_sequences(plf_ctx* ctx);
+// Frees every sequence's rectification maps (pipeline.cu); plf_set_max_sequences and plf_destroy drop them.
+void plf_rect_drop_sequences(plf_ctx* ctx);
 
 #define PLF_CUDA(ctx, call)                                                                  \
   do {                                                                                       \

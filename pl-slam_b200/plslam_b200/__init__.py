@@ -1209,6 +1209,33 @@ class Frontend:
         self._check(self.lib.plf_get_sequence_camera(self._ctx, int(s), C.byref(out)), "plf_get_sequence_camera")
         return {name: getattr(out, name) for name, _ in plf_camera._fields_}
 
+    def set_sequence_rectification(self, s, left=None, right=None):
+        """Rectifies sequence s's raw pairs on the device before extraction, byte for byte cv::remap(img, map1, map2,
+        INTER_LINEAR) with a constant 0 border.  left / right: (map1, map2) of that image, as cv2.initUndistortRectifyMap
+        (..., cv2.CV_16SC2, ...) returns them: map1 int16 [H, W, 2], map2 uint16 [H, W], for the camera's H x W.  Both None
+        clears the rectification.  Either restarts s; batches already run keep their maps.  The camera of the rectified
+        images is set with set_sequence_camera.  plf_set_sequence_rectification."""
+        if left is None and right is None:
+            self._check(self.lib.plf_set_sequence_rectification(self._ctx, int(s), None, None, None, None),
+                        "plf_set_sequence_rectification")
+            return
+        if left is None or right is None:
+            raise PlfError("set_sequence_rectification: give the maps of both images, or neither to clear")
+        H, W = self.camera.height, self.camera.width
+        maps = []
+        for side, pair in (("left", left), ("right", right)):
+            m1, m2 = pair
+            for name, a, dt, shape in (("map1", m1, np.int16, (H, W, 2)), ("map2", m2, np.uint16, (H, W))):
+                a = np.asarray(a)
+                if a.dtype != dt or a.shape != shape:
+                    raise PlfError(f"set_sequence_rectification: {side} {name} must be {np.dtype(dt)}{list(shape)} "
+                                   f"(got {a.dtype}{list(a.shape)})")
+                maps.append(np.ascontiguousarray(a))
+        m1l, m2l, m1r, m2r = maps
+        self._check(self.lib.plf_set_sequence_rectification(self._ctx, int(s), _ptr(m1l, C.c_int16), _ptr(m2l, C.c_uint16),
+                                                            _ptr(m1r, C.c_int16), _ptr(m2r, C.c_uint16)),
+                    "plf_set_sequence_rectification")
+
     def set_adaptive_fast(self, cfg=None):
         """stvo-pl's adaptative_fast for the batched pipeline: a dict of min_th, max_th, inc_th, feat_th and err_th (the
         config keys fast_*_th; missing keys take ADAPTIVE_FAST_DEFAULTS), or None to turn it off.  With it on, a batch
