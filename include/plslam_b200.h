@@ -187,6 +187,25 @@ plf_status plf_match_grid_lines(plf_ctx* ctx, const int* q_line, const uint8_t* 
                                 int grid_rows, plf_grid_window w, float nnr, double line_sim_th, int best_lr,
                                 int32_t* matches_12, int* n_matches);
 
+/* Test hook: the batched windowed matcher (that of matching_strategy 3 and of plf_match_kf2kf / plf_match_map2kf's
+ * fast_matching), unchanged, on n_prob problems laid out at uniform capacities K (queries) and Kt (train features):
+ *   q_geo [n_prob][K][2|4]  points: query cells (x, y); lines: integer end points (x1, y1, x2, y2), in grid cells;
+ *   t_geo [n_prob][Kt][2|4] the train cells / end points (a train line is in each cell of its Bresenham walk);
+ *   t_dir [n_prob][Kt][2]   lines: directions2 (may be NULL for points);
+ *   d1 [n_prob][K][32], d2 [n_prob][Kt][32], n1 [n_prob], n2 [n_prob]: the counts, each clamped to K / Kt;
+ *   q_slot [n_prob] or NULL: problem p reads the query descriptors and count of slot q_slot[p] (d1 and n1), and its own
+ *   query geometry q_geo[p].
+ * The grid is grid_cols x grid_rows cells with window w; clip (lines) walks only the steps of a query line whose window
+ * can reach the grid, for queries far outside it.  Out: matches_12 [n_prob][K] (-1 past the problem's count) and
+ * n_matches [n_prob].  PLF_ERR_INVALID before any work for n_prob outside [0, 65535], K outside [0, 65535], Kt outside
+ * [0, 8192], a grid of no cell or of more than 4096 cells, a q_slot entry outside [0, n_prob), a negative count or a
+ * NULL array. */
+plf_status plf_debug_match_grid_batch(plf_ctx* ctx, int n_prob, int K, int Kt, const int* q_geo, const int* t_geo,
+                                      const double* t_dir, const uint8_t* d1, const uint8_t* d2, const int* n1,
+                                      const int* n2, const int* q_slot, int grid_cols, int grid_rows, plf_grid_window w,
+                                      int is_lines, int clip, float nnr, double line_sim_th, int best_lr,
+                                      int32_t* matches_12, int* n_matches);
+
 /* Landmark descriptor maintenance, batched (SURVEY §8(f) f3).  Replaces the body of MapPoint::updateAverageDescDir and
  * MapLine::updateAverageDescDir (src/mapFeatures.cpp:51-93, 121-163), called on every observation add (:48, :118).
  * desc: the observed descriptors of all landmarks, concatenated, [offsets[n_landmarks]][32] (host); landmark l owns

@@ -379,7 +379,8 @@ plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int m
   if (a.g.cols * a.g.rows > 32 * MGB_MASK_WORDS) return plf_fail(ctx, PLF_ERR_INVALID, "match grid: %dx%d cells exceed the mask", a.g.cols, a.g.rows);
   const int K = a.K, Kt = a.Kt;
   const size_t nD = (size_t)K * Kt, nM = a.is_lines ? (size_t)K * MGB_MASK_WORDS : 0;   // D and qmask elements per problem
-  const size_t per = plf_align256(nD * 2) + plf_align256(nM * 4) + plf_align256((size_t)Kt * 4);
+  // per is 0 when Kt is 0 (and, for lines, K too): no problem then needs scratch, and the division below must not trap
+  const size_t per = std::max<size_t>(1, plf_align256(nD * 2) + plf_align256(nM * 4) + plf_align256((size_t)Kt * 4));
   int chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)nprob, (size_t(1) << 31) / per));   // <= 2 GB of scratch
   DevBufList scr;
   scr.add(a.D, nD * chunk); scr.add(a.qmask, nM * chunk); scr.add(a.m21, (size_t)Kt * chunk);
@@ -399,5 +400,66 @@ plf_status plf_launch_match_grid_batch(plf_ctx* ctx, MgbArgs a, int nprob, int m
     PLF_LAUNCH_CHECK(ctx);
     if (plf_status st = mgb_rows_mutual(ctx, a, p0, np, max_n1, cs)) return st;
   }
+  return PLF_OK;
+}
+
+// Test hook (plslam_b200.h): plf_launch_match_grid_batch on caller arrays at uniform capacities.  The inputs and outputs
+// are staged in PLF_SCR_KF and the matcher's D, query masks and m21 live in the keyframe matcher's slots: the keyframe
+// calls are synchronous, so no batch in flight holds either.  The launch bounds (max_n1, max_n2) are the capacities, as
+// the keyframe matcher and the pipeline pass them.
+extern "C" plf_status plf_debug_match_grid_batch(plf_ctx* ctx, int n_prob, int K, int Kt, const int* q_geo, const int* t_geo,
+                                                 const double* t_dir, const uint8_t* d1, const uint8_t* d2, const int* n1,
+                                                 const int* n2, const int* q_slot, int grid_cols, int grid_rows,
+                                                 plf_grid_window w, int is_lines, int clip, float nnr, double line_sim_th,
+                                                 int best_lr, int32_t* matches_12, int* n_matches) {
+  const char* fn = "plf_debug_match_grid_batch";
+  if (!ctx) return PLF_ERR_INVALID;
+  if (n_prob < 0 || n_prob > 65535 || K < 0 || K > 65535 || Kt < 0 || Kt > 8192)
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: n_prob = %d, K = %d, Kt = %d (at most 65535, 65535, 8192)", fn, n_prob, K, Kt);
+  if (grid_cols <= 0 || grid_rows <= 0 || grid_cols > 32 * MGB_MASK_WORDS || grid_rows > 32 * MGB_MASK_WORDS ||
+      grid_cols * grid_rows > 32 * MGB_MASK_WORDS)
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: grid %dx%d (1 to %d cells)", fn, grid_cols, grid_rows, 32 * MGB_MASK_WORDS);
+  if (!q_geo || !t_geo || (is_lines && !t_dir) || !d1 || !d2 || !n1 || !n2 || !matches_12 || !n_matches)
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: NULL array", fn);
+  for (int p = 0; p < n_prob; ++p) {
+    if (n1[p] < 0 || n2[p] < 0) return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: negative count", fn, p);
+    if (q_slot && (q_slot[p] < 0 || q_slot[p] >= n_prob))
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: q_slot %d outside [0, %d)", fn, p, q_slot[p], n_prob);
+  }
+  if (n_prob == 0) return PLF_OK;
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  const size_t P = (size_t)n_prob, gq = is_lines ? 4 : 2;
+  MgbArgs a = {};
+  a.g = {grid_cols, grid_rows, w.width_lo, w.width_hi, w.height_lo, w.height_hi};
+  a.is_lines = is_lines ? 1 : 0; a.K = K; a.Kt = Kt; a.best_lr = best_lr ? 1 : 0; a.clip = clip ? 1 : 0;
+  a.nnr = nnr; a.line_sim_th = line_sim_th;
+  a.d1_stride = (size_t)K * 32; a.d2_stride = (size_t)Kt * 32;
+  a.n1_stride = a.n2_stride = 1; a.m12_stride = K; a.count_stride = 1;
+  int *dq, *dt, *dn1, *dn2, *dslot, *dm12, *dcnt;
+  double* ddir;
+  uint8_t *dd1, *dd2;
+  DevBufList scr;
+  scr.add(dq, P * K * gq); scr.add(dt, P * Kt * gq); scr.add(ddir, is_lines ? P * Kt * 2 : 0);
+  scr.add(dd1, P * K * 32); scr.add(dd2, P * Kt * 32); scr.add(dn1, P); scr.add(dn2, P); scr.add(dslot, q_slot ? P : 0);
+  scr.add(dm12, P * K); scr.add(dcnt, P);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_KF)) return st;
+  cudaStream_t cs = ctx->stream;
+  PLF_CUDA(ctx, cudaMemcpyAsync(dq, q_geo, P * K * gq * 4, cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(dt, t_geo, P * Kt * gq * 4, cudaMemcpyHostToDevice, cs));
+  if (is_lines) PLF_CUDA(ctx, cudaMemcpyAsync(ddir, t_dir, P * Kt * 16, cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(dd1, d1, P * K * 32, cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(dd2, d2, P * Kt * 32, cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(dn1, n1, P * 4, cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(dn2, n2, P * 4, cudaMemcpyHostToDevice, cs));
+  if (q_slot) PLF_CUDA(ctx, cudaMemcpyAsync(dslot, q_slot, P * 4, cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaMemsetAsync(dm12, 0xFF, P * K * 4, cs));
+  PLF_CUDA(ctx, cudaMemsetAsync(dcnt, 0, P * 4, cs));
+  a.q_geo = dq; a.t_geo = dt; a.t_dir = is_lines ? ddir : nullptr; a.q_slot = q_slot ? dslot : nullptr;
+  a.d1 = dd1; a.d2 = dd2; a.n1 = dn1; a.n2 = dn2; a.m12 = dm12; a.count = dcnt;
+  const plf_scratch_slot slot = is_lines ? PLF_SCR_KF_MGB_LS : PLF_SCR_KF_MGB_PT;
+  if (plf_status st = plf_launch_match_grid_batch(ctx, a, n_prob, K, Kt, slot, cs)) return st;
+  PLF_CUDA(ctx, cudaMemcpyAsync(matches_12, dm12, P * K * 4, cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(n_matches, dcnt, P * 4, cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaStreamSynchronize(cs));
   return PLF_OK;
 }

@@ -31,9 +31,10 @@ enum plf_scratch_slot {
   PLF_SCR_MGB_PIPE,    // the windowed matcher of plf_batch_run (matching_strategy != 0)
   PLF_SCR_BA,          // plf_local_ba, plf_global_ba, plf_pose_graph, plf_pose_graph_batch: their staged layout;
                        // plf_debug_ldlt, plf_debug_ldlt_batch
-  PLF_SCR_KF,          // plf_match_kf2kf, plf_match_map2kf and their _batch forms: their staged layout
-  PLF_SCR_KF_MGB_PT,   // plf_match_kf2kf, plf_match_map2kf and their _batch forms: the windowed matcher of points
-  PLF_SCR_KF_MGB_LS,   //   ... and of lines
+  PLF_SCR_KF,          // plf_match_kf2kf, plf_match_map2kf and their _batch forms: their staged layout;
+                       // plf_debug_match_grid_batch's inputs and outputs
+  PLF_SCR_KF_MGB_PT,   // plf_match_kf2kf, plf_match_map2kf and their _batch forms, plf_debug_match_grid_batch: the
+  PLF_SCR_KF_MGB_LS,   //   windowed matcher of points ... and of lines
   PLF_SCR_BOW,         // plf_bow_insert, plf_bow_insert_batch
   PLF_SCR_BA_BATCH,    // plf_local_ba_batch and plf_global_ba_batch: their staged layout
   PLF_SCR_LC,          // plf_loop_closure_pose and plf_loop_closure_pose_batch: their staged layout

@@ -387,6 +387,9 @@ def load_library() -> C.CDLL:
     lib.plf_match_grid_lines.argtypes = [C.c_void_p, _pi, _pu8, C.c_int, _pi, _pi, C.POINTER(C.c_double), _pu8, C.c_int,
                                          C.c_int, C.c_int, plf_grid_window, C.c_float, C.c_double, C.c_int,
                                          C.POINTER(C.c_int32), _pi]
+    lib.plf_debug_match_grid_batch.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, _pi, _pi, C.POINTER(C.c_double),
+                                               _pu8, _pu8, _pi, _pi, _pi, C.c_int, C.c_int, plf_grid_window, C.c_int,
+                                               C.c_int, C.c_float, C.c_double, C.c_int, C.POINTER(C.c_int32), _pi]
     lib.plf_destroy.restype = None
     lib.plf_destroy.argtypes = [C.c_void_p]
     lib.plf_batch_device_images.restype = C.c_void_p
@@ -553,6 +556,35 @@ class Frontend:
                                            C.c_double(line_sim_th), int(bool(best_lr)), _ptr(m, C.c_int32), C.byref(cnt))
         self._check(st, "plf_match_grid_lines")
         return m, cnt.value
+
+    def debug_match_grid_batch(self, q_geo, t_geo, d1, d2, n1, n2, cols, rows, w, nnr, t_dir=None, line_sim_th=0.0,
+                               best_lr=True, clip=False, q_slot=None):
+        """The batched windowed matcher on P problems at uniform capacities: q_geo int32 [P,K,2] query cells (points)
+        or [P,K,4] end points (lines, then t_dir f64 [P,Kt,2] is required), t_geo [P,Kt,2|4], d1 [P,K,32],
+        d2 [P,Kt,32], counts n1 / n2 [P] (clamped to K / Kt), q_slot [P] or None.  Returns (matches_12 int32 [P,K],
+        n_matches int32 [P]).  plf_debug_match_grid_batch."""
+        q = np.ascontiguousarray(q_geo, np.int32)
+        t = np.ascontiguousarray(t_geo, np.int32)
+        P, K, g = q.shape
+        Kt = t.shape[1]
+        lines = g == 4
+        if t.shape != (P, Kt, g) or g not in (2, 4) or (lines and t_dir is None):
+            raise PlfError(f"debug_match_grid_batch: q_geo {q.shape} and t_geo {t.shape} must be [P,K,2|4] and [P,Kt,2|4]"
+                           " (t_dir with lines)")
+        d1 = _u8(d1).reshape(P, K, DESC_BYTES); d2 = _u8(d2).reshape(P, Kt, DESC_BYTES)
+        td = np.ascontiguousarray(t_dir if lines else np.zeros((P, Kt, 2)), np.float64).reshape(P, Kt, 2)
+        n1 = np.ascontiguousarray(n1, np.int32).reshape(P); n2 = np.ascontiguousarray(n2, np.int32).reshape(P)
+        qs = None if q_slot is None else np.ascontiguousarray(q_slot, np.int32).reshape(P)
+        m = np.full((P, K), -1, np.int32)
+        cnt = np.zeros(P, np.int32)
+        st = self.lib.plf_debug_match_grid_batch(self._ctx, P, K, Kt, _ptr(q, C.c_int), _ptr(t, C.c_int),
+                                                 _ptr(td, C.c_double), _ptr(d1, C.c_uint8), _ptr(d2, C.c_uint8),
+                                                 _ptr(n1, C.c_int), _ptr(n2, C.c_int), None if qs is None else _ptr(qs, C.c_int),
+                                                 int(cols), int(rows), plf_grid_window(*[int(v) for v in w]), int(lines),
+                                                 int(bool(clip)), C.c_float(nnr), C.c_double(line_sim_th),
+                                                 int(bool(best_lr)), _ptr(m, C.c_int32), _ptr(cnt, C.c_int))
+        self._check(st, "plf_debug_match_grid_batch")
+        return m, cnt
 
     def median_descriptors(self, desc, offsets, dirs=None):
         """MapPoint/MapLine::updateAverageDescDir over many landmarks: (med_idx int32[L], med_dir f64[L,3] or None)."""
