@@ -820,6 +820,29 @@ plf_status plf_set_adaptive_fast(plf_ctx* ctx, const plf_adaptive_fast* cfg);
 /* *th = the FAST threshold the next pair of sequence s will be detected with (orb_fast_th with the adaptation off or when
  * that pair is a first frame).  May be called at any time; with batches in flight it waits for their match phases. */
 plf_status plf_get_sequence_fast_th(plf_ctx* ctx, int s, int* th);
+
+/* stvo-pl's use_motion_model (config_euroc.yaml:18): each sequence's next pair starts from a constant-motion prediction.
+ * Turns it on (on != 0) or off (0, the default) for the batched pipeline.  With it on, after pair k of sequence s the
+ * prediction of s's next pair is T = inverse_se3(DT_k) (the optimiser's transform, previous frame into current) when pair
+ * k is a good solution (stvo-pl's isGoodSolution, DESIGN.md section 8):
+ *   status 0, every entry of DT finite, and none of err < 0, err > 1, min eig(DT_cov) < 0, max eig(DT_cov) > 1
+ * (so a NaN err or eigenvalue passes; a DT_cov with a non-finite entry has NaN eigenvalues), else the identity.  The next
+ * pair projects the previous frame's points and line end points through T before the windowed frame-to-frame matching
+ * (matching_strategy != 0) and seeds the pose solver with it (T_init).  Every first frame (its first pair, restart[k],
+ * plf_reset_sequence, plf_set_sequence_camera, plf_set_sequence_rectification) starts from the identity, and a successful
+ * call with on != 0 sets every sequence's prediction back to it.  As with plf_set_adaptive_fast a batch may hold at most
+ * one pair of each sequence (plf_batch_run_sequences refuses it otherwise, PLF_ERR_INVALID, before anything is enqueued).
+ * Valid only with no batch in flight (PLF_ERR_STATE). */
+plf_status plf_set_motion_model(plf_ctx* ctx, int on);
+/* T (row-major 4x4) = the prediction the next pair of sequence s will start from, *valid = 1 when it came from a good
+ * solution (identity and 0 with the model off or when that pair is a first frame).  May be called at any time; with
+ * batches in flight it waits for their match phases. */
+plf_status plf_get_sequence_motion(plf_ctx* ctx, int s, double T[16], int* valid);
+/* The device rule of plf_set_motion_model on n caller results, for tests that put a decision exactly on an edge: DT [n][16],
+ * DT_cov [n][36], err [n], status [n] in; T_out [n][16] (the prediction) and valid_out [n] out.  One launch on the
+ * context's stream.  PLF_ERR_INVALID for n < 0 or an array NULL (n > 0). */
+plf_status plf_debug_motion_prior(plf_ctx* ctx, int n, const double* DT, const double* DT_cov, const double* err,
+                                  const int32_t* status, double* T_out, int32_t* valid_out);
 /* Poses of the OLDEST batch in flight, device to device: dst_device[B][16] f64 (DT, row-major) is filled on `stream`
  * (a cudaStream_t of the caller; NULL = an internal stream, synchronised before returning) behind that batch's match
  * phase - the buffer a multi-GPU caller passes to its NCCL pose all-gather on the same stream (SURVEY 8e; the reference

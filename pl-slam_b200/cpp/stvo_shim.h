@@ -275,15 +275,17 @@ class StereoFrameHandler {
  public:
   // adaptive_fast: stvo-pl's adaptative_fast with its fast_*_th values, or NULL for a fixed orb_fast_th.  One frame per
   // call (B = 1) is what makes the adaptation exact: frame k is detected at the threshold frame k-1's pose gave.
+  // use_motion_model: stvo-pl's use_motion_model; frame k starts from the prediction frame k-1's pose gave (B = 1 again).
   explicit StereoFrameHandler(PinholeStereoCamera* cam_, const plf_params* params = nullptr, int device = 0,
-                              const plf_adaptive_fast* adaptive_fast = nullptr) : cam(cam_) {
+                              const plf_adaptive_fast* adaptive_fast = nullptr, bool use_motion_model = false) : cam(cam_) {
     plf_limits lim;
     plf_default_limits(&lim);
     lim.max_batch = 1;  // the class API is one frame per call; batched callers use plf_process_batch directly
     if (params) prm_ = *params; else plf_default_params(&prm_);
     if (plf_create(&prm_, &cam->raw(), &lim, device, &ctx_) != PLF_OK)
       throw std::runtime_error(std::string("[StereoFrameHandler] ") + plf_last_error(nullptr));
-    if (adaptive_fast && plf_set_adaptive_fast(ctx_, adaptive_fast) != PLF_OK) {
+    if ((adaptive_fast && plf_set_adaptive_fast(ctx_, adaptive_fast) != PLF_OK) ||
+        (use_motion_model && plf_set_motion_model(ctx_, 1) != PLF_OK)) {
       const std::string e = plf_last_error(ctx_);
       plf_destroy(ctx_);
       throw std::runtime_error("[StereoFrameHandler] " + e);
@@ -385,6 +387,14 @@ class StereoFrameHandler {
     int th = 0;
     check(plf_get_sequence_fast_th(ctx_, 0, &th));
     return th;
+  }
+
+  // The motion prediction (row-major 4x4) the next frame starts from: inverse(prev_frame->DT) after a good solution, else
+  // the identity (DESIGN.md section 8); returns whether it came from a good solution.
+  bool motionPrior(double T[16]) {
+    int valid = 0;
+    check(plf_get_sequence_motion(ctx_, 0, T, &valid));
+    return valid != 0;
   }
 
   // app/plslam_dataset.cpp:159

@@ -763,6 +763,10 @@ int main(int argc, char** argv) {
     bow_voc[1] = argv[argc - 1];
     argc -= 3;
   }
+  // --motion-model (last): stvo-pl's use_motion_model; prints "motion k valid T[16]", the prediction frame k started from,
+  // after each frame's line
+  bool motion_on = false;
+  if (argc >= 2 && std::string(argv[argc - 1]) == "--motion-model") { motion_on = true; --argc; }
   // --adaptive-fast min max inc feat err: stvo-pl's adaptative_fast (fast_min_th .. fast_err_th); prints "fast_th k th",
   // the threshold frame k was detected with, after each frame's line
   plf_adaptive_fast afast;
@@ -791,7 +795,7 @@ int main(int argc, char** argv) {
     plf_params prm;
     plf_default_params(&prm);
     if (argc >= 4) { prm.orb_nfeatures = std::atoi(argv[2]); prm.lsd_nfeatures = std::atoi(argv[3]); }
-    StVO::StereoFrameHandler* StVO_ = new StVO::StereoFrameHandler(&cam_pin, &prm, 0, afast_on ? &afast : nullptr);   // app:109
+    StVO::StereoFrameHandler* StVO_ = new StVO::StereoFrameHandler(&cam_pin, &prm, 0, afast_on ? &afast : nullptr, motion_on);   // app:109
     KfArrays* first_kf = nullptr;   // --kf-match-selftest: frame 0 against the last frame
     BowMap bow = {StVO_->ctx(), prm.has_points != 0, prm.has_lines != 0, {}, {}};
     LcMap lc = {bow, {}, 1, 2, 1, 20, 0};
@@ -806,6 +810,8 @@ int main(int argc, char** argv) {
       bool new_kf = false;
       StVO::StereoFrame* cur;
       const int fast_th = StVO_->orbFastTh();
+      double T_pred[16];
+      const bool pred_valid = StVO_->motionPrior(T_pred);
       if (frame_counter == 0) {
         StVO_->initialize(img_l, img_r, 0);                                             // app:115
         cur = StVO_->prev_frame;
@@ -825,6 +831,11 @@ int main(int argc, char** argv) {
       for (int i = 0; i < 16; ++i) std::printf(" %.17g", cur->Tfw.v[i]);
       std::printf("\n");
       if (afast_on) std::printf("fast_th %d %d\n", frame_counter, fast_th);
+      if (motion_on) {
+        std::printf("motion %d %d", frame_counter, pred_valid ? 1 : 0);
+        for (int i = 0; i < 16; ++i) std::printf(" %.17g", T_pred[i]);
+        std::printf("\n");
+      }
       if (bow_voc[0] && !lc_test) bow_selftest_frame(bow, cur, frame_counter);
       if (lc_test) lc_selftest_frame(lc, cur, frame_counter);
       if (kf_test && frame_counter == 0) first_kf = new KfArrays(cur);

@@ -9,7 +9,8 @@
 //
 // One call processes B stereo pairs of up to max_sequences sequences.  Everything except the final SE(3) chaining is
 // independent per pair (extraction, stereo association) or per pair and its previous frame of the same sequence
-// (tracking and the pose increment start from identity: use_motion_model = false, config_euroc.yaml:18), so all B
+// (tracking and the pose increment start from identity, or with plf_set_motion_model from the sequence's prediction,
+// which the previous batch's match phase left on the device), so all B
 // pairs run in the same launches: images [2B][H][W] (2k = left, 2k+1 = right) -> ORB / LSD / LBD over 2B images ->
 // per-pair kernels.  Pair k's previous frame is the slot prev[k] of the batch's sequence table; the last frame of each
 // sequence in the batch is carried to that sequence's carry slot for the next call.
@@ -86,6 +87,14 @@ struct PipeState {
   int* seq_th = nullptr;       // [nseq]
   int* img_th = nullptr;       // [2B]
   cudaEvent_t ev_th = nullptr;
+  // plf_set_motion_model: seq_T[s] (row-major 4x4) = the pose prediction of sequence s's next pair unless that pair is a
+  // first frame, seq_valid[s] = 1 where it came from a good solution (both written by k_motion_update on the M stream);
+  // pair_T = the prediction of each pair of the running batch, read by the f2f geometry and, through gn_probs_mm (the
+  // pose problems with T_init = pair_T + 16 k), by the pose solver
+  double* seq_T = nullptr;     // [nseq][16]
+  int* seq_valid = nullptr;    // [nseq]
+  double* pair_T = nullptr;    // [B][16]
+  GnProblem* gn_probs_mm = nullptr;   // [B]
   // matching scratch
   uint32_t* knn_keys = nullptr;   // [B][8][2][max_kp]
   int32_t* m12 = nullptr;         // [B][4][max_kp]  stereo pts, stereo lines, f2f pts, f2f lines
@@ -147,6 +156,10 @@ static void pipe_buffers(PipeState* s, bool windowed, DevBufList& b) {
 #undef PLF_FS_ALLOC
   b.add(s->seq_th, s->nseq);
   b.add(s->img_th, 2 * B);
+  b.add(s->seq_T, (size_t)s->nseq * 16);
+  b.add(s->seq_valid, s->nseq);
+  b.add(s->pair_T, B * 16);
+  b.add(s->gn_probs_mm, B);
   b.add(s->knn_keys, B * 8 * 2 * K);
   b.add(s->m12, B * 4 * K);
   b.add(s->mcount, B * 4);
@@ -566,6 +579,75 @@ static plf_status pipe_fast_th_reset(plf_ctx* ctx) {
   return PLF_OK;
 }
 
+// ---- use_motion_model (plf_set_motion_model, DESIGN.md §8).  As with adaptive FAST thresholds a batch holds at most one
+// pair of each sequence, so prev[k] is the empty slot or pair k's carry slot carry0 + s. ----
+
+// stvo-pl's isGoodSolution on a pair's result, each of its tests a rejection: so a NaN err or eigenvalue passes.  A
+// covariance with a non-finite entry has NaN eigenvalues (the library's definition; the solver gives such a covariance
+// whole, e.g. on rows at infinity).
+__device__ __forceinline__ bool motion_good(int status, const double* DT, const double* cov, double err) {
+  if (status != 0) return false;
+  for (int i = 0; i < 16; ++i)
+    if (!isfinite(DT[i])) return false;
+  if (err < 0.0 || err > 1.0) return false;
+  for (int i = 0; i < 36; ++i)
+    if (!isfinite(cov[i])) return true;
+  double A[36];
+  plf_sym6_jacobi(cov, A);
+  double lo = A[0], hi = A[0];
+  for (int i = 1; i < 6; ++i) {
+    lo = A[7 * i] < lo ? A[7 * i] : lo;
+    hi = A[7 * i] > hi ? A[7 * i] : hi;
+  }
+  return !(lo < 0.0 || hi > 1.0);
+}
+
+// The prediction a pair's result gives its sequence's next pair: the optimiser's transform inverse_se3(DT) (previous frame
+// into current) after a good solution, else the identity.  Returns the valid flag.
+__device__ __forceinline__ int motion_prior(int status, const double* DT, const double* cov, double err, double* T) {
+  const bool good = motion_good(status, DT, cov, err);
+  if (good) d_inverse_se3(DT, T);
+  else
+    for (int i = 0; i < 16; ++i) T[i] = (i % 5 == 0) ? 1.0 : 0.0;
+  return good ? 1 : 0;
+}
+
+// Carry entry j = (pair k, carry slot carry0 + s): sequence s's next prediction from pair k's result.
+__global__ void k_motion_update(const plf_frame_result* __restrict__ res, const int* __restrict__ carry, int ncarry, int carry0,
+                                double* __restrict__ seq_T, int* __restrict__ seq_valid) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= ncarry) return;
+  const plf_frame_result& r = res[carry[2 * j]];
+  const int s = carry[2 * j + 1] - carry0;
+  seq_valid[s] = motion_prior(r.status, r.DT, r.DT_cov, r.err, seq_T + 16 * (size_t)s);
+}
+
+// Block k, thread i: entry i of pair k's prediction, its sequence's or the identity for a first frame.
+__global__ void k_motion_pairs(const int* __restrict__ prev, int carry0, int empty, const double* __restrict__ seq_T,
+                               double* __restrict__ pair_T) {
+  const int k = blockIdx.x, i = threadIdx.x, p = prev[k];
+  pair_T[16 * k + i] = p == empty ? ((i % 5 == 0) ? 1.0 : 0.0) : seq_T[16 * (size_t)(p - carry0) + i];
+}
+
+// plf_debug_motion_prior: the rule on n caller results.
+__global__ void k_motion_debug(int n, const double* __restrict__ DT, const double* __restrict__ cov, const double* __restrict__ err,
+                               const int32_t* __restrict__ status, double* __restrict__ T, int32_t* __restrict__ valid) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  valid[j] = motion_prior(status[j], DT + 16 * (size_t)j, cov + 36 * (size_t)j, err[j], T + 16 * (size_t)j);
+}
+
+// Every sequence's prediction back to the identity (no batch in flight).
+static plf_status pipe_motion_reset(plf_ctx* ctx) {
+  PipeState* s = ctx->pipe;
+  std::vector<double> T((size_t)s->nseq * 16, 0.0);
+  for (size_t i = 0; i < T.size(); i += 16) T[i] = T[i + 5] = T[i + 10] = T[i + 15] = 1.0;
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->seq_T, T.data(), T.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  PLF_CUDA(ctx, cudaMemsetAsync(s->seq_valid, 0, s->nseq * sizeof(int), ctx->stream));
+  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return PLF_OK;
+}
+
 // ---- windowed matching: grid geometry on the device (oracle/frontend.py grid_match_points / grid_match_lines) ----
 // (cells and projection: plf_geom.cuh)
 
@@ -594,18 +676,27 @@ __global__ void __launch_bounds__(256) k_mg_geom_stereo(const plf_keypoint* __re
   }
 }
 
-// frame-to-frame: queries = the previous frame's 3-D features projected with DT = identity (slot prev[k]), train = the
-// current frame's image features (slot k).  The projection uses pair k's camera: both frames belong to one sequence, and
-// a new camera restarts its sequence, so the previous frame was triangulated with the same one.
+// frame-to-frame: queries = the previous frame's 3-D features (slot prev[k]) projected with DT = identity, or through pair
+// k's motion prediction T_pred[k] with the motion model on (src/mapHandler.cpp:254-256, :384-389 project through DT);
+// train = the current frame's image features (slot k).  The projection uses pair k's camera: both frames belong to one
+// sequence, and a new camera restarts its sequence, so the previous frame was triangulated with the same one.
 __global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, const int* __restrict__ prev, int K, int Ln, StereoPrm c0,
-                                                     const PlfPairCam* __restrict__ cams, double iw, double ih,
-                                                     int* __restrict__ qp, int* __restrict__ tp, int* __restrict__ ql,
-                                                     int* __restrict__ tl, double* __restrict__ tdir) {
+                                                     const PlfPairCam* __restrict__ cams, const double* __restrict__ T_pred,
+                                                     double iw, double ih, int* __restrict__ qp, int* __restrict__ tp,
+                                                     int* __restrict__ ql, int* __restrict__ tl, double* __restrict__ tdir) {
   const int k = blockIdx.y, i = blockIdx.x * 256 + threadIdx.x;
   const int ps = prev[k], cs = k;
   const StereoPrm c = pair_prm(c0, cams, k);
+  const double* T = T_pred ? T_pred + 16 * k : nullptr;
+  // the query point X of the previous frame, moved into the current frame when there is a prediction
+  auto moved = [&](const double* X, double* Y) -> const double* {
+    if (!T) return X;
+    d_transform(T, X, Y);
+    return Y;
+  };
   if (i < min(fs.pt_count[ps], K)) {
-    const double* P = fs.pt_P + 3 * ((size_t)ps * K + i);
+    double Q[3];
+    const double* P = moved(fs.pt_P + 3 * ((size_t)ps * K + i), Q);
     const double2 u = plf_project(c.fx, c.fy, c.cx, c.cy, P[0], P[1], P[2]);
     qp[((size_t)k * K + i) * 2] = plf_qcell(u.x * iw);
     qp[((size_t)k * K + i) * 2 + 1] = plf_qcell(u.y * ih);
@@ -616,8 +707,9 @@ __global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, const int* _
     tp[((size_t)k * K + i) * 2 + 1] = mg_cell(p.y * ih);
   }
   if (i < min(fs.ls_count[ps], Ln)) {
-    const double* S = fs.ls_sP + 3 * ((size_t)ps * Ln + i);
-    const double* E = fs.ls_eP + 3 * ((size_t)ps * Ln + i);
+    double QS[3], QE[3];
+    const double* S = moved(fs.ls_sP + 3 * ((size_t)ps * Ln + i), QS);
+    const double* E = moved(fs.ls_eP + 3 * ((size_t)ps * Ln + i), QE);
     int* d = ql + ((size_t)k * Ln + i) * 4;
     d[0] = plf_qcell(plf_project_u(c.fx, c.cx, S[0], S[2]) * iw); d[1] = plf_qcell(plf_project_v(c.fy, c.cy, S[1], S[2]) * ih);
     d[2] = plf_qcell(plf_project_u(c.fx, c.cx, E[0], E[2]) * iw); d[3] = plf_qcell(plf_project_v(c.fy, c.cy, E[1], E[2]) * ih);
@@ -721,8 +813,11 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
   PLF_CUDA(ctx, cudaMemcpyAsync(s->knn_stereo, ks.data(), ks.size() * sizeof(KnnProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->nnr_stereo, ns.data(), ns.size() * sizeof(NnrProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->gn_probs, gp.data(), gp.size() * sizeof(GnProblem), cudaMemcpyHostToDevice, cs));
+  for (int k = 0; k < B; ++k) gp[k].T_init = s->pair_T + 16 * (size_t)k;   // the same problems seeded with the prediction
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->gn_probs_mm, gp.data(), gp.size() * sizeof(GnProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaStreamSynchronize(cs));
-  return ctx->afast_on ? pipe_fast_th_reset(ctx) : PLF_OK;
+  if (ctx->afast_on && (st = pipe_fast_th_reset(ctx))) return st;
+  return ctx->motion_on ? pipe_motion_reset(ctx) : PLF_OK;
 }
 
 // Builds the pipeline for the camera's image size on first use; a failed setup leaves no state behind.
@@ -739,6 +834,7 @@ struct BatchRun {
   int ncarry;    // entries of the carry list in h_tab[rp]: the sequences the batch holds
   bool cams;     // h_cam[rp] holds the pairs' cameras (a sequence of the batch has its own); else the context's camera
   bool afast;    // adaptive FAST thresholds (plf_set_adaptive_fast): the sequence table goes up before the E phase, which reads it
+  bool motion;   // motion model (plf_set_motion_model): pair predictions at the start of M, the next ones behind k_finalize
   int par;       // parity of the E -> G -> M hand-off buffers
   int lp;        // parity of the LSD hand-off buffers (0 when they exist once)
   int rp;        // slot of the result ring
@@ -924,6 +1020,14 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   k_f2f_problems<<<(B + 127) / 128, 128, 0, cs>>>(s->fs, prev, B, K, Ln, s->knn_keys, s->m12, s->mcount, P.min_ratio_12_p,
                                                   P.min_ratio_12_l, P.best_lr_matches ? 1 : 0, s->knn_f2f, s->nnr_f2f);
   PLF_LAUNCH_CHECK(ctx);
+  // the pairs' motion predictions, when the model is on (null: the f2f geometry and the pose solver start from identity).
+  // The previous batch wrote its sequences' ones behind its k_finalize on this stream.
+  const double* T_pred = nullptr;
+  if (r.motion) {
+    k_motion_pairs<<<B, 16, 0, cs>>>(prev, s->B, s->B + s->nseq, s->seq_T, s->pair_T);
+    PLF_LAUNCH_CHECK(ctx);
+    T_pred = s->pair_T;
+  }
   if ((st = plf_launch_lbd(ctx, cs, s->lbd_grad[par], A, w, h, 2 * B, kls, lcnt, Ln, s->ldesc_raw, nullptr))) return st;
   plf_mark(ctx, cs, "lbd.k_lbd");
   // the rest of the match phase works on its own copy of the extraction outputs; evX releases this parity to batch i+2
@@ -982,7 +1086,7 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     // frame-to-frame: matchGrid() in a +-matching_f2f_ws window around the projected feature; the match() result above
     // stands where the window search found fewer than min_pt_matches / min_ls_matches
     PLF_CUDA(ctx, cudaMemsetAsync(s->mgcount, 0, (size_t)B * 2 * sizeof(int), cs));
-    k_mg_geom_f2f<<<dim3((std::max(K, Ln) + 255) / 256, B), 256, 0, cs>>>(s->fs, prev, K, Ln, sp, pcam, mg_iw, mg_ih,
+    k_mg_geom_f2f<<<dim3((std::max(K, Ln) + 255) / 256, B), 256, 0, cs>>>(s->fs, prev, K, Ln, sp, pcam, T_pred, mg_iw, mg_ih,
                                                                           s->mg_q[2], s->mg_t[2], s->mg_q[3], s->mg_t[3],
                                                                           s->mg_dir[1]);
     PLF_LAUNCH_CHECK(ctx);
@@ -1002,7 +1106,7 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
                                   s->gn_sP, s->gn_eP, s->gn_le, s->gnInlL, s->gnNl);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "f2f.k_nnr_mutual+k_f2f_build");
-  if ((st = plf_launch_gn(ctx, cs, s->gn_probs, B, plf_gn_opts_from_params(P), pcam))) return st;
+  if ((st = plf_launch_gn(ctx, cs, T_pred ? s->gn_probs_mm : s->gn_probs, B, plf_gn_opts_from_params(P), pcam))) return st;
   plf_mark(ctx, cs, "gn.k_gn_pose");
   k_finalize<<<(B + 127) / 128, 128, 0, cs>>>(s->gn_out, s->gnNp, s->gnNl, kcnt, lcnt, s->fs, prev, s->B + s->nseq,
                                                P.min_features, B, s->results + (size_t)rp * s->B);
@@ -1014,6 +1118,11 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
                                                              ctx->afast, s->seq_th);
     PLF_LAUNCH_CHECK(ctx);
     PLF_CUDA(ctx, cudaEventRecord(s->ev_th, cs));
+  }
+  if (r.motion) {   // the next batch's M phase, on this stream, reads its sequences' predictions
+    k_motion_update<<<(r.ncarry + 127) / 128, 128, 0, cs>>>(s->results + (size_t)rp * s->B, carry, r.ncarry, s->B, s->seq_T,
+                                                            s->seq_valid);
+    PLF_LAUNCH_CHECK(ctx);
   }
   plf_mark(ctx, cs, "k_finalize+carry");
   // results + overflow flags to pinned memory as part of this batch's stream work; evM marks them ready
@@ -1177,6 +1286,62 @@ plf_status plf_get_sequence_fast_th(plf_ctx* ctx, int s, int* th) {
   return PLF_OK;
 }
 
+plf_status plf_set_motion_model(plf_ctx* ctx, int on) {
+  if (!ctx) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_set_motion_model: ctx is NULL");
+  if (ctx->pipe && ctx->pipe->n_pending)
+    return plf_fail(ctx, PLF_ERR_STATE, "plf_set_motion_model: %d batch(es) still in flight; download them first", ctx->pipe->n_pending);
+  if (on && ctx->pipe) {
+    PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+    const plf_status st = pipe_motion_reset(ctx);
+    if (st) return st;
+  }
+  ctx->motion_on = on != 0;
+  return PLF_OK;
+}
+
+plf_status plf_get_sequence_motion(plf_ctx* ctx, int s, double T[16], int* valid) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (!T || !valid) return plf_fail(ctx, PLF_ERR_INVALID, "plf_get_sequence_motion: T and valid are required");
+  if (s < 0 || s >= ctx->max_sequences)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_get_sequence_motion: s = %d outside [0, %d)", s, ctx->max_sequences);
+  for (int i = 0; i < 16; ++i) T[i] = (i % 5 == 0) ? 1.0 : 0.0;
+  *valid = 0;
+  if (!ctx->motion_on || !ctx->pipe || !ctx->pipe->carried[s]) return PLF_OK;   // the next pair starts from identity
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  // behind the prediction updates of every batch in flight (M stream)
+  PLF_CUDA(ctx, cudaMemcpyAsync(T, ctx->pipe->seq_T + 16 * (size_t)s, 16 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  PLF_CUDA(ctx, cudaMemcpyAsync(valid, ctx->pipe->seq_valid + s, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return PLF_OK;
+}
+
+plf_status plf_debug_motion_prior(plf_ctx* ctx, int n, const double* DT, const double* DT_cov, const double* err,
+                                  const int32_t* status, double* T_out, int32_t* valid_out) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (n < 0) return plf_fail(ctx, PLF_ERR_INVALID, "plf_debug_motion_prior: n = %d < 0", n);
+  if (n == 0) return PLF_OK;
+  if (!DT || !DT_cov || !err || !status || !T_out || !valid_out)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_debug_motion_prior: every array is required");
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  const size_t N = n;
+  double *dDT, *dcov, *derr, *dT;
+  int32_t *dst, *dvalid;
+  DevBufList b;
+  b.add(dDT, 16 * N); b.add(dcov, 36 * N); b.add(derr, N); b.add(dst, N); b.add(dT, 16 * N); b.add(dvalid, N);
+  if (b.carve(ctx, PLF_SCR_GN)) return PLF_ERR_CUDA;
+  cudaStream_t cs = ctx->stream;
+  PLF_CUDA(ctx, cudaMemcpyAsync(dDT, DT, 16 * N * sizeof(double), cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(dcov, DT_cov, 36 * N * sizeof(double), cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(derr, err, N * sizeof(double), cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(dst, status, N * sizeof(int32_t), cudaMemcpyHostToDevice, cs));
+  k_motion_debug<<<(n + 127) / 128, 128, 0, cs>>>(n, dDT, dcov, derr, dst, dT, dvalid);
+  PLF_LAUNCH_CHECK(ctx);
+  PLF_CUDA(ctx, cudaMemcpyAsync(T_out, dT, 16 * N * sizeof(double), cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(valid_out, dvalid, N * sizeof(int32_t), cudaMemcpyDeviceToHost, cs));
+  PLF_CUDA(ctx, cudaStreamSynchronize(cs));
+  return PLF_OK;
+}
+
 plf_status plf_batch_upload(plf_ctx* ctx, int B, const uint8_t* left, const uint8_t* right, int stride) {
   if (!ctx || !left || !right || B < 1 || B > ctx->limits.max_batch || stride < ctx->cam.width)
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload: bad arguments (B=%d, max_batch=%d)", B, ctx ? ctx->limits.max_batch : 0);
@@ -1240,7 +1405,9 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   PipeState* s = ctx->pipe;
   if (s->n_pending >= 3)
     return plf_fail(ctx, PLF_ERR_STATE, "plf_batch_run: three batches already in flight; call plf_batch_download first");
-  if (ctx->afast_on) {   // pair k of a sequence is detected at the threshold pair k-1's pose gives: one pair per sequence
+  // pair k of a sequence is detected at the threshold pair k-1's pose gives, or starts from the prediction pair k-1's pose
+  // gives: one pair per sequence
+  if (ctx->afast_on || ctx->motion_on) {
     int first = -1, dup = -1;
     for (int k = 0; k < B && dup < 0; ++k) {
       int& last = s->last_pair[seq ? seq[k] : 0];
@@ -1249,9 +1416,9 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
     }
     for (int k = 0; k < B; ++k) s->last_pair[seq ? seq[k] : 0] = -1;
     if (dup >= 0)
-      return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_run_sequences: pairs %d and %d are both of sequence %d; with adaptive FAST "
-                      "thresholds (plf_set_adaptive_fast) a batch holds at most one pair of each sequence",
-                      first, dup, seq ? seq[dup] : 0);
+      return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_run_sequences: pairs %d and %d are both of sequence %d; with %s a batch "
+                      "holds at most one pair of each sequence", first, dup, seq ? seq[dup] : 0,
+                      ctx->afast_on ? "adaptive FAST thresholds (plf_set_adaptive_fast)" : "the motion model (plf_set_motion_model)");
   }
   BatchRun r;
   r.B = B;
@@ -1296,6 +1463,7 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   r.sG = r.piped ? ctx->aux[1] : r.sM;
   r.sP = (r.piped && r.lsd2) ? ctx->aux[2] : r.sG;   // LSD pre-grow chain: own stream when its outputs exist per parity
   r.afast = ctx->afast_on;
+  r.motion = ctx->motion_on;
   st = run_rectify(ctx, s, r, seq);
   if (!st && r.afast) st = send_tab(ctx, s, r);
   if (!st) st = run_extract(ctx, s, r);

@@ -25,7 +25,7 @@ inline size_t plf_align256(size_t x) { return (x + 255) & ~size_t(255); }
 enum plf_scratch_slot {
   PLF_SCR_MATCH,       // plf_hamming_knn2, plf_match, plf_median_descriptors, plf_match_grid_points / _lines
   PLF_SCR_LBD,         // plf_lbd_gradients, plf_lbd
-  PLF_SCR_GN,          // plf_gn_pose, plf_gn_pose_batch, plf_se3
+  PLF_SCR_GN,          // plf_gn_pose, plf_gn_pose_batch, plf_se3, plf_debug_motion_prior
   PLF_SCR_ORB,         // plf_orb
   PLF_SCR_LSD,         // plf_lsd, plf_detect_lines, plf_debug_sincosf
   PLF_SCR_MGB_PIPE,    // the windowed matcher of plf_batch_run (matching_strategy != 0)
@@ -95,6 +95,7 @@ struct plf_ctx {
   std::vector<uint8_t*> seq_rect;
   bool afast_on = false;          // plf_set_adaptive_fast: per-sequence FAST thresholds in the batched pipeline
   plf_adaptive_fast afast = {};
+  bool motion_on = false;         // plf_set_motion_model: per-sequence pose predictions in the batched pipeline
   std::string err;
   long long launches = 0;
   // scratch slots (device) of the host-pointer operator entry points

@@ -96,11 +96,10 @@ __host__ __device__ inline void d_inverse_se3(const double* T, double* Ti) {
   for (int i = 0; i < 16; ++i) Ti[i] = out[i];
 }
 
-// Largest eigenvalue of a symmetric 6x6 matrix (cyclic Jacobi; Eigen's SelfAdjointEigenSolver sorts ascending and
-// MapHandler::isLoopClosure reads element 5, src/mapHandler.cpp:3883-3885).  Host and device give the same bits: the
-// device is built --fmad=false, the host has no FMA contraction, and sqrt and the division are correctly rounded on both.
-__host__ __device__ inline double plf_sym6_max_eig(const double* A_in) {
-  double A[36];
+// Cyclic Jacobi on the symmetric part of a 6x6 matrix: A (36 entries) ends diagonal, its diagonal the eigenvalues
+// (unsorted).  Host and device give the same bits: the device is built --fmad=false, the host has no FMA contraction, and
+// sqrt and the division are correctly rounded on both.
+__host__ __device__ inline void plf_sym6_jacobi(const double* A_in, double* A) {
   for (int i = 0; i < 6; ++i)
     for (int j = 0; j < 6; ++j) A[6 * i + j] = 0.5 * (A_in[6 * i + j] + A_in[6 * j + i]);
   for (int sweep = 0; sweep < 64; ++sweep) {
@@ -127,6 +126,13 @@ __host__ __device__ inline double plf_sym6_max_eig(const double* A_in) {
         }
       }
   }
+}
+
+// Largest eigenvalue of a symmetric 6x6 matrix (Eigen's SelfAdjointEigenSolver sorts ascending and
+// MapHandler::isLoopClosure reads element 5, src/mapHandler.cpp:3883-3885).
+__host__ __device__ inline double plf_sym6_max_eig(const double* A_in) {
+  double A[36];
+  plf_sym6_jacobi(A_in, A);
   double m = A[0];
   for (int i = 1; i < 6; ++i) m = A[7 * i] > m ? A[7 * i] : m;
   return m;

@@ -442,9 +442,10 @@ class Frontend:
 
     def __init__(self, params: plf_params | None = None, camera: dict | plf_camera | None = None,
                  limits: plf_limits | None = None, device: int = 0, max_sequences: int = 1,
-                 adaptive_fast: dict | None = None, **overrides):
+                 adaptive_fast: dict | None = None, motion_model: bool = False, **overrides):
         """max_sequences: the number of sequences batch_run / process_batch can track at once (plf_set_max_sequences).
-        adaptive_fast: None, or the per-sequence FAST threshold adaptation as set_adaptive_fast takes it."""
+        adaptive_fast: None, or the per-sequence FAST threshold adaptation as set_adaptive_fast takes it.
+        motion_model: stvo-pl's use_motion_model (set_motion_model)."""
         self.lib = load_library()
         self.params = params if params is not None else default_params()
         for k, v in overrides.items():
@@ -465,6 +466,8 @@ class Frontend:
             self._check(self.lib.plf_set_max_sequences(self._ctx, int(max_sequences)), "plf_set_max_sequences")
             if adaptive_fast is not None:
                 self.set_adaptive_fast(adaptive_fast)
+            if motion_model:
+                self.set_motion_model(True)
         except PlfError:
             self.close()
             raise
@@ -1286,6 +1289,37 @@ class Frontend:
         th = C.c_int(0)
         self._check(self.lib.plf_get_sequence_fast_th(self._ctx, int(s), C.byref(th)), "plf_get_sequence_fast_th")
         return th.value
+
+    def set_motion_model(self, on=True):
+        """stvo-pl's use_motion_model for the batched pipeline: each sequence's next pair starts from the prediction its
+        last pair gave (its windowed frame-to-frame matching projects through it, and the pose solver is seeded with it).
+        With it on, a batch holds at most one pair of each sequence.  Turning it on sets every prediction back to the
+        identity.  plf_set_motion_model."""
+        self._check(self.lib.plf_set_motion_model(self._ctx, 1 if on else 0), "plf_set_motion_model")
+
+    def sequence_motion(self, s):
+        """(T, valid): the prediction (4x4 float64) the next pair of sequence s will start from, and whether it came from
+        a good solution (the identity and False otherwise).  plf_get_sequence_motion."""
+        T = np.zeros(16, np.float64)
+        valid = C.c_int(0)
+        self._check(self.lib.plf_get_sequence_motion(self._ctx, int(s), _ptr(T, C.c_double), C.byref(valid)),
+                    "plf_get_sequence_motion")
+        return T.reshape(4, 4), bool(valid.value)
+
+    def debug_motion_prior(self, DT, DT_cov, err, status):
+        """plf_debug_motion_prior: the device's prediction rule on n results (DT [n,4,4], DT_cov [n,6,6], err [n],
+        status [n]); returns (T [n,4,4], valid [n] bool)."""
+        DT = np.ascontiguousarray(DT, np.float64).reshape(-1, 16)
+        n = len(DT)
+        cov = np.ascontiguousarray(DT_cov, np.float64).reshape(n, 36)
+        err = np.ascontiguousarray(err, np.float64).reshape(n)
+        status = np.ascontiguousarray(status, np.int32).reshape(n)
+        T = np.zeros((n, 16), np.float64)
+        valid = np.zeros(n, np.int32)
+        self._check(self.lib.plf_debug_motion_prior(self._ctx, n, _ptr(DT, C.c_double), _ptr(cov, C.c_double),
+                                                    _ptr(err, C.c_double), _ptr(status, C.c_int32), _ptr(T, C.c_double),
+                                                    _ptr(valid, C.c_int32)), "plf_debug_motion_prior")
+        return T.reshape(n, 4, 4), valid.astype(bool)
 
     @staticmethod
     def _result_dicts(res, B):
