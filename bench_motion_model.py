@@ -12,7 +12,7 @@ of the rendered pool, where a constant-motion prediction points the wrong way). 
 off and on.  Reported per arm: pairs/s over the --steps timed batches after --warmup, the fraction of tracked pairs, the
 mean GN iterations (iters1 + iters2) and frame-to-frame point matches per tracked pair of the timed batches.
 
-With a windowed strategy the oracle (tests/motion_model_oracle.py, on the CPU) also runs --oracle-pairs consecutive
+With a windowed strategy the oracle (oracle/frontend.py run_sequence, on the CPU) also runs --oracle-pairs consecutive
 pairs of one camera off and on, and reports the windowed point matches per tracked pair and how many pairs fall back to
 match().  The GPU's name, power limit and SM clocks sampled during the timed regions are printed with the results.
 """
@@ -60,7 +60,6 @@ def run_arm(plf, L, R, period, N, steps, warmup, strategy, on):
 def oracle_counts(pool, n, strategy):
     """The oracle on the first n pairs of one camera's ping-pong order, off (identity predictions) and on: windowed
     point matches per tracked pair, pairs that fall back to match(), and GN iterations per tracked pair."""
-    import motion_model_oracle as mmo
     from oracle import frontend as ofe
     pairs = [pool[i] for i in (list(range(len(pool))) + list(range(len(pool) - 2, 0, -1)))[:n]]
     prm = dict(ofe.DEFAULTS, **bench.PRM, matching_strategy=strategy)
@@ -68,7 +67,7 @@ def oracle_counts(pool, n, strategy):
     out = {}
     for arm in ("off", "on"):
         preds = [np.eye(4)] * n if arm == "off" else None   # identity predictions: the off pipeline (finite points)
-        r = [o for o in mmo.run_sequence(bench.CAM, pairs, prm, preds=preds, frames=frames) if o["status"] == 0]
+        r = [o for o in ofe.run_sequence(bench.CAM, pairs, prm, motion_model=True, preds=preds, frames=frames) if o["status"] == 0]
         out[arm] = dict(tracked=len(r), pt_window=round(float(np.mean([o["stats"]["pt_window"] for o in r])), 1),
                         pt_fallback=sum(o["stats"]["pt_fallback"] for o in r),
                         gn_iters=round(float(np.mean([sum(o["res"]["iters"]) for o in r])), 3))

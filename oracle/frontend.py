@@ -9,7 +9,9 @@ detect_lines   stvo-pl StereoFrame::detectLineFeatures, LSD branch (SURVEY.md Ap
 """
 import numpy as np
 
+from oracle import adaptive_fast as af
 from oracle import clib
+from oracle import motion_model as mm
 
 
 def detect_lines(img, lsd_nfeatures=300, min_line_length=0.025, lsd_kwargs=None, segs=None):
@@ -303,73 +305,121 @@ def projection(cam, P):
         return np.stack([cam["cx"] + cam["fx"] * P[:, 0] / P[:, 2], cam["cy"] + cam["fy"] * P[:, 1] / P[:, 2]], 1)
 
 
-def track_matches(cam, prev: Frame, curr: Frame, prm, match_fn=None):
+def track_matches(cam, prev: Frame, curr: Frame, prm, match_fn=None, T_pred=None, stats=None):
     """The two matches_12 vectors of f2fTracking.  matching_strategy 0: match() on the stereo-valid descriptors (A.2).
-    Otherwise the control flow of the in-tree analogue (src/mapHandler.cpp:247-278, :379-425) with DT = identity
-    (use_motion_model false): the previous frame's 3-D features are projected, matched in a +-matching_f2f_ws window of
-    the current frame's grid, and match() takes over when fewer than min_pt_matches / min_ls_matches survive (both
-    frames holding more features than that).  Projected lines are scaled to grid units like the points (the analogue
-    leaves them in pixels, :395, which empties the window; not reproduced)."""
+    Otherwise the control flow of the in-tree analogue (src/mapHandler.cpp:247-278, :379-425): the previous frame's 3-D
+    features are projected, matched in a +-matching_f2f_ws window of the current frame's grid, and match() takes over
+    when fewer than min_pt_matches / min_ls_matches survive (both frames holding more features than that).  The points
+    and line end points are moved by T_pred before the projection when it is given (use_motion_model; the analogue
+    projects through DT, :254-256, :384-389), else projected as they are (DT = identity).  Projected lines are scaled to
+    grid units like the points (the analogue leaves them in pixels, :395, which empties the window; not reproduced).
+    stats (a dict) gets the windowed point / line match counts (pt_window, ls_window) and whether match() took over
+    (pt_fallback, ls_fallback)."""
     mfn = match_fn or om.match
     if not prm.get("matching_strategy", 0) or match_fn is not None:
         mp, _ = mfn(prev.pdesc, curr.pdesc, prm["min_ratio_12_p"], prm["best_lr_matches"])
         ml, _ = mfn(prev.ldesc, curr.ldesc, prm["min_ratio_12_l"], prm["best_lr_matches"])
         return mp, ml
+    from oracle.kfmatching import rigid   # here: oracle.kfmatching imports this module
+    proj = lambda X: projection(cam, X if T_pred is None else rigid(T_pred, X))
+    stats = {} if stats is None else stats
     ws = int(prm["matching_f2f_ws"])
     w = (ws, ws, ws, ws)
     mp, ml = np.full(len(prev.pdesc), -1, np.int32), np.full(len(prev.ldesc), -1, np.int32)
     if len(prev.pdesc) and len(curr.pdesc):
-        mp, n = grid_match_points(cam, projection(cam, prev.pt_P), prev.pdesc, curr.pt_pl, curr.pdesc, w,
+        mp, n = grid_match_points(cam, proj(prev.pt_P), prev.pdesc, curr.pt_pl, curr.pdesc, w,
                                   prm["min_ratio_12_p"], prm["best_lr_matches"])
         k = int(prm["min_pt_matches"])
-        if len(curr.pdesc) > k and len(prev.pdesc) > k and n < k:
+        fall = len(curr.pdesc) > k and len(prev.pdesc) > k and n < k
+        if fall:
             mp, _ = om.match(prev.pdesc, curr.pdesc, prm["min_ratio_12_p"], prm["best_lr_matches"])
+        stats.update(pt_window=int(n), pt_fallback=bool(fall))
     if len(prev.ldesc) and len(curr.ldesc):
-        q = np.concatenate([projection(cam, prev.ls_sP), projection(cam, prev.ls_eP)], 1)
+        q = np.concatenate([proj(prev.ls_sP), proj(prev.ls_eP)], 1)
         t = np.concatenate([curr.ls_spl, curr.ls_epl], 1)
         ml, n = grid_match_lines(cam, q, prev.ldesc, t, curr.ldesc, w, prm["min_ratio_12_l"], prm["line_sim_th"],
                                  prm["best_lr_matches"])
         k = int(prm["min_ls_matches"])
-        if len(curr.ldesc) > k and len(prev.ldesc) > k and n < k:
+        fall = len(curr.ldesc) > k and len(prev.ldesc) > k and n < k
+        if fall:
             ml, _ = om.match(prev.ldesc, curr.ldesc, prm["min_ratio_12_l"], prm["best_lr_matches"])
+        stats.update(ls_window=int(n), ls_fallback=bool(fall))
     return mp, ml
 
 
-def track(prev: Frame, curr: Frame, prm, match_fn=None, cam=None):
-    """f2fTracking: the two matches_12 vectors (track_matches), then the GN rows."""
-    mp, ml = track_matches(cam, prev, curr, prm, match_fn)
+def track(prev: Frame, curr: Frame, prm, match_fn=None, cam=None, T_pred=None):
+    """f2fTracking: the two matches_12 vectors (track_matches, with the prediction T_pred), then the GN rows; the
+    matching's stats under "stats"."""
+    stats = {}
+    mp, ml = track_matches(cam, prev, curr, prm, match_fn, T_pred, stats)
     ip = np.nonzero(mp >= 0)[0]
     P, obs = prev.pt_P[ip], curr.pt_pl[mp[ip]]
     il = np.nonzero(ml >= 0)[0]
     sP, eP, le = prev.ls_sP[il], prev.ls_eP[il], curr.ls_le[ml[il]]
-    return dict(P=P, obs=obs, sP=sP, eP=eP, le=le, mp=mp, ml=ml)
+    return dict(P=P, obs=obs, sP=sP, eP=eP, le=le, mp=mp, ml=ml, stats=stats)
 
 
-def optimize_pose(cam, tr, prm):
-    """optimizePose: two-stage GN from identity; fewer than min_features rows -> identity.  Returns curr.DT
-    (= inverse of the optimised increment), the raw result (with the solver's stop-decision trace, its options, camera
-    and rows, so that a result of another solver can be compared with it: clib.gn_decidable) and a status flag."""
+def optimize_pose(cam, tr, prm, T_pred=None):
+    """optimizePose: two-stage GN from identity, or seeded with T_pred when given (clib.gn_pose T_init); fewer than
+    min_features rows -> identity.  Returns curr.DT (= inverse of the optimised increment), the raw result (with the
+    solver's stop-decision trace, its options, camera and rows, so that a result of another solver can be compared with
+    it: clib.gn_decidable) and a status flag."""
     n = len(tr["P"]) + len(tr["sP"])
     if n < prm["min_features"]:
         return np.eye(4), None, 1
     o = clib.gn_opts(prm["homog_th"], prm["max_iters"], prm["max_iters_ref"], prm["min_error"], prm["min_error_change"])
-    r = clib.gn_pose(cam, tr["P"], tr["obs"], tr["sP"], tr["eP"], tr["le"], opts=o, trace=True)
+    r = clib.gn_pose(cam, tr["P"], tr["obs"], tr["sP"], tr["eP"], tr["le"], T_init=T_pred, opts=o, trace=True)
     r.update(opts=o, cam=cam, rows={k: tr[k] for k in ("P", "obs", "sP", "eP", "le")})
     return clib.inverse_se3(r["T"]), r, 0
 
 
-def run_sequence(cam, pairs, prm=None, orb_fn=None, lines_fn=None, match_fn=None, pool=None, frames=None):
-    """The hot loop of app/plslam_dataset.cpp:111-163 without keyframe hand-off: returns per-frame DT (4x4), Tfw."""
+def run_sequence(cam, pairs, prm=None, orb_fn=None, lines_fn=None, match_fn=None, pool=None, frames=None, restarts=(),
+                 motion_model=None, preds=None, adaptive_fast=None, fast_th=None):
+    """The hot loop of app/plslam_dataset.cpp:111-163 without keyframe hand-off: returns per-frame DT (4x4), Tfw.
+    `restarts` are pair indices that are first frames.
+
+    motion_model (oracle/motion_model.py) True: pair i starts from preds[i] when given (the predictions another run
+    used, so that a rounding difference at an edge of the rule cannot make two runs diverge), else from the prediction
+    carried from pair i - 1.  True or False (every pair from identity): each entry also holds T_pred (used), T_next /
+    valid_next (the rule on this run's own result) and stats (track_matches).
+
+    adaptive_fast (a plf_adaptive_fast dict, oracle/adaptive_fast.py): pair i is detected at the carried threshold, and
+    each entry also holds th (used), th_next (the rule on this run's own result) and branch.  fast_th[i], when given, is
+    the threshold pair i is detected at instead (the thresholds another run used); each entry also holds th."""
     prm = dict(DEFAULTS, **(prm or {}))
-    prev, Tfw, out = None, np.eye(4), []
+    prev, Tfw, T, th, out = None, np.eye(4), np.eye(4), af.fast_th0(prm), []
     for idx, (L, R) in enumerate(pairs):
-        cur = frames[idx] if frames is not None else extract_stereo(cam, L, R, prm, orb_fn, lines_fn, match_fn, pool)
+        if idx in restarts:
+            prev = None
+        if prev is None:
+            T, th = np.eye(4), af.fast_th0(prm)
+        if preds is not None:
+            T = np.asarray(preds[idx], np.float64).reshape(4, 4)
+        if fast_th is not None:
+            th = int(fast_th[idx])
+        p = prm if adaptive_fast is None and fast_th is None else dict(prm, orb_fast_th=th)
+        cur = frames[idx] if frames is not None else extract_stereo(cam, L, R, p, orb_fn, lines_fn, match_fn, pool)
+        stats = {}
         if prev is None:
             DT, status, res = np.eye(4), 2, None      # initialize(): first frame
         else:
-            tr = track(prev, cur, prm, match_fn, cam=cam)
-            DT, res, status = optimize_pose(cam, tr, prm)
+            T_pred = T if motion_model else None
+            tr = track(prev, cur, prm, match_fn, cam=cam, T_pred=T_pred)
+            DT, res, status = optimize_pose(cam, tr, prm, T_pred)
+            stats = tr["stats"]
         Tfw = Tfw @ DT
-        out.append(dict(DT=DT, Tfw=Tfw.copy(), status=status, n_pt=len(cur.pt_pl), n_ls=len(cur.ls_spl), res=res, frame=cur))
+        o = dict(DT=DT, Tfw=Tfw.copy(), status=status, n_pt=len(cur.pt_pl), n_ls=len(cur.ls_spl), res=res, frame=cur)
+        err = res["err"] if status == 0 else -1.0
+        if adaptive_fast is not None or fast_th is not None:
+            o.update(th=th)
+        if adaptive_fast is not None:
+            n_in = res["n_inliers"][0] if status == 0 else 0
+            th, o["branch"] = af.fast_th_next(th, status, DT, err, n_in, adaptive_fast, trace=True)
+            o.update(th_next=th)
+        if motion_model is not None:
+            T_next, valid = mm.prior(status, DT, res["cov"] if status == 0 else np.zeros((6, 6)), err)
+            o.update(T_pred=T, T_next=T_next, valid_next=valid, stats=stats)
+            T = T_next if motion_model else np.eye(4)
+        out.append(o)
         prev = cur
     return out

@@ -24,7 +24,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <memory>
 #include <unordered_map>
 
 #include "plf_internal.h"
@@ -63,8 +62,7 @@ struct BowDbs {
 
 struct BowState {
   BowVoc voc[2];
-  BowDbs ctx_db;                                 // seq = -1: plf_bow_insert / plf_bow_erase / plf_bow_get
-  std::vector<std::unique_ptr<BowDbs>> seq_db;   // [max_sequences] once a sequence was inserted into, else empty
+  BowDbs ctx_db;   // seq = -1: plf_bow_insert / plf_bow_erase / plf_bow_get; a sequence's are in its PlfSequence
   int n_sm = 0;
   bool attr_set = false;
 };
@@ -354,10 +352,10 @@ void free_voc(BowVoc& k) {
   k.has_voc = false;
 }
 
-// The databases of seq (-1: the context's), or nullptr for a sequence never inserted into.
-BowDbs* dbs_of(BowState* S, int seq) {
-  if (seq < 0) return &S->ctx_db;
-  return seq < (int)S->seq_db.size() ? S->seq_db[seq].get() : nullptr;
+// The databases of seq (-1: the context's, in ctx->bow), or nullptr for a sequence never inserted into.
+BowDbs* dbs_of(plf_ctx* ctx, int seq) {
+  if (seq < 0) return &ctx->bow->ctx_db;
+  return ctx->seqs.empty() ? nullptr : ctx->seqs[seq].bow;
 }
 
 BowState* bow_state(plf_ctx* ctx) {
@@ -794,9 +792,8 @@ plf_status bow_insert_problems(plf_ctx* ctx, const char* fn, bool single, int n_
   std::vector<BatchDb> bdb;
   std::vector<int> prob_db(n_problems);
   for (int p = 0; p < n_problems; ++p) {
-    const int s = seq ? seq[p] : -1;
-    if (s < -1 || s >= ctx->max_sequences)
-      return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: seq[%d] = %d outside [-1, %d)", fn, p, p, s, ctx->max_sequences);
+    int s;
+    if (plf_status st = plf_problem_camera(ctx, fn, seq, p, nullptr, &s)) return st;
     const plf_bow_problem& pr = problems[p];
     if (!pr.kf) return plf_fail(ctx, PLF_ERR_INVALID, "%s: kf is NULL", name(p));
     if (pr.kf_idx < 0 || pr.kf_idx >= BOW_MAX_KF)
@@ -805,7 +802,7 @@ plf_status bow_insert_problems(plf_ctx* ctx, const char* fn, bool single, int n_
     if (it == db_at.end()) {
       it = db_at.emplace(s, (int)bdb.size()).first;
       BatchDb b;
-      b.dbs = dbs_of(S, s);
+      b.dbs = dbs_of(ctx, s);
       for (int c = 0; c < 2; ++c) b.last[c] = b.dbs ? b.dbs->kind[c].last : -1;
       bdb.push_back(b);
     }
@@ -846,11 +843,7 @@ plf_status bow_insert_problems(plf_ctx* ctx, const char* fn, bool single, int n_
   // every database grows once, to its problems' upper bound; a sequence's first allocation is one keyframe's size
   for (const auto& e : db_at) {
     BatchDb& b = bdb[e.second];
-    if (!b.dbs) {
-      if (S->seq_db.empty()) S->seq_db.resize(ctx->max_sequences);
-      S->seq_db[e.first].reset(new BowDbs());
-      b.dbs = S->seq_db[e.first].get();
-    }
+    if (!b.dbs) b.dbs = plf_sequence(ctx, e.first).bow = new BowDbs();
     for (int c = 0; c < 2; ++c) {
       if (!on[c]) continue;
       BowDb& k = b.dbs->kind[c];
@@ -1105,25 +1098,22 @@ plf_status seq_dbs(plf_ctx* ctx, const char* fn, int s, BowDbs** d) {
   *d = nullptr;
   if (s < -1 || s >= ctx->max_sequences)
     return plf_fail(ctx, PLF_ERR_INVALID, "%s: seq %d outside [-1, %d)", fn, s, ctx->max_sequences);
-  if (ctx->bow) *d = dbs_of(ctx->bow, s);
+  if (ctx->bow) *d = dbs_of(ctx, s);
   return PLF_OK;
 }
 
 }  // namespace
 
-void plf_bow_drop_sequences(plf_ctx* ctx) {
-  if (!ctx->bow) return;
-  for (auto& d : ctx->bow->seq_db)
-    if (d) free_dbs(*d);
-  ctx->bow->seq_db.clear();
-  ctx->bow->seq_db.shrink_to_fit();
+void plf_bow_dbs_free(BowDbs* d) {
+  if (!d) return;
+  free_dbs(*d);
+  delete d;
 }
 
 extern "C" {
 
 void plf_bow_free(plf_ctx* ctx) {
   if (!ctx->bow) return;
-  plf_bow_drop_sequences(ctx);
   for (BowVoc& v : ctx->bow->voc) free_voc(v);
   free_dbs(ctx->bow->ctx_db);
   delete ctx->bow;
@@ -1200,8 +1190,8 @@ plf_status plf_bow_set_vocabulary(plf_ctx* ctx, int kind, const plf_vocab* voc) 
   free_voc(k);
   // the kind is emptied in every database
   free_db(S->ctx_db.kind[kind]);
-  for (auto& d : S->seq_db)
-    if (d) free_db(d->kind[kind]);
+  for (PlfSequence& q : ctx->seqs)
+    if (q.bow) free_db(q.bow->kind[kind]);
   const size_t n = lay.meta.size();
   if (cudaMalloc(&k.desc, n * 32) != cudaSuccess || cudaMalloc(&k.meta, n * 8) != cudaSuccess ||
       cudaMalloc(&k.weight, n * 8) != cudaSuccess) {
@@ -1304,14 +1294,13 @@ plf_status plf_bow_get(plf_ctx* ctx, int kf_idx, int kind, int cap, uint32_t* wo
 
 plf_status plf_bow_clear_sequence(plf_ctx* ctx, int s) {
   if (!ctx) return PLF_ERR_INVALID;
-  if (s < 0 || s >= ctx->max_sequences)
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_bow_clear_sequence: s = %d outside [0, %d)", s, ctx->max_sequences);
-  BowDbs* d = ctx->bow ? dbs_of(ctx->bow, s) : nullptr;
+  if (plf_status st = plf_check_sequence(ctx, "plf_bow_clear_sequence", s)) return st;
+  BowDbs* d = dbs_of(ctx, s);
   if (!d) return PLF_OK;
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  free_dbs(*d);
-  ctx->bow->seq_db[s].reset();
+  plf_bow_dbs_free(d);
+  ctx->seqs[s].bow = nullptr;
   return PLF_OK;
 }
 

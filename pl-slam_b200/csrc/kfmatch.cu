@@ -544,14 +544,7 @@ plf_status batch_cameras(plf_ctx* ctx, const char* fn, const plf_kf_match_opts* 
   if (!opts || n < 0 || (n && !problems)) return plf_fail(ctx, PLF_ERR_INVALID, "%s: bad arguments (opts, n_problems = %d, problems)", fn, n);
   if (n > KF_MAX_PROBLEMS)
     return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: n_problems = %d exceeds %d", fn, n, KF_MAX_PROBLEMS);
-  cams.resize(n);
-  for (int p = 0; p < n; ++p) {
-    const int s = seq ? seq[p] : -1;
-    if (s < -1 || s >= ctx->max_sequences)
-      return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: seq[%d] = %d outside [-1, %d)", fn, p, p, s, ctx->max_sequences);
-    cams[p] = s >= 0 && !ctx->seq_cam_own.empty() && ctx->seq_cam_own[s] ? &ctx->seq_cam[s] : &ctx->cam;
-  }
-  return PLF_OK;
+  return plf_problem_cameras(ctx, fn, n, seq, cams);
 }
 
 }  // namespace

@@ -1021,17 +1021,15 @@ static plf_status lbb_run(plf_ctx* ctx, const plf_lba_opts* opts, int n_problems
   long long tN = 0, tObs = 0, tLm = 0, tKf = 0, tFix = 0, tG = 0, tS = 0, tWp = 0, tNz = 0;
   int mObs = 0, mLm = 0, mEl = 0, mBig = 0;
   for (int p = 0; p < P; ++p) {
-    const int s = seq ? seq[p] : -1;
-    if (s < -1 || s >= ctx->max_sequences)
-      return plf_fail(ctx, PLF_ERR_INVALID, "%s: seq[%d] = %d outside [-1, %d)", fn, p, s, ctx->max_sequences);
-    const plf_camera& c = s >= 0 && !ctx->seq_cam_own.empty() && ctx->seq_cam_own[s] ? ctx->seq_cam[s] : ctx->cam;
+    const plf_camera* c;
+    if (plf_status st = plf_problem_camera(ctx, fn, seq, p, &c)) return st;
     const plf_lba_problem& pr = problems[p];
     if (plf_status st = lba_check_shape(ctx, prefix(p), &pr, global ? 4096 : 64)) return st;
     LbbProb& q = hp[p];
     q.nkf = pr.n_kf; q.npt = pr.n_pt; q.nls = pr.n_ls; q.npo = pr.n_pt_obs; q.nobs = pr.n_pt_obs + pr.n_ls_obs;
     q.nlm = pr.n_pt + pr.n_ls; q.N = 6 * pr.n_kf + 3 * pr.n_pt + 6 * pr.n_ls; q.nfix = pr.n_fixed;
     q.xo = tN; q.oo = tObs; q.lo = tLm; q.ko = tKf; q.fo = tFix; q.go = tG; q.so = tS;
-    q.cam = LbaCam{c.fx, c.fy, c.cx, c.cy};
+    q.cam = LbaCam{c->fx, c->fy, c->cx, c->cy};
     if (q.nkf > 64) {   // n > 384: the tiled LDL^T (k_gbb_*)
       const long long nt = (6 * q.nkf + GBA_T - 1) / GBA_T;
       hb.push_back(GbbBig{p, q.nkf, q.so, q.go, q.xo, tWp, tNz});

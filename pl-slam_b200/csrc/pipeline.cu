@@ -56,6 +56,7 @@ struct PipeState {
   int nseq = 1;
   std::vector<uint8_t> carried;  // [nseq] sequence s has a frame in its carry slot
   std::vector<int> last_pair;    // [nseq] scratch of plf_batch_run_sequences: the batch's last pair of each sequence, or -1
+  std::vector<int> pair_seq;     // [B] scratch of plf_batch_run_sequences: the sequence of each pair of the batch
   // The sequence table of a batch: prev[max_batch] (slot of pair k's previous frame), then the carry list [max_batch][2]
   // (frame slot, carry slot).  Rings indexed like h_results (up to three batches in flight): pinned h_tab, device seq_tab
   // [3][3 max_batch].  The copy goes on the copy stream, in order behind the batch's own images and ahead of the next
@@ -883,12 +884,12 @@ __global__ void __launch_bounds__(256) k_rectify(const PlfRectPair* __restrict__
 // reads it: on the copy stream, behind the upload, each such pair is remapped into scratch and copied back in place, and
 // ev_up[run_slot] is recorded again, so the E and P phases (which wait for it) read the rectified images.  The copy stream
 // orders one batch's scratch use before the next's.  A batch without such a pair enqueues nothing.
-static plf_status run_rectify(plf_ctx* ctx, PipeState* s, const BatchRun& r, const int32_t* seq) {
-  if (ctx->seq_rect.empty()) return PLF_OK;
+static plf_status run_rectify(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
+  if (ctx->seqs.empty()) return PLF_OK;
   PlfRectPair* ht = s->h_rect[r.rp];
   int nr = 0;
   for (int k = 0; k < r.B; ++k)
-    if (const uint8_t* maps = ctx->seq_rect[seq ? seq[k] : 0]) ht[nr++] = PlfRectPair{maps, k, 0};
+    if (const uint8_t* maps = ctx->seqs[s->pair_seq[k]].rect) ht[nr++] = PlfRectPair{maps, k, 0};
   if (nr == 0) return PLF_OK;
   const size_t AP = (size_t)s->pitch * s->h;
   PlfRectPair* tab;
@@ -1132,24 +1133,21 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   return PLF_OK;
 }
 
-extern "C" {
-
-}  // extern "C"
-
-void plf_rect_drop_sequences(plf_ctx* ctx) {
-  for (uint8_t* d : ctx->seq_rect) cudaFree(d);
-  ctx->seq_rect.clear();
+// Sequence s (-1: every sequence) restarts: its next pair in a run is a first frame (the batches run keep their tables).
+static void restart_sequence(plf_ctx* ctx, int s) {
+  if (!ctx->pipe) return;
+  std::vector<uint8_t>& c = ctx->pipe->carried;
+  if (s < 0) std::fill(c.begin(), c.end(), 0);
+  else c[s] = 0;
 }
 
 extern "C" {
 
 plf_status plf_reset_sequence(plf_ctx* ctx) {
   if (!ctx) return PLF_ERR_INVALID;
-  if (ctx->pipe) {
-    if (ctx->pipe->n_pending)
-      return plf_fail(ctx, PLF_ERR_STATE, "plf_reset_sequence: %d batch(es) still in flight; download them first", ctx->pipe->n_pending);
-    std::fill(ctx->pipe->carried.begin(), ctx->pipe->carried.end(), 0);
-  }
+  if (ctx->pipe && ctx->pipe->n_pending)
+    return plf_fail(ctx, PLF_ERR_STATE, "plf_reset_sequence: %d batch(es) still in flight; download them first", ctx->pipe->n_pending);
+  restart_sequence(ctx, -1);
   return PLF_OK;
 }
 
@@ -1158,18 +1156,14 @@ plf_status plf_set_max_sequences(plf_ctx* ctx, int n) {
   if (n < 1 || n > PLF_MAX_SEQUENCES)
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_max_sequences: n = %d, need 1 <= n <= %d", n, PLF_MAX_SEQUENCES);
   if (ctx->pipe) return plf_fail(ctx, PLF_ERR_STATE, "plf_set_max_sequences: the pipeline exists (a batch call was made)");
+  plf_drop_sequences(ctx);
   ctx->max_sequences = n;
-  ctx->seq_cam.clear();
-  ctx->seq_cam_own.clear();
-  plf_rect_drop_sequences(ctx);
-  plf_bow_drop_sequences(ctx);
   return PLF_OK;
 }
 
 plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam) {
   if (!ctx) return PLF_ERR_INVALID;
-  if (s < 0 || s >= ctx->max_sequences)
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: s = %d outside [0, %d)", s, ctx->max_sequences);
+  if (plf_status st = plf_check_sequence(ctx, "plf_set_sequence_camera", s)) return st;
   if (cam) {
     if (cam->width != ctx->cam.width)
       return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: width = %d, the context's is %d", cam->width, ctx->cam.width);
@@ -1182,22 +1176,17 @@ plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam) {
         return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: %s = %g, need a finite value%s", e.name, e.v,
                         e.positive ? " > 0" : "");
   }
-  if (ctx->seq_cam_own.empty()) {
-    ctx->seq_cam.assign(ctx->max_sequences, ctx->cam);
-    ctx->seq_cam_own.assign(ctx->max_sequences, 0);
-  }
-  ctx->seq_cam[s] = cam ? *cam : ctx->cam;
-  ctx->seq_cam_own[s] = cam ? 1 : 0;
-  // the sequence restarts: its next pair in a run is a first frame (the batches already run have their tables)
-  if (ctx->pipe) ctx->pipe->carried[s] = 0;
+  PlfSequence& q = plf_sequence(ctx, s);
+  q.own_cam = cam != nullptr;
+  q.cam = cam ? *cam : ctx->cam;
+  restart_sequence(ctx, s);
   return PLF_OK;
 }
 
 plf_status plf_set_sequence_rectification(plf_ctx* ctx, int s, const int16_t* map1_l, const uint16_t* map2_l,
                                           const int16_t* map1_r, const uint16_t* map2_r) {
   if (!ctx) return PLF_ERR_INVALID;
-  if (s < 0 || s >= ctx->max_sequences)
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_rectification: s = %d outside [0, %d)", s, ctx->max_sequences);
+  if (plf_status st = plf_check_sequence(ctx, "plf_set_sequence_rectification", s)) return st;
   const int given = !!map1_l + !!map2_l + !!map1_r + !!map2_r;
   if (given != 0 && given != 4)
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_rectification: %d of the four maps given, need all four or none (NULL clears)",
@@ -1205,7 +1194,7 @@ plf_status plf_set_sequence_rectification(plf_ctx* ctx, int s, const int16_t* ma
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   // the copy stream runs every rectification: once it is idle, no batch run so far reads sequence s's old maps
   cudaStream_t cs = ctx->pipe ? ctx->pipe->copy : ctx->stream;
-  uint8_t* old = ctx->seq_rect.empty() ? nullptr : ctx->seq_rect[s];
+  uint8_t* old = ctx->seqs.empty() ? nullptr : ctx->seqs[s].rect;
   const size_t A = (size_t)ctx->cam.width * ctx->cam.height;
   if (given) {
     uint8_t* d = old;
@@ -1225,15 +1214,14 @@ plf_status plf_set_sequence_rectification(plf_ctx* ctx, int s, const int16_t* ma
       if (!old) cudaFree(d);
       return plf_fail(ctx, PLF_ERR_CUDA, "plf_set_sequence_rectification: copying the maps: %s", cudaGetErrorString(e));
     }
-    if (ctx->seq_rect.empty()) ctx->seq_rect.assign(ctx->max_sequences, nullptr);
-    ctx->seq_rect[s] = d;
+    plf_sequence(ctx, s).rect = d;
   } else if (old) {
     PLF_CUDA(ctx, cudaStreamSynchronize(cs));
     cudaFree(old);
-    ctx->seq_rect[s] = nullptr;
+    ctx->seqs[s].rect = nullptr;
   }
-  // the sequence restarts: its carried frame was extracted from other images (the batches already run have their tables)
-  if (ctx->pipe) ctx->pipe->carried[s] = 0;
+  // its carried frame was extracted from other images
+  restart_sequence(ctx, s);
   return PLF_OK;
 }
 
@@ -1241,9 +1229,8 @@ plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out) {
   if (!ctx) return PLF_ERR_INVALID;
   plf_ctx* c = const_cast<plf_ctx*>(ctx);   // the error text is the only state a failed call writes
   if (!out) return plf_fail(c, PLF_ERR_INVALID, "plf_get_sequence_camera: out is NULL");
-  if (s < 0 || s >= ctx->max_sequences)
-    return plf_fail(c, PLF_ERR_INVALID, "plf_get_sequence_camera: s = %d outside [0, %d)", s, ctx->max_sequences);
-  *out = !ctx->seq_cam_own.empty() && ctx->seq_cam_own[s] ? ctx->seq_cam[s] : ctx->cam;
+  if (plf_status st = plf_check_sequence(c, "plf_get_sequence_camera", s)) return st;
+  *out = plf_sequence_camera(ctx, s);
   return PLF_OK;
 }
 
@@ -1274,8 +1261,7 @@ plf_status plf_set_adaptive_fast(plf_ctx* ctx, const plf_adaptive_fast* cfg) {
 plf_status plf_get_sequence_fast_th(plf_ctx* ctx, int s, int* th) {
   if (!ctx) return PLF_ERR_INVALID;
   if (!th) return plf_fail(ctx, PLF_ERR_INVALID, "plf_get_sequence_fast_th: th is NULL");
-  if (s < 0 || s >= ctx->max_sequences)
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_get_sequence_fast_th: s = %d outside [0, %d)", s, ctx->max_sequences);
+  if (plf_status st = plf_check_sequence(ctx, "plf_get_sequence_fast_th", s)) return st;
   *th = fast_th0(ctx);
   if (!ctx->afast_on || !ctx->pipe || !ctx->pipe->carried[s]) return PLF_OK;   // the next pair is detected at orb_fast_th
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -1302,8 +1288,7 @@ plf_status plf_set_motion_model(plf_ctx* ctx, int on) {
 plf_status plf_get_sequence_motion(plf_ctx* ctx, int s, double T[16], int* valid) {
   if (!ctx) return PLF_ERR_INVALID;
   if (!T || !valid) return plf_fail(ctx, PLF_ERR_INVALID, "plf_get_sequence_motion: T and valid are required");
-  if (s < 0 || s >= ctx->max_sequences)
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_get_sequence_motion: s = %d outside [0, %d)", s, ctx->max_sequences);
+  if (plf_status st = plf_check_sequence(ctx, "plf_get_sequence_motion", s)) return st;
   for (int i = 0; i < 16; ++i) T[i] = (i % 5 == 0) ? 1.0 : 0.0;
   *valid = 0;
   if (!ctx->motion_on || !ctx->pipe || !ctx->pipe->carried[s]) return PLF_OK;   // the next pair starts from identity
@@ -1397,27 +1382,29 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   if (!ctx || B < 1 || B > ctx->limits.max_batch) return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_run: bad B");
   if (seq)
     for (int k = 0; k < B; ++k)
-      if (seq[k] < 0 || seq[k] >= ctx->max_sequences)
-        return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_run_sequences: seq[%d] = %d outside [0, %d)", k, seq[k], ctx->max_sequences);
+      if (plf_status st = plf_check_sequence(ctx, "plf_batch_run_sequences", seq[k], k)) return st;
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   plf_status st = pipe_prepare(ctx);
   if (st) return st;
   PipeState* s = ctx->pipe;
   if (s->n_pending >= 3)
     return plf_fail(ctx, PLF_ERR_STATE, "plf_batch_run: three batches already in flight; call plf_batch_download first");
+  if (seq) s->pair_seq.assign(seq, seq + B);
+  else s->pair_seq.assign(B, 0);
+  const int* q = s->pair_seq.data();
   // pair k of a sequence is detected at the threshold pair k-1's pose gives, or starts from the prediction pair k-1's pose
   // gives: one pair per sequence
   if (ctx->afast_on || ctx->motion_on) {
     int first = -1, dup = -1;
     for (int k = 0; k < B && dup < 0; ++k) {
-      int& last = s->last_pair[seq ? seq[k] : 0];
+      int& last = s->last_pair[q[k]];
       if (last >= 0) { first = last; dup = k; }
       else last = k;
     }
-    for (int k = 0; k < B; ++k) s->last_pair[seq ? seq[k] : 0] = -1;
+    for (int k = 0; k < B; ++k) s->last_pair[q[k]] = -1;
     if (dup >= 0)
       return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_run_sequences: pairs %d and %d are both of sequence %d; with %s a batch "
-                      "holds at most one pair of each sequence", first, dup, seq ? seq[dup] : 0,
+                      "holds at most one pair of each sequence", first, dup, q[dup],
                       ctx->afast_on ? "adaptive FAST thresholds (plf_set_adaptive_fast)" : "the motion model (plf_set_motion_model)");
   }
   BatchRun r;
@@ -1430,29 +1417,25 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   int32_t* carry = prev + s->B;
   const int empty = s->B + s->nseq;
   for (int k = 0; k < B; ++k) {
-    const int q = seq ? seq[k] : 0;
     if (restart && restart[k]) prev[k] = empty;
-    else if (s->last_pair[q] >= 0) prev[k] = s->last_pair[q];
-    else prev[k] = s->carried[q] ? s->B + q : empty;
-    s->last_pair[q] = k;
+    else if (s->last_pair[q[k]] >= 0) prev[k] = s->last_pair[q[k]];
+    else prev[k] = s->carried[q[k]] ? s->B + q[k] : empty;
+    s->last_pair[q[k]] = k;
   }
   r.ncarry = 0;
   for (int k = 0; k < B; ++k) {
-    const int q = seq ? seq[k] : 0;
-    if (s->last_pair[q] != k) continue;
+    if (s->last_pair[q[k]] != k) continue;
     carry[2 * r.ncarry] = k;
-    carry[2 * r.ncarry + 1] = s->B + q;
+    carry[2 * r.ncarry + 1] = s->B + q[k];
     r.ncarry++;
   }
   // the cameras of the pairs, resolved now: a later plf_set_sequence_camera does not reach this batch
   r.cams = false;
-  if (!ctx->seq_cam_own.empty())
-    for (int k = 0; k < B && !r.cams; ++k) r.cams = ctx->seq_cam_own[seq ? seq[k] : 0] != 0;
-  if (r.cams)
-    for (int k = 0; k < B; ++k) {
-      const plf_camera& c = ctx->seq_cam[seq ? seq[k] : 0];
-      s->h_cam[r.rp][k] = PlfPairCam{c.fx, c.fy, c.cx, c.cy, c.b};
-    }
+  for (int k = 0; k < B; ++k) {
+    const plf_camera& c = plf_sequence_camera(ctx, q[k]);
+    s->h_cam[r.rp][k] = PlfPairCam{c.fx, c.fy, c.cx, c.cy, c.b};
+    r.cams |= &c != &ctx->cam;
+  }
   r.run_slot = s->up_slot;
   // With profiling on everything is serialised on the main stream so that the per-kernel marks are meaningful.
   r.piped = !ctx->profile || ctx->profile_piped;
@@ -1464,15 +1447,14 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   r.sP = (r.piped && r.lsd2) ? ctx->aux[2] : r.sG;   // LSD pre-grow chain: own stream when its outputs exist per parity
   r.afast = ctx->afast_on;
   r.motion = ctx->motion_on;
-  st = run_rectify(ctx, s, r, seq);
+  st = run_rectify(ctx, s, r);
   if (!st && r.afast) st = send_tab(ctx, s, r);
   if (!st) st = run_extract(ctx, s, r);
   if (!st) st = run_lsd(ctx, s, r);
   if (!st) st = run_match(ctx, s, r);
   for (int k = 0; k < B; ++k) {
-    const int q = seq ? seq[k] : 0;
-    s->last_pair[q] = -1;
-    if (!st) s->carried[q] = 1;
+    s->last_pair[q[k]] = -1;
+    if (!st) s->carried[q[k]] = 1;
   }
   if (st) return st;
   s->pend_slot[s->n_pending] = r.rp;

@@ -20,15 +20,34 @@ plf_status plf_fail(plf_ctx* ctx, plf_status code, const char* fmt, ...) {
   return code;
 }
 
+plf_status plf_check_sequence(plf_ctx* ctx, const char* fn, int s, int k) {
+  if (s >= 0 && s < ctx->max_sequences) return PLF_OK;
+  if (k < 0) return plf_fail(ctx, PLF_ERR_INVALID, "%s: s = %d outside [0, %d)", fn, s, ctx->max_sequences);
+  return plf_fail(ctx, PLF_ERR_INVALID, "%s: seq[%d] = %d outside [0, %d)", fn, k, s, ctx->max_sequences);
+}
+
+plf_status plf_problem_camera(plf_ctx* ctx, const char* fn, const int32_t* seq, int p, const plf_camera** cam, int* s) {
+  const int q = seq ? seq[p] : -1;
+  if (q < -1 || q >= ctx->max_sequences)
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: seq[%d] = %d outside [-1, %d)", fn, p, p, q, ctx->max_sequences);
+  if (cam) *cam = &plf_sequence_camera(ctx, q);
+  if (s) *s = q;
+  return PLF_OK;
+}
+
 plf_status plf_problem_cameras(plf_ctx* ctx, const char* fn, int n, const int32_t* seq, std::vector<const plf_camera*>& cams) {
   cams.resize(n);
-  for (int p = 0; p < n; ++p) {
-    const int s = seq ? seq[p] : -1;
-    if (s < -1 || s >= ctx->max_sequences)
-      return plf_fail(ctx, PLF_ERR_INVALID, "%s: problem %d: seq[%d] = %d outside [-1, %d)", fn, p, p, s, ctx->max_sequences);
-    cams[p] = s >= 0 && !ctx->seq_cam_own.empty() && ctx->seq_cam_own[s] ? &ctx->seq_cam[s] : &ctx->cam;
-  }
+  for (int p = 0; p < n; ++p)
+    if (plf_status st = plf_problem_camera(ctx, fn, seq, p, &cams[p])) return st;
   return PLF_OK;
+}
+
+void plf_drop_sequences(plf_ctx* ctx) {
+  for (PlfSequence& q : ctx->seqs) {
+    cudaFree(q.rect);
+    plf_bow_dbs_free(q.bow);
+  }
+  std::vector<PlfSequence>().swap(ctx->seqs);   // and its capacity
 }
 
 size_t DevBufList::bytes() const {
@@ -291,7 +310,7 @@ void plf_destroy(plf_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   plf_pipe_free(ctx);
-  plf_rect_drop_sequences(ctx);
+  plf_drop_sequences(ctx);
   plf_bow_free(ctx);
   plf_orb_free(ctx->orb_standalone);
   plf_lsd_free(ctx->lsd_standalone);

@@ -77,6 +77,15 @@ struct StagedLayout {
 struct OrbState;      // orb.cu
 struct LsdState;      // lsd.cu
 struct PlfTmaCache;   // plf_tma.cuh
+struct BowDbs;        // dbow.cu
+
+// What one sequence of a batched context has of its own; plf_reset_sequence keeps it, plf_drop_sequences frees it.
+struct PlfSequence {
+  bool own_cam = false;     // plf_set_sequence_camera: cam is the sequence's calibration, else it uses the context's
+  plf_camera cam = {};
+  uint8_t* rect = nullptr;  // plf_set_sequence_rectification: device block of 12 w h bytes (PLF_RECT_* layout, pipeline.cu)
+  BowDbs* bow = nullptr;    // its bag-of-words databases (dbow.cu), from its first insert
+};
 
 struct plf_ctx {
   int device = 0;
@@ -86,13 +95,8 @@ struct plf_ctx {
   plf_camera cam;
   plf_limits limits;
   int max_sequences = 1;          // plf_set_max_sequences: fixed once the pipeline exists
-  // plf_set_sequence_camera: [max_sequences] once a sequence has its own calibration, else empty; seq_cam[s] is used
-  // where seq_cam_own[s], else cam.  plf_set_max_sequences clears both.
-  std::vector<plf_camera> seq_cam;
-  std::vector<uint8_t> seq_cam_own;
-  // plf_set_sequence_rectification: [max_sequences] once a sequence has maps, else empty; seq_rect[s] is sequence s's
-  // device block of 12 w h bytes (PLF_RECT_* layout, pipeline.cu) or null.  plf_set_max_sequences and plf_destroy free them.
-  std::vector<uint8_t*> seq_rect;
+  // [max_sequences] once a sequence has something of its own (plf_sequence), else empty: every sequence at its defaults
+  std::vector<PlfSequence> seqs;
   bool afast_on = false;          // plf_set_adaptive_fast: per-sequence FAST thresholds in the batched pipeline
   plf_adaptive_fast afast = {};
   bool motion_on = false;         // plf_set_motion_model: per-sequence pose predictions in the batched pipeline
@@ -120,16 +124,28 @@ struct plf_ctx {
 void plf_mark(plf_ctx* ctx, cudaStream_t cs, const char* name);
 
 plf_status plf_fail(plf_ctx* ctx, plf_status code, const char* fmt, ...);
-// The camera of each problem of a batch call: seq NULL or seq[p] = -1 the context's, 0 <= seq[p] < max_sequences what
-// plf_get_sequence_camera returns now.  Any other entry returns PLF_ERR_INVALID naming fn, the problem and the entry.
+// Refuses a sequence index s outside [0, max_sequences), naming fn and s, or entry k of a seq array when k >= 0.
+plf_status plf_check_sequence(plf_ctx* ctx, const char* fn, int s, int k = -1);
+// Sequence s's record, sizing the records to max_sequences on the first call: call it to give s something of its own.
+inline PlfSequence& plf_sequence(plf_ctx* ctx, int s) {
+  if (ctx->seqs.empty()) ctx->seqs.resize(ctx->max_sequences);
+  return ctx->seqs[s];
+}
+// The camera of sequence s (-1: the context's): its own calibration if it has one, else the context's.
+inline const plf_camera& plf_sequence_camera(const plf_ctx* ctx, int s) {
+  return s >= 0 && !ctx->seqs.empty() && ctx->seqs[s].own_cam ? ctx->seqs[s].cam : ctx->cam;
+}
+// Problem p of a batch call: its sequence to *s (seq NULL or seq[p] = -1: the context's) and that sequence's camera now
+// to *cam, each if given.  An entry outside [-1, max_sequences) returns PLF_ERR_INVALID naming fn, the problem and entry.
+plf_status plf_problem_camera(plf_ctx* ctx, const char* fn, const int32_t* seq, int p, const plf_camera** cam, int* s = nullptr);
 plf_status plf_problem_cameras(plf_ctx* ctx, const char* fn, int n, const int32_t* seq, std::vector<const plf_camera*>& cams);
+// Frees every sequence's maps and databases and empties the records.
+void plf_drop_sequences(plf_ctx* ctx);
+// Frees one sequence's bag-of-words databases (dbow.cu); NULL is a no-op.
+void plf_bow_dbs_free(BowDbs* d);
 // Ensures scratch slot `slot` holds at least `bytes`; returns device pointer or nullptr (error set).
 void* plf_scratch(plf_ctx* ctx, plf_scratch_slot slot, size_t bytes);
 void* plf_pinned(plf_ctx* ctx, size_t bytes);
-// Frees every sequence's bag-of-words databases (dbow.cu); plf_set_max_sequences drops them.
-void plf_bow_drop_sequences(plf_ctx* ctx);
-// Frees every sequence's rectification maps (pipeline.cu); plf_set_max_sequences and plf_destroy drop them.
-void plf_rect_drop_sequences(plf_ctx* ctx);
 
 #define PLF_CUDA(ctx, call)                                                                  \
   do {                                                                                       \

@@ -1,4 +1,4 @@
-"""CPU tests of the adaptive FAST threshold (plf_set_adaptive_fast): the rule as tests/adaptive_fast_oracle.py restates it,
+"""CPU tests of the adaptive FAST threshold (plf_set_adaptive_fast): the rule as oracle/adaptive_fast.py restates it,
 branch by branch, and the argument checks of the C ABI, which run before the context is looked at."""
 import ctypes as C
 import re
@@ -7,7 +7,8 @@ from pathlib import Path
 import numpy as np
 import pytest
 
-from adaptive_fast_oracle import BRANCHES, fast_th_next, run_sequence
+from oracle import frontend as ofe
+from oracle.adaptive_fast import BRANCHES, fast_th_next
 
 ROOT = Path(__file__).resolve().parent.parent
 CFG = dict(min_th=5, max_th=50, inc_th=5, feat_th=50, err_th=0.5)   # config_euroc.yaml:36-41
@@ -68,23 +69,22 @@ def test_the_fifth_branch_is_unreachable():
 
 def test_reset_on_restart(monkeypatch):
     """The stream runner detects every first frame at orb_fast_th and carries the rule's threshold otherwise."""
-    import adaptive_fast_oracle as afo
     used = []
 
-    def extract(cam, L, R, prm):
+    def extract(cam, L, R, prm, *_):
         used.append(prm["orb_fast_th"])
-        return afo.ofe.Frame()
+        return ofe.Frame()
 
-    monkeypatch.setattr(afo.ofe, "extract_stereo", extract)   # empty frames: status 1 after the first, th - 2 inc_th
-    out = run_sequence({}, [(None, None)] * 6, dict(orb_fast_th=20), CFG, restarts={3})
+    monkeypatch.setattr(ofe, "extract_stereo", extract)   # empty frames: status 1 after the first, th - 2 inc_th
+    out = ofe.run_sequence({}, [(None, None)] * 6, dict(orb_fast_th=20), adaptive_fast=CFG, restarts={3})
     assert used == [20, 20, 10, 20, 20, 10]
     assert [o["status"] for o in out] == [2, 1, 1, 2, 1, 1]
     assert [o["branch"] for o in out] == ["first", "bad_pose", "bad_pose", "first", "bad_pose", "bad_pose"]
     used.clear()
-    run_sequence({}, [(None, None)] * 3, dict(orb_fast_th=300), CFG)
+    ofe.run_sequence({}, [(None, None)] * 3, dict(orb_fast_th=300), adaptive_fast=CFG)
     assert used == [255, 255, 245]   # orb_fast_th clamped to [0, 255] as the detector applies it
     used.clear()
-    run_sequence({}, [(None, None)] * 3, dict(orb_fast_th=20), CFG, ths=[7, 30, 0])
+    ofe.run_sequence({}, [(None, None)] * 3, dict(orb_fast_th=20), adaptive_fast=CFG, fast_th=[7, 30, 0])
     assert used == [7, 30, 0]
 
 

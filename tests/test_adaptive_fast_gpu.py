@@ -3,7 +3,7 @@
 Round-robin streams at KITTI shape, each sequence with its own camera, mix rich frames with near-flat ones (the same
 synth.World at a low albedo_sigma) and blank ones, so that the thresholds reach min_th and max_th and take every live
 branch of the rule.  Every pair is checked against the oracle pipeline run at the threshold the device used
-(tests/adaptive_fast_oracle.py), and every threshold the device carries against the rule applied to its own result."""
+(oracle/frontend.py run_sequence with oracle/adaptive_fast.py), and every threshold the device carries against the rule applied to its own result."""
 import subprocess
 
 import cv2
@@ -11,8 +11,9 @@ import numpy as np
 import pytest
 
 import plslam_b200 as plf
-from adaptive_fast_oracle import result_next, run_sequence
 from oracle import synth
+from oracle.adaptive_fast import result_next
+from oracle.frontend import run_sequence
 from test_multi_sequence_gpu import assert_same
 from test_pipeline_gpu import compare
 from test_shim import DEMO, write_frames
@@ -102,7 +103,7 @@ def test_round_robin_matches_oracle(built):
         n = len(seqs[s])
         ths_s = [th_used[(s, i)] for i in range(n)]
         assert ths_s[0] == 20   # a first frame: orb_fast_th
-        ref = run_sequence(CAMS[s], seqs[s], PRM, CFG, ths=ths_s)
+        ref = run_sequence(CAMS[s], seqs[s], PRM, adaptive_fast=CFG, fast_th=ths_s)
         res = [as_dict(got[(s, i)][0]) for i in range(n)]
         compare(ref, res, [got[(s, i)][1] for i in range(n)])
         for i in range(n):

@@ -1,4 +1,4 @@
-"""CPU tests of the motion model (plf_set_motion_model): the rule as tests/motion_model_oracle.py restates it, at each edge
+"""CPU tests of the motion model (plf_set_motion_model): the rule as oracle/motion_model.py restates it, at each edge
 of stvo-pl's isGoodSolution, the oracle pipeline with the model off and with identity predictions, and the argument
 checks of the C ABI, which run before the context is looked at."""
 import ctypes as C
@@ -8,9 +8,10 @@ from pathlib import Path
 import numpy as np
 import pytest
 
-from motion_model_oracle import eig_range, prior, run_sequence
 from oracle import clib, synth
 from oracle import frontend as ofe
+from oracle.frontend import run_sequence
+from oracle.motion_model import eig_range, prior
 
 ROOT = Path(__file__).resolve().parent.parent
 ULP0 = np.nextafter(0.0, 1.0)    # the smallest positive double
@@ -107,13 +108,13 @@ def test_off_is_todays_oracle_pipeline(strategy):
     _same(today, off)
     assert all(np.array_equal(o["T_pred"], np.eye(4)) for o in off)
     # identity predictions (finite points): the projection through I and the solver seeded with I change nothing
-    ident = run_sequence(CAM, pairs, prm, preds=[np.eye(4)] * len(pairs), frames=[o["frame"] for o in today])
+    ident = run_sequence(CAM, pairs, prm, motion_model=True, preds=[np.eye(4)] * len(pairs), frames=[o["frame"] for o in today])
     _same(today, ident)
 
 
 def test_carried_prediction_and_restart():
     pairs = _frames(4)
-    out = run_sequence(CAM, pairs, dict(PRM, matching_strategy=3), restarts={2})
+    out = run_sequence(CAM, pairs, dict(PRM, matching_strategy=3), motion_model=True, restarts={2})
     assert [o["status"] for o in out] == [2, 0, 2, 0]
     assert not out[0]["valid_next"] and np.array_equal(out[1]["T_pred"], np.eye(4))
     assert out[1]["valid_next"] and np.array_equal(out[1]["T_next"], clib.inverse_se3(out[1]["DT"]))

@@ -3,7 +3,7 @@ pipeline.
 
 Round-robin streams of several sequences, each with its own camera, at KITTI and EuRoC shape, with matching_strategy 0
 and 3 and with adaptive FAST thresholds on.  Every pair is checked against the oracle pipeline run with the predictions
-the device used (tests/motion_model_oracle.py), and every prediction the device carries against the rule applied to the
+the device used (oracle/frontend.py run_sequence with oracle/motion_model.py), and every prediction the device carries against the rule applied to the
 device's own result of the previous pair."""
 import subprocess
 
@@ -11,8 +11,9 @@ import numpy as np
 import pytest
 
 import plslam_b200 as plf
-from motion_model_oracle import prior, result_prior, run_sequence
 from oracle import synth
+from oracle.frontend import run_sequence
+from oracle.motion_model import prior, result_prior
 from test_motion_model import EDGES
 from test_multi_sequence_gpu import assert_same
 from test_pipeline_gpu import compare
@@ -107,7 +108,7 @@ def test_streams_match_oracle(built, shape, strategy, afast):
         n = len(seqs[s])
         preds = [used[(s, i)][0] for i in range(n)]
         assert np.array_equal(preds[0], np.eye(4)) and not used[(s, 0)][1]   # a first frame starts from identity
-        ref = run_sequence(cs[s], seqs[s], prm, preds=preds, fast_th=[ths[(s, i)] for i in range(n)] if afast else None)
+        ref = run_sequence(cs[s], seqs[s], prm, motion_model=True, preds=preds, fast_th=[ths[(s, i)] for i in range(n)] if afast else None)
         res = [as_dict(got[(s, i)][0]) for i in range(n)]
         compare(ref, res, [got[(s, i)][1] for i in range(n)])
         for i in range(n):
