@@ -238,6 +238,7 @@ typedef struct plf_keypoint {
  * plf_limits; nothing is written to kps / desc then, and the next call starts clean).  Work is enqueued on plf_stream in a
  * working state of its own (one image, rebuilt when the image size changes) and never touches the batched pipeline's
  * buffers, so a call between batches in flight is safe. */
+/* img is 8-bit single-channel (grey); colour input is the batched pipeline's only (plf_batch_upload_color). */
 plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, plf_keypoint* kps,
                    uint8_t* desc, int cap, int* n);
 
@@ -267,6 +268,7 @@ typedef struct plf_keyline {
  * segs, and the next call starts clean).  Work is enqueued on plf_stream in a working state of its own (one
  * image, rebuilt when the image size changes, shared with plf_detect_lines) and never touches the batched pipeline's
  * buffers, so a call between batches in flight is safe. */
+/* img is 8-bit single-channel (grey), as for plf_orb. */
 plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, float* segs, int cap, int* n);
 
 /* Line features of one image.  Replaces stvo-pl StereoFrame::detectLineFeatures (LSD branch):
@@ -277,6 +279,7 @@ plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, f
  * (PLF_ERR_CAPACITY beyond cap, max_segments, max_lines or - when lines are ranked - KL_SORT_CAP).
  * Enqueued on plf_stream in plf_lsd's working state; never touches the batched pipeline's buffers, so a call between
  * batches in flight is safe. */
+/* img is 8-bit single-channel (grey), as for plf_orb. */
 plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride,
                             plf_keyline* keylines, uint8_t* desc, int cap, int* n);
 
@@ -309,6 +312,7 @@ plf_status plf_lbd_gradients(plf_ctx* ctx, const uint8_t* img, int w, int h, int
  * Uses from each KeyLine: sPointInOctave*, ePointInOctave*, numOfPixels, angle (octave 0 only, as the
  * front-end calls it).  desc: n x 32 bytes (host).  desc_float (optional): n x 72 floats.
  * n == 0 returns PLF_OK without touching desc (the reference prints a message and returns). */
+/* img is 8-bit single-channel (grey), as for plf_orb. */
 plf_status plf_lbd(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride,
                    const plf_keyline* keylines, int n, uint8_t* desc, float* desc_float);
 
@@ -733,6 +737,25 @@ plf_status plf_batch_upload(plf_ctx* ctx, int B, const uint8_t* left, const uint
 plf_status plf_batch_run(plf_ctx* ctx, int B);
 plf_status plf_batch_download(plf_ctx* ctx, int B, plf_frame_result* out);
 
+/* The colour form of plf_batch_upload: left/right hold B images each of h rows of `stride` bytes, image k at offset
+ * k*stride*h (host), every row w pixels of `channels` interleaved bytes as in a cv::Mat: 3 = BGR (CV_8UC3), 4 = BGRA
+ * (CV_8UC4).  stride >= channels * w; dense and strided rows are both accepted.  Its place in the upload -> run ->
+ * download protocol is plf_batch_upload's (up to three batches in flight; grey and colour uploads may alternate freely).
+ *   - The run that consumes the upload converts it to grey on the device, byte for byte cv::cvtColor(COLOR_BGR2GRAY) /
+ *     (COLOR_BGRA2GRAY) of OpenCV 4 (alpha is ignored; DESIGN.md section 8), before extraction reads it.  Pairs of a
+ *     rectified sequence (plf_set_sequence_rectification) are remapped first, every channel with its maps, and converted
+ *     after, as stvo-pl's reader remaps the colour image it read and the detectors convert it; the two orders differ.
+ *   - Once the run is issued, plf_batch_device_images holds the grey (and where rectified, remapped) images.  Run each
+ *     upload once, as for grey uploads.  Everything after the conversion is the grey pipeline's.
+ *   - The standalone operators (plf_orb, plf_lsd, plf_detect_lines, plf_lbd) take grey images only.
+ * Device memory: the first colour upload allocates a landing buffer of 2 max_batch h w channels bytes (plus the batch's
+ * pair table), grown once if 4 channels follow 3, kept until plf_destroy: about 2.9 GB at 1242 x 375, max_batch 1024 and
+ * 3 channels (3.8 GB with 4).  A context that never uploads colour allocates nothing for it.
+ * PLF_ERR_INVALID, naming the argument, for channels other than 3 or 4, B outside [1, max_batch], a NULL image or
+ * stride < channels * w, with nothing changed; PLF_ERR_CUDA when the landing buffer cannot be allocated, with the
+ * earlier uploads left as they were. */
+plf_status plf_batch_upload_color(plf_ctx* ctx, int B, const uint8_t* left, const uint8_t* right, int stride, int channels);
+
 /* Number of sequences a context can track at once (default 1), 1 <= n <= 2^20.  Call it before the first plf_batch_* call:
  * PLF_ERR_STATE once the pipeline exists, PLF_ERR_INVALID for n out of range.  Each sequence keeps one carried frame slot
  * on the device (84 * max_keypoints + 156 * max_lines + 8 bytes). */
@@ -785,7 +808,8 @@ plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out);
  *   - plf_batch_run_sequences rectifies the pairs of rectified sequences in the image slot it consumes, in place, before
  *     extraction reads it (plf_batch_device_images then holds the rectified images).  Run each upload once: a second run
  *     of the same slot would rectify it again.  A batch without a pair of a rectified sequence does no rectification work.
- *   - The standalone operators (plf_orb, plf_lsd, plf_detect_lines, plf_lbd) do not rectify.
+ *   - The standalone operators (plf_orb, plf_lsd, plf_detect_lines, plf_lbd) do not rectify, nor take colour.
+ *   - A colour upload (plf_batch_upload_color) of a rectified sequence is remapped per channel, then converted to grey.
  * Device memory: 12 w h bytes per rectified sequence (4.3 MB at 752 x 480, 5.6 MB at 1242 x 375), allocated when its maps
  * are first set and freed when they are cleared, by plf_set_max_sequences or by plf_destroy.  The first run with a
  * rectified pair also allocates a scratch of 2 max_batch h pitch bytes (plus its pair table) kept until plf_destroy.
@@ -852,7 +876,7 @@ plf_status plf_batch_device_poses(plf_ctx* ctx, int B, double* dst_device, void*
 /* Device buffer [2*max_batch][h][pitch] read by plf_batch_run (image 2k = left k, 2k+1 = right k), pitch = width rounded up
  * to a multiple of 16 bytes (every halo tile of every image is then a legal TMA box).  It is the slot of the most recent
  * upload; once that upload has been run, the pairs of rectified sequences (plf_set_sequence_rectification) in it are the
- * rectified images. */
+ * rectified images, and a colour upload (plf_batch_upload_color) is its grey conversion. */
 void* plf_batch_device_images(plf_ctx* ctx);
 
 /* Stereo-valid features of frame k of the last batch (what `new KeyFrame(StVO->curr_frame)` deep-copies,

@@ -25,9 +25,11 @@
 
 namespace plf {
 
-struct Image {  // view of an 8-bit single-channel image (cv::Mat CV_8UC1: data, cols, rows, step)
+struct Image {  // view of an 8-bit image of 1 (grey), 3 (BGR) or 4 (BGRA) interleaved channels (cv::Mat CV_8UC1 / 3 / 4:
+                // data, cols, rows, step, channels())
   const uint8_t* data = nullptr;
   int cols = 0, rows = 0, step = 0;
+  int channels = 1;
 };
 
 // Fixed-size f64 matrix / vector with the Eigen accessors pl-slam uses on stvo-pl's types: (r, c), (i), [i], Identity(),
@@ -173,12 +175,17 @@ using plf::expmap_se3;
 using plf::inverse_se3;
 using plf::logmap_se3;
 // The image type of StereoFrame::img_l / img_r and of initialize / insertStereoPair: cv::Mat in a build that has OpenCV
-// (define STVO_SHIM_WITH_OPENCV after including <opencv2/core.hpp>; the shim reads data / cols / rows / step only),
-// the plf::Image view otherwise.
+// (define STVO_SHIM_WITH_OPENCV after including <opencv2/core.hpp>; the shim reads data / cols / rows / step / channels()
+// / depth() only), the plf::Image view otherwise.  Grey, BGR and BGRA frames are accepted; colour ones are converted to
+// grey on the device, as stvo-pl's detectors convert them, and StereoFrame keeps the caller's colour view.
 #ifdef STVO_SHIM_WITH_OPENCV
 typedef cv::Mat Image;
+inline int image_channels(const cv::Mat& m) { return m.channels(); }
+inline bool image_8bit(const cv::Mat& m) { return m.depth() == CV_8U; }
 #else
 typedef plf::Image Image;
+inline int image_channels(const plf::Image& m) { return m.channels; }
+inline bool image_8bit(const plf::Image&) { return true; }
 #endif
 
 // stvo-pl PinholeStereoCamera (uses: app/plslam_dataset.cpp:84,97; src/mapHandler.cpp:255,551,1384-1385,3344)
@@ -426,7 +433,16 @@ class StereoFrameHandler {
   StereoFrame* run_frame(const Image& l, const Image& r, int idx) {
     if (l.cols != cam->getWidth() || l.rows != cam->getHeight() || r.cols != l.cols || r.rows != l.rows || (size_t)l.step != (size_t)r.step)
       throw std::runtime_error("[StereoFrameHandler] image size does not match the camera");
-    check(plf_process_batch(ctx_, 1, l.data, r.data, (int)(size_t)l.step, &last_));
+    const int ch = image_channels(l);
+    if (!image_8bit(l) || !image_8bit(r) || image_channels(r) != ch || (ch != 1 && ch != 3 && ch != 4))
+      throw std::runtime_error("[StereoFrameHandler] images must be 8-bit grey, BGR or BGRA, both alike");
+    if (ch == 1) {
+      check(plf_process_batch(ctx_, 1, l.data, r.data, (int)(size_t)l.step, &last_));
+    } else {
+      check(plf_batch_upload_color(ctx_, 1, l.data, r.data, (int)(size_t)l.step, ch));
+      check(plf_batch_run(ctx_, 1));
+      check(plf_batch_download(ctx_, 1, &last_));
+    }
     auto* f = new StereoFrame(l, r, idx, cam);
     const int K = lim_.max_keypoints, Ln = lim_.max_lines;
     std::vector<double> pl(2 * (size_t)K), disp(K), P(3 * (size_t)K), spl(2 * (size_t)Ln), epl(2 * (size_t)Ln), sd(Ln), ed(Ln),

@@ -763,6 +763,13 @@ int main(int argc, char** argv) {
     bow_voc[1] = argv[argc - 1];
     argc -= 3;
   }
+  // --color C (last): frames.bin holds colour images, C = 3 (BGR) or 4 (BGRA) interleaved bytes per pixel, which the shim
+  // uploads as they are and the device converts to grey
+  int channels = 1;
+  if (argc >= 3 && std::string(argv[argc - 2]) == "--color") {
+    channels = std::atoi(argv[argc - 1]);
+    argc -= 2;
+  }
   // --motion-model (last): stvo-pl's use_motion_model; prints "motion k valid T[16]", the prediction frame k started from,
   // after each frame's line
   bool motion_on = false;
@@ -780,7 +787,7 @@ int main(int argc, char** argv) {
   if (argc >= 2 && std::string(argv[argc - 1]) == "--grid-selftest") { grid_test = true; --argc; }
   if (argc >= 2 && std::string(argv[argc - 1]) == "--kf-match-selftest") { kf_test = true; --argc; }
   if (argc < 2) {
-    std::fprintf(stderr, "usage: %s frames.bin [orb_nfeatures lsd_nfeatures]\n", argv[0]);
+    std::fprintf(stderr, "usage: %s frames.bin [orb_nfeatures lsd_nfeatures] [--color 3|4]\n", argv[0]);
     return 1;
   }
   FILE* f = std::fopen(argv[1], "rb");
@@ -789,7 +796,7 @@ int main(int argc, char** argv) {
   double cam[5];
   if (std::fread(hdr, 4, 3, f) != 3 || std::fread(cam, 8, 5, f) != 5) { std::fprintf(stderr, "bad header\n"); return 1; }
   const int n = hdr[0], w = hdr[1], h = hdr[2];
-  std::vector<uint8_t> buf((size_t)2 * w * h);
+  std::vector<uint8_t> buf((size_t)2 * w * h * channels);
   try {
     StVO::PinholeStereoCamera cam_pin(w, h, cam[0], cam[1], cam[2], cam[3], cam[4]);
     plf_params prm;
@@ -806,7 +813,7 @@ int main(int argc, char** argv) {
     int rc = 0;
     for (int frame_counter = 0; frame_counter < n; ++frame_counter) {                   // app:111
       if (std::fread(buf.data(), 1, buf.size(), f) != buf.size()) { std::fprintf(stderr, "short read\n"); return 1; }
-      plf::Image img_l{buf.data(), w, h, w}, img_r{buf.data() + (size_t)w * h, w, h, w};
+      plf::Image img_l{buf.data(), w, h, w * channels, channels}, img_r{buf.data() + (size_t)w * h * channels, w, h, w * channels, channels};
       bool new_kf = false;
       StVO::StereoFrame* cur;
       const int fast_th = StVO_->orbFastTh();

@@ -75,6 +75,9 @@ struct PipeState {
   uint8_t* imgs2[2] = {nullptr, nullptr};  // double-buffered [2B][h][pitch]: upload of batch i+1 overlaps the run of batch i
   uint8_t* stage = nullptr;    // dense [2B][h][w] landing buffer of the H2D copy (one contiguous DMA per side), repacked to the padded pitch on the device
   int up_slot = 0;             // slot written by the last plf_batch_upload
+  // channels of the last upload: 1 for plf_batch_upload (its images are in imgs2[up_slot]), 3 or 4 for
+  // plf_batch_upload_color (its images are in the colour landing buffer until the run converts them into imgs2[up_slot])
+  int up_ch = 1;
   cudaStream_t copy = nullptr; // H2D stream
   cudaEvent_t ev_up[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr}, ev_free2[2] = {nullptr, nullptr};
   OrbState* orb = nullptr;     // ORB of 2B images, outputs per batch parity
@@ -857,10 +860,22 @@ static plf_status send_tab(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   return PLF_OK;
 }
 
-// cv::remap(src, dst, map1, map2, INTER_LINEAR, BORDER_CONSTANT, 0) of one image of a rectified pair: grid.z = 2 j + side
-// for entry j of tab.  map2 & 1023 = 32 fy + fx selects OpenCV's weights 32 (32 - fx) (32 - fy), 32 fx (32 - fy),
-// 32 (32 - fx) fy and 32 fx fy of the taps (x, y), (x+1, y), (x, y+1), (x+1, y+1) (exact: no rounding excess to move),
-// so (sum w p + 2^14) >> 15 is (sum (w / 32) p + 2^9) >> 10.  Taps outside the image read 0.
+// cv::remap(src, dst, map1, map2, INTER_LINEAR, BORDER_CONSTANT, 0) at one output pixel of one channel: map1 = (sx, sy),
+// map2 & 1023 = 32 fy + fx selects OpenCV's weights 32 (32 - fx) (32 - fy), 32 fx (32 - fy), 32 (32 - fx) fy and 32 fx fy of
+// the taps (x, y), (x+1, y), (x, y+1), (x+1, y+1) (exact: no rounding excess to move), so (sum w p + 2^14) >> 15 is
+// (sum (w / 32) p + 2^9) >> 10.  src points at the channel's byte of pixel (0, 0) of a w x h image of `row` bytes per row
+// and `px` bytes per pixel (cv::remap of a multi-channel image is this per channel).  Taps outside the image read 0.
+__device__ __forceinline__ int remap_px(const uint8_t* __restrict__ src, int row, int px, int w, int h, int sx, int sy, int fx,
+                                        int fy) {
+  auto tap = [&](int u, int v) -> int {
+    return (unsigned)u < (unsigned)w && (unsigned)v < (unsigned)h ? __ldg(src + (size_t)v * row + u * px) : 0;
+  };
+  const int acc = (32 - fx) * (32 - fy) * tap(sx, sy) + fx * (32 - fy) * tap(sx + 1, sy) + (32 - fx) * fy * tap(sx, sy + 1) +
+                  fx * fy * tap(sx + 1, sy + 1);
+  return (acc + 512) >> 10;
+}
+
+// cv::remap of one image of a rectified pair: grid.z = 2 j + side for entry j of tab.
 __global__ void __launch_bounds__(256) k_rectify(const PlfRectPair* __restrict__ tab, const uint8_t* __restrict__ imgs, size_t AP,
                                                  int pitch, int w, int h, uint8_t* __restrict__ out) {
   const int x = blockIdx.x * 32 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y;
@@ -871,13 +886,33 @@ __global__ void __launch_bounds__(256) k_rectify(const PlfRectPair* __restrict__
   const short2 m = PLF_RECT_MAP1(e.maps, A, side)[i];
   const int f = PLF_RECT_MAP2(e.maps, A, side)[i] & 1023, fx = f & 31, fy = f >> 5;
   const uint8_t* src = imgs + (size_t)(2 * e.pair + side) * AP;
-  auto tap = [&](int u, int v) -> int {
-    return (unsigned)u < (unsigned)w && (unsigned)v < (unsigned)h ? __ldg(src + (size_t)v * pitch + u) : 0;
-  };
-  const int sx = m.x, sy = m.y;
-  const int acc = (32 - fx) * (32 - fy) * tap(sx, sy) + fx * (32 - fy) * tap(sx + 1, sy) + (32 - fx) * fy * tap(sx, sy + 1) +
-                  fx * fy * tap(sx + 1, sy + 1);
-  out[(size_t)blockIdx.z * AP + (size_t)y * pitch + x] = (uint8_t)((acc + 512) >> 10);
+  out[(size_t)blockIdx.z * AP + (size_t)y * pitch + x] = (uint8_t)remap_px(src, pitch, 1, w, h, m.x, m.y, fx, fy);
+}
+
+// cv::cvtColor(COLOR_BGR2GRAY) of 8-bit B, G, R as OpenCV 4 computes it (15-bit fixed point; COLOR_BGRA2GRAY ignores alpha)
+__device__ __forceinline__ int bgr_gray(int b, int g, int r) { return (3735 * b + 19235 * g + 9798 * r + (1 << 14)) >> 15; }
+
+// The grey images of a colour batch (plf_batch_upload_color): grid.z = image 2k + side.  src: the landing buffer, [2B][h][w]
+// pixels of ch = 3 (BGR) or 4 (BGRA) interleaved bytes, laid out like imgs.  Pair k of a rectified sequence (tab[k].maps
+// set; tab NULL: no pair is) is remapped per channel with its maps first and converted after, as stvo-pl's reader remaps
+// the colour image it read and the detectors convert it; every other pair is converted as it is.
+__global__ void __launch_bounds__(256) k_color(const PlfRectPair* __restrict__ tab, const uint8_t* __restrict__ src, int ch, int w,
+                                               int h, size_t AP, int pitch, uint8_t* __restrict__ out) {
+  const int x = blockIdx.x * 32 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y;
+  if (x >= w || y >= h) return;
+  const int side = blockIdx.z & 1;
+  const size_t A = (size_t)w * h, i = (size_t)y * w + x;
+  const uint8_t* img = src + (size_t)blockIdx.z * A * ch;
+  const uint8_t* maps = tab ? tab[blockIdx.z >> 1].maps : nullptr;
+  int v[3];
+  if (maps) {
+    const short2 m = PLF_RECT_MAP1(maps, A, side)[i];
+    const int f = PLF_RECT_MAP2(maps, A, side)[i] & 1023, fx = f & 31, fy = f >> 5;
+    for (int c = 0; c < 3; ++c) v[c] = remap_px(img + c, w * ch, ch, w, h, m.x, m.y, fx, fy);
+  } else {
+    for (int c = 0; c < 3; ++c) v[c] = __ldg(img + i * ch + c);
+  }
+  out[(size_t)blockIdx.z * AP + (size_t)y * pitch + x] = (uint8_t)bgr_gray(v[0], v[1], v[2]);
 }
 
 // Rectifies the pairs of the batch whose sequence has maps in the slot the run consumes, before any stream of the run
@@ -912,6 +947,63 @@ static plf_status run_rectify(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     PLF_CUDA(ctx, cudaMemcpy2DAsync(imgs + 2 * (size_t)ht[j0].pair * AP, (size_t)s->pitch, pairs + 2 * (size_t)j0 * AP, (size_t)s->pitch,
                                     (size_t)s->w, 2 * (size_t)(j1 - j0) * s->h, cudaMemcpyDeviceToDevice, cs));
   }
+  PLF_CUDA(ctx, cudaEventRecord(s->ev_up[r.run_slot], cs));
+  return PLF_OK;
+}
+
+// The pair table and the colour landing buffer of ch channels, [2 max_batch][h][w][ch] (image 2k = left k, 2k+1 = right
+// k), carved from PLF_SCR_COLOR_PIPE.  Only the copy stream touches them: the uploads land there and the runs' conversions
+// read them in call order, so one buffer serves every batch in flight.  To grow (the first colour upload, or 4 channels
+// after 3) the block waits for the copy stream, and the new block is allocated before the old one is freed: a failed
+// allocation leaves the last upload as it was.
+static plf_status color_scratch(plf_ctx* ctx, PipeState* s, int ch, PlfRectPair** tab, uint8_t** land) {
+  DevBufList b;
+  b.add(*tab, s->B);
+  b.add(*land, 2 * (size_t)s->B * s->h * s->w * ch);
+  size_t need = 0;
+  for (const DevBufList::Entry& e : b.entries) need += plf_align256(e.bytes);
+  DevBuf& slot = ctx->scratch[PLF_SCR_COLOR_PIPE];
+  if (slot.bytes < need) {
+    PLF_CUDA(ctx, cudaStreamSynchronize(s->copy));
+    void* p = nullptr;
+    const cudaError_t e = cudaMalloc(&p, need + 64);   // + the slack plf_scratch gives every slot
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      return plf_fail(ctx, PLF_ERR_CUDA, "plf_batch_upload_color: cudaMalloc(%zu) of the colour landing buffer: %s", need,
+                      cudaGetErrorString(e));
+    }
+    cudaFree(slot.p);
+    slot.p = p;
+    slot.bytes = need;
+  }
+  return b.carve(ctx, PLF_SCR_COLOR_PIPE);
+}
+
+// Converts the colour batch the run consumes (plf_batch_upload_color) into its grey image slot, before any stream of the
+// run reads it: on the copy stream, behind the upload, once the runs that read the slot before have finished with it;
+// ev_up[run_slot] is recorded again for the E and P phases.  Pairs of rectified sequences are remapped in the same pass, so
+// run_rectify has nothing to do for a colour batch.
+static plf_status run_color(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
+  PlfRectPair* ht = s->h_rect[r.rp];
+  bool rect = false;
+  for (int k = 0; k < r.B; ++k) {
+    const uint8_t* maps = ctx->seqs.empty() ? nullptr : ctx->seqs[s->pair_seq[k]].rect;
+    ht[k] = PlfRectPair{maps, k, 0};
+    rect |= maps != nullptr;
+  }
+  PlfRectPair* tab;
+  uint8_t* land;
+  if (plf_status st = color_scratch(ctx, s, s->up_ch, &tab, &land)) return st;
+  cudaStream_t cs = s->copy;
+  PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_free[r.run_slot], 0));
+  PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_free2[r.run_slot], 0));
+  if (rect) PLF_CUDA(ctx, cudaMemcpyAsync(tab, ht, sizeof(PlfRectPair) * r.B, cudaMemcpyHostToDevice, cs));
+  plf_mark(ctx, cs, "color.start");
+  k_color<<<dim3((s->w + 31) / 32, (s->h + 7) / 8, 2 * r.B), dim3(32, 8), 0, cs>>>(rect ? tab : nullptr, land, s->up_ch, s->w, s->h,
+                                                                                    (size_t)s->pitch * s->h, s->pitch,
+                                                                                    s->imgs2[r.run_slot]);
+  PLF_LAUNCH_CHECK(ctx);
+  plf_mark(ctx, cs, "color.k_color");
   PLF_CUDA(ctx, cudaEventRecord(s->ev_up[r.run_slot], cs));
   return PLF_OK;
 }
@@ -1367,6 +1459,48 @@ plf_status plf_batch_upload(plf_ctx* ctx, int B, const uint8_t* left, const uint
   }
   PLF_CUDA(ctx, cudaEventRecord(s->ev_up[slot], s->copy));
   s->up_slot = slot;
+  s->up_ch = 1;
+  return PLF_OK;
+}
+
+plf_status plf_batch_upload_color(plf_ctx* ctx, int B, const uint8_t* left, const uint8_t* right, int stride, int channels) {
+  if (!ctx) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_batch_upload_color: ctx is NULL");
+  const int w = ctx->cam.width, h = ctx->cam.height;
+  if (channels != 3 && channels != 4)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload_color: channels = %d, need 3 (BGR) or 4 (BGRA)", channels);
+  if (B < 1 || B > ctx->limits.max_batch)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload_color: B = %d, need 1 <= B <= max_batch = %d", B, ctx->limits.max_batch);
+  if (!left || !right) return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload_color: left and right are required");
+  if ((long long)stride < (long long)channels * w)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload_color: stride = %d, need at least channels * width = %d", stride,
+                    channels * w);
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  plf_status st = pipe_prepare(ctx);
+  if (st) return st;
+  PipeState* s = ctx->pipe;
+  PlfRectPair* tab;
+  uint8_t* land;
+  if ((st = color_scratch(ctx, s, channels, &tab, &land))) return st;
+  // H2D on the copy stream into the landing buffer; the run converts it into the image slot the GPU is not reading.
+  // Dense rows of ch w bytes are one contiguous block per image, so each side is one copy of B blocks (no short-row DMA
+  // to avoid, unlike the grey path's stage); strided input is one 3-D copy per side (B images of h rows of ch w bytes,
+  // the destination "height" of 2h rows skipping the other side's image of each pair).
+  const size_t row = (size_t)channels * w, AC = row * h;
+  if ((size_t)stride == row) {
+    PLF_CUDA(ctx, cudaMemcpy2DAsync(land, 2 * AC, left, AC, AC, B, cudaMemcpyHostToDevice, s->copy));
+    PLF_CUDA(ctx, cudaMemcpy2DAsync(land + AC, 2 * AC, right, AC, AC, B, cudaMemcpyHostToDevice, s->copy));
+  } else {
+    for (int side = 0; side < 2; ++side) {
+      cudaMemcpy3DParms cp = {};
+      cp.srcPtr = make_cudaPitchedPtr(const_cast<uint8_t*>(side ? right : left), (size_t)stride, row, (size_t)h);
+      cp.dstPtr = make_cudaPitchedPtr(land + (size_t)side * AC, row, row, 2 * (size_t)h);
+      cp.extent = make_cudaExtent(row, (size_t)h, (size_t)B);
+      cp.kind = cudaMemcpyHostToDevice;
+      PLF_CUDA(ctx, cudaMemcpy3DAsync(&cp, s->copy));
+    }
+  }
+  s->up_slot ^= 1;
+  s->up_ch = channels;
   return PLF_OK;
 }
 
@@ -1447,7 +1581,7 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   r.sP = (r.piped && r.lsd2) ? ctx->aux[2] : r.sG;   // LSD pre-grow chain: own stream when its outputs exist per parity
   r.afast = ctx->afast_on;
   r.motion = ctx->motion_on;
-  st = run_rectify(ctx, s, r);
+  st = s->up_ch > 1 ? run_color(ctx, s, r) : run_rectify(ctx, s, r);
   if (!st && r.afast) st = send_tab(ctx, s, r);
   if (!st) st = run_extract(ctx, s, r);
   if (!st) st = run_lsd(ctx, s, r);

@@ -40,6 +40,8 @@ enum plf_scratch_slot {
   PLF_SCR_LC,          // plf_loop_closure_pose and plf_loop_closure_pose_batch: their staged layout
   PLF_SCR_RECT_PIPE,   // the rectification of plf_batch_run_sequences (plf_set_sequence_rectification): its pair table
                        // and remapped pairs, sized for max_batch pairs once, so that it never grows under batches in flight
+  PLF_SCR_COLOR_PIPE,  // plf_batch_upload_color and the conversion of plf_batch_run_sequences: the pair table and the
+                       // colour landing buffer of max_batch pairs (color_scratch in pipeline.cu)
   PLF_SCR_COUNT
 };
 

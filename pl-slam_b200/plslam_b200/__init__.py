@@ -1334,18 +1334,28 @@ class Frontend:
         return out
 
     def _stack(self, left, right):
+        """(left, right, channels): grey uint8 [B,H,W] (or [H,W]) with channels 1, or colour uint8 [B,H,W,C] (or
+        [H,W,C]), C = 3 (BGR) or 4 (BGRA), with channels C."""
         left = np.ascontiguousarray(left, np.uint8); right = np.ascontiguousarray(right, np.uint8)
+        hw = (self.camera.height, self.camera.width)
+        if left.ndim == 3 and left.shape[:2] == hw and left.shape[2] in (3, 4) and left.shape[1:] != hw:
+            left, right = left[None], right[None]   # one colour pair
+        if left.ndim == 4:
+            if not (left.shape == right.shape and left.shape[1:3] == hw and left.shape[3] in (3, 4)):
+                raise PlfError(f"colour images must be uint8 [B, {hw[0]}, {hw[1]}, 3 | 4] (BGR or BGRA), left and right "
+                               f"alike (got {list(left.shape)} and {list(right.shape)})")
+            return left, right, left.shape[3]
         if left.ndim == 2:
             left, right = left[None], right[None]
         assert left.shape == right.shape and left.shape[1:] == (self.camera.height, self.camera.width)
-        return left, right
+        return left, right, 1
 
     def process_batch(self, left, right, seq=None, restart=None):
-        """B x (insertStereoPair + optimizePose): left/right uint8 [B,H,W] host arrays -> list of result dicts.  seq /
-        restart: as batch_run."""
-        left, right = self._stack(left, right)
+        """B x (insertStereoPair + optimizePose): left/right uint8 [B,H,W] grey or [B,H,W,3|4] BGR / BGRA host arrays
+        -> list of result dicts.  seq / restart: as batch_run."""
+        left, right, ch = self._stack(left, right)
         B = left.shape[0]
-        if seq is None and restart is None:
+        if seq is None and restart is None and ch == 1:
             res = (plf_frame_result * B)()
             st = self.lib.plf_process_batch(self._ctx, B, _ptr(left, C.c_uint8), _ptr(right, C.c_uint8),
                                             self.camera.width, res)
@@ -1357,15 +1367,28 @@ class Frontend:
         return self.batch_download(B)
 
     def batch_upload(self, left, right):
-        left, right = self._stack(left, right)
-        self._check(self.lib.plf_batch_upload(self._ctx, left.shape[0], _ptr(left, C.c_uint8), _ptr(right, C.c_uint8),
-                                              self.camera.width), "plf_batch_upload")
+        """Uploads grey uint8 [B,H,W] pairs (plf_batch_upload) or BGR / BGRA uint8 [B,H,W,3|4] pairs, which the run
+        converts to grey on the device (plf_batch_upload_color).  Returns B."""
+        left, right, ch = self._stack(left, right)
+        if ch == 1:
+            self._check(self.lib.plf_batch_upload(self._ctx, left.shape[0], _ptr(left, C.c_uint8), _ptr(right, C.c_uint8),
+                                                  self.camera.width), "plf_batch_upload")
+        else:
+            self._check(self.lib.plf_batch_upload_color(self._ctx, left.shape[0], _ptr(left, C.c_uint8),
+                                                        _ptr(right, C.c_uint8), ch * self.camera.width, ch),
+                        "plf_batch_upload_color")
         return left.shape[0]
 
-    def batch_upload_raw(self, B, left_ptr, right_ptr):
-        """Upload from raw host addresses (e.g. pinned memory)."""
-        self._check(self.lib.plf_batch_upload(self._ctx, int(B), C.c_void_p(left_ptr), C.c_void_p(right_ptr),
-                                              self.camera.width), "plf_batch_upload")
+    def batch_upload_raw(self, B, left_ptr, right_ptr, channels=1, stride=None):
+        """Upload from raw host addresses (e.g. pinned memory): B images per side of H rows of `stride` bytes (None:
+        channels * W), grey (channels 1) or BGR / BGRA (3 / 4, plf_batch_upload_color)."""
+        stride = channels * self.camera.width if stride is None else int(stride)
+        if channels == 1:
+            self._check(self.lib.plf_batch_upload(self._ctx, int(B), C.c_void_p(left_ptr), C.c_void_p(right_ptr), stride),
+                        "plf_batch_upload")
+        else:
+            self._check(self.lib.plf_batch_upload_color(self._ctx, int(B), C.c_void_p(left_ptr), C.c_void_p(right_ptr),
+                                                        stride, int(channels)), "plf_batch_upload_color")
 
     @staticmethod
     def _sequence_table(B, seq, restart):
