@@ -15,6 +15,7 @@
 // per-pair kernels.  Pair k's previous frame is the slot prev[k] of the batch's sequence table; the last frame of each
 // sequence in the batch is carried to that sequence's carry slot for the next call.
 #include <cmath>
+#include <cstddef>
 
 #include "plf_internal.h"
 #include "plf_geom.cuh"
@@ -45,8 +46,36 @@ constexpr int PLF_FS_NFIELDS = 0 PLF_PT_FIELDS(PLF_FS_ONE) PLF_LS_FIELDS(PLF_FS_
 // then map2 of the left then the right image (uint16 [2][h][w]).
 #define PLF_RECT_MAP1(base, A, side) (reinterpret_cast<const short2*>(base) + (size_t)(side) * (A))
 #define PLF_RECT_MAP2(base, A, side) (reinterpret_cast<const uint16_t*>((base) + 8 * (A)) + (size_t)(side) * (A))
-// One rectified pair of a batch: its index and its sequence's maps.
+// One pair of a batch's input table: its index and its sequence's maps (NULL: the pair is not rectified).
 struct PlfRectPair { const uint8_t* maps; int pair; int pad; };
+
+// One entry of the batch table ring, for max_batch pairs B: the sequence table (prev[B] = the frame slot of pair k's
+// previous frame, then the carry list [B][2] of (frame slot, carry slot)), the pairs' cameras [B] and the input table
+// [B].  The pinned and the device ring use the same layout.
+struct BatchTab {
+  int32_t* prev;
+  int32_t* carry;
+  PlfPairCam* cams;
+  PlfRectPair* in;
+};
+static size_t batch_tab_bytes(int B) {
+  return plf_align256(3 * sizeof(int32_t) * B) + plf_align256(sizeof(PlfPairCam) * B) + plf_align256(sizeof(PlfRectPair) * B);
+}
+static BatchTab batch_tab(uint8_t* base, int B) {
+  uint8_t* cams = base + plf_align256(3 * sizeof(int32_t) * B);
+  uint8_t* in = cams + plf_align256(sizeof(PlfPairCam) * B);
+  return {reinterpret_cast<int32_t*>(base), reinterpret_cast<int32_t*>(base) + B, reinterpret_cast<PlfPairCam*>(cams),
+          reinterpret_cast<PlfRectPair*>(in)};
+}
+
+// What each sequence carries to its next pair besides its frame slot: the pose prediction (row-major 4x4) and whether it
+// came from a good solution (plf_set_motion_model), and the FAST threshold (plf_set_adaptive_fast).  Only the fields of
+// the features that are on are kept up to date.
+struct SeqRecord {
+  double T[16];
+  int valid;
+  int th;
+};
 
 struct PipeState {
   int w = 0, h = 0, B = 0, max_kp = 0, max_ln = 0;
@@ -57,21 +86,13 @@ struct PipeState {
   std::vector<uint8_t> carried;  // [nseq] sequence s has a frame in its carry slot
   std::vector<int> last_pair;    // [nseq] scratch of plf_batch_run_sequences: the batch's last pair of each sequence, or -1
   std::vector<int> pair_seq;     // [B] scratch of plf_batch_run_sequences: the sequence of each pair of the batch
-  // The sequence table of a batch: prev[max_batch] (slot of pair k's previous frame), then the carry list [max_batch][2]
-  // (frame slot, carry slot).  Rings indexed like h_results (up to three batches in flight): pinned h_tab, device seq_tab
-  // [3][3 max_batch].  The copy goes on the copy stream, in order behind the batch's own images and ahead of the next
-  // batch's upload; ev_tab marks it for the M phase.
-  int32_t* h_tab[3] = {nullptr, nullptr, nullptr};
-  int32_t* seq_tab = nullptr;
+  // The batch tables (BatchTab), rings indexed like h_results (up to three batches in flight): one pinned block h_tab[rp]
+  // per entry, device tab [3][batch_tab_bytes].  The copy goes on the copy stream at the start of the run, in order behind
+  // the batch's own images, ahead of its input conversion and of the next batch's upload; ev_tab marks it for the E and M
+  // phases.
+  uint8_t* h_tab[3] = {nullptr, nullptr, nullptr};
+  uint8_t* tab = nullptr;
   cudaEvent_t ev_tab[3] = {nullptr, nullptr, nullptr};
-  // The camera of each pair (plf_set_sequence_camera), beside prev[k]: rings h_cam / cam_tab [3][max_batch] like h_tab and
-  // seq_tab, copied with the table behind ev_tab.  Only a batch holding a sequence with its own camera fills them; the
-  // others pass no table and the kernels take the context's camera.
-  PlfPairCam* h_cam[3] = {nullptr, nullptr, nullptr};
-  PlfPairCam* cam_tab = nullptr;
-  // The pairs to rectify (plf_set_sequence_rectification): pinned ring h_rect [3][max_batch] like h_tab; the device copy
-  // lives in scratch slot PLF_SCR_RECT_PIPE, written and read on the copy stream only.
-  PlfRectPair* h_rect[3] = {nullptr, nullptr, nullptr};
   uint8_t* imgs2[2] = {nullptr, nullptr};  // double-buffered [2B][h][pitch]: upload of batch i+1 overlaps the run of batch i
   uint8_t* stage = nullptr;    // dense [2B][h][w] landing buffer of the H2D copy (one contiguous DMA per side), repacked to the padded pitch on the device
   int up_slot = 0;             // slot written by the last plf_batch_upload
@@ -86,17 +107,13 @@ struct PipeState {
   short2* lbd_grad[2] = {nullptr, nullptr};  // [parity][2B][h*w]
   uint8_t* ldesc_raw = nullptr;  // [2B][max_ln][32]  LBD of every kept KeyLine
   FrameSlots fs;               // B + nseq + 1 slots
-  // plf_set_adaptive_fast: seq_th[s] = the FAST threshold of sequence s's next pair unless that pair is a first frame
-  // (written by k_fast_th_update, behind ev_th on the M stream); img_th = the threshold of each image of the running batch
-  int* seq_th = nullptr;       // [nseq]
+  // seq_rec[s]: what sequence s's next pair starts from unless that pair is a first frame, written by k_seq_update on the
+  // M stream (ev_th marks the thresholds for the next E phase).  img_th = the FAST threshold of each image of the running
+  // batch (plf_set_adaptive_fast); pair_T = the prediction of each pair of the running batch (plf_set_motion_model), read
+  // by the f2f geometry and, through gn_probs_mm (the pose problems with T_init = pair_T + 16 k), by the pose solver
+  SeqRecord* seq_rec = nullptr;   // [nseq]
   int* img_th = nullptr;       // [2B]
   cudaEvent_t ev_th = nullptr;
-  // plf_set_motion_model: seq_T[s] (row-major 4x4) = the pose prediction of sequence s's next pair unless that pair is a
-  // first frame, seq_valid[s] = 1 where it came from a good solution (both written by k_motion_update on the M stream);
-  // pair_T = the prediction of each pair of the running batch, read by the f2f geometry and, through gn_probs_mm (the
-  // pose problems with T_init = pair_T + 16 k), by the pose solver
-  double* seq_T = nullptr;     // [nseq][16]
-  int* seq_valid = nullptr;    // [nseq]
   double* pair_T = nullptr;    // [B][16]
   GnProblem* gn_probs_mm = nullptr;   // [B]
   // matching scratch
@@ -158,10 +175,8 @@ static void pipe_buffers(PipeState* s, bool windowed, DevBufList& b) {
   PLF_PT_FIELDS(PLF_FS_ALLOC) b.add(f.pt_count, S);
   PLF_LS_FIELDS(PLF_FS_ALLOC) b.add(f.ls_count, S);
 #undef PLF_FS_ALLOC
-  b.add(s->seq_th, s->nseq);
+  b.add(s->seq_rec, s->nseq);
   b.add(s->img_th, 2 * B);
-  b.add(s->seq_T, (size_t)s->nseq * 16);
-  b.add(s->seq_valid, s->nseq);
   b.add(s->pair_T, B * 16);
   b.add(s->gn_probs_mm, B);
   b.add(s->knn_keys, B * 8 * 2 * K);
@@ -176,8 +191,7 @@ static void pipe_buffers(PipeState* s, bool windowed, DevBufList& b) {
   b.add(s->gn_sP, B * Ln * 3); b.add(s->gn_eP, B * Ln * 3); b.add(s->gn_le, B * Ln * 3); b.add(s->gnInlL, B * Ln); b.add(s->gnNl, B);
   b.add(s->gn_probs, B); b.add(s->gn_out, B); b.add(s->results, 3 * B);
   b.add(s->d_ovf, 6);
-  b.add(s->seq_tab, 3 * 3 * B);
-  b.add(s->cam_tab, 3 * B);
+  b.add(s->tab, 3 * batch_tab_bytes(s->B));
   if (windowed) {
     for (int kind = 0; kind < 4; ++kind) {   // points: 2 cells per feature, lines: 2 end points
       b.add(s->mg_q[kind], B * (kind & 1 ? Ln * 4 : K * 2));
@@ -211,8 +225,6 @@ extern "C" void plf_pipe_free(plf_ctx* ctx) {
     if (s->h_results[i]) cudaFreeHost(s->h_results[i]);
     if (s->h_ovf[i]) cudaFreeHost(s->h_ovf[i]);
     if (s->h_tab[i]) cudaFreeHost(s->h_tab[i]);
-    if (s->h_cam[i]) cudaFreeHost(s->h_cam[i]);
-    if (s->h_rect[i]) cudaFreeHost(s->h_rect[i]);
   }
   for (const PipeEvents& a : pipe_events(s))
     for (int i = 0; i < a.n; ++i)
@@ -535,16 +547,17 @@ __global__ void k_finalize(const plf_pose_result* __restrict__ gn, const int* __
   out[k] = r;
 }
 
-// ---- adaptative_fast (plf_set_adaptive_fast, DESIGN.md §8).  A batch holds at most one pair of each sequence, so prev[k]
-// is the empty slot (a first frame) or pair k's carry slot carry0 + s, and every pair is in the carry list. ----
+// ---- what each sequence carries to its next pair: adaptative_fast (plf_set_adaptive_fast) and use_motion_model
+// (plf_set_motion_model), DESIGN.md §8.  With either on a batch holds at most one pair of each sequence, so prev[k] is the
+// empty slot (a first frame) or pair k's carry slot carry0 + s, and every pair is in the carry list. ----
 
 // The FAST threshold of both images of pair k: its sequence's, or th0 = orb_fast_th for a first frame.
 __global__ void k_fast_th_images(const int* __restrict__ prev, int B, int carry0, int empty, int th0,
-                                 const int* __restrict__ seq_th, int* __restrict__ img_th) {
+                                 const SeqRecord* __restrict__ rec, int* __restrict__ img_th) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= B) return;
   const int p = prev[k];
-  const int th = p == empty ? th0 : seq_th[p - carry0];
+  const int th = p == empty ? th0 : rec[p - carry0].th;
   img_th[2 * k] = th;
   img_th[2 * k + 1] = th;
 }
@@ -562,29 +575,8 @@ __device__ __forceinline__ int fast_th_next(int th, const plf_frame_result& r, c
   return th;
 }
 
-// Carry entry j = (pair k, carry slot carry0 + s): sequence s's next threshold from pair k's result.
-__global__ void k_fast_th_update(const plf_frame_result* __restrict__ res, const int* __restrict__ carry, int ncarry, int carry0,
-                                 const int* __restrict__ img_th, plf_adaptive_fast a, int* __restrict__ seq_th) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= ncarry) return;
-  const int k = carry[2 * j];
-  seq_th[carry[2 * j + 1] - carry0] = fast_th_next(img_th[2 * k], res[k], a);
-}
-
 // orb_fast_th as k_fast_nms applies it without a per-image threshold
 static int fast_th0(const plf_ctx* ctx) { return std::min(std::max(ctx->params.orb_fast_th, 0), 255); }
-
-// Every sequence's threshold back to orb_fast_th (no batch in flight).
-static plf_status pipe_fast_th_reset(plf_ctx* ctx) {
-  PipeState* s = ctx->pipe;
-  const std::vector<int> v(s->nseq, fast_th0(ctx));
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->seq_th, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return PLF_OK;
-}
-
-// ---- use_motion_model (plf_set_motion_model, DESIGN.md §8).  As with adaptive FAST thresholds a batch holds at most one
-// pair of each sequence, so prev[k] is the empty slot or pair k's carry slot carry0 + s. ----
 
 // stvo-pl's isGoodSolution on a pair's result, each of its tests a rejection: so a NaN err or eigenvalue passes.  A
 // covariance with a non-finite entry has NaN eigenvalues (the library's definition; the solver gives such a covariance
@@ -616,21 +608,24 @@ __device__ __forceinline__ int motion_prior(int status, const double* DT, const 
   return good ? 1 : 0;
 }
 
-// Carry entry j = (pair k, carry slot carry0 + s): sequence s's next prediction from pair k's result.
-__global__ void k_motion_update(const plf_frame_result* __restrict__ res, const int* __restrict__ carry, int ncarry, int carry0,
-                                double* __restrict__ seq_T, int* __restrict__ seq_valid) {
+// Carry entry j = (pair k, carry slot carry0 + s): sequence s's record from pair k's result, its next threshold (img_th
+// set: adaptive FAST, from the threshold pair k was detected at) and its next prediction (motion set).
+__global__ void k_seq_update(const plf_frame_result* __restrict__ res, const int* __restrict__ carry, int ncarry, int carry0,
+                             const int* __restrict__ img_th, plf_adaptive_fast a, int motion, SeqRecord* __restrict__ rec) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= ncarry) return;
-  const plf_frame_result& r = res[carry[2 * j]];
-  const int s = carry[2 * j + 1] - carry0;
-  seq_valid[s] = motion_prior(r.status, r.DT, r.DT_cov, r.err, seq_T + 16 * (size_t)s);
+  const int k = carry[2 * j];
+  const plf_frame_result& r = res[k];
+  SeqRecord& q = rec[carry[2 * j + 1] - carry0];
+  if (img_th) q.th = fast_th_next(img_th[2 * k], r, a);
+  if (motion) q.valid = motion_prior(r.status, r.DT, r.DT_cov, r.err, q.T);
 }
 
 // Block k, thread i: entry i of pair k's prediction, its sequence's or the identity for a first frame.
-__global__ void k_motion_pairs(const int* __restrict__ prev, int carry0, int empty, const double* __restrict__ seq_T,
+__global__ void k_motion_pairs(const int* __restrict__ prev, int carry0, int empty, const SeqRecord* __restrict__ rec,
                                double* __restrict__ pair_T) {
   const int k = blockIdx.x, i = threadIdx.x, p = prev[k];
-  pair_T[16 * k + i] = p == empty ? ((i % 5 == 0) ? 1.0 : 0.0) : seq_T[16 * (size_t)(p - carry0) + i];
+  pair_T[16 * k + i] = p == empty ? ((i % 5 == 0) ? 1.0 : 0.0) : rec[p - carry0].T[i];
 }
 
 // plf_debug_motion_prior: the rule on n caller results.
@@ -641,13 +636,28 @@ __global__ void k_motion_debug(int n, const double* __restrict__ DT, const doubl
   valid[j] = motion_prior(status[j], DT + 16 * (size_t)j, cov + 36 * (size_t)j, err[j], T + 16 * (size_t)j);
 }
 
-// Every sequence's prediction back to the identity (no batch in flight).
-static plf_status pipe_motion_reset(plf_ctx* ctx) {
+// Every sequence's record back to a first frame's, in the fields of the features named (no batch in flight): the
+// threshold to orb_fast_th, the prediction to the identity (not valid).  The fields T, valid, th are contiguous, so the
+// named ones are one column range of the record array.
+static plf_status pipe_seq_reset(plf_ctx* ctx, bool fast_th, bool motion) {
   PipeState* s = ctx->pipe;
-  std::vector<double> T((size_t)s->nseq * 16, 0.0);
-  for (size_t i = 0; i < T.size(); i += 16) T[i] = T[i + 5] = T[i + 10] = T[i + 15] = 1.0;
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->seq_T, T.data(), T.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-  PLF_CUDA(ctx, cudaMemsetAsync(s->seq_valid, 0, s->nseq * sizeof(int), ctx->stream));
+  SeqRecord r = {};
+  for (int i = 0; i < 16; i += 5) r.T[i] = 1.0;
+  r.th = fast_th0(ctx);
+  const std::vector<SeqRecord> v(s->nseq, r);
+  const size_t lo = motion ? 0 : offsetof(SeqRecord, th), hi = fast_th ? sizeof(SeqRecord) : offsetof(SeqRecord, th);
+  if (lo >= hi) return PLF_OK;
+  PLF_CUDA(ctx, cudaMemcpy2DAsync(reinterpret_cast<uint8_t*>(s->seq_rec) + lo, sizeof(SeqRecord),
+                                  reinterpret_cast<const uint8_t*>(v.data()) + lo, sizeof(SeqRecord), hi - lo, v.size(),
+                                  cudaMemcpyHostToDevice, ctx->stream));
+  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return PLF_OK;
+}
+
+// Sequence s's record, behind the updates of every batch in flight (M stream).
+static plf_status pipe_seq_read(plf_ctx* ctx, int s, SeqRecord* out) {
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  PLF_CUDA(ctx, cudaMemcpyAsync(out, ctx->pipe->seq_rec + s, sizeof(SeqRecord), cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return PLF_OK;
 }
@@ -773,9 +783,7 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
   for (int i = 0; i < 3; ++i) {
     PLF_CUDA(ctx, cudaHostAlloc(&s->h_results[i], sizeof(plf_frame_result) * B, cudaHostAllocDefault));
     PLF_CUDA(ctx, cudaHostAlloc(&s->h_ovf[i], 2 * sizeof(int), cudaHostAllocDefault));
-    PLF_CUDA(ctx, cudaHostAlloc(&s->h_tab[i], 3 * sizeof(int32_t) * B, cudaHostAllocDefault));
-    PLF_CUDA(ctx, cudaHostAlloc(&s->h_cam[i], sizeof(PlfPairCam) * B, cudaHostAllocDefault));
-    PLF_CUDA(ctx, cudaHostAlloc(&s->h_rect[i], sizeof(PlfRectPair) * B, cudaHostAllocDefault));
+    PLF_CUDA(ctx, cudaHostAlloc(&s->h_tab[i], batch_tab_bytes(B), cudaHostAllocDefault));
   }
   FrameSlots& f = s->fs;
   cudaStream_t cs = ctx->stream;
@@ -820,8 +828,7 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
   for (int k = 0; k < B; ++k) gp[k].T_init = s->pair_T + 16 * (size_t)k;   // the same problems seeded with the prediction
   PLF_CUDA(ctx, cudaMemcpyAsync(s->gn_probs_mm, gp.data(), gp.size() * sizeof(GnProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaStreamSynchronize(cs));
-  if (ctx->afast_on && (st = pipe_fast_th_reset(ctx))) return st;
-  return ctx->motion_on ? pipe_motion_reset(ctx) : PLF_OK;
+  return pipe_seq_reset(ctx, ctx->afast_on, ctx->motion_on);
 }
 
 // Builds the pipeline for the camera's image size on first use; a failed setup leaves no state behind.
@@ -835,9 +842,10 @@ static plf_status pipe_prepare(plf_ctx* ctx) {
 // One plf_batch_run call: its pairs, buffer parities and slots, and the streams of its phases.
 struct BatchRun {
   int B;
-  int ncarry;    // entries of the carry list in h_tab[rp]: the sequences the batch holds
-  bool cams;     // h_cam[rp] holds the pairs' cameras (a sequence of the batch has its own); else the context's camera
-  bool afast;    // adaptive FAST thresholds (plf_set_adaptive_fast): the sequence table goes up before the E phase, which reads it
+  int ncarry;    // entries of the carry list in batch table rp: the sequences the batch holds
+  bool cams;     // batch table rp holds the pairs' cameras (a sequence of the batch has its own); else the context's camera
+  int nin;       // entries of the input table in batch table rp (0: none, every pair is converted as it is)
+  bool afast;    // adaptive FAST thresholds (plf_set_adaptive_fast): pair thresholds in the E phase, the next ones behind k_finalize
   bool motion;   // motion model (plf_set_motion_model): pair predictions at the start of M, the next ones behind k_finalize
   int par;       // parity of the E -> G -> M hand-off buffers
   int lp;        // parity of the LSD hand-off buffers (0 when they exist once)
@@ -847,16 +855,20 @@ struct BatchRun {
   cudaStream_t sM, sE, sG, sP;
 };
 
-// The batch's sequence table (prev[B], then the carry list) and its pairs' cameras, to ring entry rp of the device on the
-// copy stream, in order behind the batch's own images and ahead of the next batch's upload; ev_tab[rp] marks them.
+// Entry rp of the pinned and of the device batch table ring.
+static BatchTab host_tab(const PipeState* s, int rp) { return batch_tab(s->h_tab[rp], s->B); }
+static BatchTab dev_tab(const PipeState* s, int rp) { return batch_tab(s->tab + rp * batch_tab_bytes(s->B), s->B); }
+
+// The parts of the batch's table that it uses, to ring entry rp of the device on the copy stream: the sequence table
+// always, the cameras and the input table when it has them.  ev_tab[rp] marks them.
 static plf_status send_tab(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
-  const int rp = r.rp;
-  int32_t* prev = s->seq_tab + (size_t)rp * 3 * s->B;
-  PLF_CUDA(ctx, cudaMemcpyAsync(prev, s->h_tab[rp], sizeof(int32_t) * r.B, cudaMemcpyHostToDevice, s->copy));
-  PLF_CUDA(ctx, cudaMemcpyAsync(prev + s->B, s->h_tab[rp] + s->B, sizeof(int32_t) * 2 * r.ncarry, cudaMemcpyHostToDevice, s->copy));
-  if (r.cams)
-    PLF_CUDA(ctx, cudaMemcpyAsync(s->cam_tab + (size_t)rp * s->B, s->h_cam[rp], sizeof(PlfPairCam) * r.B, cudaMemcpyHostToDevice, s->copy));
-  PLF_CUDA(ctx, cudaEventRecord(s->ev_tab[rp], s->copy));
+  const BatchTab h = host_tab(s, r.rp), d = dev_tab(s, r.rp);
+  cudaStream_t cs = s->copy;
+  PLF_CUDA(ctx, cudaMemcpyAsync(d.prev, h.prev, sizeof(int32_t) * r.B, cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaMemcpyAsync(d.carry, h.carry, sizeof(int32_t) * 2 * r.ncarry, cudaMemcpyHostToDevice, cs));
+  if (r.cams) PLF_CUDA(ctx, cudaMemcpyAsync(d.cams, h.cams, sizeof(PlfPairCam) * r.B, cudaMemcpyHostToDevice, cs));
+  if (r.nin) PLF_CUDA(ctx, cudaMemcpyAsync(d.in, h.in, sizeof(PlfRectPair) * r.nin, cudaMemcpyHostToDevice, cs));
+  PLF_CUDA(ctx, cudaEventRecord(s->ev_tab[r.rp], cs));
   return PLF_OK;
 }
 
@@ -875,90 +887,42 @@ __device__ __forceinline__ int remap_px(const uint8_t* __restrict__ src, int row
   return (acc + 512) >> 10;
 }
 
-// cv::remap of one image of a rectified pair: grid.z = 2 j + side for entry j of tab.
-__global__ void __launch_bounds__(256) k_rectify(const PlfRectPair* __restrict__ tab, const uint8_t* __restrict__ imgs, size_t AP,
-                                                 int pitch, int w, int h, uint8_t* __restrict__ out) {
-  const int x = blockIdx.x * 32 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y;
-  if (x >= w || y >= h) return;
-  const int j = blockIdx.z >> 1, side = blockIdx.z & 1;
-  const PlfRectPair e = tab[j];
-  const size_t A = (size_t)w * h, i = (size_t)y * w + x;
-  const short2 m = PLF_RECT_MAP1(e.maps, A, side)[i];
-  const int f = PLF_RECT_MAP2(e.maps, A, side)[i] & 1023, fx = f & 31, fy = f >> 5;
-  const uint8_t* src = imgs + (size_t)(2 * e.pair + side) * AP;
-  out[(size_t)blockIdx.z * AP + (size_t)y * pitch + x] = (uint8_t)remap_px(src, pitch, 1, w, h, m.x, m.y, fx, fy);
-}
-
 // cv::cvtColor(COLOR_BGR2GRAY) of 8-bit B, G, R as OpenCV 4 computes it (15-bit fixed point; COLOR_BGRA2GRAY ignores alpha)
 __device__ __forceinline__ int bgr_gray(int b, int g, int r) { return (3735 * b + 19235 * g + 9798 * r + (1 << 14)) >> 15; }
 
-// The grey images of a colour batch (plf_batch_upload_color): grid.z = image 2k + side.  src: the landing buffer, [2B][h][w]
-// pixels of ch = 3 (BGR) or 4 (BGRA) interleaved bytes, laid out like imgs.  Pair k of a rectified sequence (tab[k].maps
-// set; tab NULL: no pair is) is remapped per channel with its maps first and converted after, as stvo-pl's reader remaps
-// the colour image it read and the detectors convert it; every other pair is converted as it is.
-__global__ void __launch_bounds__(256) k_color(const PlfRectPair* __restrict__ tab, const uint8_t* __restrict__ src, int ch, int w,
-                                               int h, size_t AP, int pitch, uint8_t* __restrict__ out) {
+// Grey image z = 2 j + side of a batch's input: entry j of tab gives the pair and its maps (tab NULL: pair j, not
+// rectified).  src holds image 2k + side of pair k `img` bytes after image 0, w x h pixels of `row` bytes per row and CH
+// interleaved bytes per pixel (1: grey, 3: BGR, 4: BGRA).  A pair with maps is remapped per channel first and converted
+// after, as stvo-pl's reader remaps the colour image it read and the detectors convert it; every other pair is converted
+// as it is.
+template <int CH>
+__global__ void __launch_bounds__(256) k_input(const PlfRectPair* __restrict__ tab, const uint8_t* __restrict__ src, size_t img,
+                                               int row, int w, int h, size_t AP, int pitch, uint8_t* __restrict__ out) {
   const int x = blockIdx.x * 32 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y;
   if (x >= w || y >= h) return;
-  const int side = blockIdx.z & 1;
-  const size_t A = (size_t)w * h, i = (size_t)y * w + x;
-  const uint8_t* img = src + (size_t)blockIdx.z * A * ch;
-  const uint8_t* maps = tab ? tab[blockIdx.z >> 1].maps : nullptr;
-  int v[3];
-  if (maps) {
-    const short2 m = PLF_RECT_MAP1(maps, A, side)[i];
-    const int f = PLF_RECT_MAP2(maps, A, side)[i] & 1023, fx = f & 31, fy = f >> 5;
-    for (int c = 0; c < 3; ++c) v[c] = remap_px(img + c, w * ch, ch, w, h, m.x, m.y, fx, fy);
+  const int j = blockIdx.z >> 1, side = blockIdx.z & 1;
+  const PlfRectPair e = tab ? tab[j] : PlfRectPair{nullptr, j, 0};
+  const uint8_t* im = src + (size_t)(2 * e.pair + side) * img;
+  constexpr int NC = CH == 1 ? 1 : 3;   // the channels read: alpha is not
+  int v[3] = {0, 0, 0};
+  if (e.maps) {
+    const size_t A = (size_t)w * h, i = (size_t)y * w + x;
+    const short2 m = PLF_RECT_MAP1(e.maps, A, side)[i];
+    const int f = PLF_RECT_MAP2(e.maps, A, side)[i] & 1023, fx = f & 31, fy = f >> 5;
+    for (int c = 0; c < NC; ++c) v[c] = remap_px(im + c, row, CH, w, h, m.x, m.y, fx, fy);
   } else {
-    for (int c = 0; c < 3; ++c) v[c] = __ldg(img + i * ch + c);
+    for (int c = 0; c < NC; ++c) v[c] = __ldg(im + (size_t)y * row + x * CH + c);
   }
-  out[(size_t)blockIdx.z * AP + (size_t)y * pitch + x] = (uint8_t)bgr_gray(v[0], v[1], v[2]);
+  out[(size_t)blockIdx.z * AP + (size_t)y * pitch + x] = (uint8_t)(CH == 1 ? v[0] : bgr_gray(v[0], v[1], v[2]));
 }
 
-// Rectifies the pairs of the batch whose sequence has maps in the slot the run consumes, before any stream of the run
-// reads it: on the copy stream, behind the upload, each such pair is remapped into scratch and copied back in place, and
-// ev_up[run_slot] is recorded again, so the E and P phases (which wait for it) read the rectified images.  The copy stream
-// orders one batch's scratch use before the next's.  A batch without such a pair enqueues nothing.
-static plf_status run_rectify(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
-  if (ctx->seqs.empty()) return PLF_OK;
-  PlfRectPair* ht = s->h_rect[r.rp];
-  int nr = 0;
-  for (int k = 0; k < r.B; ++k)
-    if (const uint8_t* maps = ctx->seqs[s->pair_seq[k]].rect) ht[nr++] = PlfRectPair{maps, k, 0};
-  if (nr == 0) return PLF_OK;
-  const size_t AP = (size_t)s->pitch * s->h;
-  PlfRectPair* tab;
-  uint8_t* pairs;
+// The colour landing buffer of ch channels, [2 max_batch][h][w][ch] (image 2k = left k, 2k+1 = right k), carved from
+// PLF_SCR_COLOR_PIPE.  Only the copy stream touches it: the uploads land there and the runs' conversions read it in call
+// order, so one buffer serves every batch in flight.  To grow (the first colour upload, or 4 channels after 3) the block
+// waits for the copy stream, and the new block is allocated before the old one is freed: a failed allocation leaves the
+// last upload as it was.
+static plf_status color_scratch(plf_ctx* ctx, PipeState* s, int ch, uint8_t** land) {
   DevBufList b;
-  b.add(tab, s->B);
-  b.add(pairs, 2 * (size_t)s->B * AP);
-  if (b.carve(ctx, PLF_SCR_RECT_PIPE)) return PLF_ERR_CUDA;
-  uint8_t* imgs = s->imgs2[r.run_slot];
-  cudaStream_t cs = s->copy;
-  // a run that read this slot before (a slot run twice) has finished with it
-  PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_free[r.run_slot], 0));
-  PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_free2[r.run_slot], 0));
-  PLF_CUDA(ctx, cudaMemcpyAsync(tab, ht, sizeof(PlfRectPair) * nr, cudaMemcpyHostToDevice, cs));
-  k_rectify<<<dim3((s->w + 31) / 32, (s->h + 7) / 8, 2 * nr), dim3(32, 8), 0, cs>>>(tab, imgs, AP, s->pitch, s->w, s->h, pairs);
-  PLF_LAUNCH_CHECK(ctx);
-  // back in runs of consecutive pairs, w bytes of each row (the slot's row padding stays as the upload left it)
-  for (int j0 = 0, j1; j0 < nr; j0 = j1) {
-    for (j1 = j0 + 1; j1 < nr && ht[j1].pair == ht[j1 - 1].pair + 1;) ++j1;
-    PLF_CUDA(ctx, cudaMemcpy2DAsync(imgs + 2 * (size_t)ht[j0].pair * AP, (size_t)s->pitch, pairs + 2 * (size_t)j0 * AP, (size_t)s->pitch,
-                                    (size_t)s->w, 2 * (size_t)(j1 - j0) * s->h, cudaMemcpyDeviceToDevice, cs));
-  }
-  PLF_CUDA(ctx, cudaEventRecord(s->ev_up[r.run_slot], cs));
-  return PLF_OK;
-}
-
-// The pair table and the colour landing buffer of ch channels, [2 max_batch][h][w][ch] (image 2k = left k, 2k+1 = right
-// k), carved from PLF_SCR_COLOR_PIPE.  Only the copy stream touches them: the uploads land there and the runs' conversions
-// read them in call order, so one buffer serves every batch in flight.  To grow (the first colour upload, or 4 channels
-// after 3) the block waits for the copy stream, and the new block is allocated before the old one is freed: a failed
-// allocation leaves the last upload as it was.
-static plf_status color_scratch(plf_ctx* ctx, PipeState* s, int ch, PlfRectPair** tab, uint8_t** land) {
-  DevBufList b;
-  b.add(*tab, s->B);
   b.add(*land, 2 * (size_t)s->B * s->h * s->w * ch);
   size_t need = 0;
   for (const DevBufList::Entry& e : b.entries) need += plf_align256(e.bytes);
@@ -979,31 +943,52 @@ static plf_status color_scratch(plf_ctx* ctx, PipeState* s, int ch, PlfRectPair*
   return b.carve(ctx, PLF_SCR_COLOR_PIPE);
 }
 
-// Converts the colour batch the run consumes (plf_batch_upload_color) into its grey image slot, before any stream of the
-// run reads it: on the copy stream, behind the upload, once the runs that read the slot before have finished with it;
-// ev_up[run_slot] is recorded again for the E and P phases.  Pairs of rectified sequences are remapped in the same pass, so
-// run_rectify has nothing to do for a colour batch.
-static plf_status run_color(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
-  PlfRectPair* ht = s->h_rect[r.rp];
-  bool rect = false;
-  for (int k = 0; k < r.B; ++k) {
-    const uint8_t* maps = ctx->seqs.empty() ? nullptr : ctx->seqs[s->pair_seq[k]].rect;
-    ht[k] = PlfRectPair{maps, k, 0};
-    rect |= maps != nullptr;
+// Turns the upload the run consumes into the grey images of its slot, before any stream of the run reads them: on the
+// copy stream, behind the upload and the batch table, once the runs that read the slot before have finished with it;
+// ev_up[run_slot] is recorded again, so the E and P phases (which wait for it) read the result.  A colour upload
+// (plf_batch_upload_color) is converted from the landing buffer into the slot, the pairs of rectified sequences remapped
+// in the same pass.  A grey upload landed in the slot before the run knew its sequences: its rectified pairs are remapped
+// into scratch and copied back in place (the copy stream orders one batch's scratch use before the next's), and a grey
+// batch without one enqueues nothing.
+static plf_status run_input(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
+  const bool color = s->up_ch > 1;
+  if (!color && r.nin == 0) return PLF_OK;
+  const int w = s->w, h = s->h;
+  const size_t AP = (size_t)s->pitch * h;
+  uint8_t* imgs = s->imgs2[r.run_slot];
+  const PlfRectPair* tab = r.nin ? dev_tab(s, r.rp).in : nullptr;
+  uint8_t* land = nullptr;    // colour: the landing buffer
+  uint8_t* pairs = nullptr;   // grey: the remapped pairs
+  if (color) {
+    if (plf_status st = color_scratch(ctx, s, s->up_ch, &land)) return st;
+  } else {
+    DevBufList b;
+    b.add(pairs, 2 * (size_t)s->B * AP);
+    if (b.carve(ctx, PLF_SCR_RECT_PIPE)) return PLF_ERR_CUDA;
   }
-  PlfRectPair* tab;
-  uint8_t* land;
-  if (plf_status st = color_scratch(ctx, s, s->up_ch, &tab, &land)) return st;
   cudaStream_t cs = s->copy;
+  // a run that read this slot before (a slot run twice) has finished with it
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_free[r.run_slot], 0));
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_free2[r.run_slot], 0));
-  if (rect) PLF_CUDA(ctx, cudaMemcpyAsync(tab, ht, sizeof(PlfRectPair) * r.B, cudaMemcpyHostToDevice, cs));
-  plf_mark(ctx, cs, "color.start");
-  k_color<<<dim3((s->w + 31) / 32, (s->h + 7) / 8, 2 * r.B), dim3(32, 8), 0, cs>>>(rect ? tab : nullptr, land, s->up_ch, s->w, s->h,
-                                                                                    (size_t)s->pitch * s->h, s->pitch,
-                                                                                    s->imgs2[r.run_slot]);
-  PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, cs, "color.k_color");
+  const dim3 grid((w + 31) / 32, (h + 7) / 8, 2 * (color ? r.B : r.nin)), block(32, 8);
+  if (color) {
+    const int row = s->up_ch * w;
+    plf_mark(ctx, cs, "color.start");
+    if (s->up_ch == 3) k_input<3><<<grid, block, 0, cs>>>(tab, land, (size_t)row * h, row, w, h, AP, s->pitch, imgs);
+    else k_input<4><<<grid, block, 0, cs>>>(tab, land, (size_t)row * h, row, w, h, AP, s->pitch, imgs);
+    PLF_LAUNCH_CHECK(ctx);
+    plf_mark(ctx, cs, "color.k_color");
+  } else {
+    k_input<1><<<grid, block, 0, cs>>>(tab, imgs, AP, s->pitch, w, h, AP, s->pitch, pairs);
+    PLF_LAUNCH_CHECK(ctx);
+    // back in runs of consecutive pairs, w bytes of each row (the slot's row padding stays as the upload left it)
+    const PlfRectPair* in = host_tab(s, r.rp).in;
+    for (int j0 = 0, j1; j0 < r.nin; j0 = j1) {
+      for (j1 = j0 + 1; j1 < r.nin && in[j1].pair == in[j1 - 1].pair + 1;) ++j1;
+      PLF_CUDA(ctx, cudaMemcpy2DAsync(imgs + 2 * (size_t)in[j0].pair * AP, (size_t)s->pitch, pairs + 2 * (size_t)j0 * AP,
+                                      (size_t)s->pitch, (size_t)w, 2 * (size_t)(j1 - j0) * h, cudaMemcpyDeviceToDevice, cs));
+    }
+  }
   PLF_CUDA(ctx, cudaEventRecord(s->ev_up[r.run_slot], cs));
   return PLF_OK;
 }
@@ -1024,8 +1009,8 @@ static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     // also read img_th for the last time)
     PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_tab[r.rp], 0));
     PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_th, 0));
-    k_fast_th_images<<<(B + 127) / 128, 128, 0, sE>>>(s->seq_tab + (size_t)r.rp * 3 * s->B, B, s->B, s->B + s->nseq, fast_th0(ctx),
-                                                      s->seq_th, s->img_th);
+    k_fast_th_images<<<(B + 127) / 128, 128, 0, sE>>>(dev_tab(s, r.rp).prev, B, s->B, s->B + s->nseq, fast_th0(ctx), s->seq_rec,
+                                                      s->img_th);
     PLF_LAUNCH_CHECK(ctx);
     img_th = s->img_th;
   }
@@ -1103,12 +1088,11 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->evG[par], 0));
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->evE[par], 0));
   PLF_CUDA(ctx, cudaEventRecord(s->tM0[rp], cs));
-  // the batch's sequence table: prev[B], then the carry list
-  int32_t* prev = s->seq_tab + (size_t)rp * 3 * s->B;
-  int32_t* carry = prev + s->B;
-  // the pairs' cameras, when the batch has them (null: every kernel takes the context's camera)
-  PlfPairCam* pcam = r.cams ? s->cam_tab + (size_t)rp * s->B : nullptr;
-  if (!r.afast && (st = send_tab(ctx, s, r))) return st;   // with adaptive FAST thresholds the E phase sent it
+  // the batch's sequence table, and the pairs' cameras when the batch has them (null: every kernel takes the context's)
+  const BatchTab tab = dev_tab(s, rp);
+  const int32_t* prev = tab.prev;
+  const int32_t* carry = tab.carry;
+  const PlfPairCam* pcam = r.cams ? tab.cams : nullptr;
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_tab[rp], 0));
   k_f2f_problems<<<(B + 127) / 128, 128, 0, cs>>>(s->fs, prev, B, K, Ln, s->knn_keys, s->m12, s->mcount, P.min_ratio_12_p,
                                                   P.min_ratio_12_l, P.best_lr_matches ? 1 : 0, s->knn_f2f, s->nnr_f2f);
@@ -1117,7 +1101,7 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   // The previous batch wrote its sequences' ones behind its k_finalize on this stream.
   const double* T_pred = nullptr;
   if (r.motion) {
-    k_motion_pairs<<<B, 16, 0, cs>>>(prev, s->B, s->B + s->nseq, s->seq_T, s->pair_T);
+    k_motion_pairs<<<B, 16, 0, cs>>>(prev, s->B, s->B + s->nseq, s->seq_rec, s->pair_T);
     PLF_LAUNCH_CHECK(ctx);
     T_pred = s->pair_T;
   }
@@ -1206,16 +1190,13 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_LAUNCH_CHECK(ctx);
   k_carry<<<dim3(PLF_FS_NFIELDS, r.ncarry), 256, 0, cs>>>(s->fs, carry, K, Ln);   // the next batch tracks against these
   PLF_LAUNCH_CHECK(ctx);
-  if (r.afast) {   // the next batch's E phase waits for its sequences' thresholds
-    k_fast_th_update<<<(r.ncarry + 127) / 128, 128, 0, cs>>>(s->results + (size_t)rp * s->B, carry, r.ncarry, s->B, s->img_th,
-                                                             ctx->afast, s->seq_th);
+  if (r.afast || r.motion) {
+    // the next batch's E phase waits on ev_th for its sequences' thresholds; its M phase, on this stream, reads their
+    // predictions
+    k_seq_update<<<(r.ncarry + 127) / 128, 128, 0, cs>>>(s->results + (size_t)rp * s->B, carry, r.ncarry, s->B,
+                                                         r.afast ? s->img_th : nullptr, ctx->afast, r.motion ? 1 : 0, s->seq_rec);
     PLF_LAUNCH_CHECK(ctx);
-    PLF_CUDA(ctx, cudaEventRecord(s->ev_th, cs));
-  }
-  if (r.motion) {   // the next batch's M phase, on this stream, reads its sequences' predictions
-    k_motion_update<<<(r.ncarry + 127) / 128, 128, 0, cs>>>(s->results + (size_t)rp * s->B, carry, r.ncarry, s->B, s->seq_T,
-                                                            s->seq_valid);
-    PLF_LAUNCH_CHECK(ctx);
+    if (r.afast) PLF_CUDA(ctx, cudaEventRecord(s->ev_th, cs));
   }
   plf_mark(ctx, cs, "k_finalize+carry");
   // results + overflow flags to pinned memory as part of this batch's stream work; evM marks them ready
@@ -1231,6 +1212,29 @@ static void restart_sequence(plf_ctx* ctx, int s) {
   std::vector<uint8_t>& c = ctx->pipe->carried;
   if (s < 0) std::fill(c.begin(), c.end(), 0);
   else c[s] = 0;
+}
+
+// B pairs of w x h images of `row` bytes per row, read from left / right at `stride` bytes per row, to dst as images
+// 2k = left k, 2k+1 = right k of h rows at dpitch bytes per row, on stream cs.  Dense rows (stride = dpitch = row) are one
+// 2-D copy per side of B contiguous images ("rows" = images, pitch 2 images interleaving left and right); otherwise one
+// 3-D copy per side (B images of h rows, the destination "height" of 2h rows skipping the other side's image of each pair).
+static plf_status upload_pairs(plf_ctx* ctx, cudaStream_t cs, uint8_t* dst, int dpitch, int B, const uint8_t* left,
+                               const uint8_t* right, int stride, int row, int h) {
+  const size_t img = (size_t)dpitch * h;
+  for (int side = 0; side < 2; ++side) {
+    const uint8_t* src = side ? right : left;
+    if (stride == row && dpitch == row) {
+      PLF_CUDA(ctx, cudaMemcpy2DAsync(dst + side * img, 2 * img, src, img, img, B, cudaMemcpyHostToDevice, cs));
+    } else {
+      cudaMemcpy3DParms cp = {};
+      cp.srcPtr = make_cudaPitchedPtr(const_cast<uint8_t*>(src), (size_t)stride, (size_t)row, (size_t)h);
+      cp.dstPtr = make_cudaPitchedPtr(dst + side * img, (size_t)dpitch, (size_t)row, 2 * (size_t)h);
+      cp.extent = make_cudaExtent((size_t)row, (size_t)h, (size_t)B);
+      cp.kind = cudaMemcpyHostToDevice;
+      PLF_CUDA(ctx, cudaMemcpy3DAsync(&cp, cs));
+    }
+  }
+  return PLF_OK;
 }
 
 extern "C" {
@@ -1342,7 +1346,7 @@ plf_status plf_set_adaptive_fast(plf_ctx* ctx, const plf_adaptive_fast* cfg) {
     return plf_fail(ctx, PLF_ERR_STATE, "plf_set_adaptive_fast: %d batch(es) still in flight; download them first", ctx->pipe->n_pending);
   if (cfg && ctx->pipe) {
     PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-    const plf_status st = pipe_fast_th_reset(ctx);
+    const plf_status st = pipe_seq_reset(ctx, true, false);
     if (st) return st;
   }
   ctx->afast_on = cfg != nullptr;
@@ -1356,11 +1360,9 @@ plf_status plf_get_sequence_fast_th(plf_ctx* ctx, int s, int* th) {
   if (plf_status st = plf_check_sequence(ctx, "plf_get_sequence_fast_th", s)) return st;
   *th = fast_th0(ctx);
   if (!ctx->afast_on || !ctx->pipe || !ctx->pipe->carried[s]) return PLF_OK;   // the next pair is detected at orb_fast_th
-  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  int v = 0;   // behind the threshold updates of every batch in flight (M stream)
-  PLF_CUDA(ctx, cudaMemcpyAsync(&v, ctx->pipe->seq_th + s, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  *th = v;
+  SeqRecord q;
+  if (plf_status st = pipe_seq_read(ctx, s, &q)) return st;
+  *th = q.th;
   return PLF_OK;
 }
 
@@ -1370,7 +1372,7 @@ plf_status plf_set_motion_model(plf_ctx* ctx, int on) {
     return plf_fail(ctx, PLF_ERR_STATE, "plf_set_motion_model: %d batch(es) still in flight; download them first", ctx->pipe->n_pending);
   if (on && ctx->pipe) {
     PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-    const plf_status st = pipe_motion_reset(ctx);
+    const plf_status st = pipe_seq_reset(ctx, false, true);
     if (st) return st;
   }
   ctx->motion_on = on != 0;
@@ -1384,11 +1386,10 @@ plf_status plf_get_sequence_motion(plf_ctx* ctx, int s, double T[16], int* valid
   for (int i = 0; i < 16; ++i) T[i] = (i % 5 == 0) ? 1.0 : 0.0;
   *valid = 0;
   if (!ctx->motion_on || !ctx->pipe || !ctx->pipe->carried[s]) return PLF_OK;   // the next pair starts from identity
-  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  // behind the prediction updates of every batch in flight (M stream)
-  PLF_CUDA(ctx, cudaMemcpyAsync(T, ctx->pipe->seq_T + 16 * (size_t)s, 16 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  PLF_CUDA(ctx, cudaMemcpyAsync(valid, ctx->pipe->seq_valid + s, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  SeqRecord q;
+  if (plf_status st = pipe_seq_read(ctx, s, &q)) return st;
+  memcpy(T, q.T, sizeof q.T);
+  *valid = q.valid;
   return PLF_OK;
 }
 
@@ -1427,35 +1428,20 @@ plf_status plf_batch_upload(plf_ctx* ctx, int B, const uint8_t* left, const uint
   plf_status st = pipe_prepare(ctx);
   if (st) return st;
   PipeState* s = ctx->pipe;
-  const size_t A = (size_t)s->pitch * h;
   // H2D on the copy stream into the slot the GPU is not reading, so the copy of batch i+1 overlaps the run of batch i.
   // Device layout interleaves the pair: image 2k = left k, 2k+1 = right k; rows are padded to a 16-byte pitch.
   const int slot = s->up_slot ^ 1;
   uint8_t* dst = s->imgs2[slot];
   PLF_CUDA(ctx, cudaStreamWaitEvent(s->copy, s->ev_free[slot], 0));   // the last run that read this slot has finished with it
   PLF_CUDA(ctx, cudaStreamWaitEvent(s->copy, s->ev_free2[slot], 0));  // (ORB / LBD prelude on one stream, LSD on another)
-  const size_t A0 = (size_t)w * h;
   if (stride == w && s->stage) {
-    // densely packed input: ONE contiguous H2D copy per side into the dense landing buffer ("rows" = images, pitch 2 A0
-    // interleaves left and right), then a device-to-device 2-D copy widens the rows to the 16-byte pitch (the DMA engines
-    // move 1242-byte rows from host memory at a fraction of the contiguous rate: measured 8.9 k vs 12.7 k pairs/s end to end)
-    PLF_CUDA(ctx, cudaMemcpy2DAsync(s->stage, 2 * A0, left, A0, A0, B, cudaMemcpyHostToDevice, s->copy));
-    PLF_CUDA(ctx, cudaMemcpy2DAsync(s->stage + A0, 2 * A0, right, A0, A0, B, cudaMemcpyHostToDevice, s->copy));
+    // densely packed input: ONE contiguous H2D copy per side into the dense landing buffer, then a device-to-device 2-D
+    // copy widens the rows to the 16-byte pitch (the DMA engines move 1242-byte rows from host memory at a fraction of
+    // the contiguous rate: measured 8.9 k vs 12.7 k pairs/s end to end)
+    if ((st = upload_pairs(ctx, s->copy, s->stage, w, B, left, right, stride, w, h))) return st;
     PLF_CUDA(ctx, cudaMemcpy2DAsync(dst, (size_t)s->pitch, s->stage, (size_t)w, (size_t)w, 2 * (size_t)B * h, cudaMemcpyDeviceToDevice, s->copy));
-  } else if (stride == w) {   // pitch == w: the dense layout is the device layout
-    PLF_CUDA(ctx, cudaMemcpy2DAsync(dst, 2 * A, left, A, A, B, cudaMemcpyHostToDevice, s->copy));
-    PLF_CUDA(ctx, cudaMemcpy2DAsync(dst + A, 2 * A, right, A, A, B, cudaMemcpyHostToDevice, s->copy));
-  } else {
-    // strided input: one 3-D copy per side (rows of w bytes, h rows per image, B images; the destination "height" of 2h
-    // rows skips the other side's image of each pair)
-    for (int side = 0; side < 2; ++side) {
-      cudaMemcpy3DParms cp = {};
-      cp.srcPtr = make_cudaPitchedPtr(const_cast<uint8_t*>(side ? right : left), (size_t)stride, (size_t)w, (size_t)h);
-      cp.dstPtr = make_cudaPitchedPtr(dst + (size_t)side * A, (size_t)s->pitch, (size_t)w, 2 * (size_t)h);
-      cp.extent = make_cudaExtent((size_t)w, (size_t)h, (size_t)B);
-      cp.kind = cudaMemcpyHostToDevice;
-      PLF_CUDA(ctx, cudaMemcpy3DAsync(&cp, s->copy));
-    }
+  } else if ((st = upload_pairs(ctx, s->copy, dst, s->pitch, B, left, right, stride, w, h))) {   // pitch == w: dense rows
+    return st;
   }
   PLF_CUDA(ctx, cudaEventRecord(s->ev_up[slot], s->copy));
   s->up_slot = slot;
@@ -1478,27 +1464,12 @@ plf_status plf_batch_upload_color(plf_ctx* ctx, int B, const uint8_t* left, cons
   plf_status st = pipe_prepare(ctx);
   if (st) return st;
   PipeState* s = ctx->pipe;
-  PlfRectPair* tab;
   uint8_t* land;
-  if ((st = color_scratch(ctx, s, channels, &tab, &land))) return st;
+  if ((st = color_scratch(ctx, s, channels, &land))) return st;
   // H2D on the copy stream into the landing buffer; the run converts it into the image slot the GPU is not reading.
-  // Dense rows of ch w bytes are one contiguous block per image, so each side is one copy of B blocks (no short-row DMA
-  // to avoid, unlike the grey path's stage); strided input is one 3-D copy per side (B images of h rows of ch w bytes,
-  // the destination "height" of 2h rows skipping the other side's image of each pair).
-  const size_t row = (size_t)channels * w, AC = row * h;
-  if ((size_t)stride == row) {
-    PLF_CUDA(ctx, cudaMemcpy2DAsync(land, 2 * AC, left, AC, AC, B, cudaMemcpyHostToDevice, s->copy));
-    PLF_CUDA(ctx, cudaMemcpy2DAsync(land + AC, 2 * AC, right, AC, AC, B, cudaMemcpyHostToDevice, s->copy));
-  } else {
-    for (int side = 0; side < 2; ++side) {
-      cudaMemcpy3DParms cp = {};
-      cp.srcPtr = make_cudaPitchedPtr(const_cast<uint8_t*>(side ? right : left), (size_t)stride, row, (size_t)h);
-      cp.dstPtr = make_cudaPitchedPtr(land + (size_t)side * AC, row, row, 2 * (size_t)h);
-      cp.extent = make_cudaExtent(row, (size_t)h, (size_t)B);
-      cp.kind = cudaMemcpyHostToDevice;
-      PLF_CUDA(ctx, cudaMemcpy3DAsync(&cp, s->copy));
-    }
-  }
+  // Dense rows of ch w bytes are one contiguous block per image (no short-row DMA to avoid, unlike the grey path's stage).
+  const int row = channels * w;
+  if ((st = upload_pairs(ctx, s->copy, land, row, B, left, right, stride, row, h))) return st;
   s->up_slot ^= 1;
   s->up_ch = channels;
   return PLF_OK;
@@ -1545,10 +1516,12 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   r.B = B;
   r.par = (int)(s->seq & 1);
   r.rp = (int)(s->seq % 3);
-  // The sequence table, into the ring entry of this batch (the batch that used it last has been downloaded): pair k tracks
-  // against the batch's previous pair of its sequence, else the sequence's carried frame, else (and on a restart) nothing
-  int32_t* prev = s->h_tab[r.rp];
-  int32_t* carry = prev + s->B;
+  // The batch's table, into its ring entry (the batch that used it last has been downloaded, and its input conversion
+  // ran before its ev_up).  Pair k tracks against the batch's previous pair of its sequence, else the sequence's carried
+  // frame, else (and on a restart) nothing
+  const BatchTab tab = host_tab(s, r.rp);
+  int32_t* prev = tab.prev;
+  int32_t* carry = tab.carry;
   const int empty = s->B + s->nseq;
   for (int k = 0; k < B; ++k) {
     if (restart && restart[k]) prev[k] = empty;
@@ -1563,13 +1536,21 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
     carry[2 * r.ncarry + 1] = s->B + q[k];
     r.ncarry++;
   }
-  // the cameras of the pairs, resolved now: a later plf_set_sequence_camera does not reach this batch
+  // the cameras and maps of the pairs, resolved now: a later plf_set_sequence_camera or _rectification does not reach
+  // this batch.  The input table of a grey batch lists its rectified pairs; a colour batch, converted whole, lists every
+  // pair when one of them is rectified.
   r.cams = false;
+  r.nin = 0;
+  bool rect = false;
   for (int k = 0; k < B; ++k) {
     const plf_camera& c = plf_sequence_camera(ctx, q[k]);
-    s->h_cam[r.rp][k] = PlfPairCam{c.fx, c.fy, c.cx, c.cy, c.b};
+    tab.cams[k] = PlfPairCam{c.fx, c.fy, c.cx, c.cy, c.b};
     r.cams |= &c != &ctx->cam;
+    const uint8_t* maps = ctx->seqs.empty() ? nullptr : ctx->seqs[q[k]].rect;
+    if (maps || s->up_ch > 1) tab.in[r.nin++] = PlfRectPair{maps, k, 0};
+    rect |= maps != nullptr;
   }
+  if (!rect) r.nin = 0;
   r.run_slot = s->up_slot;
   // With profiling on everything is serialised on the main stream so that the per-kernel marks are meaningful.
   r.piped = !ctx->profile || ctx->profile_piped;
@@ -1581,8 +1562,8 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   r.sP = (r.piped && r.lsd2) ? ctx->aux[2] : r.sG;   // LSD pre-grow chain: own stream when its outputs exist per parity
   r.afast = ctx->afast_on;
   r.motion = ctx->motion_on;
-  st = s->up_ch > 1 ? run_color(ctx, s, r) : run_rectify(ctx, s, r);
-  if (!st && r.afast) st = send_tab(ctx, s, r);
+  st = send_tab(ctx, s, r);
+  if (!st) st = run_input(ctx, s, r);
   if (!st) st = run_extract(ctx, s, r);
   if (!st) st = run_lsd(ctx, s, r);
   if (!st) st = run_match(ctx, s, r);

@@ -38,10 +38,10 @@ enum plf_scratch_slot {
   PLF_SCR_BOW,         // plf_bow_insert, plf_bow_insert_batch
   PLF_SCR_BA_BATCH,    // plf_local_ba_batch and plf_global_ba_batch: their staged layout
   PLF_SCR_LC,          // plf_loop_closure_pose and plf_loop_closure_pose_batch: their staged layout
-  PLF_SCR_RECT_PIPE,   // the rectification of plf_batch_run_sequences (plf_set_sequence_rectification): its pair table
-                       // and remapped pairs, sized for max_batch pairs once, so that it never grows under batches in flight
-  PLF_SCR_COLOR_PIPE,  // plf_batch_upload_color and the conversion of plf_batch_run_sequences: the pair table and the
-                       // colour landing buffer of max_batch pairs (color_scratch in pipeline.cu)
+  PLF_SCR_RECT_PIPE,   // the rectification of a grey batch in plf_batch_run_sequences (plf_set_sequence_rectification):
+                       // its remapped pairs, sized for max_batch pairs once, so that it never grows under batches in flight
+  PLF_SCR_COLOR_PIPE,  // plf_batch_upload_color and the conversion of plf_batch_run_sequences: the colour landing buffer
+                       // of max_batch pairs (color_scratch in pipeline.cu)
   PLF_SCR_COUNT
 };
 
