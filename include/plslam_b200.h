@@ -242,6 +242,16 @@ typedef struct plf_keypoint {
 plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, plf_keypoint* kps,
                    uint8_t* desc, int cap, int* n);
 
+/* plf_orb restricted to a mask: cv::ORB::detectAndCompute(img, mask, ...).  mask: w x h uint8 host array, mask_stride bytes
+ * per row (>= w), any non-zero value allowing a corner.  Pyramid level l >= 1 uses resize(mask of level l-1,
+ * INTER_LINEAR_EXACT) thresholded to 255 (THRESH_TOZERO at 254), as OpenCV builds it, so a pixel near a mask edge is
+ * masked on the coarser levels.  FAST and its non-maximum suppression run on the whole image; masked corners are dropped
+ * after them, before the per-level retainBest, so the level quotas fill from allowed corners (a masked corner still
+ * suppresses a weaker allowed neighbour).  An all-zero mask gives no keypoints.  Same buffers, errors and working state as
+ * plf_orb; PLF_ERR_INVALID for a NULL mask or mask_stride < w. */
+plf_status plf_orb_masked(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, const uint8_t* mask, int mask_stride,
+                          plf_keypoint* kps, uint8_t* desc, int cap, int* n);
+
 /* ------------------------------------------------------------------------------------------------
  * Line features (SURVEY §8 a2/a3)
  * ---------------------------------------------------------------------------------------------- */
@@ -268,7 +278,8 @@ typedef struct plf_keyline {
  * segs, and the next call starts clean).  Work is enqueued on plf_stream in a working state of its own (one
  * image, rebuilt when the image size changes, shared with plf_detect_lines) and never touches the batched pipeline's
  * buffers, so a call between batches in flight is safe. */
-/* img is 8-bit single-channel (grey), as for plf_orb. */
+/* img is 8-bit single-channel (grey), as for plf_orb.  The segments are raw: no mask applies to them (the masks of
+ * plf_detect_lines_masked and plf_set_sequence_mask act on KeyLines). */
 plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, float* segs, int cap, int* n);
 
 /* Line features of one image.  Replaces stvo-pl StereoFrame::detectLineFeatures (LSD branch):
@@ -282,6 +293,14 @@ plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, f
 /* img is 8-bit single-channel (grey), as for plf_orb. */
 plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride,
                             plf_keyline* keylines, uint8_t* desc, int cap, int* n);
+
+/* plf_detect_lines restricted to a mask: LSDDetectorC::detect(img, lines, scale, 1, opts, mask).  mask: w x h uint8 host
+ * array, mask_stride bytes per row (>= w).  After the end point clamp and the min_length filter, a KeyLine is deleted when
+ * the mask is 0 at both (int)-truncated end points (LSDDetector_custom.cpp:310-322); one allowed end point keeps it.  The
+ * survivors keep the class_id the length filter gave them; the lsd_nfeatures top-K then ranks the survivors only.  Same
+ * buffers, errors and working state as plf_detect_lines; PLF_ERR_INVALID for a NULL mask or mask_stride < w. */
+plf_status plf_detect_lines_masked(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, const uint8_t* mask,
+                                   int mask_stride, plf_keyline* keylines, uint8_t* desc, int cap, int* n);
 
 /* Test hook: evaluates the device port of glibc sinf/cosf used by the LSD region-angle update. */
 plf_status plf_debug_sincosf(plf_ctx* ctx, const float* in, float* s, float* c, int n);
@@ -817,6 +836,30 @@ plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out);
  * when the maps cannot be allocated or copied. */
 plf_status plf_set_sequence_rectification(plf_ctx* ctx, int s, const int16_t* map1_l, const uint16_t* map2_l,
                                           const int16_t* map1_r, const uint16_t* map2_r);
+
+/* Restricts the batched pipeline's ORB and line detection on sequence s's left / right images to masks, as
+ * plf_orb_masked and plf_detect_lines_masked do (the masks the detectors' mask arguments take; stvo-pl passes none).
+ * mask_l, mask_r: w x h uint8 (host arrays, copied), stride bytes per row, in the geometry the detectors see: after
+ * rectification for a rectified sequence, one channel for colour input.  Both NULL clears them; one NULL masks only the
+ * other image.
+ *   - Each mask's ORB pyramid is built on the device once, by this call.  Extraction then reads it: features under the mask
+ *     never reach the per-level retainBest, the line top-K, stereo association, tracking or the pose.
+ *   - The call may be made at any time, like plf_set_sequence_camera: the masks are resolved when a batch is run, so
+ *     batches already run keep the masks they were run with.  When s had a mask and batches are in flight, the call waits
+ *     until their extraction and line stages have finished, then frees the old pyramids; the new ones are separate blocks.
+ *   - It does not restart s: a mask changes what is detected, not the calibration.  The next pair is tracked against the
+ *     previous frame as it was extracted.
+ *   - plf_set_max_sequences drops every sequence's masks; plf_reset_sequence keeps them.
+ *   - A batch without a masked image reads no mask and runs the unmasked kernels.
+ * Device memory: one ORB pyramid's bytes per masked image (about 2.5 w h at 4 levels of scale 1.2: 1.2 MB at 1242 x 375),
+ * allocated by the call and freed when cleared, by plf_set_max_sequences or by plf_destroy.
+ * PLF_ERR_INVALID for s out of range or, with a mask given, stride < w, with nothing changed; PLF_ERR_CUDA when a pyramid
+ * cannot be allocated or built, with nothing changed.  Errors of the ORB configuration are plf_orb's. */
+plf_status plf_set_sequence_mask(plf_ctx* ctx, int s, const uint8_t* mask_l, const uint8_t* mask_r, int stride);
+
+/* Whether sequence s has a left / right mask (plf_set_sequence_mask): *left, *right = 1 or 0.  PLF_ERR_INVALID for s out of
+ * range or a NULL pointer. */
+plf_status plf_get_sequence_mask_set(plf_ctx* ctx, int s, int* left, int* right);
 
 /* stvo-pl's adaptative_fast (config_euroc.yaml:17, :36-41): each sequence's FAST threshold follows its last tracked frame.
  * The fields are the config keys fast_min_th, fast_max_th, fast_inc_th, fast_feat_th and fast_err_th. */

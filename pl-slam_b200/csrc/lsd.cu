@@ -991,11 +991,17 @@ __global__ void __launch_bounds__(128) k_lsd_rects(const LsdPix* __restrict__ pi
 }
 
 // ---- KeyLines (LSDDetector_custom.cpp:267-308) + stvo-pl top-K ---------------------------------------------------
+// MASKED (plf_set_sequence_mask, plf_detect_lines_masked): masks[im] is image im's mask (plf_pitch16(w) bytes per row) or
+// NULL.  A KeyLine whose two end points both truncate onto a 0 of the mask is deleted after the length filter and before
+// the top-K, keeping the class_id it was given among the lines of sufficient length (LSDDetector_custom.cpp:310-322 runs
+// after :299 numbers them).  The unmasked instantiation ignores masks.
 #define KL_SORT_CAP 4096
+template <bool MASKED>
 __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ segs_all, const int* __restrict__ nsegs,
                                                    int max_regions, int w, int h, double min_length, int nfeatures,
                                                    plf_keyline* __restrict__ kls_all, plf_keyline* __restrict__ kls_out,
-                                                   int max_lines, int* __restrict__ nlines, int* __restrict__ overflow) {
+                                                   int max_lines, int* __restrict__ nlines, int* __restrict__ overflow,
+                                                   const uint8_t* const* __restrict__ masks) {
   __shared__ unsigned long long keys[KL_SORT_CAP];  // (response desc, index asc) for the top-K
   __shared__ int s_scan[1024];
   __shared__ int s_total;
@@ -1006,9 +1012,13 @@ __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ se
   plf_keyline* out = kls_out + (size_t)im * max_lines;
   // pass 1: accept flags + ordered compaction (class_id = running counter of accepted lines, :299)
   int base = 0;
+  const uint8_t* mk = nullptr;
+  const int mp = (w + 15) & ~15;
+  int cbase = 0;   // MASKED: lines of sufficient length so far (the class_id counter), base counting those the mask keeps
+  if constexpr (MASKED) mk = masks[im];
   for (int c0 = 0; c0 < n; c0 += 1024) {
     const int i = c0 + tid;
-    bool ok = false;
+    bool ok = false, len_ok = false;   // len_ok: MASKED only
     plf_keyline kl;
     if (i < n) {
       float4 e = segs[i];
@@ -1023,6 +1033,11 @@ __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ se
       const double ddx = (double)__fsub_rn(e.x, e.z), ddy = (double)__fsub_rn(e.y, e.w);
       const double length = (double)(float)sqrt(ddx * ddx + ddy * ddy);
       ok = length > min_length;
+      if constexpr (MASKED) {
+        len_ok = ok;
+        if (ok && mk)   // the end points are clamped into the image above: (int) truncates onto one of its pixels
+          ok = mk[(size_t)(int)e.y * mp + (int)e.x] != 0 || mk[(size_t)(int)e.w * mp + (int)e.z] != 0;
+      }
       if (ok) {
         kl.startPointX = e.x; kl.startPointY = e.y; kl.endPointX = e.z; kl.endPointY = e.w;  // octaveScale = 1
         kl.sPointInOctaveX = e.x; kl.sPointInOctaveY = e.y; kl.ePointInOctaveX = e.z; kl.ePointInOctaveY = e.w;
@@ -1038,8 +1053,12 @@ __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ se
         kl.pty = __fdiv_rn(__fadd_rn(kl.endPointY, kl.startPointY), 2.f);
       }
     }
-    // block exclusive scan of ok flags
-    s_scan[tid] = ok ? 1 : 0;
+    // block exclusive scan of ok flags (MASKED: the length flags counted in the high half-word, ok in the low one)
+    if constexpr (MASKED) {
+      s_scan[tid] = (len_ok ? 0x10000 : 0) | (ok ? 1 : 0);
+    } else {
+      s_scan[tid] = ok ? 1 : 0;
+    }
     __syncthreads();
     for (int off = 1; off < 1024; off <<= 1) {
       const int v = tid >= off ? s_scan[tid - off] : 0;
@@ -1049,12 +1068,22 @@ __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ se
     }
     const int incl = s_scan[tid];
     if (tid == 1023) s_total = incl;
-    if (ok) {
-      kl.class_id = base + incl - 1;
-      all[base + incl - 1] = kl;
+    if constexpr (MASKED) {
+      if (ok) {
+        kl.class_id = cbase + (incl >> 16) - 1;
+        all[base + (incl & 0xFFFF) - 1] = kl;
+      }
+      __syncthreads();
+      base += s_total & 0xFFFF;
+      cbase += s_total >> 16;
+    } else {
+      if (ok) {
+        kl.class_id = base + incl - 1;
+        all[base + incl - 1] = kl;
+      }
+      __syncthreads();
+      base += s_total;
     }
-    __syncthreads();
-    base += s_total;
     __syncthreads();
   }
   const int m = base;
@@ -1342,7 +1371,8 @@ plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t
   return PLF_OK;
 }
 
-plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int n, cudaEvent_t keylines_wait) {
+plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int n, cudaEvent_t keylines_wait,
+                        const uint8_t* const* masks) {
   if (s->nimg < n) return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_grow: %d images > the state's %d", n, s->nimg);
   const LsdTables& T = *ctx->lsd_tables;
   const int w = s->w, h = s->h;
@@ -1365,8 +1395,12 @@ plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int
   plf_mark(ctx, cs, "lsd.k_lsd_rects");
   const double min_length = (double)ctx->params.min_line_length * (double)std::min(w, h);
   if (keylines_wait) PLF_CUDA(ctx, cudaStreamWaitEvent(cs, keylines_wait, 0));
-  k_keylines<<<n, 1024, 0, cs>>>(s->segs, s->nregions, s->max_regions, w, h, min_length, ctx->params.lsd_nfeatures, s->kls_all, s->kls[par],
-                                 s->max_lines, s->nlines[par], s->overflow);
+  if (masks)
+    k_keylines<true><<<n, 1024, 0, cs>>>(s->segs, s->nregions, s->max_regions, w, h, min_length, ctx->params.lsd_nfeatures, s->kls_all,
+                                         s->kls[par], s->max_lines, s->nlines[par], s->overflow, masks);
+  else
+    k_keylines<false><<<n, 1024, 0, cs>>>(s->segs, s->nregions, s->max_regions, w, h, min_length, ctx->params.lsd_nfeatures, s->kls_all,
+                                          s->kls[par], s->max_lines, s->nlines[par], s->overflow, nullptr);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "lsd.k_keylines");
   return PLF_OK;
@@ -1395,7 +1429,7 @@ void plf_lsd_outputs(const LsdState* s, int par, plf_keyline** kls, int** nlines
 }
 
 // LSD of the standalone operators on one w x h image at dimg, in ctx->lsd_standalone (rebuilt when the size changes).
-static plf_status lsd_standalone(plf_ctx* ctx, const uint8_t* dimg, int pitch, int w, int h) {
+static plf_status lsd_standalone(plf_ctx* ctx, const uint8_t* dimg, int pitch, int w, int h, const uint8_t* const* masks) {
   LsdState*& s = ctx->lsd_standalone;
   plf_status st;
   if (s && (s->w != w || s->h != h)) {
@@ -1405,7 +1439,7 @@ static plf_status lsd_standalone(plf_ctx* ctx, const uint8_t* dimg, int pitch, i
   }
   if (!s && (st = plf_lsd_create(ctx, w, h, 1, false, &s))) return st;
   if ((st = plf_lsd_pre(ctx, ctx->stream, s, dimg, (size_t)pitch * h, pitch, 0, 1))) return st;
-  return plf_lsd_grow(ctx, ctx->stream, s, 0, 1, nullptr);
+  return plf_lsd_grow(ctx, ctx->stream, s, 0, 1, nullptr, masks);
 }
 
 // `causes`: the ones that spoil what the caller returns.  plf_lsd returns the raw segments, which the KeyLine stage's
@@ -1433,7 +1467,7 @@ extern "C" plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   uint8_t* dimg = (uint8_t*)plf_scratch(ctx, PLF_SCR_LSD, (size_t)pitch * h);
   if (!dimg) return PLF_ERR_CUDA;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  plf_status st = lsd_standalone(ctx, dimg, pitch, w, h);
+  plf_status st = lsd_standalone(ctx, dimg, pitch, w, h, nullptr);
   if (st) return st;
   const LsdState* s = ctx->lsd_standalone;
   int n = 0;
@@ -1449,19 +1483,26 @@ extern "C" plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   return PLF_OK;
 }
 
-extern "C" plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride,
-                                       plf_keyline* keylines, uint8_t* desc, int cap, int* n_out) {
-  if (!ctx || !img || !n_out || w < 3 || h < 3 || stride < w || cap < 0 || (cap > 0 && (!keylines || !desc)))
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_detect_lines: bad arguments");
-  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+// plf_detect_lines and plf_detect_lines_masked (mask NULL: unmasked).  The mask (level 0 of the pyramid layout, one
+// plane) and its one-entry table live in PLF_SCR_LSD beside the image.
+static plf_status detect_lines(plf_ctx* ctx, const char* fn, const uint8_t* img, int w, int h, int stride, const uint8_t* mask,
+                               int mask_stride, plf_keyline* keylines, uint8_t* desc, int cap, int* n_out) {
   const int pitch = plf_pitch16(w);
-  uint8_t *dimg, *ddesc;
+  uint8_t *dimg, *ddesc, *dmask = nullptr;
+  const uint8_t** dtab = nullptr;
   short2* dgrad;
   DevBufList scr;
   scr.add(dimg, (size_t)pitch * h); scr.add(dgrad, (size_t)w * h); scr.add(ddesc, (size_t)ctx->limits.max_lines * 32);
+  if (mask) { scr.add(dmask, (size_t)pitch * h); scr.add(dtab, 1); }
   if (plf_status st = scr.carve(ctx, PLF_SCR_LSD)) return st;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  plf_status st = lsd_standalone(ctx, dimg, pitch, w, h);
+  if (mask) {
+    const uint8_t* hp = dmask;
+    PLF_CUDA(ctx, cudaMemcpy2DAsync(dmask, pitch, mask, mask_stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
+    PLF_CUDA(ctx, cudaMemcpyAsync(dtab, &hp, sizeof hp, cudaMemcpyHostToDevice, ctx->stream));
+    PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // hp is on this stack frame
+  }
+  plf_status st = lsd_standalone(ctx, dimg, pitch, w, h, dtab);
   if (st) return st;
   const LsdState* s = ctx->lsd_standalone;
   PlfTmaCache tm;
@@ -1471,16 +1512,35 @@ extern "C" plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, 
   if (st) return st;
   int n = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->nlines[0], sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  st = lsd_check_overflow(ctx, s, "plf_detect_lines", PLF_LSD_OVF_SEGMENTS | PLF_LSD_OVF_LINES | PLF_LSD_OVF_SORT);
+  st = lsd_check_overflow(ctx, s, fn, PLF_LSD_OVF_SEGMENTS | PLF_LSD_OVF_LINES | PLF_LSD_OVF_SORT);
   if (st) return st;
   *n_out = n;
-  if (n > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_detect_lines: %d lines > caller capacity %d", n, cap);
+  if (n > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: %d lines > caller capacity %d", fn, n, cap);
   if (n > 0) {
     PLF_CUDA(ctx, cudaMemcpyAsync(keylines, s->kls[0], (size_t)n * sizeof(plf_keyline), cudaMemcpyDeviceToHost, ctx->stream));
     PLF_CUDA(ctx, cudaMemcpyAsync(desc, ddesc, (size_t)n * 32, cudaMemcpyDeviceToHost, ctx->stream));
     PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   }
   return PLF_OK;
+}
+
+extern "C" plf_status plf_detect_lines(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride,
+                                       plf_keyline* keylines, uint8_t* desc, int cap, int* n_out) {
+  if (!ctx || !img || !n_out || w < 3 || h < 3 || stride < w || cap < 0 || (cap > 0 && (!keylines || !desc)))
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_detect_lines: bad arguments");
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  return detect_lines(ctx, "plf_detect_lines", img, w, h, stride, nullptr, 0, keylines, desc, cap, n_out);
+}
+
+extern "C" plf_status plf_detect_lines_masked(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, const uint8_t* mask,
+                                              int mask_stride, plf_keyline* keylines, uint8_t* desc, int cap, int* n_out) {
+  if (!ctx || !img || !n_out || w < 3 || h < 3 || stride < w || cap < 0 || (cap > 0 && (!keylines || !desc)))
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_detect_lines_masked: bad arguments");
+  if (!mask || mask_stride < w)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_detect_lines_masked: mask %s, need a w x h mask of stride >= w = %d",
+                    mask ? "stride too small" : "is NULL", w);
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  return detect_lines(ctx, "plf_detect_lines_masked", img, w, h, stride, mask, mask_stride, keylines, desc, cap, n_out);
 }
 
 // glibc sinf/cosf port check hook (tests only exercise it through this entry point)

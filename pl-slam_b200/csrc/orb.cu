@@ -222,9 +222,20 @@ __device__ __forceinline__ uint32_t fast_gt4(uint32_t d, uint32_t k7, bool th_sm
   const uint32_t low = (d & 0x7f7f7f7fu) + k7;           // bit 7 <=> (d & 0x7f) > (th & 0x7f); no carry crosses a byte
   return (th_small ? (low | d) : (low & d)) & 0x80808080u;
 }
+// Byte offset of level l inside one image's mask pyramid: level 0 at pitch plf_pitch16(w) first, then levels 1.. at the
+// image pyramid's own offsets and pitches (OrbGeom pyr_off / pitch), so a level is indexed like the image level.
+__host__ __device__ __forceinline__ size_t orb_mask_off(const OrbGeom& g, int l) {
+  return l == 0 ? 0 : ((((size_t)((g.w[0] + 15) & ~15) * g.h[0]) + 255) & ~(size_t)255) + g.pyr_off[l];
+}
+
+// MASKED (plf_set_sequence_mask, plf_orb_masked): masks[img] is image img's mask pyramid, or NULL; an NMS survivor whose
+// level mask is 0 is dropped before it reaches the candidate list and the histogram (KeyPointsFilter::runByPixelsMask
+// after FAST).  The unmasked instantiation ignores masks.
+template <bool MASKED>
 __global__ void __launch_bounds__(256, 5) k_fast_nms(const __grid_constant__ CUtensorMap tmap, OrbGeom g, int l, int tiles_x,
                                                   const int* __restrict__ img_th, uint32_t* __restrict__ cand, int* __restrict__ cand_count,
-                                                  int* __restrict__ hist, int* __restrict__ overflow) {
+                                                  int* __restrict__ hist, int* __restrict__ overflow,
+                                                  const uint8_t* const* __restrict__ masks) {
   const int W = g.w[l], H = g.h[l];
   const int x0 = (blockIdx.x % tiles_x) * FN_OW, y0 = (blockIdx.x / tiles_x) * FN_OH;
   const int img = blockIdx.y;
@@ -340,6 +351,10 @@ __global__ void __launch_bounds__(256, 5) k_fast_nms(const __grid_constant__ CUt
     if (!(s > sc[sy][sx - 1] && s > sc[sy][sx + 1] && s > sc[sy - 1][sx - 1] && s > sc[sy - 1][sx] &&
           s > sc[sy - 1][sx + 1] && s > sc[sy + 1][sx - 1] && s > sc[sy + 1][sx] && s > sc[sy + 1][sx + 1]))
       continue;
+    if constexpr (MASKED) {
+      const uint8_t* mk = masks[img];
+      if (mk && mk[orb_mask_off(g, l) + (size_t)gy * ((W + 15) & ~15) + gx] == 0) continue;
+    }
     const int slot = atomicAdd(&cand_count[img * ORB_MAX_LEVELS + l], 1);
     if (slot < g.cand_cap[l])
       cand[(size_t)img * g.cand_stride + g.cand_off[l] + slot] = ((uint32_t)gy << 20) | ((uint32_t)gx << 8) | (uint32_t)s;
@@ -793,7 +808,7 @@ plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_paritie
 // Runs ORB on nimg (<= s->nimg) images of s->w x s->h resident at d_imgs ([nimg][h][pitch], pitch a multiple of 16,
 // stride img_stride bytes).  Enqueued on cs; results stay on the device.
 plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par,
-                       const int* img_th) {
+                       const int* img_th, const uint8_t* const* masks) {
   const int w = s->w, h = s->h;
   plf_status st;
   OrbGeom g = s->g;
@@ -815,8 +830,11 @@ plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t
   plf_mark(ctx, cs, "orb.k_resize_exact");
   for (int l = 0; l < g.nlevels; ++l) {
     const int tx_ = (g.w[l] + FN_OW - 1) / FN_OW, ty_ = (g.h[l] + FN_OH - 1) / FN_OH;
-    k_fast_nms<<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(l == 0 ? *tm_fast0 : s->tm_fast[l], g, l, tx_, img_th, s->cand, s->cand_count,
-                                                      s->hist, s->overflow);
+    const CUtensorMap& tm = l == 0 ? *tm_fast0 : s->tm_fast[l];
+    if (masks)
+      k_fast_nms<true><<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(tm, g, l, tx_, img_th, s->cand, s->cand_count, s->hist, s->overflow, masks);
+    else
+      k_fast_nms<false><<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(tm, g, l, tx_, img_th, s->cand, s->cand_count, s->hist, s->overflow, nullptr);
     PLF_LAUNCH_CHECK(ctx);
   }
   plf_mark(ctx, cs, "orb.k_fast_nms");
@@ -866,11 +884,44 @@ void plf_orb_outputs(const OrbState* s, int par, plf_keypoint** kps, uint8_t** d
   *kps = s->kps[par]; *desc = s->desc[par]; *counts = s->kp_count[par]; *max_kp = s->g.max_kp;
 }
 
-extern "C" plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, plf_keypoint* kps,
-                              uint8_t* desc, int cap, int* n_out) {
-  if (!ctx || !img || !n_out || w < 8 || h < 8 || stride < w || cap < 0 || (cap > 0 && (!kps || !desc)))
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_orb: bad arguments");
-  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+// ---- masks (plf_set_sequence_mask, plf_orb_masked) ------------------------------------------------------
+// One mask level to 255 where it exceeds lo, else 0: lo = 0 binarises the caller's mask (level 0), lo = 254 is
+// cv::threshold(level, level, 254, 0, THRESH_TOZERO) of a resized level (only 255 survives).
+__global__ void __launch_bounds__(256) k_mask_level(uint8_t* __restrict__ m, int pitch, int w, int lo) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+  if (x >= w) return;
+  uint8_t& v = m[(size_t)y * pitch + x];
+  v = v > lo ? 255 : 0;
+}
+
+size_t plf_orb_mask_bytes(const OrbState* s) { return plf_align256((size_t)plf_pitch16(s->w) * s->h) + s->g.pyr_stride; }
+
+// detectAndCompute's mask pyramid as cv2 4.13 applies it: level 0 = the caller's w x h mask (stride bytes per row), any
+// non-zero value 255; level l >= 1 = resize(level l-1, INTER_LINEAR_EXACT) thresholded to 255 or 0.  (Resizing the
+// caller's raw values instead would mask every level >= 1 of a mask of 1s and 254s; cv2 masks none of them.)  Written to
+// dst (plf_orb_mask_bytes(s) bytes + 64 of slack, the layout of orb_mask_off) on cs; s lends its geometry and resize
+// tables.
+plf_status plf_orb_mask_build(plf_ctx* ctx, cudaStream_t cs, const OrbState* s, const uint8_t* mask, int stride, uint8_t* dst) {
+  const OrbGeom& g = s->g;
+  PLF_CUDA(ctx, cudaMemcpy2DAsync(dst, plf_pitch16(s->w), mask, stride, s->w, s->h, cudaMemcpyHostToDevice, cs));
+  k_mask_level<<<dim3((s->w + 255) / 256, s->h), 256, 0, cs>>>(dst, plf_pitch16(s->w), s->w, 0);
+  PLF_LAUNCH_CHECK(ctx);
+  for (int l = 1; l < g.nlevels; ++l) {
+    uint8_t* lvl = dst + orb_mask_off(g, l);
+    const int sp = plf_pitch16(g.w[l - 1]), dp = plf_pitch16(g.w[l]);
+    plf_status st = plf_launch_resize_exact(ctx, cs, dst + orb_mask_off(g, l - 1), 0, sp, g.w[l - 1], g.h[l - 1], lvl, 0, dp, g.w[l],
+                                            g.h[l], s->rs_tab + s->rs_x_off[l], s->rs_tab + s->rs_xp_off[l], s->rs_tab + s->rs_y_off[l], 1);
+    if (st) return st;
+    k_mask_level<<<dim3((g.w[l] + 255) / 256, g.h[l]), 256, 0, cs>>>(lvl, dp, g.w[l], 254);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  return PLF_OK;
+}
+
+// plf_orb and plf_orb_masked (mask NULL: unmasked).  The mask pyramid and its one-entry table live in PLF_SCR_ORB beside
+// the image.
+static plf_status orb_standalone(plf_ctx* ctx, const char* fn, const uint8_t* img, int w, int h, int stride, const uint8_t* mask,
+                                 int mask_stride, plf_keypoint* kps, uint8_t* desc, int cap, int* n_out) {
   OrbState*& s = ctx->orb_standalone;
   plf_status st;
   if (s && (s->w != w || s->h != h)) {
@@ -880,10 +931,23 @@ extern "C" plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   }
   if (!s && (st = plf_orb_create(ctx, w, h, 1, false, &s))) return st;
   const int pitch = plf_pitch16(w);
-  uint8_t* dimg = (uint8_t*)plf_scratch(ctx, PLF_SCR_ORB, (size_t)pitch * h);
-  if (!dimg) return PLF_ERR_CUDA;
+  uint8_t* dimg;
+  const uint8_t** dtab = nullptr;
+  if (!mask) {
+    dimg = (uint8_t*)plf_scratch(ctx, PLF_SCR_ORB, (size_t)pitch * h);
+    if (!dimg) return PLF_ERR_CUDA;
+  } else {
+    uint8_t* dmask;
+    DevBufList scr;
+    scr.add(dimg, (size_t)pitch * h); scr.add(dmask, plf_orb_mask_bytes(s) + 64); scr.add(dtab, 1);
+    if ((st = scr.carve(ctx, PLF_SCR_ORB))) return st;
+    if ((st = plf_orb_mask_build(ctx, ctx->stream, s, mask, mask_stride, dmask))) return st;
+    const uint8_t* hp = dmask;
+    PLF_CUDA(ctx, cudaMemcpyAsync(dtab, &hp, sizeof hp, cudaMemcpyHostToDevice, ctx->stream));
+    PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // hp is on this stack frame
+  }
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  if ((st = plf_orb_run(ctx, ctx->stream, s, dimg, (size_t)pitch * h, pitch, 1, 0, nullptr))) return st;
+  if ((st = plf_orb_run(ctx, ctx->stream, s, dimg, (size_t)pitch * h, pitch, 1, 0, nullptr, dtab))) return st;
   int n = 0, ovf = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->kp_count[0], sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyAsync(&ovf, s->overflow, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
@@ -892,14 +956,33 @@ extern "C" plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, in
     cudaMemsetAsync(s->overflow, 0, sizeof(int), ctx->stream);
     char why[400];
     plf_orb_overflow_text(s, ovf, why, sizeof why);
-    return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_orb: keypoint capacity exceeded: %s", why);
+    return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: keypoint capacity exceeded: %s", fn, why);
   }
   *n_out = n;
-  if (n > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_orb: %d keypoints > caller capacity %d", n, cap);
+  if (n > cap) return plf_fail(ctx, PLF_ERR_CAPACITY, "%s: %d keypoints > caller capacity %d", fn, n, cap);
   if (n > 0) {
     PLF_CUDA(ctx, cudaMemcpyAsync(kps, s->kps[0], (size_t)n * sizeof(plf_keypoint), cudaMemcpyDeviceToHost, ctx->stream));
     PLF_CUDA(ctx, cudaMemcpyAsync(desc, s->desc[0], (size_t)n * 32, cudaMemcpyDeviceToHost, ctx->stream));
     PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   }
   return PLF_OK;
+}
+
+extern "C" plf_status plf_orb(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, plf_keypoint* kps,
+                              uint8_t* desc, int cap, int* n_out) {
+  if (!ctx || !img || !n_out || w < 8 || h < 8 || stride < w || cap < 0 || (cap > 0 && (!kps || !desc)))
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_orb: bad arguments");
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  return orb_standalone(ctx, "plf_orb", img, w, h, stride, nullptr, 0, kps, desc, cap, n_out);
+}
+
+extern "C" plf_status plf_orb_masked(plf_ctx* ctx, const uint8_t* img, int w, int h, int stride, const uint8_t* mask,
+                                     int mask_stride, plf_keypoint* kps, uint8_t* desc, int cap, int* n_out) {
+  if (!ctx || !img || !n_out || w < 8 || h < 8 || stride < w || cap < 0 || (cap > 0 && (!kps || !desc)))
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_orb_masked: bad arguments");
+  if (!mask || mask_stride < w)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_orb_masked: mask %s, need a w x h mask of stride >= w = %d",
+                    mask ? "stride too small" : "is NULL", w);
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  return orb_standalone(ctx, "plf_orb_masked", img, w, h, stride, mask, mask_stride, kps, desc, cap, n_out);
 }

@@ -50,22 +50,26 @@ constexpr int PLF_FS_NFIELDS = 0 PLF_PT_FIELDS(PLF_FS_ONE) PLF_LS_FIELDS(PLF_FS_
 struct PlfRectPair { const uint8_t* maps; int pair; int pad; };
 
 // One entry of the batch table ring, for max_batch pairs B: the sequence table (prev[B] = the frame slot of pair k's
-// previous frame, then the carry list [B][2] of (frame slot, carry slot)), the pairs' cameras [B] and the input table
-// [B].  The pinned and the device ring use the same layout.
+// previous frame, then the carry list [B][2] of (frame slot, carry slot)), the pairs' cameras [B], the input table [B]
+// and the mask table [2B] (image z's mask pyramid, plf_set_sequence_mask, or NULL).  The pinned and the device ring use
+// the same layout.
 struct BatchTab {
   int32_t* prev;
   int32_t* carry;
   PlfPairCam* cams;
   PlfRectPair* in;
+  const uint8_t** masks;
 };
 static size_t batch_tab_bytes(int B) {
-  return plf_align256(3 * sizeof(int32_t) * B) + plf_align256(sizeof(PlfPairCam) * B) + plf_align256(sizeof(PlfRectPair) * B);
+  return plf_align256(3 * sizeof(int32_t) * B) + plf_align256(sizeof(PlfPairCam) * B) + plf_align256(sizeof(PlfRectPair) * B) +
+         plf_align256(sizeof(uint8_t*) * 2 * B);
 }
 static BatchTab batch_tab(uint8_t* base, int B) {
   uint8_t* cams = base + plf_align256(3 * sizeof(int32_t) * B);
   uint8_t* in = cams + plf_align256(sizeof(PlfPairCam) * B);
+  uint8_t* masks = in + plf_align256(sizeof(PlfRectPair) * B);
   return {reinterpret_cast<int32_t*>(base), reinterpret_cast<int32_t*>(base) + B, reinterpret_cast<PlfPairCam*>(cams),
-          reinterpret_cast<PlfRectPair*>(in)};
+          reinterpret_cast<PlfRectPair*>(in), reinterpret_cast<const uint8_t**>(masks)};
 }
 
 // What each sequence carries to its next pair besides its frame slot: the pose prediction (row-major 4x4) and whether it
@@ -845,6 +849,7 @@ struct BatchRun {
   int ncarry;    // entries of the carry list in batch table rp: the sequences the batch holds
   bool cams;     // batch table rp holds the pairs' cameras (a sequence of the batch has its own); else the context's camera
   int nin;       // entries of the input table in batch table rp (0: none, every pair is converted as it is)
+  bool masked;   // batch table rp holds the images' masks (a sequence of the batch has one); else no image is masked
   bool afast;    // adaptive FAST thresholds (plf_set_adaptive_fast): pair thresholds in the E phase, the next ones behind k_finalize
   bool motion;   // motion model (plf_set_motion_model): pair predictions at the start of M, the next ones behind k_finalize
   int par;       // parity of the E -> G -> M hand-off buffers
@@ -868,6 +873,7 @@ static plf_status send_tab(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaMemcpyAsync(d.carry, h.carry, sizeof(int32_t) * 2 * r.ncarry, cudaMemcpyHostToDevice, cs));
   if (r.cams) PLF_CUDA(ctx, cudaMemcpyAsync(d.cams, h.cams, sizeof(PlfPairCam) * r.B, cudaMemcpyHostToDevice, cs));
   if (r.nin) PLF_CUDA(ctx, cudaMemcpyAsync(d.in, h.in, sizeof(PlfRectPair) * r.nin, cudaMemcpyHostToDevice, cs));
+  if (r.masked) PLF_CUDA(ctx, cudaMemcpyAsync(d.masks, h.masks, sizeof(uint8_t*) * 2 * r.B, cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaEventRecord(s->ev_tab[r.rp], cs));
   return PLF_OK;
 }
@@ -1004,17 +1010,18 @@ static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   plf_mark(ctx, sE, "start");
   PLF_CUDA(ctx, cudaEventRecord(s->tE0[par], sE));
   const int* img_th = nullptr;
+  const uint8_t* const* masks = r.masked ? dev_tab(s, r.rp).masks : nullptr;
+  if (r.afast || r.masked) PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_tab[r.rp], 0));   // the sequence or mask table
   if (r.afast) {
     // the thresholds of the batch's images: the sequence table, and the previous batch's threshold update (which has
     // also read img_th for the last time)
-    PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_tab[r.rp], 0));
     PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_th, 0));
     k_fast_th_images<<<(B + 127) / 128, 128, 0, sE>>>(dev_tab(s, r.rp).prev, B, s->B, s->B + s->nseq, fast_th0(ctx), s->seq_rec,
                                                       s->img_th);
     PLF_LAUNCH_CHECK(ctx);
     img_th = s->img_th;
   }
-  plf_status st = plf_orb_run(ctx, sE, s->orb, imgs, AP, s->pitch, 2 * B, par, img_th);
+  plf_status st = plf_orb_run(ctx, sE, s->orb, imgs, AP, s->pitch, 2 * B, par, img_th, masks);
   if (!st) st = plf_launch_blur5_sobel(ctx, sE, &s->lbd_tm, imgs, s->pitch, AP, w, h, 2 * B, s->lbd_grad[par], A);
   if (st) return st;
   plf_mark(ctx, sE, "lbd.k_blur5_sobel");
@@ -1037,6 +1044,7 @@ static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   const size_t AP = (size_t)s->pitch * s->h;
   cudaStream_t sP = r.sP, sG = r.sG;
   PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_up[r.run_slot], 0));
+  if (r.masked) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_tab[r.rp], 0));   // the mask table, read by G's KeyLine stage
   if (r.lsd2) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->evG[par], 0));   // batch i-2 (same parity) has finished growing / fitting on these maps
   PLF_CUDA(ctx, cudaEventRecord(s->tG0[par], sP));
   plf_status st = plf_lsd_pre(ctx, sP, s->lsd, s->imgs2[r.run_slot], AP, s->pitch, r.lp, 2 * r.B);
@@ -1046,7 +1054,8 @@ static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaStreamWaitEvent(sG, s->evP[par], 0));
   // the KeyLine outputs are overwritten: the match phase that read them last (batch i-2 with two parities, batch i-1 with one)
   // has taken its copy
-  st = plf_lsd_grow(ctx, sG, s->lsd, r.lp, 2 * r.B, r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr);
+  st = plf_lsd_grow(ctx, sG, s->lsd, r.lp, 2 * r.B, r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr,
+                    r.masked ? dev_tab(s, r.rp).masks : nullptr);
   if (st) return st;
   PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp + 1, plf_lsd_overflow_flag(s->lsd), sizeof(int), cudaMemcpyDeviceToDevice, sG));
   PLF_CUDA(ctx, cudaMemsetAsync(plf_lsd_overflow_flag(s->lsd), 0, sizeof(int), sG));
@@ -1321,6 +1330,73 @@ plf_status plf_set_sequence_rectification(plf_ctx* ctx, int s, const int16_t* ma
   return PLF_OK;
 }
 
+plf_status plf_set_sequence_mask(plf_ctx* ctx, int s, const uint8_t* mask_l, const uint8_t* mask_r, int stride) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (plf_status st = plf_check_sequence(ctx, "plf_set_sequence_mask", s)) return st;
+  const int w = ctx->cam.width, h = ctx->cam.height;
+  if ((mask_l || mask_r) && stride < w)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_mask: stride = %d, need stride >= width = %d", stride, w);
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  // the new pyramids, built into fresh blocks on the main stream with the pipeline's ORB geometry (or, before the pipeline
+  // exists, that of a one-image ORB state of the same size and parameters)
+  uint8_t* fresh[2] = {nullptr, nullptr};
+  if (mask_l || mask_r) {
+    OrbState* tmp = nullptr;
+    plf_status st = ctx->pipe ? PLF_OK : plf_orb_create(ctx, w, h, 1, false, &tmp);
+    if (st) return st;
+    const OrbState* geo = ctx->pipe ? ctx->pipe->orb : tmp;
+    const size_t bytes = plf_orb_mask_bytes(geo) + 64;
+    const uint8_t* src[2] = {mask_l, mask_r};
+    for (int side = 0; side < 2 && !st; ++side) {
+      if (!src[side]) continue;
+      const cudaError_t e = cudaMalloc(&fresh[side], bytes);
+      if (e != cudaSuccess) {
+        cudaGetLastError();
+        fresh[side] = nullptr;
+        st = plf_fail(ctx, PLF_ERR_CUDA, "plf_set_sequence_mask: cudaMalloc(%zu): %s", bytes, cudaGetErrorString(e));
+      } else {
+        st = plf_orb_mask_build(ctx, ctx->stream, geo, src[side], stride, fresh[side]);
+      }
+    }
+    if (!st && cudaStreamSynchronize(ctx->stream) != cudaSuccess)
+      st = plf_fail(ctx, PLF_ERR_CUDA, "plf_set_sequence_mask: building the mask pyramids: %s", cudaGetErrorString(cudaGetLastError()));
+    plf_orb_free(tmp);
+    if (st) {
+      cudaFree(fresh[0]);
+      cudaFree(fresh[1]);
+      return st;
+    }
+  }
+  // Batches in flight read the old pyramids in their extraction (ORB) and LSD (KeyLine) phases, on the E and G streams, or
+  // all on the main stream when profiling serialises them: the call waits for those streams before it frees them.
+  uint8_t** cur = ctx->seqs.empty() ? nullptr : ctx->seqs[s].mask;
+  if (cur && (cur[0] || cur[1]) && ctx->pipe) {
+    PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    PLF_CUDA(ctx, cudaStreamSynchronize(ctx->aux[0]));
+    PLF_CUDA(ctx, cudaStreamSynchronize(ctx->aux[1]));
+  }
+  if (cur) {
+    cudaFree(cur[0]);
+    cudaFree(cur[1]);
+  }
+  if (fresh[0] || fresh[1] || cur) {
+    PlfSequence& q = plf_sequence(ctx, s);
+    q.mask[0] = fresh[0];
+    q.mask[1] = fresh[1];
+  }
+  return PLF_OK;
+}
+
+plf_status plf_get_sequence_mask_set(plf_ctx* ctx, int s, int* left, int* right) {
+  if (!ctx) return PLF_ERR_INVALID;
+  if (!left || !right) return plf_fail(ctx, PLF_ERR_INVALID, "plf_get_sequence_mask_set: left and right are required");
+  if (plf_status st = plf_check_sequence(ctx, "plf_get_sequence_mask_set", s)) return st;
+  const bool any = !ctx->seqs.empty();
+  *left = any && ctx->seqs[s].mask[0] != nullptr;
+  *right = any && ctx->seqs[s].mask[1] != nullptr;
+  return PLF_OK;
+}
+
 plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out) {
   if (!ctx) return PLF_ERR_INVALID;
   plf_ctx* c = const_cast<plf_ctx*>(ctx);   // the error text is the only state a failed call writes
@@ -1536,19 +1612,25 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
     carry[2 * r.ncarry + 1] = s->B + q[k];
     r.ncarry++;
   }
-  // the cameras and maps of the pairs, resolved now: a later plf_set_sequence_camera or _rectification does not reach
-  // this batch.  The input table of a grey batch lists its rectified pairs; a colour batch, converted whole, lists every
-  // pair when one of them is rectified.
+  // the cameras, maps and masks of the pairs, resolved now: a later plf_set_sequence_camera, _rectification or _mask does
+  // not reach this batch.  The input table of a grey batch lists its rectified pairs; a colour batch, converted whole,
+  // lists every pair when one of them is rectified.
   r.cams = false;
   r.nin = 0;
+  r.masked = false;
   bool rect = false;
   for (int k = 0; k < B; ++k) {
     const plf_camera& c = plf_sequence_camera(ctx, q[k]);
     tab.cams[k] = PlfPairCam{c.fx, c.fy, c.cx, c.cy, c.b};
     r.cams |= &c != &ctx->cam;
-    const uint8_t* maps = ctx->seqs.empty() ? nullptr : ctx->seqs[q[k]].rect;
+    const PlfSequence* sq = ctx->seqs.empty() ? nullptr : &ctx->seqs[q[k]];
+    const uint8_t* maps = sq ? sq->rect : nullptr;
     if (maps || s->up_ch > 1) tab.in[r.nin++] = PlfRectPair{maps, k, 0};
     rect |= maps != nullptr;
+    for (int side = 0; side < 2; ++side) {
+      tab.masks[2 * k + side] = sq ? sq->mask[side] : nullptr;
+      r.masked |= tab.masks[2 * k + side] != nullptr;
+    }
   }
   if (!rect) r.nin = 0;
   r.run_slot = s->up_slot;

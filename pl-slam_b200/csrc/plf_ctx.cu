@@ -45,6 +45,8 @@ plf_status plf_problem_cameras(plf_ctx* ctx, const char* fn, int n, const int32_
 void plf_drop_sequences(plf_ctx* ctx) {
   for (PlfSequence& q : ctx->seqs) {
     cudaFree(q.rect);
+    cudaFree(q.mask[0]);
+    cudaFree(q.mask[1]);
     plf_bow_dbs_free(q.bow);
   }
   std::vector<PlfSequence>().swap(ctx->seqs);   // and its capacity

@@ -86,6 +86,7 @@ struct PlfSequence {
   bool own_cam = false;     // plf_set_sequence_camera: cam is the sequence's calibration, else it uses the context's
   plf_camera cam = {};
   uint8_t* rect = nullptr;  // plf_set_sequence_rectification: device block of 12 w h bytes (PLF_RECT_* layout, pipeline.cu)
+  uint8_t* mask[2] = {nullptr, nullptr};   // plf_set_sequence_mask: the left / right image's mask pyramid (plf_orb_mask_build)
   BowDbs* bow = nullptr;    // its bag-of-words databases (dbow.cu), from its first insert
 };
 
@@ -141,7 +142,7 @@ inline const plf_camera& plf_sequence_camera(const plf_ctx* ctx, int s) {
 // to *cam, each if given.  An entry outside [-1, max_sequences) returns PLF_ERR_INVALID naming fn, the problem and entry.
 plf_status plf_problem_camera(plf_ctx* ctx, const char* fn, const int32_t* seq, int p, const plf_camera** cam, int* s = nullptr);
 plf_status plf_problem_cameras(plf_ctx* ctx, const char* fn, int n, const int32_t* seq, std::vector<const plf_camera*>& cams);
-// Frees every sequence's maps and databases and empties the records.
+// Frees every sequence's maps, masks and databases and empties the records.
 void plf_drop_sequences(plf_ctx* ctx);
 // Frees one sequence's bag-of-words databases (dbow.cu); NULL is a no-op.
 void plf_bow_dbs_free(BowDbs* d);
@@ -291,8 +292,14 @@ plf_status gbb_ldlt(plf_ctx* ctx, cudaStream_t cs, const GbbLdlt& L, int nb, int
 plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, OrbState** out);
 void plf_orb_free(OrbState* s);
 // img_th: the FAST threshold of each image, on the device (plf_set_adaptive_fast), or NULL for plf_params.orb_fast_th.
+// masks: a device table of each image's mask pyramid (plf_orb_mask_build), an entry NULL for an unmasked image, or NULL
+// for no mask at all (the unmasked FAST kernel).
 plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par,
-                       const int* img_th);
+                       const int* img_th, const uint8_t* const* masks);
+// One image's mask pyramid in s's level layout: its bytes (allocate 64 more, as every image buffer), and its build from a
+// host mask of s->w x s->h, stride bytes per row, on cs.  Its first plf_pitch16(w) * h bytes are the mask itself.
+size_t plf_orb_mask_bytes(const OrbState* s);
+plf_status plf_orb_mask_build(plf_ctx* ctx, cudaStream_t cs, const OrbState* s, const uint8_t* mask, int stride, uint8_t* dst);
 void plf_orb_outputs(const OrbState* s, int par, plf_keypoint** kps, uint8_t** desc, int** counts, int* max_kp);
 // The overflow flag is a set of causes (one bit each, OR-ed in by the kernel that met it); plf_orb_overflow_text words them,
 // naming the limit that was actually hit: only max_keypoints is the caller's to raise.
@@ -317,8 +324,10 @@ plf_status plf_lsd_create(plf_ctx* ctx, int w, int h, int nimg, bool two_paritie
 void plf_lsd_free(LsdState* s);
 size_t plf_lsd_footprint(const plf_ctx* ctx, int w, int h, int nimg, bool two_parities);   // bytes plf_lsd_create allocates
 plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int par, int n);
-// keylines_wait: if set, the KeyLine outputs are overwritten only after this event
-plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int n, cudaEvent_t keylines_wait);
+// keylines_wait: if set, the KeyLine outputs are overwritten only after this event.  masks: as for plf_orb_run; the KeyLine
+// stage reads level 0 (plf_pitch16(w) bytes per row) of each listed image.
+plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int n, cudaEvent_t keylines_wait,
+                        const uint8_t* const* masks);
 void plf_lsd_outputs(const LsdState* s, int par, plf_keyline** kls, int** nlines, int* max_lines);
 // Causes of the LSD overflow flag, one bit each (as the ORB flag above)
 enum { PLF_LSD_OVF_SEGMENTS = 1,   // an image grows more regions than plf_limits.max_segments (k_lsd_grow)

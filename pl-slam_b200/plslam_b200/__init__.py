@@ -1128,17 +1128,25 @@ class Frontend:
         return x
 
     # -- point features --------------------------------------------------------------------------
-    def orb(self, img, cap=8192):
+    def orb(self, img, cap=8192, mask=None):
         """cv::ORB::detectAndCompute with the ctx parameters: returns (keypoints[KEYPOINT_DTYPE], desc u8[n,32])
-        in canonical (octave, y, x) order."""
+        in canonical (octave, y, x) order.  mask: u8 [H, W] of the image's shape (non-zero = allowed), as
+        detectAndCompute's mask argument (plf_orb_masked); None detects everywhere (plf_orb)."""
         img = _u8(img)
         h, w = img.shape
         kps = np.zeros(cap, KEYPOINT_DTYPE)
         desc = np.zeros((cap, 32), np.uint8)
         n = C.c_int(0)
-        st = self.lib.plf_orb(self._ctx, _ptr(img, C.c_uint8), w, h, img.strides[0],
-                              kps.ctypes.data_as(C.c_void_p), _ptr(desc, C.c_uint8), cap, C.byref(n))
-        self._check(st, "plf_orb")
+        if mask is None:
+            st = self.lib.plf_orb(self._ctx, _ptr(img, C.c_uint8), w, h, img.strides[0],
+                                  kps.ctypes.data_as(C.c_void_p), _ptr(desc, C.c_uint8), cap, C.byref(n))
+            self._check(st, "plf_orb")
+        else:
+            m = self._mask(mask, h, w, "orb")
+            st = self.lib.plf_orb_masked(self._ctx, _ptr(img, C.c_uint8), w, h, img.strides[0], _ptr(m, C.c_uint8),
+                                         m.strides[0], kps.ctypes.data_as(C.c_void_p), _ptr(desc, C.c_uint8), cap,
+                                         C.byref(n))
+            self._check(st, "plf_orb_masked")
         return kps[:n.value].copy(), desc[:n.value].copy()
 
     # -- line features ---------------------------------------------------------------------------
@@ -1153,16 +1161,25 @@ class Frontend:
         self._check(st, "plf_lsd")
         return segs[:n.value].copy()
 
-    def detect_lines(self, img, cap=4096):
-        """stvo-pl detectLineFeatures: (keylines[KEYLINE_DTYPE], LBD desc u8[n,32])."""
+    def detect_lines(self, img, cap=4096, mask=None):
+        """stvo-pl detectLineFeatures: (keylines[KEYLINE_DTYPE], LBD desc u8[n,32]).  mask: u8 [H, W] of the image's
+        shape, as LSDDetectorC::detect's mask argument (plf_detect_lines_masked): a line is dropped when both its end
+        points fall on 0; None detects everywhere (plf_detect_lines)."""
         img = _u8(img)
         h, w = img.shape
         kl = np.zeros(cap, KEYLINE_DTYPE)
         desc = np.zeros((cap, 32), np.uint8)
         n = C.c_int(0)
-        st = self.lib.plf_detect_lines(self._ctx, _ptr(img, C.c_uint8), w, h, img.strides[0],
-                                       kl.ctypes.data_as(C.c_void_p), _ptr(desc, C.c_uint8), cap, C.byref(n))
-        self._check(st, "plf_detect_lines")
+        if mask is None:
+            st = self.lib.plf_detect_lines(self._ctx, _ptr(img, C.c_uint8), w, h, img.strides[0],
+                                           kl.ctypes.data_as(C.c_void_p), _ptr(desc, C.c_uint8), cap, C.byref(n))
+            self._check(st, "plf_detect_lines")
+        else:
+            m = self._mask(mask, h, w, "detect_lines")
+            st = self.lib.plf_detect_lines_masked(self._ctx, _ptr(img, C.c_uint8), w, h, img.strides[0],
+                                                  _ptr(m, C.c_uint8), m.strides[0], kl.ctypes.data_as(C.c_void_p),
+                                                  _ptr(desc, C.c_uint8), cap, C.byref(n))
+            self._check(st, "plf_detect_lines_masked")
         return kl[:n.value].copy(), desc[:n.value].copy()
 
     def debug_sincosf(self, x):
@@ -1270,6 +1287,33 @@ class Frontend:
         self._check(self.lib.plf_set_sequence_rectification(self._ctx, int(s), _ptr(m1l, C.c_int16), _ptr(m2l, C.c_uint16),
                                                             _ptr(m1r, C.c_int16), _ptr(m2r, C.c_uint16)),
                     "plf_set_sequence_rectification")
+
+    @staticmethod
+    def _mask(mask, h, w, who):
+        """mask as a uint8 [h, w] array with unit column stride (rows may be strided)."""
+        m = np.asarray(mask)
+        if m.dtype != np.uint8 or m.shape != (h, w):
+            raise PlfError(f"{who}: mask must be uint8{[h, w]} (got {m.dtype}{list(m.shape)})")
+        return m if m.strides[1] == 1 and m.strides[0] >= w else np.ascontiguousarray(m)
+
+    def set_sequence_mask(self, s, left=None, right=None):
+        """Restricts sequence s's ORB and line detection in the batched pipeline to masks: uint8 [H, W] of the camera's
+        shape, in the geometry the detectors see (after rectification, one channel), non-zero = allowed.  None for an
+        image leaves it unmasked; both None clears them.  Batches already run keep their masks; s is not restarted.
+        plf_set_sequence_mask."""
+        H, W = self.camera.height, self.camera.width
+        ml = None if left is None else np.ascontiguousarray(self._mask(left, H, W, "set_sequence_mask"))
+        mr = None if right is None else np.ascontiguousarray(self._mask(right, H, W, "set_sequence_mask"))
+        self._check(self.lib.plf_set_sequence_mask(self._ctx, int(s), None if ml is None else _ptr(ml, C.c_uint8),
+                                                   None if mr is None else _ptr(mr, C.c_uint8), W),
+                    "plf_set_sequence_mask")
+
+    def sequence_mask_set(self, s):
+        """(left, right): whether sequence s has a mask on each image.  plf_get_sequence_mask_set."""
+        left, right = C.c_int(0), C.c_int(0)
+        self._check(self.lib.plf_get_sequence_mask_set(self._ctx, int(s), C.byref(left), C.byref(right)),
+                    "plf_get_sequence_mask_set")
+        return bool(left.value), bool(right.value)
 
     def set_adaptive_fast(self, cfg=None):
         """stvo-pl's adaptative_fast for the batched pipeline: a dict of min_th, max_th, inc_th, feat_th and err_th (the
