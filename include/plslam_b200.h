@@ -775,6 +775,27 @@ plf_status plf_batch_download(plf_ctx* ctx, int B, plf_frame_result* out);
  * earlier uploads left as they were. */
 plf_status plf_batch_upload_color(plf_ctx* ctx, int B, const uint8_t* left, const uint8_t* right, int stride, int channels);
 
+/* The image sizes the batched pipeline accepts besides the context's own (plf_create's camera), which it always accepts:
+ * wh holds n (width, height) pairs, 0 <= n <= 8; n = 0 restores the single-size context.  A batch is of one size, the
+ * size of the upload it runs; consecutive batches, and the batches in flight together, may be of different sizes.  A
+ * sequence takes its size from its camera (plf_set_sequence_camera).  Each pair's results are bit for bit those of that
+ * sequence alone on a context created at its size with its camera (DESIGN.md section 8).
+ *   - Valid only before the first plf_batch_* call (PLF_ERR_STATE after), like plf_set_max_sequences.
+ *   - Each size is checked as the pipeline checks the context's: every ORB level at least 2 orb_edge_th + 8 pixels wide
+ *     and high, below 4096 pixels, and an LSD scaled size inside the kernels' limits.  PLF_ERR_INVALID, naming the size
+ *     and what it fails, for a size that does not pass, for n out of range, or when a sequence has a camera of a size
+ *     the new list lacks; nothing changes on a refusal.  A size equal to the context's or repeated is accepted once.
+ *   - Device memory: every buffer of the pipeline is sized for the largest requirement over the sizes, so a context of
+ *     sizes within a few per cent in area takes about what a context of the largest one takes. */
+plf_status plf_set_image_sizes(plf_ctx* ctx, int n, const int32_t* wh);
+/* plf_batch_upload (channels 1) or plf_batch_upload_color (3 = BGR, 4 = BGRA) of B pairs of w x h images, a size the
+ * context accepts (plf_create's or one of plf_set_image_sizes').  The protocol, the landing buffer and the refusals are
+ * theirs; an undeclared size is refused (PLF_ERR_INVALID, listing the accepted sizes) with nothing changed.  The run
+ * that consumes the upload refuses a pair whose sequence is of another size.  plf_batch_upload and
+ * plf_batch_upload_color upload the context's size. */
+plf_status plf_batch_upload_sized(plf_ctx* ctx, int B, int w, int h, const uint8_t* left, const uint8_t* right, int stride,
+                                  int channels);
+
 /* Number of sequences a context can track at once (default 1), 1 <= n <= 2^20.  Call it before the first plf_batch_* call:
  * PLF_ERR_STATE once the pipeline exists, PLF_ERR_INVALID for n out of range.  Each sequence keeps one carried frame slot
  * on the device (84 * max_keypoints + 156 * max_lines + 8 bytes). */
@@ -789,11 +810,17 @@ plf_status plf_set_max_sequences(plf_ctx* ctx, int n);
  * Invalid arguments return PLF_ERR_INVALID before anything is enqueued, and no sequence state changes.
  * plf_batch_run(ctx, B) is plf_batch_run_sequences(ctx, B, NULL, NULL); plf_reset_sequence forgets every sequence's
  * previous frame.  Results, plf_get_frame(k) and plf_get_matches(k) stay indexed by pair k of the batch. */
+/* A batch is of one image size: a pair whose sequence's camera (plf_set_sequence_camera) is of another size than the upload
+ * the run consumes is refused, naming the pair, the sequence and both sizes (PLF_ERR_INVALID, before anything is
+ * enqueued). */
 plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, const uint8_t* restart);
 /* The calibration of sequence s, 0 <= s < n (plf_set_max_sequences).  The sequences of one context may differ in fx, fy,
- * cx, cy and b; they share the image size, the parameters and the limits.  cam == NULL returns s to the context's camera
- * (plf_create).  cam->width and cam->height must equal the context's; fx, fy and b must be finite and > 0; cx and cy must
- * be finite.  Anything else returns PLF_ERR_INVALID, naming the field, and changes nothing.  The call may be made at any
+ * cx, cy and b, and in the image size among the sizes the context accepts (plf_set_image_sizes); they share the
+ * parameters and the limits.  cam == NULL returns s to the context's camera (plf_create).  Without declared sizes
+ * cam->width and cam->height must equal the context's; with them, (cam->width, cam->height) must be one of the accepted
+ * sizes (the refusal lists them).  fx, fy and b must be finite and > 0; cx and cy must be finite.  A change of s's size
+ * while s has rectification maps or masks, which were built for its old size, is refused, naming them: clear them first.
+ * Anything else returns PLF_ERR_INVALID, naming the field, and changes nothing.  The call may be made at any
  * time: before or after the pipeline exists, and with batches in flight.
  *   - The camera is resolved when a batch is run, like restart flags and sequence state.  Batches already run keep the
  *     calibration they were run with; the next plf_batch_run_sequences that holds s uses the new one, for every pair of
@@ -814,7 +841,7 @@ plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out);
 /* Rectification of sequence s's raw pairs before extraction: stvo-pl's dataset reader
  * cv::remap(img, out, map1, map2, INTER_LINEAR) with the default BORDER_CONSTANT 0, per image.  map1_*: w x h x 2 int16
  * (x, y) and map2_*: w x h uint16, as cv::initUndistortRectifyMap(..., CV_16SC2) or cv::convertMaps give them, for the
- * context's w x h (host arrays, copied).  All four NULL clears it.  The camera of the rectified images (P1's fx, fy, cx, cy
+ * sequence's w x h (its camera's, plf_set_sequence_camera; host arrays, copied).  All four NULL clears it.  The camera of the rectified images (P1's fx, fy, cx, cy
  * and the baseline) is the caller's to set with plf_set_sequence_camera.
  *   - map2 is read as OpenCV reads it, map2 & 1023; map1 may point anywhere: taps outside the image read 0.  The result is
  *     byte for byte cv::remap's (DESIGN.md section 8).
@@ -839,8 +866,9 @@ plf_status plf_set_sequence_rectification(plf_ctx* ctx, int s, const int16_t* ma
 
 /* Restricts the batched pipeline's ORB and line detection on sequence s's left / right images to masks, as
  * plf_orb_masked and plf_detect_lines_masked do (the masks the detectors' mask arguments take; stvo-pl passes none).
- * mask_l, mask_r: w x h uint8 (host arrays, copied), stride bytes per row, in the geometry the detectors see: after
- * rectification for a rectified sequence, one channel for colour input.  Both NULL clears them; one NULL masks only the
+ * mask_l, mask_r: w x h uint8 (host arrays, copied), stride bytes per row, of the sequence's image size (its camera's,
+ * plf_set_sequence_camera), in the geometry the detectors see: after rectification for a rectified sequence, one channel
+ * for colour input.  The ORB pyramid of a mask is built in its size's level layout.  Both NULL clears them; one NULL masks only the
  * other image.
  *   - Each mask's ORB pyramid is built on the device once, by this call.  Extraction then reads it: features under the mask
  *     never reach the per-level retainBest, the line top-K, stereo association, tracking or the pose.
@@ -917,10 +945,28 @@ plf_status plf_debug_motion_prior(plf_ctx* ctx, int n, const double* DT, const d
  * until plf_batch_download. */
 plf_status plf_batch_device_poses(plf_ctx* ctx, int B, double* dst_device, void* stream);
 /* Device buffer [2*max_batch][h][pitch] read by plf_batch_run (image 2k = left k, 2k+1 = right k), pitch = width rounded up
- * to a multiple of 16 bytes (every halo tile of every image is then a legal TMA box).  It is the slot of the most recent
+ * to a multiple of 16 bytes (every halo tile of every image is then a legal TMA box); h, w and pitch are those of the
+ * most recent upload's image size (plf_batch_device_layout).  It is the slot of the most recent
  * upload; once that upload has been run, the pairs of rectified sequences (plf_set_sequence_rectification) in it are the
  * rectified images, and a colour upload (plf_batch_upload_color) is its grey conversion. */
 void* plf_batch_device_images(plf_ctx* ctx);
+/* The layout of plf_batch_device_images' slot: the width, height and row pitch of the most recent upload's images (the
+ * context's size before any upload; plf_batch_upload_sized uploads the others).  Image z starts pitch * h bytes after
+ * image z - 1.  PLF_ERR_INVALID for a NULL pointer. */
+plf_status plf_batch_device_layout(plf_ctx* ctx, int* w, int* h, int* pitch);
+
+/* What the front-end derives from an image size, as the library computes it (host only: needs no device or context):
+ * the 16-byte row pitch of the device images, the ORB pyramid's level sizes, the LSD scaled size and the windowed
+ * matcher's grid scales (64 / w, 48 / h).  params NULL = plf_default_params.  PLF_ERR_INVALID, with the reason in
+ * plf_last_error(NULL), for a size the pipeline would refuse (plf_set_image_sizes). */
+typedef struct plf_image_geometry {
+  int pitch;
+  int orb_nlevels;
+  int orb_w[8], orb_h[8];
+  int lsd_w, lsd_h;
+  double grid_iw, grid_ih;
+} plf_image_geometry;
+plf_status plf_get_image_geometry(const plf_params* params, int w, int h, plf_image_geometry* out);
 
 /* Stereo-valid features of frame k of the last batch (what `new KeyFrame(StVO->curr_frame)` deep-copies,
  * app/plslam_dataset.cpp:143, src/keyFrame.cpp:39-53). */

@@ -35,7 +35,7 @@ struct KfProb {
   int bf;             // the brute-force fallback can be taken (host upper bounds)
   int kmin;           // min_pt_matches / min_ls_matches
   int has_lm;         // the train features carry landmark indices (kf_*_lm): only those at -1 are train rows
-  KfCam cam;          // the problem's fx, fy, cx, cy; the context's image size and grid scales
+  KfCam cam;          // the problem's fx, fy, cx, cy; its sequence's image size and grid scales
   double T[16];       // DT / Twf, row-major
 };
 
@@ -393,8 +393,6 @@ plf_status run_kind(plf_ctx* ctx, const KindPlan& p, const KfKind& k, uint8_t* d
 // outputs of every problem (an inactive kind: 0 and every entry -1).
 plf_status kf_run(plf_ctx* ctx, bool map, const plf_kf_match_opts* o, const std::vector<HostProb>& hp) {
   const plf_params& P = ctx->params;
-  const plf_camera& cc = ctx->cam;
-  const double iw = PLF_GRID_COLS / (double)cc.width, ih = PLF_GRID_ROWS / (double)cc.height;
   KindPlan plan[2];
   StagedLayout L;
   for (int kd = 0; kd < 2; ++kd) {
@@ -410,7 +408,10 @@ plf_status kf_run(plf_ctx* ctx, bool map, const plf_kf_match_opts* o, const std:
       r.bf = r.nq > kmin && (map || r.nt > kmin);
       r.kmin = kmin;
       r.has_lm = h.host[kd].tlm != nullptr;
-      r.cam = {h.cam->fx, h.cam->fy, h.cam->cx, h.cam->cy, (double)cc.width, (double)cc.height, iw, ih};
+      // the grid and the visibility bounds of the problem's own image size (getWidth / getHeight, src/mapHandler.cpp:551)
+      const plf_camera& c = *h.cam;
+      r.cam = {c.fx, c.fy, c.cx, c.cy, (double)c.width, (double)c.height, PLF_GRID_COLS / (double)c.width,
+               PLF_GRID_ROWS / (double)c.height};
       memcpy(r.T, h.T, sizeof r.T);
       if (r.bf) {
         p.bfp.push_back((int)p.tab.size());

@@ -106,7 +106,8 @@ struct LsdState {
   int* overflow = nullptr;    // [1]
   int* rs_tab = nullptr;      // resize tables
   size_t rs_x_off = 0, rs_y_off = 0, rs_xp_off = 0;
-  DevBufList bufs;
+  DevBufList bufs;   // every buffer but rs_tab; empty in a state that borrows them (plf_lsd_create_sizes)
+  DevBufList tabs;   // rs_tab, the state's own
 };
 
 // ---- fixed-point Gaussian (ksize <= 15) ------------------------------------------------------------------
@@ -1144,6 +1145,7 @@ __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ se
 void plf_lsd_free(LsdState* s) {
   if (!s) return;
   s->bufs.release();
+  s->tabs.release();
   delete s;
 }
 
@@ -1217,16 +1219,20 @@ static void lsd_buffers(LsdState* s, DevBufList& b) {
     s->rs_x_off = 0;
     s->rs_y_off = 2 * (size_t)s->ws;
     s->rs_xp_off = (s->rs_y_off + 2 * (size_t)s->hs + 3) & ~(size_t)3;   // 16-byte aligned: read with 128-bit loads
-    b.add(s->rs_tab, s->rs_xp_off + plf_resize_packed_len(s->ws));
+    s->tabs.add(s->rs_tab, s->rs_xp_off + plf_resize_packed_len(s->ws));
   }
 }
 
-size_t plf_lsd_footprint(const plf_ctx* ctx, int w, int h, int nimg, bool two_parities) {
-  LsdState z;
-  lsd_set_sizes(ctx, &z, w, h, nimg, two_parities);
-  DevBufList b;
-  lsd_buffers(&z, b);
-  return b.bytes();
+size_t plf_lsd_footprint(const plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities) {
+  std::vector<LsdState> z(n);
+  size_t tabs = 0;
+  for (int i = 0; i < n; ++i) {
+    lsd_set_sizes(ctx, &z[i], wh[2 * i], wh[2 * i + 1], nimg, two_parities);
+    lsd_buffers(&z[i], z[i].bufs);
+    z[0].bufs.grow(z[i].bufs);
+    tabs += z[i].tabs.bytes();
+  }
+  return z[0].bufs.bytes() + tabs;
 }
 
 static plf_status lsd_tables_build(plf_ctx* ctx, LsdTables* t) {
@@ -1283,25 +1289,33 @@ void plf_lsd_tables_free(plf_ctx* ctx) {
   ctx->lsd_tables = nullptr;
 }
 
-static plf_status lsd_build(plf_ctx* ctx, LsdState* s, int w, int h, int nimg, bool two_parities) {
+// The sizes of s for nimg images of w x h, checked, and its buffers listed (not allocated).  Host only.
+static plf_status lsd_layout(plf_ctx* ctx, LsdState* s, int w, int h, int nimg, bool two_parities) {
   lsd_set_sizes(ctx, s, w, h, nimg, two_parities);
   if (s->ws >= 65536 || s->hs >= 65536 || s->ws < 3 || s->hs < 3)
     return plf_fail(ctx, PLF_ERR_INVALID, "LSD: scaled image %dx%d out of range", s->ws, s->hs);
+  lsd_buffers(s, s->bufs);
+  return PLF_OK;
+}
+
+plf_status plf_lsd_check_size(plf_ctx* ctx, int w, int h, int* ws, int* hs) {
+  LsdState s;
+  const plf_status st = lsd_layout(ctx, &s, w, h, 1, false);
+  if (!st && ws) { *ws = s.ws; *hs = s.hs; }
+  return st;
+}
+
+// s's own resize tables and record map pointers, once its buffers exist.
+static plf_status lsd_ready(plf_ctx* ctx, LsdState* s) {
   const double LOG_NT = 5 * (log10((double)s->ws) + log10((double)s->hs)) / 2 + log10(11.0);
   s->min_reg_size = (int)(size_t)(-LOG_NT / log10(ctx->lsd_tables->p));
-  lsd_buffers(s, s->bufs);
-  plf_status st = s->bufs.alloc(ctx, "LSD");
+  plf_status st = s->tabs.alloc(ctx, "LSD");
   if (st) return st;
-  for (int p = 0; p < (s->two_parities ? 2 : 1); ++p) {
-    s->pix[p] = s->pix_raw[p] + lsd_pix_pad(s);
-    k_lsd_fill_notdef<<<(unsigned)((lsd_pix_records(s) + 255) / 256), 256, 0, ctx->stream>>>(s->pix_raw[p], lsd_pix_records(s));
-    PLF_LAUNCH_CHECK(ctx);
-  }
-  PLF_CUDA(ctx, cudaMemsetAsync(s->overflow, 0, sizeof(int), ctx->stream));
+  for (int p = 0; p < (s->two_parities ? 2 : 1); ++p) s->pix[p] = s->pix_raw[p] + lsd_pix_pad(s);
   if (s->scale != 1.0) {
     std::vector<int> tab(s->rs_xp_off + plf_resize_packed_len(s->ws));
-    plf_linear_coeffs_host(w, s->ws, 1.0 / s->scale, &tab[0], &tab[s->ws]);
-    plf_linear_coeffs_host(h, s->hs, 1.0 / s->scale, &tab[s->rs_y_off], &tab[s->rs_y_off + s->hs]);
+    plf_linear_coeffs_host(s->w, s->ws, 1.0 / s->scale, &tab[0], &tab[s->ws]);
+    plf_linear_coeffs_host(s->h, s->hs, 1.0 / s->scale, &tab[s->rs_y_off], &tab[s->rs_y_off + s->hs]);
     plf_resize_pack_x(&tab[0], &tab[s->ws], s->ws, &tab[s->rs_xp_off]);
     PLF_CUDA(ctx, cudaMemcpyAsync(s->rs_tab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
   }
@@ -1309,16 +1323,45 @@ static plf_status lsd_build(plf_ctx* ctx, LsdState* s, int w, int h, int nimg, b
   return PLF_OK;
 }
 
-plf_status plf_lsd_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, LsdState** out) {
+// The states of n image sizes share one set of buffers, each sized for the largest of them.  Every record map is filled
+// with NOTDEF whole, guards and slack of every size's layout included; k_lsd_fill_notdef says why it stays so whichever
+// size the next batch has (DESIGN.md section 8).
+plf_status plf_lsd_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities, LsdState** out) {
   plf_status st = plf_lsd_tables(ctx);
   if (st) return st;
-  LsdState* s = new LsdState();
-  if ((st = lsd_build(ctx, s, w, h, nimg, two_parities))) {
-    plf_lsd_free(s);
+  std::vector<LsdState*> v(n, nullptr);
+  size_t records = 0;
+  for (int i = 0; i < n && !st; ++i) {
+    v[i] = new LsdState();
+    st = lsd_layout(ctx, v[i], wh[2 * i], wh[2 * i + 1], nimg, two_parities);
+    if (!st) records = std::max(records, lsd_pix_records(v[i]));
+  }
+  if (!st) {
+    for (int i = 1; i < n; ++i) v[0]->bufs.grow(v[i]->bufs);
+    st = v[0]->bufs.alloc(ctx, "LSD");
+  }
+  if (!st) {
+    for (int i = 1; i < n; ++i) v[0]->bufs.lend(v[i]->bufs);
+    for (int p = 0; p < (two_parities ? 2 : 1) && !st; ++p) {
+      k_lsd_fill_notdef<<<(unsigned)((records + 255) / 256), 256, 0, ctx->stream>>>(v[0]->pix_raw[p], records);
+      ctx->launches++;
+      if (cudaGetLastError() != cudaSuccess) st = plf_fail(ctx, PLF_ERR_CUDA, "LSD: filling the record maps failed");
+    }
+    if (!st && cudaMemsetAsync(v[0]->overflow, 0, sizeof(int), ctx->stream) != cudaSuccess)
+      st = plf_fail(ctx, PLF_ERR_CUDA, "LSD: clearing the overflow flag failed");
+  }
+  for (int i = 0; i < n && !st; ++i) st = lsd_ready(ctx, v[i]);
+  if (st) {
+    for (LsdState* s : v) plf_lsd_free(s);
     return st;
   }
-  *out = s;
+  std::copy(v.begin(), v.end(), out);
   return PLF_OK;
+}
+
+plf_status plf_lsd_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, LsdState** out) {
+  const int wh[2] = {w, h};
+  return plf_lsd_create_sizes(ctx, 1, wh, nimg, two_parities, out);
 }
 
 // LSD on images [0, n) of a batch resident on the device, in two phases so that callers can overlap them with other

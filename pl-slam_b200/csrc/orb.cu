@@ -78,7 +78,8 @@ struct OrbState {
   // is the caller's image buffer
   CUtensorMap tm_fast[ORB_MAX_LEVELS], tm_blur[ORB_MAX_LEVELS];
   PlfTmaCache tm_fast0, tm_blur0;
-  DevBufList bufs;
+  DevBufList bufs;   // every buffer but rs_tab; empty in a state that borrows them (plf_orb_create_sizes)
+  DevBufList tabs;   // rs_tab, the state's own
 };
 
 // ---- pyramid ---------------------------------------------------------------------------------------
@@ -668,10 +669,13 @@ void plf_linear_coeffs_host(int srcsize, int dstsize, double scale, int* ofs, in
 void plf_orb_free(OrbState* s) {
   if (!s) return;
   s->bufs.release();
+  s->tabs.release();
   delete s;
 }
 
-static plf_status orb_build(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, bool two_parities) {
+// The geometry of s for nimg images of w x h, its buffers listed in s->bufs and s->tabs (not allocated) and its resize
+// tables in tab.  Host only.
+static plf_status orb_layout(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, bool two_parities, std::vector<int>& tab) {
   const plf_params& P = ctx->params;
   if (P.orb_nlevels < 1 || P.orb_nlevels > ORB_MAX_LEVELS || P.orb_wta_k != 2 || P.orb_score != 1 ||
       P.orb_patch_size != 31)
@@ -749,7 +753,7 @@ static plf_status orb_build(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, b
     }
   }
   // resize tables
-  std::vector<int> tab;
+  tab.clear();
   for (int l = 1; l < g.nlevels; ++l) {
     const int sw = g.w[l - 1], sh = g.h[l - 1], dw = g.w[l], dh = g.h[l];
     s->rs_x_off[l] = tab.size();
@@ -770,7 +774,6 @@ static plf_status orb_build(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, b
   b.add(s->cand, cand * N);
   b.add(s->cand_count, N * ORB_MAX_LEVELS);
   b.add(s->hist, N * ORB_MAX_LEVELS * 256);
-  b.add(s->rs_tab, std::max<size_t>(tab.size(), 1));
   for (int p = 0; p < (two_parities ? 2 : 1); ++p) {  // outputs exist per batch parity (read by the match phase of batch i
     b.add(s->kps[p], N * M);                           // while batch i+1 is being extracted)
     b.add(s->kp_lxy[p], N * M);
@@ -779,30 +782,66 @@ static plf_status orb_build(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, b
   }
   b.add(s->overflow, 1);
   b.add(s->trig, N * M);
-  plf_status st = b.alloc(ctx, "ORB");
+  s->tabs.add(s->rs_tab, std::max<size_t>(tab.size(), 1));
+  return PLF_OK;
+}
+
+// s's own resize tables and the tensor maps of its pyramid levels, once its buffers exist.
+static plf_status orb_ready(plf_ctx* ctx, OrbState* s, const std::vector<int>& tab) {
+  const OrbGeom& g = s->g;
+  plf_status st = s->tabs.alloc(ctx, "ORB");
   if (st) return st;
-  PLF_CUDA(ctx, cudaMemsetAsync(s->overflow, 0, sizeof(int), ctx->stream));
   if (!tab.empty())
     PLF_CUDA(ctx, cudaMemcpyAsync(s->rs_tab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   // tensor maps of the pyramid levels (fixed addresses); level 0 = the caller's image buffer, cached per run
   for (int l = 1; l < g.nlevels; ++l) {
-    if (!plf_tma_encode_u8(&s->tm_fast[l], s->pyr + g.pyr_off[l], g.w[l], g.h[l], nimg, g.pitch[l], g.pyr_stride, 96, 38) ||
-        !plf_tma_encode_u8(&s->tm_blur[l], s->pyr + g.pyr_off[l], g.w[l], g.h[l], nimg, g.pitch[l], g.pyr_stride, 80, OBF_TH + 6))
+    if (!plf_tma_encode_u8(&s->tm_fast[l], s->pyr + g.pyr_off[l], g.w[l], g.h[l], s->nimg, g.pitch[l], g.pyr_stride, 96, 38) ||
+        !plf_tma_encode_u8(&s->tm_blur[l], s->pyr + g.pyr_off[l], g.w[l], g.h[l], s->nimg, g.pitch[l], g.pyr_stride, 80, OBF_TH + 6))
       return plf_fail(ctx, PLF_ERR_CUDA, "ORB: cuTensorMapEncodeTiled failed for pyramid level %d", l);
   }
   return PLF_OK;
 }
 
-plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, OrbState** out) {
-  OrbState* s = new OrbState();
-  const plf_status st = orb_build(ctx, s, w, h, nimg, two_parities);
+plf_status plf_orb_check_size(plf_ctx* ctx, int w, int h, int* nlevels, int* lw, int* lh) {
+  OrbState s;
+  std::vector<int> tab;
+  const plf_status st = orb_layout(ctx, &s, w, h, 1, false, tab);
+  if (st || !nlevels) return st;
+  *nlevels = s.g.nlevels;
+  for (int l = 0; l < s.g.nlevels; ++l) { lw[l] = s.g.w[l]; lh[l] = s.g.h[l]; }
+  return PLF_OK;
+}
+
+plf_status plf_orb_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities, OrbState** out) {
+  std::vector<OrbState*> v(n, nullptr);
+  std::vector<std::vector<int>> tabs(n);
+  plf_status st = PLF_OK;
+  for (int i = 0; i < n && !st; ++i) {
+    v[i] = new OrbState();
+    st = orb_layout(ctx, v[i], wh[2 * i], wh[2 * i + 1], nimg, two_parities, tabs[i]);
+  }
+  if (!st) {
+    for (int i = 1; i < n; ++i) v[0]->bufs.grow(v[i]->bufs);
+    st = v[0]->bufs.alloc(ctx, "ORB");
+  }
+  if (!st) {
+    for (int i = 1; i < n; ++i) v[0]->bufs.lend(v[i]->bufs);
+    if (cudaMemsetAsync(v[0]->overflow, 0, sizeof(int), ctx->stream) != cudaSuccess)
+      st = plf_fail(ctx, PLF_ERR_CUDA, "ORB: clearing the overflow flag failed");
+  }
+  for (int i = 0; i < n && !st; ++i) st = orb_ready(ctx, v[i], tabs[i]);
   if (st) {
-    plf_orb_free(s);
+    for (OrbState* s : v) plf_orb_free(s);
     return st;
   }
-  *out = s;
+  std::copy(v.begin(), v.end(), out);
   return PLF_OK;
+}
+
+plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, OrbState** out) {
+  const int wh[2] = {w, h};
+  return plf_orb_create_sizes(ctx, 1, wh, nimg, two_parities, out);
 }
 
 // Runs ORB on nimg (<= s->nimg) images of s->w x s->h resident at d_imgs ([nimg][h][pitch], pitch a multiple of 16,

@@ -81,9 +81,20 @@ struct SeqRecord {
   int th;
 };
 
-struct PipeState {
-  int w = 0, h = 0, B = 0, max_kp = 0, max_ln = 0;
+// One image size of the pipeline (plf_set_image_sizes; record 0 is the context's size), built once by pipe_build: its
+// row pitch, and ORB and LSD states of its own geometry, tables and tensor maps over buffers that every size shares
+// (plf_orb_create_sizes, plf_lsd_create_sizes).  A batch runs every phase with the record of its upload's size.
+struct PipeGeo {
+  int w = 0, h = 0;
   int pitch = 0;               // row pitch of the device images: plf_pitch16(w) (16-byte rows: every halo tile is a legal TMA box)
+  OrbState* orb = nullptr;     // ORB of 2B images, outputs per batch parity
+  LsdState* lsd = nullptr;     // LSD of 2B images, hand-off buffers per batch parity if lsd2
+  PlfTmaCache lbd_tm;          // tensor maps of the LBD gradient prelude over imgs2
+};
+
+struct PipeState {
+  int B = 0, max_kp = 0, max_ln = 0;
+  std::vector<PipeGeo> geo;    // [1 + plf_ctx::image_sizes / 2], in plf_image_size_index's order
   // Sequences: frame slots 0 .. B-1 hold the pairs of the running batch, B + s carries sequence s's last frame and
   // B + nseq is a slot whose counts stay 0, the "previous frame" of a first frame.
   int nseq = 1;
@@ -97,17 +108,16 @@ struct PipeState {
   uint8_t* h_tab[3] = {nullptr, nullptr, nullptr};
   uint8_t* tab = nullptr;
   cudaEvent_t ev_tab[3] = {nullptr, nullptr, nullptr};
+  // Every image buffer holds 2B images of any of the sizes, laid out at that size's h and pitch.
   uint8_t* imgs2[2] = {nullptr, nullptr};  // double-buffered [2B][h][pitch]: upload of batch i+1 overlaps the run of batch i
   uint8_t* stage = nullptr;    // dense [2B][h][w] landing buffer of the H2D copy (one contiguous DMA per side), repacked to the padded pitch on the device
   int up_slot = 0;             // slot written by the last plf_batch_upload
+  int up_geo = 0;              // size (geo record) of the last upload
   // channels of the last upload: 1 for plf_batch_upload (its images are in imgs2[up_slot]), 3 or 4 for
   // plf_batch_upload_color (its images are in the colour landing buffer until the run converts them into imgs2[up_slot])
   int up_ch = 1;
   cudaStream_t copy = nullptr; // H2D stream
   cudaEvent_t ev_up[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr}, ev_free2[2] = {nullptr, nullptr};
-  OrbState* orb = nullptr;     // ORB of 2B images, outputs per batch parity
-  LsdState* lsd = nullptr;     // LSD of 2B images, hand-off buffers per batch parity if lsd2
-  PlfTmaCache lbd_tm;          // tensor maps of the LBD gradient prelude over imgs2
   short2* lbd_grad[2] = {nullptr, nullptr};  // [parity][2B][h*w]
   uint8_t* ldesc_raw = nullptr;  // [2B][max_ln][32]  LBD of every kept KeyLine
   FrameSlots fs;               // B + nseq + 1 slots
@@ -161,16 +171,23 @@ struct PipeState {
   cudaEvent_t tE0[2] = {nullptr, nullptr}, tG0[2] = {nullptr, nullptr}, tM0[3] = {nullptr, nullptr, nullptr};  // phase starts (timeline)
   long long seq = 0;            // batches issued
   int pend_slot[3] = {0, 0, 0}, pend_B[3] = {0, 0, 0}, n_pending = 0;
+  int rp_geo[3] = {0, 0, 0};    // size (geo record) of the batch in each slot of the result ring
   DevBufList bufs;
+  // the largest image of any size: pixels w h, and bytes pitch h
+  size_t max_area() const { size_t a = 0; for (const PipeGeo& g : geo) a = std::max(a, (size_t)g.w * g.h); return a; }
+  size_t max_image() const { size_t a = 0; for (const PipeGeo& g : geo) a = std::max(a, (size_t)g.pitch * g.h); return a; }
 };
 
 // The device buffers of the pipeline for B pairs of K keypoints / Ln lines per image.
+// Image buffers are sized for the largest image of any size.
 static void pipe_buffers(PipeState* s, bool windowed, DevBufList& b) {
-  const size_t B = s->B, K = s->max_kp, Ln = s->max_ln, A = (size_t)s->w * s->h, AP = (size_t)s->pitch * s->h;
+  const size_t B = s->B, K = s->max_kp, Ln = s->max_ln, A = s->max_area(), AP = s->max_image();
   const size_t S = B + s->nseq + 1;   // frame slots, carry slots, the empty slot
   b.add(s->imgs2[0], 2 * B * AP);
   b.add(s->imgs2[1], 2 * B * AP);
-  if (s->pitch != s->w) b.add(s->stage, 2 * B * A);
+  bool padded = false;   // a size's rows are padded: its dense uploads land in stage
+  for (const PipeGeo& g : s->geo) padded |= g.pitch != g.w;
+  if (padded) b.add(s->stage, 2 * B * A);
   b.add(s->lbd_grad[0], 2 * B * A);
   b.add(s->lbd_grad[1], 2 * B * A);
   b.add(s->ldesc_raw, 2 * B * Ln * 32);
@@ -222,8 +239,10 @@ static std::vector<PipeEvents> pipe_events(PipeState* s) {
 extern "C" void plf_pipe_free(plf_ctx* ctx) {
   PipeState* s = ctx->pipe;
   if (!s) return;
-  plf_orb_free(s->orb);
-  plf_lsd_free(s->lsd);
+  for (PipeGeo& g : s->geo) {
+    plf_orb_free(g.orb);
+    plf_lsd_free(g.lsd);
+  }
   s->bufs.release();
   for (int i = 0; i < 3; ++i) {
     if (s->h_results[i]) cudaFreeHost(s->h_results[i]);
@@ -756,7 +775,8 @@ __global__ void __launch_bounds__(256) k_mg_select(const int32_t* __restrict__ m
 // with LSD_PARITY_MARGIN to spare.  PLF_LSD_PARITIES = 1 or 2 forces either layout.
 #define LSD_PARITY_MARGIN (4ull << 30)   // room left for what is allocated after the pipeline is prepared (the standalone
                                          // operators' scratch, the caller's own buffers) and for allocation granularity
-static bool lsd_want_two_parities(const plf_ctx* ctx, int w, int h, int nimg) {
+// (the footprint of every image size's LSD state: one set of buffers, each the largest any size needs)
+static bool lsd_want_two_parities(const plf_ctx* ctx, int n, const int* wh, int nimg) {
   const char* e = getenv("PLF_LSD_PARITIES");
   if (e && *e) return atoi(e) >= 2;
   size_t free_b = 0, total_b = 0;
@@ -764,16 +784,23 @@ static bool lsd_want_two_parities(const plf_ctx* ctx, int w, int h, int nimg) {
     cudaGetLastError();
     return false;
   }
-  return plf_lsd_footprint(ctx, w, h, nimg, true) + LSD_PARITY_MARGIN <= free_b;
+  return plf_lsd_footprint(ctx, n, wh, nimg, true) + LSD_PARITY_MARGIN <= free_b;
 }
 
-static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
+static plf_status pipe_build(plf_ctx* ctx) {
   PipeState* s = ctx->pipe = new PipeState();
   const int B = ctx->limits.max_batch, K = ctx->limits.max_keypoints, Ln = ctx->limits.max_lines;
   if (Ln > K || K > 65535)
     return plf_fail(ctx, PLF_ERR_INVALID, "limits: need max_lines <= max_keypoints <= 65535 (got %d, %d)", Ln, K);
-  s->w = w; s->h = h; s->B = B; s->max_kp = K; s->max_ln = Ln;
-  s->pitch = plf_pitch16(w);
+  s->B = B; s->max_kp = K; s->max_ln = Ln;
+  std::vector<int> wh = {ctx->cam.width, ctx->cam.height};   // the sizes, in plf_image_size_index's order
+  wh.insert(wh.end(), ctx->image_sizes.begin(), ctx->image_sizes.end());
+  const int ngeo = (int)wh.size() / 2;
+  s->geo.resize(ngeo);
+  for (int i = 0; i < ngeo; ++i) {
+    s->geo[i].w = wh[2 * i]; s->geo[i].h = wh[2 * i + 1];
+    s->geo[i].pitch = plf_pitch16(wh[2 * i]);
+  }
   s->nseq = ctx->max_sequences;
   s->carried.assign(s->nseq, 0);
   s->last_pair.assign(s->nseq, -1);
@@ -795,10 +822,14 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
   PLF_CUDA(ctx, cudaMemsetAsync(f.pt_count, 0, nslots * sizeof(int), cs));
   PLF_CUDA(ctx, cudaMemsetAsync(f.ls_count, 0, nslots * sizeof(int), cs));
   // sub-systems sized for 2B images; the LSD tables come first, so that the parity decision sees the memory they take
-  if ((st = plf_orb_create(ctx, w, h, 2 * B, true, &s->orb))) return st;
+  std::vector<OrbState*> orb(ngeo, nullptr);
+  std::vector<LsdState*> lsd(ngeo, nullptr);
+  if ((st = plf_orb_create_sizes(ctx, ngeo, wh.data(), 2 * B, true, orb.data()))) return st;
+  for (int i = 0; i < ngeo; ++i) s->geo[i].orb = orb[i];
   if ((st = plf_lsd_tables(ctx))) return st;
-  s->lsd2 = lsd_want_two_parities(ctx, w, h, 2 * B);
-  if ((st = plf_lsd_create(ctx, w, h, 2 * B, s->lsd2, &s->lsd))) return st;
+  s->lsd2 = lsd_want_two_parities(ctx, ngeo, wh.data(), 2 * B);
+  if ((st = plf_lsd_create_sizes(ctx, ngeo, wh.data(), 2 * B, s->lsd2, lsd.data()))) return st;
+  for (int i = 0; i < ngeo; ++i) s->geo[i].lsd = lsd[i];
   // static problem descriptors over the pipeline's own buffers (pointers never change; counts are read on the device):
   // the stereo problems read the match phase's copies of the extraction outputs.  The frame-to-frame problems depend on
   // the batch's sequence table and are built on the device per batch (k_f2f_problems).
@@ -835,10 +866,11 @@ static plf_status pipe_build(plf_ctx* ctx, int w, int h) {
   return pipe_seq_reset(ctx, ctx->afast_on, ctx->motion_on);
 }
 
-// Builds the pipeline for the camera's image size on first use; a failed setup leaves no state behind.
+// Builds the pipeline for the camera's image size and the declared ones on first use; a failed setup leaves no state
+// behind.
 static plf_status pipe_prepare(plf_ctx* ctx) {
   if (ctx->pipe) return PLF_OK;
-  const plf_status st = pipe_build(ctx, ctx->cam.width, ctx->cam.height);
+  const plf_status st = pipe_build(ctx);
   if (st) plf_pipe_free(ctx);
   return st;
 }
@@ -846,6 +878,7 @@ static plf_status pipe_prepare(plf_ctx* ctx) {
 // One plf_batch_run call: its pairs, buffer parities and slots, and the streams of its phases.
 struct BatchRun {
   int B;
+  int g;         // the batch's image size: record s->geo[g], the size of the upload it consumes
   int ncarry;    // entries of the carry list in batch table rp: the sequences the batch holds
   bool cams;     // batch table rp holds the pairs' cameras (a sequence of the batch has its own); else the context's camera
   int nin;       // entries of the input table in batch table rp (0: none, every pair is converted as it is)
@@ -922,14 +955,15 @@ __global__ void __launch_bounds__(256) k_input(const PlfRectPair* __restrict__ t
   out[(size_t)blockIdx.z * AP + (size_t)y * pitch + x] = (uint8_t)(CH == 1 ? v[0] : bgr_gray(v[0], v[1], v[2]));
 }
 
-// The colour landing buffer of ch channels, [2 max_batch][h][w][ch] (image 2k = left k, 2k+1 = right k), carved from
+// The colour landing buffer of ch channels, [2 max_batch][h][w][ch] (image 2k = left k, 2k+1 = right k) at the largest
+// image size (any size's upload lands there), carved from
 // PLF_SCR_COLOR_PIPE.  Only the copy stream touches it: the uploads land there and the runs' conversions read it in call
 // order, so one buffer serves every batch in flight.  To grow (the first colour upload, or 4 channels after 3) the block
 // waits for the copy stream, and the new block is allocated before the old one is freed: a failed allocation leaves the
 // last upload as it was.
 static plf_status color_scratch(plf_ctx* ctx, PipeState* s, int ch, uint8_t** land) {
   DevBufList b;
-  b.add(*land, 2 * (size_t)s->B * s->h * s->w * ch);
+  b.add(*land, 2 * (size_t)s->B * s->max_area() * ch);
   size_t need = 0;
   for (const DevBufList::Entry& e : b.entries) need += plf_align256(e.bytes);
   DevBuf& slot = ctx->scratch[PLF_SCR_COLOR_PIPE];
@@ -959,8 +993,9 @@ static plf_status color_scratch(plf_ctx* ctx, PipeState* s, int ch, uint8_t** la
 static plf_status run_input(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   const bool color = s->up_ch > 1;
   if (!color && r.nin == 0) return PLF_OK;
-  const int w = s->w, h = s->h;
-  const size_t AP = (size_t)s->pitch * h;
+  const PipeGeo& G = s->geo[r.g];
+  const int w = G.w, h = G.h, pitch = G.pitch;
+  const size_t AP = (size_t)pitch * h;
   uint8_t* imgs = s->imgs2[r.run_slot];
   const PlfRectPair* tab = r.nin ? dev_tab(s, r.rp).in : nullptr;
   uint8_t* land = nullptr;    // colour: the landing buffer
@@ -969,7 +1004,7 @@ static plf_status run_input(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     if (plf_status st = color_scratch(ctx, s, s->up_ch, &land)) return st;
   } else {
     DevBufList b;
-    b.add(pairs, 2 * (size_t)s->B * AP);
+    b.add(pairs, 2 * (size_t)s->B * s->max_image());
     if (b.carve(ctx, PLF_SCR_RECT_PIPE)) return PLF_ERR_CUDA;
   }
   cudaStream_t cs = s->copy;
@@ -980,19 +1015,19 @@ static plf_status run_input(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   if (color) {
     const int row = s->up_ch * w;
     plf_mark(ctx, cs, "color.start");
-    if (s->up_ch == 3) k_input<3><<<grid, block, 0, cs>>>(tab, land, (size_t)row * h, row, w, h, AP, s->pitch, imgs);
-    else k_input<4><<<grid, block, 0, cs>>>(tab, land, (size_t)row * h, row, w, h, AP, s->pitch, imgs);
+    if (s->up_ch == 3) k_input<3><<<grid, block, 0, cs>>>(tab, land, (size_t)row * h, row, w, h, AP, pitch, imgs);
+    else k_input<4><<<grid, block, 0, cs>>>(tab, land, (size_t)row * h, row, w, h, AP, pitch, imgs);
     PLF_LAUNCH_CHECK(ctx);
     plf_mark(ctx, cs, "color.k_color");
   } else {
-    k_input<1><<<grid, block, 0, cs>>>(tab, imgs, AP, s->pitch, w, h, AP, s->pitch, pairs);
+    k_input<1><<<grid, block, 0, cs>>>(tab, imgs, AP, pitch, w, h, AP, pitch, pairs);
     PLF_LAUNCH_CHECK(ctx);
     // back in runs of consecutive pairs, w bytes of each row (the slot's row padding stays as the upload left it)
     const PlfRectPair* in = host_tab(s, r.rp).in;
     for (int j0 = 0, j1; j0 < r.nin; j0 = j1) {
       for (j1 = j0 + 1; j1 < r.nin && in[j1].pair == in[j1 - 1].pair + 1;) ++j1;
-      PLF_CUDA(ctx, cudaMemcpy2DAsync(imgs + 2 * (size_t)in[j0].pair * AP, (size_t)s->pitch, pairs + 2 * (size_t)j0 * AP,
-                                      (size_t)s->pitch, (size_t)w, 2 * (size_t)(j1 - j0) * h, cudaMemcpyDeviceToDevice, cs));
+      PLF_CUDA(ctx, cudaMemcpy2DAsync(imgs + 2 * (size_t)in[j0].pair * AP, (size_t)pitch, pairs + 2 * (size_t)j0 * AP,
+                                      (size_t)pitch, (size_t)w, 2 * (size_t)(j1 - j0) * h, cudaMemcpyDeviceToDevice, cs));
     }
   }
   PLF_CUDA(ctx, cudaEventRecord(s->ev_up[r.run_slot], cs));
@@ -1001,8 +1036,9 @@ static plf_status run_input(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
 
 // ---- E phase: ORB + LBD gradient prelude (bandwidth / ALU bound); outputs per batch parity ----
 static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
-  const int w = s->w, h = s->h, B = r.B, par = r.par;
-  const size_t A = (size_t)w * h, AP = (size_t)s->pitch * h;   // dense maps / padded images
+  PipeGeo& G = s->geo[r.g];
+  const int w = G.w, h = G.h, B = r.B, par = r.par;
+  const size_t A = (size_t)w * h, AP = (size_t)G.pitch * h;   // dense maps / padded images
   const uint8_t* imgs = s->imgs2[r.run_slot];
   cudaStream_t sE = r.sE;
   PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_up[r.run_slot], 0));  // images uploaded
@@ -1021,14 +1057,14 @@ static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     PLF_LAUNCH_CHECK(ctx);
     img_th = s->img_th;
   }
-  plf_status st = plf_orb_run(ctx, sE, s->orb, imgs, AP, s->pitch, 2 * B, par, img_th, masks);
-  if (!st) st = plf_launch_blur5_sobel(ctx, sE, &s->lbd_tm, imgs, s->pitch, AP, w, h, 2 * B, s->lbd_grad[par], A);
+  plf_status st = plf_orb_run(ctx, sE, G.orb, imgs, AP, G.pitch, 2 * B, par, img_th, masks);
+  if (!st) st = plf_launch_blur5_sobel(ctx, sE, &G.lbd_tm, imgs, G.pitch, AP, w, h, 2 * B, s->lbd_grad[par], A);
   if (st) return st;
   plf_mark(ctx, sE, "lbd.k_blur5_sobel");
-  // this batch's ORB overflow flag: snapshot + clear on the E stream, so that a flag raised by batch i+1's extraction is
-  // not reported on batch i's download
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp, plf_orb_overflow_flag(s->orb), sizeof(int), cudaMemcpyDeviceToDevice, sE));
-  PLF_CUDA(ctx, cudaMemsetAsync(plf_orb_overflow_flag(s->orb), 0, sizeof(int), sE));
+  // this batch's ORB overflow flag (one for every size): snapshot + clear on the E stream, so that a flag raised by batch
+  // i+1's extraction is not reported on batch i's download
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp, plf_orb_overflow_flag(G.orb), sizeof(int), cudaMemcpyDeviceToDevice, sE));
+  PLF_CUDA(ctx, cudaMemsetAsync(plf_orb_overflow_flag(G.orb), 0, sizeof(int), sE));
   PLF_CUDA(ctx, cudaEventRecord(s->evE[par], sE));
   PLF_CUDA(ctx, cudaEventRecord(s->ev_free[r.run_slot], sE));  // the image buffer may be overwritten by the next upload
   return PLF_OK;
@@ -1041,24 +1077,25 @@ static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
 // (region points, regions, segments) exist once either way: G(i+1) follows G(i) on its stream. ----
 static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   const int par = r.par;
-  const size_t AP = (size_t)s->pitch * s->h;
+  const PipeGeo& G = s->geo[r.g];
+  const size_t AP = (size_t)G.pitch * G.h;
   cudaStream_t sP = r.sP, sG = r.sG;
   PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_up[r.run_slot], 0));
   if (r.masked) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_tab[r.rp], 0));   // the mask table, read by G's KeyLine stage
   if (r.lsd2) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->evG[par], 0));   // batch i-2 (same parity) has finished growing / fitting on these maps
   PLF_CUDA(ctx, cudaEventRecord(s->tG0[par], sP));
-  plf_status st = plf_lsd_pre(ctx, sP, s->lsd, s->imgs2[r.run_slot], AP, s->pitch, r.lp, 2 * r.B);
+  plf_status st = plf_lsd_pre(ctx, sP, G.lsd, s->imgs2[r.run_slot], AP, G.pitch, r.lp, 2 * r.B);
   if (st) return st;
   PLF_CUDA(ctx, cudaEventRecord(s->ev_free2[r.run_slot], sP));
   PLF_CUDA(ctx, cudaEventRecord(s->evP[par], sP));
   PLF_CUDA(ctx, cudaStreamWaitEvent(sG, s->evP[par], 0));
   // the KeyLine outputs are overwritten: the match phase that read them last (batch i-2 with two parities, batch i-1 with one)
   // has taken its copy
-  st = plf_lsd_grow(ctx, sG, s->lsd, r.lp, 2 * r.B, r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr,
+  st = plf_lsd_grow(ctx, sG, G.lsd, r.lp, 2 * r.B, r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr,
                     r.masked ? dev_tab(s, r.rp).masks : nullptr);
   if (st) return st;
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp + 1, plf_lsd_overflow_flag(s->lsd), sizeof(int), cudaMemcpyDeviceToDevice, sG));
-  PLF_CUDA(ctx, cudaMemsetAsync(plf_lsd_overflow_flag(s->lsd), 0, sizeof(int), sG));
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp + 1, plf_lsd_overflow_flag(G.lsd), sizeof(int), cudaMemcpyDeviceToDevice, sG));
+  PLF_CUDA(ctx, cudaMemsetAsync(plf_lsd_overflow_flag(G.lsd), 0, sizeof(int), sG));
   PLF_CUDA(ctx, cudaEventRecord(s->evG[par], sG));
   return PLF_OK;
 }
@@ -1084,14 +1121,15 @@ static MgbArgs mgb_args(const plf_params& P, MgGrid g, bool lines, int cap, int 
 
 // ---- M phase: LBD, stereo association, frame-to-frame tracking, pose (needs the previous batch's M phase) ----
 static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
-  const int w = s->w, h = s->h, B = r.B, par = r.par, rp = r.rp;
+  const PipeGeo& G = s->geo[r.g];
+  const int w = G.w, h = G.h, B = r.B, par = r.par, rp = r.rp;
   const size_t A = (size_t)w * h;
   const int K = s->max_kp, Ln = s->max_ln;
   const plf_params& P = ctx->params;
   plf_keypoint* kps; uint8_t* odesc; int* kcnt; int mk;
   plf_keyline* kls; int* lcnt; int ml;
-  plf_orb_outputs(s->orb, par, &kps, &odesc, &kcnt, &mk);
-  plf_lsd_outputs(s->lsd, r.lp, &kls, &lcnt, &ml);
+  plf_orb_outputs(G.orb, par, &kps, &odesc, &kcnt, &mk);
+  plf_lsd_outputs(G.lsd, r.lp, &kls, &lcnt, &ml);
   cudaStream_t cs = r.sM;
   plf_status st;
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->evG[par], 0));
@@ -1246,6 +1284,14 @@ static plf_status upload_pairs(plf_ctx* ctx, cudaStream_t cs, uint8_t* dst, int 
   return PLF_OK;
 }
 
+// The image sizes the context accepts, its own first: "1242x375, 1226x370".
+static std::string image_size_list(const plf_ctx* ctx) {
+  std::string out = std::to_string(ctx->cam.width) + "x" + std::to_string(ctx->cam.height);
+  for (size_t i = 0; i < ctx->image_sizes.size(); i += 2)
+    out += ", " + std::to_string(ctx->image_sizes[i]) + "x" + std::to_string(ctx->image_sizes[i + 1]);
+  return out;
+}
+
 extern "C" {
 
 plf_status plf_reset_sequence(plf_ctx* ctx) {
@@ -1270,16 +1316,32 @@ plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam) {
   if (!ctx) return PLF_ERR_INVALID;
   if (plf_status st = plf_check_sequence(ctx, "plf_set_sequence_camera", s)) return st;
   if (cam) {
-    if (cam->width != ctx->cam.width)
-      return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: width = %d, the context's is %d", cam->width, ctx->cam.width);
-    if (cam->height != ctx->cam.height)
-      return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: height = %d, the context's is %d", cam->height, ctx->cam.height);
+    if (ctx->image_sizes.empty()) {
+      if (cam->width != ctx->cam.width)
+        return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: width = %d, the context's is %d", cam->width, ctx->cam.width);
+      if (cam->height != ctx->cam.height)
+        return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: height = %d, the context's is %d", cam->height, ctx->cam.height);
+    } else if (plf_image_size_index(ctx, cam->width, cam->height) < 0) {
+      return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: size %dx%d is not one of the context's image sizes (%s)",
+                      cam->width, cam->height, image_size_list(ctx).c_str());
+    }
     const struct { const char* name; double v; bool positive; } f[] = {
         {"fx", cam->fx, true}, {"fy", cam->fy, true}, {"cx", cam->cx, false}, {"cy", cam->cy, false}, {"b", cam->b, true}};
     for (const auto& e : f)
       if (!std::isfinite(e.v) || (e.positive && !(e.v > 0.0)))
         return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: %s = %g, need a finite value%s", e.name, e.v,
                         e.positive ? " > 0" : "");
+  }
+  // the maps and mask pyramids of s were built for its present size
+  const plf_camera& now = plf_sequence_camera(ctx, s);
+  const plf_camera& next = cam ? *cam : ctx->cam;
+  if ((next.width != now.width || next.height != now.height) && !ctx->seqs.empty()) {
+    const PlfSequence& o = ctx->seqs[s];
+    const bool maps = o.rect != nullptr, masks = o.mask[0] || o.mask[1];
+    if (maps || masks)
+      return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_camera: sequence %d has %s%s%s of %dx%d; clear %s before changing "
+                      "its image size to %dx%d", s, maps ? "rectification maps" : "", maps && masks ? " and " : "",
+                      masks ? "masks" : "", now.width, now.height, maps && masks ? "them" : "it", next.width, next.height);
   }
   PlfSequence& q = plf_sequence(ctx, s);
   q.own_cam = cam != nullptr;
@@ -1300,7 +1362,8 @@ plf_status plf_set_sequence_rectification(plf_ctx* ctx, int s, const int16_t* ma
   // the copy stream runs every rectification: once it is idle, no batch run so far reads sequence s's old maps
   cudaStream_t cs = ctx->pipe ? ctx->pipe->copy : ctx->stream;
   uint8_t* old = ctx->seqs.empty() ? nullptr : ctx->seqs[s].rect;
-  const size_t A = (size_t)ctx->cam.width * ctx->cam.height;
+  const plf_camera& sc = plf_sequence_camera(ctx, s);   // the maps are of the sequence's image size
+  const size_t A = (size_t)sc.width * sc.height;
   if (given) {
     uint8_t* d = old;
     if (!d) {
@@ -1333,18 +1396,18 @@ plf_status plf_set_sequence_rectification(plf_ctx* ctx, int s, const int16_t* ma
 plf_status plf_set_sequence_mask(plf_ctx* ctx, int s, const uint8_t* mask_l, const uint8_t* mask_r, int stride) {
   if (!ctx) return PLF_ERR_INVALID;
   if (plf_status st = plf_check_sequence(ctx, "plf_set_sequence_mask", s)) return st;
-  const int w = ctx->cam.width, h = ctx->cam.height;
+  const int w = plf_sequence_camera(ctx, s).width, h = plf_sequence_camera(ctx, s).height;   // the sequence's image size
   if ((mask_l || mask_r) && stride < w)
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_mask: stride = %d, need stride >= width = %d", stride, w);
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  // the new pyramids, built into fresh blocks on the main stream with the pipeline's ORB geometry (or, before the pipeline
-  // exists, that of a one-image ORB state of the same size and parameters)
+  // the new pyramids, built into fresh blocks on the main stream with the pipeline's ORB geometry of the sequence's size
+  // (or, before the pipeline exists, that of a one-image ORB state of the same size and parameters)
   uint8_t* fresh[2] = {nullptr, nullptr};
   if (mask_l || mask_r) {
     OrbState* tmp = nullptr;
     plf_status st = ctx->pipe ? PLF_OK : plf_orb_create(ctx, w, h, 1, false, &tmp);
     if (st) return st;
-    const OrbState* geo = ctx->pipe ? ctx->pipe->orb : tmp;
+    const OrbState* geo = ctx->pipe ? ctx->pipe->geo[plf_image_size_index(ctx, w, h)].orb : tmp;
     const size_t bytes = plf_orb_mask_bytes(geo) + 64;
     const uint8_t* src[2] = {mask_l, mask_r};
     for (int side = 0; side < 2 && !st; ++side) {
@@ -1496,46 +1559,38 @@ plf_status plf_debug_motion_prior(plf_ctx* ctx, int n, const double* DT, const d
   return PLF_OK;
 }
 
-plf_status plf_batch_upload(plf_ctx* ctx, int B, const uint8_t* left, const uint8_t* right, int stride) {
-  if (!ctx || !left || !right || B < 1 || B > ctx->limits.max_batch || stride < ctx->cam.width)
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload: bad arguments (B=%d, max_batch=%d)", B, ctx ? ctx->limits.max_batch : 0);
+// The grey pairs of an upload of image size s->geo[g] (arguments checked) into the slot the GPU is not reading.
+static plf_status upload_grey(plf_ctx* ctx, int g, int B, const uint8_t* left, const uint8_t* right, int stride) {
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
-  const int w = ctx->cam.width, h = ctx->cam.height;
   plf_status st = pipe_prepare(ctx);
   if (st) return st;
   PipeState* s = ctx->pipe;
+  const PipeGeo& G = s->geo[g];
+  const int w = G.w, h = G.h;
   // H2D on the copy stream into the slot the GPU is not reading, so the copy of batch i+1 overlaps the run of batch i.
   // Device layout interleaves the pair: image 2k = left k, 2k+1 = right k; rows are padded to a 16-byte pitch.
   const int slot = s->up_slot ^ 1;
   uint8_t* dst = s->imgs2[slot];
   PLF_CUDA(ctx, cudaStreamWaitEvent(s->copy, s->ev_free[slot], 0));   // the last run that read this slot has finished with it
   PLF_CUDA(ctx, cudaStreamWaitEvent(s->copy, s->ev_free2[slot], 0));  // (ORB / LBD prelude on one stream, LSD on another)
-  if (stride == w && s->stage) {
+  if (stride == w && G.pitch != w) {
     // densely packed input: ONE contiguous H2D copy per side into the dense landing buffer, then a device-to-device 2-D
     // copy widens the rows to the 16-byte pitch (the DMA engines move 1242-byte rows from host memory at a fraction of
     // the contiguous rate: measured 8.9 k vs 12.7 k pairs/s end to end)
     if ((st = upload_pairs(ctx, s->copy, s->stage, w, B, left, right, stride, w, h))) return st;
-    PLF_CUDA(ctx, cudaMemcpy2DAsync(dst, (size_t)s->pitch, s->stage, (size_t)w, (size_t)w, 2 * (size_t)B * h, cudaMemcpyDeviceToDevice, s->copy));
-  } else if ((st = upload_pairs(ctx, s->copy, dst, s->pitch, B, left, right, stride, w, h))) {   // pitch == w: dense rows
+    PLF_CUDA(ctx, cudaMemcpy2DAsync(dst, (size_t)G.pitch, s->stage, (size_t)w, (size_t)w, 2 * (size_t)B * h, cudaMemcpyDeviceToDevice, s->copy));
+  } else if ((st = upload_pairs(ctx, s->copy, dst, G.pitch, B, left, right, stride, w, h))) {   // pitch == w: dense rows
     return st;
   }
   PLF_CUDA(ctx, cudaEventRecord(s->ev_up[slot], s->copy));
   s->up_slot = slot;
   s->up_ch = 1;
+  s->up_geo = g;
   return PLF_OK;
 }
 
-plf_status plf_batch_upload_color(plf_ctx* ctx, int B, const uint8_t* left, const uint8_t* right, int stride, int channels) {
-  if (!ctx) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_batch_upload_color: ctx is NULL");
-  const int w = ctx->cam.width, h = ctx->cam.height;
-  if (channels != 3 && channels != 4)
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload_color: channels = %d, need 3 (BGR) or 4 (BGRA)", channels);
-  if (B < 1 || B > ctx->limits.max_batch)
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload_color: B = %d, need 1 <= B <= max_batch = %d", B, ctx->limits.max_batch);
-  if (!left || !right) return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload_color: left and right are required");
-  if ((long long)stride < (long long)channels * w)
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload_color: stride = %d, need at least channels * width = %d", stride,
-                    channels * w);
+// The colour pairs of an upload of image size s->geo[g] (arguments checked) into the landing buffer.
+static plf_status upload_color(plf_ctx* ctx, int g, int B, const uint8_t* left, const uint8_t* right, int stride, int channels) {
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   plf_status st = pipe_prepare(ctx);
   if (st) return st;
@@ -1544,17 +1599,118 @@ plf_status plf_batch_upload_color(plf_ctx* ctx, int B, const uint8_t* left, cons
   if ((st = color_scratch(ctx, s, channels, &land))) return st;
   // H2D on the copy stream into the landing buffer; the run converts it into the image slot the GPU is not reading.
   // Dense rows of ch w bytes are one contiguous block per image (no short-row DMA to avoid, unlike the grey path's stage).
-  const int row = channels * w;
-  if ((st = upload_pairs(ctx, s->copy, land, row, B, left, right, stride, row, h))) return st;
+  const int row = channels * s->geo[g].w;
+  if ((st = upload_pairs(ctx, s->copy, land, row, B, left, right, stride, row, s->geo[g].h))) return st;
   s->up_slot ^= 1;
   s->up_ch = channels;
+  s->up_geo = g;
   return PLF_OK;
+}
+
+// The refusals of the colour and sized uploads, fn naming the call: channels first when the call takes grey too.
+static plf_status check_upload(plf_ctx* ctx, const char* fn, int B, int w, const uint8_t* left, const uint8_t* right,
+                               int stride, int channels) {
+  if (B < 1 || B > ctx->limits.max_batch)
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: B = %d, need 1 <= B <= max_batch = %d", fn, B, ctx->limits.max_batch);
+  if (!left || !right) return plf_fail(ctx, PLF_ERR_INVALID, "%s: left and right are required", fn);
+  if ((long long)stride < (long long)channels * w)
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: stride = %d, need at least channels * width = %d", fn, stride, channels * w);
+  return PLF_OK;
+}
+
+plf_status plf_batch_upload(plf_ctx* ctx, int B, const uint8_t* left, const uint8_t* right, int stride) {
+  if (!ctx || !left || !right || B < 1 || B > ctx->limits.max_batch || stride < ctx->cam.width)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload: bad arguments (B=%d, max_batch=%d)", B, ctx ? ctx->limits.max_batch : 0);
+  return upload_grey(ctx, 0, B, left, right, stride);
+}
+
+plf_status plf_batch_upload_color(plf_ctx* ctx, int B, const uint8_t* left, const uint8_t* right, int stride, int channels) {
+  if (!ctx) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_batch_upload_color: ctx is NULL");
+  if (channels != 3 && channels != 4)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload_color: channels = %d, need 3 (BGR) or 4 (BGRA)", channels);
+  if (plf_status st = check_upload(ctx, "plf_batch_upload_color", B, ctx->cam.width, left, right, stride, channels)) return st;
+  return upload_color(ctx, 0, B, left, right, stride, channels);
+}
+
+plf_status plf_batch_upload_sized(plf_ctx* ctx, int B, int w, int h, const uint8_t* left, const uint8_t* right, int stride,
+                                  int channels) {
+  if (!ctx) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_batch_upload_sized: ctx is NULL");
+  if (channels != 1 && channels != 3 && channels != 4)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload_sized: channels = %d, need 1 (grey), 3 (BGR) or 4 (BGRA)", channels);
+  const int g = plf_image_size_index(ctx, w, h);
+  if (g < 0)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_upload_sized: size %dx%d is not one of the context's image sizes (%s)", w, h,
+                    image_size_list(ctx).c_str());
+  if (plf_status st = check_upload(ctx, "plf_batch_upload_sized", B, w, left, right, stride, channels)) return st;
+  return channels == 1 ? upload_grey(ctx, g, B, left, right, stride) : upload_color(ctx, g, B, left, right, stride, channels);
 }
 
 void* plf_batch_device_images(plf_ctx* ctx) {
   if (!ctx) return nullptr;
   if (pipe_prepare(ctx)) return nullptr;
   return ctx->pipe->imgs2[ctx->pipe->up_slot];
+}
+
+plf_status plf_batch_device_layout(plf_ctx* ctx, int* w, int* h, int* pitch) {
+  if (!ctx) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_batch_device_layout: ctx is NULL");
+  if (!w || !h || !pitch) return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_device_layout: w, h and pitch are required");
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (plf_status st = pipe_prepare(ctx)) return st;
+  const PipeGeo& G = ctx->pipe->geo[ctx->pipe->up_geo];
+  *w = G.w; *h = G.h; *pitch = G.pitch;
+  return PLF_OK;
+}
+
+plf_status plf_set_image_sizes(plf_ctx* ctx, int n, const int32_t* wh) {
+  if (!ctx) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_set_image_sizes: ctx is NULL");
+  if (ctx->pipe) return plf_fail(ctx, PLF_ERR_STATE, "plf_set_image_sizes: the pipeline exists (a batch call was made)");
+  if (n < 0 || n > PLF_MAX_IMAGE_SIZES)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_image_sizes: n = %d, need 0 <= n <= %d", n, PLF_MAX_IMAGE_SIZES);
+  if (n > 0 && !wh) return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_image_sizes: wh is NULL");
+  std::vector<int> sizes;
+  for (int i = 0; i < n; ++i) {
+    const int w = wh[2 * i], h = wh[2 * i + 1];
+    if (w <= 0 || h <= 0)
+      return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_image_sizes: size %d is %dx%d, need a positive width and height", i, w, h);
+    plf_status st = plf_orb_check_size(ctx, w, h);
+    if (!st) st = plf_lsd_check_size(ctx, w, h);
+    if (st) {
+      const std::string why = ctx->err;
+      return plf_fail(ctx, st, "plf_set_image_sizes: size %d (%dx%d): %s", i, w, h, why.c_str());
+    }
+    bool dup = w == ctx->cam.width && h == ctx->cam.height;
+    for (size_t j = 0; j < sizes.size(); j += 2) dup |= sizes[j] == w && sizes[j + 1] == h;
+    if (!dup) { sizes.push_back(w); sizes.push_back(h); }
+  }
+  // a sequence keeps its camera: its size stays one the context accepts
+  for (size_t q = 0; q < ctx->seqs.size(); ++q) {
+    const plf_camera& c = ctx->seqs[q].cam;
+    if (!ctx->seqs[q].own_cam || (c.width == ctx->cam.width && c.height == ctx->cam.height)) continue;
+    bool kept = false;
+    for (size_t j = 0; j < sizes.size(); j += 2) kept |= sizes[j] == c.width && sizes[j + 1] == c.height;
+    if (!kept)
+      return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_image_sizes: sequence %zu has a camera of %dx%d, which the new sizes do not "
+                      "hold; give it another camera first", q, c.width, c.height);
+  }
+  ctx->image_sizes = sizes;
+  return PLF_OK;
+}
+
+plf_status plf_get_image_geometry(const plf_params* params, int w, int h, plf_image_geometry* out) {
+  if (!out) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_get_image_geometry: out is NULL");
+  plf_ctx c;   // host only: the parameters and the limits are all the checks read
+  if (params) c.params = *params;
+  else plf_default_params(&c.params);
+  plf_default_limits(&c.limits);
+  memset(out, 0, sizeof *out);
+  plf_status st = w > 0 && h > 0 ? PLF_OK : plf_fail(&c, PLF_ERR_INVALID, "size %dx%d, need a positive width and height", w, h);
+  if (!st) st = plf_orb_check_size(&c, w, h, &out->orb_nlevels, out->orb_w, out->orb_h);
+  if (!st) st = plf_lsd_check_size(&c, w, h, &out->lsd_w, &out->lsd_h);
+  if (st) return plf_fail(nullptr, st, "plf_get_image_geometry: %s", c.err.c_str());
+  out->pitch = plf_pitch16(w);
+  out->grid_iw = PLF_GRID_COLS / (double)w;
+  out->grid_ih = PLF_GRID_ROWS / (double)h;
+  return PLF_OK;
 }
 
 plf_status plf_batch_run(plf_ctx* ctx, int B) { return plf_batch_run_sequences(ctx, B, nullptr, nullptr); }
@@ -1573,6 +1729,14 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   if (seq) s->pair_seq.assign(seq, seq + B);
   else s->pair_seq.assign(B, 0);
   const int* q = s->pair_seq.data();
+  // a batch is of one image size, its upload's
+  const PipeGeo& G = s->geo[s->up_geo];
+  for (int k = 0; k < B; ++k) {
+    const plf_camera& c = plf_sequence_camera(ctx, q[k]);
+    if (c.width != G.w || c.height != G.h)
+      return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_run_sequences: pair %d is of sequence %d, of %dx%d images, and the upload it "
+                      "runs is of %dx%d; a batch holds pairs of one image size", k, q[k], c.width, c.height, G.w, G.h);
+  }
   // pair k of a sequence is detected at the threshold pair k-1's pose gives, or starts from the prediction pair k-1's pose
   // gives: one pair per sequence
   if (ctx->afast_on || ctx->motion_on) {
@@ -1590,6 +1754,7 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   }
   BatchRun r;
   r.B = B;
+  r.g = s->up_geo;
   r.par = (int)(s->seq & 1);
   r.rp = (int)(s->seq % 3);
   // The batch's table, into its ring entry (the batch that used it last has been downloaded, and its input conversion
@@ -1656,6 +1821,7 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   if (st) return st;
   s->pend_slot[s->n_pending] = r.rp;
   s->pend_B[s->n_pending] = B;
+  s->rp_geo[r.rp] = r.g;
   s->n_pending++;
   s->seq++;
   return PLF_OK;
@@ -1679,8 +1845,9 @@ plf_status plf_batch_download(plf_ctx* ctx, int B, plf_frame_result* out) {
   const int o0 = ctx->params.has_points ? s->h_ovf[par][0] : 0, o1 = ctx->params.has_lines ? s->h_ovf[par][1] : 0;
   if (o0 || o1) {
     char why0[400] = "", why1[400] = "";
-    if (o0) plf_orb_overflow_text(s->orb, o0, why0, sizeof why0);
-    if (o1) plf_lsd_overflow_text(s->lsd, o1, why1, sizeof why1);
+    const PipeGeo& G = s->geo[s->rp_geo[par]];   // the capacities of the batch's own image size
+    if (o0) plf_orb_overflow_text(G.orb, o0, why0, sizeof why0);
+    if (o1) plf_lsd_overflow_text(G.lsd, o1, why1, sizeof why1);
     return plf_fail(ctx, PLF_ERR_CAPACITY, "plf_batch_download: a fixed-capacity buffer overflowed in this batch (%s%s%s%s%s)",
                     o0 ? "ORB keypoints: " : "", why0, o0 && o1 ? "; " : "", o1 ? "LSD segments/lines: " : "", why1);
   }

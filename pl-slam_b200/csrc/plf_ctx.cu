@@ -85,6 +85,15 @@ plf_status DevBufList::carve(plf_ctx* ctx, plf_scratch_slot slot) const {
   return PLF_OK;
 }
 
+void DevBufList::grow(const DevBufList& o) {
+  for (size_t i = 0; i < entries.size(); ++i) entries[i].bytes = std::max(entries[i].bytes, o.entries[i].bytes);
+}
+
+void DevBufList::lend(DevBufList& o) const {
+  for (size_t i = 0; i < entries.size(); ++i) *o.entries[i].ptr = *entries[i].ptr;
+  o.entries.clear();
+}
+
 plf_status StagedLayout::acquire(plf_ctx* ctx, plf_scratch_slot slot, uint8_t** pin, uint8_t** dev) const {
   *pin = (uint8_t*)plf_pinned(ctx, in + out);
   if (!*pin) return PLF_ERR_CUDA;

@@ -59,6 +59,11 @@ struct DevBufList {
   // Points every entry into one block of scratch slot `slot`, each at a 256-byte boundary.  On failure returns
   // PLF_ERR_CUDA (error set) and leaves the pointers untouched.
   plf_status carve(plf_ctx* ctx, plf_scratch_slot slot) const;
+  // Buffers shared by states of several image sizes (plf_orb_create_sizes, plf_lsd_create_sizes): o lists the same
+  // entries in the same order for another size.  Before alloc, grow takes each entry to the larger of the two sizes;
+  // after, lend points o's entries at these buffers and empties o, so that only this list frees them.
+  void grow(const DevBufList& o);
+  void lend(DevBufList& o) const;
 };
 
 // The staged layout of one call: the host inputs [0, in), the outputs [in, in + out) and the device-only work after them,
@@ -75,6 +80,8 @@ struct StagedLayout {
 
 // Upper bound of plf_set_max_sequences: keeps every slot index of the pipeline an int.
 #define PLF_MAX_SEQUENCES (1 << 20)
+// Upper bound of plf_set_image_sizes' n.
+#define PLF_MAX_IMAGE_SIZES 8
 
 struct OrbState;      // orb.cu
 struct LsdState;      // lsd.cu
@@ -103,6 +110,9 @@ struct plf_ctx {
   bool afast_on = false;          // plf_set_adaptive_fast: per-sequence FAST thresholds in the batched pipeline
   plf_adaptive_fast afast = {};
   bool motion_on = false;         // plf_set_motion_model: per-sequence pose predictions in the batched pipeline
+  // plf_set_image_sizes: (w, h) of each image size the batched pipeline accepts besides cam's, none equal to it or to
+  // another; fixed once the pipeline exists
+  std::vector<int> image_sizes;
   std::string err;
   long long launches = 0;
   // scratch slots (device) of the host-pointer operator entry points
@@ -137,6 +147,14 @@ inline PlfSequence& plf_sequence(plf_ctx* ctx, int s) {
 // The camera of sequence s (-1: the context's): its own calibration if it has one, else the context's.
 inline const plf_camera& plf_sequence_camera(const plf_ctx* ctx, int s) {
   return s >= 0 && !ctx->seqs.empty() && ctx->seqs[s].own_cam ? ctx->seqs[s].cam : ctx->cam;
+}
+// The index of image size w x h in the batched pipeline's list: 0 for the context's (cam), 1 + i for image_sizes' i-th,
+// -1 for a size it does not accept.
+inline int plf_image_size_index(const plf_ctx* ctx, int w, int h) {
+  if (w == ctx->cam.width && h == ctx->cam.height) return 0;
+  for (size_t i = 0; i < ctx->image_sizes.size(); i += 2)
+    if (ctx->image_sizes[i] == w && ctx->image_sizes[i + 1] == h) return 1 + (int)(i / 2);
+  return -1;
 }
 // Problem p of a batch call: its sequence to *s (seq NULL or seq[p] = -1: the context's) and that sequence's camera now
 // to *cam, each if given.  An entry outside [-1, max_sequences) returns PLF_ERR_INVALID naming fn, the problem and entry.
@@ -290,6 +308,12 @@ plf_status gbb_ldlt(plf_ctx* ctx, cudaStream_t cs, const GbbLdlt& L, int nb, int
 // A working state for up to nimg images of w x h, with outputs once or per batch parity (two_parities).  On failure
 // nothing is left allocated and *out is untouched.
 plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, OrbState** out);
+// out[i]: a state for images of size (wh[2i], wh[2i+1]), i < n.  They share one set of buffers, sized for the largest
+// requirement of any of the sizes and owned by out[0]; each has its own geometry, resize tables and tensor maps.  So
+// only one of them may run at a time, and out[0] is freed last or with the others.
+plf_status plf_orb_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities, OrbState** out);
+// What plf_orb_create would refuse for w x h, with its message, allocating nothing; the level sizes when nlevels is given.
+plf_status plf_orb_check_size(plf_ctx* ctx, int w, int h, int* nlevels = nullptr, int* lw = nullptr, int* lh = nullptr);
 void plf_orb_free(OrbState* s);
 // img_th: the FAST threshold of each image, on the device (plf_set_adaptive_fast), or NULL for plf_params.orb_fast_th.
 // masks: a device table of each image's mask pyramid (plf_orb_mask_build), an entry NULL for an unmasked image, or NULL
@@ -321,8 +345,13 @@ void plf_lsd_tables_free(plf_ctx* ctx);
 // A working state for up to nimg images of w x h, with the hand-off buffers once or per batch parity (two_parities).
 // On failure nothing is left allocated and *out is untouched.
 plf_status plf_lsd_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, LsdState** out);
+// n states of the sizes wh, sharing their buffers, as plf_orb_create_sizes.
+plf_status plf_lsd_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities, LsdState** out);
+// What plf_lsd_create would refuse for w x h, allocating nothing; the scaled size when ws is given.
+plf_status plf_lsd_check_size(plf_ctx* ctx, int w, int h, int* ws = nullptr, int* hs = nullptr);
 void plf_lsd_free(LsdState* s);
-size_t plf_lsd_footprint(const plf_ctx* ctx, int w, int h, int nimg, bool two_parities);   // bytes plf_lsd_create allocates
+// bytes plf_lsd_create_sizes allocates
+size_t plf_lsd_footprint(const plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities);
 plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int par, int n);
 // keylines_wait: if set, the KeyLine outputs are overwritten only after this event.  masks: as for plf_orb_run; the KeyLine
 // stage reads level 0 (plf_pitch16(w) bytes per row) of each listed image.

@@ -349,6 +349,24 @@ RESULT_DTYPE =np.dtype([("DT", np.float64, (4, 4)), ("DT_cov", np.float64, (6, 6
                          ("n_inliers_ls", np.int32), ("iters1", np.int32), ("iters2", np.int32)], align=True)
 assert RESULT_DTYPE.itemsize == C.sizeof(plf_frame_result)
 
+class plf_image_geometry(C.Structure):
+    _fields_ = [("pitch", C.c_int), ("orb_nlevels", C.c_int), ("orb_w", C.c_int * 8), ("orb_h", C.c_int * 8),
+                ("lsd_w", C.c_int), ("lsd_h", C.c_int), ("grid_iw", C.c_double), ("grid_ih", C.c_double)]
+
+
+def image_geometry(width, height, params=None):
+    """What the front-end derives from a width x height image, as the library computes it (host only, no device):
+    dict of pitch, orb_levels [(w, h) per ORB level], lsd_size (w, h) and grid_scale (64 / w, 48 / h).  params: a
+    plf_params (None: the defaults).  Raises PlfError for a size the pipeline refuses.  plf_get_image_geometry."""
+    lib = load_library()
+    g = plf_image_geometry()
+    st = lib.plf_get_image_geometry(None if params is None else C.byref(params), int(width), int(height), C.byref(g))
+    if st != 0:
+        raise PlfError(f"plf_get_image_geometry failed ({st}): {lib.plf_last_error(None).decode()}")
+    return dict(pitch=g.pitch, orb_levels=[(g.orb_w[l], g.orb_h[l]) for l in range(g.orb_nlevels)],
+                lsd_size=(g.lsd_w, g.lsd_h), grid_scale=(g.grid_iw, g.grid_ih))
+
+
 RESULT_FIELDS = ["status", "n_kp_l", "n_kp_r", "n_lines_l", "n_lines_r", "n_stereo_pt", "n_stereo_ls", "n_matched_pt",
                  "n_matched_ls", "n_inliers_pt", "n_inliers_ls", "iters1", "iters2"]
 
@@ -442,8 +460,10 @@ class Frontend:
 
     def __init__(self, params: plf_params | None = None, camera: dict | plf_camera | None = None,
                  limits: plf_limits | None = None, device: int = 0, max_sequences: int = 1,
-                 adaptive_fast: dict | None = None, motion_model: bool = False, **overrides):
+                 adaptive_fast: dict | None = None, motion_model: bool = False, image_sizes=None, **overrides):
         """max_sequences: the number of sequences batch_run / process_batch can track at once (plf_set_max_sequences).
+        image_sizes: None, or the (width, height) image sizes the batched pipeline accepts besides the camera's
+        (set_image_sizes).
         adaptive_fast: None, or the per-sequence FAST threshold adaptation as set_adaptive_fast takes it.
         motion_model: stvo-pl's use_motion_model (set_motion_model)."""
         self.lib = load_library()
@@ -458,12 +478,15 @@ class Frontend:
         self.camera = camera if isinstance(camera, plf_camera) else plf_camera(**camera)
         self.limits = limits if limits is not None else default_limits()
         self._ctx = C.c_void_p()
+        self.image_sizes = []
         st = self.lib.plf_create(C.byref(self.params), C.byref(self.camera), C.byref(self.limits),
                                  int(device), C.byref(self._ctx))
         if st != 0:
             raise PlfError(f"plf_create failed ({st}): {self.lib.plf_last_error(None).decode()}")
         try:
             self._check(self.lib.plf_set_max_sequences(self._ctx, int(max_sequences)), "plf_set_max_sequences")
+            if image_sizes:
+                self.set_image_sizes(image_sizes)
             if adaptive_fast is not None:
                 self.set_adaptive_fast(adaptive_fast)
             if motion_model:
@@ -1247,9 +1270,23 @@ class Frontend:
     def reset_sequence(self):
         self._check(self.lib.plf_reset_sequence(self._ctx), "plf_reset_sequence")
 
+    def set_image_sizes(self, sizes=()):
+        """The image sizes the batched pipeline accepts besides the camera's: (width, height) pairs, at most 8; an
+        empty list restores the single-size context.  A batch is of one size; a sequence takes its size from its camera
+        (set_sequence_camera).  Valid only before the first batch call.  plf_set_image_sizes."""
+        wh = np.ascontiguousarray(np.asarray(list(sizes), np.int32).reshape(-1, 2))
+        self._check(self.lib.plf_set_image_sizes(self._ctx, len(wh), _ptr(wh, C.c_int32) if len(wh) else None),
+                    "plf_set_image_sizes")
+        own = (self.camera.width, self.camera.height)
+        self.image_sizes = list(dict.fromkeys(tuple(int(v) for v in x) for x in wh if tuple(x) != own))
+
+    def _sizes_hw(self):
+        """Every accepted image size as (height, width), the camera's first."""
+        return [(self.camera.height, self.camera.width)] + [(h, w) for w, h in self.image_sizes]
+
     def set_sequence_camera(self, s, camera=None):
         """Gives sequence s its own calibration: a camera dict as Frontend(camera=...) takes, or a plf_camera, of the
-        context's width and height.  None returns s to the context's camera.  Either restarts s: its next pair in a run is
+        context's width and height or one of image_sizes.  None returns s to the context's camera.  Either restarts s: its next pair in a run is
         a first frame.  Batches already run keep their cameras.  plf_set_sequence_camera."""
         cam = None if camera is None else (camera if isinstance(camera, plf_camera) else plf_camera(**camera))
         self._check(self.lib.plf_set_sequence_camera(self._ctx, int(s), None if cam is None else C.byref(cam)),
@@ -1264,7 +1301,7 @@ class Frontend:
     def set_sequence_rectification(self, s, left=None, right=None):
         """Rectifies sequence s's raw pairs on the device before extraction, byte for byte cv::remap(img, map1, map2,
         INTER_LINEAR) with a constant 0 border.  left / right: (map1, map2) of that image, as cv2.initUndistortRectifyMap
-        (..., cv2.CV_16SC2, ...) returns them: map1 int16 [H, W, 2], map2 uint16 [H, W], for the camera's H x W.  Both None
+        (..., cv2.CV_16SC2, ...) returns them: map1 int16 [H, W, 2], map2 uint16 [H, W], for the sequence camera's H x W.  Both None
         clears the rectification.  Either restarts s; batches already run keep their maps.  The camera of the rectified
         images is set with set_sequence_camera.  plf_set_sequence_rectification."""
         if left is None and right is None:
@@ -1273,7 +1310,8 @@ class Frontend:
             return
         if left is None or right is None:
             raise PlfError("set_sequence_rectification: give the maps of both images, or neither to clear")
-        H, W = self.camera.height, self.camera.width
+        cam = self.sequence_camera(s)
+        H, W = cam["height"], cam["width"]
         maps = []
         for side, pair in (("left", left), ("right", right)):
             m1, m2 = pair
@@ -1297,11 +1335,12 @@ class Frontend:
         return m if m.strides[1] == 1 and m.strides[0] >= w else np.ascontiguousarray(m)
 
     def set_sequence_mask(self, s, left=None, right=None):
-        """Restricts sequence s's ORB and line detection in the batched pipeline to masks: uint8 [H, W] of the camera's
-        shape, in the geometry the detectors see (after rectification, one channel), non-zero = allowed.  None for an
-        image leaves it unmasked; both None clears them.  Batches already run keep their masks; s is not restarted.
-        plf_set_sequence_mask."""
-        H, W = self.camera.height, self.camera.width
+        """Restricts sequence s's ORB and line detection in the batched pipeline to masks: uint8 [H, W] of the sequence
+        camera's shape, in the geometry the detectors see (after rectification, one channel), non-zero = allowed.  None
+        for an image leaves it unmasked; both None clears them.  Batches already run keep their masks; s is not
+        restarted.  plf_set_sequence_mask."""
+        cam = self.sequence_camera(s)
+        H, W = cam["height"], cam["width"]
         ml = None if left is None else np.ascontiguousarray(self._mask(left, H, W, "set_sequence_mask"))
         mr = None if right is None else np.ascontiguousarray(self._mask(right, H, W, "set_sequence_mask"))
         self._check(self.lib.plf_set_sequence_mask(self._ctx, int(s), None if ml is None else _ptr(ml, C.c_uint8),
@@ -1379,27 +1418,34 @@ class Frontend:
 
     def _stack(self, left, right):
         """(left, right, channels): grey uint8 [B,H,W] (or [H,W]) with channels 1, or colour uint8 [B,H,W,C] (or
-        [H,W,C]), C = 3 (BGR) or 4 (BGRA), with channels C."""
+        [H,W,C]), C = 3 (BGR) or 4 (BGRA), with channels C.  H x W is the camera's size or one of image_sizes; any
+        other shape is refused here, before the library is called."""
         left = np.ascontiguousarray(left, np.uint8); right = np.ascontiguousarray(right, np.uint8)
-        hw = (self.camera.height, self.camera.width)
-        if left.ndim == 3 and left.shape[:2] == hw and left.shape[2] in (3, 4) and left.shape[1:] != hw:
+        sizes = self._sizes_hw()
+        if left.ndim == 3 and left.shape[:2] in sizes and left.shape[2] in (3, 4) and left.shape[1:] not in sizes:
             left, right = left[None], right[None]   # one colour pair
         if left.ndim == 4:
-            if not (left.shape == right.shape and left.shape[1:3] == hw and left.shape[3] in (3, 4)):
+            if not (left.shape == right.shape and left.shape[1:3] in sizes and left.shape[3] in (3, 4)):
+                hw = sizes[0] if len(sizes) == 1 else ("H", "W")
                 raise PlfError(f"colour images must be uint8 [B, {hw[0]}, {hw[1]}, 3 | 4] (BGR or BGRA), left and right "
-                               f"alike (got {list(left.shape)} and {list(right.shape)})")
+                               f"alike{self._sizes_text()} (got {list(left.shape)} and {list(right.shape)})")
             return left, right, left.shape[3]
         if left.ndim == 2:
             left, right = left[None], right[None]
-        assert left.shape == right.shape and left.shape[1:] == (self.camera.height, self.camera.width)
+        if not (left.ndim == 3 and left.shape == right.shape and left.shape[1:] in sizes):
+            raise PlfError(f"grey images must be uint8 [B, H, W], left and right alike{self._sizes_text()} "
+                           f"(got {list(left.shape)} and {list(right.shape)})")
         return left, right, 1
 
+    def _sizes_text(self):
+        return ", H x W one of " + ", ".join(f"{h} x {w}" for h, w in self._sizes_hw())
+
     def process_batch(self, left, right, seq=None, restart=None):
-        """B x (insertStereoPair + optimizePose): left/right uint8 [B,H,W] grey or [B,H,W,3|4] BGR / BGRA host arrays
-        -> list of result dicts.  seq / restart: as batch_run."""
+        """B x (insertStereoPair + optimizePose): left/right uint8 [B,H,W] grey or [B,H,W,3|4] BGR / BGRA host arrays,
+        H x W the camera's size or one of image_sizes -> list of result dicts.  seq / restart: as batch_run."""
         left, right, ch = self._stack(left, right)
         B = left.shape[0]
-        if seq is None and restart is None and ch == 1:
+        if seq is None and restart is None and ch == 1 and left.shape[1:3] == (self.camera.height, self.camera.width):
             res = (plf_frame_result * B)()
             st = self.lib.plf_process_batch(self._ctx, B, _ptr(left, C.c_uint8), _ptr(right, C.c_uint8),
                                             self.camera.width, res)
@@ -1412,9 +1458,14 @@ class Frontend:
 
     def batch_upload(self, left, right):
         """Uploads grey uint8 [B,H,W] pairs (plf_batch_upload) or BGR / BGRA uint8 [B,H,W,3|4] pairs, which the run
-        converts to grey on the device (plf_batch_upload_color).  Returns B."""
+        converts to grey on the device (plf_batch_upload_color).  Pairs of one of image_sizes go through
+        plf_batch_upload_sized.  Returns B."""
         left, right, ch = self._stack(left, right)
-        if ch == 1:
+        H, W = left.shape[1:3]
+        if (H, W) != (self.camera.height, self.camera.width):
+            self._check(self.lib.plf_batch_upload_sized(self._ctx, left.shape[0], int(W), int(H), _ptr(left, C.c_uint8),
+                                                        _ptr(right, C.c_uint8), ch * int(W), ch), "plf_batch_upload_sized")
+        elif ch == 1:
             self._check(self.lib.plf_batch_upload(self._ctx, left.shape[0], _ptr(left, C.c_uint8), _ptr(right, C.c_uint8),
                                                   self.camera.width), "plf_batch_upload")
         else:
@@ -1423,11 +1474,16 @@ class Frontend:
                         "plf_batch_upload_color")
         return left.shape[0]
 
-    def batch_upload_raw(self, B, left_ptr, right_ptr, channels=1, stride=None):
+    def batch_upload_raw(self, B, left_ptr, right_ptr, channels=1, stride=None, size=None):
         """Upload from raw host addresses (e.g. pinned memory): B images per side of H rows of `stride` bytes (None:
-        channels * W), grey (channels 1) or BGR / BGRA (3 / 4, plf_batch_upload_color)."""
-        stride = channels * self.camera.width if stride is None else int(stride)
-        if channels == 1:
+        channels * W), grey (channels 1) or BGR / BGRA (3 / 4, plf_batch_upload_color).  size: (W, H) of the images,
+        the camera's (None) or one of image_sizes (plf_batch_upload_sized)."""
+        W, H = (self.camera.width, self.camera.height) if size is None else (int(size[0]), int(size[1]))
+        stride = channels * W if stride is None else int(stride)
+        if (W, H) != (self.camera.width, self.camera.height):
+            self._check(self.lib.plf_batch_upload_sized(self._ctx, int(B), W, H, C.c_void_p(left_ptr), C.c_void_p(right_ptr),
+                                                        stride, int(channels)), "plf_batch_upload_sized")
+        elif channels == 1:
             self._check(self.lib.plf_batch_upload(self._ctx, int(B), C.c_void_p(left_ptr), C.c_void_p(right_ptr), stride),
                         "plf_batch_upload")
         else:
@@ -1474,6 +1530,13 @@ class Frontend:
     @property
     def device_images(self) -> int:
         return int(self.lib.plf_batch_device_images(self._ctx) or 0)
+
+    @property
+    def device_layout(self):
+        """(width, height, pitch) of device_images' slot: the most recent upload's size.  plf_batch_device_layout."""
+        w, h, p = C.c_int(0), C.c_int(0), C.c_int(0)
+        self._check(self.lib.plf_batch_device_layout(self._ctx, C.byref(w), C.byref(h), C.byref(p)), "plf_batch_device_layout")
+        return w.value, h.value, p.value
 
     def get_frame(self, k):
         """Stereo-valid features of frame k of the last batch (dict of numpy arrays)."""
