@@ -838,6 +838,40 @@ plf_status plf_set_sequence_camera(plf_ctx* ctx, int s, const plf_camera* cam);
 /* The calibration the next batch will use for sequence s: its own, or the context's camera. */
 plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out);
 
+/* Front-end settings of sequence s of the batched front-end (p == NULL: back to the context's plf_params), so that
+ * recordings of different pl-slam configs (config_kitti.yaml, config_euroc.yaml, ...) share one context.  The caller
+ * fills a whole plf_params from the sequence's config, as for plf_create.  plf_sequence_param_fields classifies the fields:
+ *   - PLF_PARAM_SEQUENCE fields may differ from the context's: orb_nfeatures, orb_fast_th, orb_nlevels, lsd_nfeatures,
+ *     min_line_length, best_lr_matches, max_dist_epip, min_disp, min_ratio_12_p, min_ratio_12_l, line_sim_th,
+ *     stereo_overlap_th, line_horiz_th, ls_min_disp_ratio, matching_strategy, matching_s_ws, matching_f2f_ws,
+ *     min_pt_matches, min_ls_matches, homog_th, min_features, max_iters, max_iters_ref, min_error, min_error_change.
+ *     Each int of them must be >= 0 and each float or double finite.  orb_nlevels must also be <= the context's (the
+ *     sequence detects on its first orb_nlevels levels with its own nfeaturesPerLevel split, as cv::ORB with that many
+ *     levels does).  matching_strategy != 0 is accepted only in a context created with matching_strategy != 0, whose
+ *     windowed buffers exist; a strategy-0 sequence in such a context takes the brute-force match() result for every pair.
+ *   - PLF_PARAM_CONTEXT fields must equal the context's: has_points, has_lines, orb_scale_factor, orb_edge_th, orb_wta_k,
+ *     orb_score, orb_patch_size and every other lsd_* field.  They fix buffer geometry, tables, tensor maps or which launch
+ *     chains exist.
+ *   - PLF_PARAM_IGNORED fields (inlier_k, f2f_overlap_th) are accepted and have no effect, as for the context.
+ * A refusal returns PLF_ERR_INVALID, naming the field, and changes nothing.  plf_create does not apply these range checks.
+ * The call may be made at any time: before or after the pipeline exists, and with batches in flight.
+ *   - The settings are resolved when a batch is run.  Batches already run keep the settings they were run with.
+ *   - A successful call restarts s, even with NULL or unchanged values: its next pair is a first frame (status 2), since
+ *     its carried frame was extracted and matched under the old settings.
+ *   - plf_set_max_sequences drops every sequence's settings; plf_reset_sequence keeps them.
+ *   - plf_batch_run and plf_process_batch run sequence 0 with sequence 0's settings.
+ *   - With plf_set_adaptive_fast, a sequence's first frame is detected at its own orb_fast_th.
+ * Only the batched front-end reads them.  The keyframe and back-end batch operators (plf_match_kf2kf_batch,
+ * plf_match_map2kf_batch, plf_gn_pose_batch, plf_local_ba_batch, plf_global_ba_batch, plf_loop_closure_pose_batch, ...)
+ * and every standalone operator keep using the context's plf_params. */
+plf_status plf_set_sequence_params(plf_ctx* ctx, int s, const plf_params* p);
+/* The settings the next batch will use for sequence s: its own, or the context's plf_params. */
+plf_status plf_get_sequence_params(const plf_ctx* ctx, int s, plf_params* out);
+enum { PLF_PARAM_SEQUENCE = 1, PLF_PARAM_CONTEXT = 2, PLF_PARAM_IGNORED = 3 };
+/* The classification plf_set_sequence_params applies: for each field i of plf_params, i < min(cap, return value), its name
+ * to names[i] and its class (PLF_PARAM_*) to classes[i], either array may be NULL.  Returns the number of fields. */
+int plf_sequence_param_fields(const char** names, int* classes, int cap);
+
 /* Rectification of sequence s's raw pairs before extraction: stvo-pl's dataset reader
  * cv::remap(img, out, map1, map2, INTER_LINEAR) with the default BORDER_CONSTANT 0, per image.  map1_*: w x h x 2 int16
  * (x, y) and map2_*: w x h uint16, as cv::initUndistortRectifyMap(..., CV_16SC2) or cv::convertMaps give them, for the

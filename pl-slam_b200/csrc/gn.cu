@@ -182,10 +182,13 @@ __device__ void d_inverse6(const double* Ain, double* I) {
 
 // cams: optional per-problem cameras (a batch of several calibrations); null = launch_cam for every problem.
 // active: optional per-problem flags; a problem whose flag is 0 is skipped (nothing read or written); null = all run.
+// prm: optional per-problem settings, whose gn replaces o.
 __global__ void __launch_bounds__(GN_THREADS) k_gn_pose(const GnProblem* __restrict__ probs, GnCam launch_cam,
                                                          const PlfPairCam* __restrict__ cams,
-                                                         const int* __restrict__ active, plf_gn_opts o) {
+                                                         const int* __restrict__ active, plf_gn_opts o,
+                                                         const PlfPairPrm* __restrict__ prm) {
   if (active && !active[blockIdx.x]) return;
+  if (prm) o = prm[blockIdx.x].gn;
   const GnProblem P = probs[blockIdx.x];
   GnCam cam = launch_cam;
   if (cams) {
@@ -352,10 +355,10 @@ plf_gn_opts plf_gn_opts_from_params(const plf_params& p) {
 }
 
 plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs, int nprob, const plf_gn_opts& o,
-                         const PlfPairCam* d_cams, const int* d_active) {
+                         const PlfPairCam* d_cams, const int* d_active, const PlfPairPrm* d_prm) {
   if (nprob <= 0) return PLF_OK;
   GnCam c = {ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy};
-  k_gn_pose<<<nprob, GN_THREADS, 0, cs>>>(d_probs, c, d_cams, d_active, o);
+  k_gn_pose<<<nprob, GN_THREADS, 0, cs>>>(d_probs, c, d_cams, d_active, o, d_prm);
   PLF_LAUNCH_CHECK(ctx);
   return PLF_OK;
 }

@@ -996,17 +996,22 @@ __global__ void __launch_bounds__(128) k_lsd_rects(const LsdPix* __restrict__ pi
 // NULL.  A KeyLine whose two end points both truncate onto a 0 of the mask is deleted after the length filter and before
 // the top-K, keeping the class_id it was given among the lines of sufficient length (LSDDetector_custom.cpp:310-322 runs
 // after :299 numbers them).  The unmasked instantiation ignores masks.
+// prm (plf_lsd_grow): image im takes nfeatures and min_length from its pair's settings prm[im / 2].
 #define KL_SORT_CAP 4096
 template <bool MASKED>
 __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ segs_all, const int* __restrict__ nsegs,
                                                    int max_regions, int w, int h, double min_length, int nfeatures,
                                                    plf_keyline* __restrict__ kls_all, plf_keyline* __restrict__ kls_out,
                                                    int max_lines, int* __restrict__ nlines, int* __restrict__ overflow,
-                                                   const uint8_t* const* __restrict__ masks) {
+                                                   const uint8_t* const* __restrict__ masks, const PlfPairPrm* __restrict__ prm) {
   __shared__ unsigned long long keys[KL_SORT_CAP];  // (response desc, index asc) for the top-K
   __shared__ int s_scan[1024];
   __shared__ int s_total;
   const int im = blockIdx.x, tid = threadIdx.x;
+  if (prm) {   // as plf_lsd_grow derives them from plf_params
+    nfeatures = prm[im >> 1].lsd_nfeatures;
+    min_length = (double)prm[im >> 1].min_line_length * (double)min(w, h);
+  }
   const int n = min(nsegs[im], max_regions);
   const float4* segs = segs_all + (size_t)im * max_regions;
   plf_keyline* all = kls_all + (size_t)im * max_regions;
@@ -1415,7 +1420,7 @@ plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t
 }
 
 plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int n, cudaEvent_t keylines_wait,
-                        const uint8_t* const* masks) {
+                        const uint8_t* const* masks, const PlfPairPrm* prm) {
   if (s->nimg < n) return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_grow: %d images > the state's %d", n, s->nimg);
   const LsdTables& T = *ctx->lsd_tables;
   const int w = s->w, h = s->h;
@@ -1440,10 +1445,10 @@ plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int
   if (keylines_wait) PLF_CUDA(ctx, cudaStreamWaitEvent(cs, keylines_wait, 0));
   if (masks)
     k_keylines<true><<<n, 1024, 0, cs>>>(s->segs, s->nregions, s->max_regions, w, h, min_length, ctx->params.lsd_nfeatures, s->kls_all,
-                                         s->kls[par], s->max_lines, s->nlines[par], s->overflow, masks);
+                                         s->kls[par], s->max_lines, s->nlines[par], s->overflow, masks, prm);
   else
     k_keylines<false><<<n, 1024, 0, cs>>>(s->segs, s->nregions, s->max_regions, w, h, min_length, ctx->params.lsd_nfeatures, s->kls_all,
-                                          s->kls[par], s->max_lines, s->nlines[par], s->overflow, nullptr);
+                                          s->kls[par], s->max_lines, s->nlines[par], s->overflow, nullptr, prm);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "lsd.k_keylines");
   return PLF_OK;

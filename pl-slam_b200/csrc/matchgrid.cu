@@ -104,10 +104,23 @@ __global__ void __launch_bounds__(128) k_mg_columns(MgGrid g, int is_lines, cons
 // The slot of problem p's query rows and count (MgbArgs::q_slot).
 __device__ __forceinline__ size_t mgb_qslot(const MgbArgs& a, int p) { return a.q_slot ? (size_t)a.q_slot[p] : (size_t)p; }
 
+// Problem p's own window, ratio, best_lr and direction gate when the launch has a settings table (MgbArgs::prm).
+__device__ __forceinline__ void mgb_own(MgbArgs& a, int p) {
+  if (!a.prm) return;
+  const PlfPairPrm& q = a.prm[p];
+  const int ws = a.f2f ? q.matching_f2f_ws : q.matching_s_ws;
+  a.g.w_lo = ws;
+  a.g.w_hi = a.g.h_lo = a.g.h_hi = a.f2f ? ws : 0;
+  a.nnr = a.is_lines ? q.min_ratio_12_l : q.min_ratio_12_p;
+  a.best_lr = q.best_lr;
+  a.line_sim_th = (double)q.line_sim_th;
+}
+
 // Row and mutual passes over problems p0 .. p0 + gridDim.y - 1 (MgbArgs, plf_internal.h); D and m21 hold the problems of
 // the current chunk (pl = p - p0).
 __global__ void __launch_bounds__(128) k_mgb_rows(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
+  mgb_own(a, p);
   const int i1 = blockIdx.x * 128 + threadIdx.x;
   const int n1 = min(a.n1[mgb_qslot(a, p) * a.n1_stride], a.K), n2 = min(a.n2[(size_t)p * a.n2_stride], a.Kt);
   if (i1 >= n1) return;
@@ -125,6 +138,7 @@ __global__ void __launch_bounds__(128) k_mgb_rows(MgbArgs a, int p0) {
 
 __global__ void __launch_bounds__(128) k_mgb_mutual(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
+  mgb_own(a, p);
   const int i1 = blockIdx.x * 128 + threadIdx.x;
   const int n1 = min(a.n1[mgb_qslot(a, p) * a.n1_stride], a.K);
   bool ok = false;
@@ -241,6 +255,7 @@ extern "C" plf_status plf_match_grid_lines(plf_ctx* ctx, const int* q_line, cons
 
 __global__ void __launch_bounds__(128) k_mgb_qmask(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
+  mgb_own(a, p);
   const int i1 = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   const int n1 = min(a.n1[mgb_qslot(a, p) * a.n1_stride], a.K);
   if (i1 >= n1) return;
@@ -270,6 +285,7 @@ __global__ void __launch_bounds__(128) k_mgb_qmask(MgbArgs a, int p0) {
 // grid-unit queries of the batched front-end it takes longer than k_mgb_qmask (DESIGN.md §8).
 __global__ void __launch_bounds__(128) k_mgb_qmask_clip(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
+  mgb_own(a, p);
   const int i1 = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   const int n1 = min(a.n1[mgb_qslot(a, p) * a.n1_stride], a.K);
   if (i1 >= n1) return;
@@ -314,6 +330,7 @@ __global__ void __launch_bounds__(128) k_mgb_qmask_clip(MgbArgs a, int p0) {
 template <int IS_LINES>
 __global__ void __launch_bounds__(128) k_mgb_columns(MgbArgs a, int p0) {
   const int pl = blockIdx.y, p = p0 + pl;
+  mgb_own(a, p);
   const int i2 = blockIdx.x * 128 + threadIdx.x;
   const size_t qs = mgb_qslot(a, p);
   const int n1 = min(a.n1[qs * a.n1_stride], a.K), n2 = min(a.n2[(size_t)p * a.n2_stride], a.Kt);

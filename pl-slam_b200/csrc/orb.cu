@@ -29,6 +29,7 @@
 #include "plf_tma.cuh"
 
 #define ORB_MAX_LEVELS 8
+static_assert(ORB_MAX_LEVELS == PLF_ORB_MAX_LEVELS, "PlfPairPrm holds a count per ORB level");
 #define ORB_MIN_EDGE 19   // smallest orb_edge_th: keypoint to level border >= the 18-pixel reach of the 37 x 37 window
 #define ORB_TW 64
 #define ORB_TH 16
@@ -232,14 +233,16 @@ __host__ __device__ __forceinline__ size_t orb_mask_off(const OrbGeom& g, int l)
 // MASKED (plf_set_sequence_mask, plf_orb_masked): masks[img] is image img's mask pyramid, or NULL; an NMS survivor whose
 // level mask is 0 is dropped before it reaches the candidate list and the histogram (KeyPointsFilter::runByPixelsMask
 // after FAST).  The unmasked instantiation ignores masks.
+// prm (plf_orb_run): an image whose pair detects on fewer levels than l + 1 does nothing on level l.
 template <bool MASKED>
 __global__ void __launch_bounds__(256, 5) k_fast_nms(const __grid_constant__ CUtensorMap tmap, OrbGeom g, int l, int tiles_x,
                                                   const int* __restrict__ img_th, uint32_t* __restrict__ cand, int* __restrict__ cand_count,
                                                   int* __restrict__ hist, int* __restrict__ overflow,
-                                                  const uint8_t* const* __restrict__ masks) {
+                                                  const uint8_t* const* __restrict__ masks, const PlfPairPrm* __restrict__ prm) {
   const int W = g.w[l], H = g.h[l];
   const int x0 = (blockIdx.x % tiles_x) * FN_OW, y0 = (blockIdx.x / tiles_x) * FN_OH;
   const int img = blockIdx.y;
+  if (prm && l >= prm[img >> 1].orb_nlevels) return;
   __shared__ __align__(128) uint8_t pxb[38][96];  // the TMA box (96 x 38 bytes) from the 16-byte boundary at or below x0 - 4
   __shared__ __align__(16) uint8_t sc[32][64];    // score of pixel (x0 - 1 + sx, y0 - 1 + sy)
   __shared__ unsigned short clist[32 * 64];
@@ -366,11 +369,13 @@ __global__ void __launch_bounds__(256, 5) k_fast_nms(const __grid_constant__ CUt
 }
 
 // ---- retainBest + canonical ordering -----------------------------------------------------------------
+// prm (plf_orb_run): image z keeps prm[z / 2].orb_nfeat[l] on level l; the levels its pair does not detect on hold no
+// candidates.
 __global__ void __launch_bounds__(1024) k_select_sort(OrbGeom g, const uint32_t* __restrict__ cand,
                                                       const int* __restrict__ cand_count,
                                                       const int* __restrict__ hist, plf_keypoint* __restrict__ kps,
                                                       short2* __restrict__ kp_lxy, int* __restrict__ kp_count,
-                                                      int* __restrict__ overflow) {
+                                                      int* __restrict__ overflow, const PlfPairPrm* __restrict__ prm) {
   __shared__ uint32_t keys[ORB_SORT_CAP];
   __shared__ int s_cnt, s_thr;
   const int img = blockIdx.x, tid = threadIdx.x;
@@ -380,7 +385,7 @@ __global__ void __launch_bounds__(1024) k_select_sort(OrbGeom g, const uint32_t*
     if (tid == 0) {
       s_cnt = 0;
       int thr = 0;
-      const int want = g.nfeat[l];
+      const int want = prm ? prm[img >> 1].orb_nfeat[l] : g.nfeat[l];
       if (want < n) {
         if (want == 0) {
           thr = 256;
@@ -673,6 +678,18 @@ void plf_orb_free(OrbState* s) {
   delete s;
 }
 
+void plf_orb_level_features(int nfeatures, float scale_factor, int nlevels, int* nfeat) {
+  const float factor = (float)(1.0 / (double)scale_factor);
+  float nd = nfeatures * (1 - factor) / (1 - (float)pow((double)factor, (double)nlevels));
+  int sum = 0;
+  for (int l = 0; l < nlevels - 1; ++l) {
+    nfeat[l] = cv_round_f(nd);
+    sum += nfeat[l];
+    nd *= factor;
+  }
+  nfeat[nlevels - 1] = std::max(nfeatures - sum, 0);
+}
+
 // The geometry of s for nimg images of w x h, its buffers listed in s->bufs and s->tabs (not allocated) and its resize
 // tables in tab.  Host only.
 static plf_status orb_layout(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, bool two_parities, std::vector<int>& tab) {
@@ -721,17 +738,7 @@ static plf_status orb_layout(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, 
   g.tile_start[g.nlevels] = tiles;
   for (int l = g.nlevels + 1; l <= ORB_MAX_LEVELS; ++l) g.tile_start[l] = tiles;
   g.pyr_stride = pyr; g.blur_stride = blur; g.cand_stride = cand;
-  {  // nfeaturesPerLevel (orb.cpp computeKeyPoints)
-    const float factor = (float)(1.0 / scaleFactor);
-    float nd = P.orb_nfeatures * (1 - factor) / (1 - (float)pow((double)factor, (double)g.nlevels));
-    int sum = 0;
-    for (int l = 0; l < g.nlevels - 1; ++l) {
-      g.nfeat[l] = cv_round_f(nd);
-      sum += g.nfeat[l];
-      nd *= factor;
-    }
-    g.nfeat[g.nlevels - 1] = std::max(P.orb_nfeatures - sum, 0);
-  }
+  plf_orb_level_features(P.orb_nfeatures, P.orb_scale_factor, g.nlevels, g.nfeat);
   {  // getGaussianKernel(7, 2, CV_32F): host doubles -> float (pinned equal to cv2 in tests)
     double d[7], sum = 0;
     for (int i = 0; i < 7; ++i) {
@@ -847,7 +854,7 @@ plf_status plf_orb_create(plf_ctx* ctx, int w, int h, int nimg, bool two_paritie
 // Runs ORB on nimg (<= s->nimg) images of s->w x s->h resident at d_imgs ([nimg][h][pitch], pitch a multiple of 16,
 // stride img_stride bytes).  Enqueued on cs; results stay on the device.
 plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par,
-                       const int* img_th, const uint8_t* const* masks) {
+                       const int* img_th, const uint8_t* const* masks, const PlfPairPrm* prm) {
   const int w = s->w, h = s->h;
   plf_status st;
   OrbGeom g = s->g;
@@ -871,13 +878,13 @@ plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t
     const int tx_ = (g.w[l] + FN_OW - 1) / FN_OW, ty_ = (g.h[l] + FN_OH - 1) / FN_OH;
     const CUtensorMap& tm = l == 0 ? *tm_fast0 : s->tm_fast[l];
     if (masks)
-      k_fast_nms<true><<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(tm, g, l, tx_, img_th, s->cand, s->cand_count, s->hist, s->overflow, masks);
+      k_fast_nms<true><<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(tm, g, l, tx_, img_th, s->cand, s->cand_count, s->hist, s->overflow, masks, prm);
     else
-      k_fast_nms<false><<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(tm, g, l, tx_, img_th, s->cand, s->cand_count, s->hist, s->overflow, nullptr);
+      k_fast_nms<false><<<dim3(tx_ * ty_, nimg), 256, 0, cs>>>(tm, g, l, tx_, img_th, s->cand, s->cand_count, s->hist, s->overflow, nullptr, prm);
     PLF_LAUNCH_CHECK(ctx);
   }
   plf_mark(ctx, cs, "orb.k_fast_nms");
-  k_select_sort<<<nimg, 1024, 0, cs>>>(g, s->cand, s->cand_count, s->hist, s->kps[par], s->kp_lxy[par], s->kp_count[par], s->overflow);
+  k_select_sort<<<nimg, 1024, 0, cs>>>(g, s->cand, s->cand_count, s->hist, s->kps[par], s->kp_lxy[par], s->kp_count[par], s->overflow, prm);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "orb.k_select_sort");
   k_ic_angle<<<dim3((g.max_kp + 7) / 8, nimg), 256, 0, cs>>>(d_imgs, img_stride, s->pyr, g, s->kps[par], s->kp_lxy[par], s->kp_count[par]);

@@ -50,26 +50,28 @@ constexpr int PLF_FS_NFIELDS = 0 PLF_PT_FIELDS(PLF_FS_ONE) PLF_LS_FIELDS(PLF_FS_
 struct PlfRectPair { const uint8_t* maps; int pair; int pad; };
 
 // One entry of the batch table ring, for max_batch pairs B: the sequence table (prev[B] = the frame slot of pair k's
-// previous frame, then the carry list [B][2] of (frame slot, carry slot)), the pairs' cameras [B], the input table [B]
-// and the mask table [2B] (image z's mask pyramid, plf_set_sequence_mask, or NULL).  The pinned and the device ring use
-// the same layout.
+// previous frame, then the carry list [B][2] of (frame slot, carry slot)), the pairs' cameras [B], the input table [B],
+// the mask table [2B] (image z's mask pyramid, plf_set_sequence_mask, or NULL) and the pairs' settings [B]
+// (plf_set_sequence_params).  The pinned and the device ring use the same layout.
 struct BatchTab {
   int32_t* prev;
   int32_t* carry;
   PlfPairCam* cams;
   PlfRectPair* in;
   const uint8_t** masks;
+  PlfPairPrm* prm;
 };
 static size_t batch_tab_bytes(int B) {
   return plf_align256(3 * sizeof(int32_t) * B) + plf_align256(sizeof(PlfPairCam) * B) + plf_align256(sizeof(PlfRectPair) * B) +
-         plf_align256(sizeof(uint8_t*) * 2 * B);
+         plf_align256(sizeof(uint8_t*) * 2 * B) + plf_align256(sizeof(PlfPairPrm) * B);
 }
 static BatchTab batch_tab(uint8_t* base, int B) {
   uint8_t* cams = base + plf_align256(3 * sizeof(int32_t) * B);
   uint8_t* in = cams + plf_align256(sizeof(PlfPairCam) * B);
   uint8_t* masks = in + plf_align256(sizeof(PlfRectPair) * B);
+  uint8_t* prm = masks + plf_align256(sizeof(uint8_t*) * 2 * B);
   return {reinterpret_cast<int32_t*>(base), reinterpret_cast<int32_t*>(base) + B, reinterpret_cast<PlfPairCam*>(cams),
-          reinterpret_cast<PlfRectPair*>(in), reinterpret_cast<const uint8_t**>(masks)};
+          reinterpret_cast<PlfRectPair*>(in), reinterpret_cast<const uint8_t**>(masks), reinterpret_cast<PlfPairPrm*>(prm)};
 }
 
 // What each sequence carries to its next pair besides its frame slot: the pose prediction (row-major 4x4) and whether it
@@ -142,6 +144,7 @@ struct PipeState {
   int* rev_flags = nullptr; int* rev_list = nullptr; int* rev_count = nullptr;  // [2B][max_kp], [2B][max_kp], [2B]
   KnnProblem* knn_f2f = nullptr;     // [B*4]
   NnrProblem* nnr_stereo = nullptr;  // [B*2]
+  NnrProblem* nnr_own = nullptr;     // [B*2] the stereo problems of a batch with pair settings (k_pair_nnr)
   NnrProblem* nnr_f2f = nullptr;     // [B*2]
   // GN inputs / outputs
   double* gnP = nullptr; double* gnObs = nullptr; uint8_t* gnInlP = nullptr; int* gnNp = nullptr;
@@ -204,7 +207,7 @@ static void pipe_buffers(PipeState* s, bool windowed, DevBufList& b) {
   b.add(s->m12, B * 4 * K);
   b.add(s->mcount, B * 4);
   b.add(s->knn_stereo, B * 4); b.add(s->knn_f2f, B * 4);
-  b.add(s->nnr_stereo, B * 2); b.add(s->nnr_f2f, B * 2);
+  b.add(s->nnr_stereo, B * 2); b.add(s->nnr_f2f, B * 2); b.add(s->nnr_own, B * 2);
   b.add(s->rev_flags, 2 * B * K); b.add(s->rev_list, 2 * B * K); b.add(s->rev_count, 2 * B);
   b.add(s->kpsM, 2 * B * K); b.add(s->descM, 2 * B * K * 32); b.add(s->kcntM, 2 * B);
   b.add(s->klsM, 2 * B * Ln); b.add(s->lcntM, 2 * B);
@@ -262,11 +265,18 @@ struct StereoPrm {
   double fx, fy, cx, cy, b;   // the context's camera
 };
 
-// The parameters of pair k: prm with the pair's camera from the batch's camera table, or prm itself without a table.
-__device__ __forceinline__ StereoPrm pair_prm(StereoPrm c, const PlfPairCam* __restrict__ cams, int k) {
+// The parameters of pair k: prm with the pair's camera from the batch's camera table and its gates from the batch's
+// settings table, or prm itself without them.
+__device__ __forceinline__ StereoPrm pair_prm(StereoPrm c, const PlfPairCam* __restrict__ cams, int k,
+                                              const PlfPairPrm* __restrict__ own = nullptr) {
   if (cams) {
     const PlfPairCam q = cams[k];
     c.fx = q.fx; c.fy = q.fy; c.cx = q.cx; c.cy = q.cy; c.b = q.b;
+  }
+  if (own) {
+    const PlfPairPrm& q = own[k];
+    c.max_dist_epip = q.max_dist_epip; c.min_disp = q.min_disp; c.line_horiz_th = q.line_horiz_th;
+    c.stereo_overlap_th = q.stereo_overlap_th; c.ls_min_disp_ratio = q.ls_min_disp_ratio;
   }
   return c;
 }
@@ -295,16 +305,19 @@ __device__ __forceinline__ int block_scan_flags(bool flag, int* s_scan, int* s_t
   return incl;
 }
 
-// matchStereoPoints: epipolar + disparity gates, back-projection, compaction in left-index order.
+// matchStereoPoints: epipolar + disparity gates, back-projection, compaction in left-index order.  OWN: the gates of pair k
+// from own[k] (a batch with pair settings); the other instantiation ignores own.
+template <bool OWN>
 __global__ void __launch_bounds__(1024) k_stereo_points(const plf_keypoint* __restrict__ kps, const uint8_t* __restrict__ desc,
                                                          const int* __restrict__ kp_count, int max_kp,
                                                          const int32_t* __restrict__ m12_all, int m12_stride, StereoPrm prm0,
-                                                         const PlfPairCam* __restrict__ cams, FrameSlots fs) {
+                                                         const PlfPairCam* __restrict__ cams, FrameSlots fs,
+                                                         const PlfPairPrm* __restrict__ own) {
   __shared__ int s_scan[1024];
   __shared__ int s_total;
   const int k = blockIdx.x, tid = threadIdx.x;
   const int il = 2 * k, ir = 2 * k + 1, slot = k;
-  const StereoPrm prm = pair_prm(prm0, cams, k);
+  const StereoPrm prm = pair_prm(prm0, cams, k, OWN ? own : nullptr);
   const plf_keypoint* kl = kps + (size_t)il * max_kp;
   const plf_keypoint* kr = kps + (size_t)ir * max_kp;
   const int32_t* m12 = m12_all + (size_t)k * m12_stride;
@@ -361,16 +374,18 @@ __device__ __forceinline__ double line_overlap_stereo(double spl_obs, double epl
   return overlap;
 }
 
-// matchStereoLines
+// matchStereoLines (OWN: as k_stereo_points)
+template <bool OWN>
 __global__ void __launch_bounds__(1024) k_stereo_lines(const plf_keyline* __restrict__ kls, const uint8_t* __restrict__ ldesc,
                                                         const int* __restrict__ nlines, int max_ln,
                                                         const int32_t* __restrict__ m12_all, int m12_stride, StereoPrm prm0,
-                                                        const PlfPairCam* __restrict__ cams, FrameSlots fs) {
+                                                        const PlfPairCam* __restrict__ cams, FrameSlots fs,
+                                                        const PlfPairPrm* __restrict__ own) {
   __shared__ int s_scan[1024];
   __shared__ int s_total;
   const int k = blockIdx.x, tid = threadIdx.x;
   const int il = 2 * k, ir = 2 * k + 1, slot = k;
-  const StereoPrm prm = pair_prm(prm0, cams, k);
+  const StereoPrm prm = pair_prm(prm0, cams, k, OWN ? own : nullptr);
   const plf_keyline* L = kls + (size_t)il * max_ln;
   const plf_keyline* R = kls + (size_t)ir * max_ln;
   const int32_t* m12 = m12_all + (size_t)k * m12_stride;
@@ -449,6 +464,27 @@ __global__ void k_f2f_problems(FrameSlots fs, const int* __restrict__ prev, int 
                              mcount + 4 * k + 2};
   nf[2 * k + 1] = NnrProblem{key(6, 0), key(6, 1), key(7, 0), key(7, 1), lnp, lnc, 0, 0, nnr_l, best_lr, m12 + ((size_t)k * 4 + 3) * K,
                              mcount + 4 * k + 3};
+}
+
+// The matching settings of a batch with pair settings (prm): its stereo problems ns_own, copies of the context's ns with
+// each pair's ratios and best_lr, and the same in place in its frame-to-frame problems nf (k_f2f_problems).  A pair of a
+// windowed sequence (matching_strategy != 0) gets its stereo matches from the windowed matcher: its problems here read
+// their query count at zero, an int that stays 0, so they write no row.
+__global__ void k_pair_nnr(const PlfPairPrm* __restrict__ prm, int B, const NnrProblem* __restrict__ ns, const int* zero,
+                           NnrProblem* __restrict__ ns_own, NnrProblem* __restrict__ nf) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= B) return;
+  const PlfPairPrm& q = prm[k];
+  for (int c = 0; c < 2; ++c) {
+    const float nnr = c ? q.min_ratio_12_l : q.min_ratio_12_p;
+    NnrProblem p = ns[2 * k + c];
+    p.nnr = nnr;
+    p.best_lr = q.best_lr;
+    if (q.matching_strategy) p.n1_ptr = zero;
+    ns_own[2 * k + c] = p;
+    nf[2 * k + c].nnr = nnr;
+    nf[2 * k + c].best_lr = q.best_lr;
+  }
 }
 
 // Copies `rows` rows of row_bytes (a multiple of 4) from slot `from` to slot `to` of an array of `cap` rows per slot.
@@ -540,9 +576,10 @@ __global__ void __launch_bounds__(1024) k_f2f_build(FrameSlots fs, const int* __
 __global__ void k_finalize(const plf_pose_result* __restrict__ gn, const int* __restrict__ gnNp, const int* __restrict__ gnNl,
                            const int* __restrict__ kp_count, const int* __restrict__ nlines, FrameSlots fs,
                            const int* __restrict__ prev, int empty_slot, int min_features, int B,
-                           plf_frame_result* __restrict__ out) {
+                           plf_frame_result* __restrict__ out, const PlfPairPrm* __restrict__ prm) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= B) return;
+  if (prm) min_features = prm[k].min_features;
   plf_frame_result r;
   for (int i = 0; i < 16; ++i) r.DT[i] = (i % 5 == 0) ? 1.0 : 0.0;
   for (int i = 0; i < 36; ++i) r.DT_cov[i] = 0.0;
@@ -574,13 +611,14 @@ __global__ void k_finalize(const plf_pose_result* __restrict__ gn, const int* __
 // (plf_set_motion_model), DESIGN.md §8.  With either on a batch holds at most one pair of each sequence, so prev[k] is the
 // empty slot (a first frame) or pair k's carry slot carry0 + s, and every pair is in the carry list. ----
 
-// The FAST threshold of both images of pair k: its sequence's, or th0 = orb_fast_th for a first frame.
+// The FAST threshold of both images of pair k: its sequence's (rec, with adaptive FAST), or for a first frame and without
+// rec the first frame's, the pair's own settings' (prm) or th0 = orb_fast_th.
 __global__ void k_fast_th_images(const int* __restrict__ prev, int B, int carry0, int empty, int th0,
-                                 const SeqRecord* __restrict__ rec, int* __restrict__ img_th) {
+                                 const SeqRecord* __restrict__ rec, const PlfPairPrm* __restrict__ prm, int* __restrict__ img_th) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= B) return;
   const int p = prev[k];
-  const int th = p == empty ? th0 : rec[p - carry0].th;
+  const int th = rec && p != empty ? rec[p - carry0].th : prm ? prm[k].fast_th : th0;
   img_th[2 * k] = th;
   img_th[2 * k + 1] = th;
 }
@@ -599,7 +637,25 @@ __device__ __forceinline__ int fast_th_next(int th, const plf_frame_result& r, c
 }
 
 // orb_fast_th as k_fast_nms applies it without a per-image threshold
-static int fast_th0(const plf_ctx* ctx) { return std::min(std::max(ctx->params.orb_fast_th, 0), 255); }
+static int fast_th0(const plf_params& P) { return std::min(std::max(P.orb_fast_th, 0), 255); }
+static int fast_th0(const plf_ctx* ctx) { return fast_th0(ctx->params); }
+
+PlfPairPrm plf_pair_prm(const plf_params& P) {
+  PlfPairPrm q = {};
+  q.orb_nlevels = P.orb_nlevels;
+  plf_orb_level_features(P.orb_nfeatures, P.orb_scale_factor, P.orb_nlevels, q.orb_nfeat);
+  q.fast_th = fast_th0(P);
+  q.lsd_nfeatures = P.lsd_nfeatures;
+  q.min_line_length = P.min_line_length;
+  q.max_dist_epip = P.max_dist_epip; q.min_disp = P.min_disp; q.line_horiz_th = P.line_horiz_th;
+  q.stereo_overlap_th = P.stereo_overlap_th; q.ls_min_disp_ratio = P.ls_min_disp_ratio;
+  q.min_ratio_12_p = P.min_ratio_12_p; q.min_ratio_12_l = P.min_ratio_12_l; q.line_sim_th = P.line_sim_th;
+  q.best_lr = P.best_lr_matches ? 1 : 0;
+  q.matching_strategy = P.matching_strategy; q.matching_s_ws = P.matching_s_ws; q.matching_f2f_ws = P.matching_f2f_ws;
+  q.min_pt_matches = P.min_pt_matches; q.min_ls_matches = P.min_ls_matches; q.min_features = P.min_features;
+  q.gn = plf_gn_opts_from_params(P);
+  return q;
+}
 
 // stvo-pl's isGoodSolution on a pair's result, each of its tests a rejection: so a NaN err or eigenvalue passes.  A
 // covariance with a non-finite entry has NaN eigenvalues (the library's definition; the solver gives such a covariance
@@ -757,11 +813,16 @@ __global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, const int* _
 }
 
 // src/mapHandler.cpp:274-278 / :421-425: keep the windowed result unless both frames hold more than `kmin` features and
-// fewer than `kmin` matches survived - then the brute-force match() result (already in m12) stands.
+// fewer than `kmin` matches survived - then the brute-force match() result (already in m12) stands.  With pair settings
+// (prm) kmin is the pair's, and a pair of a sequence at matching_strategy 0 keeps its match() result.
 __global__ void __launch_bounds__(256) k_mg_select(const int32_t* __restrict__ m12g, const int* __restrict__ mgcount,
                                                    const int* __restrict__ cnt, const int* __restrict__ prev, int cap, int K,
-                                                   int which, int kmin, int32_t* __restrict__ m12) {
+                                                   int which, int kmin, int32_t* __restrict__ m12, const PlfPairPrm* __restrict__ prm) {
   const int k = blockIdx.y, i = blockIdx.x * 256 + threadIdx.x;
+  if (prm) {
+    if (!prm[k].matching_strategy) return;
+    kmin = which ? prm[k].min_ls_matches : prm[k].min_pt_matches;
+  }
   const int n1 = min(cnt[prev[k]], cap), n2 = min(cnt[k], cap);
   if (i >= n1) return;
   const bool fall_back = n2 > kmin && n1 > kmin && mgcount[2 * k + which] < kmin;
@@ -883,6 +944,9 @@ struct BatchRun {
   bool cams;     // batch table rp holds the pairs' cameras (a sequence of the batch has its own); else the context's camera
   int nin;       // entries of the input table in batch table rp (0: none, every pair is converted as it is)
   bool masked;   // batch table rp holds the images' masks (a sequence of the batch has one); else no image is masked
+  bool prm;      // batch table rp holds the pairs' settings (a sequence of the batch has its own); else the context's
+  int nwin;      // pairs at matching_strategy != 0 (with prm; else every pair or none, as the context's)
+  bool best_lr;  // some pair matches with best_lr_matches (with prm; else the context's)
   bool afast;    // adaptive FAST thresholds (plf_set_adaptive_fast): pair thresholds in the E phase, the next ones behind k_finalize
   bool motion;   // motion model (plf_set_motion_model): pair predictions at the start of M, the next ones behind k_finalize
   int par;       // parity of the E -> G -> M hand-off buffers
@@ -898,7 +962,7 @@ static BatchTab host_tab(const PipeState* s, int rp) { return batch_tab(s->h_tab
 static BatchTab dev_tab(const PipeState* s, int rp) { return batch_tab(s->tab + rp * batch_tab_bytes(s->B), s->B); }
 
 // The parts of the batch's table that it uses, to ring entry rp of the device on the copy stream: the sequence table
-// always, the cameras and the input table when it has them.  ev_tab[rp] marks them.
+// always, the cameras, the input table, the masks and the settings when it has them.  ev_tab[rp] marks them.
 static plf_status send_tab(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   const BatchTab h = host_tab(s, r.rp), d = dev_tab(s, r.rp);
   cudaStream_t cs = s->copy;
@@ -907,6 +971,7 @@ static plf_status send_tab(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   if (r.cams) PLF_CUDA(ctx, cudaMemcpyAsync(d.cams, h.cams, sizeof(PlfPairCam) * r.B, cudaMemcpyHostToDevice, cs));
   if (r.nin) PLF_CUDA(ctx, cudaMemcpyAsync(d.in, h.in, sizeof(PlfRectPair) * r.nin, cudaMemcpyHostToDevice, cs));
   if (r.masked) PLF_CUDA(ctx, cudaMemcpyAsync(d.masks, h.masks, sizeof(uint8_t*) * 2 * r.B, cudaMemcpyHostToDevice, cs));
+  if (r.prm) PLF_CUDA(ctx, cudaMemcpyAsync(d.prm, h.prm, sizeof(PlfPairPrm) * r.B, cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaEventRecord(s->ev_tab[r.rp], cs));
   return PLF_OK;
 }
@@ -1047,17 +1112,18 @@ static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaEventRecord(s->tE0[par], sE));
   const int* img_th = nullptr;
   const uint8_t* const* masks = r.masked ? dev_tab(s, r.rp).masks : nullptr;
-  if (r.afast || r.masked) PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_tab[r.rp], 0));   // the sequence or mask table
-  if (r.afast) {
+  const PlfPairPrm* prm = r.prm ? dev_tab(s, r.rp).prm : nullptr;
+  if (r.afast || r.masked || r.prm) PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_tab[r.rp], 0));   // the sequence, mask or settings table
+  if (r.afast || r.prm) {
     // the thresholds of the batch's images: the sequence table, and the previous batch's threshold update (which has
-    // also read img_th for the last time)
-    PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_th, 0));
-    k_fast_th_images<<<(B + 127) / 128, 128, 0, sE>>>(dev_tab(s, r.rp).prev, B, s->B, s->B + s->nseq, fast_th0(ctx), s->seq_rec,
-                                                      s->img_th);
+    // also read img_th for the last time); without adaptive FAST each pair's first-frame threshold
+    if (r.afast) PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_th, 0));
+    k_fast_th_images<<<(B + 127) / 128, 128, 0, sE>>>(dev_tab(s, r.rp).prev, B, s->B, s->B + s->nseq, fast_th0(ctx),
+                                                      r.afast ? s->seq_rec : nullptr, prm, s->img_th);
     PLF_LAUNCH_CHECK(ctx);
     img_th = s->img_th;
   }
-  plf_status st = plf_orb_run(ctx, sE, G.orb, imgs, AP, G.pitch, 2 * B, par, img_th, masks);
+  plf_status st = plf_orb_run(ctx, sE, G.orb, imgs, AP, G.pitch, 2 * B, par, img_th, masks, prm);
   if (!st) st = plf_launch_blur5_sobel(ctx, sE, &G.lbd_tm, imgs, G.pitch, AP, w, h, 2 * B, s->lbd_grad[par], A);
   if (st) return st;
   plf_mark(ctx, sE, "lbd.k_blur5_sobel");
@@ -1081,7 +1147,7 @@ static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   const size_t AP = (size_t)G.pitch * G.h;
   cudaStream_t sP = r.sP, sG = r.sG;
   PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_up[r.run_slot], 0));
-  if (r.masked) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_tab[r.rp], 0));   // the mask table, read by G's KeyLine stage
+  if (r.masked || r.prm) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_tab[r.rp], 0));   // the mask and settings tables, read by G's KeyLine stage
   if (r.lsd2) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->evG[par], 0));   // batch i-2 (same parity) has finished growing / fitting on these maps
   PLF_CUDA(ctx, cudaEventRecord(s->tG0[par], sP));
   plf_status st = plf_lsd_pre(ctx, sP, G.lsd, s->imgs2[r.run_slot], AP, G.pitch, r.lp, 2 * r.B);
@@ -1092,7 +1158,7 @@ static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   // the KeyLine outputs are overwritten: the match phase that read them last (batch i-2 with two parities, batch i-1 with one)
   // has taken its copy
   st = plf_lsd_grow(ctx, sG, G.lsd, r.lp, 2 * r.B, r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr,
-                    r.masked ? dev_tab(s, r.rp).masks : nullptr);
+                    r.masked ? dev_tab(s, r.rp).masks : nullptr, r.prm ? dev_tab(s, r.rp).prm : nullptr);
   if (st) return st;
   PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp + 1, plf_lsd_overflow_flag(G.lsd), sizeof(int), cudaMemcpyDeviceToDevice, sG));
   PLF_CUDA(ctx, cudaMemsetAsync(plf_lsd_overflow_flag(G.lsd), 0, sizeof(int), sG));
@@ -1102,10 +1168,10 @@ static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
 
 // One windowed-matching launch over B problems of one kind (points: cap = K, lines: cap = Ln).  Problem p matches the
 // descriptor rows of image / slot q_slot[p] * step of `desc` (p * step without q_slot; cnt[...] of them) against those of
-// image / slot p * step + t_off.
+// image / slot p * step + t_off.  prm: the pairs' settings, f2f: the frame-to-frame window (MgbArgs).
 static MgbArgs mgb_args(const plf_params& P, MgGrid g, bool lines, int cap, int step, const int* q_slot, int t_off,
                         const int* q_geo, const int* t_geo, const double* t_dir, const uint8_t* desc, const int* cnt,
-                        int32_t* m12, size_t m12_stride, int* count, int count_stride) {
+                        int32_t* m12, size_t m12_stride, int* count, int count_stride, const PlfPairPrm* prm, int f2f) {
   MgbArgs a = {};
   a.g = g;
   a.is_lines = lines ? 1 : 0; a.K = a.Kt = cap; a.best_lr = P.best_lr_matches ? 1 : 0;
@@ -1116,6 +1182,7 @@ static MgbArgs mgb_args(const plf_params& P, MgGrid g, bool lines, int cap, int 
   a.d1 = desc; a.d2 = desc + (size_t)t_off * cap * 32; a.d1_stride = a.d2_stride = (size_t)step * cap * 32;
   a.n1 = cnt; a.n2 = cnt + t_off; a.n1_stride = a.n2_stride = step;
   a.m12 = m12; a.m12_stride = m12_stride; a.count = count; a.count_stride = count_stride;
+  a.prm = prm; a.f2f = f2f;
   return a;
 }
 
@@ -1140,10 +1207,17 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   const int32_t* prev = tab.prev;
   const int32_t* carry = tab.carry;
   const PlfPairCam* pcam = r.cams ? tab.cams : nullptr;
+  const PlfPairPrm* prm = r.prm ? tab.prm : nullptr;   // the pairs' settings (null: every kernel takes plf_params')
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_tab[rp], 0));
   k_f2f_problems<<<(B + 127) / 128, 128, 0, cs>>>(s->fs, prev, B, K, Ln, s->knn_keys, s->m12, s->mcount, P.min_ratio_12_p,
                                                   P.min_ratio_12_l, P.best_lr_matches ? 1 : 0, s->knn_f2f, s->nnr_f2f);
   PLF_LAUNCH_CHECK(ctx);
+  const NnrProblem* nnr_stereo = s->nnr_stereo;
+  if (prm) {
+    k_pair_nnr<<<(B + 127) / 128, 128, 0, cs>>>(prm, B, s->nnr_stereo, s->fs.pt_count + s->B + s->nseq, s->nnr_own, s->nnr_f2f);
+    PLF_LAUNCH_CHECK(ctx);
+    nnr_stereo = s->nnr_own;
+  }
   // the pairs' motion predictions, when the model is on (null: the f2f geometry and the pose solver start from identity).
   // The previous batch wrote its sequences' ones behind its k_finalize on this stream.
   const double* T_pred = nullptr;
@@ -1169,44 +1243,50 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   plf_mark(ctx, cs, "copy extraction outputs");
   PLF_CUDA(ctx, cudaMemsetAsync(s->mcount, 0, (size_t)B * 4 * sizeof(int), cs));
   const double mg_iw = PLF_GRID_COLS / (double)w, mg_ih = PLF_GRID_ROWS / (double)h;   // StereoFrame::inv_width / inv_height
-  if (P.matching_strategy) {
+  // The windowed matcher runs over every pair when one of them is windowed; then match() over every pair when one is not
+  // (its problems of windowed pairs write nothing, k_pair_nnr), so each pair keeps the association of its own strategy.
+  const bool windowed = r.nwin > 0, brute = r.nwin < B;
+  if (windowed) {
     // stereo association through matchGrid(): window (matching_s_ws, 0) x (0, 0) over the right image's grid
     k_mg_geom_stereo<<<dim3((std::max(K, Ln) + 255) / 256, 2 * B), 256, 0, cs>>>(kps, kcnt, K, kls, lcnt, Ln, mg_iw, mg_ih, s->mg_q[0],
                                                                                  s->mg_t[0], s->mg_q[1], s->mg_t[1], s->mg_dir[0]);
     PLF_LAUNCH_CHECK(ctx);
     const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, P.matching_s_ws, 0, 0, 0};
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 2, nullptr, 1, s->mg_q[0], s->mg_t[0], nullptr, odesc, kcnt,
-                                                        s->m12, 4 * (size_t)K, s->mcount, 4), B, K, K, PLF_SCR_MGB_PIPE, cs))) return st;
+                                                        s->m12, 4 * (size_t)K, s->mcount, 4, prm, 0), B, K, K, PLF_SCR_MGB_PIPE, cs))) return st;
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 2, nullptr, 1, s->mg_q[1], s->mg_t[1], s->mg_dir[0], s->ldesc_raw,
-                                                        lcnt, s->m12 + K, 4 * (size_t)K, s->mcount + 1, 4), B, Ln, Ln, PLF_SCR_MGB_PIPE, cs))) return st;
+                                                        lcnt, s->m12 + K, 4 * (size_t)K, s->mcount + 1, 4, prm, 0), B, Ln, Ln, PLF_SCR_MGB_PIPE, cs))) return st;
     plf_mark(ctx, cs, "stereo.k_mgb (matchGrid)");
-  } else {
+  }
+  if (brute) {
     // L->R 2-NN for every left feature; R->L only for the right features that are somebody's accepted best match
     // (k_nnr_mutual reads nothing else of the reverse direction): the same matches for ~2/3 of the popcounts
     if ((st = plf_launch_knn2(ctx, cs, s->knn_stereo, 2 * B, std::max(K, Ln)))) return st;
-    if (P.best_lr_matches) {
+    if (r.best_lr) {
       PLF_CUDA(ctx, cudaMemsetAsync(s->rev_flags, 0, 2 * (size_t)B * K * sizeof(int), cs));
       PLF_CUDA(ctx, cudaMemsetAsync(s->rev_count, 0, 2 * (size_t)B * sizeof(int), cs));
-      if ((st = plf_launch_nnr_mark(ctx, cs, s->nnr_stereo, 2 * B, std::max(K, Ln), s->rev_flags, s->rev_list, s->rev_count, K))) return st;
+      if ((st = plf_launch_nnr_mark(ctx, cs, nnr_stereo, 2 * B, std::max(K, Ln), s->rev_flags, s->rev_list, s->rev_count, K))) return st;
       // the reverse problems are laid out after the forward problems of ALL max_batch pairs (pipe_prepare), not of this
       // call's B pairs: a partial batch (B < max_batch) must still start at 2 * max_batch
       if ((st = plf_launch_knn2(ctx, cs, s->knn_stereo + 2 * s->B, 2 * B, std::max(K, Ln)))) return st;
     }
     plf_mark(ctx, cs, "stereo.k_hamming_knn2");
-    if ((st = plf_launch_nnr(ctx, cs, s->nnr_stereo, 2 * B, std::max(K, Ln)))) return st;
+    if ((st = plf_launch_nnr(ctx, cs, nnr_stereo, 2 * B, std::max(K, Ln)))) return st;
     plf_mark(ctx, cs, "stereo.k_nnr_mutual");
   }
   StereoPrm sp = {P.max_dist_epip, P.min_disp, P.line_horiz_th, P.stereo_overlap_th, P.ls_min_disp_ratio,
                   ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy, ctx->cam.b};
-  k_stereo_points<<<B, 1024, 0, cs>>>(kps, odesc, kcnt, K, s->m12, 4 * K, sp, pcam, s->fs);
+  if (prm) k_stereo_points<true><<<B, 1024, 0, cs>>>(kps, odesc, kcnt, K, s->m12, 4 * K, sp, pcam, s->fs, prm);
+  else k_stereo_points<false><<<B, 1024, 0, cs>>>(kps, odesc, kcnt, K, s->m12, 4 * K, sp, pcam, s->fs, nullptr);
   PLF_LAUNCH_CHECK(ctx);
-  k_stereo_lines<<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, sp, pcam, s->fs);
+  if (prm) k_stereo_lines<true><<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, sp, pcam, s->fs, prm);
+  else k_stereo_lines<false><<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, sp, pcam, s->fs, nullptr);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "stereo.k_stereo_points+lines");
   if ((st = plf_launch_knn2(ctx, cs, s->knn_f2f, 4 * B, std::max(K, Ln)))) return st;
   plf_mark(ctx, cs, "f2f.k_hamming_knn2");
   if ((st = plf_launch_nnr(ctx, cs, s->nnr_f2f, 2 * B, std::max(K, Ln)))) return st;
-  if (P.matching_strategy) {
+  if (windowed) {
     // frame-to-frame: matchGrid() in a +-matching_f2f_ws window around the projected feature; the match() result above
     // stands where the window search found fewer than min_pt_matches / min_ls_matches
     PLF_CUDA(ctx, cudaMemsetAsync(s->mgcount, 0, (size_t)B * 2 * sizeof(int), cs));
@@ -1217,12 +1297,12 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     const int ws = P.matching_f2f_ws;
     const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, ws, ws, ws, ws};
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 1, prev, 0, s->mg_q[2], s->mg_t[2], nullptr, s->fs.pdesc,
-                                                        s->fs.pt_count, s->m12g, 2 * (size_t)K, s->mgcount, 2), B, K, K, PLF_SCR_MGB_PIPE, cs))) return st;
+                                                        s->fs.pt_count, s->m12g, 2 * (size_t)K, s->mgcount, 2, prm, 1), B, K, K, PLF_SCR_MGB_PIPE, cs))) return st;
     if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 1, prev, 0, s->mg_q[3], s->mg_t[3], s->mg_dir[1], s->fs.ldesc,
-                                                        s->fs.ls_count, s->m12g + K, 2 * (size_t)K, s->mgcount + 1, 2), B, Ln, Ln, PLF_SCR_MGB_PIPE, cs))) return st;
-    k_mg_select<<<dim3((K + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.pt_count, prev, K, K, 0, P.min_pt_matches, s->m12);
+                                                        s->fs.ls_count, s->m12g + K, 2 * (size_t)K, s->mgcount + 1, 2, prm, 1), B, Ln, Ln, PLF_SCR_MGB_PIPE, cs))) return st;
+    k_mg_select<<<dim3((K + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.pt_count, prev, K, K, 0, P.min_pt_matches, s->m12, prm);
     PLF_LAUNCH_CHECK(ctx);
-    k_mg_select<<<dim3((Ln + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.ls_count, prev, Ln, K, 1, P.min_ls_matches, s->m12);
+    k_mg_select<<<dim3((Ln + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.ls_count, prev, Ln, K, 1, P.min_ls_matches, s->m12, prm);
     PLF_LAUNCH_CHECK(ctx);
     plf_mark(ctx, cs, "f2f.k_mgb (matchGrid)");
   }
@@ -1230,10 +1310,10 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
                                   s->gn_sP, s->gn_eP, s->gn_le, s->gnInlL, s->gnNl);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "f2f.k_nnr_mutual+k_f2f_build");
-  if ((st = plf_launch_gn(ctx, cs, T_pred ? s->gn_probs_mm : s->gn_probs, B, plf_gn_opts_from_params(P), pcam))) return st;
+  if ((st = plf_launch_gn(ctx, cs, T_pred ? s->gn_probs_mm : s->gn_probs, B, plf_gn_opts_from_params(P), pcam, nullptr, prm))) return st;
   plf_mark(ctx, cs, "gn.k_gn_pose");
   k_finalize<<<(B + 127) / 128, 128, 0, cs>>>(s->gn_out, s->gnNp, s->gnNl, kcnt, lcnt, s->fs, prev, s->B + s->nseq,
-                                               P.min_features, B, s->results + (size_t)rp * s->B);
+                                               P.min_features, B, s->results + (size_t)rp * s->B, prm);
   PLF_LAUNCH_CHECK(ctx);
   k_carry<<<dim3(PLF_FS_NFIELDS, r.ncarry), 256, 0, cs>>>(s->fs, carry, K, Ln);   // the next batch tracks against these
   PLF_LAUNCH_CHECK(ctx);
@@ -1281,6 +1361,69 @@ static plf_status upload_pairs(plf_ctx* ctx, cudaStream_t cs, uint8_t* dst, int 
       PLF_CUDA(ctx, cudaMemcpy3DAsync(&cp, cs));
     }
   }
+  return PLF_OK;
+}
+
+// ---- plf_set_sequence_params: the classification of plf_params' fields, the one place the library and the binding read
+// it from (plf_sequence_param_fields).  SEQUENCE: read per pair or per image by the batched front-end; CONTEXT: fixes
+// buffer geometry, lookup tables, tensor maps or which launch chains exist; IGNORED: has no effect for the context either.
+struct ParamField {
+  const char* name;
+  size_t off;
+  char type;   // 'i' int, 'f' float, 'd' double
+  int cls;
+};
+#define PLF_PF(f, t, c) {#f, offsetof(plf_params, f), t, PLF_PARAM_##c}
+static const ParamField kParamFields[] = {
+    PLF_PF(has_points, 'i', CONTEXT),       PLF_PF(has_lines, 'i', CONTEXT),          PLF_PF(best_lr_matches, 'i', SEQUENCE),
+    PLF_PF(max_dist_epip, 'f', SEQUENCE),   PLF_PF(min_disp, 'f', SEQUENCE),          PLF_PF(min_ratio_12_p, 'f', SEQUENCE),
+    PLF_PF(line_sim_th, 'f', SEQUENCE),     PLF_PF(stereo_overlap_th, 'f', SEQUENCE), PLF_PF(f2f_overlap_th, 'f', IGNORED),
+    PLF_PF(min_line_length, 'f', SEQUENCE), PLF_PF(line_horiz_th, 'f', SEQUENCE),     PLF_PF(min_ratio_12_l, 'f', SEQUENCE),
+    PLF_PF(ls_min_disp_ratio, 'f', SEQUENCE), PLF_PF(homog_th, 'd', SEQUENCE),        PLF_PF(min_features, 'i', SEQUENCE),
+    PLF_PF(max_iters, 'i', SEQUENCE),       PLF_PF(max_iters_ref, 'i', SEQUENCE),     PLF_PF(min_error, 'd', SEQUENCE),
+    PLF_PF(min_error_change, 'd', SEQUENCE), PLF_PF(inlier_k, 'd', IGNORED),          PLF_PF(orb_nfeatures, 'i', SEQUENCE),
+    PLF_PF(orb_scale_factor, 'f', CONTEXT), PLF_PF(orb_nlevels, 'i', SEQUENCE),       PLF_PF(orb_edge_th, 'i', CONTEXT),
+    PLF_PF(orb_wta_k, 'i', CONTEXT),        PLF_PF(orb_score, 'i', CONTEXT),          PLF_PF(orb_patch_size, 'i', CONTEXT),
+    PLF_PF(orb_fast_th, 'i', SEQUENCE),     PLF_PF(lsd_nfeatures, 'i', SEQUENCE),     PLF_PF(lsd_refine, 'i', CONTEXT),
+    PLF_PF(lsd_scale, 'd', CONTEXT),        PLF_PF(lsd_sigma_scale, 'd', CONTEXT),    PLF_PF(lsd_quant, 'd', CONTEXT),
+    PLF_PF(lsd_ang_th, 'd', CONTEXT),       PLF_PF(lsd_log_eps, 'd', CONTEXT),        PLF_PF(lsd_density_th, 'd', CONTEXT),
+    PLF_PF(lsd_n_bins, 'i', CONTEXT),       PLF_PF(matching_strategy, 'i', SEQUENCE), PLF_PF(matching_s_ws, 'i', SEQUENCE),
+    PLF_PF(matching_f2f_ws, 'i', SEQUENCE), PLF_PF(min_pt_matches, 'i', SEQUENCE),    PLF_PF(min_ls_matches, 'i', SEQUENCE),
+};
+#undef PLF_PF
+
+static double param_value(const plf_params& p, const ParamField& f) {
+  const uint8_t* a = reinterpret_cast<const uint8_t*>(&p) + f.off;
+  if (f.type == 'i') return *reinterpret_cast<const int*>(a);
+  if (f.type == 'f') return *reinterpret_cast<const float*>(a);
+  return *reinterpret_cast<const double*>(a);
+}
+
+// What plf_set_sequence_params refuses in p for a context of settings c, naming the field; PLF_OK if nothing.
+static plf_status check_sequence_params(plf_ctx* ctx, const plf_params& p) {
+  const plf_params& c = ctx->params;
+  for (const ParamField& f : kParamFields) {
+    const double v = param_value(p, f), cv = param_value(c, f);
+    if (f.cls == PLF_PARAM_CONTEXT) {
+      if (v != cv && !(std::isnan(v) && std::isnan(cv)))
+        return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_params: %s = %.17g, the context's is %.17g; it fixes the context's "
+                        "buffers, tables or launches and must equal it", f.name, v, cv);
+    } else if (f.cls == PLF_PARAM_SEQUENCE) {
+      // counts and integer thresholds >= 0, real thresholds finite
+      if (f.type == 'i' && v < 0)
+        return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_params: %s = %d, need %s >= 0", f.name, (int)v, f.name);
+      if (f.type != 'i' && !std::isfinite(v))
+        return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_params: %s = %g, need a finite value", f.name, v);
+    }
+  }
+  // the ORB buffers, tables and tensor maps hold the context's levels; a level does not depend on those after it
+  if (p.orb_nlevels < 1 || p.orb_nlevels > c.orb_nlevels)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_params: orb_nlevels = %d, need 1 <= orb_nlevels <= the context's %d",
+                    p.orb_nlevels, c.orb_nlevels);
+  // the windowed matcher's buffers exist only in a context created windowed
+  if (p.matching_strategy != 0 && c.matching_strategy == 0)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_set_sequence_params: matching_strategy = %d, and the context's is 0: a sequence may "
+                    "be windowed only in a context created with matching_strategy != 0", p.matching_strategy);
   return PLF_OK;
 }
 
@@ -1469,6 +1612,41 @@ plf_status plf_get_sequence_camera(const plf_ctx* ctx, int s, plf_camera* out) {
   return PLF_OK;
 }
 
+int plf_sequence_param_fields(const char** names, int* classes, int cap) {
+  const int n = (int)(sizeof kParamFields / sizeof kParamFields[0]);
+  for (int i = 0; i < n && i < cap; ++i) {
+    if (names) names[i] = kParamFields[i].name;
+    if (classes) classes[i] = kParamFields[i].cls;
+  }
+  return n;
+}
+
+plf_status plf_set_sequence_params(plf_ctx* ctx, int s, const plf_params* p) {
+  if (!ctx) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_set_sequence_params: ctx is NULL");
+  if (plf_status st = plf_check_sequence(ctx, "plf_set_sequence_params", s)) return st;
+  if (p) {
+    if (plf_status st = check_sequence_params(ctx, *p)) return st;
+    PlfSequence& q = plf_sequence(ctx, s);
+    q.own_prm = true;
+    q.prm = *p;
+    q.pair = plf_pair_prm(*p);
+  } else if (!ctx->seqs.empty()) {
+    ctx->seqs[s].own_prm = false;
+  }
+  // its carried frame was extracted and matched under the old settings
+  restart_sequence(ctx, s);
+  return PLF_OK;
+}
+
+plf_status plf_get_sequence_params(const plf_ctx* ctx, int s, plf_params* out) {
+  if (!ctx) return plf_fail(nullptr, PLF_ERR_INVALID, "plf_get_sequence_params: ctx is NULL");
+  plf_ctx* c = const_cast<plf_ctx*>(ctx);   // the error text is the only state a failed call writes
+  if (!out) return plf_fail(c, PLF_ERR_INVALID, "plf_get_sequence_params: out is NULL");
+  if (plf_status st = plf_check_sequence(c, "plf_get_sequence_params", s)) return st;
+  *out = !ctx->seqs.empty() && ctx->seqs[s].own_prm ? ctx->seqs[s].prm : ctx->params;
+  return PLF_OK;
+}
+
 plf_status plf_set_adaptive_fast(plf_ctx* ctx, const plf_adaptive_fast* cfg) {
   if (cfg) {   // checked first, so that a NULL context reports the field too (plf_last_error(NULL))
     const plf_adaptive_fast& a = *cfg;
@@ -1497,7 +1675,7 @@ plf_status plf_get_sequence_fast_th(plf_ctx* ctx, int s, int* th) {
   if (!ctx) return PLF_ERR_INVALID;
   if (!th) return plf_fail(ctx, PLF_ERR_INVALID, "plf_get_sequence_fast_th: th is NULL");
   if (plf_status st = plf_check_sequence(ctx, "plf_get_sequence_fast_th", s)) return st;
-  *th = fast_th0(ctx);
+  *th = !ctx->seqs.empty() && ctx->seqs[s].own_prm ? ctx->seqs[s].pair.fast_th : fast_th0(ctx);
   if (!ctx->afast_on || !ctx->pipe || !ctx->pipe->carried[s]) return PLF_OK;   // the next pair is detected at orb_fast_th
   SeqRecord q;
   if (plf_status st = pipe_seq_read(ctx, s, &q)) return st;
@@ -1783,8 +1961,10 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   r.cams = false;
   r.nin = 0;
   r.masked = false;
+  r.prm = false;
   bool rect = false;
   for (int k = 0; k < B; ++k) {
+    r.prm |= !ctx->seqs.empty() && ctx->seqs[q[k]].own_prm;
     const plf_camera& c = plf_sequence_camera(ctx, q[k]);
     tab.cams[k] = PlfPairCam{c.fx, c.fy, c.cx, c.cy, c.b};
     r.cams |= &c != &ctx->cam;
@@ -1798,6 +1978,20 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
     }
   }
   if (!rect) r.nin = 0;
+  // the settings of the pairs, resolved now as the cameras are: a table only when a sequence of the batch has its own
+  r.nwin = ctx->params.matching_strategy ? B : 0;
+  r.best_lr = ctx->params.best_lr_matches != 0;
+  if (r.prm) {
+    const PlfPairPrm own0 = plf_pair_prm(ctx->params);
+    r.nwin = 0;
+    r.best_lr = false;
+    for (int k = 0; k < B; ++k) {
+      const PlfSequence& sq = ctx->seqs[q[k]];
+      tab.prm[k] = sq.own_prm ? sq.pair : own0;
+      r.nwin += tab.prm[k].matching_strategy != 0;
+      r.best_lr |= tab.prm[k].best_lr != 0;
+    }
+  }
   r.run_slot = s->up_slot;
   // With profiling on everything is serialised on the main stream so that the per-kernel marks are meaningful.
   r.piped = !ctx->profile || ctx->profile_piped;

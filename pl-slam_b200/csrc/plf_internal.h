@@ -88,8 +88,28 @@ struct LsdState;      // lsd.cu
 struct PlfTmaCache;   // plf_tma.cuh
 struct BowDbs;        // dbow.cu
 
+#define PLF_ORB_MAX_LEVELS 8
+// The front-end settings of one pair of a batch (plf_set_sequence_params): its sequence's plf_params, as the consumers read
+// them, resolved when the batch was run.  A consumer given no table reads the context's plf_params instead.
+struct PlfPairPrm {
+  int orb_nlevels;                       // <= the context's: the levels the pair's images detect on
+  int orb_nfeat[PLF_ORB_MAX_LEVELS];     // nfeaturesPerLevel of orb_nfeatures over orb_nlevels (plf_orb_level_features)
+  int fast_th;                           // orb_fast_th clamped to [0, 255], the first frame's FAST threshold
+  int lsd_nfeatures;
+  float min_line_length;
+  float max_dist_epip, min_disp, line_horiz_th, stereo_overlap_th, ls_min_disp_ratio;
+  float min_ratio_12_p, min_ratio_12_l, line_sim_th;
+  int best_lr;
+  int matching_strategy, matching_s_ws, matching_f2f_ws, min_pt_matches, min_ls_matches, min_features;
+  plf_gn_opts gn;                        // plf_gn_opts_from_params
+};
+PlfPairPrm plf_pair_prm(const plf_params& p);
+
 // What one sequence of a batched context has of its own; plf_reset_sequence keeps it, plf_drop_sequences frees it.
 struct PlfSequence {
+  bool own_prm = false;     // plf_set_sequence_params: prm (and pair, its device form) are the sequence's settings
+  plf_params prm = {};
+  PlfPairPrm pair = {};
   bool own_cam = false;     // plf_set_sequence_camera: cam is the sequence's calibration, else it uses the context's
   plf_camera cam = {};
   uint8_t* rect = nullptr;  // plf_set_sequence_rectification: device block of 12 w h bytes (PLF_RECT_* layout, pipeline.cu)
@@ -243,6 +263,10 @@ struct MgbArgs {
   int* m21;
   int32_t* m12; size_t m12_stride;       // output rows of problem p: m12 + p * m12_stride
   int* count; int count_stride;          // matches of problem p (accumulated; zeroed by the caller)
+  // optional [P]: problem p takes its window (matching_f2f_ws on every side when f2f, else (matching_s_ws, 0) x (0, 0)),
+  // nnr, best_lr and line_sim_th from prm[p] instead of the fields above (the batched front-end's pairs)
+  const struct PlfPairPrm* prm;
+  int f2f;
 };
 // max_n1 / max_n2: upper bounds of the query / train counts; slot: the scratch slot D, the query masks and m21 live in;
 // cs: the stream the launches are enqueued on.
@@ -278,8 +302,9 @@ struct PlfPairCam { double fx, fy, cx, cy, b; };
 plf_gn_opts plf_gn_opts_from_params(const plf_params& p);
 // d_cams: optional [nprob] device array, the camera of each problem (b unused); null = the context's camera.
 // d_active: optional [nprob] device flags; a problem whose flag is 0 is not solved (its out and flags are not written).
+// d_prm: optional [nprob] device array; problem p solves with d_prm[p].gn instead of o.
 plf_status plf_launch_gn(plf_ctx* ctx, cudaStream_t cs, const GnProblem* d_probs, int nprob, const plf_gn_opts& o,
-                         const PlfPairCam* d_cams = nullptr, const int* d_active = nullptr);
+                         const PlfPairCam* d_cams = nullptr, const int* d_active = nullptr, const PlfPairPrm* d_prm = nullptr);
 
 // ---- tiled LDL^T (lba.cu) ------------------------------------------------------------------------
 // Factors each symmetric n x n matrix S (n = 6 nkf; row-major, leading dimension n; only its lower triangle is read) in
@@ -318,8 +343,12 @@ void plf_orb_free(OrbState* s);
 // img_th: the FAST threshold of each image, on the device (plf_set_adaptive_fast), or NULL for plf_params.orb_fast_th.
 // masks: a device table of each image's mask pyramid (plf_orb_mask_build), an entry NULL for an unmasked image, or NULL
 // for no mask at all (the unmasked FAST kernel).
+// prm: a device table of pair settings, prm[z / 2] for image z (plf_set_sequence_params: its level count, at most the
+// state's, and per-level counts), or NULL for plf_params' own.
 plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par,
-                       const int* img_th, const uint8_t* const* masks);
+                       const int* img_th, const uint8_t* const* masks, const PlfPairPrm* prm = nullptr);
+// nfeaturesPerLevel of cv::ORB (orb.cpp computeKeyPoints): nfeat[l] for l < nlevels.
+void plf_orb_level_features(int nfeatures, float scale_factor, int nlevels, int* nfeat);
 // One image's mask pyramid in s's level layout: its bytes (allocate 64 more, as every image buffer), and its build from a
 // host mask of s->w x s->h, stride bytes per row, on cs.  Its first plf_pitch16(w) * h bytes are the mask itself.
 size_t plf_orb_mask_bytes(const OrbState* s);
@@ -354,9 +383,10 @@ void plf_lsd_free(LsdState* s);
 size_t plf_lsd_footprint(const plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities);
 plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int par, int n);
 // keylines_wait: if set, the KeyLine outputs are overwritten only after this event.  masks: as for plf_orb_run; the KeyLine
-// stage reads level 0 (plf_pitch16(w) bytes per row) of each listed image.
+// stage reads level 0 (plf_pitch16(w) bytes per row) of each listed image.  prm: as for plf_orb_run, image z's
+// lsd_nfeatures and min_line_length from prm[z / 2].
 plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int n, cudaEvent_t keylines_wait,
-                        const uint8_t* const* masks);
+                        const uint8_t* const* masks, const PlfPairPrm* prm = nullptr);
 void plf_lsd_outputs(const LsdState* s, int par, plf_keyline** kls, int** nlines, int* max_lines);
 // Causes of the LSD overflow flag, one bit each (as the ORB flag above)
 enum { PLF_LSD_OVF_SEGMENTS = 1,   // an image grows more regions than plf_limits.max_segments (k_lsd_grow)

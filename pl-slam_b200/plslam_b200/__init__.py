@@ -395,6 +395,8 @@ def load_library() -> C.CDLL:
     lib = C.CDLL(str(LIB_PATH))
     lib.plf_last_error.restype = C.c_char_p
     lib.plf_last_error.argtypes = [C.c_void_p]
+    lib.plf_sequence_param_fields.restype = C.c_int
+    lib.plf_sequence_param_fields.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.c_int]
     lib.plf_launch_count.restype = C.c_longlong
     lib.plf_launch_count.argtypes = [C.c_void_p]
     lib.plf_stream.restype = C.c_void_p
@@ -452,6 +454,20 @@ def _i32_or_null(a):
 
 def _lba_opts(lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, ref_quirks):
     return plf_lba_opts(lambda_, lambda_k, max_iters, homog_th, min_error, min_error_change, int(ref_quirks))
+
+
+PARAM_CLASSES = {1: "sequence", 2: "context", 3: "ignored"}   # PLF_PARAM_SEQUENCE, _CONTEXT, _IGNORED
+
+
+def sequence_param_fields():
+    """{plf_params field: "sequence" | "context" | "ignored"}: how Frontend.set_sequence_params treats each field, as the
+    library classifies them (plf_sequence_param_fields).  "sequence" fields may differ per sequence, "context" fields
+    must equal the context's, "ignored" fields have no effect."""
+    lib = load_library()
+    n = lib.plf_sequence_param_fields(None, None, 0)
+    names, classes = (C.c_char_p * n)(), (C.c_int * n)()
+    lib.plf_sequence_param_fields(names, classes, n)
+    return {names[i].decode(): PARAM_CLASSES[classes[i]] for i in range(n)}
 
 
 class Frontend:
@@ -1291,6 +1307,30 @@ class Frontend:
         cam = None if camera is None else (camera if isinstance(camera, plf_camera) else plf_camera(**camera))
         self._check(self.lib.plf_set_sequence_camera(self._ctx, int(s), None if cam is None else C.byref(cam)),
                     "plf_set_sequence_camera")
+
+    def set_sequence_params(self, s, params=None, **fields):
+        """Gives sequence s its own front-end settings: params (a plf_params, default the context's) with the named fields
+        replaced, e.g. set_sequence_params(1, lsd_nfeatures=300, matching_strategy=3).  No params and no fields returns s
+        to the context's settings.  sequence_param_fields() tells which fields may differ.  Either restarts s: its next
+        pair in a run is a first frame.  Batches already run keep their settings.  plf_set_sequence_params."""
+        if params is None and not fields:
+            self._check(self.lib.plf_set_sequence_params(self._ctx, int(s), None), "plf_set_sequence_params")
+            return
+        p = plf_params()
+        C.pointer(p)[0] = params if params is not None else self.params
+        names = {name for name, _ in plf_params._fields_}
+        for k, v in fields.items():
+            if k not in names:
+                raise PlfError(f"unknown parameter {k}")
+            setattr(p, k, v)
+        self._check(self.lib.plf_set_sequence_params(self._ctx, int(s), C.byref(p)), "plf_set_sequence_params")
+
+    def get_sequence_params(self, s):
+        """The settings the next batch uses for sequence s, its own or the context's, as a plf_params.
+        plf_get_sequence_params."""
+        out = plf_params()
+        self._check(self.lib.plf_get_sequence_params(self._ctx, int(s), C.byref(out)), "plf_get_sequence_params")
+        return out
 
     def sequence_camera(self, s):
         """The calibration the next batch uses for sequence s, as a camera dict.  plf_get_sequence_camera."""
