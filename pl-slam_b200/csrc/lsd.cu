@@ -996,11 +996,12 @@ __global__ void __launch_bounds__(128) k_lsd_rects(const LsdPix* __restrict__ pi
 // NULL.  A KeyLine whose two end points both truncate onto a 0 of the mask is deleted after the length filter and before
 // the top-K, keeping the class_id it was given among the lines of sufficient length (LSDDetector_custom.cpp:310-322 runs
 // after :299 numbers them).  The unmasked instantiation ignores masks.
-// prm (plf_lsd_grow): image im takes nfeatures and min_length from its pair's settings prm[im / 2].
+// prm (plf_lsd_grow): image im keeps the top lsd_nfeatures of the lines longer than min_line_length min(w, h), its pair's
+// settings prm[im / 2].
 #define KL_SORT_CAP 4096
 template <bool MASKED>
 __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ segs_all, const int* __restrict__ nsegs,
-                                                   int max_regions, int w, int h, double min_length, int nfeatures,
+                                                   int max_regions, int w, int h,
                                                    plf_keyline* __restrict__ kls_all, plf_keyline* __restrict__ kls_out,
                                                    int max_lines, int* __restrict__ nlines, int* __restrict__ overflow,
                                                    const uint8_t* const* __restrict__ masks, const PlfPairPrm* __restrict__ prm) {
@@ -1008,10 +1009,8 @@ __global__ void __launch_bounds__(1024) k_keylines(const float4* __restrict__ se
   __shared__ int s_scan[1024];
   __shared__ int s_total;
   const int im = blockIdx.x, tid = threadIdx.x;
-  if (prm) {   // as plf_lsd_grow derives them from plf_params
-    nfeatures = prm[im >> 1].lsd_nfeatures;
-    min_length = (double)prm[im >> 1].min_line_length * (double)min(w, h);
-  }
+  const int nfeatures = prm[im >> 1].lsd_nfeatures;
+  const double min_length = (double)prm[im >> 1].min_line_length * (double)min(w, h);
   const int n = min(nsegs[im], max_regions);
   const float4* segs = segs_all + (size_t)im * max_regions;
   plf_keyline* all = kls_all + (size_t)im * max_regions;
@@ -1441,13 +1440,12 @@ plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int
                                                                      s->rect_perm, T.prec, s->scale, s->segs);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "lsd.k_lsd_rects");
-  const double min_length = (double)ctx->params.min_line_length * (double)std::min(w, h);
   if (keylines_wait) PLF_CUDA(ctx, cudaStreamWaitEvent(cs, keylines_wait, 0));
   if (masks)
-    k_keylines<true><<<n, 1024, 0, cs>>>(s->segs, s->nregions, s->max_regions, w, h, min_length, ctx->params.lsd_nfeatures, s->kls_all,
+    k_keylines<true><<<n, 1024, 0, cs>>>(s->segs, s->nregions, s->max_regions, w, h, s->kls_all,
                                          s->kls[par], s->max_lines, s->nlines[par], s->overflow, masks, prm);
   else
-    k_keylines<false><<<n, 1024, 0, cs>>>(s->segs, s->nregions, s->max_regions, w, h, min_length, ctx->params.lsd_nfeatures, s->kls_all,
+    k_keylines<false><<<n, 1024, 0, cs>>>(s->segs, s->nregions, s->max_regions, w, h, s->kls_all,
                                           s->kls[par], s->max_lines, s->nlines[par], s->overflow, nullptr, prm);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "lsd.k_keylines");
@@ -1476,8 +1474,10 @@ void plf_lsd_outputs(const LsdState* s, int par, plf_keyline** kls, int** nlines
   *kls = s->kls[par]; *nlines = s->nlines[par]; *max_lines = s->max_lines;
 }
 
-// LSD of the standalone operators on one w x h image at dimg, in ctx->lsd_standalone (rebuilt when the size changes).
-static plf_status lsd_standalone(plf_ctx* ctx, const uint8_t* dimg, int pitch, int w, int h, const uint8_t* const* masks) {
+// LSD of the standalone operators on one w x h image at dimg, in ctx->lsd_standalone (rebuilt when the size changes).  prm:
+// a one-entry device table of the context's settings.
+static plf_status lsd_standalone(plf_ctx* ctx, const uint8_t* dimg, int pitch, int w, int h, const uint8_t* const* masks,
+                                 const PlfPairPrm* prm) {
   LsdState*& s = ctx->lsd_standalone;
   plf_status st;
   if (s && (s->w != w || s->h != h)) {
@@ -1487,7 +1487,7 @@ static plf_status lsd_standalone(plf_ctx* ctx, const uint8_t* dimg, int pitch, i
   }
   if (!s && (st = plf_lsd_create(ctx, w, h, 1, false, &s))) return st;
   if ((st = plf_lsd_pre(ctx, ctx->stream, s, dimg, (size_t)pitch * h, pitch, 0, 1))) return st;
-  return plf_lsd_grow(ctx, ctx->stream, s, 0, 1, nullptr, masks);
+  return plf_lsd_grow(ctx, ctx->stream, s, 0, 1, nullptr, masks, prm);
 }
 
 // `causes`: the ones that spoil what the caller returns.  plf_lsd returns the raw segments, which the KeyLine stage's
@@ -1512,10 +1512,14 @@ extern "C" plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_lsd: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   const int pitch = plf_pitch16(w);
-  uint8_t* dimg = (uint8_t*)plf_scratch(ctx, PLF_SCR_LSD, (size_t)pitch * h);
-  if (!dimg) return PLF_ERR_CUDA;
+  uint8_t* dimg;
+  PlfPairPrm* dprm;
+  DevBufList scr;
+  scr.add(dimg, (size_t)pitch * h); scr.add(dprm, 1);
+  if (plf_status st = scr.carve(ctx, PLF_SCR_LSD)) return st;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  plf_status st = lsd_standalone(ctx, dimg, pitch, w, h, nullptr);
+  PLF_CUDA(ctx, cudaMemcpyAsync(dprm, &ctx->pair, sizeof(PlfPairPrm), cudaMemcpyHostToDevice, ctx->stream));
+  plf_status st = lsd_standalone(ctx, dimg, pitch, w, h, nullptr, dprm);
   if (st) return st;
   const LsdState* s = ctx->lsd_standalone;
   int n = 0;
@@ -1531,26 +1535,29 @@ extern "C" plf_status plf_lsd(plf_ctx* ctx, const uint8_t* img, int w, int h, in
   return PLF_OK;
 }
 
-// plf_detect_lines and plf_detect_lines_masked (mask NULL: unmasked).  The mask (level 0 of the pyramid layout, one
-// plane) and its one-entry table live in PLF_SCR_LSD beside the image.
+// plf_detect_lines and plf_detect_lines_masked (mask NULL: unmasked).  The one-entry settings table (the context's), and the
+// mask (level 0 of the pyramid layout, one plane) and its one-entry table, live in PLF_SCR_LSD beside the image.
 static plf_status detect_lines(plf_ctx* ctx, const char* fn, const uint8_t* img, int w, int h, int stride, const uint8_t* mask,
                                int mask_stride, plf_keyline* keylines, uint8_t* desc, int cap, int* n_out) {
   const int pitch = plf_pitch16(w);
   uint8_t *dimg, *ddesc, *dmask = nullptr;
   const uint8_t** dtab = nullptr;
   short2* dgrad;
+  PlfPairPrm* dprm;
   DevBufList scr;
   scr.add(dimg, (size_t)pitch * h); scr.add(dgrad, (size_t)w * h); scr.add(ddesc, (size_t)ctx->limits.max_lines * 32);
+  scr.add(dprm, 1);
   if (mask) { scr.add(dmask, (size_t)pitch * h); scr.add(dtab, 1); }
   if (plf_status st = scr.carve(ctx, PLF_SCR_LSD)) return st;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
+  PLF_CUDA(ctx, cudaMemcpyAsync(dprm, &ctx->pair, sizeof(PlfPairPrm), cudaMemcpyHostToDevice, ctx->stream));
   if (mask) {
     const uint8_t* hp = dmask;
     PLF_CUDA(ctx, cudaMemcpy2DAsync(dmask, pitch, mask, mask_stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
     PLF_CUDA(ctx, cudaMemcpyAsync(dtab, &hp, sizeof hp, cudaMemcpyHostToDevice, ctx->stream));
     PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // hp is on this stack frame
   }
-  plf_status st = lsd_standalone(ctx, dimg, pitch, w, h, dtab);
+  plf_status st = lsd_standalone(ctx, dimg, pitch, w, h, dtab, dprm);
   if (st) return st;
   const LsdState* s = ctx->lsd_standalone;
   PlfTmaCache tm;

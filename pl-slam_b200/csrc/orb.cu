@@ -41,7 +41,6 @@ struct OrbGeom {
   int pitch[ORB_MAX_LEVELS];        // row pitch (bytes, multiple of 16) of level l; level 0 = the caller's image pitch
   int bpitch[ORB_MAX_LEVELS];       // row pitch of the blurred level l
   float scale[ORB_MAX_LEVELS];
-  int nfeat[ORB_MAX_LEVELS];
   int umax[20];
   size_t pyr_off[ORB_MAX_LEVELS];   // byte offset of level l (l>=1) inside one image's pyramid block
   size_t pyr_stride;                // bytes of levels 1.. per image
@@ -52,7 +51,7 @@ struct OrbGeom {
   size_t cand_stride;
   int tile_start[ORB_MAX_LEVELS + 1];  // FAST tiles: prefix over levels
   int tiles_x[ORB_MAX_LEVELS];
-  int edge, fast_th, patch, half_patch;
+  int edge, patch, half_patch;
   int max_kp;
   float blur7[7];                   // getGaussianKernel(7, 2, CV_32F), the taps of k_orb_blur7_fast
 };
@@ -233,7 +232,8 @@ __host__ __device__ __forceinline__ size_t orb_mask_off(const OrbGeom& g, int l)
 // MASKED (plf_set_sequence_mask, plf_orb_masked): masks[img] is image img's mask pyramid, or NULL; an NMS survivor whose
 // level mask is 0 is dropped before it reaches the candidate list and the histogram (KeyPointsFilter::runByPixelsMask
 // after FAST).  The unmasked instantiation ignores masks.
-// prm (plf_orb_run): an image whose pair detects on fewer levels than l + 1 does nothing on level l.
+// prm (plf_orb_run): an image whose pair detects on fewer levels than l + 1 writes nothing on level l; without img_th an
+// image detects at its pair's fast_th.
 template <bool MASKED>
 __global__ void __launch_bounds__(256, 5) k_fast_nms(const __grid_constant__ CUtensorMap tmap, OrbGeom g, int l, int tiles_x,
                                                   const int* __restrict__ img_th, uint32_t* __restrict__ cand, int* __restrict__ cand_count,
@@ -242,7 +242,8 @@ __global__ void __launch_bounds__(256, 5) k_fast_nms(const __grid_constant__ CUt
   const int W = g.w[l], H = g.h[l];
   const int x0 = (blockIdx.x % tiles_x) * FN_OW, y0 = (blockIdx.x / tiles_x) * FN_OH;
   const int img = blockIdx.y;
-  if (prm && l >= prm[img >> 1].orb_nlevels) return;
+  // the pair's settings, read before the tile's copy is issued and used once it has landed
+  const int nlevels = prm[img >> 1].orb_nlevels, fast_th = prm[img >> 1].fast_th;
   __shared__ __align__(128) uint8_t pxb[38][96];  // the TMA box (96 x 38 bytes) from the 16-byte boundary at or below x0 - 4
   __shared__ __align__(16) uint8_t sc[32][64];    // score of pixel (x0 - 1 + sx, y0 - 1 + sy)
   __shared__ unsigned short clist[32 * 64];
@@ -262,10 +263,11 @@ __global__ void __launch_bounds__(256, 5) k_fast_nms(const __grid_constant__ CUt
   const int boxoff = (x0 - 4) - xs;   // box column of pixel x0 - 4
   // px[ry][rx] = pixel (x0 - 4 + rx, y0 - 4 + ry)
   const uint8_t (*px)[96] = reinterpret_cast<const uint8_t (*)[96]>(&pxb[0][boxoff]);
-  const int th = img_th ? img_th[img] : g.fast_th;   // per image with the adaptive FAST threshold, in [0, 255] either way
+  const int th = img_th ? img_th[img] : fast_th;   // per image with the adaptive FAST threshold, in [0, 255] either way
   const uint32_t k7 = (uint32_t)(0x7f - (th & 0x7f)) * 0x01010101u;
   const bool th_small = th < 128;
   plf_mbar_wait(&bar, 0);
+  if (l >= nlevels) return;   // the whole block: nothing written yet, and the tile's copy has completed
   // ---- pass A: score pixel (sy, sx) sits at box row sy + 3, box column c_first + sx
   const int c_first = boxoff + 3, w_first = c_first >> 2, nwords = ((c_first + 63) >> 2) - w_first + 1;   // 16 or 17 words
   for (int gi = tid; gi < 32 * 17; gi += 256) {
@@ -385,7 +387,7 @@ __global__ void __launch_bounds__(1024) k_select_sort(OrbGeom g, const uint32_t*
     if (tid == 0) {
       s_cnt = 0;
       int thr = 0;
-      const int want = prm ? prm[img >> 1].orb_nfeat[l] : g.nfeat[l];
+      const int want = prm[img >> 1].orb_nfeat[l];
       if (want < n) {
         if (want == 0) {
           thr = 256;
@@ -710,7 +712,7 @@ static plf_status orb_layout(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, 
   OrbGeom& g = s->g;
   memset(&g, 0, sizeof g);
   g.nlevels = P.orb_nlevels;
-  g.edge = P.orb_edge_th; g.fast_th = min(max(P.orb_fast_th, 0), 255);
+  g.edge = P.orb_edge_th;
   g.patch = P.orb_patch_size; g.half_patch = P.orb_patch_size / 2;
   g.max_kp = ctx->limits.max_keypoints;
   const double scaleFactor = (double)P.orb_scale_factor;
@@ -738,7 +740,6 @@ static plf_status orb_layout(plf_ctx* ctx, OrbState* s, int w, int h, int nimg, 
   g.tile_start[g.nlevels] = tiles;
   for (int l = g.nlevels + 1; l <= ORB_MAX_LEVELS; ++l) g.tile_start[l] = tiles;
   g.pyr_stride = pyr; g.blur_stride = blur; g.cand_stride = cand;
-  plf_orb_level_features(P.orb_nfeatures, P.orb_scale_factor, g.nlevels, g.nfeat);
   {  // getGaussianKernel(7, 2, CV_32F): host doubles -> float (pinned equal to cv2 in tests)
     double d[7], sum = 0;
     for (int i = 0; i < 7; ++i) {
@@ -964,8 +965,8 @@ plf_status plf_orb_mask_build(plf_ctx* ctx, cudaStream_t cs, const OrbState* s, 
   return PLF_OK;
 }
 
-// plf_orb and plf_orb_masked (mask NULL: unmasked).  The mask pyramid and its one-entry table live in PLF_SCR_ORB beside
-// the image.
+// plf_orb and plf_orb_masked (mask NULL: unmasked).  The one-entry settings table (the context's), and the mask pyramid
+// and its one-entry table, live in PLF_SCR_ORB beside the image.
 static plf_status orb_standalone(plf_ctx* ctx, const char* fn, const uint8_t* img, int w, int h, int stride, const uint8_t* mask,
                                  int mask_stride, plf_keypoint* kps, uint8_t* desc, int cap, int* n_out) {
   OrbState*& s = ctx->orb_standalone;
@@ -977,23 +978,22 @@ static plf_status orb_standalone(plf_ctx* ctx, const char* fn, const uint8_t* im
   }
   if (!s && (st = plf_orb_create(ctx, w, h, 1, false, &s))) return st;
   const int pitch = plf_pitch16(w);
-  uint8_t* dimg;
+  uint8_t *dimg, *dmask;
   const uint8_t** dtab = nullptr;
-  if (!mask) {
-    dimg = (uint8_t*)plf_scratch(ctx, PLF_SCR_ORB, (size_t)pitch * h);
-    if (!dimg) return PLF_ERR_CUDA;
-  } else {
-    uint8_t* dmask;
-    DevBufList scr;
-    scr.add(dimg, (size_t)pitch * h); scr.add(dmask, plf_orb_mask_bytes(s) + 64); scr.add(dtab, 1);
-    if ((st = scr.carve(ctx, PLF_SCR_ORB))) return st;
+  PlfPairPrm* dprm;
+  DevBufList scr;
+  scr.add(dimg, (size_t)pitch * h); scr.add(dprm, 1);
+  if (mask) { scr.add(dmask, plf_orb_mask_bytes(s) + 64); scr.add(dtab, 1); }
+  if ((st = scr.carve(ctx, PLF_SCR_ORB))) return st;
+  PLF_CUDA(ctx, cudaMemcpyAsync(dprm, &ctx->pair, sizeof(PlfPairPrm), cudaMemcpyHostToDevice, ctx->stream));
+  if (mask) {
     if ((st = plf_orb_mask_build(ctx, ctx->stream, s, mask, mask_stride, dmask))) return st;
     const uint8_t* hp = dmask;
     PLF_CUDA(ctx, cudaMemcpyAsync(dtab, &hp, sizeof hp, cudaMemcpyHostToDevice, ctx->stream));
     PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // hp is on this stack frame
   }
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dimg, pitch, img, stride, w, h, cudaMemcpyHostToDevice, ctx->stream));
-  if ((st = plf_orb_run(ctx, ctx->stream, s, dimg, (size_t)pitch * h, pitch, 1, 0, nullptr, dtab))) return st;
+  if ((st = plf_orb_run(ctx, ctx->stream, s, dimg, (size_t)pitch * h, pitch, 1, 0, nullptr, dtab, dprm))) return st;
   int n = 0, ovf = 0;
   PLF_CUDA(ctx, cudaMemcpyAsync(&n, s->kp_count[0], sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaMemcpyAsync(&ovf, s->overflow, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));

@@ -50,28 +50,29 @@ constexpr int PLF_FS_NFIELDS = 0 PLF_PT_FIELDS(PLF_FS_ONE) PLF_LS_FIELDS(PLF_FS_
 struct PlfRectPair { const uint8_t* maps; int pair; int pad; };
 
 // One entry of the batch table ring, for max_batch pairs B: the sequence table (prev[B] = the frame slot of pair k's
-// previous frame, then the carry list [B][2] of (frame slot, carry slot)), the pairs' cameras [B], the input table [B],
-// the mask table [2B] (image z's mask pyramid, plf_set_sequence_mask, or NULL) and the pairs' settings [B]
-// (plf_set_sequence_params).  The pinned and the device ring use the same layout.
+// previous frame, then the carry list [B][2] of (frame slot, carry slot)), the pairs' cameras [B] and settings [B]
+// (plf_set_sequence_camera, plf_set_sequence_params, else the context's), then the input table [B] and the mask table
+// [2B] (image z's mask pyramid, plf_set_sequence_mask, or NULL).  Every batch uses the parts before the input table: they
+// are one copy.  The pinned and the device ring use the same layout.
 struct BatchTab {
   int32_t* prev;
   int32_t* carry;
   PlfPairCam* cams;
+  PlfPairPrm* prm;
   PlfRectPair* in;
   const uint8_t** masks;
-  PlfPairPrm* prm;
 };
 static size_t batch_tab_bytes(int B) {
-  return plf_align256(3 * sizeof(int32_t) * B) + plf_align256(sizeof(PlfPairCam) * B) + plf_align256(sizeof(PlfRectPair) * B) +
-         plf_align256(sizeof(uint8_t*) * 2 * B) + plf_align256(sizeof(PlfPairPrm) * B);
+  return plf_align256(3 * sizeof(int32_t) * B) + plf_align256(sizeof(PlfPairCam) * B) + plf_align256(sizeof(PlfPairPrm) * B) +
+         plf_align256(sizeof(PlfRectPair) * B) + plf_align256(sizeof(uint8_t*) * 2 * B);
 }
 static BatchTab batch_tab(uint8_t* base, int B) {
   uint8_t* cams = base + plf_align256(3 * sizeof(int32_t) * B);
-  uint8_t* in = cams + plf_align256(sizeof(PlfPairCam) * B);
+  uint8_t* prm = cams + plf_align256(sizeof(PlfPairCam) * B);
+  uint8_t* in = prm + plf_align256(sizeof(PlfPairPrm) * B);
   uint8_t* masks = in + plf_align256(sizeof(PlfRectPair) * B);
-  uint8_t* prm = masks + plf_align256(sizeof(uint8_t*) * 2 * B);
   return {reinterpret_cast<int32_t*>(base), reinterpret_cast<int32_t*>(base) + B, reinterpret_cast<PlfPairCam*>(cams),
-          reinterpret_cast<PlfRectPair*>(in), reinterpret_cast<const uint8_t**>(masks), reinterpret_cast<PlfPairPrm*>(prm)};
+          reinterpret_cast<PlfPairPrm*>(prm), reinterpret_cast<PlfRectPair*>(in), reinterpret_cast<const uint8_t**>(masks)};
 }
 
 // What each sequence carries to its next pair besides its frame slot: the pose prediction (row-major 4x4) and whether it
@@ -144,7 +145,6 @@ struct PipeState {
   int* rev_flags = nullptr; int* rev_list = nullptr; int* rev_count = nullptr;  // [2B][max_kp], [2B][max_kp], [2B]
   KnnProblem* knn_f2f = nullptr;     // [B*4]
   NnrProblem* nnr_stereo = nullptr;  // [B*2]
-  NnrProblem* nnr_own = nullptr;     // [B*2] the stereo problems of a batch with pair settings (k_pair_nnr)
   NnrProblem* nnr_f2f = nullptr;     // [B*2]
   // GN inputs / outputs
   double* gnP = nullptr; double* gnObs = nullptr; uint8_t* gnInlP = nullptr; int* gnNp = nullptr;
@@ -207,7 +207,7 @@ static void pipe_buffers(PipeState* s, bool windowed, DevBufList& b) {
   b.add(s->m12, B * 4 * K);
   b.add(s->mcount, B * 4);
   b.add(s->knn_stereo, B * 4); b.add(s->knn_f2f, B * 4);
-  b.add(s->nnr_stereo, B * 2); b.add(s->nnr_f2f, B * 2); b.add(s->nnr_own, B * 2);
+  b.add(s->nnr_stereo, B * 2); b.add(s->nnr_f2f, B * 2);
   b.add(s->rev_flags, 2 * B * K); b.add(s->rev_list, 2 * B * K); b.add(s->rev_count, 2 * B);
   b.add(s->kpsM, 2 * B * K); b.add(s->descM, 2 * B * K * 32); b.add(s->kcntM, 2 * B);
   b.add(s->klsM, 2 * B * Ln); b.add(s->lcntM, 2 * B);
@@ -260,28 +260,7 @@ extern "C" void plf_pipe_free(plf_ctx* ctx) {
   ctx->pipe = nullptr;
 }
 
-struct StereoPrm {
-  float max_dist_epip, min_disp, line_horiz_th, stereo_overlap_th, ls_min_disp_ratio;
-  double fx, fy, cx, cy, b;   // the context's camera
-};
-
-// The parameters of pair k: prm with the pair's camera from the batch's camera table and its gates from the batch's
-// settings table, or prm itself without them.
-__device__ __forceinline__ StereoPrm pair_prm(StereoPrm c, const PlfPairCam* __restrict__ cams, int k,
-                                              const PlfPairPrm* __restrict__ own = nullptr) {
-  if (cams) {
-    const PlfPairCam q = cams[k];
-    c.fx = q.fx; c.fy = q.fy; c.cx = q.cx; c.cy = q.cy; c.b = q.b;
-  }
-  if (own) {
-    const PlfPairPrm& q = own[k];
-    c.max_dist_epip = q.max_dist_epip; c.min_disp = q.min_disp; c.line_horiz_th = q.line_horiz_th;
-    c.stereo_overlap_th = q.stereo_overlap_th; c.ls_min_disp_ratio = q.ls_min_disp_ratio;
-  }
-  return c;
-}
-
-__device__ __forceinline__ void back_projection(const StereoPrm& c, double u, double v, double disp, double* P) {
+__device__ __forceinline__ void back_projection(const PlfPairCam& c, double u, double v, double disp, double* P) {
   const double Z = c.fx * c.b / disp;  // PinholeStereoCamera::backProjection (SURVEY A.4)
   P[0] = Z * (u - c.cx) / c.fx;
   P[1] = Z * (v - c.cy) / c.fy;
@@ -305,19 +284,19 @@ __device__ __forceinline__ int block_scan_flags(bool flag, int* s_scan, int* s_t
   return incl;
 }
 
-// matchStereoPoints: epipolar + disparity gates, back-projection, compaction in left-index order.  OWN: the gates of pair k
-// from own[k] (a batch with pair settings); the other instantiation ignores own.
-template <bool OWN>
+// matchStereoPoints: epipolar + disparity gates, back-projection, compaction in left-index order, with pair k's camera
+// cams[k] and gates prm[k].
 __global__ void __launch_bounds__(1024) k_stereo_points(const plf_keypoint* __restrict__ kps, const uint8_t* __restrict__ desc,
                                                          const int* __restrict__ kp_count, int max_kp,
-                                                         const int32_t* __restrict__ m12_all, int m12_stride, StereoPrm prm0,
-                                                         const PlfPairCam* __restrict__ cams, FrameSlots fs,
-                                                         const PlfPairPrm* __restrict__ own) {
+                                                         const int32_t* __restrict__ m12_all, int m12_stride,
+                                                         const PlfPairCam* __restrict__ cams, const PlfPairPrm* __restrict__ prm,
+                                                         FrameSlots fs) {
   __shared__ int s_scan[1024];
   __shared__ int s_total;
   const int k = blockIdx.x, tid = threadIdx.x;
   const int il = 2 * k, ir = 2 * k + 1, slot = k;
-  const StereoPrm prm = pair_prm(prm0, cams, k, OWN ? own : nullptr);
+  const PlfPairCam cam = cams[k];
+  const PlfPairPrm& q = prm[k];
   const plf_keypoint* kl = kps + (size_t)il * max_kp;
   const plf_keypoint* kr = kps + (size_t)ir * max_kp;
   const int32_t* m12 = m12_all + (size_t)k * m12_stride;
@@ -334,9 +313,9 @@ __global__ void __launch_bounds__(1024) k_stereo_points(const plf_keypoint* __re
       if (j >= 0) {
         const plf_keypoint a = kl[i], b = kr[j];
         xl = a.x; yl = a.y; oct = a.octave;
-        if (fabsf(__fsub_rn(a.y, b.y)) <= prm.max_dist_epip) {
+        if (fabsf(__fsub_rn(a.y, b.y)) <= q.max_dist_epip) {
           d = (double)__fsub_rn(a.x, b.x);
-          ok = d >= (double)prm.min_disp;
+          ok = d >= (double)q.min_disp;
         }
       }
     }
@@ -345,7 +324,7 @@ __global__ void __launch_bounds__(1024) k_stereo_points(const plf_keypoint* __re
       const size_t o = (size_t)slot * max_kp + base + incl - 1;
       fs.pt_pl[o] = make_double2((double)xl, (double)yl);
       fs.pt_disp[o] = d;
-      back_projection(prm, (double)xl, (double)yl, d, fs.pt_P + 3 * o);
+      back_projection(cam, (double)xl, (double)yl, d, fs.pt_P + 3 * o);
       fs.pt_octave[o] = oct;
       const uint4* src = reinterpret_cast<const uint4*>(desc + ((size_t)il * max_kp + i) * 32);
       uint4* dst = reinterpret_cast<uint4*>(fs.pdesc + o * 32);
@@ -374,18 +353,18 @@ __device__ __forceinline__ double line_overlap_stereo(double spl_obs, double epl
   return overlap;
 }
 
-// matchStereoLines (OWN: as k_stereo_points)
-template <bool OWN>
+// matchStereoLines (camera and gates: as k_stereo_points)
 __global__ void __launch_bounds__(1024) k_stereo_lines(const plf_keyline* __restrict__ kls, const uint8_t* __restrict__ ldesc,
                                                         const int* __restrict__ nlines, int max_ln,
-                                                        const int32_t* __restrict__ m12_all, int m12_stride, StereoPrm prm0,
-                                                        const PlfPairCam* __restrict__ cams, FrameSlots fs,
-                                                        const PlfPairPrm* __restrict__ own) {
+                                                        const int32_t* __restrict__ m12_all, int m12_stride,
+                                                        const PlfPairCam* __restrict__ cams, const PlfPairPrm* __restrict__ prm,
+                                                        FrameSlots fs) {
   __shared__ int s_scan[1024];
   __shared__ int s_total;
   const int k = blockIdx.x, tid = threadIdx.x;
   const int il = 2 * k, ir = 2 * k + 1, slot = k;
-  const StereoPrm prm = pair_prm(prm0, cams, k, OWN ? own : nullptr);
+  const PlfPairCam cam = cams[k];
+  const PlfPairPrm& q = prm[k];
   const plf_keyline* L = kls + (size_t)il * max_ln;
   const plf_keyline* R = kls + (size_t)ir * max_ln;
   const int32_t* m12 = m12_all + (size_t)k * m12_stride;
@@ -407,14 +386,14 @@ __global__ void __launch_bounds__(1024) k_stereo_lines(const plf_keyline* __rest
         const double nrm = sqrt(l0 * l0 + l1 * l1);
         le_l[0] = l0 / nrm; le_l[1] = l1 / nrm; le_l[2] = l2 / nrm;
         const double r0 = syr * 1.0 - 1.0 * eyr, r1 = 1.0 * exr - sxr * 1.0, r2 = sxr * eyr - syr * exr;
-        const double overlap = line_overlap_stereo(syl, eyl, syr, eyr, (double)prm.line_horiz_th);
+        const double overlap = line_overlap_stereo(syl, eyl, syr, eyr, (double)q.line_horiz_th);
         const double sx_on_r = -(r2 + r1 * syl) / r0;
         const double ex_on_r = -(r2 + r1 * eyl) / r0;
         disp_s = sxl - sx_on_r;
         disp_e = exl - ex_on_r;
-        if (!(fmin(disp_s, disp_e) / fmax(disp_s, disp_e) >= (double)prm.ls_min_disp_ratio)) disp_s = disp_e = -1.0;
-        ok = disp_s >= (double)prm.min_disp && disp_e >= (double)prm.min_disp &&
-             fabsf((float)r0) > prm.line_horiz_th && overlap > (double)prm.stereo_overlap_th;
+        if (!(fmin(disp_s, disp_e) / fmax(disp_s, disp_e) >= (double)q.ls_min_disp_ratio)) disp_s = disp_e = -1.0;
+        ok = disp_s >= (double)q.min_disp && disp_e >= (double)q.min_disp &&
+             fabsf((float)r0) > q.line_horiz_th && overlap > (double)q.stereo_overlap_th;
         spl[0] = sxl; spl[1] = syl; epl[0] = exl; epl[1] = eyl;
         angle = a.angle;
       }
@@ -426,8 +405,8 @@ __global__ void __launch_bounds__(1024) k_stereo_lines(const plf_keyline* __rest
       fs.ls_epl[o] = make_double2(epl[0], epl[1]);
       fs.ls_sdisp[o] = disp_s;
       fs.ls_edisp[o] = disp_e;
-      back_projection(prm, spl[0], spl[1], disp_s, fs.ls_sP + 3 * o);
-      back_projection(prm, epl[0], epl[1], disp_e, fs.ls_eP + 3 * o);
+      back_projection(cam, spl[0], spl[1], disp_s, fs.ls_sP + 3 * o);
+      back_projection(cam, epl[0], epl[1], disp_e, fs.ls_eP + 3 * o);
       fs.ls_le[3 * o] = le_l[0]; fs.ls_le[3 * o + 1] = le_l[1]; fs.ls_le[3 * o + 2] = le_l[2];
       fs.ls_angle[o] = angle;
       const uint4* src = reinterpret_cast<const uint4*>(ldesc + ((size_t)il * max_ln + i) * 32);
@@ -441,14 +420,19 @@ __global__ void __launch_bounds__(1024) k_stereo_lines(const plf_keyline* __rest
   if (tid == 0) fs.ls_count[slot] = base;
 }
 
-// f2fTracking problems of pair k: the previous frame (slot prev[k]) against the current one (slot k), 2-NN both ways
-// for points and lines, then the mutual NNR check; the forward best / second keys of problem kind c (4 = points,
-// 6 = lines) and the reverse ones (c + 1) live in the pair's knn_keys rows.
+// The matching problems of pair k that depend on the batch, with its ratios and best_lr from prm[k].  f2fTracking: the
+// previous frame (slot prev[k]) against the current one (slot k), 2-NN both ways for points and lines, then the mutual NNR
+// check; the forward best / second keys of problem kind c (4 = points, 6 = lines) and the reverse ones (c + 1) live in the
+// pair's knn_keys rows.  Stereo: the NNR check of the static kNN problems (pipe_build) over the left (kinds 0, 2) and right
+// (1, 3) images' counts kcnt, lcnt.  A windowed pair (matching_strategy != 0) gets its stereo matches from the windowed
+// matcher: its stereo problems read their query count at zero, an int that stays 0, so they write no row.
 __global__ void k_f2f_problems(FrameSlots fs, const int* __restrict__ prev, int B, int K, int Ln, uint32_t* __restrict__ knn_keys,
-                               int32_t* __restrict__ m12, int* __restrict__ mcount, float nnr_p, float nnr_l, int best_lr,
-                               KnnProblem* __restrict__ kf, NnrProblem* __restrict__ nf) {
+                               int32_t* __restrict__ m12, int* __restrict__ mcount, const int* kcnt, const int* lcnt,
+                               const int* zero, const PlfPairPrm* __restrict__ prm, KnnProblem* __restrict__ kf,
+                               NnrProblem* __restrict__ nf, NnrProblem* __restrict__ ns) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= B) return;
+  const PlfPairPrm& q = prm[k];
   const int ps = prev[k], cs = k;
   auto key = [&](int prob, int which) { return knn_keys + (((size_t)k * 8 + prob) * 2 + which) * K; };
   const uint32_t* pp = (const uint32_t*)(fs.pdesc + (size_t)ps * K * 32);
@@ -460,31 +444,14 @@ __global__ void k_f2f_problems(FrameSlots fs, const int* __restrict__ prev, int 
   kf[4 * k + 1] = KnnProblem{pc, pp, nc, np, 0, 0, key(5, 0), key(5, 1), nullptr};
   kf[4 * k + 2] = KnnProblem{lp, lc, lnp, lnc, 0, 0, key(6, 0), key(6, 1), nullptr};
   kf[4 * k + 3] = KnnProblem{lc, lp, lnc, lnp, 0, 0, key(7, 0), key(7, 1), nullptr};
-  nf[2 * k + 0] = NnrProblem{key(4, 0), key(4, 1), key(5, 0), key(5, 1), np, nc, 0, 0, nnr_p, best_lr, m12 + ((size_t)k * 4 + 2) * K,
-                             mcount + 4 * k + 2};
-  nf[2 * k + 1] = NnrProblem{key(6, 0), key(6, 1), key(7, 0), key(7, 1), lnp, lnc, 0, 0, nnr_l, best_lr, m12 + ((size_t)k * 4 + 3) * K,
-                             mcount + 4 * k + 3};
-}
-
-// The matching settings of a batch with pair settings (prm): its stereo problems ns_own, copies of the context's ns with
-// each pair's ratios and best_lr, and the same in place in its frame-to-frame problems nf (k_f2f_problems).  A pair of a
-// windowed sequence (matching_strategy != 0) gets its stereo matches from the windowed matcher: its problems here read
-// their query count at zero, an int that stays 0, so they write no row.
-__global__ void k_pair_nnr(const PlfPairPrm* __restrict__ prm, int B, const NnrProblem* __restrict__ ns, const int* zero,
-                           NnrProblem* __restrict__ ns_own, NnrProblem* __restrict__ nf) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= B) return;
-  const PlfPairPrm& q = prm[k];
-  for (int c = 0; c < 2; ++c) {
-    const float nnr = c ? q.min_ratio_12_l : q.min_ratio_12_p;
-    NnrProblem p = ns[2 * k + c];
-    p.nnr = nnr;
-    p.best_lr = q.best_lr;
-    if (q.matching_strategy) p.n1_ptr = zero;
-    ns_own[2 * k + c] = p;
-    nf[2 * k + c].nnr = nnr;
-    nf[2 * k + c].best_lr = q.best_lr;
-  }
+  nf[2 * k + 0] = NnrProblem{key(4, 0), key(4, 1), key(5, 0), key(5, 1), np, nc, 0, 0, q.min_ratio_12_p, q.best_lr,
+                             m12 + ((size_t)k * 4 + 2) * K, mcount + 4 * k + 2};
+  nf[2 * k + 1] = NnrProblem{key(6, 0), key(6, 1), key(7, 0), key(7, 1), lnp, lnc, 0, 0, q.min_ratio_12_l, q.best_lr,
+                             m12 + ((size_t)k * 4 + 3) * K, mcount + 4 * k + 3};
+  ns[2 * k + 0] = NnrProblem{key(0, 0), key(0, 1), key(1, 0), key(1, 1), q.matching_strategy ? zero : kcnt + 2 * k, kcnt + 2 * k + 1,
+                             0, 0, q.min_ratio_12_p, q.best_lr, m12 + (size_t)k * 4 * K, mcount + 4 * k};
+  ns[2 * k + 1] = NnrProblem{key(2, 0), key(2, 1), key(3, 0), key(3, 1), q.matching_strategy ? zero : lcnt + 2 * k, lcnt + 2 * k + 1,
+                             0, 0, q.min_ratio_12_l, q.best_lr, m12 + ((size_t)k * 4 + 1) * K, mcount + 4 * k + 1};
 }
 
 // Copies `rows` rows of row_bytes (a multiple of 4) from slot `from` to slot `to` of an array of `cap` rows per slot.
@@ -575,11 +542,11 @@ __global__ void __launch_bounds__(1024) k_f2f_build(FrameSlots fs, const int* __
 // previous frame is the empty slot is a first frame (initialize())
 __global__ void k_finalize(const plf_pose_result* __restrict__ gn, const int* __restrict__ gnNp, const int* __restrict__ gnNl,
                            const int* __restrict__ kp_count, const int* __restrict__ nlines, FrameSlots fs,
-                           const int* __restrict__ prev, int empty_slot, int min_features, int B,
-                           plf_frame_result* __restrict__ out, const PlfPairPrm* __restrict__ prm) {
+                           const int* __restrict__ prev, int empty_slot, int B, plf_frame_result* __restrict__ out,
+                           const PlfPairPrm* __restrict__ prm) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= B) return;
-  if (prm) min_features = prm[k].min_features;
+  const int min_features = prm[k].min_features;
   plf_frame_result r;
   for (int i = 0; i < 16; ++i) r.DT[i] = (i % 5 == 0) ? 1.0 : 0.0;
   for (int i = 0; i < 36; ++i) r.DT_cov[i] = 0.0;
@@ -611,14 +578,13 @@ __global__ void k_finalize(const plf_pose_result* __restrict__ gn, const int* __
 // (plf_set_motion_model), DESIGN.md §8.  With either on a batch holds at most one pair of each sequence, so prev[k] is the
 // empty slot (a first frame) or pair k's carry slot carry0 + s, and every pair is in the carry list. ----
 
-// The FAST threshold of both images of pair k: its sequence's (rec, with adaptive FAST), or for a first frame and without
-// rec the first frame's, the pair's own settings' (prm) or th0 = orb_fast_th.
-__global__ void k_fast_th_images(const int* __restrict__ prev, int B, int carry0, int empty, int th0,
-                                 const SeqRecord* __restrict__ rec, const PlfPairPrm* __restrict__ prm, int* __restrict__ img_th) {
+// The FAST threshold of both images of pair k: its sequence's, or its settings' first-frame one for a first frame.
+__global__ void k_fast_th_images(const int* __restrict__ prev, int B, int carry0, int empty, const SeqRecord* __restrict__ rec,
+                                 const PlfPairPrm* __restrict__ prm, int* __restrict__ img_th) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= B) return;
   const int p = prev[k];
-  const int th = rec && p != empty ? rec[p - carry0].th : prm ? prm[k].fast_th : th0;
+  const int th = p != empty ? rec[p - carry0].th : prm[k].fast_th;
   img_th[2 * k] = th;
   img_th[2 * k + 1] = th;
 }
@@ -636,15 +602,12 @@ __device__ __forceinline__ int fast_th_next(int th, const plf_frame_result& r, c
   return th;
 }
 
-// orb_fast_th as k_fast_nms applies it without a per-image threshold
-static int fast_th0(const plf_params& P) { return std::min(std::max(P.orb_fast_th, 0), 255); }
-static int fast_th0(const plf_ctx* ctx) { return fast_th0(ctx->params); }
-
 PlfPairPrm plf_pair_prm(const plf_params& P) {
   PlfPairPrm q = {};
   q.orb_nlevels = P.orb_nlevels;
-  plf_orb_level_features(P.orb_nfeatures, P.orb_scale_factor, P.orb_nlevels, q.orb_nfeat);
-  q.fast_th = fast_th0(P);
+  if (P.orb_nlevels >= 1 && P.orb_nlevels <= PLF_ORB_MAX_LEVELS)
+    plf_orb_level_features(P.orb_nfeatures, P.orb_scale_factor, P.orb_nlevels, q.orb_nfeat);
+  q.fast_th = std::min(std::max(P.orb_fast_th, 0), 255);
   q.lsd_nfeatures = P.lsd_nfeatures;
   q.min_line_length = P.min_line_length;
   q.max_dist_epip = P.max_dist_epip; q.min_disp = P.min_disp; q.line_horiz_th = P.line_horiz_th;
@@ -722,7 +685,7 @@ static plf_status pipe_seq_reset(plf_ctx* ctx, bool fast_th, bool motion) {
   PipeState* s = ctx->pipe;
   SeqRecord r = {};
   for (int i = 0; i < 16; i += 5) r.T[i] = 1.0;
-  r.th = fast_th0(ctx);
+  r.th = ctx->pair.fast_th;
   const std::vector<SeqRecord> v(s->nseq, r);
   const size_t lo = motion ? 0 : offsetof(SeqRecord, th), hi = fast_th ? sizeof(SeqRecord) : offsetof(SeqRecord, th);
   if (lo >= hi) return PLF_OK;
@@ -773,13 +736,13 @@ __global__ void __launch_bounds__(256) k_mg_geom_stereo(const plf_keypoint* __re
 // k's motion prediction T_pred[k] with the motion model on (src/mapHandler.cpp:254-256, :384-389 project through DT);
 // train = the current frame's image features (slot k).  The projection uses pair k's camera: both frames belong to one
 // sequence, and a new camera restarts its sequence, so the previous frame was triangulated with the same one.
-__global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, const int* __restrict__ prev, int K, int Ln, StereoPrm c0,
+__global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, const int* __restrict__ prev, int K, int Ln,
                                                      const PlfPairCam* __restrict__ cams, const double* __restrict__ T_pred,
                                                      double iw, double ih, int* __restrict__ qp, int* __restrict__ tp,
                                                      int* __restrict__ ql, int* __restrict__ tl, double* __restrict__ tdir) {
   const int k = blockIdx.y, i = blockIdx.x * 256 + threadIdx.x;
   const int ps = prev[k], cs = k;
-  const StereoPrm c = pair_prm(c0, cams, k);
+  const PlfPairCam c = cams[k];
   const double* T = T_pred ? T_pred + 16 * k : nullptr;
   // the query point X of the previous frame, moved into the current frame when there is a prediction
   auto moved = [&](const double* X, double* Y) -> const double* {
@@ -813,16 +776,14 @@ __global__ void __launch_bounds__(256) k_mg_geom_f2f(FrameSlots fs, const int* _
 }
 
 // src/mapHandler.cpp:274-278 / :421-425: keep the windowed result unless both frames hold more than `kmin` features and
-// fewer than `kmin` matches survived - then the brute-force match() result (already in m12) stands.  With pair settings
-// (prm) kmin is the pair's, and a pair of a sequence at matching_strategy 0 keeps its match() result.
+// fewer than `kmin` matches survived - then the brute-force match() result (already in m12) stands.  kmin is the pair's
+// min_pt_matches / min_ls_matches, and a pair at matching_strategy 0 keeps its match() result.
 __global__ void __launch_bounds__(256) k_mg_select(const int32_t* __restrict__ m12g, const int* __restrict__ mgcount,
                                                    const int* __restrict__ cnt, const int* __restrict__ prev, int cap, int K,
-                                                   int which, int kmin, int32_t* __restrict__ m12, const PlfPairPrm* __restrict__ prm) {
+                                                   int which, int32_t* __restrict__ m12, const PlfPairPrm* __restrict__ prm) {
   const int k = blockIdx.y, i = blockIdx.x * 256 + threadIdx.x;
-  if (prm) {
-    if (!prm[k].matching_strategy) return;
-    kmin = which ? prm[k].min_ls_matches : prm[k].min_pt_matches;
-  }
+  if (!prm[k].matching_strategy) return;
+  const int kmin = which ? prm[k].min_ls_matches : prm[k].min_pt_matches;
   const int n1 = min(cnt[prev[k]], cap), n2 = min(cnt[k], cap);
   if (i >= n1) return;
   const bool fall_back = n2 > kmin && n1 > kmin && mgcount[2 * k + which] < kmin;
@@ -892,17 +853,14 @@ static plf_status pipe_build(plf_ctx* ctx) {
   if ((st = plf_lsd_create_sizes(ctx, ngeo, wh.data(), 2 * B, s->lsd2, lsd.data()))) return st;
   for (int i = 0; i < ngeo; ++i) s->geo[i].lsd = lsd[i];
   // static problem descriptors over the pipeline's own buffers (pointers never change; counts are read on the device):
-  // the stereo problems read the match phase's copies of the extraction outputs.  The frame-to-frame problems depend on
-  // the batch's sequence table and are built on the device per batch (k_f2f_problems).
+  // the stereo problems read the match phase's copies of the extraction outputs.  The NNR problems depend on the batch's
+  // sequence table and settings and are built on the device per batch (k_f2f_problems).
   const int* kcnt = s->kcntM;
   const int* lcnt = s->lcntM;
-  const int best_lr = P.best_lr_matches ? 1 : 0;
   std::vector<KnnProblem> ks(B * 4);
-  std::vector<NnrProblem> ns(B * 2);
   std::vector<GnProblem> gp(B);
   for (int k = 0; k < B; ++k) {
     auto key = [&](int prob, int which) { return s->knn_keys + (((size_t)k * 8 + prob) * 2 + which) * K; };
-    auto m12 = [&](int kind) { return s->m12 + ((size_t)k * 4 + kind) * K; };
     const uint32_t* dl = (const uint32_t*)(s->descM + (size_t)(2 * k) * K * 32);
     const uint32_t* dr = (const uint32_t*)(s->descM + (size_t)(2 * k + 1) * K * 32);
     const uint32_t* ll = (const uint32_t*)(s->ldesc_raw + (size_t)(2 * k) * Ln * 32);
@@ -912,14 +870,11 @@ static plf_status pipe_build(plf_ctx* ctx) {
     ks[2 * k + 1] = {ll, lr, lcnt + 2 * k, lcnt + 2 * k + 1, 0, 0, key(2, 0), key(2, 1), nullptr};
     ks[2 * B + 2 * k + 0] = {dr, dl, s->rev_count + 2 * k, kcnt + 2 * k, 0, 0, key(1, 0), key(1, 1), s->rev_list + (size_t)(2 * k) * K};
     ks[2 * B + 2 * k + 1] = {lr, ll, s->rev_count + 2 * k + 1, lcnt + 2 * k, 0, 0, key(3, 0), key(3, 1), s->rev_list + (size_t)(2 * k + 1) * K};
-    ns[2 * k + 0] = {key(0, 0), key(0, 1), key(1, 0), key(1, 1), kcnt + 2 * k, kcnt + 2 * k + 1, 0, 0, P.min_ratio_12_p, best_lr, m12(0), s->mcount + 4 * k + 0};
-    ns[2 * k + 1] = {key(2, 0), key(2, 1), key(3, 0), key(3, 1), lcnt + 2 * k, lcnt + 2 * k + 1, 0, 0, P.min_ratio_12_l, best_lr, m12(1), s->mcount + 4 * k + 1};
     gp[k] ={s->gnP + (size_t)k * K * 3, s->gnObs + (size_t)k * K * 2, s->gnInlP + (size_t)k * K, s->gnNp + k, 0,
              s->gn_sP + (size_t)k * Ln * 3, s->gn_eP + (size_t)k * Ln * 3, s->gn_le + (size_t)k * Ln * 3,
              s->gnInlL + (size_t)k * Ln, s->gnNl + k, 0, nullptr, s->gn_out + k};
   }
   PLF_CUDA(ctx, cudaMemcpyAsync(s->knn_stereo, ks.data(), ks.size() * sizeof(KnnProblem), cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(s->nnr_stereo, ns.data(), ns.size() * sizeof(NnrProblem), cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->gn_probs, gp.data(), gp.size() * sizeof(GnProblem), cudaMemcpyHostToDevice, cs));
   for (int k = 0; k < B; ++k) gp[k].T_init = s->pair_T + 16 * (size_t)k;   // the same problems seeded with the prediction
   PLF_CUDA(ctx, cudaMemcpyAsync(s->gn_probs_mm, gp.data(), gp.size() * sizeof(GnProblem), cudaMemcpyHostToDevice, cs));
@@ -941,12 +896,10 @@ struct BatchRun {
   int B;
   int g;         // the batch's image size: record s->geo[g], the size of the upload it consumes
   int ncarry;    // entries of the carry list in batch table rp: the sequences the batch holds
-  bool cams;     // batch table rp holds the pairs' cameras (a sequence of the batch has its own); else the context's camera
   int nin;       // entries of the input table in batch table rp (0: none, every pair is converted as it is)
   bool masked;   // batch table rp holds the images' masks (a sequence of the batch has one); else no image is masked
-  bool prm;      // batch table rp holds the pairs' settings (a sequence of the batch has its own); else the context's
-  int nwin;      // pairs at matching_strategy != 0 (with prm; else every pair or none, as the context's)
-  bool best_lr;  // some pair matches with best_lr_matches (with prm; else the context's)
+  int nwin;      // pairs at matching_strategy != 0
+  bool best_lr;  // some pair matches with best_lr_matches
   bool afast;    // adaptive FAST thresholds (plf_set_adaptive_fast): pair thresholds in the E phase, the next ones behind k_finalize
   bool motion;   // motion model (plf_set_motion_model): pair predictions at the start of M, the next ones behind k_finalize
   int par;       // parity of the E -> G -> M hand-off buffers
@@ -961,17 +914,16 @@ struct BatchRun {
 static BatchTab host_tab(const PipeState* s, int rp) { return batch_tab(s->h_tab[rp], s->B); }
 static BatchTab dev_tab(const PipeState* s, int rp) { return batch_tab(s->tab + rp * batch_tab_bytes(s->B), s->B); }
 
-// The parts of the batch's table that it uses, to ring entry rp of the device on the copy stream: the sequence table
-// always, the cameras, the input table, the masks and the settings when it has them.  ev_tab[rp] marks them.
+// The parts of the batch's table that it uses, to ring entry rp of the device on the copy stream: the sequence table, the
+// cameras and the settings always (one copy, up to the batch's last settings), the input table and the masks when it has
+// them.  ev_tab[rp] marks them.
 static plf_status send_tab(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   const BatchTab h = host_tab(s, r.rp), d = dev_tab(s, r.rp);
   cudaStream_t cs = s->copy;
-  PLF_CUDA(ctx, cudaMemcpyAsync(d.prev, h.prev, sizeof(int32_t) * r.B, cudaMemcpyHostToDevice, cs));
-  PLF_CUDA(ctx, cudaMemcpyAsync(d.carry, h.carry, sizeof(int32_t) * 2 * r.ncarry, cudaMemcpyHostToDevice, cs));
-  if (r.cams) PLF_CUDA(ctx, cudaMemcpyAsync(d.cams, h.cams, sizeof(PlfPairCam) * r.B, cudaMemcpyHostToDevice, cs));
+  const size_t head = reinterpret_cast<const uint8_t*>(h.prm + r.B) - reinterpret_cast<const uint8_t*>(h.prev);
+  PLF_CUDA(ctx, cudaMemcpyAsync(d.prev, h.prev, head, cudaMemcpyHostToDevice, cs));
   if (r.nin) PLF_CUDA(ctx, cudaMemcpyAsync(d.in, h.in, sizeof(PlfRectPair) * r.nin, cudaMemcpyHostToDevice, cs));
   if (r.masked) PLF_CUDA(ctx, cudaMemcpyAsync(d.masks, h.masks, sizeof(uint8_t*) * 2 * r.B, cudaMemcpyHostToDevice, cs));
-  if (r.prm) PLF_CUDA(ctx, cudaMemcpyAsync(d.prm, h.prm, sizeof(PlfPairPrm) * r.B, cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaEventRecord(s->ev_tab[r.rp], cs));
   return PLF_OK;
 }
@@ -1110,20 +1062,19 @@ static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->evX[par], 0));           // batch i-2 (same parity) no longer reads these buffers
   plf_mark(ctx, sE, "start");
   PLF_CUDA(ctx, cudaEventRecord(s->tE0[par], sE));
-  const int* img_th = nullptr;
-  const uint8_t* const* masks = r.masked ? dev_tab(s, r.rp).masks : nullptr;
-  const PlfPairPrm* prm = r.prm ? dev_tab(s, r.rp).prm : nullptr;
-  if (r.afast || r.masked || r.prm) PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_tab[r.rp], 0));   // the sequence, mask or settings table
-  if (r.afast || r.prm) {
+  const BatchTab tab = dev_tab(s, r.rp);
+  const int* img_th = nullptr;   // without adaptive FAST each image detects at its pair's settings' threshold
+  const uint8_t* const* masks = r.masked ? tab.masks : nullptr;
+  PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_tab[r.rp], 0));   // the settings, sequence and mask tables
+  if (r.afast) {
     // the thresholds of the batch's images: the sequence table, and the previous batch's threshold update (which has
-    // also read img_th for the last time); without adaptive FAST each pair's first-frame threshold
-    if (r.afast) PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_th, 0));
-    k_fast_th_images<<<(B + 127) / 128, 128, 0, sE>>>(dev_tab(s, r.rp).prev, B, s->B, s->B + s->nseq, fast_th0(ctx),
-                                                      r.afast ? s->seq_rec : nullptr, prm, s->img_th);
+    // also read img_th for the last time)
+    PLF_CUDA(ctx, cudaStreamWaitEvent(sE, s->ev_th, 0));
+    k_fast_th_images<<<(B + 127) / 128, 128, 0, sE>>>(tab.prev, B, s->B, s->B + s->nseq, s->seq_rec, tab.prm, s->img_th);
     PLF_LAUNCH_CHECK(ctx);
     img_th = s->img_th;
   }
-  plf_status st = plf_orb_run(ctx, sE, G.orb, imgs, AP, G.pitch, 2 * B, par, img_th, masks, prm);
+  plf_status st = plf_orb_run(ctx, sE, G.orb, imgs, AP, G.pitch, 2 * B, par, img_th, masks, tab.prm);
   if (!st) st = plf_launch_blur5_sobel(ctx, sE, &G.lbd_tm, imgs, G.pitch, AP, w, h, 2 * B, s->lbd_grad[par], A);
   if (st) return st;
   plf_mark(ctx, sE, "lbd.k_blur5_sobel");
@@ -1147,7 +1098,7 @@ static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   const size_t AP = (size_t)G.pitch * G.h;
   cudaStream_t sP = r.sP, sG = r.sG;
   PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_up[r.run_slot], 0));
-  if (r.masked || r.prm) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_tab[r.rp], 0));   // the mask and settings tables, read by G's KeyLine stage
+  PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->ev_tab[r.rp], 0));   // the settings and mask tables, read by G's KeyLine stage
   if (r.lsd2) PLF_CUDA(ctx, cudaStreamWaitEvent(sP, s->evG[par], 0));   // batch i-2 (same parity) has finished growing / fitting on these maps
   PLF_CUDA(ctx, cudaEventRecord(s->tG0[par], sP));
   plf_status st = plf_lsd_pre(ctx, sP, G.lsd, s->imgs2[r.run_slot], AP, G.pitch, r.lp, 2 * r.B);
@@ -1157,8 +1108,9 @@ static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaStreamWaitEvent(sG, s->evP[par], 0));
   // the KeyLine outputs are overwritten: the match phase that read them last (batch i-2 with two parities, batch i-1 with one)
   // has taken its copy
-  st = plf_lsd_grow(ctx, sG, G.lsd, r.lp, 2 * r.B, r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr,
-                    r.masked ? dev_tab(s, r.rp).masks : nullptr, r.prm ? dev_tab(s, r.rp).prm : nullptr);
+  const BatchTab tab = dev_tab(s, r.rp);
+  st = plf_lsd_grow(ctx, sG, G.lsd, r.lp, 2 * r.B, r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr, r.masked ? tab.masks : nullptr,
+                    tab.prm);
   if (st) return st;
   PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp + 1, plf_lsd_overflow_flag(G.lsd), sizeof(int), cudaMemcpyDeviceToDevice, sG));
   PLF_CUDA(ctx, cudaMemsetAsync(plf_lsd_overflow_flag(G.lsd), 0, sizeof(int), sG));
@@ -1168,15 +1120,14 @@ static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
 
 // One windowed-matching launch over B problems of one kind (points: cap = K, lines: cap = Ln).  Problem p matches the
 // descriptor rows of image / slot q_slot[p] * step of `desc` (p * step without q_slot; cnt[...] of them) against those of
-// image / slot p * step + t_off.  prm: the pairs' settings, f2f: the frame-to-frame window (MgbArgs).
-static MgbArgs mgb_args(const plf_params& P, MgGrid g, bool lines, int cap, int step, const int* q_slot, int t_off,
-                        const int* q_geo, const int* t_geo, const double* t_dir, const uint8_t* desc, const int* cnt,
-                        int32_t* m12, size_t m12_stride, int* count, int count_stride, const PlfPairPrm* prm, int f2f) {
+// image / slot p * step + t_off.  Problem p takes its window, ratio, best_lr and direction gate from the pair's settings
+// prm[p] (f2f: the frame-to-frame window, else the stereo one).
+static MgbArgs mgb_args(bool lines, int cap, int step, const int* q_slot, int t_off, const int* q_geo, const int* t_geo,
+                        const double* t_dir, const uint8_t* desc, const int* cnt, int32_t* m12, size_t m12_stride, int* count,
+                        int count_stride, const PlfPairPrm* prm, int f2f) {
   MgbArgs a = {};
-  a.g = g;
-  a.is_lines = lines ? 1 : 0; a.K = a.Kt = cap; a.best_lr = P.best_lr_matches ? 1 : 0;
-  a.nnr = lines ? P.min_ratio_12_l : P.min_ratio_12_p;
-  a.line_sim_th = (double)P.line_sim_th;
+  a.g.cols = PLF_GRID_COLS; a.g.rows = PLF_GRID_ROWS;
+  a.is_lines = lines ? 1 : 0; a.K = a.Kt = cap;
   a.q_geo = q_geo; a.t_geo = t_geo; a.t_dir = t_dir;
   a.q_slot = q_slot;
   a.d1 = desc; a.d2 = desc + (size_t)t_off * cap * 32; a.d1_stride = a.d2_stride = (size_t)step * cap * 32;
@@ -1202,22 +1153,16 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->evG[par], 0));
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->evE[par], 0));
   PLF_CUDA(ctx, cudaEventRecord(s->tM0[rp], cs));
-  // the batch's sequence table, and the pairs' cameras when the batch has them (null: every kernel takes the context's)
+  // the batch's sequence table, and the pairs' cameras and settings
   const BatchTab tab = dev_tab(s, rp);
   const int32_t* prev = tab.prev;
   const int32_t* carry = tab.carry;
-  const PlfPairCam* pcam = r.cams ? tab.cams : nullptr;
-  const PlfPairPrm* prm = r.prm ? tab.prm : nullptr;   // the pairs' settings (null: every kernel takes plf_params')
+  const PlfPairCam* pcam = tab.cams;
+  const PlfPairPrm* prm = tab.prm;
   PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_tab[rp], 0));
-  k_f2f_problems<<<(B + 127) / 128, 128, 0, cs>>>(s->fs, prev, B, K, Ln, s->knn_keys, s->m12, s->mcount, P.min_ratio_12_p,
-                                                  P.min_ratio_12_l, P.best_lr_matches ? 1 : 0, s->knn_f2f, s->nnr_f2f);
+  k_f2f_problems<<<(B + 127) / 128, 128, 0, cs>>>(s->fs, prev, B, K, Ln, s->knn_keys, s->m12, s->mcount, s->kcntM, s->lcntM,
+                                                  s->fs.pt_count + s->B + s->nseq, prm, s->knn_f2f, s->nnr_f2f, s->nnr_stereo);
   PLF_LAUNCH_CHECK(ctx);
-  const NnrProblem* nnr_stereo = s->nnr_stereo;
-  if (prm) {
-    k_pair_nnr<<<(B + 127) / 128, 128, 0, cs>>>(prm, B, s->nnr_stereo, s->fs.pt_count + s->B + s->nseq, s->nnr_own, s->nnr_f2f);
-    PLF_LAUNCH_CHECK(ctx);
-    nnr_stereo = s->nnr_own;
-  }
   // the pairs' motion predictions, when the model is on (null: the f2f geometry and the pose solver start from identity).
   // The previous batch wrote its sequences' ones behind its k_finalize on this stream.
   const double* T_pred = nullptr;
@@ -1244,17 +1189,16 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaMemsetAsync(s->mcount, 0, (size_t)B * 4 * sizeof(int), cs));
   const double mg_iw = PLF_GRID_COLS / (double)w, mg_ih = PLF_GRID_ROWS / (double)h;   // StereoFrame::inv_width / inv_height
   // The windowed matcher runs over every pair when one of them is windowed; then match() over every pair when one is not
-  // (its problems of windowed pairs write nothing, k_pair_nnr), so each pair keeps the association of its own strategy.
+  // (its problems of windowed pairs write nothing, k_f2f_problems), so each pair keeps the association of its own strategy.
   const bool windowed = r.nwin > 0, brute = r.nwin < B;
   if (windowed) {
     // stereo association through matchGrid(): window (matching_s_ws, 0) x (0, 0) over the right image's grid
     k_mg_geom_stereo<<<dim3((std::max(K, Ln) + 255) / 256, 2 * B), 256, 0, cs>>>(kps, kcnt, K, kls, lcnt, Ln, mg_iw, mg_ih, s->mg_q[0],
                                                                                  s->mg_t[0], s->mg_q[1], s->mg_t[1], s->mg_dir[0]);
     PLF_LAUNCH_CHECK(ctx);
-    const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, P.matching_s_ws, 0, 0, 0};
-    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 2, nullptr, 1, s->mg_q[0], s->mg_t[0], nullptr, odesc, kcnt,
+    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(false, K, 2, nullptr, 1, s->mg_q[0], s->mg_t[0], nullptr, odesc, kcnt,
                                                         s->m12, 4 * (size_t)K, s->mcount, 4, prm, 0), B, K, K, PLF_SCR_MGB_PIPE, cs))) return st;
-    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 2, nullptr, 1, s->mg_q[1], s->mg_t[1], s->mg_dir[0], s->ldesc_raw,
+    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(true, Ln, 2, nullptr, 1, s->mg_q[1], s->mg_t[1], s->mg_dir[0], s->ldesc_raw,
                                                         lcnt, s->m12 + K, 4 * (size_t)K, s->mcount + 1, 4, prm, 0), B, Ln, Ln, PLF_SCR_MGB_PIPE, cs))) return st;
     plf_mark(ctx, cs, "stereo.k_mgb (matchGrid)");
   }
@@ -1265,22 +1209,18 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     if (r.best_lr) {
       PLF_CUDA(ctx, cudaMemsetAsync(s->rev_flags, 0, 2 * (size_t)B * K * sizeof(int), cs));
       PLF_CUDA(ctx, cudaMemsetAsync(s->rev_count, 0, 2 * (size_t)B * sizeof(int), cs));
-      if ((st = plf_launch_nnr_mark(ctx, cs, nnr_stereo, 2 * B, std::max(K, Ln), s->rev_flags, s->rev_list, s->rev_count, K))) return st;
+      if ((st = plf_launch_nnr_mark(ctx, cs, s->nnr_stereo, 2 * B, std::max(K, Ln), s->rev_flags, s->rev_list, s->rev_count, K))) return st;
       // the reverse problems are laid out after the forward problems of ALL max_batch pairs (pipe_prepare), not of this
       // call's B pairs: a partial batch (B < max_batch) must still start at 2 * max_batch
       if ((st = plf_launch_knn2(ctx, cs, s->knn_stereo + 2 * s->B, 2 * B, std::max(K, Ln)))) return st;
     }
     plf_mark(ctx, cs, "stereo.k_hamming_knn2");
-    if ((st = plf_launch_nnr(ctx, cs, nnr_stereo, 2 * B, std::max(K, Ln)))) return st;
+    if ((st = plf_launch_nnr(ctx, cs, s->nnr_stereo, 2 * B, std::max(K, Ln)))) return st;
     plf_mark(ctx, cs, "stereo.k_nnr_mutual");
   }
-  StereoPrm sp = {P.max_dist_epip, P.min_disp, P.line_horiz_th, P.stereo_overlap_th, P.ls_min_disp_ratio,
-                  ctx->cam.fx, ctx->cam.fy, ctx->cam.cx, ctx->cam.cy, ctx->cam.b};
-  if (prm) k_stereo_points<true><<<B, 1024, 0, cs>>>(kps, odesc, kcnt, K, s->m12, 4 * K, sp, pcam, s->fs, prm);
-  else k_stereo_points<false><<<B, 1024, 0, cs>>>(kps, odesc, kcnt, K, s->m12, 4 * K, sp, pcam, s->fs, nullptr);
+  k_stereo_points<<<B, 1024, 0, cs>>>(kps, odesc, kcnt, K, s->m12, 4 * K, pcam, prm, s->fs);
   PLF_LAUNCH_CHECK(ctx);
-  if (prm) k_stereo_lines<true><<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, sp, pcam, s->fs, prm);
-  else k_stereo_lines<false><<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, sp, pcam, s->fs, nullptr);
+  k_stereo_lines<<<B, 1024, 0, cs>>>(kls, s->ldesc_raw, lcnt, Ln, s->m12 + K, 4 * K, pcam, prm, s->fs);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "stereo.k_stereo_points+lines");
   if ((st = plf_launch_knn2(ctx, cs, s->knn_f2f, 4 * B, std::max(K, Ln)))) return st;
@@ -1290,19 +1230,17 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
     // frame-to-frame: matchGrid() in a +-matching_f2f_ws window around the projected feature; the match() result above
     // stands where the window search found fewer than min_pt_matches / min_ls_matches
     PLF_CUDA(ctx, cudaMemsetAsync(s->mgcount, 0, (size_t)B * 2 * sizeof(int), cs));
-    k_mg_geom_f2f<<<dim3((std::max(K, Ln) + 255) / 256, B), 256, 0, cs>>>(s->fs, prev, K, Ln, sp, pcam, T_pred, mg_iw, mg_ih,
+    k_mg_geom_f2f<<<dim3((std::max(K, Ln) + 255) / 256, B), 256, 0, cs>>>(s->fs, prev, K, Ln, pcam, T_pred, mg_iw, mg_ih,
                                                                           s->mg_q[2], s->mg_t[2], s->mg_q[3], s->mg_t[3],
                                                                           s->mg_dir[1]);
     PLF_LAUNCH_CHECK(ctx);
-    const int ws = P.matching_f2f_ws;
-    const MgGrid g = {PLF_GRID_COLS, PLF_GRID_ROWS, ws, ws, ws, ws};
-    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, false, K, 1, prev, 0, s->mg_q[2], s->mg_t[2], nullptr, s->fs.pdesc,
+    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(false, K, 1, prev, 0, s->mg_q[2], s->mg_t[2], nullptr, s->fs.pdesc,
                                                         s->fs.pt_count, s->m12g, 2 * (size_t)K, s->mgcount, 2, prm, 1), B, K, K, PLF_SCR_MGB_PIPE, cs))) return st;
-    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(P, g, true, Ln, 1, prev, 0, s->mg_q[3], s->mg_t[3], s->mg_dir[1], s->fs.ldesc,
+    if ((st = plf_launch_match_grid_batch(ctx, mgb_args(true, Ln, 1, prev, 0, s->mg_q[3], s->mg_t[3], s->mg_dir[1], s->fs.ldesc,
                                                         s->fs.ls_count, s->m12g + K, 2 * (size_t)K, s->mgcount + 1, 2, prm, 1), B, Ln, Ln, PLF_SCR_MGB_PIPE, cs))) return st;
-    k_mg_select<<<dim3((K + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.pt_count, prev, K, K, 0, P.min_pt_matches, s->m12, prm);
+    k_mg_select<<<dim3((K + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.pt_count, prev, K, K, 0, s->m12, prm);
     PLF_LAUNCH_CHECK(ctx);
-    k_mg_select<<<dim3((Ln + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.ls_count, prev, Ln, K, 1, P.min_ls_matches, s->m12, prm);
+    k_mg_select<<<dim3((Ln + 255) / 256, B), 256, 0, cs>>>(s->m12g, s->mgcount, s->fs.ls_count, prev, Ln, K, 1, s->m12, prm);
     PLF_LAUNCH_CHECK(ctx);
     plf_mark(ctx, cs, "f2f.k_mgb (matchGrid)");
   }
@@ -1312,8 +1250,8 @@ static plf_status run_match(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   plf_mark(ctx, cs, "f2f.k_nnr_mutual+k_f2f_build");
   if ((st = plf_launch_gn(ctx, cs, T_pred ? s->gn_probs_mm : s->gn_probs, B, plf_gn_opts_from_params(P), pcam, nullptr, prm))) return st;
   plf_mark(ctx, cs, "gn.k_gn_pose");
-  k_finalize<<<(B + 127) / 128, 128, 0, cs>>>(s->gn_out, s->gnNp, s->gnNl, kcnt, lcnt, s->fs, prev, s->B + s->nseq,
-                                               P.min_features, B, s->results + (size_t)rp * s->B, prm);
+  k_finalize<<<(B + 127) / 128, 128, 0, cs>>>(s->gn_out, s->gnNp, s->gnNl, kcnt, lcnt, s->fs, prev, s->B + s->nseq, B,
+                                               s->results + (size_t)rp * s->B, prm);
   PLF_LAUNCH_CHECK(ctx);
   k_carry<<<dim3(PLF_FS_NFIELDS, r.ncarry), 256, 0, cs>>>(s->fs, carry, K, Ln);   // the next batch tracks against these
   PLF_LAUNCH_CHECK(ctx);
@@ -1643,7 +1581,8 @@ plf_status plf_get_sequence_params(const plf_ctx* ctx, int s, plf_params* out) {
   plf_ctx* c = const_cast<plf_ctx*>(ctx);   // the error text is the only state a failed call writes
   if (!out) return plf_fail(c, PLF_ERR_INVALID, "plf_get_sequence_params: out is NULL");
   if (plf_status st = plf_check_sequence(c, "plf_get_sequence_params", s)) return st;
-  *out = !ctx->seqs.empty() && ctx->seqs[s].own_prm ? ctx->seqs[s].prm : ctx->params;
+  const bool own = !ctx->seqs.empty() && ctx->seqs[s].own_prm;
+  *out = own ? ctx->seqs[s].prm : ctx->params;
   return PLF_OK;
 }
 
@@ -1675,7 +1614,7 @@ plf_status plf_get_sequence_fast_th(plf_ctx* ctx, int s, int* th) {
   if (!ctx) return PLF_ERR_INVALID;
   if (!th) return plf_fail(ctx, PLF_ERR_INVALID, "plf_get_sequence_fast_th: th is NULL");
   if (plf_status st = plf_check_sequence(ctx, "plf_get_sequence_fast_th", s)) return st;
-  *th = !ctx->seqs.empty() && ctx->seqs[s].own_prm ? ctx->seqs[s].pair.fast_th : fast_th0(ctx);
+  *th = plf_sequence_pair(ctx, s).fast_th;
   if (!ctx->afast_on || !ctx->pipe || !ctx->pipe->carried[s]) return PLF_OK;   // the next pair is detected at orb_fast_th
   SeqRecord q;
   if (plf_status st = pipe_seq_read(ctx, s, &q)) return st;
@@ -1955,19 +1894,20 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
     carry[2 * r.ncarry + 1] = s->B + q[k];
     r.ncarry++;
   }
-  // the cameras, maps and masks of the pairs, resolved now: a later plf_set_sequence_camera, _rectification or _mask does
-  // not reach this batch.  The input table of a grey batch lists its rectified pairs; a colour batch, converted whole,
-  // lists every pair when one of them is rectified.
-  r.cams = false;
+  // the cameras, settings, maps and masks of the pairs, resolved now: a later plf_set_sequence_camera, _params,
+  // _rectification or _mask does not reach this batch.  The input table of a grey batch lists its rectified pairs; a colour
+  // batch, converted whole, lists every pair when one of them is rectified.
   r.nin = 0;
   r.masked = false;
-  r.prm = false;
+  r.nwin = 0;
+  r.best_lr = false;
   bool rect = false;
   for (int k = 0; k < B; ++k) {
-    r.prm |= !ctx->seqs.empty() && ctx->seqs[q[k]].own_prm;
     const plf_camera& c = plf_sequence_camera(ctx, q[k]);
     tab.cams[k] = PlfPairCam{c.fx, c.fy, c.cx, c.cy, c.b};
-    r.cams |= &c != &ctx->cam;
+    tab.prm[k] = plf_sequence_pair(ctx, q[k]);
+    r.nwin += tab.prm[k].matching_strategy != 0;
+    r.best_lr |= tab.prm[k].best_lr != 0;
     const PlfSequence* sq = ctx->seqs.empty() ? nullptr : &ctx->seqs[q[k]];
     const uint8_t* maps = sq ? sq->rect : nullptr;
     if (maps || s->up_ch > 1) tab.in[r.nin++] = PlfRectPair{maps, k, 0};
@@ -1978,20 +1918,6 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
     }
   }
   if (!rect) r.nin = 0;
-  // the settings of the pairs, resolved now as the cameras are: a table only when a sequence of the batch has its own
-  r.nwin = ctx->params.matching_strategy ? B : 0;
-  r.best_lr = ctx->params.best_lr_matches != 0;
-  if (r.prm) {
-    const PlfPairPrm own0 = plf_pair_prm(ctx->params);
-    r.nwin = 0;
-    r.best_lr = false;
-    for (int k = 0; k < B; ++k) {
-      const PlfSequence& sq = ctx->seqs[q[k]];
-      tab.prm[k] = sq.own_prm ? sq.pair : own0;
-      r.nwin += tab.prm[k].matching_strategy != 0;
-      r.best_lr |= tab.prm[k].best_lr != 0;
-    }
-  }
   r.run_slot = s->up_slot;
   // With profiling on everything is serialised on the main stream so that the per-kernel marks are meaningful.
   r.piped = !ctx->profile || ctx->profile_piped;

@@ -277,6 +277,7 @@ plf_status plf_create(const plf_params* params, const plf_camera* cam, const plf
     ctx->params = *params;
   else
     plf_default_params(&ctx->params);
+  ctx->pair = plf_pair_prm(ctx->params);
   if (cam)
     ctx->cam = *cam;
   else {

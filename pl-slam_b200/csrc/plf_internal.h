@@ -89,8 +89,9 @@ struct PlfTmaCache;   // plf_tma.cuh
 struct BowDbs;        // dbow.cu
 
 #define PLF_ORB_MAX_LEVELS 8
-// The front-end settings of one pair of a batch (plf_set_sequence_params): its sequence's plf_params, as the consumers read
-// them, resolved when the batch was run.  A consumer given no table reads the context's plf_params instead.
+// The front-end settings of one pair of a batch (plf_set_sequence_params): its sequence's plf_params, or the context's, as
+// the consumers read them, resolved when the batch was run.  The standalone detectors read a one-entry table of the
+// context's.
 struct PlfPairPrm {
   int orb_nlevels;                       // <= the context's: the levels the pair's images detect on
   int orb_nfeat[PLF_ORB_MAX_LEVELS];     // nfeaturesPerLevel of orb_nfeatures over orb_nlevels (plf_orb_level_features)
@@ -103,7 +104,7 @@ struct PlfPairPrm {
   int matching_strategy, matching_s_ws, matching_f2f_ws, min_pt_matches, min_ls_matches, min_features;
   plf_gn_opts gn;                        // plf_gn_opts_from_params
 };
-PlfPairPrm plf_pair_prm(const plf_params& p);
+PlfPairPrm plf_pair_prm(const plf_params& p);   // orb_nfeat stays 0 for an orb_nlevels no ORB state accepts
 
 // What one sequence of a batched context has of its own; plf_reset_sequence keeps it, plf_drop_sequences frees it.
 struct PlfSequence {
@@ -122,6 +123,7 @@ struct plf_ctx {
   cudaStream_t stream = nullptr;  // main stream: copies, the serial part of the pipeline, standalone operators
   cudaStream_t aux[3] = {nullptr, nullptr, nullptr};  // streams of the extraction (E), LSD growing (G) and LSD pre-grow (P) phases of plf_batch_run
   plf_params params;
+  PlfPairPrm pair;                // plf_pair_prm(params), built by plf_create: params do not change after it
   plf_camera cam;
   plf_limits limits;
   int max_sequences = 1;          // plf_set_max_sequences: fixed once the pipeline exists
@@ -167,6 +169,11 @@ inline PlfSequence& plf_sequence(plf_ctx* ctx, int s) {
 // The camera of sequence s (-1: the context's): its own calibration if it has one, else the context's.
 inline const plf_camera& plf_sequence_camera(const plf_ctx* ctx, int s) {
   return s >= 0 && !ctx->seqs.empty() && ctx->seqs[s].own_cam ? ctx->seqs[s].cam : ctx->cam;
+}
+// The settings of sequence s as the front-end reads them: its own if it has them, else the context's.
+inline const PlfPairPrm& plf_sequence_pair(const plf_ctx* ctx, int s) {
+  const bool own = !ctx->seqs.empty() && ctx->seqs[s].own_prm;
+  return own ? ctx->seqs[s].pair : ctx->pair;
 }
 // The index of image size w x h in the batched pipeline's list: 0 for the context's (cam), 1 + i for image_sizes' i-th,
 // -1 for a size it does not accept.
@@ -340,13 +347,13 @@ plf_status plf_orb_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg, bo
 // What plf_orb_create would refuse for w x h, with its message, allocating nothing; the level sizes when nlevels is given.
 plf_status plf_orb_check_size(plf_ctx* ctx, int w, int h, int* nlevels = nullptr, int* lw = nullptr, int* lh = nullptr);
 void plf_orb_free(OrbState* s);
-// img_th: the FAST threshold of each image, on the device (plf_set_adaptive_fast), or NULL for plf_params.orb_fast_th.
+// prm: a device table of pair settings, prm[z / 2] for image z: its level count (at most the state's), per-level counts and
+// FAST threshold.
+// img_th: the FAST threshold of each image, on the device (plf_set_adaptive_fast), or NULL for prm's.
 // masks: a device table of each image's mask pyramid (plf_orb_mask_build), an entry NULL for an unmasked image, or NULL
 // for no mask at all (the unmasked FAST kernel).
-// prm: a device table of pair settings, prm[z / 2] for image z (plf_set_sequence_params: its level count, at most the
-// state's, and per-level counts), or NULL for plf_params' own.
 plf_status plf_orb_run(plf_ctx* ctx, cudaStream_t cs, OrbState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int nimg, int par,
-                       const int* img_th, const uint8_t* const* masks, const PlfPairPrm* prm = nullptr);
+                       const int* img_th, const uint8_t* const* masks, const PlfPairPrm* prm);
 // nfeaturesPerLevel of cv::ORB (orb.cpp computeKeyPoints): nfeat[l] for l < nlevels.
 void plf_orb_level_features(int nfeatures, float scale_factor, int nlevels, int* nfeat);
 // One image's mask pyramid in s's level layout: its bytes (allocate 64 more, as every image buffer), and its build from a
@@ -386,7 +393,7 @@ plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t
 // stage reads level 0 (plf_pitch16(w) bytes per row) of each listed image.  prm: as for plf_orb_run, image z's
 // lsd_nfeatures and min_line_length from prm[z / 2].
 plf_status plf_lsd_grow(plf_ctx* ctx, cudaStream_t cs, LsdState* s, int par, int n, cudaEvent_t keylines_wait,
-                        const uint8_t* const* masks, const PlfPairPrm* prm = nullptr);
+                        const uint8_t* const* masks, const PlfPairPrm* prm);
 void plf_lsd_outputs(const LsdState* s, int par, plf_keyline** kls, int** nlines, int* max_lines);
 // Causes of the LSD overflow flag, one bit each (as the ORB flag above)
 enum { PLF_LSD_OVF_SEGMENTS = 1,   // an image grows more regions than plf_limits.max_segments (k_lsd_grow)

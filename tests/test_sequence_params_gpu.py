@@ -318,7 +318,7 @@ def test_defaults_refusals_and_launch_count(built):
     """plf_get_sequence_params round-trips and NULL restores the context's; every refusal returns PLF_ERR_INVALID naming
     the field and changes nothing (the next batch tracks on, equal to the uninterrupted run); plf_set_max_sequences drops
     the settings and plf_reset_sequence keeps them; a batch with no sequence settings launches what it launches on a
-    context that never called plf_set_sequence_params."""
+    context that never called plf_set_sequence_params, and so does a batch of the sequence that has them."""
     seqs = sequences()
     ctx = full(matching_strategy=0)
     kit = full("kitti")
@@ -370,16 +370,17 @@ def test_defaults_refusals_and_launch_count(built):
         fe.set_sequence_params(1, **kit)
         fe._check(fe.lib.plf_set_max_sequences(fe._ctx, 3), "plf_set_max_sequences")
         assert all(params_dict(fe.get_sequence_params(s)) == params_dict(fe.params) for s in range(3))
-    # launches: a batch of sequence 0 only, on a context whose sequence 1 has settings, and on one that never set any
+    # launches: a batch of sequence 0 only, on a context that never set any settings and on one whose sequence 1 has
+    # settings, and a batch of sequence 1 only
     counts = []
-    for setit in (False, True):
+    for setit, s in ((False, 0), (True, 0), (True, 1)):
         with plf.Frontend(camera=CAM, limits=limits(4), max_sequences=2, **ctx) as fe:
             if setit:
                 fe.set_sequence_params(1, **kit)
-            L, R, seq = batch_args(seqs, [(0, i) for i in range(4)])
+            L, R, seq = batch_args(seqs, [(s, i) for i in range(4)])
             fe.batch_upload(L, R)
             n0 = fe.lib.plf_launch_count(fe._ctx)
             fe.batch_run(4, seq=seq)
             fe.batch_download_array(4)
             counts.append(fe.lib.plf_launch_count(fe._ctx) - n0)
-    assert counts[0] == counts[1], counts
+    assert counts[0] == counts[1] == counts[2], counts
