@@ -796,6 +796,32 @@ plf_status plf_set_image_sizes(plf_ctx* ctx, int n, const int32_t* wh);
 plf_status plf_batch_upload_sized(plf_ctx* ctx, int B, int w, int h, const uint8_t* left, const uint8_t* right, int stride,
                                   int channels);
 
+/* Restricts ORB and line detection on the pairs of the most recent upload to masks that come with it, one per image, as
+ * the detectors' mask arguments do (cv::ORB::detectAndCompute(img, mask), LSDDetectorC::detect(..., mask)): for masks that
+ * change every frame, such as a segmentation network's dynamic objects.
+ *   - Layout: mask_l / mask_r hold B masks each, h rows of `stride` bytes, mask k at offset k*stride*h, like
+ *     plf_batch_upload's images.  One channel, any non-zero value allowed, of the most recent upload's size
+ *     (plf_batch_device_layout) and in the geometry the detectors see: after rectification and after the grey conversion.
+ *   - They belong to the most recent upload (grey, colour, sized, or images written through plf_batch_device_images), and
+ *     the run that consumes it uses them.  The next upload, and any later run, starts without them.  Calling again before
+ *     the run replaces them.
+ *   - A NULL side has no pair masks; its images keep their sequence's mask (plf_set_sequence_mask), if any.
+ *   - An image with a pair mask and a sequence mask is restricted to their pixelwise AND (non-zero where both are).  ORB's
+ *     mask pyramid is built from that AND, as one mask given to detectAndCompute.
+ *   - Memory: host memory, pageable or pinned, or device memory of the context's device (a torch CUDA tensor's
+ *     data_ptr(), say).  Finish writing the masks before the call (for a PyTorch producer, synchronise its stream), and
+ *     keep them unchanged until that batch's plf_batch_download returns.
+ *   - The copy is asynchronous, on the upload stream, and waits for the earlier runs of the same image slot to have read
+ *     that slot's masks.  The rest of each mask's pyramid is built on the device by the run.
+ * Device memory: the first call allocates two blocks, one per upload slot, each of 2 max_batch ORB mask pyramids of the
+ * largest image size (about 2.5 w h bytes each at 4 levels of scale 1.2), kept until plf_destroy: about 4.8 GB at
+ * 1242 x 375, 4 levels and max_batch 1024.  A context that never calls it allocates, copies and launches nothing for it.
+ * Refusals happen before anything is enqueued, name the argument and change nothing: PLF_ERR_STATE before the first upload;
+ * PLF_ERR_INVALID for B outside [1, max_batch], both masks NULL, stride < w, or device memory of another device;
+ * PLF_ERR_CUDA when the blocks cannot be allocated.  plf_batch_run_sequences refuses a B other than the masks' B
+ * (PLF_ERR_INVALID, before anything is enqueued). */
+plf_status plf_batch_upload_masks(plf_ctx* ctx, int B, const uint8_t* mask_l, const uint8_t* mask_r, int stride);
+
 /* Number of sequences a context can track at once (default 1), 1 <= n <= 2^20.  Call it before the first plf_batch_* call:
  * PLF_ERR_STATE once the pipeline exists, PLF_ERR_INVALID for n out of range.  Each sequence keeps one carried frame slot
  * on the device (84 * max_keypoints + 156 * max_lines + 8 bytes). */

@@ -931,17 +931,64 @@ void plf_orb_outputs(const OrbState* s, int par, plf_keypoint** kps, uint8_t** d
   *kps = s->kps[par]; *desc = s->desc[par]; *counts = s->kp_count[par]; *max_kp = s->g.max_kp;
 }
 
-// ---- masks (plf_set_sequence_mask, plf_orb_masked) ------------------------------------------------------
-// One mask level to 255 where it exceeds lo, else 0: lo = 0 binarises the caller's mask (level 0), lo = 254 is
-// cv::threshold(level, level, 254, 0, THRESH_TOZERO) of a resized level (only 255 survives).
-__global__ void __launch_bounds__(256) k_mask_level(uint8_t* __restrict__ m, int pitch, int w, int lo) {
-  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
-  if (x >= w) return;
-  uint8_t& v = m[(size_t)y * pitch + x];
-  v = v > lo ? 255 : 0;
+// ---- masks (plf_set_sequence_mask, plf_orb_masked, plf_batch_upload_masks) ------------------------------
+// Level l of every pyramid of a batched build (plf_orb_mask_pyramids), gridded [tile of 128 x 8 pixels, pyramid], four
+// adjacent pixels per thread (rows are 16-byte aligned, so one 32-bit store; bytes past the level's width land in the
+// row's padding, which nothing reads).
+//   l = 0   in place: 255 where the caller's mask and the and_with pyramid's level 0 are both non-zero, else 0.
+//   l >= 1  the INTER_LINEAR_EXACT resize of level l-1 (k_resize_exact's integer arithmetic, tables tabx / taby) fused
+//           with cv::threshold(254, THRESH_TOZERO): only a 255 survives, as 255.
+// tab NULL: the one pyramid `one`.
+__global__ void __launch_bounds__(256) k_mask_pyramid(const PlfMaskBuild* __restrict__ tab, PlfMaskBuild one, OrbGeom g, int l,
+                                                      int tiles_x, const int* __restrict__ tabx, const int* __restrict__ taby) {
+  const int W = g.w[l], H = g.h[l];
+  const int x = ((blockIdx.x % tiles_x) * 32 + threadIdx.x) * 4, y = (blockIdx.x / tiles_x) * 8 + threadIdx.y;
+  if (x >= W || y >= H) return;
+  const PlfMaskBuild e = tab ? tab[blockIdx.y] : one;
+  const int dp = (W + 15) & ~15;
+  uint32_t* d = reinterpret_cast<uint32_t*>(e.dst + orb_mask_off(g, l) + (size_t)y * dp + x);
+  if (l == 0) {
+    uint32_t m = *d;
+    if (e.and_with) {
+      const uint32_t a = *reinterpret_cast<const uint32_t*>(e.and_with + (size_t)y * dp + x);
+      m = __vcmpne4(m, 0u) & __vcmpne4(a, 0u);
+    } else {
+      m = __vcmpne4(m, 0u);
+    }
+    *d = m;
+    return;
+  }
+  const int sw = g.w[l - 1], sh = g.h[l - 1], sp = (sw + 15) & ~15;
+  const uint8_t* src = e.dst + orb_mask_off(g, l - 1);
+  const int oy = taby[y], cy = taby[H + y];
+  const uint8_t* r0 = src + (size_t)oy * sp;
+  const uint8_t* r1 = oy + 1 < sh ? r0 + sp : r0;   // cy is 0 on the last source row
+  uint32_t out = 0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int xi = min(x + i, W - 1);   // past the width: a copy of the last column, into the padding
+    const int ox = tabx[xi], cx = tabx[W + xi];
+    const uint32_t h0 = r0[ox] * (256 - cx) + r0[ox + 1] * cx;
+    const uint32_t h1 = r1[ox] * (256 - cx) + r1[ox + 1] * cx;
+    const uint32_t v = (h0 * (256 - cy) + h1 * cy + 32768u) >> 16;
+    out |= (v > 254 ? 255u : 0u) << (8 * i);
+  }
+  *d = out;
 }
 
 size_t plf_orb_mask_bytes(const OrbState* s) { return plf_align256((size_t)plf_pitch16(s->w) * s->h) + s->g.pyr_stride; }
+
+plf_status plf_orb_mask_pyramids(plf_ctx* ctx, cudaStream_t cs, const OrbState* s, const PlfMaskBuild* tab, PlfMaskBuild one, int n) {
+  const OrbGeom& g = s->g;
+  for (int l = 0; l < g.nlevels; ++l) {
+    const int tx_ = (g.w[l] + 127) / 128, ty_ = (g.h[l] + 7) / 8;
+    const int* tabx = l ? s->rs_tab + s->rs_x_off[l] : nullptr;
+    const int* taby = l ? s->rs_tab + s->rs_y_off[l] : nullptr;
+    k_mask_pyramid<<<dim3(tx_ * ty_, n), dim3(32, 8), 0, cs>>>(tab, one, g, l, tx_, tabx, taby);
+    PLF_LAUNCH_CHECK(ctx);
+  }
+  return PLF_OK;
+}
 
 // detectAndCompute's mask pyramid as cv2 4.13 applies it: level 0 = the caller's w x h mask (stride bytes per row), any
 // non-zero value 255; level l >= 1 = resize(level l-1, INTER_LINEAR_EXACT) thresholded to 255 or 0.  (Resizing the
@@ -949,20 +996,8 @@ size_t plf_orb_mask_bytes(const OrbState* s) { return plf_align256((size_t)plf_p
 // dst (plf_orb_mask_bytes(s) bytes + 64 of slack, the layout of orb_mask_off) on cs; s lends its geometry and resize
 // tables.
 plf_status plf_orb_mask_build(plf_ctx* ctx, cudaStream_t cs, const OrbState* s, const uint8_t* mask, int stride, uint8_t* dst) {
-  const OrbGeom& g = s->g;
   PLF_CUDA(ctx, cudaMemcpy2DAsync(dst, plf_pitch16(s->w), mask, stride, s->w, s->h, cudaMemcpyHostToDevice, cs));
-  k_mask_level<<<dim3((s->w + 255) / 256, s->h), 256, 0, cs>>>(dst, plf_pitch16(s->w), s->w, 0);
-  PLF_LAUNCH_CHECK(ctx);
-  for (int l = 1; l < g.nlevels; ++l) {
-    uint8_t* lvl = dst + orb_mask_off(g, l);
-    const int sp = plf_pitch16(g.w[l - 1]), dp = plf_pitch16(g.w[l]);
-    plf_status st = plf_launch_resize_exact(ctx, cs, dst + orb_mask_off(g, l - 1), 0, sp, g.w[l - 1], g.h[l - 1], lvl, 0, dp, g.w[l],
-                                            g.h[l], s->rs_tab + s->rs_x_off[l], s->rs_tab + s->rs_xp_off[l], s->rs_tab + s->rs_y_off[l], 1);
-    if (st) return st;
-    k_mask_level<<<dim3((g.w[l] + 255) / 256, g.h[l]), 256, 0, cs>>>(lvl, dp, g.w[l], 254);
-    PLF_LAUNCH_CHECK(ctx);
-  }
-  return PLF_OK;
+  return plf_orb_mask_pyramids(ctx, cs, s, nullptr, PlfMaskBuild{dst, nullptr}, 1);
 }
 
 // plf_orb and plf_orb_masked (mask NULL: unmasked).  The one-entry settings table (the context's), and the mask pyramid

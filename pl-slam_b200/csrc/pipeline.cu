@@ -51,9 +51,10 @@ struct PlfRectPair { const uint8_t* maps; int pair; int pad; };
 
 // One entry of the batch table ring, for max_batch pairs B: the sequence table (prev[B] = the frame slot of pair k's
 // previous frame, then the carry list [B][2] of (frame slot, carry slot)), the pairs' cameras [B] and settings [B]
-// (plf_set_sequence_camera, plf_set_sequence_params, else the context's), then the input table [B] and the mask table
-// [2B] (image z's mask pyramid, plf_set_sequence_mask, or NULL).  Every batch uses the parts before the input table: they
-// are one copy.  The pinned and the device ring use the same layout.
+// (plf_set_sequence_camera, plf_set_sequence_params, else the context's), then the input table [B], the mask table [2B]
+// (image z's mask pyramid: its pair mask's, plf_batch_upload_masks, else its sequence's, plf_set_sequence_mask, else
+// NULL) and the build list [2B] of the pair masks' pyramids.  Every batch uses the parts before the input table: they are
+// one copy.  The pinned and the device ring use the same layout.
 struct BatchTab {
   int32_t* prev;
   int32_t* carry;
@@ -61,18 +62,21 @@ struct BatchTab {
   PlfPairPrm* prm;
   PlfRectPair* in;
   const uint8_t** masks;
+  PlfMaskBuild* build;
 };
 static size_t batch_tab_bytes(int B) {
   return plf_align256(3 * sizeof(int32_t) * B) + plf_align256(sizeof(PlfPairCam) * B) + plf_align256(sizeof(PlfPairPrm) * B) +
-         plf_align256(sizeof(PlfRectPair) * B) + plf_align256(sizeof(uint8_t*) * 2 * B);
+         plf_align256(sizeof(PlfRectPair) * B) + plf_align256(sizeof(uint8_t*) * 2 * B) + plf_align256(sizeof(PlfMaskBuild) * 2 * B);
 }
 static BatchTab batch_tab(uint8_t* base, int B) {
   uint8_t* cams = base + plf_align256(3 * sizeof(int32_t) * B);
   uint8_t* prm = cams + plf_align256(sizeof(PlfPairCam) * B);
   uint8_t* in = prm + plf_align256(sizeof(PlfPairPrm) * B);
   uint8_t* masks = in + plf_align256(sizeof(PlfRectPair) * B);
+  uint8_t* build = masks + plf_align256(sizeof(uint8_t*) * 2 * B);
   return {reinterpret_cast<int32_t*>(base), reinterpret_cast<int32_t*>(base) + B, reinterpret_cast<PlfPairCam*>(cams),
-          reinterpret_cast<PlfPairPrm*>(prm), reinterpret_cast<PlfRectPair*>(in), reinterpret_cast<const uint8_t**>(masks)};
+          reinterpret_cast<PlfPairPrm*>(prm), reinterpret_cast<PlfRectPair*>(in), reinterpret_cast<const uint8_t**>(masks),
+          reinterpret_cast<PlfMaskBuild*>(build)};
 }
 
 // What each sequence carries to its next pair besides its frame slot: the pose prediction (row-major 4x4) and whether it
@@ -119,8 +123,17 @@ struct PipeState {
   // channels of the last upload: 1 for plf_batch_upload (its images are in imgs2[up_slot]), 3 or 4 for
   // plf_batch_upload_color (its images are in the colour landing buffer until the run converts them into imgs2[up_slot])
   int up_ch = 1;
+  bool uploaded = false;       // an upload was made, or device_images handed out a slot
   cudaStream_t copy = nullptr; // H2D stream
   cudaEvent_t ev_up[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr}, ev_free2[2] = {nullptr, nullptr};
+  // Pair masks (plf_batch_upload_masks): mpyr[slot] holds the mask pyramids of images 0 .. 2 max_batch - 1 of the upload
+  // in that slot, one every mask_stride(size) bytes (PLF_SCR_MASK_PIPE, carved at the first mask upload).  mask_B pairs of
+  // the most recent upload have masks on the sides mask_side (0: none); the run that consumes the upload takes them.
+  // ev_mfree[slot]: the KeyLine stage of the last run with pair masks in that slot has read them.
+  uint8_t* mpyr[2] = {nullptr, nullptr};
+  int mask_B = 0;
+  bool mask_side[2] = {false, false};
+  cudaEvent_t ev_mfree[2] = {nullptr, nullptr};
   short2* lbd_grad[2] = {nullptr, nullptr};  // [parity][2B][h*w]
   uint8_t* ldesc_raw = nullptr;  // [2B][max_ln][32]  LBD of every kept KeyLine
   FrameSlots fs;               // B + nseq + 1 slots
@@ -236,7 +249,7 @@ static std::vector<PipeEvents> pipe_events(PipeState* s) {
           {s->evM, 3, cudaEventBlockingSync},    {s->tM0, 3, cudaEventDefault},           {s->evE, 2, cudaEventDefault},
           {s->evG, 2, cudaEventDefault},         {s->evX, 2, cudaEventDisableTiming},     {s->evP, 2, cudaEventDisableTiming},
           {s->tE0, 2, cudaEventDefault},         {s->tG0, 2, cudaEventDefault},           {s->ev_tab, 3, cudaEventDisableTiming},
-          {&s->ev_th, 1, cudaEventDisableTiming}};
+          {&s->ev_th, 1, cudaEventDisableTiming}, {s->ev_mfree, 2, cudaEventDisableTiming}};
 }
 
 extern "C" void plf_pipe_free(plf_ctx* ctx) {
@@ -897,7 +910,8 @@ struct BatchRun {
   int g;         // the batch's image size: record s->geo[g], the size of the upload it consumes
   int ncarry;    // entries of the carry list in batch table rp: the sequences the batch holds
   int nin;       // entries of the input table in batch table rp (0: none, every pair is converted as it is)
-  bool masked;   // batch table rp holds the images' masks (a sequence of the batch has one); else no image is masked
+  bool masked;   // batch table rp holds the images' masks (a pair or a sequence of the batch has one); else no image is masked
+  int nbuild;    // entries of the build list in batch table rp: the images with a pair mask (plf_batch_upload_masks)
   int nwin;      // pairs at matching_strategy != 0
   bool best_lr;  // some pair matches with best_lr_matches
   bool afast;    // adaptive FAST thresholds (plf_set_adaptive_fast): pair thresholds in the E phase, the next ones behind k_finalize
@@ -915,8 +929,8 @@ static BatchTab host_tab(const PipeState* s, int rp) { return batch_tab(s->h_tab
 static BatchTab dev_tab(const PipeState* s, int rp) { return batch_tab(s->tab + rp * batch_tab_bytes(s->B), s->B); }
 
 // The parts of the batch's table that it uses, to ring entry rp of the device on the copy stream: the sequence table, the
-// cameras and the settings always (one copy, up to the batch's last settings), the input table and the masks when it has
-// them.  ev_tab[rp] marks them.
+// cameras and the settings always (one copy, up to the batch's last settings), the input table, the masks and the build
+// list when it has them.  ev_tab[rp] marks them.
 static plf_status send_tab(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   const BatchTab h = host_tab(s, r.rp), d = dev_tab(s, r.rp);
   cudaStream_t cs = s->copy;
@@ -924,6 +938,7 @@ static plf_status send_tab(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PLF_CUDA(ctx, cudaMemcpyAsync(d.prev, h.prev, head, cudaMemcpyHostToDevice, cs));
   if (r.nin) PLF_CUDA(ctx, cudaMemcpyAsync(d.in, h.in, sizeof(PlfRectPair) * r.nin, cudaMemcpyHostToDevice, cs));
   if (r.masked) PLF_CUDA(ctx, cudaMemcpyAsync(d.masks, h.masks, sizeof(uint8_t*) * 2 * r.B, cudaMemcpyHostToDevice, cs));
+  if (r.nbuild) PLF_CUDA(ctx, cudaMemcpyAsync(d.build, h.build, sizeof(PlfMaskBuild) * r.nbuild, cudaMemcpyHostToDevice, cs));
   PLF_CUDA(ctx, cudaEventRecord(s->ev_tab[r.rp], cs));
   return PLF_OK;
 }
@@ -1051,6 +1066,37 @@ static plf_status run_input(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   return PLF_OK;
 }
 
+// Bytes between two images' mask pyramids in a block of PLF_SCR_MASK_PIPE at image size G: a multiple of the row pitch,
+// so that one 3-D copy per side lands an upload's level 0 planes.
+static size_t mask_stride(const PipeGeo& G) {
+  const size_t b = plf_orb_mask_bytes(G.orb);
+  return (b + G.pitch - 1) / G.pitch * G.pitch;
+}
+
+// The pair masks' pyramid blocks, one per upload slot, each of 2 max_batch pyramids at the largest mask_stride of any
+// size: carved from PLF_SCR_MASK_PIPE, which is allocated at the first call and never grows after it.
+static plf_status mask_scratch(plf_ctx* ctx, PipeState* s) {
+  size_t img = 0;
+  for (const PipeGeo& G : s->geo) img = std::max(img, mask_stride(G));
+  DevBufList b;
+  b.add(s->mpyr[0], 2 * (size_t)s->B * img);
+  b.add(s->mpyr[1], 2 * (size_t)s->B * img);
+  return b.carve(ctx, PLF_SCR_MASK_PIPE);
+}
+
+// Builds the pair masks' pyramids of the upload the run consumes (plf_batch_upload_masks landed their level 0): on the
+// copy stream, behind the upload, the mask copy and the batch table, each ANDed with its sequence's mask as the build list
+// gives it; ev_up[run_slot] is recorded again, so the E and P phases (which wait for it) read the result.
+static plf_status run_masks(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
+  if (r.nbuild == 0) return PLF_OK;
+  cudaStream_t cs = s->copy;
+  plf_mark(ctx, cs, "masks.start");
+  if (plf_status st = plf_orb_mask_pyramids(ctx, cs, s->geo[r.g].orb, dev_tab(s, r.rp).build, PlfMaskBuild{}, r.nbuild)) return st;
+  plf_mark(ctx, cs, "masks.k_mask_pyramid");
+  PLF_CUDA(ctx, cudaEventRecord(s->ev_up[r.run_slot], cs));
+  return PLF_OK;
+}
+
 // ---- E phase: ORB + LBD gradient prelude (bandwidth / ALU bound); outputs per batch parity ----
 static plf_status run_extract(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   PipeGeo& G = s->geo[r.g];
@@ -1112,6 +1158,8 @@ static plf_status run_lsd(plf_ctx* ctx, PipeState* s, const BatchRun& r) {
   st = plf_lsd_grow(ctx, sG, G.lsd, r.lp, 2 * r.B, r.piped ? s->evX[r.lsd2 ? par : par ^ 1] : nullptr, r.masked ? tab.masks : nullptr,
                     tab.prm);
   if (st) return st;
+  // the KeyLine stage has read the pair masks' level 0: the next mask upload into the slot may overwrite them
+  if (r.nbuild) PLF_CUDA(ctx, cudaEventRecord(s->ev_mfree[r.run_slot], sG));
   PLF_CUDA(ctx, cudaMemcpyAsync(s->d_ovf + 2 * r.rp + 1, plf_lsd_overflow_flag(G.lsd), sizeof(int), cudaMemcpyDeviceToDevice, sG));
   PLF_CUDA(ctx, cudaMemsetAsync(plf_lsd_overflow_flag(G.lsd), 0, sizeof(int), sG));
   PLF_CUDA(ctx, cudaEventRecord(s->evG[par], sG));
@@ -1703,6 +1751,8 @@ static plf_status upload_grey(plf_ctx* ctx, int g, int B, const uint8_t* left, c
   s->up_slot = slot;
   s->up_ch = 1;
   s->up_geo = g;
+  s->uploaded = true;
+  s->mask_B = 0;
   return PLF_OK;
 }
 
@@ -1721,6 +1771,8 @@ static plf_status upload_color(plf_ctx* ctx, int g, int B, const uint8_t* left, 
   s->up_slot ^= 1;
   s->up_ch = channels;
   s->up_geo = g;
+  s->uploaded = true;
+  s->mask_B = 0;
   return PLF_OK;
 }
 
@@ -1765,7 +1817,57 @@ plf_status plf_batch_upload_sized(plf_ctx* ctx, int B, int w, int h, const uint8
 void* plf_batch_device_images(plf_ctx* ctx) {
   if (!ctx) return nullptr;
   if (pipe_prepare(ctx)) return nullptr;
+  ctx->pipe->uploaded = true;
   return ctx->pipe->imgs2[ctx->pipe->up_slot];
+}
+
+plf_status plf_batch_upload_masks(plf_ctx* ctx, int B, const uint8_t* mask_l, const uint8_t* mask_r, int stride) {
+  const char* fn = "plf_batch_upload_masks";
+  if (!ctx) return plf_fail(nullptr, PLF_ERR_INVALID, "%s: ctx is NULL", fn);
+  PipeState* s = ctx->pipe;
+  if (!s || !s->uploaded)
+    return plf_fail(ctx, PLF_ERR_STATE, "%s: no upload yet; the masks belong to the most recent upload, so upload the images first", fn);
+  if (B < 1 || B > s->B) return plf_fail(ctx, PLF_ERR_INVALID, "%s: B = %d, need 1 <= B <= max_batch = %d", fn, B, s->B);
+  if (!mask_l && !mask_r) return plf_fail(ctx, PLF_ERR_INVALID, "%s: mask_l and mask_r are both NULL; give at least one", fn);
+  const PipeGeo& G = s->geo[s->up_geo];
+  if (stride < G.w)
+    return plf_fail(ctx, PLF_ERR_INVALID, "%s: stride = %d, need stride >= width = %d of the upload's images", fn, stride, G.w);
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  const uint8_t* src[2] = {mask_l, mask_r};
+  const char* name[2] = {"mask_l", "mask_r"};
+  for (int side = 0; side < 2; ++side) {
+    if (!src[side]) continue;
+    cudaPointerAttributes a = {};
+    if (cudaPointerGetAttributes(&a, src[side]) != cudaSuccess) {
+      cudaGetLastError();
+      a.type = cudaMemoryTypeUnregistered;   // pageable host memory
+    }
+    if (a.type == cudaMemoryTypeDevice && a.device != ctx->device)
+      return plf_fail(ctx, PLF_ERR_INVALID, "%s: %s is memory of device %d, and the context runs on device %d", fn, name[side], a.device,
+                      ctx->device);
+  }
+  if (plf_status st = mask_scratch(ctx, s)) return st;
+  // level 0 of image 2k + side's pyramid: mask k of that side, one 3-D copy per side (the destination "height" spans two
+  // pyramids, skipping the other side's).  The copy waits for the runs that read the slot's pyramids before: their ORB
+  // (ev_free) and KeyLine (ev_mfree) stages.
+  const int slot = s->up_slot;
+  const size_t img = mask_stride(G);
+  cudaStream_t cs = s->copy;
+  PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_free[slot], 0));
+  PLF_CUDA(ctx, cudaStreamWaitEvent(cs, s->ev_mfree[slot], 0));
+  for (int side = 0; side < 2; ++side) {
+    if (!src[side]) continue;
+    cudaMemcpy3DParms cp = {};
+    cp.srcPtr = make_cudaPitchedPtr(const_cast<uint8_t*>(src[side]), (size_t)stride, (size_t)G.w, (size_t)G.h);
+    cp.dstPtr = make_cudaPitchedPtr(s->mpyr[slot] + side * img, (size_t)G.pitch, (size_t)G.w, 2 * img / G.pitch);
+    cp.extent = make_cudaExtent((size_t)G.w, (size_t)G.h, (size_t)B);
+    cp.kind = cudaMemcpyDefault;
+    PLF_CUDA(ctx, cudaMemcpy3DAsync(&cp, cs));
+  }
+  s->mask_B = B;
+  s->mask_side[0] = mask_l != nullptr;
+  s->mask_side[1] = mask_r != nullptr;
+  return PLF_OK;
 }
 
 plf_status plf_batch_device_layout(plf_ctx* ctx, int* w, int* h, int* pitch) {
@@ -1846,6 +1948,9 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   if (seq) s->pair_seq.assign(seq, seq + B);
   else s->pair_seq.assign(B, 0);
   const int* q = s->pair_seq.data();
+  if (s->mask_B && B != s->mask_B)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_batch_run_sequences: B = %d, and the masks of the upload it runs (plf_batch_upload_masks) "
+                    "are of %d pairs", B, s->mask_B);
   // a batch is of one image size, its upload's
   const PipeGeo& G = s->geo[s->up_geo];
   for (int k = 0; k < B; ++k) {
@@ -1899,6 +2004,7 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   // batch, converted whole, lists every pair when one of them is rectified.
   r.nin = 0;
   r.masked = false;
+  r.nbuild = 0;
   r.nwin = 0;
   r.best_lr = false;
   bool rect = false;
@@ -1913,8 +2019,16 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
     if (maps || s->up_ch > 1) tab.in[r.nin++] = PlfRectPair{maps, k, 0};
     rect |= maps != nullptr;
     for (int side = 0; side < 2; ++side) {
-      tab.masks[2 * k + side] = sq ? sq->mask[side] : nullptr;
-      r.masked |= tab.masks[2 * k + side] != nullptr;
+      const int z = 2 * k + side;
+      const uint8_t* seq_mask = sq ? sq->mask[side] : nullptr;
+      if (s->mask_B && s->mask_side[side]) {
+        uint8_t* pyr = s->mpyr[s->up_slot] + z * mask_stride(G);
+        tab.build[r.nbuild++] = PlfMaskBuild{pyr, seq_mask};
+        tab.masks[z] = pyr;
+      } else {
+        tab.masks[z] = seq_mask;
+      }
+      r.masked |= tab.masks[z] != nullptr;
     }
   }
   if (!rect) r.nin = 0;
@@ -1931,6 +2045,7 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
   r.motion = ctx->motion_on;
   st = send_tab(ctx, s, r);
   if (!st) st = run_input(ctx, s, r);
+  if (!st) st = run_masks(ctx, s, r);
   if (!st) st = run_extract(ctx, s, r);
   if (!st) st = run_lsd(ctx, s, r);
   if (!st) st = run_match(ctx, s, r);
@@ -1939,6 +2054,7 @@ plf_status plf_batch_run_sequences(plf_ctx* ctx, int B, const int32_t* seq, cons
     if (!st) s->carried[q[k]] = 1;
   }
   if (st) return st;
+  s->mask_B = 0;   // the run has taken the upload's masks
   s->pend_slot[s->n_pending] = r.rp;
   s->pend_B[s->n_pending] = B;
   s->rp_geo[r.rp] = r.g;

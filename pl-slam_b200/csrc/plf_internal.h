@@ -42,6 +42,8 @@ enum plf_scratch_slot {
                        // its remapped pairs, sized for max_batch pairs once, so that it never grows under batches in flight
   PLF_SCR_COLOR_PIPE,  // plf_batch_upload_color and the conversion of plf_batch_run_sequences: the colour landing buffer
                        // of max_batch pairs (color_scratch in pipeline.cu)
+  PLF_SCR_MASK_PIPE,   // plf_batch_upload_masks and the mask build of plf_batch_run_sequences: the pair masks' pyramids,
+                       // 2 max_batch per upload slot at the largest image size (mask_scratch in pipeline.cu)
   PLF_SCR_COUNT
 };
 
@@ -360,6 +362,16 @@ void plf_orb_level_features(int nfeatures, float scale_factor, int nlevels, int*
 // host mask of s->w x s->h, stride bytes per row, on cs.  Its first plf_pitch16(w) * h bytes are the mask itself.
 size_t plf_orb_mask_bytes(const OrbState* s);
 plf_status plf_orb_mask_build(plf_ctx* ctx, cudaStream_t cs, const OrbState* s, const uint8_t* mask, int stride, uint8_t* dst);
+// One mask pyramid of a batched build (plf_orb_mask_pyramids): dst holds the caller's mask as its level 0 (any non-zero
+// value allowed), and the build ANDs in the pyramid and_with (its level 0), or nothing when that is NULL.
+struct PlfMaskBuild {
+  uint8_t* dst;
+  const uint8_t* and_with;
+};
+// Builds n mask pyramids of s's level layout in place from their level 0, one launch per level on cs: entries tab[0 .. n)
+// of a device table, or the one entry `one` when tab is NULL.  Level 0 becomes 255 where the mask and and_with are both
+// non-zero, else 0; level l >= 1 is resize(level l-1, INTER_LINEAR_EXACT) thresholded at 254, as plf_orb_mask_build.
+plf_status plf_orb_mask_pyramids(plf_ctx* ctx, cudaStream_t cs, const OrbState* s, const PlfMaskBuild* tab, PlfMaskBuild one, int n);
 void plf_orb_outputs(const OrbState* s, int par, plf_keypoint** kps, uint8_t** desc, int** counts, int* max_kp);
 // The overflow flag is a set of causes (one bit each, OR-ed in by the kernel that met it); plf_orb_overflow_text words them,
 // naming the limit that was actually hit: only max_keypoints is the caller's to raise.

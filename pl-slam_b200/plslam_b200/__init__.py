@@ -1367,12 +1367,16 @@ class Frontend:
                     "plf_set_sequence_rectification")
 
     @staticmethod
-    def _mask(mask, h, w, who):
-        """mask as a uint8 [h, w] array with unit column stride (rows may be strided)."""
+    def _mask(mask, h, w, who, B=None):
+        """mask as a uint8 [h, w] array (B given: [B, h, w], mask k h rows after mask k-1) with unit column stride (rows
+        may be strided)."""
         m = np.asarray(mask)
-        if m.dtype != np.uint8 or m.shape != (h, w):
-            raise PlfError(f"{who}: mask must be uint8{[h, w]} (got {m.dtype}{list(m.shape)})")
-        return m if m.strides[1] == 1 and m.strides[0] >= w else np.ascontiguousarray(m)
+        shape = (h, w) if B is None else (B, h, w)
+        if m.dtype != np.uint8 or m.shape != shape:
+            raise PlfError(f"{who}: mask must be uint8{list(shape)} (got {m.dtype}{list(m.shape)})")
+        rows = m.strides[-2]
+        ok = m.strides[-1] == 1 and rows >= w and (B is None or m.strides[0] == rows * h)
+        return m if ok else np.ascontiguousarray(m)
 
     def set_sequence_mask(self, s, left=None, right=None):
         """Restricts sequence s's ORB and line detection in the batched pipeline to masks: uint8 [H, W] of the sequence
@@ -1386,6 +1390,36 @@ class Frontend:
         self._check(self.lib.plf_set_sequence_mask(self._ctx, int(s), None if ml is None else _ptr(ml, C.c_uint8),
                                                    None if mr is None else _ptr(mr, C.c_uint8), W),
                     "plf_set_sequence_mask")
+
+    def batch_upload_masks(self, left=None, right=None):
+        """Restricts detection on the pairs of the most recent upload to masks of their own: uint8 [B, H, W] host arrays
+        of that upload's size (device_layout), dense or row-strided, in the geometry the detectors see (after
+        rectification, one channel), non-zero = allowed.  None leaves a side to its sequences' masks; with a sequence mask
+        an image is restricted to the AND of the two.  The run that consumes the upload uses them, and only it.
+        plf_batch_upload_masks."""
+        if left is None and right is None:
+            raise PlfError("batch_upload_masks: give the masks of at least one side")
+        W, H, _ = self.device_layout
+        B = (left if left is not None else right).shape[0]
+        ml = None if left is None else self._mask(left, H, W, "batch_upload_masks", B)
+        mr = None if right is None else self._mask(right, H, W, "batch_upload_masks", B)
+        strides = {m.strides[1] for m in (ml, mr) if m is not None}
+        if len(strides) > 1:   # one stride for both sides
+            ml, mr = (None if m is None else np.ascontiguousarray(m) for m in (ml, mr))
+        stride = (ml if ml is not None else mr).strides[1]
+        self._check(self.lib.plf_batch_upload_masks(self._ctx, int(B), None if ml is None else _ptr(ml, C.c_uint8),
+                                                    None if mr is None else _ptr(mr, C.c_uint8), int(stride)),
+                    "plf_batch_upload_masks")
+
+    def batch_upload_masks_raw(self, B, left_ptr, right_ptr, stride=None):
+        """batch_upload_masks from raw addresses (0 / None: that side has no pair masks): B masks per side of H rows of
+        `stride` bytes (None: W), mask k at offset k * stride * H.  Host memory, pageable or pinned, or device memory of
+        the context's device: a torch CUDA uint8 tensor's data_ptr(), its producer's stream synchronised first.  Keep
+        them unchanged until that batch's download.  plf_batch_upload_masks."""
+        W, _, _ = self.device_layout
+        stride = W if stride is None else int(stride)
+        self._check(self.lib.plf_batch_upload_masks(self._ctx, int(B), C.c_void_p(left_ptr or None), C.c_void_p(right_ptr or None),
+                                                    stride), "plf_batch_upload_masks")
 
     def sequence_mask_set(self, s):
         """(left, right): whether sequence s has a mask on each image.  plf_get_sequence_mask_set."""
@@ -1480,12 +1514,14 @@ class Frontend:
     def _sizes_text(self):
         return ", H x W one of " + ", ".join(f"{h} x {w}" for h, w in self._sizes_hw())
 
-    def process_batch(self, left, right, seq=None, restart=None):
+    def process_batch(self, left, right, seq=None, restart=None, masks=None):
         """B x (insertStereoPair + optimizePose): left/right uint8 [B,H,W] grey or [B,H,W,3|4] BGR / BGRA host arrays,
-        H x W the camera's size or one of image_sizes -> list of result dicts.  seq / restart: as batch_run."""
+        H x W the camera's size or one of image_sizes -> list of result dicts.  seq / restart: as batch_run.  masks:
+        (left, right) pair masks of the batch, as batch_upload_masks takes them."""
         left, right, ch = self._stack(left, right)
         B = left.shape[0]
-        if seq is None and restart is None and ch == 1 and left.shape[1:3] == (self.camera.height, self.camera.width):
+        if (seq is None and restart is None and masks is None and ch == 1
+                and left.shape[1:3] == (self.camera.height, self.camera.width)):
             res = (plf_frame_result * B)()
             st = self.lib.plf_process_batch(self._ctx, B, _ptr(left, C.c_uint8), _ptr(right, C.c_uint8),
                                             self.camera.width, res)
@@ -1493,6 +1529,8 @@ class Frontend:
             return self._result_dicts(res, B)
         seq_a, restart_a = self._sequence_table(B, seq, restart)   # checked before anything is uploaded
         self.batch_upload(left, right)
+        if masks is not None:
+            self.batch_upload_masks(*masks)
         self._run_sequences(B, seq_a, restart_a)
         return self.batch_download(B)
 
