@@ -21,6 +21,9 @@
 //                    (cv::fastAtan2 = plf_fast_atan2, degrees, f32, from a table keyed by (gx,gy)), table index}, and one packed entry
 //                    (column, |grad|^2) of the raster-ordered seed list of the pixel's row segment; per-image max of |grad|^2.
 //                    Nothing dense leaves the kernel (the record map restores itself to "undefined", see k_lsd_fill_notdef)
+//   k_lsd_pre_fused  the three kernels above in one tile kernel, from the source image (one TMA box per CTA) to the records,
+//                    seed lists, segcnt and maxmag2 k_lsd_grad writes, with no blurred or resampled map in between; it runs
+//                    where its footprint fits (5 or 7 u8 taps, the default parameters), the three kernels elsewhere
 //   k_lsd_seed_order stable counting sort of the seed lists by magnitude bin (descending), raster order inside a
 //                    bin == OpenCV's ordered_points; one CTA per image, bin counts in shared memory
 //   k_lsd_grow       region growing.  The algorithm is a sequential greedy partition (each accepted pixel updates the
@@ -78,6 +81,8 @@ struct LsdState {
   int min_reg_size = 0;
   int max_regions = 0, max_lines = 0;
   bool two_parities = false;
+  bool fused = false;         // k_lsd_pre_fused runs (lsd_pre_fused_fits); else blur, resample and gradient as three kernels
+  bool chain_maps = false;    // blur and scaled exist: the three-kernel chain can run (scale != 1 and not fused, or a test state)
   uint8_t* blur = nullptr;    // [nimg][h][bp]   bp = plf_pitch16(w)
   uint8_t* scaled = nullptr;  // [nimg][hs][sp]  sp = plf_pitch16(ws)
   int bp = 0, sp = 0;
@@ -375,6 +380,243 @@ __global__ void __launch_bounds__(LSD_GRAD_THREADS) k_lsd_grad(const uint8_t* __
     if (y0 + 1 < H) sc[(size_t)(y0 + 1) * nxb + blockIdx.x] = tot[1];
     const int m = max(max(s_max[0], s_max[1]), max(s_max[2], s_max[3]));
     if (m >= 0 && m > __ldcg(&maxmag2[im])) atomicMax(&maxmag2[im], m);   // only touch the (contended) address when it would grow
+  }
+}
+
+// ---- fused pre-blur + resample + gradient ------------------------------------------------------------------
+// k_lsd_pre_fused: what k_blur_q8_fast -> k_resize_exact4 -> k_lsd_grad compute, from the source image to the records,
+// seed lists, segcnt and maxmag2, without the blurred and resampled maps in between.  A CTA owns one 512-column row
+// segment (LSD_SEG) of LSD_PF_TH scaled rows.  Its source footprint - the blurred rows and columns the resample of its
+// scaled rows LSD_PF_TH + 1 and columns LSD_SEG + 1 reads, plus the blur halo - arrives as ONE TMA box (LSD_PF_BOXH rows of
+// LSD_PF_BOXW bytes, wider than the 256 elements a box dimension holds: the tensor map views a row as 16-byte blocks, so
+// the box is {16 bytes, LSD_PF_BOXW / 16 blocks, rows, 1 image}); border CTAs rebuild BORDER_REFLECT_101 in shared memory.
+//   blur     : k_blur_q8_fast's DP4A row pass into u16, then the column pass and its one rounding, over the footprint only
+//   resample : k_resize_exact4's integer blend from the state's tables, four scaled columns of one row per thread
+//   gradient : a warp per scaled row, four 128-column chunks of 4 columns per lane, k_lsd_grad's arithmetic, records and
+//              ordered compaction (per chunk: one warp scan; the row is the segment, so no barrier)
+// Measured on an H100 80GB HBM3 (700 W power limit), KITTI shape, 2048 images: 5.42 ms against 8.26 ms for the three
+// kernels; 8 scaled rows per CTA (16-row box) took 6.69 ms.
+// The blur, resample and gradient are exact integer arithmetic, so the records and lists are those of the three kernels,
+// byte for byte.  Which states can use it: lsd_pre_fused_fits (5 or 7 u8 taps, every footprint inside the box).
+#define LSD_PF_TH 16         // scaled rows per CTA
+#define LSD_PF_THREADS 256   // 8 warps: the gradient takes rows wrp, wrp + 8
+#define LSD_PF_BOXW 544      // TMA box width, bytes (34 blocks of 16)
+#define LSD_PF_BOXH 24       // TMA box rows
+#define LSD_PF_HW 528        // blurred columns a CTA can produce (132 groups of 4: the row pass reads < LSD_PF_BOXW)
+#define LSD_PF_SP 528        // row pitch of the staged scaled tile (>= LSD_SEG + 4)
+static_assert(LSD_PF_HW % 4 == 0 && 4 * (LSD_PF_HW / 4 - 1) + 12 <= LSD_PF_BOXW, "row pass: a group reads 12 bytes");
+static_assert(LSD_PF_BOXW % 16 == 0 && LSD_PF_BOXW / 16 <= 256, "box: 16-byte blocks, at most 256 of them");
+static_assert((LSD_PF_TH + 1) * LSD_PF_SP <= LSD_PF_BOXH * LSD_PF_HW * 2, "the scaled tile reuses the u16 row-pass tile");
+
+// The source footprint of one CTA, from the resample tables (ox / oy non-decreasing): blurred columns [bxc, sx1] and rows
+// [sy0, sy1]; the box starts at column bxc - R (on a 16-byte boundary) and row sy0 - R.
+struct LsdPfFoot { int bxc, sx1, sy0, sy1; };
+__host__ __device__ __forceinline__ LsdPfFoot lsd_pf_foot(const int* ox, const int* oy, int W, int H, int xb, int yb, int R) {
+  const int X0 = xb * LSD_SEG, Xl = min(X0 + LSD_SEG, W - 1);
+  const int Y0 = yb * LSD_PF_TH, Yl = min(Y0 + LSD_PF_TH, H - 1);
+  LsdPfFoot f;
+  f.bxc = ((ox[X0] - R) & ~15) + R;   // floor to a 16-byte boundary (two's complement: also below column 0)
+  f.sx1 = ox[Xl] + 1;
+  f.sy0 = oy[Y0];
+  f.sy1 = oy[Yl] + 1;
+  return f;
+}
+
+// tabx = [ox(W) | cx(W)], taby = [oy(H) | cy(H)] (plf_linear_coeffs_host), tabxp = the packed x table of k_resize_exact4
+// (plf_resize_pack_x); pix / list / segcnt / maxmag2 as k_lsd_grad.
+template <int KS>
+__global__ void __launch_bounds__(LSD_PF_THREADS, 5) k_lsd_pre_fused(const __grid_constant__ CUtensorMap tmap, int w, int h, int W, int H,
+                                                                  uint32_t tapsA, uint32_t tapsB, const int* __restrict__ tabx,
+                                                                  const int4* __restrict__ tabxp, const int* __restrict__ taby,
+                                                                  const float* __restrict__ lut_angle,
+                                                                  int m2_min, size_t stride, LsdPix* __restrict__ pix, size_t pix_stride,
+                                                                  uint32_t* __restrict__ list, int* __restrict__ segcnt, int nxb,
+                                                                  int* __restrict__ maxmag2) {
+  constexpr int R = KS / 2;
+  constexpr int BP = LSD_PF_BOXW;
+  __shared__ __align__(128) uint8_t raw[LSD_PF_BOXH][BP];       // the box; then the blurred tile (pitch BP)
+  __shared__ __align__(16) uint16_t hrow[LSD_PF_BOXH][LSD_PF_HW]; // row-pass sums; then the scaled tile (pitch LSD_PF_SP)
+  __shared__ __align__(8) uint64_t bar;
+  __shared__ int s_max[LSD_PF_THREADS / 32];
+  uint8_t* blur = &raw[0][0];
+  uint8_t* sc = reinterpret_cast<uint8_t*>(&hrow[0][0]);
+  const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
+  const int xb = blockIdx.x, im = blockIdx.z;
+  const int X0 = xb * LSD_SEG, Y0 = blockIdx.y * LSD_PF_TH;
+  const LsdPfFoot f = lsd_pf_foot(tabx, taby, W, H, xb, blockIdx.y, R);
+  const int gx0 = f.bxc - R, gy0 = f.sy0 - R;   // source pixel of raw[0][0]
+  if (tid == 0) plf_mbar_init(&bar);
+  __syncthreads();
+  if (tid == 0) {
+    const uint32_t b = plf_smem_u32(&bar);
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(b), "r"(LSD_PF_BOXH * BP) : "memory");
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];" ::"r"(
+            plf_smem_u32(&raw[0][0])),
+        "l"(&tmap), "r"(0), "r"(gx0 >> 4), "r"(gy0), "r"(im), "r"(b)
+        : "memory");
+  }
+  const int ncol = f.sx1 - f.bxc + 1, nrow = f.sy1 - f.sy0 + 1;   // blurred tile: nrow x ncol
+  const int need_w = ncol + 2 * R, need_h = nrow + 2 * R;        // box cells the blur reads
+  plf_mbar_wait(&bar, 0);
+  // BORDER_REFLECT_101: the cells outside the image among those read, from their mirror pixel (inside this box: the
+  // footprint reaches at most R + 15 columns / R rows past an edge).  In-image rows first, then whole rows.  Cells past the
+  // image's last column hold the pitch padding or zeros; rows outside it zeros.
+  if (gx0 < 0 || gx0 + need_w > w || gy0 < 0 || gy0 + need_h > h) {
+    const int ry_lo = max(0, -gy0), ry_hi = min(need_h, h - gy0);
+    const int nl = min(need_w, max(0, -gx0)), rx_r = max(0, w - gx0), nr = max(0, need_w - rx_r);
+    if (nl + nr > 0)
+      for (int i = tid; i < (ry_hi - ry_lo) * (nl + nr); i += LSD_PF_THREADS) {
+        const int k = i / (nl + nr), j = i - k * (nl + nr);
+        const int rx = j < nl ? j : rx_r + (j - nl);
+        raw[ry_lo + k][rx] = raw[ry_lo + k][plf_reflect101(gx0 + rx, w) - gx0];
+      }
+    __syncthreads();
+    const int nw = (need_w + 3) >> 2;
+    for (int i = tid; i < (ry_lo + need_h - ry_hi) * nw; i += LSD_PF_THREADS) {
+      const int k = i / nw, j = i - k * nw;
+      const int ry = k < ry_lo ? k : ry_hi + (k - ry_lo);
+      const int m = plf_reflect101(gy0 + ry, h) - gy0;
+      reinterpret_cast<uint32_t*>(raw[ry])[j] = reinterpret_cast<const uint32_t*>(raw[m])[j];
+    }
+  }
+  __syncthreads();
+  // row pass: 4 adjacent sums of a row per group, k_blur_q8_fast's PRMT + DP4A (sum of column c: box columns c .. c + 2R)
+  const int ngrp = (ncol + 3) >> 2;
+  for (int ry = wrp; ry < need_h; ry += LSD_PF_THREADS / 32)
+    for (int j = lane; j < ngrp; j += 32) {
+      const uint32_t* wp = reinterpret_cast<const uint32_t*>(&raw[ry][4 * j]);
+      const uint32_t w0 = wp[0], w1 = wp[1], w2 = wp[2];
+      uint32_t o[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const uint32_t lo = __byte_perm(w0, w1, 0x3210 + 0x1111 * i);
+        const uint32_t hi = __byte_perm(w1, w2, 0x3210 + 0x1111 * i);
+        o[i] = __dp4a(hi, tapsB, __dp4a(lo, tapsA, 0u));
+      }
+      *reinterpret_cast<uint2*>(&hrow[ry][4 * j]) = make_uint2(o[0] | (o[1] << 16), o[2] | (o[3] << 16));
+    }
+  __syncthreads();
+  // column pass: one column per thread, the taps in registers, one rounding (the box is dead: the blurred tile replaces it)
+  {
+    uint32_t t[KS];
+#pragma unroll
+    for (int k = 0; k < KS; ++k) t[k] = k < 4 ? ((tapsA >> (8 * k)) & 0xFFu) : ((tapsB >> (8 * (k - 4))) & 0xFFu);
+    for (int c = tid; c < ncol; c += LSD_PF_THREADS) {
+      uint32_t v[LSD_PF_BOXH];
+#pragma unroll
+      for (int k = 0; k < LSD_PF_BOXH; ++k) v[k] = hrow[k][c];
+#pragma unroll
+      for (int r = 0; r < LSD_PF_BOXH - 2 * R; ++r)
+        if (r < nrow) {
+          uint32_t a = 0;
+#pragma unroll
+          for (int k = 0; k < KS; ++k) a += t[k] * v[r + k];
+          const uint32_t o = (a + (1u << 15)) >> 16;
+          blur[r * BP + c] = (uint8_t)(o > 255 ? 255 : o);
+        }
+    }
+  }
+  __syncthreads();
+  // resample: scaled rows Y0 .. Y0 + LSD_PF_TH and columns X0 .. X0 + LSD_SEG that exist (the u16 tile is dead).
+  // k_resize_exact4's form: four adjacent columns per thread from three words per blurred row (the four read at most 8
+  // blurred columns: the box's rows admit no scale below 0.8), each output's byte pair by one PRMT, the horizontal blend by one IDP.2A on the packed
+  // weight pair; thread = (4-column group tid % 128, row parity tid / 128).  Column LSD_SEG (the right neighbour of the
+  // segment's last column) alone by the scalar form.
+  const int nsc = min(LSD_SEG + 1, W - X0), nsr = min(LSD_PF_TH + 1, H - Y0);
+  {
+    const int g = tid & 127, x = X0 + 4 * g;
+    if (x < W) {
+      const int4 t0 = __ldg(&tabxp[2 * (x >> 2)]), t1 = __ldg(&tabxp[2 * (x >> 2) + 1]);
+      const int ox0 = t0.x - f.bxc, mis = ox0 & 3, s8 = 8 * mis;
+      const int ofs[4] = {t0.x, t0.z, t1.x, t1.z};
+      const uint32_t wx[4] = {(uint32_t)t0.y, (uint32_t)t0.w, (uint32_t)t1.y, (uint32_t)t1.w};
+      for (int r = tid >> 7; r < nsr; r += 2) {
+        const int oy = __ldg(&taby[Y0 + r]) - f.sy0, cy = __ldg(&taby[H + Y0 + r]);
+        const uint32_t* pa = reinterpret_cast<const uint32_t*>(blur + oy * BP + ox0 - mis);
+        const uint32_t* pb = pa + BP / 4;
+        const uint32_t alo = __funnelshift_r(pa[0], pa[1], s8), ahi = __funnelshift_r(pa[1], pa[2], s8);
+        const uint32_t blo = __funnelshift_r(pb[0], pb[1], s8), bhi = __funnelshift_r(pb[1], pb[2], s8);
+        const uint32_t wy0 = (uint32_t)(256 - cy), wy1 = (uint32_t)cy;
+        uint32_t v[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const uint32_t sel = (uint32_t)(ofs[i] - ofs[0]) * 0x11u + 0x10u;
+          const uint32_t h0 = __dp2a_lo(wx[i], __byte_perm(alo, ahi, sel), 0u);
+          const uint32_t h1 = __dp2a_lo(wx[i], __byte_perm(blo, bhi, sel), 0u);
+          v[i] = (h0 * wy0 + h1 * wy1 + 32768u) >> 16;
+        }
+        *reinterpret_cast<uint32_t*>(sc + r * LSD_PF_SP + 4 * g) = (v[0] | (v[1] << 8)) | ((v[2] | (v[3] << 8)) << 16);
+      }
+    }
+    if (nsc > LSD_SEG && tid < nsr) {
+      const int r = tid, u = LSD_SEG;
+      const int ox = __ldg(&tabx[X0 + u]) - f.bxc, cx = __ldg(&tabx[W + X0 + u]);
+      const int oy = __ldg(&taby[Y0 + r]) - f.sy0, cy = __ldg(&taby[H + Y0 + r]);
+      const uint8_t* b0 = blur + oy * BP + ox;
+      const uint32_t h0 = (uint32_t)b0[0] * (uint32_t)(256 - cx) + (uint32_t)b0[1] * (uint32_t)cx;
+      const uint32_t h1 = (uint32_t)b0[BP] * (uint32_t)(256 - cx) + (uint32_t)b0[BP + 1] * (uint32_t)cx;
+      sc[r * LSD_PF_SP + u] = (uint8_t)((h0 * (uint32_t)(256 - cy) + h1 * (uint32_t)cy + 32768u) >> 16);
+    }
+  }
+  __syncthreads();
+  // gradient: warp wrp takes scaled rows y = Y0 + t, t = wrp, wrp + 8 (cells of the tile outside the image are never read
+  // into a defined pixel)
+  int mag2 = -1;
+  for (int t = wrp; t < LSD_PF_TH && Y0 + t < H; t += LSD_PF_THREADS / 32) {
+    const int y = Y0 + t;
+    const uint32_t* s0 = reinterpret_cast<const uint32_t*>(sc + t * LSD_PF_SP);
+    const uint32_t* s1 = reinterpret_cast<const uint32_t*>(sc + (t + 1) * LSD_PF_SP);
+    const bool rok = y < H - 1;
+    LsdPix* prow = pix + (size_t)im * pix_stride + (size_t)y * W + X0;
+    uint32_t* lrow = list + (size_t)im * stride + (size_t)y * W + X0;
+    int base = 0;   // entries of the row segment so far (chunks in x order)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int wi = 32 * k + lane, x4 = X0 + 4 * wi;
+      const uint32_t a0 = s0[wi], a1 = s0[wi + 1], c0 = s1[wi], c1 = s1[wi + 1];
+      int li[4], m2v[4];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        li[c] = -1; m2v[c] = 0;
+        // pixel (x, y): A = (x, y), B = (x+1, y), C = (x, y+1), D = (x+1, y+1)
+        const int A = (a0 >> (8 * c)) & 0xFF, C = (c0 >> (8 * c)) & 0xFF;
+        const int B = c < 3 ? (int)((a0 >> (8 * c + 8)) & 0xFF) : (int)(a1 & 0xFF);
+        const int D = c < 3 ? (int)((c0 >> (8 * c + 8)) & 0xFF) : (int)(c1 & 0xFF);
+        if (rok && x4 + c < W - 1) {
+          const int DA = D - A, BC = B - C, gx = DA + BC, gy = DA - BC, m2 = gx * gx + gy * gy;
+          if (m2 >= m2_min) { li[c] = (gx + 510) * LSD_LUT_DIM + (gy + 510); m2v[c] = m2; mag2 = max(mag2, m2); }
+        }
+      }
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        if (li[c] >= 0)
+          *reinterpret_cast<uint2*>(&prow[4 * wi + c]) = make_uint2(__float_as_uint(__ldg(&lut_angle[li[c]])), (uint32_t)li[c]);
+      // ordered compaction: one warp scan per chunk
+      const int cnt = (li[0] >= 0) + (li[1] >= 0) + (li[2] >= 0) + (li[3] >= 0);
+      int incl = cnt;
+#pragma unroll
+      for (int off = 1; off < 32; off <<= 1) {
+        const int v = __shfl_up_sync(0xFFFFFFFFu, incl, off);
+        if (lane >= off) incl += v;
+      }
+      int o = base + incl - cnt;
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        if (li[c] >= 0) lrow[o++] = (uint32_t)(4 * wi + c) | ((uint32_t)m2v[c] << LSD_COL_BITS);
+      base += __shfl_sync(0xFFFFFFFFu, incl, 31);
+    }
+    if (lane == 0) segcnt[(size_t)im * ((size_t)H * nxb) + (size_t)y * nxb + xb] = base;
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) mag2 = max(mag2, __shfl_xor_sync(0xFFFFFFFFu, mag2, off));
+  if (lane == 0) s_max[wrp] = mag2;
+  __syncthreads();
+  if (tid == 0) {
+    int m = s_max[0];
+#pragma unroll
+    for (int k = 1; k < LSD_PF_THREADS / 32; ++k) m = max(m, s_max[k]);
+    if (m >= 0 && m > __ldcg(&maxmag2[im])) atomicMax(&maxmag2[im], m);
   }
 }
 
@@ -1175,6 +1417,44 @@ static void gaussian_taps_q8(int ksize, double sigma, int* taps) {
   taps[ksize / 2] = 256 - 2 * s;
 }
 
+// The Gaussian pre-blur of scale != 1: its size (0 at scale 1), Q8 taps, and whether every tap is <= 255.
+static void lsd_blur_taps(const plf_params& P, int* ksize, int* taps, bool* taps_u8) {
+  *ksize = 0;
+  *taps_u8 = false;
+  if (P.lsd_scale == 1.0) return;
+  const double scale = P.lsd_scale;
+  const double sigma = (scale < 1) ? (P.lsd_sigma_scale / scale) : P.lsd_sigma_scale;
+  const unsigned hk = (unsigned)(ceil(sigma * sqrt(2 * 3.0 * log(10.0))));
+  *ksize = 1 + 2 * (int)hk;
+  if (*ksize > 15) return;
+  gaussian_taps_q8(*ksize, sigma, taps);
+  *taps_u8 = true;
+  for (int k = 0; k < *ksize; ++k) *taps_u8 = *taps_u8 && taps[k] <= 255;
+}
+
+// Whether k_lsd_pre_fused runs for a w x h image resampled to ws x hs: 5 or 7 taps <= 255 (its DP4A row pass), and the
+// footprint of every CTA inside the box (every scale from 1 up at 7 taps, and from 0.9 or so at 5; below, the three kernels run).
+static bool lsd_pre_fused_fits(const plf_params& P, int w, int h, int ws, int hs) {
+  int ksize, taps[16];
+  bool u8;
+  lsd_blur_taps(P, &ksize, taps, &u8);
+  if (!((ksize == 5 || ksize == 7) && u8) || ws < 2 || hs < 2) return false;
+  const int R = ksize / 2;
+  std::vector<int> tx(2 * (size_t)ws), ty(2 * (size_t)hs);
+  plf_linear_coeffs_host(w, ws, 1.0 / P.lsd_scale, &tx[0], &tx[ws]);
+  plf_linear_coeffs_host(h, hs, 1.0 / P.lsd_scale, &ty[0], &ty[hs]);
+  const int nxb = (ws + LSD_SEG - 1) / LSD_SEG, nyb = (hs + LSD_PF_TH - 1) / LSD_PF_TH;
+  for (int xb = 0; xb < nxb; ++xb) {
+    const LsdPfFoot f = lsd_pf_foot(tx.data(), ty.data(), ws, hs, xb, 0, R);
+    if (f.sx1 - f.bxc + 1 > LSD_PF_HW) return false;
+  }
+  for (int yb = 0; yb < nyb; ++yb) {
+    const LsdPfFoot f = lsd_pf_foot(tx.data(), ty.data(), ws, hs, 0, yb, R);
+    if (f.sy1 - f.sy0 + 1 + 2 * R > LSD_PF_BOXH) return false;
+  }
+  return true;
+}
+
 // The sizes an LSD state for nimg images of w x h takes from the context's parameters and limits.
 static void lsd_set_sizes(const plf_ctx* ctx, LsdState* s, int w, int h, int nimg, bool two_parities) {
   s->w = w; s->h = h; s->nimg = nimg;
@@ -1185,6 +1465,8 @@ static void lsd_set_sizes(const plf_ctx* ctx, LsdState* s, int w, int h, int nim
   s->hs = s->scale != 1.0 ? (int)nearbyint(h * s->scale) : h;
   s->max_regions = ctx->limits.max_segments;
   s->max_lines = ctx->limits.max_lines;
+  s->fused = s->scale != 1.0 && lsd_pre_fused_fits(ctx->params, w, h, s->ws, s->hs);
+  s->chain_maps = s->scale != 1.0 && !s->fused;
 }
 
 // Records of one record map: nimg images of pix_stride records, plus 3 rows + 8 records of slack on both sides (the
@@ -1198,8 +1480,11 @@ static void lsd_buffers(LsdState* s, DevBufList& b) {
   s->bp = plf_pitch16(s->w); s->sp = plf_pitch16(s->ws);
   s->nxb = (s->ws + LSD_SEG - 1) / LSD_SEG;
   s->pix_stride = As + (size_t)s->ws + 1;
-  b.add(s->blur, (size_t)s->bp * s->h * N);
-  b.add(s->scaled, (size_t)s->sp * s->hs * N);
+  // the hand-off maps of the three-kernel chain: listed for every state, empty where the chain does not run, so that the
+  // states of several image sizes list the same entries and share the largest (DevBufList::grow / lend); a size that runs
+  // fused borrows the maps another size needs and never touches them
+  b.add(s->blur, s->chain_maps ? (size_t)s->bp * s->h * N : 0);
+  b.add(s->scaled, s->chain_maps ? (size_t)s->sp * s->hs * N : 0);
   b.add(s->seedlist, As * N);
   b.add(s->segcnt, N * s->hs * s->nxb);
   b.add(s->rect_perm, N * R);
@@ -1248,16 +1533,8 @@ static plf_status lsd_tables_build(plf_ctx* ctx, LsdTables* t) {
   t->prec = LSD_PI * P.lsd_ang_th / 180;
   t->p = P.lsd_ang_th / 180;
   t->rho = P.lsd_quant / sin(t->prec);
-  const double scale = P.lsd_scale;
-  if (scale != 1.0) {
-    const double sigma = (scale < 1) ? (P.lsd_sigma_scale / scale) : P.lsd_sigma_scale;
-    const unsigned hk = (unsigned)(ceil(sigma * sqrt(2 * 3.0 * log(10.0))));
-    t->ksize = 1 + 2 * (int)hk;
-    if (t->ksize > 15) return plf_fail(ctx, PLF_ERR_INVALID, "LSD: Gaussian kernel %d > 15 unsupported", t->ksize);
-    gaussian_taps_q8(t->ksize, sigma, t->taps.k);
-    t->taps_u8 = true;
-    for (int k = 0; k < t->ksize; ++k) t->taps_u8 = t->taps_u8 && t->taps.k[k] <= 255;
-  }
+  lsd_blur_taps(P, &t->ksize, t->taps.k, &t->taps_u8);
+  if (t->ksize > 15) return plf_fail(ctx, PLF_ERR_INVALID, "LSD: Gaussian kernel %d > 15 unsupported", t->ksize);
   for (t->m2_min = 0; t->m2_min <= 2 * 510 * 510; ++t->m2_min)  // same double expression as the kernels
     if (!(sqrt((double)t->m2_min / 4.0) <= t->rho)) break;
   const size_t LUT = (size_t)LSD_LUT_DIM * LSD_LUT_DIM;
@@ -1294,8 +1571,10 @@ void plf_lsd_tables_free(plf_ctx* ctx) {
 }
 
 // The sizes of s for nimg images of w x h, checked, and its buffers listed (not allocated).  Host only.
-static plf_status lsd_layout(plf_ctx* ctx, LsdState* s, int w, int h, int nimg, bool two_parities) {
+// chain_maps: also the maps of the three-kernel chain where the fused kernel runs (a test state that runs both).
+static plf_status lsd_layout(plf_ctx* ctx, LsdState* s, int w, int h, int nimg, bool two_parities, bool chain_maps = false) {
   lsd_set_sizes(ctx, s, w, h, nimg, two_parities);
+  s->chain_maps = s->chain_maps || (chain_maps && s->scale != 1.0);
   if (s->ws >= 65536 || s->hs >= 65536 || s->ws < 3 || s->hs < 3)
     return plf_fail(ctx, PLF_ERR_INVALID, "LSD: scaled image %dx%d out of range", s->ws, s->hs);
   lsd_buffers(s, s->bufs);
@@ -1330,14 +1609,14 @@ static plf_status lsd_ready(plf_ctx* ctx, LsdState* s) {
 // The states of n image sizes share one set of buffers, each sized for the largest of them.  Every record map is filled
 // with NOTDEF whole, guards and slack of every size's layout included; k_lsd_fill_notdef says why it stays so whichever
 // size the next batch has (DESIGN.md section 8).
-plf_status plf_lsd_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities, LsdState** out) {
+static plf_status lsd_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities, bool chain_maps, LsdState** out) {
   plf_status st = plf_lsd_tables(ctx);
   if (st) return st;
   std::vector<LsdState*> v(n, nullptr);
   size_t records = 0;
   for (int i = 0; i < n && !st; ++i) {
     v[i] = new LsdState();
-    st = lsd_layout(ctx, v[i], wh[2 * i], wh[2 * i + 1], nimg, two_parities);
+    st = lsd_layout(ctx, v[i], wh[2 * i], wh[2 * i + 1], nimg, two_parities, chain_maps);
     if (!st) records = std::max(records, lsd_pix_records(v[i]));
   }
   if (!st) {
@@ -1363,23 +1642,67 @@ plf_status plf_lsd_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg, bo
   return PLF_OK;
 }
 
+plf_status plf_lsd_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities, LsdState** out) {
+  return lsd_create_sizes(ctx, n, wh, nimg, two_parities, false, out);
+}
+
 plf_status plf_lsd_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, LsdState** out) {
   const int wh[2] = {w, h};
   return plf_lsd_create_sizes(ctx, 1, wh, nimg, two_parities, out);
 }
 
-// LSD on images [0, n) of a batch resident on the device, in two phases so that callers can overlap them with other
-// work: `pre` = blur, resample, gradient and seed ordering (bandwidth-bound), `grow` = region growing, rectangle fit and
-// the KeyLine stage (latency-bound).  `par` selects the buffer set that carries data from pre to grow.  The state must
-// hold >= n images.  Enqueued on cs; results stay on the device.
-plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int par, int n) {
-  if (s->nimg < n) return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_pre: %d images > the state's %d", n, s->nimg);
+// Tensor map of k_lsd_pre_fused over nimg source images: a row is viewed as 16-byte blocks, {16, blocks, rows, images},
+// so that one box spans LSD_PF_BOXW bytes of a row.  Encoded per call (host only, a few microseconds per batch).
+static bool lsd_pf_encode(CUtensorMap* map, const void* base, int w, int h, int nimg, size_t pitch, size_t img_stride) {
+  typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  static encode_fn fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess || !p) return false;
+    fn = (encode_fn)p;
+  }
+  if ((pitch & 15) || (img_stride & 15) || ((uintptr_t)base & 15) || (size_t)w > pitch) return false;
+  const cuuint64_t dims[4] = {16u, (cuuint64_t)((w + 15) / 16), (cuuint64_t)h, (cuuint64_t)nimg};
+  const cuuint64_t strides[3] = {16u, (cuuint64_t)pitch, (cuuint64_t)img_stride};
+  const cuuint32_t box[4] = {16u, (cuuint32_t)(LSD_PF_BOXW / 16), (cuuint32_t)LSD_PF_BOXH, 1u};
+  const cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
+  return fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// The records, seed lists, segcnt and maxmag2 of images [0, n) into record map `pix`: by k_lsd_pre_fused (fused, which
+// the state must allow: s->fused) or by the pre-blur, resample and gradient kernels (s->chain_maps, or scale 1: the
+// gradient alone).
+static plf_status lsd_pre_grad(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch,
+                               LsdPix* pix, int n, bool fused) {
   const LsdTables& T = *ctx->lsd_tables;
   const int w = s->w, h = s->h;
   const int W = s->ws, H = s->hs;
   const size_t As = (size_t)W * H, A = (size_t)s->bp * h, Asp = (size_t)s->sp * H;
-  LsdPix* pix = s->pix[par] + (s->ws + 1);  // pixel (0,0) of the first image
-  plf_status st;
+  PLF_CUDA(ctx, cudaMemsetAsync(s->maxmag2, 0xFF, (size_t)n * sizeof(int), cs));  // -1
+  uint32_t tA = 0, tB = 0;
+  for (int k = 0; k < T.ksize; ++k) (k < 4 ? tA : tB) |= (uint32_t)T.taps.k[k] << (8 * (k & 3));
+  if (fused) {
+    CUtensorMap tm;
+    if (!lsd_pf_encode(&tm, d_imgs, w, h, n, pitch, img_stride))
+      return plf_fail(ctx, PLF_ERR_CUDA, "LSD: cuTensorMapEncodeTiled failed for the source images (pitch %d, stride %zu)", pitch, img_stride);
+    const dim3 g(s->nxb, (H + LSD_PF_TH - 1) / LSD_PF_TH, n);
+    const int* tx = s->rs_tab + s->rs_x_off;
+    const int* ty = s->rs_tab + s->rs_y_off;
+    const int4* txp = reinterpret_cast<const int4*>(s->rs_tab + s->rs_xp_off);
+    if (T.ksize == 7)
+      k_lsd_pre_fused<7><<<g, LSD_PF_THREADS, 0, cs>>>(tm, w, h, W, H, tA, tB, tx, txp, ty, T.angle_lut, T.m2_min, As, pix, s->pix_stride,
+                                                       s->seedlist, s->segcnt, s->nxb, s->maxmag2);
+    else
+      k_lsd_pre_fused<5><<<g, LSD_PF_THREADS, 0, cs>>>(tm, w, h, W, H, tA, tB, tx, txp, ty, T.angle_lut, T.m2_min, As, pix, s->pix_stride,
+                                                       s->seedlist, s->segcnt, s->nxb, s->maxmag2);
+    PLF_LAUNCH_CHECK(ctx);
+    plf_mark(ctx, cs, "lsd.k_lsd_pre_fused");
+    return PLF_OK;
+  }
   const uint8_t* scaled = d_imgs;
   size_t scaled_stride = img_stride;
   int scaled_pitch = pitch;
@@ -1388,8 +1711,6 @@ plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t
       const CUtensorMap* tm = s->tm_blur.get(d_imgs, w, h, n, pitch, img_stride, 80, BF_TH + T.ksize - 1);
       if (!tm)
         return plf_fail(ctx, PLF_ERR_CUDA, "LSD: cuTensorMapEncodeTiled failed for the source images (pitch %d, stride %zu)", pitch, img_stride);
-      uint32_t tA = 0, tB = 0;
-      for (int k = 0; k < T.ksize; ++k) (k < 4 ? tA : tB) |= (uint32_t)T.taps.k[k] << (8 * (k & 3));
       dim3 gf(plf_tma_tiles_x(w, T.ksize / 2), (h + BF_TH - 1) / BF_TH, n);
       if (T.ksize == 7) k_blur_q8_fast<7><<<gf, 256, 0, cs>>>(*tm, 0, w, h, tA, tB, s->blur, A, s->bp);
       else k_blur_q8_fast<5><<<gf, 256, 0, cs>>>(*tm, 0, w, h, tA, tB, s->blur, A, s->bp);
@@ -1399,18 +1720,32 @@ plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t
     }
     PLF_LAUNCH_CHECK(ctx);
     plf_mark(ctx, cs, "lsd.k_blur_q8");
-    st = plf_launch_resize_exact(ctx, cs, s->blur, A, s->bp, w, h, s->scaled, Asp, s->sp, W, H, s->rs_tab + s->rs_x_off, s->rs_tab + s->rs_xp_off, s->rs_tab + s->rs_y_off, n);
+    const plf_status st = plf_launch_resize_exact(ctx, cs, s->blur, A, s->bp, w, h, s->scaled, Asp, s->sp, W, H, s->rs_tab + s->rs_x_off,
+                                                  s->rs_tab + s->rs_xp_off, s->rs_tab + s->rs_y_off, n);
     if (st) return st;
     plf_mark(ctx, cs, "lsd.k_resize_exact");
     scaled = s->scaled;
     scaled_stride = Asp;
     scaled_pitch = s->sp;
   }
-  PLF_CUDA(ctx, cudaMemsetAsync(s->maxmag2, 0xFF, (size_t)n * sizeof(int), cs));  // -1
   k_lsd_grad<<<dim3(s->nxb, (H + 1) / 2, n), LSD_GRAD_THREADS, 0, cs>>>(scaled, scaled_stride, scaled_pitch, W, H, T.angle_lut, T.m2_min, As, pix, s->pix_stride,
                                                                s->seedlist, s->segcnt, s->nxb, s->maxmag2);
   PLF_LAUNCH_CHECK(ctx);
   plf_mark(ctx, cs, "lsd.k_lsd_grad");
+  return PLF_OK;
+}
+
+// LSD on images [0, n) of a batch resident on the device, in two phases so that callers can overlap them with other
+// work: `pre` = blur, resample, gradient and seed ordering (bandwidth-bound), `grow` = region growing, rectangle fit and
+// the KeyLine stage (latency-bound).  `par` selects the buffer set that carries data from pre to grow.  The state must
+// hold >= n images.  Enqueued on cs; results stay on the device.
+plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int par, int n) {
+  if (s->nimg < n) return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_pre: %d images > the state's %d", n, s->nimg);
+  const int W = s->ws, H = s->hs;
+  const size_t As = (size_t)W * H;
+  LsdPix* pix = s->pix[par] + (s->ws + 1);  // pixel (0,0) of the first image
+  const plf_status st = lsd_pre_grad(ctx, cs, s, d_imgs, img_stride, pitch, pix, n, s->fused);
+  if (st) return st;
   k_lsd_seed_order<<<n, LSD_SO_THREADS, lsd_seed_order_smem(s->n_bins), cs>>>(s->seedlist, s->segcnt, As, W, H, s->nxb, s->n_bins,
                                                                               s->maxmag2, s->order[par], s->nseeds[par]);
   PLF_LAUNCH_CHECK(ctx);
@@ -1621,6 +1956,49 @@ extern "C" plf_status plf_debug_sincosf(plf_ctx* ctx, const float* in, float* s,
   PLF_CUDA(ctx, cudaMemcpyAsync(c, dc, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return PLF_OK;
+}
+
+// The gradient stage of LSD (records, seed lists, segcnt, maxmag2) of n source images, by k_lsd_pre_fused (fused = 1) or
+// by the pre-blur, resample and gradient kernels (fused = 0), in a state of its own: tests compare the two byte for byte.
+extern "C" plf_status plf_debug_lsd_pre(plf_ctx* ctx, const uint8_t* imgs, int n, int w, int h, int pitch, size_t img_stride,
+                                        int fused, int* sizes, uint32_t* pix, uint32_t* seedlist, int* segcnt, int* maxmag2) {
+  if (!ctx || n < 1 || w < 3 || h < 3 || pitch < w || (pitch & 15) || img_stride < (size_t)pitch * h || (img_stride & 15) || !sizes)
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_debug_lsd_pre: bad arguments");
+  PLF_CUDA(ctx, cudaSetDevice(ctx->device));
+  LsdState* s = nullptr;
+  const int wh[2] = {w, h};
+  plf_status st = lsd_create_sizes(ctx, 1, wh, n, false, true, &s);
+  if (st) return st;
+  sizes[0] = s->ws; sizes[1] = s->hs; sizes[2] = s->nxb; sizes[3] = s->fused;
+  if (!imgs || !pix || !seedlist || !segcnt || !maxmag2) {   // sizes only
+    plf_lsd_free(s);
+    return PLF_OK;
+  }
+  if (fused && !s->fused) {
+    plf_lsd_free(s);
+    return plf_fail(ctx, PLF_ERR_INVALID, "plf_debug_lsd_pre: the fused kernel does not apply to %dx%d at these parameters", w, h);
+  }
+  const size_t As = (size_t)s->ws * s->hs, nseg = (size_t)n * s->hs * s->nxb;
+  uint8_t* dimg = nullptr;
+  DevBufList ib;
+  ib.add(dimg, (size_t)n * img_stride);
+  st = ib.alloc(ctx, "plf_debug_lsd_pre");
+  if (!st && (cudaMemcpyAsync(dimg, imgs, (size_t)n * img_stride, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
+              cudaMemsetAsync(s->seedlist, 0, As * n * sizeof(uint32_t), ctx->stream) != cudaSuccess ||
+              cudaMemsetAsync(s->segcnt, 0, nseg * sizeof(int), ctx->stream) != cudaSuccess))
+    st = plf_fail(ctx, PLF_ERR_CUDA, "plf_debug_lsd_pre: upload failed");
+  if (!st) st = lsd_pre_grad(ctx, ctx->stream, s, dimg, img_stride, pitch, s->pix[0] + (s->ws + 1), n, fused != 0);
+  if (!st && (cudaMemcpy2DAsync(pix, As * sizeof(LsdPix), s->pix[0] + (s->ws + 1), s->pix_stride * sizeof(LsdPix), As * sizeof(LsdPix), n,
+                                cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
+              cudaMemcpyAsync(seedlist, s->seedlist, As * n * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
+              cudaMemcpyAsync(segcnt, s->segcnt, nseg * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
+              cudaMemcpyAsync(maxmag2, s->maxmag2, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
+              cudaStreamSynchronize(ctx->stream) != cudaSuccess))
+    st = plf_fail(ctx, PLF_ERR_CUDA, "plf_debug_lsd_pre: %s", cudaGetErrorString(cudaGetLastError()));
+  cudaStreamSynchronize(ctx->stream);
+  ib.release();
+  plf_lsd_free(s);
+  return st;
 }
 
 // The region-growing kernel stays resident for tens of milliseconds while the next batch's extraction kernels are

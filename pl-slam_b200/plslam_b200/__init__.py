@@ -1228,6 +1228,38 @@ class Frontend:
         self._check(st, "plf_debug_sincosf")
         return s, c
 
+    def debug_lsd_pre(self, imgs, fused, pitch=None, img_stride=None, pad_byte=0xA5):
+        """LSD's gradient stage on the (n, h, w) uint8 images, by the fused pre-blur + resample + gradient kernel
+        (fused=True) or by the three kernels it replaces.  The images are laid out with row pitch `pitch` and image
+        stride `img_stride` bytes (multiples of 16; default: the pipeline's) and the padding filled with pad_byte.
+        Returns dict(pix=(n, hs*ws) uint64 records, seedlist=(n, hs*ws) uint32, segcnt=(n, hs, nxb) int32,
+        maxmag2=(n,) int32, fused_applies=bool); fused_applies alone (no run) when fused is None."""
+        imgs = np.ascontiguousarray(imgs, np.uint8)
+        n, h, w = imgs.shape
+        pitch = pitch or (w + 15) // 16 * 16
+        img_stride = img_stride or pitch * h
+        sizes = np.zeros(4, np.int32)
+        f = self.lib.plf_debug_lsd_pre
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_int, C.c_void_p,
+                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, None, n, w, h, pitch, img_stride, 0, sizes.ctypes.data, None, None, None, None),
+                    "plf_debug_lsd_pre")
+        ws, hs, nxb, applies = (int(v) for v in sizes)
+        if fused is None:
+            return dict(fused_applies=bool(applies))
+        buf = np.full(n * img_stride, pad_byte, np.uint8)
+        for i in range(n):
+            v = buf[i * img_stride:i * img_stride + pitch * h].reshape(h, pitch)
+            v[:, :w] = imgs[i]
+        pix = np.empty((n, hs * ws), np.uint64)
+        seed = np.empty((n, hs * ws), np.uint32)
+        seg = np.empty((n, hs, nxb), np.int32)
+        mm = np.empty(n, np.int32)
+        st = f(self._ctx, buf.ctypes.data, n, w, h, pitch, img_stride, int(bool(fused)), sizes.ctypes.data, pix.ctypes.data,
+               seed.ctypes.data, seg.ctypes.data, mm.ctypes.data)
+        self._check(st, "plf_debug_lsd_pre")
+        return dict(pix=pix, seedlist=seed, segcnt=seg, maxmag2=mm, fused_applies=bool(applies))
+
     def debug_ldlt(self, S, g, path=0, overwrite_s=False):
         """LDL^T without pivoting of the symmetric S (6 n6 x 6 n6, lower triangle read) and the solution of S x = g, by
         the tiled factorisation of global_ba / pose_graph beyond 64 keyframes, on one system (path 0), or the one-CTA
