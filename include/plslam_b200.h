@@ -305,13 +305,13 @@ plf_status plf_detect_lines_masked(plf_ctx* ctx, const uint8_t* img, int w, int 
 /* Test hook: evaluates the device port of glibc sinf/cosf used by the LSD region-angle update. */
 plf_status plf_debug_sincosf(plf_ctx* ctx, const float* in, float* s, float* c, int n);
 
-/* Test hook: the gradient stage of LSD on n w x h uint8 images (row pitch `pitch`, image stride img_stride bytes, both
- * multiples of 16), by the fused pre-blur + resample + gradient kernel (fused = 1) or by the three kernels it replaces
- * (fused = 0).  sizes[4] receives {ws, hs, nxb, whether the fused kernel applies}; with any output NULL nothing runs.
- * Outputs: pix [n][hs*ws] records as 2 uint32 {angle bits, table index} (untouched pixels read {-1024.f, 0}), seedlist
- * [n][hs*ws] (entries past a segment's count read 0), segcnt [n][hs][nxb], maxmag2 [n].  PLF_ERR_INVALID for fused = 1
- * where the fused kernel does not apply. */
-plf_status plf_debug_lsd_pre(plf_ctx* ctx, const uint8_t* imgs, int n, int w, int h, int pitch, size_t img_stride, int fused,
+/* Test hook: the gradient stage of LSD (pre-blur, resample and gradient in one kernel) on n w x h uint8 images (row pitch
+ * `pitch`, image stride img_stride bytes, both multiples of 16).  sizes[6] receives {ws, hs, nxb, KS, TH, P}: the scaled
+ * size, the 512-column segments per row, and the kernel's launch (pre-blur taps, scaled rows per CTA, column pieces per
+ * segment); with any output NULL nothing runs.  Outputs: pix [n][hs*ws] records as 2 uint32 {angle bits, table index}
+ * (untouched pixels read {-1024.f, 0}), seedlist [n][hs*ws] (entries past a segment's count read 0), segcnt [n][hs][nxb],
+ * maxmag2 [n]. */
+plf_status plf_debug_lsd_pre(plf_ctx* ctx, const uint8_t* imgs, int n, int w, int h, int pitch, size_t img_stride,
                              int* sizes, uint32_t* pix, uint32_t* seedlist, int* segcnt, int* maxmag2);
 
 /* Test hook: factors the symmetric n x n matrix S (n = 6 n6, row-major, only its lower triangle is read) as L D L^T

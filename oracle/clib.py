@@ -221,6 +221,20 @@ def orb(img, nfeatures=800, scale_factor=1.2, nlevels=4, edge_th=19, patch_size=
 
 
 # ---- LSD (oracle/lsd.c) ------------------------------------------------------------------------------
+def lsd_scaled_image(img, scale=1.2, sigma_scale=0.6):
+    """The image flsd takes the gradient of: the Gaussian pre-blur and INTER_LINEAR_EXACT resample (a copy at scale 1)."""
+    img = np.ascontiguousarray(img, np.uint8)
+    f = lib().orc_lsd_scaled_image
+    f.restype = C.c_void_p
+    f.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_void_p, C.c_void_p]
+    ow, oh = C.c_int(), C.c_int()
+    p = f(_p(img), img.shape[1], img.shape[0], scale, sigma_scale, C.byref(ow), C.byref(oh))
+    try:
+        return np.frombuffer((C.c_uint8 * (ow.value * oh.value)).from_address(p), np.uint8).reshape(oh.value, ow.value).copy()
+    finally:
+        C.CDLL(None).free(C.c_void_p(p))
+
+
 def lsd(img, scale=1.2, sigma_scale=0.6, quant=2.0, ang_th=22.5, n_bins=1024, order_mode=0, trig_mode=0, cap=65536):
     img = np.ascontiguousarray(img, np.uint8)
     segs = np.zeros((cap, 4), np.float32)

@@ -14,16 +14,13 @@
 //   k_lsd_build_lut  once per context: the gradient lookup tables (LsdTables)
 //   k_lsd_fill_notdef
 //                    once per state: every record of the record maps set to "undefined"
-//   k_blur_q8_fast   separable Q8.8 Gaussian of 5 or 7 taps <= 255 (tile + halo staged by one TMA bulk-tensor copy, DP4A
-//                    row pass), one rounding (k_blur_q8: generic variant for the other kernels, up to 15 taps)
-//   k_resize_exact4  (orb.cu) INTER_LINEAR_EXACT resample to scale
-//   k_lsd_grad       2x2 gradient; for the DEFINED pixels only (|grad| > rho, ~12 %): the 8-byte record {angle
-//                    (cv::fastAtan2 = plf_fast_atan2, degrees, f32, from a table keyed by (gx,gy)), table index}, and one packed entry
-//                    (column, |grad|^2) of the raster-ordered seed list of the pixel's row segment; per-image max of |grad|^2.
-//                    Nothing dense leaves the kernel (the record map restores itself to "undefined", see k_lsd_fill_notdef)
-//   k_lsd_pre_fused  the three kernels above in one tile kernel, from the source image (one TMA box per CTA) to the records,
-//                    seed lists, segcnt and maxmag2 k_lsd_grad writes, with no blurred or resampled map in between; it runs
-//                    where its footprint fits (5 or 7 u8 taps, the default parameters), the three kernels elsewhere
+//   k_lsd_pre        one tile kernel from the source image to the gradient records: separable Q8.8 Gaussian pre-blur
+//                    (DP4A row pass, one rounding), INTER_LINEAR_EXACT resample to scale, 2x2 gradient, staged by TMA box
+//                    loads with no blurred or resampled map in global memory.  For the DEFINED pixels only (|grad| > rho,
+//                    ~12 %) it writes the 8-byte record {angle (cv::fastAtan2 = plf_fast_atan2, degrees, f32, from a table
+//                    keyed by (gx,gy)), table index} and one packed entry (column, |grad|^2) of the raster-ordered seed list
+//                    of the pixel's row segment; and the per-image max of |grad|^2.  Nothing dense leaves the kernel (the
+//                    record map restores itself to "undefined", see k_lsd_fill_notdef)
 //   k_lsd_seed_order stable counting sort of the seed lists by magnitude bin (descending), raster order inside a
 //                    bin == OpenCV's ordered_points; one CTA per image, bin counts in shared memory
 //   k_lsd_grow       region growing.  The algorithm is a sequential greedy partition (each accepted pixel updates the
@@ -57,14 +54,17 @@
 #define LSD_BINS_MAX 1024
 #define LSD_QCAP 256   // shared-memory window of the region queue (entries)
 
-// The Q8 taps of the Gaussian pre-blur; k_blur_q8 takes them by value (8-byte aligned: read in pairs).
-struct __align__(8) LsdTaps { int k[16]; };
+// The launch of k_lsd_pre for one image size at the context's parameters (lsd_pre_geom): the pre-blur's KS Q8 taps (KS = 1:
+// no blur, at scale 1 or when the centre tap is 256), TH scaled rows per CTA, and each CTA's 512-column row segment cut
+// into NP pieces of PW scaled columns, one TMA box each.
+struct LsdPreGeom {
+  int ks = 1, th = 0, np = 0, pw = 0;
+  bool packed = true;            // the resample takes four scaled columns per thread (plf_resize_packed_ok); else one
+  uint4 taps = {0u, 0u, 0u, 0u}; // tap k in byte k % 4 of word k / 4
+};
 
 // What LSD derives from the context's parameters alone, built once per context and read by every LSD state.
 struct LsdTables {
-  int ksize = 0;            // Gaussian pre-blur (0: scale 1, no blur)
-  LsdTaps taps;
-  bool taps_u8 = false;     // every tap <= 255: the packed-byte fast blur applies (a 256 centre tap at small sigma does not)
   double prec = 0, p = 0, rho = 0;
   int m2_min = 0;           // smallest gx^2+gy^2 whose gradient norm exceeds rho (defined pixel)
   float* angle_lut = nullptr;   // [1021*1021] gradient (gx,gy) -> level-line angle (degrees) of a defined pixel
@@ -81,23 +81,18 @@ struct LsdState {
   int min_reg_size = 0;
   int max_regions = 0, max_lines = 0;
   bool two_parities = false;
-  bool fused = false;         // k_lsd_pre_fused runs (lsd_pre_fused_fits); else blur, resample and gradient as three kernels
-  bool chain_maps = false;    // blur and scaled exist: the three-kernel chain can run (scale != 1 and not fused, or a test state)
-  uint8_t* blur = nullptr;    // [nimg][h][bp]   bp = plf_pitch16(w)
-  uint8_t* scaled = nullptr;  // [nimg][hs][sp]  sp = plf_pitch16(ws)
-  int bp = 0, sp = 0;
-  PlfTmaCache tm_blur;        // source images of k_blur_q8_fast
+  LsdPreGeom pre;             // k_lsd_pre's launch (lsd_pre_geom)
   uint32_t* rect_perm = nullptr;  // [nimg][max_regions] regions in size-class order (k_lsd_rect_order)
   struct LsdPix* pix_raw[2] = {nullptr, nullptr};  // allocation (pix + look-ahead slack on both sides)
   struct LsdPix* pix[2] = {nullptr, nullptr};  // [nimg][guard + hs*ws]  {angle (deg, f32) | NOTDEF = undefined/used, table index}
   size_t pix_stride = 0;      // entries per image = guard (ws+1, permanently NOTDEF) + hs*ws
   // seed lists per row segment (LSD_SEG columns): segment (y, xb) owns the entries [y * ws + LSD_SEG * xb, ...);
-  // an entry is column-in-segment | gx^2+gy^2 << LSD_COL_BITS (k_lsd_grad)
+  // an entry is column-in-segment | gx^2+gy^2 << LSD_COL_BITS (k_lsd_pre)
   uint32_t* seedlist = nullptr; // [nimg][hs*ws]
   int* segcnt = nullptr;        // [nimg][hs][nxb] entries per segment
   int nxb = 0;                  // segments per row
   int* maxmag2 = nullptr;     // [nimg]
-  // per batch parity: what crosses from the pre-grow chain to the growing (pix, order, nseeds) and what the match phase
+  // per batch parity: what crosses from the pre-grow phase to the growing (pix, order, nseeds) and what the match phase
   // reads (kls, nlines).  One copy: what only the growing / rectangle / KeyLine kernels of one batch write and read.
   int* nseeds[2] = {nullptr, nullptr};      // [nimg]
   uint32_t* order[2] = {nullptr, nullptr};  // [nimg][hs*ws]
@@ -115,115 +110,6 @@ struct LsdState {
   DevBufList tabs;   // rs_tab, the state's own
 };
 
-// ---- fixed-point Gaussian (ksize <= 15) ------------------------------------------------------------------
-#define BQ_TW 64
-#define BQ_TH 16
-#define BQ_R 7
-__global__ void __launch_bounds__(256) k_blur_q8(const uint8_t* __restrict__ src, size_t src_stride, int pitch,
-                                                 int w, int h, int r, uint8_t* __restrict__ dst, size_t dst_stride, int dpitch,
-                                                 const __grid_constant__ LsdTaps taps) {
-  __shared__ uint8_t raw[BQ_TH + 2 * BQ_R][BQ_TW + 2 * BQ_R + 2];
-  __shared__ uint16_t hrow[BQ_TH + 2 * BQ_R][BQ_TW];
-  const uint8_t* s = src + (size_t)blockIdx.z * src_stride;
-  uint8_t* d = dst + (size_t)blockIdx.z * dst_stride;
-  const int x0 = blockIdx.x * BQ_TW, y0 = blockIdx.y * BQ_TH, tid = threadIdx.x;
-  const int RW = BQ_TW + 2 * r, RH = BQ_TH + 2 * r;
-  const int lane = tid & 31, wrp = tid >> 5;
-  const bool interior = x0 >= r && x0 + BQ_TW + r <= w && y0 >= r && y0 + BQ_TH + r <= h;
-  for (int ry = wrp; ry < RH; ry += 8) {  // one warp per row, lanes along x
-    const int gy = interior ? y0 - r + ry : plf_reflect101(y0 - r + ry, h);
-    const uint8_t* row = s + (size_t)gy * pitch;
-    for (int rx = lane; rx < RW; rx += 32) raw[ry][rx] = row[interior ? x0 - r + rx : plf_reflect101(x0 - r + rx, w)];
-  }
-  __syncthreads();
-  const int ks = 2 * r + 1;
-  const int tx = tid & (BQ_TW - 1), rg = tid >> 6;  // BQ_TW == 64
-  for (int ry = rg; ry < RH; ry += 4) {
-    uint32_t a = 0;
-    for (int k = 0; k < ks; ++k) a += (uint32_t)taps.k[k] * raw[ry][tx + k];
-    hrow[ry][tx] = (uint16_t)a;
-  }
-  __syncthreads();
-  const int gx = x0 + tx;
-  if (gx < w) {
-    for (int ty = rg; ty < BQ_TH; ty += 4) {
-      const int gy = y0 + ty;
-      if (gy >= h) break;
-      uint32_t a = 0;
-      for (int k = 0; k < ks; ++k) a += (uint32_t)taps.k[k] * hrow[ty + k][tx];
-      const uint32_t v = (a + (1u << 15)) >> 16;
-      d[(size_t)gy * dpitch + gx] = (uint8_t)(v > 255 ? 255 : v);
-    }
-  }
-}
-
-// Fast path for KS <= 8 taps (7x7 at the reference's scale 1.2 / 0.8): 64x32 output tile staged by ONE TMA bulk-tensor
-// copy (plf_tma.cuh; border CTAs rebuild BORDER_REFLECT_101 inside shared memory), DP4A row pass.
-//   row pass : a thread produces 4 adjacent outputs of one row from three aligned 32-bit words of the staged tile;
-//              the KS byte window of each output is assembled with PRMT (byte_perm) and reduced with two DP4As against
-//              the packed u8 taps (taps <= 255, products summed exactly in 32 bits, result < 2^16);
-//   col pass : a thread slides down 8 rows of one column with the KS taps in registers.
-// ~30 thread-instructions per pixel instead of ~200 for the generic kernel; bit-identical results.
-#define BF_TW 64
-#define BF_TH 32
-template <int KS>
-__global__ void __launch_bounds__(256) k_blur_q8_fast(const __grid_constant__ CUtensorMap tmap, int z0, int w, int h,
-                                                      uint32_t tapsA, uint32_t tapsB, uint8_t* __restrict__ dst,
-                                                      size_t dst_stride, int dpitch) {
-  constexpr int R = KS / 2;
-  constexpr int RH = BF_TH + 2 * R;
-  constexpr int RP = 80;     // TMA box width (bytes, multiple of 16)
-  constexpr int NEED = 72;   // columns the row pass reads (64 outputs + 2R taps, whole 32-bit words)
-  __shared__ __align__(128) uint8_t raw[RH][RP];
-  __shared__ __align__(16) uint16_t hrow[RH][BF_TW];
-  __shared__ __align__(8) uint64_t bar;
-  uint8_t* d = dst + (size_t)blockIdx.z * dst_stride;
-  const int x0 = blockIdx.x * BF_TW - (16 - R), y0 = blockIdx.y * BF_TH, tid = threadIdx.x;   // x0 - R on a 16-byte boundary (TMA)
-  if (tid == 0) plf_mbar_init(&bar);
-  __syncthreads();
-  if (tid == 0) plf_tma_load_3d(&raw[0][0], &tmap, x0 - R, y0 - R, z0 + (int)blockIdx.z, &bar, RH * RP);
-  plf_mbar_wait(&bar, 0);
-  if (!(x0 >= R && x0 - R + NEED <= w && y0 >= R && y0 + BF_TH + R <= h))   // border tile: BORDER_REFLECT_101 in place
-    plf_tma_reflect_fix<RH, RP>(raw, x0 - R, y0 - R, w, h, NEED);
-  __syncthreads();
-  for (int it = tid; it < RH * (BF_TW / 4); it += 256) {
-    const int ry = it >> 4, j = it & 15;  // BF_TW / 4 == 16 groups per row
-    const uint32_t* wp = reinterpret_cast<const uint32_t*>(&raw[ry][4 * j]);
-    const uint32_t w0 = wp[0], w1 = wp[1], w2 = wp[2];
-    uint32_t o[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const uint32_t lo = __byte_perm(w0, w1, 0x3210 + 0x1111 * i);
-      const uint32_t hi = __byte_perm(w1, w2, 0x3210 + 0x1111 * i);
-      o[i] = __dp4a(hi, tapsB, __dp4a(lo, tapsA, 0u));
-    }
-    uint2 pk = make_uint2(o[0] | (o[1] << 16), o[2] | (o[3] << 16));
-    *reinterpret_cast<uint2*>(&hrow[ry][4 * j]) = pk;
-  }
-  __syncthreads();
-  const int c = tid & 63, q = tid >> 6;
-  const int gx = x0 + c;
-  if (gx >= 0 && gx < w) {
-    uint32_t t[KS];
-#pragma unroll
-    for (int k = 0; k < KS; ++k) t[k] = k < 4 ? ((tapsA >> (8 * k)) & 0xFFu) : ((tapsB >> (8 * (k - 4))) & 0xFFu);
-    uint32_t v[8 + KS - 1];
-#pragma unroll
-    for (int k = 0; k < 8 + KS - 1; ++k) v[k] = hrow[q * 8 + k][c];
-#pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      const int gy = y0 + q * 8 + r;
-      if (gy < h) {
-        uint32_t a = 0;
-#pragma unroll
-        for (int k = 0; k < KS; ++k) a += t[k] * v[r + k];
-        const uint32_t o = (a + (1u << 15)) >> 16;
-        d[(size_t)gy * dpitch + gx] = (uint8_t)(o > 255 ? 255 : o);
-      }
-    }
-  }
-}
-
 // ---- gradient ---------------------------------------------------------------------------------------------
 // Per-pixel record read by the region-growing kernel: one 8-byte load per neighbour.
 struct __align__(8) LsdPix {
@@ -239,7 +125,7 @@ struct __align__(8) LsdPix {
 // context with exactly the device functions used elsewhere (4 + 8 + 8 MB, L2-resident), which turns ~200 dependent
 // instructions per defined pixel into table loads.
 #define LSD_LUT_DIM 1021
-// lut_angle: the angle of a defined gradient (NOTDEF otherwise; k_lsd_grad only looks up defined ones);
+// lut_angle: the angle of a defined gradient (NOTDEF otherwise; k_lsd_pre only looks up defined ones);
 // lut_cs: (cos(float(angle)), sin(float(angle))) as region_grow adds them, host libm -> glibc port;
 // lut_seed: the unit vector region_grow starts its sums from, float(cos(angle)), float(sin(angle)) of the f64 angle.
 __global__ void __launch_bounds__(256) k_lsd_build_lut(double rho, float* __restrict__ lut_angle, float2* __restrict__ lut_cs,
@@ -275,298 +161,225 @@ __global__ void k_lsd_fill_notdef(LsdPix* __restrict__ pix, size_t n) {
   pix[i] = e;
 }
 
-// pix points at pixel (0,0) of image 0 (i.e. past the guard); image stride pix_stride.
-// Only the DEFINED pixels (gradient norm above rho, ~12 %) leave the kernel: their 8-byte record (the map's other records
-// already read "undefined", see k_lsd_fill_notdef) and one entry (column in the segment, gx^2 + gy^2) of the raster-ordered
-// SEED LIST of their row segment - the LSD_SEG columns of this block; segment (y, xb) stores its entries at the segment's own
-// pixel offset y * W + LSD_SEG * xb of the list array, so it can never overflow, and its length in segcnt.  Nothing dense is
-// written: the seed ordering works on the lists, and the rectangle fit reads the gradient of a region point back from its
-// record (li).
+// ---- pre-blur + resample + gradient ----------------------------------------------------------------------------
+// k_lsd_pre: from the source image to the records, seed lists, segcnt and maxmag2, with no blurred or resampled map in
+// between.  A CTA owns one 512-column row segment (LSD_SEG) of TH <= LSD_PRE_TH scaled rows.  The segment is cut into NP
+// pieces of scaled columns; a piece's source footprint - the blurred rows and columns the resample of its scaled columns
+// and of the scaled rows TH + 1 reads, plus the blur halo - arrives as ONE TMA box (LSD_PRE_BOXH rows of LSD_PRE_BOXW
+// bytes, wider than the 256 elements a box dimension holds: plf_tma_encode_u8_blocks); border CTAs rebuild
+// BORDER_REFLECT_101 in shared memory.  Per piece:
+//   blur     : a PRMT + DP4A row pass into u16 (four sums of a row per group, the taps packed as bytes), then the column
+//              pass and its one rounding, over the footprint only (KS = 1: no blur, the box is the blurred tile)
+//   resample : the integer INTER_LINEAR_EXACT blend from the state's tables into the segment's scaled tile: four scaled
+//              columns of one row per thread (k_resize_exact4's form) where four span at most 8 blurred bytes, else one
+// Then, once over the tile:
+//   gradient : a warp per scaled row, four 128-column chunks of 4 columns per lane; the records of the defined pixels and
+//              the ordered compaction of the row segment's seed list (per chunk: one warp scan; the row is the segment, so
+//              no barrier)
+// pix points at pixel (0,0) of image 0 (i.e. past the guard); image stride pix_stride.  Only the DEFINED pixels (gradient
+// norm above rho, ~12 %) leave the kernel: their 8-byte record (the map's other records already read "undefined", see
+// k_lsd_fill_notdef) and one entry (column in the segment, gx^2 + gy^2) of the raster-ordered SEED LIST of their row
+// segment; segment (y, xb) stores its entries at the segment's own pixel offset y * W + LSD_SEG * xb of the list array, so
+// it can never overflow, and its length in segcnt.  Nothing dense is written: the seed ordering works on the lists, and the
+// rectangle fit reads the gradient of a region point back from its record (li).
+// The blur, resample and gradient are exact integer arithmetic: the records and lists are those of cv::GaussianBlur,
+// cv::resize(INTER_LINEAR_EXACT) and the 2x2 gradient run one after the other.
+// Measured on an H100 80GB HBM3 (700 W power limit), KITTI shape, 2048 images, default parameters (KS 7, TH 16, one
+// piece): 5.42 ms against 8.26 ms for separate blur, resample and gradient kernels; 8 scaled rows per CTA took 6.69 ms.
 #define LSD_SEG 512
-#define LSD_GRAD_THREADS (LSD_SEG / 4)
 // list entry: the low LSD_COL_BITS hold the column inside the segment, the high bits gx^2 + gy^2 (<= 2 * 510^2 over the
 // table's gradient range)
 #define LSD_COL_BITS 9
 static_assert(LSD_SEG <= (1 << LSD_COL_BITS), "seed list: a segment column must fit the column field");
 static_assert(2u * 510u * 510u < (1u << (32 - LSD_COL_BITS)), "seed list: gx^2 + gy^2 must fit above the column field");
-// A thread produces FOUR adjacent columns of two rows from three aligned 32-bit words of the (16-byte pitched) image - the
-// fifth column of each row comes from the neighbour lane's word (lane 31 loads it) - so a warp issues 3 (+3) load instructions
-// for 256 pixels instead of 6 for 64.
-__global__ void __launch_bounds__(LSD_GRAD_THREADS) k_lsd_grad(const uint8_t* __restrict__ img, size_t img_stride, int IP, int W, int H,
-                                                               const float* __restrict__ lut_angle, int m2_min, size_t stride,
-                                                               LsdPix* __restrict__ pix, size_t pix_stride,
-                                                               uint32_t* __restrict__ list, int* __restrict__ segcnt, int nxb,
-                                                               int* __restrict__ maxmag2) {
-  const int x4 = blockIdx.x * LSD_SEG + threadIdx.x * 4, y0 = blockIdx.y * 2, im = blockIdx.z;
-  const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
-  // words of rows y0 .. y0+2 at columns x4 .. x4+3 (rows / words beyond the image read as 0: those pixels are never defined -
-  // the last column and the last row of the map are excluded below)
-  uint32_t w[3] = {0u, 0u, 0u}, wn[3] = {0u, 0u, 0u};
-  const uint8_t* p = img + (size_t)im * img_stride + (size_t)y0 * IP + x4;
-#pragma unroll
-  for (int r = 0; r < 3; ++r)
-    if (x4 < W && y0 + r < H) w[r] = __ldg(reinterpret_cast<const uint32_t*>(p + (size_t)r * IP));   // IP is a multiple of 16, x4 of 4
-#pragma unroll
-  for (int r = 0; r < 3; ++r) {
-    wn[r] = __shfl_down_sync(0xFFFFFFFFu, w[r], 1);
-    if (lane == 31) wn[r] = (x4 + 4 < IP && y0 + r < H) ? __ldg(reinterpret_cast<const uint32_t*>(p + (size_t)r * IP + 4)) : 0u;
-  }
-  int mag2 = -1;
-  int li[2][4], m2v[2][4];
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const bool rok = y0 + r < H - 1;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      li[r][c] = -1; m2v[r][c] = 0;
-      // pixel (x, y) = (x4 + c, y0 + r): A = (x, y), B = (x+1, y), C = (x, y+1), D = (x+1, y+1)
-      const int A = (w[r] >> (8 * c)) & 0xFF, C = (w[r + 1] >> (8 * c)) & 0xFF;
-      const int B = c < 3 ? (int)((w[r] >> (8 * c + 8)) & 0xFF) : (int)(wn[r] & 0xFF);
-      const int D = c < 3 ? (int)((w[r + 1] >> (8 * c + 8)) & 0xFF) : (int)(wn[r + 1] & 0xFF);
-      if (rok && x4 + c < W - 1) {
-        const int DA = D - A, BC = B - C, gx = DA + BC, gy = DA - BC, m2 = gx * gx + gy * gy;
-        if (m2 >= m2_min) { li[r][c] = (gx + 510) * LSD_LUT_DIM + (gy + 510); m2v[r][c] = m2; mag2 = max(mag2, m2); }  // defined angle
-      }
-    }
-  }
-  // records of the defined pixels
-#pragma unroll
-  for (int r = 0; r < 2; ++r)
-#pragma unroll
-    for (int c = 0; c < 4; ++c)
-      if (li[r][c] >= 0)
-        *reinterpret_cast<uint2*>(&pix[(size_t)im * pix_stride + (size_t)(y0 + r) * W + x4 + c]) =
-            make_uint2(__float_as_uint(__ldg(&lut_angle[li[r][c]])), (uint32_t)li[r][c]);
-  // ordered compaction of the two row segments (x ascending) + the per-image maximum: one barrier
-  __shared__ int s_max[4], s_c[2][4];
-  int cnt[2], incl[2];
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    cnt[r] = (li[r][0] >= 0) + (li[r][1] >= 0) + (li[r][2] >= 0) + (li[r][3] >= 0);
-    incl[r] = cnt[r];
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int v = __shfl_up_sync(0xFFFFFFFFu, incl[r], off);
-      if (lane >= off) incl[r] += v;
-    }
-  }
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) mag2 = max(mag2, __shfl_xor_sync(0xFFFFFFFFu, mag2, off));
-  if (lane == 31) { s_c[0][wrp] = incl[0]; s_c[1][wrp] = incl[1]; }
-  if (lane == 0) s_max[wrp] = mag2;
-  __syncthreads();
-  const size_t lbase = (size_t)im * stride + (size_t)blockIdx.x * LSD_SEG;
-  int tot[2];
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    int woff = 0;
-    tot[r] = 0;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (k < wrp) woff += s_c[r][k];
-      tot[r] += s_c[r][k];
-    }
-    size_t o = lbase + (size_t)(y0 + r) * W + woff + incl[r] - cnt[r];
-#pragma unroll
-    for (int c = 0; c < 4; ++c)
-      if (li[r][c] >= 0) {
-        list[o] = (uint32_t)(threadIdx.x * 4 + c) | ((uint32_t)m2v[r][c] << LSD_COL_BITS);
-        ++o;
-      }
-  }
-  if (threadIdx.x == 0) {
-    int* sc = segcnt + (size_t)im * ((size_t)H * nxb);
-    sc[(size_t)y0 * nxb + blockIdx.x] = tot[0];
-    if (y0 + 1 < H) sc[(size_t)(y0 + 1) * nxb + blockIdx.x] = tot[1];
-    const int m = max(max(s_max[0], s_max[1]), max(s_max[2], s_max[3]));
-    if (m >= 0 && m > __ldcg(&maxmag2[im])) atomicMax(&maxmag2[im], m);   // only touch the (contended) address when it would grow
-  }
-}
+#define LSD_PRE_TH 16         // scaled rows per CTA, at most
+#define LSD_PRE_THREADS 256   // 8 warps: the gradient takes rows wrp, wrp + 8
+#define LSD_PRE_BOXW 544      // TMA box width, bytes (34 blocks of 16)
+#define LSD_PRE_BOXH 24       // TMA box rows
+#define LSD_PRE_HW 528        // blurred columns a piece can produce (132 groups of 4: the row pass reads < LSD_PRE_BOXW)
+#define LSD_PRE_SP 528        // row pitch of the staged scaled tile (>= LSD_SEG + 4)
+#define LSD_PRE_KS_MAX 15
+// The image-size sweep the front-end's geometry tests run every detector at (tests/test_frontend_geometry.py) keeps the
+// edges of the two LSD blur tile grids this kernel replaced - 64 x 32 tiles placed at 64 bx - (16 - R), and 64 x 16 tiles
+// - and reads their sizes here, so that the sweep and the tests written against it stay as they are.  No kernel uses them.
+#define BF_TW 64
+#define BF_TH 32
+#define BQ_TW 64
+#define BQ_TH 16
+static_assert(LSD_PRE_HW % 4 == 0 && 4 * (LSD_PRE_HW / 4 - 1) + 4 * ((LSD_PRE_KS_MAX + 3) / 4 + 1) <= LSD_PRE_BOXW,
+              "row pass: a group reads (KS + 3) / 4 + 1 words");
+static_assert(LSD_PRE_HW + LSD_PRE_KS_MAX - 1 <= LSD_PRE_BOXW, "blur: the halo of the blurred columns lies in the box");
+static_assert(LSD_PRE_BOXW % 16 == 0 && LSD_PRE_BOXW / 16 <= 256, "box: 16-byte blocks, at most 256 of them");
+static_assert((LSD_PRE_TH + 1) * LSD_PRE_SP <= LSD_PRE_BOXH * LSD_PRE_HW * 2, "one piece: the scaled tile reuses the u16 row-pass tile");
 
-// ---- fused pre-blur + resample + gradient ------------------------------------------------------------------
-// k_lsd_pre_fused: what k_blur_q8_fast -> k_resize_exact4 -> k_lsd_grad compute, from the source image to the records,
-// seed lists, segcnt and maxmag2, without the blurred and resampled maps in between.  A CTA owns one 512-column row
-// segment (LSD_SEG) of LSD_PF_TH scaled rows.  Its source footprint - the blurred rows and columns the resample of its
-// scaled rows LSD_PF_TH + 1 and columns LSD_SEG + 1 reads, plus the blur halo - arrives as ONE TMA box (LSD_PF_BOXH rows of
-// LSD_PF_BOXW bytes, wider than the 256 elements a box dimension holds: the tensor map views a row as 16-byte blocks, so
-// the box is {16 bytes, LSD_PF_BOXW / 16 blocks, rows, 1 image}); border CTAs rebuild BORDER_REFLECT_101 in shared memory.
-//   blur     : k_blur_q8_fast's DP4A row pass into u16, then the column pass and its one rounding, over the footprint only
-//   resample : k_resize_exact4's integer blend from the state's tables, four scaled columns of one row per thread
-//   gradient : a warp per scaled row, four 128-column chunks of 4 columns per lane, k_lsd_grad's arithmetic, records and
-//              ordered compaction (per chunk: one warp scan; the row is the segment, so no barrier)
-// Measured on an H100 80GB HBM3 (700 W power limit), KITTI shape, 2048 images: 5.42 ms against 8.26 ms for the three
-// kernels; 8 scaled rows per CTA (16-row box) took 6.69 ms.
-// The blur, resample and gradient are exact integer arithmetic, so the records and lists are those of the three kernels,
-// byte for byte.  Which states can use it: lsd_pre_fused_fits (5 or 7 u8 taps, every footprint inside the box).
-#define LSD_PF_TH 16         // scaled rows per CTA
-#define LSD_PF_THREADS 256   // 8 warps: the gradient takes rows wrp, wrp + 8
-#define LSD_PF_BOXW 544      // TMA box width, bytes (34 blocks of 16)
-#define LSD_PF_BOXH 24       // TMA box rows
-#define LSD_PF_HW 528        // blurred columns a CTA can produce (132 groups of 4: the row pass reads < LSD_PF_BOXW)
-#define LSD_PF_SP 528        // row pitch of the staged scaled tile (>= LSD_SEG + 4)
-static_assert(LSD_PF_HW % 4 == 0 && 4 * (LSD_PF_HW / 4 - 1) + 12 <= LSD_PF_BOXW, "row pass: a group reads 12 bytes");
-static_assert(LSD_PF_BOXW % 16 == 0 && LSD_PF_BOXW / 16 <= 256, "box: 16-byte blocks, at most 256 of them");
-static_assert((LSD_PF_TH + 1) * LSD_PF_SP <= LSD_PF_BOXH * LSD_PF_HW * 2, "the scaled tile reuses the u16 row-pass tile");
-
-// The source footprint of one CTA, from the resample tables (ox / oy non-decreasing): blurred columns [bxc, sx1] and rows
-// [sy0, sy1]; the box starts at column bxc - R (on a 16-byte boundary) and row sy0 - R.
-struct LsdPfFoot { int bxc, sx1, sy0, sy1; };
-__host__ __device__ __forceinline__ LsdPfFoot lsd_pf_foot(const int* ox, const int* oy, int W, int H, int xb, int yb, int R) {
-  const int X0 = xb * LSD_SEG, Xl = min(X0 + LSD_SEG, W - 1);
-  const int Y0 = yb * LSD_PF_TH, Yl = min(Y0 + LSD_PF_TH, H - 1);
-  LsdPfFoot f;
-  f.bxc = ((ox[X0] - R) & ~15) + R;   // floor to a 16-byte boundary (two's complement: also below column 0)
-  f.sx1 = ox[Xl] + 1;
-  f.sy0 = oy[Y0];
-  f.sy1 = oy[Yl] + 1;
+// The source footprint of scaled columns [xa, xl] and rows [ya, yl], from the resample tables (ox / oy non-decreasing,
+// at most the source size - 2): blurred columns [bxc, sx1] and rows [sy0, sy1]; the box starts at column bxc - R (on a
+// 16-byte boundary) and row sy0 - R.
+struct LsdPreFoot { int bxc, sx1, sy0, sy1; };
+__host__ __device__ __forceinline__ LsdPreFoot lsd_pre_foot(const int* ox, const int* oy, int xa, int xl, int ya, int yl, int R) {
+  LsdPreFoot f;
+  f.bxc = ((ox[xa] - R) & ~15) + R;   // floor to a 16-byte boundary (two's complement: also below column 0)
+  f.sx1 = ox[xl] + 1;
+  f.sy0 = oy[ya];
+  f.sy1 = oy[yl] + 1;
   return f;
 }
 
 // tabx = [ox(W) | cx(W)], taby = [oy(H) | cy(H)] (plf_linear_coeffs_host), tabxp = the packed x table of k_resize_exact4
-// (plf_resize_pack_x); pix / list / segcnt / maxmag2 as k_lsd_grad.
+// (plf_resize_pack_x); g = the state's LsdPreGeom; dynamic shared memory: the scaled tile ((TH + 1) x LSD_PRE_SP) when
+// NP > 1, none otherwise.
 template <int KS>
-__global__ void __launch_bounds__(LSD_PF_THREADS, 5) k_lsd_pre_fused(const __grid_constant__ CUtensorMap tmap, int w, int h, int W, int H,
-                                                                  uint32_t tapsA, uint32_t tapsB, const int* __restrict__ tabx,
-                                                                  const int4* __restrict__ tabxp, const int* __restrict__ taby,
-                                                                  const float* __restrict__ lut_angle,
-                                                                  int m2_min, size_t stride, LsdPix* __restrict__ pix, size_t pix_stride,
-                                                                  uint32_t* __restrict__ list, int* __restrict__ segcnt, int nxb,
-                                                                  int* __restrict__ maxmag2) {
-  constexpr int R = KS / 2;
-  constexpr int BP = LSD_PF_BOXW;
-  __shared__ __align__(128) uint8_t raw[LSD_PF_BOXH][BP];       // the box; then the blurred tile (pitch BP)
-  __shared__ __align__(16) uint16_t hrow[LSD_PF_BOXH][LSD_PF_HW]; // row-pass sums; then the scaled tile (pitch LSD_PF_SP)
+__global__ void __launch_bounds__(LSD_PRE_THREADS, 5) k_lsd_pre(const __grid_constant__ CUtensorMap tmap, int w, int h, int W, int H,
+                                                             const LsdPreGeom g, const int* __restrict__ tabx,
+                                                             const int4* __restrict__ tabxp, const int* __restrict__ taby,
+                                                             const float* __restrict__ lut_angle,
+                                                             int m2_min, size_t stride, LsdPix* __restrict__ pix, size_t pix_stride,
+                                                             uint32_t* __restrict__ list, int* __restrict__ segcnt, int nxb,
+                                                             int* __restrict__ maxmag2) {
+  constexpr int R = KS / 2, NW = (KS + 3) / 4;   // NW tap words
+  constexpr int BP = LSD_PRE_BOXW;
+  __shared__ __align__(128) uint8_t raw[LSD_PRE_BOXH][BP];        // the box; then the blurred tile (pitch BP)
+  __shared__ __align__(16) uint16_t hrow[LSD_PRE_BOXH][LSD_PRE_HW]; // row-pass sums; with one piece then the scaled tile
   __shared__ __align__(8) uint64_t bar;
-  __shared__ int s_max[LSD_PF_THREADS / 32];
+  __shared__ int s_max[LSD_PRE_THREADS / 32];
+  extern __shared__ __align__(16) uint8_t sc_own[];
   uint8_t* blur = &raw[0][0];
-  uint8_t* sc = reinterpret_cast<uint8_t*>(&hrow[0][0]);
+  uint8_t* sc = g.np > 1 ? sc_own : reinterpret_cast<uint8_t*>(&hrow[0][0]);   // pitch LSD_PRE_SP
   const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
-  const int xb = blockIdx.x, im = blockIdx.z;
-  const int X0 = xb * LSD_SEG, Y0 = blockIdx.y * LSD_PF_TH;
-  const LsdPfFoot f = lsd_pf_foot(tabx, taby, W, H, xb, blockIdx.y, R);
-  const int gx0 = f.bxc - R, gy0 = f.sy0 - R;   // source pixel of raw[0][0]
+  const int xb = blockIdx.x, im = blockIdx.z, TH = g.th;
+  const int X0 = xb * LSD_SEG, Y0 = blockIdx.y * TH;
+  const int nsc = min(LSD_SEG + 1, W - X0), nsr = min(TH + 1, H - Y0);   // scaled columns / rows of the tile that exist
+  uint32_t tw[NW];
+#pragma unroll
+  for (int k = 0; k < NW; ++k) tw[k] = k == 0 ? g.taps.x : k == 1 ? g.taps.y : k == 2 ? g.taps.z : g.taps.w;
   if (tid == 0) plf_mbar_init(&bar);
   __syncthreads();
-  if (tid == 0) {
-    const uint32_t b = plf_smem_u32(&bar);
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(b), "r"(LSD_PF_BOXH * BP) : "memory");
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];" ::"r"(
-            plf_smem_u32(&raw[0][0])),
-        "l"(&tmap), "r"(0), "r"(gx0 >> 4), "r"(gy0), "r"(im), "r"(b)
-        : "memory");
-  }
-  const int ncol = f.sx1 - f.bxc + 1, nrow = f.sy1 - f.sy0 + 1;   // blurred tile: nrow x ncol
-  const int need_w = ncol + 2 * R, need_h = nrow + 2 * R;        // box cells the blur reads
-  plf_mbar_wait(&bar, 0);
-  // BORDER_REFLECT_101: the cells outside the image among those read, from their mirror pixel (inside this box: the
-  // footprint reaches at most R + 15 columns / R rows past an edge).  In-image rows first, then whole rows.  Cells past the
-  // image's last column hold the pitch padding or zeros; rows outside it zeros.
-  if (gx0 < 0 || gx0 + need_w > w || gy0 < 0 || gy0 + need_h > h) {
-    const int ry_lo = max(0, -gy0), ry_hi = min(need_h, h - gy0);
-    const int nl = min(need_w, max(0, -gx0)), rx_r = max(0, w - gx0), nr = max(0, need_w - rx_r);
-    if (nl + nr > 0)
-      for (int i = tid; i < (ry_hi - ry_lo) * (nl + nr); i += LSD_PF_THREADS) {
-        const int k = i / (nl + nr), j = i - k * (nl + nr);
-        const int rx = j < nl ? j : rx_r + (j - nl);
-        raw[ry_lo + k][rx] = raw[ry_lo + k][plf_reflect101(gx0 + rx, w) - gx0];
+  for (int p = 0; p < g.np && p * g.pw < nsc; ++p) {
+    const int u0 = p * g.pw, u1 = min(u0 + g.pw, nsc);   // the piece's scaled columns, from X0
+    const LsdPreFoot f = lsd_pre_foot(tabx, taby, X0 + u0, X0 + u1 - 1, Y0, min(Y0 + TH, H - 1), R);
+    const int gx0 = f.bxc - R, gy0 = f.sy0 - R;   // source pixel of raw[0][0]
+    if (p > 0) {   // the previous piece's blurred tile is read
+      plf_fence_proxy_async();
+      __syncthreads();
+    }
+    if (tid == 0) plf_tma_load_4d(&raw[0][0], &tmap, 0, gx0 >> 4, gy0, im, &bar, LSD_PRE_BOXH * BP);
+    const int ncol = f.sx1 - f.bxc + 1, nrow = f.sy1 - f.sy0 + 1;   // blurred tile: nrow x ncol
+    const int need_w = ncol + 2 * R, need_h = nrow + 2 * R;        // box cells the blur reads
+    plf_mbar_wait(&bar, p & 1);
+    // BORDER_REFLECT_101: the cells outside the image among those read, from their mirror pixel (inside this box: the
+    // footprint reaches at most R + 15 columns / R rows past an edge, and its tables end at the source size - 2).
+    // In-image rows first, then whole rows.  Cells past the image's last column hold the pitch padding or zeros; rows
+    // outside it zeros.
+    if (gx0 < 0 || gx0 + need_w > w || gy0 < 0 || gy0 + need_h > h) {
+      const int ry_lo = max(0, -gy0), ry_hi = min(need_h, h - gy0);
+      const int nl = min(need_w, max(0, -gx0)), rx_r = max(0, w - gx0), nr = max(0, need_w - rx_r);
+      if (nl + nr > 0)
+        for (int i = tid; i < (ry_hi - ry_lo) * (nl + nr); i += LSD_PRE_THREADS) {
+          const int k = i / (nl + nr), j = i - k * (nl + nr);
+          const int rx = j < nl ? j : rx_r + (j - nl);
+          raw[ry_lo + k][rx] = raw[ry_lo + k][plf_reflect101(gx0 + rx, w) - gx0];
+        }
+      __syncthreads();
+      const int nw = (need_w + 3) >> 2;
+      for (int i = tid; i < (ry_lo + need_h - ry_hi) * nw; i += LSD_PRE_THREADS) {
+        const int k = i / nw, j = i - k * nw;
+        const int ry = k < ry_lo ? k : ry_hi + (k - ry_lo);
+        const int m = plf_reflect101(gy0 + ry, h) - gy0;
+        reinterpret_cast<uint32_t*>(raw[ry])[j] = reinterpret_cast<const uint32_t*>(raw[m])[j];
       }
+    }
     __syncthreads();
-    const int nw = (need_w + 3) >> 2;
-    for (int i = tid; i < (ry_lo + need_h - ry_hi) * nw; i += LSD_PF_THREADS) {
-      const int k = i / nw, j = i - k * nw;
-      const int ry = k < ry_lo ? k : ry_hi + (k - ry_lo);
-      const int m = plf_reflect101(gy0 + ry, h) - gy0;
-      reinterpret_cast<uint32_t*>(raw[ry])[j] = reinterpret_cast<const uint32_t*>(raw[m])[j];
-    }
-  }
-  __syncthreads();
-  // row pass: 4 adjacent sums of a row per group, k_blur_q8_fast's PRMT + DP4A (sum of column c: box columns c .. c + 2R)
-  const int ngrp = (ncol + 3) >> 2;
-  for (int ry = wrp; ry < need_h; ry += LSD_PF_THREADS / 32)
-    for (int j = lane; j < ngrp; j += 32) {
-      const uint32_t* wp = reinterpret_cast<const uint32_t*>(&raw[ry][4 * j]);
-      const uint32_t w0 = wp[0], w1 = wp[1], w2 = wp[2];
-      uint32_t o[4];
+    if (KS > 1) {
+      // row pass: 4 adjacent sums of a row per group (sum of column c: box columns c .. c + 2R); output i of tap word k is
+      // the byte window 4k + i .. 4k + i + 3, one PRMT of words k, k + 1, reduced by one DP4A (taps <= 255, exact in 32 bits,
+      // result < 2^16)
+      const int ngrp = (ncol + 3) >> 2;
+      for (int ry = wrp; ry < need_h; ry += LSD_PRE_THREADS / 32)
+        for (int j = lane; j < ngrp; j += 32) {
+          const uint32_t* wp = reinterpret_cast<const uint32_t*>(&raw[ry][4 * j]);
+          uint32_t wv[NW + 1];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const uint32_t lo = __byte_perm(w0, w1, 0x3210 + 0x1111 * i);
-        const uint32_t hi = __byte_perm(w1, w2, 0x3210 + 0x1111 * i);
-        o[i] = __dp4a(hi, tapsB, __dp4a(lo, tapsA, 0u));
+          for (int k = 0; k <= NW; ++k) wv[k] = wp[k];
+          uint32_t o[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            o[i] = 0u;
+#pragma unroll
+            for (int k = 0; k < NW; ++k) o[i] = __dp4a(__byte_perm(wv[k], wv[k + 1], 0x3210 + 0x1111 * i), tw[k], o[i]);
+          }
+          *reinterpret_cast<uint2*>(&hrow[ry][4 * j]) = make_uint2(o[0] | (o[1] << 16), o[2] | (o[3] << 16));
+        }
+      __syncthreads();
+      // column pass: one column per thread, the taps in registers, one rounding (the box is dead: the blurred tile replaces it)
+      uint32_t t[KS];
+#pragma unroll
+      for (int k = 0; k < KS; ++k) t[k] = (tw[k >> 2] >> (8 * (k & 3))) & 0xFFu;
+      for (int c = tid; c < ncol; c += LSD_PRE_THREADS) {
+        uint32_t v[LSD_PRE_BOXH];
+#pragma unroll
+        for (int k = 0; k < LSD_PRE_BOXH; ++k) v[k] = hrow[k][c];
+#pragma unroll
+        for (int r = 0; r < LSD_PRE_BOXH - 2 * R; ++r)
+          if (r < nrow) {
+            uint32_t a = 0;
+#pragma unroll
+            for (int k = 0; k < KS; ++k) a += t[k] * v[r + k];
+            const uint32_t o = (a + (1u << 15)) >> 16;
+            blur[r * BP + c] = (uint8_t)(o > 255 ? 255 : o);
+          }
       }
-      *reinterpret_cast<uint2*>(&hrow[ry][4 * j]) = make_uint2(o[0] | (o[1] << 16), o[2] | (o[3] << 16));
+      __syncthreads();
     }
-  __syncthreads();
-  // column pass: one column per thread, the taps in registers, one rounding (the box is dead: the blurred tile replaces it)
-  {
-    uint32_t t[KS];
+    // resample of the piece's scaled columns [u0, u1) and the rows Y0 .. Y0 + TH that exist.  Packed form: four adjacent
+    // columns per thread from three words per blurred row, each output's byte pair by one PRMT, the horizontal blend by one
+    // IDP.2A on the packed weight pair; thread = (4-column group tid % 128, row parity tid / 128).  Column LSD_SEG (the
+    // right neighbour of the segment's last column), and every column where the packed form does not apply, by the scalar
+    // form.
+    if (g.packed) {
+      const int gi = tid & 127, x = X0 + 4 * gi;
+      if (4 * gi >= u0 && 4 * gi < min(u1, LSD_SEG)) {
+        const int4 t0 = __ldg(&tabxp[2 * (x >> 2)]), t1 = __ldg(&tabxp[2 * (x >> 2) + 1]);
+        const int ox0 = t0.x - f.bxc, mis = ox0 & 3, s8 = 8 * mis;
+        const int ofs[4] = {t0.x, t0.z, t1.x, t1.z};
+        const uint32_t wx[4] = {(uint32_t)t0.y, (uint32_t)t0.w, (uint32_t)t1.y, (uint32_t)t1.w};
+        for (int r = tid >> 7; r < nsr; r += 2) {
+          const int oy = __ldg(&taby[Y0 + r]) - f.sy0, cy = __ldg(&taby[H + Y0 + r]);
+          const uint32_t* pa = reinterpret_cast<const uint32_t*>(blur + oy * BP + ox0 - mis);
+          const uint32_t* pb = pa + BP / 4;
+          const uint32_t alo = __funnelshift_r(pa[0], pa[1], s8), ahi = __funnelshift_r(pa[1], pa[2], s8);
+          const uint32_t blo = __funnelshift_r(pb[0], pb[1], s8), bhi = __funnelshift_r(pb[1], pb[2], s8);
+          const uint32_t wy0 = (uint32_t)(256 - cy), wy1 = (uint32_t)cy;
+          uint32_t v[4];
 #pragma unroll
-    for (int k = 0; k < KS; ++k) t[k] = k < 4 ? ((tapsA >> (8 * k)) & 0xFFu) : ((tapsB >> (8 * (k - 4))) & 0xFFu);
-    for (int c = tid; c < ncol; c += LSD_PF_THREADS) {
-      uint32_t v[LSD_PF_BOXH];
-#pragma unroll
-      for (int k = 0; k < LSD_PF_BOXH; ++k) v[k] = hrow[k][c];
-#pragma unroll
-      for (int r = 0; r < LSD_PF_BOXH - 2 * R; ++r)
-        if (r < nrow) {
-          uint32_t a = 0;
-#pragma unroll
-          for (int k = 0; k < KS; ++k) a += t[k] * v[r + k];
-          const uint32_t o = (a + (1u << 15)) >> 16;
-          blur[r * BP + c] = (uint8_t)(o > 255 ? 255 : o);
+          for (int i = 0; i < 4; ++i) {
+            const uint32_t sel = (uint32_t)(ofs[i] - ofs[0]) * 0x11u + 0x10u;
+            const uint32_t h0 = __dp2a_lo(wx[i], __byte_perm(alo, ahi, sel), 0u);
+            const uint32_t h1 = __dp2a_lo(wx[i], __byte_perm(blo, bhi, sel), 0u);
+            v[i] = (h0 * wy0 + h1 * wy1 + 32768u) >> 16;
+          }
+          *reinterpret_cast<uint32_t*>(sc + r * LSD_PRE_SP + 4 * gi) = (v[0] | (v[1] << 8)) | ((v[2] | (v[3] << 8)) << 16);
         }
-    }
-  }
-  __syncthreads();
-  // resample: scaled rows Y0 .. Y0 + LSD_PF_TH and columns X0 .. X0 + LSD_SEG that exist (the u16 tile is dead).
-  // k_resize_exact4's form: four adjacent columns per thread from three words per blurred row (the four read at most 8
-  // blurred columns: the box's rows admit no scale below 0.8), each output's byte pair by one PRMT, the horizontal blend by one IDP.2A on the packed
-  // weight pair; thread = (4-column group tid % 128, row parity tid / 128).  Column LSD_SEG (the right neighbour of the
-  // segment's last column) alone by the scalar form.
-  const int nsc = min(LSD_SEG + 1, W - X0), nsr = min(LSD_PF_TH + 1, H - Y0);
-  {
-    const int g = tid & 127, x = X0 + 4 * g;
-    if (x < W) {
-      const int4 t0 = __ldg(&tabxp[2 * (x >> 2)]), t1 = __ldg(&tabxp[2 * (x >> 2) + 1]);
-      const int ox0 = t0.x - f.bxc, mis = ox0 & 3, s8 = 8 * mis;
-      const int ofs[4] = {t0.x, t0.z, t1.x, t1.z};
-      const uint32_t wx[4] = {(uint32_t)t0.y, (uint32_t)t0.w, (uint32_t)t1.y, (uint32_t)t1.w};
-      for (int r = tid >> 7; r < nsr; r += 2) {
-        const int oy = __ldg(&taby[Y0 + r]) - f.sy0, cy = __ldg(&taby[H + Y0 + r]);
-        const uint32_t* pa = reinterpret_cast<const uint32_t*>(blur + oy * BP + ox0 - mis);
-        const uint32_t* pb = pa + BP / 4;
-        const uint32_t alo = __funnelshift_r(pa[0], pa[1], s8), ahi = __funnelshift_r(pa[1], pa[2], s8);
-        const uint32_t blo = __funnelshift_r(pb[0], pb[1], s8), bhi = __funnelshift_r(pb[1], pb[2], s8);
-        const uint32_t wy0 = (uint32_t)(256 - cy), wy1 = (uint32_t)cy;
-        uint32_t v[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const uint32_t sel = (uint32_t)(ofs[i] - ofs[0]) * 0x11u + 0x10u;
-          const uint32_t h0 = __dp2a_lo(wx[i], __byte_perm(alo, ahi, sel), 0u);
-          const uint32_t h1 = __dp2a_lo(wx[i], __byte_perm(blo, bhi, sel), 0u);
-          v[i] = (h0 * wy0 + h1 * wy1 + 32768u) >> 16;
-        }
-        *reinterpret_cast<uint32_t*>(sc + r * LSD_PF_SP + 4 * g) = (v[0] | (v[1] << 8)) | ((v[2] | (v[3] << 8)) << 16);
       }
     }
-    if (nsc > LSD_SEG && tid < nsr) {
-      const int r = tid, u = LSD_SEG;
+    const int us = g.packed ? max(u0, LSD_SEG) : u0, nu = u1 - us;
+    for (int i = tid; i < nu * nsr; i += LSD_PRE_THREADS) {
+      const int r = i / nu, u = us + (i - r * nu);
       const int ox = __ldg(&tabx[X0 + u]) - f.bxc, cx = __ldg(&tabx[W + X0 + u]);
       const int oy = __ldg(&taby[Y0 + r]) - f.sy0, cy = __ldg(&taby[H + Y0 + r]);
       const uint8_t* b0 = blur + oy * BP + ox;
       const uint32_t h0 = (uint32_t)b0[0] * (uint32_t)(256 - cx) + (uint32_t)b0[1] * (uint32_t)cx;
       const uint32_t h1 = (uint32_t)b0[BP] * (uint32_t)(256 - cx) + (uint32_t)b0[BP + 1] * (uint32_t)cx;
-      sc[r * LSD_PF_SP + u] = (uint8_t)((h0 * (uint32_t)(256 - cy) + h1 * (uint32_t)cy + 32768u) >> 16);
+      sc[r * LSD_PRE_SP + u] = (uint8_t)((h0 * (uint32_t)(256 - cy) + h1 * (uint32_t)cy + 32768u) >> 16);
     }
   }
   __syncthreads();
-  // gradient: warp wrp takes scaled rows y = Y0 + t, t = wrp, wrp + 8 (cells of the tile outside the image are never read
-  // into a defined pixel)
+  // gradient: warp wrp takes scaled rows y = Y0 + t, t = wrp, wrp + 8, ... (cells of the tile outside the image are never
+  // read into a defined pixel)
   int mag2 = -1;
-  for (int t = wrp; t < LSD_PF_TH && Y0 + t < H; t += LSD_PF_THREADS / 32) {
+  for (int t = wrp; t < TH && Y0 + t < H; t += LSD_PRE_THREADS / 32) {
     const int y = Y0 + t;
-    const uint32_t* s0 = reinterpret_cast<const uint32_t*>(sc + t * LSD_PF_SP);
-    const uint32_t* s1 = reinterpret_cast<const uint32_t*>(sc + (t + 1) * LSD_PF_SP);
+    const uint32_t* s0 = reinterpret_cast<const uint32_t*>(sc + t * LSD_PRE_SP);
+    const uint32_t* s1 = reinterpret_cast<const uint32_t*>(sc + (t + 1) * LSD_PRE_SP);
     const bool rok = y < H - 1;
     LsdPix* prow = pix + (size_t)im * pix_stride + (size_t)y * W + X0;
     uint32_t* lrow = list + (size_t)im * stride + (size_t)y * W + X0;
@@ -615,7 +428,7 @@ __global__ void __launch_bounds__(LSD_PF_THREADS, 5) k_lsd_pre_fused(const __gri
   if (tid == 0) {
     int m = s_max[0];
 #pragma unroll
-    for (int k = 1; k < LSD_PF_THREADS / 32; ++k) m = max(m, s_max[k]);
+    for (int k = 1; k < LSD_PRE_THREADS / 32; ++k) m = max(m, s_max[k]);
     if (m >= 0 && m > __ldcg(&maxmag2[im])) atomicMax(&maxmag2[im], m);
   }
 }
@@ -1417,41 +1230,61 @@ static void gaussian_taps_q8(int ksize, double sigma, int* taps) {
   taps[ksize / 2] = 256 - 2 * s;
 }
 
-// The Gaussian pre-blur of scale != 1: its size (0 at scale 1), Q8 taps, and whether every tap is <= 255.
-static void lsd_blur_taps(const plf_params& P, int* ksize, int* taps, bool* taps_u8) {
+// The Gaussian pre-blur of scale != 1: its size (0 at scale 1) and, up to LSD_PRE_KS_MAX, its Q8 taps.
+static void lsd_blur_taps(const plf_params& P, int* ksize, int* taps) {
   *ksize = 0;
-  *taps_u8 = false;
   if (P.lsd_scale == 1.0) return;
   const double scale = P.lsd_scale;
   const double sigma = (scale < 1) ? (P.lsd_sigma_scale / scale) : P.lsd_sigma_scale;
   const unsigned hk = (unsigned)(ceil(sigma * sqrt(2 * 3.0 * log(10.0))));
   *ksize = 1 + 2 * (int)hk;
-  if (*ksize > 15) return;
-  gaussian_taps_q8(*ksize, sigma, taps);
-  *taps_u8 = true;
-  for (int k = 0; k < *ksize; ++k) *taps_u8 = *taps_u8 && taps[k] <= 255;
+  if (*ksize <= LSD_PRE_KS_MAX) gaussian_taps_q8(*ksize, sigma, taps);
 }
 
-// Whether k_lsd_pre_fused runs for a w x h image resampled to ws x hs: 5 or 7 taps <= 255 (its DP4A row pass), and the
-// footprint of every CTA inside the box (every scale from 1 up at 7 taps, and from 0.9 or so at 5; below, the three kernels run).
-static bool lsd_pre_fused_fits(const plf_params& P, int w, int h, int ws, int hs) {
-  int ksize, taps[16];
-  bool u8;
-  lsd_blur_taps(P, &ksize, taps, &u8);
-  if (!((ksize == 5 || ksize == 7) && u8) || ws < 2 || hs < 2) return false;
-  const int R = ksize / 2;
-  std::vector<int> tx(2 * (size_t)ws), ty(2 * (size_t)hs);
-  plf_linear_coeffs_host(w, ws, 1.0 / P.lsd_scale, &tx[0], &tx[ws]);
-  plf_linear_coeffs_host(h, hs, 1.0 / P.lsd_scale, &ty[0], &ty[hs]);
-  const int nxb = (ws + LSD_SEG - 1) / LSD_SEG, nyb = (hs + LSD_PF_TH - 1) / LSD_PF_TH;
-  for (int xb = 0; xb < nxb; ++xb) {
-    const LsdPfFoot f = lsd_pf_foot(tx.data(), ty.data(), ws, hs, xb, 0, R);
-    if (f.sx1 - f.bxc + 1 > LSD_PF_HW) return false;
+// k_lsd_pre's launch for a w x h image resampled to ws x hs, from the resize tables ox, oy:
+//   KS      the pre-blur's taps; 1 at scale 1 and where the centre tap is 256.  gaussian_taps_q8 makes the side taps
+//           non-negative and below 128, so a 256 centre (the one tap a byte cannot hold) means every side tap is 0 and
+//           the blur is a copy;
+//   TH      the most scaled rows (<= LSD_PRE_TH) whose footprint plus the blur halo fits the box's rows in every band;
+//   NP, PW  the fewest pieces of PW scaled columns (a multiple of 4) per segment whose footprints fit LSD_PRE_HW blurred
+//           columns in every segment;
+//   packed  plf_resize_packed_ok.
+// false where even one scaled row does not fit the box (downsampling by more than about 1 / (22 - 2R)).
+static bool lsd_pre_geom(const plf_params& P, int w, int ws, int hs, const int* ox, const int* oy, LsdPreGeom* g) {
+  int ks, taps[LSD_PRE_KS_MAX];
+  lsd_blur_taps(P, &ks, taps);
+  *g = LsdPreGeom();
+  if (ks > LSD_PRE_KS_MAX) return false;
+  if (ks > 1 && taps[ks / 2] < 256) {
+    uint32_t tw[4] = {0u, 0u, 0u, 0u};
+    for (int k = 0; k < ks; ++k) tw[k >> 2] |= (uint32_t)taps[k] << (8 * (k & 3));
+    g->ks = ks;
+    g->taps = make_uint4(tw[0], tw[1], tw[2], tw[3]);
   }
-  for (int yb = 0; yb < nyb; ++yb) {
-    const LsdPfFoot f = lsd_pf_foot(tx.data(), ty.data(), ws, hs, 0, yb, R);
-    if (f.sy1 - f.sy0 + 1 + 2 * R > LSD_PF_BOXH) return false;
+  const int R = g->ks / 2;
+  for (g->th = LSD_PRE_TH; g->th > 0; --g->th) {
+    bool fits = true;
+    for (int y0 = 0; y0 < hs && fits; y0 += g->th) {
+      const LsdPreFoot f = lsd_pre_foot(ox, oy, 0, 0, y0, std::min(y0 + g->th, hs - 1), R);
+      fits = f.sy1 - f.sy0 + 1 + 2 * R <= LSD_PRE_BOXH;
+    }
+    if (fits) break;
   }
+  if (g->th == 0) return false;
+  for (g->np = 1;; ++g->np) {
+    g->pw = ((LSD_SEG + g->np) / g->np + 3) & ~3;   // ceil((LSD_SEG + 1) / np), whole groups of four
+    bool fits = true;
+    for (int x0 = 0; x0 < ws && fits; x0 += LSD_SEG) {
+      const int nsc = std::min(LSD_SEG + 1, ws - x0);
+      for (int u0 = 0; u0 < nsc && fits; u0 += g->pw) {
+        const LsdPreFoot f = lsd_pre_foot(ox, oy, x0 + u0, x0 + std::min(u0 + g->pw, nsc) - 1, 0, 0, R);
+        fits = f.sx1 - f.bxc + 1 <= LSD_PRE_HW;
+      }
+    }
+    if (fits) break;
+    if (g->pw == 4) return false;
+  }
+  g->packed = plf_resize_packed_ok(w, ws);
   return true;
 }
 
@@ -1465,8 +1298,6 @@ static void lsd_set_sizes(const plf_ctx* ctx, LsdState* s, int w, int h, int nim
   s->hs = s->scale != 1.0 ? (int)nearbyint(h * s->scale) : h;
   s->max_regions = ctx->limits.max_segments;
   s->max_lines = ctx->limits.max_lines;
-  s->fused = s->scale != 1.0 && lsd_pre_fused_fits(ctx->params, w, h, s->ws, s->hs);
-  s->chain_maps = s->scale != 1.0 && !s->fused;
 }
 
 // Records of one record map: nimg images of pix_stride records, plus 3 rows + 8 records of slack on both sides (the
@@ -1477,14 +1308,8 @@ static size_t lsd_pix_records(const LsdState* s) { return s->pix_stride * s->nim
 // The device buffers of an LSD state whose sizes are set (lsd_set_sizes), and the layout derived from those sizes.
 static void lsd_buffers(LsdState* s, DevBufList& b) {
   const size_t N = (size_t)s->nimg, As = (size_t)s->ws * s->hs, R = (size_t)s->max_regions;
-  s->bp = plf_pitch16(s->w); s->sp = plf_pitch16(s->ws);
   s->nxb = (s->ws + LSD_SEG - 1) / LSD_SEG;
   s->pix_stride = As + (size_t)s->ws + 1;
-  // the hand-off maps of the three-kernel chain: listed for every state, empty where the chain does not run, so that the
-  // states of several image sizes list the same entries and share the largest (DevBufList::grow / lend); a size that runs
-  // fused borrows the maps another size needs and never touches them
-  b.add(s->blur, s->chain_maps ? (size_t)s->bp * s->h * N : 0);
-  b.add(s->scaled, s->chain_maps ? (size_t)s->sp * s->hs * N : 0);
   b.add(s->seedlist, As * N);
   b.add(s->segcnt, N * s->hs * s->nxb);
   b.add(s->rect_perm, N * R);
@@ -1504,12 +1329,19 @@ static void lsd_buffers(LsdState* s, DevBufList& b) {
     b.add(s->nlines[p], N);
   }
   b.add(s->overflow, 1);
-  if (s->scale != 1.0) {
-    s->rs_x_off = 0;
-    s->rs_y_off = 2 * (size_t)s->ws;
-    s->rs_xp_off = (s->rs_y_off + 2 * (size_t)s->hs + 3) & ~(size_t)3;   // 16-byte aligned: read with 128-bit loads
-    s->tabs.add(s->rs_tab, s->rs_xp_off + plf_resize_packed_len(s->ws));
-  }
+  s->rs_x_off = 0;
+  s->rs_y_off = 2 * (size_t)s->ws;
+  s->rs_xp_off = (s->rs_y_off + 2 * (size_t)s->hs + 3) & ~(size_t)3;   // 16-byte aligned: read with 128-bit loads
+  s->tabs.add(s->rs_tab, s->rs_xp_off + plf_resize_packed_len(s->ws));
+}
+
+// The resize tables of s (identity at scale 1), laid out as rs_tab (lsd_buffers).
+static std::vector<int> lsd_resize_tables(const LsdState* s) {
+  std::vector<int> tab(s->rs_xp_off + plf_resize_packed_len(s->ws));
+  plf_linear_coeffs_host(s->w, s->ws, 1.0 / s->scale, &tab[s->rs_x_off], &tab[s->rs_x_off + s->ws]);
+  plf_linear_coeffs_host(s->h, s->hs, 1.0 / s->scale, &tab[s->rs_y_off], &tab[s->rs_y_off + s->hs]);
+  plf_resize_pack_x(&tab[s->rs_x_off], &tab[s->rs_x_off + s->ws], s->ws, &tab[s->rs_xp_off]);
+  return tab;
 }
 
 size_t plf_lsd_footprint(const plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities) {
@@ -1533,8 +1365,10 @@ static plf_status lsd_tables_build(plf_ctx* ctx, LsdTables* t) {
   t->prec = LSD_PI * P.lsd_ang_th / 180;
   t->p = P.lsd_ang_th / 180;
   t->rho = P.lsd_quant / sin(t->prec);
-  lsd_blur_taps(P, &t->ksize, t->taps.k, &t->taps_u8);
-  if (t->ksize > 15) return plf_fail(ctx, PLF_ERR_INVALID, "LSD: Gaussian kernel %d > 15 unsupported", t->ksize);
+  int ksize, taps[LSD_PRE_KS_MAX];
+  lsd_blur_taps(P, &ksize, taps);
+  if (ksize > LSD_PRE_KS_MAX)
+    return plf_fail(ctx, PLF_ERR_INVALID, "LSD: Gaussian kernel %d > %d unsupported", ksize, LSD_PRE_KS_MAX);
   for (t->m2_min = 0; t->m2_min <= 2 * 510 * 510; ++t->m2_min)  // same double expression as the kernels
     if (!(sqrt((double)t->m2_min / 4.0) <= t->rho)) break;
   const size_t LUT = (size_t)LSD_LUT_DIM * LSD_LUT_DIM;
@@ -1570,14 +1404,17 @@ void plf_lsd_tables_free(plf_ctx* ctx) {
   ctx->lsd_tables = nullptr;
 }
 
-// The sizes of s for nimg images of w x h, checked, and its buffers listed (not allocated).  Host only.
-// chain_maps: also the maps of the three-kernel chain where the fused kernel runs (a test state that runs both).
-static plf_status lsd_layout(plf_ctx* ctx, LsdState* s, int w, int h, int nimg, bool two_parities, bool chain_maps = false) {
+// The sizes of s for nimg images of w x h, checked, its pre-grow launch chosen and its buffers listed (not allocated).
+// Host only.
+static plf_status lsd_layout(plf_ctx* ctx, LsdState* s, int w, int h, int nimg, bool two_parities) {
   lsd_set_sizes(ctx, s, w, h, nimg, two_parities);
-  s->chain_maps = s->chain_maps || (chain_maps && s->scale != 1.0);
   if (s->ws >= 65536 || s->hs >= 65536 || s->ws < 3 || s->hs < 3)
     return plf_fail(ctx, PLF_ERR_INVALID, "LSD: scaled image %dx%d out of range", s->ws, s->hs);
   lsd_buffers(s, s->bufs);
+  const std::vector<int> tab = lsd_resize_tables(s);
+  if (!lsd_pre_geom(ctx->params, w, s->ws, s->hs, &tab[s->rs_x_off], &tab[s->rs_y_off], &s->pre))
+    return plf_fail(ctx, PLF_ERR_INVALID, "LSD: lsd_scale %g with lsd_sigma_scale %g: one scaled row of %dx%d needs more source rows "
+                    "than the pre-grow tile holds", s->scale, ctx->params.lsd_sigma_scale, w, h);
   return PLF_OK;
 }
 
@@ -1595,13 +1432,8 @@ static plf_status lsd_ready(plf_ctx* ctx, LsdState* s) {
   plf_status st = s->tabs.alloc(ctx, "LSD");
   if (st) return st;
   for (int p = 0; p < (s->two_parities ? 2 : 1); ++p) s->pix[p] = s->pix_raw[p] + lsd_pix_pad(s);
-  if (s->scale != 1.0) {
-    std::vector<int> tab(s->rs_xp_off + plf_resize_packed_len(s->ws));
-    plf_linear_coeffs_host(s->w, s->ws, 1.0 / s->scale, &tab[0], &tab[s->ws]);
-    plf_linear_coeffs_host(s->h, s->hs, 1.0 / s->scale, &tab[s->rs_y_off], &tab[s->rs_y_off + s->hs]);
-    plf_resize_pack_x(&tab[0], &tab[s->ws], s->ws, &tab[s->rs_xp_off]);
-    PLF_CUDA(ctx, cudaMemcpyAsync(s->rs_tab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-  }
+  const std::vector<int> tab = lsd_resize_tables(s);
+  PLF_CUDA(ctx, cudaMemcpyAsync(s->rs_tab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
   PLF_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return PLF_OK;
 }
@@ -1609,14 +1441,14 @@ static plf_status lsd_ready(plf_ctx* ctx, LsdState* s) {
 // The states of n image sizes share one set of buffers, each sized for the largest of them.  Every record map is filled
 // with NOTDEF whole, guards and slack of every size's layout included; k_lsd_fill_notdef says why it stays so whichever
 // size the next batch has (DESIGN.md section 8).
-static plf_status lsd_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities, bool chain_maps, LsdState** out) {
+plf_status plf_lsd_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities, LsdState** out) {
   plf_status st = plf_lsd_tables(ctx);
   if (st) return st;
   std::vector<LsdState*> v(n, nullptr);
   size_t records = 0;
   for (int i = 0; i < n && !st; ++i) {
     v[i] = new LsdState();
-    st = lsd_layout(ctx, v[i], wh[2 * i], wh[2 * i + 1], nimg, two_parities, chain_maps);
+    st = lsd_layout(ctx, v[i], wh[2 * i], wh[2 * i + 1], nimg, two_parities);
     if (!st) records = std::max(records, lsd_pix_records(v[i]));
   }
   if (!st) {
@@ -1642,97 +1474,9 @@ static plf_status lsd_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg,
   return PLF_OK;
 }
 
-plf_status plf_lsd_create_sizes(plf_ctx* ctx, int n, const int* wh, int nimg, bool two_parities, LsdState** out) {
-  return lsd_create_sizes(ctx, n, wh, nimg, two_parities, false, out);
-}
-
 plf_status plf_lsd_create(plf_ctx* ctx, int w, int h, int nimg, bool two_parities, LsdState** out) {
   const int wh[2] = {w, h};
   return plf_lsd_create_sizes(ctx, 1, wh, nimg, two_parities, out);
-}
-
-// Tensor map of k_lsd_pre_fused over nimg source images: a row is viewed as 16-byte blocks, {16, blocks, rows, images},
-// so that one box spans LSD_PF_BOXW bytes of a row.  Encoded per call (host only, a few microseconds per batch).
-static bool lsd_pf_encode(CUtensorMap* map, const void* base, int w, int h, int nimg, size_t pitch, size_t img_stride) {
-  typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static encode_fn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess || !p) return false;
-    fn = (encode_fn)p;
-  }
-  if ((pitch & 15) || (img_stride & 15) || ((uintptr_t)base & 15) || (size_t)w > pitch) return false;
-  const cuuint64_t dims[4] = {16u, (cuuint64_t)((w + 15) / 16), (cuuint64_t)h, (cuuint64_t)nimg};
-  const cuuint64_t strides[3] = {16u, (cuuint64_t)pitch, (cuuint64_t)img_stride};
-  const cuuint32_t box[4] = {16u, (cuuint32_t)(LSD_PF_BOXW / 16), (cuuint32_t)LSD_PF_BOXH, 1u};
-  const cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-  return fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-// The records, seed lists, segcnt and maxmag2 of images [0, n) into record map `pix`: by k_lsd_pre_fused (fused, which
-// the state must allow: s->fused) or by the pre-blur, resample and gradient kernels (s->chain_maps, or scale 1: the
-// gradient alone).
-static plf_status lsd_pre_grad(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch,
-                               LsdPix* pix, int n, bool fused) {
-  const LsdTables& T = *ctx->lsd_tables;
-  const int w = s->w, h = s->h;
-  const int W = s->ws, H = s->hs;
-  const size_t As = (size_t)W * H, A = (size_t)s->bp * h, Asp = (size_t)s->sp * H;
-  PLF_CUDA(ctx, cudaMemsetAsync(s->maxmag2, 0xFF, (size_t)n * sizeof(int), cs));  // -1
-  uint32_t tA = 0, tB = 0;
-  for (int k = 0; k < T.ksize; ++k) (k < 4 ? tA : tB) |= (uint32_t)T.taps.k[k] << (8 * (k & 3));
-  if (fused) {
-    CUtensorMap tm;
-    if (!lsd_pf_encode(&tm, d_imgs, w, h, n, pitch, img_stride))
-      return plf_fail(ctx, PLF_ERR_CUDA, "LSD: cuTensorMapEncodeTiled failed for the source images (pitch %d, stride %zu)", pitch, img_stride);
-    const dim3 g(s->nxb, (H + LSD_PF_TH - 1) / LSD_PF_TH, n);
-    const int* tx = s->rs_tab + s->rs_x_off;
-    const int* ty = s->rs_tab + s->rs_y_off;
-    const int4* txp = reinterpret_cast<const int4*>(s->rs_tab + s->rs_xp_off);
-    if (T.ksize == 7)
-      k_lsd_pre_fused<7><<<g, LSD_PF_THREADS, 0, cs>>>(tm, w, h, W, H, tA, tB, tx, txp, ty, T.angle_lut, T.m2_min, As, pix, s->pix_stride,
-                                                       s->seedlist, s->segcnt, s->nxb, s->maxmag2);
-    else
-      k_lsd_pre_fused<5><<<g, LSD_PF_THREADS, 0, cs>>>(tm, w, h, W, H, tA, tB, tx, txp, ty, T.angle_lut, T.m2_min, As, pix, s->pix_stride,
-                                                       s->seedlist, s->segcnt, s->nxb, s->maxmag2);
-    PLF_LAUNCH_CHECK(ctx);
-    plf_mark(ctx, cs, "lsd.k_lsd_pre_fused");
-    return PLF_OK;
-  }
-  const uint8_t* scaled = d_imgs;
-  size_t scaled_stride = img_stride;
-  int scaled_pitch = pitch;
-  if (s->scale != 1.0) {
-    if ((T.ksize == 7 || T.ksize == 5) && T.taps_u8) {
-      const CUtensorMap* tm = s->tm_blur.get(d_imgs, w, h, n, pitch, img_stride, 80, BF_TH + T.ksize - 1);
-      if (!tm)
-        return plf_fail(ctx, PLF_ERR_CUDA, "LSD: cuTensorMapEncodeTiled failed for the source images (pitch %d, stride %zu)", pitch, img_stride);
-      dim3 gf(plf_tma_tiles_x(w, T.ksize / 2), (h + BF_TH - 1) / BF_TH, n);
-      if (T.ksize == 7) k_blur_q8_fast<7><<<gf, 256, 0, cs>>>(*tm, 0, w, h, tA, tB, s->blur, A, s->bp);
-      else k_blur_q8_fast<5><<<gf, 256, 0, cs>>>(*tm, 0, w, h, tA, tB, s->blur, A, s->bp);
-    } else {
-      dim3 gb((w + BQ_TW - 1) / BQ_TW, (h + BQ_TH - 1) / BQ_TH, n);
-      k_blur_q8<<<gb, 256, 0, cs>>>(d_imgs, img_stride, pitch, w, h, T.ksize / 2, s->blur, A, s->bp, T.taps);
-    }
-    PLF_LAUNCH_CHECK(ctx);
-    plf_mark(ctx, cs, "lsd.k_blur_q8");
-    const plf_status st = plf_launch_resize_exact(ctx, cs, s->blur, A, s->bp, w, h, s->scaled, Asp, s->sp, W, H, s->rs_tab + s->rs_x_off,
-                                                  s->rs_tab + s->rs_xp_off, s->rs_tab + s->rs_y_off, n);
-    if (st) return st;
-    plf_mark(ctx, cs, "lsd.k_resize_exact");
-    scaled = s->scaled;
-    scaled_stride = Asp;
-    scaled_pitch = s->sp;
-  }
-  k_lsd_grad<<<dim3(s->nxb, (H + 1) / 2, n), LSD_GRAD_THREADS, 0, cs>>>(scaled, scaled_stride, scaled_pitch, W, H, T.angle_lut, T.m2_min, As, pix, s->pix_stride,
-                                                               s->seedlist, s->segcnt, s->nxb, s->maxmag2);
-  PLF_LAUNCH_CHECK(ctx);
-  plf_mark(ctx, cs, "lsd.k_lsd_grad");
-  return PLF_OK;
 }
 
 // LSD on images [0, n) of a batch resident on the device, in two phases so that callers can overlap them with other
@@ -1741,11 +1485,26 @@ static plf_status lsd_pre_grad(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const
 // hold >= n images.  Enqueued on cs; results stay on the device.
 plf_status plf_lsd_pre(plf_ctx* ctx, cudaStream_t cs, LsdState* s, const uint8_t* d_imgs, size_t img_stride, int pitch, int par, int n) {
   if (s->nimg < n) return plf_fail(ctx, PLF_ERR_STATE, "plf_lsd_pre: %d images > the state's %d", n, s->nimg);
+  const LsdTables& T = *ctx->lsd_tables;
+  const LsdPreGeom& g = s->pre;
   const int W = s->ws, H = s->hs;
   const size_t As = (size_t)W * H;
   LsdPix* pix = s->pix[par] + (s->ws + 1);  // pixel (0,0) of the first image
-  const plf_status st = lsd_pre_grad(ctx, cs, s, d_imgs, img_stride, pitch, pix, n, s->fused);
-  if (st) return st;
+  // the tensor map is encoded per call (host only, a few microseconds per batch)
+  CUtensorMap tm;
+  if (!plf_tma_encode_u8_blocks(&tm, d_imgs, s->w, s->h, n, pitch, img_stride, LSD_PRE_BOXW / 16, LSD_PRE_BOXH))
+    return plf_fail(ctx, PLF_ERR_CUDA, "LSD: cuTensorMapEncodeTiled failed for the source images (pitch %d, stride %zu)", pitch, img_stride);
+  PLF_CUDA(ctx, cudaMemsetAsync(s->maxmag2, 0xFF, (size_t)n * sizeof(int), cs));  // -1
+  // no 3-tap kernel: its side tap (sigma <= 0.27) rounds to 0, so it is the copy KS = 1 runs
+  static const decltype(&k_lsd_pre<1>) kern[] = {k_lsd_pre<1>, nullptr, k_lsd_pre<5>, k_lsd_pre<7>,
+                                                 k_lsd_pre<9>, k_lsd_pre<11>, k_lsd_pre<13>, k_lsd_pre<15>};
+  static_assert(sizeof kern / sizeof kern[0] == LSD_PRE_KS_MAX / 2 + 1, "one entry per odd KS");
+  const size_t smem = g.np > 1 ? (size_t)(g.th + 1) * LSD_PRE_SP : 0;
+  kern[g.ks / 2]<<<dim3(s->nxb, (H + g.th - 1) / g.th, n), LSD_PRE_THREADS, smem, cs>>>(
+      tm, s->w, s->h, W, H, g, s->rs_tab + s->rs_x_off, reinterpret_cast<const int4*>(s->rs_tab + s->rs_xp_off),
+      s->rs_tab + s->rs_y_off, T.angle_lut, T.m2_min, As, pix, s->pix_stride, s->seedlist, s->segcnt, s->nxb, s->maxmag2);
+  PLF_LAUNCH_CHECK(ctx);
+  plf_mark(ctx, cs, "lsd.k_lsd_pre");
   k_lsd_seed_order<<<n, LSD_SO_THREADS, lsd_seed_order_smem(s->n_bins), cs>>>(s->seedlist, s->segcnt, As, W, H, s->nxb, s->n_bins,
                                                                               s->maxmag2, s->order[par], s->nseeds[par]);
   PLF_LAUNCH_CHECK(ctx);
@@ -1958,25 +1717,22 @@ extern "C" plf_status plf_debug_sincosf(plf_ctx* ctx, const float* in, float* s,
   return PLF_OK;
 }
 
-// The gradient stage of LSD (records, seed lists, segcnt, maxmag2) of n source images, by k_lsd_pre_fused (fused = 1) or
-// by the pre-blur, resample and gradient kernels (fused = 0), in a state of its own: tests compare the two byte for byte.
+// The gradient stage of LSD (records, seed lists, segcnt, maxmag2) of n source images by k_lsd_pre, in a state of its
+// own: tests compare it byte for byte with a CPU reference.
 extern "C" plf_status plf_debug_lsd_pre(plf_ctx* ctx, const uint8_t* imgs, int n, int w, int h, int pitch, size_t img_stride,
-                                        int fused, int* sizes, uint32_t* pix, uint32_t* seedlist, int* segcnt, int* maxmag2) {
+                                        int* sizes, uint32_t* pix, uint32_t* seedlist, int* segcnt, int* maxmag2) {
   if (!ctx || n < 1 || w < 3 || h < 3 || pitch < w || (pitch & 15) || img_stride < (size_t)pitch * h || (img_stride & 15) || !sizes)
     return plf_fail(ctx, PLF_ERR_INVALID, "plf_debug_lsd_pre: bad arguments");
   PLF_CUDA(ctx, cudaSetDevice(ctx->device));
   LsdState* s = nullptr;
   const int wh[2] = {w, h};
-  plf_status st = lsd_create_sizes(ctx, 1, wh, n, false, true, &s);
+  plf_status st = plf_lsd_create_sizes(ctx, 1, wh, n, false, &s);
   if (st) return st;
-  sizes[0] = s->ws; sizes[1] = s->hs; sizes[2] = s->nxb; sizes[3] = s->fused;
+  const int sz[6] = {s->ws, s->hs, s->nxb, s->pre.ks, s->pre.th, s->pre.np};
+  std::copy(sz, sz + 6, sizes);
   if (!imgs || !pix || !seedlist || !segcnt || !maxmag2) {   // sizes only
     plf_lsd_free(s);
     return PLF_OK;
-  }
-  if (fused && !s->fused) {
-    plf_lsd_free(s);
-    return plf_fail(ctx, PLF_ERR_INVALID, "plf_debug_lsd_pre: the fused kernel does not apply to %dx%d at these parameters", w, h);
   }
   const size_t As = (size_t)s->ws * s->hs, nseg = (size_t)n * s->hs * s->nxb;
   uint8_t* dimg = nullptr;
@@ -1987,7 +1743,7 @@ extern "C" plf_status plf_debug_lsd_pre(plf_ctx* ctx, const uint8_t* imgs, int n
               cudaMemsetAsync(s->seedlist, 0, As * n * sizeof(uint32_t), ctx->stream) != cudaSuccess ||
               cudaMemsetAsync(s->segcnt, 0, nseg * sizeof(int), ctx->stream) != cudaSuccess))
     st = plf_fail(ctx, PLF_ERR_CUDA, "plf_debug_lsd_pre: upload failed");
-  if (!st) st = lsd_pre_grad(ctx, ctx->stream, s, dimg, img_stride, pitch, s->pix[0] + (s->ws + 1), n, fused != 0);
+  if (!st) st = plf_lsd_pre(ctx, ctx->stream, s, dimg, img_stride, pitch, 0, n);
   if (!st && (cudaMemcpy2DAsync(pix, As * sizeof(LsdPix), s->pix[0] + (s->ws + 1), s->pix_stride * sizeof(LsdPix), As * sizeof(LsdPix), n,
                                 cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
               cudaMemcpyAsync(seedlist, s->seedlist, As * n * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||

@@ -159,7 +159,7 @@ void plf_resize_pack_x(const int* ofs, const int* c1, int dw, int* out) {
 
 plf_status plf_launch_resize_exact(plf_ctx* ctx, cudaStream_t cs, const uint8_t* src, size_t src_stride, int sp, int sw, int sh, uint8_t* dst,
                                    size_t dst_stride, int dp, int dw, int dh, const int* tabx, const int* tabxp, const int* taby, int nimg) {
-  if ((double)sw <= 1.9 * (double)dw) {  // four outputs span at most 3 * 1.9 + 2 < 8 source columns
+  if (plf_resize_packed_ok(sw, dw)) {
     dim3 grid((dw + 255) / 256, (dh + 3) / 4, nimg);
     k_resize_exact4<<<grid, dim3(64, 4), 0, cs>>>(src, src_stride, sp, sw, sh, dst, dst_stride, dp, dw, dh,
                                                   reinterpret_cast<const int4*>(tabxp), taby);

@@ -384,6 +384,9 @@ void plf_linear_coeffs_host(int srcsize, int dstsize, double scale, int* ofs, in
 plf_status plf_launch_resize_exact(plf_ctx* ctx, cudaStream_t cs, const uint8_t* src, size_t src_stride, int sp, int sw, int sh, uint8_t* dst,
                                    size_t dst_stride, int dp, int dw, int dh, const int* tabx, const int* tabxp, const int* taby, int nimg);
 size_t plf_resize_packed_len(int dw);                                 // ints of the packed x table of k_resize_exact4
+// k_resize_exact4's form (four outputs from an 8-byte source window) applies: four outputs span at most 3 * 1.9 + 2 < 8
+// source columns
+static inline bool plf_resize_packed_ok(int sw, int dw) { return (double)sw <= 1.9 * (double)dw; }
 void plf_resize_pack_x(const int* ofs, const int* c1, int dw, int* out);   // out: 16-byte aligned
 
 // ---- LSD (lsd.cu) --------------------------------------------------------------------------------

@@ -20,27 +20,49 @@ static inline int plf_pitch16(int w) { return (w + 15) & ~15; }
 // number of 64-column tiles when the tile grid is shifted left by (16 - R) columns (see above)
 static inline int plf_tma_tiles_x(int w, int R) { return (w + (16 - R) + 63) / 64; }
 
-// Host: tensor map over nimg images of w x h bytes, row pitch `pitch`, image stride `img_stride` (both multiples of
-// 16), box = box_w x box_h x 1 (box_w a multiple of 16).  The driver entry point is resolved through the runtime so
-// that the library keeps linking against the static CUDA runtime only.
-static inline bool plf_tma_encode_u8(CUtensorMap* map, const void* base, int w, int h, int nimg, size_t pitch,
-                                     size_t img_stride, int box_w, int box_h) {
-  typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static encode_fn fn = nullptr;
+// Host: cuTensorMapEncodeTiled, resolved through the runtime so that the library keeps linking against the static CUDA
+// runtime only (nullptr if the driver has no such entry point).
+typedef CUresult (*plf_tma_encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                      const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                      CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+static inline plf_tma_encode_fn plf_tma_encoder() {
+  static plf_tma_encode_fn fn = nullptr;
   if (!fn) {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess || !p) return false;
-    fn = (encode_fn)p;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess || !p) return nullptr;
+    fn = (plf_tma_encode_fn)p;
   }
-  if ((pitch & 15) || (img_stride & 15) || (box_w & 15) || ((uintptr_t)base & 15) || box_w > 256 || box_h > 256) return false;
+  return fn;
+}
+
+// Host: tensor map over nimg images of w x h bytes, row pitch `pitch`, image stride `img_stride` (both multiples of
+// 16), box = box_w x box_h x 1 (box_w a multiple of 16).
+static inline bool plf_tma_encode_u8(CUtensorMap* map, const void* base, int w, int h, int nimg, size_t pitch,
+                                     size_t img_stride, int box_w, int box_h) {
+  const plf_tma_encode_fn fn = plf_tma_encoder();
+  if (!fn || (pitch & 15) || (img_stride & 15) || (box_w & 15) || ((uintptr_t)base & 15) || box_w > 256 || box_h > 256) return false;
   const cuuint64_t dims[3] = {(cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)nimg};
   const cuuint64_t strides[2] = {(cuuint64_t)pitch, (cuuint64_t)img_stride};
   const cuuint32_t box[3] = {(cuuint32_t)box_w, (cuuint32_t)box_h, 1u};
   const cuuint32_t estr[3] = {1u, 1u, 1u};
   return fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// Host: the same images viewed as rows of 16-byte blocks, {16 bytes, blocks, rows, images}, so that a box can span more
+// than the 256 elements one box dimension holds: box = 16 x box_blocks x box_h x 1, loaded with plf_tma_load_4d at
+// coordinates {0, x / 16, y, image}.
+static inline bool plf_tma_encode_u8_blocks(CUtensorMap* map, const void* base, int w, int h, int nimg, size_t pitch,
+                                            size_t img_stride, int box_blocks, int box_h) {
+  const plf_tma_encode_fn fn = plf_tma_encoder();
+  if (!fn || (pitch & 15) || (img_stride & 15) || ((uintptr_t)base & 15) || (size_t)w > pitch || box_blocks > 256 || box_h > 256)
+    return false;
+  const cuuint64_t dims[4] = {16u, (cuuint64_t)((w + 15) / 16), (cuuint64_t)h, (cuuint64_t)nimg};
+  const cuuint64_t strides[3] = {16u, (cuuint64_t)pitch, (cuuint64_t)img_stride};
+  const cuuint32_t box[4] = {16u, (cuuint32_t)box_blocks, (cuuint32_t)box_h, 1u};
+  const cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
+  return fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
@@ -93,6 +115,20 @@ __device__ __forceinline__ void plf_tma_load_3d(void* smem_dst, const CUtensorMa
       "l"(map), "r"(x), "r"(y), "r"(z), "r"(b)
       : "memory");
 }
+// One thread: expect `bytes`, then issue the 4-D box load of a plf_tma_encode_u8_blocks map.
+__device__ __forceinline__ void plf_tma_load_4d(void* smem_dst, const CUtensorMap* map, int c0, int c1, int c2, int c3,
+                                                uint64_t* bar, uint32_t bytes) {
+  const uint32_t b = plf_smem_u32(bar);
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(b), "r"(bytes) : "memory");
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];" ::"r"(
+          plf_smem_u32(smem_dst)),
+      "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(b)
+      : "memory");
+}
+// Every thread that wrote shared memory which a later box load overwrites: order those writes before the load (the
+// load is issued after a __syncthreads that follows this fence).
+__device__ __forceinline__ void plf_fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // All threads: wait for phase `parity` of the barrier.
 __device__ __forceinline__ void plf_mbar_wait(uint64_t* bar, uint32_t parity) {
   const uint32_t b = plf_smem_u32(bar);

@@ -1228,25 +1228,35 @@ class Frontend:
         self._check(st, "plf_debug_sincosf")
         return s, c
 
-    def debug_lsd_pre(self, imgs, fused, pitch=None, img_stride=None, pad_byte=0xA5):
-        """LSD's gradient stage on the (n, h, w) uint8 images, by the fused pre-blur + resample + gradient kernel
-        (fused=True) or by the three kernels it replaces.  The images are laid out with row pitch `pitch` and image
-        stride `img_stride` bytes (multiples of 16; default: the pipeline's) and the padding filled with pad_byte.
-        Returns dict(pix=(n, hs*ws) uint64 records, seedlist=(n, hs*ws) uint32, segcnt=(n, hs, nxb) int32,
-        maxmag2=(n,) int32, fused_applies=bool); fused_applies alone (no run) when fused is None."""
+    def _debug_lsd_pre(self, n, w, h, pitch, img_stride, bufs=(None,) * 5):
+        """plf_debug_lsd_pre on bufs = (images, pix, seedlist, segcnt, maxmag2); all None: the launch only."""
+        f = self.lib.plf_debug_lsd_pre
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p,
+                      C.c_void_p, C.c_void_p, C.c_void_p]
+        sizes = np.zeros(6, np.int32)
+        ptrs = [None if a is None else a.ctypes.data for a in bufs]
+        self._check(f(self._ctx, ptrs[0], n, w, h, pitch, img_stride, sizes.ctypes.data, *ptrs[1:]), "plf_debug_lsd_pre")
+        return dict(zip(("ws", "hs", "nxb", "ks", "th", "np"), (int(v) for v in sizes)))
+
+    def debug_lsd_pre_geometry(self, w, h):
+        """The launch LSD's pre-grow kernel takes for w x h images at this context's parameters: dict(ws, hs, nxb, ks, th,
+        np) - the scaled size, the 512-column segments per row, the pre-blur's taps (1: none), the scaled rows per CTA
+        and the column pieces per segment."""
+        pitch = (w + 15) // 16 * 16
+        return self._debug_lsd_pre(1, w, h, pitch, pitch * h)
+
+    def debug_lsd_pre(self, imgs, pitch=None, img_stride=None, pad_byte=0xA5):
+        """LSD's gradient stage on the (n, h, w) uint8 images, by the pre-blur + resample + gradient kernel.  The images
+        are laid out with row pitch `pitch` and image stride `img_stride` bytes (multiples of 16; default: the
+        pipeline's) and the padding filled with pad_byte.  Returns dict(pix=(n, hs*ws) uint64 records,
+        seedlist=(n, hs*ws) uint32, segcnt=(n, hs, nxb) int32, maxmag2=(n,) int32) and the launch
+        (debug_lsd_pre_geometry's keys)."""
         imgs = np.ascontiguousarray(imgs, np.uint8)
         n, h, w = imgs.shape
         pitch = pitch or (w + 15) // 16 * 16
         img_stride = img_stride or pitch * h
-        sizes = np.zeros(4, np.int32)
-        f = self.lib.plf_debug_lsd_pre
-        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_int, C.c_void_p,
-                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        self._check(f(self._ctx, None, n, w, h, pitch, img_stride, 0, sizes.ctypes.data, None, None, None, None),
-                    "plf_debug_lsd_pre")
-        ws, hs, nxb, applies = (int(v) for v in sizes)
-        if fused is None:
-            return dict(fused_applies=bool(applies))
+        geo = self.debug_lsd_pre_geometry(w, h)
+        ws, hs, nxb = geo["ws"], geo["hs"], geo["nxb"]
         buf = np.full(n * img_stride, pad_byte, np.uint8)
         for i in range(n):
             v = buf[i * img_stride:i * img_stride + pitch * h].reshape(h, pitch)
@@ -1255,10 +1265,8 @@ class Frontend:
         seed = np.empty((n, hs * ws), np.uint32)
         seg = np.empty((n, hs, nxb), np.int32)
         mm = np.empty(n, np.int32)
-        st = f(self._ctx, buf.ctypes.data, n, w, h, pitch, img_stride, int(bool(fused)), sizes.ctypes.data, pix.ctypes.data,
-               seed.ctypes.data, seg.ctypes.data, mm.ctypes.data)
-        self._check(st, "plf_debug_lsd_pre")
-        return dict(pix=pix, seedlist=seed, segcnt=seg, maxmag2=mm, fused_applies=bool(applies))
+        self._debug_lsd_pre(n, w, h, pitch, img_stride, (buf, pix, seed, seg, mm))
+        return dict(geo, pix=pix, seedlist=seed, segcnt=seg, maxmag2=mm)
 
     def debug_ldlt(self, S, g, path=0, overwrite_s=False):
         """LDL^T without pivoting of the symmetric S (6 n6 x 6 n6, lower triangle read) and the solution of S x = g, by

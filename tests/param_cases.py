@@ -116,6 +116,17 @@ def lsd_ksize(prm):
     return 1 + 2 * math.ceil(sigma * math.sqrt(6 * math.log(10)))
 
 
+def lsd_pre_ks(prm):
+    """The taps LSD's pre-grow kernel blurs with for prm (its template argument): lsd_ksize, or 1 at scale 1 and where the
+    Q8 centre tap is 256 (every side tap 0: the blur is a copy)."""
+    from oracle import clib
+    ks = lsd_ksize(prm)
+    if ks == 0:
+        return 1
+    scale, sigma = prm.get("lsd_scale", 1.2), prm.get("lsd_sigma_scale", 0.6)
+    return 1 if clib.gaussian_kernel_q8(ks, sigma / scale if scale < 1 else sigma)[ks // 2] == 256 else ks
+
+
 # one change at a time through the whole pipeline.  base: the run the change is measured against ({} = the defaults);
 # moves: what the change must visibly alter there, so that no case is vacuous - "stereo" = n_stereo_pt / n_stereo_ls,
 # "pose" = the GN iteration counts or the pose by more than the parity tolerance.

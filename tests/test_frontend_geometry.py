@@ -23,11 +23,12 @@ from pathlib import Path
 import numpy as np
 import pytest
 
-from param_cases import LSD_CASES, ORB_CASES, lsd_ksize
+from param_cases import LSD_CASES, ORB_CASES, lsd_ksize, lsd_pre_ks
 
 CSRC = Path(__file__).resolve().parent.parent / "pl-slam_b200" / "csrc"
 TILE_NAMES = ("FN_OW", "FN_OH", "OBF_TW", "OBF_TH", "ORB_TW", "ORB_TH", "BF_TW", "BF_TH", "BQ_TW", "BQ_TH",
-              "LBF_TW", "LBF_TH", "LBD_TW", "LBD_TH")
+              "LBF_TW", "LBF_TH", "LBD_TW", "LBD_TH", "LSD_SEG", "LSD_PRE_TH", "LSD_PRE_BOXW", "LSD_PRE_BOXH", "LSD_PRE_HW",
+              "LSD_PRE_KS_MAX")
 
 
 def tile_consts():
@@ -45,7 +46,6 @@ T = tile_consts()
 ORB_BLUR_R = 3                       # k_orb_blur7_fast: 7 x 7 Gaussian
 LBD_R = 3                            # k_blur5_sobel_fast: 5 x 5 blur + 3 x 3 Sobel
 LSD_RADII = sorted({lsd_ksize(c) // 2 for c in [{}, *LSD_CASES.values()] if lsd_ksize(c)})
-LSD_FAST_RADII = [r for r in LSD_RADII if 2 * r + 1 in (5, 7)]   # the TMA blur (k_blur_q8_fast); others: k_blur_q8
 ORB_MIN_EDGE = 19
 
 
@@ -57,10 +57,7 @@ def tma_tiles_x(w, r):
 
 # shifted TMA blur tiles: (tile width, tile height, box width RP, columns read NEED, radius)
 def shifted_kernels():
-    ks = {"orb_blur7": (T["OBF_TW"], T["OBF_TH"], 80, 72, ORB_BLUR_R), "lbd_blur5_sobel": (T["LBF_TW"], T["LBF_TH"], 80, 76, LBD_R)}
-    for r in LSD_FAST_RADII:
-        ks[f"lsd_blur{2 * r + 1}"] = (T["BF_TW"], T["BF_TH"], 80, 72, r)
-    return ks
+    return {"orb_blur7": (T["OBF_TW"], T["OBF_TH"], 80, 72, ORB_BLUR_R), "lbd_blur5_sobel": (T["LBF_TW"], T["LBF_TH"], 80, 76, LBD_R)}
 
 
 def reflect101(i, n):
@@ -185,19 +182,21 @@ def orb_ok(w, h, nlevels=4, edge=ORB_MIN_EDGE, scale_factor=1.2):
 
 # ---- the sweep -----------------------------------------------------------------------------------------------------
 def x_boundaries():
-    """{kind: widths}: k T and k T +- 1 of the unshifted tile grids (FAST, the generic LSD / LBD blurs), 64 k - (16 - R)
-    and +- 1 of the shifted ones."""
+    """{kind: widths}: k T and k T +- 1 of the unshifted tile grids (FAST, the generic LBD blur, the sweep's LSD grid BQ),
+    64 k - (16 - R) and +- 1 of the shifted ones (and of the sweep's shifted LSD grid BF at the 5- and 7-tap radii)."""
     out = {}
     for name, t in (("FN_OW", T["FN_OW"]), ("BQ_TW", T["BQ_TW"]), ("LBD_TW", T["LBD_TW"])):
         out[name] = sorted({k * t + d for k in (1, 2) for d in (-1, 0, 1)})
-    for name, (TW, _, _, _, R) in shifted_kernels().items():
+    grids = {name: (TW, R) for name, (TW, _, _, _, R) in shifted_kernels().items()}
+    grids.update({f"BF_TW_r{r}": (T["BF_TW"], r) for r in (2, 3)})
+    for name, (TW, R) in grids.items():
         out[name] = sorted({TW * k - (16 - R) + d for k in (1, 2, 3) for d in (-1, 0, 1)})
     return out
 
 
 def y_boundaries():
     out = {}
-    for name in ("FN_OH", "OBF_TH", "BF_TH", "BQ_TH", "LBF_TH", "LBD_TH"):
+    for name in ("FN_OH", "OBF_TH", "BF_TH", "BQ_TH", "LSD_PRE_TH", "LBF_TH", "LBD_TH"):
         out[name] = sorted({k * T[name] + d for k in (1, 2, 3) for d in (-1, 0, 1)})
     return out
 
@@ -323,7 +322,8 @@ def test_tile_constants_read_from_the_kernels():
     assert T["FN_OW"] < 64 and T["FN_OH"] < 32          # the FAST tile + its 1-pixel NMS halo fits the 64 x 32 score tile
     for name, (TW, TH, RP, NEED, R) in shifted_kernels().items():
         assert TW == 64 and RP % 16 == 0 and NEED <= RP and TW + 2 * R <= NEED, name
-    assert LSD_FAST_RADII == [2, 3] and max(LSD_RADII) >= 4
+    assert T["LSD_PRE_BOXW"] % 16 == 0 and T["LSD_PRE_HW"] + 2 * max(LSD_RADII) <= T["LSD_PRE_BOXW"]
+    assert max(LSD_RADII) == T["LSD_PRE_KS_MAX"] // 2
 
 
 def test_sweep_covers_residues_and_boundaries():
@@ -341,7 +341,7 @@ def test_sweep_covers_residues_and_boundaries():
         assert all(k * t + d in ws for k in (1, 2) for d in (-1, 0, 1)), t
     for _, (TW, _, _, _, R) in shifted_kernels().items():
         assert all(TW * k - (16 - R) + d in ws for k in (1, 2, 3) for d in (-1, 0, 1)), R
-    for t in (T["FN_OH"], T["OBF_TH"], T["BF_TH"], T["BQ_TH"], T["LBF_TH"], T["LBD_TH"]):
+    for t in (T["FN_OH"], T["OBF_TH"], T["BF_TH"], T["BQ_TH"], T["LSD_PRE_TH"], T["LBF_TH"], T["LBD_TH"]):
         assert all(k * t + d in hs for k in (1, 2, 3) for d in (-1, 0, 1)), t
     assert max(max(s) for s in shapes) <= 320
 
@@ -395,7 +395,6 @@ def test_tile_model_every_shape():
             names = ["orb_blur7"] if orb_ok(lw, lh, 1) else []
             if lw >= 8 and lh >= 8:
                 names.append("lbd_blur5_sobel")    # smaller images take the generic LBD kernel (reflect on load)
-            names += [f"lsd_blur{2 * r + 1}" for r in LSD_FAST_RADII]
             for name in names:
                 check_shifted_kernel(name, lw, lh)
                 n += 1
@@ -435,6 +434,94 @@ def test_resize_tables_every_level(built):
     for sw, dw in sorted(pairs):
         check_resize_exact4(sw, dw)
     assert any(dw % 4 for _, dw in pairs) and any(dw % 4 == 0 for _, dw in pairs)
+
+
+# ---- the LSD pre-grow kernel's boxes (k_lsd_pre, lsd_pre_geom) -------------------------------------------------------
+def lsd_tables(s, d, scale):
+    """The LSD resample table of one axis as the library builds it (plf_linear_coeffs_host at 1 / scale): ofs."""
+    coeffs = _plf_lib()["_Z22plf_linear_coeffs_hostiidPiS_"]
+    coeffs.argtypes = [C.c_int, C.c_int, C.c_double, C.c_void_p, C.c_void_p]
+    ofs, c1 = np.zeros(d, np.int32), np.zeros(d, np.int32)
+    coeffs(s, d, 1.0 / scale, ofs.ctypes.data, c1.ctypes.data)
+    return ofs
+
+
+def lsd_pre_foot(ox, oy, xa, xl, ya, yl, R):
+    """lsd_pre_foot: (bxc, sx1, sy0, sy1)"""
+    return ((int(ox[xa]) - R) & ~15) + R, int(ox[xl]) + 1, int(oy[ya]), int(oy[yl]) + 1
+
+
+def lsd_pre_launch(ox, oy, W, H, R):
+    """lsd_pre_geom's TH, NP and PW: the most rows and the fewest pieces whose footprints fit the box."""
+    th = next(t for t in range(T["LSD_PRE_TH"], 0, -1)
+              if all(lsd_pre_foot(ox, oy, 0, 0, y0, min(y0 + t, H - 1), R)[3] - oy[y0] + 1 + 2 * R <= T["LSD_PRE_BOXH"]
+                     for y0 in range(0, H, t)))
+    seg = T["LSD_SEG"]
+    for np_ in range(1, seg + 2):
+        pw = ((seg + np_) // np_ + 3) & ~3
+        ok = True
+        for x0 in range(0, W, seg):
+            nsc = min(seg + 1, W - x0)
+            for u0 in range(0, nsc, pw):
+                bxc, sx1, _, _ = lsd_pre_foot(ox, oy, x0 + u0, x0 + min(u0 + pw, nsc) - 1, 0, 0, R)
+                ok = ok and sx1 - bxc + 1 <= T["LSD_PRE_HW"]
+        if ok:
+            return th, np_, pw
+    raise AssertionError("no piece count fits")
+
+
+def check_lsd_pre(w, h, scale, R):
+    """Every piece of every CTA of k_lsd_pre over a w x h image: its box starts on a 16-byte boundary, the blurred columns
+    and rows the resample reads (ofs, ofs + 1) and their blur halo lie inside the box, the packed resample's 12-byte read
+    lies inside the blurred tile's row, and every cell outside the image among those the blur reads is rebuilt from a
+    mirror cell inside the box (so it holds its BORDER_REFLECT_101 pixel).  Returns (TH, NP)."""
+    W, H = (w, h) if scale == 1.0 else (int(np.rint(w * scale)), int(np.rint(h * scale)))
+    if W < 3 or H < 3:
+        return None
+    ox, oy = lsd_tables(w, W, scale), lsd_tables(h, H, scale)
+    th, np_, pw = lsd_pre_launch(ox, oy, W, H, R)
+    BW, BH, seg = T["LSD_PRE_BOXW"], T["LSD_PRE_BOXH"], T["LSD_SEG"]
+    for X0 in range(0, W, seg):
+        nsc = min(seg + 1, W - X0)
+        for Y0 in range(0, H, th):
+            nsr = min(th + 1, H - Y0)
+            for u0 in range(0, nsc, pw):
+                u1 = min(u0 + pw, nsc)
+                bxc, sx1, sy0, sy1 = lsd_pre_foot(ox, oy, X0 + u0, X0 + u1 - 1, Y0, min(Y0 + th, H - 1), R)
+                gx0, gy0 = bxc - R, sy0 - R
+                assert gx0 % 16 == 0, (w, h, scale, X0, u0)
+                ncol, nrow = sx1 - bxc + 1, sy1 - sy0 + 1
+                need_w, need_h = ncol + 2 * R, nrow + 2 * R
+                assert ncol <= T["LSD_PRE_HW"] and need_w <= BW and need_h <= BH, (w, h, scale, X0, Y0, u0)
+                cols, rows = ox[X0 + u0:X0 + u1], oy[Y0:Y0 + nsr]
+                assert cols.min() >= bxc and cols.max() + 1 <= sx1 and rows.min() >= sy0 and rows.max() + 1 <= sy1
+                assert ((cols - bxc) // 4 * 4 + 12 <= BW).all()    # packed form: three words from the aligned word below ofs
+                if gx0 >= 0 and gx0 + need_w <= w and gy0 >= 0 and gy0 + need_h <= h:
+                    continue
+                mx = reflect101(gx0 + np.arange(need_w), w) - gx0
+                my = reflect101(gy0 + np.arange(need_h), h) - gy0
+                assert mx.min() >= 0 and mx.max() < BW and my.min() >= 0 and my.max() < need_h, (w, h, scale, X0, Y0, u0)
+                raw = reflect_fix_model(gx0, gy0, w, h, need_h, BW, need_w)
+                want = (gy0 + my)[:, None] * w + (gx0 + mx)[None, :]
+                bad = np.argwhere(raw[:, :need_w] != want)
+                assert len(bad) == 0, (w, h, scale, X0, Y0, u0, bad[:4].tolist())
+    return th, np_
+
+
+def test_lsd_pre_boxes_every_shape(built):
+    """check_lsd_pre for every sweep shape, the tiny LSD sizes and a KITTI-class frame at the default and every LSD case's
+    scale and radius (LSD_CASES, test_lsd_pre_gpu's LSD_PRE_CASES); the defaults keep TH 16 and one piece, downsampling takes several."""
+    from test_lsd_pre_gpu import LSD_PRE_CASES
+    settings = {(c.get("lsd_scale", 1.2), lsd_pre_ks(c) // 2) for c in [{}, *LSD_CASES.values(), *LSD_PRE_CASES.values()]}
+    assert (1.2, 3) in settings and (1.0, 0) in settings and max(r for _, r in settings) == T["LSD_PRE_KS_MAX"] // 2
+    launches = {}
+    for w, h in sorted(set(sweep_shapes()) | set(LSD_TINY) | {(1241, 376), (853, 35)}):
+        for scale, R in sorted(settings):
+            got = check_lsd_pre(w, h, scale, R)
+            if got:
+                launches.setdefault((scale, R), set()).add(got)
+    assert launches[(1.2, 3)] == {(16, 1)}
+    assert max(p for _, p in launches[(0.5, 5)]) > 1 and max(p for _, p in launches[(0.35, 7)]) > 1
 
 
 # ---- the C restatements against cv2 at the new shapes ----------------------------------------------------------------

@@ -66,6 +66,12 @@ def test_reference_configs_are_complete():
 
 
 def test_lsd_cases_cover_every_blur_kernel():
-    """k_blur_q8_fast<5>, <7> and the generic k_blur_q8 at 3, 9, 11 and 15 taps all run in some LSD case."""
+    """The Gaussian kernels of 3, 5, 7, 9, 11 and 15 taps all occur in some LSD case, and every instantiation of the
+    pre-grow kernel, k_lsd_pre<KS>, runs in an LSD case or in its own test's cases: KS 1 (scale 1, a 256 centre tap) up to
+    15 (3 taps always have a 256 centre)."""
     sizes = {pc.lsd_ksize(dict(ofe.DEFAULTS, **c)) for c in pc.LSD_CASES.values()}
     assert {3, 5, 7, 9, 11, 15} <= sizes
+    from test_lsd_pre_gpu import LSD_PRE_CASES
+    cases = [dict(ofe.DEFAULTS, **c) for c in [*pc.LSD_CASES.values(), *LSD_PRE_CASES.values()]]
+    assert {pc.lsd_pre_ks(c) for c in cases} == {1, 5, 7, 9, 11, 13, 15}
+    assert all(pc.lsd_pre_ks(dict(ofe.DEFAULTS, lsd_sigma_scale=s)) == 1 for s in np.linspace(0.01, 0.269, 40))
